@@ -1,9 +1,10 @@
 #!/usr/bin/env python
-"""bench.py -- BASELINE.json's headline metric ("BPR-MF triples/sec and item-to-item top-k vectors/sec at 1/2/4/8 B200").
+"""bench.py -- BASELINE.json's headline metric ("BPR-MF triples/sec and item-to-item top-k vectors/sec at 1/2/4/8 GPUs").
 
   python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--workload c2|c3|c4|c5|c1|small]
+                  [--dump-outputs DIR]
 
-Default (what the driver runs): BASELINE configs[1] ("c2": BPR, 1M users x 100K items x 10M feedback, d=64).  A "step" is
+Default: BASELINE configs[1] ("c2": BPR, 1M users x 100K items x 10M feedback, d=64).  A "step" is
 one BPR epoch = |R| fused sample-gather-dot-sigmoid-scatter triples.  For N > 1 (torchrun, one rank per GPU) the workload
 is weak-scaled: every rank owns 1M users / 10M feedback and hands the C ABI ONLY ITS OWN ROWS; the item table is replicated
 and its deltas are exchanged (NCCL) once per epoch.
@@ -14,8 +15,11 @@ One JSON line on rank 0 (DESIGN.md "measurement" explains every key):
              (Init, NEpochs epochs, Evaluate every Verbose epochs like cf.BPR.Fit) + get_factors (D2H), wall clock
   roofline   algorithmic bytes / epoch duration against the measured HBM copy peak
   also       at N = 1: compact records of BASELINE configs[2] (eALS, "c3") and configs[3] (all-pairs top-k, "c4"), each
-             with its own value / e2e / roofline / cpu_baseline / clocks, so that the driver's line carries the second half
+             with its own value / e2e / roofline / cpu_baseline / clocks, so that the default line carries the second half
              of the metric too (--no-also skips them)
+`--dump-outputs DIR` writes what the timed path computed in its last timed step as DIR/<name>.npy (float32 / float64; fixed,
+seeded row samples of the large tables, under 64 MB in all), so that two builds can be compared output for output: the
+inputs depend only on the arguments.
 `--impl reference` times the reference's CPU path for the same workload (oracle/_ref = the reference's own C kernels
 compiled here; threads pinned, median of the samples).
 """
@@ -52,7 +56,7 @@ def bytes_per_triple(d):
 
 def read_peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    hbm, tf, src = 6650.0, 1427.2, "fallback (B200_PROFILING.md)"
+    hbm, tf, src = 3350.0, 989.0, "H100 SXM data sheet (HBM3 bandwidth, dense bf16), not measured"
     if os.path.exists(p):
         try:
             j = json.load(open(p))
@@ -67,7 +71,7 @@ def bpr_config(wl, world):
     upr, n_items, fpr, d, desc = WORKLOADS[wl]
     return {"workload": desc, "users_per_rank": upr, "items": n_items, "train_feedback_per_rank": fpr, "d": d, "lr": LR, "reg": REG,
             "item_popularity": f"zipf({ZIPF_S})", "split": "leave-one-out (dataset.SplitCF(0, seed)): one test item per user beside the train rows",
-            "cache": "inputs larger than L2: the user table (256 MB per rank at c2) exceeds the 126 MB L2; no flush between steps"}
+            "cache": "inputs larger than L2: the user table (256 MB per rank at c2) exceeds the 50 MB L2; no flush between steps"}
 
 
 class ClockSampler:
@@ -109,6 +113,22 @@ class ClockSampler:
         return {"sm_mhz": sm[len(sm) // 2], "sm_max_mhz": float(rows[0][1]), "reasons": reasons, "samples": len(rows)}
 
 
+DUMP_ROWS = 16384   # rows of a table --dump-outputs keeps (a fixed, seeded sample of the larger ones)
+
+
+def dump_outputs(args, name, arrays):
+    """DIR/<name>_<key>.npy for every array; tables with more than DUMP_ROWS rows are sampled with a fixed seed"""
+    if not args.dump_outputs:
+        return
+    os.makedirs(args.dump_outputs, exist_ok=True)
+    for key, a in arrays.items():
+        a = np.asarray(a)
+        if a.shape[0] > DUMP_ROWS:
+            a = a[np.sort(np.random.default_rng(20261015).choice(a.shape[0], DUMP_ROWS, replace=False))]
+        a = a.astype(np.float32 if a.dtype in (np.float32, np.float16) else np.float64)
+        np.save(os.path.join(args.dump_outputs, f"{name}_{key}.npy"), a)
+
+
 def dist_env():
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
@@ -147,7 +167,7 @@ _CPU_CACHE = {}
 def cpu_bpr(wl, seconds_budget=2.0, samples=5):
     """The reference's CPU path for the same step on this box's host cores: per triple the reference's own call sequence
     (2x dot, exp, 3 row copies, 10 vector ops, model/cf/model.go:469-488) through the reference's C kernels (oracle/_ref,
-    compiled from /root/reference/common/floats/src) when present and the CPU has AVX-512, else through the oracle port;
+    compiled from the reference's common/floats/src) when present and the CPU has AVX-512, else through the oracle port;
     Hogwild over all host cores, worker t pinned to the t-th allowed CPU, tables first-touched page-interleaved over the
     workers; `samples` bounded samples of one epoch, MEDIAN reported."""
     import oracle
@@ -258,6 +278,10 @@ def run_bpr(args):
     t1 = time.time()
     launches = ctx.launch_count() - l0
     clocks = sampler.stop(t0, t1) if sampler else None
+    if rank == 0:
+        P_, Q_ = model.get_factors()
+        dump_outputs(args, "bpr", {"user_factors": P_, "item_factors": Q_})
+        del P_, Q_
     ms_total = max_over_ranks(ms_total)
     ms_per_step = ms_total / args.steps
     value = steps_per_epoch / (ms_per_step * 1e-3)
@@ -271,16 +295,9 @@ def run_bpr(args):
     k_ms = float(np.mean(kms))
     hbm, _, peak_src = read_peaks()
     achieved = bytes_per_triple(d) * n_local / (k_ms * 1e-3) / 1e9
-    traffic = None
-    tp = os.path.join(ROOT, "profiles", "bpr_epoch_traffic.json")
-    if os.path.exists(tp):
-        try:
-            traffic = json.load(open(tp)).get(f"{wl}_dram_bytes_per_launch")
-        except Exception:
-            traffic = None
+    traffic = None   # measured DRAM bytes per epoch: not available without a profiler
     roofline = {"bound": "hbm", "achieved": achieved, "peak": hbm, "unit": "GB/s", "frac": achieved / hbm, "traffic": traffic,
-                "kernel": f"one epoch on one rank = bpr_epoch_kernel<{d // 16 if d % 16 == 0 else 0}> (free-running) + bpr_hot_apply_kernel (capped hot rows) "
-                          "+ queue kernels" + (" + item-delta exchange" if world > 1 else ""),
+                "kernel": f"one epoch on one rank = bpr_round_kernel<{d // 16 if d % 16 == 0 else 0}> (rounds of 8192 triples)" + (" + item-delta exchange" if world > 1 else ""),
                 "kernel_ms": k_ms, "algorithmic_bytes_per_launch": bytes_per_triple(d) * n_local,
                 "dram_frac": (traffic / (k_ms * 1e-3) / 1e9 / hbm) if traffic else None, "peak_source": peak_src}
     model.close()
@@ -368,7 +385,7 @@ def run_als(args):
     else:
         (off, items), (test_off, test_items) = get_data("c2", 1000)
     ioff, iusers = gb.transpose_csr(off, items, I)
-    steps, warm = min(args.steps, 10), args.warmup
+    steps, warm = args.steps, args.warmup
     with gb.Context(0) as ctx:
         with gb.CFModel(ctx, U, I, d, off, items, ioff, iusers) as m:
             m.init_normal(0.0, ALS_STD, 0)
@@ -383,6 +400,9 @@ def run_als(args):
             t1 = time.time()
             launches = ctx.launch_count() - l0
             clocks = sampler.stop(t0, t1)
+            P_, Q_ = m.get_factors()
+            dump_outputs(args, "als", {"user_factors": P_, "item_factors": Q_})
+            del P_, Q_
         e2e = None
         if not args.no_e2e:
             hp, hq = gb.PinnedArray((U, d)), gb.PinnedArray((I, d))
@@ -449,7 +469,7 @@ def run_topk(args):
     rng = np.random.default_rng(0)
     X = rng.standard_normal((N, d), dtype=np.float32)
     X /= np.linalg.norm(X, axis=1, keepdims=True)
-    steps = min(args.steps, 10)
+    steps = args.steps
     with gb.Context(local) as ctx:
         with gb.BruteforceIndex(ctx, d, gb.METRIC_NEG_DOT) as ix:
             ix.add(X)
@@ -474,6 +494,8 @@ def run_topk(args):
             s1_ms, s1_flop, fb = ix.stage1_stats()
             clocks = sampler.stop(t0, t1) if sampler else None
             assert cnt.min() == k
+            if rank == 0:
+                dump_outputs(args, "topk", {"indices": idx, "distances": dist_})
         # end to end from host buffers: build the index (vectors H2D + mirror) and answer nq queries into host memory
         e2e = None
         if not args.no_e2e:
@@ -516,7 +538,7 @@ def run_topk(args):
                                    + (f" x {world} ranks, vectors replicated, queries sharded, no collective" if world > 1 else ""),
                        "metric": "-dot (cosine on unit vectors)", "fallback_rows": int(fb)},
             "roofline": {"bound": "tensor", "achieved": s1_flop / (s1_ms * 1e-3) / 1e12, "peak": peak, "unit": "TFLOP/s",
-                         "frac": s1_flop / (s1_ms * 1e-3) / 1e12 / peak, "traffic": None, "kernel": "mma::topk_mma_kernel (tcgen05 sweep)",
+                         "frac": s1_flop / (s1_ms * 1e-3) / 1e12 / peak, "traffic": None, "kernel": "mma::topk_mma_kernel (wgmma sweep)",
                          "kernel_ms": s1_ms / steps, "algorithmic_flop_per_launch": s1_flop / steps,
                          "whole_call_tflops": flop / (ms * 1e-3) / 1e12, "peak_source": src + " sustained bf16"},
             "cpu_baseline": cb, "e2e": e2e, "gpu_launches": int(launches), "clocks": clocks}
@@ -530,12 +552,14 @@ def build_parser():
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--workload", default="c2", choices=sorted(WORKLOADS) + ["c3", "c4"])
     ap.add_argument("--small", action="store_true", help="c3/c4 at reduced size (not a bench number)")
-    ap.add_argument("--queries", type=int, default=151552, help="c4: query rows per step")
+    ap.add_argument("--queries", type=int, default=151552, help="c4: query rows per step (on 132 SMs one 135168-row chunk plus a 16384-row tail, DESIGN 5.3)")
     ap.add_argument("--e2e-epochs", type=int, default=100, help="BPR default NEpochs, model/cf/model.go:390")
     ap.add_argument("--zipf", type=float, default=None, help="item popularity exponent of the synthetic data (default 1.0; 0 = uniform)")
     ap.add_argument("--no-e2e", action="store_true")
     ap.add_argument("--no-cpu", action="store_true")
     ap.add_argument("--no-also", action="store_true", help="default run: skip the c3 / c4 sub-records")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's outputs as DIR/<name>.npy (seeded row samples of large tables)")
     return ap
 
 

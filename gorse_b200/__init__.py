@@ -1,4 +1,4 @@
-"""gorse_b200 -- B200 (sm_100a) implementation of Gorse's collaborative-filtering training and
+"""gorse_b200 -- H100 (sm_90a) implementation of Gorse's collaborative-filtering training and
 brute-force top-k hot path.
 
 The product is the C-ABI shared library (include/gorse_b200.h, gorse_b200/libgorse_b200.so).  This
@@ -282,7 +282,7 @@ class BruteforceIndex:
         return n.value
 
     def stage1_stats(self):
-        """(device ms, algorithmic flop, fallback rows) of the tcgen05 candidate sweep since the last call."""
+        """(device ms, algorithmic flop, fallback rows) of the tensor-core candidate sweep since the last call."""
         ms, fl, fb = C.c_double(0), C.c_double(0), C.c_int64(0)
         check(lib.gorse_b200_index_stats(self.h, C.byref(ms), C.byref(fl), C.byref(fb)))
         return ms.value, fl.value, fb.value

@@ -10,7 +10,7 @@
 //   * als_thread_kernel (als_thread.cu; d % 32 == 0, d <= 128, rows up to 4 entries): one thread per row;
 //   * als_rows_group_blocked_kernel (same d, rows up to 96 entries): a group of 8/16/32 lanes per row, g = S x kept
 //     current in registers, the gathered rows staged one block of G coordinates at a time;
-//   * Gram form for longer rows (tcgen05 chunk Grams at d = 128, als_gram_tc.cu, else als_chunk_gram_kernel; then
+//   * Gram form for longer rows (tensor-core chunk Grams at d = 128, als_gram_tc.cu, else als_chunk_gram_kernel; then
 //     als_solve_kernel): one Gauss-Seidel sweep on A x = h;
 //   * als_rows_kernel, one warp per row with the reference's loop structure, for the remaining shapes (d not a
 //     multiple of 32 or > 128).  The gathered rows Y[R_x] are staged once in shared memory ([n][d+1], the +1 makes the
@@ -36,70 +36,35 @@ __device__ __forceinline__ float warp_sum(float v)
     return v;
 }
 
-// Two fp32 FMAs per instruction (Blackwell FFMA2, PTX fma.rn.f32x2): both halves are ordinary IEEE fp32 FMAs.
-__device__ __forceinline__ unsigned long long pack2(float lo, float hi)
-{
-    return ((unsigned long long)__float_as_uint(hi) << 32) | (unsigned long long)__float_as_uint(lo);
-}
-__device__ __forceinline__ unsigned long long ffma2(unsigned long long a, unsigned long long b, unsigned long long c)
-{
-    unsigned long long d;
-    asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(a), "l"(b), "l"(c));
-    return d;
-}
-// acc[x][y] += a[x] * b[y] over a TxT register tile; F2 pairs the y direction (T even)
-template <int T, bool F2>
+// acc[x][y] += a[x] * b[y] over a TxT register tile
+template <int T>
 struct GramTile {
     float acc[T][T];
-    unsigned long long acc2[T][F2 ? T / 2 : 1];
     __device__ __forceinline__ void zero()
     {
 #pragma unroll
-        for (int x = 0; x < T; x++) {
+        for (int x = 0; x < T; x++)
 #pragma unroll
             for (int y = 0; y < T; y++) acc[x][y] = 0.f;
-#pragma unroll
-            for (int y = 0; y < (F2 ? T / 2 : 1); y++) acc2[x][y] = 0ull;
-        }
     }
     __device__ __forceinline__ void mac(const float (&a)[T], const float (&b)[T])
     {
-        if constexpr (F2) {
-            unsigned long long b2[T / 2];
 #pragma unroll
-            for (int y = 0; y < T / 2; y++) b2[y] = pack2(b[2 * y], b[2 * y + 1]);
+        for (int x = 0; x < T; x++)
 #pragma unroll
-            for (int x = 0; x < T; x++) {
-                const unsigned long long ax = pack2(a[x], a[x]);
-#pragma unroll
-                for (int y = 0; y < T / 2; y++) acc2[x][y] = ffma2(ax, b2[y], acc2[x][y]);
-            }
-        } else {
-#pragma unroll
-            for (int x = 0; x < T; x++)
-#pragma unroll
-                for (int y = 0; y < T; y++) acc[x][y] = __fmaf_rn(a[x], b[y], acc[x][y]);
-        }
+            for (int y = 0; y < T; y++) acc[x][y] = __fmaf_rn(a[x], b[y], acc[x][y]);
     }
-    __device__ __forceinline__ float get(int x, int y) const
-    {
-        if constexpr (F2) {
-            const unsigned long long v = acc2[x][y >> 1];
-            return __uint_as_float((unsigned)((y & 1) ? (v >> 32) : v));
-        } else {
-            return acc[x][y];
-        }
-    }
+    __device__ __forceinline__ float get(int x, int y) const { return acc[x][y]; }
 };
 
 // Partial Gram of rows [r0, r1) handled by this CTA; TxT register tile per thread, 16x16 threads.
-template <int T, bool F2>
+template <int T>
 __global__ void __launch_bounds__(256) gram_kernel(const float *X, int32_t rows, int d, const int64_t *off, float *partial)
 {
     extern __shared__ float xs[];  // [16][dp]
     const int dp = 16 * T;         // padded width
     const int ti = threadIdx.x >> 4, tj = threadIdx.x & 15;
-    GramTile<T, F2> tile;
+    GramTile<T> tile;
     tile.zero();
     int64_t per = ((int64_t)rows + gridDim.x - 1) / gridDim.x;
     int64_t r0 = (int64_t)blockIdx.x * per, r1 = min((int64_t)rows, r0 + per);
@@ -286,7 +251,7 @@ __device__ __forceinline__ float group_sum(float v)
 // als_rows_group_kernel, removed): n * (G+1) floats per row in shared memory instead of n * (D+1).  The whole-row version held 33 KB (rows up
 // to 32 entries, two rows per warp) / 49.5 KB (rows up to 96 entries) per warp next to the 64 KB copy of S, i.e. 3-4 warps per
 // SM, and each of those warps runs a dependent shuffle chain per coordinate: 2.3 + 3.0 ms per half-sweep for 7 % of the rows
-// (profiles/r02_launches_c3.md).  Lane j of the group owns coordinate i*G + j of block i, so a block is exactly what the group
+// Lane j of the group owns coordinate i*G + j of block i, so a block is exactly what the group
 // works on at a time:
 //   pass A  per sub-range of G entries and per block: stage G x G floats, partial_tt += x_i * y (registers, one per entry of
 //           the sub-range), h_i, c_i column sums; the partials are reduced across the group once per sub-range -> pred;
@@ -469,14 +434,14 @@ static int32_t launch_group_blocked_d(gorse_b200_cf *cf, float *X, const float *
 // same 16x16-thread register tiling as gram_kernel, and one CTA per row sums the partials and does the sweep.
 #define GB_ALS_CHUNK 2048
 
-template <int T, bool F2>
+template <int T>
 __global__ void __launch_bounds__(256) als_chunk_gram_kernel(const float *Y, int d, const int32_t *idx, const int32_t *chunk_row,
                                                              const int64_t *chunk_begin, const int32_t *chunk_len, float *partial)
 {
     extern __shared__ float xs[];  // [16][dp]
     const int dp = 16 * T;
     const int ti = threadIdx.x >> 4, tj = threadIdx.x & 15;
-    GramTile<T, F2> tile;
+    GramTile<T> tile;
     tile.zero();
     float hacc[T];
 #pragma unroll
@@ -641,7 +606,6 @@ __global__ void __launch_bounds__(256) als_solve_kernel(float *X, int d, const f
     }
 }
 
-// (FFMA2 register tiles -- fma.rn.f32x2 -- were measured in round 2: 49.3 vs 35.0 ms per C3 epoch, slower; removed.)
 
 // S = sum over rows with >= 1 feedback of x x^T.  `X`, `off` and `rows` describe THIS RANK's row range (off is the rank's
 // rebased offsets); in a distributed context the d x d partial sums are all-reduced, so every rank ends with the same bits.
@@ -672,10 +636,10 @@ static int32_t run_gram(gorse_b200_cf *cf, int side, const float *X_base, const 
         int T = d <= 16 ? 1 : d <= 32 ? 2 : d <= 64 ? 4 : 8;
         size_t sm = sizeof(float) * 16 * 16 * T;
         switch (T) {
-            case 1: gram_kernel<1, false><<<parts, 256, sm, c->stream>>>(X, rows, d, off, cf->scratch.p); break;
-            case 2: gram_kernel<2, false><<<parts, 256, sm, c->stream>>>(X, rows, d, off, cf->scratch.p); break;
-            case 4: gram_kernel<4, false><<<parts, 256, sm, c->stream>>>(X, rows, d, off, cf->scratch.p); break;
-            default: gram_kernel<8, false><<<parts, 256, sm, c->stream>>>(X, rows, d, off, cf->scratch.p); break;
+            case 1: gram_kernel<1><<<parts, 256, sm, c->stream>>>(X, rows, d, off, cf->scratch.p); break;
+            case 2: gram_kernel<2><<<parts, 256, sm, c->stream>>>(X, rows, d, off, cf->scratch.p); break;
+            case 4: gram_kernel<4><<<parts, 256, sm, c->stream>>>(X, rows, d, off, cf->scratch.p); break;
+            default: gram_kernel<8><<<parts, 256, sm, c->stream>>>(X, rows, d, off, cf->scratch.p); break;
         }
     } else {
         gram_generic_kernel<<<parts, 256, 0, c->stream>>>(X, rows, d, off, cf->scratch.p);
@@ -806,7 +770,7 @@ static int32_t prepare_als(gorse_b200_cf *cf)
 }
 
 // (Round 1's whole-row lane-group kernel and its B = 4 variant -- four coordinates per shuffle butterfly, 72 vs 43 ms/epoch --
-// are gone: the blocked-staging kernel above replaced them in every class, profiles/r02_launches_c3.md.)
+// are gone: the blocked-staging kernel above replaced them in every class.)
 static int32_t run_rows(gorse_b200_cf *cf, int side, float *X, const float *Y, const int64_t *off, const int32_t *idx,
                         float reg, float w, float *pred_scratch)
 {
@@ -820,12 +784,12 @@ static int32_t run_rows(gorse_b200_cf *cf, int side, float *X, const float *Y, c
             const int d = cf->d, T = d <= 16 ? 1 : d <= 32 ? 2 : d <= 64 ? 4 : 8;
             const size_t gsm = sizeof(float) * 16 * 16 * T;
             const int nc = cf->als_n_chunks[side];
-            auto *ck = als_chunk_gram_kernel<1, false>;
+            auto *ck = als_chunk_gram_kernel<1>;
                 switch (T) {
                 case 1: break;
-                case 2: ck = als_chunk_gram_kernel<2, false>; break;
-                case 4: ck = als_chunk_gram_kernel<4, false>; break;
-                default: ck = als_chunk_gram_kernel<8, false>; break;
+                case 2: ck = als_chunk_gram_kernel<2>; break;
+                case 4: ck = als_chunk_gram_kernel<4>; break;
+                default: ck = als_chunk_gram_kernel<8>; break;
             }
             if (d == 128) {
                 GB_TRY(als_chunk_gram_tc(c, Y, idx, cf->als_chunk_begin[side].p, cf->als_chunk_len[side].p, nc, cf->als_partial.p));
@@ -845,7 +809,7 @@ static int32_t run_rows(gorse_b200_cf *cf, int side, float *X, const float *Y, c
         }
         if (grouped && k != GB_ALS_LONG) {
             const RowClass rc = kRowClasses[k];
-            // Round 2 A/B (profiles/r02_launches_c3.md): lane groups with blocked staging beat the thread-per-row kernel in
+            // A/B: lane groups with blocked staging beat the thread-per-row kernel in
             // every class above 4 entries (<=8: 0.80 vs 1.16 ms, <=16: 1.27 vs 1.99 ms per half-sweep at C3) and the
             // whole-row staging of the first lane-group kernels in the two longer classes; the thread kernel keeps the
             // shortest rows, where it is 0.14 ms ahead (also when they are many: the 300 K short user rows of C3 take 1.69 ms

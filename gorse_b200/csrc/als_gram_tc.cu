@@ -1,51 +1,39 @@
-// als_gram_tc.cu -- the Gram form of long eALS rows on the 5th-generation tensor cores (d = 128).
+// als_gram_tc.cu -- the Gram form of long eALS rows on the Hopper tensor cores (d = 128).
 //
 // For a row with many entries the coordinate sweep of model/cf/model.go:664-686 is one Gauss-Seidel sweep on A x = h with
-// A = (1-w) G + w S + reg I,  G = sum_t y_t y_t^T,  h = sum_t y_t  (als.cu, "Gram form").  G is |R_row| * d^2 multiply-adds:
-// at BASELINE configs[2] three quarters of the item side's feedback sit in rows longer than 96 entries, 123 G multiply-adds
-// per epoch, and the fp32 register-tiled kernel that computed them was 26 % of the epoch (8.5 ms, profiles/r02_launches_c3.md).
-// It is the one dense contraction of the eALS epoch, so it goes to tcgen05:
+// A = (1-w) G + w S + reg I,  G = sum_t y_t y_t^T,  h = sum_t y_t  (als.cu, "Gram form").  G is |R_row| * d^2 multiply-adds,
+// and most of the item side's feedback sits in long rows, so this one dense contraction of the eALS epoch goes to wgmma:
 //
-//   D[128 x 128] (fp32, TMEM) += A[128 x 8] * B[128 x 8]^T   per instruction, kind::tf32, cta_group::1
+//   D[64 x 128] (fp32, registers) += A[64 x 8] * B[128 x 8]^T   per instruction, kind tf32, one warpgroup
 //
-// with A = B = the transposed tile of gathered rows.  The gathered data lie in memory as [entry][d] (d contiguous): exactly
-// the MN-MAJOR operand layout (the K index = entry is the slow one), so the tile is written to shared memory as it arrives,
-// 16 bytes per thread, with the swizzle applied to the chunk index -- no transpose.  MN-major 32-bit operands have exactly one
-// legal layout, SWIZZLE_128B_BASE32B (CUTLASS cute/atom/mma_traits_sm100.hpp:72, builders/sm100_common.inl:92):
-//   Swizzle<2,5,2> o ((T,8,m),(4,k)) : ((1,T,LBO),(8T,SBO)),  T = 4 fp32
-// i.e. an atom is 4 entries x 32 floats (4 rows of 128 bytes) whose 32-BYTE chunks are XOR-ed with the row index mod 4
-// (address bits 5-6 ^= bits 7-8); the 4 atoms along d (m = 4) are LBO = KT*128 bytes apart (one 32-float column panel per
-// atom column), the next 4 entries SBO = 512 bytes further (rows stay contiguous), and one K = 8 instruction spans two atoms.
-// (The first version used the plain 128-byte swizzle, which the hardware only accepts for K-major or 16-bit MN-major
-// operands: it ran at full speed and produced garbage.)
+// with A = rows 64 g .. 64 g + 63 (warpgroup g of two) and B = all 128 rows of the tile of gathered entries, transposed.
+// wgmma takes 32-bit operands K-major only (K = entry contiguous), while the gathered data lie in memory as [entry][d]; the
+// tile is therefore written transposed, [d][entry], one 4-byte store per value: thread = entry, so a warp's 32 stores of
+// one d row land in 32 different banks.  A stage is KT = 32 entries = one 128-byte row per d, stored in the 128-byte swizzle
+// (16-byte chunk index ^= d % 8) that the descriptor names; one K = 8 instruction advances 32 bytes along the row.
 //
 // fp32-grade accuracy from tf32 operands ("3xTF32"): y = hi + lo with hi = y rounded to tf32 and lo = (y - hi) rounded to tf32;
 // G ~= hi hi^T + hi lo^T + lo hi^T, three MMAs per k-step into the same accumulator.  Dropped: lo lo^T and the rounding of
 // lo, both <= 2^-22 relative per product and of random sign.
 //
-// One CTA = one chunk (<= GB_ALS_CHUNK entries of one row): 256 threads gather KT = 32 entries per stage (each warp reads
-// whole 512-byte rows), split them into the hi and lo tiles of a 3-stage ring, thread 0 issues the 12 MMAs of the stage and
-// commits them to the stage's mbarrier; the gathers of the next stages overlap the MMAs.  Epilogue: tcgen05.ld, one thread per
-// accumulator row, straight into the partial (G, h) buffer als_solve_kernel sums.
+// One CTA = one chunk (<= GB_ALS_CHUNK entries of one row): 256 threads gather KT = 32 entries per stage into registers,
+// split them into the hi and lo tiles of a 3-stage ring and issue the stage's 12 MMAs per warpgroup asynchronously; the
+// gather of the next stage overlaps them.  Epilogue: each thread stores its accumulator fragment straight into the partial
+// (G, h) buffer als_solve_kernel sums.
 #include "als.cuh"
-#include "umma.cuh"
+#include "wgmma.cuh"
 
 namespace gb {
 
 namespace {
 
 constexpr int TC_D = 128, TC_KT = 32, TC_STAGES = 3, TC_THREADS = 256;
-constexpr uint32_t TC_TILE_BYTES = TC_KT * TC_D * 4;          // one [32 entries x 128 floats] tile = 16 KB
-constexpr uint32_t TC_PANEL_BYTES = TC_KT * 128;              // one 32-float column panel of the tile = LBO
-// instruction descriptor (cute/arch/mma_sm100_desc.hpp): D fp32 (bits 4-5 = 1), A/B tf32 (bits 7-9, 10-12 = 2), A and B
-// MN-major (bits 15, 16), N>>3 at 17, M>>4 at 24
-constexpr uint32_t TC_IDESC = (1u << 4) | (2u << 7) | (2u << 10) | (1u << 15) | (1u << 16) | ((uint32_t)(TC_D >> 3) << 17) |
-                              ((uint32_t)(TC_D >> 4) << 24);
+constexpr uint32_t TC_TILE_BYTES = TC_D * TC_KT * 4;          // one [128 d x 32 entries] tile = 16 KB
 
 // fp32 -> tf32 with round-to-nearest (the tensor core itself TRUNCATES the low 13 mantissa bits of an fp32 word: splitting by
 // truncation leaves |lo| < 2^-10 |y| with the sign of y, and the dropped lo*lo term and the truncation of lo then bias every
-// entry of G by ~1e-6 relative in the same direction -- enough, through the conditioning of A, to push one parity case to
-// 1.6e-4.  Rounded: |lo| <= 2^-11 |y| with random sign, and lo is exactly representable, so nothing is truncated.)
+// entry of G by ~1e-6 relative in the same direction.  Rounded: |lo| <= 2^-11 |y| with random sign, and lo is exactly
+// representable, so nothing is truncated.)
 __device__ __forceinline__ float to_tf32(float x)
 {
     uint32_t r;
@@ -58,114 +46,86 @@ als_chunk_gram_tc_kernel(const float *Y, const int32_t *idx, const int64_t *chun
 {
     using namespace mma;
     extern __shared__ __align__(1024) uint8_t smem_raw[];
-    uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-    uint8_t *tiles = smem;                                                     // [STAGES][hi, lo] tiles
-    uint64_t *bars = reinterpret_cast<uint64_t *>(tiles + (size_t)TC_STAGES * 2 * TC_TILE_BYTES);   // [STAGES] "MMAs of this stage retired"
-    uint64_t *done = bars + TC_STAGES;
-    uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(done + 1);
-    float *hred = reinterpret_cast<float *>(reinterpret_cast<uint8_t *>(bars) + 64);   // [8][128] column sums per row group (16-byte aligned)
+    uint8_t *tiles = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);   // [STAGES][hi, lo]
 
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    if (tid == 0) {
-        for (int s = 0; s < TC_STAGES; s++) mbar_init(&bars[s], 1);
-        mbar_init(done, 1);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(s32(tmem_slot)), "r"(128u) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem_base = *tmem_slot;
-
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wg = warp >> 2;
     const int64_t b0 = chunk_begin[blockIdx.x];
     const int len = chunk_len[blockIdx.x];
     const int n_stage = (len + TC_KT - 1) / TC_KT;
-    // thread -> 16-byte chunk c of a row (32 per row), row group rr; per stage rows k = rr + 8 i
-    const int c = lane, rr = warp;
-    const int panel = c >> 3, cc = c & 7;
-    float4 hsum = make_float4(0.f, 0.f, 0.f, 0.f);
-    float4 pre[TC_KT / 8];
-    auto gather = [&](int st) {
+    // thread -> entry `lane` of a stage and the 16-byte chunks c = 4 warp + i (i < 4) of its row: d = 16 warp .. 16 warp + 15
+    float4 pre[4], hsum[4];
 #pragma unroll
-        for (int i = 0; i < TC_KT / 8; i++) {
-            const int k = st * TC_KT + rr + 8 * i;
-            pre[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-            if (k < len) pre[i] = __ldg(reinterpret_cast<const float4 *>(Y + (int64_t)__ldg(idx + b0 + k) * TC_D) + c);
-        }
+    for (int i = 0; i < 4; i++) hsum[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+    auto gather = [&](int st) {
+        const int k = st * TC_KT + lane;
+        const float4 *src = k < len ? reinterpret_cast<const float4 *>(Y + (int64_t)__ldg(idx + b0 + k) * TC_D) + 4 * warp : nullptr;
+#pragma unroll
+        for (int i = 0; i < 4; i++) pre[i] = src ? __ldg(src + i) : make_float4(0.f, 0.f, 0.f, 0.f);
     };
+    float acc[64];   // written first by an MMA with the accumulate flag off (an explicit zeroing would serialise the MMAs)
     if (n_stage > 0) gather(0);
     for (int st = 0; st < n_stage; st++) {
         const int slot = st % TC_STAGES;
-        // the MMAs that read this ring slot (iteration st - STAGES) must have retired
-        if (st >= TC_STAGES) mbar_wait(&bars[slot], ((st / TC_STAGES) - 1) & 1);
+        // the MMAs that read this ring slot (stage st - STAGES) have retired: this warpgroup's by the wait, the other's by the barrier
+        wgmma_wait<TC_STAGES - 1>();
+        __syncthreads();
         uint8_t *hi = tiles + (size_t)slot * 2 * TC_TILE_BYTES, *lo = hi + TC_TILE_BYTES;
 #pragma unroll
-        for (int i = 0; i < TC_KT / 8; i++) {
-            const int k = rr + 8 * i;
+        for (int i = 0; i < 4; i++) {
             const float4 v = pre[i];
-            hsum.x += v.x; hsum.y += v.y; hsum.z += v.z; hsum.w += v.w;
-            float4 h4, l4;
-            h4.x = to_tf32(v.x); h4.y = to_tf32(v.y); h4.z = to_tf32(v.z); h4.w = to_tf32(v.w);
-            l4.x = to_tf32(v.x - h4.x); l4.y = to_tf32(v.y - h4.y); l4.z = to_tf32(v.z - h4.z); l4.w = to_tf32(v.w - h4.w);
-            const uint32_t o = (uint32_t)panel * TC_PANEL_BYTES + (uint32_t)k * 128u + (uint32_t)((((cc >> 1) ^ (k & 3)) << 5) | ((cc & 1) << 4));
-            *reinterpret_cast<float4 *>(hi + o) = h4;
-            *reinterpret_cast<float4 *>(lo + o) = l4;
+            hsum[i].x += v.x; hsum[i].y += v.y; hsum[i].z += v.z; hsum[i].w += v.w;
+            const float vv[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+            for (int q = 0; q < 4; q++) {
+                const int m = 16 * warp + 4 * i + q;   // d index = tile row
+                const uint32_t o = (uint32_t)m * 128u + ((((uint32_t)lane >> 2) ^ ((uint32_t)m & 7u)) << 4) + (((uint32_t)lane & 3u) << 2);
+                const float h = to_tf32(vv[q]);
+                *reinterpret_cast<float *>(hi + o) = h;
+                *reinterpret_cast<float *>(lo + o) = to_tf32(vv[q] - h);
+            }
         }
-        if (st + 1 < n_stage) gather(st + 1);   // in flight while this stage's MMAs are issued
+        if (st + 1 < n_stage) gather(st + 1);   // in flight while this stage's MMAs run
         // generic-proxy stores -> async-proxy (tensor core) reads
         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
         __syncthreads();
-        if (warp == 0 && elect_one()) {   // an elected lane, not `tid == 0`: keeps the descriptor arithmetic on the uniform datapath
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            const uint32_t a_hi = s32(hi), a_lo = s32(lo);
+        wgmma_fence();
+        const uint32_t b_hi = s32(hi), b_lo = s32(lo), a_hi = b_hi + (uint32_t)wg * 64u * 128u, a_lo = b_lo + (uint32_t)wg * 64u * 128u;
 #pragma unroll
-            for (int ks = 0; ks < TC_KT / 8; ks++) {
-                const uint64_t dh = umma_desc_any(a_hi + ks * 1024u, TC_PANEL_BYTES, 512u, 1u);
-                const uint64_t dl = umma_desc_any(a_lo + ks * 1024u, TC_PANEL_BYTES, 512u, 1u);
-                umma_tf32(tmem_base, dh, dh, TC_IDESC, (st | ks) != 0);
-                umma_tf32(tmem_base, dh, dl, TC_IDESC, 1);
-                umma_tf32(tmem_base, dl, dh, TC_IDESC, 1);
-            }
-            umma_commit(&bars[slot]);
-            if (st == n_stage - 1) umma_commit(done);
+        for (int ks = 0; ks < TC_KT / 8; ks++) {
+            const uint32_t ko = (uint32_t)ks * 32u;   // 8 tf32 = 32 bytes along the row
+            wgmma_m64n128k8_tf32(acc, wgmma_desc(a_hi + ko), wgmma_desc(b_hi + ko), (st | ks) != 0);
+            wgmma_m64n128k8_tf32(acc, wgmma_desc(a_hi + ko), wgmma_desc(b_lo + ko), 1);
+            wgmma_m64n128k8_tf32(acc, wgmma_desc(a_lo + ko), wgmma_desc(b_hi + ko), 1);
         }
+        wgmma_commit();
     }
-    // column sums h: reduce the 8 row groups
-    *reinterpret_cast<float4 *>(hred + rr * TC_D + 4 * c) = hsum;
-    __syncthreads();
+    wgmma_wait<0>();
     float *out = partial + (int64_t)blockIdx.x * (TC_D * TC_D + TC_D);
-    if (tid < TC_D) {
-        float s = 0.f;
+    if (n_stage == 0) {
 #pragma unroll
-        for (int g = 0; g < 8; g++) s += hred[g * TC_D + tid];
-        out[TC_D * TC_D + tid] = s;
+        for (int e = 0; e < 64; e++) acc[e] = 0.f;
     }
-    if (n_stage > 0) {
-        mbar_wait(done, 0);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        if (warp < 4) {
-            // accumulator row i = TMEM lane 32*warp + lane, 128 columns
-            const int i = 32 * warp + lane;
-            const uint32_t taddr = tmem_base + ((uint32_t)(32 * warp) << 16);
-#pragma unroll 1
-            for (int j0 = 0; j0 < TC_D; j0 += 32) {
-                uint32_t v[32];
-                tmem_ld32(taddr + j0, v);
+    {
+        // accumulator fragment -> G rows 64 wg + 16 (warp % 4) + lane / 4 (+ 8), columns 8 j + 2 (lane % 4) + {0, 1}
+        const int r = 64 * wg + 16 * (warp & 3) + (lane >> 2), c0 = 2 * (lane & 3);
 #pragma unroll
-                for (int e = 0; e < 32; e += 4)
-                    *reinterpret_cast<float4 *>(out + i * TC_D + j0 + e) =
-                        make_float4(__uint_as_float(v[e]), __uint_as_float(v[e + 1]), __uint_as_float(v[e + 2]), __uint_as_float(v[e + 3]));
-            }
+        for (int j = 0; j < TC_D / 8; j++) {
+            *reinterpret_cast<float2 *>(out + r * TC_D + 8 * j + c0) = make_float2(acc[4 * j], acc[4 * j + 1]);
+            *reinterpret_cast<float2 *>(out + (r + 8) * TC_D + 8 * j + c0) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
         }
-    } else if (tid < TC_D) {
-        for (int j = 0; j < TC_D; j++) out[tid * TC_D + j] = 0.f;
     }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if (warp == 1) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(128u) : "memory");
+    // column sums h: reduce the 32 entries (lanes) of every chunk
+#pragma unroll
+    for (int i = 0; i < 4; i++) {
+#pragma unroll
+        for (int o = 16; o; o >>= 1) {
+            hsum[i].x += __shfl_xor_sync(0xffffffffu, hsum[i].x, o);
+            hsum[i].y += __shfl_xor_sync(0xffffffffu, hsum[i].y, o);
+            hsum[i].z += __shfl_xor_sync(0xffffffffu, hsum[i].z, o);
+            hsum[i].w += __shfl_xor_sync(0xffffffffu, hsum[i].w, o);
+        }
+        if (lane == 0) *reinterpret_cast<float4 *>(out + TC_D * TC_D + 16 * warp + 4 * i) = hsum[i];
+    }
 }
 
 }  // namespace
@@ -174,7 +134,7 @@ als_chunk_gram_tc_kernel(const float *Y, const int32_t *idx, const int64_t *chun
 int32_t als_chunk_gram_tc(gorse_b200_ctx *c, const float *Y, const int32_t *idx, const int64_t *chunk_begin, const int32_t *chunk_len,
                           int32_t n_chunks, float *partial)
 {
-    const size_t sm = (size_t)TC_STAGES * 2 * TC_TILE_BYTES + 1024 /* alignment */ + 64 /* barriers, tmem slot */ + sizeof(float) * 8 * TC_D;
+    const size_t sm = (size_t)TC_STAGES * 2 * TC_TILE_BYTES + 1024 /* alignment */;
     GB_CUDA(cudaFuncSetAttribute(als_chunk_gram_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm));
     als_chunk_gram_tc_kernel<<<n_chunks, TC_THREADS, sm, c->stream>>>(Y, idx, chunk_begin, chunk_len, partial);
     GB_LAUNCHED(c);

@@ -52,7 +52,7 @@ __device__ __forceinline__ void stage_block(float *ys, const float *Y, const int
 }
 
 // BCU coordinates are unrolled inside the (rolled) sweep loop.  The first version unrolled all D coordinates (600 KB of
-// straight-line code at D = 128, five minutes of ptxas) and was no faster (profiles/r02_als_thread.md).
+// straight-line code at D = 128, five minutes of ptxas) and was no faster.
 #define GB_ALS_BCU 4
 
 template <int D, int NMAX, int BC, int WARPS>

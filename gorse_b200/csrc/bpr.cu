@@ -4,6 +4,8 @@
 // Roofline class: HBM/L2 bandwidth.  Algorithmic bytes per triple = 6*d*4 + 12 (3 rows read, 3 rows
 // written, 3 ids).  One quad (4 lanes) owns one triple; see cf.cuh for the row->lane mapping that keeps
 // the reference's AVX-512 summation order with 128-bit coalesced loads.
+#include <cooperative_groups.h>
+
 #include <algorithm>
 #include <cstdlib>
 
@@ -17,10 +19,6 @@ struct BprView {
     const int32_t *user_items;
     const int32_t *active;      // nullptr when every user of the shard has feedback (active[k] == u_lo + k)
     int32_t n_active, n_items, d, u_lo;
-    // items whose positive-sampling mass is large are not trained by the free-running kernel: see bpr_hot.cuh
-    const int32_t *hot_slot;    // per item: slot or -1; nullptr when no item is hot / the hot path is off
-    float *hot;                 // striped side table of the hot rows (bpr_hot.cuh), valid during an epoch
-    int32_t hot_pad;
 };
 
 // factor rows are read and written by every SM concurrently: keep them out of the (non-coherent) L1
@@ -33,9 +31,8 @@ __device__ __forceinline__ void red_row(float *p, float4 v)
                  : "memory");
 }
 
-}  // namespace gb
-#include "bpr_hot.cuh"
-namespace gb {
+
+#define GB_BPR_ROUND 8192   // triples per round of the atomic-scatter epoch (bpr_round_kernel)
 
 #define GB_F4_OP(dst, expr)                            \
     do {                                               \
@@ -73,20 +70,26 @@ __device__ __forceinline__ void load_rows(Rows<C> &r, const float *Pu, const flo
     for (int c = 0; c < C; c++) r.qj[c] = ld_row(Qj + sj * c);
 }
 
-// one SGD step by a quad on rows already in registers
-template <int C, bool ATOMIC>
-__device__ __forceinline__ void bpr_step_rows(const Rows<C> &r, float *Pu, float *Qi, int si, float *Qj, int sj, unsigned mask,
-                                              float lr, float reg)
+// the gradient factor of one triple whose rows are in registers (:469-471)
+template <int C>
+__device__ __forceinline__ float bpr_grad_rows(const Rows<C> &r, unsigned mask)
 {
-    const float4 *p = r.p, *qi = r.qi, *qj = r.qj;
     float4 ai = make_float4(0.f, 0.f, 0.f, 0.f), aj = ai;
 #pragma unroll
     for (int c = 0; c < C; c++) {
-        dot_chunk(ai, p[c], qi[c], c == 0);
-        dot_chunk(aj, p[c], qj[c], c == 0);
+        dot_chunk(ai, r.p[c], r.qi[c], c == 0);
+        dot_chunk(aj, r.p[c], r.qj[c], c == 0);
     }
-    float diff = __fsub_rn(quad_tree(ai, mask), quad_tree(aj, mask));  // :469
-    float g = bpr_grad(diff), ng = -g, nreg = -reg;
+    return bpr_grad(__fsub_rn(quad_tree(ai, mask), quad_tree(aj, mask)));
+}
+
+// the three row updates of one triple (:477-488), from the rows in registers and the gradient factor g
+template <int C, bool ATOMIC>
+__device__ __forceinline__ void bpr_scatter_rows(const Rows<C> &r, float g, float *Pu, float *Qi, int si, float *Qj, int sj,
+                                                 float lr, float reg)
+{
+    const float4 *p = r.p, *qi = r.qi, *qj = r.qj;
+    const float ng = -g, nreg = -reg;
 #pragma unroll
     for (int c = 0; c < C; c++) {
         float4 t, o;
@@ -105,34 +108,12 @@ __device__ __forceinline__ void bpr_step_rows(const Rows<C> &r, float *Pu, float
     }
 }
 
-// same step, atomic flavour, but the positive (hot) row's delta lr*(g*p - reg*q_i) is returned in dq instead of
-// being issued: the caller sums it over the 8 quads of its warp (all on the same hot row) and issues one red
-template <int C>
-__device__ __forceinline__ void bpr_step_rows_hot(const Rows<C> &r, bool live, float *Pu, float *Qj, int sj, unsigned mask,
-                                                  float lr, float reg, float4 (&dq)[C])
+// one SGD step by a quad on rows already in registers
+template <int C, bool ATOMIC>
+__device__ __forceinline__ void bpr_step_rows(const Rows<C> &r, float *Pu, float *Qi, int si, float *Qj, int sj, unsigned mask,
+                                              float lr, float reg)
 {
-    const float4 *p = r.p, *qi = r.qi, *qj = r.qj;
-#pragma unroll
-    for (int c = 0; c < C; c++) dq[c] = make_float4(0.f, 0.f, 0.f, 0.f);
-    if (!live) return;
-    float4 ai = make_float4(0.f, 0.f, 0.f, 0.f), aj = ai;
-#pragma unroll
-    for (int c = 0; c < C; c++) {
-        dot_chunk(ai, p[c], qi[c], c == 0);
-        dot_chunk(aj, p[c], qj[c], c == 0);
-    }
-    float diff = __fsub_rn(quad_tree(ai, mask), quad_tree(aj, mask));
-    float g = bpr_grad(diff), ng = -g, nreg = -reg;
-#pragma unroll
-    for (int c = 0; c < C; c++) {
-        float4 t, o;
-        GB_F4_OP(t, __fmaf_rn(f4get(qi[c], k_), nreg, __fmul_rn(g, f4get(p[c], k_))));
-        GB_F4_OP(dq[c], __fmul_rn(f4get(t, k_), lr));
-        GB_F4_OP(t, __fmaf_rn(f4get(qj[c], k_), nreg, __fmul_rn(ng, f4get(p[c], k_))));
-        GB_F4_OP(o, __fmul_rn(f4get(t, k_), lr)); red_row(Qj + sj * c, o);
-        GB_F4_OP(t, __fmaf_rn(f4get(p[c], k_), nreg, __fmul_rn(__fsub_rn(f4get(qi[c], k_), f4get(qj[c], k_)), g)));
-        GB_F4_OP(o, __fmul_rn(f4get(t, k_), lr)); red_row(Pu + 16 * c, o);
-    }
+    bpr_scatter_rows<C, ATOMIC>(r, bpr_grad_rows<C>(r, mask), Pu, Qi, si, Qj, sj, lr, reg);
 }
 
 template <int C, bool ATOMIC>
@@ -219,117 +200,9 @@ __device__ __forceinline__ void sample_triple(const BprView &v, uint64_t base, i
     }
 }
 
-// lane-local reference of item row `it` (base, chunk stride in floats): the striped side table while it is live
-__device__ __forceinline__ float *item_ref(const BprView &v, int32_t it, int32_t slot, int lane4, int &stride)
-{
-    if (slot < 0) {
-        stride = 16;
-        return v.Q + (int64_t)it * v.d + 4 * lane4;
-    }
-    stride = 4 * v.hot_pad * GB_HOT_SLOT_FLOATS;
-    return v.hot + ((int64_t)lane4 * v.hot_pad + slot) * GB_HOT_SLOT_FLOATS;
-}
-
-// The capped-concurrency half of the epoch.  Slot h owns k_h quads (a multiple of 8, so every warp serves exactly one
-// hot row); quad r of the slot walks entries b + r, b + r + k_h, ...  The 8 quads of a warp read the hot row with the
-// same addresses (one coalesced request per piece), sum their 8 row deltas with shuffles and issue ONE red per piece:
-// 8x fewer operations on the row's L2 atomic units, which otherwise bound the top item (measured: 16 loads + 16 reds
-// per triple on one striped row sustain only ~2*10^8 updates/s).
-// (Prefetching the user row two rounds ahead into L2 was measured in round 2: 3.770 vs 3.772 ms per C2 epoch, no effect;
-// removed.)
-// (Round 2 also tried to lift the concurrency cap: the instability of round 1 is the row's REGULARISATION applied k_h times
-// per round from stale copies -- k_h*lr*reg reached ~2 where it diverged -- so the shrink was moved to one leader warp per slot
-// that applies (1 - lr*reg)^count to the current value.  That is stable at any cap (100 epochs at 3072, Zipf 1.0 and 1.3), but
-// it buys nothing: 4.21 / 3.81 / 3.87 ms per epoch at cap 768 / 1536 / 3072 against 3.87 ms for this kernel at 768, and the
-// fit gets WORSE with the cap (NDCG@10 0.584 / 0.573 / 0.553 at Zipf 1.0; 0.839 / 0.817 / 0.751 at Zipf 1.3): stale gradients
-// on the head of the popularity distribution cost quality long before they cost stability.  The cap is a quality knob, not
-// only a stability knob; profiles/r02_bpr_hot_cap_sweep.md.  Removed.)
-template <int C>
-__global__ void __launch_bounds__(256) bpr_hot_apply_kernel(BprView v, int n_hot, const unsigned *begin, const unsigned *first_quad,
-                                                            const int32_t *sorted, float lr, float reg)
-{
-    const int lane = threadIdx.x & 31, lane4 = lane & 3;
-    const unsigned mask = quad_mask();
-    const unsigned g = (unsigned)(((size_t)blockIdx.x * blockDim.x + threadIdx.x) >> 2);
-    if (g >= first_quad[n_hot]) return;  // warp-uniform: first_quad entries are multiples of 8
-    int lo = 0, hi = n_hot - 1;  // last slot with first_quad[slot] <= g
-    while (lo < hi) {
-        int mid = (lo + hi + 1) >> 1;
-        if (first_quad[mid] <= g) lo = mid; else hi = mid - 1;
-    }
-    const int slot = lo;
-    const unsigned k = first_quad[slot + 1] - first_quad[slot], r0 = g - first_quad[slot];
-    const unsigned b = begin[slot], e = begin[slot + 1];
-    const int sh = 4 * v.hot_pad * GB_HOT_SLOT_FLOATS;
-    float *Qh = v.hot + ((int64_t)lane4 * v.hot_pad + slot) * GB_HOT_SLOT_FLOATS;
-    // three-deep software pipeline per quad: entry t is computed while the cold rows (p_u, q_j) of entry t+k are in
-    // flight and the (u, j, slot_j) of entry t+2k are being fetched.  The hot row is read just in time.
-    auto fetch_idx = [&](unsigned tt, int32_t &uu, int32_t &jj, int32_t &hh) {
-        uu = -1; jj = 0; hh = -1;
-        if (tt < e) {
-            uu = __ldg(sorted + 2 * (size_t)tt);
-            jj = __ldg(sorted + 2 * (size_t)tt + 1);
-            hh = __ldg(v.hot_slot + jj);
-        }
-    };
-    unsigned t = b + r0;
-    const unsigned t_warp0 = b + (r0 & ~7u);  // entry of the warp's first quad: the warp loops while ANY quad has work
-    int32_t u1, j1, h1, u2, j2, h2;
-    fetch_idx(t, u1, j1, h1);
-    fetch_idx(t + k, u2, j2, h2);
-    Rows<C> r;
-    float *Pu = nullptr, *Qj = nullptr;
-    int sj = 16;
-    bool live = u1 >= 0;
-    if (live) {
-        Pu = v.P + (int64_t)(u1 - v.u_lo) * v.d + 4 * lane4;
-        Qj = item_ref(v, j1, h1, lane4, sj);
-#pragma unroll
-        for (int c = 0; c < C; c++) r.p[c] = ld_row(Pu + 16 * c);
-#pragma unroll
-        for (int c = 0; c < C; c++) r.qj[c] = ld_row(Qj + sj * c);
-    }
-    for (unsigned tw = t_warp0; tw < e; tw += k) {
-        if (live) {
-#pragma unroll
-            for (int c = 0; c < C; c++) r.qi[c] = ld_row(Qh + sh * c);
-        }
-        Rows<C> rn;
-        float *Pun = nullptr, *Qjn = nullptr;
-        int sjn = 16;
-        const bool live_n = u2 >= 0;
-        if (live_n) {
-            Pun = v.P + (int64_t)(u2 - v.u_lo) * v.d + 4 * lane4;
-            Qjn = item_ref(v, j2, h2, lane4, sjn);
-#pragma unroll
-            for (int c = 0; c < C; c++) rn.p[c] = ld_row(Pun + 16 * c);
-#pragma unroll
-            for (int c = 0; c < C; c++) rn.qj[c] = ld_row(Qjn + sjn * c);
-        }
-        int32_t u3, j3, h3;
-        fetch_idx(t + 2 * k, u3, j3, h3);
-        float4 dq[C];
-        bpr_step_rows_hot<C>(r, live, Pu, Qj, sj, mask, lr, reg, dq);
-        __syncwarp();
-#pragma unroll
-        for (int c = 0; c < C; c++) {
-#pragma unroll
-            for (int sft = 4; sft <= 16; sft <<= 1) {
-                dq[c].x += __shfl_xor_sync(0xffffffffu, dq[c].x, sft); dq[c].y += __shfl_xor_sync(0xffffffffu, dq[c].y, sft);
-                dq[c].z += __shfl_xor_sync(0xffffffffu, dq[c].z, sft); dq[c].w += __shfl_xor_sync(0xffffffffu, dq[c].w, sft);
-            }
-            if (lane < 4) red_row(Qh + sh * c, dq[c]);
-        }
-#pragma unroll
-        for (int c = 0; c < C; c++) { r.p[c] = rn.p[c]; r.qj[c] = rn.qj[c]; }
-        t += k; Pu = Pun; Qj = Qjn; sj = sjn; live = live_n;
-        u2 = u3; j2 = j3; h2 = h3;
-    }
-}
-
 // ---- kernels -----------------------------------------------------------------------------------
 template <int C, bool ATOMIC>
-__global__ void __launch_bounds__(256) bpr_epoch_kernel(BprView v, HotQueue hq, int64_t step0, int64_t n_steps, uint64_t base, float lr, float reg)
+__global__ void __launch_bounds__(256) bpr_epoch_kernel(BprView v, int64_t step0, int64_t n_steps, uint64_t base, float lr, float reg)
 {
     const int lane4 = threadIdx.x & 3;
     const unsigned mask = quad_mask();
@@ -339,36 +212,19 @@ __global__ void __launch_bounds__(256) bpr_epoch_kernel(BprView v, HotQueue hq, 
         // software pipeline: the row gathers of step k are in flight while step k+1 is being sampled
         // (its own chain of 2-3 dependent index loads), so one iteration costs one memory round trip
         constexpr int CC = C > 0 ? C : 1;
-        int32_t u = 0, i = 0, j = -1, hi = -1, hj = -1;
-        // a triple whose positive item is hot goes to the hot queue instead of being applied here; hot rows that are
-        // still touched here (as negatives, or when the queue is full) are addressed in the striped side table
-        auto route = [&](int32_t uu, int32_t ii, int32_t &jj, int32_t &si_, int32_t &sj_) {
-            si_ = sj_ = -1;
-            if (v.hot_slot == nullptr || jj < 0) return;
-            si_ = __ldg(v.hot_slot + ii);
-            sj_ = __ldg(v.hot_slot + jj);
-            const bool hot = si_ >= 0;
-            if (hotq_append(hq, hot, lane4, si_, uu, jj) && hot) jj = -1;
-        };
-        if (q < n_steps) {
-            sample_triple(v, base, step0 + q, u, i, j);
-            route(u, i, j, hi, hj);
-        }
+        int32_t u = 0, i = 0, j = -1;
+        if (q < n_steps) sample_triple(v, base, step0 + q, u, i, j);
         while (q < n_steps) {
             Rows<CC> r;
             const bool live = j >= 0;
-            float *Pu = v.P + (int64_t)(u - v.u_lo) * v.d + 4 * lane4;
-            int si = 16, sj = 16;
-            float *Qi = item_ref(v, i, hi, lane4, si), *Qj = item_ref(v, live ? j : 0, hj, lane4, sj);
-            if (live) load_rows<CC>(r, Pu, Qi, si, Qj, sj);
+            float *Pu = v.P + (int64_t)(u - v.u_lo) * v.d + 4 * lane4, *Qi = v.Q + (int64_t)i * v.d + 4 * lane4,
+                  *Qj = v.Q + (int64_t)(live ? j : 0) * v.d + 4 * lane4;
+            if (live) load_rows<CC>(r, Pu, Qi, 16, Qj, 16);
             const int64_t qn = q + nq;
-            int32_t un = 0, in = 0, jn = -1, hin = -1, hjn = -1;
-            if (qn < n_steps) {
-                sample_triple(v, base, step0 + qn, un, in, jn);
-                route(un, in, jn, hin, hjn);
-            }
-            if (live) bpr_step_rows<CC, ATOMIC>(r, Pu, Qi, si, Qj, sj, mask, lr, reg);
-            q = qn; u = un; i = in; j = jn; hi = hin; hj = hjn;
+            int32_t un = 0, in = 0, jn = -1;
+            if (qn < n_steps) sample_triple(v, base, step0 + qn, un, in, jn);
+            if (live) bpr_step_rows<CC, ATOMIC>(r, Pu, Qi, 16, Qj, 16, mask, lr, reg);
+            q = qn; u = un; i = in; j = jn;
         }
     } else {
         for (; q < n_steps; q += nq) {
@@ -378,6 +234,42 @@ __global__ void __launch_bounds__(256) bpr_epoch_kernel(BprView v, HotQueue hq, 
             bpr_step_dispatch<C, ATOMIC>(v.P + (int64_t)(u - v.u_lo) * v.d, v.Q + (int64_t)i * v.d, v.Q + (int64_t)j * v.d,
                                          v.d, lane4, mask, lr, reg);
         }
+    }
+}
+
+// The epoch with atomic scatter, in rounds of one triple per quad of the (co-resident) grid: every triple of a round reads
+// its rows as the previous round left them, a grid-wide barrier separates those reads from the round's additions, and a
+// second one ends the round.  What a triple reads therefore depends only on the step stream and the round size, not on
+// timing; the order of the float additions into a row that several triples of one round update is the only freedom left
+// (rounding).  The round size bounds the staleness of a popular row: at GB_BPR_ROUND triples the most popular item of a
+// Zipf(1) catalogue of 10^5 items takes ~700 updates from one copy per round, lr * reg * 700 << 2.
+template <int C>
+__global__ void __launch_bounds__(256) bpr_round_kernel(BprView v, int64_t step0, int64_t n_steps, uint64_t base, float lr, float reg)
+{
+    namespace cg = cooperative_groups;
+    cg::grid_group grid = cg::this_grid();
+    const int lane4 = threadIdx.x & 3;
+    const unsigned mask = quad_mask();
+    const int64_t q = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 2;
+    const int64_t nq = ((int64_t)gridDim.x * blockDim.x) >> 2;
+    int32_t u = 0, i = 0, j = -1;
+    if (q < n_steps) sample_triple(v, base, step0 + q, u, i, j);
+    for (int64_t r0 = 0; r0 < n_steps; r0 += nq) {
+        const bool live = j >= 0;
+        float *Pu = v.P + (int64_t)(u - v.u_lo) * v.d + 4 * lane4, *Qi = v.Q + (int64_t)i * v.d + 4 * lane4,
+              *Qj = v.Q + (int64_t)(live ? j : 0) * v.d + 4 * lane4;
+        Rows<C> r;
+        float g = 0.f;
+        if (live) {
+            load_rows<C>(r, Pu, Qi, 16, Qj, 16);
+            g = bpr_grad_rows<C>(r, mask);   // consumes every loaded value before the barrier
+        }
+        grid.sync();
+        if (live) bpr_scatter_rows<C, true>(r, g, Pu, Qi, 16, Qj, 16, lr, reg);
+        // the next round's triple (the sampler reads only the immutable CSR) while the additions drain
+        j = -1;
+        if (r0 + nq + q < n_steps) sample_triple(v, base, step0 + r0 + nq + q, u, i, j);
+        grid.sync();
     }
 }
 
@@ -517,11 +409,10 @@ static BprView make_view(gorse_b200_cf *cf)
     v.meta = cf->user_meta.p; v.user_items = cf->user_items.p;
     v.active = cf->all_active ? nullptr : cf->active.p;
     v.n_active = cf->n_active; v.n_items = cf->n_items; v.d = cf->d; v.u_lo = cf->u_lo;
-    v.hot_slot = nullptr; v.hot = nullptr; v.hot_pad = 0;  // the hot path is switched on by bpr_epoch only
     return v;
 }
 
-// grid: persistent, a multiple of the SM count (B200: 148 SMs); 256 threads = 64 quads per CTA
+// grid: persistent, a multiple of the SM count (H100: 132 SMs); 256 threads = 64 quads per CTA
 static int quad_grid(const gorse_b200_ctx *c, int64_t n_quads, int ctas_per_sm)
 {
     int64_t want = (n_quads + 63) / 64;
@@ -530,8 +421,23 @@ static int quad_grid(const gorse_b200_ctx *c, int64_t n_quads, int ctas_per_sm)
     return (int)std::max<int64_t>(1, std::min(want, cap));
 }
 
+template <int C>
+static int32_t launch_round_epoch(gorse_b200_cf *cf, BprView v, int64_t step0, int64_t n, uint64_t base, float lr, float reg)
+{
+    gorse_b200_ctx *c = cf->ctx;
+    auto *k = bpr_round_kernel<C>;
+    int per_sm = 0;
+    GB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k, 256, 0));
+    // the round size is fixed (GB_BPR_ROUND triples) unless the device cannot hold that many quads at once
+    const int g = (int)std::min<int64_t>(GB_BPR_ROUND / 64, (int64_t)per_sm * c->sm_count);
+    if (g < 1) { set_error("bpr_round_kernel does not fit on the device"); return GORSE_B200_ERR_UNSUPPORTED; }
+    void *args[] = {&v, &step0, &n, &base, &lr, &reg};
+    GB_CUDA(cudaLaunchCooperativeKernel((const void *)k, dim3(g), dim3(256), args, 0, c->stream));
+    return GORSE_B200_OK;
+}
+
 template <bool ATOMIC>
-static void launch_epoch(gorse_b200_cf *cf, const BprView &v, const HotQueue &hq, int64_t step0, int64_t n, uint64_t base, float lr, float reg)
+static void launch_epoch(gorse_b200_cf *cf, const BprView &v, int64_t step0, int64_t n, uint64_t base, float lr, float reg)
 {
     gorse_b200_ctx *c = cf->ctx;
     cudaStream_t s = c->stream;
@@ -539,11 +445,11 @@ static void launch_epoch(gorse_b200_cf *cf, const BprView &v, const HotQueue &hq
         int C = cf->d / 16;
         int g = quad_grid(c, n, C <= 4 ? 8 : 4);
         switch (C) {
-            case 1: bpr_epoch_kernel<1, ATOMIC><<<g, 256, 0, s>>>(v, hq, step0, n, base, lr, reg); break;
-            case 2: bpr_epoch_kernel<2, ATOMIC><<<g, 256, 0, s>>>(v, hq, step0, n, base, lr, reg); break;
-            case 4: bpr_epoch_kernel<4, ATOMIC><<<g, 256, 0, s>>>(v, hq, step0, n, base, lr, reg); break;
-            case 8: bpr_epoch_kernel<8, ATOMIC><<<g, 256, 0, s>>>(v, hq, step0, n, base, lr, reg); break;
-            default: bpr_epoch_kernel<0, ATOMIC><<<g, 256, 0, s>>>(v, hq, step0, n, base, lr, reg); break;
+            case 1: bpr_epoch_kernel<1, ATOMIC><<<g, 256, 0, s>>>(v, step0, n, base, lr, reg); break;
+            case 2: bpr_epoch_kernel<2, ATOMIC><<<g, 256, 0, s>>>(v, step0, n, base, lr, reg); break;
+            case 4: bpr_epoch_kernel<4, ATOMIC><<<g, 256, 0, s>>>(v, step0, n, base, lr, reg); break;
+            case 8: bpr_epoch_kernel<8, ATOMIC><<<g, 256, 0, s>>>(v, step0, n, base, lr, reg); break;
+            default: bpr_epoch_kernel<0, ATOMIC><<<g, 256, 0, s>>>(v, step0, n, base, lr, reg); break;
         }
     } else {
         int g = (int)std::max<int64_t>(1, std::min<int64_t>((n + 127) / 128, (int64_t)c->sm_count * 8));
@@ -695,58 +601,19 @@ int32_t gorse_b200_bpr_epoch(gorse_b200_cf *cf, float lr, float reg, int64_t n_s
     if (s1 > s0 && cf->n_active > 0) {
         BprView v = make_view(cf);
         const int C = cf->d / 16;
-        const bool use_hot = cf->n_hot > 0 && cf->d % 16 == 0 && (C == 1 || C == 2 || C == 4 || C == 8) && scatter == GORSE_B200_SCATTER_ATOMIC;
-        HotQueue hq{nullptr, nullptr, 0};
         const int64_t n_local = s1 - s0;
-        if (use_hot) {
-            // queue regions are sized for the whole step stream (worst case: every positive is hot)
-            const int64_t region_cap = (n_local + GB_HOTQ_REGIONS - 1) / GB_HOTQ_REGIONS * 2 + 1024;
-            const size_t need = (size_t)GB_HOTQ_REGIONS * region_cap * 3;
-            if (cf->hotq.n < need) GB_TRY(cf->hotq.alloc(need));
-            if (cf->hot_sorted.n < (size_t)2 * n_local + 2) GB_TRY(cf->hot_sorted.alloc((size_t)2 * n_local + 2));
-            if (cf->hot_ctr.n == 0) GB_TRY(cf->hot_ctr.alloc(GB_HOTQ_REGIONS * 2 + 4 * 1032));
-            GB_CUDA(cudaMemsetAsync(cf->hot_ctr.p, 0, cf->hot_ctr.n * sizeof(unsigned), c->stream));
-            hq.entries = cf->hotq.p;
-            hq.counts = reinterpret_cast<unsigned long long *>(cf->hot_ctr.p);
-            hq.region_cap = region_cap;
-            v.hot_slot = cf->hot_slot.p; v.hot = cf->hot.p; v.hot_pad = cf->hot_pad;
-            hot_gather_kernel<<<div_up((int64_t)cf->n_hot * (cf->d / 4), 256), 256, 0, c->stream>>>(cf->Q.p, cf->d, cf->hot_items.p, cf->n_hot, cf->hot_pad, cf->hot.p);
-            GB_LAUNCHED(c);
+        if (scatter == GORSE_B200_SCATTER_ATOMIC && cf->d % 16 == 0 && (C == 1 || C == 2 || C == 4 || C == 8)) {
+            int32_t st = C == 1 ? launch_round_epoch<1>(cf, v, s0, n_local, mix64(seed), lr, reg)
+                       : C == 2 ? launch_round_epoch<2>(cf, v, s0, n_local, mix64(seed), lr, reg)
+                       : C == 4 ? launch_round_epoch<4>(cf, v, s0, n_local, mix64(seed), lr, reg)
+                                : launch_round_epoch<8>(cf, v, s0, n_local, mix64(seed), lr, reg);
+            if (st) return st;
+        } else if (scatter == GORSE_B200_SCATTER_ATOMIC) {
+            launch_epoch<true>(cf, v, s0, n_local, mix64(seed), lr, reg);
+        } else {
+            launch_epoch<false>(cf, v, s0, n_local, mix64(seed), lr, reg);
         }
-        if (scatter == GORSE_B200_SCATTER_ATOMIC) launch_epoch<true>(cf, v, hq, s0, n_local, mix64(seed), lr, reg);
-        else launch_epoch<false>(cf, v, hq, s0, n_local, mix64(seed), lr, reg);
         GB_LAUNCHED(c);
-        if (use_hot) {
-            unsigned *hist = cf->hot_ctr.p + GB_HOTQ_REGIONS * 2, *begin = hist + 1032, *cursor = begin + 1032, *first_quad = cursor + 1032;
-            const int nh = cf->n_hot;
-            // stale overlapping updates of one row are stable while lr * curvature * overlap stays well below 2;
-            // scale the cap with 1/lr around the measured-safe 512 at the reference's default lr = 0.05
-            unsigned cap = (unsigned)std::min(1024.0f, std::max(32.0f, GB_HOT_ROW_CONCURRENCY * 0.05f / std::max(lr, 1e-6f)));
-            if (const char *e = getenv("GORSE_B200_HOT_ROW_CONCURRENCY")) { int x = atoi(e); if (x > 0) cap = (unsigned)x; }
-            // quad budget: what the machine holds at this kernel's occupancy (2-3 CTAs of 64 quads per SM)
-            const unsigned quad_budget = (unsigned)c->sm_count * 3u * 64u;
-            dim3 sg(std::max(1, c->sm_count / 8), GB_HOTQ_REGIONS);
-            hot_hist_kernel<<<sg, 256, nh * sizeof(unsigned), c->stream>>>(hq, nh, hist);
-            GB_LAUNCHED(c);
-            hot_scan_kernel<<<1, 1024, 0, c->stream>>>(hist, nh, begin, cursor, quad_budget, cap, first_quad);
-            GB_LAUNCHED(c);
-            hot_fill_kernel<<<sg, 256, nh * sizeof(unsigned), c->stream>>>(hq, nh, cursor, cf->hot_sorted.p);
-            GB_LAUNCHED(c);
-            // upper bound of quads in use (the rest exit): hot_scan_kernel gives slot t ceil(share) <= share + 1 quads, then rounds up to
-            // a multiple of 8 (< +8), so sum k_t < quad_budget + 8 * nh
-            const int hg = (int)((quad_budget + 8u * (unsigned)nh + 63u) / 64u);
-            auto *hk = bpr_hot_apply_kernel<1>;
-            switch (C) {
-                case 1: break;
-                case 2: hk = bpr_hot_apply_kernel<2>; break;
-                case 4: hk = bpr_hot_apply_kernel<4>; break;
-                default: hk = bpr_hot_apply_kernel<8>; break;
-            }
-            hk<<<hg, 256, 0, c->stream>>>(v, nh, begin, first_quad, cf->hot_sorted.p, lr, reg);
-            GB_LAUNCHED(c);
-            hot_scatter_kernel<<<div_up((int64_t)cf->n_hot * (cf->d / 4), 256), 256, 0, c->stream>>>(cf->Q.p, cf->d, cf->hot_items.p, cf->n_hot, cf->hot_pad, cf->hot.p);
-            GB_LAUNCHED(c);
-        }
     }
     if (c->world > 1) {
         int64_t n = (int64_t)cf->Q.n;

@@ -201,11 +201,10 @@ int32_t gorse_b200_cf_create(gorse_b200_ctx *ctx, int32_t n_users, int32_t n_ite
     cf->n_active = (int32_t)active.size();
     cf->all_active = cf->n_active == nu;
 
-    // hot items: an item drawn as the positive of more than ~0.02% of an epoch's triples would serialise on one
-    // L2 atomic unit; P(i) is proportional to sum_{u in R_i} 1/|R_u| (user uniform, then item uniform in the row)
-    std::vector<int32_t> hot_items, hot_slot;
+    // multi-GPU exchange: expected updates of item i per local step.  The positive-sampling mass P(i) is proportional to
+    // sum_{u in R_i} 1/|R_u| (user uniform, then item uniform in the row)
     std::vector<float> item_rate;
-    {
+    if (multi) {
         // per-thread partial masses, added in thread order: deterministic for a given thread count
         std::vector<std::vector<double>> part(16);
         parallel_rows(nu, n_fb_local, [&](int32_t r0, int32_t r1, unsigned t) {
@@ -220,24 +219,10 @@ int32_t gorse_b200_cf_create(gorse_b200_ctx *ctx, int32_t n_users, int32_t n_ite
         std::vector<double> mass((size_t)n_items, 0.0);
         for (auto &m : part)
             if (!m.empty()) for (int32_t i = 0; i < n_items; i++) mass[(size_t)i] += m[(size_t)i];
-        const double total = std::max(1, cf->n_active), thresh = 2e-4 * total;
-        std::vector<int32_t> cand;
-        for (int32_t i = 0; i < n_items; i++) if (mass[i] > thresh) cand.push_back(i);
-        std::sort(cand.begin(), cand.end(), [&](int32_t a, int32_t b) { return mass[a] > mass[b] || (mass[a] == mass[b] && a < b); });
-        if (cand.size() > 1024) cand.resize(1024);
-        if (const char *e = getenv("GORSE_B200_NO_HOT")) { if (*e == '1') cand.clear(); }
-        hot_items = cand;
-        if (!hot_items.empty()) {
-            hot_slot.assign((size_t)n_items, -1);
-            for (size_t s = 0; s < hot_items.size(); s++) hot_slot[(size_t)hot_items[s]] = (int32_t)s;
-        }
-        cf->n_hot = (int32_t)hot_items.size();
-        cf->hot_pad = std::max(64, (cf->n_hot + 63) / 64 * 64);
-        if (multi) {
-            // expected updates of item i per local step: P(i is the positive) + P(i is the negative ~ uniform)
-            item_rate.resize((size_t)n_items);
-            for (int32_t i = 0; i < n_items; i++) item_rate[(size_t)i] = (float)(mass[(size_t)i] / total + 1.0 / (double)n_items);
-        }
+        const double total = std::max(1, cf->n_active);
+        // P(i is the positive) + P(i is the negative ~ uniform)
+        item_rate.resize((size_t)n_items);
+        for (int32_t i = 0; i < n_items; i++) item_rate[(size_t)i] = (float)(mass[(size_t)i] / total + 1.0 / (double)n_items);
     }
     if ((st = cf->P.alloc((size_t)nu * n_factors)) != 0) return fail(st);
     if ((st = cf->Q.alloc((size_t)n_items * n_factors)) != 0) return fail(st);
@@ -250,11 +235,6 @@ int32_t gorse_b200_cf_create(gorse_b200_ctx *ctx, int32_t n_users, int32_t n_ite
     if ((st = cf->user_items.alloc((size_t)n_fb_local)) != 0) return fail(st);
     if ((st = cf->active.alloc(active.size())) != 0) return fail(st);
     if ((st = cf->user_meta.alloc((size_t)nu)) != 0) return fail(st);
-    if (cf->n_hot) {
-        if ((st = cf->hot_items.alloc(hot_items.size())) != 0) return fail(st);
-        if ((st = cf->hot_slot.alloc(hot_slot.size())) != 0) return fail(st);
-        if ((st = cf->hot.alloc((size_t)(n_factors / 4 + 1) * cf->hot_pad * 32)) != 0) return fail(st);
-    }
     cudaStream_t s = ctx->stream;
     auto up = [&](void *dst, const void *src, size_t bytes) -> int32_t {
         if (bytes == 0) return GORSE_B200_OK;
@@ -266,10 +246,6 @@ int32_t gorse_b200_cf_create(gorse_b200_ctx *ctx, int32_t n_users, int32_t n_ite
     if ((st = up(cf->active.p, active.data(), sizeof(int32_t) * active.size())) != 0) return fail(st);
     if ((st = up(cf->user_meta.p, meta.data(), sizeof(UserMeta) * meta.size())) != 0) return fail(st);
     if ((st = up(cf->item_rate.p, item_rate.data(), sizeof(float) * item_rate.size())) != 0) return fail(st);
-    if (cf->n_hot) {
-        if ((st = up(cf->hot_items.p, hot_items.data(), sizeof(int32_t) * hot_items.size())) != 0) return fail(st);
-        if ((st = up(cf->hot_slot.p, hot_slot.data(), sizeof(int32_t) * hot_slot.size())) != 0) return fail(st);
-    }
     if (has_items) {
         if ((st = cf->item_off.alloc((size_t)ni + 1)) != 0) return fail(st);
         if ((st = cf->item_users.alloc((size_t)cf->n_item_feedback)) != 0) return fail(st);
@@ -295,7 +271,6 @@ int32_t gorse_b200_cf_destroy(gorse_b200_cf *cf)
     cf->P.free(); cf->Q.free(); cf->Q0.free(); cf->item_rate.free(); cf->xchg.free(); cf->P_all.free();
     cf->user_off.free(); cf->item_off.free();
     cf->user_items.free(); cf->item_users.free(); cf->active.free(); cf->user_meta.free();
-    cf->hot_items.free(); cf->hot_slot.free(); cf->hot.free(); cf->hotq.free(); cf->hot_sorted.free(); cf->hot_ctr.free();
     cf->gram.free(); cf->scratch.free();
     for (int a = 0; a < 2; a++) {
         for (int b = 0; b < 7; b++) cf->als_rows[a][b].free();

@@ -49,12 +49,6 @@ struct gorse_b200_cf {
     gb::DevBuf<int32_t> user_items, item_users, active;
     gb::DevBuf<gb::UserMeta> user_meta;
     bool all_active = false;  // every user of the shard has feedback: active[k] == u_lo + k
-    // hot items (BPR): the head of the popularity distribution, applied with capped per-row concurrency (bpr_hot.cuh)
-    int32_t n_hot = 0, hot_pad = 0;
-    gb::DevBuf<int32_t> hot_items, hot_slot;   // slot -> item (decreasing mass), item -> slot or -1
-    gb::DevBuf<float> hot;                     // striped side table the hot rows live in during an epoch
-    gb::DevBuf<int32_t> hotq, hot_sorted;      // per-epoch queue of (slot, u, j) and its slot-grouped (u, j) form
-    gb::DevBuf<unsigned> hot_ctr;              // queue counters, histogram, scan, cursors, ticket
     // ALS scratch
     gb::DevBuf<float> gram;      // d x d
     gb::DevBuf<float> als_pred;  // eALS scratch: one prediction per entry of the longer CSR side, kept across epochs

@@ -1,5 +1,5 @@
 // common.cuh -- shared plumbing of libgorse_b200.so (error handling, context, device buffers).
-// sm_100a only; no CPU fallback anywhere: every entry point needs a CUDA device.
+// sm_90a only; no CPU fallback anywhere: every entry point needs a CUDA device.
 #pragma once
 #include <cuda_runtime.h>
 #include <nccl.h>
@@ -82,7 +82,7 @@ const NcclApi *nccl();  // nullptr (and last_error set) when libnccl cannot be l
 
 struct gorse_b200_ctx {
     int device = 0;
-    int sm_count = 148;
+    int sm_count = 132;
     int rank = 0, world = 1;
     cudaStream_t stream = nullptr;
     cudaStream_t copy_stream = nullptr;   // result downloads that overlap the next chunk's kernels (topk)

@@ -86,8 +86,8 @@ static int32_t ctx_create_common(int32_t device, gorse_b200_ctx **out)
     GB_CUDA(cudaSetDevice(device));
     cudaDeviceProp prop;
     GB_CUDA(cudaGetDeviceProperties(&prop, device));
-    if (prop.major != 10) {
-        gb::set_error("device %d is sm_%d%d; this library is built for sm_100a (B200) only", device, prop.major,
+    if (prop.major != 9 || prop.minor != 0) {
+        gb::set_error("device %d is sm_%d%d; this library is built for sm_90a (H100) only", device, prop.major,
                       prop.minor);
         return GORSE_B200_ERR_UNSUPPORTED;
     }
@@ -204,7 +204,7 @@ int32_t gorse_b200_ctx_flush_l2(gorse_b200_ctx *ctx)
     GB_CHECK_ARG(ctx != nullptr, "ctx is NULL");
     gb::ScopedDevice sd(ctx->device);
     if (!ctx->flush_buf) {
-        ctx->flush_bytes = (size_t)256 << 20;  // 2x the 126 MB L2
+        ctx->flush_bytes = (size_t)256 << 20;  // 5x the 50 MB L2
         GB_CUDA(cudaMalloc(&ctx->flush_buf, ctx->flush_bytes));
     }
     gb::flush_kernel<<<ctx->sm_count * 4, 256, 0, ctx->stream>>>((float4 *)ctx->flush_buf, ctx->flush_bytes / 16,

@@ -3,7 +3,7 @@
 // master.newCollaborativeFilteringModel would (model/cf/model.go:408-530, 609-775) and print the tables cmd/gorse-bench
 // prints for its other sub-commands (cmd/gorse-bench/main.go:517-555: dataset sizes, then NDCG / Precision / Recall).
 // Plain C++ over the C ABI of libgorse_b200.so -- the calls a Go `benchCFCmd` would make through cgo.  No CPU fallback:
-// without a B200 the fit fails loudly.
+// without an H100 the fit fails loudly.
 //
 //   gorse-bench-cf --train ml-100k.train.rating --test ml-100k.test.negative [--model bpr|als] [--factors 16] [--epochs 100]
 //                  [--lr 0.05] [--reg 0.01] [--alpha 0.001] [--top 10] [--verbose 10] [--seed 0] [--device 0]
@@ -93,7 +93,7 @@ int main(int argc, char **argv)
     p.seed = seed;
 
     gorse_b200_ctx *ctx = nullptr;
-    CHECK(gorse_b200_ctx_create(device, &ctx), "context (this tool needs a B200: there is no CPU fallback)");
+    CHECK(gorse_b200_ctx_create(device, &ctx), "context (this tool needs an H100: there is no CPU fallback)");
     gorse_b200_cf *cf = nullptr;
     auto t0 = std::chrono::steady_clock::now();
     CHECK(gorse_b200_cf_create(ctx, U, I, p.n_factors, tr_off.data(), tr_items.data(), als ? it_off.data() : nullptr, als ? it_users.data() : nullptr, &cf),

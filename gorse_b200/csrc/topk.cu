@@ -3,7 +3,7 @@
 // Two stages share one result contract (k smallest distances, ascending; ties broken by ascending index --
 // the reference's tie order is an artefact of Go's container/heap and is not pinned by any reference test):
 //   stage 1  candidate generation.  Small problems: exact scan (this file).  Large d % 16 == 0 problems:
-//            bf16 tcgen05 GEMM with a fused threshold filter (topk_mma.cu), which over-fetches by a rigorous
+//            bf16 wgmma GEMM with a fused threshold filter (topk_mma.cu), which over-fetches by a rigorous
 //            error margin so the true top-k is always among the candidates.
 //   stage 2  exact re-rank of the candidates with the reference's fp32 summation order
 //            (floats.Euclidean / -floats.Dot, AVX-512 tree), final sort, prune0.

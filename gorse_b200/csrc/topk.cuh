@@ -1,4 +1,4 @@
-// topk.cuh -- brute-force index state shared by topk.cu (exact scan / re-rank) and topk_mma.cu (tcgen05 stage 1).
+// topk.cuh -- brute-force index state shared by topk.cu (exact scan / re-rank) and topk_mma.cu (tensor-core stage 1).
 #pragma once
 #include <cuda_bf16.h>
 

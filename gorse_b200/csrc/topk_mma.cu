@@ -1,12 +1,11 @@
-// topk_mma.cu -- stage 1 of the brute-force search on the 5th-generation tensor cores.
+// topk_mma.cu -- stage 1 of the brute-force search on the Hopper tensor cores.
 //
 //   scores[q][x] = <bf16(q'), bf16(x')>   (q', x' = vectors, for Euclidean augmented so that the score is
 //                                          q.x - |x|^2/2, i.e. larger = closer for both metrics)
-// computed by tcgen05.mma (cta_group::1, kind::f16, M=128, N=128, K=16 per instruction, fp32 accumulators in TMEM),
-// operands staged by TMA (cp.async.bulk.tensor, 128-byte swizzle) through an mbarrier ring.  The N x N score matrix
-// is never written: the epilogue warps read each accumulator tile out of TMEM (tcgen05.ld 32x32b: one thread = one
-// query row) and keep only columns whose score clears a per-row threshold, appending (column, score) to a small
-// per-row candidate list.  Stage 2 (topk.cu) re-ranks the candidates exactly in the reference's fp32 order.
+// computed by wgmma (m64n128k16, bf16 operands, fp32 accumulators in registers), operands staged by TMA
+// (cp.async.bulk.tensor, 128-byte swizzle) through an mbarrier ring.  The N x N score matrix is never written: each consumer
+// warpgroup keeps only the columns whose score clears a per-row threshold, appending (column, score) to a small per-row
+// candidate list.  Stage 2 (topk.cu) re-ranks the candidates exactly in the reference's fp32 order.
 //
 // Threshold without a second pass: the vectors are stored in a random column permutation, so the first m columns are a
 // uniform sample.  For those the epilogue tracks each row's 16 best scores; theta = 16th best - 2*eps is then fixed,
@@ -14,7 +13,7 @@
 //   * soundness: every true top-k element has score >= (k-th best approximate score) - 2*eps  (|score - exact| <= eps,
 //     eps from bf16 rounding: 1.02 * 2^-8 * |q| * max|x| + ...).  Stage 2 verifies that at least k candidates clear
 //     theta + 2*eps, which makes the candidate set a superset of the true top-k; rows that fail the check (or overflow
-//     their list) are redone by the exact scan.  With m = 5N/k and the 16th best, a row fails with probability ~2e-4.
+//     their list) are redone by the exact scan.  With m = 4N/k and the 16th best, a row fails with probability ~1e-6.
 //
 // Roofline class: tensor pipe.  F = 2 * nq * N * Kp flop per sweep.
 #include <cuda.h>
@@ -25,20 +24,22 @@
 
 #include "cf.cuh"
 #include "topk.cuh"
-#include "umma.cuh"
+#include "wgmma.cuh"
 
 namespace gb {
 namespace mma {
 
-constexpr int BM = 128, BN = 128, BK = 64;     // tile rows (queries), tile columns (vectors), k-block (bf16 elements)
-constexpr int TILES_M = 2;                     // query tiles per CTA (both multiply every B tile)
+constexpr int BM = 64, BN = 128, BK = 64;      // rows per consumer warpgroup (queries), tile columns (vectors), k-block (bf16)
+constexpr int CONSUMERS = 2;                   // consumer warpgroups per CTA; both multiply every B tile
+constexpr int GROUP_ROWS = CONSUMERS * BM;     // query rows of one CTA pass over all vectors
 constexpr int MAX_KB = 3;                      // k-blocks per tile: Kp <= 192
 constexpr int CAP = 2048;                      // candidate slots per query row
+constexpr int PARTS = 4;                       // a row's columns are split over the 4 threads of an accumulator quad
+constexpr int PART_CAP = CAP / PARTS;          // candidate slots per (row, part)
 constexpr int R_TOP = 16;                      // sample order statistic that fixes the threshold
-constexpr int EPI_WARPS = 16;                  // 2 query tiles x 4 lane quarters x 2 column halves
-constexpr int HALF_CAP = CAP / 2;              // candidate slots per (row, column half)
-constexpr int THREADS = 128 + 32 * EPI_WARPS;  // warp 0 TMA, 1 MMA, 2 TMEM alloc, 3 idle, 4..19 epilogue
-constexpr uint32_t TILE_BYTES = BM * BK * 2;   // one [128 x 64] bf16 k-block tile = 16 KB
+constexpr int THREADS = 128 * (1 + CONSUMERS); // warpgroup 0: warp 0 = TMA producer, warps 1-3 idle; then the consumers
+constexpr uint32_t A_TILE_BYTES = BM * BK * 2; // one [64 x 64] bf16 k-block of queries = 8 KB
+constexpr uint32_t B_TILE_BYTES = BN * BK * 2; // one [128 x 64] bf16 k-block of vectors = 16 KB
 
 struct Params {
     int64_t n;            // real vectors
@@ -46,289 +47,222 @@ struct Params {
     int32_t m_tiles;      // sample tiles (the sweep revisits them at the end)
     int32_t kb;           // k-blocks (Kp / 64)
     int64_t nq;           // real query rows of this launch
-    int32_t n_groups;     // ceil(nq / 256)
+    int32_t n_groups;     // ceil(nq / GROUP_ROWS)
     const float *eps;     // [nq] error margin per query row
     int32_t *cand_col;    // [nq][CAP] permuted column index
     float *cand_val;      // [nq][CAP]
-    int32_t *cand_cnt;    // [nq][2] pushes per column half (may exceed HALF_CAP)
-    float *theta;         // [nq][2] threshold used by each half
+    int32_t *cand_cnt;    // [nq][PARTS] pushes per part (may exceed PART_CAP)
+    float *theta;         // [nq][PARTS] threshold used by each part
     float *dbg;           // optional dense [nq][n_tiles*128] score dump (tests)
 };
 
-// instruction descriptor: D fp32 (bits 4-5 = 1), A/B bf16 (bits 7-9, 10-12 = 1), K-major both, N>>3 at 17, M>>4 at 24
-constexpr uint32_t IDESC = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(BN >> 3) << 17) | ((uint32_t)(BM >> 4) << 24);
-
-// three-input max (Blackwell FMNMX3)
-__device__ __forceinline__ float max3(float a, float b, float c)
-{
-    float r;
-    asm("max.f32 %0, %1, %2, %3;" : "=f"(r) : "f"(a), "f"(b), "f"(c));
-    return r;
-}
-// (An epilogue testing 8 columns per branch with a 3-input max tree was measured in round 2: stage-1 fraction 0.515 vs
-// 0.565 with 4 columns per branch; removed.)
-// Round 2, what bounds this kernel (profiles/r02_topk_epilogue.md): NOT the epilogue's instruction count as round 1 read it
-// (a 3x lighter instruction stream changed nothing) and not the operand traffic of the MMAs (query tiles in tensor memory,
-// the "TS" form, were slower: one accumulator per tile instead of two stages).  A stage's accumulators are released when the
-// SLOWEST of the 16 epilogue warps is done, and what made warps slow was the push of the rare columns that clear the
-// threshold: ~1 hit per warp and 32-column batch on average, so per tile step SOME warp nearly always runs the push code
-// (divergent 4-column blocks in round 1, a shared-memory transpose + ballots, then a per-lane bit mask in round 2: ~100+
-// instructions at ~9 cycles each with 5 warps per scheduler), and the other 15 spin on t_full (12-20 % of all stall samples
-// sit on that one branch).  So: (1) both 32-column batches of a step are loaded into registers and the stage is released
-// BEFORE they are examined -- a warp with hits delays only itself, and the two accumulator stages average its load out;
-// (2) one 16-instruction max tree per 32 columns; a lane whose maximum clears theta walks back down the tree (4 + 3 + 3
-// compares for the usual single hit) and pushes into its own row's list, no cross-lane step (a 32-bit hit mask + scores
-// parked in local memory cost ~125 instructions per hitting batch: more than the 1024-cycle MMA of a step); (3) the two halves
-// of a row merge their sample lists into ONE threshold, which halves the candidates (and ends the list overflows that sent
-// ~35 rows per call to the exact fallback).
+// One CTA: a producer warp streams the vector tiles through a STAGES-deep ring (and the group's query tiles once per group);
+// each consumer warpgroup multiplies its 64 query rows with every tile (8 or fewer wgmma, K = 16 each, into one 64 x 128
+// accumulator), waits, hands the ring slot back and examines the scores in registers.  The two consumers meet on the same
+// slots, so the tensor core runs one warpgroup's MMAs while the other examines its scores.
+// Accumulator fragment (wgmma.cuh): a thread holds 2 rows x 32 columns of a tile, and the 4 threads of a quad share their
+// rows; a (row, quad lane) pair is a PART with its own sample, candidate list and push count.  The 4 parts of a row merge
+// their 16 best into ONE threshold by shuffles.
 template <int STAGES, bool DBG>
 __global__ void __launch_bounds__(THREADS, 1)
 topk_mma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b, Params P)
 {
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-    uint8_t *smem_a = smem;                                              // [TILES_M][kb] tiles
-    uint8_t *smem_b = smem_a + (size_t)TILES_M * P.kb * TILE_BYTES;      // [STAGES][kb] tiles
-    uint64_t *bars = reinterpret_cast<uint64_t *>(smem_b + (size_t)STAGES * P.kb * TILE_BYTES);
+    uint8_t *smem_a = smem;                                                  // [CONSUMERS][kb] query tiles
+    uint8_t *smem_b = smem_a + (size_t)CONSUMERS * P.kb * A_TILE_BYTES;      // [STAGES][kb] vector tiles
+    uint64_t *bars = reinterpret_cast<uint64_t *>(smem_b + (size_t)STAGES * P.kb * B_TILE_BYTES);
     uint64_t *full = bars, *empty = bars + STAGES, *a_full = bars + 2 * STAGES, *a_empty = a_full + 1;
-    uint64_t *t_full = a_empty + 1, *t_empty = t_full + 4;   // one pair per accumulator (tile m, stage as): index m * 2 + as
-    uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(t_empty + 4);
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    if (warp == 0 && lane == 0) {
-        for (int s = 0; s < STAGES; s++) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
+    if (threadIdx.x == 0) {
+        // a slot / the query tiles are free again once every consumer WARP has waited for its MMAs
+        for (int s = 0; s < STAGES; s++) { mbar_init(&full[s], 1); mbar_init(&empty[s], CONSUMERS * 4); }
         mbar_init(a_full, 1);
-        mbar_init(a_empty, 1);
-        for (int s = 0; s < 4; s++) { mbar_init(&t_full[s], 1); mbar_init(&t_empty[s], EPI_WARPS / TILES_M); }
+        mbar_init(a_empty, CONSUMERS * 4);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 2) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(s32(tmem_slot)), "r"(512u) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem_base = *tmem_slot;
     const int total_tiles = P.n_tiles + P.m_tiles;
 
     if (warp == 0) {
-        // ===== TMA producer: the warp waits together, one elected lane issues (see the MMA warp for why not `lane == 0`)
-        {
-            uint32_t it = 0, ag = 0;
-            for (int g = blockIdx.x; g < P.n_groups; g += gridDim.x, ag++) {
-                mbar_wait_backoff(a_empty, (ag & 1) ^ 1);  // MMA of the previous group no longer reads A
-                if (elect_one()) {
-                    mbar_expect_tx(a_full, (uint32_t)TILES_M * P.kb * TILE_BYTES);
-                    for (int m = 0; m < TILES_M; m++)
-                        for (int kb = 0; kb < P.kb; kb++)
-                            tma_load_2d(smem_a + ((size_t)m * P.kb + kb) * TILE_BYTES, &map_a, kb * BK, (g * TILES_M + m) * BM, a_full);
-                }
-                __syncwarp();
-                for (int t = 0; t < total_tiles; t++, it++) {
-                    const int s = it % STAGES;
-                    mbar_wait_backoff(&empty[s], ((it / STAGES) & 1) ^ 1);
-                    if (elect_one()) {
-                        mbar_expect_tx(&full[s], (uint32_t)P.kb * TILE_BYTES);
-                        const int bt = t < P.n_tiles ? t : t - P.n_tiles;
-                        for (int kb = 0; kb < P.kb; kb++)
-                            tma_load_2d(smem_b + ((size_t)s * P.kb + kb) * TILE_BYTES, &map_b, kb * BK, bt * BN, &full[s]);
-                    }
-                    __syncwarp();
-                }
+        // ===== TMA producer: the warp waits together, one elected lane issues
+        uint32_t it = 0, ag = 0;
+        for (int g = blockIdx.x; g < P.n_groups; g += gridDim.x, ag++) {
+            mbar_wait_backoff(a_empty, (ag & 1) ^ 1);  // MMAs of the previous group no longer read the query tiles
+            if (elect_one()) {
+                mbar_expect_tx(a_full, (uint32_t)CONSUMERS * P.kb * A_TILE_BYTES);
+                for (int m = 0; m < CONSUMERS; m++)
+                    for (int kb = 0; kb < P.kb; kb++)
+                        tma_load_2d(smem_a + ((size_t)m * P.kb + kb) * A_TILE_BYTES, &map_a, kb * BK, (g * CONSUMERS + m) * BM, a_full);
             }
-        }
-    } else if (warp == 1) {
-        // ===== MMA issuer (one thread) =====
-        // This thread's instruction stream is the pace of the whole kernel when it is long: round 1 rebuilt both 64-bit
-        // shared-memory descriptors from generic pointers for every MMA (341 instructions per tile step, one warp, ~6.7
-        // cycles each = 2300 cycles against 1084 cycles of tensor work: the "48 % tensor pipe" plateau that no epilogue
-        // change moved, profiles/r02_topk_epilogue.md).  The descriptors differ only in the 14-bit address field: one add each.
-        // The whole warp runs the loop and the waits; one ELECTED lane issues (the compiler knows an elect.sync predicate
-        // selects exactly one thread and keeps the descriptor arithmetic on the uniform datapath; behind `lane == 0` it
-        // wrapped every MMA in a loop over the active lanes).
-        {
-            const uint64_t da = umma_desc(smem_a, 0), db = umma_desc(smem_b, 0);
-            const uint32_t a_hi = (uint32_t)(da >> 32), b_hi = (uint32_t)(db >> 32), a_lo0 = (uint32_t)da, b_lo0 = (uint32_t)db;
-            constexpr uint32_t TILE16 = TILE_BYTES >> 4;          // descriptor address units are 16 bytes
-            const uint32_t stage16 = (uint32_t)P.kb * TILE16;
-            auto desc = [](uint32_t lo, uint32_t hi) {
-                uint64_t d;
-                asm("mov.b64 %0, {%1, %2};" : "=l"(d) : "r"(lo), "r"(hi));
-                return d;
-            };
-            uint32_t it = 0, ag = 0, at = 0;
-            for (int g = blockIdx.x; g < P.n_groups; g += gridDim.x, ag++) {
-                mbar_wait_backoff(a_full, ag & 1);
-                for (int t = 0; t < total_tiles; t++, it++, at++) {
-                    const uint32_t s = it % STAGES, as = at & 1;
-                    mbar_wait(&full[s], (it / STAGES) & 1);
-                    const uint32_t b_lo = b_lo0 + s * stage16;
-#pragma unroll
-                    for (int m = 0; m < TILES_M; m++) {
-                        // hand-off per ACCUMULATOR, not per pair: an accumulator is refilled every 2 steps, and from the commit of
-                        // its MMAs to the first MMA of the refill (commit -> epilogue wakes -> tcgen05.ld -> arrive -> this warp
-                        // wakes -> issue -> tensor pipe) ~1300 cycles pass (tools/micro/umma_pipe.cu).  With one barrier per
-                        // stage that latency followed 1024 cycles of MMAs of both tiles (budget 2048: period 1175+); per
-                        // accumulator it follows 512.
-                        mbar_wait(&t_empty[m * 2 + as], ((at >> 1) & 1) ^ 1);
-                        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                        if (elect_one()) {
-                            const uint32_t d = tmem_base + (uint32_t)((m * 2 + as) * BN);
-                            const uint32_t a_lo = a_lo0 + (uint32_t)m * stage16;
-                            for (uint32_t kb = 0; kb < (uint32_t)P.kb; kb++) {
-#pragma unroll
-                                for (uint32_t k = 0; k < BK / 16; k++) {   // 16 bf16 = 32 bytes = 2 address units along K
-                                    const uint32_t off = kb * TILE16 + k * 2;
-                                    umma_bf16(d, desc(a_lo + off, a_hi), desc(b_lo + off, b_hi), IDESC, (kb | k) != 0);
-                                }
-                            }
-                            if (m == TILES_M - 1) umma_commit(&empty[s]);      // B stage reusable once these MMAs retire
-                            umma_commit(&t_full[m * 2 + as]);
-                        }
-                        __syncwarp();
-                    }
-                    __syncwarp();
+            __syncwarp();
+            for (int t = 0; t < total_tiles; t++, it++) {
+                const int s = it % STAGES;
+                mbar_wait_backoff(&empty[s], ((it / STAGES) & 1) ^ 1);
+                if (elect_one()) {
+                    mbar_expect_tx(&full[s], (uint32_t)P.kb * B_TILE_BYTES);
+                    const int bt = t < P.n_tiles ? t : t - P.n_tiles;
+                    for (int kb = 0; kb < P.kb; kb++)
+                        tma_load_2d(smem_b + ((size_t)s * P.kb + kb) * B_TILE_BYTES, &map_b, kb * BK, bt * BN, &full[s]);
                 }
-                if (elect_one()) umma_commit(a_empty);
                 __syncwarp();
             }
         }
     } else if (warp >= 4) {
-        // ===== epilogue: 16 warps = 2 query tiles x 4 lane quarters x 2 column halves.  A (row, half) pair is one thread:
-        // it samples and pushes on its own 64 of every 128 columns.  The two halves of a row meet once per group, after the
-        // sample, to merge their 16 best into one threshold (through the row's still empty candidate lists).
-        const int ew = warp - 4, m = ew >> 3, half = (ew >> 2) & 1;
-        // a warp may only touch its own 32 TMEM lanes (bits 16+); its columns are half a tile of accumulator m
-        const uint32_t acc0 = tmem_base + ((uint32_t)((ew & 3) * 32) << 16) + (uint32_t)(m * 2 * BN + half * (BN / 2));
-        uint32_t at = 0;
-        auto release = [&](int as) {      // the accumulators of stage `as` are in registers: hand the stage back to the MMA warp
-            asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&t_empty[m * 2 + as]);
-        };
-        for (int g = blockIdx.x; g < P.n_groups; g += gridDim.x) {
-            const int64_t row = (int64_t)(g * TILES_M + m) * BM + (ew & 3) * 32 + lane;
-            const bool row_ok = row < P.nq;
-            int32_t *ccol = P.cand_col + (row_ok ? row : 0) * CAP + half * HALF_CAP;
-            float *cval = P.cand_val + (row_ok ? row : 0) * CAP + half * HALF_CAP;
-            [[maybe_unused]] auto dump = [&](const uint32_t (&v)[32], int64_t col0) {
-                if (P.dbg && row_ok) {
+        // ===== consumer warpgroup wg: query rows [(g * CONSUMERS + wg) * 64, +64)
+        const int wg = (warp >> 2) - 1, quad = lane & 3;
+        const uint32_t a_base = s32(smem_a) + (uint32_t)wg * (uint32_t)P.kb * A_TILE_BYTES, b_base = s32(smem_b);
+        float acc[64];
+        // the MMAs of one ring slot into acc, then the slot goes back to the producer
+        auto mma_tile = [&](uint32_t s) {
+            const uint32_t b_slot = b_base + s * (uint32_t)P.kb * B_TILE_BYTES;
+            wgmma_fence();
+            for (int kb = 0; kb < P.kb; kb++) {
 #pragma unroll
-                    for (int e = 0; e < 32; e++) P.dbg[row * ((int64_t)P.n_tiles * BN) + col0 + e] = __uint_as_float(v[e]);
+                for (int k = 0; k < BK / 16; k++) {   // 16 bf16 = 32 bytes along the 128-byte row
+                    const uint32_t off = (uint32_t)k * 32u;
+                    wgmma_m64n128k16_bf16(acc, wgmma_desc(a_base + (uint32_t)kb * A_TILE_BYTES + off),
+                                          wgmma_desc(b_slot + (uint32_t)kb * B_TILE_BYTES + off), (kb | k) != 0);
+                }
+            }
+            wgmma_commit();
+            wgmma_wait<0>();
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&empty[s]);
+        };
+        uint32_t it = 0, ag = 0;
+        for (int g = blockIdx.x; g < P.n_groups; g += gridDim.x, ag++) {
+            int64_t row[2];
+            bool row_ok[2];
+            row[0] = (int64_t)(g * CONSUMERS + wg) * BM + (warp & 3) * 16 + (lane >> 2);
+            row[1] = row[0] + 8;
+            row_ok[0] = row[0] < P.nq;
+            row_ok[1] = row[1] < P.nq;
+            [[maybe_unused]] auto dump = [&](int64_t col0) {
+                if (P.dbg) {
+                    const int64_t ld = (int64_t)P.n_tiles * BN;
+#pragma unroll
+                    for (int h = 0; h < 2; h++)
+                        if (row_ok[h]) {
+#pragma unroll
+                            for (int j = 0; j < BN / 8; j++) {
+                                P.dbg[row[h] * ld + col0 + 8 * j] = acc[4 * j + 2 * h];
+                                P.dbg[row[h] * ld + col0 + 8 * j + 1] = acc[4 * j + 2 * h + 1];
+                            }
+                        }
                 }
             };
-            float theta;
+            mbar_wait(a_full, ag & 1);
+            float theta[2];
             {
-                // ---- the sample: the R_TOP best scores of the first m_tiles tiles
-                float top[R_TOP];
+                // ---- the sample: each part's R_TOP best scores of the first m_tiles tiles
+                float top[2][R_TOP];
 #pragma unroll
-                for (int r = 0; r < R_TOP; r++) top[r] = -INFINITY;
-                auto insert = [&](float cur) {   // into the sorted 16 best
+                for (int h = 0; h < 2; h++)
+#pragma unroll
+                    for (int r = 0; r < R_TOP; r++) top[h][r] = -INFINITY;
+                auto insert = [&](int h, float cur) {   // into the sorted 16 best
 #pragma unroll
                     for (int r = 0; r < R_TOP; r++) {
-                        const float hi = fmaxf(top[r], cur);
-                        cur = fminf(top[r], cur);
-                        top[r] = hi;
+                        const float hi = fmaxf(top[h][r], cur);
+                        cur = fminf(top[h][r], cur);
+                        top[h][r] = hi;
                     }
                 };
-                for (int t = 0; t < P.m_tiles; t++, at++) {
-                    const int as = at & 1;
-                    mbar_wait(&t_full[m * 2 + as], (at >> 1) & 1);
-                    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-#pragma unroll 1
-                    for (int c0 = 0; c0 < BN / 2; c0 += 32) {
-                        uint32_t v[32];
-                        tmem_ld32(acc0 + (uint32_t)(as * BN + c0), v);
-                        const int64_t col0 = (int64_t)t * BN + half * (BN / 2) + c0;
-                        if constexpr (DBG) dump(v, col0);
+                for (int t = 0; t < P.m_tiles; t++, it++) {
+                    const uint32_t s = it % STAGES;
+                    mbar_wait(&full[s], (it / STAGES) & 1);
+                    mma_tile(s);
+                    const int64_t col0 = (int64_t)t * BN + 2 * quad;
+                    if constexpr (DBG) dump(col0);
 #pragma unroll
-                        for (int e = 0; e < 32; e++) {
-                            const float x = __uint_as_float(v[e]);
-                            if (x > top[R_TOP - 1] && col0 + e < P.n) insert(x);   // rare after the first few hundred columns
-                        }
-                        __syncwarp();   // tcgen05.ld is warp-collective: reconverge after the data-dependent code
+                    for (int j = 0; j < BN / 8; j++)
+#pragma unroll
+                        for (int e = 0; e < 2; e++)
+#pragma unroll
+                            for (int h = 0; h < 2; h++) {
+                                const float x = acc[4 * j + 2 * h + e];
+                                if (x > top[h][R_TOP - 1] && col0 + 8 * j + e < P.n) insert(h, x);   // rare after the first columns
+                            }
+                }
+                // ---- one threshold per row: merge the 16 best of the quad's 4 parts (butterfly over lane ^ 1, lane ^ 2;
+                // every lane ends with the same 16 values).  Two sorted lists merge as a bitonic sequence: max(a[r], b[15-r])
+                // holds the 16 best of both, and four half-cleaner steps sort it.
+#pragma unroll
+                for (int x = 1; x <= 2; x <<= 1)
+#pragma unroll
+                    for (int h = 0; h < 2; h++) {
+                        float c[R_TOP];
+#pragma unroll
+                        for (int r = 0; r < R_TOP; r++) c[r] = fmaxf(top[h][r], __shfl_xor_sync(0xffffffffu, top[h][R_TOP - 1 - r], x));
+#pragma unroll
+                        for (int w = R_TOP / 2; w; w >>= 1)
+#pragma unroll
+                            for (int r = 0; r < R_TOP; r++)
+                                if ((r & w) == 0) {
+                                    const float hi = fmaxf(c[r], c[r + w]);
+                                    c[r + w] = fminf(c[r], c[r + w]);
+                                    c[r] = hi;
+                                }
+#pragma unroll
+                        for (int r = 0; r < R_TOP; r++) top[h][r] = c[r];
                     }
-                    release(as);
-                }
-                // ---- one threshold per row: merge the other half's 16 best (it sits in the row's other candidate list)
-                if (row_ok) {
 #pragma unroll
-                    for (int r = 0; r < R_TOP; r++) cval[r] = top[r];
-                }
-                asm volatile("bar.sync 1, %0;" ::"n"(32 * EPI_WARPS) : "memory");
-                if (row_ok) {
-                    const float *other = P.cand_val + row * CAP + (1 - half) * HALF_CAP;
-                    float o[R_TOP];
-#pragma unroll
-                    for (int r = 0; r < R_TOP; r++) o[r] = other[r];
-#pragma unroll 1
-                    for (int r = 0; r < R_TOP; r++) {
-                        float cur = o[0];
-#pragma unroll
-                        for (int q = 0; q + 1 < R_TOP; q++) o[q] = o[q + 1];
-                        if (cur > top[R_TOP - 1]) insert(cur);
-                    }
-                }
-                asm volatile("bar.sync 1, %0;" ::"n"(32 * EPI_WARPS) : "memory");   // lists are free for the pushes from here
-                theta = row_ok ? top[R_TOP - 1] - 2.f * P.eps[row] : INFINITY;   // padding rows never hit
+                for (int h = 0; h < 2; h++) theta[h] = row_ok[h] ? top[h][R_TOP - 1] - 2.f * P.eps[row[h]] : INFINITY;   // padding rows never hit
             }
-            // ---- the sweep: every column at or above theta goes to the row's list
-            int cnt = 0;
-            auto hits = [&](const uint32_t (&v)[32], int64_t col0) {
-                // a 3-input max tree over the 32 scores (16 instructions, depth 4); only a lane whose maximum clears theta
-                // (~1.5 % of them) walks back down the tree to the columns that did: ~30 instructions for the usual single hit
-#define GB_F(i) __uint_as_float(v[i])
-                const float a0 = max3(GB_F(0), GB_F(1), GB_F(2)), a1 = max3(GB_F(3), GB_F(4), GB_F(5)), a2 = max3(GB_F(6), GB_F(7), GB_F(8)),
-                            a3 = max3(GB_F(9), GB_F(10), GB_F(11)), a4 = max3(GB_F(12), GB_F(13), GB_F(14)),
-                            a5 = max3(GB_F(15), GB_F(16), GB_F(17)), a6 = max3(GB_F(18), GB_F(19), GB_F(20)),
-                            a7 = max3(GB_F(21), GB_F(22), GB_F(23)), a8 = max3(GB_F(24), GB_F(25), GB_F(26)),
-                            a9 = max3(GB_F(27), GB_F(28), GB_F(29));
-                const float b0 = max3(a0, a1, a2), b1 = max3(a3, a4, a5), b2 = max3(a6, a7, a8), b3 = max3(a9, GB_F(30), GB_F(31));
-                if (fmaxf(max3(b0, b1, b2), b3) >= theta) {
-                    const int32_t c32 = (int32_t)col0;
-                    const int lim = (int)min((int64_t)32, P.n - col0);   // real columns in this batch (padding only in the last tile)
-#define GB_PUSH(e)                                                                                     \
-    if (GB_F(e) >= theta && e < lim) {                                                                 \
-        if (cnt < HALF_CAP) { ccol[cnt] = c32 + e; cval[cnt] = GB_F(e); }                             \
-        cnt++;                                                                                         \
-    }
-#define GB_PUSH3(a, e) if (a >= theta) { GB_PUSH(e) GB_PUSH(e + 1) GB_PUSH(e + 2) }
-                    if (b0 >= theta) { GB_PUSH3(a0, 0) GB_PUSH3(a1, 3) GB_PUSH3(a2, 6) }
-                    if (b1 >= theta) { GB_PUSH3(a3, 9) GB_PUSH3(a4, 12) GB_PUSH3(a5, 15) }
-                    if (b2 >= theta) { GB_PUSH3(a6, 18) GB_PUSH3(a7, 21) GB_PUSH3(a8, 24) }
-                    if (b3 >= theta) { GB_PUSH3(a9, 27) GB_PUSH(30) GB_PUSH(31) }
-#undef GB_PUSH3
-#undef GB_PUSH
-                }
-#undef GB_F
-            };
-            for (int t = P.m_tiles; t < total_tiles; t++, at++) {
-                const int as = at & 1;
+            // ---- the sweep: every column at or above theta goes to the part's list
+            int cnt[2] = {0, 0};
+            int32_t *ccol[2];
+            float *cval[2];
+#pragma unroll
+            for (int h = 0; h < 2; h++) {
+                const int64_t base = (row_ok[h] ? row[h] : 0) * CAP + quad * PART_CAP;
+                ccol[h] = P.cand_col + base;
+                cval[h] = P.cand_val + base;
+            }
+            for (int t = P.m_tiles; t < total_tiles; t++, it++) {
+                const uint32_t s = it % STAGES;
                 const int bt = t < P.n_tiles ? t : t - P.n_tiles;
-                mbar_wait(&t_full[m * 2 + as], (at >> 1) & 1);
-                asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                // both batches into registers, then the stage goes back BEFORE they are looked at: a warp that has hits to
-                // push delays only itself, not the 15 others and the tensor pipe (see the note above the kernel)
-                uint32_t v0[32], v1[32];
-                tmem_ld32_issue(acc0 + (uint32_t)(as * BN), v0);
-                tmem_ld32_issue(acc0 + (uint32_t)(as * BN + 32), v1);
-                tmem_ld_wait();
-                release(as);
-                const int64_t col0 = (int64_t)bt * BN + half * (BN / 2);
+                mbar_wait(&full[s], (it / STAGES) & 1);
+                mma_tile(s);
+                const int64_t col0 = (int64_t)bt * BN + 2 * quad;
                 if constexpr (DBG) {
-                    if (t < P.n_tiles) { dump(v0, col0); dump(v1, col0 + 32); }
+                    if (t < P.n_tiles) dump(col0);
                 }
-                hits(v0, col0);
-                hits(v1, col0 + 32);
-                __syncwarp();   // tcgen05.ld is warp-collective: reconverge after the data-dependent code
+#pragma unroll
+                for (int h = 0; h < 2; h++) {
+                    // a max tree over the part's 32 scores; only a part whose maximum clears theta (~1 % of them) walks the
+                    // columns and pushes the ones that do
+                    float m0 = -INFINITY, m1 = -INFINITY, m2 = -INFINITY, m3 = -INFINITY;   // 4 independent chains
+#pragma unroll
+                    for (int j = 0; j < BN / 8; j += 2) {
+                        m0 = fmaxf(m0, acc[4 * j + 2 * h]);
+                        m1 = fmaxf(m1, acc[4 * j + 2 * h + 1]);
+                        m2 = fmaxf(m2, acc[4 * j + 4 + 2 * h]);
+                        m3 = fmaxf(m3, acc[4 * j + 4 + 2 * h + 1]);
+                    }
+                    if (fmaxf(fmaxf(m0, m1), fmaxf(m2, m3)) >= theta[h]) {
+#pragma unroll
+                        for (int j = 0; j < BN / 8; j++)
+#pragma unroll
+                            for (int e = 0; e < 2; e++) {
+                                const float x = acc[4 * j + 2 * h + e];
+                                const int64_t col = col0 + 8 * j + e;
+                                if (x >= theta[h] && col < P.n) {   // padding columns only in the last tile
+                                    if (cnt[h] < PART_CAP) { ccol[h][cnt[h]] = (int32_t)col; cval[h][cnt[h]] = x; }
+                                    cnt[h]++;
+                                }
+                            }
+                    }
+                }
             }
-            if (row_ok) { P.cand_cnt[2 * row + half] = cnt; P.theta[2 * row + half] = theta; }
+#pragma unroll
+            for (int h = 0; h < 2; h++)
+                if (row_ok[h]) { P.cand_cnt[PARTS * row[h] + quad] = cnt[h]; P.theta[PARTS * row[h] + quad] = theta[h]; }
+            __syncwarp();
+            if (lane == 0) mbar_arrive(a_empty);   // this warp's MMAs of the group have all been waited for
         }
-    }
-    __syncthreads();
-    if (warp == 2) {
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512u) : "memory");
     }
 }
 
@@ -432,17 +366,28 @@ prune_kernel(const int32_t *cand_col, const float *cand_val, const int32_t *cand
     uint32_t *sk = reinterpret_cast<uint32_t *>(sm) + (size_t)warp * mma::CAP;                                          // keys
     int32_t *sc = reinterpret_cast<int32_t *>(reinterpret_cast<uint32_t *>(sm) + (size_t)nw * mma::CAP) + (size_t)warp * mma::CAP;  // ids
     for (int64_t row = (int64_t)blockIdx.x * nw + warp; row < nq; row += (int64_t)gridDim.x * nw) {
-        const int raw0 = cand_cnt[2 * row], raw1 = cand_cnt[2 * row + 1];
-        const int n0 = min(raw0, mma::HALF_CAP), n1 = min(raw1, mma::HALF_CAP);
-        // every column with score >= max(theta_0, theta_1) was pushed by one of the two halves
-        const float th = fmaxf(theta[2 * row], theta[2 * row + 1]);
+        // every column with score >= max over the parts' thresholds was pushed by one of the parts
+        int np[mma::PARTS], n = 0;
+        float th = -INFINITY;
+        bool bad = !(eps[row] == eps[row]);
+#pragma unroll
+        for (int p = 0; p < mma::PARTS; p++) {
+            const int raw = cand_cnt[mma::PARTS * row + p];
+            bad |= raw > mma::PART_CAP;
+            np[p] = min(raw, mma::PART_CAP);
+            n += np[p];
+            th = fmaxf(th, theta[mma::PARTS * row + p]);
+        }
+        if (!(th == th)) bad = true;
         int32_t *oi = out_ids + row * mma::CAP;
         const int64_t self = self_skip ? (q_idx ? q_idx[row] : q0 + row) : -1;
-        bool bad = raw0 > mma::HALF_CAP || raw1 > mma::HALF_CAP || !(eps[row] == eps[row]) || !(th == th);
-        const int n = n0 + n1;
         int have = 0;
         for (int e = lane; e < n; e += 32) {
-            const int64_t src = row * mma::CAP + (e < n0 ? e : mma::HALF_CAP + (e - n0));
+            int p = 0, r = e;   // entry e of the concatenated part lists
+#pragma unroll
+            for (int q = 0; q + 1 < mma::PARTS; q++)
+                if (p == q && r >= np[q]) { r -= np[q]; p++; }
+            const int64_t src = row * mma::CAP + p * mma::PART_CAP + r;
             const int32_t c = perm[cand_col[src]];  // original id
             const float v = cand_val[src];
             const bool keep = c != self && v == v;   // SearchIndex never returns the query itself
@@ -511,13 +456,13 @@ static EncodeTiledFn encode_fn()
     return fn;
 }
 
-static int32_t make_map(CUtensorMap *map, const void *base, int64_t rows, int kp)
+static int32_t make_map(CUtensorMap *map, const void *base, int64_t rows, int kp, int box_rows)
 {
     EncodeTiledFn fn = encode_fn();
     if (!fn) { set_error("cuTensorMapEncodeTiled is not available from the driver"); return GORSE_B200_ERR_CUDA; }
     cuuint64_t dims[2] = {(cuuint64_t)kp, (cuuint64_t)rows};
     cuuint64_t strides[1] = {(cuuint64_t)kp * 2};
-    cuuint32_t box[2] = {(cuuint32_t)mma::BK, (cuuint32_t)mma::BM};
+    cuuint32_t box[2] = {(cuuint32_t)mma::BK, (cuuint32_t)box_rows};
     cuuint32_t estr[2] = {1, 1};
     CUresult r = fn(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void *>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                     CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
@@ -574,29 +519,24 @@ int32_t search_mma(gorse_b200_index *ix, const float *d_q, const int64_t *d_qidx
     const int64_t n_pad = (ix->n + mma::BN - 1) / mma::BN * mma::BN;
     const int n_tiles = (int)(n_pad / mma::BN);
     // sample size: the R_TOP-th best of m random columns leaves on average R_TOP * N / m columns above it (Gamma(R_TOP)
-    // spread).  Both column halves of a row now share ONE threshold from the whole sample, aimed at 4k columns per row: the
-    // row has fewer than k candidates when >= R_TOP of its true top k fell into the sample, Poisson(k m / N = R_TOP / 4):
-    // ~1e-6 per row (0 rows of 151 552 measured; at 3.2k: 25 rows, each a full exact scan; at 2.4k: 690), and a half's
-    // HALF_CAP-slot list holds 4x the expected count.  (Round 1 / early round 2: 3.2k PER HALF, lists overflowing for ~35
-    // rows per call; 4.5k / 6k per half overflowed for 1 % / 20 % of the rows.  profiles/r02_topk_margin_chunk.md,
-    // profiles/r02_topk_epilogue.md.)
+    // spread).  The parts of a row share ONE threshold from the whole sample, aimed at 4k columns per row: the row has
+    // fewer than k candidates when >= R_TOP of its true top k fell into the sample, Poisson(k m / N = R_TOP / 4): ~1e-6 per
+    // row, and a part's PART_CAP-slot list holds 4x its expected k columns (k <= 128).
     int m_tiles = (int)((double)mma::R_TOP * (double)ix->n / (4.0 * k) / mma::BN);
     m_tiles = std::max(1, std::min(m_tiles, n_tiles));
     const bool self_skip = d_q == nullptr;
-    // stages from the shared-memory budget
-    const size_t a_bytes = (size_t)mma::TILES_M * kb * mma::TILE_BYTES, b_stage = (size_t)kb * mma::TILE_BYTES;
-    // at most 4: a fifth stage fits (230 KB) but leaves the epilogue's global traffic no L1 and measured 6 % slower
-    int stages = (int)std::min<size_t>(4, (226 * 1024 - 1280 - a_bytes) / b_stage);
+    // stages from the shared-memory budget (227 KB per block), at most 4: the epilogue's global traffic keeps some L1
+    const size_t a_bytes = (size_t)mma::CONSUMERS * kb * mma::A_TILE_BYTES, b_stage = (size_t)kb * mma::B_TILE_BYTES;
+    int stages = (int)std::min<size_t>(4, (227 * 1024 - 1280 - a_bytes) / b_stage);
     if (stages < 2) { set_error("search_mma: Kp = %d does not fit", kp); return GORSE_B200_ERR_UNSUPPORTED; }
     const size_t smem = a_bytes + (size_t)stages * b_stage + 1024 /*align*/ + 256 /*barriers*/;
 
     CUtensorMap map_b;
-    GB_TRY(make_map(&map_b, ix->Xb.p, n_pad, kp));
-    // queries are processed in chunks of four 256-row groups per SM so that the candidate lists stay modest (one group per SM
-    // with the downloads of finished chunks overlapped was measured slower, 88.8 vs 68.5 ms per 151 552-row call: every chunk
-    // pays a kernel tail, a host sync for the fallback count and its own fallback launches); a finished chunk is downloaded
-    // on the copy stream while the next one computes
-    const int64_t chunk = (int64_t)c->sm_count * mma::TILES_M * mma::BM * 4;
+    GB_TRY(make_map(&map_b, ix->Xb.p, n_pad, kp, mma::BN));
+    // queries are processed in chunks of 1024 rows per SM so that the candidate lists stay modest while every chunk's kernel
+    // tail, host sync for the fallback count and fallback launches are amortised; a finished chunk is downloaded on the copy
+    // stream while the next one computes
+    const int64_t chunk = (int64_t)c->sm_count * mma::GROUP_ROWS * 8;
     // work buffers live in the index and are reused by later searches (multi-GB cudaMalloc/cudaFree per call otherwise)
     DevBuf<__nv_bfloat16> &Qb = ix->w_qb;
     DevBuf<float> &eps = ix->w_eps, &cval = ix->w_cval, &theta = ix->w_theta;
@@ -607,11 +547,11 @@ int32_t search_mma(gorse_b200_index *ix, const float *d_q, const int64_t *d_qidx
         cudaStreamSynchronize(c->copy_stream);
         return s;
     };
-    const int64_t cq = std::min(nq, chunk), cq_pad = (cq + 255) / 256 * 256;
+    const int64_t cq = std::min(nq, chunk), cq_pad = (cq + mma::GROUP_ROWS - 1) / mma::GROUP_ROWS * mma::GROUP_ROWS;
     if (ix->w_cq >= cq && ix->w_kp == kp) {
         // reuse
-    } else if ((ix->w_cq = 0, false) || (st = Qb.alloc((size_t)cq_pad * kp)) || (st = eps.alloc(cq)) || (st = cval.alloc((size_t)cq * mma::CAP)) || (st = theta.alloc(2 * cq)) ||
-        (st = ccol.alloc((size_t)cq * mma::CAP)) || (st = ccnt.alloc(2 * cq)) || (st = ids.alloc((size_t)cq * mma::CAP)) || (st = idcnt.alloc(cq)) ||
+    } else if ((ix->w_cq = 0, false) || (st = Qb.alloc((size_t)cq_pad * kp)) || (st = eps.alloc(cq)) || (st = cval.alloc((size_t)cq * mma::CAP)) || (st = theta.alloc(mma::PARTS * cq)) ||
+        (st = ccol.alloc((size_t)cq * mma::CAP)) || (st = ccnt.alloc(mma::PARTS * cq)) || (st = ids.alloc((size_t)cq * mma::CAP)) || (st = idcnt.alloc(cq)) ||
         (st = flag.alloc(cq)) || (st = flist.alloc(cq + 1)))
         return done(st);
     else { ix->w_cq = cq; ix->w_kp = kp; }
@@ -623,16 +563,16 @@ int32_t search_mma(gorse_b200_index *ix, const float *d_q, const int64_t *d_qidx
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) { set_error("search_mma smem attr: %s", cudaGetErrorString(e)); return done(GORSE_B200_ERR_CUDA); }
     for (int64_t off = 0; off < nq; off += cq) {
-        const int64_t n_this = std::min(cq, nq - off), n_this_pad = (n_this + 255) / 256 * 256;
+        const int64_t n_this = std::min(cq, nq - off), n_this_pad = (n_this + mma::GROUP_ROWS - 1) / mma::GROUP_ROWS * mma::GROUP_ROWS;
         const float *qp = d_q ? d_q + off * ix->d : nullptr;
         const int64_t *qi = d_qidx ? d_qidx + off : nullptr;
         mma::build_queries_kernel<<<(unsigned)n_this_pad, 128, 0, c->stream>>>(ix->X.p, qp, qi, q0 + off, n_this, n_this_pad, ix->d, kp, ix->metric,
                                                                               ix->max_norm, Qb.p, eps.p);
         c->launches++;
         CUtensorMap map_a;
-        if ((st = make_map(&map_a, Qb.p, n_this_pad, kp))) return done(st);
+        if ((st = make_map(&map_a, Qb.p, n_this_pad, kp, mma::BM))) return done(st);
         mma::Params P;
-        P.n = ix->n; P.n_tiles = n_tiles; P.m_tiles = m_tiles; P.kb = kb; P.nq = n_this; P.n_groups = (int)(n_this_pad / 256);
+        P.n = ix->n; P.n_tiles = n_tiles; P.m_tiles = m_tiles; P.kb = kb; P.nq = n_this; P.n_groups = (int)(n_this_pad / mma::GROUP_ROWS);
         P.eps = eps.p; P.cand_col = ccol.p; P.cand_val = cval.p; P.cand_cnt = ccnt.p; P.theta = theta.p; P.dbg = ix->dbg_scores;
         const int grid = std::min(P.n_groups, c->sm_count);
         if (!ix->ev0) { cudaEventCreate(&ix->ev0); cudaEventCreate(&ix->ev1); }

@@ -1,5 +1,5 @@
 /*
- * gorse_b200.h -- C ABI of libgorse_b200.so: the B200 (sm_100a) implementation of Gorse's
+ * gorse_b200.h -- C ABI of libgorse_b200.so: the H100 (sm_90a) implementation of Gorse's
  * collaborative-filtering training and brute-force top-k hot path.
  *
  * This is exactly what the reference-side cgo shim binds (go/ in this repo, INTEGRATION.md):
@@ -122,7 +122,8 @@ typedef enum {
      * fma(t, lr, row as read by this step).  Bit-exact vs the oracle when the triples of one launch
      * touch disjoint rows. */
     GORSE_B200_SCATTER_STORE = 0,
-    /* Hogwild with vectorised atomics (red.global.add.v4.f32): no update is ever lost */
+    /* vectorised atomics (red.global.add.v4.f32): no update is ever lost; gorse_b200_bpr_epoch runs in rounds whose
+       triples read the rows as the previous round left them, so an epoch gives the same factors every run up to rounding */
     GORSE_B200_SCATTER_ATOMIC = 1
 } gorse_b200_scatter;
 
@@ -255,7 +256,7 @@ int32_t gorse_b200_index_search_indices(gorse_b200_index *ix, const int64_t *q_i
 int32_t gorse_b200_index_search_range(gorse_b200_index *ix, int64_t q0, int64_t q1, int32_t k, int32_t prune0,
                                       int32_t *idx_out, float *dist_out, int32_t *count_out);
 /* measurement hook (bench.py), like gorse_b200_ctx_timer_*: since the previous call, the device time (ms) and algorithmic
- * flop (2 nq N d) of the tcgen05 candidate sweep, and the number of query rows that were redone by the exact scan because
+ * flop (2 nq N d) of the tensor-core candidate sweep, and the number of query rows that were redone by the exact scan because
  * their candidate set could not be certified.  Any pointer may be NULL. */
 int32_t gorse_b200_index_stats(gorse_b200_index *ix, double *stage1_ms, double *stage1_flop, int64_t *fallback_rows);
 /* test hook: the dense tensor-core scores of stored vectors [q0, q1) against all N vectors, original column order,

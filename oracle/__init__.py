@@ -6,6 +6,7 @@ cpu_baseline / --impl reference legs.  The product package (gorse_b200) never im
 import ctypes as C
 import os
 import subprocess
+import sys
 
 import numpy as np
 
@@ -17,12 +18,40 @@ METRIC_EUCLIDEAN = 0
 METRIC_NEG_DOT = 1
 
 
+REF_KERNELS = os.path.join("common", "floats", "src", "floats_avx512.c")
+
+
+def reference_dir():
+    """The checkout of the reference project whose C kernels oracle/_ref is built from: $GORSE_REFERENCE_DIR, else a
+    directory named `reference` next to this repository or next to any directory above it; None when there is none."""
+    env = os.environ.get("GORSE_REFERENCE_DIR")
+    if env:
+        return env if os.path.isfile(os.path.join(env, REF_KERNELS)) else None
+    d = os.path.dirname(os.path.dirname(_HERE))   # the directory holding the repository
+    while True:
+        cand = os.path.join(d, "reference")
+        if os.path.isfile(os.path.join(cand, REF_KERNELS)):
+            return cand
+        up = os.path.dirname(d)
+        if up == d:
+            return None
+        d = up
+
+
 def build(force=False):
-    """Compile the oracle (and oracle/_ref when /root/reference is mounted)."""
+    """Compile the oracle and, whenever the reference project is found (reference_dir()), oracle/_ref from its own C
+    kernels.  Without the reference a prebuilt oracle/_ref is kept; a missing one is reported on stderr, because the CPU
+    baseline then times the oracle port and the reference-comparison tests fall back to stored outputs."""
     src_newer = (not os.path.exists(_SO)) or os.path.getmtime(_SO) < os.path.getmtime(
         os.path.join(_HERE, "gorse_oracle.c"))
-    if force or src_newer or (os.path.isdir("/root/reference") and not os.path.exists(REF_SO)):
-        subprocess.check_call(["make", "-C", _HERE, "--no-print-directory"], stdout=subprocess.DEVNULL)
+    ref = reference_dir()
+    if force or src_newer or (ref and not os.path.exists(REF_SO)):
+        env = dict(os.environ, GORSE_REFERENCE_DIR=ref or "")
+        subprocess.check_call(["make", "-C", _HERE, "--no-print-directory"], stdout=subprocess.DEVNULL, env=env)
+    if not os.path.exists(REF_SO):
+        print("oracle: the reference project was not found (set GORSE_REFERENCE_DIR to its checkout); oracle/_ref is not "
+              "built: CPU baselines time the oracle port and the reference-comparison tests use stored outputs",
+              file=sys.stderr)
 
 
 _lib = None

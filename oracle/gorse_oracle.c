@@ -143,7 +143,7 @@ float gbo_euclidean_scalar(const float *a, const float *b, int64_t n)
 }
 
 /* ------------------------------------------------------------------------------------------
- * chewxy/math32 v1.11.1 (go.mod:13), not under /root/reference.  PARITY UNPINNED.
+ * chewxy/math32 v1.11.1 (go.mod:13), not in the reference.  PARITY UNPINNED.
  * Exp: the FreeBSD e_expf.c algorithm (argument reduction x = k*ln2 + r with a split float32 ln2,
  * degree-5 minimax on r*r, Ldexp) in the form of math32's portable exp.go.  Used at
  * model/cf/model.go:470-471.  Every operation rounds to float32 individually.
@@ -970,7 +970,7 @@ int32_t gbo_similar_scores(int32_t euclidean, double score_scale, int32_t self_i
 /* Sparse similarity search (the "tags" / "users" / "auto" item-to-item and user-to-user types): what the reference
  * asks its vector store for with sparse vectors and the Dot metric (storage/vectors/xvec.go:244-248 flat sparse index,
  * :405 query).  The arithmetic lives in gorse-io/xvec v0.0.0-20260821023012-cf0c34c6025f (go.mod:31), which is NOT under
- * /root/reference: PARITY UNPINNED except for the neighbour-id orders the reference's tests assert
+ * the reference: PARITY UNPINNED except for the neighbour-id orders the reference's tests assert
  * (logics/item_to_item_test.go:212-316).  Restated as: indices ascending in every vector (item_to_item.go:191,213,
  * 236-237 sort the ids before appendSparseVector), dot = merge-join summed in index order in fp32, the k largest dots
  * through the same bounded Go heap as Bruteforce (distance = -dot, ties as container/heap leaves them). */

@@ -14,7 +14,7 @@
  *   - metrics: PINNED by model/cf/evaluator_test.go known answers
  *   - BPR step / ALS epoch / Bruteforce: restated from model/cf/model.go and common/ann/bruteforce.go;
  *     the Go code cannot run here (no Go toolchain) -> anchored on the pinned primitives above and on
- *     the reference's call sites.  math32.Exp (chewxy/math32 v1.11.1, absent from /root/reference) is
+ *     the reference's call sites.  math32.Exp (chewxy/math32 v1.11.1, absent from the reference) is
  *     restated from its published algorithm: PARITY UNPINNED for Exp (<= 1-2 ulp expected).
  *   - RNG streams (Go math/rand): PARITY UNPINNED and unreproducible (SURVEY F9); samplers here are
  *     our own counter-based design shared bit-for-bit with the CUDA path.

@@ -1,11 +1,10 @@
 """Generates tests/golden/floats_golden.npz by RUNNING THE REFERENCE's own C kernels
-(/root/reference/common/floats/src/floats_avx512.c + floats_avx.c, compiled by oracle/Makefile into
-oracle/_ref/libfloats_ref.so) on seeded random inputs.  Run in the build container only:
+(common/floats/src/floats_avx512.c + floats_avx.c of the reference project, compiled by oracle/Makefile into
+oracle/_ref/libfloats_ref.so) on seeded random inputs.  Needs a CPU with AVX-512 and a checkout of the reference:
 
-    python tests/golden/make_floats_golden.py
+    GORSE_REFERENCE_DIR=<reference checkout> python tests/golden/make_floats_golden.py
 
-The fixture pins the oracle restatement (tests/test_oracle_floats.py) on boxes where
-/root/reference is absent (the GPU box).
+The fixture pins the oracle restatement (tests/test_oracle_floats.py) on machines without the reference.
 """
 import os
 import sys

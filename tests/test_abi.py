@@ -28,7 +28,7 @@ def test_library_exports_every_declared_symbol(gb):
     assert _lib.lib.gorse_b200_version() == 1
 
 
-def test_only_sm100a_code_in_library(gb):
+def test_only_sm90a_code_in_library(gb):
     import shutil
     import subprocess
 
@@ -38,7 +38,7 @@ def test_only_sm100a_code_in_library(gb):
         pytest.skip("cuobjdump not on PATH")
     out = subprocess.run(["cuobjdump", "-lelf", _lib.LIB_PATH], capture_output=True, text=True).stdout
     archs = set(re.findall(r"sm_\d+a?", out))
-    assert archs == {"sm_100a"}, archs
+    assert archs == {"sm_90a"}, archs
 
 
 def test_product_never_touches_the_oracle():

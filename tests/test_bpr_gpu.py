@@ -189,3 +189,29 @@ def test_full_fit_matches_oracle_ndcg(gb, orc, ctx):
     assert np.isfinite(Pg).all() and np.isfinite(Qg).all()
     assert abs(got - want) < 0.01, (base, want, got)
     assert got_dev == got  # device Evaluate == oracle Evaluate on the same factors
+
+
+@pytest.mark.parametrize("d", [64, 128])
+def test_atomic_epochs_repeat_up_to_rounding(gb, ctx, d):
+    """Epochs with atomic scatter run in rounds whose triples read the rows the previous round left: the same factors and
+    seeds give the same factors on every run, except for the order of float additions into a row that several triples of
+    one round update.  Zipf(1) data with many rounds per epoch and a heavy popularity head."""
+    from gorse_b200 import synth
+
+    U, I, R = 200_000, 20_000, 2_000_000
+    off, items = synth.make_feedback(U, I, R, seed=d, zipf_s=1.0, exact=True)
+    rng = np.random.default_rng(d)
+    P0 = (rng.standard_normal((U, d)) * 0.01).astype(np.float32)
+    Q0 = (rng.standard_normal((I, d)) * 0.01).astype(np.float32)
+    runs = []
+    for _ in range(2):
+        with gb.CFModel(ctx, U, I, d, off, items) as m:
+            m.set_factors(P0, Q0)
+            for ep in range(3):
+                m.bpr_epoch(0.05, 0.01, R, 500 + ep, gb.SCATTER_ATOMIC)
+            runs.append(m.get_factors())
+    (P1, Q1), (P2, Q2) = runs
+    assert not np.array_equal(Q1, Q0)
+    for a, b in ((P1, P2), (Q1, Q2)):
+        assert np.isfinite(a).all()
+        assert np.abs(a.astype(np.float64) - b).max() <= 1e-5 * np.abs(a).max()

@@ -1,7 +1,7 @@
 """BASELINE.json's FULL sizes, checked through size-independent properties and spot checks against the oracle
 (the oracle cannot run whole configs in seconds, so it is used on samples):
   C2  BPR 1M x 100K x 10M, d=64: sampler validity on 10^6 triples, a sampled triple stream applied in order is bit-exact
-      vs the oracle on the full tables, one free-running epoch keeps the factors finite and moves hot and cold rows
+      vs the oracle on the full tables, one epoch keeps the factors finite and moves hot and cold rows
   C3  eALS at full size lives in tests/test_xl_als_gpu.py
   C4  top-100 over 1M x 128: every row sorted, self-free, k results; 12 rows bit-exact vs the oracle's Bruteforce
 """
@@ -40,7 +40,7 @@ def test_c2_bpr_full_size(gb, orc):
         Po, Qo = P.copy(), Q.copy()
         orc.bpr_apply_triples(Po, Qo, t[:20000], 0.05, 0.01)
         assert Pg.tobytes() == Po.tobytes() and Qg.tobytes() == Qo.tobytes()
-        # one free-running epoch (hot queue + capped hot apply): finite, and both the hottest and a cold item moved
+        # one epoch (rounds of 8192 triples): finite, and both the hottest and a cold item moved
         m.set_factors(P, Q)
         m.bpr_epoch(0.05, 0.01, R, 77)
         P1, Q1 = m.get_factors()

@@ -1,6 +1,6 @@
-"""The tensor-core stage of the brute-force search (csrc/topk_mma.cu): tcgen05 GEMM + fused threshold filter, then the
+"""The tensor-core stage of the brute-force search (csrc/topk_mma.cu): wgmma GEMM + fused threshold filter, then the
 exact re-rank.  Results must equal the oracle's ann.Bruteforce bit for bit (indices AND distances), like the exact
-scan; the dense stage-1 scores are checked against a bf16 matmul to validate descriptors / swizzle / TMEM layout."""
+scan; the dense stage-1 scores are checked against a bf16 matmul to validate descriptors / swizzle / accumulator layout."""
 import os
 
 import numpy as np

@@ -14,5 +14,5 @@ with gb.Context(0) as ctx, gb.CFModel(ctx,U,I,d,off,items) as m:
         if ep%10==9:
             P,Q=m.get_factors()
             fin=np.isfinite(Q).all() and np.isfinite(P).all()
-            print(os.environ.get("GORSE_B200_NO_HOT","0"),"small" if small else "c2",ep+1,"finite",fin,"max|Q|",np.sqrt((Q*Q).sum(1)).max() if fin else None,"max|P|",np.sqrt((P*P).sum(1)).max() if fin else None, "nan rows Q",int((~np.isfinite(Q)).any(1).sum()), flush=True)
+            print("small" if small else "c2",ep+1,"finite",fin,"max|Q|",np.sqrt((Q*Q).sum(1)).max() if fin else None,"max|P|",np.sqrt((P*P).sum(1)).max() if fin else None, "nan rows Q",int((~np.isfinite(Q)).any(1).sum()), flush=True)
             if not fin: break
