@@ -1,20 +1,27 @@
 // als.cu -- eALS ("CCD") epoch: model/cf/model.go:641-738.
-//   S^q = sum_{i: |R_i|>0} q_i q_i^T          (:645-658)   gram_kernel + gram_reduce_kernel
-//   user rows, coordinate descent over f      (:659-687)   als_rows_kernel
+//   S^q = sum_{i: |R_i|>0} q_i q_i^T          (:645-658)   run_gram
+//   user rows, coordinate descent over f      (:659-687)   run_rows
 //   S^p = sum_{u: |R_u|>0} p_u p_u^T          (:693-706)
 //   item rows                                 (:707-735)
 // Roofline class: HBM bandwidth (one gather of the opposite table's rows per feedback + own row + one
 // Gram pass): B_epoch = 2|R|(4d+4) + 3(U+I)4d bytes.
 //
-// Row updates come in four forms, chosen per row by its length (prepare_als):
-//   * als_thread_kernel (als_thread.cu; d % 32 == 0, d <= 128, rows up to 4 entries): one thread per row;
-//   * als_rows_group_blocked_kernel (same d, rows up to 96 entries): a group of 8/16/32 lanes per row, g = S x kept
-//     current in registers, the gathered rows staged one block of G coordinates at a time;
-//   * Gram form for longer rows (tensor-core chunk Grams at d = 128, als_gram_tc.cu, else als_chunk_gram_kernel; then
-//     als_solve_kernel): one Gauss-Seidel sweep on A x = h;
-//   * als_rows_kernel, one warp per row with the reference's loop structure, for the remaining shapes (d not a
-//     multiple of 32 or > 128).  The gathered rows Y[R_x] are staged once in shared memory ([n][d+1], the +1 makes the
-//     per-f column walk conflict-free), the running predictions live in registers.
+// Grams.  A Gram is taken over a list of rows cut into chunks of <= GB_ALS_CHUNK: every chunk becomes one partial (G, h)
+// in cf->als_partial, als_partial_stride(d) floats apart.  The chunk kernel is als_chunk_gram_tc (tensor cores,
+// als_gram_tc.cu) at d = 128, als_chunk_gram_kernel at other d <= 128 and als_chunk_gram_generic_kernel at d > 128.
+// S runs it over the rows with feedback and sums the partials in chunk order (gram_reduce_kernel); a long row runs it
+// over its own entries (d <= 128 only).
+//
+// Row updates, chosen per row by d and its length n (prepare_als, kRowClasses):
+//   d % 32 == 0, d <= 128:  n <= 4            als_thread_kernel (als_thread.cu), one thread per row
+//                           n <= 96           als_rows_group_blocked_kernel<G, E>, a group of 8/16/32 lanes per row, g = S x
+//                                             kept current in registers, the gathered rows staged G coordinates at a time
+//   other d:                n (d+1) <= 12288  als_rows_kernel, one warp per row with the reference's loop structure; the
+//                                             gathered rows Y[R_x] staged once in shared memory ([n][d+1], the +1 makes the
+//                                             per-f column walk conflict-free), the running predictions in registers
+//   longer, d <= 128:       Gram form: chunk Grams, als_partial_reduce_kernel, als_solve_kernel (one Gauss-Seidel sweep
+//                           on A x = h)
+//   longer, d > 128:        als_rows_kernel gathering from L2 without staging
 // In all forms sums over the row's feedback are taken lane-parallel, so results differ from the reference's serial
 // order by reassociation only (parity budget 1e-4 relative, observed ~1e-6).
 #include <cstdlib>
@@ -57,62 +64,7 @@ struct GramTile {
     __device__ __forceinline__ float get(int x, int y) const { return acc[x][y]; }
 };
 
-// Partial Gram of rows [r0, r1) handled by this CTA; TxT register tile per thread, 16x16 threads.
-template <int T>
-__global__ void __launch_bounds__(256) gram_kernel(const float *X, int32_t rows, int d, const int64_t *off, float *partial)
-{
-    extern __shared__ float xs[];  // [16][dp]
-    const int dp = 16 * T;         // padded width
-    const int ti = threadIdx.x >> 4, tj = threadIdx.x & 15;
-    GramTile<T> tile;
-    tile.zero();
-    int64_t per = ((int64_t)rows + gridDim.x - 1) / gridDim.x;
-    int64_t r0 = (int64_t)blockIdx.x * per, r1 = min((int64_t)rows, r0 + per);
-    for (int64_t base = r0; base < r1; base += 16) {
-        // stage 16 rows (zero-filled when masked or out of range)
-        for (int e = threadIdx.x; e < 16 * dp; e += 256) {
-            int rr = e / dp, k = e - rr * dp;
-            int64_t r = base + rr;
-            float v = 0.f;
-            if (r < r1 && k < d && off[r + 1] > off[r]) v = X[r * d + k];
-            xs[e] = v;
-        }
-        __syncthreads();
-#pragma unroll 4
-        for (int rr = 0; rr < 16; rr++) {
-            float a[T], b[T];
-#pragma unroll
-            for (int k = 0; k < T; k++) { a[k] = xs[rr * dp + ti * T + k]; b[k] = xs[rr * dp + tj * T + k]; }
-            tile.mac(a, b);
-        }
-        __syncthreads();
-    }
-    float *out = partial + (int64_t)blockIdx.x * d * d;
-#pragma unroll
-    for (int x = 0; x < T; x++)
-#pragma unroll
-        for (int y = 0; y < T; y++) {
-            int i = ti * T + x, j = tj * T + y;
-            if (i < d && j < d) out[i * d + j] = tile.get(x, y);
-        }
-}
-
-// generic d > 128: one thread per output element, rows streamed from global
-__global__ void gram_generic_kernel(const float *X, int32_t rows, int d, const int64_t *off, float *partial)
-{
-    int64_t per = ((int64_t)rows + gridDim.x - 1) / gridDim.x;
-    int64_t r0 = (int64_t)blockIdx.x * per, r1 = min((int64_t)rows, r0 + per);
-    float *out = partial + (int64_t)blockIdx.x * d * d;
-    for (int e = threadIdx.x; e < d * d; e += blockDim.x) {
-        int i = e / d, j = e - i * d;
-        float acc = 0.f;
-        for (int64_t r = r0; r < r1; r++)
-            if (off[r + 1] > off[r]) acc = __fmaf_rn(X[r * d + i], X[r * d + j], acc);
-        out[e] = acc;
-    }
-}
-
-// fixed-order reduction of the per-CTA partials: deterministic run to run
+// fixed-order reduction of the chunk partials: deterministic run to run
 __global__ void gram_reduce_kernel(const float *partial, int n_parts, int dd, int64_t stride, float *S)
 {
     int e = blockIdx.x * blockDim.x + threadIdx.x;
@@ -122,12 +74,11 @@ __global__ void gram_reduce_kernel(const float *partial, int n_parts, int dd, in
     S[e] = s;
 }
 
-// One warp per row.  X: table being updated (row index r - x_lo), Y: the opposite table (index y - y_lo).
+// One warp per row.  X: table being updated, Y: the opposite table.
 // smem per warp: xrow[d] + (staged ? ys[cap_n][d+1] : 0)
 __global__ void __launch_bounds__(32 * GB_ALS_WARPS)
-als_rows_kernel(float *X, const float *Y, int d, int32_t x_lo, int32_t y_lo, const int64_t *off, const int32_t *idx,
-                const float *S, float reg, float w, const int32_t *row_ids, int32_t n_rows, int stage_floats_per_warp,
-                float *pred_scratch)
+als_rows_kernel(float *X, const float *Y, int d, const int64_t *off, const int32_t *idx, const float *S, float reg, float w,
+                const int32_t *row_ids, int32_t n_rows, int stage_floats_per_warp, float *pred_scratch)
 {
     extern __shared__ float smem[];
     const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
@@ -142,7 +93,7 @@ als_rows_kernel(float *X, const float *Y, int d, int32_t x_lo, int32_t y_lo, con
         const int32_t r = row_ids[slot];
         const int64_t o = off[r];
         const int n = (int)(off[r + 1] - o);
-        float *xg = X + (int64_t)(r - x_lo) * d;
+        float *xg = X + (int64_t)r * d;
         for (int k = lane; k < d; k += 32) xrow[k] = xg[k];
         const bool staged = (int64_t)n * dp <= stage_floats_per_warp;
         const bool pred_in_regs = n <= 32 * GB_ALS_PRED_REGS;
@@ -151,7 +102,7 @@ als_rows_kernel(float *X, const float *Y, int d, int32_t x_lo, int32_t y_lo, con
         if (staged) {
             // coalesced row copies: lane walks the row, one row at a time
             for (int t = 0; t < n; t++) {
-                const float *yr = Y + (int64_t)(idx[o + t] - y_lo) * d;
+                const float *yr = Y + (int64_t)idx[o + t] * d;
                 for (int k = lane; k < d; k += 32) ys[t * dp + k] = yr[k];
             }
             __syncwarp();
@@ -169,7 +120,7 @@ als_rows_kernel(float *X, const float *Y, int d, int32_t x_lo, int32_t y_lo, con
                     const float *yr = ys + t * dp;
                     v = dot_any(xrow, yr, d);
                 } else {
-                    v = dot_any(xrow, Y + (int64_t)(idx[o + t] - y_lo) * d, d);
+                    v = dot_any(xrow, Y + (int64_t)idx[o + t] * d, d);
                 }
             }
             if (pred_in_regs) {
@@ -184,7 +135,7 @@ als_rows_kernel(float *X, const float *Y, int d, int32_t x_lo, int32_t y_lo, con
             for (int t0 = 0, q = 0; t0 < n; t0 += 32, q++) {
                 int t = t0 + lane;
                 if (t < n) {
-                    float y = staged ? ys[t * dp + f] : __ldg(Y + (int64_t)(idx[o + t] - y_lo) * d + f);
+                    float y = staged ? ys[t * dp + f] : __ldg(Y + (int64_t)idx[o + t] * d + f);
                     float p;
                     if (pred_in_regs) {
                         p = pr[0];
@@ -207,7 +158,7 @@ als_rows_kernel(float *X, const float *Y, int d, int32_t x_lo, int32_t y_lo, con
             for (int t0 = 0, q = 0; t0 < n; t0 += 32, q++) {
                 int t = t0 + lane;
                 if (t < n) {
-                    float y = staged ? ys[t * dp + f] : __ldg(Y + (int64_t)(idx[o + t] - y_lo) * d + f);
+                    float y = staged ? ys[t * dp + f] : __ldg(Y + (int64_t)idx[o + t] * d + f);
                     if (pred_in_regs) {
 #pragma unroll
                         for (int qq = 0; qq < GB_ALS_PRED_REGS; qq++)
@@ -228,7 +179,7 @@ als_rows_kernel(float *X, const float *Y, int d, int32_t x_lo, int32_t y_lo, con
 }
 
 // ---- short rows, lane-group form (d % 32 == 0, d <= 128) ---------------------------------------------------
-// A group of G lanes (8 or 32) owns one row; 32/G rows share a warp.  With h_f = sum_t y_tf, c_f = (1-w) sum_t y_tf^2
+// A group of G lanes (8, 16 or 32) owns one row; 32/G rows share a warp.  With h_f = sum_t y_tf, c_f = (1-w) sum_t y_tf^2
 // and g = S x kept CURRENT (g += delta * S[f,:] after every coordinate), the reference's step (model.go:666-680) is
 //     x_f <- ( h_f - (1-w) * sum_t pred_t y_tf + x_f * (c_f + w S_ff) - w * g_f ) / (c_f + w S_ff + reg)
 // (a = h_f - (1-w) z_f + x_f c_f,  b = w (g_f - S_ff x_f)): the only reduction on the strictly sequential f chain is
@@ -246,13 +197,12 @@ __device__ __forceinline__ float group_sum(float v)
     return v;
 }
 
-// ---- lane-group form with BLOCKED staging (round 2) ------------------------------------------------------------------
-// The arithmetic above with the gathered rows staged one block of G coordinates at a time instead of whole (round 1's
-// als_rows_group_kernel, removed): n * (G+1) floats per row in shared memory instead of n * (D+1).  The whole-row version held 33 KB (rows up
-// to 32 entries, two rows per warp) / 49.5 KB (rows up to 96 entries) per warp next to the 64 KB copy of S, i.e. 3-4 warps per
-// SM, and each of those warps runs a dependent shuffle chain per coordinate: 2.3 + 3.0 ms per half-sweep for 7 % of the rows
-// Lane j of the group owns coordinate i*G + j of block i, so a block is exactly what the group
-// works on at a time:
+// ---- lane-group form with BLOCKED staging ------------------------------------------------------------------------------
+// The arithmetic above with the gathered rows staged one block of G coordinates at a time: n * (G+1) floats per row in
+// shared memory instead of n * (D+1).  Staging whole rows holds 33 KB (rows up to 32 entries, two rows per warp) / 49.5 KB
+// (rows up to 96 entries) per warp next to the 64 KB copy of S, i.e. 3-4 warps per SM, each running a dependent shuffle
+// chain per coordinate: that measured 2.3 + 3.0 ms per half-sweep for 7 % of the rows.
+// Lane j of the group owns coordinate i*G + j of block i, so a block is exactly what the group works on at a time:
 //   pass A  per sub-range of G entries and per block: stage G x G floats, partial_tt += x_i * y (registers, one per entry of
 //           the sub-range), h_i, c_i column sums; the partials are reduced across the group once per sub-range -> pred;
 //   sweep   per block: stage all n entries of the block, then the G coordinates as before.
@@ -426,17 +376,20 @@ static int32_t launch_group_blocked_d(gorse_b200_cf *cf, float *X, const float *
     }
 }
 
-// ---- Gram form for rows too long to stage (DESIGN.md 5.2) ---------------------------------------------------
+// ---- chunk Grams, and the Gram form for rows too long to stage (DESIGN.md 5.2) --------------------------------------
 // eALS over f for one row is exactly one Gauss-Seidel sweep on  A x = h  with
 //     A = (1-w) * G + w * S + reg * I,   G = sum_{t in R} y_t y_t^T,   h = sum_{t in R} y_t
 // (a = h_f - (1-w) sum_{k!=f} x_k G[k][f],  b = w sum_{k!=f} x_k S[k][f],  c = (1-w) G[f][f]; model.go:666-680).
-// A long row is cut into chunks of <= GB_ALS_CHUNK entries; each CTA turns one chunk into a partial (G, h) with the
-// same 16x16-thread register tiling as gram_kernel, and one CTA per row sums the partials and does the sweep.
+// A long row is cut into chunks of <= GB_ALS_CHUNK entries; each CTA turns one chunk into a partial (G, h), the partials
+// of a row are summed into its first one, and one CTA per row does the sweep.  S takes the same chunk kernels over the
+// list of rows with feedback.
 #define GB_ALS_CHUNK 2048
 
+// partial[c] = (G, h) over the rows Y[idx[chunk_begin[c] + t]], t < chunk_len[c]; d <= 128, 16x16 threads with a TxT
+// register tile each
 template <int T>
-__global__ void __launch_bounds__(256) als_chunk_gram_kernel(const float *Y, int d, const int32_t *idx, const int32_t *chunk_row,
-                                                             const int64_t *chunk_begin, const int32_t *chunk_len, float *partial)
+__global__ void __launch_bounds__(256) als_chunk_gram_kernel(const float *Y, int d, const int32_t *idx, const int64_t *chunk_begin,
+                                                             const int32_t *chunk_len, float *partial)
 {
     extern __shared__ float xs[];  // [16][dp]
     const int dp = 16 * T;
@@ -469,7 +422,7 @@ __global__ void __launch_bounds__(256) als_chunk_gram_kernel(const float *Y, int
         }
         __syncthreads();
     }
-    float *out = partial + (int64_t)blockIdx.x * (d * d + d);
+    float *out = partial + (int64_t)blockIdx.x * als_partial_stride(d);
 #pragma unroll
     for (int x = 0; x < T; x++)
 #pragma unroll
@@ -483,9 +436,26 @@ __global__ void __launch_bounds__(256) als_chunk_gram_kernel(const float *Y, int
     }
 }
 
+// the same partial (G, h) at d > 128: one thread per element (row d of G is h), grid (chunks, element tiles)
+__global__ void __launch_bounds__(256) als_chunk_gram_generic_kernel(const float *Y, int d, const int32_t *idx, const int64_t *chunk_begin,
+                                                                     const int32_t *chunk_len, float *partial)
+{
+    const int e = blockIdx.y * 256 + threadIdx.x;
+    if (e >= d * d + d) return;
+    const int i = e / d, j = e - i * d;
+    const int64_t b0 = chunk_begin[blockIdx.x];
+    const int len = chunk_len[blockIdx.x];
+    float acc = 0.f;
+    for (int t = 0; t < len; t++) {
+        const float *y = Y + (int64_t)__ldg(idx + b0 + t) * d;
+        acc = i < d ? __fmaf_rn(__ldg(y + i), __ldg(y + j), acc) : acc + __ldg(y + j);
+    }
+    partial[(int64_t)blockIdx.x * als_partial_stride(d) + e] = acc;
+}
+
 // partial[first chunk of the row] = sum of the row's chunk partials, in chunk order (deterministic); grid (rows, element tiles).
-// Without it one CTA of als_solve_kernel walked all chunks of its row alone: the hottest item of C3 has 232 chunks = 15 MB,
-// and that single CTA was the tail of the whole kernel.
+// Summing inside als_solve_kernel leaves one CTA to walk all chunks of its row alone: the hottest item of C3 has 232 chunks
+// = 15 MB, and that single CTA was the tail of the whole kernel.
 __global__ void __launch_bounds__(256) als_partial_reduce_kernel(const int32_t *row_chunk0, int stride4, float *partial)
 {
     const int c0 = row_chunk0[blockIdx.x], c1 = row_chunk0[blockIdx.x + 1];
@@ -505,56 +475,39 @@ __global__ void __launch_bounds__(256) als_partial_reduce_kernel(const int32_t *
 //     r = h - A x (all warps);   for f:  delta = r_f / A_ff,  x_f += delta,  r -= delta * A[:, f]
 // which is the same sweep (x_f + r_f / A_ff == (h_f - sum_{k != f} A_fk x_k) / A_ff) without a reduction on the sequential
 // chain: lane l holds r, x and 1 / A_kk for k = l + 32 j, a step is one multiply, one shuffle and d / 32 FMAs whose A operands
-// (column f, conflict-free thanks to the d + 1 row pitch) do not depend on the chain.  Round 1/2's version summed a
-// 128-element dot across the warp per coordinate (5 dependent shuffles + a divide): 1.03 ms per half-sweep at C3.
-// d % 32 == 0, d <= 128 (the only shapes prepare_als sends here).
+// (column f, conflict-free thanks to the d + 1 row pitch) do not depend on the chain.  A 128-element dot summed across the
+// warp per coordinate (5 dependent shuffles + a divide) measured 1.03 ms per half-sweep at C3.
+// Any d <= 128: lane-block j covers k = 32 j .. 32 j + 31, and coordinates k >= d are masked.
 __global__ void __launch_bounds__(256) als_solve_kernel(float *X, int d, const float *S, float reg, float w, const int32_t *rows,
-                                                        const int32_t *row_chunk0, const float *partial, int reduced)
+                                                        const int32_t *row_chunk0, const float *partial)
 {
     extern __shared__ float sm[];
     float *A = sm;                 // [d][d+1]
     float *h = A + d * (d + 1);    // [d]   h, then the residual
     float *x = h + d;              // [d]
     const int r = rows[blockIdx.x];
-    const int c0 = row_chunk0[blockIdx.x], c1 = reduced ? c0 + 1 : row_chunk0[blockIdx.x + 1];
-    const int dd = d * d, stride = dd + d, dp = d + 1;
+    const int dd = d * d, dp = d + 1;
+    const float *g0 = partial + (int64_t)row_chunk0[blockIdx.x] * als_partial_stride(d);
     const float omw = 1.0f - w;
-    if (reduced) {
-        // the row's partial is one (G, h) block, 16-byte aligned (d % 4 == 0): float4 loads, four in flight per thread.  (The
-        // scalar loop below it has a run-time inner trip count, so its 64 loads per thread went out one DRAM latency after
-        // the other: 0.27 + 1.13 ms per epoch at C3 for what is 0.13 GB of traffic.)
-        const float4 *p4 = reinterpret_cast<const float4 *>(partial + (int64_t)c0 * stride);
-        const float4 *s4 = reinterpret_cast<const float4 *>(S);
+    // the row's summed partial is one 16-byte aligned (G, h) block, and S is allocated to a multiple of 4 floats: float4
+    // loads, four in flight per thread.  (A scalar loop with a run-time inner trip count sends its 64 loads per thread one
+    // DRAM latency after the other: 0.27 + 1.13 ms per epoch at C3 for what is 0.13 GB of traffic.)
+    const float4 *p4 = reinterpret_cast<const float4 *>(g0);
+    const float4 *s4 = reinterpret_cast<const float4 *>(S);
 #pragma unroll 4
-        for (int e4 = threadIdx.x; e4 < dd / 4; e4 += blockDim.x) {
-            const float4 g = p4[e4], sv = __ldg(s4 + e4);
-            const int e = 4 * e4, i = e / d, j = e - i * d;     // the four elements share row i
-            float a[4] = {omw * g.x + w * sv.x, omw * g.y + w * sv.y, omw * g.z + w * sv.z, omw * g.w + w * sv.w};
+    for (int e4 = threadIdx.x; 4 * e4 < dd; e4 += blockDim.x) {
+        const float4 g = p4[e4], sv = __ldg(s4 + e4);
+        const float a[4] = {omw * g.x + w * sv.x, omw * g.y + w * sv.y, omw * g.z + w * sv.z, omw * g.w + w * sv.w};
+        int i = 4 * e4 / d, j = 4 * e4 - i * d;   // element 4 e4 + q is (i, j) of G, wrapping to the next row at j = d
 #pragma unroll
-            for (int q = 0; q < 4; q++) {
-                if (i == j + q) a[q] += reg;
-                A[i * dp + j + q] = a[q];
-            }
+        for (int q = 0; q < 4; q++) {
+            if (4 * e4 + q < dd) A[i * dp + j] = i == j ? a[q] + reg : a[q];
+            if (++j == d) { i++; j = 0; }
         }
-        for (int e = threadIdx.x; e < d; e += blockDim.x) {
-            h[e] = partial[(int64_t)c0 * stride + dd + e];
-            x[e] = X[(int64_t)r * d + e];
-        }
-    } else {
-        for (int e = threadIdx.x; e < dd; e += blockDim.x) {
-            float g = 0.f;
-            for (int c = c0; c < c1; c++) g += partial[(int64_t)c * stride + e];
-            const int i = e / d, j = e - i * d;
-            float a = omw * g + w * __ldg(S + e);
-            if (i == j) a += reg;
-            A[i * dp + j] = a;
-        }
-        for (int e = threadIdx.x; e < d; e += blockDim.x) {
-            float g = 0.f;
-            for (int c = c0; c < c1; c++) g += partial[(int64_t)c * stride + dd + e];
-            h[e] = g;
-            x[e] = X[(int64_t)r * d + e];
-        }
+    }
+    for (int e = threadIdx.x; e < d; e += blockDim.x) {
+        h[e] = g0[dd + e];
+        x[e] = X[(int64_t)r * d + e];
     }
     __syncthreads();
     const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5, nw = blockDim.x >> 5;
@@ -576,98 +529,98 @@ __global__ void __launch_bounds__(256) als_solve_kernel(float *X, int d, const f
     }
     __syncthreads();
     if (wid == 0) {
-        const int kpl = d >> 5;
+        const int kpl = (d + 31) >> 5;
+        bool ok[4];
         float rr[4], xv[4], inv[4];
 #pragma unroll
         for (int jx = 0; jx < 4; jx++) {
             const int k = lane + 32 * jx;
-            const bool ok = jx < kpl;
-            rr[jx] = ok ? h[k] : 0.f;
-            xv[jx] = ok ? x[k] : 0.f;
-            inv[jx] = ok ? 1.0f / A[k * dp + k] : 0.f;
+            ok[jx] = k < d;
+            rr[jx] = ok[jx] ? h[k] : 0.f;
+            xv[jx] = ok[jx] ? x[k] : 0.f;
+            inv[jx] = ok[jx] ? 1.0f / A[k * dp + k] : 0.f;
         }
+        // the last block stops at f = d - 1 through its trip count.  (A break at f = d inside the unrolled loop keeps the
+        // compiler from issuing the A loads of later steps early, which puts their latency on the chain.)
 #pragma unroll
         for (int jf = 0; jf < 4; jf++) {
             if (jf < kpl) {
+                const int n_o = min(32, d - 32 * jf);
 #pragma unroll 4
-                for (int o = 0; o < 32; o++) {
+                for (int o = 0; o < n_o; o++) {
                     const int f = 32 * jf + o;
                     const float delta = __shfl_sync(0xffffffffu, rr[jf] * inv[jf], o);
                     if (lane == o) xv[jf] += delta;
 #pragma unroll
                     for (int jx = 0; jx < 4; jx++)
-                        if (jx < kpl) rr[jx] = fmaf(-delta, A[(lane + 32 * jx) * dp + f], rr[jx]);
+                        if (ok[jx]) rr[jx] = fmaf(-delta, A[(lane + 32 * jx) * dp + f], rr[jx]);
                 }
             }
         }
 #pragma unroll
         for (int jx = 0; jx < 4; jx++)
-            if (jx < kpl) X[(int64_t)r * d + lane + 32 * jx] = xv[jx];
+            if (ok[jx]) X[(int64_t)r * d + lane + 32 * jx] = xv[jx];
     }
 }
 
-
-// S = sum over rows with >= 1 feedback of x x^T.  `X`, `off` and `rows` describe THIS RANK's row range (off is the rank's
-// rebased offsets); in a distributed context the d x d partial sums are all-reduced, so every rank ends with the same bits.
-static int32_t run_gram(gorse_b200_cf *cf, int side, const float *X_base, const float *X, int32_t rows, const int64_t *off)
+// partial[c] = (G, h) of chunk c: the rows Y[idx[begin[c] + t]], t < len[c]
+static int32_t chunk_gram(gorse_b200_cf *cf, const float *Y, const int32_t *idx, const int64_t *begin, const int32_t *len, int32_t nc)
 {
     gorse_b200_ctx *c = cf->ctx;
-    const int d = cf->d, dd = d * d;
-    if (d == 128) {
-        // S = sum of x x^T over the rows with feedback: the same tensor-core kernel as the row Grams, fed with the list of
-        // those rows in chunks of GB_ALS_CHUNK (als_gram_tc.cu); the chunk partials are summed in order (deterministic)
-        const int nc = cf->als_s_chunks[side];
-        const size_t need = (size_t)std::max(nc, 1) * (dd + d);
-        if (cf->scratch.n < need) GB_TRY(cf->scratch.alloc(need));
-        if (nc > 0) GB_TRY(als_chunk_gram_tc(c, X_base, cf->als_s_rows[side].p, cf->als_s_begin[side].p, cf->als_s_len[side].p, nc, cf->scratch.p));
-        else GB_CUDA(cudaMemsetAsync(cf->scratch.p, 0, sizeof(float) * need, c->stream));
-        gram_reduce_kernel<<<(dd + 255) / 256, 256, 0, c->stream>>>(cf->scratch.p, std::max(nc, 1), dd, (int64_t)dd + d, cf->gram.p);
+    const int d = cf->d;
+    float *partial = cf->als_partial.p;
+    if (d == 128) return als_chunk_gram_tc(c, Y, idx, begin, len, nc, partial);
+    if (d > 128) als_chunk_gram_generic_kernel<<<dim3(nc, div_up(d * d + d, 256)), 256, 0, c->stream>>>(Y, d, idx, begin, len, partial);
+    else if (d > 64) als_chunk_gram_kernel<8><<<nc, 256, sizeof(float) * 16 * 16 * 8, c->stream>>>(Y, d, idx, begin, len, partial);
+    else if (d > 32) als_chunk_gram_kernel<4><<<nc, 256, sizeof(float) * 16 * 16 * 4, c->stream>>>(Y, d, idx, begin, len, partial);
+    else if (d > 16) als_chunk_gram_kernel<2><<<nc, 256, sizeof(float) * 16 * 16 * 2, c->stream>>>(Y, d, idx, begin, len, partial);
+    else als_chunk_gram_kernel<1><<<nc, 256, sizeof(float) * 16 * 16 * 1, c->stream>>>(Y, d, idx, begin, len, partial);
+    GB_LAUNCHED(c);
+    return GORSE_B200_OK;
+}
+
+// S = sum of x x^T over this rank's rows with feedback (X is the whole table): the chunk partials are summed in chunk order,
+// so S is the same every run; in a distributed context the d x d sums are all-reduced, so every rank ends with the same bits.
+static int32_t run_gram(gorse_b200_cf *cf, int side, const float *X)
+{
+    gorse_b200_ctx *c = cf->ctx;
+    const int dd = cf->d * cf->d, nc = cf->als_s_chunks[side];
+    if (nc > 0) {
+        GB_TRY(chunk_gram(cf, X, cf->als_s_rows[side].p, cf->als_s_begin[side].p, cf->als_s_len[side].p, nc));
+        gram_reduce_kernel<<<div_up(dd, 256), 256, 0, c->stream>>>(cf->als_partial.p, nc, dd, als_partial_stride(cf->d), cf->gram.p);
         GB_LAUNCHED(c);
-        if (c->world > 1) {
-            GB_NCCL_API(nc_api);
-            GB_NCCL(nc_api, AllReduce(cf->gram.p, cf->gram.p, (size_t)dd, ncclFloat32, ncclSum, c->comm, c->stream));
-        }
-        return GORSE_B200_OK;
-    }
-    int parts = (int)std::max<int64_t>(1, std::min<int64_t>(((int64_t)rows + 63) / 64, (int64_t)c->sm_count * 2));
-    size_t need = (size_t)parts * dd;
-    if (cf->scratch.n < need) GB_TRY(cf->scratch.alloc(need));
-    if (d <= 128) {
-        int T = d <= 16 ? 1 : d <= 32 ? 2 : d <= 64 ? 4 : 8;
-        size_t sm = sizeof(float) * 16 * 16 * T;
-        switch (T) {
-            case 1: gram_kernel<1><<<parts, 256, sm, c->stream>>>(X, rows, d, off, cf->scratch.p); break;
-            case 2: gram_kernel<2><<<parts, 256, sm, c->stream>>>(X, rows, d, off, cf->scratch.p); break;
-            case 4: gram_kernel<4><<<parts, 256, sm, c->stream>>>(X, rows, d, off, cf->scratch.p); break;
-            default: gram_kernel<8><<<parts, 256, sm, c->stream>>>(X, rows, d, off, cf->scratch.p); break;
-        }
     } else {
-        gram_generic_kernel<<<parts, 256, 0, c->stream>>>(X, rows, d, off, cf->scratch.p);
+        GB_CUDA(cudaMemsetAsync(cf->gram.p, 0, sizeof(float) * dd, c->stream));
     }
-    GB_LAUNCHED(c);
-    gram_reduce_kernel<<<(dd + 255) / 256, 256, 0, c->stream>>>(cf->scratch.p, parts, dd, (int64_t)dd, cf->gram.p);
-    GB_LAUNCHED(c);
     if (c->world > 1) {
-        GB_NCCL_API(nc);
-        GB_NCCL(nc, AllReduce(cf->gram.p, cf->gram.p, (size_t)dd, ncclFloat32, ncclSum, c->comm, c->stream));
+        GB_NCCL_API(nc_api);
+        GB_NCCL(nc_api, AllReduce(cf->gram.p, cf->gram.p, (size_t)dd, ncclFloat32, ncclSum, c->comm, c->stream));
     }
     return GORSE_B200_OK;
 }
 
-// rows bucketed by length, one launch per class:
-//   d % 32 == 0, d <= 128:  n <= 4 | n <= 8 | n <= 16  one THREAD per row (als_thread.cu)
-//                           n <= 32 (16 lanes per row) | n <= 96 (a warp per row)  lane-group form (als_rows_group_blocked_kernel)
-//                           longer -> Gram form
-//   otherwise (als_rows_kernel, one warp per row):  n*(d+1) <= 3072 floats (12 KB/warp) | <= 12288 (48 KB/warp)
-//   longer -> Gram form when d <= 128, else gathered from L2 without staging
-static const int kStageFloats[2] = {3072, 12288};
+// Rows are bucketed by length, one launch per class.  At d % 32 == 0, d <= 128 the short classes are kRowClasses: a row of
+// n entries takes the first class with n <= max_n, run by `launch`.  Lane groups with blocked staging beat the thread-per-row
+// kernel in every class above 4 entries (<= 8: 0.80 vs 1.16 ms, <= 16: 1.27 vs 1.99 ms per half-sweep at C3); the thread
+// kernel keeps the shortest rows, where it is 0.14 ms ahead (also when they are many: the 300 K short user rows of C3 take
+// 1.69 ms there and 2.0 ms on the 8-lane kernel).  33..64 entries are a class of their own: 8.4 instead of 12.7 KB of
+// staging per warp, so 16 warps per SM instead of 12.
+// At other d, als_rows_kernel takes the rows with n (d+1) <= kStageFloats[k] floats (12 / 48 KB per warp) as class k.
+// Longer rows form class GB_ALS_LONG: the Gram form at d <= 128, als_rows_kernel without staging above.
+using RowLauncher = int32_t (*)(gorse_b200_cf *cf, float *X, const float *Y, const int64_t *off, const int32_t *idx, float reg, float w,
+                                const int32_t *rows, int32_t n_rows);
+struct RowClass { int max_n; RowLauncher launch; };
 #define GB_ALS_CLASSES 7
 #define GB_ALS_LONG 6   // index of the long-row class
-// kind 0: thread per row (max_n entries); kind 1: lane group of G lanes, E entries per lane
-struct RowClass { int max_n, kind, G, E; };
-// (33..64 entries are a class of their own since the end of round 2: 8.4 instead of 12.7 KB of staging per warp -> 16 warps
-// per SM instead of 12)
-static const RowClass kRowClasses[GB_ALS_LONG] = {{4, 0, 0, 0}, {8, 0, 0, 0}, {16, 0, 0, 0}, {32, 1, 16, 2}, {64, 1, 32, 2}, {96, 1, 32, 3}};
+static const RowClass kRowClasses[GB_ALS_LONG] = {
+    {4, als_thread_rows},
+    {8, launch_group_blocked_d<8, 1>},
+    {16, launch_group_blocked_d<16, 1>},
+    {32, launch_group_blocked_d<16, 2>},
+    {64, launch_group_blocked_d<32, 2>},
+    {96, launch_group_blocked_d<32, 3>},
+};
+static const int kStageFloats[2] = {3072, 12288};
 
 static bool als_grouped(const gorse_b200_cf *cf) { return cf->d % 32 == 0 && cf->d <= 128; }
 
@@ -678,21 +631,39 @@ static void shard_range(const gorse_b200_cf *cf, int side, int32_t &lo, int32_t 
     hi = side == 0 ? cf->u_hi : cf->i_hi;
 }
 
+// [b, e) in chunks of at most GB_ALS_CHUNK
+static void cut_chunks(int64_t b, int64_t e, std::vector<int64_t> &begin, std::vector<int32_t> &len)
+{
+    for (int64_t p = b; p < e; p += GB_ALS_CHUNK) {
+        begin.push_back(p);
+        len.push_back((int32_t)std::min<int64_t>(GB_ALS_CHUNK, e - p));
+    }
+}
+
+template <typename T>
+static int32_t upload(DevBuf<T> &dst, const std::vector<T> &src)
+{
+    GB_TRY(dst.alloc(src.size()));
+    if (!src.empty()) GB_CUDA(cudaMemcpy(dst.p, src.data(), sizeof(T) * src.size(), cudaMemcpyHostToDevice));
+    return GORSE_B200_OK;
+}
+
 static int32_t prepare_als(gorse_b200_cf *cf)
 {
     if (cf->als_ready) return GORSE_B200_OK;
-    const int dp = cf->d + 1;
+    const int d = cf->d, dp = d + 1;
     const bool grouped = als_grouped(cf);
+    int32_t max_chunks = 0;
     for (int side = 0; side < 2; side++) {
-        // host offsets hold this rank's rows only, rebased: row r sits at index r - r_lo
-        const int64_t *off = (side == 0 ? cf->h_user_off : cf->h_item_off).data();
-        std::vector<int32_t> cls[GB_ALS_CLASSES];
-        // multi-rank: this rank updates its own range of users and of items only (SURVEY 8e)
+        // multi-rank: this rank updates its own range of users and of items only (SURVEY 8e).  The host offsets hold this
+        // rank's rows only, rebased: row r sits at index r - r_lo
         int32_t r_lo = 0, r_hi = 0;
         shard_range(cf, side, r_lo, r_hi);
-        off -= r_lo;
+        const int64_t *off = (side == 0 ? cf->h_user_off : cf->h_item_off).data() - r_lo;
+        std::vector<int32_t> cls[GB_ALS_CLASSES], s_rows;
         for (int32_t r = r_lo; r < r_hi; r++) {
-            int64_t n = off[(size_t)r + 1] - off[r];
+            const int64_t n = off[(size_t)r + 1] - off[r];
+            if (n > 0) s_rows.push_back(r);   // the rows S sums over (model.go:651,699)
             int k;
             if (grouped) {
                 k = GB_ALS_LONG;
@@ -706,129 +677,68 @@ static int32_t prepare_als(gorse_b200_cf *cf)
                 return off[(size_t)a + 1] - off[a] > off[(size_t)b + 1] - off[b];
             });
             cf->als_rows_n[side][k] = (int32_t)cls[k].size();
-            GB_TRY(cf->als_rows[side][k].alloc(cls[k].size()));
-            if (!cls[k].empty())
-                GB_CUDA(cudaMemcpy(cf->als_rows[side][k].p, cls[k].data(), sizeof(int32_t) * cls[k].size(), cudaMemcpyHostToDevice));
+            GB_TRY(upload(cf->als_rows[side][k], cls[k]));
         }
-    }
-    // long rows take the Gram form when d <= 128: cut them into chunks
-    for (int side = 0; side < 2 && cf->d <= 128; side++) {
-        const int64_t *off = (side == 0 ? cf->h_user_off : cf->h_item_off).data() - (side == 0 ? cf->u_lo : cf->i_lo);
-        std::vector<int32_t> rows((size_t)cf->als_rows_n[side][GB_ALS_LONG]);
-        if (rows.empty()) continue;
-        GB_CUDA(cudaMemcpy(rows.data(), cf->als_rows[side][GB_ALS_LONG].p, sizeof(int32_t) * rows.size(), cudaMemcpyDeviceToHost));
-        std::vector<int32_t> chunk_row, chunk_len, row_chunk0;
-        std::vector<int64_t> chunk_begin;
-        for (size_t i = 0; i < rows.size(); i++) {
-            row_chunk0.push_back((int32_t)chunk_row.size());
-            const int64_t b = off[(size_t)rows[i]], e = off[(size_t)rows[i] + 1];
-            for (int64_t p = b; p < e; p += GB_ALS_CHUNK) {
-                chunk_row.push_back(rows[i]);
-                chunk_begin.push_back(p);
-                chunk_len.push_back((int32_t)std::min<int64_t>(GB_ALS_CHUNK, e - p));
+        // long rows take the Gram form when d <= 128: their entries in chunks, row i's from chunk row_chunk0[i] on
+        std::vector<int64_t> chunk_begin, s_begin;
+        std::vector<int32_t> chunk_len, row_chunk0, s_len;
+        if (d <= 128) {
+            for (const int32_t r : cls[GB_ALS_LONG]) {
+                row_chunk0.push_back((int32_t)chunk_begin.size());
+                cut_chunks(off[r], off[(size_t)r + 1], chunk_begin, chunk_len);
             }
+            row_chunk0.push_back((int32_t)chunk_begin.size());
         }
-        row_chunk0.push_back((int32_t)chunk_row.size());
-        cf->als_n_chunks[side] = (int32_t)chunk_row.size();
-        GB_TRY(cf->als_chunk_row[side].alloc(chunk_row.size()));
-        GB_TRY(cf->als_chunk_len[side].alloc(chunk_len.size()));
-        GB_TRY(cf->als_chunk_begin[side].alloc(chunk_begin.size()));
-        GB_TRY(cf->als_row_chunk0[side].alloc(row_chunk0.size()));
-        GB_CUDA(cudaMemcpy(cf->als_chunk_row[side].p, chunk_row.data(), sizeof(int32_t) * chunk_row.size(), cudaMemcpyHostToDevice));
-        GB_CUDA(cudaMemcpy(cf->als_chunk_len[side].p, chunk_len.data(), sizeof(int32_t) * chunk_len.size(), cudaMemcpyHostToDevice));
-        GB_CUDA(cudaMemcpy(cf->als_chunk_begin[side].p, chunk_begin.data(), sizeof(int64_t) * chunk_begin.size(), cudaMemcpyHostToDevice));
-        GB_CUDA(cudaMemcpy(cf->als_row_chunk0[side].p, row_chunk0.data(), sizeof(int32_t) * row_chunk0.size(), cudaMemcpyHostToDevice));
+        cut_chunks(0, (int64_t)s_rows.size(), s_begin, s_len);
+        cf->als_n_chunks[side] = (int32_t)chunk_begin.size();
+        cf->als_s_chunks[side] = (int32_t)s_begin.size();
+        max_chunks = std::max({max_chunks, cf->als_n_chunks[side], cf->als_s_chunks[side]});
+        GB_TRY(upload(cf->als_chunk_begin[side], chunk_begin));
+        GB_TRY(upload(cf->als_chunk_len[side], chunk_len));
+        GB_TRY(upload(cf->als_row_chunk0[side], row_chunk0));
+        GB_TRY(upload(cf->als_s_rows[side], s_rows));
+        GB_TRY(upload(cf->als_s_begin[side], s_begin));
+        GB_TRY(upload(cf->als_s_len[side], s_len));
     }
-    {
-        const size_t need = (size_t)std::max(cf->als_n_chunks[0], cf->als_n_chunks[1]) * ((size_t)cf->d * cf->d + cf->d);
-        if (need) GB_TRY(cf->als_partial.alloc(need));
-    }
-    // rows with feedback of this rank's range (the rows S sums over, model.go:651,699), cut into chunks for the tensor-core Gram
-    for (int side = 0; side < 2 && cf->d == 128; side++) {
-        int32_t r_lo = 0, r_hi = 0;
-        shard_range(cf, side, r_lo, r_hi);
-        const int64_t *off = (side == 0 ? cf->h_user_off : cf->h_item_off).data() - r_lo;
-        std::vector<int32_t> rows, len;
-        std::vector<int64_t> begin;
-        for (int32_t r = r_lo; r < r_hi; r++) if (off[(size_t)r + 1] > off[r]) rows.push_back(r);
-        for (size_t p = 0; p < rows.size(); p += GB_ALS_CHUNK) { begin.push_back((int64_t)p); len.push_back((int32_t)std::min<size_t>(GB_ALS_CHUNK, rows.size() - p)); }
-        cf->als_s_chunks[side] = (int32_t)begin.size();
-        GB_TRY(cf->als_s_rows[side].alloc(rows.size()));
-        GB_TRY(cf->als_s_begin[side].alloc(begin.size()));
-        GB_TRY(cf->als_s_len[side].alloc(len.size()));
-        if (!rows.empty()) {
-            GB_CUDA(cudaMemcpy(cf->als_s_rows[side].p, rows.data(), sizeof(int32_t) * rows.size(), cudaMemcpyHostToDevice));
-            GB_CUDA(cudaMemcpy(cf->als_s_begin[side].p, begin.data(), sizeof(int64_t) * begin.size(), cudaMemcpyHostToDevice));
-            GB_CUDA(cudaMemcpy(cf->als_s_len[side].p, len.data(), sizeof(int32_t) * len.size(), cudaMemcpyHostToDevice));
-        }
-    }
+    GB_TRY(cf->als_partial.alloc((size_t)max_chunks * als_partial_stride(d)));
+    GB_TRY(cf->gram.alloc(((size_t)d * d + 3) & ~(size_t)3));   // a multiple of 4 floats: als_solve_kernel reads S as float4
     GB_CUDA(cudaFuncSetAttribute(als_solve_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
-    GB_TRY(cf->gram.alloc((size_t)cf->d * cf->d));
     GB_CUDA(cudaFuncSetAttribute(als_rows_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024));
     cf->als_ready = true;
     return GORSE_B200_OK;
 }
 
-// (Round 1's whole-row lane-group kernel and its B = 4 variant -- four coordinates per shuffle butterfly, 72 vs 43 ms/epoch --
-// are gone: the blocked-staging kernel above replaced them in every class.)
 static int32_t run_rows(gorse_b200_cf *cf, int side, float *X, const float *Y, const int64_t *off, const int32_t *idx,
                         float reg, float w, float *pred_scratch)
 {
     gorse_b200_ctx *c = cf->ctx;
+    const int d = cf->d;
     const bool grouped = als_grouped(cf);
     for (int k = 0; k < GB_ALS_CLASSES; k++) {
-        int32_t n_rows = cf->als_rows_n[side][k];
+        const int32_t n_rows = cf->als_rows_n[side][k];
         if (n_rows == 0) continue;
         const int32_t *rows = cf->als_rows[side][k].p;
-        if (k == GB_ALS_LONG && cf->als_n_chunks[side] > 0) {
-            const int d = cf->d, T = d <= 16 ? 1 : d <= 32 ? 2 : d <= 64 ? 4 : 8;
-            const size_t gsm = sizeof(float) * 16 * 16 * T;
-            const int nc = cf->als_n_chunks[side];
-            auto *ck = als_chunk_gram_kernel<1>;
-                switch (T) {
-                case 1: break;
-                case 2: ck = als_chunk_gram_kernel<2>; break;
-                case 4: ck = als_chunk_gram_kernel<4>; break;
-                default: ck = als_chunk_gram_kernel<8>; break;
-            }
-            if (d == 128) {
-                GB_TRY(als_chunk_gram_tc(c, Y, idx, cf->als_chunk_begin[side].p, cf->als_chunk_len[side].p, nc, cf->als_partial.p));
-            } else {
-                ck<<<nc, 256, gsm, c->stream>>>(Y, d, idx, cf->als_chunk_row[side].p, cf->als_chunk_begin[side].p, cf->als_chunk_len[side].p, cf->als_partial.p);
-                GB_LAUNCHED(c);
-            }
-            const size_t ssm = sizeof(float) * ((size_t)d * (d + 1) + 2 * d);
-            const int reduced = (d * d + d) % 4 == 0;
-            if (reduced) {
-                als_partial_reduce_kernel<<<dim3(n_rows, div_up((d * d + d) / 4, 256)), 256, 0, c->stream>>>(cf->als_row_chunk0[side].p, (d * d + d) / 4, cf->als_partial.p);
-                GB_LAUNCHED(c);
-            }
-            als_solve_kernel<<<n_rows, 256, ssm, c->stream>>>(X, d, cf->gram.p, reg, w, rows, cf->als_row_chunk0[side].p, cf->als_partial.p, reduced);
-            GB_LAUNCHED(c);
-            continue;
-        }
         if (grouped && k != GB_ALS_LONG) {
-            const RowClass rc = kRowClasses[k];
-            // A/B: lane groups with blocked staging beat the thread-per-row kernel in
-            // every class above 4 entries (<=8: 0.80 vs 1.16 ms, <=16: 1.27 vs 1.99 ms per half-sweep at C3) and the
-            // whole-row staging of the first lane-group kernels in the two longer classes; the thread kernel keeps the
-            // shortest rows, where it is 0.14 ms ahead (also when they are many: the 300 K short user rows of C3 take 1.69 ms
-            // there and 2.0 ms on the 8-lane kernel).
-            if (rc.kind == 0 && rc.max_n <= 4) GB_TRY(als_thread_rows(c, cf->d, rc.max_n, X, Y, off, idx, cf->gram.p, reg, w, rows, n_rows));
-            else if (rc.kind == 0 && rc.max_n <= 8) GB_TRY((launch_group_blocked_d<8, 1>(cf, X, Y, off, idx, reg, w, rows, n_rows)));
-            else if (rc.kind == 0) GB_TRY((launch_group_blocked_d<16, 1>(cf, X, Y, off, idx, reg, w, rows, n_rows)));
-            else if (rc.G == 16) GB_TRY((launch_group_blocked_d<16, 2>(cf, X, Y, off, idx, reg, w, rows, n_rows)));
-            else if (rc.E == 2) GB_TRY((launch_group_blocked_d<32, 2>(cf, X, Y, off, idx, reg, w, rows, n_rows)));
-            else GB_TRY((launch_group_blocked_d<32, 3>(cf, X, Y, off, idx, reg, w, rows, n_rows)));
-            continue;
+            GB_TRY(kRowClasses[k].launch(cf, X, Y, off, idx, reg, w, rows, n_rows));
+        } else if (k == GB_ALS_LONG && d <= 128) {
+            // Gram form: chunk partials, summed per row into its first chunk, then one sweep per row
+            const int32_t *row_chunk0 = cf->als_row_chunk0[side].p;
+            const int stride4 = als_partial_stride(d) / 4;
+            GB_TRY(chunk_gram(cf, Y, idx, cf->als_chunk_begin[side].p, cf->als_chunk_len[side].p, cf->als_n_chunks[side]));
+            als_partial_reduce_kernel<<<dim3(n_rows, div_up(stride4, 256)), 256, 0, c->stream>>>(row_chunk0, stride4, cf->als_partial.p);
+            GB_LAUNCHED(c);
+            const size_t sm = sizeof(float) * ((size_t)d * (d + 1) + 2 * d);
+            als_solve_kernel<<<n_rows, 256, sm, c->stream>>>(X, d, cf->gram.p, reg, w, rows, row_chunk0, cf->als_partial.p);
+            GB_LAUNCHED(c);
+        } else {
+            // one warp per row; the long class (d > 128) gathers from L2 without staging
+            const int stage = k == GB_ALS_LONG ? 0 : kStageFloats[k];
+            const size_t sm = sizeof(float) * GB_ALS_WARPS * (size_t)(d + stage);
+            const int ctas_per_sm = k == 0 ? 4 : 1;
+            const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((n_rows + GB_ALS_WARPS - 1) / GB_ALS_WARPS, (int64_t)c->sm_count * ctas_per_sm * (k == GB_ALS_LONG ? 8 : 1)));
+            als_rows_kernel<<<grid, 32 * GB_ALS_WARPS, sm, c->stream>>>(X, Y, d, off, idx, cf->gram.p, reg, w, rows, n_rows, stage, pred_scratch);
+            GB_LAUNCHED(c);
         }
-        // one warp per row; the long class without a Gram form (d > 128) gathers from L2 without staging
-        const int stage = k == GB_ALS_LONG ? 0 : kStageFloats[k];
-        size_t sm = sizeof(float) * GB_ALS_WARPS * (size_t)(cf->d + stage);
-        int ctas_per_sm = k == 0 ? 4 : 1;
-        int grid = (int)std::max<int64_t>(1, std::min<int64_t>((n_rows + GB_ALS_WARPS - 1) / GB_ALS_WARPS, (int64_t)c->sm_count * ctas_per_sm * (k == GB_ALS_LONG ? 8 : 1)));
-        als_rows_kernel<<<grid, 32 * GB_ALS_WARPS, sm, c->stream>>>(X, Y, cf->d, 0, 0, off, idx, cf->gram.p, reg, w, rows, n_rows, stage, pred_scratch);
-        GB_LAUNCHED(c);
     }
     return GORSE_B200_OK;
 }
@@ -892,10 +802,10 @@ extern "C" int32_t gorse_b200_als_epoch(gorse_b200_cf *cf, float reg, float alph
     }
     // the row kernels index the offsets with GLOBAL row ids: hand them the rank's arrays shifted by the range start
     const int64_t *uoff = cf->user_off.p - cf->u_lo, *ioff = cf->item_off.p - cf->i_lo;
-    if ((st = run_gram(cf, 1, cf->Q.p, cf->Q.p + (int64_t)cf->i_lo * cf->d, cf->i_hi - cf->i_lo, cf->item_off.p))) return done(st);
+    if ((st = run_gram(cf, 1, cf->Q.p))) return done(st);
     if ((st = run_rows(cf, 0, P, cf->Q.p, uoff, cf->user_items.p, reg, alpha, pred.p))) return done(st);
     if (multi && (st = exchange_shards(cf, 0, P))) return done(st);
-    if ((st = run_gram(cf, 0, P, P + (int64_t)cf->u_lo * cf->d, cf->u_hi - cf->u_lo, cf->user_off.p))) return done(st);
+    if ((st = run_gram(cf, 0, P))) return done(st);
     if ((st = run_rows(cf, 1, cf->Q.p, P, ioff, cf->item_users.p, reg, alpha, pred.p))) return done(st);
     if (multi) {
         if ((st = exchange_shards(cf, 1, cf->Q.p))) return done(st);

@@ -16,10 +16,10 @@
 // G ~= hi hi^T + hi lo^T + lo hi^T, three MMAs per k-step into the same accumulator.  Dropped: lo lo^T and the rounding of
 // lo, both <= 2^-22 relative per product and of random sign.
 //
-// One CTA = one chunk (<= GB_ALS_CHUNK entries of one row): 256 threads gather KT = 32 entries per stage into registers,
+// One CTA = one chunk (<= GB_ALS_CHUNK entries of one row, or rows with feedback for S): 256 threads gather KT = 32 entries per stage into registers,
 // split them into the hi and lo tiles of a 3-stage ring and issue the stage's 12 MMAs per warpgroup asynchronously; the
 // gather of the next stage overlaps them.  Epilogue: each thread stores its accumulator fragment straight into the partial
-// (G, h) buffer als_solve_kernel sums.
+// (G, h) buffer that gram_reduce_kernel (for S) or als_partial_reduce_kernel (for a long row) sums.
 #include "als.cuh"
 #include "wgmma.cuh"
 
@@ -100,7 +100,7 @@ als_chunk_gram_tc_kernel(const float *Y, const int32_t *idx, const int64_t *chun
         wgmma_commit();
     }
     wgmma_wait<0>();
-    float *out = partial + (int64_t)blockIdx.x * (TC_D * TC_D + TC_D);
+    float *out = partial + (int64_t)blockIdx.x * als_partial_stride(TC_D);
     if (n_stage == 0) {
 #pragma unroll
         for (int e = 0; e < 64; e++) acc[e] = 0.f;

@@ -194,28 +194,20 @@ static int32_t launch_thread_rows(gorse_b200_ctx *c, float *X, const float *Y, c
     return GORSE_B200_OK;
 }
 
-template <int D>
-static int32_t launch_thread_d(gorse_b200_ctx *c, int nmax, float *X, const float *Y, const int64_t *off, const int32_t *idx,
-                               const float *S, float reg, float w, const int32_t *rows, int32_t n_rows)
+// rows with at most 4 entries, d in {32, 64, 96, 128}.  Only the shortest class runs here: NMAX = 8 / 16 (staging blocks of
+// 16 / 8 coordinates) lost to the lane-group kernels with blocked staging, 1.16 vs 0.80 and 1.99 vs 1.27 ms per half-sweep at C3.
+int32_t als_thread_rows(gorse_b200_cf *cf, float *X, const float *Y, const int64_t *off, const int32_t *idx, float reg, float w,
+                        const int32_t *rows, int32_t n_rows)
 {
-    // Only the shortest class runs here since the end of round 2: NMAX = 8 / 16 (staging blocks of 16 / 8 coordinates) lost
-    // to the lane-group kernels with blocked staging, 1.16 vs 0.80 and 1.99 vs 1.27 ms per half-sweep at C3.
-    if (nmax <= 4) return launch_thread_rows<D, 4, 32>(c, X, Y, off, idx, S, reg, w, rows, n_rows);
-    set_error("als_thread_rows: rows of up to %d entries do not run on the thread-per-row kernel", nmax);
-    return GORSE_B200_ERR_UNSUPPORTED;
-}
-
-// rows with at most `nmax` (<= 4) entries, d in {32, 64, 96, 128}
-int32_t als_thread_rows(gorse_b200_ctx *c, int d, int nmax, float *X, const float *Y, const int64_t *off, const int32_t *idx,
-                        const float *S, float reg, float w, const int32_t *rows, int32_t n_rows)
-{
-    switch (d) {
-        case 32: return launch_thread_d<32>(c, nmax, X, Y, off, idx, S, reg, w, rows, n_rows);
-        case 64: return launch_thread_d<64>(c, nmax, X, Y, off, idx, S, reg, w, rows, n_rows);
-        case 96: return launch_thread_d<96>(c, nmax, X, Y, off, idx, S, reg, w, rows, n_rows);
-        case 128: return launch_thread_d<128>(c, nmax, X, Y, off, idx, S, reg, w, rows, n_rows);
+    gorse_b200_ctx *c = cf->ctx;
+    const float *S = cf->gram.p;
+    switch (cf->d) {
+        case 32: return launch_thread_rows<32, 4, 32>(c, X, Y, off, idx, S, reg, w, rows, n_rows);
+        case 64: return launch_thread_rows<64, 4, 32>(c, X, Y, off, idx, S, reg, w, rows, n_rows);
+        case 96: return launch_thread_rows<96, 4, 32>(c, X, Y, off, idx, S, reg, w, rows, n_rows);
+        case 128: return launch_thread_rows<128, 4, 32>(c, X, Y, off, idx, S, reg, w, rows, n_rows);
     }
-    set_error("als_thread_rows: unsupported d = %d", d);
+    set_error("als_thread_rows: unsupported d = %d", cf->d);
     return GORSE_B200_ERR_UNSUPPORTED;
 }
 

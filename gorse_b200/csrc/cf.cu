@@ -271,10 +271,10 @@ int32_t gorse_b200_cf_destroy(gorse_b200_cf *cf)
     cf->P.free(); cf->Q.free(); cf->Q0.free(); cf->item_rate.free(); cf->xchg.free(); cf->P_all.free();
     cf->user_off.free(); cf->item_off.free();
     cf->user_items.free(); cf->item_users.free(); cf->active.free(); cf->user_meta.free();
-    cf->gram.free(); cf->scratch.free();
+    cf->gram.free();
     for (int a = 0; a < 2; a++) {
         for (int b = 0; b < 7; b++) cf->als_rows[a][b].free();
-        cf->als_chunk_row[a].free(); cf->als_chunk_len[a].free(); cf->als_row_chunk0[a].free(); cf->als_chunk_begin[a].free();
+        cf->als_chunk_len[a].free(); cf->als_row_chunk0[a].free(); cf->als_chunk_begin[a].free();
         cf->als_s_rows[a].free(); cf->als_s_len[a].free(); cf->als_s_begin[a].free();
     }
     cf->als_partial.free(); cf->als_pred.free();

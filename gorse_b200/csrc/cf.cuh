@@ -52,16 +52,16 @@ struct gorse_b200_cf {
     // ALS scratch
     gb::DevBuf<float> gram;      // d x d
     gb::DevBuf<float> als_pred;  // eALS scratch: one prediction per entry of the longer CSR side, kept across epochs
-    gb::DevBuf<float> scratch;   // per-row pred/res for long rows + partial grams
     gb::DevBuf<int32_t> als_rows[2][7];  // [side][class] row ids bucketed by length (built lazily; als.cu prepare_als)
     int32_t als_rows_n[2][7] = {{0, 0, 0, 0, 0, 0, 0}, {0, 0, 0, 0, 0, 0, 0}};
     bool als_ready = false;
-    // long rows in Gram form: chunk work list per side and the partial (G, h) scratch
+    // long rows in Gram form (d <= 128): chunk work list per side
     int32_t als_n_chunks[2] = {0, 0};
-    gb::DevBuf<int32_t> als_chunk_row[2], als_chunk_len[2], als_row_chunk0[2];
+    gb::DevBuf<int32_t> als_chunk_len[2], als_row_chunk0[2];
     gb::DevBuf<int64_t> als_chunk_begin[2];
+    // one partial (G, h) per chunk, of a long row or of S, als_partial_stride(d) floats apart
     gb::DevBuf<float> als_partial;
-    // rows with feedback, in chunks: what S = sum x x^T runs over on the tensor cores (d = 128)
+    // rows with feedback, in chunks: what S = sum x x^T runs over
     int32_t als_s_chunks[2] = {0, 0};
     gb::DevBuf<int32_t> als_s_rows[2], als_s_len[2];
     gb::DevBuf<int64_t> als_s_begin[2];

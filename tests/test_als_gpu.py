@@ -49,11 +49,11 @@ def test_one_epoch_matches_oracle(gb, orc, ctx, d, U, I, R):
     assert np.isfinite(P2).all() and not np.array_equal(P1, P)
 
 
-def test_long_rows_take_every_row_class(gb, orc, ctx):
+def check_long_rows(gb, orc, ctx, d):
     # a hot item with thousands of users (no shared-memory staging) next to tiny rows
     from gorse_b200 import synth
 
-    U, I, d = 3000, 40, 32
+    U, I = 3000, 40
     off, items = synth.make_feedback(U, I, 20000, seed=3, zipf_s=1.3)
     ioff, iusers = gb.transpose_csr(off, items, I)
     assert np.diff(ioff).max() > 1500
@@ -67,6 +67,18 @@ def test_long_rows_take_every_row_class(gb, orc, ctx):
     Po, Qo = P.copy(), Q.copy()
     orc.als_epoch(Po, Qo, off, items, ioff, iusers, 0.06, 0.01)
     assert rel_err(P1, Po) < 1e-4 and rel_err(Q1, Qo) < 1e-4, (rel_err(P1, Po), rel_err(Q1, Qo))
+
+
+def test_long_rows_take_every_row_class(gb, orc, ctx):
+    check_long_rows(gb, orc, ctx, 32)
+
+
+# Below d = 128 the long rows take the Gram form: d = 16 / 10 / 48 check that it updates every coordinate when d is not a
+# multiple of 32, d = 10 that the partial stride is padded (10 * 11 floats is not a multiple of 4); d = 160 takes S and the
+# long rows above 128.
+@pytest.mark.parametrize("d", [16, 10, 48, 160])
+def test_long_rows_at_other_d(gb, orc, ctx, d):
+    check_long_rows(gb, orc, ctx, d)
 
 
 def test_deterministic_run_to_run(gb, orc, ctx):
