@@ -4,12 +4,11 @@
 // Roofline class: HBM/L2 bandwidth.  Algorithmic bytes per triple = 6*d*4 + 12 (3 rows read, 3 rows
 // written, 3 ids).  One quad (4 lanes) owns one triple; see cf.cuh for the row->lane mapping that keeps
 // the reference's AVX-512 summation order with 128-bit coalesced loads.
-#include <cooperative_groups.h>
-
 #include <algorithm>
 #include <cstdlib>
 
 #include "cf.cuh"
+#include "wgmma.cuh"
 
 namespace gb {
 
@@ -83,28 +82,37 @@ __device__ __forceinline__ float bpr_grad_rows(const Rows<C> &r, unsigned mask)
     return bpr_grad(__fsub_rn(quad_tree(ai, mask), quad_tree(aj, mask)));
 }
 
+// chunk c of the three update directions of one triple: row += lr * t for q_i, q_j, p_u
+template <int C>
+__device__ __forceinline__ void bpr_dirs(const Rows<C> &r, int c, float g, float nreg, float4 &ti, float4 &tj, float4 &tp)
+{
+    const float4 *p = r.p, *qi = r.qi, *qj = r.qj;
+    const float ng = -g;
+    // :477-479  q_i += lr * (g*p - reg*q_i)
+    GB_F4_OP(ti, __fmaf_rn(f4get(qi[c], k_), nreg, __fmul_rn(g, f4get(p[c], k_))));
+    // :481-483  q_j += lr * (-g*p - reg*q_j)
+    GB_F4_OP(tj, __fmaf_rn(f4get(qj[c], k_), nreg, __fmul_rn(ng, f4get(p[c], k_))));
+    // :485-488  p_u += lr * (g*(q_i - q_j) - reg*p_u)
+    GB_F4_OP(tp, __fmaf_rn(f4get(p[c], k_), nreg, __fmul_rn(__fsub_rn(f4get(qi[c], k_), f4get(qj[c], k_)), g)));
+}
+
 // the three row updates of one triple (:477-488), from the rows in registers and the gradient factor g
 template <int C, bool ATOMIC>
 __device__ __forceinline__ void bpr_scatter_rows(const Rows<C> &r, float g, float *Pu, float *Qi, int si, float *Qj, int sj,
                                                  float lr, float reg)
 {
     const float4 *p = r.p, *qi = r.qi, *qj = r.qj;
-    const float ng = -g, nreg = -reg;
+    const float nreg = -reg;
 #pragma unroll
     for (int c = 0; c < C; c++) {
-        float4 t, o;
-        // :477-479  q_i += lr * (g*p - reg*q_i)
-        GB_F4_OP(t, __fmaf_rn(f4get(qi[c], k_), nreg, __fmul_rn(g, f4get(p[c], k_))));
-        if (ATOMIC) { GB_F4_OP(o, __fmul_rn(f4get(t, k_), lr)); red_row(Qi + si * c, o); }
-        else { GB_F4_OP(o, __fmaf_rn(f4get(t, k_), lr, f4get(qi[c], k_))); st_row(Qi + si * c, o); }
-        // :481-483  q_j += lr * (-g*p - reg*q_j)
-        GB_F4_OP(t, __fmaf_rn(f4get(qj[c], k_), nreg, __fmul_rn(ng, f4get(p[c], k_))));
-        if (ATOMIC) { GB_F4_OP(o, __fmul_rn(f4get(t, k_), lr)); red_row(Qj + sj * c, o); }
-        else { GB_F4_OP(o, __fmaf_rn(f4get(t, k_), lr, f4get(qj[c], k_))); st_row(Qj + sj * c, o); }
-        // :485-488  p_u += lr * (g*(q_i - q_j) - reg*p_u)
-        GB_F4_OP(t, __fmaf_rn(f4get(p[c], k_), nreg, __fmul_rn(__fsub_rn(f4get(qi[c], k_), f4get(qj[c], k_)), g)));
-        if (ATOMIC) { GB_F4_OP(o, __fmul_rn(f4get(t, k_), lr)); red_row(Pu + 16 * c, o); }
-        else { GB_F4_OP(o, __fmaf_rn(f4get(t, k_), lr, f4get(p[c], k_))); st_row(Pu + 16 * c, o); }
+        float4 ti, tj, tp, o;
+        bpr_dirs<C>(r, c, g, nreg, ti, tj, tp);
+        if (ATOMIC) { GB_F4_OP(o, __fmul_rn(f4get(ti, k_), lr)); red_row(Qi + si * c, o); }
+        else { GB_F4_OP(o, __fmaf_rn(f4get(ti, k_), lr, f4get(qi[c], k_))); st_row(Qi + si * c, o); }
+        if (ATOMIC) { GB_F4_OP(o, __fmul_rn(f4get(tj, k_), lr)); red_row(Qj + sj * c, o); }
+        else { GB_F4_OP(o, __fmaf_rn(f4get(tj, k_), lr, f4get(qj[c], k_))); st_row(Qj + sj * c, o); }
+        if (ATOMIC) { GB_F4_OP(o, __fmul_rn(f4get(tp, k_), lr)); red_row(Pu + 16 * c, o); }
+        else { GB_F4_OP(o, __fmaf_rn(f4get(tp, k_), lr, f4get(p[c], k_))); st_row(Pu + 16 * c, o); }
     }
 }
 
@@ -237,39 +245,169 @@ __global__ void __launch_bounds__(256) bpr_epoch_kernel(BprView v, int64_t step0
     }
 }
 
+// ---- the round epoch ------------------------------------------------------------------------------
+// A CTA of bpr_round_kernel is 8 consumer warps (64 quads: one triple each per round) and sampler warps (one thread per
+// quad and round).  The samplers draw the CTA's triples up to kRing rounds ahead into a shared-memory ring, prefetch the rows those
+// triples will gather into L2, and link the entries of a round that update the same item row, so that the consumers sum
+// those deltas in shared memory and send one reduction per distinct item row and CTA.
+constexpr int kRoundQuads = 64, kConsumers = 4 * kRoundQuads, kSamplers = kRoundQuads;
+// one sampler thread draws one triple per round, a chain of 3-4 dependent loads that takes about as long as a round:
+// two groups of samplers take alternate rounds
+constexpr int kSamplerGroups = 2, kRoundThreads = kConsumers + kSamplerGroups * kSamplers;
+constexpr int kRing = 2 * kSamplerGroups;
+constexpr int kConsumerBar = 1, kSamplerBar0 = 2;   // named barriers (0 is __syncthreads; kSamplerBar0 + g for sampler group g)
+
+// one round of one CTA, as the samplers hand it to the consumers.  Entry e of the item arrays is the Q row that triple e
+// (e < 64: its positive i) or triple e - 64 (its negative j) updates; -1 when the triple has no update (no valid
+// negative, or past the last step).
+struct __align__(16) RoundSlot {
+    int32_t u[kRoundQuads];
+    int32_t item[2 * kRoundQuads];
+    int32_t next[2 * kRoundQuads];    // the next entry with the same item, -1 at the end of the chain
+    uint8_t first[2 * kRoundQuads];   // 1 when no earlier entry has the same item: this entry sends the row's sum
+};
+
+__device__ __forceinline__ void consumer_bar() { asm volatile("bar.sync %0, %1;" ::"n"(kConsumerBar), "n"(kConsumers) : "memory"); }
+__device__ __forceinline__ void sampler_bar(int group) { asm volatile("bar.sync %0, %1;" ::"r"(kSamplerBar0 + group), "n"(kSamplers) : "memory"); }
+
+// Grid barrier over the consumer threads only (the samplers run ahead and never join it): `count` starts at 0 and
+// `target` is the number of the barrier within the launch times the grid size.
+__device__ __forceinline__ void consumer_grid_sync(uint32_t *count, uint32_t target)
+{
+    consumer_bar();
+    if (threadIdx.x == 0) {
+        asm volatile("fence.acq_rel.gpu;\n\tred.release.gpu.global.add.u32 [%0], 1;" ::"l"(count) : "memory");
+        uint32_t seen;
+        do {
+            asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(seen) : "l"(count) : "memory");
+        } while ((int32_t)(seen - target) < 0);
+    }
+    consumer_bar();
+}
+
+__device__ __forceinline__ void prefetch_l2(const float *p, uint32_t bytes)
+{
+    asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(p), "r"(bytes) : "memory");
+}
+
 // The epoch with atomic scatter, in rounds of one triple per quad of the (co-resident) grid: every triple of a round reads
 // its rows as the previous round left them, a grid-wide barrier separates those reads from the round's additions, and a
 // second one ends the round.  What a triple reads therefore depends only on the step stream and the round size, not on
 // timing; the order of the float additions into a row that several triples of one round update is the only freedom left
 // (rounding).  The round size bounds the staleness of a popular row: at GB_BPR_ROUND triples the most popular item of a
 // Zipf(1) catalogue of 10^5 items takes ~700 updates from one copy per round, lr * reg * 700 << 2.
+// Dynamic shared memory: the round's item-row deltas, 2 * kRoundQuads rows of d floats.
 template <int C>
-__global__ void __launch_bounds__(256) bpr_round_kernel(BprView v, int64_t step0, int64_t n_steps, uint64_t base, float lr, float reg)
+__global__ void __launch_bounds__(kRoundThreads, 1)
+    bpr_round_kernel(BprView v, int64_t step0, int64_t n_steps, uint64_t base, float lr, float reg, uint32_t *barrier_count)
 {
-    namespace cg = cooperative_groups;
-    cg::grid_group grid = cg::this_grid();
-    const int lane4 = threadIdx.x & 3;
+    __shared__ RoundSlot ring[kRing];
+    __shared__ uint64_t full[kRing], empty[kRing];
+    extern __shared__ float4 delta_smem[];
+    const int64_t nq = (int64_t)gridDim.x * kRoundQuads;
+    const int64_t n_rounds = (n_steps + nq - 1) / nq;
+    if (threadIdx.x == 0) {
+        for (int s = 0; s < kRing; s++) {
+            mma::mbar_init(&full[s], kSamplers);
+            mma::mbar_init(&empty[s], kConsumers / 32);
+        }
+    }
+    __syncthreads();
+
+    if (threadIdx.x >= kConsumers) {
+        // sampler: triple t of this CTA in every kSamplerGroups-th round; the ring slot of round r is free once round
+        // r - kRing is done
+        const int t = (threadIdx.x - kConsumers) % kSamplers, group = (threadIdx.x - kConsumers) / kSamplers;
+        for (int64_t r = group; r < n_rounds; r += kSamplerGroups) {
+            const int s = (int)(r % kRing);
+            if (r >= kRing) mma::mbar_wait_backoff(&empty[s], (uint32_t)((r / kRing - 1) & 1));
+            RoundSlot &S = ring[s];
+            const int64_t q = r * nq + (int64_t)blockIdx.x * kRoundQuads + t;
+            int32_t u = v.u_lo, i = -1, j = -1;
+            if (q < n_steps) sample_triple(v, base, step0 + q, u, i, j);
+            if (j < 0) i = -1;
+            else {
+                // the rows leave L2 only by eviction: the round's additions are performed there, so these lines are never stale
+                prefetch_l2(v.P + (int64_t)(u - v.u_lo) * v.d, 64 * C);
+                prefetch_l2(v.Q + (int64_t)j * v.d, 64 * C);
+            }
+            S.u[t] = u; S.item[t] = i; S.item[kRoundQuads + t] = j;
+            sampler_bar(group);
+            // link this triple's two entries to the other entries of the round with the same item
+            const int e0 = t, e1 = kRoundQuads + t;
+            int nxt0 = -1, nxt1 = -1;
+            bool first0 = i >= 0, first1 = j >= 0;
+            auto see = [&](int32_t id, int k) {
+                if (id == i) { if (k < e0) first0 = false; else if (k > e0) nxt0 = k; }
+                if (id == j) { if (k < e1) first1 = false; else if (k > e1) nxt1 = k; }
+            };
+            const int4 *items4 = reinterpret_cast<const int4 *>(S.item);
+            for (int k = 2 * kRoundQuads - 4; k >= 0; k -= 4) {   // descending: the last match after e is the next one
+                const int4 x = items4[k / 4];
+                see(x.w, k + 3); see(x.z, k + 2); see(x.y, k + 1); see(x.x, k);
+            }
+            S.next[e0] = nxt0; S.first[e0] = first0;
+            S.next[e1] = nxt1; S.first[e1] = first1;
+            mma::mbar_arrive(&full[s]);
+        }
+        return;
+    }
+
+    // consumer: quad t of this CTA
+    const int t = threadIdx.x >> 2, lane4 = threadIdx.x & 3;
     const unsigned mask = quad_mask();
-    const int64_t q = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 2;
-    const int64_t nq = ((int64_t)gridDim.x * blockDim.x) >> 2;
-    int32_t u = 0, i = 0, j = -1;
-    if (q < n_steps) sample_triple(v, base, step0 + q, u, i, j);
-    for (int64_t r0 = 0; r0 < n_steps; r0 += nq) {
+    const float nreg = -reg;
+    constexpr int d = 16 * C;
+    float *const D = reinterpret_cast<float *>(delta_smem) + 4 * lane4;   // entry e, chunk c at D + e * d + 16 * c
+    uint32_t n_sync = 0;
+    for (int64_t r = 0; r < n_rounds; r++) {
+        const int s = (int)(r % kRing);
+        mma::mbar_wait(&full[s], (uint32_t)((r / kRing) & 1));
+        const RoundSlot &S = ring[s];
+        const int32_t u = S.u[t], i = S.item[t], j = S.item[kRoundQuads + t];
         const bool live = j >= 0;
-        float *Pu = v.P + (int64_t)(u - v.u_lo) * v.d + 4 * lane4, *Qi = v.Q + (int64_t)i * v.d + 4 * lane4,
-              *Qj = v.Q + (int64_t)(live ? j : 0) * v.d + 4 * lane4;
-        Rows<C> r;
+        float *Pu = v.P + (int64_t)(u - v.u_lo) * v.d + 4 * lane4;
+        Rows<C> rw;
         float g = 0.f;
         if (live) {
-            load_rows<C>(r, Pu, Qi, 16, Qj, 16);
-            g = bpr_grad_rows<C>(r, mask);   // consumes every loaded value before the barrier
+            load_rows<C>(rw, Pu, v.Q + (int64_t)i * v.d + 4 * lane4, 16, v.Q + (int64_t)j * v.d + 4 * lane4, 16);
+            g = bpr_grad_rows<C>(rw, mask);   // consumes every loaded value before the barrier
         }
-        grid.sync();
-        if (live) bpr_scatter_rows<C, true>(r, g, Pu, Qi, 16, Qj, 16, lr, reg);
-        // the next round's triple (the sampler reads only the immutable CSR) while the additions drain
-        j = -1;
-        if (r0 + nq + q < n_steps) sample_triple(v, base, step0 + r0 + nq + q, u, i, j);
-        grid.sync();
+        consumer_grid_sync(barrier_count, ++n_sync * gridDim.x);
+        if (live) {
+            float *Di = D + t * d, *Dj = D + (kRoundQuads + t) * d;
+#pragma unroll
+            for (int c = 0; c < C; c++) {
+                float4 ti, tj, tp, o;
+                bpr_dirs<C>(rw, c, g, nreg, ti, tj, tp);
+                GB_F4_OP(o, __fmul_rn(f4get(tp, k_), lr)); red_row(Pu + 16 * c, o);
+                GB_F4_OP(o, __fmul_rn(f4get(ti, k_), lr)); *reinterpret_cast<float4 *>(Di + 16 * c) = o;
+                GB_F4_OP(o, __fmul_rn(f4get(tj, k_), lr)); *reinterpret_cast<float4 *>(Dj + 16 * c) = o;
+            }
+        }
+        consumer_bar();
+        // the first entry of each item chain adds the chain's deltas in entry order and sends one reduction
+#pragma unroll
+        for (int h = 0; h < 2; h++) {
+            const int e = t + h * kRoundQuads;
+            if (!S.first[e]) continue;
+            float4 acc[C];
+#pragma unroll
+            for (int c = 0; c < C; c++) acc[c] = *reinterpret_cast<const float4 *>(D + e * d + 16 * c);
+            for (int k = S.next[e]; k >= 0; k = S.next[k]) {
+#pragma unroll
+                for (int c = 0; c < C; c++) {
+                    const float4 x = *reinterpret_cast<const float4 *>(D + k * d + 16 * c);
+                    GB_F4_OP(acc[c], __fadd_rn(f4get(acc[c], k_), f4get(x, k_)));
+                }
+            }
+            float *Qe = v.Q + (int64_t)S.item[e] * v.d + 4 * lane4;
+#pragma unroll
+            for (int c = 0; c < C; c++) red_row(Qe + 16 * c, acc[c]);
+        }
+        __syncwarp();
+        if ((threadIdx.x & 31) == 0) mma::mbar_arrive(&empty[s]);
+        consumer_grid_sync(barrier_count, ++n_sync * gridDim.x);
     }
 }
 
@@ -426,13 +564,17 @@ static int32_t launch_round_epoch(gorse_b200_cf *cf, BprView v, int64_t step0, i
 {
     gorse_b200_ctx *c = cf->ctx;
     auto *k = bpr_round_kernel<C>;
+    const size_t smem = (size_t)2 * kRoundQuads * 16 * C * sizeof(float);
+    GB_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     int per_sm = 0;
-    GB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k, 256, 0));
+    GB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k, kRoundThreads, smem));
     // the round size is fixed (GB_BPR_ROUND triples) unless the device cannot hold that many quads at once
-    const int g = (int)std::min<int64_t>(GB_BPR_ROUND / 64, (int64_t)per_sm * c->sm_count);
+    const int g = (int)std::min<int64_t>(GB_BPR_ROUND / kRoundQuads, (int64_t)per_sm * c->sm_count);
     if (g < 1) { set_error("bpr_round_kernel does not fit on the device"); return GORSE_B200_ERR_UNSUPPORTED; }
-    void *args[] = {&v, &step0, &n, &base, &lr, &reg};
-    GB_CUDA(cudaLaunchCooperativeKernel((const void *)k, dim3(g), dim3(256), args, 0, c->stream));
+    uint32_t *count = cf->bpr_barrier.p;
+    GB_CUDA(cudaMemsetAsync(count, 0, sizeof(uint32_t), c->stream));
+    void *args[] = {&v, &step0, &n, &base, &lr, &reg, &count};
+    GB_CUDA(cudaLaunchCooperativeKernel((const void *)k, dim3(g), dim3(kRoundThreads), args, smem, c->stream));
     return GORSE_B200_OK;
 }
 

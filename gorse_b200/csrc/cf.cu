@@ -235,6 +235,7 @@ int32_t gorse_b200_cf_create(gorse_b200_ctx *ctx, int32_t n_users, int32_t n_ite
     if ((st = cf->user_items.alloc((size_t)n_fb_local)) != 0) return fail(st);
     if ((st = cf->active.alloc(active.size())) != 0) return fail(st);
     if ((st = cf->user_meta.alloc((size_t)nu)) != 0) return fail(st);
+    if ((st = cf->bpr_barrier.alloc(1)) != 0) return fail(st);
     cudaStream_t s = ctx->stream;
     auto up = [&](void *dst, const void *src, size_t bytes) -> int32_t {
         if (bytes == 0) return GORSE_B200_OK;
@@ -270,7 +271,7 @@ int32_t gorse_b200_cf_destroy(gorse_b200_cf *cf)
     cudaStreamSynchronize(cf->ctx->stream);
     cf->P.free(); cf->Q.free(); cf->Q0.free(); cf->item_rate.free(); cf->xchg.free(); cf->P_all.free();
     cf->user_off.free(); cf->item_off.free();
-    cf->user_items.free(); cf->item_users.free(); cf->active.free(); cf->user_meta.free();
+    cf->user_items.free(); cf->item_users.free(); cf->active.free(); cf->user_meta.free(); cf->bpr_barrier.free();
     cf->gram.free();
     for (int a = 0; a < 2; a++) {
         for (int b = 0; b < 7; b++) cf->als_rows[a][b].free();

@@ -48,6 +48,7 @@ struct gorse_b200_cf {
     gb::DevBuf<int64_t> user_off, item_off;
     gb::DevBuf<int32_t> user_items, item_users, active;
     gb::DevBuf<gb::UserMeta> user_meta;
+    gb::DevBuf<uint32_t> bpr_barrier;  // arrival counter of the round epoch's grid barrier (bpr.cu), zeroed before each launch
     bool all_active = false;  // every user of the shard has feedback: active[k] == u_lo + k
     // ALS scratch
     gb::DevBuf<float> gram;      // d x d
