@@ -271,16 +271,21 @@ __device__ __forceinline__ void consumer_bar() { asm volatile("bar.sync %0, %1;"
 __device__ __forceinline__ void sampler_bar(int group) { asm volatile("bar.sync %0, %1;" ::"r"(kSamplerBar0 + group), "n"(kSamplers) : "memory"); }
 
 // Grid barrier over the consumer threads only (the samplers run ahead and never join it): `count` starts at 0 and
-// `target` is the number of the barrier within the launch times the grid size.
+// `target` is the number of the barrier within the launch times the grid size.  One memory barrier per grid barrier:
+// the fence before the relaxed add releases what the CTA's consumers wrote before the named barrier, and waits for their
+// reductions to complete (a red.release after it would fence a second time).  The spin polls relaxed; one ld.acquire
+// once the count is reached acquires what every CTA released, since all the adds are read-modify-writes of one counter.
+// An ld.acquire in the loop would invalidate L1 on every poll.
 __device__ __forceinline__ void consumer_grid_sync(uint32_t *count, uint32_t target)
 {
     consumer_bar();
     if (threadIdx.x == 0) {
-        asm volatile("fence.acq_rel.gpu;\n\tred.release.gpu.global.add.u32 [%0], 1;" ::"l"(count) : "memory");
+        asm volatile("fence.acq_rel.gpu;\n\tred.relaxed.gpu.global.add.u32 [%0], 1;" ::"l"(count) : "memory");
         uint32_t seen;
         do {
-            asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(seen) : "l"(count) : "memory");
+            asm volatile("ld.relaxed.gpu.global.u32 %0, [%1];" : "=r"(seen) : "l"(count) : "memory");
         } while ((int32_t)(seen - target) < 0);
+        asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(seen) : "l"(count) : "memory");
     }
     consumer_bar();
 }
