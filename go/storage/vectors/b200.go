@@ -31,8 +31,10 @@ import (
 	"time"
 	"unsafe"
 
+	"github.com/gorse-io/gorse/common/log"
 	"github.com/gorse-io/gorse/storage"
 	"github.com/juju/errors"
+	"go.uber.org/zap"
 )
 
 const b200Prefix = "b200://"
@@ -351,6 +353,68 @@ func (db *B200) QueryVectors(ctx context.Context, name string, q Vector, categor
 			return nil, err
 		}
 		results = append(results, ScoredVector{Vector: v, Score: scores[i]})
+	}
+	return results, nil
+}
+
+// QueryVectorsExcluding answers the worker's CF recall (worker/pipeline.go:403-449) for many users in one call: row i is
+// QueryVectors(queries[i], nil, n+len(exclude[i])) without the ids in exclude[i] (the user's excludeSet,
+// logics/recommend.go:67-80), so a row may hold more than n results, as in the reference.  The ids of one row must be distinct,
+// as a set's are; ids the collection does not hold are passed as -1 and still count in topK.
+func (db *B200) QueryVectorsExcluding(ctx context.Context, name string, queries [][]float32, exclude [][]string, n int) ([][]ScoredVector, error) {
+	if len(queries) != len(exclude) {
+		return nil, errors.Errorf("%d queries with %d exclude sets", len(queries), len(exclude))
+	}
+	results := make([][]ScoredVector, len(queries))
+	if len(queries) == 0 || n <= 0 {
+		return results, nil
+	}
+	db.mu.RLock()
+	defer db.mu.RUnlock()
+	c, err := db.collection(name)
+	if err != nil {
+		return nil, err
+	}
+	dim := c.info.Dimension
+	values := make([]float32, 0, len(queries)*dim)
+	exOff := make([]int64, len(queries)+1)
+	exSlots := []int64{}
+	for i, q := range queries {
+		if len(q) != dim {
+			return nil, errors.Errorf("query %d has dimension %d, want %d", i, len(q), dim)
+		}
+		values = append(values, q...)
+		for _, id := range exclude[i] {
+			slot, ok := c.slotOf[id]
+			if !ok {
+				slot = -1
+			}
+			exSlots = append(exSlots, slot)
+		}
+		exOff[i+1] = int64(len(exSlots))
+	}
+	total := len(queries)*n + len(exSlots)
+	slots, scores, counts := make([]int64, total), make([]float32, total), make([]int32, len(queries))
+	var exact C.int64_t
+	st := C.gorse_b200_vecdb_query_excluding(c.handle, C.int64_t(len(queries)), f32p(values), nil, 0, C.int32_t(n), i64p(exOff),
+		i64p(exSlots), i64p(slots), f32p(scores), i32p(counts), &exact)
+	runtime.KeepAlive(values)
+	runtime.KeepAlive(exSlots)
+	if err := b200Err(st); err != nil {
+		return nil, err
+	}
+	log.Logger().Debug("batched CF recall", zap.Int("users", len(queries)), zap.Int64("exact_rows", int64(exact)))
+	for i := range queries {
+		start := int64(i)*int64(n) + exOff[i]
+		row := make([]ScoredVector, 0, counts[i])
+		for j := int64(0); j < int64(counts[i]); j++ {
+			v, err := db.getSlot(c, slots[start+j])
+			if err != nil {
+				return nil, err
+			}
+			row = append(row, ScoredVector{Vector: v, Score: scores[start+j]})
+		}
+		results[i] = row
 	}
 	return results, nil
 }

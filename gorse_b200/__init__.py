@@ -449,6 +449,26 @@ class VectorCollection:
                                          ptr(slots), ptr(scores), ptr(cnt)))
         return slots, scores, cnt
 
+    def query_excluding(self, q, exclude_lists, n, categories=()):
+        """Batched CF recall (gorse_b200_vecdb_query_excluding; worker/pipeline.go:403-449): row i is the first
+        n + len(exclude_lists[i]) results of query(q[i], categories) minus the slots in exclude_lists[i] (-1 = an excluded id
+        the collection does not hold).  -> ([(slots int64, scores float32) per row], rows answered by the exact scan)"""
+        qv = np.ascontiguousarray(q, np.float32).reshape(-1, self.dim)
+        nq = qv.shape[0]
+        if len(exclude_lists) != nq:
+            raise ValueError(f"{len(exclude_lists)} exclude lists for {nq} queries")
+        off = np.zeros(nq + 1, np.int64)
+        np.cumsum([len(e) for e in exclude_lists], out=off[1:])
+        ex = np.ascontiguousarray(np.concatenate([np.asarray(e, np.int64).reshape(-1) for e in exclude_lists]) if nq else [], np.int64)
+        cats = np.ascontiguousarray(list(categories), np.int32)
+        total = nq * max(n, 0) + int(off[-1])
+        slots, scores, cnt = np.full(max(total, 1), -1, np.int64), np.zeros(max(total, 1), np.float32), np.zeros(nq, np.int32)
+        exact = C.c_int64(0)
+        check(lib.gorse_b200_vecdb_query_excluding(self.h, nq, ptr(qv), ptr(cats) if cats.size else None, cats.size, n, ptr(off),
+                                                   ptr(ex) if ex.size else None, ptr(slots), ptr(scores), ptr(cnt), C.byref(exact)))
+        starts = np.arange(nq, dtype=np.int64) * max(n, 0) + off[:-1]
+        return [(slots[s:s + c].copy(), scores[s:s + c].copy()) for s, c in zip(starts, cnt)], exact.value
+
     def __enter__(self):
         return self
 

@@ -94,6 +94,8 @@ PROTOTYPES = {
     "gorse_b200_vecdb_add_item_factors": (C.c_int32, [VP, VP, VP, C.c_int64, VP, VP, VP]),
     "gorse_b200_marshal_latent_factors": (C.c_int32, [VP, C.c_int32, C.c_int32, VP, VP, VP, C.c_size_t, C.POINTER(C.c_size_t)]),
     "gorse_b200_vecdb_query": (C.c_int32, [VP, C.c_int64, VP, VP, VP, VP, C.c_int32, C.c_int32, VP, VP, VP]),
+    "gorse_b200_vecdb_query_excluding": (C.c_int32, [VP, C.c_int64, VP, VP, C.c_int32, C.c_int32, VP, VP, VP, VP, VP,
+                                                     C.POINTER(C.c_int64)]),
     "gorse_b200_ncf_load": (C.c_int32, [C.c_char_p, C.c_char_p, PVP]),
     "gorse_b200_ncf_shape": (C.c_int32, [VP, C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.POINTER(C.c_int64), C.POINTER(C.c_int64),
                                          C.POINTER(C.c_int64)]),

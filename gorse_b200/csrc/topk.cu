@@ -15,73 +15,6 @@
 
 namespace gb {
 
-// exact distance by a quad, d % 16 == 0.  Euclidean: floats_avx512.c:374-441 (sub, mul, add: no fusing).
-__device__ __forceinline__ float quad_dist(const float4 *q /* C regs, query chunk c at q[c] */, const float *x, int chunks,
-                                           int lane4, unsigned mask, int metric, float qq)
-{
-    const float4 *x4 = reinterpret_cast<const float4 *>(x) + lane4;
-    float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
-    if (metric == GORSE_B200_METRIC_COSINE) {   // 1 - q.x / (|q| |x|); the reference's arithmetic lives in its vector store (unpinned)
-        float4 xx = make_float4(0.f, 0.f, 0.f, 0.f);
-        for (int c = 0; c < chunks; c++) {
-            const float4 b = __ldg(x4 + 4 * c);
-            dot_chunk(acc, q[c], b, c == 0);
-            dot_chunk(xx, b, b, c == 0);
-        }
-        const float dot = quad_tree(acc, mask), nx = quad_tree(xx, mask);
-        return __fsub_rn(1.0f, __fdiv_rn(dot, __fmul_rn(__fsqrt_rn(qq), __fsqrt_rn(nx))));
-    }
-    if (metric == GORSE_B200_METRIC_NEG_DOT) {
-        for (int c = 0; c < chunks; c++) dot_chunk(acc, q[c], __ldg(x4 + 4 * c), c == 0);
-        return -quad_tree(acc, mask);
-    }
-    for (int c = 0; c < chunks; c++) {
-        float4 b = __ldg(x4 + 4 * c), v;
-        v.x = __fsub_rn(q[c].x, b.x); v.y = __fsub_rn(q[c].y, b.y); v.z = __fsub_rn(q[c].z, b.z); v.w = __fsub_rn(q[c].w, b.w);
-        v.x = __fmul_rn(v.x, v.x); v.y = __fmul_rn(v.y, v.y); v.z = __fmul_rn(v.z, v.z); v.w = __fmul_rn(v.w, v.w);
-        if (c == 0) acc = v;
-        else { acc.x = __fadd_rn(v.x, acc.x); acc.y = __fadd_rn(v.y, acc.y); acc.z = __fadd_rn(v.z, acc.z); acc.w = __fadd_rn(v.w, acc.w); }
-    }
-    return __fsqrt_rn(quad_tree(acc, mask));
-}
-
-// any d, one thread (8-lane block + fused tails as in the reference)
-__device__ inline float dist_any(const float *a, const float *b, int n, int metric, float qq)
-{
-    if (metric == GORSE_B200_METRIC_NEG_DOT) return -dot_any(a, b, n);
-    if (metric == GORSE_B200_METRIC_COSINE)
-        return __fsub_rn(1.0f, __fdiv_rn(dot_any(a, b, n), __fmul_rn(__fsqrt_rn(qq), __fsqrt_rn(dot_any(b, b, n)))));
-    int epoch = n / 16, remain = n % 16;
-    float s[16];
-#pragma unroll
-    for (int l = 0; l < 16; l++) s[l] = 0.f;
-    if (epoch > 0) {
-#pragma unroll
-        for (int l = 0; l < 16; l++) { float v = __fsub_rn(a[l], b[l]); s[l] = __fmul_rn(v, v); }
-    }
-    for (int c = 1; c < epoch; c++) {
-#pragma unroll
-        for (int l = 0; l < 16; l++) { float v = __fsub_rn(a[16 * c + l], b[16 * c + l]); s[l] = __fadd_rn(__fmul_rn(v, v), s[l]); }
-    }
-    float r4[4];
-#pragma unroll
-    for (int l = 0; l < 4; l++) r4[l] = __fadd_rn(__fadd_rn(s[l + 12], s[l + 4]), __fadd_rn(s[l + 8], s[l]));
-    float sum = __fadd_rn(__fadd_rn(r4[0], r4[2]), __fadd_rn(r4[1], r4[3]));
-    a += 16 * epoch; b += 16 * epoch;
-    if (remain >= 8) {
-        float p[8];
-#pragma unroll
-        for (int l = 0; l < 8; l++) { float v = __fsub_rn(a[l], b[l]); p[l] = __fmul_rn(v, v); }
-        float q4[4];
-#pragma unroll
-        for (int l = 0; l < 4; l++) q4[l] = __fadd_rn(p[l + 4], p[l]);
-        sum = __fadd_rn(sum, __fadd_rn(__fadd_rn(q4[0], q4[2]), __fadd_rn(q4[1], q4[3])));
-        a += 8; b += 8; remain -= 8;
-    }
-    for (int i = 0; i < remain; i++) { float v = __fsub_rn(a[i], b[i]); sum = __fmaf_rn(v, v, sum); }
-    return __fsqrt_rn(sum);
-}
-
 // (dist, idx) ordering used everywhere: ascending distance, then ascending index
 __device__ __forceinline__ bool before(float da, int32_t ia, float db, int32_t ib) { return da < db || (da == db && ia < ib); }
 

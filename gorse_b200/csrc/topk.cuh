@@ -2,6 +2,7 @@
 #pragma once
 #include <cuda_bf16.h>
 
+#include "cf.cuh"
 #include "common.cuh"
 
 struct gorse_b200_index {
@@ -32,6 +33,102 @@ struct gorse_b200_index {
 
 namespace gb {
 
+// geometry of the tensor-core sweep (topk_mma.cu) and of its candidate lists
+namespace mma {
+constexpr int BM = 64, BN = 128, BK = 64;      // rows per consumer warpgroup (queries), tile columns (vectors), k-block (bf16)
+constexpr int CONSUMERS = 2;                   // consumer warpgroups per CTA; both multiply every B tile
+constexpr int GROUP_ROWS = CONSUMERS * BM;     // query rows of one CTA pass over all vectors
+constexpr int MAX_KB = 3;                      // k-blocks per tile: Kp <= 192
+constexpr int CAP = 2048;                      // candidate slots per query row
+constexpr int PARTS = 4;                       // a row's columns are split over the 4 threads of an accumulator quad
+constexpr int PART_CAP = CAP / PARTS;          // candidate slots per (row, part)
+constexpr int R_TOP = 16;                      // sample order statistic that fixes the threshold
+constexpr int THREADS = 128 * (1 + CONSUMERS); // warpgroup 0: warp 0 = TMA producer, warps 1-3 idle; then the consumers
+constexpr uint32_t A_TILE_BYTES = BM * BK * 2; // one [64 x 64] bf16 k-block of queries = 8 KB
+constexpr uint32_t B_TILE_BYTES = BN * BK * 2; // one [128 x 64] bf16 k-block of vectors = 16 KB
+}  // namespace mma
+
+#ifdef __CUDACC__
+// the exact scan's arithmetic, shared by the index search (topk.cu) and the batched recall (recall.cu)
+// exact distance by a quad, d % 16 == 0.  Euclidean: floats_avx512.c:374-441 (sub, mul, add: no fusing).
+__device__ __forceinline__ float quad_dist(const float4 *q /* C regs, query chunk c at q[c] */, const float *x, int chunks,
+                                           int lane4, unsigned mask, int metric, float qq)
+{
+    const float4 *x4 = reinterpret_cast<const float4 *>(x) + lane4;
+    float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (metric == GORSE_B200_METRIC_COSINE) {   // 1 - q.x / (|q| |x|); the reference's arithmetic lives in its vector store (unpinned)
+        float4 xx = make_float4(0.f, 0.f, 0.f, 0.f);
+        for (int c = 0; c < chunks; c++) {
+            const float4 b = __ldg(x4 + 4 * c);
+            dot_chunk(acc, q[c], b, c == 0);
+            dot_chunk(xx, b, b, c == 0);
+        }
+        const float dot = quad_tree(acc, mask), nx = quad_tree(xx, mask);
+        return __fsub_rn(1.0f, __fdiv_rn(dot, __fmul_rn(__fsqrt_rn(qq), __fsqrt_rn(nx))));
+    }
+    if (metric == GORSE_B200_METRIC_NEG_DOT) {
+        for (int c = 0; c < chunks; c++) dot_chunk(acc, q[c], __ldg(x4 + 4 * c), c == 0);
+        return -quad_tree(acc, mask);
+    }
+    for (int c = 0; c < chunks; c++) {
+        float4 b = __ldg(x4 + 4 * c), v;
+        v.x = __fsub_rn(q[c].x, b.x); v.y = __fsub_rn(q[c].y, b.y); v.z = __fsub_rn(q[c].z, b.z); v.w = __fsub_rn(q[c].w, b.w);
+        v.x = __fmul_rn(v.x, v.x); v.y = __fmul_rn(v.y, v.y); v.z = __fmul_rn(v.z, v.z); v.w = __fmul_rn(v.w, v.w);
+        if (c == 0) acc = v;
+        else { acc.x = __fadd_rn(v.x, acc.x); acc.y = __fadd_rn(v.y, acc.y); acc.z = __fadd_rn(v.z, acc.z); acc.w = __fadd_rn(v.w, acc.w); }
+    }
+    return __fsqrt_rn(quad_tree(acc, mask));
+}
+
+// any d, one thread (8-lane block + fused tails as in the reference)
+__device__ inline float dist_any(const float *a, const float *b, int n, int metric, float qq)
+{
+    if (metric == GORSE_B200_METRIC_NEG_DOT) return -dot_any(a, b, n);
+    if (metric == GORSE_B200_METRIC_COSINE)
+        return __fsub_rn(1.0f, __fdiv_rn(dot_any(a, b, n), __fmul_rn(__fsqrt_rn(qq), __fsqrt_rn(dot_any(b, b, n)))));
+    int epoch = n / 16, remain = n % 16;
+    float s[16];
+#pragma unroll
+    for (int l = 0; l < 16; l++) s[l] = 0.f;
+    if (epoch > 0) {
+#pragma unroll
+        for (int l = 0; l < 16; l++) { float v = __fsub_rn(a[l], b[l]); s[l] = __fmul_rn(v, v); }
+    }
+    for (int c = 1; c < epoch; c++) {
+#pragma unroll
+        for (int l = 0; l < 16; l++) { float v = __fsub_rn(a[16 * c + l], b[16 * c + l]); s[l] = __fadd_rn(__fmul_rn(v, v), s[l]); }
+    }
+    float r4[4];
+#pragma unroll
+    for (int l = 0; l < 4; l++) r4[l] = __fadd_rn(__fadd_rn(s[l + 12], s[l + 4]), __fadd_rn(s[l + 8], s[l]));
+    float sum = __fadd_rn(__fadd_rn(r4[0], r4[2]), __fadd_rn(r4[1], r4[3]));
+    a += 16 * epoch; b += 16 * epoch;
+    if (remain >= 8) {
+        float p[8];
+#pragma unroll
+        for (int l = 0; l < 8; l++) { float v = __fsub_rn(a[l], b[l]); p[l] = __fmul_rn(v, v); }
+        float q4[4];
+#pragma unroll
+        for (int l = 0; l < 4; l++) q4[l] = __fadd_rn(p[l + 4], p[l]);
+        sum = __fadd_rn(sum, __fadd_rn(__fadd_rn(q4[0], q4[2]), __fadd_rn(q4[1], q4[3])));
+        a += 8; b += 8; remain -= 8;
+    }
+    for (int i = 0; i < remain; i++) { float v = __fsub_rn(a[i], b[i]); sum = __fmaf_rn(v, v, sum); }
+    return __fsqrt_rn(sum);
+}
+
+// order-preserving 32-bit keys of fp32 scores (larger score = larger key)
+__device__ __forceinline__ uint32_t float_key(float v)
+{
+    const uint32_t u = __float_as_uint(v);
+    return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+}
+__device__ __forceinline__ float key_float(uint32_t k)
+{
+    return __uint_as_float((k & 0x80000000u) ? (k & 0x7fffffffu) : ~k);
+}
+#endif  // __CUDACC__
+
 // exact scan / re-rank.  row_list != nullptr: only those query rows (nq = length of the list) are processed
 int32_t launch_exact(gorse_b200_index *ix, const float *d_q, const int64_t *d_qidx, int64_t q0, int64_t nq, int k,
                      const int32_t *d_cand, const int32_t *d_cand_count, int cand_stride, const int32_t *row_list,
@@ -42,6 +139,15 @@ int32_t launch_exact_split(gorse_b200_index *ix, const float *d_q, const int64_t
                            const uint8_t *allow = nullptr);
 
 int32_t index_reserve(gorse_b200_index *ix, int64_t need);
+// the tensor-core candidate sweep (topk_mma.cu), shared by search_mma and the batched recall (recall.cu).
+// mma_reserve: the bf16 mirror and the work buffers for up to cq query rows per sweep.  mma_sample_tiles: the sample size
+// that leaves about `cands` columns per row above its threshold.  mma_sweep: query rows (q_base, d_q, d_qidx, q0 as in
+// build_queries_kernel) -> candidate lists in ix->w_ccol / w_cval / w_ccnt / w_theta, eps in ix->w_eps; ev0 / ev1 (may be
+// nullptr) are recorded around the sweep kernel.
+int32_t mma_reserve(gorse_b200_index *ix, int64_t cq);
+int mma_sample_tiles(const gorse_b200_index *ix, double cands);
+int32_t mma_sweep(gorse_b200_index *ix, const float *q_base, const float *d_q, const int64_t *d_qidx, int64_t q0, int64_t nq, int m_tiles,
+                  cudaEvent_t ev0, cudaEvent_t ev1);
 bool mma_path_eligible(const gorse_b200_index *ix, int64_t nq, int k);
 // h_*: optional host result buffers; when given, every finished chunk of queries is downloaded on the context's copy stream
 // while the next chunk's kernels run

@@ -29,18 +29,6 @@
 namespace gb {
 namespace mma {
 
-constexpr int BM = 64, BN = 128, BK = 64;      // rows per consumer warpgroup (queries), tile columns (vectors), k-block (bf16)
-constexpr int CONSUMERS = 2;                   // consumer warpgroups per CTA; both multiply every B tile
-constexpr int GROUP_ROWS = CONSUMERS * BM;     // query rows of one CTA pass over all vectors
-constexpr int MAX_KB = 3;                      // k-blocks per tile: Kp <= 192
-constexpr int CAP = 2048;                      // candidate slots per query row
-constexpr int PARTS = 4;                       // a row's columns are split over the 4 threads of an accumulator quad
-constexpr int PART_CAP = CAP / PARTS;          // candidate slots per (row, part)
-constexpr int R_TOP = 16;                      // sample order statistic that fixes the threshold
-constexpr int THREADS = 128 * (1 + CONSUMERS); // warpgroup 0: warp 0 = TMA producer, warps 1-3 idle; then the consumers
-constexpr uint32_t A_TILE_BYTES = BM * BK * 2; // one [64 x 64] bf16 k-block of queries = 8 KB
-constexpr uint32_t B_TILE_BYTES = BN * BK * 2; // one [128 x 64] bf16 k-block of vectors = 16 KB
-
 struct Params {
     int64_t n;            // real vectors
     int32_t n_tiles;      // ceil(n / 128)
@@ -346,16 +334,6 @@ __global__ void max_kernel(const float *v, int64_t n, float *out)
 // ---- stage 2a: prune each row's candidates to the rigorous window and translate to original ids -------------
 // One warp per row.  The k-th largest approximate score is found WITHOUT sorting: the scores are mapped to order-preserving
 // 32-bit keys and the key is built bit by bit from the top (32 counting passes over <= CAP values held in shared memory).
-__device__ __forceinline__ uint32_t float_key(float v)
-{
-    const uint32_t u = __float_as_uint(v);
-    return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
-}
-__device__ __forceinline__ float key_float(uint32_t k)
-{
-    return __uint_as_float((k & 0x80000000u) ? (k & 0x7fffffffu) : ~k);
-}
-
 __global__ void __launch_bounds__(128)
 prune_kernel(const int32_t *cand_col, const float *cand_val, const int32_t *cand_cnt, const float *theta, const float *eps,
              const int32_t *perm, const int64_t *q_idx, int64_t q0, bool self_skip, int64_t nq, int k, int32_t *out_ids /* [nq][CAP] */,
@@ -510,35 +488,84 @@ static int32_t ensure_mirror(gorse_b200_index *ix)
     return GORSE_B200_OK;
 }
 
+int32_t mma_reserve(gorse_b200_index *ix, int64_t cq)
+{
+    GB_TRY(ensure_mirror(ix));
+    const int kp = kp_of(ix);
+    if (ix->w_cq >= cq && ix->w_kp == kp) return GORSE_B200_OK;   // reuse
+    // work buffers live in the index and are reused by later searches (multi-GB cudaMalloc/cudaFree per call otherwise)
+    ix->w_cq = 0;
+    const int64_t cq_pad = (cq + mma::GROUP_ROWS - 1) / mma::GROUP_ROWS * mma::GROUP_ROWS;
+    GB_TRY(ix->w_qb.alloc((size_t)cq_pad * kp));
+    GB_TRY(ix->w_eps.alloc(cq));
+    GB_TRY(ix->w_cval.alloc((size_t)cq * mma::CAP));
+    GB_TRY(ix->w_theta.alloc(mma::PARTS * cq));
+    GB_TRY(ix->w_ccol.alloc((size_t)cq * mma::CAP));
+    GB_TRY(ix->w_ccnt.alloc(mma::PARTS * cq));
+    GB_TRY(ix->w_ids.alloc((size_t)cq * mma::CAP));
+    GB_TRY(ix->w_idcnt.alloc(cq));
+    GB_TRY(ix->w_flag.alloc(cq));
+    GB_TRY(ix->w_flist.alloc(cq + 1));
+    ix->w_cq = cq;
+    ix->w_kp = kp;
+    return GORSE_B200_OK;
+}
+
+// sample size: the R_TOP-th best of m random columns leaves on average R_TOP * N / m columns above it (Gamma(R_TOP) spread)
+int mma_sample_tiles(const gorse_b200_index *ix, double cands)
+{
+    const int n_tiles = (int)((ix->n + mma::BN - 1) / mma::BN);
+    const int m_tiles = (int)((double)mma::R_TOP * (double)ix->n / cands / mma::BN);
+    return std::max(1, std::min(m_tiles, n_tiles));
+}
+
+int32_t mma_sweep(gorse_b200_index *ix, const float *q_base, const float *d_q, const int64_t *d_qidx, int64_t q0, int64_t nq, int m_tiles,
+                  cudaEvent_t ev0, cudaEvent_t ev1)
+{
+    gorse_b200_ctx *c = ix->ctx;
+    const int kp = kp_of(ix), kb = kp / mma::BK;
+    const int64_t n_pad = (ix->n + mma::BN - 1) / mma::BN * mma::BN;
+    // stages from the shared-memory budget (227 KB per block), at most 4: the epilogue's global traffic keeps some L1
+    const size_t a_bytes = (size_t)mma::CONSUMERS * kb * mma::A_TILE_BYTES, b_stage = (size_t)kb * mma::B_TILE_BYTES;
+    const int stages = (int)std::min<size_t>(4, (227 * 1024 - 1280 - a_bytes) / b_stage);
+    if (stages < 2) { set_error("mma_sweep: Kp = %d does not fit", kp); return GORSE_B200_ERR_UNSUPPORTED; }
+    const size_t smem = a_bytes + (size_t)stages * b_stage + 1024 /*align*/ + 256 /*barriers*/;
+    const bool dbg = ix->dbg_scores != nullptr;   // the dense score dump of the test hook is compiled out of the production kernel
+    auto pick = [&](auto s4, auto s3, auto s2) { return stages >= 4 ? s4 : stages == 3 ? s3 : s2; };
+    auto kern = dbg ? pick(mma::topk_mma_kernel<4, true>, mma::topk_mma_kernel<3, true>, mma::topk_mma_kernel<2, true>)
+                    : pick(mma::topk_mma_kernel<4, false>, mma::topk_mma_kernel<3, false>, mma::topk_mma_kernel<2, false>);
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) { set_error("mma_sweep smem attr: %s", cudaGetErrorString(e)); return GORSE_B200_ERR_CUDA; }
+    CUtensorMap map_a, map_b;
+    GB_TRY(make_map(&map_b, ix->Xb.p, n_pad, kp, mma::BN));
+    const int64_t nq_pad = (nq + mma::GROUP_ROWS - 1) / mma::GROUP_ROWS * mma::GROUP_ROWS;
+    mma::build_queries_kernel<<<(unsigned)nq_pad, 128, 0, c->stream>>>(q_base, d_q, d_qidx, q0, nq, nq_pad, ix->d, kp, ix->metric, ix->max_norm,
+                                                                      ix->w_qb.p, ix->w_eps.p);
+    c->launches++;
+    GB_TRY(make_map(&map_a, ix->w_qb.p, nq_pad, kp, mma::BM));
+    mma::Params P;
+    P.n = ix->n; P.n_tiles = (int)(n_pad / mma::BN); P.m_tiles = m_tiles; P.kb = kb; P.nq = nq; P.n_groups = (int)(nq_pad / mma::GROUP_ROWS);
+    P.eps = ix->w_eps.p; P.cand_col = ix->w_ccol.p; P.cand_val = ix->w_cval.p; P.cand_cnt = ix->w_ccnt.p; P.theta = ix->w_theta.p; P.dbg = ix->dbg_scores;
+    const int grid = std::min(P.n_groups, c->sm_count);
+    if (ev0) cudaEventRecord(ev0, c->stream);
+    kern<<<grid, mma::THREADS, smem, c->stream>>>(map_a, map_b, P);
+    if (ev1) cudaEventRecord(ev1, c->stream);
+    GB_LAUNCHED(c);
+    return GORSE_B200_OK;
+}
+
 int32_t search_mma(gorse_b200_index *ix, const float *d_q, const int64_t *d_qidx, int64_t q0, int64_t nq, int k, int prune0,
                    int32_t *d_idx, float *d_dist, int32_t *d_count, int *d_nan, int32_t *h_idx, float *h_dist, int32_t *h_count)
 {
     gorse_b200_ctx *c = ix->ctx;
-    GB_TRY(ensure_mirror(ix));
-    const int kp = kp_of(ix), kb = kp / mma::BK;
-    const int64_t n_pad = (ix->n + mma::BN - 1) / mma::BN * mma::BN;
-    const int n_tiles = (int)(n_pad / mma::BN);
-    // sample size: the R_TOP-th best of m random columns leaves on average R_TOP * N / m columns above it (Gamma(R_TOP)
-    // spread).  The parts of a row share ONE threshold from the whole sample, aimed at 4k columns per row: the row has
-    // fewer than k candidates when >= R_TOP of its true top k fell into the sample, Poisson(k m / N = R_TOP / 4): ~1e-6 per
-    // row, and a part's PART_CAP-slot list holds 4x its expected k columns (k <= 128).
-    int m_tiles = (int)((double)mma::R_TOP * (double)ix->n / (4.0 * k) / mma::BN);
-    m_tiles = std::max(1, std::min(m_tiles, n_tiles));
+    // The parts of a row share ONE threshold from the whole sample, aimed at 4k columns per row: the row has fewer than k
+    // candidates when >= R_TOP of its true top k fell into the sample, Poisson(k m / N = R_TOP / 4): ~1e-6 per row, and a
+    // part's PART_CAP-slot list holds 4x its expected k columns (k <= 128).
     const bool self_skip = d_q == nullptr;
-    // stages from the shared-memory budget (227 KB per block), at most 4: the epilogue's global traffic keeps some L1
-    const size_t a_bytes = (size_t)mma::CONSUMERS * kb * mma::A_TILE_BYTES, b_stage = (size_t)kb * mma::B_TILE_BYTES;
-    int stages = (int)std::min<size_t>(4, (227 * 1024 - 1280 - a_bytes) / b_stage);
-    if (stages < 2) { set_error("search_mma: Kp = %d does not fit", kp); return GORSE_B200_ERR_UNSUPPORTED; }
-    const size_t smem = a_bytes + (size_t)stages * b_stage + 1024 /*align*/ + 256 /*barriers*/;
-
-    CUtensorMap map_b;
-    GB_TRY(make_map(&map_b, ix->Xb.p, n_pad, kp, mma::BN));
     // queries are processed in chunks of 1024 rows per SM so that the candidate lists stay modest while every chunk's kernel
     // tail, host sync for the fallback count and fallback launches are amortised; a finished chunk is downloaded on the copy
     // stream while the next one computes
     const int64_t chunk = (int64_t)c->sm_count * mma::GROUP_ROWS * 8;
-    // work buffers live in the index and are reused by later searches (multi-GB cudaMalloc/cudaFree per call otherwise)
-    DevBuf<__nv_bfloat16> &Qb = ix->w_qb;
     DevBuf<float> &eps = ix->w_eps, &cval = ix->w_cval, &theta = ix->w_theta;
     DevBuf<int32_t> &ccol = ix->w_ccol, &ccnt = ix->w_ccnt, &ids = ix->w_ids, &idcnt = ix->w_idcnt, &flag = ix->w_flag, &flist = ix->w_flist;
     int32_t st = GORSE_B200_OK;
@@ -547,39 +574,17 @@ int32_t search_mma(gorse_b200_index *ix, const float *d_q, const int64_t *d_qidx
         cudaStreamSynchronize(c->copy_stream);
         return s;
     };
-    const int64_t cq = std::min(nq, chunk), cq_pad = (cq + mma::GROUP_ROWS - 1) / mma::GROUP_ROWS * mma::GROUP_ROWS;
-    if (ix->w_cq >= cq && ix->w_kp == kp) {
-        // reuse
-    } else if ((ix->w_cq = 0, false) || (st = Qb.alloc((size_t)cq_pad * kp)) || (st = eps.alloc(cq)) || (st = cval.alloc((size_t)cq * mma::CAP)) || (st = theta.alloc(mma::PARTS * cq)) ||
-        (st = ccol.alloc((size_t)cq * mma::CAP)) || (st = ccnt.alloc(mma::PARTS * cq)) || (st = ids.alloc((size_t)cq * mma::CAP)) || (st = idcnt.alloc(cq)) ||
-        (st = flag.alloc(cq)) || (st = flist.alloc(cq + 1)))
-        return done(st);
-    else { ix->w_cq = cq; ix->w_kp = kp; }
+    const int64_t cq = std::min(nq, chunk);
+    if ((st = mma_reserve(ix, cq))) return done(st);
+    const int m_tiles = mma_sample_tiles(ix, 4.0 * k);
     const int64_t fl_off = ix->w_cq;  // the fallback counter sits after the list
-    const bool dbg = ix->dbg_scores != nullptr;   // the dense score dump of the test hook is compiled out of the production kernel
-    auto pick = [&](auto s4, auto s3, auto s2) { return stages >= 4 ? s4 : stages == 3 ? s3 : s2; };
-    auto kern = dbg ? pick(mma::topk_mma_kernel<4, true>, mma::topk_mma_kernel<3, true>, mma::topk_mma_kernel<2, true>)
-                    : pick(mma::topk_mma_kernel<4, false>, mma::topk_mma_kernel<3, false>, mma::topk_mma_kernel<2, false>);
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) { set_error("search_mma smem attr: %s", cudaGetErrorString(e)); return done(GORSE_B200_ERR_CUDA); }
+    if (!ix->ev0) { cudaEventCreate(&ix->ev0); cudaEventCreate(&ix->ev1); }
+    cudaError_t e;
     for (int64_t off = 0; off < nq; off += cq) {
-        const int64_t n_this = std::min(cq, nq - off), n_this_pad = (n_this + mma::GROUP_ROWS - 1) / mma::GROUP_ROWS * mma::GROUP_ROWS;
+        const int64_t n_this = std::min(cq, nq - off);
         const float *qp = d_q ? d_q + off * ix->d : nullptr;
         const int64_t *qi = d_qidx ? d_qidx + off : nullptr;
-        mma::build_queries_kernel<<<(unsigned)n_this_pad, 128, 0, c->stream>>>(ix->X.p, qp, qi, q0 + off, n_this, n_this_pad, ix->d, kp, ix->metric,
-                                                                              ix->max_norm, Qb.p, eps.p);
-        c->launches++;
-        CUtensorMap map_a;
-        if ((st = make_map(&map_a, Qb.p, n_this_pad, kp, mma::BM))) return done(st);
-        mma::Params P;
-        P.n = ix->n; P.n_tiles = n_tiles; P.m_tiles = m_tiles; P.kb = kb; P.nq = n_this; P.n_groups = (int)(n_this_pad / mma::GROUP_ROWS);
-        P.eps = eps.p; P.cand_col = ccol.p; P.cand_val = cval.p; P.cand_cnt = ccnt.p; P.theta = theta.p; P.dbg = ix->dbg_scores;
-        const int grid = std::min(P.n_groups, c->sm_count);
-        if (!ix->ev0) { cudaEventCreate(&ix->ev0); cudaEventCreate(&ix->ev1); }
-        cudaEventRecord(ix->ev0, c->stream);
-        kern<<<grid, mma::THREADS, smem, c->stream>>>(map_a, map_b, P);
-        cudaEventRecord(ix->ev1, c->stream);
-        c->launches++;
+        if ((st = mma_sweep(ix, ix->X.p, qp, qi, q0 + off, n_this, m_tiles, ix->ev0, ix->ev1))) return done(st);
         if ((e = cudaMemsetAsync(flag.p, 0, sizeof(int32_t) * n_this, c->stream)) != cudaSuccess ||
             (e = cudaMemsetAsync(flist.p + fl_off, 0, sizeof(int32_t), c->stream)) != cudaSuccess) {
             set_error("search_mma memset: %s", cudaGetErrorString(e));

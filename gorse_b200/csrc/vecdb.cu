@@ -18,30 +18,12 @@
 
 #include "cf.cuh"
 #include "sparse.cuh"
-#include "topk.cuh"
+#include "vecdb.cuh"
 
 extern "C" {
 int32_t gorse_b200_sparse_index_create(gorse_b200_ctx *ctx, gorse_b200_sparse_index **out);
 int32_t gorse_b200_sparse_index_destroy(gorse_b200_sparse_index *ix);
 }
-
-struct gorse_b200_vecdb {
-    gorse_b200_ctx *ctx = nullptr;
-    int32_t dim = 0, distance = 0;
-    gorse_b200_index *dense = nullptr;           // dim > 0
-    gorse_b200_sparse_index *sparse = nullptr;   // dim == 0
-    std::mutex mu;
-    // host metadata (authoritative) + lazily refreshed device copies for the filter kernel
-    std::vector<uint8_t> hidden, dead;
-    std::vector<int64_t> ts;
-    std::vector<int64_t> cat_off{0};
-    std::vector<int32_t> cats;
-    int64_t live = 0;
-    bool meta_dirty = true;
-    gb::DevBuf<uint8_t> d_blocked, d_allow;   // blocked = hidden | dead
-    gb::DevBuf<int64_t> d_cat_off;
-    gb::DevBuf<int32_t> d_cats, d_want;
-};
 
 namespace gb {
 
@@ -97,6 +79,20 @@ static int32_t sync_meta(gorse_b200_vecdb *db)
     return GORSE_B200_OK;
 }
 
+int32_t vecdb_allow(gorse_b200_vecdb *db, const int32_t *categories, int32_t n_categories)
+{
+    gorse_b200_ctx *c = db->ctx;
+    const int64_t n = (int64_t)db->ts.size();
+    GB_TRY(sync_meta(db));
+    if (n_categories) {
+        GB_TRY(db->d_want.alloc((size_t)n_categories));
+        GB_CUDA(cudaMemcpyAsync(db->d_want.p, categories, sizeof(int32_t) * (size_t)n_categories, cudaMemcpyHostToDevice, c->stream));
+    }
+    vecdb_allow_kernel<<<div_up(n, 256), 256, 0, c->stream>>>(db->d_blocked.p, db->d_cat_off.p, db->d_cats.p, db->d_want.p, n_categories, n, db->d_allow.p);
+    GB_LAUNCHED(c);
+    return GORSE_B200_OK;
+}
+
 }  // namespace gb
 
 using namespace gb;
@@ -133,6 +129,7 @@ int32_t gorse_b200_vecdb_destroy(gorse_b200_vecdb *db)
         ScopedDevice sd(db->ctx->device);
         cudaStreamSynchronize(db->ctx->stream);
         db->d_blocked.free(); db->d_allow.free(); db->d_cat_off.free(); db->d_cats.free(); db->d_want.free();
+        db->recall.free();
     }
     gorse_b200_index_destroy(db->dense);
     gorse_b200_sparse_index_destroy(db->sparse);
@@ -266,13 +263,7 @@ int32_t gorse_b200_vecdb_query(gorse_b200_vecdb *db, int64_t nq, const float *q_
         for (int64_t q = 0; q < nq; q++) count_out[q] = 0;
         return GORSE_B200_OK;
     }
-    GB_TRY(sync_meta(db));
-    if (n_categories) {
-        GB_TRY(db->d_want.alloc((size_t)n_categories));
-        GB_CUDA(cudaMemcpyAsync(db->d_want.p, categories, sizeof(int32_t) * (size_t)n_categories, cudaMemcpyHostToDevice, c->stream));
-    }
-    vecdb_allow_kernel<<<div_up(n, 256), 256, 0, c->stream>>>(db->d_blocked.p, db->d_cat_off.p, db->d_cats.p, db->d_want.p, n_categories, n, db->d_allow.p);
-    GB_LAUNCHED(c);
+    GB_TRY(vecdb_allow(db, categories, n_categories));
     std::vector<int32_t> idx((size_t)nq * topk);
     int32_t st = GORSE_B200_OK;
     if (db->dim > 0) {

@@ -1,0 +1,42 @@
+// vecdb.cuh -- state of one vector collection (vecdb.cu), shared with the batched recall (recall.cu).
+#pragma once
+#include "topk.cuh"
+
+namespace gb {
+// grow-only work buffers of gorse_b200_vecdb_query_excluding, kept with the collection
+struct RecallWork {
+    DevBuf<float> q, scores, scratch;
+    DevBuf<int64_t> ex_off, ex, out_off, rows, slots;
+    DevBuf<int32_t> k, need, count, flags;
+    void free()
+    {
+        q.free(); scores.free(); scratch.free();
+        ex_off.free(); ex.free(); out_off.free(); rows.free(); slots.free();
+        k.free(); need.free(); count.free(); flags.free();
+    }
+};
+}  // namespace gb
+
+struct gorse_b200_vecdb {
+    gorse_b200_ctx *ctx = nullptr;
+    int32_t dim = 0, distance = 0;
+    gorse_b200_index *dense = nullptr;           // dim > 0
+    gorse_b200_sparse_index *sparse = nullptr;   // dim == 0
+    std::mutex mu;
+    // host metadata (authoritative) + lazily refreshed device copies for the filter kernel
+    std::vector<uint8_t> hidden, dead;
+    std::vector<int64_t> ts;
+    std::vector<int64_t> cat_off{0};
+    std::vector<int32_t> cats;
+    int64_t live = 0;
+    bool meta_dirty = true;
+    gb::DevBuf<uint8_t> d_blocked, d_allow;   // blocked = hidden | dead
+    gb::DevBuf<int64_t> d_cat_off;
+    gb::DevBuf<int32_t> d_cats, d_want;
+    gb::RecallWork recall;   // batched recall (recall.cu)
+};
+
+namespace gb {
+// allow mask d_allow[slot] of one query filter (live, not hidden, every wanted category); the caller holds db->mu
+int32_t vecdb_allow(gorse_b200_vecdb *db, const int32_t *categories, int32_t n_categories);
+}  // namespace gb

@@ -358,6 +358,21 @@ int32_t gorse_b200_vecdb_add_item_factors(gorse_b200_vecdb *db, gorse_b200_cf *c
 int32_t gorse_b200_vecdb_query(gorse_b200_vecdb *db, int64_t nq, const float *q_values, const int64_t *q_sp_off, const uint32_t *q_sp_indices,
                                const int32_t *categories, int32_t n_categories, int32_t topk, int64_t *slots_out, float *scores_out,
                                int32_t *count_out);
+/* Batched CF recall: for nq users at once, what the worker's collaborative-filtering recall does per user
+ * (worker/pipeline.go:403-449): QueryVectors(user embedding, categories, topK = n + |E_q|) followed by dropping every id of the
+ * user's exclude set E_q (the feedback items, logics/recommend.go:67-80).
+ *   E_q = excl_slots[excl_off[q] .. excl_off[q+1]) (excl_off[0] = 0), any order; an entry is a slot of this collection or -1
+ *   for an excluded id the collection does not hold (it still counts in |E_q|).  A slot twice in one row is GORSE_B200_ERR_ARG.
+ *   Row q: the candidates of gorse_b200_vecdb_query (live, not hidden, CONTAIN_ALL categories) by score descending, exact ties
+ *   by lower slot; the first k_q = n + |E_q| of them; minus the slots in E_q -- so a row may hold more than n results, as in
+ *   the reference.  Scores are bit-identical to gorse_b200_vecdb_query's (dot, or the negated distance).
+ *   Output: row q starts at q*n + excl_off[q] in slots_out / scores_out and has room for n + |E_q| entries (buffers of
+ *   nq*n + excl_off[nq]); count_out[q] = entries written.  n <= 0: every count is 0.  A NaN score: GORSE_B200_ERR_ARG.
+ *   Sparse collections: GORSE_B200_ERR_UNSUPPORTED.  exact_rows_out (may be NULL): rows answered by the exact scan rather than
+ *   the tensor-core sweep; the answer does not depend on it.  Thread-safe per collection. */
+int32_t gorse_b200_vecdb_query_excluding(gorse_b200_vecdb *db, int64_t nq, const float *q_values, const int32_t *categories,
+                                         int32_t n_categories, int32_t n, const int64_t *excl_off, const int64_t *excl_slots,
+                                         int64_t *slots_out, float *scores_out, int32_t *count_out, int64_t *exact_rows_out);
 
 /* ------------------------------------------------------------------------------------------
  * NCF-format datasets: dataset.LoadDataFromBuiltIn (dataset/dataset.go:398-490), the loader `gorse-bench cf`
