@@ -287,10 +287,13 @@ class BruteforceIndex:
         check(lib.gorse_b200_index_stats(self.h, C.byref(ms), C.byref(fl), C.byref(fb)))
         return ms.value, fl.value, fb.value
 
-    def stage1_scores(self, q0, q1):
+    def stage1_scores(self, q0, q1, with_eps=False):
+        """dense tensor-core scores of stored rows [q0, q1) against every vector [nq, N]; with_eps: (scores, each row's eps
+        [nq]), the margin the sweep relies on: |score - exact score| <= eps."""
         out = np.zeros((q1 - q0, len(self)), np.float32)
-        check(lib.gorse_b200_index_stage1_scores(self.h, q0, q1, ptr(out)))
-        return out
+        eps = np.zeros(q1 - q0, np.float32) if with_eps else None
+        check(lib.gorse_b200_index_stage1_scores(self.h, q0, q1, ptr(out), ptr(eps)))
+        return (out, eps) if with_eps else out
 
     def _out(self, nq, k):
         return (np.full((nq, max(k, 1)), -1, np.int32), np.zeros((nq, max(k, 1)), np.float32), np.zeros(nq, np.int32))

@@ -73,7 +73,7 @@ PROTOTYPES = {
     "gorse_b200_index_search_indices": (C.c_int32, [VP, VP, C.c_int64, C.c_int32, C.c_int32, VP, VP, VP]),
     "gorse_b200_index_search_range": (C.c_int32, [VP, C.c_int64, C.c_int64, C.c_int32, C.c_int32, VP, VP, VP]),
     "gorse_b200_index_stats": (C.c_int32, [VP, C.POINTER(C.c_double), C.POINTER(C.c_double), C.POINTER(C.c_int64)]),
-    "gorse_b200_index_stage1_scores": (C.c_int32, [VP, C.c_int64, C.c_int64, VP]),
+    "gorse_b200_index_stage1_scores": (C.c_int32, [VP, C.c_int64, C.c_int64, VP, VP]),
     "gorse_b200_bf16_truncate": (C.c_int32, [VP, C.c_int64, VP]),
     "gorse_b200_sparse_vector": (C.c_int32, [VP, C.c_int32, VP, C.c_int32, C.c_uint32, VP, VP, C.POINTER(C.c_int32)]),
     "gorse_b200_similar_scores": (C.c_int32, [C.c_int32, C.c_double, C.c_int32, C.c_int32, VP, VP, C.c_int32, VP, VP,

@@ -405,8 +405,8 @@ int32_t gorse_b200_index_stats(gorse_b200_index *ix, double *stage1_ms, double *
 }
 
 // dense stage-1 (tensor core) scores of stored vectors [q0, q1) against all vectors, in ORIGINAL column order:
-// out[(q - q0) * n + x].  Small problems only.
-int32_t gorse_b200_index_stage1_scores(gorse_b200_index *ix, int64_t q0, int64_t q1, float *out)
+// out[(q - q0) * n + x], and (eps_out != NULL) each row's error margin eps.  Small problems only (one chunk of rows).
+int32_t gorse_b200_index_stage1_scores(gorse_b200_index *ix, int64_t q0, int64_t q1, float *out, float *eps_out)
 {
     GB_CHECK_ARG(ix != nullptr && out != nullptr, "NULL argument");
     std::lock_guard<std::mutex> lk(ix->mu);
@@ -423,10 +423,12 @@ int32_t gorse_b200_index_stage1_scores(gorse_b200_index *ix, int64_t q0, int64_t
     cudaMemsetAsync(d_nan.p, 0, sizeof(int), c->stream);
     ix->dbg_scores = dense.p;
     if ((st = search_mma(ix, nullptr, nullptr, q0, nq, 1, 0, d_idx.p, d_dist.p, d_count.p, d_nan.p))) return done(st);
+    if (ix->w_cq < nq) { set_error("stage1_scores: %lld rows do not fit one sweep", (long long)nq); return done(GORSE_B200_ERR_ARG); }
     std::vector<float> h((size_t)nq * n_cols);
     std::vector<int32_t> perm((size_t)ix->n);
     cudaError_t e = cudaMemcpyAsync(h.data(), dense.p, sizeof(float) * h.size(), cudaMemcpyDeviceToHost, c->stream);
     if (e == cudaSuccess) e = cudaMemcpyAsync(perm.data(), ix->perm.p, sizeof(int32_t) * perm.size(), cudaMemcpyDeviceToHost, c->stream);
+    if (e == cudaSuccess && eps_out) e = cudaMemcpyAsync(eps_out, ix->w_eps.p, sizeof(float) * nq, cudaMemcpyDeviceToHost, c->stream);
     if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
     if (e != cudaSuccess) { set_error("debug scores: %s", cudaGetErrorString(e)); return done(GORSE_B200_ERR_CUDA); }
     for (int64_t r = 0; r < nq; r++)

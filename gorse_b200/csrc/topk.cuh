@@ -11,9 +11,10 @@ struct gorse_b200_index {
     int64_t n = 0, cap = 0;
     gb::DevBuf<float> X;            // [cap x d] fp32, row-major: the vectors as added (exact re-rank reads these)
     gb::DevBuf<__nv_bfloat16> Xb;   // [n_pad x d] bf16 mirror feeding the tensor cores (built lazily)
-    gb::DevBuf<float> norm;         // per-vector fp32 norms (+ max at [n]), built lazily
+    gb::DevBuf<float> norm;         // per-vector fp32 norms (+ max at [n], max |bf16(x) - x| at [n + 1]), built lazily
     gb::DevBuf<int32_t> perm;       // mirror row p holds vector perm[p] (random: the first columns are a uniform sample)
-    float max_norm = 0.f;
+    float max_norm = 0.f;           // max |x| and max |bf16(x) - x| over the vectors: the per-row eps of stage 1 (topk_mma.cu)
+    float max_dx = 0.f;
     bool mma_ready = false;
     float *dbg_scores = nullptr;    // tests only: dense stage-1 scores
     int64_t last_fallback_rows = 0; // rows of the last searches that needed the exact scan

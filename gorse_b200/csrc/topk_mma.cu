@@ -10,8 +10,10 @@
 // Threshold without a second pass: the vectors are stored in a random column permutation, so the first m columns are a
 // uniform sample.  For those the epilogue tracks each row's 16 best scores; theta = 16th best - 2*eps is then fixed,
 // the sweep continues over all columns (the first m are revisited at the end) and pushes score >= theta.
-//   * soundness: every true top-k element has score >= (k-th best approximate score) - 2*eps  (|score - exact| <= eps,
-//     eps from bf16 rounding: 1.02 * 2^-8 * |q| * max|x| + ...).  Stage 2 verifies that at least k candidates clear
+//   * soundness: every true top-k element has score >= (k-th best approximate score) - 2*eps, because |score - reference|
+//     <= eps for every column.  eps is an upper bound, not an estimate (build_queries_kernel derives it): |bf16(q)| max|bf16(x)
+//     - x| + |bf16(q) - q| max|x| for the bf16 rounding of both operands, plus the fp32 accumulation here and in the
+//     reference and, for Euclidean, the |x|^2/2 and distance roundings.  Stage 2 verifies that at least k candidates clear
 //     theta + 2*eps, which makes the candidate set a superset of the true top-k; rows that fail the check (or overflow
 //     their list) are redone by the exact scan.  With m = 4N/k and the 16th best, a row fails with probability ~1e-6.
 //
@@ -255,9 +257,10 @@ topk_mma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant
 }
 
 // ---- mirror construction ----------------------------------------------------------------------------
-// row p of the mirror = bf16 of vector perm[p] (zero rows beyond n); Euclidean appends hi/lo of -|x|^2/2
+// row p of the mirror = bf16 of vector perm[p] (zero rows beyond n); Euclidean appends hi/lo of -|x|^2/2.
+// max_dx: running max over the vectors of |bf16(x) - x| (the ints of non-negative floats order as the floats; NaN -> Inf)
 __global__ void build_mirror_kernel(const float *X, int64_t n, int d, const int32_t *perm, int64_t n_pad, int kp, int metric,
-                                    __nv_bfloat16 *Xb, float *norm /* [n] |x| by original index */)
+                                    __nv_bfloat16 *Xb, float *norm /* [n] |x| by original index */, float *max_dx)
 {
     const int64_t p = blockIdx.x;
     __nv_bfloat16 *dst = Xb + p * kp;
@@ -267,16 +270,25 @@ __global__ void build_mirror_kernel(const float *X, int64_t n, int d, const int3
     }
     const int64_t src = perm[p];
     const float *x = X + src * d;
-    __shared__ float s_sum[32];
-    float ss = 0.f;
-    for (int k = threadIdx.x; k < d; k += blockDim.x) { float v = x[k]; ss = __fmaf_rn(v, v, ss); dst[k] = __float2bfloat16(v); }
-    for (int o = 16; o; o >>= 1) ss += __shfl_xor_sync(0xffffffffu, ss, o);
-    if ((threadIdx.x & 31) == 0) s_sum[threadIdx.x >> 5] = ss;
+    __shared__ float s_sum[32], s_dd[32];
+    float ss = 0.f, dd = 0.f;
+    for (int k = threadIdx.x; k < d; k += blockDim.x) {
+        const float v = x[k];
+        const __nv_bfloat16 b = __float2bfloat16(v);
+        const float r = __fsub_rn(__bfloat162float(b), v);   // exact: the bits bf16 drops
+        ss = __fmaf_rn(v, v, ss);
+        dd = __fmaf_rn(r, r, dd);
+        dst[k] = b;
+    }
+    for (int o = 16; o; o >>= 1) { ss += __shfl_xor_sync(0xffffffffu, ss, o); dd += __shfl_xor_sync(0xffffffffu, dd, o); }
+    if ((threadIdx.x & 31) == 0) { s_sum[threadIdx.x >> 5] = ss; s_dd[threadIdx.x >> 5] = dd; }
     __syncthreads();
     if (threadIdx.x == 0) {
-        float tot = 0.f;
-        for (int w = 0; w < (int)(blockDim.x >> 5); w++) tot += s_sum[w];
+        float tot = 0.f, dtot = 0.f;
+        for (int w = 0; w < (int)(blockDim.x >> 5); w++) { tot += s_sum[w]; dtot += s_dd[w]; }
         norm[src] = sqrtf(tot);
+        const float dx = sqrtf(dtot);
+        atomicMax(reinterpret_cast<int *>(max_dx), __float_as_int(dx == dx ? dx : INFINITY));
         int k = d;
         if (metric == GORSE_B200_METRIC_EUCLIDEAN) {
             const float a = -0.5f * tot;
@@ -292,7 +304,7 @@ __global__ void build_mirror_kernel(const float *X, int64_t n, int d, const int3
 
 // query mirror rows + per-row eps; queries come from q_ptr, or from X rows (q_idx / q0 + i)
 __global__ void build_queries_kernel(const float *X, const float *q_ptr, const int64_t *q_idx, int64_t q0, int64_t nq, int64_t nq_pad,
-                                     int d, int kp, int metric, float max_norm, __nv_bfloat16 *Qb, float *eps)
+                                     int d, int kp, int metric, float max_norm, float max_dx, __nv_bfloat16 *Qb, float *eps)
 {
     const int64_t r = blockIdx.x;
     __nv_bfloat16 *dst = Qb + r * kp;
@@ -301,25 +313,45 @@ __global__ void build_queries_kernel(const float *X, const float *q_ptr, const i
         return;
     }
     const float *q = q_ptr ? q_ptr + r * d : X + (q_idx ? q_idx[r] : q0 + r) * d;
-    __shared__ float s_sum[32];
-    float ss = 0.f;
-    for (int k = threadIdx.x; k < d; k += blockDim.x) { float v = q[k]; ss = __fmaf_rn(v, v, ss); dst[k] = __float2bfloat16(v); }
-    for (int o = 16; o; o >>= 1) ss += __shfl_xor_sync(0xffffffffu, ss, o);
-    if ((threadIdx.x & 31) == 0) s_sum[threadIdx.x >> 5] = ss;
+    __shared__ float s_sum[3][32];
+    float ss = 0.f, sh = 0.f, sd = 0.f;   // |q|^2, |bf16(q)|^2, |bf16(q) - q|^2
+    for (int k = threadIdx.x; k < d; k += blockDim.x) {
+        const float v = q[k];
+        const __nv_bfloat16 b = __float2bfloat16(v);
+        const float h = __bfloat162float(b), rd = __fsub_rn(h, v);
+        ss = __fmaf_rn(v, v, ss);
+        sh = __fmaf_rn(h, h, sh);
+        sd = __fmaf_rn(rd, rd, sd);
+        dst[k] = b;
+    }
+    for (int o = 16; o; o >>= 1) {
+        ss += __shfl_xor_sync(0xffffffffu, ss, o);
+        sh += __shfl_xor_sync(0xffffffffu, sh, o);
+        sd += __shfl_xor_sync(0xffffffffu, sd, o);
+    }
+    if ((threadIdx.x & 31) == 0) { s_sum[0][threadIdx.x >> 5] = ss; s_sum[1][threadIdx.x >> 5] = sh; s_sum[2][threadIdx.x >> 5] = sd; }
     __syncthreads();
     if (threadIdx.x == 0) {
-        float tot = 0.f;
-        for (int w = 0; w < (int)(blockDim.x >> 5); w++) tot += s_sum[w];
-        const float qn = sqrtf(tot);
+        float tot = 0.f, toth = 0.f, totd = 0.f;
+        for (int w = 0; w < (int)(blockDim.x >> 5); w++) { tot += s_sum[0][w]; toth += s_sum[1][w]; totd += s_sum[2][w]; }
+        const float qh = sqrtf(toth), dq = sqrtf(totd);
         int k = d;
         if (metric == GORSE_B200_METRIC_EUCLIDEAN) { dst[k++] = __float2bfloat16(1.f); dst[k++] = __float2bfloat16(1.f); }
         for (; k < kp; k++) dst[k] = __float2bfloat16(0.f);
-        // |approx - exact| <= eps: bf16 rounding of both operands (2^-8 relative on each product, Cauchy-Schwarz), fp32
-        // accumulation in the tensor core and in the reference, and for Euclidean the hi/lo split of |x|^2/2 plus the
-        // rounding of the reference's own distance.  NaN/Inf inputs make eps NaN -> every compare fails -> exact fallback.
-        float e = 1.02f * 0.00390625f * qn * max_norm;
-        if (metric == GORSE_B200_METRIC_EUCLIDEAN) e += 6.2e-5f * (tot + max_norm * max_norm);
-        eps[r] = e;
+        // |stage-1 score - reference score| <= eps, with q^ = bf16(q), x^ = bf16(x), M = max|x|, Dx = max|x^ - x|, u = 2^-24:
+        //   bf16 rounding      q^.x^ - q.x = q^.(x^ - x) + (q^ - q).x, so by Cauchy-Schwarz |.| <= |q^| Dx + |q^ - q| M.
+        //                      (Each operand moves by up to 2^-8 relative, so no single-operand bound like 2^-8 |q| M holds.)
+        //   fp32 accumulation  the tensor core's sum of the Kp exact products, <= 6 Kp u sum|q^_i x^_i| for aligned, truncated
+        //                      partial sums, plus the reference's own fp32 dot, <= 1.02 d u |q| |x|; both <= 8 Kp u |q^| (M + Dx).
+        //   Euclidean          the score is q.x - |x|^2/2 with the last two columns (1, 1) x (hi, lo) of -|x|^2/2: the fp32 norm
+        //                      (d u M^2 / 2), the hi/lo split (2^-19 M^2 = 32 u M^2), the tensor core's accumulation of hi and lo
+        //                      (4.02 Kp u M^2) and the rounding of the reference's distance ((d + 5) u (|q|^2 + M^2), as a score)
+        //                      sum to less than (6 Kp + 64) u (|q|^2 + M^2) for d <= Kp.
+        //   fp32 evaluation    the norms here and in the mirror carry < (Kp + 2) u relative error each: a 1.001 pad covers them.
+        // NaN/Inf inputs make eps NaN or Inf (Inf norms, Inf Dx) -> the certification compares fail -> exact fallback.
+        float e = qh * max_dx + dq * max_norm + (float)kp * 0x1p-21f * qh * (max_norm + max_dx);
+        if (metric == GORSE_B200_METRIC_EUCLIDEAN) e += (6.f * (float)kp + 64.f) * 0x1p-24f * (tot + max_norm * max_norm);
+        eps[r] = 1.001f * e;
     }
 }
 
@@ -470,20 +502,24 @@ static int32_t ensure_mirror(gorse_b200_index *ix)
     const int kp = kp_of(ix);
     const int64_t n_pad = (ix->n + mma::BN - 1) / mma::BN * mma::BN;
     GB_TRY(ix->Xb.alloc((size_t)n_pad * kp));
-    GB_TRY(ix->norm.alloc((size_t)ix->n + 1));
+    GB_TRY(ix->norm.alloc((size_t)ix->n + 2));
     GB_TRY(ix->perm.alloc((size_t)ix->n));
     std::vector<int32_t> perm((size_t)ix->n);
     for (int64_t i = 0; i < ix->n; i++) perm[i] = (int32_t)i;
     std::mt19937_64 rng(0x9E3779B97F4A7C15ull ^ (uint64_t)ix->n);
     std::shuffle(perm.begin(), perm.end(), rng);
     GB_CUDA(cudaMemcpyAsync(ix->perm.p, perm.data(), sizeof(int32_t) * perm.size(), cudaMemcpyHostToDevice, c->stream));
-    mma::build_mirror_kernel<<<(unsigned)n_pad, 128, 0, c->stream>>>(ix->X.p, ix->n, ix->d, ix->perm.p, n_pad, kp, ix->metric, ix->Xb.p, ix->norm.p);
+    GB_CUDA(cudaMemsetAsync(ix->norm.p + ix->n, 0, 2 * sizeof(float), c->stream));   // max |x|, max |bf16(x) - x|
+    mma::build_mirror_kernel<<<(unsigned)n_pad, 128, 0, c->stream>>>(ix->X.p, ix->n, ix->d, ix->perm.p, n_pad, kp, ix->metric, ix->Xb.p, ix->norm.p,
+                                                                     ix->norm.p + ix->n + 1);
     GB_LAUNCHED(c);
-    GB_CUDA(cudaMemsetAsync(ix->norm.p + ix->n, 0, sizeof(float), c->stream));
     mma::max_kernel<<<c->sm_count * 2, 256, 0, c->stream>>>(ix->norm.p, ix->n, ix->norm.p + ix->n);
     GB_LAUNCHED(c);
-    GB_CUDA(cudaMemcpyAsync(&ix->max_norm, ix->norm.p + ix->n, sizeof(float), cudaMemcpyDeviceToHost, c->stream));
+    float maxes[2];
+    GB_CUDA(cudaMemcpyAsync(maxes, ix->norm.p + ix->n, sizeof(maxes), cudaMemcpyDeviceToHost, c->stream));
     GB_CUDA(cudaStreamSynchronize(c->stream));  // perm (host) dies here
+    ix->max_norm = maxes[0];
+    ix->max_dx = maxes[1];
     ix->mma_ready = true;
     return GORSE_B200_OK;
 }
@@ -540,7 +576,7 @@ int32_t mma_sweep(gorse_b200_index *ix, const float *q_base, const float *d_q, c
     GB_TRY(make_map(&map_b, ix->Xb.p, n_pad, kp, mma::BN));
     const int64_t nq_pad = (nq + mma::GROUP_ROWS - 1) / mma::GROUP_ROWS * mma::GROUP_ROWS;
     mma::build_queries_kernel<<<(unsigned)nq_pad, 128, 0, c->stream>>>(q_base, d_q, d_qidx, q0, nq, nq_pad, ix->d, kp, ix->metric, ix->max_norm,
-                                                                      ix->w_qb.p, ix->w_eps.p);
+                                                                      ix->max_dx, ix->w_qb.p, ix->w_eps.p);
     c->launches++;
     GB_TRY(make_map(&map_a, ix->w_qb.p, nq_pad, kp, mma::BM));
     mma::Params P;

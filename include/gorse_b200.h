@@ -260,8 +260,9 @@ int32_t gorse_b200_index_search_range(gorse_b200_index *ix, int64_t q0, int64_t 
  * their candidate set could not be certified.  Any pointer may be NULL. */
 int32_t gorse_b200_index_stats(gorse_b200_index *ix, double *stage1_ms, double *stage1_flop, int64_t *fallback_rows);
 /* test hook: the dense tensor-core scores of stored vectors [q0, q1) against all N vectors, original column order,
- * out[(q - q0) * N + x] (what the candidate sweep thresholds; small problems only) */
-int32_t gorse_b200_index_stage1_scores(gorse_b200_index *ix, int64_t q0, int64_t q1, float *out);
+ * out[(q - q0) * N + x] (what the candidate sweep thresholds; small problems only), and when eps_out is not NULL each row's
+ * error margin, eps_out[q - q0]: the sweep relies on |score - exact score| <= eps for every column */
+int32_t gorse_b200_index_stage1_scores(gorse_b200_index *ix, int64_t q0, int64_t q1, float *out, float *eps_out);
 
 
 /* ------------------------------------------------------------------------------------------
