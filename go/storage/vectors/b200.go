@@ -33,6 +33,7 @@ import (
 
 	"github.com/gorse-io/gorse/common/log"
 	"github.com/gorse-io/gorse/storage"
+	"github.com/gorse-io/gorse/storage/cache"
 	"github.com/juju/errors"
 	"go.uber.org/zap"
 )
@@ -413,6 +414,75 @@ func (db *B200) QueryVectorsExcluding(ctx context.Context, name string, queries 
 				return nil, err
 			}
 			row = append(row, ScoredVector{Vector: v, Score: scores[start+j]})
+		}
+		results[i] = row
+	}
+	return results, nil
+}
+
+// ItemToItemRecommend answers the worker's item-to-item recommender (Recommender.recommendItemToItem,
+// logics/recommend.go:244-283) for many users in one call on the collection ItemToItemCollection(name): row i is what the loop
+// returns for a user with positive feedback contextIds[i] (in the order the loop visits them, newest first) and exclude set
+// excludeIds[i] -- the neighbours of every context item (QueryItemToItem, logics/item_to_item.go:50-86) summed per id in
+// float64 in context order, without the excluded ids, the best n.  scoreScale is 0.5 for type "auto", else 1.  Ids without a
+// vector are passed as -1 (skipped as context, harmless as exclusions); the ids of one exclude set must be distinct, as a
+// set's are.  Exact score ties are ordered by slot; the reference's map order there is unpinned.
+func (db *B200) ItemToItemRecommend(ctx context.Context, collection string, contextIds [][]string, excludeIds [][]string, categories []string,
+	n int, scoreScale float64) ([][]cache.Score, error) {
+	if len(contextIds) != len(excludeIds) {
+		return nil, errors.Errorf("%d context lists with %d exclude sets", len(contextIds), len(excludeIds))
+	}
+	results := make([][]cache.Score, len(contextIds))
+	if len(contextIds) == 0 || n <= 0 {
+		return results, nil
+	}
+	db.mu.RLock()
+	defer db.mu.RUnlock()
+	c, err := db.collection(collection)
+	if err != nil {
+		return nil, err
+	}
+	want := make([]int32, 0, len(categories))
+	for _, cat := range categories {
+		id, ok := c.catID[cat]
+		if !ok {
+			return results, nil // nobody carries this category: every neighbour list is empty
+		}
+		want = append(want, id)
+	}
+	slotsOf := func(lists [][]string) ([]int64, []int64) {
+		off := make([]int64, len(lists)+1)
+		slots := []int64{}
+		for i, ids := range lists {
+			for _, id := range ids {
+				slot, ok := c.slotOf[id]
+				if !ok {
+					slot = -1
+				}
+				slots = append(slots, slot)
+			}
+			off[i+1] = int64(len(slots))
+		}
+		return off, slots
+	}
+	ctxOff, ctxSlots := slotsOf(contextIds)
+	exOff, exSlots := slotsOf(excludeIds)
+	users := len(contextIds)
+	slots, scores, counts := make([]int64, users*n), make([]float64, users*n), make([]int32, users)
+	stats := make([]int64, 4)
+	st := C.gorse_b200_vecdb_item_to_item(c.handle, C.int64_t(users), i64p(ctxOff), i64p(ctxSlots), i64p(exOff), i64p(exSlots), i32p(want),
+		C.int32_t(len(want)), C.int32_t(n), C.double(scoreScale), i64p(slots), (*C.double)(unsafe.Pointer(&scores[0])), i32p(counts), i64p(stats))
+	runtime.KeepAlive(ctxSlots)
+	runtime.KeepAlive(exSlots)
+	runtime.KeepAlive(want)
+	if err := b200Err(st); err != nil {
+		return nil, err
+	}
+	log.Logger().Debug("batched item-to-item", zap.Int("users", users), zap.Int64("context_items", stats[0]), zap.Int64("exact_rows", stats[1]))
+	for i := range results {
+		row := make([]cache.Score, 0, counts[i])
+		for j := i * n; j < i*n+int(counts[i]); j++ {
+			row = append(row, cache.Score{Id: c.idOf[slots[j]], Score: scores[j], Categories: c.catsOf[slots[j]]})
 		}
 		results[i] = row
 	}

@@ -472,6 +472,33 @@ class VectorCollection:
         starts = np.arange(nq, dtype=np.int64) * max(n, 0) + off[:-1]
         return [(slots[s:s + c].copy(), scores[s:s + c].copy()) for s, c in zip(starts, cnt)], exact.value
 
+    def item_to_item(self, context_lists, exclude_lists, n, categories=(), score_scale=1.0):
+        """Batched item-to-item recommendation (gorse_b200_vecdb_item_to_item; logics/recommend.go:244-283): for user i, the
+        neighbours of every slot of context_lists[i] in order (-1 = an id without a vector), their scores summed per slot in
+        float64 without the slots of exclude_lists[i], the best n.  score_scale: 0.5 for type "auto", else 1.
+        -> ([(slots int64, scores float64) per user], stats {context_items, exact_rows, shared_users, global_users})"""
+        nu = len(context_lists)
+        if len(exclude_lists) != nu:
+            raise ValueError(f"{len(exclude_lists)} exclude lists for {nu} users")
+
+        def csr(lists):
+            off = np.zeros(nu + 1, np.int64)
+            np.cumsum([len(x) for x in lists], out=off[1:])
+            flat = np.ascontiguousarray(np.concatenate([np.asarray(x, np.int64).reshape(-1) for x in lists]) if nu else [], np.int64)
+            return off, flat
+
+        coff, cs = csr(context_lists)
+        eoff, es = csr(exclude_lists)
+        cats = np.ascontiguousarray(list(categories), np.int32)
+        m = max(n, 0)
+        slots, scores, cnt = np.full(max(nu * m, 1), -1, np.int64), np.zeros(max(nu * m, 1), np.float64), np.zeros(max(nu, 1), np.int32)
+        stats = np.zeros(4, np.int64)
+        check(lib.gorse_b200_vecdb_item_to_item(self.h, nu, ptr(coff), ptr(cs) if cs.size else None, ptr(eoff), ptr(es) if es.size else None,
+                                                ptr(cats) if cats.size else None, cats.size, n, float(score_scale), ptr(slots), ptr(scores),
+                                                ptr(cnt), ptr(stats)))
+        rows = [(slots[u * m:u * m + c].copy(), scores[u * m:u * m + c].copy()) for u, c in zip(range(nu), cnt)]
+        return rows, dict(zip(("context_items", "exact_rows", "shared_users", "global_users"), (int(x) for x in stats)))
+
     def __enter__(self):
         return self
 

@@ -1,0 +1,406 @@
+// item_to_item.cu -- batched item-to-item recommendation: gorse_b200_vecdb_item_to_item.
+//
+// The worker's item-to-item recommender (logics/recommend.go:244-283) asks, per user, QueryItemToItem(c, categories, n) for
+// every positive feedback item c, newest first (logics/item_to_item.go:50-86: top n + 1, drop c itself, drop Dot scores <= 0,
+// stop at n), sums the neighbour scores per item id in float64, skipping the user's exclude set, and keeps the best n.  Here
+// one call answers many users:
+//
+//   stage A   the neighbour table, once per call: the distinct live context items of the whole batch are queried once each.
+//             Dense collections run the recall pipeline of recall.cu (recall_rows) with E = {c} and k = n + 1 on the stored
+//             vectors, then i2i_table_kernel cuts each row to n and drops Dot scores <= 0.  Sparse collections run
+//             sparse_search_kernel on the list of stored rows (a row never finds itself; it keeps positive dots only).
+//             The table holds n (int32 slot, float32 score) entries per item, scores bit-identical to gorse_b200_vecdb_query.
+//   stage B   i2i_aggregate_kernel, one CTA per user: walks C_u in order and adds s = (double)score * scale (Euclidean:
+//             1 / (1 - s)) per neighbour slot not in E_u, with a barrier between context entries so that every sum is formed
+//             in the reference's order; then selects the first n by (score desc, slot asc) with a 64-bit radix select and
+//             sorts them.  The accumulator is an open-addressing table in shared memory when |C_u| * n <= TABLE_KEYS, else
+//             this CTA's float64 row of length N in global memory, with a touched flag per slot and the list of touched slots.
+#include <algorithm>
+
+#include "recall.cuh"
+#include "sparse.cuh"
+#include "vecdb.cuh"
+
+namespace gb {
+namespace i2i {
+
+using u128 = unsigned __int128;
+
+constexpr int AGG_THREADS = 256;
+constexpr int TABLE_CAP = 8192;                  // shared-memory table entries: int32 slot + float64 sum, 96 KB
+constexpr int TABLE_KEYS = TABLE_CAP / 4 * 3;    // a user takes the table when |C_u| * n <= this (load <= 3/4)
+constexpr int MAX_N_DENSE = 1024;                // the sort buffer holds n entries
+constexpr int MAX_N_SPARSE = 128;                // sparse_search_kernel's k
+
+struct Users {                // one chunk of users (chunk-local ids)
+    const int64_t *c_off;     // [users + 1] into c_row
+    const int32_t *c_row;     // the neighbour-table row of each live context entry, in the caller's order
+    const int64_t *ex_off;    // [users + 1] into ex
+    const int64_t *ex;        // each user's excluded slots, ascending (-1 entries dropped)
+    int64_t *slots;           // [users x n]
+    double *scores;           // [users x n]
+    int32_t *count;           // [users]
+};
+
+struct Table {                // stage A: the first n neighbours of each distinct context item
+    const int32_t *slot;      // [rows x n]
+    const float *score;       // [rows x n] the vector store's score (dot, or the negated distance)
+    const int32_t *cnt;       // [rows]
+};
+
+// order-preserving 64-bit key of a float64 sum (never 0: the sums are not NaN)
+__device__ __forceinline__ uint64_t sum_key(double v)
+{
+    const uint64_t u = (uint64_t)__double_as_longlong(v);
+    return (u >> 63) ? ~u : (u | (1ull << 63));
+}
+
+// QueryItemToItem's score (logics/item_to_item.go:76-79), rounded step by step as Go does
+__device__ __forceinline__ double neighbour_score(float raw, double scale, bool euclid)
+{
+    const double s = __dmul_rn((double)raw, scale);
+    return euclid ? __ddiv_rn(1.0, __dsub_rn(1.0, s)) : s;
+}
+
+// row r of the recall with k = n + 1 (at r * (n + 1)): its first n entries; Dot keeps scores > 0 only (a prefix: rows are
+// sorted by score descending)
+__global__ void i2i_table_kernel(const int64_t *slots, const float *scores, const int32_t *count, int64_t rows, int n, int dot,
+                                 int32_t *t_slot, float *t_score, int32_t *t_cnt)
+{
+    for (int64_t r = blockIdx.x; r < rows; r += gridDim.x) {
+        const int c = min(count[r], n);
+        const int64_t src = r * (n + 1), dst = r * n;
+        int kept = 0;
+        for (int base = 0; base < c; base += blockDim.x) {
+            const int j = base + threadIdx.x;
+            const float s = j < c ? scores[src + j] : 0.f;
+            const bool keep = j < c && (!dot || s > 0.f);
+            if (keep) {
+                t_slot[dst + j] = (int32_t)slots[src + j];
+                t_score[dst + j] = s;
+            }
+            kept += __syncthreads_count(keep);
+        }
+        if (threadIdx.x == 0) t_cnt[r] = kept;
+    }
+}
+
+// one CTA per user of `users`.  SHARED: the accumulator is a table in shared memory; else acc_rows / seen_rows /
+// touched_rows hold one [N] float64 row, one [N] flag row (all zero between users) and one [N] slot list per CTA.
+template <bool SHARED>
+__global__ void __launch_bounds__(AGG_THREADS)
+i2i_aggregate_kernel(const int32_t *users, int64_t n_users, Users U, Table T, int n, double scale, int euclid, int64_t N, double *acc_rows,
+                     uint8_t *seen_rows, int32_t *touched_rows)
+{
+    using namespace gb::recall;
+    constexpr int NT = AGG_THREADS;
+    extern __shared__ __align__(16) uint8_t sm[];
+    const int p2 = pow2_at_least(n);
+    u128 *s_key = reinterpret_cast<u128 *>(sm);                    // [p2] sort keys: ~sum key, then slot
+    double *s_val = reinterpret_cast<double *>(s_key + p2);        // [p2]
+    int *hist = reinterpret_cast<int *>(s_val + p2);               // [256]
+    int *s_warp = hist + 256;                                      // [32]
+    int *s_bc = s_warp + 32;                                       // [4]: select, [2] gather fill, [3] distinct slots
+    int32_t *t_key = reinterpret_cast<int32_t *>(s_bc + 4);        // SHARED: [TABLE_CAP] slot, -1 = empty
+    double *t_val = reinterpret_cast<double *>(t_key + TABLE_CAP); // SHARED: [TABLE_CAP] sum
+    double *acc = SHARED ? nullptr : acc_rows + (int64_t)blockIdx.x * N;
+    uint8_t *seen = SHARED ? nullptr : seen_rows + (int64_t)blockIdx.x * N;
+    int32_t *touched = SHARED ? nullptr : touched_rows + (int64_t)blockIdx.x * N;
+    for (int64_t i = blockIdx.x; i < n_users; i += gridDim.x) {
+        const int64_t u = users[i];
+        const int64_t cb = U.c_off[u], ce = U.c_off[u + 1];
+        const int64_t *ex = U.ex + U.ex_off[u], n_ex = U.ex_off[u + 1] - U.ex_off[u];
+        int cap = 0, lg = 0;
+        if (SHARED) {   // a power of two >= 2 |C_u| n, at most TABLE_CAP: the load stays <= 3/4
+            cap = min(TABLE_CAP, pow2_at_least(max(64, (int)(2 * (ce - cb) * n))));
+            lg = __ffs(cap) - 1;
+            for (int j = threadIdx.x; j < cap; j += NT) t_key[j] = -1;
+        }
+        if (threadIdx.x == 0) s_bc[3] = 0;
+        __syncthreads();
+        // C_u in order.  The neighbours of one entry are distinct slots, so its adds touch distinct sums; the barrier after
+        // each entry makes every sum the reference's left-to-right sum over the context.
+        for (int64_t e = cb; e < ce; e++) {
+            const int64_t r = U.c_row[e];
+            const int cnt = T.cnt[r];
+            for (int j = threadIdx.x; j < cnt; j += NT) {
+                const int32_t slot = T.slot[r * n + j];
+                if (contains(ex, n_ex, (int64_t)slot)) continue;
+                const double s = neighbour_score(T.score[r * n + j], scale, euclid);
+                if (SHARED) {
+                    uint32_t h = ((uint32_t)slot * 0x9E3779B1u) >> (32 - lg);
+                    for (;;) {
+                        const int32_t k = t_key[h];
+                        if (k == slot) { t_val[h] = __dadd_rn(t_val[h], s); break; }
+                        if (k < 0 && atomicCAS(&t_key[h], -1, slot) == -1) {
+                            t_val[h] = __dadd_rn(0.0, s);   // the reference's map starts every sum at 0
+                            atomicAdd(&s_bc[3], 1);
+                            break;
+                        }
+                        h = (h + 1) & (uint32_t)(cap - 1);
+                    }
+                } else if (seen[slot]) {
+                    acc[slot] = __dadd_rn(acc[slot], s);
+                } else {
+                    seen[slot] = 1;
+                    touched[atomicAdd(&s_bc[3], 1)] = slot;
+                    acc[slot] = __dadd_rn(0.0, s);
+                }
+            }
+            __syncthreads();
+        }
+        const int distinct = s_bc[3];
+        const int m = min(n, distinct);
+        if (m > 0) {
+            const int64_t range = SHARED ? cap : distinct;
+            auto slot_at = [&](int64_t j) -> int32_t { return SHARED ? t_key[j] : touched[j]; };
+            auto val_at = [&](int64_t j) -> double { return SHARED ? t_val[j] : acc[touched[j]]; };
+            auto key_at = [&](int64_t j) -> uint64_t { return slot_at(j) >= 0 ? sum_key(val_at(j)) : 0ull; };
+            int ties;
+            const uint64_t K = block_select<NT>(range, m, key_at, hist, s_bc, &ties);
+            // of the sums equal to the m-th, the `ties` lowest slots are kept
+            int eq = 0;
+            for (int64_t j = threadIdx.x; j < range; j += NT) eq += key_at(j) == K;
+            eq = block_sum<NT>(eq, s_warp);
+            uint32_t last = 0xffffffffu;
+            if (eq > ties) {
+                int t2;
+                last = ~block_select<NT>(range, ties, [&](int64_t j) { return key_at(j) == K ? ~(uint32_t)slot_at(j) : 0u; }, hist, s_bc, &t2);
+            }
+            if (threadIdx.x == 0) s_bc[2] = 0;
+            __syncthreads();
+            for (int64_t j = threadIdx.x; j < range; j += NT) {
+                const uint64_t k = key_at(j);
+                if (k > K || (k == K && (uint32_t)slot_at(j) <= last)) {
+                    const int pos = atomicAdd(&s_bc[2], 1);
+                    s_key[pos] = ((u128)~k << 64) | (uint32_t)slot_at(j);
+                    s_val[pos] = val_at(j);
+                }
+            }
+            for (int j = m + threadIdx.x; j < p2; j += NT) s_key[j] = ~(u128)0;
+            __syncthreads();
+            block_sort<NT>(s_key, s_val, p2);
+            for (int j = threadIdx.x; j < m; j += NT) {
+                U.slots[u * n + j] = (int64_t)(uint32_t)s_key[j];
+                U.scores[u * n + j] = s_val[j];
+            }
+        }
+        if (threadIdx.x == 0) U.count[u] = m;
+        if (!SHARED)
+            for (int j = threadIdx.x; j < distinct; j += NT) seen[touched[j]] = 0;
+        __syncthreads();
+    }
+}
+
+size_t aggregate_smem(int n, bool shared)
+{
+    const size_t p2 = (size_t)recall::pow2_at_least(n);
+    return p2 * 24 + (256 + 32 + 4) * 4 + (shared ? (size_t)TABLE_CAP * 12 : 0);
+}
+
+// grow b to n entries; a new allocation is zeroed
+template <typename T>
+int32_t grow_zeroed(DevBuf<T> &b, size_t n, cudaStream_t s)
+{
+    if (b.n >= n) return GORSE_B200_OK;
+    GB_TRY(b.alloc(n));
+    GB_CUDA(cudaMemsetAsync(b.p, 0, sizeof(T) * n, s));
+    return GORSE_B200_OK;
+}
+
+}  // namespace i2i
+}  // namespace gb
+
+using namespace gb;
+
+extern "C" int32_t gorse_b200_vecdb_item_to_item(gorse_b200_vecdb *db, int64_t n_users, const int64_t *ctx_off, const int64_t *ctx_slots,
+                                                 const int64_t *excl_off, const int64_t *excl_slots, const int32_t *categories,
+                                                 int32_t n_categories, int32_t n, double score_scale, int64_t *slots_out, double *scores_out,
+                                                 int32_t *count_out, int64_t *stats_out)
+{
+    using namespace gb::i2i;
+    using gb::recall::grow;
+    GB_CHECK_ARG(db != nullptr, "collection is NULL");
+    GB_CHECK_ARG(n_users >= 0 && n_categories >= 0, "negative count");
+    if (stats_out) std::fill(stats_out, stats_out + 4, 0);
+    if (n_users == 0) return GORSE_B200_OK;
+    GB_CHECK_ARG(count_out != nullptr && ctx_off != nullptr && excl_off != nullptr, "count_out / ctx_off / excl_off is NULL");
+    GB_CHECK_ARG(ctx_off[0] == 0 && excl_off[0] == 0, "ctx_off[0] and excl_off[0] must be 0");
+    for (int64_t u = 0; u < n_users; u++) {
+        GB_CHECK_ARG(ctx_off[u + 1] >= ctx_off[u], "ctx_off not non-decreasing at %lld", (long long)u);
+        GB_CHECK_ARG(excl_off[u + 1] >= excl_off[u], "excl_off not non-decreasing at %lld", (long long)u);
+    }
+    GB_CHECK_ARG(ctx_off[n_users] == 0 || ctx_slots != nullptr, "ctx_slots is NULL");
+    GB_CHECK_ARG(excl_off[n_users] == 0 || excl_slots != nullptr, "excl_slots is NULL");
+    GB_CHECK_ARG(score_scale == score_scale, "score_scale is NaN");
+    if (db->distance == GORSE_B200_DISTANCE_COSINE) {
+        set_error("item-to-item collections are Dot or Euclidean");
+        return GORSE_B200_ERR_UNSUPPORTED;
+    }
+    if (n <= 0) {
+        for (int64_t u = 0; u < n_users; u++) count_out[u] = 0;
+        return GORSE_B200_OK;
+    }
+    const bool sparse = db->dim == 0;
+    if (n > (sparse ? MAX_N_SPARSE : MAX_N_DENSE)) {
+        set_error("item_to_item: n = %d above %d for a %s collection", n, sparse ? MAX_N_SPARSE : MAX_N_DENSE, sparse ? "sparse" : "dense");
+        return GORSE_B200_ERR_UNSUPPORTED;
+    }
+    GB_CHECK_ARG(slots_out != nullptr && scores_out != nullptr, "NULL output");
+    GB_CHECK_ARG(n_categories == 0 || categories != nullptr, "categories is NULL");
+    std::lock_guard<std::mutex> lk(db->mu);
+    const int64_t n_slots = (int64_t)db->ts.size();
+    if (n_slots > INT32_MAX) { set_error("item_to_item: more than 2^31 slots"); return GORSE_B200_ERR_UNSUPPORTED; }
+    // each user's exclusions once, sorted, -1 entries dropped (as gorse_b200_vecdb_query_excluding)
+    std::vector<int64_t> ex, ex_off((size_t)n_users + 1, 0);
+    ex.reserve((size_t)excl_off[n_users]);
+    for (int64_t u = 0; u < n_users; u++) {
+        for (int64_t t = ctx_off[u]; t < ctx_off[u + 1]; t++)
+            GB_CHECK_ARG(ctx_slots[t] >= -1 && ctx_slots[t] < n_slots, "user %lld: context slot %lld is not a slot of the collection",
+                         (long long)u, (long long)ctx_slots[t]);
+        const size_t b = ex.size();
+        for (int64_t t = excl_off[u]; t < excl_off[u + 1]; t++) {
+            const int64_t s = excl_slots[t];
+            GB_CHECK_ARG(s >= -1 && s < n_slots, "user %lld: excluded slot %lld is not a slot of the collection", (long long)u, (long long)s);
+            if (s >= 0) ex.push_back(s);
+        }
+        std::sort(ex.begin() + b, ex.end());
+        for (size_t t = b + 1; t < ex.size(); t++)
+            GB_CHECK_ARG(ex[t] != ex[t - 1], "user %lld: slot %lld is excluded twice", (long long)u, (long long)ex[t]);
+        ex_off[(size_t)u + 1] = (int64_t)ex.size();
+    }
+    // the live context entries of every user as rows of the neighbour table: one row per distinct item, in first-visit order.
+    // -1 and deleted slots are skipped (GetVectors returns nothing, logics/item_to_item.go:56-58); hidden ones are queried.
+    std::vector<int32_t> row_of((size_t)n_slots, -1), c_row;
+    std::vector<int64_t> nb, c_off((size_t)n_users + 1, 0);
+    c_row.reserve((size_t)ctx_off[n_users]);
+    for (int64_t u = 0; u < n_users; u++) {
+        for (int64_t t = ctx_off[u]; t < ctx_off[u + 1]; t++) {
+            const int64_t s = ctx_slots[t];
+            if (s < 0 || db->dead[(size_t)s]) continue;
+            if (row_of[(size_t)s] < 0) {
+                row_of[(size_t)s] = (int32_t)nb.size();
+                nb.push_back(s);
+            }
+            c_row.push_back(row_of[(size_t)s]);
+        }
+        c_off[(size_t)u + 1] = (int64_t)c_row.size();
+    }
+    const int64_t R = (int64_t)nb.size();
+    if (R == 0) {
+        for (int64_t u = 0; u < n_users; u++) count_out[u] = 0;
+        return GORSE_B200_OK;
+    }
+    gorse_b200_ctx *c = db->ctx;
+    ScopedDevice sd(c->device);
+    GB_TRY(vecdb_allow(db, categories, n_categories));
+    ItemToItemWork &V = db->i2i;
+    int32_t st = GORSE_B200_OK;
+    auto done = [&](int32_t s) {
+        cudaStreamSynchronize(c->stream);
+        cudaStreamSynchronize(c->copy_stream);
+        return s;
+    };
+    if ((st = grow(V.nb, (size_t)R)) || (st = grow(V.t_slot, (size_t)R * n)) || (st = grow(V.t_score, (size_t)R * n)) || (st = grow(V.t_cnt, (size_t)R)))
+        return done(st);
+    cudaError_t e = cudaMemcpyAsync(V.nb.p, nb.data(), sizeof(int64_t) * R, cudaMemcpyHostToDevice, c->stream);
+    if (e != cudaSuccess) { set_error("item_to_item upload: %s", cudaGetErrorString(e)); return done(GORSE_B200_ERR_CUDA); }
+
+    // ---- stage A: the neighbour table
+    int64_t exact_rows = 0;
+    if (!sparse) {
+        std::vector<int64_t> self_off((size_t)R + 1);   // E = {c}: row r excludes nb[r], k = n + 1
+        for (int64_t r = 0; r <= R; r++) self_off[(size_t)r] = r;
+        std::vector<int64_t> self(nb);
+        if ((st = recall::recall_rows(db, R, nullptr, V.nb.p, n, self_off.data(), self, self_off, nullptr, nullptr, nullptr, &exact_rows)))
+            return done(st);
+        const RecallWork &W = db->recall;
+        i2i_table_kernel<<<(unsigned)std::min<int64_t>(R, (int64_t)c->sm_count * 16), 128, 0, c->stream>>>(
+            W.slots.p, W.scores.p, W.count.p, R, n, db->distance == GORSE_B200_DISTANCE_DOT, V.t_slot.p, V.t_score.p, V.t_cnt.p);
+        c->launches++;
+    } else {
+        std::lock_guard<std::mutex> lk2(db->sparse->mu);
+        if ((st = sparse_search_rows(db->sparse, V.nb.p, R, db->d_allow.p, n, V.t_slot.p, V.t_score.p, V.t_cnt.p))) return done(st);
+    }
+    if ((e = cudaGetLastError()) != cudaSuccess) { set_error("item_to_item: %s", cudaGetErrorString(e)); return done(GORSE_B200_ERR_CUDA); }
+
+    // ---- stage B: users in chunks; a finished chunk is downloaded on the copy stream while the next one computes
+    const int64_t cu = std::min<int64_t>(n_users, (int64_t)c->sm_count * 1024);
+    const int64_t N = n_slots;
+    // global accumulators: one [N] float64 row, flag row and slot list per CTA, at most 512 MB
+    const int heavy_grid = (int)std::max<int64_t>(1, std::min<int64_t>((int64_t)c->sm_count * 2, (512ll << 20) / (13 * N)));
+    const int64_t total_ctx = c_off[(size_t)n_users];
+    if ((st = grow(V.c_off, (size_t)cu + 1)) || (st = grow(V.ex_off, (size_t)cu + 1)) || (st = grow(V.users, (size_t)cu)) ||
+        (st = grow(V.c_row, (size_t)std::max<int64_t>(total_ctx, 1))) || (st = grow(V.ex, std::max<size_t>(ex.size(), 1))) ||
+        (st = grow(V.slots, (size_t)n_users * n)) || (st = grow(V.scores, (size_t)n_users * n)) || (st = grow(V.count, (size_t)n_users)))
+        return done(st);
+    const size_t sm_shared = aggregate_smem(n, true), sm_global = aggregate_smem(n, false);
+    e = cudaFuncSetAttribute(i2i_aggregate_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm_shared);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(i2i_aggregate_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm_global);
+    if (e != cudaSuccess) { set_error("item_to_item: %s", cudaGetErrorString(e)); return done(GORSE_B200_ERR_CUDA); }
+    Table T;
+    T.slot = V.t_slot.p; T.score = V.t_score.p; T.cnt = V.t_cnt.p;
+    const bool euclid = db->distance == GORSE_B200_DISTANCE_EUCLIDEAN;
+    int64_t n_shared = 0, n_heavy = 0;
+    std::vector<int64_t> h_coff, h_exoff;
+    std::vector<int32_t> h_users;
+    for (int64_t u0 = 0; u0 < n_users; u0 += cu) {
+        const int64_t rows = std::min(cu, n_users - u0);
+        h_coff.resize(rows + 1); h_exoff.resize(rows + 1); h_users.resize(rows);
+        int64_t fill = 0, back = rows;   // table users from the front, heavy users from the back
+        for (int64_t r = 0; r <= rows; r++) {
+            h_coff[r] = c_off[u0 + r] - c_off[u0];
+            h_exoff[r] = ex_off[u0 + r] - ex_off[u0];
+        }
+        for (int64_t r = 0; r < rows; r++) {
+            if ((h_coff[r + 1] - h_coff[r]) * n <= TABLE_KEYS) h_users[fill++] = (int32_t)r;
+            else h_users[--back] = (int32_t)r;
+        }
+        n_shared += fill;
+        n_heavy += rows - fill;
+        if (rows - fill > 0 && ((st = grow(V.acc, (size_t)heavy_grid * N)) || (st = grow_zeroed(V.seen, (size_t)heavy_grid * N, c->stream)) ||
+                                (st = grow(V.touched, (size_t)heavy_grid * N))))
+            return done(st);
+        const int64_t n_c = h_coff[rows], n_e = h_exoff[rows];
+        if ((e = cudaMemcpyAsync(V.c_off.p, h_coff.data(), sizeof(int64_t) * (rows + 1), cudaMemcpyHostToDevice, c->stream)) != cudaSuccess ||
+            (e = cudaMemcpyAsync(V.ex_off.p, h_exoff.data(), sizeof(int64_t) * (rows + 1), cudaMemcpyHostToDevice, c->stream)) != cudaSuccess ||
+            (e = cudaMemcpyAsync(V.users.p, h_users.data(), sizeof(int32_t) * rows, cudaMemcpyHostToDevice, c->stream)) != cudaSuccess ||
+            (n_c && (e = cudaMemcpyAsync(V.c_row.p + c_off[u0], c_row.data() + c_off[u0], sizeof(int32_t) * n_c, cudaMemcpyHostToDevice, c->stream)) != cudaSuccess) ||
+            (n_e && (e = cudaMemcpyAsync(V.ex.p + ex_off[u0], ex.data() + ex_off[u0], sizeof(int64_t) * n_e, cudaMemcpyHostToDevice, c->stream)) != cudaSuccess)) {
+            set_error("item_to_item upload: %s", cudaGetErrorString(e));
+            return done(GORSE_B200_ERR_CUDA);
+        }
+        Users U;
+        U.c_off = V.c_off.p; U.c_row = V.c_row.p + c_off[u0]; U.ex_off = V.ex_off.p; U.ex = V.ex.p + ex_off[u0];
+        U.slots = V.slots.p + u0 * n; U.scores = V.scores.p + u0 * n; U.count = V.count.p + u0;
+        if (fill > 0) {
+            i2i_aggregate_kernel<true><<<(unsigned)std::min<int64_t>(fill, (int64_t)c->sm_count * 8), AGG_THREADS, sm_shared, c->stream>>>(
+                V.users.p, fill, U, T, n, score_scale, euclid, N, nullptr, nullptr, nullptr);
+            c->launches++;
+        }
+        if (rows - fill > 0) {
+            i2i_aggregate_kernel<false><<<(unsigned)std::min<int64_t>(rows - fill, heavy_grid), AGG_THREADS, sm_global, c->stream>>>(
+                V.users.p + fill, rows - fill, U, T, n, score_scale, euclid, N, V.acc.p, V.seen.p, V.touched.p);
+            c->launches++;
+        }
+        if ((e = cudaGetLastError()) != cudaSuccess) { set_error("item_to_item: %s", cudaGetErrorString(e)); return done(GORSE_B200_ERR_CUDA); }
+        if ((e = cudaEventRecord(c->copy_ev, c->stream)) != cudaSuccess || (e = cudaStreamWaitEvent(c->copy_stream, c->copy_ev, 0)) != cudaSuccess ||
+            (e = cudaMemcpyAsync(count_out + u0, V.count.p + u0, sizeof(int32_t) * rows, cudaMemcpyDeviceToHost, c->copy_stream)) != cudaSuccess ||
+            (e = cudaMemcpyAsync(slots_out + u0 * n, V.slots.p + u0 * n, sizeof(int64_t) * rows * n, cudaMemcpyDeviceToHost, c->copy_stream)) != cudaSuccess ||
+            (e = cudaMemcpyAsync(scores_out + u0 * n, V.scores.p + u0 * n, sizeof(double) * rows * n, cudaMemcpyDeviceToHost, c->copy_stream)) != cudaSuccess) {
+            set_error("item_to_item download: %s", cudaGetErrorString(e));
+            return done(GORSE_B200_ERR_CUDA);
+        }
+    }
+    if ((e = cudaStreamSynchronize(c->stream)) != cudaSuccess || (e = cudaStreamSynchronize(c->copy_stream)) != cudaSuccess) {
+        set_error("item_to_item: %s", cudaGetErrorString(e));
+        return done(GORSE_B200_ERR_CUDA);
+    }
+    if (stats_out) {
+        stats_out[0] = R;
+        stats_out[1] = exact_rows;
+        stats_out[2] = n_shared;
+        stats_out[3] = n_heavy;
+    }
+    return done(GORSE_B200_OK);
+}

@@ -17,6 +17,7 @@
 #include <algorithm>
 
 #include "cf.cuh"
+#include "recall.cuh"
 #include "topk.cuh"
 #include "vecdb.cuh"
 
@@ -45,107 +46,6 @@ struct RowInfo {              // per row of a chunk (chunk-local row ids)
     int32_t *count;           // [rows]
     int *flags;               // [0] NaN score seen, [1] rows the window kernel handed to the exact kernel
 };
-
-__device__ __forceinline__ bool contains(const int64_t *a, int64_t n, int64_t v)
-{
-    int64_t lo = 0, hi = n;
-    while (lo < hi) {
-        const int64_t mid = (lo + hi) >> 1;
-        if (a[mid] < v) lo = mid + 1;
-        else hi = mid;
-    }
-    return lo < n && a[lo] == v;
-}
-
-// exclusive rank of f among the CTA's threads in thread order; total = how many are set.  Every thread calls it.
-template <int NT>
-__device__ __forceinline__ int block_rank(bool f, int *s_warp, int &total)
-{
-    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-    const unsigned b = __ballot_sync(0xffffffffu, f);
-    __syncthreads();   // s_warp is free again
-    if (lane == 0) s_warp[w] = __popc(b);
-    __syncthreads();
-    int before = 0;
-    total = 0;
-#pragma unroll
-    for (int i = 0; i < NT / 32; i++) {
-        const int c = s_warp[i];
-        before += i < w ? c : 0;
-        total += c;
-    }
-    return before + __popc(b & ((1u << lane) - 1));
-}
-
-template <int NT>
-__device__ __forceinline__ int block_sum(int v, int *s_warp)
-{
-    for (int o = 16; o; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    __syncthreads();
-    if ((threadIdx.x & 31) == 0) s_warp[threadIdx.x >> 5] = v;
-    __syncthreads();
-    int t = 0;
-#pragma unroll
-    for (int i = 0; i < NT / 32; i++) t += s_warp[i];
-    return t;
-}
-
-// the m-th largest non-zero key of key_at(0 .. n-1) (at least m of them are non-zero), 8 bits per pass.  *ties = how many
-// entries equal to the result belong to the m largest.
-template <int NT, typename KeyAt>
-__device__ uint32_t block_select(int64_t n, int m, KeyAt key_at, int *hist /* [256] */, int *s_bc /* [2] */, int *ties)
-{
-    uint32_t prefix = 0, mask = 0;
-    int need = m;
-    for (int shift = 24; shift >= 0; shift -= 8) {
-        for (int b = threadIdx.x; b < 256; b += NT) hist[b] = 0;
-        __syncthreads();
-        for (int64_t i = threadIdx.x; i < n; i += NT) {
-            const uint32_t k = key_at(i);
-            if (k != 0u && (k & mask) == prefix) atomicAdd(&hist[(k >> shift) & 255u], 1);
-        }
-        __syncthreads();
-        if (threadIdx.x == 0) {
-            int above = 0, b = 255;
-            for (; b > 0 && above + hist[b] < need; b--) above += hist[b];
-            s_bc[0] = b;
-            s_bc[1] = need - above;
-        }
-        __syncthreads();
-        prefix |= (uint32_t)s_bc[0] << shift;
-        mask |= 255u << shift;
-        need = s_bc[1];
-        __syncthreads();
-    }
-    *ties = need;
-    return prefix;
-}
-
-// ascending bitonic sort of key[0, p) with a payload, p a power of two
-template <int NT>
-__device__ void block_sort(uint64_t *key, float *val, int p)
-{
-    for (int size = 2; size <= p; size <<= 1)
-        for (int stride = size >> 1; stride > 0; stride >>= 1) {
-            for (int i = threadIdx.x; i < p / 2; i += NT) {
-                const int lo = 2 * i - (i & (stride - 1)), hi = lo + stride;
-                const bool up = (lo & size) == 0;
-                const uint64_t a = key[lo], b = key[hi];
-                if ((a > b) == up) {
-                    key[lo] = b; key[hi] = a;
-                    const float t = val[lo]; val[lo] = val[hi]; val[hi] = t;
-                }
-            }
-            __syncthreads();
-        }
-}
-
-__host__ __device__ __forceinline__ int pow2_at_least(int m)
-{
-    int p = 1;
-    while (p < m) p <<= 1;
-    return p;
-}
 
 // the sorted entries [0, m) minus the row's excluded slots, appended at out + written
 template <int NT>
@@ -348,14 +248,15 @@ recall_exact_kernel(const float *X, int64_t N, int d, int metric, const uint8_t 
     }
 }
 
+// q[r] = X[slots[r]]: the query rows of stored vectors, one CTA per row
+__global__ void recall_gather_kernel(const float *X, int d, const int64_t *slots, int64_t rows, float *q)
+{
+    for (int64_t r = blockIdx.x; r < rows; r += gridDim.x)
+        for (int e = threadIdx.x; e < d; e += blockDim.x) q[r * d + e] = X[slots[r] * d + e];
+}
+
 size_t window_smem(int d) { return (size_t)SORT_CAP * 12 + (size_t)mma::CAP * 8 + (256 + 32 + 4) * 4 + (size_t)d * 4; }
 size_t exact_smem(int d) { return (size_t)SORT_CAP * 12 + (256 + 32 + 4) * 4 + (size_t)d * 4; }
-
-template <typename T>
-int32_t grow(DevBuf<T> &b, size_t n)
-{
-    return b.n >= n ? GORSE_B200_OK : b.alloc(n);
-}
 
 }  // namespace recall
 }  // namespace gb
@@ -409,9 +310,19 @@ extern "C" int32_t gorse_b200_vecdb_query_excluding(gorse_b200_vecdb *db, int64_
         for (int64_t q = 0; q < nq; q++) count_out[q] = 0;
         return GORSE_B200_OK;
     }
-    gorse_b200_ctx *c = db->ctx;
-    ScopedDevice sd(c->device);
+    ScopedDevice sd(db->ctx->device);
     GB_TRY(vecdb_allow(db, categories, n_categories));
+    return recall_rows(db, nq, q_values, nullptr, n, excl_off, ex, ex_off, slots_out, scores_out, count_out, exact_rows_out);
+}
+
+namespace gb {
+namespace recall {
+
+int32_t recall_rows(gorse_b200_vecdb *db, int64_t nq, const float *q_host, const int64_t *d_qslots, int32_t n, const int64_t *excl_off,
+                    const std::vector<int64_t> &ex, const std::vector<int64_t> &ex_off, int64_t *slots_out, float *scores_out,
+                    int32_t *count_out, int64_t *exact_rows_out)
+{
+    gorse_b200_ctx *c = db->ctx;
     gorse_b200_index *ix = db->dense;
     std::lock_guard<std::mutex> lk2(ix->mu);
     RecallWork &W = db->recall;
@@ -472,7 +383,11 @@ extern "C" int32_t gorse_b200_vecdb_query_excluding(gorse_b200_vecdb *db, int64_
         }
         host_exact += cls_begin[N_CLASSES + 1] - cls_begin[N_CLASSES];
         const int64_t n_ex = h_exoff[rows];
-        if ((e = cudaMemcpyAsync(W.q.p, q_values + q0 * d, sizeof(float) * rows * d, cudaMemcpyHostToDevice, c->stream)) != cudaSuccess ||
+        if (!q_host) {   // stored vectors: gathered from the collection in place of the upload
+            recall_gather_kernel<<<(unsigned)std::min<int64_t>(rows, (int64_t)c->sm_count * 16), 128, 0, c->stream>>>(ix->X.p, d, d_qslots + q0, rows, W.q.p);
+            c->launches++;
+        }
+        if ((q_host && (e = cudaMemcpyAsync(W.q.p, q_host + q0 * d, sizeof(float) * rows * d, cudaMemcpyHostToDevice, c->stream)) != cudaSuccess) ||
             (e = cudaMemcpyAsync(W.k.p, h_k.data(), sizeof(int32_t) * rows, cudaMemcpyHostToDevice, c->stream)) != cudaSuccess ||
             (e = cudaMemcpyAsync(W.need.p, h_need.data(), sizeof(int32_t) * rows, cudaMemcpyHostToDevice, c->stream)) != cudaSuccess ||
             (e = cudaMemcpyAsync(W.ex_off.p, h_exoff.data(), sizeof(int64_t) * (rows + 1), cudaMemcpyHostToDevice, c->stream)) != cudaSuccess ||
@@ -500,6 +415,7 @@ extern "C" int32_t gorse_b200_vecdb_query_excluding(gorse_b200_vecdb *db, int64_
             ix->X.p, N, d, ix->metric, db->d_allow.p, rows, R, W.scratch.p);
         c->launches++;
         if ((e = cudaGetLastError()) != cudaSuccess) { set_error("query_excluding: %s", cudaGetErrorString(e)); return done(GORSE_B200_ERR_CUDA); }
+        if (!slots_out) continue;   // the caller reads the answers on the device
         // this chunk is final: download it on the copy stream while the next chunk computes
         const int64_t o0 = out_at(q0), o1 = out_at(q0 + rows);
         if ((e = cudaEventRecord(c->copy_ev, c->stream)) != cudaSuccess || (e = cudaStreamWaitEvent(c->copy_stream, c->copy_ev, 0)) != cudaSuccess ||
@@ -520,3 +436,6 @@ extern "C" int32_t gorse_b200_vecdb_query_excluding(gorse_b200_vecdb *db, int64_
     if (exact_rows_out) *exact_rows_out = host_exact + flags[1];
     return done(GORSE_B200_OK);
 }
+
+}  // namespace recall
+}  // namespace gb

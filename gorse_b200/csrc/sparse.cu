@@ -52,21 +52,23 @@ __device__ __forceinline__ void list_insert_warp(float *ld, int32_t *li, int &le
     __syncwarp();
 }
 
+template <bool ROW_LIST>
 __global__ void __launch_bounds__(128)
 sparse_search_kernel(const int64_t *off, const uint32_t *ind, const float *val, const int64_t *foff, const int32_t *frow,
                      const float *fval, int64_t N, uint32_t n_features, int64_t q0, int64_t nq, int k, float *acc, int32_t *out_idx,
                      float *out_dot, int32_t *out_count, const int64_t *q_off, const uint32_t *q_ind, const float *q_val,
-                     const uint8_t *allow)
+                     const uint8_t *allow, const int64_t *q_rows)
 {
-    // queries: stored rows q0 + q (never returned themselves), or -- q_off != nullptr -- rows of an external CSR
-    // (vecdb.cu: QueryVectors passes the vector, not its id); allow: optional per-row filter
+    // queries: stored rows q0 + q, or q_rows[q] with ROW_LIST (a device list, item_to_item.cu) -- never returned themselves --
+    // or, q_off != nullptr, rows of an external CSR (vecdb.cu: QueryVectors passes the vector, not its id); allow: optional
+    // per-row filter
     extern __shared__ unsigned char sm_raw[];
     const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5, nw = blockDim.x >> 5;
     float *ld = reinterpret_cast<float *>(sm_raw) + (size_t)wid * k;
     int32_t *li = reinterpret_cast<int32_t *>(reinterpret_cast<float *>(sm_raw) + (size_t)nw * k) + (size_t)wid * k;
     float *a = acc + ((int64_t)blockIdx.x * nw + wid) * N;   // this warp's accumulator row, all zero between queries
     for (int64_t q = (int64_t)blockIdx.x * nw + wid; q < nq; q += (int64_t)gridDim.x * nw) {
-        const int64_t row = q_off ? -1 : q0 + q;
+        const int64_t row = q_off ? -1 : ROW_LIST ? q_rows[q] : q0 + q;
         const int64_t tb = q_off ? q_off[q] : off[row], te = q_off ? q_off[q + 1] : off[row + 1];
         const uint32_t *qi = q_off ? q_ind : ind;
         const float *qv = q_off ? q_val : val;
@@ -236,6 +238,39 @@ namespace gb {
 
 // queries = stored rows [q0, q0 + nq) (q_off == nullptr) or nq rows of a HOST CSR (q_off/q_ind/q_val); allow = optional DEVICE
 // per-row filter; results to host buffers.  The caller holds ix->mu.
+static constexpr int SEARCH_WARPS = 4;
+
+// one accumulator row per resident warp, at most ~1 GB of them; returns the grid of sparse_search_kernel
+static int32_t reserve_acc(gorse_b200_sparse_index *ix, int64_t n, int64_t nq, int *grid)
+{
+    gorse_b200_ctx *c = ix->ctx;
+    const int warps = SEARCH_WARPS;
+    int64_t slots = std::min<int64_t>((nq + warps - 1) / warps * warps, (int64_t)c->sm_count * 4 * warps);
+    slots = std::max<int64_t>(warps, std::min<int64_t>(slots, ((1ll << 30) / 4 / std::max<int64_t>(1, n)) / warps * warps));
+    if (ix->acc_slots < slots) {
+        GB_TRY(ix->acc.alloc((size_t)slots * (size_t)n));
+        GB_CUDA(cudaMemsetAsync(ix->acc.p, 0, sizeof(float) * (size_t)slots * (size_t)n, c->stream));
+        ix->acc_slots = slots;
+    }
+    *grid = (int)(slots / warps);
+    return GORSE_B200_OK;
+}
+
+int32_t sparse_search_rows(gorse_b200_sparse_index *ix, const int64_t *d_rows, int64_t nq, const uint8_t *d_allow, int32_t k, int32_t *d_idx,
+                           float *d_dot, int32_t *d_cnt)
+{
+    const int64_t n = (int64_t)ix->h_off.size() - 1;
+    gorse_b200_ctx *c = ix->ctx;
+    GB_TRY(sync_device(ix));
+    int grid = 0;
+    GB_TRY(reserve_acc(ix, n, nq, &grid));
+    sparse_search_kernel<true><<<grid, 32 * SEARCH_WARPS, (size_t)SEARCH_WARPS * 2 * (size_t)k * 4, c->stream>>>(
+        ix->off.p, ix->ind.p, ix->val.p, ix->foff.p, ix->frow.p, ix->fval.p, n, ix->n_features, 0, nq, k, ix->acc.p, d_idx, d_dot, d_cnt,
+        nullptr, nullptr, nullptr, d_allow, d_rows);
+    GB_LAUNCHED(c);
+    return GORSE_B200_OK;
+}
+
 int32_t sparse_search_host(gorse_b200_sparse_index *ix, int64_t q0, int64_t nq, const int64_t *q_off, const uint32_t *q_ind,
                            const float *q_val, const uint8_t *d_allow, int32_t k, int32_t *idx_out, float *dot_out, int32_t *count_out)
 {
@@ -247,15 +282,9 @@ int32_t sparse_search_host(gorse_b200_sparse_index *ix, int64_t q0, int64_t nq, 
         for (int64_t q = 0; q < nq; q++) count_out[q] = 0;
         return GORSE_B200_OK;
     }
-    const int warps = 4;
-    // one accumulator row per resident warp, at most ~1 GB of them
-    int64_t slots = std::min<int64_t>((nq + warps - 1) / warps * warps, (int64_t)c->sm_count * 4 * warps);
-    slots = std::max<int64_t>(warps, std::min<int64_t>(slots, ((1ll << 30) / 4 / std::max<int64_t>(1, n)) / warps * warps));
-    if (ix->acc_slots < slots) {
-        GB_TRY(ix->acc.alloc((size_t)slots * (size_t)n));
-        GB_CUDA(cudaMemsetAsync(ix->acc.p, 0, sizeof(float) * (size_t)slots * (size_t)n, c->stream));
-        ix->acc_slots = slots;
-    }
+    const int warps = SEARCH_WARPS;
+    int grid = 0;
+    GB_TRY(reserve_acc(ix, n, nq, &grid));
     DevBuf<int32_t> d_idx, d_cnt;
     DevBuf<float> d_dot, dq_val;
     DevBuf<int64_t> dq_off;
@@ -272,11 +301,10 @@ int32_t sparse_search_host(gorse_b200_sparse_index *ix, int64_t q0, int64_t nq, 
         if (e == cudaSuccess && qn) e = cudaMemcpyAsync(dq_val.p, q_val, sizeof(float) * (size_t)qn, cudaMemcpyHostToDevice, c->stream);
         if (e != cudaSuccess) { set_error("sparse search upload: %s", cudaGetErrorString(e)); return done(GORSE_B200_ERR_CUDA); }
     }
-    const int grid = (int)(slots / warps);
     const size_t sm = (size_t)warps * 2 * (size_t)k * 4;
-    sparse_search_kernel<<<grid, 32 * warps, sm, c->stream>>>(ix->off.p, ix->ind.p, ix->val.p, ix->foff.p, ix->frow.p, ix->fval.p, n,
+    sparse_search_kernel<false><<<grid, 32 * warps, sm, c->stream>>>(ix->off.p, ix->ind.p, ix->val.p, ix->foff.p, ix->frow.p, ix->fval.p, n,
                                                              ix->n_features, q0, nq, k, ix->acc.p, d_idx.p, d_dot.p, d_cnt.p,
-                                                             q_off ? dq_off.p : nullptr, dq_ind.p, dq_val.p, d_allow);
+                                                             q_off ? dq_off.p : nullptr, dq_ind.p, dq_val.p, d_allow, nullptr);
     c->launches++;
     e = cudaGetLastError();
     if (e == cudaSuccess) e = cudaMemcpyAsync(idx_out, d_idx.p, sizeof(int32_t) * (size_t)nq * k, cudaMemcpyDeviceToHost, c->stream);

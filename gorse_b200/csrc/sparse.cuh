@@ -26,4 +26,9 @@ struct gorse_b200_sparse_index {
 namespace gb {
 int32_t sparse_search_host(gorse_b200_sparse_index *ix, int64_t q0, int64_t nq, const int64_t *q_off, const uint32_t *q_ind,
                            const float *q_val, const uint8_t *d_allow, int32_t k, int32_t *idx_out, float *dot_out, int32_t *count_out);
+// queries = the stored rows of the DEVICE list d_rows[nq] (each never returned itself), results left on the device in the
+// layout of sparse_search_host (d_idx / d_dot [nq x k] padded with -1 / 0, d_cnt[nq]); enqueued on the context's stream.  The
+// index holds at least one vector; the caller holds ix->mu and the device.
+int32_t sparse_search_rows(gorse_b200_sparse_index *ix, const int64_t *d_rows, int64_t nq, const uint8_t *d_allow, int32_t k, int32_t *d_idx,
+                           float *d_dot, int32_t *d_cnt);
 }

@@ -15,6 +15,22 @@ struct RecallWork {
         k.free(); need.free(); count.free(); flags.free();
     }
 };
+// grow-only work buffers of gorse_b200_vecdb_item_to_item (item_to_item.cu): the neighbour table of stage A and the user
+// batches, answers and accumulator scratch of stage B
+struct ItemToItemWork {
+    DevBuf<int64_t> nb, c_off, ex_off, ex, slots;
+    DevBuf<int32_t> t_slot, t_cnt, c_row, users, count;
+    DevBuf<float> t_score;
+    DevBuf<double> scores, acc;
+    DevBuf<uint8_t> seen;
+    DevBuf<int32_t> touched;
+    void free()
+    {
+        nb.free(); c_off.free(); ex_off.free(); ex.free(); slots.free();
+        t_slot.free(); t_cnt.free(); c_row.free(); users.free(); count.free();
+        t_score.free(); scores.free(); acc.free(); seen.free(); touched.free();
+    }
+};
 }  // namespace gb
 
 struct gorse_b200_vecdb {
@@ -34,6 +50,7 @@ struct gorse_b200_vecdb {
     gb::DevBuf<int64_t> d_cat_off;
     gb::DevBuf<int32_t> d_cats, d_want;
     gb::RecallWork recall;   // batched recall (recall.cu)
+    gb::ItemToItemWork i2i;  // batched item-to-item recommendation (item_to_item.cu)
 };
 
 namespace gb {

@@ -374,6 +374,32 @@ int32_t gorse_b200_vecdb_query(gorse_b200_vecdb *db, int64_t nq, const float *q_
 int32_t gorse_b200_vecdb_query_excluding(gorse_b200_vecdb *db, int64_t nq, const float *q_values, const int32_t *categories,
                                          int32_t n_categories, int32_t n, const int64_t *excl_off, const int64_t *excl_slots,
                                          int64_t *slots_out, float *scores_out, int32_t *count_out, int64_t *exact_rows_out);
+/* Batched item-to-item recommendation: for n_users users at once, what the worker's item-to-item recommender does per user
+ * (Recommender.recommendItemToItem, logics/recommend.go:244-283) on one item-to-item collection: Euclidean for type
+ * "embedding", sparse Dot for "tags" / "users" / "auto".
+ *   C_u = ctx_slots[ctx_off[u] .. ctx_off[u+1]) (ctx_off[0] = 0): the user's positive feedback items, visited in the given
+ *   order (the reference's is newest first); a slot may repeat (its neighbours are then added again).  Entries -1 (an id
+ *   without a vector) and deleted slots are skipped; a hidden item is still a context item.  A slot outside [-1, slots) is
+ *   GORSE_B200_ERR_ARG.
+ *   E_u = excl_slots[excl_off[u] .. excl_off[u+1]): the user's exclude set, with the rules of
+ *   gorse_b200_vecdb_query_excluding (-1 allowed, a slot twice in one row is GORSE_B200_ERR_ARG).
+ *   Neighbours of a context item c: the candidates of gorse_b200_vecdb_query (live, not hidden, ALL of
+ *   categories[n_categories]) other than c, by score descending, exact ties by lower slot; Dot collections drop scores <= 0;
+ *   the first n.  Their scores are bit-identical to gorse_b200_vecdb_query's.
+ *   Neighbour score s = (double)score * score_scale (0.5 for type "auto", else 1); Euclidean: s = 1 / (1 - s).
+ *   Row u: for every context entry in order and every neighbour j not in E_u, acc[j] += s in float64; the first n of acc by
+ *   score descending, exact ties by lower slot.  Each sum is formed in context order, as the reference's, so the scores match
+ *   it bit for bit.  The reference ranks exact ties in Go map order, so which of them it keeps at the cut is unpinned.
+ *   Output: row u at u*n in slots_out / scores_out (buffers of n_users*n), count_out[u] <= n entries.  n <= 0: every count
+ *   is 0.  n above 128 (sparse) or 1024 (dense): GORSE_B200_ERR_UNSUPPORTED; Cosine collections: GORSE_B200_ERR_UNSUPPORTED.
+ *   A NaN score (or score_scale): GORSE_B200_ERR_ARG.  Every argument is checked before the device is touched.
+ *   stats_out[4] (may be NULL): distinct context items queried, of them answered by the exact scan rather than the tensor-core
+ *   sweep (dense), users aggregated in shared memory, users aggregated in a global-memory row; the answer does not depend
+ *   on them.  Thread-safe per collection. */
+int32_t gorse_b200_vecdb_item_to_item(gorse_b200_vecdb *db, int64_t n_users, const int64_t *ctx_off, const int64_t *ctx_slots,
+                                      const int64_t *excl_off, const int64_t *excl_slots, const int32_t *categories, int32_t n_categories,
+                                      int32_t n, double score_scale, int64_t *slots_out, double *scores_out, int32_t *count_out,
+                                      int64_t *stats_out);
 
 /* ------------------------------------------------------------------------------------------
  * NCF-format datasets: dataset.LoadDataFromBuiltIn (dataset/dataset.go:398-490), the loader `gorse-bench cf`
