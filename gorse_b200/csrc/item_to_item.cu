@@ -6,8 +6,8 @@
 // one call answers many users:
 //
 //   stage A   the neighbour table, once per call: the distinct live context items of the whole batch are queried once each.
-//             Dense collections run the recall pipeline of recall.cu (recall_rows) with E = {c} and k = n + 1 on the stored
-//             vectors, then i2i_table_kernel cuts each row to n and drops Dot scores <= 0.  Sparse collections run
+//             Dense collections run the index's top-k pipeline (recall_rows, topk.cu) with k = n on the stored vectors (a
+//             row never returns its own vector), and its table keeps Dot scores > 0 only.  Sparse collections run
 //             sparse_search_kernel on the list of stored rows (a row never finds itself; it keeps positive dots only).
 //             The table holds n (int32 slot, float32 score) entries per item, scores bit-identical to gorse_b200_vecdb_query.
 //   stage B   i2i_aggregate_kernel, one CTA per user: walks C_u in order and adds s = (double)score * scale (Euclidean:
@@ -60,29 +60,6 @@ __device__ __forceinline__ double neighbour_score(float raw, double scale, bool 
 {
     const double s = __dmul_rn((double)raw, scale);
     return euclid ? __ddiv_rn(1.0, __dsub_rn(1.0, s)) : s;
-}
-
-// row r of the recall with k = n + 1 (at r * (n + 1)): its first n entries; Dot keeps scores > 0 only (a prefix: rows are
-// sorted by score descending)
-__global__ void i2i_table_kernel(const int64_t *slots, const float *scores, const int32_t *count, int64_t rows, int n, int dot,
-                                 int32_t *t_slot, float *t_score, int32_t *t_cnt)
-{
-    for (int64_t r = blockIdx.x; r < rows; r += gridDim.x) {
-        const int c = min(count[r], n);
-        const int64_t src = r * (n + 1), dst = r * n;
-        int kept = 0;
-        for (int base = 0; base < c; base += blockDim.x) {
-            const int j = base + threadIdx.x;
-            const float s = j < c ? scores[src + j] : 0.f;
-            const bool keep = j < c && (!dot || s > 0.f);
-            if (keep) {
-                t_slot[dst + j] = (int32_t)slots[src + j];
-                t_score[dst + j] = s;
-            }
-            kept += __syncthreads_count(keep);
-        }
-        if (threadIdx.x == 0) t_cnt[r] = kept;
-    }
 }
 
 // one CTA per user of `users`.  SHARED: the accumulator is a table in shared memory; else acc_rows / seen_rows /
@@ -309,15 +286,11 @@ extern "C" int32_t gorse_b200_vecdb_item_to_item(gorse_b200_vecdb *db, int64_t n
     // ---- stage A: the neighbour table
     int64_t exact_rows = 0;
     if (!sparse) {
-        std::vector<int64_t> self_off((size_t)R + 1);   // E = {c}: row r excludes nb[r], k = n + 1
-        for (int64_t r = 0; r <= R; r++) self_off[(size_t)r] = r;
-        std::vector<int64_t> self(nb);
-        if ((st = recall::recall_rows(db, R, nullptr, V.nb.p, n, self_off.data(), self, self_off, nullptr, nullptr, nullptr, &exact_rows)))
+        std::lock_guard<std::mutex> lk2(db->dense->mu);
+        const recall::Table table{V.t_slot.p, V.t_score.p, V.t_cnt.p, false, db->distance == GORSE_B200_DISTANCE_DOT, nullptr, nullptr, nullptr};
+        if ((st = recall::recall_rows(db->dense, db->d_allow.p, R, nullptr, V.nb.p, n, nullptr, nullptr, nullptr, &table, nullptr, nullptr, nullptr,
+                                      &exact_rows)))
             return done(st);
-        const RecallWork &W = db->recall;
-        i2i_table_kernel<<<(unsigned)std::min<int64_t>(R, (int64_t)c->sm_count * 16), 128, 0, c->stream>>>(
-            W.slots.p, W.scores.p, W.count.p, R, n, db->distance == GORSE_B200_DISTANCE_DOT, V.t_slot.p, V.t_score.p, V.t_cnt.p);
-        c->launches++;
     } else {
         std::lock_guard<std::mutex> lk2(db->sparse->mu);
         if ((st = sparse_search_rows(db->sparse, V.nb.p, R, db->d_allow.p, n, V.t_slot.p, V.t_score.p, V.t_cnt.p))) return done(st);

@@ -1,9 +1,7 @@
-// recall.cuh -- block-wide selection and sorting helpers of the batched recall (recall.cu), shared with the item-to-item
-// aggregation (item_to_item.cu), and the recall's chunked row pipeline.
+// recall.cuh -- block-wide selection and sorting helpers of the top-k pipeline (topk.cu), shared with the item-to-item
+// aggregation (item_to_item.cu).
 #pragma once
-#include <vector>
-
-#include "vecdb.cuh"
+#include "common.cuh"
 
 namespace gb {
 namespace recall {
@@ -61,6 +59,7 @@ __device__ auto block_select(int64_t n, int m, KeyAt key_at, int *hist /* [256] 
     using K = decltype(key_at(0));
     K prefix = 0, mask = 0;
     int need = m;
+    const int lane = threadIdx.x & 31;
     for (int shift = 8 * (int)sizeof(K) - 8; shift >= 0; shift -= 8) {
         for (int b = threadIdx.x; b < 256; b += NT) hist[b] = 0;
         __syncthreads();
@@ -69,11 +68,34 @@ __device__ auto block_select(int64_t n, int m, KeyAt key_at, int *hist /* [256] 
             if (k != 0u && (k & mask) == prefix) atomicAdd(&hist[(uint32_t)(k >> shift) & 255u], 1);
         }
         __syncthreads();
-        if (threadIdx.x == 0) {
-            int above = 0, b = 255;
-            for (; b > 0 && above + hist[b] < need; b--) above += hist[b];
-            s_bc[0] = b;
-            s_bc[1] = need - above;
+        if (threadIdx.x < 32) {
+            // the bin holding the need-th largest key, from the top: lane l sums bins 255 - 8 l .. 248 - 8 l, a warp scan
+            // gives the keys above each lane's bins, and the lane where the running count reaches need picks the bin (bins
+            // 255 .. 1; bin 0 when they hold fewer than need keys)
+            int sum = 0;
+#pragma unroll
+            for (int j = 0; j < 8; j++) sum += hist[255 - 8 * lane - j];
+            int incl = sum;
+#pragma unroll
+            for (int o = 1; o < 32; o <<= 1) {
+                const int t = __shfl_up_sync(0xffffffffu, incl, o);
+                if (lane >= o) incl += t;
+            }
+            int above = incl - sum, pick = -1;
+#pragma unroll
+            for (int j = 0; j < 8; j++) {
+                const int b = 255 - 8 * lane - j;
+                if (pick < 0 && b > 0 && above + hist[b] >= need) pick = b;
+                if (pick < 0 && b > 0) above += hist[b];
+            }
+            const unsigned found = __ballot_sync(0xffffffffu, pick >= 0);
+            const int src = found ? __ffs(found) - 1 : 31;   // none: bin 0, above = the keys of bins 255 .. 1
+            const int b = __shfl_sync(0xffffffffu, pick >= 0 ? pick : 0, src);
+            const int ab = __shfl_sync(0xffffffffu, above, src);
+            if (lane == 0) {
+                s_bc[0] = b;
+                s_bc[1] = need - ab;
+            }
         }
         __syncthreads();
         prefix |= (K)s_bc[0] << shift;
@@ -118,17 +140,6 @@ int32_t grow(DevBuf<T> &b, size_t n)
 {
     return b.n >= n ? GORSE_B200_OK : b.alloc(n);
 }
-
-// The chunked row pipeline of gorse_b200_vecdb_query_excluding (routing, tensor-core sweep, window and exact kernels), for
-// nq rows of one collection whose allow mask is current.  Row q is a host query q_host[q * d ..] or, with q_host == nullptr,
-// the stored vector of slot d_qslots[q] (a device list), gathered on the device.  k_q = n + (excl_off[q + 1] - excl_off[q]);
-// ex / ex_off: each row's exclusions sorted, -1 entries dropped.  Row q's answer starts at q * n + excl_off[q] in
-// db->recall.slots / scores, count in db->recall.count[q]; with slots_out != nullptr every finished chunk is also downloaded
-// to the host buffers while the next one computes.  *exact_rows_out: rows the exact kernel answered.  The caller holds
-// db->mu; the call ends with both streams synchronised.
-int32_t recall_rows(gorse_b200_vecdb *db, int64_t nq, const float *q_host, const int64_t *d_qslots, int32_t n, const int64_t *excl_off,
-                    const std::vector<int64_t> &ex, const std::vector<int64_t> &ex_off, int64_t *slots_out, float *scores_out,
-                    int32_t *count_out, int64_t *exact_rows_out);
 
 }  // namespace recall
 }  // namespace gb

@@ -1,217 +1,483 @@
-// topk.cu -- brute-force vector index: ann.Bruteforce (common/ann/bruteforce.go:24-83) behind ann.Index.
+// topk.cu -- the dense top-k pipeline, and the brute-force vector index on it: ann.Bruteforce (common/ann/bruteforce.go:24-83)
+// behind ann.Index.
 //
-// Two stages share one result contract (k smallest distances, ascending; ties broken by ascending index --
-// the reference's tie order is an artefact of Go's container/heap and is not pinned by any reference test):
-//   stage 1  candidate generation.  Small problems: exact scan (this file).  Large d % 16 == 0 problems:
-//            bf16 wgmma GEMM with a fused threshold filter (topk_mma.cu), which over-fetches by a rigorous
-//            error margin so the true top-k is always among the candidates.
-//   stage 2  exact re-rank of the candidates with the reference's fp32 summation order
-//            (floats.Euclidean / -floats.Dot, AVX-512 tree), final sort, prune0.
+// One result contract for every caller (the index's searches, the collection query, the batched recall and item-to-item):
+// the first k allowed vectors by (distance ascending = score descending, slot ascending), scored with the reference's fp32
+// summation order (floats.Euclidean / -floats.Dot, AVX-512 tree).  The reference's tie order is an artefact of Go's
+// container/heap and is not pinned by any reference test.  A row whose query is a stored vector never returns that vector
+// (bruteforce.go:47).
+//
+//   routing   rows with k_q <= 128 / 256 / 512 form classes; each class is swept by the tensor-core stage 1 (topk_mma.cu) with
+//             a sample aimed at min(4 x the class's largest k_q, CAP / 2) columns per row.  Rows above 512, calls the sweep does
+//             not serve (mma_path_eligible: small indexes, few rows, Cosine) and rows whose window cannot be certified go to
+//             the exact kernel.
+//   stage 2   recall_window_kernel, one CTA per row: drops the candidates the filter rejects and the row's own vector,
+//             certifies the row against its own k_q (k_q-th best approximate score >= theta + 2 eps), re-scores the window
+//             exactly, sorts it in shared memory and writes the first k_q minus the row's exclusions.
+//   exact     recall_exact_kernel, one CTA per row: scores every allowed vector into scratch, selects the k_q-th key by radix
+//             select, and emits the result in sorted rounds of at most SORT_CAP entries.
+//   table     table_kernel: the answers as a fixed-stride table (the index's int32 ids and distances, prune0; item-to-item's
+//             neighbour table).
+// Both paths order by the same key and write the same score bits, so a row's answer does not depend on its path.
 #include <algorithm>
 #include <cmath>
 
 #include "cf.cuh"
+#include "recall.cuh"
 #include "topk.cuh"
 
 namespace gb {
+namespace recall {
 
-// (dist, idx) ordering used everywhere: ascending distance, then ascending index
-__device__ __forceinline__ bool before(float da, int32_t ia, float db, int32_t ib) { return da < db || (da == db && ia < ib); }
+constexpr int N_CLASSES = 3;
+constexpr int CLASS_K[N_CLASSES] = {128, 256, 512};
+constexpr int SORT_CAP = mma::CAP;   // entries one CTA sorts at a time (a window never holds more)
+constexpr int WIN_THREADS = 256, EXACT_THREADS = 256;
 
-// sorted insertion into a warp-private list kept in shared memory (lane 0 only); list holds <= k entries
-__device__ __forceinline__ void list_insert(float *ld, int32_t *li, int &len, int k, float dv, int32_t iv)
+// order key of a score: larger score = larger key; -0 and +0 are one score (the exact scan compares floats); NaN = 0 = no entry
+__device__ __forceinline__ uint32_t rank_key(float s) { return s != s ? 0u : float_key(s == 0.f ? 0.f : s); }
+// sort key: ascending order = score descending, then slot ascending
+__device__ __forceinline__ uint64_t sort_key(uint32_t key, int64_t slot) { return ((uint64_t)~key << 32) | (uint32_t)slot; }
+
+struct RowInfo {              // per row of a chunk (chunk-local row ids)
+    const float *q;           // [rows][d] queries
+    const int32_t *k;         // n + |E_q|
+    const int64_t *ex_off;    // [rows + 1] into ex
+    const int64_t *ex;        // each row's excluded slots, ascending (-1 entries dropped)
+    const int64_t *out_off;   // where the row's answer starts in slots / scores
+    const int64_t *self;      // [rows] the slot of a stored query (never returned), or nullptr
+    int64_t *exact;           // rows the exact kernel answers: n_routed routed by the host, then the window kernel's hand-offs
+    int64_t n_routed;
+    int64_t *slots;
+    float *scores;
+    int32_t *count;           // [rows]
+    int *flags;               // [0] NaN score seen, [1] rows the window kernel handed to the exact kernel, [2] of them in this chunk
+};
+
+// the sorted entries [0, m) minus the row's excluded slots, appended at out + written
+template <int NT>
+__device__ void block_emit(const uint64_t *key, const float *val, int m, const int64_t *ex, int64_t n_ex, int64_t *out_slots,
+                           float *out_scores, int &written, int *s_warp)
 {
-    if (len == k && !before(dv, iv, ld[k - 1], li[k - 1])) return;
-    int pos = len < k ? len : k - 1;
-    while (pos > 0 && before(dv, iv, ld[pos - 1], li[pos - 1])) {
-        ld[pos] = ld[pos - 1];
-        li[pos] = li[pos - 1];
-        pos--;
+    for (int base = 0; base < m; base += NT) {
+        const int i = base + threadIdx.x;
+        int64_t slot = 0;
+        bool keep = false;
+        if (i < m) {
+            slot = (int64_t)(uint32_t)key[i];
+            keep = !contains(ex, n_ex, slot);
+        }
+        int total;
+        const int r = block_rank<NT>(keep, s_warp, total);
+        if (keep) {
+            out_slots[written + r] = slot;
+            out_scores[written + r] = val[i];
+        }
+        written += total;
     }
-    ld[pos] = dv;
-    li[pos] = iv;
-    if (len < k) len++;
 }
 
-// the same insertion done by the whole warp: every lane owns list slots lane, lane+32, ...; the position is a ballot count
-// and the shift is one read + one write per owned slot.  All arguments are warp-uniform; len lives in every lane.
-__device__ __forceinline__ void list_insert_warp(float *ld, int32_t *li, int &len, int k, float dv, int32_t iv, int lane)
+// score = -distance in the reference's arithmetic for count vectors: slot_at(j) < 0 skips entry j.
+// put(j, score, valid) is called once per entry.
+template <int NT, typename SlotAt, typename Put>
+__device__ __forceinline__ void block_score(const float *X, int d, int metric, const float *qs, float qq, int64_t count, SlotAt slot_at, Put put)
 {
-    if (len == k && !before(dv, iv, ld[k - 1], li[k - 1])) return;
-    const int n = len;
-    float od[4];
-    int32_t oi[4];
-    int pos = 0;
+    if (d % 16 == 0 && d <= 256) {
+        const int lane4 = threadIdx.x & 3, chunks = d / 16;
+        const unsigned qmask = quad_mask();
+        float4 qreg[16];
 #pragma unroll
-    for (int r = 0; r < 4; r++) {
-        const int e = lane + 32 * r;
-        const bool has = e < n;
-        od[r] = has ? ld[e] : 0.f;
-        oi[r] = has ? li[e] : 0;
-        pos += __popc(__ballot_sync(0xffffffffu, has && before(od[r], oi[r], dv, iv)));
+        for (int c = 0; c < 16; c++)
+            if (c < chunks) qreg[c] = *reinterpret_cast<const float4 *>(qs + 16 * c + 4 * lane4);
+        for (int64_t j = threadIdx.x >> 2; j < count; j += NT / 4) {   // a quad per entry: its 4 lanes share j
+            const int64_t v = slot_at(j);
+            float s = 0.f;
+            if (v >= 0) s = -quad_dist(qreg, X + v * d, chunks, lane4, qmask, metric, qq);
+            if (lane4 == 0) put(j, s, v >= 0);
+        }
+    } else {
+        for (int64_t j = threadIdx.x; j < count; j += NT) {
+            const int64_t v = slot_at(j);
+            put(j, v >= 0 ? -dist_any(qs, X + v * d, d, metric, qq) : 0.f, v >= 0);
+        }
     }
-    __syncwarp();
-#pragma unroll
-    for (int r = 0; r < 4; r++) {
-        const int e = lane + 32 * r;
-        if (e < n && e >= pos && e + 1 < k) { ld[e + 1] = od[r]; li[e + 1] = oi[r]; }
-    }
-    if (lane == 0) { ld[pos] = dv; li[pos] = iv; }
-    if (len < k) len++;
-    __syncwarp();
 }
 
-// Exact scan: one warp per query over vectors [0, N) or over a candidate list.
-//   queries:   nq rows of d floats (q_ptr), or rows of X selected by q_idx when q_ptr == nullptr
-//   self skip: SearchIndex never returns q itself (bruteforce.go:47)
-//   cand:      optional candidate lists [nq][cand_stride] (idx < 0 = empty slot) -> stage-2 re-rank
-__global__ void __launch_bounds__(128)
-topk_exact_kernel(const float *X, int64_t N, int d, int metric, const float *q_ptr, const int64_t *q_idx, int64_t q0,
-                  int64_t nq, int k, const int32_t *cand, const int32_t *cand_count, int cand_stride, const int32_t *row_list,
-                  int32_t *out_idx, float *out_dist, int32_t *out_count, int prune0, int *nan_flag, int n_seg, int64_t seg_len,
-                  int cand_by_slot, const uint8_t *allow /* optional per-vector filter (vecdb.cu): 0 = never returned */)
+template <int NT>
+__device__ __forceinline__ float load_query(const float *q, int d, int metric, float *qs)
 {
-    extern __shared__ unsigned char sm_raw[];
-    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5, nw = blockDim.x >> 5;
-    float *ld = reinterpret_cast<float *>(sm_raw) + (size_t)wid * k;
-    int32_t *li = reinterpret_cast<int32_t *>(reinterpret_cast<float *>(sm_raw) + (size_t)nw * k) + (size_t)wid * k;
-    float *qs = reinterpret_cast<float *>(sm_raw) + (size_t)2 * nw * k + (size_t)wid * d;
-    const int lane4 = lane & 3, quad = lane >> 2;
-    const unsigned qmask = quad_mask();
-    // nq counts work slots: slot = (row_slot, segment).  With n_seg > 1 every slot scans one segment of the vectors and
-    // writes its own partial top-k at out[slot]; a second pass merges the partial lists (cand_by_slot) into out[row].
-    for (int64_t slot = (int64_t)blockIdx.x * nw + wid; slot < nq; slot += (int64_t)gridDim.x * nw) {
-        const int64_t row_slot = slot / n_seg;
-        const int seg = (int)(slot % n_seg);
-        const int64_t qi = row_list ? (int64_t)row_list[row_slot] : row_slot;
-        const int64_t oq = n_seg > 1 ? slot : qi;
-        int64_t self = -1;
-        const float *qsrc;
-        if (q_ptr) qsrc = q_ptr + qi * d;
-        else { self = q_idx ? q_idx[qi] : q0 + qi; qsrc = X + self * d; }
-        for (int e = lane; e < d; e += 32) qs[e] = qsrc[e];
-        __syncwarp();
-        const float qq = metric == GORSE_B200_METRIC_COSINE ? dot_any(qs, qs, d) : 0.f;
-        int len = 0;
-        const int64_t cidx = cand_by_slot ? row_slot : qi;
-        const int32_t *cl = cand ? cand + cidx * cand_stride : nullptr;
-        const int64_t begin = cand ? 0 : (int64_t)seg * seg_len;
-        const int64_t total = cand ? (cand_count ? (int64_t)min(cand_count[cidx], cand_stride) : (int64_t)cand_stride) : min(N, begin + seg_len);
-        if (d % 16 == 0 && d <= 256) {
-            const int chunks = d / 16;
-            float4 qreg[16];
+    for (int e = threadIdx.x; e < d; e += NT) qs[e] = q[e];
+    __syncthreads();
+    return metric == GORSE_B200_METRIC_COSINE ? dot_any(qs, qs, d) : 0.f;
+}
+
+// ---- stage 2: one CTA per row of a class (rows[i] = chunk-local row; candidate list i belongs to it) ------------------------
+__global__ void __launch_bounds__(WIN_THREADS)
+recall_window_kernel(const int32_t *cand_col, const float *cand_val, const int32_t *cand_cnt, const float *theta, const float *eps,
+                     const int32_t *perm, const uint8_t *allow, const float *X, int d, int metric, const int64_t *rows, int64_t n_rows,
+                     RowInfo R)
+{
+    constexpr int NT = WIN_THREADS;
+    extern __shared__ __align__(16) uint8_t sm[];
+    uint64_t *s_key = reinterpret_cast<uint64_t *>(sm);                     // [SORT_CAP] window, sort keys
+    int32_t *g_slot = reinterpret_cast<int32_t *>(s_key + SORT_CAP);       // [CAP] candidates: slot
+    uint32_t *g_key = reinterpret_cast<uint32_t *>(g_slot + mma::CAP);     // [CAP] candidates: approximate key (0 = dropped)
+    float *s_val = reinterpret_cast<float *>(g_key);                       // [SORT_CAP] window, exact scores (g_key is read by then)
+    int *hist = reinterpret_cast<int *>(g_key + mma::CAP);                 // [256]
+    int *s_warp = hist + 256;                                              // [32]
+    int *s_bc = s_warp + 32;                                               // [4]
+    float *qs = reinterpret_cast<float *>(s_bc + 4);                       // [d]
+    for (int64_t i = blockIdx.x; i < n_rows; i += gridDim.x) {
+        const int64_t r = rows[i];
+        const int k = R.k[r];
+        const int64_t self = R.self ? R.self[r] : -1;
+        // every column with approximate score >= max over the parts' thresholds was pushed by one of the parts
+        int np[mma::PARTS], n = 0;
+        float th = -INFINITY;
+        bool bad = !(eps[i] == eps[i]);
 #pragma unroll
-            for (int c = 0; c < 16; c++)
-                if (c < chunks) qreg[c] = *reinterpret_cast<const float4 *>(qs + 16 * c + 4 * lane4);
-            for (int64_t base = begin; base < total; base += 8) {
-                int64_t t = base + quad;
-                int64_t v = -1;
-                if (t < total) v = cl ? (int64_t)cl[t] : t;
-                bool valid = v >= 0 && v != self && (allow == nullptr || allow[v] != 0);
-                float dv = 0.f;
-                if (valid) dv = quad_dist(qreg, X + v * d, chunks, lane4, qmask, metric, qq);
-                // lane 0 consumes the 8 quads' results in index order
-                for (int s = 0; s < 8; s++) {
-                    float dd = __shfl_sync(0xffffffffu, dv, 4 * s);
-                    int64_t vv = __shfl_sync(0xffffffffu, v, 4 * s);
-                    int ok = __shfl_sync(0xffffffffu, (int)valid, 4 * s);
-                    if (ok) {
-                        if (dd != dd) { if (lane == 0) *nan_flag = 1; }
-                        else if (k <= 128) list_insert_warp(ld, li, len, k, dd, (int32_t)vv, lane);
-                        else if (lane == 0) list_insert(ld, li, len, k, dd, (int32_t)vv);
-                    }
-                }
-                __syncwarp();
+        for (int p = 0; p < mma::PARTS; p++) {
+            const int raw = cand_cnt[mma::PARTS * i + p];
+            bad |= raw > mma::PART_CAP;
+            np[p] = min(raw, mma::PART_CAP);
+            n += np[p];
+            th = fmaxf(th, theta[mma::PARTS * i + p]);
+        }
+        if (!(th == th)) bad = true;
+        int have = 0;
+        for (int e = threadIdx.x; e < n; e += NT) {
+            int p = 0, rr = e;   // entry e of the concatenated part lists
+#pragma unroll
+            for (int q = 0; q + 1 < mma::PARTS; q++)
+                if (p == q && rr >= np[q]) { rr -= np[q]; p++; }
+            const int64_t src = i * mma::CAP + p * mma::PART_CAP + rr;
+            const int32_t slot = perm[cand_col[src]];
+            const uint32_t key = slot != self && (!allow || allow[slot]) ? rank_key(cand_val[src]) : 0u;
+            g_slot[e] = slot;
+            g_key[e] = key;
+            have += key != 0u;
+        }
+        have = block_sum<NT>(have, s_warp);   // (synchronises: g_* are complete)
+        if (have < k) bad = true;
+        float kth = 0.f;
+        if (!bad) {
+            int ties;
+            kth = key_float(block_select<NT>(n, k, [&](int64_t e) { return g_key[e]; }, hist, s_bc, &ties));
+            // at least k allowed candidates clear theta + 2 eps: every allowed column outside the list ranks below them
+            if (!(kth >= th + 2.f * eps[i])) bad = true;
+        }
+        if (bad) {
+            if (threadIdx.x == 0) { R.exact[R.n_routed + atomicAdd(&R.flags[2], 1)] = r; atomicAdd(&R.flags[1], 1); }
+            continue;
+        }
+        // the window: candidates whose exact score can reach the k-th best (approximate >= kth - 2 eps)
+        const uint32_t lim = rank_key(kth - 2.f * eps[i]);
+        if (threadIdx.x == 0) s_bc[2] = 0;
+        __syncthreads();
+        for (int e0 = 0; e0 < n; e0 += NT) {   // a warp takes its places in the window with one atomic
+            const int e = e0 + threadIdx.x, lane = threadIdx.x & 31;
+            const bool in = e < n && g_key[e] != 0u && g_key[e] >= lim;
+            const unsigned b = __ballot_sync(0xffffffffu, in);
+            int at = 0;
+            if (lane == 0 && b) at = atomicAdd(&s_bc[2], __popc(b));
+            at = __shfl_sync(0xffffffffu, at, 0);
+            if (in) s_key[at + __popc(b & ((1u << lane) - 1))] = (uint64_t)g_slot[e];
+        }
+        const float qq = load_query<NT>(R.q + r * d, d, metric, qs);   // (synchronises)
+        const int w = s_bc[2];
+        block_score<NT>(X, d, metric, qs, qq, w, [&](int64_t j) { return (int64_t)s_key[j]; }, [&](int64_t j, float s, bool) {
+            if (s != s) R.flags[0] = 1;
+            s_val[j] = s;
+        });
+        __syncthreads();
+        const int p2 = pow2_at_least(w);
+        for (int j = threadIdx.x; j < p2; j += NT)
+            s_key[j] = j < w ? sort_key(rank_key(s_val[j]), (int64_t)s_key[j]) : ~0ull;
+        __syncthreads();
+        block_sort<NT>(s_key, s_val, p2);
+        int written = 0;
+        block_emit<NT>(s_key, s_val, min(k, w), R.ex + R.ex_off[r], R.ex_off[r + 1] - R.ex_off[r], R.slots + R.out_off[r],
+                       R.scores + R.out_off[r], written, s_warp);
+        if (threadIdx.x == 0) R.count[r] = written;
+        __syncthreads();
+    }
+}
+
+// ---- exact path: one CTA per row of R.exact; sc = this CTA's [N] score scratch ---------------------------------------------
+__global__ void __launch_bounds__(EXACT_THREADS)
+recall_exact_kernel(const float *X, int64_t N, int d, int metric, const uint8_t *allow, RowInfo R, float *scratch)
+{
+    constexpr int NT = EXACT_THREADS;
+    extern __shared__ __align__(16) uint8_t sm[];
+    uint64_t *s_key = reinterpret_cast<uint64_t *>(sm);                // [SORT_CAP]
+    float *s_val = reinterpret_cast<float *>(s_key + SORT_CAP);       // [SORT_CAP]
+    int *hist = reinterpret_cast<int *>(s_val + SORT_CAP);            // [256]
+    int *s_warp = hist + 256;                                         // [32]
+    int *s_bc = s_warp + 32;                                          // [4]
+    float *qs = reinterpret_cast<float *>(s_bc + 4);                  // [d]
+    float *sc = scratch + (int64_t)blockIdx.x * N;
+    const float none = __int_as_float(0x7fffffff);                    // NaN: rank_key 0
+    const int64_t n_rows = R.n_routed + R.flags[2];
+    for (int64_t i = blockIdx.x; i < n_rows; i += gridDim.x) {
+        const int64_t r = R.exact[i];
+        const int64_t self = R.self ? R.self[r] : -1;
+        const float qq = load_query<NT>(R.q + r * d, d, metric, qs);
+        int have = 0;
+        block_score<NT>(X, d, metric, qs, qq, N, [&](int64_t j) { return j != self && (!allow || allow[j]) ? j : (int64_t)-1; }, [&](int64_t j, float s, bool valid) {
+            if (valid && s != s) R.flags[0] = 1;
+            sc[j] = valid ? s : none;
+            have += valid && s == s;
+        });
+        have = block_sum<NT>(have, s_warp);   // (synchronises: sc is complete)
+        const int K = min(R.k[r], have);
+        int written = 0;
+        // rounds of at most SORT_CAP: select the round's last key, gather, sort, emit, then retire the emitted entries
+        for (int emitted = 0; emitted < K;) {
+            const int m = min(SORT_CAP, K - emitted);
+            int ties;
+            const uint32_t t = block_select<NT>(N, m, [&](int64_t j) { return rank_key(sc[j]); }, hist, s_bc, &ties);
+            if (threadIdx.x == 0) s_bc[2] = 0;
+            int eq_taken = 0;   // entries equal to t go in slot order: the lowest slots win the tie
+            __syncthreads();
+            for (int64_t base = 0; base < N; base += NT) {
+                const int64_t j = base + threadIdx.x;
+                const uint32_t key = j < N ? rank_key(sc[j]) : 0u;
+                int n_eq;
+                const int er = block_rank<NT>(key == t, s_warp, n_eq);
+                int pos = -1;
+                if (key > t) pos = atomicAdd(&s_bc[2], 1);
+                else if (key == t && eq_taken + er < ties) pos = m - ties + eq_taken + er;
+                if (pos >= 0) { s_key[pos] = sort_key(key, j); s_val[pos] = sc[j]; }
+                eq_taken += n_eq;
             }
+            const int p2 = pow2_at_least(m);
+            for (int j = m + threadIdx.x; j < p2; j += NT) s_key[j] = ~0ull;
+            __syncthreads();
+            block_sort<NT>(s_key, s_val, p2);
+            block_emit<NT>(s_key, s_val, m, R.ex + R.ex_off[r], R.ex_off[r + 1] - R.ex_off[r], R.slots + R.out_off[r], R.scores + R.out_off[r],
+                           written, s_warp);
+            for (int j = threadIdx.x; j < m; j += NT) sc[(uint32_t)s_key[j]] = none;
+            __syncthreads();
+            emitted += m;
+        }
+        if (threadIdx.x == 0) R.count[r] = written;
+        __syncthreads();
+    }
+}
+
+// the Table rows of one chunk's rows [0, rows), at t_slot / t_val + r * n and t_cnt[r]
+template <int NT>
+__global__ void __launch_bounds__(NT)
+table_kernel(const int64_t *slots, const float *scores, const int32_t *count, const int64_t *out_off, int64_t rows, int n, bool negate,
+             bool positive, int32_t *t_slot, float *t_val, int32_t *t_cnt)
+{
+    __shared__ int s_warp[32];
+    for (int64_t r = blockIdx.x; r < rows; r += gridDim.x) {
+        const int c = count[r];
+        const int64_t src = out_off[r], dst = r * n;
+        int kept = 0;
+        for (int base = 0; base < c; base += NT) {
+            const int j = base + threadIdx.x;
+            const float v = j < c ? (negate ? -scores[src + j] : scores[src + j]) : 0.f;
+            const bool keep = j < c && (!positive || v > 0.f);
+            int total;
+            const int at = kept + block_rank<NT>(keep, s_warp, total);
+            if (keep) { t_slot[dst + at] = (int32_t)slots[src + j]; t_val[dst + at] = v; }
+            kept += total;
+        }
+        for (int j = kept + threadIdx.x; j < n; j += NT) { t_slot[dst + j] = -1; t_val[dst + j] = 0.f; }
+        if (threadIdx.x == 0) t_cnt[r] = kept;
+    }
+}
+
+// slots[r] = q0 + r: the stored rows of a range
+__global__ void range_slots_kernel(int64_t *slots, int64_t rows, int64_t q0)
+{
+    const int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (r < rows) slots[r] = q0 + r;
+}
+
+// q[r] = X[slots[r]]: the query rows of stored vectors, one CTA per row
+__global__ void recall_gather_kernel(const float *X, int d, const int64_t *slots, int64_t rows, float *q)
+{
+    for (int64_t r = blockIdx.x; r < rows; r += gridDim.x)
+        for (int e = threadIdx.x; e < d; e += blockDim.x) q[r * d + e] = X[slots[r] * d + e];
+}
+
+// the row tables of a chunk without exclusions: k = n, answers at q * n, one class in row order
+__global__ void uniform_rows_kernel(int64_t rows, int64_t q0, int n, int32_t *k, int64_t *ex_off, int64_t *out_off, int64_t *order)
+{
+    const int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (r <= rows) ex_off[r] = 0;
+    if (r < rows) { k[r] = n; out_off[r] = (q0 + r) * n; order[r] = r; }
+}
+
+size_t window_smem(int d) { return (size_t)SORT_CAP * 8 + (size_t)mma::CAP * 8 + (256 + 32 + 4) * 4 + (size_t)d * 4; }
+size_t exact_smem(int d) { return (size_t)SORT_CAP * 12 + (256 + 32 + 4) * 4 + (size_t)d * 4; }
+
+
+int32_t recall_rows(gorse_b200_index *ix, const uint8_t *allow, int64_t nq, const float *q_host, const int64_t *d_qslots, int32_t n,
+                    const int64_t *excl_off, const int64_t *ex, const int64_t *ex_off, const Table *table, int64_t *slots_out,
+                    float *scores_out, int32_t *count_out, int64_t *exact_rows_out)
+{
+    gorse_b200_ctx *c = ix->ctx;
+    RecallWork &W = ix->recall;
+    const int d = ix->d;
+    auto out_at = [&](int64_t q) { return q * (int64_t)n + (excl_off ? excl_off[q] : 0); };
+    const int64_t N = ix->n, total_out = out_at(nq);
+    const bool tensor = mma_path_eligible(ix, nq);
+    const int64_t cq = std::min<int64_t>(nq, (int64_t)c->sm_count * mma::GROUP_ROWS * 8);
+    // exact scratch: one [N] score row per CTA, at most 512 MB
+    const int exact_grid = (int)std::max<int64_t>(1, std::min<int64_t>({(int64_t)c->sm_count * 2, cq, (512ll << 20) / (4 * N)}));
+    int32_t st = GORSE_B200_OK;
+    auto done = [&](int32_t s) {
+        cudaStreamSynchronize(c->stream);
+        cudaStreamSynchronize(c->copy_stream);
+        return s;
+    };
+    if ((st = grow(W.q, (size_t)cq * d)) || (st = grow(W.k, (size_t)cq)) || (st = grow(W.ex_off, (size_t)cq + 1)) || (st = grow(W.out_off, (size_t)cq)) ||
+        (st = grow(W.rows, 2 * (size_t)cq)) || (st = grow(W.count, (size_t)nq)) || (st = grow(W.flags, 3)) ||
+        (st = grow(W.slots, (size_t)std::max<int64_t>(total_out, 1))) || (st = grow(W.scores, (size_t)std::max<int64_t>(total_out, 1))) ||
+        (st = grow(W.scratch, (size_t)exact_grid * N)) || (st = grow(W.ex, (size_t)std::max<int64_t>(excl_off ? ex_off[nq] : 0, 1))))
+        return done(st);
+    if (tensor && (st = mma_reserve(ix, cq))) return done(st);
+    cudaError_t e = cudaFuncSetAttribute(recall_window_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)window_smem(d));
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(recall_exact_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)exact_smem(d));
+    if (e == cudaSuccess) e = cudaMemsetAsync(W.flags.p, 0, 2 * sizeof(int), c->stream);
+    if (e != cudaSuccess) { set_error("top-k: %s", cudaGetErrorString(e)); return done(GORSE_B200_ERR_CUDA); }
+    int64_t host_exact = 0;
+    size_t sweeps = 0;   // event pairs ix->ev[2 s], [2 s + 1] around sweep s
+    std::vector<int32_t> &h_k = W.h_k;
+    std::vector<int64_t> &h_exoff = W.h_exoff, &h_outoff = W.h_outoff, &h_rows = W.h_rows;
+    std::vector<int8_t> &cls = W.h_cls;
+    auto class_of = [&](int32_t k) {   // class N_CLASSES = the exact kernel
+        int8_t cl = N_CLASSES;
+        if (tensor)
+            for (int8_t t = N_CLASSES - 1; t >= 0; t--)
+                if (k <= CLASS_K[t]) cl = t;
+        return cl;
+    };
+    for (int64_t q0 = 0; q0 < nq; q0 += cq) {
+        const int64_t rows = std::min(cq, nq - q0);
+        if (!q_host) {   // stored vectors: gathered from the collection in place of the upload
+            recall_gather_kernel<<<(unsigned)std::min<int64_t>(rows, (int64_t)c->sm_count * 16), 128, 0, c->stream>>>(ix->X.p, d, d_qslots + q0, rows, W.q.p);
+            c->launches++;
+        }
+        if ((q_host && (e = cudaMemcpyAsync(W.q.p, q_host + q0 * d, sizeof(float) * rows * d, cudaMemcpyHostToDevice, c->stream)) != cudaSuccess) ||
+            (e = cudaMemsetAsync(W.flags.p + 2, 0, sizeof(int), c->stream)) != cudaSuccess) {
+            set_error("top-k upload: %s", cudaGetErrorString(e));
+            return done(GORSE_B200_ERR_CUDA);
+        }
+        // rows grouped by class: class t holds rows W.rows[cls_begin[t] .. cls_begin[t + 1])
+        int64_t cls_begin[N_CLASSES + 2] = {0};
+        int cls_k[N_CLASSES] = {0};   // the largest k_q of each class
+        if (!excl_off) {   // every row in one class, in row order; the tables are written on the device
+            const int8_t t = class_of(n);
+            for (int u = t + 1; u <= N_CLASSES + 1; u++) cls_begin[u] = rows;
+            if (t < N_CLASSES) cls_k[t] = n;
+            uniform_rows_kernel<<<div_up(rows + 1, 256), 256, 0, c->stream>>>(rows, q0, n, W.k.p, W.ex_off.p, W.out_off.p, W.rows.p);
+            c->launches++;
         } else {
-            for (int64_t base = begin; base < total; base += 32) {
-                int64_t t = base + lane;
-                int64_t v = -1;
-                if (t < total) v = cl ? (int64_t)cl[t] : t;
-                bool valid = v >= 0 && v != self && (allow == nullptr || allow[v] != 0);
-                float dv = 0.f;
-                if (valid) dv = dist_any(qs, X + v * d, d, metric, qq);
-                for (int s = 0; s < 32; s++) {
-                    float dd = __shfl_sync(0xffffffffu, dv, s);
-                    int64_t vv = __shfl_sync(0xffffffffu, v, s);
-                    int ok = __shfl_sync(0xffffffffu, (int)valid, s);
-                    if (ok) {
-                        if (dd != dd) { if (lane == 0) *nan_flag = 1; }
-                        else if (k <= 128) list_insert_warp(ld, li, len, k, dd, (int32_t)vv, lane);
-                        else if (lane == 0) list_insert(ld, li, len, k, dd, (int32_t)vv);
-                    }
-                }
-                __syncwarp();
+            h_k.resize(rows); h_exoff.resize(rows + 1); h_outoff.resize(rows); h_rows.resize(rows); cls.resize(rows);
+            for (int64_t r = 0; r < rows; r++) {
+                const int64_t q = q0 + r;
+                h_k[r] = n + (int32_t)(excl_off[q + 1] - excl_off[q]);
+                h_exoff[r] = ex_off[q] - ex_off[q0];
+                h_outoff[r] = out_at(q);
+                cls[r] = class_of(h_k[r]);
+                cls_begin[cls[r] + 1]++;
+                if (cls[r] < N_CLASSES) cls_k[cls[r]] = std::max(cls_k[cls[r]], h_k[r]);
+            }
+            h_exoff[rows] = ex_off[q0 + rows] - ex_off[q0];
+            for (int t = 0; t <= N_CLASSES; t++) cls_begin[t + 1] += cls_begin[t];
+            int64_t fill[N_CLASSES + 1];
+            std::copy(cls_begin, cls_begin + N_CLASSES + 1, fill);
+            for (int64_t r = 0; r < rows; r++) h_rows[fill[cls[r]]++] = r;
+            const int64_t n_ex = h_exoff[rows];
+            if ((e = cudaMemcpyAsync(W.k.p, h_k.data(), sizeof(int32_t) * rows, cudaMemcpyHostToDevice, c->stream)) != cudaSuccess ||
+                (e = cudaMemcpyAsync(W.ex_off.p, h_exoff.data(), sizeof(int64_t) * (rows + 1), cudaMemcpyHostToDevice, c->stream)) != cudaSuccess ||
+                (e = cudaMemcpyAsync(W.out_off.p, h_outoff.data(), sizeof(int64_t) * rows, cudaMemcpyHostToDevice, c->stream)) != cudaSuccess ||
+                (e = cudaMemcpyAsync(W.rows.p, h_rows.data(), sizeof(int64_t) * rows, cudaMemcpyHostToDevice, c->stream)) != cudaSuccess ||
+                (n_ex && (e = cudaMemcpyAsync(W.ex.p, ex + ex_off[q0], sizeof(int64_t) * n_ex, cudaMemcpyHostToDevice, c->stream)) != cudaSuccess)) {
+                set_error("top-k upload: %s", cudaGetErrorString(e));
+                return done(GORSE_B200_ERR_CUDA);
             }
         }
-        len = __shfl_sync(0xffffffffu, len, 0);
-        __syncwarp();
-        // prune0 keeps score > 0 while popping (bruteforce.go:58,78); the list is ascending so survivors are a suffix
-        int first = 0;
-        if (prune0) {
-            while (first < len && !(ld[first] > 0.f)) first++;
+        host_exact += cls_begin[N_CLASSES + 1] - cls_begin[N_CLASSES];
+        RowInfo R;
+        R.q = W.q.p; R.k = W.k.p; R.ex_off = W.ex_off.p; R.ex = W.ex.p; R.out_off = W.out_off.p;
+        R.exact = W.rows.p + cls_begin[N_CLASSES]; R.n_routed = cls_begin[N_CLASSES + 1] - cls_begin[N_CLASSES];
+        R.self = q_host ? nullptr : d_qslots + q0;
+        R.slots = W.slots.p; R.scores = W.scores.p; R.count = W.count.p + q0; R.flags = W.flags.p;
+        for (int t = 0; t < N_CLASSES; t++) {
+            const int64_t nr = cls_begin[t + 1] - cls_begin[t];
+            if (nr == 0) continue;
+            // the sample aims at 4 k columns per row, at most CAP / 2 so that a row's lists rarely overflow (Gamma(R_TOP) spread)
+            const int m_tiles = mma_sample_tiles(ix, std::min(4.0 * cls_k[t], mma::CAP / 2.0));
+            if (ix->ev.size() < 2 * sweeps + 2) {
+                ix->ev.resize(2 * sweeps + 2, nullptr);
+                if ((e = cudaEventCreate(&ix->ev[2 * sweeps])) != cudaSuccess || (e = cudaEventCreate(&ix->ev[2 * sweeps + 1])) != cudaSuccess) {
+                    set_error("top-k events: %s", cudaGetErrorString(e));
+                    return done(GORSE_B200_ERR_CUDA);
+                }
+            }
+            if ((st = mma_sweep(ix, W.q.p, nullptr, W.rows.p + cls_begin[t], 0, nr, m_tiles, ix->ev[2 * sweeps], ix->ev[2 * sweeps + 1])))
+                return done(st);
+            sweeps++;
+            ix->stage1_flop += 2.0 * (double)nr * (double)N * (double)d;
+            recall_window_kernel<<<(unsigned)std::min<int64_t>(nr, (int64_t)c->sm_count * 16), WIN_THREADS, window_smem(d), c->stream>>>(
+                ix->w_ccol.p, ix->w_cval.p, ix->w_ccnt.p, ix->w_theta.p, ix->w_eps.p, ix->perm.p, allow, ix->X.p, d, ix->metric,
+                W.rows.p + cls_begin[t], nr, R);
+            c->launches++;
         }
-        int cnt = len - first;
-        for (int e = lane; e < k; e += 32) {
-            bool has = e < cnt;
-            out_idx[oq * k + e] = has ? li[first + e] : -1;
-            out_dist[oq * k + e] = has ? ld[first + e] : 0.f;
+        recall_exact_kernel<<<(unsigned)std::min<int64_t>(rows, exact_grid), EXACT_THREADS, exact_smem(d), c->stream>>>(
+            ix->X.p, N, d, ix->metric, allow, R, W.scratch.p);
+        c->launches++;
+        const int64_t t0 = q0 * n;
+        if (table) {
+            table_kernel<128><<<(unsigned)std::min<int64_t>(rows, (int64_t)c->sm_count * 16), 128, 0, c->stream>>>(
+                W.slots.p, W.scores.p, R.count, W.out_off.p, rows, n, table->negate, table->positive, table->slot + t0, table->val + t0,
+                table->cnt + q0);
+            c->launches++;
         }
-        if (lane == 0) out_count[oq] = cnt;
-        __syncwarp();
+        if ((e = cudaGetLastError()) != cudaSuccess) { set_error("top-k: %s", cudaGetErrorString(e)); return done(GORSE_B200_ERR_CUDA); }
+        const bool h_table = table && table->h_slot;
+        if (!slots_out && !h_table) continue;   // the caller reads the answers on the device
+        // this chunk is final: download it on the copy stream while the next chunk computes
+        const int64_t o0 = out_at(q0), o1 = out_at(q0 + rows);
+        if ((e = cudaEventRecord(c->copy_ev, c->stream)) != cudaSuccess || (e = cudaStreamWaitEvent(c->copy_stream, c->copy_ev, 0)) != cudaSuccess ||
+            (slots_out &&
+             ((e = cudaMemcpyAsync(count_out + q0, W.count.p + q0, sizeof(int32_t) * rows, cudaMemcpyDeviceToHost, c->copy_stream)) != cudaSuccess ||
+              (o1 > o0 && ((e = cudaMemcpyAsync(slots_out + o0, W.slots.p + o0, sizeof(int64_t) * (o1 - o0), cudaMemcpyDeviceToHost, c->copy_stream)) != cudaSuccess ||
+                           (e = cudaMemcpyAsync(scores_out + o0, W.scores.p + o0, sizeof(float) * (o1 - o0), cudaMemcpyDeviceToHost, c->copy_stream)) != cudaSuccess)))) ||
+            (h_table &&
+             ((e = cudaMemcpyAsync(table->h_slot + t0, table->slot + t0, sizeof(int32_t) * rows * n, cudaMemcpyDeviceToHost, c->copy_stream)) != cudaSuccess ||
+              (e = cudaMemcpyAsync(table->h_val + t0, table->val + t0, sizeof(float) * rows * n, cudaMemcpyDeviceToHost, c->copy_stream)) != cudaSuccess ||
+              (e = cudaMemcpyAsync(table->h_cnt + q0, table->cnt + q0, sizeof(int32_t) * rows, cudaMemcpyDeviceToHost, c->copy_stream)) != cudaSuccess))) {
+            set_error("top-k download: %s", cudaGetErrorString(e));
+            return done(GORSE_B200_ERR_CUDA);
+        }
     }
-}
-
-int32_t launch_exact(gorse_b200_index *ix, const float *d_q, const int64_t *d_qidx, int64_t q0, int64_t nq, int k,
-                     const int32_t *d_cand, const int32_t *d_cand_count, int cand_stride, const int32_t *row_list,
-                     int32_t *d_idx, float *d_dist, int32_t *d_count, int prune0, int *d_nan)
-{
-    gorse_b200_ctx *c = ix->ctx;
-    const int warps = 4;
-    size_t sm = (size_t)warps * (2 * (size_t)k * 4 + (size_t)ix->d * 4);
-    if (sm > 200 * 1024) { set_error("k = %d with dim = %d needs %zu bytes of shared memory per CTA", k, ix->d, sm); return GORSE_B200_ERR_UNSUPPORTED; }
-    GB_CUDA(cudaFuncSetAttribute(topk_exact_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-    int grid = (int)std::max<int64_t>(1, std::min<int64_t>((nq + warps - 1) / warps, (int64_t)c->sm_count * 8));
-    topk_exact_kernel<<<grid, 32 * warps, sm, c->stream>>>(ix->X.p, ix->n, ix->d, ix->metric, d_q, d_qidx, q0, nq, k, d_cand,
-                                                         d_cand_count, cand_stride, row_list, d_idx, d_dist, d_count, prune0, d_nan, 1, ix->n, 0, nullptr);
-    GB_LAUNCHED(c);
-    return GORSE_B200_OK;
-}
-
-// A few rows, each against ALL vectors (the tensor path's certified-fallback): split every row's scan into segments
-// handled by different warps (partial top-k per segment, no prune0 yet), then merge the partial lists exactly.
-int32_t launch_exact_split(gorse_b200_index *ix, const float *d_q, const int64_t *d_qidx, int64_t q0, int32_t n_rows, int k,
-                           const int32_t *row_list, int32_t *d_idx, float *d_dist, int32_t *d_count, int prune0, int *d_nan,
-                           const uint8_t *allow)
-{
-    gorse_b200_ctx *c = ix->ctx;
-    const int warps = 4;
-    size_t sm = (size_t)warps * (2 * (size_t)k * 4 + (size_t)ix->d * 4);
-    // (round 2 tried finer segments to fill the machine with a handful of rows: the scan got faster but the merge, one
-    // warp re-scoring n_seg * k candidates per row, took 4x longer than what was saved)
-    const int64_t seg_len = 16384;
-    const int n_seg = (int)((ix->n + seg_len - 1) / seg_len);
-    DevBuf<int32_t> p_idx, p_cnt;
-    DevBuf<float> p_dist;
-    int32_t st;
-    auto done = [&](int32_t s) { cudaStreamSynchronize(c->stream); p_idx.free(); p_cnt.free(); p_dist.free(); return s; };
-    const int64_t slots = (int64_t)n_rows * n_seg;
-    if ((st = p_idx.alloc((size_t)slots * k)) || (st = p_dist.alloc((size_t)slots * k)) || (st = p_cnt.alloc(slots))) return done(st);
-    GB_CUDA(cudaFuncSetAttribute(topk_exact_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-    int grid = (int)std::max<int64_t>(1, std::min<int64_t>((slots + warps - 1) / warps, (int64_t)c->sm_count * 16));
-    topk_exact_kernel<<<grid, 32 * warps, sm, c->stream>>>(ix->X.p, ix->n, ix->d, ix->metric, d_q, d_qidx, q0, slots, k, nullptr, nullptr, 0,
-                                                         row_list, p_idx.p, p_dist.p, p_cnt.p, 0, d_nan, n_seg, seg_len, 0, allow);
-    c->launches++;
-    grid = (int)std::max<int64_t>(1, std::min<int64_t>((n_rows + warps - 1) / warps, (int64_t)c->sm_count * 8));
-    topk_exact_kernel<<<grid, 32 * warps, sm, c->stream>>>(ix->X.p, ix->n, ix->d, ix->metric, d_q, d_qidx, q0, n_rows, k, p_idx.p, nullptr,
-                                                         n_seg * k, row_list, d_idx, d_dist, d_count, prune0, d_nan, 1, ix->n, 1, nullptr);
-    c->launches++;
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) { set_error("exact fallback: %s", cudaGetErrorString(e)); return done(GORSE_B200_ERR_CUDA); }
+    int flags[2] = {0, 0};
+    if ((e = cudaMemcpyAsync(flags, W.flags.p, sizeof(flags), cudaMemcpyDeviceToHost, c->stream)) != cudaSuccess ||
+        (e = cudaStreamSynchronize(c->stream)) != cudaSuccess || (e = cudaStreamSynchronize(c->copy_stream)) != cudaSuccess) {
+        set_error("top-k: %s", cudaGetErrorString(e));
+        return done(GORSE_B200_ERR_CUDA);
+    }
+    for (size_t s = 0; s < sweeps; s++) {
+        float ms = 0.f;
+        if (cudaEventElapsedTime(&ms, ix->ev[2 * s], ix->ev[2 * s + 1]) == cudaSuccess) ix->stage1_ms += ms;
+    }
+    ix->last_fallback_rows += flags[1];
+    if (flags[0]) { set_error("NaN distance"); return done(GORSE_B200_ERR_ARG); }
+    if (exact_rows_out) *exact_rows_out = host_exact + flags[1];
     return done(GORSE_B200_OK);
 }
 
-// run a search whose queries are already described by (d_q | d_qidx | q0); copies results to the host
+}  // namespace recall
+
+// the index's searches: rows from host vectors, a host list of stored rows, or the stored rows [q0, q0 + nq); the distances and
+// int32 ids go through the pipeline's table (prune0 keeps distance > 0, bruteforce.go:58,78) into the host buffers
 static int32_t search_common(gorse_b200_index *ix, const float *h_queries, const int64_t *h_qidx, int64_t q0, int64_t nq,
                              int32_t k, int32_t prune0, int32_t *idx_out, float *dist_out, int32_t *count_out)
 {
@@ -226,50 +492,24 @@ static int32_t search_common(gorse_b200_index *ix, const float *h_queries, const
     GB_CHECK_ARG(idx_out != nullptr && dist_out != nullptr, "NULL output");
     ScopedDevice sd(ix->ctx->device);
     gorse_b200_ctx *c = ix->ctx;
-    DevBuf<float> d_q;
     DevBuf<int64_t> d_qidx;
-    DevBuf<int> d_nan;
-    DevBuf<int32_t> &d_idx = ix->r_idx, &d_count = ix->r_count;   // grow-only staging kept in the index
-    DevBuf<float> &d_dist = ix->r_dist;
     int32_t st = GORSE_B200_OK;
-    auto done = [&](int32_t s) {
-        cudaStreamSynchronize(c->stream);
-        cudaStreamSynchronize(c->copy_stream);
-        d_q.free(); d_qidx.free(); d_nan.free();
-        return s;
-    };
-    if ((d_idx.n < (size_t)nq * k && (st = d_idx.alloc((size_t)nq * k))) || (d_dist.n < (size_t)nq * k && (st = d_dist.alloc((size_t)nq * k))) ||
-        (d_count.n < (size_t)nq && (st = d_count.alloc(nq))) || (st = d_nan.alloc(1)))
+    auto done = [&](int32_t s) { cudaStreamSynchronize(c->stream); d_qidx.free(); return s; };
+    if ((st = recall::grow(ix->r_idx, (size_t)nq * k)) || (st = recall::grow(ix->r_dist, (size_t)nq * k)) || (st = recall::grow(ix->r_count, (size_t)nq)))
         return done(st);
-    cudaError_t e = cudaMemsetAsync(d_nan.p, 0, sizeof(int), c->stream);
-    if (h_queries) {
-        if ((st = d_q.alloc((size_t)nq * ix->d))) return done(st);
-        if (e == cudaSuccess) e = cudaMemcpyAsync(d_q.p, h_queries, sizeof(float) * nq * ix->d, cudaMemcpyHostToDevice, c->stream);
-    } else if (h_qidx) {
+    if (!h_queries) {   // stored rows: a device slot list
         if ((st = d_qidx.alloc(nq))) return done(st);
-        if (e == cudaSuccess) e = cudaMemcpyAsync(d_qidx.p, h_qidx, sizeof(int64_t) * nq, cudaMemcpyHostToDevice, c->stream);
+        cudaError_t e = cudaSuccess;
+        if (h_qidx) e = cudaMemcpyAsync(d_qidx.p, h_qidx, sizeof(int64_t) * nq, cudaMemcpyHostToDevice, c->stream);
+        else {
+            recall::range_slots_kernel<<<div_up(nq, 256), 256, 0, c->stream>>>(d_qidx.p, nq, q0);
+            c->launches++;
+        }
+        if (e == cudaSuccess) e = cudaGetLastError();
+        if (e != cudaSuccess) { set_error("search upload: %s", cudaGetErrorString(e)); return done(GORSE_B200_ERR_CUDA); }
     }
-    if (e != cudaSuccess) { set_error("search upload: %s", cudaGetErrorString(e)); return done(GORSE_B200_ERR_CUDA); }
-    // large all-pairs / batched problems go through the tensor-core candidate generator + exact re-rank
-    bool downloaded = false;
-    if (mma_path_eligible(ix, nq, k)) {
-        st = search_mma(ix, d_q.p, d_qidx.p, q0, nq, k, prune0, d_idx.p, d_dist.p, d_count.p, d_nan.p, idx_out, dist_out, count_out);
-        downloaded = true;
-    } else {
-        st = launch_exact(ix, d_q.p, d_qidx.p, q0, nq, k, nullptr, nullptr, 0, nullptr, d_idx.p, d_dist.p, d_count.p, prune0, d_nan.p);
-    }
-    if (st) return done(st);
-    int h_nan = 0;
-    if ((!downloaded && ((e = cudaMemcpyAsync(idx_out, d_idx.p, sizeof(int32_t) * nq * k, cudaMemcpyDeviceToHost, c->stream)) != cudaSuccess ||
-                         (e = cudaMemcpyAsync(dist_out, d_dist.p, sizeof(float) * nq * k, cudaMemcpyDeviceToHost, c->stream)) != cudaSuccess ||
-                         (e = cudaMemcpyAsync(count_out, d_count.p, sizeof(int32_t) * nq, cudaMemcpyDeviceToHost, c->stream)) != cudaSuccess)) ||
-        (e = cudaMemcpyAsync(&h_nan, d_nan.p, sizeof(int), cudaMemcpyDeviceToHost, c->stream)) != cudaSuccess ||
-        (e = cudaStreamSynchronize(c->stream)) != cudaSuccess || (e = cudaStreamSynchronize(c->copy_stream)) != cudaSuccess) {
-        set_error("search: %s", cudaGetErrorString(e));
-        return done(GORSE_B200_ERR_CUDA);
-    }
-    if (h_nan) { set_error("NaN weight is forbidden");  /* the reference panics, common/heap/pq.go:82-83 */ return done(GORSE_B200_ERR_ARG); }
-    return done(GORSE_B200_OK);
+    const recall::Table table{ix->r_idx.p, ix->r_dist.p, ix->r_count.p, true, prune0 != 0, idx_out, dist_out, count_out};
+    return done(recall::recall_rows(ix, nullptr, nq, h_queries, d_qidx.p, k, nullptr, nullptr, nullptr, &table, nullptr, nullptr, nullptr, nullptr));
 }
 
 // make room for `need` vectors (amortised doubling); the caller holds ix->mu
@@ -319,9 +559,10 @@ int32_t gorse_b200_index_destroy(gorse_b200_index *ix)
     ix->Xb.free();
     ix->norm.free();
     ix->perm.free();
-    if (ix->ev0) { cudaEventDestroy(ix->ev0); cudaEventDestroy(ix->ev1); }
-    ix->w_qb.free(); ix->w_eps.free(); ix->w_cval.free(); ix->w_theta.free();
-    ix->w_ccol.free(); ix->w_ccnt.free(); ix->w_ids.free(); ix->w_idcnt.free(); ix->w_flag.free(); ix->w_flist.free();
+    for (cudaEvent_t e : ix->ev)
+        if (e) cudaEventDestroy(e);
+    ix->w_qb.free(); ix->w_eps.free(); ix->w_cval.free(); ix->w_theta.free(); ix->w_ccol.free(); ix->w_ccnt.free();
+    ix->recall.free();
     ix->r_idx.free(); ix->r_count.free(); ix->r_dist.free();
     delete ix;
     return GORSE_B200_OK;
@@ -390,8 +631,8 @@ int32_t gorse_b200_index_search_range(gorse_b200_index *ix, int64_t q0, int64_t 
 }
 
 // ---- measurement / test hooks (declared in include/gorse_b200.h) ----------------------------------------
-// since the last call: device time and algorithmic flop (2 * nq * N * d) of the stage-1 tensor-core kernel, and the rows
-// that fell back to the exact scan
+// since the last call: device time and algorithmic flop (2 * nq * N * d) of the stage-1 tensor-core kernels, and the rows
+// whose candidate set failed certification (the window kernel handed them to the exact kernel)
 int32_t gorse_b200_index_stats(gorse_b200_index *ix, double *stage1_ms, double *stage1_flop, int64_t *fallback_rows)
 {
     GB_CHECK_ARG(ix != nullptr, "ix is NULL");
@@ -405,7 +646,7 @@ int32_t gorse_b200_index_stats(gorse_b200_index *ix, double *stage1_ms, double *
 }
 
 // dense stage-1 (tensor core) scores of stored vectors [q0, q1) against all vectors, in ORIGINAL column order:
-// out[(q - q0) * n + x], and (eps_out != NULL) each row's error margin eps.  Small problems only (one chunk of rows).
+// out[(q - q0) * n + x], and (eps_out != NULL) each row's error margin eps.  Small problems only (one sweep of all rows).
 int32_t gorse_b200_index_stage1_scores(gorse_b200_index *ix, int64_t q0, int64_t q1, float *out, float *eps_out)
 {
     GB_CHECK_ARG(ix != nullptr && out != nullptr, "NULL argument");
@@ -414,16 +655,12 @@ int32_t gorse_b200_index_stage1_scores(gorse_b200_index *ix, int64_t q0, int64_t
     ScopedDevice sd(ix->ctx->device);
     gorse_b200_ctx *c = ix->ctx;
     const int64_t nq = q1 - q0, n_cols = (ix->n + 127) / 128 * 128;
-    DevBuf<float> dense, d_dist;
-    DevBuf<int32_t> d_idx, d_count;
-    DevBuf<int> d_nan;
+    DevBuf<float> dense;
     int32_t st;
-    auto done = [&](int32_t s) { cudaStreamSynchronize(c->stream); dense.free(); d_dist.free(); d_idx.free(); d_count.free(); d_nan.free(); ix->dbg_scores = nullptr; return s; };
-    if ((st = dense.alloc((size_t)nq * n_cols)) || (st = d_idx.alloc(nq)) || (st = d_dist.alloc(nq)) || (st = d_count.alloc(nq)) || (st = d_nan.alloc(1))) return done(st);
-    cudaMemsetAsync(d_nan.p, 0, sizeof(int), c->stream);
+    auto done = [&](int32_t s) { cudaStreamSynchronize(c->stream); dense.free(); ix->dbg_scores = nullptr; return s; };
+    if ((st = dense.alloc((size_t)nq * n_cols)) || (st = mma_reserve(ix, nq))) return done(st);
     ix->dbg_scores = dense.p;
-    if ((st = search_mma(ix, nullptr, nullptr, q0, nq, 1, 0, d_idx.p, d_dist.p, d_count.p, d_nan.p))) return done(st);
-    if (ix->w_cq < nq) { set_error("stage1_scores: %lld rows do not fit one sweep", (long long)nq); return done(GORSE_B200_ERR_ARG); }
+    if ((st = mma_sweep(ix, ix->X.p, nullptr, nullptr, q0, nq, mma_sample_tiles(ix, 4.0), nullptr, nullptr))) return done(st);
     std::vector<float> h((size_t)nq * n_cols);
     std::vector<int32_t> perm((size_t)ix->n);
     cudaError_t e = cudaMemcpyAsync(h.data(), dense.p, sizeof(float) * h.size(), cudaMemcpyDeviceToHost, c->stream);

@@ -1,9 +1,28 @@
-// topk.cuh -- brute-force index state shared by topk.cu (exact scan / re-rank) and topk_mma.cu (tensor-core stage 1).
+// topk.cuh -- brute-force index state shared by topk.cu (the top-k pipeline) and topk_mma.cu (tensor-core stage 1).
 #pragma once
 #include <cuda_bf16.h>
 
 #include "cf.cuh"
 #include "common.cuh"
+
+namespace gb {
+// grow-only work buffers of the top-k pipeline (recall::recall_rows), kept with the index, and the host side of a chunk's
+// row tables
+struct RecallWork {
+    DevBuf<float> q, scores, scratch;
+    DevBuf<int64_t> ex_off, ex, out_off, rows, slots;
+    DevBuf<int32_t> k, count, flags;
+    std::vector<int32_t> h_k;
+    std::vector<int64_t> h_exoff, h_outoff, h_rows;
+    std::vector<int8_t> h_cls;
+    void free()
+    {
+        q.free(); scores.free(); scratch.free();
+        ex_off.free(); ex.free(); out_off.free(); rows.free(); slots.free();
+        k.free(); count.free(); flags.free();
+    }
+};
+}  // namespace gb
 
 struct gorse_b200_index {
     gorse_b200_ctx *ctx = nullptr;
@@ -17,15 +36,16 @@ struct gorse_b200_index {
     float max_dx = 0.f;
     bool mma_ready = false;
     float *dbg_scores = nullptr;    // tests only: dense stage-1 scores
-    int64_t last_fallback_rows = 0; // rows of the last searches that needed the exact scan
-    cudaEvent_t ev0 = nullptr, ev1 = nullptr;  // CUDA events around the stage-1 kernel (bench.py roofline)
+    int64_t last_fallback_rows = 0; // rows of the last searches whose candidate set failed certification
+    std::vector<cudaEvent_t> ev;    // CUDA event pairs around the stage-1 kernels of one call (bench.py roofline)
     double stage1_ms = 0.0, stage1_flop = 0.0; // accumulated since the last debug read
     // reusable work buffers of the tensor path (sized for w_cq query rows at mirror width w_kp)
     int64_t w_cq = 0;
     int w_kp = 0;
     gb::DevBuf<__nv_bfloat16> w_qb;
     gb::DevBuf<float> w_eps, w_cval, w_theta;
-    gb::DevBuf<int32_t> w_ccol, w_ccnt, w_ids, w_idcnt, w_flag, w_flist;
+    gb::DevBuf<int32_t> w_ccol, w_ccnt;
+    gb::RecallWork recall;
     // result staging of search_common (grow-only: a 120 MB cudaMalloc + cudaFree per all-pairs call otherwise)
     gb::DevBuf<int32_t> r_idx, r_count;
     gb::DevBuf<float> r_dist;
@@ -130,17 +150,8 @@ __device__ __forceinline__ float key_float(uint32_t k)
 }
 #endif  // __CUDACC__
 
-// exact scan / re-rank.  row_list != nullptr: only those query rows (nq = length of the list) are processed
-int32_t launch_exact(gorse_b200_index *ix, const float *d_q, const int64_t *d_qidx, int64_t q0, int64_t nq, int k,
-                     const int32_t *d_cand, const int32_t *d_cand_count, int cand_stride, const int32_t *row_list,
-                     int32_t *d_idx, float *d_dist, int32_t *d_count, int prune0, int *d_nan);
-
-int32_t launch_exact_split(gorse_b200_index *ix, const float *d_q, const int64_t *d_qidx, int64_t q0, int32_t n_rows, int k,
-                           const int32_t *row_list, int32_t *d_idx, float *d_dist, int32_t *d_count, int prune0, int *d_nan,
-                           const uint8_t *allow = nullptr);
-
 int32_t index_reserve(gorse_b200_index *ix, int64_t need);
-// the tensor-core candidate sweep (topk_mma.cu), shared by search_mma and the batched recall (recall.cu).
+// the tensor-core candidate sweep (topk_mma.cu) of the top-k pipeline (recall_rows) and of the stage-1 test hook.
 // mma_reserve: the bf16 mirror and the work buffers for up to cq query rows per sweep.  mma_sample_tiles: the sample size
 // that leaves about `cands` columns per row above its threshold.  mma_sweep: query rows (q_base, d_q, d_qidx, q0 as in
 // build_queries_kernel) -> candidate lists in ix->w_ccol / w_cval / w_ccnt / w_theta, eps in ix->w_eps; ev0 / ev1 (may be
@@ -149,11 +160,36 @@ int32_t mma_reserve(gorse_b200_index *ix, int64_t cq);
 int mma_sample_tiles(const gorse_b200_index *ix, double cands);
 int32_t mma_sweep(gorse_b200_index *ix, const float *q_base, const float *d_q, const int64_t *d_qidx, int64_t q0, int64_t nq, int m_tiles,
                   cudaEvent_t ev0, cudaEvent_t ev1);
-bool mma_path_eligible(const gorse_b200_index *ix, int64_t nq, int k);
-// h_*: optional host result buffers; when given, every finished chunk of queries is downloaded on the context's copy stream
-// while the next chunk's kernels run
-int32_t search_mma(gorse_b200_index *ix, const float *d_q, const int64_t *d_qidx, int64_t q0, int64_t nq, int k, int prune0,
-                   int32_t *d_idx, float *d_dist, int32_t *d_count, int *d_nan, int32_t *h_idx = nullptr, float *h_dist = nullptr,
-                   int32_t *h_count = nullptr);
+// the sweep serves Dot and Euclidean indexes of >= 32768 vectors for >= 64 rows; GORSE_B200_TOPK_EXACT=1 turns it off
+bool mma_path_eligible(const gorse_b200_index *ix, int64_t nq);
+
+namespace recall {
+// A fixed-stride copy of the pipeline's answers (table_kernel): row q's entries at q * n, in order, with int32 slots; the
+// value is the score, negated when negate (the index's distance); with positive only values > 0 are kept; the row is padded
+// with slot -1 / value 0 and cnt[q] holds the kept entries.  h_*: host copies downloaded per chunk, or all nullptr.
+struct Table {
+    int32_t *slot;
+    float *val;
+    int32_t *cnt;
+    bool negate, positive;
+    int32_t *h_slot;
+    float *h_val;
+    int32_t *h_cnt;
+};
+
+// The dense top-k pipeline (topk.cu): routing, tensor-core sweep, window and exact kernels, for nq rows of the index.  Row q
+// is a host query q_host[q * d ..] or, with q_host == nullptr, the stored vector of slot d_qslots[q] (a device list), which
+// the row never returns.  allow (device, may be nullptr = every vector): 0 = never returned.  k_q = n + (excl_off[q + 1] -
+// excl_off[q]); ex[ex_off[q] ..]: each row's exclusions sorted, -1 entries dropped; excl_off == nullptr: no exclusions, k_q = n
+// (ex and ex_off are not read).  Row q's answer is the first k_q allowed
+// vectors by (score desc, slot asc) minus its exclusions, score = -distance; it starts at q * n + excl_off[q] in
+// ix->recall.slots / scores, count in ix->recall.count[q].  Every finished chunk is copied into `table` (may be nullptr) and
+// downloaded to the host buffers slots_out / scores_out / count_out (may be nullptr) and the table's host copies while the
+// next one computes.  *exact_rows_out (may be nullptr): rows the exact kernel answered.  The caller holds ix->mu; the call
+// ends with both streams synchronised.
+int32_t recall_rows(gorse_b200_index *ix, const uint8_t *allow, int64_t nq, const float *q_host, const int64_t *d_qslots, int32_t n,
+                    const int64_t *excl_off, const int64_t *ex, const int64_t *ex_off, const Table *table, int64_t *slots_out,
+                    float *scores_out, int32_t *count_out, int64_t *exact_rows_out);
+}  // namespace recall
 
 }  // namespace gb

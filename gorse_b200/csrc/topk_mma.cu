@@ -5,7 +5,7 @@
 // computed by wgmma (m64n128k16, bf16 operands, fp32 accumulators in registers), operands staged by TMA
 // (cp.async.bulk.tensor, 128-byte swizzle) through an mbarrier ring.  The N x N score matrix is never written: each consumer
 // warpgroup keeps only the columns whose score clears a per-row threshold, appending (column, score) to a small per-row
-// candidate list.  Stage 2 (topk.cu) re-ranks the candidates exactly in the reference's fp32 order.
+// candidate list.  The window kernel (topk.cu) certifies each row and re-ranks its window exactly in the reference's fp32 order.
 //
 // Threshold without a second pass: the vectors are stored in a random column permutation, so the first m columns are a
 // uniform sample.  For those the epilogue tracks each row's 16 best scores; theta = 16th best - 2*eps is then fixed,
@@ -13,9 +13,9 @@
 //   * soundness: every true top-k element has score >= (k-th best approximate score) - 2*eps, because |score - reference|
 //     <= eps for every column.  eps is an upper bound, not an estimate (build_queries_kernel derives it): |bf16(q)| max|bf16(x)
 //     - x| + |bf16(q) - q| max|x| for the bf16 rounding of both operands, plus the fp32 accumulation here and in the
-//     reference and, for Euclidean, the |x|^2/2 and distance roundings.  Stage 2 verifies that at least k candidates clear
-//     theta + 2*eps, which makes the candidate set a superset of the true top-k; rows that fail the check (or overflow
-//     their list) are redone by the exact scan.  With m = 4N/k and the 16th best, a row fails with probability ~1e-6.
+//     reference and, for Euclidean, the |x|^2/2 and distance roundings.  The window kernel verifies that at least k
+//     candidates clear theta + 2*eps, which makes the candidate set a superset of the true top-k; rows that fail the check
+//     (or overflow their list) go to the exact kernel.  With m = 4N/k and the 16th best, a row fails with probability ~1e-6.
 //
 // Roofline class: tensor pipe.  F = 2 * nq * N * Kp flop per sweep.
 #include <cuda.h>
@@ -363,90 +363,6 @@ __global__ void max_kernel(const float *v, int64_t n, float *out)
     if ((threadIdx.x & 31) == 0) atomicMax(reinterpret_cast<int *>(out), __float_as_int(m));  // non-negative floats order as ints
 }
 
-// ---- stage 2a: prune each row's candidates to the rigorous window and translate to original ids -------------
-// One warp per row.  The k-th largest approximate score is found WITHOUT sorting: the scores are mapped to order-preserving
-// 32-bit keys and the key is built bit by bit from the top (32 counting passes over <= CAP values held in shared memory).
-__global__ void __launch_bounds__(128)
-prune_kernel(const int32_t *cand_col, const float *cand_val, const int32_t *cand_cnt, const float *theta, const float *eps,
-             const int32_t *perm, const int64_t *q_idx, int64_t q0, bool self_skip, int64_t nq, int k, int32_t *out_ids /* [nq][CAP] */,
-             int32_t *out_cnt, int32_t *fallback_flag)
-{
-    extern __shared__ uint8_t sm[];
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nw = blockDim.x >> 5;
-    uint32_t *sk = reinterpret_cast<uint32_t *>(sm) + (size_t)warp * mma::CAP;                                          // keys
-    int32_t *sc = reinterpret_cast<int32_t *>(reinterpret_cast<uint32_t *>(sm) + (size_t)nw * mma::CAP) + (size_t)warp * mma::CAP;  // ids
-    for (int64_t row = (int64_t)blockIdx.x * nw + warp; row < nq; row += (int64_t)gridDim.x * nw) {
-        // every column with score >= max over the parts' thresholds was pushed by one of the parts
-        int np[mma::PARTS], n = 0;
-        float th = -INFINITY;
-        bool bad = !(eps[row] == eps[row]);
-#pragma unroll
-        for (int p = 0; p < mma::PARTS; p++) {
-            const int raw = cand_cnt[mma::PARTS * row + p];
-            bad |= raw > mma::PART_CAP;
-            np[p] = min(raw, mma::PART_CAP);
-            n += np[p];
-            th = fmaxf(th, theta[mma::PARTS * row + p]);
-        }
-        if (!(th == th)) bad = true;
-        int32_t *oi = out_ids + row * mma::CAP;
-        const int64_t self = self_skip ? (q_idx ? q_idx[row] : q0 + row) : -1;
-        int have = 0;
-        for (int e = lane; e < n; e += 32) {
-            int p = 0, r = e;   // entry e of the concatenated part lists
-#pragma unroll
-            for (int q = 0; q + 1 < mma::PARTS; q++)
-                if (p == q && r >= np[q]) { r -= np[q]; p++; }
-            const int64_t src = row * mma::CAP + p * mma::PART_CAP + r;
-            const int32_t c = perm[cand_col[src]];  // original id
-            const float v = cand_val[src];
-            const bool keep = c != self && v == v;   // SearchIndex never returns the query itself
-            sk[e] = keep ? float_key(v) : 0u;
-            sc[e] = c;
-            have += keep;
-        }
-        for (int o = 16; o; o >>= 1) have += __shfl_xor_sync(0xffffffffu, have, o);
-        __syncwarp();
-        if (have < k) bad = true;
-        int w = 0;
-        if (!bad) {
-            uint32_t t = 0;
-            for (int bit = 31; bit >= 0; bit--) {
-                const uint32_t candk = t | (1u << bit);
-                int cnt = 0;
-                for (int e = lane; e < n; e += 32) cnt += sk[e] >= candk;
-                for (int o = 16; o; o >>= 1) cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
-                if (cnt >= k) t = candk;
-            }
-            const float kth = key_float(t);            // the k-th largest approximate score
-            const float two_eps = 2.f * eps[row];
-            // validity: at least k candidates clear theta + 2 eps, i.e. the k-th best approximate score is known exactly
-            if (!(kth >= th + two_eps)) bad = true;
-            else {
-                const uint32_t lim = float_key(kth - two_eps);
-                for (int e0 = 0; e0 < n; e0 += 32) {
-                    const int e = e0 + lane;
-                    const bool in = e < n && sk[e] >= lim && sk[e] != 0u;
-                    const unsigned mk = __ballot_sync(0xffffffffu, in);
-                    if (in) oi[w + __popc(mk & ((1u << lane) - 1))] = sc[e];
-                    w += __popc(mk);
-                }
-            }
-        }
-        if (lane == 0) {
-            out_cnt[row] = bad ? 0 : w;
-            if (bad) fallback_flag[row] = 1;
-        }
-        __syncwarp();
-    }
-}
-
-__global__ void compact_flags_kernel(const int32_t *flag, int64_t nq, int32_t *list, int32_t *n_list)
-{
-    const int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (r < nq && flag[r]) list[atomicAdd(n_list, 1)] = (int32_t)r;
-}
-
 }  // namespace mma
 
 // ---- host side --------------------------------------------------------------------------------------------
@@ -486,13 +402,13 @@ static int kp_of(const gorse_b200_index *ix)
     return (d + mma::BK - 1) / mma::BK * mma::BK;
 }
 
-bool mma_path_eligible(const gorse_b200_index *ix, int64_t nq, int k)
+bool mma_path_eligible(const gorse_b200_index *ix, int64_t nq)
 {
     if (const char *e = getenv("GORSE_B200_TOPK_EXACT")) if (*e == '1') return false;
     const int kp = kp_of(ix);
     // the sample needs >= 32 tiles to make theta tight; small problems are faster on the exact scan anyway
     if (ix->metric != GORSE_B200_METRIC_EUCLIDEAN && ix->metric != GORSE_B200_METRIC_NEG_DOT) return false;   // cosine (vecdb.cu): exact scan
-    return kp <= mma::BK * mma::MAX_KB && k >= 1 && k <= 128 && ix->n >= 32768 && nq >= 64 && ix->n < (1ll << 31);
+    return kp <= mma::BK * mma::MAX_KB && ix->n >= 32768 && nq >= 64 && ix->n < (1ll << 31);
 }
 
 static int32_t ensure_mirror(gorse_b200_index *ix)
@@ -538,10 +454,6 @@ int32_t mma_reserve(gorse_b200_index *ix, int64_t cq)
     GB_TRY(ix->w_theta.alloc(mma::PARTS * cq));
     GB_TRY(ix->w_ccol.alloc((size_t)cq * mma::CAP));
     GB_TRY(ix->w_ccnt.alloc(mma::PARTS * cq));
-    GB_TRY(ix->w_ids.alloc((size_t)cq * mma::CAP));
-    GB_TRY(ix->w_idcnt.alloc(cq));
-    GB_TRY(ix->w_flag.alloc(cq));
-    GB_TRY(ix->w_flist.alloc(cq + 1));
     ix->w_cq = cq;
     ix->w_kp = kp;
     return GORSE_B200_OK;
@@ -588,88 +500,6 @@ int32_t mma_sweep(gorse_b200_index *ix, const float *q_base, const float *d_q, c
     if (ev1) cudaEventRecord(ev1, c->stream);
     GB_LAUNCHED(c);
     return GORSE_B200_OK;
-}
-
-int32_t search_mma(gorse_b200_index *ix, const float *d_q, const int64_t *d_qidx, int64_t q0, int64_t nq, int k, int prune0,
-                   int32_t *d_idx, float *d_dist, int32_t *d_count, int *d_nan, int32_t *h_idx, float *h_dist, int32_t *h_count)
-{
-    gorse_b200_ctx *c = ix->ctx;
-    // The parts of a row share ONE threshold from the whole sample, aimed at 4k columns per row: the row has fewer than k
-    // candidates when >= R_TOP of its true top k fell into the sample, Poisson(k m / N = R_TOP / 4): ~1e-6 per row, and a
-    // part's PART_CAP-slot list holds 4x its expected k columns (k <= 128).
-    const bool self_skip = d_q == nullptr;
-    // queries are processed in chunks of 1024 rows per SM so that the candidate lists stay modest while every chunk's kernel
-    // tail, host sync for the fallback count and fallback launches are amortised; a finished chunk is downloaded on the copy
-    // stream while the next one computes
-    const int64_t chunk = (int64_t)c->sm_count * mma::GROUP_ROWS * 8;
-    DevBuf<float> &eps = ix->w_eps, &cval = ix->w_cval, &theta = ix->w_theta;
-    DevBuf<int32_t> &ccol = ix->w_ccol, &ccnt = ix->w_ccnt, &ids = ix->w_ids, &idcnt = ix->w_idcnt, &flag = ix->w_flag, &flist = ix->w_flist;
-    int32_t st = GORSE_B200_OK;
-    auto done = [&](int32_t s) {
-        cudaStreamSynchronize(c->stream);
-        cudaStreamSynchronize(c->copy_stream);
-        return s;
-    };
-    const int64_t cq = std::min(nq, chunk);
-    if ((st = mma_reserve(ix, cq))) return done(st);
-    const int m_tiles = mma_sample_tiles(ix, 4.0 * k);
-    const int64_t fl_off = ix->w_cq;  // the fallback counter sits after the list
-    if (!ix->ev0) { cudaEventCreate(&ix->ev0); cudaEventCreate(&ix->ev1); }
-    cudaError_t e;
-    for (int64_t off = 0; off < nq; off += cq) {
-        const int64_t n_this = std::min(cq, nq - off);
-        const float *qp = d_q ? d_q + off * ix->d : nullptr;
-        const int64_t *qi = d_qidx ? d_qidx + off : nullptr;
-        if ((st = mma_sweep(ix, ix->X.p, qp, qi, q0 + off, n_this, m_tiles, ix->ev0, ix->ev1))) return done(st);
-        if ((e = cudaMemsetAsync(flag.p, 0, sizeof(int32_t) * n_this, c->stream)) != cudaSuccess ||
-            (e = cudaMemsetAsync(flist.p + fl_off, 0, sizeof(int32_t), c->stream)) != cudaSuccess) {
-            set_error("search_mma memset: %s", cudaGetErrorString(e));
-            return done(GORSE_B200_ERR_CUDA);
-        }
-        const int pw = 4;
-        const size_t psm = (size_t)pw * mma::CAP * 8;
-        if ((e = cudaFuncSetAttribute(mma::prune_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)psm)) != cudaSuccess) {
-            set_error("prune smem attr: %s", cudaGetErrorString(e));
-            return done(GORSE_B200_ERR_CUDA);
-        }
-        mma::prune_kernel<<<(unsigned)std::min<int64_t>((n_this + pw - 1) / pw, (int64_t)c->sm_count * 8), 32 * pw, psm, c->stream>>>(
-            ccol.p, cval.p, ccnt.p, theta.p, eps.p, ix->perm.p, qi, q0 + off, self_skip, n_this, k, ids.p, idcnt.p, flag.p);
-        c->launches++;
-        // stage 2: exact re-rank of the window, reference fp32 order
-        if ((st = launch_exact(ix, qp, qi, q0 + off, n_this, k, ids.p, idcnt.p, mma::CAP, nullptr, d_idx + off * k, d_dist + off * k, d_count + off,
-                               prune0, d_nan)))
-            return done(st);
-        // rows whose candidate set could not be certified: exact scan over everything
-        mma::compact_flags_kernel<<<(unsigned)((n_this + 255) / 256), 256, 0, c->stream>>>(flag.p, n_this, flist.p, flist.p + fl_off);
-        c->launches++;
-        int32_t n_fb = 0;
-        if ((e = cudaMemcpyAsync(&n_fb, flist.p + fl_off, sizeof(int32_t), cudaMemcpyDeviceToHost, c->stream)) != cudaSuccess ||
-            (e = cudaStreamSynchronize(c->stream)) != cudaSuccess) {
-            set_error("search_mma: %s", cudaGetErrorString(e));
-            return done(GORSE_B200_ERR_CUDA);
-        }
-        ix->last_fallback_rows += n_fb;
-        {
-            float ms = 0.f;  // the stream was synchronised just above
-            if (cudaEventElapsedTime(&ms, ix->ev0, ix->ev1) == cudaSuccess) { ix->stage1_ms += ms; ix->stage1_flop += 2.0 * (double)n_this * (double)ix->n * (double)ix->d; }
-        }
-        if (n_fb > 0) {
-            if ((st = launch_exact_split(ix, qp, qi, q0 + off, n_fb, k, flist.p, d_idx + off * k, d_dist + off * k, d_count + off, prune0, d_nan)))
-                return done(st);
-        }
-        if (h_idx) {
-            // this chunk is final: download it on the copy stream while the next chunk computes
-            if ((e = cudaEventRecord(c->copy_ev, c->stream)) != cudaSuccess || (e = cudaStreamWaitEvent(c->copy_stream, c->copy_ev, 0)) != cudaSuccess ||
-                (e = cudaMemcpyAsync(h_idx + off * k, d_idx + off * k, sizeof(int32_t) * n_this * k, cudaMemcpyDeviceToHost, c->copy_stream)) != cudaSuccess ||
-                (e = cudaMemcpyAsync(h_dist + off * k, d_dist + off * k, sizeof(float) * n_this * k, cudaMemcpyDeviceToHost, c->copy_stream)) != cudaSuccess ||
-                (e = cudaMemcpyAsync(h_count + off, d_count + off, sizeof(int32_t) * n_this, cudaMemcpyDeviceToHost, c->copy_stream)) != cudaSuccess) {
-                set_error("search_mma download: %s", cudaGetErrorString(e));
-                return done(GORSE_B200_ERR_CUDA);
-            }
-        }
-    }
-    if ((e = cudaGetLastError()) != cudaSuccess) { set_error("search_mma: %s", cudaGetErrorString(e)); return done(GORSE_B200_ERR_CUDA); }
-    return done(GORSE_B200_OK);
 }
 
 }  // namespace gb

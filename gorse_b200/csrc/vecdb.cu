@@ -129,7 +129,6 @@ int32_t gorse_b200_vecdb_destroy(gorse_b200_vecdb *db)
         ScopedDevice sd(db->ctx->device);
         cudaStreamSynchronize(db->ctx->stream);
         db->d_blocked.free(); db->d_allow.free(); db->d_cat_off.free(); db->d_cats.free(); db->d_want.free();
-        db->recall.free();
         db->i2i.free();
     }
     gorse_b200_index_destroy(db->dense);
@@ -265,44 +264,20 @@ int32_t gorse_b200_vecdb_query(gorse_b200_vecdb *db, int64_t nq, const float *q_
         return GORSE_B200_OK;
     }
     GB_TRY(vecdb_allow(db, categories, n_categories));
-    std::vector<int32_t> idx((size_t)nq * topk);
-    int32_t st = GORSE_B200_OK;
-    if (db->dim > 0) {
-        gorse_b200_index *ix = db->dense;
-        std::lock_guard<std::mutex> lk2(ix->mu);
-        DevBuf<float> d_q, d_dist;
-        DevBuf<int32_t> d_idx, d_cnt;
-        DevBuf<int> d_nan;
-        auto done = [&](int32_t s) { cudaStreamSynchronize(c->stream); d_q.free(); d_dist.free(); d_idx.free(); d_cnt.free(); d_nan.free(); return s; };
-        if ((st = d_q.alloc((size_t)nq * db->dim)) || (st = d_dist.alloc((size_t)nq * topk)) || (st = d_idx.alloc((size_t)nq * topk)) ||
-            (st = d_cnt.alloc((size_t)nq)) || (st = d_nan.alloc(1)))
-            return done(st);
-        cudaError_t e = cudaMemsetAsync(d_nan.p, 0, sizeof(int), c->stream);
-        if (e == cudaSuccess) e = cudaMemcpyAsync(d_q.p, q_values, sizeof(float) * (size_t)nq * db->dim, cudaMemcpyHostToDevice, c->stream);
-        if (e != cudaSuccess) { set_error("vecdb query upload: %s", cudaGetErrorString(e)); return done(GORSE_B200_ERR_CUDA); }
-        if ((st = launch_exact_split(ix, d_q.p, nullptr, 0, (int32_t)nq, topk, nullptr, d_idx.p, d_dist.p, d_cnt.p, 0, d_nan.p, db->d_allow.p))) return done(st);
-        int h_nan = 0;
-        if ((e = cudaMemcpyAsync(idx.data(), d_idx.p, sizeof(int32_t) * (size_t)nq * topk, cudaMemcpyDeviceToHost, c->stream)) != cudaSuccess ||
-            (e = cudaMemcpyAsync(scores_out, d_dist.p, sizeof(float) * (size_t)nq * topk, cudaMemcpyDeviceToHost, c->stream)) != cudaSuccess ||
-            (e = cudaMemcpyAsync(count_out, d_cnt.p, sizeof(int32_t) * (size_t)nq, cudaMemcpyDeviceToHost, c->stream)) != cudaSuccess ||
-            (e = cudaMemcpyAsync(&h_nan, d_nan.p, sizeof(int), cudaMemcpyDeviceToHost, c->stream)) != cudaSuccess ||
-            (e = cudaStreamSynchronize(c->stream)) != cudaSuccess) {
-            set_error("vecdb query: %s", cudaGetErrorString(e));
-            return done(GORSE_B200_ERR_CUDA);
-        }
-        if (h_nan) { set_error("NaN distance"); return done(GORSE_B200_ERR_ARG); }
-        // both metrics of the index are distances (-dot / Euclidean): the score is their negation (xvec.go:425-427; Dot -> dot)
-        for (int64_t t = 0; t < nq * topk; t++) scores_out[t] = -scores_out[t];
-        st = done(GORSE_B200_OK);
-    } else {
-        GB_CHECK_ARG(topk <= 128, "sparse collections answer topK <= 128 (got %d)", topk);
-        for (int64_t q = 0; q < nq; q++)
-            for (int64_t t = q_sp_off[q]; t < q_sp_off[q + 1]; t++)
-                GB_CHECK_ARG(t == q_sp_off[q] || q_sp_indices[t] > q_sp_indices[t - 1], "query %lld: indices not strictly ascending", (long long)q);
-        std::lock_guard<std::mutex> lk2(db->sparse->mu);
-        st = sparse_search_host(db->sparse, 0, nq, q_sp_off, q_sp_indices, q_values, db->d_allow.p, topk, idx.data(), scores_out, count_out);
+    if (db->dim > 0) {   // the pipeline's score is the negated distance of the index (-dot / Euclidean): xvec.go:425-427, Dot -> dot
+        std::lock_guard<std::mutex> lk2(db->dense->mu);
+        return recall::recall_rows(db->dense, db->d_allow.p, nq, q_values, nullptr, topk, nullptr, nullptr, nullptr, nullptr, slots_out, scores_out,
+                                   count_out, nullptr);   // no exclusions: row q at q * topk
     }
-    if (st) return st;
+    GB_CHECK_ARG(topk <= 128, "sparse collections answer topK <= 128 (got %d)", topk);
+    for (int64_t q = 0; q < nq; q++)
+        for (int64_t t = q_sp_off[q]; t < q_sp_off[q + 1]; t++)
+            GB_CHECK_ARG(t == q_sp_off[q] || q_sp_indices[t] > q_sp_indices[t - 1], "query %lld: indices not strictly ascending", (long long)q);
+    std::vector<int32_t> idx((size_t)nq * topk);
+    {
+        std::lock_guard<std::mutex> lk2(db->sparse->mu);
+        GB_TRY(sparse_search_host(db->sparse, 0, nq, q_sp_off, q_sp_indices, q_values, db->d_allow.p, topk, idx.data(), scores_out, count_out));
+    }
     for (int64_t t = 0; t < nq * topk; t++) slots_out[t] = idx[(size_t)t];
     return GORSE_B200_OK;
 }

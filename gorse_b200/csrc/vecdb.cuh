@@ -1,20 +1,8 @@
-// vecdb.cuh -- state of one vector collection (vecdb.cu), shared with the batched recall (recall.cu).
+// vecdb.cuh -- state of one vector collection (vecdb.cu), shared with the batched recall (recall.cu) and item-to-item.
 #pragma once
 #include "topk.cuh"
 
 namespace gb {
-// grow-only work buffers of gorse_b200_vecdb_query_excluding, kept with the collection
-struct RecallWork {
-    DevBuf<float> q, scores, scratch;
-    DevBuf<int64_t> ex_off, ex, out_off, rows, slots;
-    DevBuf<int32_t> k, need, count, flags;
-    void free()
-    {
-        q.free(); scores.free(); scratch.free();
-        ex_off.free(); ex.free(); out_off.free(); rows.free(); slots.free();
-        k.free(); need.free(); count.free(); flags.free();
-    }
-};
 // grow-only work buffers of gorse_b200_vecdb_item_to_item (item_to_item.cu): the neighbour table of stage A and the user
 // batches, answers and accumulator scratch of stage B
 struct ItemToItemWork {
@@ -49,7 +37,6 @@ struct gorse_b200_vecdb {
     gb::DevBuf<uint8_t> d_blocked, d_allow;   // blocked = hidden | dead
     gb::DevBuf<int64_t> d_cat_off;
     gb::DevBuf<int32_t> d_cats, d_want;
-    gb::RecallWork recall;   // batched recall (recall.cu)
     gb::ItemToItemWork i2i;  // batched item-to-item recommendation (item_to_item.cu)
 };
 

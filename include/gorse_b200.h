@@ -348,7 +348,7 @@ int32_t gorse_b200_vecdb_get_sparse(gorse_b200_vecdb *db, int64_t slot, uint32_t
 int32_t gorse_b200_vecdb_delete_before(gorse_b200_vecdb *db, int64_t timestamp_ms, int64_t *slots_out, int64_t cap, int64_t *count_out);
 /* QueryVectors (xvec.go:373-449) for nq query vectors sharing one category filter: candidates are live, not hidden and
  * carry ALL of categories[n_categories] (CONTAIN_ALL, :381-389).  Results per query: slots_out / scores_out [nq x topk],
- * best first, count_out[nq]; score = dot (Dot) or the NEGATED distance (Euclidean, Cosine) -- higher is more similar
+ * best first, count_out[nq]; entries past count_out[q] in a row are not part of the answer and are left unspecified; score = dot (Dot) or the NEGATED distance (Euclidean, Cosine) -- higher is more similar
  * (database.go:101, xvec.go:425-427).  Sparse: only positive dots are returned (the reference drops score 0, :421-423, and
  * its callers drop score <= 0, logics/item_to_item.go:73); topk <= 128.  topk <= 0 -> no results (:374-376). */
 /* Model hand-off (master/tasks.go:925-961): the item factors of every item with >= 1 training feedback (IsItemPredictable)

@@ -246,18 +246,20 @@ def test_repeatable_and_path_independent(gb, ctx, monkeypatch, kind):
 
 @gpu
 @pytest.mark.parametrize("kind,scale", [("euclid", 1.0), ("sparse", 0.5)])
-def test_matches_the_per_item_path(gb, ctx, kind, scale):
-    """vecdb_query(c, topK = n + 1) per context item + similar_scores + a host sum: what the library served before"""
+def test_matches_the_per_item_path(gb, orc, ctx, kind, scale):
+    """vecdb_query(c, topK = n + 1) per context item + similar_scores + a host sum: what the library served before.  Dense
+    vecdb_query runs the same top-k pipeline as item_to_item, so the oracle's restatement is checked too."""
     rng = np.random.default_rng(51)
     N, n = 3000, 25
     if kind == "sparse":
-        col, _, hidden, dead, _ = sparse_collection(gb, ctx, rng, N)
+        col, store, hidden, dead, cats = sparse_collection(gb, ctx, rng, N)
     else:
-        col, _, hidden, dead, _ = dense_collection(gb, ctx, rng, N, 32, gb.DISTANCE_EUCLIDEAN)
+        col, store, hidden, dead, cats = dense_collection(gb, ctx, rng, N, 32, gb.DISTANCE_EUCLIDEAN)
     metric = gb.METRIC_NEG_DOT if kind == "sparse" else gb.METRIC_EUCLIDEAN
     with col:
         contexts, excludes = make_users(rng, N, hidden, dead, 12)
         rows, _ = col.item_to_item(contexts, excludes, n, categories=[2], score_scale=scale)
+        assert_rows_equal(rows, expected(orc, store, allow_mask(hidden, dead, cats, [2]), dead, contexts, excludes, n, scale))
         _, _, _, live = col.get(np.arange(N))
         for (gs, gv), ctx_u, ex_u in zip(rows, contexts, excludes):
             acc, drop = {}, set(ex_u.tolist())

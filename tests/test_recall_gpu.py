@@ -123,9 +123,25 @@ def test_dot_matches_the_oracle(gb, orc, ctx, N, nq):
                            for i, r in enumerate(rows))
 
 
+def cosine_expected(orc, X, allow, Q, excl, n):
+    """the collection's Cosine query restated: 1 - q.x / (|q| |x|) with the reference's fp32 dots, ascending, then slot"""
+    ids = np.nonzero(allow)[0]
+    nx = np.array([np.sqrt(orc.dot(X[i], X[i])) for i in ids], np.float32)
+    out = []
+    for q in range(Q.shape[0]):
+        nq_ = np.sqrt(orc.dot(Q[q], Q[q]))
+        dist = np.array([np.float32(1) - orc.dot(Q[q], X[i]) / (nq_ * nx[j]) for j, i in enumerate(ids)], np.float32)
+        order = np.lexsort((ids, dist))[: n + len(excl[q])]
+        keep = ~np.isin(ids[order], excl[q])
+        out.append((ids[order][keep].astype(np.int64), (-dist[order][keep]).astype(np.float32)))
+    return out
+
+
 @gpu
 @pytest.mark.parametrize("dist,d", [("euclid", 40), ("cosine", 32)])
-def test_euclidean_and_cosine_match_vecdb_query(gb, ctx, dist, d):
+def test_euclidean_and_cosine_match_vecdb_query(gb, orc, ctx, dist, d):
+    """vecdb_query and query_excluding run one top-k pipeline; a sample of rows is also checked against the oracle (Euclidean)
+    or a restatement of the Cosine query"""
     rng = np.random.default_rng(d)
     N, nq, n = 40000, 128, 50
     gd = gb.DISTANCE_EUCLIDEAN if dist == "euclid" else gb.DISTANCE_COSINE
@@ -135,6 +151,13 @@ def test_euclidean_and_cosine_match_vecdb_query(gb, ctx, dist, d):
         sizes = [0 if i % 8 == 0 else int(rng.integers(1, 300)) for i in range(nq)]
         excl = [rng.choice(N, size=m, replace=False).astype(np.int64) for m in sizes]
         rows, _ = col.query_excluding(Q, excl, n)
+        allow = (hidden == 0) & ~dead
+        sample = list(range(0, nq, 16))
+        if dist == "euclid":
+            want = expected(orc, X, allow, Q[sample], [excl[q] for q in sample], n, orc.METRIC_EUCLIDEAN)
+        else:
+            want = cosine_expected(orc, X, allow, Q[sample], [excl[q] for q in sample], n)
+        assert_rows_equal([rows[q] for q in sample], want)
         kmax = n + max(sizes)
         s, sc, cnt = col.query(Q, [], kmax)   # a prefix of the top kmax is the top k_q (one total order)
         for q in range(nq):
