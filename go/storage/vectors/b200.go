@@ -489,6 +489,106 @@ func (db *B200) ItemToItemRecommend(ctx context.Context, collection string, cont
 	return results, nil
 }
 
+// UserToUserRecommend answers the worker's user-to-user recommender (Recommender.recommendUserToUser,
+// logics/recommend.go:285-348) for many users in one call on the collection UserToUserCollection(name): row i is what the
+// recommender returns for user userIds[i] with exclude set excludeIds[i] -- the first n similar users (QueryUserToUser,
+// logics/user_to_user.go:50-86), each one's score added to every item of its positive feedback in float64 without the
+// excluded ids, the best n, and of those only the items with itemOK set.  itemIds is the caller's item dictionary;
+// feedback[userId] holds that user's positive feedback as indices into it (an item may repeat, once per positive feedback
+// type); itemOK[j] reports whether itemIds[j] exists, is not hidden, is within ItemTTL and holds the requested categories.
+// scoreScale is 0.5 for type "auto", else 1.  Users without a vector get an empty row; excluded ids outside the dictionary
+// are harmless; the ids of one exclude set must be distinct, as a set's are.  Exact score ties are ordered by item index;
+// the reference's map order there is unpinned.  The caller adds each item's categories from its own item metadata.
+func (db *B200) UserToUserRecommend(ctx context.Context, collection string, userIds []string, itemIds []string, feedback map[string][]int32,
+	itemOK []bool, excludeIds [][]string, n int, scoreScale float64) ([][]cache.Score, error) {
+	if len(userIds) != len(excludeIds) {
+		return nil, errors.Errorf("%d users with %d exclude sets", len(userIds), len(excludeIds))
+	}
+	if len(itemOK) != len(itemIds) {
+		return nil, errors.Errorf("%d item flags for %d items", len(itemOK), len(itemIds))
+	}
+	results := make([][]cache.Score, len(userIds))
+	if len(userIds) == 0 || n <= 0 {
+		return results, nil
+	}
+	db.mu.RLock()
+	defer db.mu.RUnlock()
+	c, err := db.collection(collection)
+	if err != nil {
+		return nil, err
+	}
+	userSlots := make([]int64, len(userIds))
+	for i, id := range userIds {
+		slot, ok := c.slotOf[id]
+		if !ok {
+			slot = -1
+		}
+		userSlots[i] = slot
+	}
+	// the feedback rows by slot: only live slots can be neighbours
+	rows := make([][]int32, len(c.idOf))
+	for id, items := range feedback {
+		if slot, ok := c.slotOf[id]; ok {
+			rows[slot] = items
+		}
+	}
+	fbOff := make([]int64, len(rows)+1)
+	fbItems := []int32{}
+	for s, items := range rows {
+		for _, j := range items {
+			if j < 0 || int(j) >= len(itemIds) {
+				return nil, errors.Errorf("feedback of %s: item index %d outside the %d items", c.idOf[s], j, len(itemIds))
+			}
+		}
+		fbItems = append(fbItems, items...)
+		fbOff[s+1] = int64(len(fbItems))
+	}
+	okFlags := make([]uint8, len(itemIds))
+	for j, v := range itemOK {
+		if v {
+			okFlags[j] = 1
+		}
+	}
+	index := make(map[string]int64, len(itemIds))
+	for j, id := range itemIds {
+		index[id] = int64(j)
+	}
+	exOff := make([]int64, len(excludeIds)+1)
+	exItems := []int64{}
+	for i, ids := range excludeIds {
+		for _, id := range ids {
+			j, found := index[id]
+			if !found {
+				j = -1
+			}
+			exItems = append(exItems, j)
+		}
+		exOff[i+1] = int64(len(exItems))
+	}
+	users := len(userIds)
+	items, scores, counts := make([]int64, users*n), make([]float64, users*n), make([]int32, users)
+	stats := make([]int64, 4)
+	st := C.gorse_b200_vecdb_user_to_user(c.handle, C.int64_t(users), i64p(userSlots), C.int64_t(len(rows)), i64p(fbOff), i32p(fbItems),
+		C.int32_t(len(itemIds)), u8p(okFlags), i64p(exOff), i64p(exItems), C.int32_t(n), C.double(scoreScale), i64p(items),
+		(*C.double)(unsafe.Pointer(&scores[0])), i32p(counts), i64p(stats))
+	runtime.KeepAlive(userSlots)
+	runtime.KeepAlive(fbItems)
+	runtime.KeepAlive(okFlags)
+	runtime.KeepAlive(exItems)
+	if err := b200Err(st); err != nil {
+		return nil, err
+	}
+	log.Logger().Debug("batched user-to-user", zap.Int("users", users), zap.Int64("query_users", stats[0]), zap.Int64("exact_rows", stats[1]))
+	for i := range results {
+		row := make([]cache.Score, 0, counts[i])
+		for j := i * n; j < i*n+int(counts[i]); j++ {
+			row = append(row, cache.Score{Id: itemIds[items[j]], Score: scores[j]})
+		}
+		results[i] = row
+	}
+	return results, nil
+}
+
 func f32p(s []float32) *C.float {
 	if len(s) == 0 {
 		return nil

@@ -499,6 +499,36 @@ class VectorCollection:
         rows = [(slots[u * m:u * m + c].copy(), scores[u * m:u * m + c].copy()) for u, c in zip(range(nu), cnt)]
         return rows, dict(zip(("context_items", "exact_rows", "shared_users", "global_users"), (int(x) for x in stats)))
 
+    def user_to_user(self, user_slots, feedback_lists, exclude_lists, n, n_items, item_ok=None, score_scale=1.0):
+        """Batched user-to-user recommendation (gorse_b200_vecdb_user_to_user; logics/recommend.go:285-348): for user i, the
+        first n neighbours of slot user_slots[i] (-1 = a user without a vector), each neighbour v's score added to every item
+        of feedback_lists[v] (item indices in [0, n_items); slots past the list have no feedback) not in exclude_lists[i]
+        (-1 = an id outside the dictionary), summed in float64; the best n, then only the items with item_ok[item] != 0 (None:
+        all).  score_scale: 0.5 for type "auto", else 1.
+        -> ([(items int64, scores float64) per user], stats {query_users, exact_rows, shared_users, global_users})"""
+        slots = np.ascontiguousarray(user_slots, np.int64).reshape(-1)
+        nu = slots.size
+        if len(exclude_lists) != nu:
+            raise ValueError(f"{len(exclude_lists)} exclude lists for {nu} users")
+        nf = len(feedback_lists)
+        foff = np.zeros(nf + 1, np.int64)
+        np.cumsum([len(x) for x in feedback_lists], out=foff[1:])
+        fitems = np.ascontiguousarray(np.concatenate([np.asarray(x, np.int32).reshape(-1) for x in feedback_lists]) if nf else [], np.int32)
+        eoff = np.zeros(nu + 1, np.int64)
+        np.cumsum([len(x) for x in exclude_lists], out=eoff[1:])
+        es = np.ascontiguousarray(np.concatenate([np.asarray(x, np.int64).reshape(-1) for x in exclude_lists]) if nu else [], np.int64)
+        ok = None if item_ok is None else np.ascontiguousarray(item_ok, np.uint8)
+        if ok is not None and ok.size != n_items:
+            raise ValueError(f"item_ok has {ok.size} entries for {n_items} items")
+        m = max(n, 0)
+        items, scores, cnt = np.full(max(nu * m, 1), -1, np.int64), np.zeros(max(nu * m, 1), np.float64), np.zeros(max(nu, 1), np.int32)
+        stats = np.zeros(4, np.int64)
+        check(lib.gorse_b200_vecdb_user_to_user(self.h, nu, ptr(slots), nf, ptr(foff), ptr(fitems) if fitems.size else None, int(n_items),
+                                                ptr(ok) if ok is not None and ok.size else None, ptr(eoff), ptr(es) if es.size else None, n,
+                                                float(score_scale), ptr(items), ptr(scores), ptr(cnt), ptr(stats)))
+        rows = [(items[u * m:u * m + c].copy(), scores[u * m:u * m + c].copy()) for u, c in zip(range(nu), cnt)]
+        return rows, dict(zip(("query_users", "exact_rows", "shared_users", "global_users"), (int(x) for x in stats)))
+
     def __enter__(self):
         return self
 

@@ -13,22 +13,20 @@
 //   stage B   i2i_aggregate_kernel, one CTA per user: walks C_u in order and adds s = (double)score * scale (Euclidean:
 //             1 / (1 - s)) per neighbour slot not in E_u, with a barrier between context entries so that every sum is formed
 //             in the reference's order; then selects the first n by (score desc, slot asc) with a 64-bit radix select and
-//             sorts them.  The accumulator is an open-addressing table in shared memory when |C_u| * n <= TABLE_KEYS, else
+//             sorts them (agg::select_first_n, aggregate.cuh, shared with user_to_user.cu).  The accumulator is an open-addressing table in shared memory when |C_u| * n <= TABLE_KEYS, else
 //             this CTA's float64 row of length N in global memory, with a touched flag per slot and the list of touched slots.
 #include <algorithm>
 
-#include "recall.cuh"
+#include "aggregate.cuh"
 #include "sparse.cuh"
 #include "vecdb.cuh"
 
 namespace gb {
 namespace i2i {
 
-using u128 = unsigned __int128;
-
-constexpr int AGG_THREADS = 256;
-constexpr int TABLE_CAP = 8192;                  // shared-memory table entries: int32 slot + float64 sum, 96 KB
-constexpr int TABLE_KEYS = TABLE_CAP / 4 * 3;    // a user takes the table when |C_u| * n <= this (load <= 3/4)
+using agg::TABLE_CAP;
+using agg::TABLE_KEYS;                           // a user takes the table when |C_u| * n <= this
+constexpr int AGG_THREADS = agg::THREADS;
 constexpr int MAX_N_DENSE = 1024;                // the sort buffer holds n entries
 constexpr int MAX_N_SPARSE = 128;                // sparse_search_kernel's k
 
@@ -48,20 +46,6 @@ struct Table {                // stage A: the first n neighbours of each distinc
     const int32_t *cnt;       // [rows]
 };
 
-// order-preserving 64-bit key of a float64 sum (never 0: the sums are not NaN)
-__device__ __forceinline__ uint64_t sum_key(double v)
-{
-    const uint64_t u = (uint64_t)__double_as_longlong(v);
-    return (u >> 63) ? ~u : (u | (1ull << 63));
-}
-
-// QueryItemToItem's score (logics/item_to_item.go:76-79), rounded step by step as Go does
-__device__ __forceinline__ double neighbour_score(float raw, double scale, bool euclid)
-{
-    const double s = __dmul_rn((double)raw, scale);
-    return euclid ? __ddiv_rn(1.0, __dsub_rn(1.0, s)) : s;
-}
-
 // one CTA per user of `users`.  SHARED: the accumulator is a table in shared memory; else acc_rows / seen_rows /
 // touched_rows hold one [N] float64 row, one [N] flag row (all zero between users) and one [N] slot list per CTA.
 template <bool SHARED>
@@ -70,16 +54,14 @@ i2i_aggregate_kernel(const int32_t *users, int64_t n_users, Users U, Table T, in
                      uint8_t *seen_rows, int32_t *touched_rows)
 {
     using namespace gb::recall;
+    using namespace gb::agg;
     constexpr int NT = AGG_THREADS;
     extern __shared__ __align__(16) uint8_t sm[];
     const int p2 = pow2_at_least(n);
-    u128 *s_key = reinterpret_cast<u128 *>(sm);                    // [p2] sort keys: ~sum key, then slot
-    double *s_val = reinterpret_cast<double *>(s_key + p2);        // [p2]
-    int *hist = reinterpret_cast<int *>(s_val + p2);               // [256]
-    int *s_warp = hist + 256;                                      // [32]
-    int *s_bc = s_warp + 32;                                       // [4]: select, [2] gather fill, [3] distinct slots
-    int32_t *t_key = reinterpret_cast<int32_t *>(s_bc + 4);        // SHARED: [TABLE_CAP] slot, -1 = empty
-    double *t_val = reinterpret_cast<double *>(t_key + TABLE_CAP); // SHARED: [TABLE_CAP] sum
+    const Smem S = carve(sm, p2);
+    int *s_bc = S.s_bc;                                            // [3]: distinct slots
+    int32_t *t_key = S.t_key;                                      // SHARED: slot, -1 = empty
+    double *t_val = S.t_val;                                       // SHARED: sum
     double *acc = SHARED ? nullptr : acc_rows + (int64_t)blockIdx.x * N;
     uint8_t *seen = SHARED ? nullptr : seen_rows + (int64_t)blockIdx.x * N;
     int32_t *touched = SHARED ? nullptr : touched_rows + (int64_t)blockIdx.x * N;
@@ -127,62 +109,18 @@ i2i_aggregate_kernel(const int32_t *users, int64_t n_users, Users U, Table T, in
             __syncthreads();
         }
         const int distinct = s_bc[3];
-        const int m = min(n, distinct);
-        if (m > 0) {
-            const int64_t range = SHARED ? cap : distinct;
-            auto slot_at = [&](int64_t j) -> int32_t { return SHARED ? t_key[j] : touched[j]; };
-            auto val_at = [&](int64_t j) -> double { return SHARED ? t_val[j] : acc[touched[j]]; };
-            auto key_at = [&](int64_t j) -> uint64_t { return slot_at(j) >= 0 ? sum_key(val_at(j)) : 0ull; };
-            int ties;
-            const uint64_t K = block_select<NT>(range, m, key_at, hist, s_bc, &ties);
-            // of the sums equal to the m-th, the `ties` lowest slots are kept
-            int eq = 0;
-            for (int64_t j = threadIdx.x; j < range; j += NT) eq += key_at(j) == K;
-            eq = block_sum<NT>(eq, s_warp);
-            uint32_t last = 0xffffffffu;
-            if (eq > ties) {
-                int t2;
-                last = ~block_select<NT>(range, ties, [&](int64_t j) { return key_at(j) == K ? ~(uint32_t)slot_at(j) : 0u; }, hist, s_bc, &t2);
-            }
-            if (threadIdx.x == 0) s_bc[2] = 0;
-            __syncthreads();
-            for (int64_t j = threadIdx.x; j < range; j += NT) {
-                const uint64_t k = key_at(j);
-                if (k > K || (k == K && (uint32_t)slot_at(j) <= last)) {
-                    const int pos = atomicAdd(&s_bc[2], 1);
-                    s_key[pos] = ((u128)~k << 64) | (uint32_t)slot_at(j);
-                    s_val[pos] = val_at(j);
-                }
-            }
-            for (int j = m + threadIdx.x; j < p2; j += NT) s_key[j] = ~(u128)0;
-            __syncthreads();
-            block_sort<NT>(s_key, s_val, p2);
-            for (int j = threadIdx.x; j < m; j += NT) {
-                U.slots[u * n + j] = (int64_t)(uint32_t)s_key[j];
-                U.scores[u * n + j] = s_val[j];
-            }
+        auto slot_at = [&](int64_t j) -> int32_t { return SHARED ? t_key[j] : touched[j]; };
+        auto val_at = [&](int64_t j) -> double { return SHARED ? t_val[j] : acc[touched[j]]; };
+        const int m = select_first_n<NT>(SHARED ? cap : distinct, distinct, n, p2, slot_at, val_at, S);
+        for (int j = threadIdx.x; j < m; j += NT) {
+            U.slots[u * n + j] = (int64_t)(uint32_t)S.s_key[j];
+            U.scores[u * n + j] = S.s_val[j];
         }
         if (threadIdx.x == 0) U.count[u] = m;
         if (!SHARED)
             for (int j = threadIdx.x; j < distinct; j += NT) seen[touched[j]] = 0;
         __syncthreads();
     }
-}
-
-size_t aggregate_smem(int n, bool shared)
-{
-    const size_t p2 = (size_t)recall::pow2_at_least(n);
-    return p2 * 24 + (256 + 32 + 4) * 4 + (shared ? (size_t)TABLE_CAP * 12 : 0);
-}
-
-// grow b to n entries; a new allocation is zeroed
-template <typename T>
-int32_t grow_zeroed(DevBuf<T> &b, size_t n, cudaStream_t s)
-{
-    if (b.n >= n) return GORSE_B200_OK;
-    GB_TRY(b.alloc(n));
-    GB_CUDA(cudaMemsetAsync(b.p, 0, sizeof(T) * n, s));
-    return GORSE_B200_OK;
 }
 
 }  // namespace i2i
@@ -196,6 +134,7 @@ extern "C" int32_t gorse_b200_vecdb_item_to_item(gorse_b200_vecdb *db, int64_t n
                                                  int32_t *count_out, int64_t *stats_out)
 {
     using namespace gb::i2i;
+    using gb::agg::grow_zeroed;
     using gb::recall::grow;
     GB_CHECK_ARG(db != nullptr, "collection is NULL");
     GB_CHECK_ARG(n_users >= 0 && n_categories >= 0, "negative count");
@@ -307,7 +246,7 @@ extern "C" int32_t gorse_b200_vecdb_item_to_item(gorse_b200_vecdb *db, int64_t n
         (st = grow(V.c_row, (size_t)std::max<int64_t>(total_ctx, 1))) || (st = grow(V.ex, std::max<size_t>(ex.size(), 1))) ||
         (st = grow(V.slots, (size_t)n_users * n)) || (st = grow(V.scores, (size_t)n_users * n)) || (st = grow(V.count, (size_t)n_users)))
         return done(st);
-    const size_t sm_shared = aggregate_smem(n, true), sm_global = aggregate_smem(n, false);
+    const size_t sm_shared = agg::smem_bytes(n, true), sm_global = agg::smem_bytes(n, false);
     e = cudaFuncSetAttribute(i2i_aggregate_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm_shared);
     if (e == cudaSuccess) e = cudaFuncSetAttribute(i2i_aggregate_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm_global);
     if (e != cudaSuccess) { set_error("item_to_item: %s", cudaGetErrorString(e)); return done(GORSE_B200_ERR_CUDA); }

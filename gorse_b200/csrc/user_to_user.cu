@@ -1,0 +1,382 @@
+// user_to_user.cu -- batched user-to-user recommendation: gorse_b200_vecdb_user_to_user.
+//
+// The worker's user-to-user recommender (logics/recommend.go:285-348) asks, per user, QueryUserToUser(u, n)
+// (logics/user_to_user.go:50-86: top n + 1, drop u itself, drop Dot scores <= 0, stop at n), then for each similar user v
+// in that order adds v's score to every item of v's positive feedback that is not in the exclude set, in float64, keeps
+// the best n with TopKFilter and only then drops the items that are missing, hidden, too old or outside the categories.
+// Here one call answers many users:
+//
+//   stage A   the neighbour table, once per call: the distinct live query slots of the batch are searched once each, with
+//             the same stage A as item-to-item (item_to_item.cu): recall_rows with k = n and self-skip on dense
+//             collections, sparse_search_rows on sparse ones, and no category filter.
+//   routing   u2u_route_kernel, one thread per user: W_u = the feedback entries of u's neighbours; empty users are answered
+//             here, the rest go to the shared-memory list (W_u <= TABLE_KEYS) or the global-row list.
+//   stage B   u2u_aggregate_kernel, one CTA per user: walks the neighbours in table order with a barrier after each one;
+//             the threads split the neighbour's feedback row and add s_v with float64 atomics; then the first n by
+//             (sum desc, item asc) (agg::select_first_n), then the item filter as an ordered compaction.
+#include <algorithm>
+
+#include "aggregate.cuh"
+#include "sparse.cuh"
+#include "vecdb.cuh"
+
+namespace gb {
+namespace u2u {
+
+using agg::TABLE_CAP;
+using agg::TABLE_KEYS;                           // a user takes the table when W_u <= this
+constexpr int AGG_THREADS = agg::THREADS;
+constexpr int MAX_N_DENSE = 1024;                // the sort buffer holds n entries
+constexpr int MAX_N_SPARSE = 128;                // sparse_search_kernel's k
+
+struct Table {                // stage A: the first n neighbours of each distinct query user
+    const int32_t *slot;      // [rows x n]
+    const float *score;       // [rows x n] the vector store's score (dot, or the negated distance)
+    const int32_t *cnt;       // [rows]
+};
+
+struct Feedback {             // the caller's positive feedback per slot, as item indices
+    const int64_t *off;       // [rows + 1]
+    const int32_t *items;
+    int64_t rows;             // slots at or beyond have none
+};
+
+struct Users {                // one chunk of users (chunk-local ids)
+    const int32_t *q_row;     // [users] the neighbour-table row of each user, -1 = no vector
+    const int64_t *ex_off;    // [users + 1] into ex
+    const int64_t *ex;        // each user's excluded items, ascending (-1 entries dropped)
+    const uint8_t *item_ok;   // [n_items] or NULL
+    int64_t *items;           // [users x n]
+    double *scores;           // [users x n]
+    int32_t *count;           // [users]
+};
+
+struct Route {                // the device's routing of one chunk
+    int32_t *list;            // [users]: shared-memory users from the front, global-row users from the back
+    int32_t *cnt;             // [2]: how many of each
+    int32_t *work;            // [users] W_u
+    int64_t users;
+};
+
+// W_u for each user of the chunk.  Users without a vector, neighbours or feedback get an empty row here.
+__global__ void u2u_route_kernel(Users U, Table T, Feedback F, int n, Route R)
+{
+    const int64_t u = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (u >= R.users) return;
+    const int32_t r = U.q_row[u];
+    int64_t w = 0;
+    if (r >= 0)
+        for (int j = 0, cnt = T.cnt[r]; j < cnt; j++) {
+            const int32_t v = T.slot[(int64_t)r * n + j];
+            if (v < F.rows) w += F.off[v + 1] - F.off[v];
+        }
+    if (w == 0) {
+        U.count[u] = 0;
+        return;
+    }
+    if (w <= TABLE_KEYS) {
+        R.work[u] = (int32_t)w;
+        R.list[atomicAdd(&R.cnt[0], 1)] = (int32_t)u;
+    } else {
+        R.list[R.users - 1 - atomicAdd(&R.cnt[1], 1)] = (int32_t)u;
+    }
+}
+
+// one CTA per user of the routed list, a fixed grid looping over the device's count.  SHARED: the accumulator is a table in
+// shared memory; else acc_rows / flag_rows / touched_rows hold one [n_items] float64 row, one [n_items] flag row (all zero
+// between users) and one [n_items] item list per CTA.
+template <bool SHARED>
+__global__ void __launch_bounds__(AGG_THREADS)
+u2u_aggregate_kernel(Route R, Users U, Table T, Feedback F, int n, double scale, int euclid, int64_t n_items, double *acc_rows,
+                     int32_t *flag_rows, int32_t *touched_rows)
+{
+    using namespace gb::recall;
+    using namespace gb::agg;
+    constexpr int NT = AGG_THREADS;
+    extern __shared__ __align__(16) uint8_t sm[];
+    const int p2 = pow2_at_least(n);
+    const Smem S = carve(sm, p2);
+    double *acc = SHARED ? nullptr : acc_rows + (int64_t)blockIdx.x * n_items;
+    int32_t *flag = SHARED ? nullptr : flag_rows + (int64_t)blockIdx.x * n_items;
+    int32_t *touched = SHARED ? nullptr : touched_rows + (int64_t)blockIdx.x * n_items;
+    const int n_list = R.cnt[SHARED ? 0 : 1];
+    for (int64_t i = blockIdx.x; i < n_list; i += gridDim.x) {
+        const int64_t u = SHARED ? R.list[i] : R.list[R.users - 1 - i];
+        const int64_t r = U.q_row[u];
+        const int64_t *ex = U.ex + U.ex_off[u], n_ex = U.ex_off[u + 1] - U.ex_off[u];
+        int cap = 0, lg = 0;
+        if (SHARED) {   // a power of two >= 2 W_u, at most TABLE_CAP: the load stays <= 3/4
+            cap = min(TABLE_CAP, pow2_at_least(max(64, 2 * R.work[u])));
+            lg = __ffs(cap) - 1;
+            for (int j = threadIdx.x; j < cap; j += NT) {
+                S.t_key[j] = -1;
+                S.t_val[j] = 0.0;
+            }
+        }
+        if (threadIdx.x == 0) S.s_bc[3] = 0;
+        __syncthreads();
+        // The neighbours in order, one step each.  Every sum starts at +0.0, the Go map's zero value, and each add is an
+        // atomic float64 add, which rounds once like __dadd_rn.  Inside one step every add to an item adds the same s_v
+        // (one neighbour's row may hold an item twice), so the sequence of values an item's sum takes does not depend on
+        // the order of the atomics: the sum after the step is exactly the reference's sequential one.  The barrier after
+        // each step orders the steps, so every sum is formed in neighbour order, as the reference forms it.
+        for (int j = 0, cnt = T.cnt[r]; j < cnt; j++) {
+            const int32_t v = T.slot[r * n + j];
+            if (v >= F.rows) continue;   // no feedback: nothing to add, for every thread
+            const double s = neighbour_score(T.score[r * n + j], scale, euclid);
+            for (int64_t t = F.off[v] + threadIdx.x, e = F.off[v + 1]; t < e; t += NT) {
+                const int32_t item = F.items[t];
+                if (contains(ex, n_ex, (int64_t)item)) continue;
+                if (SHARED) {
+                    uint32_t h = ((uint32_t)item * 0x9E3779B1u) >> (32 - lg);
+                    for (;;) {
+                        const int32_t k = ((volatile int32_t *)S.t_key)[h];
+                        if (k == item) break;
+                        if (k < 0) {
+                            // a failed claim returns what the bucket now holds: another thread's claim for the same item
+                            // is this item's bucket; only another item's sends the probe on
+                            const int32_t old = atomicCAS(&S.t_key[h], -1, item);
+                            if (old == -1) atomicAdd(&S.s_bc[3], 1);
+                            if (old == -1 || old == item) break;
+                        }
+                        h = (h + 1) & (uint32_t)(cap - 1);
+                    }
+                    atomicAdd(&S.t_val[h], s);
+                } else {
+                    // the first thread to flip the flag lists the item; a plain flag store could list it twice
+                    if (atomicExch(&flag[item], 1) == 0) touched[atomicAdd(&S.s_bc[3], 1)] = item;
+                    atomicAdd(&acc[item], s);
+                }
+            }
+            __syncthreads();
+        }
+        const int distinct = S.s_bc[3];
+        auto item_at = [&](int64_t j) -> int32_t { return SHARED ? S.t_key[j] : touched[j]; };
+        auto val_at = [&](int64_t j) -> double { return SHARED ? S.t_val[j] : acc[touched[j]]; };
+        const int m = select_first_n<NT>(SHARED ? cap : distinct, distinct, n, p2, item_at, val_at, S);
+        // the item filter after the cut (the reference's BatchGetItems + categories check), keeping the order
+        int kept = 0;
+        for (int base = 0; base < m; base += NT) {
+            const int j = base + threadIdx.x;
+            const int32_t item = j < m ? (int32_t)(uint32_t)S.s_key[j] : 0;
+            const bool ok = j < m && (U.item_ok == nullptr || U.item_ok[item]);
+            int total;
+            const int pos = kept + block_rank<NT>(ok, S.s_warp, total);
+            if (ok) {
+                U.items[u * n + pos] = item;
+                U.scores[u * n + pos] = S.s_val[j];
+            }
+            kept += total;
+        }
+        if (threadIdx.x == 0) U.count[u] = kept;
+        if (!SHARED)
+            for (int j = threadIdx.x; j < distinct; j += NT) {
+                const int32_t item = touched[j];
+                flag[item] = 0;
+                acc[item] = 0.0;
+            }
+        __syncthreads();
+    }
+}
+
+}  // namespace u2u
+}  // namespace gb
+
+using namespace gb;
+
+extern "C" int32_t gorse_b200_vecdb_user_to_user(gorse_b200_vecdb *db, int64_t n_users, const int64_t *user_slots, int64_t n_fb_rows,
+                                                 const int64_t *fb_off, const int32_t *fb_items, int32_t n_items, const uint8_t *item_ok,
+                                                 const int64_t *excl_off, const int64_t *excl_items, int32_t n, double score_scale,
+                                                 int64_t *items_out, double *scores_out, int32_t *count_out, int64_t *stats_out)
+{
+    using namespace gb::u2u;
+    using gb::agg::grow_zeroed;
+    using gb::recall::grow;
+    GB_CHECK_ARG(db != nullptr, "collection is NULL");
+    GB_CHECK_ARG(n_users >= 0 && n_fb_rows >= 0 && n_items >= 0, "negative count");
+    if (stats_out) std::fill(stats_out, stats_out + 4, 0);
+    if (n_users == 0) return GORSE_B200_OK;
+    GB_CHECK_ARG(count_out != nullptr && user_slots != nullptr && excl_off != nullptr, "count_out / user_slots / excl_off is NULL");
+    GB_CHECK_ARG(n_fb_rows == 0 || fb_off != nullptr, "fb_off is NULL");
+    GB_CHECK_ARG(excl_off[0] == 0 && (n_fb_rows == 0 || fb_off[0] == 0), "fb_off[0] and excl_off[0] must be 0");
+    for (int64_t u = 0; u < n_users; u++)
+        GB_CHECK_ARG(excl_off[u + 1] >= excl_off[u], "excl_off not non-decreasing at %lld", (long long)u);
+    for (int64_t v = 0; v < n_fb_rows; v++)
+        GB_CHECK_ARG(fb_off[v + 1] >= fb_off[v], "fb_off not non-decreasing at %lld", (long long)v);
+    const int64_t n_fb = n_fb_rows ? fb_off[n_fb_rows] : 0;
+    GB_CHECK_ARG(n_fb == 0 || fb_items != nullptr, "fb_items is NULL");
+    GB_CHECK_ARG(excl_off[n_users] == 0 || excl_items != nullptr, "excl_items is NULL");
+    for (int64_t t = 0; t < n_fb; t++)
+        GB_CHECK_ARG(fb_items[t] >= 0 && fb_items[t] < n_items, "feedback entry %lld: item %d is not in [0, %d)", (long long)t, fb_items[t], n_items);
+    GB_CHECK_ARG(score_scale == score_scale, "score_scale is NaN");
+    if (db->distance == GORSE_B200_DISTANCE_COSINE) {
+        set_error("user-to-user collections are Dot or Euclidean");
+        return GORSE_B200_ERR_UNSUPPORTED;
+    }
+    if (n <= 0) {
+        for (int64_t u = 0; u < n_users; u++) count_out[u] = 0;
+        return GORSE_B200_OK;
+    }
+    const bool sparse = db->dim == 0;
+    if (n > (sparse ? MAX_N_SPARSE : MAX_N_DENSE)) {
+        set_error("user_to_user: n = %d above %d for a %s collection", n, sparse ? MAX_N_SPARSE : MAX_N_DENSE, sparse ? "sparse" : "dense");
+        return GORSE_B200_ERR_UNSUPPORTED;
+    }
+    GB_CHECK_ARG(items_out != nullptr && scores_out != nullptr, "NULL output");
+    std::lock_guard<std::mutex> lk(db->mu);
+    const int64_t n_slots = (int64_t)db->ts.size();
+    if (n_slots > INT32_MAX) { set_error("user_to_user: more than 2^31 slots"); return GORSE_B200_ERR_UNSUPPORTED; }
+    // each user's exclusions once, sorted, -1 entries dropped
+    std::vector<int64_t> ex, ex_off((size_t)n_users + 1, 0);
+    ex.reserve((size_t)excl_off[n_users]);
+    for (int64_t u = 0; u < n_users; u++) {
+        GB_CHECK_ARG(user_slots[u] >= -1 && user_slots[u] < n_slots, "user %lld: slot %lld is not a slot of the collection", (long long)u,
+                     (long long)user_slots[u]);
+        const size_t b = ex.size();
+        for (int64_t t = excl_off[u]; t < excl_off[u + 1]; t++) {
+            const int64_t s = excl_items[t];
+            GB_CHECK_ARG(s >= -1 && s < n_items, "user %lld: excluded item %lld is not in [-1, %d)", (long long)u, (long long)s, n_items);
+            if (s >= 0) ex.push_back(s);
+        }
+        std::sort(ex.begin() + b, ex.end());
+        for (size_t t = b + 1; t < ex.size(); t++)
+            GB_CHECK_ARG(ex[t] != ex[t - 1], "user %lld: item %lld is excluded twice", (long long)u, (long long)ex[t]);
+        ex_off[(size_t)u + 1] = (int64_t)ex.size();
+    }
+    // the live query slots as rows of the neighbour table, one row per distinct slot in first-visit order.  -1 and deleted
+    // slots have no row (GetVectors returns nothing, logics/user_to_user.go:55-58); hidden ones are searched.
+    std::vector<int32_t> row_of((size_t)n_slots, -1), q_row((size_t)n_users, -1);
+    std::vector<int64_t> nb;
+    for (int64_t u = 0; u < n_users; u++) {
+        const int64_t s = user_slots[u];
+        if (s < 0 || db->dead[(size_t)s]) continue;
+        if (row_of[(size_t)s] < 0) {
+            row_of[(size_t)s] = (int32_t)nb.size();
+            nb.push_back(s);
+        }
+        q_row[(size_t)u] = row_of[(size_t)s];
+    }
+    const int64_t R = (int64_t)nb.size();
+    if (R == 0) {
+        for (int64_t u = 0; u < n_users; u++) count_out[u] = 0;
+        return GORSE_B200_OK;
+    }
+    // the most any user can add: n neighbours with the longest feedback row.  Below the table's limit no user needs a
+    // global row, so none is allocated.
+    int64_t longest = 0;
+    for (int64_t v = 0; v < n_fb_rows; v++) longest = std::max(longest, fb_off[v + 1] - fb_off[v]);
+    const bool heavy_possible = longest * n > TABLE_KEYS;
+
+    gorse_b200_ctx *c = db->ctx;
+    ScopedDevice sd(c->device);
+    GB_TRY(vecdb_allow(db, nullptr, 0));
+    UserToUserWork &V = db->u2u;
+    int32_t st = GORSE_B200_OK;
+    auto done = [&](int32_t s) {
+        cudaStreamSynchronize(c->stream);
+        cudaStreamSynchronize(c->copy_stream);
+        return s;
+    };
+    if ((st = grow(V.nb, (size_t)R)) || (st = grow(V.t_slot, (size_t)R * n)) || (st = grow(V.t_score, (size_t)R * n)) || (st = grow(V.t_cnt, (size_t)R)))
+        return done(st);
+    cudaError_t e = cudaMemcpyAsync(V.nb.p, nb.data(), sizeof(int64_t) * R, cudaMemcpyHostToDevice, c->stream);
+    if (e != cudaSuccess) { set_error("user_to_user upload: %s", cudaGetErrorString(e)); return done(GORSE_B200_ERR_CUDA); }
+
+    // ---- stage A: the neighbour table
+    int64_t exact_rows = 0;
+    if (!sparse) {
+        std::lock_guard<std::mutex> lk2(db->dense->mu);
+        const recall::Table table{V.t_slot.p, V.t_score.p, V.t_cnt.p, false, db->distance == GORSE_B200_DISTANCE_DOT, nullptr, nullptr, nullptr};
+        if ((st = recall::recall_rows(db->dense, db->d_allow.p, R, nullptr, V.nb.p, n, nullptr, nullptr, nullptr, &table, nullptr, nullptr, nullptr,
+                                      &exact_rows)))
+            return done(st);
+    } else {
+        std::lock_guard<std::mutex> lk2(db->sparse->mu);
+        if ((st = sparse_search_rows(db->sparse, V.nb.p, R, db->d_allow.p, n, V.t_slot.p, V.t_score.p, V.t_cnt.p))) return done(st);
+    }
+    if ((e = cudaGetLastError()) != cudaSuccess) { set_error("user_to_user: %s", cudaGetErrorString(e)); return done(GORSE_B200_ERR_CUDA); }
+
+    // ---- the feedback rows and the item filter, once per call
+    const int64_t cu = std::min<int64_t>(n_users, (int64_t)c->sm_count * 1024);
+    const int64_t n_chunks = (n_users + cu - 1) / cu;
+    if ((st = grow(V.fb_off, (size_t)n_fb_rows + 1)) || (st = grow(V.fb_items, (size_t)std::max<int64_t>(n_fb, 1))) ||
+        (st = grow(V.item_ok, (size_t)std::max<int32_t>(n_items, 1))) || (st = grow(V.q_row, (size_t)cu)) ||
+        (st = grow(V.ex_off, (size_t)cu + 1)) || (st = grow(V.ex, std::max<size_t>(ex.size(), 1))) || (st = grow(V.list, (size_t)cu)) ||
+        (st = grow(V.work, (size_t)cu)) || (st = grow(V.route_cnt, (size_t)n_chunks * 2)) || (st = grow(V.items, (size_t)n_users * n)) ||
+        (st = grow(V.scores, (size_t)n_users * n)) || (st = grow(V.count, (size_t)n_users)))
+        return done(st);
+    if ((n_fb_rows && (e = cudaMemcpyAsync(V.fb_off.p, fb_off, sizeof(int64_t) * (n_fb_rows + 1), cudaMemcpyHostToDevice, c->stream)) != cudaSuccess) ||
+        (n_fb && (e = cudaMemcpyAsync(V.fb_items.p, fb_items, sizeof(int32_t) * n_fb, cudaMemcpyHostToDevice, c->stream)) != cudaSuccess) ||
+        (item_ok && n_items && (e = cudaMemcpyAsync(V.item_ok.p, item_ok, n_items, cudaMemcpyHostToDevice, c->stream)) != cudaSuccess) ||
+        (e = cudaMemsetAsync(V.route_cnt.p, 0, sizeof(int32_t) * n_chunks * 2, c->stream)) != cudaSuccess) {
+        set_error("user_to_user upload: %s", cudaGetErrorString(e));
+        return done(GORSE_B200_ERR_CUDA);
+    }
+
+    // ---- routing and stage B: users in chunks; a finished chunk is downloaded on the copy stream while the next one computes
+    // global accumulators: one [n_items] float64 row, flag row and item list per CTA, at most 512 MB
+    const int64_t NI = std::max<int64_t>(n_items, 1);
+    const int heavy_grid = (int)std::max<int64_t>(1, std::min<int64_t>((int64_t)c->sm_count * 2, (512ll << 20) / (16 * NI)));
+    if (heavy_possible && ((st = grow_zeroed(V.acc, (size_t)heavy_grid * NI, c->stream)) || (st = grow_zeroed(V.flag, (size_t)heavy_grid * NI, c->stream)) ||
+                           (st = grow(V.touched, (size_t)heavy_grid * NI))))
+        return done(st);
+    const size_t sm_shared = agg::smem_bytes(n, true), sm_global = agg::smem_bytes(n, false);
+    e = cudaFuncSetAttribute(u2u_aggregate_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm_shared);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(u2u_aggregate_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm_global);
+    if (e != cudaSuccess) { set_error("user_to_user: %s", cudaGetErrorString(e)); return done(GORSE_B200_ERR_CUDA); }
+    Table T;
+    T.slot = V.t_slot.p; T.score = V.t_score.p; T.cnt = V.t_cnt.p;
+    Feedback F;
+    F.off = V.fb_off.p; F.items = V.fb_items.p; F.rows = n_fb_rows;
+    const bool euclid = db->distance == GORSE_B200_DISTANCE_EUCLIDEAN;
+    std::vector<int64_t> h_exoff;
+    for (int64_t ci = 0, u0 = 0; u0 < n_users; ci++, u0 += cu) {
+        const int64_t rows = std::min(cu, n_users - u0);
+        h_exoff.resize(rows + 1);
+        for (int64_t r = 0; r <= rows; r++) h_exoff[r] = ex_off[u0 + r] - ex_off[u0];
+        const int64_t n_e = h_exoff[rows];
+        if ((e = cudaMemcpyAsync(V.q_row.p, q_row.data() + u0, sizeof(int32_t) * rows, cudaMemcpyHostToDevice, c->stream)) != cudaSuccess ||
+            (e = cudaMemcpyAsync(V.ex_off.p, h_exoff.data(), sizeof(int64_t) * (rows + 1), cudaMemcpyHostToDevice, c->stream)) != cudaSuccess ||
+            (n_e && (e = cudaMemcpyAsync(V.ex.p + ex_off[u0], ex.data() + ex_off[u0], sizeof(int64_t) * n_e, cudaMemcpyHostToDevice, c->stream)) != cudaSuccess)) {
+            set_error("user_to_user upload: %s", cudaGetErrorString(e));
+            return done(GORSE_B200_ERR_CUDA);
+        }
+        Users U;
+        U.q_row = V.q_row.p; U.ex_off = V.ex_off.p; U.ex = V.ex.p + ex_off[u0]; U.item_ok = item_ok ? V.item_ok.p : nullptr;
+        U.items = V.items.p + u0 * n; U.scores = V.scores.p + u0 * n; U.count = V.count.p + u0;
+        Route Rt;
+        Rt.list = V.list.p; Rt.cnt = V.route_cnt.p + 2 * ci; Rt.work = V.work.p; Rt.users = rows;
+        u2u_route_kernel<<<(unsigned)((rows + 255) / 256), 256, 0, c->stream>>>(U, T, F, n, Rt);
+        u2u_aggregate_kernel<true><<<(unsigned)std::min<int64_t>(rows, (int64_t)c->sm_count * 8), AGG_THREADS, sm_shared, c->stream>>>(
+            Rt, U, T, F, n, score_scale, euclid, NI, nullptr, nullptr, nullptr);
+        c->launches += 2;
+        if (heavy_possible) {
+            u2u_aggregate_kernel<false><<<(unsigned)std::min<int64_t>(rows, heavy_grid), AGG_THREADS, sm_global, c->stream>>>(
+                Rt, U, T, F, n, score_scale, euclid, NI, V.acc.p, V.flag.p, V.touched.p);
+            c->launches++;
+        }
+        if ((e = cudaGetLastError()) != cudaSuccess) { set_error("user_to_user: %s", cudaGetErrorString(e)); return done(GORSE_B200_ERR_CUDA); }
+        if ((e = cudaEventRecord(c->copy_ev, c->stream)) != cudaSuccess || (e = cudaStreamWaitEvent(c->copy_stream, c->copy_ev, 0)) != cudaSuccess ||
+            (e = cudaMemcpyAsync(count_out + u0, V.count.p + u0, sizeof(int32_t) * rows, cudaMemcpyDeviceToHost, c->copy_stream)) != cudaSuccess ||
+            (e = cudaMemcpyAsync(items_out + u0 * n, V.items.p + u0 * n, sizeof(int64_t) * rows * n, cudaMemcpyDeviceToHost, c->copy_stream)) != cudaSuccess ||
+            (e = cudaMemcpyAsync(scores_out + u0 * n, V.scores.p + u0 * n, sizeof(double) * rows * n, cudaMemcpyDeviceToHost, c->copy_stream)) != cudaSuccess) {
+            set_error("user_to_user download: %s", cudaGetErrorString(e));
+            return done(GORSE_B200_ERR_CUDA);
+        }
+    }
+    std::vector<int32_t> routed((size_t)n_chunks * 2);
+    if ((e = cudaMemcpyAsync(routed.data(), V.route_cnt.p, sizeof(int32_t) * n_chunks * 2, cudaMemcpyDeviceToHost, c->stream)) != cudaSuccess ||
+        (e = cudaStreamSynchronize(c->stream)) != cudaSuccess || (e = cudaStreamSynchronize(c->copy_stream)) != cudaSuccess) {
+        set_error("user_to_user: %s", cudaGetErrorString(e));
+        return done(GORSE_B200_ERR_CUDA);
+    }
+    if (stats_out) {
+        stats_out[0] = R;
+        stats_out[1] = exact_rows;
+        for (int64_t ci = 0; ci < n_chunks; ci++) {
+            stats_out[2] += routed[(size_t)ci * 2];
+            stats_out[3] += routed[(size_t)ci * 2 + 1];
+        }
+    }
+    return done(GORSE_B200_OK);
+}

@@ -130,6 +130,7 @@ int32_t gorse_b200_vecdb_destroy(gorse_b200_vecdb *db)
         cudaStreamSynchronize(db->ctx->stream);
         db->d_blocked.free(); db->d_allow.free(); db->d_cat_off.free(); db->d_cats.free(); db->d_want.free();
         db->i2i.free();
+        db->u2u.free();
     }
     gorse_b200_index_destroy(db->dense);
     gorse_b200_sparse_index_destroy(db->sparse);

@@ -1,4 +1,5 @@
-// vecdb.cuh -- state of one vector collection (vecdb.cu), shared with the batched recall (recall.cu) and item-to-item.
+// vecdb.cuh -- state of one vector collection (vecdb.cu), shared with the batched recall (recall.cu), item-to-item and
+// user-to-user.
 #pragma once
 #include "topk.cuh"
 
@@ -17,6 +18,22 @@ struct ItemToItemWork {
         nb.free(); c_off.free(); ex_off.free(); ex.free(); slots.free();
         t_slot.free(); t_cnt.free(); c_row.free(); users.free(); count.free();
         t_score.free(); scores.free(); acc.free(); seen.free(); touched.free();
+    }
+};
+
+// grow-only work buffers of gorse_b200_vecdb_user_to_user (user_to_user.cu): the neighbour table of stage A, the caller's
+// feedback rows and item filter, the user chunks, their routing and answers, and the global-row accumulators of stage B
+struct UserToUserWork {
+    DevBuf<int64_t> nb, fb_off, ex_off, ex, items;
+    DevBuf<int32_t> t_slot, t_cnt, fb_items, q_row, list, work, route_cnt, count, flag, touched;
+    DevBuf<uint8_t> item_ok;
+    DevBuf<float> t_score;
+    DevBuf<double> scores, acc;
+    void free()
+    {
+        nb.free(); fb_off.free(); ex_off.free(); ex.free(); items.free();
+        t_slot.free(); t_cnt.free(); fb_items.free(); q_row.free(); list.free(); work.free(); route_cnt.free(); count.free(); flag.free(); touched.free();
+        item_ok.free(); t_score.free(); scores.free(); acc.free();
     }
 };
 }  // namespace gb
@@ -38,6 +55,7 @@ struct gorse_b200_vecdb {
     gb::DevBuf<int64_t> d_cat_off;
     gb::DevBuf<int32_t> d_cats, d_want;
     gb::ItemToItemWork i2i;  // batched item-to-item recommendation (item_to_item.cu)
+    gb::UserToUserWork u2u;  // batched user-to-user recommendation (user_to_user.cu)
 };
 
 namespace gb {

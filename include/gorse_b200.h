@@ -400,6 +400,37 @@ int32_t gorse_b200_vecdb_item_to_item(gorse_b200_vecdb *db, int64_t n_users, con
                                       const int64_t *excl_off, const int64_t *excl_slots, const int32_t *categories, int32_t n_categories,
                                       int32_t n, double score_scale, int64_t *slots_out, double *scores_out, int32_t *count_out,
                                       int64_t *stats_out);
+/* Batched user-to-user recommendation: for n_users users at once, what the worker's user-to-user recommender does per user
+ * (Recommender.recommendUserToUser, logics/recommend.go:285-348) on one user-to-user collection: Euclidean for type
+ * "embedding", sparse Dot for "tags" / "items" / "auto" (a dense Dot collection follows the Dot rules).
+ *   user_slots[u]: the user's slot, or -1 for a user without a vector; -1 and deleted slots give an empty row, a hidden user
+ *   is still queried, a slot may repeat.  A slot outside [-1, slots) is GORSE_B200_ERR_ARG.
+ *   Neighbours of u: the live, not hidden vectors other than u (no category filter) by score descending, exact ties by lower
+ *   slot; Dot collections drop scores <= 0; the first n (QueryUserToUser, logics/user_to_user.go:50-86).  Their scores are
+ *   bit-identical to gorse_b200_vecdb_query's.  Neighbour score s = (double)score * score_scale (0.5 for type "auto",
+ *   else 1); Euclidean: s = 1 / (1 - s).
+ *   Feedback: fb_off[n_fb_rows + 1] (fb_off[0] = 0; may be NULL when n_fb_rows = 0) / fb_items: each slot's positive
+ *   feedback as item indices in [0, n_items) of the caller's item dictionary; slots at or beyond n_fb_rows have none.  A row
+ *   may repeat an item (it is then added again); the order within a row does not matter.
+ *   E_u = excl_items[excl_off[u] .. excl_off[u+1]) (excl_off[0] = 0): the user's exclude set as item indices, -1 for an id
+ *   outside the dictionary; an item twice in one row is GORSE_B200_ERR_ARG.
+ *   item_ok[n_items] (may be NULL = every item passes): 1 for the items that exist, are not hidden, are within the TTL and
+ *   hold all of the requested categories; the same filter for every user of the call.
+ *   Row u: for every neighbour in order and every feedback entry of it not in E_u, acc[item] += s in float64 (each sum
+ *   starting at 0 + s); the first n by (sum descending, item ascending); then the entries with item_ok = 0 are dropped,
+ *   keeping the order, so a row may hold fewer than n.  Each sum is formed in neighbour order, as the reference's, so the
+ *   scores match it bit for bit.  The reference ranks exact ties in Go map order, so which of them it keeps at the cut is
+ *   unpinned.
+ *   Output: row u at u*n in items_out / scores_out (buffers of n_users*n), count_out[u] <= n entries.  n <= 0: every count
+ *   is 0.  n above 128 (sparse) or 1024 (dense): GORSE_B200_ERR_UNSUPPORTED; Cosine collections: GORSE_B200_ERR_UNSUPPORTED.
+ *   A NaN score (or score_scale): GORSE_B200_ERR_ARG.  Every argument, each fb_items entry included, is checked before the
+ *   device is touched.  stats_out[4] (may be NULL): distinct query users searched, of them answered by the exact scan
+ *   rather than the tensor-core sweep (dense), users aggregated in shared memory, users aggregated in a global-memory row
+ *   (users with nothing to add are in neither); the answer does not depend on them.  Thread-safe per collection. */
+int32_t gorse_b200_vecdb_user_to_user(gorse_b200_vecdb *db, int64_t n_users, const int64_t *user_slots, int64_t n_fb_rows,
+                                      const int64_t *fb_off, const int32_t *fb_items, int32_t n_items, const uint8_t *item_ok,
+                                      const int64_t *excl_off, const int64_t *excl_items, int32_t n, double score_scale,
+                                      int64_t *items_out, double *scores_out, int32_t *count_out, int64_t *stats_out);
 
 /* ------------------------------------------------------------------------------------------
  * NCF-format datasets: dataset.LoadDataFromBuiltIn (dataset/dataset.go:398-490), the loader `gorse-bench cf`
