@@ -536,6 +536,77 @@ class VectorCollection:
         self.close()
 
 
+class FMInput:
+    """The factored input of gorse_b200_fm_rank, packed from Python lists.
+    user_feat[u]: the user-id feature or -1; user_labels[u]: [(feature, scaled value)] in label order.
+    item_feat / item_labels: the same per row of the call's item table.  item_emb[s]: uint16 (bf16 bits) [n_items, dim_s];
+    item_emb_mask: uint8 [n_items, n_emb] (None: all present).  candidates[u]: item-table rows of user u."""
+
+    def __init__(self, user_feat, user_labels, item_feat, item_labels, candidates, item_emb=(), item_emb_mask=None):
+        def csr(rows):
+            off = np.zeros(len(rows) + 1, np.int64)
+            np.cumsum([len(r) for r in rows], out=off[1:])
+            idx = np.ascontiguousarray([f for r in rows for f, _ in r] or [0], np.int32)
+            val = np.ascontiguousarray([v for r in rows for _, v in r] or [0], np.float32)
+            return off, idx, val
+
+        self.user_feat = np.ascontiguousarray(user_feat, np.int32).reshape(-1)
+        self.item_feat = np.ascontiguousarray(item_feat, np.int32).reshape(-1)
+        self.n_users, self.n_items = self.user_feat.size, self.item_feat.size
+        if len(user_labels) != self.n_users or len(candidates) != self.n_users or len(item_labels) != self.n_items:
+            raise ValueError("one label list per user / item and one candidate list per user")
+        self.user_lab_off, self.user_lab_idx, self.user_lab_val = csr(user_labels)
+        self.item_lab_off, self.item_lab_idx, self.item_lab_val = csr(item_labels)
+        self.cand_off = np.zeros(self.n_users + 1, np.int64)
+        np.cumsum([len(c) for c in candidates], out=self.cand_off[1:])
+        self.cand_items = np.ascontiguousarray(np.concatenate([np.asarray(c, np.int32).reshape(-1) for c in candidates] + [np.zeros(1, np.int32)]),
+                                               np.int32)
+        self.item_emb = [np.ascontiguousarray(e, np.uint16) for e in item_emb]
+        self.item_emb_mask = None if item_emb_mask is None else np.ascontiguousarray(item_emb_mask, np.uint8)
+
+    def split(self, scores, order):
+        """per-user lists of (scores, order) from flat outputs"""
+        return [(scores[a:b], order[a:b]) for a, b in zip(self.cand_off[:-1], self.cand_off[1:])]
+
+
+class FMRanker:
+    """A trained factorization machine on the GPU (gorse_b200_fm_*; model/ctr/fm.go AFM inference).  params: fm.Parameters()
+    concatenated (B, V, W, then H, AW, Ab, EW, Eb per embedding slot)."""
+
+    def __init__(self, ctx, n_features, n_factors, num_dimension, batch_size=1024, emb_dims=(), params=None):
+        self.ctx, self.n_factors = ctx, int(n_factors)
+        dims = np.ascontiguousarray(list(emb_dims) or [0], np.int32)
+        self.n_emb = len(list(emb_dims))
+        p = np.ascontiguousarray(params, np.float32).reshape(-1)
+        h = C.c_void_p()
+        check(lib.gorse_b200_fm_create(ctx.h, int(n_features), int(n_factors), int(num_dimension), int(batch_size), self.n_emb, ptr(dims),
+                                       ptr(p), p.size, C.byref(h)))
+        self.h = h
+
+    def close(self):
+        if self.h:
+            lib.gorse_b200_fm_destroy(self.h)
+            self.h = None
+
+    def rank(self, inp):
+        """-> (scores float32 [pairs] in candidate order, order int32 [pairs]: each user's candidate positions by score
+        descending, ties by position, NaN last; stats {pairs, chunks, passes, global_sorts})"""
+        total = int(inp.cand_off[-1])
+        scores, order, stats = np.zeros(max(total, 1), np.float32), np.zeros(max(total, 1), np.int32), np.zeros(4, np.int64)
+        embs = (C.c_void_p * max(self.n_emb, 1))(*[ptr(e) for e in inp.item_emb])
+        check(lib.gorse_b200_fm_rank(self.h, inp.n_users, ptr(inp.user_feat), ptr(inp.user_lab_off), ptr(inp.user_lab_idx), ptr(inp.user_lab_val),
+                                     inp.n_items, ptr(inp.item_feat), ptr(inp.item_lab_off), ptr(inp.item_lab_idx), ptr(inp.item_lab_val),
+                                     C.cast(embs, C.c_void_p) if inp.item_emb else None, ptr(inp.item_emb_mask), ptr(inp.cand_off),
+                                     ptr(inp.cand_items), ptr(scores), ptr(order), ptr(stats)))
+        return scores[:total], order[:total], dict(zip(("pairs", "chunks", "passes", "global_sorts"), (int(x) for x in stats)))
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *a):
+        self.close()
+
+
 def load_ncf(train_path, test_path=None):
     """dataset.LoadDataFromBuiltIn's NCF parsers (dataset/dataset.go:398-490) ->
     (n_users, n_items, (train_off, train_items), (test_off, test_items), (neg_off, neg_items))."""

@@ -433,6 +433,43 @@ int32_t gorse_b200_vecdb_user_to_user(gorse_b200_vecdb *db, int64_t n_users, con
                                       int64_t *items_out, double *scores_out, int32_t *count_out, int64_t *stats_out);
 
 /* ------------------------------------------------------------------------------------------
+ * Batched FM ranking: the worker's "fm" ranker (rankByClickTroughRate, worker/pipeline.go:450-499) for many users in one
+ * call -- AFM.BatchPredict (model/ctr/fm.go:180-229) on every (user, candidate) pair of each user, then the candidates by
+ * score.  Inference only; training (AFM.Fit) stays in the reference.
+ * gorse_b200_fm_create uploads one trained model once; the handle is read-only afterwards and thread-safe.
+ *   n_features = fm.numFeatures (the unified index's Len), n_factors = nFactors, num_dimension = fm.numDimension,
+ *   batch_size = the BatchSize param (default 1024), emb_dim[n_emb] = fm.embeddingDim.
+ *   params[n_params]: fm.Parameters() (fm.go:136-146) concatenated in order: B[1], V[n_features x n_factors],
+ *   W[n_features], then per slot H[n_factors x dim], AW[dim x n_factors], Ab[n_factors], EW[dim x n_factors],
+ *   Eb[n_factors].  A wrong n_params is GORSE_B200_ERR_ARG.  n_factors above 32, an embedding dim above 1024 or more than 8
+ *   slots: GORSE_B200_ERR_UNSUPPORTED.
+ * gorse_b200_fm_rank takes the pairs factored, as the reference builds them once per user and once per item:
+ *   users: user_feat[n_users] (fm.Index.EncodeUser, -1 = unknown) and the known labels as a CSR user_lab_off[n_users + 1]
+ *   (from 0) / user_lab_idx / user_lab_val, in label order, values already through fm.Scalers (applyScalers, fm.go:232-245).
+ *   item table of the call: item_feat[n_items], item_lab_off / item_lab_idx / item_lab_val the same way; item_emb[s]
+ *   [n_items x emb_dim[s]] bf16 bits per slot, item_emb_mask[n_items x n_emb] 1 where the item's embedding of slot s is
+ *   present with the right length (NULL: all present); an absent one is zeros (convertToTensors, fm.go:555-561).
+ *   candidates: cand_off[n_users + 1] (from 0) / cand_items, rows of the item table, repeats allowed.
+ *   Row of pair (u, i): user id (value 1), item id (value 1), user labels, item labels; padded to
+ *   D_u = max(num_dimension, the user's longest row) with index 0, value 0; indices travel as float32; chunks of
+ *   batch_size pairs in candidate order; the softmax of a chunk couples its rows as the reference's does (DESIGN §8.4).
+ *   Output: scores_out[cand_off[n_users]] float32 in candidate order, bit-identical to the reference's restatement;
+ *   order_out[cand_off[n_users]]: per user, the candidate positions (0-based within the user) by score descending, exact
+ *   ties (-0 == +0) by position, NaN last.  The reference's sort (cache.SortDocuments) is not stable, so its order on ties is
+ *   unpinned.  stats_out[4] (may be NULL): pairs, attention chunks, device passes, users sorted in global memory.
+ *   Every index is checked on the host before the device is touched (GORSE_B200_ERR_ARG): a feature outside
+ *   [0, n_features) -- also after rounding to float32 -- an item row outside the table, decreasing offsets. */
+typedef struct gorse_b200_fm gorse_b200_fm;
+int32_t gorse_b200_fm_create(gorse_b200_ctx *ctx, int64_t n_features, int32_t n_factors, int32_t num_dimension, int32_t batch_size,
+                             int32_t n_emb, const int32_t *emb_dim, const float *params, int64_t n_params, gorse_b200_fm **out);
+int32_t gorse_b200_fm_destroy(gorse_b200_fm *fm);
+int32_t gorse_b200_fm_rank(gorse_b200_fm *fm, int64_t n_users, const int32_t *user_feat, const int64_t *user_lab_off,
+                           const int32_t *user_lab_idx, const float *user_lab_val, int64_t n_items, const int32_t *item_feat,
+                           const int64_t *item_lab_off, const int32_t *item_lab_idx, const float *item_lab_val,
+                           const uint16_t *const *item_emb, const uint8_t *item_emb_mask, const int64_t *cand_off,
+                           const int32_t *cand_items, float *scores_out, int32_t *order_out, int64_t *stats_out);
+
+/* ------------------------------------------------------------------------------------------
  * NCF-format datasets: dataset.LoadDataFromBuiltIn (dataset/dataset.go:398-490), the loader `gorse-bench cf`
  * (gorse_b200/csrc/gorse_bench_cf.cpp; BASELINE configs[0]) feeds the model with.  Host code.
  *   train file  "user<TAB>item[<TAB>...]" per line (loadTrain :420-453)
