@@ -31,7 +31,7 @@ __device__ __forceinline__ void red_row(float *p, float4 v)
 }
 
 
-#define GB_BPR_ROUND 8192   // triples per round of the atomic-scatter epoch (bpr_round_kernel)
+#define GB_BPR_ROUND 8192   // triples per round of the atomic-scatter epoch (bpr_round_kernel, bpr_round_delta_*_kernel)
 
 #define GB_F4_OP(dst, expr)                            \
     do {                                               \
@@ -209,7 +209,8 @@ __device__ __forceinline__ void sample_triple(const BprView &v, uint64_t base, i
 }
 
 // ---- kernels -----------------------------------------------------------------------------------
-template <int C, bool ATOMIC>
+// The store-scatter epoch, free-running: every triple reads its rows whenever it runs and stores what it computed.
+template <int C>
 __global__ void __launch_bounds__(256) bpr_epoch_kernel(BprView v, int64_t step0, int64_t n_steps, uint64_t base, float lr, float reg)
 {
     const int lane4 = threadIdx.x & 3;
@@ -231,7 +232,7 @@ __global__ void __launch_bounds__(256) bpr_epoch_kernel(BprView v, int64_t step0
             const int64_t qn = q + nq;
             int32_t un = 0, in = 0, jn = -1;
             if (qn < n_steps) sample_triple(v, base, step0 + qn, un, in, jn);
-            if (live) bpr_step_rows<CC, ATOMIC>(r, Pu, Qi, 16, Qj, 16, mask, lr, reg);
+            if (live) bpr_step_rows<CC, false>(r, Pu, Qi, 16, Qj, 16, mask, lr, reg);
             q = qn; u = un; i = in; j = jn;
         }
     } else {
@@ -239,8 +240,8 @@ __global__ void __launch_bounds__(256) bpr_epoch_kernel(BprView v, int64_t step0
             int32_t u, i, j;
             sample_triple(v, base, step0 + q, u, i, j);
             if (j < 0) continue;
-            bpr_step_dispatch<C, ATOMIC>(v.P + (int64_t)(u - v.u_lo) * v.d, v.Q + (int64_t)i * v.d, v.Q + (int64_t)j * v.d,
-                                         v.d, lane4, mask, lr, reg);
+            bpr_step_dispatch<C, false>(v.P + (int64_t)(u - v.u_lo) * v.d, v.Q + (int64_t)i * v.d, v.Q + (int64_t)j * v.d,
+                                        v.d, lane4, mask, lr, reg);
         }
     }
 }
@@ -431,7 +432,7 @@ __global__ void __launch_bounds__(256) bpr_apply_kernel(BprView v, const int32_t
     }
 }
 
-template <bool ATOMIC>
+// the store-scatter epoch for d % 16 != 0, free-running like bpr_epoch_kernel
 __global__ void __launch_bounds__(128) bpr_epoch_any_kernel(BprView v, int64_t step0, int64_t n_steps, uint64_t base, float lr, float reg)
 {
     int64_t q = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -440,8 +441,99 @@ __global__ void __launch_bounds__(128) bpr_epoch_any_kernel(BprView v, int64_t s
         int32_t u, i, j;
         sample_triple(v, base, step0 + q, u, i, j);
         if (j < 0) continue;
-        bpr_step_any<ATOMIC>(v.P + (int64_t)(u - v.u_lo) * v.d, v.Q + (int64_t)i * v.d, v.Q + (int64_t)j * v.d, v.d, lr, reg);
+        bpr_step_any<false>(v.P + (int64_t)(u - v.u_lo) * v.d, v.Q + (int64_t)i * v.d, v.Q + (int64_t)j * v.d, v.d, lr, reg);
     }
+}
+
+// ---- the round epoch at the other d: two stream-ordered launches per round ---------------------------------------------
+// bpr_round_kernel keeps a CTA's rows in registers and its item deltas in shared memory, which bounds it to d = 16...128.
+// At any other d a round is a delta launch, in which each triple of the round reads its rows and writes lr * t for its three
+// rows into a buffer, then an add launch, which adds the buffer into the rows.  Stream order puts every read of round r
+// after every addition of round r - 1 and before any addition of round r: the same semantics as bpr_round_kernel.
+// Buffer layout: entry e = role * GB_BPR_ROUND + t of triple t (role 0: its user row, 1: q_i, 2: q_j) is the d floats at
+// delta + e * d, added to P or Q row rows[e] (a row of the shard's P for role 0); rows[e] = -1 for no addition.
+
+// one quad per triple, d % 16 == 0: the arithmetic of bpr_step_quad_dyn
+__global__ void __launch_bounds__(256) bpr_round_delta_quad_kernel(BprView v, int64_t step0, int64_t n_steps, uint64_t base,
+                                                                   float lr, float reg, float *delta, int32_t *rows)
+{
+    const int lane4 = threadIdx.x & 3;
+    const unsigned mask = quad_mask();
+    const int t = (int)(((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 2);
+    int32_t u = v.u_lo, i = -1, j = -1;
+    if (t < n_steps) sample_triple(v, base, step0 + t, u, i, j);
+    const bool live = j >= 0;
+    if (lane4 == 0) {
+        rows[t] = live ? u - v.u_lo : -1;
+        rows[GB_BPR_ROUND + t] = live ? i : -1;
+        rows[2 * GB_BPR_ROUND + t] = live ? j : -1;
+    }
+    if (!live) return;   // the whole quad leaves together
+    const int d = v.d, chunks = d / 16;
+    const float4 *Pu = reinterpret_cast<const float4 *>(v.P + (int64_t)(u - v.u_lo) * d) + lane4;
+    const float4 *Qi = reinterpret_cast<const float4 *>(v.Q + (int64_t)i * d) + lane4;
+    const float4 *Qj = reinterpret_cast<const float4 *>(v.Q + (int64_t)j * d) + lane4;
+    // nothing writes the tables during this launch, so the rows may come through L1 (the second pass re-reads them)
+    float4 ai = make_float4(0.f, 0.f, 0.f, 0.f), aj = ai;
+    for (int c = 0; c < chunks; c++) {
+        const float4 p = __ldg(Pu + 4 * c);
+        dot_chunk(ai, p, __ldg(Qi + 4 * c), c == 0);
+        dot_chunk(aj, p, __ldg(Qj + 4 * c), c == 0);
+    }
+    const float g = bpr_grad(__fsub_rn(quad_tree(ai, mask), quad_tree(aj, mask))), ng = -g, nreg = -reg;
+    float4 *Dp = reinterpret_cast<float4 *>(delta + (int64_t)t * d) + lane4;
+    float4 *Di = reinterpret_cast<float4 *>(delta + (int64_t)(GB_BPR_ROUND + t) * d) + lane4;
+    float4 *Dj = reinterpret_cast<float4 *>(delta + (int64_t)(2 * GB_BPR_ROUND + t) * d) + lane4;
+    for (int c = 0; c < chunks; c++) {
+        const float4 p = __ldg(Pu + 4 * c), qi = __ldg(Qi + 4 * c), qj = __ldg(Qj + 4 * c);
+        float4 tt, o;
+        GB_F4_OP(tt, __fmaf_rn(f4get(qi, k_), nreg, __fmul_rn(g, f4get(p, k_))));
+        GB_F4_OP(o, __fmul_rn(f4get(tt, k_), lr)); Di[4 * c] = o;
+        GB_F4_OP(tt, __fmaf_rn(f4get(qj, k_), nreg, __fmul_rn(ng, f4get(p, k_))));
+        GB_F4_OP(o, __fmul_rn(f4get(tt, k_), lr)); Dj[4 * c] = o;
+        GB_F4_OP(tt, __fmaf_rn(f4get(p, k_), nreg, __fmul_rn(__fsub_rn(f4get(qi, k_), f4get(qj, k_)), g)));
+        GB_F4_OP(o, __fmul_rn(f4get(tt, k_), lr)); Dp[4 * c] = o;
+    }
+}
+
+// one thread per triple, any d: the arithmetic of bpr_step_any
+__global__ void __launch_bounds__(64) bpr_round_delta_any_kernel(BprView v, int64_t step0, int64_t n_steps, uint64_t base,
+                                                                 float lr, float reg, float *delta, int32_t *rows)
+{
+    const int t = blockIdx.x * blockDim.x + threadIdx.x;
+    int32_t u = v.u_lo, i = -1, j = -1;
+    if (t < n_steps) sample_triple(v, base, step0 + t, u, i, j);
+    const bool live = j >= 0;
+    rows[t] = live ? u - v.u_lo : -1;
+    rows[GB_BPR_ROUND + t] = live ? i : -1;
+    rows[2 * GB_BPR_ROUND + t] = live ? j : -1;
+    if (!live) return;
+    const int d = v.d;
+    const float *Pu = v.P + (int64_t)(u - v.u_lo) * d, *Qi = v.Q + (int64_t)i * d, *Qj = v.Q + (int64_t)j * d;
+    float *Dp = delta + (int64_t)t * d, *Di = delta + (int64_t)(GB_BPR_ROUND + t) * d,
+          *Dj = delta + (int64_t)(2 * GB_BPR_ROUND + t) * d;
+    const float g = bpr_grad(__fsub_rn(dot_any(Pu, Qi, d), dot_any(Pu, Qj, d))), ng = -g, nreg = -reg;
+    for (int k = 0; k < d; k++) {
+        const float p = Pu[k], qi = Qi[k], qj = Qj[k];
+        Di[k] = __fmul_rn(axpy_elem(qi, nreg, __fmul_rn(p, g), k, d), lr);
+        Dj[k] = __fmul_rn(axpy_elem(qj, nreg, __fmul_rn(p, ng), k, d), lr);
+        Dp[k] = __fmul_rn(axpy_elem(p, nreg, __fmul_rn(__fsub_rn(qi, qj), g), k, d), lr);
+    }
+}
+
+// adds the round's deltas into the rows: one thread per float4 of an entry when d % 4 == 0, per float otherwise
+template <bool V4>
+__global__ void __launch_bounds__(256) bpr_round_add_kernel(float *P, float *Q, int d, const float *delta, const int32_t *rows)
+{
+    const int per = V4 ? d / 4 : d;
+    const int64_t x = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (x >= (int64_t)3 * GB_BPR_ROUND * per) return;
+    const int e = (int)(x / per), k = (int)(x % per);
+    const int32_t r = __ldg(rows + e);
+    if (r < 0) return;
+    float *row = (e < GB_BPR_ROUND ? P : Q) + (int64_t)r * d;
+    if (V4) red_row(row + 4 * k, __ldg(reinterpret_cast<const float4 *>(delta + (int64_t)e * d) + k));
+    else atomicAdd(row + k, __ldg(delta + (int64_t)e * d + k));
 }
 
 template <bool ATOMIC>
@@ -583,8 +675,32 @@ static int32_t launch_round_epoch(gorse_b200_cf *cf, BprView v, int64_t step0, i
     return GORSE_B200_OK;
 }
 
-template <bool ATOMIC>
-static void launch_epoch(gorse_b200_cf *cf, const BprView &v, int64_t step0, int64_t n, uint64_t base, float lr, float reg)
+// the atomic-scatter epoch at d outside 16/32/64/128: rounds of GB_BPR_ROUND steps, a delta and an add launch each
+static int32_t launch_round_epoch_any(gorse_b200_cf *cf, BprView v, int64_t step0, int64_t n, uint64_t base, float lr, float reg)
+{
+    gorse_b200_ctx *c = cf->ctx;
+    cudaStream_t s = c->stream;
+    const int d = cf->d;
+    if (cf->bpr_delta.n == 0) GB_TRY(cf->bpr_delta.alloc((size_t)3 * GB_BPR_ROUND * d));
+    if (cf->bpr_rows.n == 0) GB_TRY(cf->bpr_rows.alloc((size_t)3 * GB_BPR_ROUND));
+    float *delta = cf->bpr_delta.p;
+    int32_t *rows = cf->bpr_rows.p;
+    const bool quad = d % 16 == 0, v4 = d % 4 == 0;
+    const int per = v4 ? d / 4 : d;
+    const int add_grid = (int)div_up((int64_t)3 * GB_BPR_ROUND * per, 256);
+    for (int64_t r0 = 0; r0 < n; r0 += GB_BPR_ROUND) {
+        const int64_t nr = std::min<int64_t>(GB_BPR_ROUND, n - r0);
+        if (quad) bpr_round_delta_quad_kernel<<<GB_BPR_ROUND / 64, 256, 0, s>>>(v, step0 + r0, nr, base, lr, reg, delta, rows);
+        else bpr_round_delta_any_kernel<<<GB_BPR_ROUND / 64, 64, 0, s>>>(v, step0 + r0, nr, base, lr, reg, delta, rows);
+        GB_LAUNCHED(c);
+        if (v4) bpr_round_add_kernel<true><<<add_grid, 256, 0, s>>>(v.P, v.Q, d, delta, rows);
+        else bpr_round_add_kernel<false><<<add_grid, 256, 0, s>>>(v.P, v.Q, d, delta, rows);
+        GB_LAUNCHED(c);
+    }
+    return GORSE_B200_OK;
+}
+
+static void launch_store_epoch(gorse_b200_cf *cf, const BprView &v, int64_t step0, int64_t n, uint64_t base, float lr, float reg)
 {
     gorse_b200_ctx *c = cf->ctx;
     cudaStream_t s = c->stream;
@@ -592,15 +708,15 @@ static void launch_epoch(gorse_b200_cf *cf, const BprView &v, int64_t step0, int
         int C = cf->d / 16;
         int g = quad_grid(c, n, C <= 4 ? 8 : 4);
         switch (C) {
-            case 1: bpr_epoch_kernel<1, ATOMIC><<<g, 256, 0, s>>>(v, step0, n, base, lr, reg); break;
-            case 2: bpr_epoch_kernel<2, ATOMIC><<<g, 256, 0, s>>>(v, step0, n, base, lr, reg); break;
-            case 4: bpr_epoch_kernel<4, ATOMIC><<<g, 256, 0, s>>>(v, step0, n, base, lr, reg); break;
-            case 8: bpr_epoch_kernel<8, ATOMIC><<<g, 256, 0, s>>>(v, step0, n, base, lr, reg); break;
-            default: bpr_epoch_kernel<0, ATOMIC><<<g, 256, 0, s>>>(v, step0, n, base, lr, reg); break;
+            case 1: bpr_epoch_kernel<1><<<g, 256, 0, s>>>(v, step0, n, base, lr, reg); break;
+            case 2: bpr_epoch_kernel<2><<<g, 256, 0, s>>>(v, step0, n, base, lr, reg); break;
+            case 4: bpr_epoch_kernel<4><<<g, 256, 0, s>>>(v, step0, n, base, lr, reg); break;
+            case 8: bpr_epoch_kernel<8><<<g, 256, 0, s>>>(v, step0, n, base, lr, reg); break;
+            default: bpr_epoch_kernel<0><<<g, 256, 0, s>>>(v, step0, n, base, lr, reg); break;
         }
     } else {
         int g = (int)std::max<int64_t>(1, std::min<int64_t>((n + 127) / 128, (int64_t)c->sm_count * 8));
-        bpr_epoch_any_kernel<ATOMIC><<<g, 128, 0, s>>>(v, step0, n, base, lr, reg);
+        bpr_epoch_any_kernel<<<g, 128, 0, s>>>(v, step0, n, base, lr, reg);
     }
 }
 
@@ -755,12 +871,13 @@ int32_t gorse_b200_bpr_epoch(gorse_b200_cf *cf, float lr, float reg, int64_t n_s
                        : C == 4 ? launch_round_epoch<4>(cf, v, s0, n_local, mix64(seed), lr, reg)
                                 : launch_round_epoch<8>(cf, v, s0, n_local, mix64(seed), lr, reg);
             if (st) return st;
+            GB_LAUNCHED(c);
         } else if (scatter == GORSE_B200_SCATTER_ATOMIC) {
-            launch_epoch<true>(cf, v, s0, n_local, mix64(seed), lr, reg);
+            GB_TRY(launch_round_epoch_any(cf, v, s0, n_local, mix64(seed), lr, reg));
         } else {
-            launch_epoch<false>(cf, v, s0, n_local, mix64(seed), lr, reg);
+            launch_store_epoch(cf, v, s0, n_local, mix64(seed), lr, reg);
+            GB_LAUNCHED(c);
         }
-        GB_LAUNCHED(c);
     }
     if (c->world > 1) {
         int64_t n = (int64_t)cf->Q.n;

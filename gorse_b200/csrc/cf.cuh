@@ -49,6 +49,10 @@ struct gorse_b200_cf {
     gb::DevBuf<int32_t> user_items, item_users, active;
     gb::DevBuf<gb::UserMeta> user_meta;
     gb::DevBuf<uint32_t> bpr_barrier;  // arrival counter of the round epoch's grid barrier (bpr.cu), zeroed before each launch
+    // the two-launch round epoch (bpr.cu, d outside 16/32/64/128): one round's row deltas, 3 * GB_BPR_ROUND rows of d
+    // floats, and the rows they go to; allocated by the first such epoch
+    gb::DevBuf<float> bpr_delta;
+    gb::DevBuf<int32_t> bpr_rows;
     bool all_active = false;  // every user of the shard has feedback: active[k] == u_lo + k
     // ALS scratch
     gb::DevBuf<float> gram;      // d x d

@@ -142,9 +142,12 @@ int32_t gorse_b200_bpr_apply_triples(gorse_b200_cf *cf, const int32_t *uij, int6
  * (model/cf/model.go:449-468).  A user whose row covers every item yields j = -1. */
 int32_t gorse_b200_bpr_sample_triples(gorse_b200_cf *cf, uint64_t seed, int64_t first_step, int64_t n,
                                       int32_t *uij_out);
-/* one epoch = n_steps fused sample-gather-dot-sigmoid-scatter steps in ONE kernel launch
- * (n_steps = trainSet.CountFeedback(), model/cf/model.go:448).  In a distributed context each
- * rank runs n_steps/world steps on its user shard, then item-factor deltas are all-reduced. */
+/* one epoch = n_steps fused sample-gather-dot-sigmoid-scatter steps (n_steps = trainSet.CountFeedback(),
+ * model/cf/model.go:448).  SCATTER_STORE: one free-running kernel launch.  SCATTER_ATOMIC: rounds of 8192 steps at
+ * every d, in one cooperative launch at d = 16, 32, 64, 128 and two launches per round (deltas, then additions) at
+ * any other d; the first ATOMIC epoch at such a d allocates a 3 * 8192 * d float buffer that lives as long as cf.
+ * In a distributed context each rank runs n_steps/world steps on its user shard, then item-factor deltas are
+ * all-reduced. */
 int32_t gorse_b200_bpr_epoch(gorse_b200_cf *cf, float lr, float reg, int64_t n_steps, uint64_t seed,
                              int32_t scatter);
 

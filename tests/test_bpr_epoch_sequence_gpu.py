@@ -59,7 +59,7 @@ def start(d, seed=0):
 
 @pytest.mark.parametrize("epochs", [2, 3])
 @pytest.mark.parametrize("n_rounds", [5, 6])
-@pytest.mark.parametrize("d", [16, 64, 128])
+@pytest.mark.parametrize("d", [16, 64, 128, 8, 48])
 def test_back_to_back_epochs(gb, ctx, data, d, n_rounds, epochs):
     off, items, _, _ = data
     with gb.CFModel(ctx, U, I, d, off, items) as m:

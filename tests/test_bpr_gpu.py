@@ -156,14 +156,26 @@ def ndcg_of(orc, P, Q, test, neg):
 
 
 def test_full_fit_matches_oracle_ndcg(gb, orc, ctx):
-    # level 3: planted-cluster data; GPU Hogwild epochs (SCATTER_ATOMIC: no update is lost) vs oracle sequential
+    # level 3: planted-cluster data; GPU round epochs (SCATTER_ATOMIC: no update is lost) vs oracle sequential
     # epochs from the same init.  SCATTER_STORE is the parity mode: with ~10^4 triples in flight on a 400-item
     # table its racy read-modify-write loses most updates (measured NDCG 0.07 vs 0.49), exactly as the
     # reference's lock-free goroutines would at that concurrency, so it is not the training default.
+    # d = 16 runs the one-launch round kernel.
+    full_fit_matches_oracle_ndcg(gb, orc, ctx, 16)
+
+
+@pytest.mark.parametrize("d", [8, 48])
+def test_full_fit_matches_oracle_ndcg_two_launch_rounds(gb, orc, ctx, d):
+    # the same fit where the atomic epoch runs as two launches per round; d = 8 is the reference's own BPR test
+    # configuration (model/cf/model_test.go, TestBPR_MovieLens)
+    full_fit_matches_oracle_ndcg(gb, orc, ctx, d)
+
+
+def full_fit_matches_oracle_ndcg(gb, orc, ctx, d):
     scatter = "atomic"
     from gorse_b200 import synth
 
-    U, I, d = 1500, 400, 16
+    U, I = 1500, 400
     off, items = synth.make_feedback(U, I, 30000, seed=9, n_clusters=8)
     train, test = synth.leave_one_out(off, items, seed=1)
     neg = synth.sample_negatives(I, train, test, 100, seed=2)
@@ -191,7 +203,7 @@ def test_full_fit_matches_oracle_ndcg(gb, orc, ctx):
     assert got_dev == got  # device Evaluate == oracle Evaluate on the same factors
 
 
-@pytest.mark.parametrize("d", [64, 128])
+@pytest.mark.parametrize("d", [64, 128, 8, 48])
 def test_atomic_epochs_repeat_up_to_rounding(gb, ctx, d):
     """Epochs with atomic scatter run in rounds whose triples read the rows the previous round left: the same factors and
     seeds give the same factors on every run, except for the order of float additions into a row that several triples of

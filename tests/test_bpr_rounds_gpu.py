@@ -53,7 +53,7 @@ def ctx(gb):
     c.close()
 
 
-@pytest.mark.parametrize("d", [16, 32, 64, 128])
+@pytest.mark.parametrize("d", [16, 32, 64, 128, 3, 8, 10, 48, 80, 256])
 def test_round_epoch_matches_round_model(gb, orc, ctx, data, d):
     off, items = data
     n = int(off[-1])
