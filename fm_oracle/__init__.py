@@ -11,14 +11,15 @@ import numpy as np
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 _SO = os.path.join(_HERE, "libfm_oracle.so")
-_SRC = [os.path.join(_HERE, "fm_oracle.c"), os.path.join(_HERE, "..", "gorse_b200", "csrc", "fm_exp.h")]
+_SRC = [os.path.join(_HERE, "fm_oracle.c"), os.path.join(_HERE, "fm_fit_oracle.c"), os.path.join(_HERE, "..", "gorse_b200", "csrc", "fm_exp.h"),
+        os.path.join(_HERE, "..", "gorse_b200", "csrc", "fm_fit_math.h")]
 
 
 def build(force=False):
     if force or not os.path.exists(_SO) or any(os.path.getmtime(_SO) < os.path.getmtime(s) for s in _SRC):
         # -ffp-contract=off: only the explicit fmaf() calls fuse, as in the reference's floats.MM
         subprocess.check_call(["gcc", "-O2", "-std=gnu11", "-fPIC", "-shared", "-ffp-contract=off", "-fno-fast-math", "-mfma",
-                               "-o", _SO, _SRC[0], "-lm"])
+                               "-o", _SO, _SRC[0], _SRC[1], "-lm"])
 
 
 _lib = None
@@ -42,6 +43,26 @@ def lib():
         L.fmo_rank.restype = C.c_int32
         L.fmo_rank.argtypes = [C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_int32, VP, VP, C.c_int64, VP, VP, VP, VP, C.c_int64, VP,
                                VP, VP, VP, VP, VP, VP, VP, C.c_int32, VP, VP]
+        L.fmf_logf.restype = C.c_float
+        L.fmf_logf.argtypes = [C.c_float]
+        L.fmf_pow_steps.restype = C.c_float
+        L.fmf_pow_steps.argtypes = [C.c_float, C.c_int64]
+        L.fmf_p_order.restype = C.c_int32
+        L.fmf_p_order.argtypes = [VP]
+        L.fmf_set_p_order.argtypes = [VP]
+        L.fmf_mul_const_add_to.argtypes = [VP, C.c_float, VP, VP, C.c_int64]
+        L.fmf_mul_const_add.argtypes = [VP, C.c_float, VP, C.c_int64]
+        L.fmf_metrics.argtypes = [C.c_int64, VP, C.c_int64, VP, VP]
+        L.fmf_evaluate.argtypes = [C.c_int64, C.c_int32, C.c_int32, VP, C.c_int64, VP, VP, VP, VP, VP]
+        L.fmf_op_binary.argtypes = [C.c_int32, VP, C.c_int64, VP, C.c_int64, VP, VP, VP, VP]
+        L.fmf_op_unary.argtypes = [C.c_int32, VP, C.c_int64, VP, VP, VP]
+        L.fmf_op_sum.argtypes = [C.c_int32, VP, C.c_int64, C.c_float, VP, VP]
+        L.fmf_op_sum_axis.argtypes = [VP, C.c_int64, C.c_int64, C.c_int64, VP, VP, VP]
+        L.fmf_op_bmm.argtypes = [C.c_int32, C.c_int32, C.c_int64, C.c_int64, C.c_int64, C.c_int64, C.c_int64, VP, VP, VP, VP, VP, VP]
+        L.fmf_op_embedding.argtypes = [VP, C.c_int64, C.c_int64, VP, C.c_int64, VP, VP, VP]
+        L.fmf_op_broadcast.argtypes = [VP, C.c_int64, C.c_int64, VP, VP, VP]
+        L.fmf_fit.restype = C.c_int32
+        L.fmf_fit.argtypes = [C.c_int64, C.c_int32, VP, VP, C.c_int64, C.c_int64, VP, VP, VP, VP, C.c_int64, VP, VP, VP, VP, VP, VP, VP, VP, VP]
         _lib = L
     return _lib
 
@@ -119,6 +140,170 @@ class Model:
                               inp.n_items, _p(inp.item_feat), _p(inp.item_lab_off), _p(inp.item_lab_idx), _p(inp.item_lab_val), arr,
                               _p(inp.item_emb_mask), _p(inp.cand_off), _p(inp.cand_items), int(coupled), _p(scores), _p(order)) == 0
         return scores[:total], order[:total]
+
+
+# ---- FM training (fm_fit_oracle.c) -------------------------------------------------------------------------------------
+P_GRAD_NAMES = ("ReLU", "Mul", "Abs")
+
+
+def logf(x):
+    return np.float32(lib().fmf_logf(float(x)))
+
+
+def pow_steps(beta, t):
+    return np.float32(lib().fmf_pow_steps(float(beta), int(t)))
+
+
+def p_grad_order():
+    """the order in which ReLU (0), Mul (1) and Abs (2) hand their gradients to the logit, from the replayed backward heap"""
+    out = np.zeros(3, np.int32)
+    assert lib().fmf_p_order(_p(out)) == 0
+    return out.tolist()
+
+
+def set_p_grad_order(order=None):
+    """tests only: make fit() add the logit's gradients in another order (None: the replayed one)"""
+    lib().fmf_set_p_order(None if order is None else _p(_c(order, np.int32)))
+
+
+# the ops of the training graph as the restatement forms them (fmf_op_*): forward and gradients for an output gradient dy
+# (default: ones, what Tensor.Backward seeds)
+_BINARY = {"add": 0, "sub": 1, "mul": 2, "div": 3}
+_UNARY = {"square": 0, "exp": 1, "log": 2, "abs": 3, "relu": 4, "neg": 5}
+
+
+def op_binary(name, x0, x1, dy=None):
+    """-> (y, dx0, dx1); x1 broadcasts over x0 as a suffix"""
+    x0, x1 = _c(x0, np.float32), _c(x1, np.float32)
+    dy = np.ones(x0.shape, np.float32) if dy is None else _c(dy, np.float32)
+    y, g0, g1 = np.empty_like(x0), np.empty_like(x0), np.empty_like(x1)
+    lib().fmf_op_binary(_BINARY[name], _p(x0), x0.size, _p(x1), x1.size, _p(dy), _p(y), _p(g0), _p(g1))
+    return y, g0, g1
+
+
+def op_unary(name, x, dy=None):
+    x = _c(x, np.float32)
+    dy = np.ones(x.shape, np.float32) if dy is None else _c(dy, np.float32)
+    y, g = np.empty_like(x), np.empty_like(x)
+    lib().fmf_op_unary(_UNARY[name], _p(x), x.size, _p(dy), _p(y), _p(g))
+    return y, g
+
+
+def op_sum(x, mean=False, dy=1.0):
+    x = _c(x, np.float32)
+    y, g = np.zeros(1, np.float32), np.empty_like(x)
+    lib().fmf_op_sum(int(mean), _p(x), x.size, float(dy), _p(y), _p(g))
+    return y, g
+
+
+def op_sum_axis(x, axis, dy=None):
+    x = _c(x, np.float32)
+    s1, s2, s3 = int(np.prod(x.shape[:axis])), x.shape[axis], int(np.prod(x.shape[axis + 1:]))
+    oshape = x.shape[:axis] + x.shape[axis + 1:]
+    dy = np.ones(oshape, np.float32) if dy is None else _c(dy, np.float32)
+    y, g = np.empty(oshape, np.float32), np.empty_like(x)
+    lib().fmf_op_sum_axis(_p(x), s1, s2, s3, _p(dy), _p(y), _p(g))
+    return y, g
+
+
+def op_bmm(x, y, t1=False, t2=False, dz=None):
+    """BMM of x [b, xr, xc] and y [b, yr, yc] -> (z, dx, dy)"""
+    x, y = _c(x, np.float32), _c(y, np.float32)
+    b, xr, xc = x.shape
+    _, yr, yc = y.shape
+    m, n = (xc if t1 else xr), (yr if t2 else yc)
+    dz = np.ones((b, m, n), np.float32) if dz is None else _c(dz, np.float32)
+    z, gx, gy = np.empty((b, m, n), np.float32), np.empty_like(x), np.empty_like(y)
+    lib().fmf_op_bmm(int(t1), int(t2), b, xr, xc, yr, yc, _p(x), _p(y), _p(dz), _p(z), _p(gx), _p(gy))
+    return z, gx, gy
+
+
+def op_embedding(w, idx, dy=None):
+    w, idx = _c(w, np.float32), _c(idx, np.float32)
+    rows, dim = w.shape[0], int(np.prod(w.shape[1:]))
+    dy = np.ones(idx.shape + w.shape[1:], np.float32) if dy is None else _c(dy, np.float32)
+    y, gw = np.empty(idx.shape + w.shape[1:], np.float32), np.empty_like(w)
+    lib().fmf_op_embedding(_p(w), rows, dim, _p(idx), idx.size, _p(dy), _p(y), _p(gw))
+    return y, gw
+
+
+def op_broadcast(x, w, dy=None):
+    x = _c(x, np.float32)
+    dy = np.ones(x.shape + (w,), np.float32) if dy is None else _c(dy, np.float32)
+    y, g = np.empty(x.shape + (w,), np.float32), np.empty_like(x)
+    lib().fmf_op_broadcast(_p(x), x.size, w, _p(dy), _p(y), _p(g))
+    return y, g
+
+
+def mul_const_add_to(a, c, b):
+    a, b = _c(a, np.float32), _c(b, np.float32)
+    d = np.empty_like(a)
+    lib().fmf_mul_const_add_to(_p(a), float(c), _p(b), _p(d), a.size)
+    return d
+
+
+def mul_const_add(a, c, dst):
+    a, d = _c(a, np.float32), _c(dst, np.float32).copy()
+    lib().fmf_mul_const_add(_p(a), float(c), _p(d), a.size)
+    return d
+
+
+def metrics(pos_pred, neg_pred):
+    """Precision, Recall, Accuracy, AUC of two prediction lists (evaluator.go:85-153)"""
+    p, n = _c(pos_pred, np.float32).copy(), _c(neg_pred, np.float32).copy()
+    out = np.zeros(4, np.float32)
+    lib().fmf_metrics(p.size, _p(p), n.size, _p(n), _p(out))
+    return out
+
+
+def _rows(r):
+    off, idx, val, tgt = r
+    return (len(off) - 1, _c(off, np.int64), _c(np.concatenate([np.asarray(idx, np.int32), [0]]), np.int32),
+            _c(np.concatenate([np.asarray(val, np.float32), [0]]), np.float32), _c(np.concatenate([np.asarray(tgt, np.float32), [0]]), np.float32))
+
+
+def evaluate(n_features, k, num_dimension, params, test):
+    n, off, idx, val, tgt = _rows(test)
+    out = np.zeros(4, np.float32)
+    lib().fmf_evaluate(int(n_features), int(k), int(num_dimension), _p(_c(params, np.float32)), n, _p(off), _p(idx), _p(val), _p(tgt), _p(out))
+    return out
+
+
+def fit(n_features, num_dimension, train, test, params_in, n_factors=16, n_epochs=50, lr=0.001, reg=0.0002, optimizer=0, batch_size=1024,
+        verbose=10, patience=10, max_steps=0, cancel_epoch=-1):
+    """AFM.Fit restated (see fm_fit_oracle.c); train / test = (off, idx, val, target).
+    -> (params, result dict with gorse_b200_fm_fit_result's fields, moments [2, n_params])"""
+    tr, te = _rows(train), _rows(test)
+    pin = _c(params_in, np.float32)
+    pout, mom = np.zeros(pin.size, np.float32), np.zeros((2, pin.size), np.float32)
+    ip = _c([n_factors, n_epochs, optimizer, batch_size, verbose, patience, cancel_epoch], np.int32)
+    fp = _c([lr, reg], np.float32)
+    rf, ri = np.zeros(5, np.float32), np.zeros(6, np.int64)
+    assert lib().fmf_fit(int(n_features), int(num_dimension), _p(ip), _p(fp), int(max_steps), tr[0], _p(tr[1]), _p(tr[2]), _p(tr[3]), _p(tr[4]),
+                         te[0], _p(te[1]), _p(te[2]), _p(te[3]), _p(te[4]), _p(pin), _p(pout), _p(mom), _p(rf), _p(ri)) == 0
+    res = dict(zip(("auc", "precision", "recall", "accuracy", "cost"), (np.float32(x) for x in rf)))
+    res.update(zip(("epochs_run", "best_epoch", "early_stopped", "diverged", "cancelled", "steps"), (int(x) for x in ri)))
+    return pout, res, mom
+
+
+def random_ctr(rng, n_features, n_rows, labels=4, p_num=0.3, n_ids=None):
+    """CTR rows shaped like the reference's: a user id, an item id and 0 .. labels label features (numerical with
+    probability p_num), target +1 or -1.  -> (off, idx, val, target)"""
+    n_ids = n_ids or n_features
+    lens = 2 + rng.integers(0, labels + 1, n_rows)
+    off = np.zeros(n_rows + 1, np.int64)
+    np.cumsum(lens, out=off[1:])
+    idx = rng.integers(0, n_features, int(off[-1])).astype(np.int32)
+    idx[off[:-1]] = rng.integers(0, n_ids, n_rows)
+    val = np.where(rng.random(int(off[-1])) < p_num, rng.standard_normal(int(off[-1])), 1.0).astype(np.float32)
+    val[off[:-1]] = 1.0
+    tgt = np.where(rng.random(n_rows) < 0.5, 1.0, -1.0).astype(np.float32)
+    return off, idx, val, tgt
+
+
+def init_params(rng, n_features, k, std=0.01):
+    """B = 0, V and W ~ N(0, std) as AFM.Init draws them (fm.go:254-256, nn.NewEmbedding)"""
+    return np.concatenate([[0.0], rng.standard_normal(n_features * k) * std, rng.standard_normal(n_features) * std]).astype(np.float32)
 
 
 # ---- seeded models and inputs (tests and tools/fm_rank_bench.py) ---------------------------------------------------------

@@ -6,7 +6,9 @@
 // Build:  go build -tags "b200 cgo" ./...   with  CGO_CFLAGS=-I<repo>/include  CGO_LDFLAGS="-L<repo>/gorse_b200 -lgorse_b200"
 // (*AFM).B200Ranker uploads a trained AFM once; (*AFMB200).Rank ranks the candidates of many users in one call, as
 // rankByClickTroughRate (worker/pipeline.go:450-499) does for one user with BatchPredict (fm.go:180-229) and
-// cache.SortDocuments.  Inference only: Fit, the XLA AFM and the LLM ranker are unchanged.
+// cache.SortDocuments.  (*AFM).Fit trains a model without embedding slots on the GPU (gorse_b200_fm_fit) and any other
+// model with the reference's Fit, which the integration renames fitCPU (INTEGRATION.md; fm_fit_cpu.go keeps the name Fit
+// for builds without the tag).  The XLA AFM and the LLM ranker are unchanged.
 //go:build b200 && cgo && !xla
 
 package ctr
@@ -16,15 +18,29 @@ package ctr
 #include <stdlib.h>
 #include <string.h>
 #include "gorse_b200.h"
+
+// cgo cannot call Go closures from C directly: Fit's progress callback goes through this exported trampoline.
+extern int32_t gorseB200FMProgress(void *user, int32_t epoch, int32_t nEpochs, float auc);
+static int32_t gorse_b200_fm_progress_tramp(void *user, int32_t epoch, int32_t n, float auc) {
+    return gorseB200FMProgress(user, epoch, n, auc);
+}
+static gorse_b200_progress_fn gorse_b200_fm_progress_ptr(void) { return gorse_b200_fm_progress_tramp; }
 */
 import "C"
 
 import (
+	"context"
 	"errors"
+	"fmt"
+	"runtime/cgo"
 	"sync"
 	"unsafe"
 
+	"github.com/gorse-io/gorse/common/log"
+	"github.com/gorse-io/gorse/common/monitor"
 	"github.com/gorse-io/gorse/dataset"
+	"github.com/gorse-io/gorse/model"
+	"go.uber.org/zap"
 )
 
 func afmB200Error(st C.int32_t) error {
@@ -193,4 +209,131 @@ func (r *AFMB200) Rank(userIds []string, userLabels [][]Label, itemIds []string,
 		scores[u], order[u] = flatScores[a:b], flatOrder[a:b]
 	}
 	return scores, order, nil
+}
+
+// ---- training ------------------------------------------------------------------------------------------------------
+
+// the CTR rows of a split in dataset order as a CSR; scale applies fm.Scalers to the values: Fit does so for the
+// training rows (fm.go:331-344), and BatchInternalPredict for the test rows when autoScale is set (fm.go:159-165)
+func (fm *AFM) b200Rows(set dataset.CTRSplit, scale bool) (off []C.int64_t, idx []C.int32_t, val []C.float, tgt []C.float) {
+	off = make([]C.int64_t, 1, set.Count()+1)
+	tgt = make([]C.float, 0, set.Count()+1)
+	for i := 0; i < set.Count(); i++ {
+		indices, values, _, target := set.Get(i)
+		for j, x := range indices {
+			v := values[j]
+			if scale {
+				if s, ok := fm.Scalers[x]; ok {
+					v = s.Transform(v)
+				}
+			}
+			idx = append(idx, C.int32_t(x))
+			val = append(val, C.float(v))
+		}
+		off = append(off, C.int64_t(len(idx)))
+		tgt = append(tgt, C.float(target))
+	}
+	return off, idx, val, tgt
+}
+
+func ptrF32(s []C.float) *C.float {
+	if len(s) == 0 {
+		return nil
+	}
+	return &s[0]
+}
+
+type afmFitProgress struct {
+	ctx     context.Context
+	span    *monitor.Span
+	nEpochs int
+}
+
+//export gorseB200FMProgress
+func gorseB200FMProgress(user unsafe.Pointer, epoch, nEpochs C.int32_t, auc C.float) C.int32_t {
+	p := (*(*cgo.Handle)(user)).Value().(*afmFitProgress) // user = &handle, the documented way to carry a Handle in a void*
+	if epoch > 0 {
+		p.span.Add(1) // fm.go:414
+	}
+	if auc >= 0 {
+		log.Logger().Info(fmt.Sprintf("fit AFM %v/%v", int(epoch), p.nEpochs), zap.Float32("AUC", float32(auc)))
+	}
+	if p.ctx.Err() != nil {
+		return 1 // Fit returns Score{} where the reference checks ctx.Err(), before the next batch (fm.go:364-367)
+	}
+	return 0
+}
+
+// Fit is AFM.Fit (fm.go:307-417).  A model without item-embedding slots and with at most 32 factors trains on the GPU,
+// step for step as the reference: Init stays here, the library gets fm.Parameters() and the scaled rows, and the fitted
+// parameters are copied back into the model's tensors.  Any other model, or GORSE_B200_ERR_UNSUPPORTED from the library,
+// trains with the reference's Fit (fitCPU).
+func (fm *AFM) Fit(ctx context.Context, trainSet, testSet dataset.CTRSplit, config *FitConfig) Score {
+	if len(trainSet.GetItemEmbeddingDim()) > 0 || fm.nFactors > 32 {
+		return fm.fitCPU(ctx, trainSet, testSet, config)
+	}
+	c, err := afmB200Context()
+	if err != nil {
+		log.Logger().Error("gorse_b200 context", zap.Error(err))
+		return Score{}
+	}
+	log.Logger().Info("fit AFM on the GPU",
+		zap.Int("train_set_size", trainSet.Count()),
+		zap.Int("test_set_size", testSet.Count()),
+		zap.Any("params", fm.GetParams()),
+		zap.Any("config", config))
+	fm.Init(trainSet)
+	var params []float32
+	for _, p := range fm.Parameters() {
+		params = append(params, p.Data()...)
+	}
+	trOff, trIdx, trVal, trTgt := fm.b200Rows(trainSet, true)
+	teOff, teIdx, teVal, teTgt := fm.b200Rows(testSet, fm.autoScale)
+	var p C.gorse_b200_fm_fit_params
+	p.n_factors, p.n_epochs, p.lr, p.reg = C.int32_t(fm.nFactors), C.int32_t(fm.nEpochs), C.float(fm.lr), C.float(fm.reg)
+	switch fm.optimizer {
+	case model.SGD:
+		p.optimizer = C.GORSE_B200_FM_SGD
+	case model.Adam:
+		p.optimizer = C.GORSE_B200_FM_ADAM
+	default:
+		panic("unknown optimizer")
+	}
+	p.batch_size, p.verbose, p.patience = C.int32_t(fm.batchSize), C.int32_t(config.Verbose), C.int32_t(config.Patience)
+
+	_, span := monitor.Start(ctx, "FM.Fit", fm.nEpochs)
+	defer span.End()
+	h := cgo.NewHandle(&afmFitProgress{ctx: ctx, span: span, nEpochs: fm.nEpochs})
+	defer h.Delete()
+	out := make([]float32, len(params))
+	var res C.gorse_b200_fm_fit_result
+	// the library copies during the call and keeps no Go pointer (cgo rule)
+	st := C.gorse_b200_fm_fit(c, C.int64_t(fm.numFeatures), C.int32_t(fm.numDimension), 0, &p,
+		C.int64_t(trainSet.Count()), &trOff[0], ptrI32(trIdx), ptrF32(trVal), ptrF32(trTgt),
+		C.int64_t(testSet.Count()), &teOff[0], ptrI32(teIdx), ptrF32(teVal), ptrF32(teTgt),
+		(*C.float)(unsafe.Pointer(&params[0])), C.int64_t(len(params)), (*C.float)(unsafe.Pointer(&out[0])), nil,
+		C.gorse_b200_fm_progress_ptr(), unsafe.Pointer(&h), &res)
+	if st == C.GORSE_B200_ERR_UNSUPPORTED {
+		log.Logger().Info("gorse_b200 cannot fit this AFM; fitting on the CPU", zap.Error(afmB200Error(st)))
+		return fm.fitCPU(ctx, trainSet, testSet, config)
+	}
+	if err := afmB200Error(st); err != nil {
+		log.Logger().Error("gorse_b200 fm_fit", zap.Error(err))
+		return Score{}
+	}
+	o := 0
+	for _, t := range fm.Parameters() { // B, V, W: the layout params_in had
+		o += copy(t.Data(), out[o:])
+	}
+	if res.cancelled != 0 {
+		log.Logger().Info("fit AFM canceled", zap.Error(ctx.Err()))
+		return Score{}
+	}
+	if res.diverged != 0 {
+		log.Logger().Warn("model diverged", zap.Float32("lr", fm.lr))
+	}
+	if res.early_stopped != 0 {
+		log.Logger().Info("early stopping", zap.Int("best_epoch", int(res.best_epoch)), zap.Int("patience", config.Patience))
+	}
+	return Score{Precision: float32(res.precision), Recall: float32(res.recall), Accuracy: float32(res.accuracy), AUC: float32(res.auc)}
 }

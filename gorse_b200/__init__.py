@@ -10,7 +10,7 @@ import ctypes as C
 import numpy as np
 
 from . import _lib
-from ._lib import (DISTANCE_COSINE, DISTANCE_DOT, DISTANCE_EUCLIDEAN, GorseB200Error, METRIC_COSINE, METRIC_EUCLIDEAN,  # noqa: F401
+from ._lib import (DISTANCE_COSINE, DISTANCE_DOT, DISTANCE_EUCLIDEAN, FM_ADAM, FM_SGD, GorseB200Error, METRIC_COSINE, METRIC_EUCLIDEAN,  # noqa: F401
                    METRIC_NEG_DOT, ORDER_HOGWILD, ORDER_SEQUENTIAL,
                    SCATTER_ATOMIC, SCATTER_STORE, check, lib, ptr)
 
@@ -605,6 +605,44 @@ class FMRanker:
 
     def __exit__(self, *a):
         self.close()
+
+
+class FMTrainer:
+    """AFM.Fit (model/ctr/fm.go:307-417) on the GPU for a model without embedding slots (gorse_b200_fm_fit).  The rows are
+    CSRs (off int64 [n + 1], idx int32, val float32, already through fm.Scalers) with float32 targets; params_in is
+    fm.Parameters() after Init (B, V, W), the layout FMRanker takes."""
+
+    def __init__(self, ctx, n_features, num_dimension, n_factors=16, n_epochs=50, lr=0.001, reg=0.0002, optimizer=FM_ADAM,
+                 batch_size=1024, verbose=10, patience=10, max_steps=0, n_emb=0):
+        self.ctx, self.n_features, self.num_dimension, self.n_emb = ctx, int(n_features), int(num_dimension), int(n_emb)
+        self.params = _lib.FMFitParams(int(n_factors), int(n_epochs), float(lr), float(reg), int(optimizer), int(batch_size), int(verbose),
+                                       int(patience), int(max_steps))
+
+    def n_params(self):
+        return 1 + self.n_features * self.params.n_factors + self.n_features
+
+    def fit(self, train, test, params_in, progress=None, moments=False):
+        """train / test = (off, idx, val, target); progress(epoch, n_epochs, auc) -> truthy to cancel.
+        -> (params float32 [n_params], result dict, moments float32 [2, n_params] or None)"""
+        def rows(r):
+            off, idx, val, tgt = r
+            off = np.ascontiguousarray(off, np.int64)
+            return (off.size - 1, off, np.ascontiguousarray(idx, np.int32), np.ascontiguousarray(val, np.float32),
+                    np.ascontiguousarray(tgt, np.float32))
+
+        tr, te = rows(train), rows(test)
+        pin = np.ascontiguousarray(params_in, np.float32).reshape(-1)
+        if pin.size != self.n_params():
+            raise ValueError(f"params_in holds {pin.size} floats, the model has {self.n_params()}")
+        pout = np.zeros(max(pin.size, 1), np.float32)
+        mom = np.zeros((2, pin.size), np.float32) if moments else None
+        res = _lib.FMFitResult()
+        cb = _lib.PROGRESS_FN(lambda user, ep, n, auc: int(bool(progress(ep, n, auc)))) if progress else None
+        check(lib.gorse_b200_fm_fit(self.ctx.h, self.n_features, self.num_dimension, self.n_emb, C.byref(self.params), tr[0], ptr(tr[1]),
+                                    ptr(tr[2]), ptr(tr[3]), ptr(tr[4]), te[0], ptr(te[1]), ptr(te[2]), ptr(te[3]), ptr(te[4]), ptr(pin),
+                                    pin.size, ptr(pout), ptr(mom), cb, None, C.byref(res)))
+        out = {f: getattr(res, f) for f, _ in _lib.FMFitResult._fields_}
+        return pout[:pin.size], out, mom
 
 
 def load_ncf(train_path, test_path=None):

@@ -102,6 +102,9 @@ PROTOTYPES = {
     "gorse_b200_fm_create": (C.c_int32, [VP, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_int32, VP, VP, C.c_int64, PVP]),
     "gorse_b200_fm_destroy": (C.c_int32, [VP]),
     "gorse_b200_fm_rank": (C.c_int32, [VP, C.c_int64, VP, VP, VP, VP, C.c_int64, VP, VP, VP, VP, VP, VP, VP, VP, VP, VP, VP]),
+    "gorse_b200_fm_fit_params_default": (C.c_int32, [VP]),
+    "gorse_b200_fm_fit": (C.c_int32, [VP, C.c_int64, C.c_int32, C.c_int32, VP, C.c_int64, VP, VP, VP, VP, C.c_int64, VP, VP, VP, VP, VP, C.c_int64,
+                                      VP, VP, VP, VP, VP]),
     "gorse_b200_ncf_load":(C.c_int32, [C.c_char_p, C.c_char_p, PVP]),
     "gorse_b200_ncf_shape": (C.c_int32, [VP, C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.POINTER(C.c_int64), C.POINTER(C.c_int64),
                                          C.POINTER(C.c_int64)]),
@@ -119,6 +122,20 @@ class FitParams(C.Structure):
 class FitResult(C.Structure):
     _fields_ = [("ndcg", C.c_float), ("precision", C.c_float), ("recall", C.c_float), ("epochs_run", C.c_int32),
                 ("early_stopped", C.c_int32), ("best_epoch", C.c_int32), ("cancelled", C.c_int32)]
+
+
+FM_ADAM, FM_SGD = 0, 1
+
+
+class FMFitParams(C.Structure):
+    _fields_ = [("n_factors", C.c_int32), ("n_epochs", C.c_int32), ("lr", C.c_float), ("reg", C.c_float), ("optimizer", C.c_int32),
+                ("batch_size", C.c_int32), ("verbose", C.c_int32), ("patience", C.c_int32), ("max_steps", C.c_int64)]
+
+
+class FMFitResult(C.Structure):
+    _fields_ = [("auc", C.c_float), ("precision", C.c_float), ("recall", C.c_float), ("accuracy", C.c_float), ("cost", C.c_float),
+                ("epochs_run", C.c_int32), ("best_epoch", C.c_int32), ("early_stopped", C.c_int32), ("diverged", C.c_int32),
+                ("cancelled", C.c_int32), ("steps", C.c_int64)]
 
 
 PROGRESS_FN = C.CFUNCTYPE(C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_float)

@@ -438,7 +438,8 @@ int32_t gorse_b200_vecdb_user_to_user(gorse_b200_vecdb *db, int64_t n_users, con
 /* ------------------------------------------------------------------------------------------
  * Batched FM ranking: the worker's "fm" ranker (rankByClickTroughRate, worker/pipeline.go:450-499) for many users in one
  * call -- AFM.BatchPredict (model/ctr/fm.go:180-229) on every (user, candidate) pair of each user, then the candidates by
- * score.  Inference only; training (AFM.Fit) stays in the reference.
+ * score.  Training is gorse_b200_fm_fit below, for models without embedding slots; a model with slots is still trained by
+ * the reference's AFM.Fit.
  * gorse_b200_fm_create uploads one trained model once; the handle is read-only afterwards and thread-safe.
  *   n_features = fm.numFeatures (the unified index's Len), n_factors = nFactors, num_dimension = fm.numDimension,
  *   batch_size = the BatchSize param (default 1024), emb_dim[n_emb] = fm.embeddingDim.
@@ -471,6 +472,60 @@ int32_t gorse_b200_fm_rank(gorse_b200_fm *fm, int64_t n_users, const int32_t *us
                            const int64_t *item_lab_off, const int32_t *item_lab_idx, const float *item_lab_val,
                            const uint16_t *const *item_emb, const uint8_t *item_emb_mask, const int64_t *cand_off,
                            const int32_t *cand_items, float *scores_out, int32_t *order_out, int64_t *stats_out);
+
+/* ------------------------------------------------------------------------------------------
+ * FM training: AFM.Fit (model/ctr/fm.go:307-417) for a model without item-embedding slots (plain FM: bias, linear and
+ * pairwise terms), step for step.  The master runs it every ranker.fit_period (master/tasks.go:1047-1155) and
+ * optimize_trials more times (:1318-1363).  Init and the scalers stay with the caller: it passes fm.Parameters() after
+ * Init as params_in, and rows already through fm.Scalers.
+ *   n_features = the unified index's Len, num_dimension = fm.numDimension (the longest training row), n_emb = the number
+ *   of embedding slots: any slot, or n_factors above 32, is GORSE_B200_ERR_UNSUPPORTED (train those with the reference).
+ *   train rows: CSR train_off[n_train + 1] (from 0) / train_idx / train_val, one row per trainSet.Get(i) in dataset order,
+ *   train_target[n_train]; test rows the same way (targets > 0 are the positives of EvaluateClassification).
+ *   params_in / params_out[n_params], n_params = 1 + n_features n_factors + n_features (another length is
+ *   GORSE_B200_ERR_ARG): B, V, W in gorse_b200_fm_create's layout, so a fitted model goes straight into the ranker.  moments_out[2 n_params] (may be NULL): Adam's m then v (zeros for SGD).
+ * What runs: evaluation at epoch 0; per epoch, the rows in dataset order in batches of batch_size (the last may be
+ * partial), each padded to D = max(num_dimension, the longest training row) with index 0, value 0, indices through
+ * float32; BCEWithLogits, its backward in the reference's order, then Adam (default) or SGD with weight decay `reg` over
+ * every parameter; evaluation every `verbose` epochs and on the last one, then the NaN break (cost or Precision, which is
+ * score.GetValue()) and early stopping on AUC with `patience` (0: none), best = the first maximum.  Every parameter and
+ * moment is bit-identical to the project's CPU restatement (DESIGN §8.5); Log and Adam's Pow are restated algorithms whose
+ * agreement with Go's math32 is not pinned.
+ * progress (may be NULL) is called after the epoch-0 evaluation and after every epoch with the epoch and its AUC (-1 when
+ * the epoch was not evaluated); a non-zero return cancels where the reference would see ctx.Err() -- at the next batch --
+ * and Fit returns a zero score with `cancelled` set.  An epoch runs as one CUDA graph, so the callback and with it a
+ * cancel come at most one epoch late; params_out then holds that epoch's updates.  max_steps > 0 stops after that many optimiser steps (tests and
+ * benchmarks); the scores are then those of the last evaluation.
+ * Every index is checked on the host before the device is touched (GORSE_B200_ERR_ARG), also after rounding to float32. */
+typedef struct {
+    int32_t n_factors;   /* NFactors, default 16 */
+    int32_t n_epochs;    /* NEpochs, default 50 */
+    float lr;            /* Lr, default 0.001 */
+    float reg;           /* Reg (weight decay), default 0.0002 */
+    int32_t optimizer;   /* GORSE_B200_FM_ADAM (default) or GORSE_B200_FM_SGD */
+    int32_t batch_size;  /* BatchSize, default 1024 */
+    int32_t verbose;     /* FitConfig.Verbose, default 10; must be >= 1 */
+    int32_t patience;    /* FitConfig.Patience, default 10; 0 = no early stopping */
+    int64_t max_steps;   /* 0 = no limit */
+} gorse_b200_fm_fit_params;
+
+enum { GORSE_B200_FM_ADAM = 0, GORSE_B200_FM_SGD = 1 };
+
+typedef struct {
+    float auc, precision, recall, accuracy; /* Score of the LAST evaluation; all zero when cancelled */
+    float cost;                             /* sum of the batch losses of the last epoch run */
+    int32_t epochs_run, best_epoch;         /* best_epoch: the first epoch with the highest AUC among the evaluations */
+    int32_t early_stopped, diverged, cancelled;
+    int64_t steps;                          /* optimiser steps run */
+} gorse_b200_fm_fit_result;
+
+int32_t gorse_b200_fm_fit_params_default(gorse_b200_fm_fit_params *params);
+int32_t gorse_b200_fm_fit(gorse_b200_ctx *ctx, int64_t n_features, int32_t num_dimension, int32_t n_emb,
+                          const gorse_b200_fm_fit_params *params, int64_t n_train, const int64_t *train_off, const int32_t *train_idx,
+                          const float *train_val, const float *train_target, int64_t n_test, const int64_t *test_off,
+                          const int32_t *test_idx, const float *test_val, const float *test_target, const float *params_in,
+                          int64_t n_params, float *params_out, float *moments_out, gorse_b200_progress_fn progress, void *user,
+                          gorse_b200_fm_fit_result *result);
 
 /* ------------------------------------------------------------------------------------------
  * NCF-format datasets: dataset.LoadDataFromBuiltIn (dataset/dataset.go:398-490), the loader `gorse-bench cf`
