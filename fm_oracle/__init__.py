@@ -50,6 +50,15 @@ def lib():
         L.fmf_p_order.restype = C.c_int32
         L.fmf_p_order.argtypes = [VP]
         L.fmf_set_p_order.argtypes = [VP]
+        L.fmf_backward_order.restype = C.c_int32
+        L.fmf_backward_order.argtypes = [C.c_int32, VP, VP]
+        L.fmf_set_vx_order.argtypes = [VP, C.c_int32]
+        L.fmf_set_alternative.argtypes = [C.c_int32]
+        L.fmf_heap_order.restype = C.c_int32
+        L.fmf_heap_order.argtypes = [C.c_int32, VP, VP]
+        L.fmf_op_softmax.argtypes = [VP, C.c_int64, C.c_int64, VP, C.c_int32, VP, VP]
+        L.fmo_dot.restype = C.c_float
+        L.fmo_dot.argtypes = [VP, VP, C.c_int64]
         L.fmf_mul_const_add_to.argtypes = [VP, C.c_float, VP, VP, C.c_int64]
         L.fmf_mul_const_add.argtypes = [VP, C.c_float, VP, C.c_int64]
         L.fmf_metrics.argtypes = [C.c_int64, VP, C.c_int64, VP, VP]
@@ -63,6 +72,9 @@ def lib():
         L.fmf_op_broadcast.argtypes = [VP, C.c_int64, C.c_int64, VP, VP, VP]
         L.fmf_fit.restype = C.c_int32
         L.fmf_fit.argtypes = [C.c_int64, C.c_int32, VP, VP, C.c_int64, C.c_int64, VP, VP, VP, VP, C.c_int64, VP, VP, VP, VP, VP, VP, VP, VP, VP]
+        L.fmf_fit_emb.restype = C.c_int32
+        L.fmf_fit_emb.argtypes = [C.c_int64, C.c_int32, VP, VP, C.c_int64, C.c_int64, VP, VP, VP, VP, C.c_int64, VP, VP, VP, VP, C.c_int32, VP, VP,
+                                  VP, VP, VP, VP, VP, VP, VP, VP]
         _lib = L
     return _lib
 
@@ -79,6 +91,12 @@ def mm(transA, transB, m, n, k, a, lda, b, ldb, c, ldc):
     """floats.MM restated (c += op(a) op(b), a fused chain over the contracted index); c updated in place"""
     assert a.dtype == b.dtype == c.dtype == np.float32 and c.flags.c_contiguous
     lib().fmo_mm(int(transA), int(transB), m, n, k, _p(_c(a, np.float32)), lda, _p(_c(b, np.float32)), ldb, _p(c), ldc)
+
+
+def dot(a, b):
+    """floats.Dot restated: what floats.MM's transB path assigns to every output element"""
+    a, b = _c(a, np.float32), _c(b, np.float32)
+    return np.float32(lib().fmo_dot(_p(a), _p(b), a.size))
 
 
 def mul_to(a, b):
@@ -164,6 +182,49 @@ def p_grad_order():
 def set_p_grad_order(order=None):
     """tests only: make fit() add the logit's gradients in another order (None: the replayed one)"""
     lib().fmf_set_p_order(None if order is None else _p(_c(order, np.int32)))
+
+
+VX_GRAD_NAMES = ("Square", "BMM slot 0", "BMM slot 1", "BMM slot 2", "BMM slot 3", "BMM slot 4", "BMM slot 5", "BMM slot 6", "BMM slot 7")
+
+
+def backward_order(n_emb):
+    """-> (the order of p's gradients as p_grad_order gives it, the order in which Square (0) and slot s's BMM (1 + s) hand
+    their gradients to vx), from the backward heap replayed on the graph with n_emb slots"""
+    p, vx = np.zeros(3, np.int32), np.zeros(1 + n_emb, np.int32)
+    assert lib().fmf_backward_order(int(n_emb), _p(p), _p(vx)) == 0
+    return p.tolist(), vx.tolist()
+
+
+def set_vx_grad_order(order=None):
+    """tests only: make fit() add vx's gradients in another order (None: the replayed one)"""
+    lib().fmf_set_vx_order(None if order is None else _p(_c(order, np.int32)), 0 if order is None else len(order))
+
+
+ALTERNATIVES = {"softmax_rowwise": 1, "contraction_reversed": 2, "bias_reversed": 4}
+
+
+def set_alternative(name=None):
+    """tests only: make fit() use the alternative to one pinned rule of the slots' backward (None: the pinned rules)"""
+    lib().fmf_set_alternative(0 if name is None else ALTERNATIVES[name])
+
+
+def heap_order(inputs):
+    """Tensor.Backward's pop order on a graph: inputs[o] = the (up to two) ops producing op o's inputs, -1 for a leaf, in
+    creation order; the last op is the one Backward is called on"""
+    a = _c([(list(i) + [-1, -1])[:2] for i in inputs], np.int32)
+    out = np.zeros(len(inputs), np.int32)
+    n = lib().fmf_heap_order(len(inputs), _p(a), _p(out))
+    assert n >= 0
+    return out[:n].tolist()
+
+
+def op_softmax(x, dy=None, coupled=True):
+    """Softmax(x, 1) of a [B, dim] tensor -> (y, dx)"""
+    x = _c(x, np.float32)
+    dy = np.ones(x.shape, np.float32) if dy is None else _c(dy, np.float32)
+    y, g = np.empty_like(x), np.empty_like(x)
+    lib().fmf_op_softmax(_p(x), x.shape[0], x.shape[1], _p(dy), int(coupled), _p(y), _p(g))
+    return y, g
 
 
 # the ops of the training graph as the restatement forms them (fmf_op_*): forward and gradients for an output gradient dy
@@ -269,9 +330,24 @@ def evaluate(n_features, k, num_dimension, params, test):
     return out
 
 
+class Embeddings:
+    """The item-embedding side of a fit: dims [n_emb], table[s] = bf16 bits [n_rows, dim_s], mask [n_rows, n_emb] uint8 or
+    None (every embedding present), and the table row (-1: none) of every training and test sample."""
+
+    def __init__(self, dims, table, mask, train_rows, test_rows):
+        self.dims = _c(list(dims), np.int32)
+        self.table = [_c(t, np.uint16) for t in table]
+        self.n_rows = self.table[0].shape[0] if self.table else 0
+        self.mask = None if mask is None else _c(mask, np.uint8)
+        self.train_rows, self.test_rows = _c(np.append(train_rows, 0), np.int32)[:-1], _c(np.append(test_rows, 0), np.int32)[:-1]
+
+    def n_slot_params(self, k):
+        return int(sum(3 * k * int(d) + 2 * k for d in self.dims))
+
+
 def fit(n_features, num_dimension, train, test, params_in, n_factors=16, n_epochs=50, lr=0.001, reg=0.0002, optimizer=0, batch_size=1024,
-        verbose=10, patience=10, max_steps=0, cancel_epoch=-1):
-    """AFM.Fit restated (see fm_fit_oracle.c); train / test = (off, idx, val, target).
+        verbose=10, patience=10, max_steps=0, cancel_epoch=-1, emb=None):
+    """AFM.Fit restated (see fm_fit_oracle.c); train / test = (off, idx, val, target); emb = Embeddings for a model with slots.
     -> (params, result dict with gorse_b200_fm_fit_result's fields, moments [2, n_params])"""
     tr, te = _rows(train), _rows(test)
     pin = _c(params_in, np.float32)
@@ -279,8 +355,15 @@ def fit(n_features, num_dimension, train, test, params_in, n_factors=16, n_epoch
     ip = _c([n_factors, n_epochs, optimizer, batch_size, verbose, patience, cancel_epoch], np.int32)
     fp = _c([lr, reg], np.float32)
     rf, ri = np.zeros(5, np.float32), np.zeros(6, np.int64)
-    assert lib().fmf_fit(int(n_features), int(num_dimension), _p(ip), _p(fp), int(max_steps), tr[0], _p(tr[1]), _p(tr[2]), _p(tr[3]), _p(tr[4]),
-                         te[0], _p(te[1]), _p(te[2]), _p(te[3]), _p(te[4]), _p(pin), _p(pout), _p(mom), _p(rf), _p(ri)) == 0
+    head = (int(n_features), int(num_dimension), _p(ip), _p(fp), int(max_steps), tr[0], _p(tr[1]), _p(tr[2]), _p(tr[3]), _p(tr[4]),
+            te[0], _p(te[1]), _p(te[2]), _p(te[3]), _p(te[4]))
+    if emb is None:
+        assert lib().fmf_fit(*head, _p(pin), _p(pout), _p(mom), _p(rf), _p(ri)) == 0
+    else:
+        arr = (C.c_void_p * max(len(emb.table), 1))(*[_p(t) for t in emb.table])
+        tr_row, te_row = np.append(emb.train_rows, 0).astype(np.int32), np.append(emb.test_rows, 0).astype(np.int32)
+        assert lib().fmf_fit_emb(*head, emb.dims.size, _p(emb.dims), arr, _p(emb.mask), _p(tr_row), _p(te_row), _p(pin), _p(pout), _p(mom),
+                                 _p(rf), _p(ri)) == 0
     res = dict(zip(("auc", "precision", "recall", "accuracy", "cost"), (np.float32(x) for x in rf)))
     res.update(zip(("epochs_run", "best_epoch", "early_stopped", "diverged", "cancelled", "steps"), (int(x) for x in ri)))
     return pout, res, mom
@@ -301,9 +384,22 @@ def random_ctr(rng, n_features, n_rows, labels=4, p_num=0.3, n_ids=None):
     return off, idx, val, tgt
 
 
-def init_params(rng, n_features, k, std=0.01):
-    """B = 0, V and W ~ N(0, std) as AFM.Init draws them (fm.go:254-256, nn.NewEmbedding)"""
-    return np.concatenate([[0.0], rng.standard_normal(n_features * k) * std, rng.standard_normal(n_features) * std]).astype(np.float32)
+def init_params(rng, n_features, k, std=0.01, emb_dims=()):
+    """B = 0, V and W ~ N(0, std) as AFM.Init draws them (fm.go:254-256, nn.NewEmbedding); per slot H ~ N(0, std), AW and EW
+    uniform in +-1/sqrt(dim), Ab = Eb = 0 (NewAttention, NewLinear, layers.go:42-48, 166-171)"""
+    parts = [[0.0], rng.standard_normal(n_features * k) * std, rng.standard_normal(n_features) * std]
+    for d in emb_dims:
+        b = 1 / np.sqrt(d)
+        parts += [rng.standard_normal(k * d) * std, rng.uniform(-b, b, d * k), np.zeros(k), rng.uniform(-b, b, d * k), np.zeros(k)]
+    return np.concatenate(parts).astype(np.float32)
+
+
+def random_embeddings(rng, n_rows, dims, n_train, n_test, p_absent=0.15, p_no_item=0.1):
+    """A seeded Embeddings: a bf16 table, slots absent with probability p_absent, samples without an item with p_no_item"""
+    table = [to_bf16(rng.standard_normal((n_rows, d), dtype=np.float32)) for d in dims]
+    mask = (rng.random((n_rows, len(dims))) >= p_absent).astype(np.uint8)
+    rows = [np.where(rng.random(n) < p_no_item, -1, rng.integers(0, n_rows, n)).astype(np.int32) for n in (n_train, n_test)]
+    return Embeddings(dims, table, mask, rows[0], rows[1])
 
 
 # ---- seeded models and inputs (tests and tools/fm_rank_bench.py) ---------------------------------------------------------

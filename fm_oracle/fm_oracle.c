@@ -12,7 +12,8 @@
  *                                            (r, c) of a chunk uses row (r dim + c) % B's max and sum.  fmo_softmax with
  *                                            coupled = 0 is the textbook row-wise softmax, kept only to show the difference.
  * Arithmetic: floats.MM (_mm512_mm, common/floats/src/floats_avx512.c:443-480; the committed Go assembly fuses every
- * update, vfmadd231ss / vfmadd231ps) is a fused chain over the contracted index from +0 -- fmaf here; Tensor.square is
+ * update, vfmadd231ss / vfmadd231ps) is a fused chain over the contracted index from +0 -- fmaf here -- except x y^T, which
+ * assigns floats.Dot (lane accumulators and a reduce tree, fmo_dot) to every element; Tensor.square is
  * _mm512_mul_to; Tensor.add with a scalar is _mm512_add_const, otherwise floats.Add (a Go loop); everything else is a
  * plain float32 operation.  Go's max(a, b) propagates NaN and orders -0 below +0.  Build: -ffp-contract=off. */
 #include <math.h>
@@ -23,9 +24,40 @@
 #include "../gorse_b200/csrc/fm_exp.h"
 
 /* ---- the floats kernels the forward uses ------------------------------------------------------------------------- */
+/* the dot of two contiguous vectors (floats_avx512.c:306-367): 16 lane accumulators (a product, then fused updates), a
+ * fixed reduce tree, one 8-lane block of unfused products through its own tree, then a fused scalar tail */
+float fmo_dot(const float *a, const float *b, int64_t n)
+{
+    const int64_t epoch = n / 16;
+    int64_t remain = n % 16;
+    float s[16], r8[8], r4[4];
+    for (int l = 0; l < 16; l++) s[l] = epoch > 0 ? a[l] * b[l] : 0.0f;
+    for (int64_t c = 1; c < epoch; c++)
+        for (int l = 0; l < 16; l++) s[l] = fmaf(a[16 * c + l], b[16 * c + l], s[l]);
+    for (int l = 0; l < 8; l++) r8[l] = s[l + 8] + s[l];
+    for (int l = 0; l < 4; l++) r4[l] = r8[l + 4] + r8[l];
+    float sum = (r4[0] + r4[2]) + (r4[1] + r4[3]);
+    a += 16 * epoch;
+    b += 16 * epoch;
+    if (remain >= 8) {
+        for (int l = 0; l < 4; l++) r4[l] = a[l + 4] * b[l + 4] + a[l] * b[l];
+        sum = sum + ((r4[0] + r4[2]) + (r4[1] + r4[3]));
+        a += 8;
+        b += 8;
+        remain -= 8;
+    }
+    for (int64_t i = 0; i < remain; i++) sum = fmaf(a[i], b[i], sum);
+    return sum;
+}
+
 void fmo_mm(int transA, int transB, int64_t m, int64_t n, int64_t k, const float *a, int64_t lda, const float *b, int64_t ldb,
             float *c, int64_t ldc)
 {
+    if (!transA && transB) { /* c = dot(row of a, row of b): assigned, not accumulated (floats_avx512.c:454-460) */
+        for (int64_t i = 0; i < m; i++)
+            for (int64_t j = 0; j < n; j++) c[i * ldc + j] = fmo_dot(a + i * lda, b + j * ldb, k);
+        return;
+    }
     for (int64_t i = 0; i < m; i++)
         for (int64_t l = 0; l < k; l++)
             for (int64_t j = 0; j < n; j++) {

@@ -6,9 +6,10 @@
 // Build:  go build -tags "b200 cgo" ./...   with  CGO_CFLAGS=-I<repo>/include  CGO_LDFLAGS="-L<repo>/gorse_b200 -lgorse_b200"
 // (*AFM).B200Ranker uploads a trained AFM once; (*AFMB200).Rank ranks the candidates of many users in one call, as
 // rankByClickTroughRate (worker/pipeline.go:450-499) does for one user with BatchPredict (fm.go:180-229) and
-// cache.SortDocuments.  (*AFM).Fit trains a model without embedding slots on the GPU (gorse_b200_fm_fit) and any other
-// model with the reference's Fit, which the integration renames fitCPU (INTEGRATION.md; fm_fit_cpu.go keeps the name Fit
-// for builds without the tag).  The XLA AFM and the LLM ranker are unchanged.
+// cache.SortDocuments.  (*AFM).Fit trains on the GPU: a model without embedding slots through gorse_b200_fm_fit, one with
+// slots through gorse_b200_fm_fit_emb; a model beyond the library's limits trains with the reference's Fit, which the
+// integration renames fitCPU (INTEGRATION.md; fm_fit_cpu.go keeps the name Fit for builds without the tag).  The XLA AFM
+// and the LLM ranker are unchanged.
 //go:build b200 && cgo && !xla
 
 package ctr
@@ -236,6 +237,65 @@ func (fm *AFM) b200Rows(set dataset.CTRSplit, scale bool) (off []C.int64_t, idx 
 	return off, idx, val, tgt
 }
 
+// afmEmbTable is the item-embedding table of a fit in C memory (an array of pointers into Go memory may not cross into C):
+// one row per distinct item of the splits, bf16 bits per slot, and the presence mask of convertToTensors' rule
+// (fm.go:555-561): the slot exists for the item and has the slot's length.
+type afmEmbTable struct {
+	dims  []C.int32_t
+	slots *[1 << 20]*C.uint16_t
+	mask  []C.uint8_t
+	rows  int
+}
+
+func (t *afmEmbTable) free() {
+	for s := range t.dims {
+		C.free(unsafe.Pointer(t.slots[s]))
+	}
+	C.free(unsafe.Pointer(t.slots))
+}
+
+// b200EmbTable builds the table and the table row of every sample of the splits (-1: the sample has no embeddings).
+// CTRSplit.Get hands out ItemEmbeddings[Items[i]] (model/ctr/data.go:221-240), so samples of one item share one slice:
+// its identity is the item, and the splits of one dataset share the item table.
+func b200EmbTable(dims []int, sets ...dataset.CTRSplit) (*afmEmbTable, [][]C.int32_t) {
+	rowOf := make(map[*[]uint16]int32)
+	var items [][][]uint16
+	sampleRows := make([][]C.int32_t, len(sets))
+	for q, set := range sets {
+		sampleRows[q] = make([]C.int32_t, set.Count()+1)
+		for i := 0; i < set.Count(); i++ {
+			_, _, e, _ := set.Get(i)
+			if len(e) == 0 {
+				sampleRows[q][i] = -1
+				continue
+			}
+			r, ok := rowOf[&e[0]]
+			if !ok {
+				r = int32(len(items))
+				rowOf[&e[0]] = r
+				items = append(items, e)
+			}
+			sampleRows[q][i] = C.int32_t(r)
+		}
+	}
+	nEmb := len(dims)
+	t := &afmEmbTable{dims: make([]C.int32_t, nEmb), mask: make([]C.uint8_t, len(items)*nEmb+1), rows: len(items)}
+	t.slots = (*[1 << 20]*C.uint16_t)(C.malloc(C.size_t(nEmb+1) * C.size_t(unsafe.Sizeof(uintptr(0)))))
+	for s, d := range dims {
+		t.dims[s] = C.int32_t(d)
+		bytes := C.size_t(len(items)*d*2 + 2)
+		t.slots[s] = (*C.uint16_t)(C.malloc(bytes))
+		C.memset(unsafe.Pointer(t.slots[s]), 0, bytes)
+		for r, e := range items {
+			if len(e) > s && len(e[s]) == d && d > 0 {
+				t.mask[r*nEmb+s] = 1
+				C.memcpy(unsafe.Add(unsafe.Pointer(t.slots[s]), r*d*2), unsafe.Pointer(&e[s][0]), C.size_t(d*2))
+			}
+		}
+	}
+	return t, sampleRows
+}
+
 func ptrF32(s []C.float) *C.float {
 	if len(s) == 0 {
 		return nil
@@ -264,14 +324,12 @@ func gorseB200FMProgress(user unsafe.Pointer, epoch, nEpochs C.int32_t, auc C.fl
 	return 0
 }
 
-// Fit is AFM.Fit (fm.go:307-417).  A model without item-embedding slots and with at most 32 factors trains on the GPU,
-// step for step as the reference: Init stays here, the library gets fm.Parameters() and the scaled rows, and the fitted
-// parameters are copied back into the model's tensors.  Any other model, or GORSE_B200_ERR_UNSUPPORTED from the library,
-// trains with the reference's Fit (fitCPU).
+// Fit is AFM.Fit (fm.go:307-417) on the GPU, step for step as the reference: Init stays here, the library gets
+// fm.Parameters() and the scaled rows, and the fitted parameters are copied back into the model's tensors.  A model with
+// item-embedding slots also sends the splits' item-embedding table and every sample's row of it (gorse_b200_fm_fit_emb).
+// Only GORSE_B200_ERR_UNSUPPORTED from the library (more than 32 factors, 8 slots or an embedding wider than 1024) trains
+// with the reference's Fit (fitCPU).
 func (fm *AFM) Fit(ctx context.Context, trainSet, testSet dataset.CTRSplit, config *FitConfig) Score {
-	if len(trainSet.GetItemEmbeddingDim()) > 0 || fm.nFactors > 32 {
-		return fm.fitCPU(ctx, trainSet, testSet, config)
-	}
 	c, err := afmB200Context()
 	if err != nil {
 		log.Logger().Error("gorse_b200 context", zap.Error(err))
@@ -308,11 +366,23 @@ func (fm *AFM) Fit(ctx context.Context, trainSet, testSet dataset.CTRSplit, conf
 	out := make([]float32, len(params))
 	var res C.gorse_b200_fm_fit_result
 	// the library copies during the call and keeps no Go pointer (cgo rule)
-	st := C.gorse_b200_fm_fit(c, C.int64_t(fm.numFeatures), C.int32_t(fm.numDimension), 0, &p,
-		C.int64_t(trainSet.Count()), &trOff[0], ptrI32(trIdx), ptrF32(trVal), ptrF32(trTgt),
-		C.int64_t(testSet.Count()), &teOff[0], ptrI32(teIdx), ptrF32(teVal), ptrF32(teTgt),
-		(*C.float)(unsafe.Pointer(&params[0])), C.int64_t(len(params)), (*C.float)(unsafe.Pointer(&out[0])), nil,
-		C.gorse_b200_fm_progress_ptr(), unsafe.Pointer(&h), &res)
+	var st C.int32_t
+	if len(fm.embeddingDim) == 0 {
+		st = C.gorse_b200_fm_fit(c, C.int64_t(fm.numFeatures), C.int32_t(fm.numDimension), 0, &p,
+			C.int64_t(trainSet.Count()), &trOff[0], ptrI32(trIdx), ptrF32(trVal), ptrF32(trTgt),
+			C.int64_t(testSet.Count()), &teOff[0], ptrI32(teIdx), ptrF32(teVal), ptrF32(teTgt),
+			(*C.float)(unsafe.Pointer(&params[0])), C.int64_t(len(params)), (*C.float)(unsafe.Pointer(&out[0])), nil,
+			C.gorse_b200_fm_progress_ptr(), unsafe.Pointer(&h), &res)
+	} else {
+		table, rows := b200EmbTable(fm.embeddingDim, trainSet, testSet)
+		defer table.free()
+		st = C.gorse_b200_fm_fit_emb(c, C.int64_t(fm.numFeatures), C.int32_t(fm.numDimension), &p,
+			C.int64_t(trainSet.Count()), &trOff[0], ptrI32(trIdx), ptrF32(trVal), ptrF32(trTgt), &rows[0][0],
+			C.int64_t(testSet.Count()), &teOff[0], ptrI32(teIdx), ptrF32(teVal), ptrF32(teTgt), &rows[1][0],
+			C.int32_t(len(table.dims)), &table.dims[0], C.int64_t(table.rows), (**C.uint16_t)(unsafe.Pointer(table.slots)), &table.mask[0],
+			(*C.float)(unsafe.Pointer(&params[0])), C.int64_t(len(params)), (*C.float)(unsafe.Pointer(&out[0])), nil,
+			C.gorse_b200_fm_progress_ptr(), unsafe.Pointer(&h), &res)
+	}
 	if st == C.GORSE_B200_ERR_UNSUPPORTED {
 		log.Logger().Info("gorse_b200 cannot fit this AFM; fitting on the CPU", zap.Error(afmB200Error(st)))
 		return fm.fitCPU(ctx, trainSet, testSet, config)
@@ -322,7 +392,7 @@ func (fm *AFM) Fit(ctx context.Context, trainSet, testSet dataset.CTRSplit, conf
 		return Score{}
 	}
 	o := 0
-	for _, t := range fm.Parameters() { // B, V, W: the layout params_in had
+	for _, t := range fm.Parameters() { // B, V, W, then every slot's H, AW, Ab, EW, Eb: the layout params_in had
 		o += copy(t.Data(), out[o:])
 	}
 	if res.cancelled != 0 {

@@ -608,9 +608,9 @@ class FMRanker:
 
 
 class FMTrainer:
-    """AFM.Fit (model/ctr/fm.go:307-417) on the GPU for a model without embedding slots (gorse_b200_fm_fit).  The rows are
-    CSRs (off int64 [n + 1], idx int32, val float32, already through fm.Scalers) with float32 targets; params_in is
-    fm.Parameters() after Init (B, V, W), the layout FMRanker takes."""
+    """AFM.Fit (model/ctr/fm.go:307-417) on the GPU: fit() for a model without embedding slots (gorse_b200_fm_fit), fit_emb()
+    for one with them (gorse_b200_fm_fit_emb).  The rows are CSRs (off int64 [n + 1], idx int32, val float32, already
+    through fm.Scalers) with float32 targets; params_in is fm.Parameters() after Init, the layout FMRanker takes."""
 
     def __init__(self, ctx, n_features, num_dimension, n_factors=16, n_epochs=50, lr=0.001, reg=0.0002, optimizer=FM_ADAM,
                  batch_size=1024, verbose=10, patience=10, max_steps=0, n_emb=0):
@@ -621,9 +621,19 @@ class FMTrainer:
     def n_params(self):
         return 1 + self.n_features * self.params.n_factors + self.n_features
 
+    def fit_emb(self, train, test, params_in, emb_dims, item_emb, item_emb_mask, train_emb_row, test_emb_row, progress=None,
+                moments=False):
+        """fit() for a model with item-embedding slots: emb_dims [n_emb]; item_emb[s] = bf16 bits uint16 [n_rows, dim_s];
+        item_emb_mask uint8 [n_rows, n_emb] or None (all present); train_emb_row / test_emb_row int32: the table row of
+        every sample, -1 for none.  params_in holds B, V, W, then per slot H, AW, Ab, EW, Eb."""
+        return self._fit(train, test, params_in, progress, moments, (emb_dims, item_emb, item_emb_mask, train_emb_row, test_emb_row))
+
     def fit(self, train, test, params_in, progress=None, moments=False):
         """train / test = (off, idx, val, target); progress(epoch, n_epochs, auc) -> truthy to cancel.
         -> (params float32 [n_params], result dict, moments float32 [2, n_params] or None)"""
+        return self._fit(train, test, params_in, progress, moments, None)
+
+    def _fit(self, train, test, params_in, progress, moments, _emb):
         def rows(r):
             off, idx, val, tgt = r
             off = np.ascontiguousarray(off, np.int64)
@@ -632,15 +642,34 @@ class FMTrainer:
 
         tr, te = rows(train), rows(test)
         pin = np.ascontiguousarray(params_in, np.float32).reshape(-1)
-        if pin.size != self.n_params():
-            raise ValueError(f"params_in holds {pin.size} floats, the model has {self.n_params()}")
+        want = self.n_params() + (sum(self.params.n_factors * (3 * int(d) + 2) for d in _emb[0]) if _emb else 0)
+        if pin.size != want:
+            raise ValueError(f"params_in holds {pin.size} floats, the model has {want}")
         pout = np.zeros(max(pin.size, 1), np.float32)
         mom = np.zeros((2, pin.size), np.float32) if moments else None
         res = _lib.FMFitResult()
         cb = _lib.PROGRESS_FN(lambda user, ep, n, auc: int(bool(progress(ep, n, auc)))) if progress else None
-        check(lib.gorse_b200_fm_fit(self.ctx.h, self.n_features, self.num_dimension, self.n_emb, C.byref(self.params), tr[0], ptr(tr[1]),
-                                    ptr(tr[2]), ptr(tr[3]), ptr(tr[4]), te[0], ptr(te[1]), ptr(te[2]), ptr(te[3]), ptr(te[4]), ptr(pin),
-                                    pin.size, ptr(pout), ptr(mom), cb, None, C.byref(res)))
+        if _emb is None:
+            check(lib.gorse_b200_fm_fit(self.ctx.h, self.n_features, self.num_dimension, self.n_emb, C.byref(self.params), tr[0], ptr(tr[1]),
+                                        ptr(tr[2]), ptr(tr[3]), ptr(tr[4]), te[0], ptr(te[1]), ptr(te[2]), ptr(te[3]), ptr(te[4]), ptr(pin),
+                                        pin.size, ptr(pout), ptr(mom), cb, None, C.byref(res)))
+        else:
+            dims = np.ascontiguousarray(list(_emb[0]), np.int32)
+            tabs = [np.ascontiguousarray(t, np.uint16) for t in _emb[1]]
+            if len(tabs) != dims.size or any(t.ndim != 2 or t.shape[1] != d or t.shape[0] != tabs[0].shape[0] for t, d in zip(tabs, dims)):
+                raise ValueError("item_emb needs one [n_rows, dim] table per slot")
+            n_rows = tabs[0].shape[0] if tabs else 0
+            mask = None if _emb[2] is None else np.ascontiguousarray(_emb[2], np.uint8)
+            if mask is not None and mask.shape != (n_rows, dims.size):
+                raise ValueError("item_emb_mask must be [n_rows, n_emb]")
+            er = [np.ascontiguousarray(r, np.int32).reshape(-1) for r in _emb[3:5]]
+            if er[0].size != tr[0] or er[1].size != te[0]:
+                raise ValueError("one table row per training and per test sample")
+            arr = (C.c_void_p * max(len(tabs), 1))(*[ptr(t) for t in tabs])
+            check(lib.gorse_b200_fm_fit_emb(self.ctx.h, self.n_features, self.num_dimension, C.byref(self.params), tr[0], ptr(tr[1]), ptr(tr[2]),
+                                            ptr(tr[3]), ptr(tr[4]), ptr(er[0]), te[0], ptr(te[1]), ptr(te[2]), ptr(te[3]), ptr(te[4]),
+                                            ptr(er[1]), dims.size, ptr(dims), n_rows, arr, ptr(mask), ptr(pin), pin.size, ptr(pout), ptr(mom),
+                                            cb, None, C.byref(res)))
         out = {f: getattr(res, f) for f, _ in _lib.FMFitResult._fields_}
         return pout[:pin.size], out, mom
 

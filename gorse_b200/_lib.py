@@ -105,6 +105,8 @@ PROTOTYPES = {
     "gorse_b200_fm_fit_params_default": (C.c_int32, [VP]),
     "gorse_b200_fm_fit": (C.c_int32, [VP, C.c_int64, C.c_int32, C.c_int32, VP, C.c_int64, VP, VP, VP, VP, C.c_int64, VP, VP, VP, VP, VP, C.c_int64,
                                       VP, VP, VP, VP, VP]),
+    "gorse_b200_fm_fit_emb": (C.c_int32, [VP, C.c_int64, C.c_int32, VP, C.c_int64, VP, VP, VP, VP, VP, C.c_int64, VP, VP, VP, VP, VP, C.c_int32,
+                                          VP, C.c_int64, VP, VP, VP, C.c_int64, VP, VP, VP, VP, VP]),
     "gorse_b200_ncf_load":(C.c_int32, [C.c_char_p, C.c_char_p, PVP]),
     "gorse_b200_ncf_shape": (C.c_int32, [VP, C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.POINTER(C.c_int64), C.POINTER(C.c_int64),
                                          C.POINTER(C.c_int64)]),

@@ -1,4 +1,5 @@
-// fm_fit.cu -- FM training: gorse_b200_fm_fit, AFM.Fit (model/ctr/fm.go:307-417) for models without embedding slots.
+// fm_fit.cu -- FM training: gorse_b200_fm_fit, AFM.Fit (model/ctr/fm.go:307-417) for models without embedding slots, and
+// gorse_b200_fm_fit_emb for models with them (the slots' kernels and what they add to a step: fm_fit_emb.cuh).
 //
 // The reference's fit is deterministic: each epoch walks the training rows in dataset order in batches, with no
 // shuffling, and only the initial parameters come from Go's RNG (the caller hands them over).  So every step here forms
@@ -92,18 +93,43 @@ __global__ void fm_fit_predict_kernel(const float *P, int64_t nf, int k, Rows R,
 // dL/d(squareSum) of a row from its dL/dsum: Sub's second input gets 0 - dy
 __device__ __forceinline__ float dss_b(float dsub) { return __fsub_rn(0.0f, dsub); }
 
-// forward, BCEWithLogits and its backward for rows [r0, r0 + B)
+constexpr int MAX_SLOTS = 8;
+constexpr int MAX_EMB_DIM = 1024;
+
+// The order in which Tensor.Backward hands vx its gradients in the graph with n slots: 0 is Square(vx)'s, 1 + s is slot s's
+// BMM(vx, enc).  The ops of equal generation leave the container/heap in this order (the restatement replays the heap:
+// fmf_backward_order); the terms are added in it, and fp32 addition does not associate.
+constexpr int8_t VX_ORDER[MAX_SLOTS + 1][MAX_SLOTS + 1] = {
+    {0}, {1, 0}, {2, 1, 0}, {1, 3, 2, 0}, {3, 4, 2, 1, 0}, {4, 5, 1, 2, 3, 0}, {3, 6, 4, 2, 5, 1, 0}, {7, 4, 2, 5, 3, 1, 6, 0},
+    {8, 5, 6, 2, 1, 4, 3, 7, 0}};
+
+struct SlotLogits {              // what the slots leave for the loss: the rows' logits and vx, and every slot's enc
+    const float *p, *vx;
+    const float *enc[MAX_SLOTS];
+    int n;
+    int8_t ord[MAX_SLOTS + 1];
+};
+
+// forward, BCEWithLogits and its backward for rows [r0, r0 + B).  EMB: the forward (with the slots' terms) has already run
+// and left p and vx in L; vx's gradient then collects Square's term and every slot's enc dp in L.ord's order.
+template <bool EMB>
 __global__ void __launch_bounds__(WARPS * 32) fm_fit_forward_kernel(const float *P, int64_t nf, int k, Rows R, const float *tgt,
                                                                    int64_t bs, int64_t n, int s, float *g, float *dss, float *dvx,
-                                                                   float *loss, const int32_t *row_len, int32_t *padnan, const int64_t *t_base)
+                                                                   float *loss, const int32_t *row_len, int32_t *padnan, const int64_t *t_base,
+                                                                   const __grid_constant__ SlotLogits L)
 {
     const int lane = threadIdx.x & 31;
     const int64_t r0 = (int64_t)s * bs;
     const int B = (int)(n - r0 < bs ? n - r0 : bs);
     const float m = __fdiv_rn(1.0f, (float)B);                  // Mean's backward: dy / len
     for (int b = blockIdx.x * WARPS + (threadIdx.x >> 5); b < B; b += gridDim.x * WARPS) {
-        float vx;
-        const float p = row_forward(P, nf, k, R, r0 + b, lane, vx);
+        float vx, p;
+        if (EMB) {
+            p = L.p[b];
+            vx = lane < k ? L.vx[(int64_t)b * k + lane] : 0.0f;
+        } else {
+            p = row_forward(P, nf, k, R, r0 + b, lane, vx);
+        }
         const float t = tgt[r0 + b];
         const float y = __fdiv_rn(__fadd_rn(t, 1.0f), 2.0f);    // Div(Add(1, target), 2)
         const float a = p < 0.0f ? -p : p;                       // Abs
@@ -123,7 +149,15 @@ __global__ void __launch_bounds__(WARPS * 32) fm_fit_forward_kernel(const float 
             g[b] = gp;
             dss[b] = dss_b(dsub);
         }
-        const float dvx_f = __fmul_rn(__fmul_rn(vx, dsub), 2.0f);
+        float dvx_f = __fmul_rn(__fmul_rn(vx, dsub), 2.0f);
+        if (EMB && lane < k) {
+            const float sq = dvx_f, dp = __fadd_rn(0.0f, gp);   // Add(fmOutput, .): the slot's dot gets 0 + dp
+            for (int q = 0; q <= L.n; q++) {
+                const int o = L.ord[q];
+                const float term = o == 0 ? sq : __fmaf_rn(L.enc[o - 1][(int64_t)b * k + lane], dp, 0.0f);   // enc dp^T, a dot of length 1
+                dvx_f = q == 0 ? term : __fadd_rn(dvx_f, term);
+            }
+        }
         if (lane < k) dvx[(int64_t)b * k + lane] = dvx_f;
         // A padded position (index 0, value 0) adds fma(0, dvx, 0) + (V[0] fma(0, dss, 0)) 2 to V's row 0 and fma(0, g, 0)
         // to W's: +0, a no-op on a sum that starts at +0, or NaN when dvx, dss, g or V[0] is not finite.  So the padding
@@ -222,6 +256,28 @@ struct Opt {
     const float *lr_tab;   // Adam's step size per global step
 };
 
+// element e of the parameters, the i-th of a tensor of n, through Adam or SGD
+__device__ __forceinline__ void opt_element(float *P, float *M, float *Vm, int64_t e, float grad, int64_t i, int64_t n, float lr, const Opt &o)
+{
+    const float p = P[e];
+    float b1 = mca(p, o.wd, grad, i, n);             // MulConstAddTo: grad + wd p
+    if (!o.adam) {
+        P[e] = mca(b1, -lr, p, i, n);
+        return;
+    }
+    float m = M[e], v = Vm[e];
+    float b2 = __fsub_rn(b1, m);                     // SubTo
+    m = mca(b2, o.c1, m, i, n);                      // m += (1 - beta1) (grad - m)
+    b2 = __fmul_rn(b1, b1);                          // MulTo
+    b2 = __fsub_rn(b2, v);                           // Sub
+    v = mca(b2, o.c2, v, i, n);                      // v += (1 - beta2) (grad^2 - v)
+    b2 = __fadd_rn(__fsqrt_rn(v), o.eps);            // SqrtTo, AddConst
+    b1 = __fdiv_rn(m, b2);                           // DivTo
+    P[e] = mca(b1, -lr, p, i, n);                    // MulConstAdd(., -lr, param)
+    M[e] = m;
+    Vm[e] = v;
+}
+
 // one optimiser step over B, V and W: the elementwise sequences of optimizers.go:138-151 (Adam) and :78-79 (SGD)
 __global__ void fm_fit_opt_kernel(float *P, float *M, float *Vm, int64_t nf, int k, const float *gV, const float *gW, const float *gB,
                                   const int32_t *stamp, const int64_t *t_base, int s, Opt o)
@@ -235,25 +291,32 @@ __global__ void fm_fit_opt_kernel(float *P, float *M, float *Vm, int64_t nf, int
         if (e == 0) { i = 0; n = 1; grad = *gB; }
         else if (e <= nV) { i = e - 1; n = nV; grad = stamp[i / k] == (int32_t)t ? gV[i] : 0.0f; }
         else { i = e - 1 - nV; n = nf; grad = stamp[i] == (int32_t)t ? gW[i] : 0.0f; }
-        const float p = P[e];
-        float b1 = mca(p, o.wd, grad, i, n);             // MulConstAddTo: grad + wd p
-        if (!o.adam) {
-            P[e] = mca(b1, -lr, p, i, n);
-            continue;
-        }
-        float m = M[e], v = Vm[e];
-        float b2 = __fsub_rn(b1, m);                     // SubTo
-        m = mca(b2, o.c1, m, i, n);                      // m += (1 - beta1) (grad - m)
-        b2 = __fmul_rn(b1, b1);                          // MulTo
-        b2 = __fsub_rn(b2, v);                           // Sub
-        v = mca(b2, o.c2, v, i, n);                      // v += (1 - beta2) (grad^2 - v)
-        b2 = __fadd_rn(__fsqrt_rn(v), o.eps);            // SqrtTo, AddConst
-        b1 = __fdiv_rn(m, b2);                           // DivTo
-        P[e] = mca(b1, -lr, p, i, n);                    // MulConstAdd(., -lr, param)
-        M[e] = m;
-        Vm[e] = v;
+        opt_element(P, M, Vm, e, grad, i, n, lr, o);
     }
 }
+
+struct SlotTensors {             // the 5 tensors of every slot in parameter order: where each ends, counted from the first
+    int32_t end[5 * MAX_SLOTS];
+    int n;
+};
+
+// the same step over the slots' tensors (dense gradients gS, laid out as the parameters from `base`); the fusing rule
+// takes each element's index in its own tensor
+__global__ void fm_fit_emb_opt_kernel(float *P, float *M, float *Vm, int64_t base, const float *gS, SlotTensors T, const int64_t *t_base, int s,
+                                      Opt o)
+{
+    const int64_t t = *t_base + s + 1;
+    const float lr = o.adam ? o.lr_tab[t - 1] : o.sgd_lr;
+    const int32_t total = T.end[T.n - 1];
+    for (int32_t e = blockIdx.x * blockDim.x + threadIdx.x; e < total; e += gridDim.x * blockDim.x) {
+        int q = 0;
+        while (e >= T.end[q]) q++;
+        const int32_t start = q ? T.end[q - 1] : 0;
+        opt_element(P, M, Vm, base + e, gS[e], e - start, T.end[q] - start, lr, o);
+    }
+}
+
+#include "fm_fit_emb.cuh"
 
 __global__ void fm_fit_set_kernel(int64_t *dst, int64_t v) { *dst = v; }
 
@@ -363,8 +426,8 @@ struct Buf : DevBuf<T> {
     }
 };
 
-struct TestSet {                  // one list of EvaluateClassification: padded rows and their predictions
-    Buf<int32_t> idx;
+struct TestSet {                  // one list of EvaluateClassification: padded rows, their table rows and their predictions
+    Buf<int32_t> idx, emb_row;
     Buf<float> val, pred, sorted;
     int64_t n = 0;
     int32_t D = 0;
@@ -417,6 +480,15 @@ using namespace gb::fmfit;
 
 namespace {
 
+struct EmbArgs {                  // the item-embedding side of gorse_b200_fm_fit_emb
+    int32_t n_emb;
+    const int32_t *dim;
+    int64_t n_rows;
+    const uint16_t *const *table;
+    const uint8_t *mask;
+    const int32_t *train_row, *test_row;
+};
+
 struct Fit {
     gorse_b200_ctx *ctx;
     cudaStream_t st;
@@ -440,8 +512,23 @@ struct Fit {
     Buf<float> auc_sum;
     Buf<unsigned char> cub_tmp;
 
+    // item-embedding slots
+    int n_emb = 0;
+    int64_t base = 0;             // parameters before the first slot
+    Buf<uint16_t> table[MAX_SLOTS];
+    Buf<uint8_t> mask;
+    Buf<int32_t> tr_row;
+    Buf<float> s_e[MAX_SLOTS], s_y[MAX_SLOTS], s_att[MAX_SLOTS], s_h[MAX_SLOTS], s_enc[MAX_SLOTS];
+    Buf<float> zmax, rowsum, gx, denc, dh, sumdx, p, vx, gS;
+    Slot slot[MAX_SLOTS];
+    SlotTensors tens{};
+    SlotLogits logits{};
+    unsigned row_grid = 1;
+
     int32_t upload_train(const int64_t *off, const int32_t *idx, const float *val, const float *tgt);
-    int32_t upload_test(const int64_t *off, const int32_t *idx, const float *val, const float *tgt, int64_t n);
+    int32_t upload_test(const int64_t *off, const int32_t *idx, const float *val, const float *tgt, int64_t n, const int32_t *emb_row);
+    int32_t setup_slots(const EmbArgs &E, size_t rows);
+    int32_t slots_forward(const int32_t *emb_row, Batch T, float *logit);
     int32_t run_steps(int s0, int s1);
     int32_t evaluate(float *score);
 };
@@ -518,7 +605,7 @@ int32_t Fit::upload_train(const int64_t *off, const int32_t *idx, const float *v
     return GORSE_B200_OK;
 }
 
-int32_t Fit::upload_test(const int64_t *off, const int32_t *idx, const float *val, const float *tgt, int64_t n)
+int32_t Fit::upload_test(const int64_t *off, const int32_t *idx, const float *val, const float *tgt, int64_t n, const int32_t *emb_row)
 {
     std::vector<int64_t> rows[2];
     for (int64_t r = 0; r < n; r++) rows[tgt[r] > 0 ? 0 : 1].push_back(r);
@@ -532,6 +619,11 @@ int32_t Fit::upload_test(const int64_t *off, const int32_t *idx, const float *va
         pad_rows(off, idx, val, rows[s], T.D, pi, pv);
         GB_TRY(T.idx.put(pi, st));
         GB_TRY(T.val.put(pv, st));
+        if (emb_row) {
+            std::vector<int32_t> er(rows[s].size());
+            for (size_t i = 0; i < er.size(); i++) er[i] = emb_row[rows[s][i]];
+            GB_TRY(T.emb_row.put(er, st));
+        }
         GB_TRY(T.pred.alloc((size_t)std::max<int64_t>(T.n, 1)));
         GB_TRY(T.sorted.alloc((size_t)std::max<int64_t>(T.n, 1)));
         most = std::max(most, T.n);
@@ -555,8 +647,18 @@ int32_t Fit::evaluate(float *score)
         TestSet &T = te[s];
         if (T.n == 0) continue;
         const unsigned grid = (unsigned)std::min<int64_t>(div_up(T.n, WARPS), (int64_t)ctx->sm_count * 16);
-        fm_fit_predict_kernel<<<grid, WARPS * 32, 0, st>>>(Pp, nf, k, Rows{T.idx.p, T.val.p, T.D}, T.n, T.pred.p);
-        GB_LAUNCHED(ctx);
+        if (n_emb == 0) {
+            fm_fit_predict_kernel<<<grid, WARPS * 32, 0, st>>>(Pp, nf, k, Rows{T.idx.p, T.val.p, T.D}, T.n, T.pred.p);
+            GB_LAUNCHED(ctx);
+        } else {   // BatchInternalPredict's chunks of batch_size rows, each with its own softmax coupling
+            const int64_t bs = prm->batch_size;
+            for (int64_t ch = 0; ch * bs < T.n; ch++) {
+                const Batch C{bs, T.n, (int)ch};
+                fm_fit_emb_base_kernel<<<row_grid, WARPS * 32, 0, st>>>(Pp, nf, k, Rows{T.idx.p, T.val.p, T.D}, C, T.pred.p + ch * bs, vx.p);
+                GB_LAUNCHED(ctx);
+                GB_TRY(slots_forward(T.emb_row.p, C, T.pred.p + ch * bs));
+            }
+        }
         size_t bytes = cub_tmp.n;
         GB_CUDA(cub::DeviceRadixSort::SortKeys(cub_tmp.p, bytes, T.pred.p, T.sorted.p, (int)T.n, 0, 32, st));
     }
@@ -589,14 +691,90 @@ int32_t Fit::run_steps(int s0, int s1)
     const unsigned fwd_grid = (unsigned)div_up(std::min<int64_t>(bs, n_train), WARPS);
     const unsigned opt_grid = (unsigned)std::min<int64_t>(div_up(n_params, 256), (int64_t)ctx->sm_count * 8);
     for (int s = s0; s < s1; s++) {
-        fm_fit_forward_kernel<<<fwd_grid, WARPS * 32, 0, st>>>(P.p, nf, k, R, tr_tgt.p, bs, n_train, s, g.p, dss.p, dvx.p, loss.p,
-                                                                tr_len.p, padnan.p, t_base.p);
-        GB_LAUNCHED(ctx);
+        const Batch T{bs, n_train, s};
+        if (n_emb == 0) {
+            fm_fit_forward_kernel<false><<<fwd_grid, WARPS * 32, 0, st>>>(P.p, nf, k, R, tr_tgt.p, bs, n_train, s, g.p, dss.p, dvx.p, loss.p,
+                                                                           tr_len.p, padnan.p, t_base.p, logits);
+            GB_LAUNCHED(ctx);
+        } else {
+            fm_fit_emb_base_kernel<<<row_grid, WARPS * 32, 0, st>>>(P.p, nf, k, R, T, p.p, vx.p);
+            GB_LAUNCHED(ctx);
+            GB_TRY(slots_forward(tr_row.p, T, p.p));
+            fm_fit_forward_kernel<true><<<fwd_grid, WARPS * 32, 0, st>>>(P.p, nf, k, R, tr_tgt.p, bs, n_train, s, g.p, dss.p, dvx.p, loss.p,
+                                                                          tr_len.p, padnan.p, t_base.p, logits);
+            GB_LAUNCHED(ctx);
+        }
         fm_fit_grad_kernel<<<grad_grid, WARPS * 32, 0, st>>>(P.p, nf, k, R, bs, n_train, s, batch_seg.p, seg_start.p, seg_feat.p, seg_pos.p,
                                                              g.p, dss.p, dvx.p, loss.p, gV.p, gW.p, gB.p, stamp.p, batch_loss.p, t_base.p,
                                                              padnan.p);
         GB_LAUNCHED(ctx);
+        for (int q = 0; q < n_emb; q++) {
+            fm_fit_emb_datt_kernel<<<row_grid, WARPS * 32, 0, st>>>(slot[q], k, T, vx.p, g.p);
+            GB_LAUNCHED(ctx);
+            fm_fit_emb_dh_kernel<<<row_grid, WARPS * 32, 0, st>>>(slot[q], k, T);
+            GB_LAUNCHED(ctx);
+            fm_fit_emb_wgrad_kernel<<<(unsigned)div_up(2 * (int64_t)slot[q].dim * k + 2 * k, 128), 128, 0, st>>>(slot[q], k, T);
+            GB_LAUNCHED(ctx);
+        }
         fm_fit_opt_kernel<<<opt_grid, 256, 0, st>>>(P.p, M.p, Vm.p, nf, k, gV.p, gW.p, gB.p, stamp.p, t_base.p, s, o);
+        GB_LAUNCHED(ctx);
+        if (n_emb > 0) {
+            fm_fit_emb_opt_kernel<<<(unsigned)div_up((int64_t)tens.end[tens.n - 1], 256), 256, 0, st>>>(P.p, M.p, Vm.p, base, gS.p, tens, t_base.p,
+                                                                                                      s, o);
+            GB_LAUNCHED(ctx);
+        }
+    }
+    return GORSE_B200_OK;
+}
+
+// the table, and per slot the batch's tensors (rows: the largest batch or evaluation chunk) and the parameter pointers
+int32_t Fit::setup_slots(const EmbArgs &E, size_t rows)
+{
+    n_emb = E.n_emb;
+    base = 1 + nf * k + nf;
+    if (n_emb == 0) return GORSE_B200_OK;
+    row_grid = (unsigned)div_up((int64_t)rows, WARPS);
+    int maxdim = 1;
+    int64_t total = 0;
+    for (int s = 0; s < n_emb; s++) {
+        maxdim = std::max(maxdim, E.dim[s]);
+        const int64_t kd = (int64_t)k * E.dim[s], len[5] = {kd, kd, k, kd, k};
+        for (int q = 0; q < 5; q++) tens.end[tens.n++] = (int32_t)(total += len[q]);
+    }
+    if (E.mask) GB_TRY(mask.put(std::vector<uint8_t>(E.mask, E.mask + E.n_rows * n_emb), st));
+    GB_TRY(tr_row.put(std::vector<int32_t>(E.train_row, E.train_row + n_train), st));
+    GB_TRY(gS.alloc((size_t)total));
+    for (auto *b : {&zmax, &rowsum, &sumdx, &p}) GB_TRY(b->alloc(rows));
+    for (auto *b : {&denc, &dh, &vx}) GB_TRY(b->alloc(rows * k));
+    GB_TRY(gx.alloc(rows * maxdim));
+    int64_t o = base;
+    logits = SlotLogits{p.p, vx.p, {}, n_emb, {}};
+    for (int q = 0; q <= n_emb; q++) logits.ord[q] = VX_ORDER[n_emb][q];
+    for (int s = 0; s < n_emb; s++) {
+        const int d = E.dim[s];
+        const int64_t kd = (int64_t)k * d;
+        GB_TRY(table[s].put(std::vector<uint16_t>(E.table[s], E.table[s] + E.n_rows * d), st));
+        for (auto *b : {&s_e[s], &s_y[s], &s_att[s]}) GB_TRY(b->alloc(rows * d));
+        for (auto *b : {&s_h[s], &s_enc[s]}) GB_TRY(b->alloc(rows * k));
+        float *w = P.p + o, *gw = gS.p + (o - base);
+        slot[s] = Slot{w, w + kd, w + 2 * kd, w + 2 * kd + k, w + 3 * kd + k, gw, gw + kd, gw + 2 * kd, gw + 2 * kd + k, gw + 3 * kd + k,
+                       table[s].p, E.mask ? mask.p : nullptr, n_emb, s, d, s_e[s].p, s_y[s].p, s_att[s].p, s_h[s].p, s_enc[s].p,
+                       zmax.p, rowsum.p, gx.p, denc.p, dh.p, sumdx.p};
+        logits.enc[s] = s_enc[s].p;
+        o += 3 * kd + 2 * k;
+    }
+    return GORSE_B200_OK;
+}
+
+// every slot's attention and encoder on the batch, in slot order: `logit` gets + <vx, enc> per slot
+int32_t Fit::slots_forward(const int32_t *emb_row, Batch T, float *logit)
+{
+    for (int q = 0; q < n_emb; q++) {
+        fm_fit_emb_hz_kernel<<<row_grid, WARPS * 32, 0, st>>>(slot[q], k, emb_row, T);
+        GB_LAUNCHED(ctx);
+        fm_fit_emb_exp_kernel<<<row_grid, WARPS * 32, 0, st>>>(slot[q], T);
+        GB_LAUNCHED(ctx);
+        fm_fit_emb_enc_kernel<<<row_grid, WARPS * 32, 0, st>>>(slot[q], k, T, vx.p, logit);
         GB_LAUNCHED(ctx);
     }
     return GORSE_B200_OK;
@@ -622,12 +800,13 @@ extern "C" int32_t gorse_b200_fm_fit_params_default(gorse_b200_fm_fit_params *p)
     return GORSE_B200_OK;
 }
 
-extern "C" int32_t gorse_b200_fm_fit(gorse_b200_ctx *ctx, int64_t n_features, int32_t num_dimension, int32_t n_emb,
-                                     const gorse_b200_fm_fit_params *params, int64_t n_train, const int64_t *train_off, const int32_t *train_idx,
-                                     const float *train_val, const float *train_target, int64_t n_test, const int64_t *test_off,
-                                     const int32_t *test_idx, const float *test_val, const float *test_target, const float *params_in,
-                                     int64_t n_params, float *params_out, float *moments_out, gorse_b200_progress_fn progress, void *user,
-                                     gorse_b200_fm_fit_result *result)
+namespace {
+// E == nullptr: gorse_b200_fm_fit, which takes no embeddings and so no model with slots
+int32_t fit_run(gorse_b200_ctx *ctx, int64_t n_features, int32_t num_dimension, int32_t n_emb, const EmbArgs *E,
+                const gorse_b200_fm_fit_params *params, int64_t n_train, const int64_t *train_off, const int32_t *train_idx,
+                const float *train_val, const float *train_target, int64_t n_test, const int64_t *test_off, const int32_t *test_idx,
+                const float *test_val, const float *test_target, const float *params_in, int64_t n_params, float *params_out,
+                float *moments_out, gorse_b200_progress_fn progress, void *user, gorse_b200_fm_fit_result *result)
 {
     GB_CHECK_ARG(ctx != nullptr && params != nullptr && result != nullptr, "NULL ctx/params/result");
     *result = gorse_b200_fm_fit_result{};
@@ -635,15 +814,38 @@ extern "C" int32_t gorse_b200_fm_fit(gorse_b200_ctx *ctx, int64_t n_features, in
     GB_CHECK_ARG(num_dimension >= 0 && n_emb >= 0, "negative num_dimension or n_emb");
     GB_TRY(check_params(params));
     GB_CHECK_ARG(params_in != nullptr && params_out != nullptr, "NULL params_in/params_out");
-    if (n_emb > 0 || params->n_factors > MAX_FACTORS) {
+    if ((n_emb > 0 && !E) || params->n_factors > MAX_FACTORS) {
         set_error("fm_fit: %d embedding slots (none supported) or n_factors %d (at most %d)", n_emb, params->n_factors, MAX_FACTORS);
         return GORSE_B200_ERR_UNSUPPORTED;
+    }
+    int64_t want = 1 + n_features * (int64_t)params->n_factors + n_features;
+    if (n_emb > 0) {
+        GB_CHECK_ARG(E->dim != nullptr && E->table != nullptr && E->n_rows >= 0, "NULL emb_dim or item_emb, or a negative n_emb_rows");
+        if (n_emb > MAX_SLOTS) {
+            set_error("fm_fit_emb: %d embedding slots, at most %d", n_emb, MAX_SLOTS);
+            return GORSE_B200_ERR_UNSUPPORTED;
+        }
+        for (int s = 0; s < n_emb; s++) {
+            GB_CHECK_ARG(E->dim[s] >= 1, "embedding slot %d: dim %d", s, E->dim[s]);
+            if (E->dim[s] > MAX_EMB_DIM) {
+                set_error("fm_fit_emb: embedding slot %d has dim %d, at most %d", s, E->dim[s], MAX_EMB_DIM);
+                return GORSE_B200_ERR_UNSUPPORTED;
+            }
+            GB_CHECK_ARG(E->n_rows == 0 || E->table[s] != nullptr, "item_emb[%d] is NULL", s);
+            want += 3 * (int64_t)params->n_factors * E->dim[s] + 2 * (int64_t)params->n_factors;
+        }
+        GB_CHECK_ARG((n_train == 0 || E->train_row != nullptr) && (n_test == 0 || E->test_row != nullptr), "NULL train_emb_row or test_emb_row");
+        for (int64_t i = 0; i < n_train; i++)
+            GB_CHECK_ARG(E->train_row[i] >= -1 && E->train_row[i] < E->n_rows, "train row %lld: table row %d is not -1 or in [0, %lld)",
+                         (long long)i, E->train_row[i], (long long)E->n_rows);
+        for (int64_t i = 0; i < n_test; i++)
+            GB_CHECK_ARG(E->test_row[i] >= -1 && E->test_row[i] < E->n_rows, "test row %lld: table row %d is not -1 or in [0, %lld)",
+                         (long long)i, E->test_row[i], (long long)E->n_rows);
     }
     GB_TRY(check_rows("train", n_train, train_off, train_idx, train_val, train_target, n_features));
     GB_TRY(check_rows("test", n_test, test_off, test_idx, test_val, test_target, n_features));
     const int k = params->n_factors;
-    GB_CHECK_ARG(n_params == 1 + n_features * k + n_features, "n_params = %lld, the model has %lld", (long long)n_params,
-                 (long long)(1 + n_features * k + n_features));
+    GB_CHECK_ARG(n_params == want, "n_params = %lld, the model has %lld", (long long)n_params, (long long)want);
     const int64_t bs = params->batch_size, n_batches = (n_train + bs - 1) / bs;
     int64_t total_steps = (int64_t)params->n_epochs * n_batches;
     if (params->max_steps > 0) total_steps = std::min<int64_t>(total_steps, params->max_steps);
@@ -663,7 +865,7 @@ extern "C" int32_t gorse_b200_fm_fit(gorse_b200_ctx *ctx, int64_t n_features, in
     F.n_train = n_train;
     cudaStream_t st = F.st;
     GB_TRY(F.upload_train(train_off, train_idx, train_val, train_target));
-    GB_TRY(F.upload_test(test_off, test_idx, test_val, test_target, n_test));
+    GB_TRY(F.upload_test(test_off, test_idx, test_val, test_target, n_test, n_emb > 0 ? E->test_row : nullptr));
     GB_TRY(F.P.put(std::vector<float>(params_in, params_in + n_params), st));
     GB_TRY(F.M.alloc((size_t)n_params));
     GB_TRY(F.Vm.alloc((size_t)n_params));
@@ -677,6 +879,8 @@ extern "C" int32_t gorse_b200_fm_fit(gorse_b200_ctx *ctx, int64_t n_features, in
     GB_TRY(F.padnan.alloc((size_t)k + 1));
     GB_CUDA(cudaMemsetAsync(F.padnan.p, 0, ((size_t)k + 1) * sizeof(int32_t), st));
     const size_t rows = (size_t)std::max<int64_t>(1, std::min<int64_t>(bs, n_train));
+    if (n_emb > 0)   // the slots also run on the evaluation lists' chunks
+        GB_TRY(F.setup_slots(*E, (size_t)std::max<int64_t>(1, std::min<int64_t>(bs, std::max({n_train, F.te[0].n, F.te[1].n})))));
     GB_TRY(F.g.alloc(rows));
     GB_TRY(F.dss.alloc(rows));
     GB_TRY(F.loss.alloc(rows));
@@ -784,4 +988,29 @@ extern "C" int32_t gorse_b200_fm_fit(gorse_b200_ctx *ctx, int64_t n_features, in
     result->accuracy = score[2];
     result->cost = cost;
     return GORSE_B200_OK;
+}
+}  // namespace
+
+extern "C" int32_t gorse_b200_fm_fit(gorse_b200_ctx *ctx, int64_t n_features, int32_t num_dimension, int32_t n_emb,
+                                     const gorse_b200_fm_fit_params *params, int64_t n_train, const int64_t *train_off, const int32_t *train_idx,
+                                     const float *train_val, const float *train_target, int64_t n_test, const int64_t *test_off,
+                                     const int32_t *test_idx, const float *test_val, const float *test_target, const float *params_in,
+                                     int64_t n_params, float *params_out, float *moments_out, gorse_b200_progress_fn progress, void *user,
+                                     gorse_b200_fm_fit_result *result)
+{
+    return fit_run(ctx, n_features, num_dimension, n_emb, nullptr, params, n_train, train_off, train_idx, train_val, train_target, n_test,
+                   test_off, test_idx, test_val, test_target, params_in, n_params, params_out, moments_out, progress, user, result);
+}
+
+extern "C" int32_t gorse_b200_fm_fit_emb(gorse_b200_ctx *ctx, int64_t n_features, int32_t num_dimension, const gorse_b200_fm_fit_params *params,
+                                         int64_t n_train, const int64_t *train_off, const int32_t *train_idx, const float *train_val,
+                                         const float *train_target, const int32_t *train_emb_row, int64_t n_test, const int64_t *test_off,
+                                         const int32_t *test_idx, const float *test_val, const float *test_target, const int32_t *test_emb_row,
+                                         int32_t n_emb, const int32_t *emb_dim, int64_t n_emb_rows, const uint16_t *const *item_emb,
+                                         const uint8_t *item_emb_mask, const float *params_in, int64_t n_params, float *params_out,
+                                         float *moments_out, gorse_b200_progress_fn progress, void *user, gorse_b200_fm_fit_result *result)
+{
+    const EmbArgs E{n_emb, emb_dim, n_emb_rows, item_emb, item_emb_mask, train_emb_row, test_emb_row};
+    return fit_run(ctx, n_features, num_dimension, n_emb, &E, params, n_train, train_off, train_idx, train_val, train_target, n_test, test_off,
+                   test_idx, test_val, test_target, params_in, n_params, params_out, moments_out, progress, user, result);
 }

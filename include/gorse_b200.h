@@ -438,8 +438,8 @@ int32_t gorse_b200_vecdb_user_to_user(gorse_b200_vecdb *db, int64_t n_users, con
 /* ------------------------------------------------------------------------------------------
  * Batched FM ranking: the worker's "fm" ranker (rankByClickTroughRate, worker/pipeline.go:450-499) for many users in one
  * call -- AFM.BatchPredict (model/ctr/fm.go:180-229) on every (user, candidate) pair of each user, then the candidates by
- * score.  Training is gorse_b200_fm_fit below, for models without embedding slots; a model with slots is still trained by
- * the reference's AFM.Fit.
+ * score.  Training is gorse_b200_fm_fit below for models without embedding slots, and gorse_b200_fm_fit_emb for models
+ * with them.
  * gorse_b200_fm_create uploads one trained model once; the handle is read-only afterwards and thread-safe.
  *   n_features = fm.numFeatures (the unified index's Len), n_factors = nFactors, num_dimension = fm.numDimension,
  *   batch_size = the BatchSize param (default 1024), emb_dim[n_emb] = fm.embeddingDim.
@@ -526,6 +526,30 @@ int32_t gorse_b200_fm_fit(gorse_b200_ctx *ctx, int64_t n_features, int32_t num_d
                           const int32_t *test_idx, const float *test_val, const float *test_target, const float *params_in,
                           int64_t n_params, float *params_out, float *moments_out, gorse_b200_progress_fn progress, void *user,
                           gorse_b200_fm_fit_result *result);
+
+/* FM training of a model with item-embedding slots: the same fit, with the attention and encoder layers of every slot
+ * (common/nn/layers.go:160-185, fm.go:128-132) trained too.  gorse_b200_fm_fit's arguments, its params / result structs
+ * and its progress / cancel / max_steps contract, plus
+ *   n_emb, emb_dim[n_emb] = fm.embeddingDim; n_emb = 0 is gorse_b200_fm_fit, bit for bit.  n_factors above 32, a dim above
+ *   1024 or more than 8 slots: GORSE_B200_ERR_UNSUPPORTED.
+ *   the item-embedding table as gorse_b200_fm_rank takes it: item_emb[s] [n_emb_rows x emb_dim[s]] bf16 bits per slot,
+ *   item_emb_mask[n_emb_rows x n_emb] 1 where the row's embedding of slot s is present (NULL: all present); an absent one
+ *   is a row of zeros (convertToTensors, fm.go:555-561).  A mask that marks the wrong rows cannot be detected.
+ *   train_emb_row[n_train] / test_emb_row[n_test]: the table row of each sample (dataset.Items[i]), -1 = no embeddings
+ *   (zeros in every slot).  The kernels gather from the table.
+ *   params_in / params_out[n_params] in gorse_b200_fm_create's layout: B, V, W, then per slot H, AW, Ab, EW, Eb; a fitted
+ *   model goes straight into gorse_b200_fm_create.  moments_out[2 n_params] as above.
+ * The softmax of a batch, and of every chunk of batch_size rows of the two evaluation lists, couples its rows as the
+ * reference's does, in the forward and in the backward.  Every parameter and moment is bit-identical to the project's CPU
+ * restatement (DESIGN §8.5).  A table row outside [-1, n_emb_rows), a NULL table with n_emb > 0 and a wrong n_params are
+ * GORSE_B200_ERR_ARG, checked on the host before the device is touched. */
+int32_t gorse_b200_fm_fit_emb(gorse_b200_ctx *ctx, int64_t n_features, int32_t num_dimension, const gorse_b200_fm_fit_params *params,
+                              int64_t n_train, const int64_t *train_off, const int32_t *train_idx, const float *train_val,
+                              const float *train_target, const int32_t *train_emb_row, int64_t n_test, const int64_t *test_off,
+                              const int32_t *test_idx, const float *test_val, const float *test_target, const int32_t *test_emb_row,
+                              int32_t n_emb, const int32_t *emb_dim, int64_t n_emb_rows, const uint16_t *const *item_emb,
+                              const uint8_t *item_emb_mask, const float *params_in, int64_t n_params, float *params_out,
+                              float *moments_out, gorse_b200_progress_fn progress, void *user, gorse_b200_fm_fit_result *result);
 
 /* ------------------------------------------------------------------------------------------
  * NCF-format datasets: dataset.LoadDataFromBuiltIn (dataset/dataset.go:398-490), the loader `gorse-bench cf`
