@@ -607,6 +607,145 @@ class FMRanker:
         self.close()
 
 
+def _flat(lists, dtype):
+    off = np.zeros(len(lists) + 1, np.int64)
+    np.cumsum([len(x) for x in lists], out=off[1:])
+    flat = np.ascontiguousarray(np.concatenate([np.asarray(x, dtype).reshape(-1) for x in lists] + [np.zeros(0, dtype)]), dtype)
+    return off, flat
+
+
+class ListStage:
+    """A list recommender of gorse_b200_recommend: non-personalized or latest (items / scores: one list for every user) or
+    external (per_user: one (items, scores) pair per user).  Items are dictionary indices."""
+
+    def __init__(self, items=None, scores=None, per_user=None):
+        self.items, self.scores, self.per_user = items, scores, per_user
+
+
+class CollaborativeStage:
+    """The collaborative recommender: the CF recall row (the `cf` argument of recommend) as the cache would serve it."""
+
+
+class ItemToItemStage:
+    """An item-to-item recommender on `collection`: context_lists[u] are item indices, newest first (-1 = outside the
+    dictionary); slot_of_item [n_items] / item_of_slot [slots] map between the dictionary and the collection."""
+
+    def __init__(self, collection, n, context_lists, slot_of_item, item_of_slot, categories=(), score_scale=1.0):
+        self.collection, self.n, self.context_lists, self.categories, self.score_scale = collection, n, context_lists, categories, score_scale
+        self.slot_of_item, self.item_of_slot = slot_of_item, item_of_slot
+
+
+class UserToUserStage:
+    """A user-to-user recommender on `collection`: user_slots[u] (-1 = no vector), feedback_lists[slot] as item indices,
+    item_ok [n_items] (None: every item passes)."""
+
+    def __init__(self, collection, n, user_slots, feedback_lists, item_ok=None, score_scale=1.0):
+        self.collection, self.n, self.user_slots, self.feedback_lists, self.item_ok, self.score_scale = collection, n, user_slots, feedback_lists, item_ok, score_scale
+
+
+def recommend(ctx, exclude_lists, n_items, item_live, stages, cf=None, ranker=None, replacement=None, positive_decay=1.0, read_decay=1.0):
+    """Batched offline recommendation (gorse_b200_recommend; worker/pipeline.go:124-319): for user u, E0 = exclude_lists[u]
+    (dictionary indices, -1 = an id outside it), the stages in order with one growing exclude set, the live candidates,
+    then with a ranker the replacement items and the FM ranking with the decay.
+    cf: (collection, user_vectors [n_users, dim], slot_of_item, item_of_slot, n) for a CollaborativeStage.
+    ranker: (FMRanker, FMInput of the users and the dictionary's item table; its candidates are ignored).
+    replacement: per user a list of (item, positive) pairs.
+    -> ([(items int32, scores float64) per user], stats {chunks, candidates, table_rows, exact_rows})"""
+    nu = len(exclude_lists)
+    keep = []
+
+    def p(a):
+        if a is None:
+            return None
+        keep.append(a)
+        return a.ctypes.data
+
+    eoff, eitems = _flat(exclude_lists, np.int32)
+    live = np.ascontiguousarray(item_live, np.uint8)
+    arr = (_lib.RecommendStage * max(len(stages), 1))()
+    for i, s in enumerate(stages):
+        d = arr[i]
+        if isinstance(s, ListStage):
+            d.kind = _lib.STAGE_LIST
+            if s.per_user is not None:
+                loff, li = _flat([x[0] for x in s.per_user], np.int32)
+                _, ls = _flat([x[1] for x in s.per_user], np.float64)
+                d.list_off = p(loff)
+            else:
+                li, ls = np.ascontiguousarray(s.items, np.int32), np.ascontiguousarray(s.scores, np.float64)
+                d.list_len = li.size
+            d.list_items, d.list_scores = p(li), p(ls)
+        elif isinstance(s, CollaborativeStage):
+            d.kind = _lib.STAGE_COLLABORATIVE
+        elif isinstance(s, ItemToItemStage):
+            d.kind = _lib.STAGE_ITEM_TO_ITEM
+            d.db, d.n, d.score_scale = s.collection.h.value, int(s.n), float(s.score_scale)
+            coff, citems = _flat(s.context_lists, np.int32)
+            d.ctx_off, d.ctx_items = p(coff), p(citems)
+            d.slot_of_item = p(np.ascontiguousarray(s.slot_of_item, np.int64))
+            d.item_of_slot = p(np.ascontiguousarray(s.item_of_slot, np.int32))
+            cats = np.ascontiguousarray(list(s.categories), np.int32)
+            d.categories, d.n_categories = (p(cats) if cats.size else None), cats.size
+        elif isinstance(s, UserToUserStage):
+            d.kind = _lib.STAGE_USER_TO_USER
+            d.db, d.n, d.score_scale = s.collection.h.value, int(s.n), float(s.score_scale)
+            d.user_slots = p(np.ascontiguousarray(s.user_slots, np.int64))
+            foff, fitems = _flat(s.feedback_lists, np.int32)
+            d.n_fb_rows, d.fb_off, d.fb_items = len(s.feedback_lists), p(foff), p(fitems)
+            d.item_ok = None if s.item_ok is None else p(np.ascontiguousarray(s.item_ok, np.uint8))
+        else:
+            raise TypeError(f"unknown stage {s!r}")
+    cfs = None
+    if cf is not None:
+        coll, vecs, soi, ios, n = cf
+        cfs = _lib.RecommendCF(coll.h.value, p(np.ascontiguousarray(vecs, np.float32)), p(np.ascontiguousarray(soi, np.int64)),
+                               p(np.ascontiguousarray(ios, np.int32)), int(n))
+    rk = None
+    if ranker is not None:
+        fm, inp = ranker
+        i32, i64, f32 = (lambda a: p(np.ascontiguousarray(a, np.int32))), (lambda a: p(np.ascontiguousarray(a, np.int64))), \
+            (lambda a: p(np.ascontiguousarray(a, np.float32)))
+        emb = [np.ascontiguousarray(e, np.uint16) for e in inp.item_emb]
+        keep.extend(emb)
+        embs = (C.c_void_p * max(fm.n_emb, 1))(*[ptr(e) for e in emb])
+        keep.append(embs)
+        mask = None if inp.item_emb_mask is None else np.ascontiguousarray(inp.item_emb_mask, np.uint8)
+        rk = _lib.RecommendRanker(fm.h.value, i32(inp.user_feat), i64(inp.user_lab_off), i32(inp.user_lab_idx), f32(inp.user_lab_val),
+                                  i32(inp.item_feat), i64(inp.item_lab_off), i32(inp.item_lab_idx), f32(inp.item_lab_val),
+                                  C.cast(embs, C.c_void_p).value if emb else None, p(mask))
+    roff = ritems = rpos = None
+    if replacement is not None:
+        roff, ritems = _flat([[it for it, _ in r] for r in replacement], np.int32)
+        _, rpos = _flat([[1 if pos else 0 for _, pos in r] for r in replacement], np.uint8)
+    bound = recommend_bounds(nu, stages, cf, replacement if ranker is not None else None)
+    out_at = np.zeros(nu + 1, np.int64)
+    np.cumsum(bound, out=out_at[1:])
+    total = int(out_at[-1])
+    items, scores, cnt, stats = np.zeros(max(total, 1), np.int32), np.zeros(max(total, 1), np.float64), np.zeros(max(nu, 1), np.int32), np.zeros(4, np.int64)
+    check(lib.gorse_b200_recommend(ctx.h if ctx is not None else None, nu, ptr(eoff), ptr(eitems) if eitems.size else None, int(n_items), ptr(live) if live.size else None,
+                                   len(stages), C.cast(arr, C.c_void_p), C.byref(cfs) if cfs is not None else None,
+                                   C.byref(rk) if rk is not None else None, ptr(roff), ptr(ritems) if ritems is not None and ritems.size else None,
+                                   ptr(rpos) if rpos is not None and rpos.size else None, float(positive_decay), float(read_decay), ptr(items), ptr(scores),
+                                   ptr(cnt), ptr(stats)))
+    rows = [(items[a:a + c].copy(), scores[a:a + c].copy()) for a, c in zip(out_at[:-1], cnt[:nu])]
+    return rows, dict(zip(("chunks", "candidates", "table_rows", "exact_rows"), (int(x) for x in stats)))
+
+
+def recommend_bounds(n_users, stages, cf=None, replacement=None):
+    """B_u of gorse_b200_recommend: the stage bounds (list length, or n) plus the replacement count (ranked calls only)."""
+    b = np.zeros(n_users, np.int64)
+    for s in stages:
+        if isinstance(s, ListStage):
+            b += np.array([len(x[0]) for x in s.per_user], np.int64) if s.per_user is not None else len(s.items)
+        elif isinstance(s, CollaborativeStage):
+            b += max(int(cf[4]), 0) if cf is not None else 0
+        else:
+            b += max(int(s.n), 0)
+    if replacement is not None:
+        b += np.array([len(r) for r in replacement], np.int64)
+    return b
+
+
 class FMTrainer:
     """AFM.Fit (model/ctr/fm.go:307-417) on the GPU: fit() for a model without embedding slots (gorse_b200_fm_fit), fit_emb()
     for one with them (gorse_b200_fm_fit_emb).  The rows are CSRs (off int64 [n + 1], idx int32, val float32, already

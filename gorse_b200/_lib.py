@@ -102,6 +102,8 @@ PROTOTYPES = {
     "gorse_b200_fm_create": (C.c_int32, [VP, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_int32, VP, VP, C.c_int64, PVP]),
     "gorse_b200_fm_destroy": (C.c_int32, [VP]),
     "gorse_b200_fm_rank": (C.c_int32, [VP, C.c_int64, VP, VP, VP, VP, C.c_int64, VP, VP, VP, VP, VP, VP, VP, VP, VP, VP, VP]),
+    "gorse_b200_recommend": (C.c_int32, [VP, C.c_int64, VP, VP, C.c_int32, VP, C.c_int32, VP, VP, VP, VP, VP, VP, C.c_double, C.c_double, VP, VP,
+                                         VP, VP]),
     "gorse_b200_fm_fit_params_default": (C.c_int32, [VP]),
     "gorse_b200_fm_fit": (C.c_int32, [VP, C.c_int64, C.c_int32, C.c_int32, VP, C.c_int64, VP, VP, VP, VP, C.c_int64, VP, VP, VP, VP, VP, C.c_int64,
                                       VP, VP, VP, VP, VP]),
@@ -138,6 +140,26 @@ class FMFitResult(C.Structure):
     _fields_ = [("auc", C.c_float), ("precision", C.c_float), ("recall", C.c_float), ("accuracy", C.c_float), ("cost", C.c_float),
                 ("epochs_run", C.c_int32), ("best_epoch", C.c_int32), ("early_stopped", C.c_int32), ("diverged", C.c_int32),
                 ("cancelled", C.c_int32), ("steps", C.c_int64)]
+
+
+STAGE_LIST, STAGE_COLLABORATIVE, STAGE_ITEM_TO_ITEM, STAGE_USER_TO_USER = 0, 1, 2, 3
+
+
+class RecommendStage(C.Structure):
+    _fields_ = [("kind", C.c_int32), ("list_len", C.c_int64), ("list_off", C.c_void_p), ("list_items", C.c_void_p), ("list_scores", C.c_void_p),
+                ("db", C.c_void_p), ("n", C.c_int32), ("score_scale", C.c_double), ("ctx_off", C.c_void_p), ("ctx_items", C.c_void_p),
+                ("slot_of_item", C.c_void_p), ("item_of_slot", C.c_void_p), ("categories", C.c_void_p), ("n_categories", C.c_int32),
+                ("user_slots", C.c_void_p), ("n_fb_rows", C.c_int64), ("fb_off", C.c_void_p), ("fb_items", C.c_void_p), ("item_ok", C.c_void_p)]
+
+
+class RecommendCF(C.Structure):
+    _fields_ = [("db", C.c_void_p), ("user_vectors", C.c_void_p), ("slot_of_item", C.c_void_p), ("item_of_slot", C.c_void_p), ("n", C.c_int32)]
+
+
+class RecommendRanker(C.Structure):
+    _fields_ = [("fm", C.c_void_p), ("user_feat", C.c_void_p), ("user_lab_off", C.c_void_p), ("user_lab_idx", C.c_void_p),
+                ("user_lab_val", C.c_void_p), ("item_feat", C.c_void_p), ("item_lab_off", C.c_void_p), ("item_lab_idx", C.c_void_p),
+                ("item_lab_val", C.c_void_p), ("item_emb", C.c_void_p), ("item_emb_mask", C.c_void_p)]
 
 
 PROGRESS_FN = C.CFUNCTYPE(C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_float)

@@ -93,7 +93,12 @@ struct gorse_b200_ctx {
     void *flush_buf = nullptr;
     size_t flush_bytes = 0;
     int *nccl_token = nullptr;
+    void *rec_work = nullptr;   // gorse_b200_recommend's grow-only device buffers (recommend.cu)
 };
+
+namespace gb {
+void recommend_work_free(gorse_b200_ctx *ctx);   // frees ctx->rec_work (recommend.cu)
+}  // namespace gb
 
 namespace gb {
 

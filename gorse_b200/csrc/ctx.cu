@@ -149,6 +149,7 @@ int32_t gorse_b200_ctx_destroy(gorse_b200_ctx *ctx)
     if (ctx->comm && gb::nccl()) gb::nccl()->CommDestroy(ctx->comm);
     if (ctx->nccl_token) cudaFree(ctx->nccl_token);
     if (ctx->flush_buf) cudaFree(ctx->flush_buf);
+    gb::recommend_work_free(ctx);
     cudaEventDestroy(ctx->ev0);
     cudaEventDestroy(ctx->ev1);
     cudaStreamDestroy(ctx->stream);

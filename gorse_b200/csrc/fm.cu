@@ -20,40 +20,11 @@
 // reference's chains are sequential, which the tensor cores cannot reproduce.  The softmax's double exp is fm_exp.h.
 #include <algorithm>
 
+#include "fm.cuh"
 #include "fm_exp.h"
-#include "recall.cuh"
 
 namespace gb {
 namespace fm {
-
-constexpr int MAX_FACTORS = 32;     // one factor per lane of a warp
-constexpr int MAX_EMB_DIM = 1024;   // fm_attn_kernel keeps one row of Mul(softmax, e) per warp in shared memory
-constexpr int MAX_SLOTS = 8;
-constexpr int ATTN_WARPS = 8;
-constexpr int SORT_THREADS = 256;
-constexpr int SORT_SMEM = 2048;     // users with more candidates sort in a global-memory buffer
-constexpr int64_t GROUP_PAIRS = int64_t(1) << 22;   // pairs per device pass (bounds the vx / row-sum buffers)
-
-struct Model {
-    const float *V, *W;
-    float bias;
-    int k;
-};
-
-struct Feats {                // id feature + labels CSR, per user or per item-table row
-    const int32_t *feat;      // [rows] or -1
-    const int64_t *off;       // [rows + 1]
-    const int32_t *idx;
-    const float *val;
-};
-
-struct Slot {
-    const float *H, *AW, *Ab, *EW, *Eb;
-    const uint16_t *emb;      // [n_items x dim] bf16 bits
-    const uint8_t *mask;      // [n_items x n_emb] or NULL (every embedding present)
-    int n_emb, s, dim;
-    float *z, *zmax;          // [n_items x dim], [n_items]
-};
 
 // Go's max(a, b) on float32: NaN propagates, max(-0, +0) = +0
 __device__ __forceinline__ float go_max(float a, float b)
@@ -239,42 +210,67 @@ __global__ void __launch_bounds__(SORT_THREADS) fm_sort_kernel(const int64_t *ca
     }
 }
 
-template <typename T>
-int32_t put(DevBuf<T> &b, const T *h, size_t n, cudaStream_t st)
+Model model(const gorse_b200_fm *m)
 {
-    GB_TRY(recall::grow(b, std::max<size_t>(n, 1)));
-    if (n) GB_CUDA(cudaMemcpyAsync(b.p, h, n * sizeof(T), cudaMemcpyHostToDevice, st));
+    const float *P = m->params.p;
+    return Model{P + 1, P + 1 + (size_t)m->n_features * m->k, m->bias, m->k};
+}
+
+int32_t item_tables(gorse_b200_fm *m, int64_t n_items, bool masked, Slot *S)
+{
+    gorse_b200_ctx *ctx = m->ctx;
+    const float *P = m->params.p;
+    for (int s = 0; s < m->n_emb; s++) {
+        const int d = m->dim[(size_t)s];
+        GB_TRY(recall::grow(m->z[s], (size_t)std::max<int64_t>(n_items, 1) * d));
+        GB_TRY(recall::grow(m->zmax[s], (size_t)std::max<int64_t>(n_items, 1)));
+        const float *b = P + m->slot_off[(size_t)s];
+        const size_t kd = (size_t)m->k * d;
+        S[s] = Slot{b, b + kd, b + 2 * kd, b + 2 * kd + m->k, b + 3 * kd + m->k, m->emb[s].p, masked ? m->mask.p : nullptr,
+                    m->n_emb, s, d, m->z[s].p, m->zmax[s].p};
+        if (n_items == 0) continue;
+        fm_item_kernel<<<(unsigned)std::min<int64_t>((n_items + 7) / 8, (int64_t)ctx->sm_count * 16), 256, 0, ctx->stream>>>(S[s], m->k, n_items);
+        GB_LAUNCHED(ctx);
+    }
     return GORSE_B200_OK;
 }
 
-// the row of V / W an index selects once it has travelled as float32; false when it leaves the table (Go panics there)
-inline bool feature_ok(int64_t idx, int64_t n_features)
+int32_t rank_pass(gorse_b200_fm *m, const Feats &U, const Feats &I, const int64_t *c_off, const int32_t *cand, const int32_t *dims, int64_t u0,
+                  int64_t u1, int64_t pair_base, const Slot *S, const int64_t *ch_start, const int32_t *ch_rows, int64_t ch0, int64_t ch1,
+                  int64_t max_n, float *score, int32_t *order, bool *global_sort)
 {
-    if (idx < 0 || idx >= n_features) return false;
-    return (int64_t)(float)idx < n_features;
+    gorse_b200_ctx *ctx = m->ctx;
+    cudaStream_t st = ctx->stream;
+    const Model M = model(m);
+    const int n_emb = m->n_emb;
+    const unsigned pg = (unsigned)std::min<int64_t>((u1 - u0 + 7) / 8, (int64_t)ctx->sm_count * 16);
+    float *vx = n_emb > 0 ? m->vx.p : nullptr;
+    if (m->k <= 8) fm_pair_kernel<8><<<pg, 256, 0, st>>>(M, U, I, c_off, cand, dims, u0, u1, pair_base, score, vx);
+    else if (m->k <= 16) fm_pair_kernel<16><<<pg, 256, 0, st>>>(M, U, I, c_off, cand, dims, u0, u1, pair_base, score, vx);
+    else fm_pair_kernel<32><<<pg, 256, 0, st>>>(M, U, I, c_off, cand, dims, u0, u1, pair_base, score, vx);
+    GB_LAUNCHED(ctx);
+    for (int s = 0; s < n_emb && ch1 > ch0; s++) {
+        const size_t smem = (size_t)ATTN_WARPS * S[s].dim * sizeof(float);
+        fm_attn_kernel<<<(unsigned)std::min<int64_t>(ch1 - ch0, (int64_t)ctx->sm_count * 16), ATTN_WARPS * 32, smem, st>>>(
+            S[s], m->k, ch_start, ch_rows, ch0, ch1, cand, pair_base, m->vx.p, m->rowsum.p, score);
+        GB_LAUNCHED(ctx);
+    }
+    int64_t sg = std::min<int64_t>(u1 - u0, (int64_t)ctx->sm_count * 8), stride = 0;
+    const int64_t max_p = recall::pow2_at_least((int)std::max<int64_t>(max_n, 1));
+    *global_sort = max_p > SORT_SMEM;
+    if (*global_sort) {   // a global key / position buffer per CTA, at most 256 MB of them
+        stride = max_p;
+        sg = std::max<int64_t>(1, std::min<int64_t>(sg, (int64_t(256) << 20) / (max_p * 12)));
+        GB_TRY(recall::grow(m->sort_key, (size_t)(sg * stride)));
+        GB_TRY(recall::grow(m->sort_val, (size_t)(sg * stride)));
+    }
+    fm_sort_kernel<<<(unsigned)sg, SORT_THREADS, 0, st>>>(c_off, u0, u1, score, order, m->sort_key.p, m->sort_val.p, stride);
+    GB_LAUNCHED(ctx);
+    return GORSE_B200_OK;
 }
 
 }  // namespace fm
 }  // namespace gb
-
-struct gorse_b200_fm {
-    gorse_b200_ctx *ctx = nullptr;
-    int64_t n_features = 0;
-    int32_t k = 0, num_dimension = 0, batch_size = 0, n_emb = 0;
-    std::vector<int32_t> dim;
-    std::vector<size_t> slot_off;        // per slot: offset of H in params (AW, Ab, EW, Eb follow)
-    float bias = 0.0f;
-    gb::DevBuf<float> params;
-    std::mutex mu;
-    // per-call buffers, grow-only
-    gb::DevBuf<int32_t> u_feat, u_idx, i_feat, i_idx, cand, dims, ch_rows, order, sort_val;
-    gb::DevBuf<int64_t> u_off, i_off, c_off, ch_start;
-    gb::DevBuf<float> u_val, i_val, score, vx, rowsum;
-    gb::DevBuf<uint16_t> emb[gb::fm::MAX_SLOTS];
-    gb::DevBuf<float> z[gb::fm::MAX_SLOTS], zmax[gb::fm::MAX_SLOTS];
-    gb::DevBuf<uint8_t> mask;
-    gb::DevBuf<uint64_t> sort_key;
-};
 
 using namespace gb;
 
@@ -431,8 +427,6 @@ extern "C" int32_t gorse_b200_fm_rank(gorse_b200_fm *m, int64_t n_users, const i
     GB_TRY(recall::grow(m->score, (size_t)total));
     GB_TRY(recall::grow(m->order, (size_t)total));
 
-    const float *P = m->params.p;
-    Model M{P + 1, P + 1 + (size_t)m->n_features * m->k, m->bias, m->k};
     Feats U{m->u_feat.p, m->u_off.p, m->u_idx.p, m->u_val.p};
     Feats I{m->i_feat.p, m->i_off.p, m->i_idx.p, m->i_val.p};
     Slot S[MAX_SLOTS];
@@ -440,18 +434,8 @@ extern "C" int32_t gorse_b200_fm_rank(gorse_b200_fm *m, int64_t n_users, const i
         GB_TRY(put(m->ch_start, ch_start.data(), ch_start.size(), st));
         GB_TRY(put(m->ch_rows, ch_rows.data(), ch_rows.size(), st));
         if (item_emb_mask) GB_TRY(put(m->mask, item_emb_mask, (size_t)n_items * n_emb, st));
-        for (int s = 0; s < n_emb; s++) {
-            const int d = m->dim[(size_t)s];
-            GB_TRY(put(m->emb[s], item_emb[s], (size_t)n_items * d, st));
-            GB_TRY(recall::grow(m->z[s], (size_t)n_items * d));
-            GB_TRY(recall::grow(m->zmax[s], (size_t)n_items));
-            const float *b = P + m->slot_off[(size_t)s];
-            const size_t kd = (size_t)m->k * d;
-            S[s] = Slot{b, b + kd, b + 2 * kd, b + 2 * kd + m->k, b + 3 * kd + m->k, m->emb[s].p, item_emb_mask ? m->mask.p : nullptr,
-                        n_emb, s, d, m->z[s].p, m->zmax[s].p};
-            fm_item_kernel<<<(unsigned)std::min<int64_t>((n_items + 7) / 8, (int64_t)ctx->sm_count * 16), 256, 0, st>>>(S[s], m->k, n_items);
-            GB_LAUNCHED(ctx);
-        }
+        for (int s = 0; s < n_emb; s++) GB_TRY(put(m->emb[s], item_emb[s], (size_t)n_items * m->dim[(size_t)s], st));
+        GB_TRY(item_tables(m, n_items, item_emb_mask != nullptr, S));
     }
     // device passes over consecutive users holding at most GROUP_PAIRS pairs (or one user)
     int64_t passes = 0, global_sorts = 0;
@@ -467,30 +451,11 @@ extern "C" int32_t gorse_b200_fm_rank(gorse_b200_fm *m, int64_t n_users, const i
                 GB_TRY(recall::grow(m->vx, (size_t)np * m->k));
                 GB_TRY(recall::grow(m->rowsum, (size_t)np));
             }
-            const unsigned pg = (unsigned)std::min<int64_t>((u1 - u0 + 7) / 8, (int64_t)ctx->sm_count * 16);
-            float *vx = n_emb > 0 ? m->vx.p : nullptr;
-            if (m->k <= 8) fm_pair_kernel<8><<<pg, 256, 0, st>>>(M, U, I, m->c_off.p, m->cand.p, m->dims.p, u0, u1, pb, m->score.p, vx);
-            else if (m->k <= 16) fm_pair_kernel<16><<<pg, 256, 0, st>>>(M, U, I, m->c_off.p, m->cand.p, m->dims.p, u0, u1, pb, m->score.p, vx);
-            else fm_pair_kernel<32><<<pg, 256, 0, st>>>(M, U, I, m->c_off.p, m->cand.p, m->dims.p, u0, u1, pb, m->score.p, vx);
-            GB_LAUNCHED(ctx);
-            const int64_t ch0 = first_chunk[(size_t)u0], ch1 = first_chunk[(size_t)u1];
-            for (int s = 0; s < n_emb; s++) {
-                const size_t smem = (size_t)ATTN_WARPS * S[s].dim * sizeof(float);
-                fm_attn_kernel<<<(unsigned)std::min<int64_t>(ch1 - ch0, (int64_t)ctx->sm_count * 16), ATTN_WARPS * 32, smem, st>>>(
-                    S[s], m->k, m->ch_start.p, m->ch_rows.p, ch0, ch1, m->cand.p, pb, m->vx.p, m->rowsum.p, m->score.p);
-                GB_LAUNCHED(ctx);
-            }
-            int64_t sg = std::min<int64_t>(u1 - u0, (int64_t)ctx->sm_count * 8), stride = 0;
-            const int64_t max_p = recall::pow2_at_least((int)max_n);
-            if (max_p > SORT_SMEM) {   // a global key / position buffer per CTA, at most 256 MB of them
-                stride = max_p;
-                sg = std::max<int64_t>(1, std::min<int64_t>(sg, (int64_t(256) << 20) / (max_p * 12)));
-                GB_TRY(recall::grow(m->sort_key, (size_t)(sg * stride)));
-                GB_TRY(recall::grow(m->sort_val, (size_t)(sg * stride)));
+            bool global_sort = false;
+            GB_TRY(rank_pass(m, U, I, m->c_off.p, m->cand.p, m->dims.p, u0, u1, pb, S, m->ch_start.p, m->ch_rows.p, first_chunk[(size_t)u0],
+                             first_chunk[(size_t)u1], max_n, m->score.p, m->order.p, &global_sort));
+            if (global_sort)
                 for (int64_t u = u0; u < u1; u++) global_sorts += recall::pow2_at_least((int)(cand_off[u + 1] - cand_off[u])) > SORT_SMEM;
-            }
-            fm_sort_kernel<<<(unsigned)sg, SORT_THREADS, 0, st>>>(m->c_off.p, u0, u1, m->score.p, m->order.p, m->sort_key.p, m->sort_val.p, stride);
-            GB_LAUNCHED(ctx);
         }
         u0 = u1;
     }

@@ -17,9 +17,8 @@
 //             this CTA's float64 row of length N in global memory, with a touched flag per slot and the list of touched slots.
 #include <algorithm>
 
-#include "aggregate.cuh"
 #include "sparse.cuh"
-#include "vecdb.cuh"
+#include "stages.cuh"
 
 namespace gb {
 namespace i2i {
@@ -27,24 +26,6 @@ namespace i2i {
 using agg::TABLE_CAP;
 using agg::TABLE_KEYS;                           // a user takes the table when |C_u| * n <= this
 constexpr int AGG_THREADS = agg::THREADS;
-constexpr int MAX_N_DENSE = 1024;                // the sort buffer holds n entries
-constexpr int MAX_N_SPARSE = 128;                // sparse_search_kernel's k
-
-struct Users {                // one chunk of users (chunk-local ids)
-    const int64_t *c_off;     // [users + 1] into c_row
-    const int32_t *c_row;     // the neighbour-table row of each live context entry, in the caller's order
-    const int64_t *ex_off;    // [users + 1] into ex
-    const int64_t *ex;        // each user's excluded slots, ascending (-1 entries dropped)
-    int64_t *slots;           // [users x n]
-    double *scores;           // [users x n]
-    int32_t *count;           // [users]
-};
-
-struct Table {                // stage A: the first n neighbours of each distinct context item
-    const int32_t *slot;      // [rows x n]
-    const float *score;       // [rows x n] the vector store's score (dot, or the negated distance)
-    const int32_t *cnt;       // [rows]
-};
 
 // one CTA per user of `users`.  SHARED: the accumulator is a table in shared memory; else acc_rows / seen_rows /
 // touched_rows hold one [N] float64 row, one [N] flag row (all zero between users) and one [N] slot list per CTA.
@@ -123,7 +104,41 @@ i2i_aggregate_kernel(const int32_t *users, int64_t n_users, Users U, Table T, in
     }
 }
 
+int32_t aggregate(gorse_b200_ctx *c, const int32_t *d_users, int64_t fill, int64_t heavy, const Users &U, const Table &T, int n, double scale,
+                  bool euclid, int64_t N, double *acc, uint8_t *seen, int32_t *touched)
+{
+    const size_t sm_shared = agg::smem_bytes(n, true), sm_global = agg::smem_bytes(n, false);
+    GB_CUDA(cudaFuncSetAttribute(i2i_aggregate_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm_shared));
+    GB_CUDA(cudaFuncSetAttribute(i2i_aggregate_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm_global));
+    if (fill > 0) {
+        i2i_aggregate_kernel<true><<<(unsigned)std::min<int64_t>(fill, (int64_t)c->sm_count * 8), AGG_THREADS, sm_shared, c->stream>>>(
+            d_users, fill, U, T, n, scale, euclid, N, nullptr, nullptr, nullptr);
+        c->launches++;
+    }
+    if (heavy > 0) {
+        i2i_aggregate_kernel<false><<<(unsigned)std::min<int64_t>(heavy, heavy_grid(c, N)), AGG_THREADS, sm_global, c->stream>>>(
+            d_users + fill, heavy, U, T, n, scale, euclid, N, acc, seen, touched);
+        c->launches++;
+    }
+    GB_CUDA(cudaGetLastError());
+    return GORSE_B200_OK;
+}
+
 }  // namespace i2i
+
+int32_t neighbour_table(gorse_b200_vecdb *db, int64_t R, const int64_t *d_nb, int n, int32_t *t_slot, float *t_score, int32_t *t_cnt,
+                        int64_t *exact_rows)
+{
+    if (db->dim > 0) {
+        std::lock_guard<std::mutex> lk2(db->dense->mu);
+        const recall::Table table{t_slot, t_score, t_cnt, false, db->distance == GORSE_B200_DISTANCE_DOT, nullptr, nullptr, nullptr};
+        return recall::recall_rows(db->dense, db->d_allow.p, R, nullptr, d_nb, n, nullptr, nullptr, nullptr, &table, nullptr, nullptr, nullptr,
+                                   exact_rows);
+    }
+    std::lock_guard<std::mutex> lk2(db->sparse->mu);
+    return sparse_search_rows(db->sparse, d_nb, R, db->d_allow.p, n, t_slot, t_score, t_cnt);
+}
+
 }  // namespace gb
 
 using namespace gb;
@@ -224,32 +239,18 @@ extern "C" int32_t gorse_b200_vecdb_item_to_item(gorse_b200_vecdb *db, int64_t n
 
     // ---- stage A: the neighbour table
     int64_t exact_rows = 0;
-    if (!sparse) {
-        std::lock_guard<std::mutex> lk2(db->dense->mu);
-        const recall::Table table{V.t_slot.p, V.t_score.p, V.t_cnt.p, false, db->distance == GORSE_B200_DISTANCE_DOT, nullptr, nullptr, nullptr};
-        if ((st = recall::recall_rows(db->dense, db->d_allow.p, R, nullptr, V.nb.p, n, nullptr, nullptr, nullptr, &table, nullptr, nullptr, nullptr,
-                                      &exact_rows)))
-            return done(st);
-    } else {
-        std::lock_guard<std::mutex> lk2(db->sparse->mu);
-        if ((st = sparse_search_rows(db->sparse, V.nb.p, R, db->d_allow.p, n, V.t_slot.p, V.t_score.p, V.t_cnt.p))) return done(st);
-    }
+    if ((st = neighbour_table(db, R, V.nb.p, n, V.t_slot.p, V.t_score.p, V.t_cnt.p, &exact_rows))) return done(st);
     if ((e = cudaGetLastError()) != cudaSuccess) { set_error("item_to_item: %s", cudaGetErrorString(e)); return done(GORSE_B200_ERR_CUDA); }
 
     // ---- stage B: users in chunks; a finished chunk is downloaded on the copy stream while the next one computes
     const int64_t cu = std::min<int64_t>(n_users, (int64_t)c->sm_count * 1024);
     const int64_t N = n_slots;
-    // global accumulators: one [N] float64 row, flag row and slot list per CTA, at most 512 MB
-    const int heavy_grid = (int)std::max<int64_t>(1, std::min<int64_t>((int64_t)c->sm_count * 2, (512ll << 20) / (13 * N)));
+    const int hg = heavy_grid(c, N);
     const int64_t total_ctx = c_off[(size_t)n_users];
     if ((st = grow(V.c_off, (size_t)cu + 1)) || (st = grow(V.ex_off, (size_t)cu + 1)) || (st = grow(V.users, (size_t)cu)) ||
         (st = grow(V.c_row, (size_t)std::max<int64_t>(total_ctx, 1))) || (st = grow(V.ex, std::max<size_t>(ex.size(), 1))) ||
         (st = grow(V.slots, (size_t)n_users * n)) || (st = grow(V.scores, (size_t)n_users * n)) || (st = grow(V.count, (size_t)n_users)))
         return done(st);
-    const size_t sm_shared = agg::smem_bytes(n, true), sm_global = agg::smem_bytes(n, false);
-    e = cudaFuncSetAttribute(i2i_aggregate_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm_shared);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(i2i_aggregate_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm_global);
-    if (e != cudaSuccess) { set_error("item_to_item: %s", cudaGetErrorString(e)); return done(GORSE_B200_ERR_CUDA); }
     Table T;
     T.slot = V.t_slot.p; T.score = V.t_score.p; T.cnt = V.t_cnt.p;
     const bool euclid = db->distance == GORSE_B200_DISTANCE_EUCLIDEAN;
@@ -270,8 +271,8 @@ extern "C" int32_t gorse_b200_vecdb_item_to_item(gorse_b200_vecdb *db, int64_t n
         }
         n_shared += fill;
         n_heavy += rows - fill;
-        if (rows - fill > 0 && ((st = grow(V.acc, (size_t)heavy_grid * N)) || (st = grow_zeroed(V.seen, (size_t)heavy_grid * N, c->stream)) ||
-                                (st = grow(V.touched, (size_t)heavy_grid * N))))
+        if (rows - fill > 0 && ((st = grow(V.acc, (size_t)hg * N)) || (st = grow_zeroed(V.seen, (size_t)hg * N, c->stream)) ||
+                                (st = grow(V.touched, (size_t)hg * N))))
             return done(st);
         const int64_t n_c = h_coff[rows], n_e = h_exoff[rows];
         if ((e = cudaMemcpyAsync(V.c_off.p, h_coff.data(), sizeof(int64_t) * (rows + 1), cudaMemcpyHostToDevice, c->stream)) != cudaSuccess ||
@@ -285,17 +286,7 @@ extern "C" int32_t gorse_b200_vecdb_item_to_item(gorse_b200_vecdb *db, int64_t n
         Users U;
         U.c_off = V.c_off.p; U.c_row = V.c_row.p + c_off[u0]; U.ex_off = V.ex_off.p; U.ex = V.ex.p + ex_off[u0];
         U.slots = V.slots.p + u0 * n; U.scores = V.scores.p + u0 * n; U.count = V.count.p + u0;
-        if (fill > 0) {
-            i2i_aggregate_kernel<true><<<(unsigned)std::min<int64_t>(fill, (int64_t)c->sm_count * 8), AGG_THREADS, sm_shared, c->stream>>>(
-                V.users.p, fill, U, T, n, score_scale, euclid, N, nullptr, nullptr, nullptr);
-            c->launches++;
-        }
-        if (rows - fill > 0) {
-            i2i_aggregate_kernel<false><<<(unsigned)std::min<int64_t>(rows - fill, heavy_grid), AGG_THREADS, sm_global, c->stream>>>(
-                V.users.p + fill, rows - fill, U, T, n, score_scale, euclid, N, V.acc.p, V.seen.p, V.touched.p);
-            c->launches++;
-        }
-        if ((e = cudaGetLastError()) != cudaSuccess) { set_error("item_to_item: %s", cudaGetErrorString(e)); return done(GORSE_B200_ERR_CUDA); }
+        if ((st = aggregate(c, V.users.p, fill, rows - fill, U, T, n, score_scale, euclid, N, V.acc.p, V.seen.p, V.touched.p))) return done(st);
         if ((e = cudaEventRecord(c->copy_ev, c->stream)) != cudaSuccess || (e = cudaStreamWaitEvent(c->copy_stream, c->copy_ev, 0)) != cudaSuccess ||
             (e = cudaMemcpyAsync(count_out + u0, V.count.p + u0, sizeof(int32_t) * rows, cudaMemcpyDeviceToHost, c->copy_stream)) != cudaSuccess ||
             (e = cudaMemcpyAsync(slots_out + u0 * n, V.slots.p + u0 * n, sizeof(int64_t) * rows * n, cudaMemcpyDeviceToHost, c->copy_stream)) != cudaSuccess ||

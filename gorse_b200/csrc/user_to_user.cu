@@ -16,9 +16,8 @@
 //             (sum desc, item asc) (agg::select_first_n), then the item filter as an ordered compaction.
 #include <algorithm>
 
-#include "aggregate.cuh"
 #include "sparse.cuh"
-#include "vecdb.cuh"
+#include "stages.cuh"
 
 namespace gb {
 namespace u2u {
@@ -26,37 +25,6 @@ namespace u2u {
 using agg::TABLE_CAP;
 using agg::TABLE_KEYS;                           // a user takes the table when W_u <= this
 constexpr int AGG_THREADS = agg::THREADS;
-constexpr int MAX_N_DENSE = 1024;                // the sort buffer holds n entries
-constexpr int MAX_N_SPARSE = 128;                // sparse_search_kernel's k
-
-struct Table {                // stage A: the first n neighbours of each distinct query user
-    const int32_t *slot;      // [rows x n]
-    const float *score;       // [rows x n] the vector store's score (dot, or the negated distance)
-    const int32_t *cnt;       // [rows]
-};
-
-struct Feedback {             // the caller's positive feedback per slot, as item indices
-    const int64_t *off;       // [rows + 1]
-    const int32_t *items;
-    int64_t rows;             // slots at or beyond have none
-};
-
-struct Users {                // one chunk of users (chunk-local ids)
-    const int32_t *q_row;     // [users] the neighbour-table row of each user, -1 = no vector
-    const int64_t *ex_off;    // [users + 1] into ex
-    const int64_t *ex;        // each user's excluded items, ascending (-1 entries dropped)
-    const uint8_t *item_ok;   // [n_items] or NULL
-    int64_t *items;           // [users x n]
-    double *scores;           // [users x n]
-    int32_t *count;           // [users]
-};
-
-struct Route {                // the device's routing of one chunk
-    int32_t *list;            // [users]: shared-memory users from the front, global-row users from the back
-    int32_t *cnt;             // [2]: how many of each
-    int32_t *work;            // [users] W_u
-    int64_t users;
-};
 
 // W_u for each user of the chunk.  Users without a vector, neighbours or feedback get an empty row here.
 __global__ void u2u_route_kernel(Users U, Table T, Feedback F, int n, Route R)
@@ -179,6 +147,26 @@ u2u_aggregate_kernel(Route R, Users U, Table T, Feedback F, int n, double scale,
     }
 }
 
+int32_t aggregate(gorse_b200_ctx *c, const Route &R, const Users &U, const Table &T, const Feedback &F, int n, double scale, bool euclid,
+                  int64_t NI, bool heavy, double *acc, int32_t *flag, int32_t *touched)
+{
+    const size_t sm_shared = agg::smem_bytes(n, true), sm_global = agg::smem_bytes(n, false);
+    GB_CUDA(cudaFuncSetAttribute(u2u_aggregate_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm_shared));
+    GB_CUDA(cudaFuncSetAttribute(u2u_aggregate_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm_global));
+    const int64_t rows = R.users;
+    u2u_route_kernel<<<(unsigned)((rows + 255) / 256), 256, 0, c->stream>>>(U, T, F, n, R);
+    u2u_aggregate_kernel<true><<<(unsigned)std::min<int64_t>(rows, (int64_t)c->sm_count * 8), AGG_THREADS, sm_shared, c->stream>>>(
+        R, U, T, F, n, scale, euclid, NI, nullptr, nullptr, nullptr);
+    c->launches += 2;
+    if (heavy) {
+        u2u_aggregate_kernel<false><<<(unsigned)std::min<int64_t>(rows, heavy_grid(c, NI)), AGG_THREADS, sm_global, c->stream>>>(
+            R, U, T, F, n, scale, euclid, NI, acc, flag, touched);
+        c->launches++;
+    }
+    GB_CUDA(cudaGetLastError());
+    return GORSE_B200_OK;
+}
+
 }  // namespace u2u
 }  // namespace gb
 
@@ -284,16 +272,7 @@ extern "C" int32_t gorse_b200_vecdb_user_to_user(gorse_b200_vecdb *db, int64_t n
 
     // ---- stage A: the neighbour table
     int64_t exact_rows = 0;
-    if (!sparse) {
-        std::lock_guard<std::mutex> lk2(db->dense->mu);
-        const recall::Table table{V.t_slot.p, V.t_score.p, V.t_cnt.p, false, db->distance == GORSE_B200_DISTANCE_DOT, nullptr, nullptr, nullptr};
-        if ((st = recall::recall_rows(db->dense, db->d_allow.p, R, nullptr, V.nb.p, n, nullptr, nullptr, nullptr, &table, nullptr, nullptr, nullptr,
-                                      &exact_rows)))
-            return done(st);
-    } else {
-        std::lock_guard<std::mutex> lk2(db->sparse->mu);
-        if ((st = sparse_search_rows(db->sparse, V.nb.p, R, db->d_allow.p, n, V.t_slot.p, V.t_score.p, V.t_cnt.p))) return done(st);
-    }
+    if ((st = neighbour_table(db, R, V.nb.p, n, V.t_slot.p, V.t_score.p, V.t_cnt.p, &exact_rows))) return done(st);
     if ((e = cudaGetLastError()) != cudaSuccess) { set_error("user_to_user: %s", cudaGetErrorString(e)); return done(GORSE_B200_ERR_CUDA); }
 
     // ---- the feedback rows and the item filter, once per call
@@ -316,14 +295,10 @@ extern "C" int32_t gorse_b200_vecdb_user_to_user(gorse_b200_vecdb *db, int64_t n
     // ---- routing and stage B: users in chunks; a finished chunk is downloaded on the copy stream while the next one computes
     // global accumulators: one [n_items] float64 row, flag row and item list per CTA, at most 512 MB
     const int64_t NI = std::max<int64_t>(n_items, 1);
-    const int heavy_grid = (int)std::max<int64_t>(1, std::min<int64_t>((int64_t)c->sm_count * 2, (512ll << 20) / (16 * NI)));
-    if (heavy_possible && ((st = grow_zeroed(V.acc, (size_t)heavy_grid * NI, c->stream)) || (st = grow_zeroed(V.flag, (size_t)heavy_grid * NI, c->stream)) ||
-                           (st = grow(V.touched, (size_t)heavy_grid * NI))))
+    const int hg = heavy_grid(c, NI);
+    if (heavy_possible && ((st = grow_zeroed(V.acc, (size_t)hg * NI, c->stream)) || (st = grow_zeroed(V.flag, (size_t)hg * NI, c->stream)) ||
+                           (st = grow(V.touched, (size_t)hg * NI))))
         return done(st);
-    const size_t sm_shared = agg::smem_bytes(n, true), sm_global = agg::smem_bytes(n, false);
-    e = cudaFuncSetAttribute(u2u_aggregate_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm_shared);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(u2u_aggregate_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm_global);
-    if (e != cudaSuccess) { set_error("user_to_user: %s", cudaGetErrorString(e)); return done(GORSE_B200_ERR_CUDA); }
     Table T;
     T.slot = V.t_slot.p; T.score = V.t_score.p; T.cnt = V.t_cnt.p;
     Feedback F;
@@ -346,16 +321,7 @@ extern "C" int32_t gorse_b200_vecdb_user_to_user(gorse_b200_vecdb *db, int64_t n
         U.items = V.items.p + u0 * n; U.scores = V.scores.p + u0 * n; U.count = V.count.p + u0;
         Route Rt;
         Rt.list = V.list.p; Rt.cnt = V.route_cnt.p + 2 * ci; Rt.work = V.work.p; Rt.users = rows;
-        u2u_route_kernel<<<(unsigned)((rows + 255) / 256), 256, 0, c->stream>>>(U, T, F, n, Rt);
-        u2u_aggregate_kernel<true><<<(unsigned)std::min<int64_t>(rows, (int64_t)c->sm_count * 8), AGG_THREADS, sm_shared, c->stream>>>(
-            Rt, U, T, F, n, score_scale, euclid, NI, nullptr, nullptr, nullptr);
-        c->launches += 2;
-        if (heavy_possible) {
-            u2u_aggregate_kernel<false><<<(unsigned)std::min<int64_t>(rows, heavy_grid), AGG_THREADS, sm_global, c->stream>>>(
-                Rt, U, T, F, n, score_scale, euclid, NI, V.acc.p, V.flag.p, V.touched.p);
-            c->launches++;
-        }
-        if ((e = cudaGetLastError()) != cudaSuccess) { set_error("user_to_user: %s", cudaGetErrorString(e)); return done(GORSE_B200_ERR_CUDA); }
+        if ((st = aggregate(c, Rt, U, T, F, n, score_scale, euclid, NI, heavy_possible, V.acc.p, V.flag.p, V.touched.p))) return done(st);
         if ((e = cudaEventRecord(c->copy_ev, c->stream)) != cudaSuccess || (e = cudaStreamWaitEvent(c->copy_stream, c->copy_ev, 0)) != cudaSuccess ||
             (e = cudaMemcpyAsync(count_out + u0, V.count.p + u0, sizeof(int32_t) * rows, cudaMemcpyDeviceToHost, c->copy_stream)) != cudaSuccess ||
             (e = cudaMemcpyAsync(items_out + u0 * n, V.items.p + u0 * n, sizeof(int64_t) * rows * n, cudaMemcpyDeviceToHost, c->copy_stream)) != cudaSuccess ||

@@ -474,6 +474,112 @@ int32_t gorse_b200_fm_rank(gorse_b200_fm *fm, int64_t n_users, const int32_t *us
                            const int32_t *cand_items, float *scores_out, int32_t *order_out, int64_t *stats_out);
 
 /* ------------------------------------------------------------------------------------------
+ * Batched offline recommendation: for n_users users at once, what the worker's offline loop does per user after
+ * NewRecommender (worker/pipeline.go:124-319): the CF recall (updateCollaborativeRecommend, :403-449), the recommenders in the
+ * configured order (Recommender.RecommendSequential with limit 0, logics/recommend.go:135-156), the candidate list
+ * (pipeline.go:228-243), the replacement items (addReplacementCandidates, :573-611) and the FM ranking
+ * (rankByClickTroughRate, :451-499) followed by the replacement decay (applyReplacementDecay, :613-643).  The exclude set
+ * and the candidates of every user stay on the device from the first stage to the ranked list.  Everything runs in the item
+ * index space [0, n_items) of the call's item DICTIONARY, which must hold every id a stage can return.
+ *   E0_u = excl_items[excl_off[u] .. excl_off[u+1]) (excl_off[0] = 0): the user's feedback items (NewRecommender,
+ *   logics/recommend.go:61-93, offline: every feedback item), an item index or -1 for an id outside the dictionary; every
+ *   entry counts in |E0_u| (excludeSet.Cardinality()); an item twice is GORSE_B200_ERR_ARG.
+ *   item_live[n_items]: 1 for the items that exist and are not hidden (ItemCache).
+ *   CF recall (cf, needed by a COLLABORATIVE stage): the first cf->n + |E0_u| results of gorse_b200_vecdb_query_excluding on
+ *   the CF collection for the user's vector, minus E0_u; scores float64(float32).
+ *   Stages, in order.  Each produces a list; entries in the running exclude set E_u are dropped as the reference's
+ *   recommender drops them; the list is appended to the candidates, and only then is every produced id added to E_u (so a
+ *   duplicate inside one stage survives).  Kinds (gorse_b200_recommend_stage.kind):
+ *     LIST            non-personalized / latest (list_off == NULL: one list list_items / list_scores[list_len] for every
+ *                     user) or external (list_off[n_users + 1] from 0: one list per user); entries in E_u are dropped
+ *                     (recommend.go:180-225, :350-384).  Bound: the list's length.
+ *     COLLABORATIVE   the CF recall row, minus the items with item_live = 0, cut at cf->n, then minus E_u
+ *                     (recommend.go:227-242: SearchScores(0, CacheSize) on the cached row, then the filter).  Bound: cf->n.
+ *     ITEM_TO_ITEM    gorse_b200_vecdb_item_to_item's row on db (n, score_scale, categories) with E_u as its exclude set;
+ *                     context ctx_items[ctx_off[u] ..) as item indices, newest first, -1 skipped; slot_of_item[n_items] /
+ *                     item_of_slot[slots of db] map between the dictionary and the collection (-1 = none).  Bound: n.
+ *     USER_TO_USER    gorse_b200_vecdb_user_to_user's row on db (user_slots, feedback rows, item_ok, n, score_scale) with
+ *                     E_u as its exclude set.  Bound: n.
+ *   Candidates: the stage lists concatenated in order, minus the items with item_live = 0, in order (a dropped item still
+ *   excludes).  With a ranker and a replacement CSR repl_off[n_users + 1] (from 0) / repl_items / repl_positive (distinct
+ *   feedback items per user, 1 = positive, 0 = read): the live replacement items that are not candidates yet are appended in
+ *   the given order.  The reference's order here is mapset order, so it is unpinned.
+ *   Ranking (ranker != NULL): gorse_b200_fm_rank's semantics on the final candidates -- D_u, the attention chunks in
+ *   candidate order, float32 scores; then the scores of the live positive / read replacement items are multiplied in
+ *   float64 by positive_decay / read_decay, and the row is sorted by score descending, exact ties (-0 == +0) by candidate
+ *   position, NaN last.  The reference's sort is not stable, so its order on ties is unpinned.  ranker == NULL
+ *   (Ranker.Type = "none"): the candidates in merged order with their stage scores, no replacement.
+ *   Output: B_u = the sum of the stage bounds + |repl_u| (the replacement count only with a ranker).  Row u starts at
+ *   B_0 + ... + B_{u-1} in items_out (int32 item indices) / scores_out (float64); count_out[u] <= B_u entries.
+ *   Limits are those of the entries reused: n <= 1024 (dense) / 128 (sparse), Cosine collections and sparse CF collections
+ *   are GORSE_B200_ERR_UNSUPPORTED, gorse_b200_fm_create's limits; a list may hold at most 4096 entries.  Every argument is
+ *   checked on the host before the device is touched (GORSE_B200_ERR_ARG): offsets, items, slots, a live slot whose
+ *   item_of_slot is -1 or whose slot_of_item does not point back, NaN scores or decays, features as gorse_b200_fm_rank
+ *   checks them, collections or a ranker of another context.  The library keeps no host pointer after the call.
+ *   stats_out[4] (may be NULL): chunks, candidates ranked or returned, neighbour-table rows of all stages, rows answered
+ *   by the exact scan rather than the tensor-core sweep; the answer does not depend on them. */
+typedef enum {
+    GORSE_B200_STAGE_LIST = 0,
+    GORSE_B200_STAGE_COLLABORATIVE = 1,
+    GORSE_B200_STAGE_ITEM_TO_ITEM = 2,
+    GORSE_B200_STAGE_USER_TO_USER = 3
+} gorse_b200_stage_kind;
+
+typedef struct {
+    int32_t kind;                  /* gorse_b200_stage_kind */
+    /* LIST */
+    int64_t list_len;              /* shared list: its length; per-user lists: ignored */
+    const int64_t *list_off;       /* NULL = one shared list; else [n_users + 1] from 0 */
+    const int32_t *list_items;     /* item indices */
+    const double *list_scores;     /* not NaN */
+    /* ITEM_TO_ITEM, USER_TO_USER */
+    gorse_b200_vecdb *db;
+    int32_t n;                     /* CacheSize */
+    double score_scale;            /* 0.5 for type "auto", else 1 */
+    /* ITEM_TO_ITEM */
+    const int64_t *ctx_off;        /* [n_users + 1] from 0 */
+    const int32_t *ctx_items;      /* item indices, -1 = an id outside the dictionary */
+    const int64_t *slot_of_item;   /* [n_items] */
+    const int32_t *item_of_slot;   /* [slots of db] */
+    const int32_t *categories;
+    int32_t n_categories;
+    /* USER_TO_USER */
+    const int64_t *user_slots;     /* [n_users], -1 = no vector */
+    int64_t n_fb_rows;
+    const int64_t *fb_off;         /* [n_fb_rows + 1] from 0 */
+    const int32_t *fb_items;       /* item indices */
+    const uint8_t *item_ok;        /* [n_items] or NULL */
+} gorse_b200_recommend_stage;
+
+typedef struct {
+    gorse_b200_vecdb *db;          /* the dense CF collection (collaborative_filtering_<id>) */
+    const float *user_vectors;     /* [n_users x dim] */
+    const int64_t *slot_of_item;   /* [n_items] */
+    const int32_t *item_of_slot;   /* [slots of db] */
+    int32_t n;                     /* CacheSize */
+} gorse_b200_recommend_cf;
+
+typedef struct {
+    gorse_b200_fm *fm;
+    const int32_t *user_feat;      /* users as gorse_b200_fm_rank takes them, [n_users] */
+    const int64_t *user_lab_off;
+    const int32_t *user_lab_idx;
+    const float *user_lab_val;
+    const int32_t *item_feat;      /* the dictionary's item table, [n_items] rows */
+    const int64_t *item_lab_off;
+    const int32_t *item_lab_idx;
+    const float *item_lab_val;
+    const uint16_t *const *item_emb;
+    const uint8_t *item_emb_mask;
+} gorse_b200_recommend_ranker;
+
+int32_t gorse_b200_recommend(gorse_b200_ctx *ctx, int64_t n_users, const int64_t *excl_off, const int32_t *excl_items, int32_t n_items,
+                             const uint8_t *item_live, int32_t n_stages, const gorse_b200_recommend_stage *stages,
+                             const gorse_b200_recommend_cf *cf, const gorse_b200_recommend_ranker *ranker, const int64_t *repl_off,
+                             const int32_t *repl_items, const uint8_t *repl_positive, double positive_decay, double read_decay,
+                             int32_t *items_out, double *scores_out, int32_t *count_out, int64_t *stats_out);
+
+/* ------------------------------------------------------------------------------------------
  * FM training: AFM.Fit (model/ctr/fm.go:307-417) for a model without item-embedding slots (plain FM: bias, linear and
  * pairwise terms), step for step.  The master runs it every ranker.fit_period (master/tasks.go:1047-1155) and
  * optimize_trials more times (:1318-1363).  Init and the scalers stay with the caller: it passes fm.Parameters() after
