@@ -194,6 +194,42 @@ class CFModel:
                  C.cast(cb, C.c_void_p) if cb else None, None, C.byref(res)))
         return res
 
+    def fit_trials(self, trials, test_off, test_items, neg_off, neg_items, progress=None, factors=False):
+        """ModelSearch's trials in one gorse_b200_cf_fit_trials call.  trials: a list of (kind, params) with kind "bpr" or
+        "als" and params overriding that kind's defaults as in fit(); the fields the trials share (seed, verbose, candidates,
+        topk, patience) must be equal.  progress(epoch, states), states a list of (epochs_run, ndcg or -1, finished) per
+        trial, returns True to cancel.  Returns the list of FitResult, and with factors=True also a list of (P, Q)."""
+        n = len(trials)
+        als = np.array([1 if kind == "als" else 0 for kind, _ in trials], np.int32)
+        fps = (_lib.FitParams * n)()
+        for k, (kind, params) in enumerate(trials):
+            check(lib.gorse_b200_fit_params_default(int(als[k]), C.byref(fps[k])))
+            fps[k].n_factors = self.d
+            for key, v in params.items():
+                setattr(fps[k], key, v)
+        res = (_lib.FitResult * n)()
+        test_off = np.ascontiguousarray(test_off, np.int64)
+        test_items = np.ascontiguousarray(test_items, np.int32)
+        if neg_off is not None:   # None: the negatives are sampled on the device (params: candidates)
+            neg_off = np.ascontiguousarray(neg_off, np.int64)
+            neg_items = np.ascontiguousarray(neg_items, np.int32)
+        out = None
+        p_ptrs = q_ptrs = None
+        if factors:
+            out = [(np.zeros((self.n_users, self.d), np.float32), np.zeros((self.n_items, self.d), np.float32)) for _ in range(n)]
+            p_ptrs = (C.c_void_p * n)(*[P.ctypes.data for P, _ in out])
+            q_ptrs = (C.c_void_p * n)(*[Q.ctypes.data for _, Q in out])
+
+        def on_epoch(user, epoch, n_trials, states):
+            return int(bool(progress(epoch, [(states[k].epochs_run, states[k].ndcg, bool(states[k].finished)) for k in range(n_trials)])))
+
+        cb = _lib.TRIALS_PROGRESS_FN(on_epoch) if progress else None
+        check(lib.gorse_b200_cf_fit_trials(self.h, n, ptr(als), C.cast(fps, C.c_void_p), ptr(test_off), ptr(test_items), ptr(neg_off),
+                                           ptr(neg_items), C.cast(cb, C.c_void_p) if cb else None, None, C.cast(res, C.c_void_p),
+                                           C.cast(p_ptrs, C.c_void_p) if factors else None, C.cast(q_ptrs, C.c_void_p) if factors else None))
+        res = list(res)
+        return (res, out) if factors else res
+
     def eval_plan(self, test_off, test_items, neg_off=None, neg_items=None, n_candidates=100, seed=0, topk=10):
         return EvalPlan(self, test_off, test_items, neg_off, neg_items, n_candidates, seed, topk)
 

@@ -65,6 +65,7 @@ PROTOTYPES = {
     "gorse_b200_fit_params_default": (C.c_int32, [C.c_int32, VP]),
     "gorse_b200_bpr_fit": (C.c_int32, [VP, VP, VP, VP, VP, VP, VP, VP, VP]),
     "gorse_b200_als_fit": (C.c_int32, [VP, VP, VP, VP, VP, VP, VP, VP, VP]),
+    "gorse_b200_cf_fit_trials": (C.c_int32, [VP, C.c_int32, VP, VP, VP, VP, VP, VP, VP, VP, VP, VP, VP]),
     "gorse_b200_index_create": (C.c_int32, [VP, C.c_int32, C.c_int32, PVP]),
     "gorse_b200_index_destroy": (C.c_int32, [VP]),
     "gorse_b200_index_add": (C.c_int32, [VP, VP, C.c_int64, C.POINTER(C.c_int64)]),
@@ -128,6 +129,10 @@ class FitResult(C.Structure):
                 ("early_stopped", C.c_int32), ("best_epoch", C.c_int32), ("cancelled", C.c_int32)]
 
 
+class TrialState(C.Structure):
+    _fields_ = [("epochs_run", C.c_int32), ("ndcg", C.c_float), ("finished", C.c_int32)]
+
+
 FM_ADAM, FM_SGD = 0, 1
 
 
@@ -163,6 +168,7 @@ class RecommendRanker(C.Structure):
 
 
 PROGRESS_FN = C.CFUNCTYPE(C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_float)
+TRIALS_PROGRESS_FN = C.CFUNCTYPE(C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.POINTER(TrialState))
 
 
 class GorseB200Error(RuntimeError):

@@ -27,6 +27,7 @@
 #include <cstdlib>
 
 #include "als.cuh"
+#include "tables.cuh"
 
 namespace gb {
 
@@ -768,11 +769,8 @@ static int32_t exchange_shards(gorse_b200_cf *cf, int side, float *table)
     return GORSE_B200_OK;
 }
 
-extern "C" int32_t gorse_b200_als_epoch(gorse_b200_cf *cf, float reg, float alpha)
+int32_t gb::als_epoch_tables(gorse_b200_cf *cf, float *P_own, float *Q, float reg, float alpha)
 {
-    GB_CHECK_ARG(cf != nullptr, "cf is NULL");
-    if (!cf->has_item_csr) { set_error("als_epoch needs the item CSR (item_off/item_users) at cf_create"); return GORSE_B200_ERR_STATE; }
-    ScopedDevice sd(cf->ctx->device);
     gorse_b200_ctx *c = cf->ctx;
     const bool multi = c->world > 1;
     GB_TRY(prepare_als(cf));
@@ -790,32 +788,40 @@ extern "C" int32_t gorse_b200_als_epoch(gorse_b200_cf *cf, float reg, float alph
     // exchanged, S^p and the item sweep (own item range) on P_all, item ranges of Q exchanged, own rows of P_all back.
     // Each Gram is the all-reduced sum of the ranks' partial Grams over their own row ranges, so every rank holds
     // bit-identical S^q, S^p and Q (the sums differ from the single-GPU epoch by reassociation only).
-    float *P = cf->P.p;
+    float *P = P_own;
     const int64_t own = (int64_t)(cf->u_hi - cf->u_lo) * cf->d;
     if (multi) {
         if (cf->P_all.n == 0 && (st = cf->P_all.alloc((size_t)cf->n_users * cf->d))) return done(st);
         P = cf->P_all.p;
         if (own) {
-            cudaError_t e = cudaMemcpyAsync(P + (int64_t)cf->u_lo * cf->d, cf->P.p, own * sizeof(float), cudaMemcpyDeviceToDevice, c->stream);
+            cudaError_t e = cudaMemcpyAsync(P + (int64_t)cf->u_lo * cf->d, P_own, own * sizeof(float), cudaMemcpyDeviceToDevice, c->stream);
             if (e != cudaSuccess) { set_error("als_epoch: %s", cudaGetErrorString(e)); return done(GORSE_B200_ERR_CUDA); }
         }
     }
     // the row kernels index the offsets with GLOBAL row ids: hand them the rank's arrays shifted by the range start
     const int64_t *uoff = cf->user_off.p - cf->u_lo, *ioff = cf->item_off.p - cf->i_lo;
-    if ((st = run_gram(cf, 1, cf->Q.p))) return done(st);
-    if ((st = run_rows(cf, 0, P, cf->Q.p, uoff, cf->user_items.p, reg, alpha, pred.p))) return done(st);
+    if ((st = run_gram(cf, 1, Q))) return done(st);
+    if ((st = run_rows(cf, 0, P, Q, uoff, cf->user_items.p, reg, alpha, pred.p))) return done(st);
     if (multi && (st = exchange_shards(cf, 0, P))) return done(st);
     if ((st = run_gram(cf, 0, P))) return done(st);
-    if ((st = run_rows(cf, 1, cf->Q.p, P, ioff, cf->item_users.p, reg, alpha, pred.p))) return done(st);
+    if ((st = run_rows(cf, 1, Q, P, ioff, cf->item_users.p, reg, alpha, pred.p))) return done(st);
     if (multi) {
-        if ((st = exchange_shards(cf, 1, cf->Q.p))) return done(st);
+        if ((st = exchange_shards(cf, 1, Q))) return done(st);
         cudaError_t e = cudaSuccess;
-        if (own) e = cudaMemcpyAsync(cf->P.p, P + (int64_t)cf->u_lo * cf->d, own * sizeof(float), cudaMemcpyDeviceToDevice, c->stream);
+        if (own) e = cudaMemcpyAsync(P_own, P + (int64_t)cf->u_lo * cf->d, own * sizeof(float), cudaMemcpyDeviceToDevice, c->stream);
         // the BPR exchange keeps the last synchronised item table in Q0
-        if (e == cudaSuccess && cf->Q0.n) e = cudaMemcpyAsync(cf->Q0.p, cf->Q.p, cf->Q.n * sizeof(float), cudaMemcpyDeviceToDevice, c->stream);
+        if (e == cudaSuccess && cf->Q0.n) e = cudaMemcpyAsync(cf->Q0.p, Q, cf->Q.n * sizeof(float), cudaMemcpyDeviceToDevice, c->stream);
         if (e != cudaSuccess) { set_error("als_epoch: %s", cudaGetErrorString(e)); return done(GORSE_B200_ERR_CUDA); }
     }
     cudaError_t e = cudaStreamSynchronize(c->stream);
     if (e != cudaSuccess) { set_error("als_epoch: %s", cudaGetErrorString(e)); return done(GORSE_B200_ERR_CUDA); }
     return done(GORSE_B200_OK);
+}
+
+extern "C" int32_t gorse_b200_als_epoch(gorse_b200_cf *cf, float reg, float alpha)
+{
+    GB_CHECK_ARG(cf != nullptr, "cf is NULL");
+    if (!cf->has_item_csr) { set_error("als_epoch needs the item CSR (item_off/item_users) at cf_create"); return GORSE_B200_ERR_STATE; }
+    ScopedDevice sd(cf->ctx->device);
+    return als_epoch_tables(cf, cf->P.p, cf->Q.p, reg, alpha);
 }

@@ -8,6 +8,7 @@
 #include <cstdlib>
 
 #include "cf.cuh"
+#include "tables.cuh"
 #include "wgmma.cuh"
 
 namespace gb {
@@ -417,6 +418,144 @@ __global__ void __launch_bounds__(kRoundThreads, 1)
     }
 }
 
+// ---- the round epoch of several models on one triple stream (gorse_b200_cf_fit_trials) -------------------------------
+// The trials of a model search share the CSR, the seed and the factor count, so their epochs sample the same triples.
+// bpr_trials_round_kernel runs one round epoch for up to kMaxTrialModels models: the samplers draw and link each triple once,
+// and the consumers do each model's arithmetic on that model's rows.  The rounds, the triple-to-(CTA, quad) placement and
+// the chain order are bpr_round_kernel's, so every model reads what its solo epoch reads and computes the same deltas.
+constexpr int kMaxTrialModels = 16;
+struct TrialModels {
+    float *P[kMaxTrialModels], *Q[kMaxTrialModels];
+    float lr[kMaxTrialModels], reg[kMaxTrialModels];
+    int32_t n;
+};
+
+// Dynamic shared memory: per model, the round's deltas of 64 user rows and 2 * 64 item rows of d floats (3 * 64 * d floats).
+// A consumer writes its triple's three deltas for every model before the first grid barrier, so no model's rows need to
+// stay in registers across it; after the barrier it sends the user row and sums the item chains of every model.
+template <int C>
+__global__ void __launch_bounds__(kRoundThreads, 1)
+    bpr_trials_round_kernel(BprView v, TrialModels M, int64_t step0, int64_t n_steps, uint64_t base, uint32_t *barrier_count)
+{
+    __shared__ RoundSlot ring[kRing];
+    __shared__ uint64_t full[kRing], empty[kRing];
+    extern __shared__ float4 delta_smem[];
+    constexpr int d = 16 * C;
+    constexpr int kModelFloats = 3 * kRoundQuads * d;
+    const int64_t nq = (int64_t)gridDim.x * kRoundQuads;
+    const int64_t n_rounds = (n_steps + nq - 1) / nq;
+    if (threadIdx.x == 0) {
+        for (int s = 0; s < kRing; s++) {
+            mma::mbar_init(&full[s], kSamplers);
+            mma::mbar_init(&empty[s], kConsumers / 32);
+        }
+    }
+    __syncthreads();
+
+    if (threadIdx.x >= kConsumers) {
+        // sampler: as in bpr_round_kernel, with the rows of every model prefetched
+        const int t = (threadIdx.x - kConsumers) % kSamplers, group = (threadIdx.x - kConsumers) / kSamplers;
+        for (int64_t r = group; r < n_rounds; r += kSamplerGroups) {
+            const int s = (int)(r % kRing);
+            if (r >= kRing) mma::mbar_wait_backoff(&empty[s], (uint32_t)((r / kRing - 1) & 1));
+            RoundSlot &S = ring[s];
+            const int64_t q = r * nq + (int64_t)blockIdx.x * kRoundQuads + t;
+            int32_t u = v.u_lo, i = -1, j = -1;
+            if (q < n_steps) sample_triple(v, base, step0 + q, u, i, j);
+            if (j < 0) i = -1;
+            else {
+                for (int m = 0; m < M.n; m++) {
+                    prefetch_l2(M.P[m] + (int64_t)(u - v.u_lo) * d, 64 * C);
+                    prefetch_l2(M.Q[m] + (int64_t)j * d, 64 * C);
+                }
+            }
+            S.u[t] = u; S.item[t] = i; S.item[kRoundQuads + t] = j;
+            sampler_bar(group);
+            const int e0 = t, e1 = kRoundQuads + t;
+            int nxt0 = -1, nxt1 = -1;
+            bool first0 = i >= 0, first1 = j >= 0;
+            auto see = [&](int32_t id, int k) {
+                if (id == i) { if (k < e0) first0 = false; else if (k > e0) nxt0 = k; }
+                if (id == j) { if (k < e1) first1 = false; else if (k > e1) nxt1 = k; }
+            };
+            const int4 *items4 = reinterpret_cast<const int4 *>(S.item);
+            for (int k = 2 * kRoundQuads - 4; k >= 0; k -= 4) {
+                const int4 x = items4[k / 4];
+                see(x.w, k + 3); see(x.z, k + 2); see(x.y, k + 1); see(x.x, k);
+            }
+            S.next[e0] = nxt0; S.first[e0] = first0;
+            S.next[e1] = nxt1; S.first[e1] = first1;
+            mma::mbar_arrive(&full[s]);
+        }
+        return;
+    }
+
+    // consumer: quad t of this CTA; entry e of model m, chunk c at D + m * kModelFloats + e * d + 16 * c, where entries
+    // 0..63 are the user rows and 64..191 the item entries of the ring slot (item entry k at 64 + k)
+    const int t = threadIdx.x >> 2, lane4 = threadIdx.x & 3;
+    const unsigned mask = quad_mask();
+    float *const D = reinterpret_cast<float *>(delta_smem) + 4 * lane4;
+    uint32_t n_sync = 0;
+    for (int64_t r = 0; r < n_rounds; r++) {
+        const int s = (int)(r % kRing);
+        mma::mbar_wait(&full[s], (uint32_t)((r / kRing) & 1));
+        const RoundSlot &S = ring[s];
+        const int32_t u = S.u[t], i = S.item[t], j = S.item[kRoundQuads + t];
+        if (j >= 0) {
+#pragma unroll 1
+            for (int m = 0; m < M.n; m++) {
+                const float lr = M.lr[m], nreg = -M.reg[m];
+                Rows<C> rw;
+                load_rows<C>(rw, M.P[m] + (int64_t)(u - v.u_lo) * d + 4 * lane4, M.Q[m] + (int64_t)i * d + 4 * lane4, 16,
+                             M.Q[m] + (int64_t)j * d + 4 * lane4, 16);
+                const float g = bpr_grad_rows<C>(rw, mask);
+                float *Dm = D + m * kModelFloats, *Dp = Dm + t * d, *Di = Dm + (kRoundQuads + t) * d, *Dj = Dm + (2 * kRoundQuads + t) * d;
+#pragma unroll
+                for (int c = 0; c < C; c++) {
+                    float4 ti, tj, tp, o;
+                    bpr_dirs<C>(rw, c, g, nreg, ti, tj, tp);
+                    GB_F4_OP(o, __fmul_rn(f4get(tp, k_), lr)); *reinterpret_cast<float4 *>(Dp + 16 * c) = o;
+                    GB_F4_OP(o, __fmul_rn(f4get(ti, k_), lr)); *reinterpret_cast<float4 *>(Di + 16 * c) = o;
+                    GB_F4_OP(o, __fmul_rn(f4get(tj, k_), lr)); *reinterpret_cast<float4 *>(Dj + 16 * c) = o;
+                }
+            }
+        }
+        consumer_grid_sync(barrier_count, ++n_sync * gridDim.x);
+#pragma unroll 1
+        for (int m = 0; m < M.n; m++) {
+            const float *Dm = D + m * kModelFloats;
+            if (j >= 0) {
+                float *Pu = M.P[m] + (int64_t)(u - v.u_lo) * d + 4 * lane4;
+#pragma unroll
+                for (int c = 0; c < C; c++) red_row(Pu + 16 * c, *reinterpret_cast<const float4 *>(Dm + t * d + 16 * c));
+            }
+            // the first entry of each item chain adds the chain's deltas in entry order and sends one reduction
+#pragma unroll
+            for (int h = 0; h < 2; h++) {
+                const int e = t + h * kRoundQuads;
+                if (!S.first[e]) continue;
+                const float *De = Dm + kRoundQuads * d;
+                float4 acc[C];
+#pragma unroll
+                for (int c = 0; c < C; c++) acc[c] = *reinterpret_cast<const float4 *>(De + e * d + 16 * c);
+                for (int k = S.next[e]; k >= 0; k = S.next[k]) {
+#pragma unroll
+                    for (int c = 0; c < C; c++) {
+                        const float4 x = *reinterpret_cast<const float4 *>(De + k * d + 16 * c);
+                        GB_F4_OP(acc[c], __fadd_rn(f4get(acc[c], k_), f4get(x, k_)));
+                    }
+                }
+                float *Qe = M.Q[m] + (int64_t)S.item[e] * d + 4 * lane4;
+#pragma unroll
+                for (int c = 0; c < C; c++) red_row(Qe + 16 * c, acc[c]);
+            }
+        }
+        __syncwarp();
+        if ((threadIdx.x & 31) == 0) mma::mbar_arrive(&empty[s]);
+        consumer_grid_sync(barrier_count, ++n_sync * gridDim.x);
+    }
+}
+
 template <int C, bool ATOMIC>
 __global__ void __launch_bounds__(256) bpr_apply_kernel(BprView v, const int32_t *uij, int64_t n, float lr, float reg)
 {
@@ -675,6 +814,44 @@ static int32_t launch_round_epoch(gorse_b200_cf *cf, BprView v, int64_t step0, i
     return GORSE_B200_OK;
 }
 
+// One atomic round epoch for each of n models on cf's triple stream, in launches of as many models as the kernel's shared
+// memory holds.  The grid is launch_round_epoch's, so the rounds and the placement are the solo epoch's.
+template <int C>
+static int32_t launch_trials_epoch(gorse_b200_cf *cf, int n, float *const *P, float *const *Q, const float *lr, const float *reg,
+                                   uint64_t base)
+{
+    gorse_b200_ctx *c = cf->ctx;
+    auto *k = bpr_trials_round_kernel<C>;
+    const size_t per_model = (size_t)3 * kRoundQuads * 16 * C * sizeof(float);
+    int optin = 0;
+    GB_CUDA(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, c->device));
+    cudaFuncAttributes fa;
+    GB_CUDA(cudaFuncGetAttributes(&fa, k));
+    const int cap = (int)std::min<size_t>(kMaxTrialModels, ((size_t)optin - fa.sharedSizeBytes) / per_model);
+    if (cap < 1) { set_error("bpr_trials_round_kernel does not fit on the device"); return GORSE_B200_ERR_UNSUPPORTED; }
+    const int group = std::min(cap, n);
+    const size_t smem_max = (size_t)group * per_model;
+    GB_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_max));
+    int per_sm = 0;
+    GB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k, kRoundThreads, smem_max));
+    const int g = (int)std::min<int64_t>(GB_BPR_ROUND / kRoundQuads, (int64_t)per_sm * c->sm_count);
+    if (g < 1) { set_error("bpr_trials_round_kernel does not fit on the device"); return GORSE_B200_ERR_UNSUPPORTED; }
+    BprView v = make_view(cf);
+    int64_t step0 = 0, n_steps = cf->n_feedback_global;
+    uint32_t *count = cf->bpr_barrier.p;
+    for (int m0 = 0; m0 < n; m0 += group) {
+        TrialModels M{};
+        M.n = std::min(group, n - m0);
+        for (int m = 0; m < M.n; m++) { M.P[m] = P[m0 + m]; M.Q[m] = Q[m0 + m]; M.lr[m] = lr[m0 + m]; M.reg[m] = reg[m0 + m]; }
+        const size_t smem = (size_t)M.n * per_model;
+        GB_CUDA(cudaMemsetAsync(count, 0, sizeof(uint32_t), c->stream));
+        void *args[] = {&v, &M, &step0, &n_steps, &base, &count};
+        GB_CUDA(cudaLaunchCooperativeKernel((const void *)k, dim3(g), dim3(kRoundThreads), args, smem, c->stream));
+        GB_LAUNCHED(c);
+    }
+    return GORSE_B200_OK;
+}
+
 // the atomic-scatter epoch at d outside 16/32/64/128: rounds of GB_BPR_ROUND steps, a delta and an add launch each
 static int32_t launch_round_epoch_any(gorse_b200_cf *cf, BprView v, int64_t step0, int64_t n, uint64_t base, float lr, float reg)
 {
@@ -738,6 +915,19 @@ static void launch_apply(gorse_b200_cf *cf, const BprView &v, const int32_t *d_u
     } else {
         int g = (int)std::max<int64_t>(1, std::min<int64_t>((n + 127) / 128, (int64_t)c->sm_count * 8));
         bpr_apply_any_kernel<ATOMIC><<<g, 128, 0, s>>>(v, d_uij, n, lr, reg);
+    }
+}
+
+int32_t bpr_trials_epoch(gorse_b200_cf *cf, int n, float *const *P, float *const *Q, const float *lr, const float *reg, uint64_t seed)
+{
+    if (n == 0 || cf->n_feedback_global == 0) return GORSE_B200_OK;
+    const uint64_t base = mix64(seed);
+    switch (cf->d) {
+        case 16: return launch_trials_epoch<1>(cf, n, P, Q, lr, reg, base);
+        case 32: return launch_trials_epoch<2>(cf, n, P, Q, lr, reg, base);
+        case 64: return launch_trials_epoch<4>(cf, n, P, Q, lr, reg, base);
+        case 128: return launch_trials_epoch<8>(cf, n, P, Q, lr, reg, base);
+        default: set_error("batched BPR trials need d in {16, 32, 64, 128}, not %d", cf->d); return GORSE_B200_ERR_UNSUPPORTED;
     }
 }
 

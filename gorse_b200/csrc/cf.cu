@@ -4,6 +4,7 @@
 #include <thread>
 
 #include "cf.cuh"
+#include "tables.cuh"
 
 namespace gb {
 
@@ -88,6 +89,22 @@ static void parallel_rows(int32_t rows, int64_t nnz, F &&work)
     for (unsigned t = 0; t < nt; t++)
         th.emplace_back(work, (int32_t)((int64_t)rows * t / nt), (int32_t)((int64_t)rows * (t + 1) / nt), t);
     for (auto &x : th) x.join();
+}
+
+int32_t init_normal_tables(gorse_b200_cf *cf, float *P, float *Q, float mean, float stddev, uint64_t seed)
+{
+    gorse_b200_ctx *c = cf->ctx;
+    uint64_t base = mix64(seed ^ 0x6a09e667f3bcc908ull);
+    // element index in the reference's stream order: users then items (model/cf/model.go:534-535)
+    if (cf->P.n) {
+        init_normal_kernel<<<c->sm_count * 8, 256, 0, c->stream>>>(P, (int64_t)cf->P.n, (int64_t)cf->u_lo * cf->d, base, mean, stddev);
+        GB_LAUNCHED(c);
+    }
+    if (cf->Q.n) {
+        init_normal_kernel<<<c->sm_count * 8, 256, 0, c->stream>>>(Q, (int64_t)cf->Q.n, (int64_t)cf->n_users * cf->d, base, mean, stddev);
+        GB_LAUNCHED(c);
+    }
+    return GORSE_B200_OK;
 }
 
 }  // namespace gb
@@ -316,18 +333,7 @@ int32_t gorse_b200_cf_init_normal(gorse_b200_cf *cf, float mean, float stddev, u
     GB_CHECK_ARG(cf != nullptr, "cf is NULL");
     ScopedDevice sd(cf->ctx->device);
     gorse_b200_ctx *c = cf->ctx;
-    uint64_t base = mix64(seed ^ 0x6a09e667f3bcc908ull);
-    // element index in the reference's stream order: users then items (model/cf/model.go:534-535)
-    if (cf->P.n) {
-        init_normal_kernel<<<c->sm_count * 8, 256, 0, c->stream>>>(cf->P.p, (int64_t)cf->P.n,
-                                                                  (int64_t)cf->u_lo * cf->d, base, mean, stddev);
-        GB_LAUNCHED(c);
-    }
-    if (cf->Q.n) {
-        init_normal_kernel<<<c->sm_count * 8, 256, 0, c->stream>>>(cf->Q.p, (int64_t)cf->Q.n,
-                                                                  (int64_t)cf->n_users * cf->d, base, mean, stddev);
-        GB_LAUNCHED(c);
-    }
+    GB_TRY(init_normal_tables(cf, cf->P.p, cf->Q.p, mean, stddev, seed));
     // every rank generates the same replicated Q; keep the epoch-start copy used by the delta exchange
     if (cf->Q0.n) GB_CUDA(cudaMemcpyAsync(cf->Q0.p, cf->Q.p, cf->Q.n * sizeof(float), cudaMemcpyDeviceToDevice, c->stream));
     return GORSE_B200_OK;

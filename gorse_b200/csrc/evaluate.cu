@@ -5,6 +5,7 @@
 #include <cmath>
 
 #include "cf.cuh"
+#include "tables.cuh"
 
 namespace gb {
 
@@ -209,6 +210,64 @@ struct gorse_b200_eval {
     std::vector<int64_t> h_neg_off;
 };
 
+int32_t gb::eval_run_tables(gorse_b200_eval *ev, const float *P, const float *Q, float *out)
+{
+    gorse_b200_cf *cf = ev->cf;
+    gorse_b200_ctx *c = cf->ctx;
+    const bool multi = c->world > 1;
+    const int32_t U = ev->U;
+    const int64_t nc = ev->nc;
+    out[0] = out[1] = out[2] = 0.f;
+    if (nc == 0 && !multi) { out[0] = out[1] = out[2] = NAN; return GORSE_B200_OK; }  // 0 * (1/0), like the reference
+    ScopedDevice sd(c->device);
+    cudaStream_t s = c->stream;
+    cudaError_t e = cudaSuccess;
+    if (nc > 0) {
+        int threads = 256;
+        int64_t work = cf->d % 16 == 0 ? nc * 4 : nc;
+        int blocks = (int)std::max<int64_t>(1, std::min<int64_t>((work + threads - 1) / threads, (int64_t)c->sm_count * 16));
+        eval_score_kernel<<<blocks, threads, 0, s>>>(P, Q, cf->d, cf->u_lo, ev->cand_user.p, ev->cand_item.p, nc, ev->score.p);
+        c->launches++;
+        eval_rank_kernel<<<(U + 127) / 128, 128, 0, s>>>(ev->cand_off.p, ev->cand_item.p, ev->score.p, ev->test_off.p, ev->test_items.p, U, ev->topk,
+                                                         ev->inv.p, ev->metrics.p);
+        c->launches++;
+        if ((e = cudaGetLastError()) != cudaSuccess) { set_error("evaluate launch: %s", cudaGetErrorString(e)); return GORSE_B200_ERR_CUDA; }
+        if ((e = cudaMemcpyAsync(ev->h_metrics.data(), ev->metrics.p, sizeof(float) * 4 * (size_t)U, cudaMemcpyDeviceToHost, s)) != cudaSuccess ||
+            (e = cudaStreamSynchronize(s)) != cudaSuccess) {
+            set_error("evaluate: %s", cudaGetErrorString(e));
+            return GORSE_B200_ERR_CUDA;
+        }
+    }
+    // evaluator.go:63-71 with one worker: fp32 sums in user order, then * (1/count)
+    volatile float sum0 = 0.f, sum1 = 0.f, sum2 = 0.f, count = 0.f;
+    if (nc > 0)
+        for (int32_t u = 0; u < U; u++) {
+            const float *m = ev->h_metrics.data() + 4 * (size_t)u;
+            if (m[3] != 0.f) {
+                count = count + 1.0f;
+                sum0 = sum0 + m[0]; sum1 = sum1 + m[1]; sum2 = sum2 + m[2];
+            }
+        }
+    if (multi) {
+        // sum of the per-rank partial sums (the reference with Jobs = world: one partial sum per worker, evaluator.go:63-71)
+        float h[4] = {sum0, sum1, sum2, count};
+        DevBuf<float> dsum;
+        GB_NCCL_API(nc_api);
+        GB_TRY(dsum.alloc(4));
+        e = cudaMemcpyAsync(dsum.p, h, sizeof(h), cudaMemcpyHostToDevice, s);
+        ncclResult_t r = e == cudaSuccess ? nc_api->AllReduce(dsum.p, dsum.p, 4, ncclFloat32, ncclSum, c->comm, s) : ncclSuccess;
+        if (e == cudaSuccess && r == ncclSuccess) e = cudaMemcpyAsync(h, dsum.p, sizeof(h), cudaMemcpyDeviceToHost, s);
+        if (e == cudaSuccess && r == ncclSuccess) e = cudaStreamSynchronize(s);
+        dsum.free();
+        if (r != ncclSuccess) { set_error("evaluate: ncclAllReduce -> %s", nc_api->GetErrorString(r)); return GORSE_B200_ERR_NCCL; }
+        if (e != cudaSuccess) { set_error("evaluate: %s", cudaGetErrorString(e)); return GORSE_B200_ERR_CUDA; }
+        sum0 = h[0]; sum1 = h[1]; sum2 = h[2]; count = h[3];
+    }
+    volatile float inv = 1.0f / count;
+    out[0] = sum0 * inv; out[1] = sum1 * inv; out[2] = sum2 * inv;
+    return GORSE_B200_OK;
+}
+
 extern "C" {
 
 int32_t gorse_b200_eval_destroy(gorse_b200_eval *ev)
@@ -328,60 +387,7 @@ int32_t gorse_b200_eval_negatives(gorse_b200_eval *ev, int64_t *neg_off_out, int
 int32_t gorse_b200_eval_run(gorse_b200_eval *ev, float *out)
 {
     GB_CHECK_ARG(ev != nullptr && out != nullptr, "NULL eval/out");
-    gorse_b200_cf *cf = ev->cf;
-    gorse_b200_ctx *c = cf->ctx;
-    const bool multi = c->world > 1;
-    const int32_t U = ev->U;
-    const int64_t nc = ev->nc;
-    out[0] = out[1] = out[2] = 0.f;
-    if (nc == 0 && !multi) { out[0] = out[1] = out[2] = NAN; return GORSE_B200_OK; }  // 0 * (1/0), like the reference
-    ScopedDevice sd(c->device);
-    cudaStream_t s = c->stream;
-    cudaError_t e = cudaSuccess;
-    if (nc > 0) {
-        int threads = 256;
-        int64_t work = cf->d % 16 == 0 ? nc * 4 : nc;
-        int blocks = (int)std::max<int64_t>(1, std::min<int64_t>((work + threads - 1) / threads, (int64_t)c->sm_count * 16));
-        eval_score_kernel<<<blocks, threads, 0, s>>>(cf->P.p, cf->Q.p, cf->d, cf->u_lo, ev->cand_user.p, ev->cand_item.p, nc, ev->score.p);
-        c->launches++;
-        eval_rank_kernel<<<(U + 127) / 128, 128, 0, s>>>(ev->cand_off.p, ev->cand_item.p, ev->score.p, ev->test_off.p, ev->test_items.p, U, ev->topk,
-                                                         ev->inv.p, ev->metrics.p);
-        c->launches++;
-        if ((e = cudaGetLastError()) != cudaSuccess) { set_error("evaluate launch: %s", cudaGetErrorString(e)); return GORSE_B200_ERR_CUDA; }
-        if ((e = cudaMemcpyAsync(ev->h_metrics.data(), ev->metrics.p, sizeof(float) * 4 * (size_t)U, cudaMemcpyDeviceToHost, s)) != cudaSuccess ||
-            (e = cudaStreamSynchronize(s)) != cudaSuccess) {
-            set_error("evaluate: %s", cudaGetErrorString(e));
-            return GORSE_B200_ERR_CUDA;
-        }
-    }
-    // evaluator.go:63-71 with one worker: fp32 sums in user order, then * (1/count)
-    volatile float sum0 = 0.f, sum1 = 0.f, sum2 = 0.f, count = 0.f;
-    if (nc > 0)
-        for (int32_t u = 0; u < U; u++) {
-            const float *m = ev->h_metrics.data() + 4 * (size_t)u;
-            if (m[3] != 0.f) {
-                count = count + 1.0f;
-                sum0 = sum0 + m[0]; sum1 = sum1 + m[1]; sum2 = sum2 + m[2];
-            }
-        }
-    if (multi) {
-        // sum of the per-rank partial sums (the reference with Jobs = world: one partial sum per worker, evaluator.go:63-71)
-        float h[4] = {sum0, sum1, sum2, count};
-        DevBuf<float> dsum;
-        GB_NCCL_API(nc_api);
-        GB_TRY(dsum.alloc(4));
-        e = cudaMemcpyAsync(dsum.p, h, sizeof(h), cudaMemcpyHostToDevice, s);
-        ncclResult_t r = e == cudaSuccess ? nc_api->AllReduce(dsum.p, dsum.p, 4, ncclFloat32, ncclSum, c->comm, s) : ncclSuccess;
-        if (e == cudaSuccess && r == ncclSuccess) e = cudaMemcpyAsync(h, dsum.p, sizeof(h), cudaMemcpyDeviceToHost, s);
-        if (e == cudaSuccess && r == ncclSuccess) e = cudaStreamSynchronize(s);
-        dsum.free();
-        if (r != ncclSuccess) { set_error("evaluate: ncclAllReduce -> %s", nc_api->GetErrorString(r)); return GORSE_B200_ERR_NCCL; }
-        if (e != cudaSuccess) { set_error("evaluate: %s", cudaGetErrorString(e)); return GORSE_B200_ERR_CUDA; }
-        sum0 = h[0]; sum1 = h[1]; sum2 = h[2]; count = h[3];
-    }
-    volatile float inv = 1.0f / count;
-    out[0] = sum0 * inv; out[1] = sum1 * inv; out[2] = sum2 * inv;
-    return GORSE_B200_OK;
+    return eval_run_tables(ev, ev->cf->P.p, ev->cf->Q.p, out);
 }
 
 int32_t gorse_b200_cf_evaluate(gorse_b200_cf *cf, const int64_t *test_off, const int32_t *test_items,

@@ -230,6 +230,39 @@ int32_t gorse_b200_als_fit(gorse_b200_cf *cf, const gorse_b200_fit_params *param
                            gorse_b200_progress_fn progress, void *user, gorse_b200_fit_result *result);
 
 /* ------------------------------------------------------------------------------------------
+ * Model search.  The trials of ModelSearch.Objective (model/cf/optimize.go:61-81), which
+ * optimizeCollaborativeFiltering (master/tasks.go:1268-1316) runs on every dataset load when
+ * recommend.collaborative.optimize_period > 0, fitted in one call.  Trial k (als[k] != 0: eALS, else BPR) is what
+ * gorse_b200_als_fit / gorse_b200_bpr_fit does with trials[k] on tables of its own: Init, Evaluate at epoch 0, n_epochs
+ * epochs, Evaluate every `verbose` epochs and on the last one, Patience with the first-maximum rule; results[k] equals
+ * that fit's result.  The trials share the search's FitConfig and RandomState: n_factors (== cf's d), seed, verbose,
+ * candidates, topk and patience must be equal in every trial (else GORSE_B200_ERR_ARG); n_epochs and the model's
+ * hyper-parameters may differ.  At one seed every BPR trial samples the same triples, so each epoch samples every triple
+ * once for all the BPR trials and runs their arithmetic in the same cooperative launch (16 models per launch at d = 16,
+ * 9 at 32, 4 at 64, 2 at 128; more run as successive launches); ALS trials run gorse_b200_als_epoch's kernels on their
+ * own tables.  One evaluation plan serves every trial (negatives drawn at seed 0 when neg_off is NULL, as each solo fit
+ * draws them).  A trial that stops or finishes leaves the batch with its tables as they are.
+ * progress (may be NULL) is called once per epoch of the batch with the state of every trial; a non-zero return
+ * cancels: a trial not reported finished in that call returns cancelled = 1 and a zero score, the others keep theirs.
+ * P_out / Q_out (each may be NULL, as may any entry): trial k's final factors are copied to P_out[k] (n_users x d) and
+ * Q_out[k] (n_items x d).  The trial tables are allocated in the call and freed before it returns; cf's own factors are
+ * not touched.  Every argument is checked on the host before the device is touched (cf last): BPR trials need d in
+ * {16, 32, 64, 128} and ALS trials the item CSR (GORSE_B200_ERR_UNSUPPORTED / GORSE_B200_ERR_STATE); a distributed
+ * context is GORSE_B200_ERR_UNSUPPORTED.
+ * ---------------------------------------------------------------------------------------- */
+typedef struct {
+    int32_t epochs_run;  /* epochs the trial has run so far */
+    float ndcg;          /* NDCG of this epoch's evaluation, < 0 when the trial was not evaluated in this epoch */
+    int32_t finished;    /* 1 once the trial has run its n_epochs or stopped early */
+} gorse_b200_trial_state;
+typedef int32_t (*gorse_b200_trials_progress_fn)(void *user, int32_t epoch, int32_t n_trials, const gorse_b200_trial_state *states);
+
+int32_t gorse_b200_cf_fit_trials(gorse_b200_cf *cf, int32_t n_trials, const int32_t *als, const gorse_b200_fit_params *trials,
+                                 const int64_t *test_off, const int32_t *test_items, const int64_t *neg_off,
+                                 const int32_t *neg_items, gorse_b200_trials_progress_fn progress, void *user,
+                                 gorse_b200_fit_result *results, float *const *P_out, float *const *Q_out);
+
+/* ------------------------------------------------------------------------------------------
  * Brute-force index.  Replaces ann.Bruteforce[[]float32] (common/ann/bruteforce.go:24-83)
  * behind ann.Index (common/ann/ann.go:21-25).
  * ---------------------------------------------------------------------------------------- */
