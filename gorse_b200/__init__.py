@@ -848,6 +848,74 @@ class FMTrainer:
         out = {f: getattr(res, f) for f, _ in _lib.FMFitResult._fields_}
         return pout[:pin.size], out, mom
 
+    def fit_trials(self, trials, train, test, params_in_list, emb=None, progress=None, moments=False):
+        """AFM's ModelSearch trials in one gorse_b200_fm_fit_trials call.  trials: one dict per trial overriding this trainer's
+        params (lr, reg, optimizer and n_epochs may differ; n_factors, batch_size, verbose, patience and max_steps are
+        shared); params_in_list: each trial's fm.Parameters() after its own Init.  emb: None, or (emb_dims, item_emb,
+        item_emb_mask, train_emb_row, test_emb_row) as fit_emb takes them.  progress(epoch, states), states a list of
+        (epochs_run, auc or -1, finished) per trial, returns True to cancel.
+        -> one (params, result dict, moments or None) per trial, each equal to that trial's solo fit bit for bit"""
+        n = len(trials)
+        if n != len(params_in_list):
+            raise ValueError("one params_in per trial")
+        tr, te = self._rows(train), self._rows(test)
+        fps = (_lib.FMFitParams * max(n, 1))()
+        for i, over in enumerate(trials):
+            C.memmove(C.byref(fps[i]), C.byref(self.params), C.sizeof(_lib.FMFitParams))
+            for key, v in over.items():
+                setattr(fps[i], key, v)
+        dims, tabs, mask, er = self._emb(emb, tr, te)
+        k = self.params.n_factors
+        want = self.n_params() + sum(k * (3 * int(d) + 2) for d in dims)
+        pins = [np.ascontiguousarray(p, np.float32).reshape(-1) for p in params_in_list]
+        if any(p.size != want for p in pins):
+            raise ValueError(f"every params_in must hold the model's {want} floats")
+        pouts = [np.zeros(max(want, 1), np.float32) for _ in range(n)]
+        moms = [np.zeros((2, want), np.float32) for _ in range(n)] if moments else None
+        pin_arr = (C.c_void_p * max(n, 1))(*[ptr(p) for p in pins])
+        pout_arr = (C.c_void_p * max(n, 1))(*[ptr(p) for p in pouts])
+        mom_arr = (C.c_void_p * max(n, 1))(*[ptr(m) for m in moms]) if moments else None
+        res = (_lib.FMFitResult * max(n, 1))()
+
+        def on_epoch(user, epoch, n_trials, states):
+            return int(bool(progress(epoch, [(states[i].epochs_run, states[i].auc, bool(states[i].finished)) for i in range(n_trials)])))
+
+        cb = _lib.FM_TRIALS_PROGRESS_FN(on_epoch) if progress else None
+        arr = (C.c_void_p * max(len(tabs), 1))(*[ptr(t) for t in tabs])
+        n_rows = tabs[0].shape[0] if tabs else 0
+        check(lib.gorse_b200_fm_fit_trials(self.ctx.h, self.n_features, self.num_dimension, n, C.cast(fps, C.c_void_p), tr[0], ptr(tr[1]),
+                                           ptr(tr[2]), ptr(tr[3]), ptr(tr[4]), ptr(er[0]), te[0], ptr(te[1]), ptr(te[2]), ptr(te[3]),
+                                           ptr(te[4]), ptr(er[1]), dims.size, ptr(dims), n_rows, arr if tabs else None, ptr(mask),
+                                           C.cast(pin_arr, C.c_void_p), want, C.cast(pout_arr, C.c_void_p),
+                                           C.cast(mom_arr, C.c_void_p) if moments else None, C.cast(cb, C.c_void_p) if cb else None, None,
+                                           C.cast(res, C.c_void_p)))
+        return [(pouts[i][:want], {f: getattr(res[i], f) for f, _ in _lib.FMFitResult._fields_}, moms[i] if moments else None)
+                for i in range(n)]
+
+    @staticmethod
+    def _rows(r):
+        off, idx, val, tgt = r
+        off = np.ascontiguousarray(off, np.int64)
+        return (off.size - 1, off, np.ascontiguousarray(idx, np.int32), np.ascontiguousarray(val, np.float32), np.ascontiguousarray(tgt, np.float32))
+
+    @staticmethod
+    def _emb(emb, tr, te):
+        """(dims, tables, mask, (train rows, test rows)) of fit_trials' emb argument; None: no slots"""
+        if emb is None:
+            return np.zeros(0, np.int32), [], None, (None, None)
+        dims = np.ascontiguousarray(list(emb[0]), np.int32)
+        tabs = [np.ascontiguousarray(t, np.uint16) for t in emb[1]]
+        if len(tabs) != dims.size or any(t.ndim != 2 or t.shape[1] != d or t.shape[0] != tabs[0].shape[0] for t, d in zip(tabs, dims)):
+            raise ValueError("item_emb needs one [n_rows, dim] table per slot")
+        n_rows = tabs[0].shape[0] if tabs else 0
+        mask = None if emb[2] is None else np.ascontiguousarray(emb[2], np.uint8)
+        if mask is not None and mask.shape != (n_rows, dims.size):
+            raise ValueError("item_emb_mask must be [n_rows, n_emb]")
+        er = [np.ascontiguousarray(r, np.int32).reshape(-1) for r in emb[3:5]]
+        if er[0].size != tr[0] or er[1].size != te[0]:
+            raise ValueError("one table row per training and per test sample")
+        return dims, tabs, mask, er
+
 
 def load_ncf(train_path, test_path=None):
     """dataset.LoadDataFromBuiltIn's NCF parsers (dataset/dataset.go:398-490) ->

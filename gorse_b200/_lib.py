@@ -110,6 +110,8 @@ PROTOTYPES = {
                                       VP, VP, VP, VP, VP]),
     "gorse_b200_fm_fit_emb": (C.c_int32, [VP, C.c_int64, C.c_int32, VP, C.c_int64, VP, VP, VP, VP, VP, C.c_int64, VP, VP, VP, VP, VP, C.c_int32,
                                           VP, C.c_int64, VP, VP, VP, C.c_int64, VP, VP, VP, VP, VP]),
+    "gorse_b200_fm_fit_trials": (C.c_int32, [VP, C.c_int64, C.c_int32, C.c_int32, VP, C.c_int64, VP, VP, VP, VP, VP, C.c_int64, VP, VP, VP, VP, VP,
+                                             C.c_int32, VP, C.c_int64, VP, VP, VP, C.c_int64, VP, VP, VP, VP, VP]),
     "gorse_b200_ncf_load":(C.c_int32, [C.c_char_p, C.c_char_p, PVP]),
     "gorse_b200_ncf_shape": (C.c_int32, [VP, C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.POINTER(C.c_int64), C.POINTER(C.c_int64),
                                          C.POINTER(C.c_int64)]),
@@ -141,6 +143,10 @@ class FMFitParams(C.Structure):
                 ("batch_size", C.c_int32), ("verbose", C.c_int32), ("patience", C.c_int32), ("max_steps", C.c_int64)]
 
 
+class FMTrialState(C.Structure):
+    _fields_ = [("epochs_run", C.c_int32), ("auc", C.c_float), ("finished", C.c_int32)]
+
+
 class FMFitResult(C.Structure):
     _fields_ = [("auc", C.c_float), ("precision", C.c_float), ("recall", C.c_float), ("accuracy", C.c_float), ("cost", C.c_float),
                 ("epochs_run", C.c_int32), ("best_epoch", C.c_int32), ("early_stopped", C.c_int32), ("diverged", C.c_int32),
@@ -169,6 +175,7 @@ class RecommendRanker(C.Structure):
 
 PROGRESS_FN = C.CFUNCTYPE(C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_float)
 TRIALS_PROGRESS_FN = C.CFUNCTYPE(C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.POINTER(TrialState))
+FM_TRIALS_PROGRESS_FN = C.CFUNCTYPE(C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.POINTER(FMTrialState))
 
 
 class GorseB200Error(RuntimeError):

@@ -34,6 +34,15 @@ struct Batch {                               // rows [s bs, s bs + B) of a list 
     __device__ int rows() const { return (int)(n - r0() < bs ? n - r0() : bs); }
 };
 
+// trial `off`'s view of a slot: its parameters, gradients and batch tensors; the table and the mask are shared
+__device__ __forceinline__ Slot slot_at(const Slot &S, int64_t off)
+{
+    return Slot{at(S.H, off), at(S.AW, off), at(S.Ab, off), at(S.EW, off), at(S.Eb, off), at(S.gH, off), at(S.gAW, off), at(S.gAb, off),
+                at(S.gEW, off), at(S.gEb, off), S.table, S.mask, S.n_emb, S.s, S.dim, at(S.e, off), at(S.y, off), at(S.att, off),
+                at(S.h, off), at(S.enc, off), at(S.zmax, off), at(S.rowsum, off), at(S.gx, off), at(S.denc, off), at(S.dh, off),
+                at(S.sumdx, off)};
+}
+
 // floats.Dot (floats_avx512.c:306-367) by one thread
 __device__ __forceinline__ float avx_dot(const float *a, const float *b, int n)
 {
@@ -106,10 +115,13 @@ __device__ __forceinline__ float row_sum_step(float sum, float v, int c0, int di
     return sum;
 }
 
-__global__ void __launch_bounds__(WARPS * 32) fm_fit_emb_hz_kernel(Slot S, int k, const int32_t *emb_row, Batch T)
+__global__ void __launch_bounds__(WARPS * 32) fm_fit_emb_hz_kernel(Group G, Slot S0, int k, const int32_t *emb_row, Batch T)
 {
+    Blk tb;
+    if (!trial_block(G, tb)) return;
+    const Slot S = slot_at(S0, tb.off);
     const int lane = threadIdx.x & 31, B = T.rows(), dim = S.dim;
-    for (int b = blockIdx.x * WARPS + (threadIdx.x >> 5); b < B; b += gridDim.x * WARPS) {
+    for (int b = tb.x * WARPS + (threadIdx.x >> 5); b < B; b += tb.nx * WARPS) {
         const int64_t row = emb_row[T.r0() + b];
         const bool present = row >= 0 && (!S.mask || S.mask[row * S.n_emb + S.s]);
         float *e = S.e + (int64_t)b * dim, *z = S.y + (int64_t)b * dim;
@@ -141,10 +153,13 @@ __global__ void __launch_bounds__(WARPS * 32) fm_fit_emb_hz_kernel(Slot S, int k
     }
 }
 
-__global__ void __launch_bounds__(WARPS * 32) fm_fit_emb_exp_kernel(Slot S, Batch T)
+__global__ void __launch_bounds__(WARPS * 32) fm_fit_emb_exp_kernel(Group G, Slot S0, Batch T)
 {
+    Blk tb;
+    if (!trial_block(G, tb)) return;
+    const Slot S = slot_at(S0, tb.off);
     const int lane = threadIdx.x & 31, B = T.rows(), dim = S.dim;
-    for (int r = blockIdx.x * WARPS + (threadIdx.x >> 5); r < B; r += gridDim.x * WARPS) {
+    for (int r = tb.x * WARPS + (threadIdx.x >> 5); r < B; r += tb.nx * WARPS) {
         float *y = S.y + (int64_t)r * dim;
         float sum = 0.0f;
         for (int c0 = 0; c0 < dim; c0 += 32) {
@@ -160,14 +175,20 @@ __global__ void __launch_bounds__(WARPS * 32) fm_fit_emb_exp_kernel(Slot S, Batc
     }
 }
 
-__global__ void __launch_bounds__(WARPS * 32) fm_fit_emb_enc_kernel(Slot S, int k, Batch T, const float *vx, float *p)
+__global__ void __launch_bounds__(WARPS * 32, 1) fm_fit_emb_enc_kernel(Group G, Slot S0, int k, Batch T, const float *vx, float *p)
 {
+    Blk tb;
+    if (!trial_block(G, tb)) return;
+    const int64_t o = tb.off;   // the slot's pointers are offset where they are used
+    const Slot &S = S0;
+    vx = at(vx, o);
+    p = at(p, o);
     const int lane = threadIdx.x & 31, B = T.rows(), dim = S.dim;
-    for (int r = blockIdx.x * WARPS + (threadIdx.x >> 5); r < B; r += gridDim.x * WARPS) {
-        float *y = S.y + (int64_t)r * dim, *att = S.att + (int64_t)r * dim;
-        const float *e = S.e + (int64_t)r * dim;
+    for (int r = tb.x * WARPS + (threadIdx.x >> 5); r < B; r += tb.nx * WARPS) {
+        float *y = at(S.y, o) + (int64_t)r * dim, *att = at(S.att, o) + (int64_t)r * dim;
+        const float *e = at(S.e, o) + (int64_t)r * dim;
         for (int c = lane; c < dim; c += 32) {
-            const float a = __fdiv_rn(y[c], S.rowsum[((int64_t)r * dim + c) % B]);   // y.div(sum): row (r dim + c) % B's
+            const float a = __fdiv_rn(y[c], at(S.rowsum, o)[((int64_t)r * dim + c) % B]);   // y.div(sum): row (r dim + c) % B's
             y[c] = a;
             att[c] = __fmul_rn(a, e[c]);                                              // Mul(softmax, e)
         }
@@ -175,9 +196,9 @@ __global__ void __launch_bounds__(WARPS * 32) fm_fit_emb_enc_kernel(Slot S, int 
         float enc = 0.0f, v = 0.0f;
         if (lane < k) {
 #pragma unroll 8
-            for (int c = 0; c < dim; c++) enc = __fmaf_rn(att[c], S.EW[c * k + lane], enc);   // MatMul(., EW)
-            enc = __fadd_rn(enc, S.Eb[lane]);                                                // + Eb
-            S.enc[(int64_t)r * k + lane] = enc;
+            for (int c = 0; c < dim; c++) enc = __fmaf_rn(att[c], at(S.EW, o)[c * k + lane], enc);   // MatMul(., EW)
+            enc = __fadd_rn(enc, at(S.Eb, o)[lane]);                                                // + Eb
+            at(S.enc, o)[(int64_t)r * k + lane] = enc;
             v = vx[(int64_t)r * k + lane];
         }
         float dot = 0.0f;
@@ -186,10 +207,15 @@ __global__ void __launch_bounds__(WARPS * 32) fm_fit_emb_enc_kernel(Slot S, int 
     }
 }
 
-__global__ void __launch_bounds__(WARPS * 32) fm_fit_emb_datt_kernel(Slot S, int k, Batch T, const float *vx, const float *g)
+__global__ void __launch_bounds__(WARPS * 32) fm_fit_emb_datt_kernel(Group G, Slot S0, int k, Batch T, const float *vx, const float *g)
 {
+    Blk tb;
+    if (!trial_block(G, tb)) return;
+    const Slot S = slot_at(S0, tb.off);
+    vx = at(vx, tb.off);
+    g = at(g, tb.off);
     const int lane = threadIdx.x & 31, B = T.rows(), dim = S.dim;
-    for (int r = blockIdx.x * WARPS + (threadIdx.x >> 5); r < B; r += gridDim.x * WARPS) {
+    for (int r = tb.x * WARPS + (threadIdx.x >> 5); r < B; r += tb.nx * WARPS) {
         float *denc = S.denc + (int64_t)r * k, *gx = S.gx + (int64_t)r * dim;
         // Add(fmOutput, .): 0 + dp; BMM(vx, enc): denc = vx dp; Add(., Eb): a clone
         if (lane < k) denc[lane] = __fmaf_rn(vx[(int64_t)r * k + lane], __fadd_rn(0.0f, g[r]), 0.0f);
@@ -210,10 +236,13 @@ __global__ void __launch_bounds__(WARPS * 32) fm_fit_emb_datt_kernel(Slot S, int
     }
 }
 
-__global__ void __launch_bounds__(WARPS * 32) fm_fit_emb_dh_kernel(Slot S, int k, Batch T)
+__global__ void __launch_bounds__(WARPS * 32) fm_fit_emb_dh_kernel(Group G, Slot S0, int k, Batch T)
 {
+    Blk tb;
+    if (!trial_block(G, tb)) return;
+    const Slot S = slot_at(S0, tb.off);
     const int lane = threadIdx.x & 31, B = T.rows(), dim = S.dim;
-    for (int r = blockIdx.x * WARPS + (threadIdx.x >> 5); r < B; r += gridDim.x * WARPS) {
+    for (int r = tb.x * WARPS + (threadIdx.x >> 5); r < B; r += tb.nx * WARPS) {
         float *dz = S.gx + (int64_t)r * dim;
         const float *y = S.y + (int64_t)r * dim;
         // y.mul(sumdx) and gx.sub(y), sumdx indexed i % B: two roundings
@@ -231,10 +260,13 @@ __global__ void __launch_bounds__(WARPS * 32) fm_fit_emb_dh_kernel(Slot S, int k
 }
 
 // dx1 = x0^T dy of the three MatMuls and the two biases' gx1[i % k] += dy[i]: per element one chain over the batch rows
-__global__ void fm_fit_emb_wgrad_kernel(Slot S, int k, Batch T)
+__global__ void fm_fit_emb_wgrad_kernel(Group G, Slot S0, int k, Batch T)
 {
+    Blk tb;
+    if (!trial_block(G, tb)) return;
+    const Slot S = slot_at(S0, tb.off);
     const int B = T.rows(), dim = S.dim, dk = dim * k;
-    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < 2 * dk + 2 * k; i += gridDim.x * blockDim.x) {
+    for (int i = tb.x * blockDim.x + threadIdx.x; i < 2 * dk + 2 * k; i += tb.nx * blockDim.x) {
         if (i < dk) {                     // dEW = att^T denc and dAW = e^T dh, element (c, f)
             const int c = i / k, f = i % k;
             float ew = 0.0f, aw = 0.0f;
@@ -263,10 +295,15 @@ __global__ void fm_fit_emb_wgrad_kernel(Slot S, int k, Batch T)
 }
 
 // the forward of the slot-free part on a batch, kept for the slots: the rows' logits and vx
-__global__ void __launch_bounds__(WARPS * 32) fm_fit_emb_base_kernel(const float *P, int64_t nf, int k, Rows R, Batch T, float *p, float *vx)
+__global__ void __launch_bounds__(WARPS * 32) fm_fit_emb_base_kernel(Group G, const float *P, int64_t nf, int k, Rows R, Batch T, float *p, float *vx)
 {
+    Blk tb;
+    if (!trial_block(G, tb)) return;
+    P = at(P, tb.off);
+    p = at(p, tb.off);
+    vx = at(vx, tb.off);
     const int lane = threadIdx.x & 31, B = T.rows();
-    for (int b = blockIdx.x * WARPS + (threadIdx.x >> 5); b < B; b += gridDim.x * WARPS) {
+    for (int b = tb.x * WARPS + (threadIdx.x >> 5); b < B; b += tb.nx * WARPS) {
         float v;
         const float pb = row_forward(P, nf, k, R, T.r0() + b, lane, v);
         if (lane == 0) p[b] = pb;

@@ -690,6 +690,46 @@ int32_t gorse_b200_fm_fit_emb(gorse_b200_ctx *ctx, int64_t n_features, int32_t n
                               const uint8_t *item_emb_mask, const float *params_in, int64_t n_params, float *params_out,
                               float *moments_out, gorse_b200_progress_fn progress, void *user, gorse_b200_fm_fit_result *result);
 
+/* FM model search: the trials of AFM's ModelSearch (model/ctr/fm.go SuggestParams), which
+ * optimizeClickThroughRatePrediction (master/tasks.go:1318-1363) runs on every dataset load when the ranker's
+ * optimize_period > 0, fitted in one call.  gorse_b200_fm_fit_emb's arguments (n_emb = 0: the model without slots), with
+ * per trial k: trials[k], params_in[k] (fm.Parameters() after the trial's own Init), params_out[k] and moments_out[k]
+ * (each array and each entry may be NULL) and results[k].
+ *   What each result equals: results[k], params_out[k] and moments_out[k] are bit-identical to what
+ *   gorse_b200_fm_fit_emb returns for trials[k] and params_in[k] alone (with n_emb = 0 that is also gorse_b200_fm_fit),
+ *   NaN payloads aside as there: every score, cost, epochs_run, best_epoch, the flags and steps.
+ *   What the trials share: n_factors, batch_size, verbose, patience and max_steps must be equal in every trial (else
+ *   GORSE_B200_ERR_ARG); lr, reg, optimizer and n_epochs may differ.  n_params is one value for all trials.
+ *   Leaving the batch: a trial leaves when it has run its n_epochs, stops early or diverges; its tables are not touched
+ *   after that.
+ *   progress (may be NULL) gets every trial's state after the epoch-0 evaluation and after every epoch of the batch (not
+ *   after an epoch cut short by max_steps, as the solo fit); auc is -1 for a trial not evaluated in that epoch.  A non-zero
+ *   return cancels: each unfinished trial then gets exactly what a solo fit cancelled at that epoch gets (cancelled = 1, a
+ *   zero score, params_out holding that epoch's updates); finished trials keep their results.  The callback is not
+ *   called again.
+ *   Groups: the trials run in groups of at most 16, one CUDA graph per epoch of a group, fewer when their tables do not
+ *   fit the free device memory (DESIGN §8.8 has the bytes per trial); the groups run one after another, a later group's
+ *   trials reporting {0, -1, 0} until it starts.  A cancel also cancels the trials of the later groups at their epoch 0.
+ *   The trial tables are allocated in the call and freed before it returns.
+ * Every argument is checked on the host before the device is touched, ctx last; n_factors above 32, more than 8 slots or a
+ * dim above 1024 are GORSE_B200_ERR_UNSUPPORTED. */
+typedef struct {
+    int32_t epochs_run;  /* epochs the trial has run so far */
+    float auc;           /* AUC of this epoch's evaluation, -1 when the trial was not evaluated in this epoch */
+    int32_t finished;    /* 1 once the trial has run its n_epochs, stopped early or diverged */
+} gorse_b200_fm_trial_state;
+typedef int32_t (*gorse_b200_fm_trials_progress_fn)(void *user, int32_t epoch, int32_t n_trials, const gorse_b200_fm_trial_state *states);
+
+int32_t gorse_b200_fm_fit_trials(gorse_b200_ctx *ctx, int64_t n_features, int32_t num_dimension, int32_t n_trials,
+                                 const gorse_b200_fm_fit_params *trials, int64_t n_train, const int64_t *train_off,
+                                 const int32_t *train_idx, const float *train_val, const float *train_target,
+                                 const int32_t *train_emb_row, int64_t n_test, const int64_t *test_off, const int32_t *test_idx,
+                                 const float *test_val, const float *test_target, const int32_t *test_emb_row, int32_t n_emb,
+                                 const int32_t *emb_dim, int64_t n_emb_rows, const uint16_t *const *item_emb,
+                                 const uint8_t *item_emb_mask, const float *const *params_in, int64_t n_params,
+                                 float *const *params_out, float *const *moments_out, gorse_b200_fm_trials_progress_fn progress,
+                                 void *user, gorse_b200_fm_fit_result *results);
+
 /* ------------------------------------------------------------------------------------------
  * NCF-format datasets: dataset.LoadDataFromBuiltIn (dataset/dataset.go:398-490), the loader `gorse-bench cf`
  * (gorse_b200/csrc/gorse_bench_cf.cpp; BASELINE configs[0]) feeds the model with.  Host code.
