@@ -934,6 +934,31 @@ def load_ncf(train_path, test_path=None):
     return U.value, I.value, (offs[0], idx[0]), (offs[1], idx[1]), (offs[2], idx[2])
 
 
+def evaluate_embeddings(ctx, emb, mask, shots, test, excl, negatives=None, n_candidates=99, seed=0, topk=10):
+    """`gorse-bench embedding`'s scoring (gorse_b200_embedding_eval) for every user at once.  emb [n_items, dim] float32, mask
+    [n_items] (None: every item has an embedding); shots, test, excl and negatives are (off, items) CSRs over the users; with
+    negatives None they are sampled on the device under seed, excluding test(u) and excl(u).
+    -> (ndcg, precision, recall, users scored)"""
+    emb = np.ascontiguousarray(emb, np.float32)
+    if emb.ndim != 2:
+        raise ValueError("emb must be [n_items, dim]")
+    mask = None if mask is None else np.ascontiguousarray(mask, np.uint8)
+    if mask is not None and mask.shape != (emb.shape[0],):
+        raise ValueError("mask must be [n_items]")
+
+    def csr(pair):
+        if pair is None:
+            return None, None
+        off = np.ascontiguousarray(pair[0], np.int64)
+        return off, np.ascontiguousarray(pair[1], np.int32)
+
+    (so, si), (to, ti), (xo, xi), (no, ni) = csr(shots), csr(test), csr(excl), csr(negatives)
+    out, users = np.zeros(3, np.float32), C.c_int64(0)
+    check(lib.gorse_b200_embedding_eval(ctx.h, emb.shape[0], emb.shape[1], ptr(emb), ptr(mask), len(so) - 1, ptr(so), ptr(si), ptr(to), ptr(ti),
+                                        ptr(xo), ptr(xi), ptr(no), ptr(ni), int(n_candidates), int(seed), int(topk), ptr(out), C.byref(users)))
+    return np.float32(out[0]), np.float32(out[1]), np.float32(out[2]), users.value
+
+
 # ---- logics: similarity vectors and scores (host functions; SURVEY 8a row J) ---------------------------------
 def bf16_truncate(a):
     """bfloats.FromFloat32 + ToFloat32 (common/bfloats/bfloats.go:23-37): how the reference stores dense embeddings."""

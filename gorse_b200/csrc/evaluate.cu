@@ -5,11 +5,10 @@
 #include <cmath>
 
 #include "cf.cuh"
+#include "evaluate.cuh"
 #include "tables.cuh"
 
 namespace gb {
-
-#define GB_EVAL_MAX_TOPK 128
 
 __global__ void eval_score_kernel(const float *P, const float *Q, int d, int32_t u_lo, const int32_t *cand_user,
                                   const int32_t *cand_item, int64_t n, float *score)
@@ -194,6 +193,27 @@ __global__ void eval_candidates_kernel(const int64_t *test_off, const int32_t *t
     for (int64_t a = neg_off[u]; a < neg_off[u + 1]; a++, p++) { cand_user[p] = u_lo + u; cand_item[p] = neg_items[a]; }
 }
 
+void eval_inv_log2(int32_t topk, float *out)
+{
+    for (int i = 0; i < topk; i++) out[i] = 1.0f / log2_math32((float)i + 2.0f);
+}
+
+void launch_eval_rank(cudaStream_t s, const int64_t *cand_off, const int32_t *cand_item, const float *score, const int64_t *test_off,
+                      const int32_t *test_items, int32_t n_users, int32_t topk, const float *inv_log2, float *metrics)
+{
+    if (n_users > 0)
+        eval_rank_kernel<<<(n_users + 127) / 128, 128, 0, s>>>(cand_off, cand_item, score, test_off, test_items, n_users, topk, inv_log2, metrics);
+}
+
+void launch_eval_negatives(cudaStream_t s, const int64_t *excl_off, const int32_t *excl_items, const int64_t *test_off,
+                           const int32_t *test_items, int32_t n_users, int32_t u_lo, int32_t n_items, int32_t n_cand, uint64_t base,
+                           bool count_only, int32_t *n_neg, const int64_t *neg_off, int32_t *neg_items)
+{
+    if (n_users > 0)
+        eval_negatives_kernel<<<(n_users + 127) / 128, 128, 0, s>>>(excl_off, excl_items, test_off, test_items, n_users, u_lo, n_items,
+                                                                     n_cand, base, count_only, n_neg, neg_off, neg_items);
+}
+
 }  // namespace gb
 
 using namespace gb;
@@ -332,7 +352,7 @@ int32_t gorse_b200_eval_create(gorse_b200_cf *cf, const int64_t *test_off, const
         // sample on the device against the training rows that already live there
         DevBuf<int32_t> cnt;
         if ((st = cnt.alloc((size_t)U))) return fail(st);
-        const uint64_t base = mix64(seed ^ 0xbb67ae8584caa73bull);
+        const uint64_t base = eval_negatives_base(seed);
         eval_negatives_kernel<<<ub, 128, 0, s>>>(cf->user_off.p, cf->user_items.p, ev->test_off.p, ev->test_items.p, U, cf->u_lo, cf->n_items,
                                                  n_candidates, base, true, cnt.p, nullptr, nullptr);
         c->launches++;

@@ -731,6 +731,40 @@ int32_t gorse_b200_fm_fit_trials(gorse_b200_ctx *ctx, int64_t n_features, int32_
                                  void *user, gorse_b200_fm_fit_result *results);
 
 /* ------------------------------------------------------------------------------------------
+ * Embedding evaluation: `gorse-bench embedding`'s scoring (EvaluateEmbedding, cmd/gorse-bench/main.go:322-467) for every test
+ * user in one call -- how an operator picks the embedding behind an "embedding" item-to-item recommender.
+ *   emb[n_items x dim] fp32 as the column expression returns it (no bf16 truncation); emb_mask[n_items] 1 where the item has
+ *   an embedding (NULL: every item has one).  dim outside [1, 16384]: GORSE_B200_ERR_ARG.  A non-finite value in a present
+ *   row is GORSE_B200_ERR_ARG (the reference would push NaN into its heap); it is found on the device before anything is scored.
+ *   Per user u, as CSRs over [n_users] (offsets non-decreasing, need not start at 0; the items pointer points at the entry
+ *   off[0] refers to; every id in [0, n_items)):
+ *     shot_off / shot_items   the train side of dataset.SplitLatest(shots): newest first, the order the totals are formed in;
+ *     test_off / test_items   the test side (the newest item);
+ *     excl_off / excl_items   the user's whole dataset feedback, what the cached negatives exclude (SampleUserNegatives called
+ *                             on the full dataset, main.go:517-518); read only when neg_off is NULL;
+ *     neg_off / neg_items     the negatives; NULL: n_candidates distinct items outside test(u) and excl(u) are sampled on the
+ *                             device under `seed`, or all remaining items ascending when fewer are left, exactly as
+ *                             gorse_b200_eval_create samples them (the Go math/rand stream is not reproducible, SURVEY F9).
+ *   Per user (main.go:410-456): skipped without a test item or a shot; candidates = test(u) then negatives(u), a candidate
+ *   without an embedding skipped; total = 0, then total -= floats.Euclidean(candidate, shot) in fp32 for every shot with an
+ *   embedding, in shot order; a candidate enters TopKFilter(topk) only when some shot had an embedding; a user whose filter
+ *   stays empty is skipped; else NDCG, Precision and Recall of the ranked list against the set of test items.  Every distance
+ *   is bit for bit the reference's AVX-512 Euclidean and every total its sequential sum.
+ *   out[3] = {NDCG, Precision, Recall}: the per-user values summed in fp32 in user order (the reference with jobs = 1; with
+ *   more jobs its summation order is unpinned), each divided by the number of scored users; all zero when no user is scored.
+ *   *users_out (may be NULL) = that number.
+ *   Bounds: topk in [1, 128] (GORSE_B200_ERR_ARG).  A user's distances are held at once: (|test(u)| + its negatives, or
+ *   n_candidates when sampling) x (its shots with an embedding) above 2^28 is GORSE_B200_ERR_UNSUPPORTED.  Users run in
+ *   chunks of at most 2^26 distances (or one user's); the answer does not depend on the chunking.
+ *   Every argument is checked on the host before the device is touched, ctx last.  Thread-safe per context: the call keeps
+ *   no state and frees its device buffers before it returns. */
+int32_t gorse_b200_embedding_eval(gorse_b200_ctx *ctx, int32_t n_items, int32_t dim, const float *emb, const uint8_t *emb_mask,
+                                  int64_t n_users, const int64_t *shot_off, const int32_t *shot_items, const int64_t *test_off,
+                                  const int32_t *test_items, const int64_t *excl_off, const int32_t *excl_items,
+                                  const int64_t *neg_off, const int32_t *neg_items, int32_t n_candidates, uint64_t seed,
+                                  int32_t topk, float *out, int64_t *users_out);
+
+/* ------------------------------------------------------------------------------------------
  * NCF-format datasets: dataset.LoadDataFromBuiltIn (dataset/dataset.go:398-490), the loader `gorse-bench cf`
  * (gorse_b200/csrc/gorse_bench_cf.cpp; BASELINE configs[0]) feeds the model with.  Host code.
  *   train file  "user<TAB>item[<TAB>...]" per line (loadTrain :420-453)
