@@ -75,6 +75,8 @@ def lib():
         L.fmf_fit_emb.restype = C.c_int32
         L.fmf_fit_emb.argtypes = [C.c_int64, C.c_int32, VP, VP, C.c_int64, C.c_int64, VP, VP, VP, VP, C.c_int64, VP, VP, VP, VP, C.c_int32, VP, VP,
                                   VP, VP, VP, VP, VP, VP, VP, VP]
+        L.fmo_gauc.restype = C.c_int64
+        L.fmo_gauc.argtypes = [C.c_int64, VP, VP, VP, C.c_int64, VP, C.c_int64, VP, VP, VP, VP]
         _lib = L
     return _lib
 
@@ -328,6 +330,19 @@ def evaluate(n_features, k, num_dimension, params, test):
     out = np.zeros(4, np.float32)
     lib().fmf_evaluate(int(n_features), int(k), int(num_dimension), _p(_c(params, np.float32)), n, _p(off), _p(idx), _p(val), _p(tgt), _p(out))
     return out
+
+
+def gauc(pred, users, target, n_users, feedback, context_size=100):
+    """EvaluateAFM's per-user AUC and GAUC (cmd/gorse-bench/main.go:133-206) on the predictions of the whole test list:
+    users[i] = the user of test row i, feedback[u] = the user's positive training rows; users in ascending order.
+    -> (gauc float64, users int32, candidates int64, auc float32), one entry per scored user"""
+    pred, users, target = _c(np.append(pred, 0), np.float32), _c(np.append(users, 0), np.int32), _c(np.append(target, 0), np.float32)
+    fb = _c(np.append(feedback, 0), np.int64)
+    n = pred.size - 1
+    uo, co, ao = np.zeros(n_users + 1, np.int32), np.zeros(n_users + 1, np.int64), np.zeros(n_users + 1, np.float32)
+    g = C.c_double(0)
+    ns = lib().fmo_gauc(n, _p(pred), _p(users), _p(target), int(n_users), _p(fb), int(context_size), _p(uo), _p(co), _p(ao), C.byref(g))
+    return g.value, uo[:ns], co[:ns], ao[:ns]
 
 
 class Embeddings:

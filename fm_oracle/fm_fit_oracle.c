@@ -847,3 +847,56 @@ int32_t fmf_fit_emb(int64_t nf, int32_t num_dim, const int32_t *ip, const float 
     return fit(nf, num_dim, ip, fp, max_steps, n_train, tr_off, tr_idx, tr_val, tr_tgt, n_test, te_off, te_idx, te_val, te_tgt, &E, params_in,
                params_out, moments_out, res_f, res_i);
 }
+
+/* ---- GAUC ---------------------------------------------------------------------------------------------------------- */
+/* EvaluateAFM's scoring after the fit (cmd/gorse-bench/main.go:133-206), literally, on the predictions of the whole test
+ * list in test order (fmo_batch_predict): user[i] = indices[0] of test row i, tgt[i] its target, feedback[u] the user's
+ * positive training rows.  The users are visited in ascending order (the reference's map order is unpinned); a user with a
+ * NaN prediction gets AUC = NaN (Go's sort order on NaN is unpinned).  Per scored user j: user_out[j], cand_out[j] = P + N,
+ * auc_out[j] (each sized n_users); returns the number of users scored, *gauc the GAUC. */
+int64_t fmo_gauc(int64_t n, const float *pred, const int32_t *user, const float *tgt, int64_t n_users, const int64_t *feedback,
+                 int64_t context_size, int32_t *user_out, int64_t *cand_out, float *auc_out, double *gauc)
+{
+    int64_t *po = calloc((size_t)n_users + 1, sizeof(int64_t)), *no = calloc((size_t)n_users + 1, sizeof(int64_t));
+    for (int64_t i = 0; i < n; i++) (tgt[i] > 0 ? po : no)[user[i] + 1]++;
+    for (int64_t u = 0; u < n_users; u++) { po[u + 1] += po[u]; no[u + 1] += no[u]; }
+    float *pos = malloc(sizeof(float) * (size_t)(po[n_users] + 1)), *neg = malloc(sizeof(float) * (size_t)(no[n_users] + 1));
+    int64_t *pf = calloc((size_t)n_users + 1, sizeof(int64_t)), *nf = calloc((size_t)n_users + 1, sizeof(int64_t));
+    for (int64_t i = 0; i < n; i++) {   /* positives[u] and negatives[u] in test order */
+        const int32_t u = user[i];
+        if (tgt[i] > 0) pos[po[u] + pf[u]++] = pred[i];
+        else neg[no[u] + nf[u]++] = pred[i];
+    }
+    float sum = 0, count = 0;
+    int64_t ns = 0;
+    for (int64_t u = 0; u < n_users; u++) {
+        const int64_t P = po[u + 1] - po[u], N = no[u + 1] - no[u];
+        if (P == 0 || N == 0 || feedback[u] == 0 || feedback[u] > context_size) continue;
+        float *pp = pos + po[u], *nn = neg + no[u];
+        int nan = 0;
+        for (int64_t i = 0; i < P; i++) nan |= isnan(pp[i]);
+        for (int64_t i = 0; i < N; i++) nan |= isnan(nn[i]);
+        float auc = NAN;
+        if (!nan) {   /* ctr.AUC (evaluator.go:136-153) */
+            qsort(pp, (size_t)P, sizeof(float), cmp_f32);
+            qsort(nn, (size_t)N, sizeof(float), cmp_f32);
+            float s = 0;
+            int64_t j = 0;
+            for (int64_t i = 0; i < P; i++) {
+                while (j < N && nn[j] < pp[i]) j++;
+                s += (float)j;
+            }
+            auc = s / (float)(P * N);
+        }
+        user_out[ns] = (int32_t)u;
+        cand_out[ns] = P + N;
+        auc_out[ns] = auc;
+        ns++;
+        const float cnt = (float)(P + N);
+        sum += auc * cnt;
+        count += cnt;
+    }
+    *gauc = count > 0 ? (double)(sum / count) : 0.0;
+    free(po); free(no); free(pos); free(neg); free(pf); free(nf);
+    return ns;
+}

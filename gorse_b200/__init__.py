@@ -917,6 +917,46 @@ class FMTrainer:
         return dims, tabs, mask, er
 
 
+def user_feedback_counts(train, n_users):
+    """feedbackCount of `gorse-bench reranker` (cmd/gorse-bench/main.go:133-140): per user, the training rows with target > 0
+    whose first index is the user.  train = (off, idx, val, target) -> int64 [n_users]"""
+    off, idx, _, tgt = train
+    off = np.asarray(off, np.int64)
+    first = np.asarray(idx, np.int64)[off[:-1][np.diff(off) > 0]]
+    pos = np.asarray(tgt, np.float32)[np.diff(off) > 0] > 0
+    return np.bincount(first[pos], minlength=n_users).astype(np.int64)
+
+
+def ranker_gauc(ctx, n_features, n_factors, num_dimension, params, test, n_users, feedback_count, context_size=100, batch_size=1024,
+                emb=None, predictions=False):
+    """The AFM half of `gorse-bench reranker` after the fit (gorse_b200_fm_gauc): every test row predicted as one list in test
+    order, then per user (the first index of its rows) the AUC of its positives against its negatives, and GAUC.
+    params: fm.Parameters() as FMRanker takes them; test = (off, idx, val, target) with values through fm.Scalers;
+    feedback_count [n_users] (user_feedback_counts); emb: None, or (emb_dims, item_emb, item_emb_mask, test_emb_row) as
+    FMTrainer.fit_emb takes them.
+    -> dict: gauc (float), users, feedback, candidates, auc (one entry per scored user, ascending user), stats {rows,
+    users, scored, chained, nan} and predictions (float32 [n_test] when asked for, else None)"""
+    n, off, idx, val, tgt = FMTrainer._rows(test)
+    p = np.ascontiguousarray(params, np.float32).reshape(-1)
+    dims, tabs, mask, er = FMTrainer._emb(None if emb is None else (emb[0], emb[1], emb[2], np.zeros(0, np.int32), emb[3]), (0,), (n,))
+    fb = np.ascontiguousarray(feedback_count, np.int64).reshape(-1)
+    if fb.size != n_users:
+        raise ValueError("one feedback count per user")
+    m = max(int(n_users), 1)
+    users, feedback, cand, auc = np.zeros(m, np.int32), np.zeros(m, np.int64), np.zeros(m, np.int64), np.zeros(m, np.float32)
+    pred = np.zeros(max(n, 1), np.float32) if predictions else None
+    stats, ns, g = np.zeros(5, np.int64), C.c_int64(0), C.c_double(0)
+    arr = (C.c_void_p * max(len(tabs), 1))(*[ptr(t) for t in tabs])
+    check(lib.gorse_b200_fm_gauc(ctx.h, int(n_features), int(n_factors), int(num_dimension), int(batch_size), dims.size, ptr(dims), ptr(p), p.size,
+                                 n, ptr(off), ptr(idx), ptr(val), ptr(tgt), ptr(er[1]), tabs[0].shape[0] if tabs else 0, arr if tabs else None,
+                                 ptr(mask), int(n_users), ptr(fb), int(context_size), ptr(pred), ptr(users), ptr(feedback), ptr(cand), ptr(auc),
+                                 C.byref(ns), C.byref(g), ptr(stats)))
+    k = ns.value
+    return dict(gauc=g.value, users=users[:k], feedback=feedback[:k], candidates=cand[:k], auc=auc[:k],
+                stats=dict(zip(("rows", "users", "scored", "chained", "nan"), (int(x) for x in stats))),
+                predictions=None if pred is None else pred[:n])
+
+
 def load_ncf(train_path, test_path=None):
     """dataset.LoadDataFromBuiltIn's NCF parsers (dataset/dataset.go:398-490) ->
     (n_users, n_items, (train_off, train_items), (test_off, test_items), (neg_off, neg_items))."""

@@ -112,7 +112,10 @@ PROTOTYPES = {
                                           VP, C.c_int64, VP, VP, VP, C.c_int64, VP, VP, VP, VP, VP]),
     "gorse_b200_fm_fit_trials": (C.c_int32, [VP, C.c_int64, C.c_int32, C.c_int32, VP, C.c_int64, VP, VP, VP, VP, VP, C.c_int64, VP, VP, VP, VP, VP,
                                              C.c_int32, VP, C.c_int64, VP, VP, VP, C.c_int64, VP, VP, VP, VP, VP]),
-    "gorse_b200_embedding_eval": (C.c_int32, [VP, C.c_int32, C.c_int32, VP, VP, C.c_int64, VP, VP, VP, VP, VP, VP, VP, VP, C.c_int32, C.c_uint64,
+    "gorse_b200_fm_gauc": (C.c_int32, [VP, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_int32, VP, VP, C.c_int64, C.c_int64, VP, VP, VP, VP,
+                                       VP, C.c_int64, VP, VP, C.c_int64, VP, C.c_int64, VP, VP, VP, VP, VP, C.POINTER(C.c_int64),
+                                       C.POINTER(C.c_double), VP]),
+    "gorse_b200_embedding_eval":(C.c_int32, [VP, C.c_int32, C.c_int32, VP, VP, C.c_int64, VP, VP, VP, VP, VP, VP, VP, VP, C.c_int32, C.c_uint64,
                                               C.c_int32, VP, C.POINTER(C.c_int64)]),
     "gorse_b200_ncf_load":(C.c_int32, [C.c_char_p, C.c_char_p, PVP]),
     "gorse_b200_ncf_shape": (C.c_int32, [VP, C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.POINTER(C.c_int64), C.POINTER(C.c_int64),

@@ -23,6 +23,8 @@
 // The arithmetic is fp32 with explicit __fmaf_rn / __fmul_rn / __fadd_rn / __fsub_rn / __fdiv_rn / __fsqrt_rn.
 // gorse_b200_fm_fit_trials fits several trials in lockstep through the same kernels: each kernel takes a Group and block b
 // runs trial b % n on that trial's tables (DESIGN §8.8); a solo fit is one trial.
+// gorse_b200_fm_gauc predicts every test row as one list through Fit::predict, the evaluation's forward, and scores each
+// user's rows with the kernels of fm_gauc.cuh (DESIGN §8.10).
 #include <cub/cub.cuh>
 
 #include <algorithm>
@@ -394,6 +396,7 @@ __global__ void fm_fit_emb_opt_kernel(Group G, float *P, float *M, float *Vm, in
 }
 
 #include "fm_fit_emb.cuh"
+#include "fm_gauc.cuh"
 
 __global__ void fm_fit_set_kernel(int64_t *dst, int64_t v) { *dst = v; }
 
@@ -611,6 +614,7 @@ struct Fit {
     int k;
     int32_t num_dimension;
     const gorse_b200_fm_fit_params *prm;   // trial 0's: its shared fields are every trial's
+    bool train = true;                     // false: predictions only (gorse_b200_fm_gauc), no optimiser tables
     int64_t n_params = 0, max_total = 0;   // max_total: the most optimiser steps of any trial
     // training set, shared by the trials (so is the stamp: they step in lockstep)
     Buf<int32_t> tr_idx, tr_len, seg_start, seg_feat, seg_pos, stamp;
@@ -648,6 +652,8 @@ struct Fit {
     Opts opts{};
 
     int32_t upload_train(const int64_t *off, const int32_t *idx, const float *val, const float *tgt);
+    int32_t upload_list(TestSet &T, const int64_t *off, const int32_t *idx, const float *val, const std::vector<int64_t> &rows_,
+                        const int32_t *emb_row);
     int32_t upload_test(const int64_t *off, const int32_t *idx, const float *val, const float *tgt, int64_t n, const int32_t *emb_row);
     int32_t upload_slots();
     size_t carve(uintptr_t b);
@@ -655,6 +661,7 @@ struct Fit {
     unsigned grid(int64_t blocks) const { return (unsigned)(std::min<int64_t>(blocks, INT32_MAX / G) * G); }
     int32_t slots_forward(Group Gr, const int32_t *emb_row, Batch T, float *logit);
     int32_t run_steps(int s0, int s1);
+    int32_t predict(Group Ev, TestSet &T);
     int32_t evaluate(const bool *which, float (*score)[4]);
 };
 
@@ -730,26 +737,33 @@ int32_t Fit::upload_train(const int64_t *off, const int32_t *idx, const float *v
     return GORSE_B200_OK;
 }
 
+// rows [rows] of a CSR as one prediction list, padded to its own longest row
+int32_t Fit::upload_list(TestSet &T, const int64_t *off, const int32_t *idx, const float *val, const std::vector<int64_t> &rows_,
+                         const int32_t *emb_row)
+{
+    T.n = (int64_t)rows_.size();
+    GB_TRY(longest(off, rows_, num_dimension, &T.D));
+    std::vector<int32_t> pi;
+    std::vector<float> pv;
+    pad_rows(off, idx, val, rows_, T.D, pi, pv);
+    GB_TRY(T.idx.put(pi, st));
+    GB_TRY(T.val.put(pv, st));
+    if (emb_row) {
+        std::vector<int32_t> er(rows_.size());
+        for (size_t i = 0; i < er.size(); i++) er[i] = emb_row[rows_[i]];
+        GB_TRY(T.emb_row.put(er, st));
+    }
+    return GORSE_B200_OK;
+}
+
 int32_t Fit::upload_test(const int64_t *off, const int32_t *idx, const float *val, const float *tgt, int64_t n, const int32_t *emb_row)
 {
     std::vector<int64_t> rows_[2];
     for (int64_t r = 0; r < n; r++) rows_[tgt[r] > 0 ? 0 : 1].push_back(r);
     int64_t most = 0;
     for (int s = 0; s < 2; s++) {
-        TestSet &T = te[s];
-        T.n = (int64_t)rows_[s].size();
-        GB_TRY(longest(off, rows_[s], num_dimension, &T.D));   // each list is padded to its own longest row
-        std::vector<int32_t> pi;
-        std::vector<float> pv;
-        pad_rows(off, idx, val, rows_[s], T.D, pi, pv);
-        GB_TRY(T.idx.put(pi, st));
-        GB_TRY(T.val.put(pv, st));
-        if (emb_row) {
-            std::vector<int32_t> er(rows_[s].size());
-            for (size_t i = 0; i < er.size(); i++) er[i] = emb_row[rows_[s][i]];
-            GB_TRY(T.emb_row.put(er, st));
-        }
-        most = std::max(most, T.n);
+        GB_TRY(upload_list(te[s], off, idx, val, rows_[s], emb_row));
+        most = std::max(most, te[s].n);
     }
     GB_TRY(counts.alloc(3 * MAX_TRIALS));
     GB_TRY(auc_sum.alloc(MAX_TRIALS));
@@ -782,11 +796,12 @@ int32_t Fit::upload_slots()
 size_t Fit::carve(uintptr_t b)
 {
     Carver c{b};
+    const int64_t opt = train ? n_params : 0;   // predictions only: no moments and no gradients
     c.take(P, n_params);
-    c.take(M, n_params);
-    c.take(Vm, n_params);
-    c.take(gV, nf * k);
-    c.take(gW, nf);
+    c.take(M, opt);
+    c.take(Vm, opt);
+    c.take(gV, train ? nf * k : 0);
+    c.take(gW, train ? nf : 0);
     c.take(gB, 1);
     c.take(g, rows);
     c.take(dss, rows);
@@ -801,7 +816,7 @@ size_t Fit::carve(uintptr_t b)
     }
     c.take(below, te[0].n);
     if (n_emb > 0) {
-        c.take(gS, tens.end[tens.n - 1]);
+        c.take(gS, train ? tens.end[tens.n - 1] : 0);
         for (float **q : {&zmax, &rowsum, &sumdx, &p}) c.take(*q, slot_rows);
         for (float **q : {&denc, &dh, &vx}) c.take(*q, slot_rows * k);
         c.take(gx, slot_rows * maxdim);
@@ -822,7 +837,7 @@ int32_t Fit::alloc_group(int g)
     GB_TRY(arena.alloc((size_t)stride * g));
     carve((uintptr_t)arena.p);
     GB_CUDA(cudaMemsetAsync(arena.p, 0, arena.n, st));
-    GB_CUDA(cudaMemsetAsync(stamp.p, 0, (size_t)nf * sizeof(int32_t), st));   // steps count from 1
+    if (train) GB_CUDA(cudaMemsetAsync(stamp.p, 0, (size_t)nf * sizeof(int32_t), st));   // steps count from 1
     if (n_emb == 0) return GORSE_B200_OK;
     int64_t o = base;
     logits = SlotLogits{p, vx, {}, n_emb, {}};
@@ -836,6 +851,27 @@ int32_t Fit::alloc_group(int g)
                        zmax, rowsum, gx, denc, dh, sumdx};
         logits.enc[s] = s_enc[s];
         o += 3 * kd + 2 * k;
+    }
+    return GORSE_B200_OK;
+}
+
+// BatchInternalPredict (fm.go:156-178) of the list T into T.pred for the trials of Ev
+int32_t Fit::predict(Group Ev, TestSet &T)
+{
+    if (T.n == 0) return GORSE_B200_OK;
+    if (n_emb == 0) {
+        fm_fit_predict_kernel<<<grid(std::min<int64_t>(div_up(T.n, WARPS), (int64_t)ctx->sm_count * 16)), WARPS * 32, 0, st>>>(
+            Ev, P, nf, k, Rows{T.idx.p, T.val.p, T.D}, T.n, T.pred);
+        GB_LAUNCHED(ctx);
+        return GORSE_B200_OK;
+    }
+    // chunks of batch_size rows, each with its own softmax coupling
+    const int64_t bs = prm->batch_size;
+    for (int64_t ch = 0; ch * bs < T.n; ch++) {
+        const Batch C{bs, T.n, (int)ch};
+        fm_fit_emb_base_kernel<<<grid(row_grid), WARPS * 32, 0, st>>>(Ev, P, nf, k, Rows{T.idx.p, T.val.p, T.D}, C, T.pred + ch * bs, vx);
+        GB_LAUNCHED(ctx);
+        GB_TRY(slots_forward(Ev, T.emb_row.p, C, T.pred + ch * bs));
     }
     return GORSE_B200_OK;
 }
@@ -857,19 +893,7 @@ int32_t Fit::evaluate(const bool *which, float (*score)[4])
     for (int s = 0; s < 2; s++) {
         TestSet &T = te[s];
         if (T.n == 0) continue;
-        if (n_emb == 0) {
-            fm_fit_predict_kernel<<<grid(std::min<int64_t>(div_up(T.n, WARPS), (int64_t)ctx->sm_count * 16)), WARPS * 32, 0, st>>>(
-                Ev, P, nf, k, Rows{T.idx.p, T.val.p, T.D}, T.n, T.pred);
-            GB_LAUNCHED(ctx);
-        } else {   // BatchInternalPredict's chunks of batch_size rows, each with its own softmax coupling
-            const int64_t bs = prm->batch_size;
-            for (int64_t ch = 0; ch * bs < T.n; ch++) {
-                const Batch C{bs, T.n, (int)ch};
-                fm_fit_emb_base_kernel<<<grid(row_grid), WARPS * 32, 0, st>>>(Ev, P, nf, k, Rows{T.idx.p, T.val.p, T.D}, C, T.pred + ch * bs, vx);
-                GB_LAUNCHED(ctx);
-                GB_TRY(slots_forward(Ev, T.emb_row.p, C, T.pred + ch * bs));
-            }
-        }
+        GB_TRY(predict(Ev, T));
         for (int i = 0; i < G; i++) {
             if (!which[i]) continue;
             size_t bytes = cub_tmp.n;
@@ -1294,6 +1318,124 @@ int32_t fit_run(gorse_b200_ctx *ctx, const Data &d, const gorse_b200_fm_fit_para
     Progress pg{progress ? solo_progress : nullptr, &sp, d.n_train > 0, {}};
     return fit_groups(ctx, d, 1, params, &params_in, &params_out, &moments_out, pg, result);
 }
+
+struct GaucOut {                  // gorse_b200_fm_gauc's outputs; any may be NULL but n_scored and gauc
+    float *pred;
+    int32_t *user;
+    int64_t *feedback, *cand;
+    float *auc;
+    int64_t *n_scored;
+    double *gauc;
+    int64_t *stats;
+};
+
+// EvaluateAFM's scoring after the fit (cmd/gorse-bench/main.go:133-206) on checked arguments: the predictions of every test
+// row as one list in test order, then per user the AUC of its positives against its negatives, and GAUC
+int32_t gauc_run(gorse_b200_ctx *ctx, const Data &d, const gorse_b200_fm_fit_params *prm, const float *params, int64_t n_users,
+                 const int64_t *feedback, int64_t context_size, const GaucOut &o)
+{
+    const int64_t n = d.n_test;
+    // per user: P and N, its first key in the sorted list, and whether main.go:184 scores it
+    std::vector<int32_t> P((size_t)n_users, 0), N((size_t)n_users, 0);
+    std::vector<uint32_t> row_hi((size_t)n);
+    for (int64_t r = 0; r < n; r++) {
+        const int32_t u = d.test_idx[d.test_off[r]];
+        const bool neg = !(d.test_target[r] > 0);
+        (neg ? N : P)[(size_t)u]++;
+        row_hi[(size_t)r] = (uint32_t)u << 1 | (uint32_t)neg;
+    }
+    std::vector<GaucUser> scored;
+    std::vector<int32_t> who;
+    int64_t with_rows = 0, chained = 0;
+    for (int64_t u = 0, start = 0; u < n_users; u++) {
+        const int32_t p = P[(size_t)u], q = N[(size_t)u];
+        with_rows += p + q > 0;
+        if (p > 0 && q > 0 && feedback[u] != 0 && feedback[u] <= context_size) {
+            scored.push_back(GaucUser{(int32_t)start, p, q});
+            who.push_back((int32_t)u);
+            chained += (int64_t)p * q > (1 << 24);
+        }
+        start += p + q;
+    }
+    const int64_t ns = (int64_t)scored.size();
+    std::vector<float> auc((size_t)ns);
+    if (n > 0) {
+        ScopedDevice sd(ctx->device);
+        Fit F;
+        F.ctx = ctx;
+        F.st = ctx->stream;
+        F.nf = d.n_features;
+        F.k = prm->n_factors;
+        F.num_dimension = d.num_dimension;
+        F.prm = prm;
+        F.train = false;
+        F.n_params = d.n_params;
+        F.n_emb = d.n_emb;
+        F.E = d.E;
+        cudaStream_t st = F.st;
+        std::vector<int64_t> all((size_t)n);
+        for (int64_t r = 0; r < n; r++) all[(size_t)r] = r;
+        GB_TRY(F.upload_list(F.te[0], d.test_off, d.test_idx, d.test_val, all, d.n_emb > 0 ? d.E->test_row : nullptr));
+        F.slot_rows = std::min<int64_t>(prm->batch_size, n);
+        GB_TRY(F.upload_slots());
+        GB_TRY(F.ev_on.alloc(1));
+        GB_TRY(F.alloc_group(1));
+        const int32_t one = 1;
+        GB_CUDA(cudaMemcpyAsync(F.ev_on.p, &one, sizeof(int32_t), cudaMemcpyHostToDevice, st));
+        GB_CUDA(cudaMemcpyAsync(F.P, params, (size_t)d.n_params * sizeof(float), cudaMemcpyHostToDevice, st));
+        TestSet &T = F.te[0];
+        GB_TRY(F.predict(Group{1, F.stride, F.ev_on.p}, T));
+        if (o.pred) GB_CUDA(cudaMemcpyAsync(o.pred, T.pred, (size_t)n * sizeof(float), cudaMemcpyDeviceToHost, st));
+        if (ns > 0) {
+            Buf<uint32_t> hi;
+            Buf<uint64_t> key, sorted;
+            Buf<GaucUser> us;
+            Buf<float> auc_d;
+            Buf<unsigned char> tmp;
+            GB_TRY(hi.put(row_hi, st));
+            GB_TRY(us.put(scored, st));
+            GB_TRY(key.alloc((size_t)n));
+            GB_TRY(sorted.alloc((size_t)n));
+            GB_TRY(auc_d.alloc((size_t)ns));
+            fm_gauc_keys_kernel<<<(unsigned)std::min<int64_t>(div_up(n, 256), (int64_t)ctx->sm_count * 16), 256, 0, st>>>(T.pred, hi.p, n, key.p);
+            GB_LAUNCHED(ctx);
+            int end_bit = 33;   // the bits of the largest user index above the prediction and the list bit
+            while ((n_users - 1) >> (end_bit - 33)) end_bit++;
+            size_t bytes = 0;
+            GB_CUDA(cub::DeviceRadixSort::SortKeys(nullptr, bytes, key.p, sorted.p, (int)n, 0, end_bit, st));
+            GB_TRY(tmp.alloc(std::max<size_t>(bytes, 1)));
+            GB_CUDA(cub::DeviceRadixSort::SortKeys(tmp.p, bytes, key.p, sorted.p, (int)n, 0, end_bit, st));
+            fm_gauc_user_kernel<<<(unsigned)std::min<int64_t>(div_up(ns, WARPS), (int64_t)ctx->sm_count * 32), WARPS * 32, 0, st>>>(
+                sorted.p, us.p, ns, auc_d.p);
+            GB_LAUNCHED(ctx);
+            GB_CUDA(cudaMemcpyAsync(auc.data(), auc_d.p, (size_t)ns * sizeof(float), cudaMemcpyDeviceToHost, st));
+            GB_CUDA(cudaStreamSynchronize(st));   // the temporaries above are freed on return
+        }
+        GB_CUDA(cudaStreamSynchronize(st));
+    }
+    // main.go:199-206: sum += userAUC userCount and count += userCount in float32, in ascending user order, unfused
+    float sum = 0.0f, count = 0.0f;
+    int64_t with_nan = 0;
+    for (int64_t j = 0; j < ns; j++) {
+        const GaucUser &u = scored[(size_t)j];
+        const float cnt = (float)((int64_t)u.P + u.N), term = auc[(size_t)j] * cnt;
+        sum = sum + term;
+        count = count + cnt;
+        with_nan += std::isnan(auc[(size_t)j]);
+        const int32_t w = who[(size_t)j];
+        if (o.user) o.user[j] = w;
+        if (o.feedback) o.feedback[j] = feedback[w];
+        if (o.cand) o.cand[j] = (int64_t)u.P + u.N;
+        if (o.auc) o.auc[j] = auc[(size_t)j];
+    }
+    *o.n_scored = ns;
+    *o.gauc = count > 0.0f ? (double)(sum / count) : 0.0;
+    if (o.stats) {
+        const int64_t s[5] = {n, with_rows, ns, chained, with_nan};
+        std::copy(s, s + 5, o.stats);
+    }
+    return GORSE_B200_OK;
+}
 }  // namespace
 
 extern "C" int32_t gorse_b200_fm_fit_params_default(gorse_b200_fm_fit_params *p)
@@ -1363,4 +1505,44 @@ extern "C" int32_t gorse_b200_fm_fit_trials(gorse_b200_ctx *ctx, int64_t n_featu
     GB_CHECK_ARG(ctx != nullptr, "ctx is NULL");
     Progress pg{progress, user, n_train > 0, {}};
     return fit_groups(ctx, d, n_trials, trials, params_in, params_out, moments_out, pg, results);
+}
+
+extern "C" int32_t gorse_b200_fm_gauc(gorse_b200_ctx *ctx, int64_t n_features, int32_t n_factors, int32_t num_dimension, int32_t batch_size,
+                                      int32_t n_emb, const int32_t *emb_dim, const float *params, int64_t n_params, int64_t n_test,
+                                      const int64_t *test_off, const int32_t *test_idx, const float *test_val, const float *test_target,
+                                      const int32_t *test_emb_row, int64_t n_emb_rows, const uint16_t *const *item_emb,
+                                      const uint8_t *item_emb_mask, int64_t n_users, const int64_t *feedback_count, int64_t context_size,
+                                      float *pred_out, int32_t *user_out, int64_t *feedback_out, int64_t *cand_out, float *auc_out,
+                                      int64_t *n_scored_out, double *gauc_out, int64_t *stats_out)
+{
+    GB_CHECK_ARG(n_scored_out != nullptr && gauc_out != nullptr, "NULL n_scored_out/gauc_out");
+    *n_scored_out = 0;
+    *gauc_out = 0.0;
+    GB_CHECK_ARG(batch_size >= 1, "batch_size must be >= 1, not %d", batch_size);
+    GB_CHECK_ARG(n_params == 0 || params != nullptr, "params is NULL");
+    GB_CHECK_ARG(n_users >= 0 && n_users <= INT32_MAX, "n_users = %lld is not in [0, 2^31)", (long long)n_users);
+    GB_CHECK_ARG(n_users == 0 || feedback_count != nullptr, "feedback_count is NULL");
+    if (n_test > INT32_MAX) {
+        set_error("fm_gauc: %lld test rows, at most 2^31 - 1 (the radix sort counts in int)", (long long)n_test);
+        return GORSE_B200_ERR_UNSUPPORTED;
+    }
+    // the model as gorse_b200_fm_create takes it, the rows as gorse_b200_fm_fit_emb takes its test rows; no training rows
+    gorse_b200_fm_fit_params prm{};
+    GB_TRY(gorse_b200_fm_fit_params_default(&prm));
+    prm.n_factors = n_factors;
+    prm.batch_size = batch_size;
+    const EmbArgs E{n_emb, emb_dim, n_emb_rows, item_emb, item_emb_mask, nullptr, test_emb_row};
+    const Data d{n_features, num_dimension, n_emb, &E, 0, nullptr, nullptr, nullptr, nullptr,
+                 n_test, test_off, test_idx, test_val, test_target, n_params};
+    GB_TRY(check_data(d, &prm));
+    for (int64_t r = 0; r < n_test; r++) {
+        GB_CHECK_ARG(test_off[r + 1] > test_off[r], "test row %lld has no features, so no user", (long long)r);
+        const int32_t u = test_idx[test_off[r]];
+        GB_CHECK_ARG(u >= 0 && u < n_users, "test row %lld: user %d is not in [0, %lld)", (long long)r, u, (long long)n_users);
+    }
+    for (int64_t u = 0; u < n_users; u++)
+        GB_CHECK_ARG(feedback_count[u] >= 0, "user %lld: negative feedback count", (long long)u);
+    GB_CHECK_ARG(ctx != nullptr, "ctx is NULL");
+    return gauc_run(ctx, d, &prm, params, n_users, feedback_count, context_size,
+                    GaucOut{pred_out, user_out, feedback_out, cand_out, auc_out, n_scored_out, gauc_out, stats_out});
 }

@@ -730,6 +730,39 @@ int32_t gorse_b200_fm_fit_trials(gorse_b200_ctx *ctx, int64_t n_features, int32_
                                  float *const *params_out, float *const *moments_out, gorse_b200_fm_trials_progress_fn progress,
                                  void *user, gorse_b200_fm_fit_result *results);
 
+/* Ranker GAUC: the AFM half of `gorse-bench reranker` after the fit (EvaluateAFM, cmd/gorse-bench/main.go:125-207) -- how
+ * an operator weighs the factorization-machine ranker against an LLM reranker.
+ *   The model as gorse_b200_fm_create takes it (n_features .. n_params, the same limits); the test rows as
+ *   gorse_b200_fm_fit_emb takes them: CSR test_off[n_test + 1] (from 0) / test_idx / test_val (values already through
+ *   fm.Scalers), test_target[n_test], test_emb_row[n_test] (may be NULL without slots) and the bf16 item-embedding table
+ *   item_emb / item_emb_mask over n_emb_rows rows.
+ *   Per user: feedback_count[n_users] = the training rows with target > 0 whose first index is the user (main.go:133-140),
+ *   context_size = the config's recommend.context_size (default 100).  The user of test row r is test_idx[test_off[r]];
+ *   a row without features, or a user outside [0, n_users), is GORSE_B200_ERR_ARG.
+ * What runs: BatchInternalPredict (fm.go:156-178) on every test row as one list in test order, padded to
+ *   D = max(num_dimension, the longest test row), in chunks of batch_size rows whose softmax couples the chunk's rows
+ *   (DESIGN §8.4); these are not the predictions of the positive / negative lists of the fit's evaluation.  Then per user
+ *   with P > 0 positive (target > 0) and N > 0 negative rows and 0 < feedback_count <= context_size: AUC(pos, neg)
+ *   (model/ctr/evaluator.go:136-153) -- the negatives strictly below each positive (-0 == +0), summed as a float32 chain
+ *   over the positives in ascending order, divided by float32(P N).  GAUC = float64(sum / count) with sum += AUC
+ *   float32(P + N) and count += float32(P + N) in float32, unfused; 0 when no user is scored.  The reference visits the
+ *   users in Go map order, which varies from run to run: here they are visited in ascending user index.  A user with a
+ *   NaN prediction gets AUC = NaN (the reference's sort order with NaN is unpinned), which makes GAUC NaN.
+ *   Outputs: pred_out[n_test] (may be NULL) the predictions in test order, bit-identical to the project's CPU restatement;
+ *   per scored user in ascending user order, each array sized for n_users and each may be NULL: user_out, feedback_out
+ *   (feedback_count), cand_out (P + N), auc_out; *n_scored_out and *gauc_out (not NULL); stats_out[5] (may be NULL):
+ *   rows, users with rows, scored users, users summed by the sequential chain (P N > 2^24), scored users with a NaN
+ *   prediction.
+ * Every argument is checked on the host before the device is touched, ctx last, with gorse_b200_fm_fit's index and float32
+ * rounding checks.  n_test >= 2^31 is GORSE_B200_ERR_UNSUPPORTED.  The call keeps no state. */
+int32_t gorse_b200_fm_gauc(gorse_b200_ctx *ctx, int64_t n_features, int32_t n_factors, int32_t num_dimension, int32_t batch_size,
+                           int32_t n_emb, const int32_t *emb_dim, const float *params, int64_t n_params, int64_t n_test,
+                           const int64_t *test_off, const int32_t *test_idx, const float *test_val, const float *test_target,
+                           const int32_t *test_emb_row, int64_t n_emb_rows, const uint16_t *const *item_emb,
+                           const uint8_t *item_emb_mask, int64_t n_users, const int64_t *feedback_count, int64_t context_size,
+                           float *pred_out, int32_t *user_out, int64_t *feedback_out, int64_t *cand_out, float *auc_out,
+                           int64_t *n_scored_out, double *gauc_out, int64_t *stats_out);
+
 /* ------------------------------------------------------------------------------------------
  * Embedding evaluation: `gorse-bench embedding`'s scoring (EvaluateEmbedding, cmd/gorse-bench/main.go:322-467) for every test
  * user in one call -- how an operator picks the embedding behind an "embedding" item-to-item recommender.
