@@ -589,6 +589,104 @@ func (db *B200) UserToUserRecommend(ctx context.Context, collection string, user
 	return results, nil
 }
 
+// SessionRecommend answers the REST server's session recommendation (RestServer.sessionRecommend, server/rest.go:1069-1173)
+// for many sessions in one call on the collection ItemToItemCollection(name) of the first item-to-item recommender: row i
+// is the TopKFilter(top) of the handler for a session whose positive feedback items are contextIds[i] (in the order the
+// handler visits them, after data.SortFeedbacks and the positive feedback types) and whose items, of every feedback type,
+// are excludeIds[i].  Each context item's neighbours are QueryItemToItem(item, nil, n) (logics/item_to_item.go:50-86);
+// only the ones itemOK passes are kept; an item whose kept list is not empty counts, and the walk stops at the
+// contextSize-th one; the kept neighbours not in the exclude set are summed per id in float64 in context order.  top is
+// n + offset of the request; the caller slices [offset:].  scoreScale is 0.5 for type "auto", else 1.
+//
+// itemOK is FilterVisibleItemsByCategories (rest.go:815-832) for the request's categories: it receives the collection's
+// live ids once per call and returns, per id, whether the item exists in the data store, is not hidden and holds every
+// requested category; nil passes every id.  Every session of one call shares it, so a caller batches requests by
+// category.  Ids without a vector are passed as -1 (they give an empty list and do not count); the ids of one exclude set
+// must be distinct, as a set's are.  Exact score ties are ordered by slot; the reference's map order there is unpinned.
+// An error wrapping storage.ErrNotSupported (top above 1024, n outside the collection's limits, a Cosine collection) means
+// the caller runs the handler's own loop.
+func (db *B200) SessionRecommend(ctx context.Context, collection string, contextIds [][]string, excludeIds [][]string,
+	itemOK func(ids []string) ([]bool, error), n, contextSize, top int, scoreScale float64) ([][]cache.Score, error) {
+	if len(contextIds) != len(excludeIds) {
+		return nil, errors.Errorf("%d context lists with %d exclude sets", len(contextIds), len(excludeIds))
+	}
+	results := make([][]cache.Score, len(contextIds))
+	if len(contextIds) == 0 || top <= 0 {
+		return results, nil
+	}
+	db.mu.RLock()
+	defer db.mu.RUnlock()
+	c, err := db.collection(collection)
+	if err != nil {
+		return nil, err
+	}
+	var okFlags []uint8
+	if itemOK != nil {
+		// one flag per slot: the live ids are asked once, dead slots (never neighbours) stay 0
+		slots := make([]int64, 0, len(c.slotOf))
+		ids := make([]string, 0, len(c.slotOf))
+		for id, slot := range c.slotOf {
+			ids = append(ids, id)
+			slots = append(slots, slot)
+		}
+		flags, err := itemOK(ids)
+		if err != nil {
+			return nil, err
+		}
+		if len(flags) != len(ids) {
+			return nil, errors.Errorf("%d item flags for %d ids", len(flags), len(ids))
+		}
+		okFlags = make([]uint8, max(len(c.idOf), 1))
+		for i, v := range flags {
+			if v {
+				okFlags[slots[i]] = 1
+			}
+		}
+	}
+	slotsOf := func(lists [][]string) ([]int64, []int64) {
+		off := make([]int64, len(lists)+1)
+		slots := []int64{}
+		for i, ids := range lists {
+			for _, id := range ids {
+				slot, ok := c.slotOf[id]
+				if !ok {
+					slot = -1
+				}
+				slots = append(slots, slot)
+			}
+			off[i+1] = int64(len(slots))
+		}
+		return off, slots
+	}
+	ctxOff, ctxSlots := slotsOf(contextIds)
+	exOff, exSlots := slotsOf(excludeIds)
+	sessions := len(contextIds)
+	slots, scores, counts := make([]int64, sessions*top), make([]float64, sessions*top), make([]int32, sessions)
+	stats := make([]int64, 4)
+	st := C.gorse_b200_vecdb_session_recommend(c.handle, C.int64_t(sessions), i64p(ctxOff), i64p(ctxSlots), i64p(exOff), i64p(exSlots),
+		u8p(okFlags), C.int32_t(n), C.int32_t(contextSize), C.int32_t(top), C.double(scoreScale), i64p(slots),
+		(*C.double)(unsafe.Pointer(&scores[0])), i32p(counts), i64p(stats))
+	runtime.KeepAlive(ctxSlots)
+	runtime.KeepAlive(exSlots)
+	runtime.KeepAlive(okFlags)
+	if st == C.GORSE_B200_ERR_UNSUPPORTED {
+		return nil, fmt.Errorf("%s: %w", C.GoString(C.gorse_b200_last_error()), storage.ErrNotSupported)
+	}
+	if err := b200Err(st); err != nil {
+		return nil, err
+	}
+	log.Logger().Debug("batched session recommendation", zap.Int("sessions", sessions), zap.Int64("context_items", stats[0]),
+		zap.Int64("exact_rows", stats[1]))
+	for i := range results {
+		row := make([]cache.Score, 0, counts[i])
+		for j := i * top; j < i*top+int(counts[i]); j++ {
+			row = append(row, cache.Score{Id: c.idOf[slots[j]], Score: scores[j], Categories: c.catsOf[slots[j]]})
+		}
+		results[i] = row
+	}
+	return results, nil
+}
+
 func f32p(s []float32) *C.float {
 	if len(s) == 0 {
 		return nil

@@ -565,6 +565,40 @@ class VectorCollection:
         rows = [(items[u * m:u * m + c].copy(), scores[u * m:u * m + c].copy()) for u, c in zip(range(nu), cnt)]
         return rows, dict(zip(("query_users", "exact_rows", "shared_users", "global_users"), (int(x) for x in stats)))
 
+    def session_recommend(self, context_lists, exclude_lists, n, context_size, top, item_ok=None, score_scale=1.0):
+        """Batched session recommendation (gorse_b200_vecdb_session_recommend; server/rest.go:1069-1173): for session i, the
+        first n neighbours of every slot of context_lists[i] in order (-1 = an id without a vector), no category filter, then
+        only the neighbours with item_ok[slot] != 0 (None: all; one entry per slot of the collection); an entry whose filtered
+        list is not empty counts, and the walk stops at the context_size-th such entry.  The filtered neighbours not in
+        exclude_lists[i] are summed per slot in float64; the best `top` (n + offset of the request).  score_scale: 0.5 for
+        type "auto", else 1.
+        -> ([(slots int64, scores float64) per session], stats {context_items, exact_rows, shared_sessions, global_sessions})"""
+        ns = len(context_lists)
+        if len(exclude_lists) != ns:
+            raise ValueError(f"{len(exclude_lists)} exclude lists for {ns} sessions")
+
+        def csr(lists):
+            off = np.zeros(ns + 1, np.int64)
+            np.cumsum([len(x) for x in lists], out=off[1:])
+            flat = np.ascontiguousarray(np.concatenate([np.asarray(x, np.int64).reshape(-1) for x in lists]) if ns else [], np.int64)
+            return off, flat
+
+        coff, cs = csr(context_lists)
+        eoff, es = csr(exclude_lists)
+        ok = None
+        if item_ok is not None:
+            ok = np.ascontiguousarray(item_ok, np.uint8)
+            if ok.size != self.count()[1]:
+                raise ValueError(f"item_ok has {ok.size} entries for {self.count()[1]} slots")
+        m = max(top, 0)
+        slots, scores, cnt = np.full(max(ns * m, 1), -1, np.int64), np.zeros(max(ns * m, 1), np.float64), np.zeros(max(ns, 1), np.int32)
+        stats = np.zeros(4, np.int64)
+        check(lib.gorse_b200_vecdb_session_recommend(self.h, ns, ptr(coff), ptr(cs) if cs.size else None, ptr(eoff), ptr(es) if es.size else None,
+                                                     ptr(ok) if ok is not None and ok.size else None, n, context_size, top, float(score_scale),
+                                                     ptr(slots), ptr(scores), ptr(cnt), ptr(stats)))
+        rows = [(slots[s * m:s * m + c].copy(), scores[s * m:s * m + c].copy()) for s, c in zip(range(ns), cnt)]
+        return rows, dict(zip(("context_items", "exact_rows", "shared_sessions", "global_sessions"), (int(x) for x in stats)))
+
     def __enter__(self):
         return self
 

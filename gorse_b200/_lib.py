@@ -100,6 +100,8 @@ PROTOTYPES = {
     "gorse_b200_vecdb_item_to_item": (C.c_int32, [VP, C.c_int64, VP, VP, VP, VP, VP, C.c_int32, C.c_int32, C.c_double, VP, VP, VP, VP]),
     "gorse_b200_vecdb_user_to_user": (C.c_int32, [VP, C.c_int64, VP, C.c_int64, VP, VP, C.c_int32, VP, VP, VP, C.c_int32, C.c_double, VP, VP,
                                                   VP, VP]),
+    "gorse_b200_vecdb_session_recommend": (C.c_int32, [VP, C.c_int64, VP, VP, VP, VP, VP, C.c_int32, C.c_int32, C.c_int32, C.c_double, VP,
+                                                       VP, VP, VP]),
     "gorse_b200_fm_create": (C.c_int32, [VP, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_int32, VP, VP, C.c_int64, PVP]),
     "gorse_b200_fm_destroy": (C.c_int32, [VP]),
     "gorse_b200_fm_rank": (C.c_int32, [VP, C.c_int64, VP, VP, VP, VP, C.c_int64, VP, VP, VP, VP, VP, VP, VP, VP, VP, VP, VP]),

@@ -1,6 +1,6 @@
-// aggregate.cuh -- what the batched recommenders' aggregation kernels share (item_to_item.cu, user_to_user.cu): the
-// neighbour score transform, the shared-memory layout of one aggregating CTA, and the selection of the first n float64 sums
-// by (sum descending, id ascending).
+// aggregate.cuh -- what the batched recommenders' aggregation kernels share (item_to_item.cu, user_to_user.cu,
+// session.cu): the neighbour score transform, the shared-memory layout of one aggregating CTA, the float64 sum per id, and
+// the selection of the first n float64 sums by (sum descending, id ascending).
 #pragma once
 #include "recall.cuh"
 
@@ -57,6 +57,34 @@ __device__ __forceinline__ double neighbour_score(float raw, double scale, bool 
 {
     const double s = __dmul_rn((double)raw, scale);
     return euclid ? __ddiv_rn(1.0, __dsub_rn(1.0, s)) : s;
+}
+
+// sum[id] += s for one CTA's float64 sums, each starting at 0 + s as the reference's map does.  SHARED: the open-addressing
+// table t_key / t_val of cap = 2^lg entries; else the global row acc with its flag row seen and the list touched of the ids
+// set so far.  *distinct counts the ids.  Concurrent calls must add to distinct ids.
+template <bool SHARED>
+__device__ __forceinline__ void add_sum(int32_t id, double s, int32_t *t_key, double *t_val, int cap, int lg, double *acc, uint8_t *seen,
+                                        int32_t *touched, int *distinct)
+{
+    if (SHARED) {
+        uint32_t h = ((uint32_t)id * 0x9E3779B1u) >> (32 - lg);
+        for (;;) {
+            const int32_t k = t_key[h];
+            if (k == id) { t_val[h] = __dadd_rn(t_val[h], s); break; }
+            if (k < 0 && atomicCAS(&t_key[h], -1, id) == -1) {
+                t_val[h] = __dadd_rn(0.0, s);
+                atomicAdd(distinct, 1);
+                break;
+            }
+            h = (h + 1) & (uint32_t)(cap - 1);
+        }
+    } else if (seen[id]) {
+        acc[id] = __dadd_rn(acc[id], s);
+    } else {
+        seen[id] = 1;
+        touched[atomicAdd(distinct, 1)] = id;
+        acc[id] = __dadd_rn(0.0, s);
+    }
 }
 
 // The first m = min(n, distinct) of the entries 0 .. range-1 by (sum descending, id ascending), sorted into S.s_key (low 32

@@ -66,26 +66,7 @@ i2i_aggregate_kernel(const int32_t *users, int64_t n_users, Users U, Table T, in
             for (int j = threadIdx.x; j < cnt; j += NT) {
                 const int32_t slot = T.slot[r * n + j];
                 if (contains(ex, n_ex, (int64_t)slot)) continue;
-                const double s = neighbour_score(T.score[r * n + j], scale, euclid);
-                if (SHARED) {
-                    uint32_t h = ((uint32_t)slot * 0x9E3779B1u) >> (32 - lg);
-                    for (;;) {
-                        const int32_t k = t_key[h];
-                        if (k == slot) { t_val[h] = __dadd_rn(t_val[h], s); break; }
-                        if (k < 0 && atomicCAS(&t_key[h], -1, slot) == -1) {
-                            t_val[h] = __dadd_rn(0.0, s);   // the reference's map starts every sum at 0
-                            atomicAdd(&s_bc[3], 1);
-                            break;
-                        }
-                        h = (h + 1) & (uint32_t)(cap - 1);
-                    }
-                } else if (seen[slot]) {
-                    acc[slot] = __dadd_rn(acc[slot], s);
-                } else {
-                    seen[slot] = 1;
-                    touched[atomicAdd(&s_bc[3], 1)] = slot;
-                    acc[slot] = __dadd_rn(0.0, s);
-                }
+                add_sum<SHARED>(slot, neighbour_score(T.score[r * n + j], scale, euclid), t_key, t_val, cap, lg, acc, seen, touched, &s_bc[3]);
             }
             __syncthreads();
         }

@@ -4,20 +4,21 @@
 #include "topk.cuh"
 
 namespace gb {
-// grow-only work buffers of gorse_b200_vecdb_item_to_item (item_to_item.cu): the neighbour table of stage A and the user
-// batches, answers and accumulator scratch of stage B
+// grow-only work buffers of gorse_b200_vecdb_item_to_item (item_to_item.cu) and gorse_b200_vecdb_session_recommend
+// (session.cu), which both hold the collection's lock: the neighbour table of stage A, the user or session batches, answers
+// and accumulator scratch of stage B, and the session call's item mask
 struct ItemToItemWork {
     DevBuf<int64_t> nb, c_off, ex_off, ex, slots;
     DevBuf<int32_t> t_slot, t_cnt, c_row, users, count;
     DevBuf<float> t_score;
     DevBuf<double> scores, acc;
-    DevBuf<uint8_t> seen;
+    DevBuf<uint8_t> seen, item_ok;
     DevBuf<int32_t> touched;
     void free()
     {
         nb.free(); c_off.free(); ex_off.free(); ex.free(); slots.free();
         t_slot.free(); t_cnt.free(); c_row.free(); users.free(); count.free();
-        t_score.free(); scores.free(); acc.free(); seen.free(); touched.free();
+        t_score.free(); scores.free(); acc.free(); seen.free(); item_ok.free(); touched.free();
     }
 };
 
@@ -54,7 +55,7 @@ struct gorse_b200_vecdb {
     gb::DevBuf<uint8_t> d_blocked, d_allow;   // blocked = hidden | dead
     gb::DevBuf<int64_t> d_cat_off;
     gb::DevBuf<int32_t> d_cats, d_want;
-    gb::ItemToItemWork i2i;  // batched item-to-item recommendation (item_to_item.cu)
+    gb::ItemToItemWork i2i;  // batched item-to-item and session recommendation (item_to_item.cu, session.cu)
     gb::UserToUserWork u2u;  // batched user-to-user recommendation (user_to_user.cu)
 };
 

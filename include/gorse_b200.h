@@ -467,6 +467,42 @@ int32_t gorse_b200_vecdb_user_to_user(gorse_b200_vecdb *db, int64_t n_users, con
                                       const int64_t *fb_off, const int32_t *fb_items, int32_t n_items, const uint8_t *item_ok,
                                       const int64_t *excl_off, const int64_t *excl_items, int32_t n, double score_scale,
                                       int64_t *items_out, double *scores_out, int32_t *count_out, int64_t *stats_out);
+/* Batched session recommendation: for n_sessions posted sessions at once, what the REST server's session recommendation does
+ * per request (RestServer.sessionRecommend, server/rest.go:1069-1173) on the first item-to-item collection: Euclidean for
+ * type "embedding", sparse Dot for "tags" / "users" / "auto".
+ *   C_s = ctx_slots[ctx_off[s] .. ctx_off[s+1]) (ctx_off[0] = 0): the session's positive feedback items in the order the
+ *   handler visits them (after data.SortFeedbacks and MatchFeedbackTypeExpressions, rest.go:1110-1121).  Entries -1 (an id
+ *   without a vector) and deleted slots give an empty list (QueryItemToItem returns nil) and do not count; a hidden item is
+ *   still queried.  A slot may repeat: each repeat is queried, counts and adds again.  A slot outside [-1, slots) is
+ *   GORSE_B200_ERR_ARG.
+ *   E_s = excl_slots[excl_off[s] .. excl_off[s+1]) (excl_off[0] = 0): every item of the session, whatever its feedback type,
+ *   with the rules of gorse_b200_vecdb_query_excluding (-1 allowed, a slot twice in one row is GORSE_B200_ERR_ARG).
+ *   Neighbours of a context item c: QueryItemToItem(c, nil, n) (logics/item_to_item.go:50-86) -- the live, not hidden
+ *   vectors other than c, with no category filter, by score descending, exact ties by lower slot; Dot collections drop
+ *   scores <= 0; the first n.  Neighbour score s = (double)score * score_scale (0.5 for type "auto", else 1); Euclidean:
+ *   s = 1 / (1 - s).  The scores are bit-identical to gorse_b200_vecdb_query's.
+ *   item_ok[slots of db] (may be NULL = every item passes): what FilterVisibleItemsByCategories checks (rest.go:815-832):
+ *   the item exists, is not hidden in the data store and holds every requested category; one mask for every session of the
+ *   call.
+ *   Row s: for every context entry in order, its neighbours with item_ok = 1, in their order; if that list is not empty the
+ *   entry counts; every listed neighbour j not in E_s gets acc[j] += s in float64 (each sum starting at 0 + s); the walk
+ *   stops after the entry that makes the count reach context_size (context_size <= 0 stops after the first counting entry,
+ *   as the handler's `>=` does).  Then the first `top` of acc by score descending, exact ties by lower slot -- the handler's
+ *   TopKFilter(n + offset), so top = n + offset and the caller slices [offset:].  Each sum is formed in context order, as
+ *   the reference's, so the scores match it bit for bit.  The reference ranks exact ties in Go map order, so which of them
+ *   it keeps at the cut is unpinned.
+ *   Output: row s at s*top in slots_out / scores_out (buffers of n_sessions*top), count_out[s] <= top entries.  top <= 0:
+ *   every count is 0.  top above 1024: GORSE_B200_ERR_UNSUPPORTED.  n outside [1, 128] (sparse) or [1, 1024] (dense):
+ *   GORSE_B200_ERR_UNSUPPORTED (the reference's n = 0 keeps one neighbour of the n + 1 it asks for).  Cosine collections:
+ *   GORSE_B200_ERR_UNSUPPORTED.  A NaN score (or score_scale): GORSE_B200_ERR_ARG.  Every argument is checked before the
+ *   device is touched, and every one that does not depend on the collection before db is.
+ *   stats_out[4] (may be NULL): distinct context items queried, of them answered by the exact scan rather than the
+ *   tensor-core sweep (dense), sessions aggregated in shared memory, sessions aggregated in a global-memory row; the answer
+ *   does not depend on them.  Thread-safe per collection; no host pointer is kept after the call. */
+int32_t gorse_b200_vecdb_session_recommend(gorse_b200_vecdb *db, int64_t n_sessions, const int64_t *ctx_off, const int64_t *ctx_slots,
+                                           const int64_t *excl_off, const int64_t *excl_slots, const uint8_t *item_ok, int32_t n,
+                                           int32_t context_size, int32_t top, double score_scale, int64_t *slots_out, double *scores_out,
+                                           int32_t *count_out, int64_t *stats_out);
 
 /* ------------------------------------------------------------------------------------------
  * Batched FM ranking: the worker's "fm" ranker (rankByClickTroughRate, worker/pipeline.go:450-499) for many users in one
