@@ -270,24 +270,42 @@ struct __align__(16) RoundSlot {
 };
 
 __device__ __forceinline__ void consumer_bar() { asm volatile("bar.sync %0, %1;" ::"n"(kConsumerBar), "n"(kConsumers) : "memory"); }
+// the same named barrier, entered only once `dep` is in a register (see consumer_grid_sync)
+__device__ __forceinline__ void consumer_bar(float dep)
+{
+    asm volatile("bar.sync %0, %1;" ::"n"(kConsumerBar), "n"(kConsumers), "f"(dep) : "memory");
+}
 __device__ __forceinline__ void sampler_bar(int group) { asm volatile("bar.sync %0, %1;" ::"r"(kSamplerBar0 + group), "n"(kSamplers) : "memory"); }
 
 // Grid barrier over the consumer threads only (the samplers run ahead and never join it): `count` starts at 0 and
-// `target` is the number of the barrier within the launch times the grid size.  One memory barrier per grid barrier:
-// the fence before the relaxed add releases what the CTA's consumers wrote before the named barrier, and waits for their
-// reductions to complete (a red.release after it would fence a second time).  The spin polls relaxed; one ld.acquire
-// once the count is reached acquires what every CTA released, since all the adds are read-modify-writes of one counter.
-// An ld.acquire in the loop would invalidate L1 on every poll.
-__device__ __forceinline__ void consumer_grid_sync(uint32_t *count, uint32_t target)
+// `target` is the number of the barrier within the launch times the grid size.  Thread 0 of each CTA adds 1 to `count`
+// and polls it; the CTA's other consumers wait at the named barriers.  The two barriers of a round order different
+// things (PTX ISA, "Memory Consistency Model"):
+//  - The barrier that ends a round (RELEASE) orders the round's additions before the next round's loads.  The fence
+//    after the named barrier makes fence + relaxed add a release pattern, and bar.sync and the fence's cumulativity put
+//    every consumer's reductions in it; it is also what waits for those reductions to complete.  The adds are
+//    read-modify-writes of one location, so the one ld.acquire after the count is reached observes every CTA's add and
+//    synchronizes with every CTA's release.  That is one MEMBAR.GPU per barrier; a red.release would fence a second time,
+//    and an ld.acquire in the poll loop would invalidate L1 on every poll.
+//  - The barrier between a round's loads and its additions orders those loads before other CTAs' later reductions to
+//    the same rows.  It needs no fence and no acquire: every load of the CTA has returned its value before thread 0
+//    arrives, because each consumer enters the named barrier with `dep`, a value computed from all its loads (the
+//    triple's gradient factor; the trials kernel stores its deltas to shared memory before the barrier instead).  A load
+//    that read a reduction issued after the barrier would close a cycle of dependencies and observations, which the
+//    model's No Thin Air axiom rules out.  The CTA's own writes were released by the previous round's barrier.
+//    Measured in DESIGN 5.1.
+template <bool RELEASE>
+__device__ __forceinline__ void consumer_grid_sync(uint32_t *count, uint32_t target, float dep)
 {
-    consumer_bar();
+    consumer_bar(dep);
     if (threadIdx.x == 0) {
-        asm volatile("fence.acq_rel.gpu;\n\tred.relaxed.gpu.global.add.u32 [%0], 1;" ::"l"(count) : "memory");
+        if (RELEASE) asm volatile("fence.acq_rel.gpu;" ::: "memory");
+        asm volatile("red.relaxed.gpu.global.add.u32 [%0], 1;" ::"l"(count) : "memory");
         uint32_t seen;
         do {
             asm volatile("ld.relaxed.gpu.global.u32 %0, [%1];" : "=r"(seen) : "l"(count) : "memory");
         } while ((int32_t)(seen - target) < 0);
-        asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(seen) : "l"(count) : "memory");
+        if (RELEASE) asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(seen) : "l"(count) : "memory");
     }
     consumer_bar();
 }
@@ -380,7 +398,7 @@ __global__ void __launch_bounds__(kRoundThreads, 1)
             load_rows<C>(rw, Pu, v.Q + (int64_t)i * v.d + 4 * lane4, 16, v.Q + (int64_t)j * v.d + 4 * lane4, 16);
             g = bpr_grad_rows<C>(rw, mask);   // consumes every loaded value before the barrier
         }
-        consumer_grid_sync(barrier_count, ++n_sync * gridDim.x);
+        consumer_grid_sync<false>(barrier_count, ++n_sync * gridDim.x, g);
         if (live) {
             float *Di = D + t * d, *Dj = D + (kRoundQuads + t) * d;
 #pragma unroll
@@ -414,7 +432,7 @@ __global__ void __launch_bounds__(kRoundThreads, 1)
         }
         __syncwarp();
         if ((threadIdx.x & 31) == 0) mma::mbar_arrive(&empty[s]);
-        consumer_grid_sync(barrier_count, ++n_sync * gridDim.x);
+        consumer_grid_sync<true>(barrier_count, ++n_sync * gridDim.x, 0.f);
     }
 }
 
@@ -520,7 +538,7 @@ __global__ void __launch_bounds__(kRoundThreads, 1)
                 }
             }
         }
-        consumer_grid_sync(barrier_count, ++n_sync * gridDim.x);
+        consumer_grid_sync<false>(barrier_count, ++n_sync * gridDim.x, 0.f);   // the loads are consumed into shared memory
 #pragma unroll 1
         for (int m = 0; m < M.n; m++) {
             const float *Dm = D + m * kModelFloats;
@@ -552,7 +570,7 @@ __global__ void __launch_bounds__(kRoundThreads, 1)
         }
         __syncwarp();
         if ((threadIdx.x & 31) == 0) mma::mbar_arrive(&empty[s]);
-        consumer_grid_sync(barrier_count, ++n_sync * gridDim.x);
+        consumer_grid_sync<true>(barrier_count, ++n_sync * gridDim.x, 0.f);
     }
 }
 
