@@ -87,7 +87,40 @@ func (db *B200) Init() error {
 	return b200Err(C.gorse_b200_ctx_create(C.int32_t(db.device), &db.ctx))
 }
 
-func (db *B200) Optimize(ctx context.Context, name string) error { return nil } // brute force: nothing to build
+// Optimize reclaims the slots of deleted vectors (xvec.go:125-131 optimizes its index here): the live vectors keep their
+// order in slots 0 .. live-1.  Slot maps taken from this collection before the call are stale afterwards.
+func (db *B200) Optimize(ctx context.Context, name string) error {
+	db.mu.Lock()
+	defer db.mu.Unlock()
+	c, err := db.collection(name)
+	if err != nil {
+		return err
+	}
+	return c.compact()
+}
+
+// compact runs gorse_b200_vecdb_compact and renames slotOf, idOf and catsOf through its map; the caller holds db.mu for
+// writing.
+func (c *b200Collection) compact() error {
+	if len(c.idOf) == 0 {
+		return nil
+	}
+	newSlot := make([]int64, len(c.idOf))
+	if err := b200Err(C.gorse_b200_vecdb_compact(c.handle, i64p(newSlot), nil)); err != nil {
+		return err
+	}
+	idOf, catsOf := make([]string, 0, len(c.slotOf)), make([][]string, 0, len(c.slotOf))
+	for old, slot := range newSlot {
+		if slot >= 0 {
+			idOf, catsOf = append(idOf, c.idOf[old]), append(catsOf, c.catsOf[old])
+		}
+	}
+	for id, old := range c.slotOf {
+		c.slotOf[id] = newSlot[old]
+	}
+	c.idOf, c.catsOf = idOf, catsOf
+	return nil
+}
 
 func (db *B200) Close() error {
 	db.mu.Lock()
@@ -313,6 +346,15 @@ func (db *B200) DeleteVectors(ctx context.Context, name string, timestamp time.T
 		if c.slotOf[c.idOf[slot]] == slot {
 			delete(c.slotOf, c.idOf[slot])
 		}
+	}
+	// the master rewrites every vector once per cycle and then deletes the old versions here: compacting once the dead
+	// slots are as many as the live ones keeps a collection at most twice its live size
+	var live, total C.int64_t
+	if err := b200Err(C.gorse_b200_vecdb_count(c.handle, &live, &total)); err != nil {
+		return err
+	}
+	if total-live >= live {
+		return c.compact()
 	}
 	return nil
 }

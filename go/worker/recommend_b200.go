@@ -48,7 +48,8 @@ type B200Stage struct {
 	Collection unsafe.Pointer
 	N          int32
 	ScoreScale float64
-	// ITEM_TO_ITEM
+	// ITEM_TO_ITEM.  SlotOfItem / ItemOfSlot, and UserSlots / Feedback below, name slots of the collection: a DeleteVectors
+	// or Optimize on it renumbers them (gorse_b200_vecdb_compact), so they are built again for every call.
 	Context    [][]int32 // per user, positive feedback newest first, -1 = outside the dictionary
 	SlotOfItem []int64
 	ItemOfSlot []int32
@@ -91,7 +92,7 @@ func B200Stages(cfg *config.RecommendConfig) ([]B200Stage, error) {
 type B200CF struct {
 	Collection  unsafe.Pointer // *C.gorse_b200_vecdb of the "collaborative_filtering_<id>" collection
 	UserVectors []float32      // n_users x dim
-	SlotOfItem  []int64
+	SlotOfItem  []int64        // like the stages' maps, stale after a DeleteVectors or Optimize on the collection
 	ItemOfSlot  []int32
 	N           int32
 }

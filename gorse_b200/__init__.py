@@ -469,6 +469,15 @@ class VectorCollection:
         check(lib.gorse_b200_vecdb_delete_before(self.h, timestamp_ms, ptr(out), cap, C.byref(cnt)))
         return out[:min(cnt.value, cap)]
 
+    def compact(self):
+        """Reclaim the slots of deleted vectors (gorse_b200_vecdb_compact; Optimize, storage/vectors/database.go:109): live
+        slots keep their order and become 0 .. live-1, and every query answers as before with slots renamed.
+        -> (new_slot int64 [slots before the call], -1 for a deleted slot; device bytes before; device bytes after)"""
+        slots = self.count()[1]
+        new_slot, nbytes = np.zeros(max(slots, 1), np.int64), np.zeros(2, np.int64)
+        check(lib.gorse_b200_vecdb_compact(self.h, ptr(new_slot), ptr(nbytes)))
+        return new_slot[:slots], int(nbytes[0]), int(nbytes[1])
+
     def query(self, q, categories=(), topk=10):
         """q: dense [nq, dim] array, or a list of (indices, values) for a sparse collection.
         -> (slots int64 [nq, topk], scores float32 [nq, topk], count int32 [nq])"""

@@ -92,6 +92,7 @@ PROTOTYPES = {
     "gorse_b200_vecdb_get": (C.c_int32, [VP, VP, C.c_int64, VP, VP, VP, VP]),
     "gorse_b200_vecdb_get_sparse": (C.c_int32, [VP, C.c_int64, VP, VP, C.c_int32, C.POINTER(C.c_int32)]),
     "gorse_b200_vecdb_delete_before": (C.c_int32, [VP, C.c_int64, VP, C.c_int64, C.POINTER(C.c_int64)]),
+    "gorse_b200_vecdb_compact": (C.c_int32, [VP, VP, VP]),
     "gorse_b200_vecdb_add_item_factors": (C.c_int32, [VP, VP, VP, C.c_int64, VP, VP, VP]),
     "gorse_b200_marshal_latent_factors": (C.c_int32, [VP, C.c_int32, C.c_int32, VP, VP, VP, C.c_size_t, C.POINTER(C.c_size_t)]),
     "gorse_b200_vecdb_query": (C.c_int32, [VP, C.c_int64, VP, VP, VP, VP, C.c_int32, C.c_int32, VP, VP, VP]),

@@ -121,6 +121,7 @@ struct DevBuf {
         p = nullptr;
         n = 0;
     }
+    size_t bytes() const { return n * sizeof(T); }
 };
 
 struct ScopedDevice {

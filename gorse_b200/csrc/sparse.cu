@@ -16,6 +16,8 @@
 // reference drops them right after the query, logics/item_to_item.go:73).  Roofline class: HBM/L2 (N floats scanned per query).
 #include <algorithm>
 
+#include <cub/cub.cuh>
+
 #include "sparse.cuh"
 
 using namespace gb;
@@ -151,6 +153,55 @@ int32_t sync_device(gorse_b200_sparse_index *ix)
     ix->acc_slots = 0;
     ix->dirty = false;
     return GORSE_B200_OK;
+}
+
+// ---- compaction (sparse_compact): `scan` is the exclusive sum of the rows' live flags, row r is live iff scan[r + 1] != scan[r]
+// keep[t] = 1 for the CSR entries of live rows, keep[nnz] = 0; one warp per row
+__global__ void sparse_row_keep_kernel(const int64_t *off, int64_t n, const int64_t *scan, int64_t *keep)
+{
+    const int lane = threadIdx.x & 31;
+    const int64_t nw = ((int64_t)gridDim.x * blockDim.x) >> 5;
+    for (int64_t r = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5; r < n; r += nw) {
+        const int64_t k = scan[r + 1] != scan[r];
+        for (int64_t t = off[r] + lane; t < off[r + 1]; t += 32) keep[t] = k;
+    }
+    if (blockIdx.x == 0 && threadIdx.x == 0) keep[off[n]] = 0;
+}
+// keep[p] = 1 for the CSC entries whose row is live, keep[nnz] = 0
+__global__ void sparse_col_keep_kernel(const int32_t *frow, int64_t nnz, const int64_t *scan, int64_t *keep)
+{
+    const int64_t st = (int64_t)gridDim.x * blockDim.x;
+    for (int64_t p = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; p <= nnz; p += st)
+        keep[p] = p < nnz && scan[frow[p] + 1] != scan[frow[p]];
+}
+// entries are grouped by row (by feature), so a list's new offset is the entry scan read at its old one:
+// off'[scan[r]] = e_scan[off[r]] for live r and off'[live] = e_scan[nnz]; rows == nullptr: every list is kept, out[i] = e_scan[in[i]]
+__global__ void sparse_compact_off_kernel(const int64_t *in, int64_t m, const int64_t *rows, const int64_t *e_scan, int64_t *out)
+{
+    const int64_t st = (int64_t)gridDim.x * blockDim.x;
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i <= m; i += st) {
+        if (!rows) out[i] = e_scan[in[i]];
+        else if (i == m) out[rows[m]] = e_scan[in[m]];
+        else if (rows[i + 1] != rows[i]) out[rows[i]] = e_scan[in[i]];
+    }
+}
+// the kept entries to their scanned positions; CSC rows are renamed through the row scan (monotone: lists stay ascending)
+__global__ void sparse_compact_csr_kernel(const uint32_t *ind, const float *val, int64_t nnz, const int64_t *e_scan, uint32_t *ind_n, float *val_n)
+{
+    const int64_t st = (int64_t)gridDim.x * blockDim.x;
+    for (int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; t < nnz; t += st) {
+        const int64_t to = e_scan[t];
+        if (e_scan[t + 1] != to) { ind_n[to] = ind[t]; val_n[to] = val[t]; }
+    }
+}
+__global__ void sparse_compact_csc_kernel(const int32_t *frow, const float *fval, int64_t nnz, const int64_t *e_scan, const int64_t *scan,
+                                          int32_t *frow_n, float *fval_n)
+{
+    const int64_t st = (int64_t)gridDim.x * blockDim.x;
+    for (int64_t p = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; p < nnz; p += st) {
+        const int64_t to = e_scan[p];
+        if (e_scan[p + 1] != to) { frow_n[to] = (int32_t)scan[frow[p]]; fval_n[to] = fval[p]; }
+    }
 }
 
 }  // namespace
@@ -313,6 +364,71 @@ int32_t sparse_search_host(gorse_b200_sparse_index *ix, int64_t q0, int64_t nq, 
     if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
     if (e != cudaSuccess) { set_error("sparse search: %s", cudaGetErrorString(e)); return done(GORSE_B200_ERR_CUDA); }
     return done(GORSE_B200_OK);
+}
+
+int32_t sparse_compact(gorse_b200_sparse_index *ix, const int64_t *scan, int64_t live)
+{
+    GB_TRY(sync_device(ix));
+    gorse_b200_ctx *c = ix->ctx;
+    cudaStream_t s = c->stream;
+    const int64_t n = (int64_t)ix->h_off.size() - 1, nnz = (int64_t)ix->h_ind.size(), F = ix->n_features;
+    DevBuf<int64_t> rs, cs, off_n, foff_n;   // entry keep flags, scanned in place: CSR (rs) and CSC (cs)
+    DevBuf<uint8_t> tmp;
+    DevBuf<uint32_t> ind_n;
+    DevBuf<float> val_n, fval_n;
+    DevBuf<int32_t> frow_n;
+    auto done = [&](int32_t st) {
+        cudaStreamSynchronize(s);
+        rs.free(); cs.free(); tmp.free();
+        if (st) { off_n.free(); foff_n.free(); ind_n.free(); val_n.free(); fval_n.free(); frow_n.free(); }
+        return st;
+    };
+    int32_t st;
+    if ((st = rs.alloc((size_t)nnz + 1)) || (st = cs.alloc((size_t)nnz + 1))) return done(st);
+    const unsigned grid = (unsigned)c->sm_count * 8;
+    sparse_row_keep_kernel<<<grid, 256, 0, s>>>(ix->off.p, n, scan, rs.p);
+    sparse_col_keep_kernel<<<grid, 256, 0, s>>>(ix->frow.p, nnz, scan, cs.p);
+    c->launches += 2;
+    size_t tmp_bytes = 0;
+    cudaError_t e = cudaGetLastError();
+    if (e == cudaSuccess) e = cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, rs.p, nnz + 1, s);
+    if (e != cudaSuccess) { set_error("sparse compact: %s", cudaGetErrorString(e)); return done(GORSE_B200_ERR_CUDA); }
+    if ((st = tmp.alloc(tmp_bytes))) return done(st);
+    int64_t live_nnz = 0;
+    e = cub::DeviceScan::ExclusiveSum(tmp.p, tmp_bytes, rs.p, nnz + 1, s);
+    if (e == cudaSuccess) e = cub::DeviceScan::ExclusiveSum(tmp.p, tmp_bytes, cs.p, nnz + 1, s);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(&live_nnz, rs.p + nnz, sizeof(int64_t), cudaMemcpyDeviceToHost, s);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+    if (e != cudaSuccess) { set_error("sparse compact: %s", cudaGetErrorString(e)); return done(GORSE_B200_ERR_CUDA); }
+    // every buffer of the compacted index, then the host CSR, before any state changes
+    if ((st = off_n.alloc((size_t)live + 1)) || (st = foff_n.alloc((size_t)F + 1)) || (st = ind_n.alloc((size_t)live_nnz)) ||
+        (st = val_n.alloc((size_t)live_nnz)) || (st = frow_n.alloc((size_t)live_nnz)) || (st = fval_n.alloc((size_t)live_nnz)))
+        return done(st);
+    std::vector<int64_t> h_off((size_t)live + 1);
+    std::vector<uint32_t> h_ind((size_t)live_nnz);
+    std::vector<float> h_val((size_t)live_nnz);
+    sparse_compact_off_kernel<<<div_up(n + 1, 256), 256, 0, s>>>(ix->off.p, n, scan, rs.p, off_n.p);
+    sparse_compact_off_kernel<<<div_up((int64_t)F + 1, 256), 256, 0, s>>>(ix->foff.p, F, nullptr, cs.p, foff_n.p);
+    sparse_compact_csr_kernel<<<grid, 256, 0, s>>>(ix->ind.p, ix->val.p, nnz, rs.p, ind_n.p, val_n.p);
+    sparse_compact_csc_kernel<<<grid, 256, 0, s>>>(ix->frow.p, ix->fval.p, nnz, cs.p, scan, frow_n.p, fval_n.p);
+    c->launches += 4;
+    e = cudaGetLastError();
+    if (e == cudaSuccess) e = cudaMemcpyAsync(h_off.data(), off_n.p, sizeof(int64_t) * h_off.size(), cudaMemcpyDeviceToHost, s);
+    if (e == cudaSuccess && live_nnz) e = cudaMemcpyAsync(h_ind.data(), ind_n.p, sizeof(uint32_t) * h_ind.size(), cudaMemcpyDeviceToHost, s);
+    if (e == cudaSuccess && live_nnz) e = cudaMemcpyAsync(h_val.data(), val_n.p, sizeof(float) * h_val.size(), cudaMemcpyDeviceToHost, s);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+    if (e != cudaSuccess) { set_error("sparse compact: %s", cudaGetErrorString(e)); return done(GORSE_B200_ERR_CUDA); }
+    ix->off.free(); ix->foff.free(); ix->ind.free(); ix->val.free(); ix->frow.free(); ix->fval.free();
+    ix->off = off_n; ix->foff = foff_n; ix->ind = ind_n; ix->val = val_n; ix->frow = frow_n; ix->fval = fval_n;
+    ix->h_off.swap(h_off); ix->h_ind.swap(h_ind); ix->h_val.swap(h_val);
+    ix->acc.free();   // [slots x N]; reserve_acc allocates and zeroes it again for the new N
+    ix->acc_slots = 0;
+    return done(GORSE_B200_OK);
+}
+
+size_t sparse_bytes(const gorse_b200_sparse_index *ix)
+{
+    return ix->off.bytes() + ix->foff.bytes() + ix->ind.bytes() + ix->val.bytes() + ix->frow.bytes() + ix->fval.bytes() + ix->acc.bytes();
 }
 
 }  // namespace gb

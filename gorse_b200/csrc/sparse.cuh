@@ -31,4 +31,11 @@ int32_t sparse_search_host(gorse_b200_sparse_index *ix, int64_t q0, int64_t nq, 
 // index holds at least one vector; the caller holds ix->mu and the device.
 int32_t sparse_search_rows(gorse_b200_sparse_index *ix, const int64_t *d_rows, int64_t nq, const uint8_t *d_allow, int32_t k, int32_t *d_idx,
                            float *d_dot, int32_t *d_cnt);
+// compaction (gorse_b200_vecdb_compact): scan[n + 1] (device) is the exclusive sum of the live flags (row r is live iff
+// scan[r + 1] != scan[r] and then becomes row scan[r]), live = scan[n].  Both layouts are compacted on the device, the host
+// CSR is replaced by the compacted one and the index ends clean; the accumulator is released.  On an error the rows are
+// unchanged (the device mirrors may have been brought up to date).  The caller holds ix->mu and the device.
+int32_t sparse_compact(gorse_b200_sparse_index *ix, const int64_t *scan, int64_t live);
+// device bytes held by the index
+size_t sparse_bytes(const gorse_b200_sparse_index *ix);
 }

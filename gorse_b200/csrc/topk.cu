@@ -528,6 +528,59 @@ int32_t index_reserve(gorse_b200_index *ix, int64_t need)
     return GORSE_B200_OK;
 }
 
+// Xn[scan[s]] = X[s] for every live slot s (scan[s + 1] != scan[s]); V = float4 when d % 4 == 0, one V per thread
+template <typename V>
+__global__ void index_compact_rows_kernel(const V *X, int64_t n, int dv, const int64_t *scan, V *Xn)
+{
+    int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    const int64_t total = n * dv, st = (int64_t)gridDim.x * blockDim.x;
+    for (; i < total; i += st) {
+        const int64_t s = i / dv, c = i - s * dv, to = scan[s];
+        if (scan[s + 1] != to) Xn[to * dv + c] = X[i];
+    }
+}
+
+int32_t index_compact(gorse_b200_index *ix, const int64_t *scan, int64_t live)
+{
+    gorse_b200_ctx *c = ix->ctx;
+    DevBuf<float> nx;
+    int32_t st = nx.alloc((size_t)live * ix->d);
+    if (st) return st;
+    cudaError_t e = cudaSuccess;
+    if (live > 0) {
+        const unsigned grid = (unsigned)c->sm_count * 8;
+        if (ix->d % 4 == 0)
+            index_compact_rows_kernel<<<grid, 256, 0, c->stream>>>(reinterpret_cast<const float4 *>(ix->X.p), ix->n, ix->d / 4, scan,
+                                                                   reinterpret_cast<float4 *>(nx.p));
+        else
+            index_compact_rows_kernel<<<grid, 256, 0, c->stream>>>(ix->X.p, ix->n, ix->d, scan, nx.p);
+        c->launches++;
+        e = cudaGetLastError();
+    }
+    if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
+    if (e != cudaSuccess) {
+        set_error("compact: %s", cudaGetErrorString(e));
+        nx.free();
+        return GORSE_B200_ERR_CUDA;
+    }
+    ix->X.free();
+    ix->X = nx;
+    ix->n = ix->cap = live;
+    ix->mma_ready = false;   // the next sweep rebuilds the mirror, norms and permutation for the new n
+    ix->Xb.free(); ix->norm.free(); ix->perm.free();
+    ix->recall.scratch.free();   // [N] per exact CTA
+    ix->last_fallback_rows = 0;
+    ix->stage1_ms = ix->stage1_flop = 0.0;
+    return GORSE_B200_OK;
+}
+
+size_t index_bytes(const gorse_b200_index *ix)
+{
+    return ix->X.bytes() + ix->Xb.bytes() + ix->norm.bytes() + ix->perm.bytes() + ix->w_qb.bytes() + ix->w_eps.bytes() + ix->w_cval.bytes() +
+           ix->w_theta.bytes() + ix->w_ccol.bytes() + ix->w_ccnt.bytes() + ix->recall.bytes() + ix->r_idx.bytes() + ix->r_count.bytes() +
+           ix->r_dist.bytes();
+}
+
 }  // namespace gb
 
 using namespace gb;

@@ -21,6 +21,11 @@ struct RecallWork {
         ex_off.free(); ex.free(); out_off.free(); rows.free(); slots.free();
         k.free(); count.free(); flags.free();
     }
+    size_t bytes() const
+    {
+        return q.bytes() + scores.bytes() + scratch.bytes() + ex_off.bytes() + ex.bytes() + out_off.bytes() + rows.bytes() + slots.bytes() +
+               k.bytes() + count.bytes() + flags.bytes();
+    }
 };
 }  // namespace gb
 
@@ -151,6 +156,13 @@ __device__ __forceinline__ float key_float(uint32_t k)
 #endif  // __CUDACC__
 
 int32_t index_reserve(gorse_b200_index *ix, int64_t need);
+// compaction (gorse_b200_vecdb_compact): scan[n + 1] (device) is the exclusive sum of the live flags, so slot s is live iff
+// scan[s + 1] != scan[s] and then moves to scan[s]; X becomes the live rows in order, live = scan[n] of them, with cap = live,
+// and everything built from the old rows (mirror, norms, permutation, exact scratch, stage-1 counters) is dropped.  On an
+// error the index is unchanged.  The caller holds ix->mu.
+int32_t index_compact(gorse_b200_index *ix, const int64_t *scan, int64_t live);
+// device bytes held by the index and its work buffers
+size_t index_bytes(const gorse_b200_index *ix);
 // the tensor-core candidate sweep (topk_mma.cu) of the top-k pipeline (recall_rows) and of the stage-1 test hook.
 // mma_reserve: the bf16 mirror and the work buffers for up to cq query rows per sweep.  mma_sample_tiles: the sample size
 // that leaves about `cands` columns per row above its threshold.  mma_sweep: query rows (q_base, d_q, d_qidx, q0 as in

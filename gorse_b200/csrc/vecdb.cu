@@ -16,6 +16,8 @@
 // string <-> int32 map, the library works on slots (int64, in insertion order) and category ids.
 #include <algorithm>
 
+#include <cub/cub.cuh>
+
 #include "cf.cuh"
 #include "sparse.cuh"
 #include "vecdb.cuh"
@@ -58,6 +60,20 @@ __global__ void vecdb_copy_rows_kernel(const float *Q, int d4, const int32_t *it
         const int64_t s = i / d4, c = i - s * d4;
         reinterpret_cast<float4 *>(X)[s * d4 + c] = reinterpret_cast<const float4 *>(Q)[(int64_t)items[s] * d4 + c];
     }
+}
+
+// flag[s] = 1 for a live slot, flag[n] = 0: the input of the exclusive scan that renumbers the slots
+__global__ void vecdb_live_kernel(const uint8_t *dead, int64_t n, int64_t *flag)
+{
+    const int64_t st = (int64_t)gridDim.x * blockDim.x;
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i <= n; i += st) flag[i] = i < n && dead[i] == 0;
+}
+
+// device bytes held by the collection, its index and its work buffers
+static int64_t vecdb_bytes(const gorse_b200_vecdb *db)
+{
+    return (int64_t)(db->d_blocked.bytes() + db->d_allow.bytes() + db->d_cat_off.bytes() + db->d_cats.bytes() + db->d_want.bytes() +
+                     db->i2i.bytes() + db->u2u.bytes() + (db->dense ? index_bytes(db->dense) : sparse_bytes(db->sparse)));
 }
 
 static int32_t sync_meta(gorse_b200_vecdb *db)
@@ -238,6 +254,69 @@ int32_t gorse_b200_vecdb_delete_before(gorse_b200_vecdb *db, int64_t timestamp_m
     if (cnt) db->meta_dirty = true;
     if (count_out) *count_out = cnt;
     return GORSE_B200_OK;
+}
+
+// Optimize (storage/vectors/database.go:109; xvec.go:125-131).  The live flags are scanned on the device; the scan is the
+// renumbering, which the index applies to its own rows (index_compact, sparse_compact) and the host applies to the metadata.
+// Every new buffer, device or host, exists before anything of the collection changes.
+int32_t gorse_b200_vecdb_compact(gorse_b200_vecdb *db, int64_t *new_slot_out, int64_t *bytes_out)
+{
+    GB_CHECK_ARG(db != nullptr, "collection is NULL");
+    std::lock_guard<std::mutex> lk(db->mu);
+    std::lock_guard<std::mutex> lk2(db->dense ? db->dense->mu : db->sparse->mu);
+    const int64_t n = (int64_t)db->ts.size(), live = db->live;
+    if (bytes_out) bytes_out[0] = bytes_out[1] = vecdb_bytes(db);
+    if (live == n) {   // nothing to reclaim
+        if (new_slot_out)
+            for (int64_t s = 0; s < n; s++) new_slot_out[s] = s;
+        return GORSE_B200_OK;
+    }
+    gorse_b200_ctx *c = db->ctx;
+    ScopedDevice sd(c->device);
+    DevBuf<uint8_t> d_dead, tmp;
+    DevBuf<int64_t> scan;
+    auto done = [&](int32_t st) { cudaStreamSynchronize(c->stream); d_dead.free(); tmp.free(); scan.free(); return st; };
+    int32_t st;
+    if ((st = d_dead.alloc((size_t)n)) || (st = scan.alloc((size_t)n + 1))) return done(st);
+    size_t tmp_bytes = 0;
+    cudaError_t e = cudaMemcpyAsync(d_dead.p, db->dead.data(), (size_t)n, cudaMemcpyHostToDevice, c->stream);
+    if (e == cudaSuccess) {
+        vecdb_live_kernel<<<div_up(n + 1, 256), 256, 0, c->stream>>>(d_dead.p, n, scan.p);
+        c->launches++;
+        e = cudaGetLastError();
+    }
+    if (e == cudaSuccess) e = cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, scan.p, n + 1, c->stream);
+    if (e != cudaSuccess) { set_error("compact: %s", cudaGetErrorString(e)); return done(GORSE_B200_ERR_CUDA); }
+    if ((st = tmp.alloc(tmp_bytes))) return done(st);
+    std::vector<int64_t> new_slot((size_t)n + 1);
+    e = cub::DeviceScan::ExclusiveSum(tmp.p, tmp_bytes, scan.p, n + 1, c->stream);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(new_slot.data(), scan.p, sizeof(int64_t) * ((size_t)n + 1), cudaMemcpyDeviceToHost, c->stream);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
+    if (e != cudaSuccess) { set_error("compact: %s", cudaGetErrorString(e)); return done(GORSE_B200_ERR_CUDA); }
+    // the compacted host metadata
+    std::vector<uint8_t> hidden((size_t)live), dead((size_t)live, 0);
+    std::vector<int64_t> ts((size_t)live), cat_off((size_t)live + 1, 0);
+    std::vector<int32_t> cats;
+    cats.reserve(db->cats.size());
+    for (int64_t s = 0; s < n; s++) {
+        if (db->dead[(size_t)s]) continue;
+        const size_t to = (size_t)new_slot[(size_t)s];
+        hidden[to] = db->hidden[(size_t)s];
+        ts[to] = db->ts[(size_t)s];
+        cats.insert(cats.end(), db->cats.begin() + db->cat_off[(size_t)s], db->cats.begin() + db->cat_off[(size_t)s + 1]);
+        cat_off[to + 1] = (int64_t)cats.size();
+    }
+    if ((st = db->dense ? index_compact(db->dense, scan.p, live) : sparse_compact(db->sparse, scan.p, live))) return done(st);
+    db->hidden.swap(hidden); db->dead.swap(dead); db->ts.swap(ts); db->cat_off.swap(cat_off); db->cats.swap(cats);
+    db->meta_dirty = true;
+    // every device buffer whose size follows the slot count; the next call that needs one allocates (and zeroes) it again
+    db->d_blocked.free(); db->d_allow.free(); db->d_cat_off.free(); db->d_cats.free();
+    db->i2i.acc.free(); db->i2i.seen.free(); db->i2i.touched.free(); db->i2i.item_ok.free();
+    db->u2u.acc.free(); db->u2u.flag.free(); db->u2u.touched.free();
+    if (new_slot_out)   // `dead` holds the old flags after the swap
+        for (int64_t s = 0; s < n; s++) new_slot_out[s] = dead[(size_t)s] ? -1 : new_slot[(size_t)s];
+    if (bytes_out) bytes_out[1] = vecdb_bytes(db);
+    return done(GORSE_B200_OK);
 }
 
 int32_t gorse_b200_vecdb_query(gorse_b200_vecdb *db, int64_t nq, const float *q_values, const int64_t *q_sp_off, const uint32_t *q_sp_indices,

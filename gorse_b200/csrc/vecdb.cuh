@@ -20,6 +20,11 @@ struct ItemToItemWork {
         t_slot.free(); t_cnt.free(); c_row.free(); users.free(); count.free();
         t_score.free(); scores.free(); acc.free(); seen.free(); item_ok.free(); touched.free();
     }
+    size_t bytes() const
+    {
+        return nb.bytes() + c_off.bytes() + ex_off.bytes() + ex.bytes() + slots.bytes() + t_slot.bytes() + t_cnt.bytes() + c_row.bytes() +
+               users.bytes() + count.bytes() + t_score.bytes() + scores.bytes() + acc.bytes() + seen.bytes() + item_ok.bytes() + touched.bytes();
+    }
 };
 
 // grow-only work buffers of gorse_b200_vecdb_user_to_user (user_to_user.cu): the neighbour table of stage A, the caller's
@@ -35,6 +40,12 @@ struct UserToUserWork {
         nb.free(); fb_off.free(); ex_off.free(); ex.free(); items.free();
         t_slot.free(); t_cnt.free(); fb_items.free(); q_row.free(); list.free(); work.free(); route_cnt.free(); count.free(); flag.free(); touched.free();
         item_ok.free(); t_score.free(); scores.free(); acc.free();
+    }
+    size_t bytes() const
+    {
+        return nb.bytes() + fb_off.bytes() + ex_off.bytes() + ex.bytes() + items.bytes() + t_slot.bytes() + t_cnt.bytes() + fb_items.bytes() +
+               q_row.bytes() + list.bytes() + work.bytes() + route_cnt.bytes() + count.bytes() + flag.bytes() + touched.bytes() +
+               item_ok.bytes() + t_score.bytes() + scores.bytes() + acc.bytes();
     }
 };
 }  // namespace gb

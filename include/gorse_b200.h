@@ -382,6 +382,18 @@ int32_t gorse_b200_vecdb_get_sparse(gorse_b200_vecdb *db, int64_t slot, uint32_t
 /* DeleteVectors(timestamp) (xvec.go:365-371): tombstones live vectors with timestamp < timestamp_ms; the first `cap` deleted
  * slots are written to slots_out (the shim drops their ids), *count_out = how many were deleted */
 int32_t gorse_b200_vecdb_delete_before(gorse_b200_vecdb *db, int64_t timestamp_ms, int64_t *slots_out, int64_t cap, int64_t *count_out);
+/* Optimize (storage/vectors/database.go:109; xvec.go:125-131): reclaim the slots of deleted vectors, whether an upsert or
+ * gorse_b200_vecdb_delete_before tombstoned them.  Live slots keep their order and become 0 .. live-1; later adds append
+ * after them.  new_slot_out[slots] (slots = what gorse_b200_vecdb_count reported before the call; may be NULL): the new slot
+ * of every old slot, -1 for a deleted one.  bytes_out[2] (may be NULL): device bytes held by the collection before and
+ * after -- its own buffers, its index's and its work buffers' (not the context's gorse_b200_recommend buffers).  Every
+ * entry answers afterwards exactly what it answered before, with slots renamed through new_slot_out and the same score
+ * bits: each score is computed per (query, vector) pair with no position in the arithmetic, and every exact tie is ordered
+ * by slot or item index, which the renaming preserves.  (The tensor-core sweep samples by the vector count, so it may hand
+ * other rows to the exact scan; the answer does not depend on that.)  Nothing to reclaim: identity, no device work.  On
+ * any error the collection is unchanged.  Slots held by the caller (id maps, context and exclusion lists, per-slot
+ * feedback rows and masks) must be renamed before they are passed again.  NULL db: GORSE_B200_ERR_ARG. */
+int32_t gorse_b200_vecdb_compact(gorse_b200_vecdb *db, int64_t *new_slot_out, int64_t *bytes_out);
 /* QueryVectors (xvec.go:373-449) for nq query vectors sharing one category filter: candidates are live, not hidden and
  * carry ALL of categories[n_categories] (CONTAIN_ALL, :381-389).  Results per query: slots_out / scores_out [nq x topk],
  * best first, count_out[nq]; entries past count_out[q] in a row are not part of the answer and are left unspecified; score = dot (Dot) or the NEGATED distance (Euclidean, Cosine) -- higher is more similar
