@@ -505,9 +505,7 @@ class VectorCollection:
         nq = qv.shape[0]
         if len(exclude_lists) != nq:
             raise ValueError(f"{len(exclude_lists)} exclude lists for {nq} queries")
-        off = np.zeros(nq + 1, np.int64)
-        np.cumsum([len(e) for e in exclude_lists], out=off[1:])
-        ex = np.ascontiguousarray(np.concatenate([np.asarray(e, np.int64).reshape(-1) for e in exclude_lists]) if nq else [], np.int64)
+        off, ex = _flat(exclude_lists, np.int64)
         cats = np.ascontiguousarray(list(categories), np.int32)
         total = nq * max(n, 0) + int(off[-1])
         slots, scores, cnt = np.full(max(total, 1), -1, np.int64), np.zeros(max(total, 1), np.float32), np.zeros(nq, np.int32)
@@ -525,15 +523,8 @@ class VectorCollection:
         nu = len(context_lists)
         if len(exclude_lists) != nu:
             raise ValueError(f"{len(exclude_lists)} exclude lists for {nu} users")
-
-        def csr(lists):
-            off = np.zeros(nu + 1, np.int64)
-            np.cumsum([len(x) for x in lists], out=off[1:])
-            flat = np.ascontiguousarray(np.concatenate([np.asarray(x, np.int64).reshape(-1) for x in lists]) if nu else [], np.int64)
-            return off, flat
-
-        coff, cs = csr(context_lists)
-        eoff, es = csr(exclude_lists)
+        coff, cs = _flat(context_lists, np.int64)
+        eoff, es = _flat(exclude_lists, np.int64)
         cats = np.ascontiguousarray(list(categories), np.int32)
         m = max(n, 0)
         slots, scores, cnt = np.full(max(nu * m, 1), -1, np.int64), np.zeros(max(nu * m, 1), np.float64), np.zeros(max(nu, 1), np.int32)
@@ -556,12 +547,8 @@ class VectorCollection:
         if len(exclude_lists) != nu:
             raise ValueError(f"{len(exclude_lists)} exclude lists for {nu} users")
         nf = len(feedback_lists)
-        foff = np.zeros(nf + 1, np.int64)
-        np.cumsum([len(x) for x in feedback_lists], out=foff[1:])
-        fitems = np.ascontiguousarray(np.concatenate([np.asarray(x, np.int32).reshape(-1) for x in feedback_lists]) if nf else [], np.int32)
-        eoff = np.zeros(nu + 1, np.int64)
-        np.cumsum([len(x) for x in exclude_lists], out=eoff[1:])
-        es = np.ascontiguousarray(np.concatenate([np.asarray(x, np.int64).reshape(-1) for x in exclude_lists]) if nu else [], np.int64)
+        foff, fitems = _flat(feedback_lists, np.int32)
+        eoff, es = _flat(exclude_lists, np.int64)
         ok = None if item_ok is None else np.ascontiguousarray(item_ok, np.uint8)
         if ok is not None and ok.size != n_items:
             raise ValueError(f"item_ok has {ok.size} entries for {n_items} items")
@@ -585,15 +572,8 @@ class VectorCollection:
         ns = len(context_lists)
         if len(exclude_lists) != ns:
             raise ValueError(f"{len(exclude_lists)} exclude lists for {ns} sessions")
-
-        def csr(lists):
-            off = np.zeros(ns + 1, np.int64)
-            np.cumsum([len(x) for x in lists], out=off[1:])
-            flat = np.ascontiguousarray(np.concatenate([np.asarray(x, np.int64).reshape(-1) for x in lists]) if ns else [], np.int64)
-            return off, flat
-
-        coff, cs = csr(context_lists)
-        eoff, es = csr(exclude_lists)
+        coff, cs = _flat(context_lists, np.int64)
+        eoff, es = _flat(exclude_lists, np.int64)
         ok = None
         if item_ok is not None:
             ok = np.ascontiguousarray(item_ok, np.uint8)

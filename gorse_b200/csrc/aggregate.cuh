@@ -1,6 +1,7 @@
-// aggregate.cuh -- what the batched recommenders' aggregation kernels share (item_to_item.cu, user_to_user.cu,
-// session.cu): the neighbour score transform, the shared-memory layout of one aggregating CTA, the float64 sum per id, and
-// the selection of the first n float64 sums by (sum descending, id ascending).
+// aggregate.cuh -- what the batched recommenders' two aggregation kernels share (i2i_aggregate_kernel in item_to_item.cu,
+// for item-to-item and session; u2u_aggregate_kernel in user_to_user.cu): the neighbour score transform, the shared-memory
+// layout of one aggregating CTA, the float64 sum per id, and the selection of the first n float64 sums by (sum descending,
+// id ascending).
 #pragma once
 #include "recall.cuh"
 

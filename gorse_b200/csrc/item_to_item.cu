@@ -1,20 +1,26 @@
-// item_to_item.cu -- batched item-to-item recommendation: gorse_b200_vecdb_item_to_item.
+// item_to_item.cu -- batched item-to-item and session recommendation: gorse_b200_vecdb_item_to_item and
+// gorse_b200_vecdb_session_recommend.
 //
 // The worker's item-to-item recommender (logics/recommend.go:244-283) asks, per user, QueryItemToItem(c, categories, n) for
 // every positive feedback item c, newest first (logics/item_to_item.go:50-86: top n + 1, drop c itself, drop Dot scores <= 0,
-// stop at n), sums the neighbour scores per item id in float64, skipping the user's exclude set, and keeps the best n.  Here
-// one call answers many users:
+// stop at n), sums the neighbour scores per item id in float64, skipping the user's exclude set, and keeps the best n.  The
+// REST server's session recommendation (sessionRecommend, server/rest.go:1069-1173) does the same with no category filter,
+// keeps the neighbours that FilterVisibleItemsByCategories passes (rest.go:815-832), stops once ContextSize items have given
+// a non-empty filtered list, and answers TopKFilter(n + offset).  Here one call answers many users or sessions:
 //
 //   stage A   the neighbour table, once per call: the distinct live context items of the whole batch are queried once each.
 //             Dense collections run the index's top-k pipeline (recall_rows, topk.cu) with k = n on the stored vectors (a
 //             row never returns its own vector), and its table keeps Dot scores > 0 only.  Sparse collections run
 //             sparse_search_kernel on the list of stored rows (a row never finds itself; it keeps positive dots only).
 //             The table holds n (int32 slot, float32 score) entries per item, scores bit-identical to gorse_b200_vecdb_query.
-//   stage B   i2i_aggregate_kernel, one CTA per user: walks C_u in order and adds s = (double)score * scale (Euclidean:
-//             1 / (1 - s)) per neighbour slot not in E_u, with a barrier between context entries so that every sum is formed
-//             in the reference's order; then selects the first n by (score desc, slot asc) with a 64-bit radix select and
-//             sorts them (agg::select_first_n, aggregate.cuh, shared with user_to_user.cu).  The accumulator is an open-addressing table in shared memory when |C_u| * n <= TABLE_KEYS, else
-//             this CTA's float64 row of length N in global memory, with a touched flag per slot and the list of touched slots.
+//             A session's walk cannot stop at its cut here: whether an entry counts depends on its filtered list.
+//   stage B   i2i_aggregate_kernel, one CTA per user: for a session, first the cut (context_cut); then walks C_u (the
+//             session's prefix) in order and adds s = (double)score * scale (Euclidean: 1 / (1 - s)) per neighbour slot that
+//             item_ok passes and that is not in E_u, with a barrier between context entries so that every sum is formed in
+//             the reference's order; then selects the first n (session: top) by (score desc, slot asc) with a 64-bit radix
+//             select and sorts them (agg::select_first_n, aggregate.cuh).  The accumulator is an open-addressing table in
+//             shared memory when |C_u| * n <= TABLE_KEYS, else this CTA's float64 row of length N in global memory, with a
+//             touched flag per slot and the list of touched slots.
 #include <algorithm>
 
 #include "sparse.cuh"
@@ -24,21 +30,78 @@ namespace gb {
 namespace i2i {
 
 using agg::TABLE_CAP;
-using agg::TABLE_KEYS;                           // a user takes the table when |C_u| * n <= this
 constexpr int AGG_THREADS = agg::THREADS;
 
+// One past the context entry e of [cb, ce) at which the count of entries with a non-empty filtered neighbour list reaches
+// need, or ce when it never does.  Each window of NT entries: warp w tests entries w*32 .. w*32+31, its lanes splitting each
+// list (__any_sync, stopping at the first passing neighbour), and records them as one bit mask; warp 0 scans the window's
+// masks and picks the entry.  Every thread of the CTA calls it.
+template <int NT>
+__device__ int64_t context_cut(int64_t cb, int64_t ce, const int32_t *c_row, const NeighbourTable &T, int n, const uint8_t *item_ok, int need,
+                               unsigned *s_mask, int64_t *s_cut)
+{
+    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+    for (int64_t base = cb; base < ce; base += NT) {
+        unsigned mask = 0;
+        for (int i = 0; i < 32; i++) {
+            const int64_t e = base + w * 32 + i;
+            if (e >= ce) break;
+            const int64_t r = c_row[e];
+            const int cnt = T.cnt[r];
+            bool any = item_ok == nullptr && cnt > 0;
+            for (int j0 = 0; item_ok != nullptr && !any && j0 < cnt; j0 += 32) {
+                const int j = j0 + lane;
+                any = __any_sync(0xffffffffu, j < cnt && item_ok[T.slot[r * n + j]]);
+            }
+            mask |= (unsigned)any << i;
+        }
+        if (lane == 0) s_mask[w] = mask;
+        __syncthreads();
+        if (w == 0) {
+            const unsigned m = lane < NT / 32 ? s_mask[lane] : 0u;
+            const int c = __popc(m);
+            int incl = c;
+#pragma unroll
+            for (int o = 1; o < 32; o <<= 1) {
+                const int t = __shfl_up_sync(0xffffffffu, incl, o);
+                if (lane >= o) incl += t;
+            }
+            const unsigned hit = __ballot_sync(0xffffffffu, incl >= need);
+            if (hit == 0u) {
+                if (lane == 0) *s_cut = -1;
+            } else if (lane == __ffs(hit) - 1) {
+                unsigned b = m;   // the (need - before)-th set bit of this lane's mask
+                for (int k = need - (incl - c); k > 1; k--) b &= b - 1;
+                *s_cut = base + lane * 32 + __ffs(b);
+            }
+        }
+        __syncthreads();
+        const int64_t cut = *s_cut;
+        if (cut >= 0) return cut;
+#pragma unroll
+        for (int i = 0; i < NT / 32; i++) need -= __popc(s_mask[i]);
+        __syncthreads();   // s_mask and s_cut are rewritten by the next window
+    }
+    return ce;
+}
+
 // one CTA per user of `users`.  SHARED: the accumulator is a table in shared memory; else acc_rows / seen_rows /
-// touched_rows hold one [N] float64 row, one [N] flag row (all zero between users) and one [N] slot list per CTA.
-template <bool SHARED>
+// touched_rows hold one [N] float64 row, one [N] flag row (all zero between users) and one [N] slot list per CTA.  CUT
+// (session): the walk stops at context_cut's entry for need and skips the neighbours that item_ok (a slot mask or NULL) does
+// not pass; else it takes the whole context, and item_ok and need are not read.  Row u of the answer is U.slots / U.scores
+// [u * top, u * top + U.count[u]); the table's rows hold n entries.
+template <bool SHARED, bool CUT>
 __global__ void __launch_bounds__(AGG_THREADS)
-i2i_aggregate_kernel(const int32_t *users, int64_t n_users, Users U, Table T, int n, double scale, int euclid, int64_t N, double *acc_rows,
-                     uint8_t *seen_rows, int32_t *touched_rows)
+i2i_aggregate_kernel(const int32_t *users, int64_t n_users, Users U, NeighbourTable T, const uint8_t *item_ok, int n, int need, int top,
+                     double scale, int euclid, int64_t N, double *acc_rows, uint8_t *seen_rows, int32_t *touched_rows)
 {
     using namespace gb::recall;
     using namespace gb::agg;
     constexpr int NT = AGG_THREADS;
     extern __shared__ __align__(16) uint8_t sm[];
-    const int p2 = pow2_at_least(n);
+    __shared__ unsigned s_mask[NT / 32];
+    __shared__ int64_t s_cut;
+    const int p2 = pow2_at_least(top);
     const Smem S = carve(sm, p2);
     int *s_bc = S.s_bc;                                            // [3]: distinct slots
     int32_t *t_key = S.t_key;                                      // SHARED: slot, -1 = empty
@@ -48,10 +111,11 @@ i2i_aggregate_kernel(const int32_t *users, int64_t n_users, Users U, Table T, in
     int32_t *touched = SHARED ? nullptr : touched_rows + (int64_t)blockIdx.x * N;
     for (int64_t i = blockIdx.x; i < n_users; i += gridDim.x) {
         const int64_t u = users[i];
-        const int64_t cb = U.c_off[u], ce = U.c_off[u + 1];
+        const int64_t cb = U.c_off[u];
+        const int64_t ce = CUT ? context_cut<NT>(cb, U.c_off[u + 1], U.c_row, T, n, item_ok, need, s_mask, &s_cut) : U.c_off[u + 1];
         const int64_t *ex = U.ex + U.ex_off[u], n_ex = U.ex_off[u + 1] - U.ex_off[u];
         int cap = 0, lg = 0;
-        if (SHARED) {   // a power of two >= 2 |C_u| n, at most TABLE_CAP: the load stays <= 3/4
+        if (SHARED) {   // a power of two >= 2 * (the walk's adds), at most TABLE_CAP: the load stays <= 3/4
             cap = min(TABLE_CAP, pow2_at_least(max(64, (int)(2 * (ce - cb) * n))));
             lg = __ffs(cap) - 1;
             for (int j = threadIdx.x; j < cap; j += NT) t_key[j] = -1;
@@ -65,7 +129,7 @@ i2i_aggregate_kernel(const int32_t *users, int64_t n_users, Users U, Table T, in
             const int cnt = T.cnt[r];
             for (int j = threadIdx.x; j < cnt; j += NT) {
                 const int32_t slot = T.slot[r * n + j];
-                if (contains(ex, n_ex, (int64_t)slot)) continue;
+                if ((CUT && item_ok != nullptr && !item_ok[slot]) || contains(ex, n_ex, (int64_t)slot)) continue;
                 add_sum<SHARED>(slot, neighbour_score(T.score[r * n + j], scale, euclid), t_key, t_val, cap, lg, acc, seen, touched, &s_bc[3]);
             }
             __syncthreads();
@@ -73,10 +137,10 @@ i2i_aggregate_kernel(const int32_t *users, int64_t n_users, Users U, Table T, in
         const int distinct = s_bc[3];
         auto slot_at = [&](int64_t j) -> int32_t { return SHARED ? t_key[j] : touched[j]; };
         auto val_at = [&](int64_t j) -> double { return SHARED ? t_val[j] : acc[touched[j]]; };
-        const int m = select_first_n<NT>(SHARED ? cap : distinct, distinct, n, p2, slot_at, val_at, S);
+        const int m = select_first_n<NT>(SHARED ? cap : distinct, distinct, top, p2, slot_at, val_at, S);
         for (int j = threadIdx.x; j < m; j += NT) {
-            U.slots[u * n + j] = (int64_t)(uint32_t)S.s_key[j];
-            U.scores[u * n + j] = S.s_val[j];
+            U.slots[u * top + j] = (int64_t)(uint32_t)S.s_key[j];
+            U.scores[u * top + j] = S.s_val[j];
         }
         if (threadIdx.x == 0) U.count[u] = m;
         if (!SHARED)
@@ -85,24 +149,140 @@ i2i_aggregate_kernel(const int32_t *users, int64_t n_users, Users U, Table T, in
     }
 }
 
-int32_t aggregate(gorse_b200_ctx *c, const int32_t *d_users, int64_t fill, int64_t heavy, const Users &U, const Table &T, int n, double scale,
-                  bool euclid, int64_t N, double *acc, uint8_t *seen, int32_t *touched)
+int32_t aggregate(gorse_b200_ctx *c, const int32_t *d_users, int64_t fill, int64_t heavy, const Users &U, const NeighbourTable &T,
+                  const uint8_t *item_ok, int n, int need, int top, double scale, bool euclid, int64_t N, double *acc, uint8_t *seen,
+                  int32_t *touched)
 {
-    const size_t sm_shared = agg::smem_bytes(n, true), sm_global = agg::smem_bytes(n, false);
-    GB_CUDA(cudaFuncSetAttribute(i2i_aggregate_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm_shared));
-    GB_CUDA(cudaFuncSetAttribute(i2i_aggregate_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm_global));
+    // item-to-item (need <= 0) runs the instances without the cut and the item_ok test
+    auto *k_shared = need > 0 ? i2i_aggregate_kernel<true, true> : i2i_aggregate_kernel<true, false>;
+    auto *k_global = need > 0 ? i2i_aggregate_kernel<false, true> : i2i_aggregate_kernel<false, false>;
+    const size_t sm_shared = agg::smem_bytes(top, true), sm_global = agg::smem_bytes(top, false);
+    GB_CUDA(cudaFuncSetAttribute(k_shared, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm_shared));
+    GB_CUDA(cudaFuncSetAttribute(k_global, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm_global));
     if (fill > 0) {
-        i2i_aggregate_kernel<true><<<(unsigned)std::min<int64_t>(fill, (int64_t)c->sm_count * 8), AGG_THREADS, sm_shared, c->stream>>>(
-            d_users, fill, U, T, n, scale, euclid, N, nullptr, nullptr, nullptr);
+        k_shared<<<(unsigned)std::min<int64_t>(fill, (int64_t)c->sm_count * 8), AGG_THREADS, sm_shared, c->stream>>>(
+            d_users, fill, U, T, item_ok, n, need, top, scale, euclid, N, nullptr, nullptr, nullptr);
         c->launches++;
     }
     if (heavy > 0) {
-        i2i_aggregate_kernel<false><<<(unsigned)std::min<int64_t>(heavy, heavy_grid(c, N)), AGG_THREADS, sm_global, c->stream>>>(
-            d_users + fill, heavy, U, T, n, scale, euclid, N, acc, seen, touched);
+        k_global<<<(unsigned)std::min<int64_t>(heavy, heavy_grid(c, N, ROW_BYTES)), AGG_THREADS, sm_global, c->stream>>>(
+            d_users + fill, heavy, U, T, item_ok, n, need, top, scale, euclid, N, acc, seen, touched);
         c->launches++;
     }
     GB_CUDA(cudaGetLastError());
     return GORSE_B200_OK;
+}
+
+// Both vecdb entries after their own checks: the caller holds db->mu, every context slot is in [-1, slots) and ex / ex_off
+// are the checked exclusion rows.  categories: the neighbour query's filter; item_ok, need, top: aggregate's.
+int32_t neighbour_sums(gorse_b200_vecdb *db, const char *name, int64_t n_users, const int64_t *ctx_off, const int64_t *ctx_slots,
+                       const std::vector<int64_t> &ex, const std::vector<int64_t> &ex_off, const int32_t *categories, int32_t n_categories,
+                       const uint8_t *item_ok, int n, int need, int top, double score_scale, int64_t *slots_out, double *scores_out,
+                       int32_t *count_out, int64_t *stats_out)
+{
+    using gb::agg::grow_zeroed;
+    using gb::recall::grow;
+    const int64_t n_slots = (int64_t)db->ts.size();
+    // the live context entries of every user as rows of the neighbour table.  -1 and deleted slots are skipped (GetVectors
+    // returns nothing, logics/item_to_item.go:56-58) and never count for a session; hidden ones are queried.
+    std::vector<int32_t> row_of((size_t)n_slots, -1), c_row;
+    std::vector<int64_t> nb, c_off((size_t)n_users + 1, 0);
+    c_row.reserve((size_t)ctx_off[n_users]);
+    for (int64_t u = 0; u < n_users; u++) {
+        for (int64_t t = ctx_off[u]; t < ctx_off[u + 1]; t++) {
+            const int32_t r = table_row(db, ctx_slots[t], row_of, nb);
+            if (r >= 0) c_row.push_back(r);
+        }
+        c_off[(size_t)u + 1] = (int64_t)c_row.size();
+    }
+    const int64_t R = (int64_t)nb.size();
+    if (R == 0) {
+        std::fill(count_out, count_out + n_users, 0);
+        return GORSE_B200_OK;
+    }
+    gorse_b200_ctx *c = db->ctx;
+    ScopedDevice sd(c->device);
+    GB_TRY(vecdb_allow(db, categories, n_categories));
+    ItemToItemWork &V = db->i2i;
+    int32_t st = GORSE_B200_OK;
+    auto done = [&](int32_t s) {
+        cudaStreamSynchronize(c->stream);
+        cudaStreamSynchronize(c->copy_stream);
+        return s;
+    };
+    if ((st = grow(V.nb, (size_t)R)) || (st = grow(V.t_slot, (size_t)R * n)) || (st = grow(V.t_score, (size_t)R * n)) || (st = grow(V.t_cnt, (size_t)R)) ||
+        (item_ok && (st = grow(V.item_ok, (size_t)n_slots))))
+        return done(st);
+    cudaError_t e = cudaMemcpyAsync(V.nb.p, nb.data(), sizeof(int64_t) * R, cudaMemcpyHostToDevice, c->stream);
+    if (e == cudaSuccess && item_ok) e = cudaMemcpyAsync(V.item_ok.p, item_ok, (size_t)n_slots, cudaMemcpyHostToDevice, c->stream);
+    if (e != cudaSuccess) { set_error("%s upload: %s", name, cudaGetErrorString(e)); return done(GORSE_B200_ERR_CUDA); }
+
+    // ---- stage A: the neighbour table
+    int64_t exact_rows = 0;
+    if ((st = neighbour_table(db, R, V.nb.p, n, V.t_slot.p, V.t_score.p, V.t_cnt.p, &exact_rows))) return done(st);
+    if ((e = cudaGetLastError()) != cudaSuccess) { set_error("%s: %s", name, cudaGetErrorString(e)); return done(GORSE_B200_ERR_CUDA); }
+
+    // ---- stage B: users in chunks; a finished chunk is downloaded on the copy stream while the next one computes
+    const int64_t cu = std::min<int64_t>(n_users, (int64_t)c->sm_count * 1024);
+    const int64_t N = n_slots;
+    const int hg = heavy_grid(c, N, ROW_BYTES);
+    const int64_t total_ctx = c_off[(size_t)n_users];
+    if ((st = grow(V.c_off, (size_t)cu + 1)) || (st = grow(V.ex_off, (size_t)cu + 1)) || (st = grow(V.users, (size_t)cu)) ||
+        (st = grow(V.c_row, (size_t)std::max<int64_t>(total_ctx, 1))) || (st = grow(V.ex, std::max<size_t>(ex.size(), 1))) ||
+        (st = grow(V.slots, (size_t)n_users * top)) || (st = grow(V.scores, (size_t)n_users * top)) || (st = grow(V.count, (size_t)n_users)))
+        return done(st);
+    const NeighbourTable T{V.t_slot.p, V.t_score.p, V.t_cnt.p};
+    const bool euclid = db->distance == GORSE_B200_DISTANCE_EUCLIDEAN;
+    const uint8_t *d_ok = item_ok ? V.item_ok.p : nullptr;
+    int64_t n_shared = 0, n_heavy = 0;
+    std::vector<int64_t> h_coff, h_exoff;
+    std::vector<int32_t> h_users;
+    for (int64_t u0 = 0; u0 < n_users; u0 += cu) {
+        const int64_t rows = std::min(cu, n_users - u0);
+        h_coff.resize(rows + 1); h_exoff.resize(rows + 1);
+        for (int64_t r = 0; r <= rows; r++) {
+            h_coff[r] = c_off[u0 + r] - c_off[u0];
+            h_exoff[r] = ex_off[u0 + r] - ex_off[u0];
+        }
+        const int64_t fill = route(h_coff.data(), rows, n, h_users);
+        n_shared += fill;
+        n_heavy += rows - fill;
+        if (rows - fill > 0 && ((st = grow(V.acc, (size_t)hg * N)) || (st = grow_zeroed(V.seen, (size_t)hg * N, c->stream)) ||
+                                (st = grow(V.touched, (size_t)hg * N))))
+            return done(st);
+        const int64_t n_c = h_coff[rows], n_e = h_exoff[rows];
+        if ((e = cudaMemcpyAsync(V.c_off.p, h_coff.data(), sizeof(int64_t) * (rows + 1), cudaMemcpyHostToDevice, c->stream)) != cudaSuccess ||
+            (e = cudaMemcpyAsync(V.ex_off.p, h_exoff.data(), sizeof(int64_t) * (rows + 1), cudaMemcpyHostToDevice, c->stream)) != cudaSuccess ||
+            (e = cudaMemcpyAsync(V.users.p, h_users.data(), sizeof(int32_t) * rows, cudaMemcpyHostToDevice, c->stream)) != cudaSuccess ||
+            (n_c && (e = cudaMemcpyAsync(V.c_row.p + c_off[u0], c_row.data() + c_off[u0], sizeof(int32_t) * n_c, cudaMemcpyHostToDevice, c->stream)) != cudaSuccess) ||
+            (n_e && (e = cudaMemcpyAsync(V.ex.p + ex_off[u0], ex.data() + ex_off[u0], sizeof(int64_t) * n_e, cudaMemcpyHostToDevice, c->stream)) != cudaSuccess)) {
+            set_error("%s upload: %s", name, cudaGetErrorString(e));
+            return done(GORSE_B200_ERR_CUDA);
+        }
+        Users U;
+        U.c_off = V.c_off.p; U.c_row = V.c_row.p + c_off[u0]; U.ex_off = V.ex_off.p; U.ex = V.ex.p + ex_off[u0];
+        U.slots = V.slots.p + u0 * top; U.scores = V.scores.p + u0 * top; U.count = V.count.p + u0;
+        if ((st = aggregate(c, V.users.p, fill, rows - fill, U, T, d_ok, n, need, top, score_scale, euclid, N, V.acc.p, V.seen.p, V.touched.p)))
+            return done(st);
+        if ((e = cudaEventRecord(c->copy_ev, c->stream)) != cudaSuccess || (e = cudaStreamWaitEvent(c->copy_stream, c->copy_ev, 0)) != cudaSuccess ||
+            (e = cudaMemcpyAsync(count_out + u0, V.count.p + u0, sizeof(int32_t) * rows, cudaMemcpyDeviceToHost, c->copy_stream)) != cudaSuccess ||
+            (e = cudaMemcpyAsync(slots_out + u0 * top, V.slots.p + u0 * top, sizeof(int64_t) * rows * top, cudaMemcpyDeviceToHost, c->copy_stream)) != cudaSuccess ||
+            (e = cudaMemcpyAsync(scores_out + u0 * top, V.scores.p + u0 * top, sizeof(double) * rows * top, cudaMemcpyDeviceToHost, c->copy_stream)) != cudaSuccess) {
+            set_error("%s download: %s", name, cudaGetErrorString(e));
+            return done(GORSE_B200_ERR_CUDA);
+        }
+    }
+    if ((e = cudaStreamSynchronize(c->stream)) != cudaSuccess || (e = cudaStreamSynchronize(c->copy_stream)) != cudaSuccess) {
+        set_error("%s: %s", name, cudaGetErrorString(e));
+        return done(GORSE_B200_ERR_CUDA);
+    }
+    if (stats_out) {
+        stats_out[0] = R;
+        stats_out[1] = exact_rows;
+        stats_out[2] = n_shared;
+        stats_out[3] = n_heavy;
+    }
+    return done(GORSE_B200_OK);
 }
 
 }  // namespace i2i
@@ -129,9 +309,6 @@ extern "C" int32_t gorse_b200_vecdb_item_to_item(gorse_b200_vecdb *db, int64_t n
                                                  int32_t n_categories, int32_t n, double score_scale, int64_t *slots_out, double *scores_out,
                                                  int32_t *count_out, int64_t *stats_out)
 {
-    using namespace gb::i2i;
-    using gb::agg::grow_zeroed;
-    using gb::recall::grow;
     GB_CHECK_ARG(db != nullptr, "collection is NULL");
     GB_CHECK_ARG(n_users >= 0 && n_categories >= 0, "negative count");
     if (stats_out) std::fill(stats_out, stats_out + 4, 0);
@@ -163,128 +340,69 @@ extern "C" int32_t gorse_b200_vecdb_item_to_item(gorse_b200_vecdb *db, int64_t n
     std::lock_guard<std::mutex> lk(db->mu);
     const int64_t n_slots = (int64_t)db->ts.size();
     if (n_slots > INT32_MAX) { set_error("item_to_item: more than 2^31 slots"); return GORSE_B200_ERR_UNSUPPORTED; }
-    // each user's exclusions once, sorted, -1 entries dropped (as gorse_b200_vecdb_query_excluding)
-    std::vector<int64_t> ex, ex_off((size_t)n_users + 1, 0);
-    ex.reserve((size_t)excl_off[n_users]);
-    for (int64_t u = 0; u < n_users; u++) {
+    for (int64_t u = 0; u < n_users; u++)
         for (int64_t t = ctx_off[u]; t < ctx_off[u + 1]; t++)
             GB_CHECK_ARG(ctx_slots[t] >= -1 && ctx_slots[t] < n_slots, "user %lld: context slot %lld is not a slot of the collection",
                          (long long)u, (long long)ctx_slots[t]);
-        const size_t b = ex.size();
-        for (int64_t t = excl_off[u]; t < excl_off[u + 1]; t++) {
-            const int64_t s = excl_slots[t];
-            GB_CHECK_ARG(s >= -1 && s < n_slots, "user %lld: excluded slot %lld is not a slot of the collection", (long long)u, (long long)s);
-            if (s >= 0) ex.push_back(s);
+    std::vector<int64_t> ex, ex_off;
+    GB_TRY(exclusion_rows(n_users, excl_off, excl_slots, n_slots, "user", "slot", ex, ex_off));
+    return i2i::neighbour_sums(db, "item_to_item", n_users, ctx_off, ctx_slots, ex, ex_off, categories, n_categories, nullptr, n, 0, n,
+                               score_scale, slots_out, scores_out, count_out, stats_out);
+}
+
+extern "C" int32_t gorse_b200_vecdb_session_recommend(gorse_b200_vecdb *db, int64_t n_sessions, const int64_t *ctx_off, const int64_t *ctx_slots,
+                                                      const int64_t *excl_off, const int64_t *excl_slots, const uint8_t *item_ok, int32_t n,
+                                                      int32_t context_size, int32_t top, double score_scale, int64_t *slots_out,
+                                                      double *scores_out, int32_t *count_out, int64_t *stats_out)
+{
+    // every check that needs no collection comes first, so that a bad argument is reported whatever db is
+    GB_CHECK_ARG(n_sessions >= 0, "negative n_sessions");
+    if (stats_out) std::fill(stats_out, stats_out + 4, 0);
+    std::vector<int64_t> ex, ex_off;
+    if (n_sessions > 0) {
+        GB_CHECK_ARG(count_out != nullptr && ctx_off != nullptr && excl_off != nullptr, "count_out / ctx_off / excl_off is NULL");
+        GB_CHECK_ARG(ctx_off[0] == 0 && excl_off[0] == 0, "ctx_off[0] and excl_off[0] must be 0");
+        for (int64_t u = 0; u < n_sessions; u++) {
+            GB_CHECK_ARG(ctx_off[u + 1] >= ctx_off[u], "ctx_off decreases at %lld", (long long)u);
+            GB_CHECK_ARG(excl_off[u + 1] >= excl_off[u], "excl_off decreases at %lld", (long long)u);
         }
-        std::sort(ex.begin() + b, ex.end());
-        for (size_t t = b + 1; t < ex.size(); t++)
-            GB_CHECK_ARG(ex[t] != ex[t - 1], "user %lld: slot %lld is excluded twice", (long long)u, (long long)ex[t]);
-        ex_off[(size_t)u + 1] = (int64_t)ex.size();
+        GB_CHECK_ARG(ctx_off[n_sessions] == 0 || ctx_slots != nullptr, "ctx_slots is NULL");
+        GB_CHECK_ARG(excl_off[n_sessions] == 0 || excl_slots != nullptr, "excl_slots is NULL");
+        GB_CHECK_ARG(top <= 0 || (slots_out != nullptr && scores_out != nullptr), "slots_out / scores_out is NULL");
+        for (int64_t t = 0; t < ctx_off[n_sessions]; t++)
+            GB_CHECK_ARG(ctx_slots[t] >= -1, "context slot %lld is not a slot of the collection", (long long)ctx_slots[t]);
+        // the upper bound of a slot needs the collection: checked below
+        GB_TRY(exclusion_rows(n_sessions, excl_off, excl_slots, INT64_MAX, "session", "slot", ex, ex_off));
     }
-    // the live context entries of every user as rows of the neighbour table: one row per distinct item, in first-visit order.
-    // -1 and deleted slots are skipped (GetVectors returns nothing, logics/item_to_item.go:56-58); hidden ones are queried.
-    std::vector<int32_t> row_of((size_t)n_slots, -1), c_row;
-    std::vector<int64_t> nb, c_off((size_t)n_users + 1, 0);
-    c_row.reserve((size_t)ctx_off[n_users]);
-    for (int64_t u = 0; u < n_users; u++) {
-        for (int64_t t = ctx_off[u]; t < ctx_off[u + 1]; t++) {
-            const int64_t s = ctx_slots[t];
-            if (s < 0 || db->dead[(size_t)s]) continue;
-            if (row_of[(size_t)s] < 0) {
-                row_of[(size_t)s] = (int32_t)nb.size();
-                nb.push_back(s);
-            }
-            c_row.push_back(row_of[(size_t)s]);
-        }
-        c_off[(size_t)u + 1] = (int64_t)c_row.size();
+    GB_CHECK_ARG(score_scale == score_scale, "score_scale is NaN");
+    if (top > MAX_N_DENSE) {
+        set_error("session_recommend: top = %d above %d", top, MAX_N_DENSE);
+        return GORSE_B200_ERR_UNSUPPORTED;
     }
-    const int64_t R = (int64_t)nb.size();
-    if (R == 0) {
-        for (int64_t u = 0; u < n_users; u++) count_out[u] = 0;
+    GB_CHECK_ARG(db != nullptr, "collection is NULL");
+    if (db->distance == GORSE_B200_DISTANCE_COSINE) {
+        set_error("session collections are Dot or Euclidean");
+        return GORSE_B200_ERR_UNSUPPORTED;
+    }
+    const bool sparse = db->dim == 0;
+    const int max_n = sparse ? MAX_N_SPARSE : MAX_N_DENSE;
+    if (n <= 0 || n > max_n) {   // n = 0 asks the store for one neighbour (n + 1) and keeps it: not served here
+        set_error("session_recommend: n = %d outside [1, %d] for a %s collection", n, max_n, sparse ? "sparse" : "dense");
+        return GORSE_B200_ERR_UNSUPPORTED;
+    }
+    if (n_sessions == 0) return GORSE_B200_OK;
+    std::lock_guard<std::mutex> lk(db->mu);
+    const int64_t n_slots = (int64_t)db->ts.size();
+    if (n_slots > INT32_MAX) { set_error("session_recommend: more than 2^31 slots"); return GORSE_B200_ERR_UNSUPPORTED; }
+    for (int64_t t = 0; t < ctx_off[n_sessions]; t++)
+        GB_CHECK_ARG(ctx_slots[t] < n_slots, "context slot %lld is not a slot of the collection", (long long)ctx_slots[t]);
+    for (int64_t t = 0; t < (int64_t)ex.size(); t++)
+        GB_CHECK_ARG(ex[t] < n_slots, "excluded slot %lld is not a slot of the collection", (long long)ex[t]);
+    if (top <= 0) {
+        std::fill(count_out, count_out + n_sessions, 0);
         return GORSE_B200_OK;
     }
-    gorse_b200_ctx *c = db->ctx;
-    ScopedDevice sd(c->device);
-    GB_TRY(vecdb_allow(db, categories, n_categories));
-    ItemToItemWork &V = db->i2i;
-    int32_t st = GORSE_B200_OK;
-    auto done = [&](int32_t s) {
-        cudaStreamSynchronize(c->stream);
-        cudaStreamSynchronize(c->copy_stream);
-        return s;
-    };
-    if ((st = grow(V.nb, (size_t)R)) || (st = grow(V.t_slot, (size_t)R * n)) || (st = grow(V.t_score, (size_t)R * n)) || (st = grow(V.t_cnt, (size_t)R)))
-        return done(st);
-    cudaError_t e = cudaMemcpyAsync(V.nb.p, nb.data(), sizeof(int64_t) * R, cudaMemcpyHostToDevice, c->stream);
-    if (e != cudaSuccess) { set_error("item_to_item upload: %s", cudaGetErrorString(e)); return done(GORSE_B200_ERR_CUDA); }
-
-    // ---- stage A: the neighbour table
-    int64_t exact_rows = 0;
-    if ((st = neighbour_table(db, R, V.nb.p, n, V.t_slot.p, V.t_score.p, V.t_cnt.p, &exact_rows))) return done(st);
-    if ((e = cudaGetLastError()) != cudaSuccess) { set_error("item_to_item: %s", cudaGetErrorString(e)); return done(GORSE_B200_ERR_CUDA); }
-
-    // ---- stage B: users in chunks; a finished chunk is downloaded on the copy stream while the next one computes
-    const int64_t cu = std::min<int64_t>(n_users, (int64_t)c->sm_count * 1024);
-    const int64_t N = n_slots;
-    const int hg = heavy_grid(c, N);
-    const int64_t total_ctx = c_off[(size_t)n_users];
-    if ((st = grow(V.c_off, (size_t)cu + 1)) || (st = grow(V.ex_off, (size_t)cu + 1)) || (st = grow(V.users, (size_t)cu)) ||
-        (st = grow(V.c_row, (size_t)std::max<int64_t>(total_ctx, 1))) || (st = grow(V.ex, std::max<size_t>(ex.size(), 1))) ||
-        (st = grow(V.slots, (size_t)n_users * n)) || (st = grow(V.scores, (size_t)n_users * n)) || (st = grow(V.count, (size_t)n_users)))
-        return done(st);
-    Table T;
-    T.slot = V.t_slot.p; T.score = V.t_score.p; T.cnt = V.t_cnt.p;
-    const bool euclid = db->distance == GORSE_B200_DISTANCE_EUCLIDEAN;
-    int64_t n_shared = 0, n_heavy = 0;
-    std::vector<int64_t> h_coff, h_exoff;
-    std::vector<int32_t> h_users;
-    for (int64_t u0 = 0; u0 < n_users; u0 += cu) {
-        const int64_t rows = std::min(cu, n_users - u0);
-        h_coff.resize(rows + 1); h_exoff.resize(rows + 1); h_users.resize(rows);
-        int64_t fill = 0, back = rows;   // table users from the front, heavy users from the back
-        for (int64_t r = 0; r <= rows; r++) {
-            h_coff[r] = c_off[u0 + r] - c_off[u0];
-            h_exoff[r] = ex_off[u0 + r] - ex_off[u0];
-        }
-        for (int64_t r = 0; r < rows; r++) {
-            if ((h_coff[r + 1] - h_coff[r]) * n <= TABLE_KEYS) h_users[fill++] = (int32_t)r;
-            else h_users[--back] = (int32_t)r;
-        }
-        n_shared += fill;
-        n_heavy += rows - fill;
-        if (rows - fill > 0 && ((st = grow(V.acc, (size_t)hg * N)) || (st = grow_zeroed(V.seen, (size_t)hg * N, c->stream)) ||
-                                (st = grow(V.touched, (size_t)hg * N))))
-            return done(st);
-        const int64_t n_c = h_coff[rows], n_e = h_exoff[rows];
-        if ((e = cudaMemcpyAsync(V.c_off.p, h_coff.data(), sizeof(int64_t) * (rows + 1), cudaMemcpyHostToDevice, c->stream)) != cudaSuccess ||
-            (e = cudaMemcpyAsync(V.ex_off.p, h_exoff.data(), sizeof(int64_t) * (rows + 1), cudaMemcpyHostToDevice, c->stream)) != cudaSuccess ||
-            (e = cudaMemcpyAsync(V.users.p, h_users.data(), sizeof(int32_t) * rows, cudaMemcpyHostToDevice, c->stream)) != cudaSuccess ||
-            (n_c && (e = cudaMemcpyAsync(V.c_row.p + c_off[u0], c_row.data() + c_off[u0], sizeof(int32_t) * n_c, cudaMemcpyHostToDevice, c->stream)) != cudaSuccess) ||
-            (n_e && (e = cudaMemcpyAsync(V.ex.p + ex_off[u0], ex.data() + ex_off[u0], sizeof(int64_t) * n_e, cudaMemcpyHostToDevice, c->stream)) != cudaSuccess)) {
-            set_error("item_to_item upload: %s", cudaGetErrorString(e));
-            return done(GORSE_B200_ERR_CUDA);
-        }
-        Users U;
-        U.c_off = V.c_off.p; U.c_row = V.c_row.p + c_off[u0]; U.ex_off = V.ex_off.p; U.ex = V.ex.p + ex_off[u0];
-        U.slots = V.slots.p + u0 * n; U.scores = V.scores.p + u0 * n; U.count = V.count.p + u0;
-        if ((st = aggregate(c, V.users.p, fill, rows - fill, U, T, n, score_scale, euclid, N, V.acc.p, V.seen.p, V.touched.p))) return done(st);
-        if ((e = cudaEventRecord(c->copy_ev, c->stream)) != cudaSuccess || (e = cudaStreamWaitEvent(c->copy_stream, c->copy_ev, 0)) != cudaSuccess ||
-            (e = cudaMemcpyAsync(count_out + u0, V.count.p + u0, sizeof(int32_t) * rows, cudaMemcpyDeviceToHost, c->copy_stream)) != cudaSuccess ||
-            (e = cudaMemcpyAsync(slots_out + u0 * n, V.slots.p + u0 * n, sizeof(int64_t) * rows * n, cudaMemcpyDeviceToHost, c->copy_stream)) != cudaSuccess ||
-            (e = cudaMemcpyAsync(scores_out + u0 * n, V.scores.p + u0 * n, sizeof(double) * rows * n, cudaMemcpyDeviceToHost, c->copy_stream)) != cudaSuccess) {
-            set_error("item_to_item download: %s", cudaGetErrorString(e));
-            return done(GORSE_B200_ERR_CUDA);
-        }
-    }
-    if ((e = cudaStreamSynchronize(c->stream)) != cudaSuccess || (e = cudaStreamSynchronize(c->copy_stream)) != cudaSuccess) {
-        set_error("item_to_item: %s", cudaGetErrorString(e));
-        return done(GORSE_B200_ERR_CUDA);
-    }
-    if (stats_out) {
-        stats_out[0] = R;
-        stats_out[1] = exact_rows;
-        stats_out[2] = n_shared;
-        stats_out[3] = n_heavy;
-    }
-    return done(GORSE_B200_OK);
+    const int need = std::max(context_size, 1);   // the handler stops once used >= ContextSize, after at least one list
+    return i2i::neighbour_sums(db, "session_recommend", n_sessions, ctx_off, ctx_slots, ex, ex_off, nullptr, 0, item_ok, n, need, top,
+                               score_scale, slots_out, scores_out, count_out, stats_out);
 }

@@ -5,10 +5,7 @@
 // first k_q = n + |E_q| allowed slots by (score desc, slot asc), minus the slots in E_q, with the scores of
 // gorse_b200_vecdb_query, bit for bit.  This file checks the arguments and prepares the exclusion lists; the rows run through
 // the index's top-k pipeline (recall::recall_rows, topk.cu).
-#include <algorithm>
-
-#include "topk.cuh"
-#include "vecdb.cuh"
+#include "stages.cuh"
 
 using namespace gb;
 
@@ -37,23 +34,11 @@ extern "C" int32_t gorse_b200_vecdb_query_excluding(gorse_b200_vecdb *db, int64_
     GB_CHECK_ARG(n_categories == 0 || categories != nullptr, "categories is NULL");
     std::lock_guard<std::mutex> lk(db->mu);
     const int64_t n_slots = (int64_t)db->ts.size();
-    // each row's exclusions once, sorted, -1 entries dropped (they still count in k_q)
-    std::vector<int64_t> ex;
-    std::vector<int64_t> ex_off((size_t)nq + 1, 0);
-    ex.reserve((size_t)excl_off[nq]);
-    for (int64_t q = 0; q < nq; q++) {
+    for (int64_t q = 0; q < nq; q++)
         GB_CHECK_ARG((int64_t)n + (excl_off[q + 1] - excl_off[q]) <= INT32_MAX, "row %lld: n + |E| overflows", (long long)q);
-        const size_t b = ex.size();
-        for (int64_t t = excl_off[q]; t < excl_off[q + 1]; t++) {
-            const int64_t s = excl_slots[t];
-            GB_CHECK_ARG(s >= -1 && s < n_slots, "row %lld: excluded slot %lld is not a slot of the collection", (long long)q, (long long)s);
-            if (s >= 0) ex.push_back(s);
-        }
-        std::sort(ex.begin() + b, ex.end());
-        for (size_t t = b + 1; t < ex.size(); t++)
-            GB_CHECK_ARG(ex[t] != ex[t - 1], "row %lld: slot %lld is excluded twice", (long long)q, (long long)ex[t]);
-        ex_off[(size_t)q + 1] = (int64_t)ex.size();
-    }
+    // each row's exclusions once, sorted, -1 entries dropped (they still count in k_q)
+    std::vector<int64_t> ex, ex_off;
+    GB_TRY(exclusion_rows(nq, excl_off, excl_slots, n_slots, "row", "slot", ex, ex_off));
     if (n_slots == 0) {
         for (int64_t q = 0; q < nq; q++) count_out[q] = 0;
         return GORSE_B200_OK;

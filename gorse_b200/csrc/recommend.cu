@@ -450,19 +450,8 @@ extern "C" int32_t gorse_b200_recommend(gorse_b200_ctx *ctx, int64_t n_users, co
     for (int64_t u = 0; u < n_users; u++) GB_CHECK_ARG(excl_off[u + 1] >= excl_off[u], "excl_off not non-decreasing at %lld", (long long)u);
     GB_CHECK_ARG(excl_off[n_users] == 0 || excl_items != nullptr, "excl_items is NULL");
     // E0: each user's items once, sorted, -1 dropped
-    std::vector<int64_t> e0, e0_off((size_t)n_users + 1, 0);
-    e0.reserve((size_t)excl_off[n_users]);
-    for (int64_t u = 0; u < n_users; u++) {
-        const size_t b = e0.size();
-        for (int64_t t = excl_off[u]; t < excl_off[u + 1]; t++) {
-            GB_CHECK_ARG(excl_items[t] >= -1 && excl_items[t] < n_items, "user %lld: excluded item %d is not in [-1, %d)", (long long)u, excl_items[t], n_items);
-            if (excl_items[t] >= 0) e0.push_back(excl_items[t]);
-        }
-        std::sort(e0.begin() + b, e0.end());
-        for (size_t t = b + 1; t < e0.size(); t++)
-            GB_CHECK_ARG(e0[t] != e0[t - 1], "user %lld: item %lld is excluded twice", (long long)u, (long long)e0[t]);
-        e0_off[(size_t)u + 1] = (int64_t)e0.size();
-    }
+    std::vector<int64_t> e0, e0_off;
+    GB_TRY(exclusion_rows(n_users, excl_off, excl_items, n_items, "user", "item", e0, e0_off));
     auto check_map = [&](const char *what, gorse_b200_vecdb *db, const int64_t *slot_of_item, const int32_t *item_of_slot) -> int32_t {
         GB_CHECK_ARG(slot_of_item != nullptr && (item_of_slot != nullptr || db->ts.empty()), "%s: slot_of_item / item_of_slot is NULL", what);
         const int64_t S = (int64_t)db->ts.size();
@@ -546,7 +535,7 @@ extern "C" int32_t gorse_b200_recommend(gorse_b200_ctx *ctx, int64_t n_users, co
                 set_error("stage %d: item-to-item / user-to-user collections are Dot or Euclidean", s);
                 return GORSE_B200_ERR_UNSUPPORTED;
             }
-            const int lim = db->dim == 0 ? i2i::MAX_N_SPARSE : i2i::MAX_N_DENSE;
+            const int lim = db->dim == 0 ? MAX_N_SPARSE : MAX_N_DENSE;
             if (g.n > lim) {
                 set_error("stage %d: n = %d above %d", s, g.n, lim);
                 return GORSE_B200_ERR_UNSUPPORTED;
@@ -585,7 +574,7 @@ extern "C" int32_t gorse_b200_recommend(gorse_b200_ctx *ctx, int64_t n_users, co
     if (cf) {
         gorse_b200_vecdb *db = cf->db;
         if (db->dim == 0) { set_error("the CF collection must be dense"); return GORSE_B200_ERR_UNSUPPORTED; }
-        GB_CHECK_ARG(cf->n >= 0 && cf->n <= i2i::MAX_N_DENSE, "CF n = %d is not in [0, %d]", cf->n, i2i::MAX_N_DENSE);
+        GB_CHECK_ARG(cf->n >= 0 && cf->n <= MAX_N_DENSE, "CF n = %d is not in [0, %d]", cf->n, MAX_N_DENSE);
         GB_CHECK_ARG(cf->user_vectors != nullptr, "CF user_vectors is NULL");
         if ((err = check_map("CF", db, cf->slot_of_item, cf->item_of_slot))) return err;
         for (int64_t u = 0; u < n_users; u++)
@@ -671,13 +660,8 @@ extern "C" int32_t gorse_b200_recommend(gorse_b200_ctx *ctx, int64_t n_users, co
             for (int64_t u = 0; u < n_users; u++) {
                 for (int64_t t = g.ctx_off[u]; t < g.ctx_off[u + 1]; t++) {
                     const int64_t it = g.ctx_items[t];
-                    const int64_t sl = it < 0 ? -1 : g.slot_of_item[it];
-                    if (sl < 0 || g.db->dead[(size_t)sl]) continue;
-                    if (row_of[(size_t)sl] < 0) {
-                        row_of[(size_t)sl] = (int32_t)D.nb.size();
-                        D.nb.push_back(sl);
-                    }
-                    D.c_row.push_back(row_of[(size_t)sl]);
+                    const int32_t r = table_row(g.db, it < 0 ? -1 : g.slot_of_item[it], row_of, D.nb);
+                    if (r >= 0) D.c_row.push_back(r);
                 }
                 D.c_off[(size_t)u + 1] = (int64_t)D.c_row.size();
             }
@@ -692,16 +676,8 @@ extern "C" int32_t gorse_b200_recommend(gorse_b200_ctx *ctx, int64_t n_users, co
             }
         } else if (g.kind == GORSE_B200_STAGE_USER_TO_USER) {
             std::vector<int32_t> row_of(g.db->ts.size(), -1);
-            D.q_row.assign((size_t)n_users, -1);
-            for (int64_t u = 0; u < n_users; u++) {
-                const int64_t sl = g.user_slots[u];
-                if (sl < 0 || g.db->dead[(size_t)sl]) continue;
-                if (row_of[(size_t)sl] < 0) {
-                    row_of[(size_t)sl] = (int32_t)D.nb.size();
-                    D.nb.push_back(sl);
-                }
-                D.q_row[(size_t)u] = row_of[(size_t)sl];
-            }
+            D.q_row.resize((size_t)n_users);
+            for (int64_t u = 0; u < n_users; u++) D.q_row[(size_t)u] = table_row(g.db, g.user_slots[u], row_of, D.nb);
             int64_t longest = 0;
             for (int64_t v = 0; v < g.n_fb_rows; v++) longest = std::max(longest, g.fb_off[v + 1] - g.fb_off[v]);
             D.heavy = longest * std::max(g.n, 0) > agg::TABLE_KEYS;
@@ -916,15 +892,15 @@ extern "C" int32_t gorse_b200_recommend(gorse_b200_ctx *ctx, int64_t n_users, co
                 (rs = recall::grow(D.ES[1], (size_t)std::max<int64_t>(max_c, 1))))
                 return done(rs);
             const int64_t N = (int64_t)g.db->ts.size();
-            bool heavy = false;
-            for (int64_t u = 0; u < n_users && !heavy; u++) heavy = (D.c_off[(size_t)u + 1] - D.c_off[(size_t)u]) * g.n > agg::TABLE_KEYS;
-            const int hg = i2i::heavy_grid(ctx, std::max<int64_t>(N, 1));
+            std::vector<int32_t> routed;
+            const bool heavy = i2i::route(D.c_off.data(), n_users, g.n, routed) < n_users;
+            const int hg = heavy_grid(ctx, std::max<int64_t>(N, 1), i2i::ROW_BYTES);
             if (heavy && N > 0 && ((rs = recall::grow(D.acc, (size_t)hg * N)) || (rs = agg::grow_zeroed(D.seen, (size_t)hg * N, st)) ||
                                    (rs = recall::grow(D.touched, (size_t)hg * N))))
                 return done(rs);
         } else if (g.kind == GORSE_B200_STAGE_USER_TO_USER && D.heavy) {
             const int64_t NI = std::max<int64_t>(n_items, 1);
-            const int hg = u2u::heavy_grid(ctx, NI);
+            const int hg = heavy_grid(ctx, NI, u2u::ROW_BYTES);
             if ((rs = agg::grow_zeroed(D.uacc, (size_t)hg * NI, st)) || (rs = agg::grow_zeroed(D.flag, (size_t)hg * NI, st)) ||
                 (rs = recall::grow(D.touched, (size_t)hg * NI)))
                 return done(rs);
@@ -1021,29 +997,24 @@ extern "C" int32_t gorse_b200_recommend(gorse_b200_ctx *ctx, int64_t n_users, co
                 const bool euclid = g.db->distance == GORSE_B200_DISTANCE_EUCLIDEAN;
                 if (g.kind == GORSE_B200_STAGE_ITEM_TO_ITEM) {
                     // the context rows of the chunk, users routed by |C_u| n as gorse_b200_vecdb_item_to_item routes them
-                    h_i2i_off.assign((size_t)rows + 1, 0);
-                    h_users.resize((size_t)rows);
-                    int64_t fill = 0, back = rows;
-                    for (int64_t r = 0; r < rows; r++) {
-                        h_i2i_off[(size_t)r + 1] = D.c_off[(size_t)(u0 + r + 1)] - D.c_off[(size_t)u0];
-                        if ((h_i2i_off[(size_t)r + 1] - h_i2i_off[(size_t)r]) * g.n <= agg::TABLE_KEYS) h_users[(size_t)fill++] = (int32_t)r;
-                        else h_users[(size_t)--back] = (int32_t)r;
-                    }
+                    h_i2i_off.resize((size_t)rows + 1);
+                    for (int64_t r = 0; r <= rows; r++) h_i2i_off[(size_t)r] = D.c_off[(size_t)(u0 + r)] - D.c_off[(size_t)u0];
+                    const int64_t fill = i2i::route(h_i2i_off.data(), rows, g.n, h_users);
                     REC_CUDA(cudaMemcpyAsync(d_i2i_off.p, h_i2i_off.data(), sizeof(int64_t) * (rows + 1), cudaMemcpyHostToDevice, st));
                     REC_CUDA(cudaMemcpyAsync(d_users.p, h_users.data(), sizeof(int32_t) * rows, cudaMemcpyHostToDevice, st));
                     i2i::Users U;
                     U.c_off = d_i2i_off.p; U.c_row = D.d_c_row.p + D.c_off[(size_t)u0]; U.ex_off = d_E_off.p; U.ex = D.ES[e_cur].p;
                     U.slots = d_rids.p; U.scores = d_rscore.p; U.count = d_rcount.p;
-                    const i2i::Table T{D.t_slot.p, D.t_score.p, D.t_cnt.p};
-                    REC_TRY(i2i::aggregate(ctx, d_users.p, fill, rows - fill, U, T, g.n, g.score_scale, euclid, (int64_t)g.db->ts.size(), D.acc.p,
-                                           D.seen.p, D.touched.p));
+                    const NeighbourTable T{D.t_slot.p, D.t_score.p, D.t_cnt.p};
+                    REC_TRY(i2i::aggregate(ctx, d_users.p, fill, rows - fill, U, T, nullptr, g.n, 0, g.n, g.score_scale, euclid,
+                                           (int64_t)g.db->ts.size(), D.acc.p, D.seen.p, D.touched.p));
                     rec_append_kernel<<<grid, NT, 0, st>>>(d_rids.p, d_rscore.p, d_rcount.p, g.n, D.d_item_of_slot.p, d_cand.p, d_cscore.p,
                                                            d_cand_off.p, d_cnt.p, rows);
                 } else {
                     u2u::Users U;
                     U.q_row = D.d_q_row.p + u0; U.ex_off = d_E_off.p; U.ex = E; U.item_ok = g.item_ok ? D.d_item_ok.p : nullptr;
                     U.items = d_rids.p; U.scores = d_rscore.p; U.count = d_rcount.p;
-                    const u2u::Table T{D.t_slot.p, D.t_score.p, D.t_cnt.p};
+                    const NeighbourTable T{D.t_slot.p, D.t_score.p, D.t_cnt.p};
                     const u2u::Feedback F{D.d_fb_off.p, D.d_fb_items.p, g.n_fb_rows};
                     u2u::Route Rt;
                     Rt.list = d_list.p; Rt.cnt = d_route.p + 2 * (k * n_stages + s); Rt.work = d_work.p; Rt.users = rows;

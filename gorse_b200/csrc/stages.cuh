@@ -1,60 +1,111 @@
-// stages.cuh -- the device bodies of the batched item-to-item and user-to-user recommenders (item_to_item.cu,
-// user_to_user.cu), taking device pointers, so that gorse_b200_vecdb_item_to_item / _user_to_user and the batched offline
-// recommendation (recommend.cu) launch the same kernels.
+// stages.cuh -- the device bodies of the batched neighbour recommenders and their host preparation: item-to-item and
+// session (item_to_item.cu), user-to-user (user_to_user.cu), taking device pointers, so that the vecdb entries and the
+// batched offline recommendation (recommend.cu) launch the same kernels and prepare their inputs the same way.
 #pragma once
 #include <algorithm>
+#include <vector>
 
 #include "aggregate.cuh"
 #include "vecdb.cuh"
 
 namespace gb {
 
-// stage A of both recommenders: the first n neighbours of each of the R stored vectors d_nb[R] (device) of db, as a table of
-// n (int32 slot, float32 score) entries per row, Dot collections keeping scores > 0 only (dense: the index's top-k pipeline;
-// sparse: sparse_search_rows).  The caller holds db->mu and has filled db->d_allow.  *exact_rows: rows of the exact scan.
+constexpr int MAX_N_DENSE = 1024;                // the sort buffer of agg::select_first_n holds n (session: top) entries
+constexpr int MAX_N_SPARSE = 128;                // sparse_search_kernel's k
+
+// stage A of every neighbour recommender: the first n neighbours of each of the R stored vectors d_nb[R] (device) of db, as
+// a table of n (int32 slot, float32 score) entries per row, Dot collections keeping scores > 0 only (dense: the index's top-k
+// pipeline; sparse: sparse_search_rows).  The caller holds db->mu and has filled db->d_allow.  *exact_rows: rows of the exact
+// scan.
 int32_t neighbour_table(gorse_b200_vecdb *db, int64_t R, const int64_t *d_nb, int n, int32_t *t_slot, float *t_score, int32_t *t_cnt,
                         int64_t *exact_rows);
 
+struct NeighbourTable {       // stage A: the first n neighbours of each distinct query
+    const int32_t *slot;      // [rows x n]
+    const float *score;       // [rows x n] the vector store's score (dot, or the negated distance)
+    const int32_t *cnt;       // [rows]
+};
+
+// global accumulator rows (one [N] entry of row_bytes per CTA, at most 512 MB): how many CTAs
+inline int heavy_grid(const gorse_b200_ctx *c, int64_t N, int64_t row_bytes)
+{
+    return (int)std::max<int64_t>(1, std::min<int64_t>((int64_t)c->sm_count * 2, (512ll << 20) / (row_bytes * N)));
+}
+
+// Each row's ids once, ascending, -1 entries dropped: the ids [off[r], off[r + 1]) of row r into ex, with ex_off [rows + 1].
+// An id outside [-1, bound) or twice in one row is an argument error; `row` and `id` name them in its message ("user",
+// "slot").
+template <typename Id>
+int32_t exclusion_rows(int64_t rows, const int64_t *off, const Id *ids, int64_t bound, const char *row, const char *id, std::vector<int64_t> &ex,
+                       std::vector<int64_t> &ex_off)
+{
+    ex.clear();
+    ex.reserve((size_t)off[rows]);
+    ex_off.assign((size_t)rows + 1, 0);
+    for (int64_t r = 0; r < rows; r++) {
+        const size_t b = ex.size();
+        for (int64_t t = off[r]; t < off[r + 1]; t++) {
+            const int64_t s = ids[t];
+            GB_CHECK_ARG(s >= -1 && s < bound, "%s %lld: excluded %s %lld is not a%s %s", row, (long long)r, id, (long long)s,
+                         id[0] == 'i' ? "n" : "", id);
+            if (s >= 0) ex.push_back(s);
+        }
+        std::sort(ex.begin() + b, ex.end());
+        for (size_t t = b + 1; t < ex.size(); t++)
+            GB_CHECK_ARG(ex[t] != ex[t - 1], "%s %lld: %s %lld is excluded twice", row, (long long)r, id, (long long)ex[t]);
+        ex_off[(size_t)r + 1] = (int64_t)ex.size();
+    }
+    return GORSE_B200_OK;
+}
+
+// The neighbour-table row of slot s of db: -1 for -1 and for a deleted slot (GetVectors returns nothing); else the rows
+// follow the first visit of each slot, a new slot appended to nb.  row_of: [slots], all -1 before the first call.
+inline int32_t table_row(const gorse_b200_vecdb *db, int64_t s, std::vector<int32_t> &row_of, std::vector<int64_t> &nb)
+{
+    if (s < 0 || db->dead[(size_t)s]) return -1;
+    if (row_of[(size_t)s] < 0) {
+        row_of[(size_t)s] = (int32_t)nb.size();
+        nb.push_back(s);
+    }
+    return row_of[(size_t)s];
+}
+
 namespace i2i {
-constexpr int MAX_N_DENSE = 1024;                // the sort buffer holds n entries
-constexpr int MAX_N_SPARSE = 128;                // sparse_search_kernel's k
+constexpr int64_t ROW_BYTES = 8 + 1 + 4;         // a global row entry: float64 sum, seen flag, touched slot
 
 struct Users {                // one chunk of users (chunk-local ids)
     const int64_t *c_off;     // [users + 1] into c_row
     const int32_t *c_row;     // the neighbour-table row of each live context entry, in the caller's order
     const int64_t *ex_off;    // [users + 1] into ex
     const int64_t *ex;        // each user's excluded slots, ascending (-1 entries dropped; may be padded with INT64_MAX)
-    int64_t *slots;           // [users x n]
-    double *scores;           // [users x n]
+    int64_t *slots;           // [users x top]
+    double *scores;           // [users x top]
     int32_t *count;           // [users]
 };
 
-struct Table {                // stage A: the first n neighbours of each distinct context item
-    const int32_t *slot;      // [rows x n]
-    const float *score;       // [rows x n] the vector store's score (dot, or the negated distance)
-    const int32_t *cnt;       // [rows]
-};
-
-// global accumulator rows (one [N] float64 row, flag row and slot list per CTA, at most 512 MB): how many CTAs
-inline int heavy_grid(const gorse_b200_ctx *c, int64_t N)
+// The users rows [0, rows) of a context CSR c_off in routing order: users[0, fill) take the shared-memory table
+// (|C_u| * n <= TABLE_KEYS), in order, users[fill, rows) a global row, in reverse order.  Returns fill.
+inline int64_t route(const int64_t *c_off, int64_t rows, int n, std::vector<int32_t> &users)
 {
-    return (int)std::max<int64_t>(1, std::min<int64_t>((int64_t)c->sm_count * 2, (512ll << 20) / (13 * N)));
+    users.resize((size_t)rows);
+    int64_t fill = 0, back = rows;
+    for (int64_t r = 0; r < rows; r++) {
+        if ((c_off[r + 1] - c_off[r]) * n <= agg::TABLE_KEYS) users[(size_t)fill++] = (int32_t)r;
+        else users[(size_t)--back] = (int32_t)r;
+    }
+    return fill;
 }
+
 // stage B for one chunk: d_users[0, fill) aggregate in shared memory, d_users[fill, fill + heavy) in the global rows acc /
-// seen (zeroed) / touched of heavy_grid(c, N) CTAs
-int32_t aggregate(gorse_b200_ctx *c, const int32_t *d_users, int64_t fill, int64_t heavy, const Users &U, const Table &T, int n, double scale,
-                  bool euclid, int64_t N, double *acc, uint8_t *seen, int32_t *touched);
+// seen (zeroed) / touched of heavy_grid(c, N, ROW_BYTES) CTAs.  item_ok: a slot mask or NULL; need > 0: walk each context
+// only up to the need-th entry whose item_ok-filtered list is not empty (session); the answer rows hold top entries.
+int32_t aggregate(gorse_b200_ctx *c, const int32_t *d_users, int64_t fill, int64_t heavy, const Users &U, const NeighbourTable &T,
+                  const uint8_t *item_ok, int n, int need, int top, double scale, bool euclid, int64_t N, double *acc, uint8_t *seen,
+                  int32_t *touched);
 }  // namespace i2i
 
 namespace u2u {
-constexpr int MAX_N_DENSE = 1024;
-constexpr int MAX_N_SPARSE = 128;
-
-struct Table {                // stage A: the first n neighbours of each distinct query user
-    const int32_t *slot;      // [rows x n]
-    const float *score;       // [rows x n] the vector store's score (dot, or the negated distance)
-    const int32_t *cnt;       // [rows]
-};
+constexpr int64_t ROW_BYTES = 8 + 4 + 4;         // a global row entry: float64 sum, flag, touched item
 
 struct Feedback {             // the caller's positive feedback per slot, as item indices
     const int64_t *off;       // [rows + 1]
@@ -79,14 +130,10 @@ struct Route {                // the device's routing of one chunk
     int64_t users;
 };
 
-inline int heavy_grid(const gorse_b200_ctx *c, int64_t NI)
-{
-    return (int)std::max<int64_t>(1, std::min<int64_t>((int64_t)c->sm_count * 2, (512ll << 20) / (16 * NI)));
-}
 // routing and stage B for one chunk of R.users users; heavy: some user may need a global row (acc / flag zeroed, touched,
-// heavy_grid(c, NI) CTAs)
-int32_t aggregate(gorse_b200_ctx *c, const Route &R, const Users &U, const Table &T, const Feedback &F, int n, double scale, bool euclid,
-                  int64_t NI, bool heavy, double *acc, int32_t *flag, int32_t *touched);
+// heavy_grid(c, NI, ROW_BYTES) CTAs)
+int32_t aggregate(gorse_b200_ctx *c, const Route &R, const Users &U, const NeighbourTable &T, const Feedback &F, int n, double scale,
+                  bool euclid, int64_t NI, bool heavy, double *acc, int32_t *flag, int32_t *touched);
 }  // namespace u2u
 
 }  // namespace gb

@@ -27,7 +27,7 @@ using agg::TABLE_KEYS;                           // a user takes the table when 
 constexpr int AGG_THREADS = agg::THREADS;
 
 // W_u for each user of the chunk.  Users without a vector, neighbours or feedback get an empty row here.
-__global__ void u2u_route_kernel(Users U, Table T, Feedback F, int n, Route R)
+__global__ void u2u_route_kernel(Users U, NeighbourTable T, Feedback F, int n, Route R)
 {
     const int64_t u = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (u >= R.users) return;
@@ -55,7 +55,7 @@ __global__ void u2u_route_kernel(Users U, Table T, Feedback F, int n, Route R)
 // between users) and one [n_items] item list per CTA.
 template <bool SHARED>
 __global__ void __launch_bounds__(AGG_THREADS)
-u2u_aggregate_kernel(Route R, Users U, Table T, Feedback F, int n, double scale, int euclid, int64_t n_items, double *acc_rows,
+u2u_aggregate_kernel(Route R, Users U, NeighbourTable T, Feedback F, int n, double scale, int euclid, int64_t n_items, double *acc_rows,
                      int32_t *flag_rows, int32_t *touched_rows)
 {
     using namespace gb::recall;
@@ -147,8 +147,8 @@ u2u_aggregate_kernel(Route R, Users U, Table T, Feedback F, int n, double scale,
     }
 }
 
-int32_t aggregate(gorse_b200_ctx *c, const Route &R, const Users &U, const Table &T, const Feedback &F, int n, double scale, bool euclid,
-                  int64_t NI, bool heavy, double *acc, int32_t *flag, int32_t *touched)
+int32_t aggregate(gorse_b200_ctx *c, const Route &R, const Users &U, const NeighbourTable &T, const Feedback &F, int n, double scale,
+                  bool euclid, int64_t NI, bool heavy, double *acc, int32_t *flag, int32_t *touched)
 {
     const size_t sm_shared = agg::smem_bytes(n, true), sm_global = agg::smem_bytes(n, false);
     GB_CUDA(cudaFuncSetAttribute(u2u_aggregate_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm_shared));
@@ -159,7 +159,7 @@ int32_t aggregate(gorse_b200_ctx *c, const Route &R, const Users &U, const Table
         R, U, T, F, n, scale, euclid, NI, nullptr, nullptr, nullptr);
     c->launches += 2;
     if (heavy) {
-        u2u_aggregate_kernel<false><<<(unsigned)std::min<int64_t>(rows, heavy_grid(c, NI)), AGG_THREADS, sm_global, c->stream>>>(
+        u2u_aggregate_kernel<false><<<(unsigned)std::min<int64_t>(rows, heavy_grid(c, NI, ROW_BYTES)), AGG_THREADS, sm_global, c->stream>>>(
             R, U, T, F, n, scale, euclid, NI, acc, flag, touched);
         c->launches++;
     }
@@ -214,36 +214,16 @@ extern "C" int32_t gorse_b200_vecdb_user_to_user(gorse_b200_vecdb *db, int64_t n
     std::lock_guard<std::mutex> lk(db->mu);
     const int64_t n_slots = (int64_t)db->ts.size();
     if (n_slots > INT32_MAX) { set_error("user_to_user: more than 2^31 slots"); return GORSE_B200_ERR_UNSUPPORTED; }
-    // each user's exclusions once, sorted, -1 entries dropped
-    std::vector<int64_t> ex, ex_off((size_t)n_users + 1, 0);
-    ex.reserve((size_t)excl_off[n_users]);
-    for (int64_t u = 0; u < n_users; u++) {
+    for (int64_t u = 0; u < n_users; u++)
         GB_CHECK_ARG(user_slots[u] >= -1 && user_slots[u] < n_slots, "user %lld: slot %lld is not a slot of the collection", (long long)u,
                      (long long)user_slots[u]);
-        const size_t b = ex.size();
-        for (int64_t t = excl_off[u]; t < excl_off[u + 1]; t++) {
-            const int64_t s = excl_items[t];
-            GB_CHECK_ARG(s >= -1 && s < n_items, "user %lld: excluded item %lld is not in [-1, %d)", (long long)u, (long long)s, n_items);
-            if (s >= 0) ex.push_back(s);
-        }
-        std::sort(ex.begin() + b, ex.end());
-        for (size_t t = b + 1; t < ex.size(); t++)
-            GB_CHECK_ARG(ex[t] != ex[t - 1], "user %lld: item %lld is excluded twice", (long long)u, (long long)ex[t]);
-        ex_off[(size_t)u + 1] = (int64_t)ex.size();
-    }
-    // the live query slots as rows of the neighbour table, one row per distinct slot in first-visit order.  -1 and deleted
-    // slots have no row (GetVectors returns nothing, logics/user_to_user.go:55-58); hidden ones are searched.
-    std::vector<int32_t> row_of((size_t)n_slots, -1), q_row((size_t)n_users, -1);
+    std::vector<int64_t> ex, ex_off;
+    GB_TRY(exclusion_rows(n_users, excl_off, excl_items, n_items, "user", "item", ex, ex_off));
+    // the live query slots as rows of the neighbour table.  -1 and deleted slots have no row (GetVectors returns nothing,
+    // logics/user_to_user.go:55-58); hidden ones are searched.
+    std::vector<int32_t> row_of((size_t)n_slots, -1), q_row((size_t)n_users);
     std::vector<int64_t> nb;
-    for (int64_t u = 0; u < n_users; u++) {
-        const int64_t s = user_slots[u];
-        if (s < 0 || db->dead[(size_t)s]) continue;
-        if (row_of[(size_t)s] < 0) {
-            row_of[(size_t)s] = (int32_t)nb.size();
-            nb.push_back(s);
-        }
-        q_row[(size_t)u] = row_of[(size_t)s];
-    }
+    for (int64_t u = 0; u < n_users; u++) q_row[(size_t)u] = table_row(db, user_slots[u], row_of, nb);
     const int64_t R = (int64_t)nb.size();
     if (R == 0) {
         for (int64_t u = 0; u < n_users; u++) count_out[u] = 0;
@@ -295,12 +275,11 @@ extern "C" int32_t gorse_b200_vecdb_user_to_user(gorse_b200_vecdb *db, int64_t n
     // ---- routing and stage B: users in chunks; a finished chunk is downloaded on the copy stream while the next one computes
     // global accumulators: one [n_items] float64 row, flag row and item list per CTA, at most 512 MB
     const int64_t NI = std::max<int64_t>(n_items, 1);
-    const int hg = heavy_grid(c, NI);
+    const int hg = heavy_grid(c, NI, ROW_BYTES);
     if (heavy_possible && ((st = grow_zeroed(V.acc, (size_t)hg * NI, c->stream)) || (st = grow_zeroed(V.flag, (size_t)hg * NI, c->stream)) ||
                            (st = grow(V.touched, (size_t)hg * NI))))
         return done(st);
-    Table T;
-    T.slot = V.t_slot.p; T.score = V.t_score.p; T.cnt = V.t_cnt.p;
+    const NeighbourTable T{V.t_slot.p, V.t_score.p, V.t_cnt.p};
     Feedback F;
     F.off = V.fb_off.p; F.items = V.fb_items.p; F.rows = n_fb_rows;
     const bool euclid = db->distance == GORSE_B200_DISTANCE_EUCLIDEAN;

@@ -1,11 +1,11 @@
 // vecdb.cuh -- state of one vector collection (vecdb.cu), shared with the batched recall (recall.cu), item-to-item and
-// user-to-user.
+// session (item_to_item.cu) and user-to-user (user_to_user.cu).
 #pragma once
 #include "topk.cuh"
 
 namespace gb {
-// grow-only work buffers of gorse_b200_vecdb_item_to_item (item_to_item.cu) and gorse_b200_vecdb_session_recommend
-// (session.cu), which both hold the collection's lock: the neighbour table of stage A, the user or session batches, answers
+// grow-only work buffers of gorse_b200_vecdb_item_to_item and gorse_b200_vecdb_session_recommend (item_to_item.cu),
+// which both hold the collection's lock: the neighbour table of stage A, the user or session batches, answers
 // and accumulator scratch of stage B, and the session call's item mask
 struct ItemToItemWork {
     DevBuf<int64_t> nb, c_off, ex_off, ex, slots;
@@ -66,7 +66,7 @@ struct gorse_b200_vecdb {
     gb::DevBuf<uint8_t> d_blocked, d_allow;   // blocked = hidden | dead
     gb::DevBuf<int64_t> d_cat_off;
     gb::DevBuf<int32_t> d_cats, d_want;
-    gb::ItemToItemWork i2i;  // batched item-to-item and session recommendation (item_to_item.cu, session.cu)
+    gb::ItemToItemWork i2i;  // batched item-to-item and session recommendation (item_to_item.cu)
     gb::UserToUserWork u2u;  // batched user-to-user recommendation (user_to_user.cu)
 };
 

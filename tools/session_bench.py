@@ -17,7 +17,7 @@ vector).
 One JSON line, with per collection:
   card                 name, power limit and SM clock (nvidia-smi --query-gpu, read in the same run)
   wall_s               all sessions in one call, host in to host out, median of 3
-  device_ms            stage A (neighbour table) and stage B (session_aggregate_kernel) device time in one profiled call
+  device_ms            stage A (neighbour table) and stage B (i2i_aggregate_kernel) device time in one profiled call
   single_session_ms    n_sessions = 1, median over 100 seeded sessions
   stats                distinct context items, neighbour rows answered by the exact scan, sessions per accumulator
   per_item             the handler's path: one gorse_b200_vecdb_query(topK = n + 1) per context item up to the handler's cut,
@@ -169,7 +169,7 @@ def main():
                     t = getattr(e, "device_time_total", 0.0) or getattr(e, "cuda_time_total", 0.0)
                     if "Memcpy" in e.key or "Memset" in e.key or not t:
                         continue
-                    stage = "B" if "session_aggregate_kernel" in e.key else "A"
+                    stage = "B" if "i2i_aggregate_kernel" in e.key else "A"
                     dev[stage] = dev.get(stage, 0.0) + t / 1e3
 
                 # ---- the handler's path: one vecdb_query per context item up to its cut, lower bound
