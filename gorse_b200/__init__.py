@@ -402,6 +402,12 @@ class SparseIndex:
         check(lib.gorse_b200_sparse_index_search_range(self.h, q0, q1, k, ptr(idx), ptr(dot), ptr(cnt)))
         return idx, dot, cnt
 
+    def stats(self):
+        """{push, pull, tiles, search_ms} of the tiled search since the last call: work items by path, tiles walked, device ms."""
+        push, pull, tiles, ms = C.c_int64(0), C.c_int64(0), C.c_int64(0), C.c_double(0)
+        check(lib.gorse_b200_sparse_index_stats(self.h, C.byref(push), C.byref(pull), C.byref(tiles), C.byref(ms)))
+        return dict(push=push.value, pull=pull.value, tiles=tiles.value, search_ms=ms.value)
+
     def __enter__(self):
         return self
 

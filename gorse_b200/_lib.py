@@ -85,6 +85,8 @@ PROTOTYPES = {
     "gorse_b200_sparse_index_add": (C.c_int32, [VP, VP, VP, VP, C.c_int64, C.POINTER(C.c_int64)]),
     "gorse_b200_sparse_index_len": (C.c_int32, [VP, C.POINTER(C.c_int64)]),
     "gorse_b200_sparse_index_search_range": (C.c_int32, [VP, C.c_int64, C.c_int64, C.c_int32, VP, VP, VP]),
+    "gorse_b200_sparse_index_stats": (C.c_int32, [VP, C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.POINTER(C.c_int64),
+                                                  C.POINTER(C.c_double)]),
     "gorse_b200_vecdb_create": (C.c_int32, [VP, C.c_int32, C.c_int32, PVP]),
     "gorse_b200_vecdb_destroy": (C.c_int32, [VP]),
     "gorse_b200_vecdb_count": (C.c_int32, [VP, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),

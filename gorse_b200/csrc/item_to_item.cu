@@ -11,7 +11,7 @@
 //   stage A   the neighbour table, once per call: the distinct live context items of the whole batch are queried once each.
 //             Dense collections run the index's top-k pipeline (recall_rows, topk.cu) with k = n on the stored vectors (a
 //             row never returns its own vector), and its table keeps Dot scores > 0 only.  Sparse collections run
-//             sparse_search_kernel on the list of stored rows (a row never finds itself; it keeps positive dots only).
+//             the tiled sparse search (sparse.cu) on the list of stored rows (a row never finds itself; it keeps positive dots only).
 //             The table holds n (int32 slot, float32 score) entries per item, scores bit-identical to gorse_b200_vecdb_query.
 //             A session's walk cannot stop at its cut here: whether an entry counts depends on its filtered list.
 //   stage B   i2i_aggregate_kernel, one CTA per user: for a session, first the cut (context_cut); then walks C_u (the

@@ -6,14 +6,20 @@
 // sparse vectors summed in ascending index order, fp32, multiply and add unfused (the test suite's CPU restatement).
 //
 // Layout: the vectors as CSR (row -> ascending feature indices + values) and the same entries as CSC (feature -> ascending
-// rows + values, the posting lists).  One warp answers one query row r:
-//   1. for every feature f of r in ascending order: acc[c] += v_rf * v_cf over the posting list of f (the lanes take distinct
-//      rows c, a __syncwarp orders the features) -- every candidate's dot is summed in ascending feature order, i.e. exactly
-//      the merge-join order of the oracle, bit for bit;
-//   2. one coalesced pass over the warp's private accumulator row acc[0..N): keep the k largest positive dots with the
-//      warp-cooperative sorted list (order: dot descending, then row ascending) and reset the accumulator to zero.
-// Only rows that share a feature with the query can have a non-zero dot; rows with dot <= 0 are never returned (the
-// reference drops them right after the query, logics/item_to_item.go:73).  Roofline class: HBM/L2 (N floats scanned per query).
+// rows + values, the posting lists).  The stored rows are cut into tiles of TILE rows; a work item is one (query, tile) pair and
+// one CTA accumulates it in a shared-memory float per row of the tile, by one of two paths chosen per work item:
+//   push  for every feature f of the query in ascending order, add v_qf * v_cf into acc[c] for the postings c of f inside the
+//         tile (found by binary search: postings ascend by row); the threads take distinct rows and a barrier separates the
+//         features.  Cost: one CTA round per feature with postings in the tile, plus the postings / threads.
+//   pull  one warp per row c of the tile merge-joins the row's CSR against the query's features (a binary search per entry);
+//         the matched products are added in entry order by a shuffle chain.  Cost: the tile's entries / 32 plus its rows,
+//         spread over the warps, times the search depth.
+// Either way every candidate's dot is summed in ascending feature order, fp32, multiply and add unfused -- the merge-join order
+// of the oracle -- so both paths give the same bits.  Each work item keeps its tile's best k positive dots (order: dot
+// descending, then row ascending) under the allow mask and self-exclusion; a merge kernel folds each query's tile lists into
+// its answer.  Rows with dot <= 0 are never returned (the reference drops them right after the query,
+// logics/item_to_item.go:73).  Work items are taken tile-major, so the queries of one tile run together and reuse the tile's
+// posting ranges from L2, and a heavy query spreads over as many CTAs as it has tiles.
 #include <algorithm>
 
 #include <cub/cub.cuh>
@@ -54,65 +60,271 @@ __device__ __forceinline__ void list_insert_warp(float *ld, int32_t *li, int &le
     __syncwarp();
 }
 
-template <bool ROW_LIST>
-__global__ void __launch_bounds__(128)
-sparse_search_kernel(const int64_t *off, const uint32_t *ind, const float *val, const int64_t *foff, const int32_t *frow,
-                     const float *fval, int64_t N, uint32_t n_features, int64_t q0, int64_t nq, int k, float *acc, int32_t *out_idx,
-                     float *out_dot, int32_t *out_count, const int64_t *q_off, const uint32_t *q_ind, const float *q_val,
-                     const uint8_t *allow, const int64_t *q_rows)
+// merge two sorted lists (a: na, b: nb entries, all rows distinct) into the first min(k, na + nb) of out; one warp
+__device__ __forceinline__ int count_before(const float *d, const int32_t *id, int n, float dv, int32_t iv)
 {
-    // queries: stored rows q0 + q, or q_rows[q] with ROW_LIST (a device list, item_to_item.cu) -- never returned themselves --
-    // or, q_off != nullptr, rows of an external CSR (vecdb.cu: QueryVectors passes the vector, not its id); allow: optional
-    // per-row filter
-    extern __shared__ unsigned char sm_raw[];
-    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5, nw = blockDim.x >> 5;
-    float *ld = reinterpret_cast<float *>(sm_raw) + (size_t)wid * k;
-    int32_t *li = reinterpret_cast<int32_t *>(reinterpret_cast<float *>(sm_raw) + (size_t)nw * k) + (size_t)wid * k;
-    float *a = acc + ((int64_t)blockIdx.x * nw + wid) * N;   // this warp's accumulator row, all zero between queries
-    for (int64_t q = (int64_t)blockIdx.x * nw + wid; q < nq; q += (int64_t)gridDim.x * nw) {
-        const int64_t row = q_off ? -1 : ROW_LIST ? q_rows[q] : q0 + q;
-        const int64_t tb = q_off ? q_off[q] : off[row], te = q_off ? q_off[q + 1] : off[row + 1];
-        const uint32_t *qi = q_off ? q_ind : ind;
-        const float *qv = q_off ? q_val : val;
-        for (int64_t t = tb; t < te; t++) {
-            const uint32_t f = qi[t];
-            const float v = qv[t];
-            if (f >= n_features) continue;   // a feature no stored vector has (warp-uniform)
-            for (int64_t p = foff[f] + lane; p < foff[f + 1]; p += 32) {
-                const int32_t c = frow[p];
-                a[c] = a[c] + v * fval[p];        // unfused multiply and add, like the oracle (-fmad=false)
-            }
-            __syncwarp();
-        }
-        int len = 0;
-        for (int64_t base = 0; base < N; base += 32) {
-            const int64_t c = base + lane;
-            float x = 0.f;
-            if (c < N) {
-                x = a[c];
-                if (x != 0.f) a[c] = 0.f;
-            }
-            const bool valid = c < N && c != row && x > 0.f && (allow == nullptr || allow[c] != 0);
-            // cheap pre-filter against the current k-th best before the warp-wide insertion
-            const bool cand = valid && (len < k || before(-x, (int32_t)c, ld[k - 1], li[k - 1]));
-            unsigned m = __ballot_sync(0xffffffffu, cand);
-            while (m) {
-                const int s = __ffs(m) - 1;
-                m &= m - 1;
-                const float dd = __shfl_sync(0xffffffffu, -x, s);
-                const int32_t vv = (int32_t)(base + s);
-                list_insert_warp(ld, li, len, k, dd, vv, lane);
-            }
-        }
-        __syncwarp();
-        for (int e = lane; e < k; e += 32) {
-            const bool has = e < len;
-            out_idx[q * k + e] = has ? li[e] : -1;
-            out_dot[q * k + e] = has ? -ld[e] : 0.f;
-        }
-        if (lane == 0) out_count[q] = len;
-        __syncwarp();
+    int lo = 0, hi = n;
+    while (lo < hi) {
+        const int m = (lo + hi) >> 1;
+        if (before(d[m], id[m], dv, iv)) lo = m + 1;
+        else hi = m;
     }
+    return lo;
+}
+__device__ __forceinline__ int merge_warp(const float *ad, const int32_t *ai, int na, const float *bd, const int32_t *bi, int nb, float *od,
+                                          int32_t *oi, int k, int lane)
+{
+    for (int e = lane; e < na; e += 32) {
+        const int r = e + count_before(bd, bi, nb, ad[e], ai[e]);
+        if (r < k) { od[r] = ad[e]; oi[r] = ai[e]; }
+    }
+    for (int e = lane; e < nb; e += 32) {
+        const int r = e + count_before(ad, ai, na, bd[e], bi[e]);
+        if (r < k) { od[r] = bd[e]; oi[r] = bi[e]; }
+    }
+    __syncwarp();
+    return min(k, na + nb);
+}
+
+constexpr int TILE = 8192;              // rows per tile: a 32 KB accumulator, four CTAs per SM
+constexpr int NT = 256, NW = NT / 32;   // threads / warps of a work item's CTA; NT features per batch of posting ranges
+constexpr int MERGE_WARPS = 4;
+
+struct Stored {   // the index's device layouts
+    const int64_t *off; const uint32_t *ind; const float *val;    // CSR
+    const int64_t *foff; const int32_t *frow; const float *fval;  // CSC
+    int64_t n; uint32_t n_features;
+};
+// the queries of one search: rows of an external device CSR (q_off != nullptr; vecdb.cu: QueryVectors passes the vector, not its
+// id), the stored rows rows[q] (a device list, item_to_item.cu), or the stored rows q0 + q; stored query rows never return themselves
+struct Queries {
+    const int64_t *q_off; const uint32_t *q_ind; const float *q_val;
+    const int64_t *rows; int64_t q0;
+};
+
+__device__ __forceinline__ int64_t lower_row(const int32_t *frow, int64_t a, int64_t b, int64_t x)
+{
+    while (a < b) {
+        const int64_t m = (a + b) >> 1;
+        if (frow[m] < x) a = m + 1;
+        else b = m;
+    }
+    return a;
+}
+
+__device__ __forceinline__ int64_t block_sum(int64_t v, int64_t *red)
+{
+#pragma unroll
+    for (int o = 16; o; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
+    __syncthreads();
+    int64_t s = 0;
+#pragma unroll
+    for (int w = 0; w < NW; w++) s += red[w];
+    __syncthreads();
+    return s;
+}
+
+// one CTA per work item at a time, work items w = t * nqc + q (tile-major) taken from *next; the tile list of w goes to
+// tl_dot / tl_idx [w * k ...] (negated dots, best first) and tl_cnt[w]; paths[0] / [1] count the push / pull work items
+__global__ void __launch_bounds__(NT, 4)
+sparse_tile_kernel(Stored S, Queries Q, int64_t qc0, int64_t nqc, int ntiles, int k, const uint8_t *allow, unsigned long long *next,
+                   float *tl_dot, int32_t *tl_idx, int32_t *tl_cnt, unsigned long long *paths)
+{
+    extern __shared__ __align__(16) unsigned char sm_raw[];
+    float *acc = reinterpret_cast<float *>(sm_raw);                        // [TILE], zero between work items
+    uint32_t *bits = reinterpret_cast<uint32_t *>(acc + TILE);              // [TILE / 32] rows the push touched, zero between
+    int64_t *r_lo = reinterpret_cast<int64_t *>(bits + TILE / 32);          // [NT] a batch of posting ranges and query values
+    int64_t *r_hi = r_lo + NT;
+    float *r_v = reinterpret_cast<float *>(r_hi + NT);
+    float *ld = r_v + NT;                                                    // [2][NW][k] the warps' lists, two buffers
+    int32_t *li = reinterpret_cast<int32_t *>(ld + 2 * NW * k);
+    __shared__ int64_t red[NW];
+    __shared__ int lens[2][NW];
+    __shared__ unsigned long long item;
+    const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
+    for (int i = tid; i < TILE; i += NT) acc[i] = 0.f;
+    for (int i = tid; i < TILE / 32; i += NT) bits[i] = 0u;
+    const unsigned long long total = (unsigned long long)nqc * ntiles;
+    for (;;) {
+        if (tid == 0) item = atomicAdd(next, 1ull);
+        __syncthreads();
+        const unsigned long long w = item;
+        if (w >= total) return;
+        const int64_t t = (int64_t)(w / nqc), q = qc0 + (int64_t)(w % nqc);
+        const int64_t row = Q.q_off ? -1 : Q.rows ? Q.rows[q] : Q.q0 + q;
+        const int64_t tb = Q.q_off ? Q.q_off[q] : S.off[row], te = Q.q_off ? Q.q_off[q + 1] : S.off[row + 1];
+        const uint32_t *qi = Q.q_off ? Q.q_ind : S.ind;
+        const float *qv = Q.q_off ? Q.q_val : S.val;
+        const int64_t c0 = t * TILE, c1 = min(S.n, c0 + TILE);
+
+        // the paths' costs in CTA rounds; the push's is counted until it passes the pull's
+        int depth = 1;
+        while ((1ll << depth) <= te - tb) depth++;
+        const int64_t pull_cost = ((S.off[c1] - S.off[c0]) / 32 + (c1 - c0) + NW - 1) / NW * (depth + 1);
+        int64_t push_cost = 0;
+        for (int64_t b = tb; b < te && push_cost <= pull_cost; b += NT) {
+            int64_t my = 0;
+            if (b + tid < te) {
+                const uint32_t f = qi[b + tid];
+                if (f < S.n_features) {
+                    const int64_t lo = lower_row(S.frow, S.foff[f], S.foff[f + 1], c0), hi = lower_row(S.frow, lo, S.foff[f + 1], c1);
+                    if (hi > lo) my = 1 + (hi - lo + NT - 1) / NT;
+                }
+            }
+            push_cost += block_sum(my, red);
+        }
+        float *wd = ld + wid * k;
+        int32_t *wi = li + wid * k;
+        int len = 0;   // this warp's list, warp-uniform
+        const bool pull = push_cost > pull_cost;
+        if (push_cost == 0) {
+            // the query shares no feature with the tile: nothing to add
+        } else if (!pull) {
+            for (int64_t b = tb; b < te; b += NT) {
+                int64_t lo = 0, hi = 0;
+                float v = 0.f;
+                if (b + tid < te) {
+                    const uint32_t f = qi[b + tid];
+                    v = qv[b + tid];
+                    if (f < S.n_features) {   // a feature no stored vector has adds nothing
+                        lo = lower_row(S.frow, S.foff[f], S.foff[f + 1], c0);
+                        hi = lower_row(S.frow, lo, S.foff[f + 1], c1);
+                    }
+                }
+                r_lo[tid] = lo; r_hi[tid] = hi; r_v[tid] = v;
+                __syncthreads();
+                const int nb = (int)min((int64_t)NT, te - b);
+                for (int x = 0; x < nb; x++) {
+                    const int64_t plo = r_lo[x], phi = r_hi[x];
+                    if (plo == phi) continue;   // block-uniform
+                    const float fv = r_v[x];
+                    for (int64_t p = plo + tid; p < phi; p += NT) {
+                        const int c = S.frow[p] - (int)c0;
+                        acc[c] = acc[c] + fv * S.fval[p];   // unfused multiply and add, like the oracle (-fmad=false)
+                        atomicOr(&bits[c >> 5], 1u << (c & 31));
+                    }
+                    __syncthreads();   // the next feature adds after this one: each sum in ascending feature order
+                }
+                __syncthreads();
+            }
+            // thread tid owns bitmap word tid (TILE / 32 == NT): its touched rows, read and cleared
+            uint32_t m = bits[tid];
+            bits[tid] = 0u;
+            while (__any_sync(0xffffffffu, m != 0u)) {
+                float x = 0.f;
+                int32_t c = -1;
+                bool cand = false;
+                if (m) {
+                    const int i = tid * 32 + __ffs(m) - 1;
+                    m &= m - 1;
+                    x = acc[i];
+                    acc[i] = 0.f;
+                    c = (int32_t)(c0 + i);
+                    cand = x > 0.f && c != row && (allow == nullptr || allow[c] != 0);
+                }
+                cand = cand && (len < k || before(-x, c, wd[k - 1], wi[k - 1]));
+                unsigned bal = __ballot_sync(0xffffffffu, cand);
+                while (bal) {
+                    const int s = __ffs(bal) - 1;
+                    bal &= bal - 1;
+                    const float dd = __shfl_sync(0xffffffffu, -x, s);
+                    const int32_t cc = __shfl_sync(0xffffffffu, c, s);
+                    list_insert_warp(wd, wi, len, k, dd, cc, lane);
+                }
+            }
+        } else {
+            for (int64_t r = c0 + wid; r < c1; r += NW) {
+                const int64_t a = S.off[r], e = S.off[r + 1];
+                float s = 0.f;
+                int64_t lo = tb;   // the query's features below lo are below every remaining entry of the row
+                for (int64_t base = a; base < e && lo < te; base += 32) {
+                    const int64_t p = base + lane;
+                    float prod = 0.f;
+                    bool hit = false;
+                    int64_t pos = te;
+                    if (p < e) {
+                        const uint32_t g = S.ind[p];
+                        int64_t x = lo, y = te;
+                        while (x < y) {
+                            const int64_t mid = (x + y) >> 1;
+                            if (qi[mid] < g) x = mid + 1;
+                            else y = mid;
+                        }
+                        pos = x;
+                        if (x < te && qi[x] == g) { hit = true; prod = qv[x] * S.val[p]; }
+                    }
+                    unsigned hm = __ballot_sync(0xffffffffu, hit);
+                    while (hm) {   // in entry order = ascending feature order
+                        const int src = __ffs(hm) - 1;
+                        hm &= hm - 1;
+                        s = s + __shfl_sync(0xffffffffu, prod, src);
+                    }
+                    lo = __shfl_sync(0xffffffffu, pos, 31);
+                }
+                if (s > 0.f && r != row && (allow == nullptr || allow[r] != 0) && (len < k || before(-s, (int32_t)r, wd[k - 1], wi[k - 1])))
+                    list_insert_warp(wd, wi, len, k, -s, (int32_t)r, lane);
+            }
+        }
+        // the warps' lists pairwise into one: NW -> NW / 2 -> ... -> 1, alternating buffers
+        if (lane == 0) lens[0][wid] = len;
+        __syncthreads();
+        int src = 0, nl = NW;
+        for (; nl > 1; nl >>= 1, src ^= 1) {
+            if (wid < nl / 2) {
+                const float *sd = ld + (size_t)src * NW * k;
+                const int32_t *si = li + (size_t)src * NW * k;
+                const int n = merge_warp(sd + 2 * wid * k, si + 2 * wid * k, lens[src][2 * wid], sd + (2 * wid + 1) * k, si + (2 * wid + 1) * k,
+                                         lens[src][2 * wid + 1], ld + (size_t)(src ^ 1) * NW * k + wid * k,
+                                         li + (size_t)(src ^ 1) * NW * k + wid * k, k, lane);
+                if (lane == 0) lens[src ^ 1][wid] = n;
+            }
+            __syncthreads();
+        }
+        const int n = lens[src][0];
+        for (int e = tid; e < n; e += NT) {
+            tl_dot[w * k + e] = ld[(size_t)src * NW * k + e];
+            tl_idx[w * k + e] = li[(size_t)src * NW * k + e];
+        }
+        if (tid == 0) {
+            tl_cnt[w] = n;
+            if (push_cost) atomicAdd(&paths[pull], 1ull);
+        }
+        __syncthreads();   // lens, the lists and `item` are reused by the next work item
+    }
+}
+
+// one warp per query of the chunk: fold its tile lists into the answer out_*[(qc0 + q) * k ...], padded with -1 / 0
+__global__ void __launch_bounds__(32 * MERGE_WARPS)
+sparse_merge_kernel(int64_t qc0, int64_t nqc, int ntiles, int k, const float *tl_dot, const int32_t *tl_idx, const int32_t *tl_cnt,
+                    int32_t *out_idx, float *out_dot, int32_t *out_cnt)
+{
+    extern __shared__ __align__(16) unsigned char sm_raw[];
+    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+    float *bd = reinterpret_cast<float *>(sm_raw) + (size_t)wid * 3 * k;   // [3][k]: two running lists and the tile list
+    int32_t *bi = reinterpret_cast<int32_t *>(reinterpret_cast<float *>(sm_raw) + (size_t)MERGE_WARPS * 3 * k) + (size_t)wid * 3 * k;
+    const int64_t q = (int64_t)blockIdx.x * MERGE_WARPS + wid;
+    if (q >= nqc) return;
+    int len = 0, cur = 0;
+    for (int t = 0; t < ntiles; t++) {
+        const int64_t w = (int64_t)t * nqc + q;
+        const int nb = tl_cnt[w];
+        if (nb == 0) continue;
+        if (len == k && !before(tl_dot[w * k], tl_idx[w * k], bd[cur * k + k - 1], bi[cur * k + k - 1])) continue;
+        float *td = bd + 2 * k;
+        int32_t *ti = bi + 2 * k;
+        for (int e = lane; e < nb; e += 32) { td[e] = tl_dot[w * k + e]; ti[e] = tl_idx[w * k + e]; }
+        __syncwarp();
+        len = merge_warp(bd + cur * k, bi + cur * k, len, td, ti, nb, bd + (cur ^ 1) * k, bi + (cur ^ 1) * k, k, lane);
+        cur ^= 1;
+    }
+    const int64_t o = (qc0 + q) * k;
+    for (int e = lane; e < k; e += 32) {
+        const bool has = e < len;
+        out_idx[o + e] = has ? bi[cur * k + e] : -1;
+        out_dot[o + e] = has ? -bd[cur * k + e] : 0.f;
+    }
+    if (lane == 0) out_cnt[qc0 + q] = len;
 }
 
 int32_t sync_device(gorse_b200_sparse_index *ix)
@@ -149,8 +361,6 @@ int32_t sync_device(gorse_b200_sparse_index *ix)
         GB_CUDA(cudaMemcpyAsync(ix->fval.p, fval.data(), sizeof(float) * (size_t)nnz, cudaMemcpyHostToDevice, s));
     }
     GB_CUDA(cudaStreamSynchronize(s));   // the staging vectors die here
-    ix->acc.free();                      // sized for the old N
-    ix->acc_slots = 0;
     ix->dirty = false;
     return GORSE_B200_OK;
 }
@@ -204,6 +414,15 @@ __global__ void sparse_compact_csc_kernel(const int32_t *frow, const float *fval
     }
 }
 
+// the last search's device time into search_ms (every caller synchronises its stream before it returns, so this rarely waits)
+void fold_time(gorse_b200_sparse_index *ix)
+{
+    if (!ix->ev_pending) return;
+    float ms = 0.f;
+    if (cudaEventSynchronize(ix->ev[1]) == cudaSuccess && cudaEventElapsedTime(&ms, ix->ev[0], ix->ev[1]) == cudaSuccess) ix->search_ms += ms;
+    ix->ev_pending = false;
+}
+
 }  // namespace
 
 extern "C" {
@@ -223,7 +442,10 @@ int32_t gorse_b200_sparse_index_destroy(gorse_b200_sparse_index *ix)
     {
         ScopedDevice sd(ix->ctx->device);
         cudaStreamSynchronize(ix->ctx->stream);
-        ix->off.free(); ix->foff.free(); ix->ind.free(); ix->val.free(); ix->frow.free(); ix->fval.free(); ix->acc.free();
+        ix->off.free(); ix->foff.free(); ix->ind.free(); ix->val.free(); ix->frow.free(); ix->fval.free();
+        ix->tl_dot.free(); ix->tl_idx.free(); ix->tl_cnt.free(); ix->next.free(); ix->paths.free();
+        for (cudaEvent_t e : ix->ev)
+            if (e) cudaEventDestroy(e);
     }
     delete ix;
     return GORSE_B200_OK;
@@ -283,45 +505,94 @@ int32_t gorse_b200_sparse_index_search_range(gorse_b200_sparse_index *ix, int64_
     return gb::sparse_search_host(ix, q0, nq, nullptr, nullptr, nullptr, nullptr, k, idx_out, dot_out, count_out);
 }
 
+int32_t gorse_b200_sparse_index_stats(gorse_b200_sparse_index *ix, int64_t *push_items, int64_t *pull_items, int64_t *tiles, double *search_ms)
+{
+    GB_CHECK_ARG(ix != nullptr, "index is NULL");
+    std::lock_guard<std::mutex> lk(ix->mu);
+    ScopedDevice sd(ix->ctx->device);
+    cudaStream_t s = ix->ctx->stream;
+    fold_time(ix);
+    unsigned long long h[2] = {0, 0};
+    if (ix->paths.p) {
+        GB_CUDA(cudaMemcpyAsync(h, ix->paths.p, sizeof(h), cudaMemcpyDeviceToHost, s));
+        GB_CUDA(cudaMemsetAsync(ix->paths.p, 0, sizeof(h), s));
+        GB_CUDA(cudaStreamSynchronize(s));
+    }
+    if (push_items) *push_items = (int64_t)h[0];
+    if (pull_items) *pull_items = (int64_t)h[1];
+    if (tiles) *tiles = ix->tiles;
+    if (search_ms) *search_ms = ix->search_ms;
+    ix->tiles = 0;
+    ix->search_ms = 0.0;
+    return GORSE_B200_OK;
+}
+
 }  // extern "C"
 
 namespace gb {
 
-// queries = stored rows [q0, q0 + nq) (q_off == nullptr) or nq rows of a HOST CSR (q_off/q_ind/q_val); allow = optional DEVICE
-// per-row filter; results to host buffers.  The caller holds ix->mu.
-static constexpr int SEARCH_WARPS = 4;
+// the tile lists of a chunk take at most this many bytes; larger searches run in chunks of queries
+static constexpr int64_t TILE_LIST_BYTES = 512ll << 20;
 
-// one accumulator row per resident warp, at most ~1 GB of them; returns the grid of sparse_search_kernel
-static int32_t reserve_acc(gorse_b200_sparse_index *ix, int64_t n, int64_t nq, int *grid)
+// the tiled search of nq queries (see the top of this file) into the device buffers d_idx / d_dot [nq x k] and d_cnt[nq],
+// enqueued on the context's stream; the index holds at least one vector and its device layouts are current
+static int32_t tiled_search(gorse_b200_sparse_index *ix, const Queries &Q, int64_t nq, const uint8_t *d_allow, int k, int32_t *d_idx,
+                            float *d_dot, int32_t *d_cnt)
 {
     gorse_b200_ctx *c = ix->ctx;
-    const int warps = SEARCH_WARPS;
-    int64_t slots = std::min<int64_t>((nq + warps - 1) / warps * warps, (int64_t)c->sm_count * 4 * warps);
-    slots = std::max<int64_t>(warps, std::min<int64_t>(slots, ((1ll << 30) / 4 / std::max<int64_t>(1, n)) / warps * warps));
-    if (ix->acc_slots < slots) {
-        GB_TRY(ix->acc.alloc((size_t)slots * (size_t)n));
-        GB_CUDA(cudaMemsetAsync(ix->acc.p, 0, sizeof(float) * (size_t)slots * (size_t)n, c->stream));
-        ix->acc_slots = slots;
+    cudaStream_t s = c->stream;
+    const int64_t n = (int64_t)ix->h_off.size() - 1;
+    const int ntiles = div_up(n, TILE);
+    const int64_t nqc_max = std::max<int64_t>(1, std::min<int64_t>(nq, TILE_LIST_BYTES / ((int64_t)ntiles * (8 * k + 4))));
+    const int64_t chunks = (nq + nqc_max - 1) / nqc_max;
+    const size_t lists = (size_t)nqc_max * ntiles;
+    if (ix->tl_cnt.n < lists) GB_TRY(ix->tl_cnt.alloc(lists));
+    if (ix->tl_dot.n < lists * k) {
+        GB_TRY(ix->tl_dot.alloc(lists * k));
+        GB_TRY(ix->tl_idx.alloc(lists * k));
     }
-    *grid = (int)(slots / warps);
+    if (ix->next.n < (size_t)chunks) GB_TRY(ix->next.alloc((size_t)chunks));
+    if (!ix->paths.p) {
+        GB_TRY(ix->paths.alloc(2));
+        GB_CUDA(cudaMemsetAsync(ix->paths.p, 0, ix->paths.bytes(), s));
+    }
+    for (cudaEvent_t &e : ix->ev)
+        if (!e) GB_CUDA(cudaEventCreate(&e));
+    const size_t tile_smem = sizeof(float) * TILE + sizeof(uint32_t) * (TILE / 32) + (2 * sizeof(int64_t) + sizeof(float)) * NT +
+                             (size_t)2 * NW * k * (sizeof(float) + sizeof(int32_t));
+    const size_t merge_smem = (size_t)MERGE_WARPS * 3 * k * (sizeof(float) + sizeof(int32_t));
+    GB_CUDA(cudaFuncSetAttribute(sparse_tile_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tile_smem));
+    int per_sm = 0;
+    GB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, sparse_tile_kernel, NT, tile_smem));
+    const int64_t grid = (int64_t)c->sm_count * std::max(1, per_sm);
+    fold_time(ix);
+    GB_CUDA(cudaMemsetAsync(ix->next.p, 0, sizeof(unsigned long long) * (size_t)chunks, s));
+    GB_CUDA(cudaEventRecord(ix->ev[0], s));
+    const Stored S{ix->off.p, ix->ind.p, ix->val.p, ix->foff.p, ix->frow.p, ix->fval.p, n, ix->n_features};
+    for (int64_t ch = 0; ch < chunks; ch++) {
+        const int64_t qc0 = ch * nqc_max, nqc = std::min(nqc_max, nq - qc0);
+        sparse_tile_kernel<<<(unsigned)std::min<int64_t>(grid, nqc * ntiles), NT, tile_smem, s>>>(
+            S, Q, qc0, nqc, ntiles, k, d_allow, ix->next.p + ch, ix->tl_dot.p, ix->tl_idx.p, ix->tl_cnt.p, ix->paths.p);
+        GB_LAUNCHED(c);
+        sparse_merge_kernel<<<div_up(nqc, MERGE_WARPS), 32 * MERGE_WARPS, merge_smem, s>>>(qc0, nqc, ntiles, k, ix->tl_dot.p, ix->tl_idx.p,
+                                                                                         ix->tl_cnt.p, d_idx, d_dot, d_cnt);
+        GB_LAUNCHED(c);
+    }
+    GB_CUDA(cudaEventRecord(ix->ev[1], s));
+    ix->ev_pending = true;
+    ix->tiles += ntiles * chunks;
     return GORSE_B200_OK;
 }
 
 int32_t sparse_search_rows(gorse_b200_sparse_index *ix, const int64_t *d_rows, int64_t nq, const uint8_t *d_allow, int32_t k, int32_t *d_idx,
                            float *d_dot, int32_t *d_cnt)
 {
-    const int64_t n = (int64_t)ix->h_off.size() - 1;
-    gorse_b200_ctx *c = ix->ctx;
     GB_TRY(sync_device(ix));
-    int grid = 0;
-    GB_TRY(reserve_acc(ix, n, nq, &grid));
-    sparse_search_kernel<true><<<grid, 32 * SEARCH_WARPS, (size_t)SEARCH_WARPS * 2 * (size_t)k * 4, c->stream>>>(
-        ix->off.p, ix->ind.p, ix->val.p, ix->foff.p, ix->frow.p, ix->fval.p, n, ix->n_features, 0, nq, k, ix->acc.p, d_idx, d_dot, d_cnt,
-        nullptr, nullptr, nullptr, d_allow, d_rows);
-    GB_LAUNCHED(c);
-    return GORSE_B200_OK;
+    return tiled_search(ix, Queries{nullptr, nullptr, nullptr, d_rows, 0}, nq, d_allow, k, d_idx, d_dot, d_cnt);
 }
 
+// queries = stored rows [q0, q0 + nq) (q_off == nullptr) or nq rows of a HOST CSR (q_off/q_ind/q_val); allow = optional DEVICE
+// per-row filter; results to host buffers.  The caller holds ix->mu.
 int32_t sparse_search_host(gorse_b200_sparse_index *ix, int64_t q0, int64_t nq, const int64_t *q_off, const uint32_t *q_ind,
                            const float *q_val, const uint8_t *d_allow, int32_t k, int32_t *idx_out, float *dot_out, int32_t *count_out)
 {
@@ -333,9 +604,6 @@ int32_t sparse_search_host(gorse_b200_sparse_index *ix, int64_t q0, int64_t nq, 
         for (int64_t q = 0; q < nq; q++) count_out[q] = 0;
         return GORSE_B200_OK;
     }
-    const int warps = SEARCH_WARPS;
-    int grid = 0;
-    GB_TRY(reserve_acc(ix, n, nq, &grid));
     DevBuf<int32_t> d_idx, d_cnt;
     DevBuf<float> d_dot, dq_val;
     DevBuf<int64_t> dq_off;
@@ -352,13 +620,9 @@ int32_t sparse_search_host(gorse_b200_sparse_index *ix, int64_t q0, int64_t nq, 
         if (e == cudaSuccess && qn) e = cudaMemcpyAsync(dq_val.p, q_val, sizeof(float) * (size_t)qn, cudaMemcpyHostToDevice, c->stream);
         if (e != cudaSuccess) { set_error("sparse search upload: %s", cudaGetErrorString(e)); return done(GORSE_B200_ERR_CUDA); }
     }
-    const size_t sm = (size_t)warps * 2 * (size_t)k * 4;
-    sparse_search_kernel<false><<<grid, 32 * warps, sm, c->stream>>>(ix->off.p, ix->ind.p, ix->val.p, ix->foff.p, ix->frow.p, ix->fval.p, n,
-                                                             ix->n_features, q0, nq, k, ix->acc.p, d_idx.p, d_dot.p, d_cnt.p,
-                                                             q_off ? dq_off.p : nullptr, dq_ind.p, dq_val.p, d_allow, nullptr);
-    c->launches++;
-    e = cudaGetLastError();
-    if (e == cudaSuccess) e = cudaMemcpyAsync(idx_out, d_idx.p, sizeof(int32_t) * (size_t)nq * k, cudaMemcpyDeviceToHost, c->stream);
+    const Queries Q = q_off ? Queries{dq_off.p, dq_ind.p, dq_val.p, nullptr, 0} : Queries{nullptr, nullptr, nullptr, nullptr, q0};
+    if ((st = tiled_search(ix, Q, nq, d_allow, k, d_idx.p, d_dot.p, d_cnt.p))) return done(st);
+    e = cudaMemcpyAsync(idx_out, d_idx.p, sizeof(int32_t) * (size_t)nq * k, cudaMemcpyDeviceToHost, c->stream);
     if (e == cudaSuccess) e = cudaMemcpyAsync(dot_out, d_dot.p, sizeof(float) * (size_t)nq * k, cudaMemcpyDeviceToHost, c->stream);
     if (e == cudaSuccess) e = cudaMemcpyAsync(count_out, d_cnt.p, sizeof(int32_t) * (size_t)nq, cudaMemcpyDeviceToHost, c->stream);
     if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
@@ -421,14 +685,14 @@ int32_t sparse_compact(gorse_b200_sparse_index *ix, const int64_t *scan, int64_t
     ix->off.free(); ix->foff.free(); ix->ind.free(); ix->val.free(); ix->frow.free(); ix->fval.free();
     ix->off = off_n; ix->foff = foff_n; ix->ind = ind_n; ix->val = val_n; ix->frow = frow_n; ix->fval = fval_n;
     ix->h_off.swap(h_off); ix->h_ind.swap(h_ind); ix->h_val.swap(h_val);
-    ix->acc.free();   // [slots x N]; reserve_acc allocates and zeroes it again for the new N
-    ix->acc_slots = 0;
+    ix->tl_dot.free(); ix->tl_idx.free(); ix->tl_cnt.free(); ix->next.free();   // sized for the old N; the next search allocates them
     return done(GORSE_B200_OK);
 }
 
 size_t sparse_bytes(const gorse_b200_sparse_index *ix)
 {
-    return ix->off.bytes() + ix->foff.bytes() + ix->ind.bytes() + ix->val.bytes() + ix->frow.bytes() + ix->fval.bytes() + ix->acc.bytes();
+    return ix->off.bytes() + ix->foff.bytes() + ix->ind.bytes() + ix->val.bytes() + ix->frow.bytes() + ix->fval.bytes() + ix->tl_dot.bytes() +
+           ix->tl_idx.bytes() + ix->tl_cnt.bytes() + ix->next.bytes() + ix->paths.bytes();
 }
 
 }  // namespace gb

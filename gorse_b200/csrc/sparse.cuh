@@ -18,8 +18,16 @@ struct gorse_b200_sparse_index {
     gb::DevBuf<uint32_t> ind;
     gb::DevBuf<float> val, fval;
     gb::DevBuf<int32_t> frow;
-    gb::DevBuf<float> acc;
-    int64_t acc_slots = 0;
+    // grow-only work buffers of the tiled search: each (query, tile) work item's best k (tl_*), the chunks' work-item
+    // counters (next) and the push / pull work-item counts since the last gorse_b200_sparse_index_stats (paths)
+    gb::DevBuf<float> tl_dot;
+    gb::DevBuf<int32_t> tl_idx, tl_cnt;
+    gb::DevBuf<unsigned long long> next, paths;
+    // measurement: events around the last search (folded into search_ms by the next search or the stats call)
+    cudaEvent_t ev[2] = {nullptr, nullptr};
+    bool ev_pending = false;
+    double search_ms = 0.0;
+    int64_t tiles = 0;
 };
 
 
@@ -33,7 +41,7 @@ int32_t sparse_search_rows(gorse_b200_sparse_index *ix, const int64_t *d_rows, i
                            float *d_dot, int32_t *d_cnt);
 // compaction (gorse_b200_vecdb_compact): scan[n + 1] (device) is the exclusive sum of the live flags (row r is live iff
 // scan[r + 1] != scan[r] and then becomes row scan[r]), live = scan[n].  Both layouts are compacted on the device, the host
-// CSR is replaced by the compacted one and the index ends clean; the accumulator is released.  On an error the rows are
+// CSR is replaced by the compacted one and the index ends clean; the search's work buffers are released.  On an error the rows are
 // unchanged (the device mirrors may have been brought up to date).  The caller holds ix->mu and the device.
 int32_t sparse_compact(gorse_b200_sparse_index *ix, const int64_t *scan, int64_t live);
 // device bytes held by the index

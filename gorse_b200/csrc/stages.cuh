@@ -11,7 +11,7 @@
 namespace gb {
 
 constexpr int MAX_N_DENSE = 1024;                // the sort buffer of agg::select_first_n holds n (session: top) entries
-constexpr int MAX_N_SPARSE = 128;                // sparse_search_kernel's k
+constexpr int MAX_N_SPARSE = 128;                // the sparse search's k
 
 // stage A of every neighbour recommender: the first n neighbours of each of the R stored vectors d_nb[R] (device) of db, as
 // a table of n (int32 slot, float32 score) entries per row, Dot collections keeping scores > 0 only (dense: the index's top-k

@@ -349,6 +349,12 @@ int32_t gorse_b200_sparse_index_len(const gorse_b200_sparse_index *ix, int64_t *
  * Feed a row to gorse_b200_similar_scores with GORSE_B200_METRIC_NEG_DOT after negating the dots. */
 int32_t gorse_b200_sparse_index_search_range(gorse_b200_sparse_index *ix, int64_t q0, int64_t q1, int32_t k, int32_t *idx_out,
                                              float *dot_out, int32_t *count_out);
+/* measurement hook, like gorse_b200_index_stats: since the previous call, over every search of the index (search_range, the
+ * collection's query and the neighbour stages of item-to-item, user-to-user, session recommendation and gorse_b200_recommend):
+ * the (query, tile) work items accumulated by the push path (a query's posting lists added into the tile) and by the pull path
+ * (each row of the tile merge-joined against the query), the tiles walked (tiles of 8192 stored rows, per chunk of queries) and
+ * the device time (ms) of the searches.  Any pointer may be NULL; the answers do not depend on it. */
+int32_t gorse_b200_sparse_index_stats(gorse_b200_sparse_index *ix, int64_t *push_items, int64_t *pull_items, int64_t *tiles, double *search_ms);
 
 /* ------------------------------------------------------------------------------------------
  * Vector collection: the GPU backend of vectors.Database (storage/vectors/database.go:107-120; semantics of the

@@ -7,9 +7,9 @@ Data: bench.py's c2 (synth.make_feedback(1M, 100K, 11M, seed=1000, exact=True) +
 user-to-user collections over the users, slot = user id:
   embedding  dense Euclidean, all 1M users: the user factors of 20 BPR epochs truncated to bf16 -- a stand-in for an
              embedding column
-  items      sparse Dot, the first 100,000 users: each user's training items with weights sqrt(log(1 + U / freq(i))) through
-             gb.sparse_vector, as the "items" type builds them (logics/user_to_user.go, appendSparseVector).  Smaller because
-             the sparse search scans an N-long accumulator row per query.
+  items      sparse Dot, all users (--sparse-users takes the first ones): each user's training items with weights
+             sqrt(log(1 + U / freq(i))) through gb.sparse_vector, as the "items" type builds them (logics/user_to_user.go,
+             appendSparseVector).
 Feedback = the training rows (item indices), exclusions = the user's own training row, about 8 % of the items have
 item_ok = 0 (seeded), n = 100, users in batches of 131,072 as a worker would send its shard.  Before timing, a seeded sample
 of users is checked against a restatement of recommendUserToUser over the oracle's brute force.
@@ -57,7 +57,7 @@ def main():
     ap.add_argument("--epochs", type=int, default=20)
     ap.add_argument("--check", type=int, default=32, help="users per collection checked against the oracle")
     ap.add_argument("--per-user-users", type=int, default=1024)
-    ap.add_argument("--sparse-users", type=int, default=100_000)
+    ap.add_argument("--sparse-users", type=int, default=None, help="the first users in the sparse collection (default: all)")
     args = ap.parse_args()
 
     import gorse_b200 as gb
@@ -82,7 +82,7 @@ def main():
             P, _ = m.get_factors()
         X = gb.bf16_truncate(P)
         log("model trained")
-        Us = min(args.sparse_users, U)
+        Us = U if args.sparse_users is None else min(args.sparse_users, U)
         freq = np.bincount(items, minlength=I).astype(np.float64)
         idf = np.log(1 + U / np.maximum(freq, 1)).astype(np.float32)
         sp = [gb.sparse_vector(items[off[u]:off[u + 1]], idf) for u in range(Us)]
