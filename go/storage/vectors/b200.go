@@ -378,6 +378,18 @@ func (db *B200) QueryVectors(ctx context.Context, name string, q Vector, categor
 		}
 		want = append(want, id)
 	}
+	// no answer holds more than the live vectors: a large topK (the REST neighbour endpoints ask for
+	// max(offset+n+|read items|, CacheSize)+1) allocates no more than the collection's size
+	var live, total C.int64_t
+	if err := b200Err(C.gorse_b200_vecdb_count(c.handle, &live, &total)); err != nil {
+		return nil, err
+	}
+	if int64(topK) > int64(live) {
+		topK = int(live)
+	}
+	if topK == 0 {
+		return []ScoredVector{}, nil
+	}
 	slots, scores := make([]int64, topK), make([]float32, topK)
 	var count C.int32_t
 	var qOff []int64

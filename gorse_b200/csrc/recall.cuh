@@ -1,12 +1,20 @@
 // recall.cuh -- block-wide selection and sorting helpers of the top-k pipeline (topk.cu), shared with the item-to-item
-// aggregation (item_to_item.cu).
+// aggregation (item_to_item.cu) and the sparse search (sparse.cu).
 #pragma once
 #include "common.cuh"
+#include "topk.cuh"
 
 namespace gb {
 namespace recall {
 
+constexpr int SORT_CAP = mma::CAP;   // entries one CTA sorts at a time (a window never holds more)
+
 #ifdef __CUDACC__
+// order key of a score: larger score = larger key; -0 and +0 are one score (the exact scan compares floats); NaN = 0 = no entry
+__device__ __forceinline__ uint32_t rank_key(float s) { return s != s ? 0u : float_key(s == 0.f ? 0.f : s); }
+// sort key: ascending order = score descending, then slot ascending
+__device__ __forceinline__ uint64_t sort_key(uint32_t key, int64_t slot) { return ((uint64_t)~key << 32) | (uint32_t)slot; }
+
 __device__ __forceinline__ bool contains(const int64_t *a, int64_t n, int64_t v)
 {
     int64_t lo = 0, hi = n;
@@ -131,6 +139,44 @@ __host__ __device__ __forceinline__ int pow2_at_least(int m)
     int p = 1;
     while (p < m) p <<= 1;
     return p;
+}
+
+// The first K entries of the score row sc[0, N) by (score desc, slot asc), K <= its non-NaN entries, in sorted rounds of at
+// most SORT_CAP: each round radix-selects its last key, gathers its entries into s_key / s_val [SORT_CAP] (those equal to the
+// last key in slot order: the lowest slots win the tie), sorts them, hands them to emit(m) and retires them (sc = NaN).
+// Every thread calls it.
+template <int NT, typename Emit>
+__device__ __forceinline__ void emit_in_rounds(float *sc, int64_t N, int K, uint64_t *s_key, float *s_val, int *hist, int *s_warp, int *s_bc,
+                                               Emit emit)
+{
+    const float none = __int_as_float(0x7fffffff);   // NaN: rank_key 0
+    for (int emitted = 0; emitted < K;) {
+        const int m = min(SORT_CAP, K - emitted);
+        int ties;
+        const uint32_t t = block_select<NT>(N, m, [&](int64_t j) { return rank_key(sc[j]); }, hist, s_bc, &ties);
+        if (threadIdx.x == 0) s_bc[2] = 0;
+        int eq_taken = 0;   // entries equal to t go in slot order: the lowest slots win the tie
+        __syncthreads();
+        for (int64_t base = 0; base < N; base += NT) {
+            const int64_t j = base + threadIdx.x;
+            const uint32_t key = j < N ? rank_key(sc[j]) : 0u;
+            int n_eq;
+            const int er = block_rank<NT>(key == t, s_warp, n_eq);
+            int pos = -1;
+            if (key > t) pos = atomicAdd(&s_bc[2], 1);
+            else if (key == t && eq_taken + er < ties) pos = m - ties + eq_taken + er;
+            if (pos >= 0) { s_key[pos] = sort_key(key, j); s_val[pos] = sc[j]; }
+            eq_taken += n_eq;
+        }
+        const int p2 = pow2_at_least(m);
+        for (int j = m + threadIdx.x; j < p2; j += NT) s_key[j] = ~0ull;
+        __syncthreads();
+        block_sort<NT>(s_key, s_val, p2);
+        emit(m);
+        for (int j = threadIdx.x; j < m; j += NT) sc[(uint32_t)s_key[j]] = none;
+        __syncthreads();
+        emitted += m;
+    }
 }
 
 #endif  // __CUDACC__

@@ -20,10 +20,15 @@
 // its answer.  Rows with dot <= 0 are never returned (the reference drops them right after the query,
 // logics/item_to_item.go:73).  Work items are taken tile-major, so the queries of one tile run together and reuse the tile's
 // posting ranges from L2, and a heavy query spreads over as many CTAs as it has tiles.
+//
+// k > 128 (the wide path): the lists do not stretch that far, so the same work items write each query's score row [n] instead
+// (the dot of every candidate, NaN for every other row), and one CTA per query emits the answer in sorted rounds of at most
+// 2048 with the dense exact kernel's emission (recall::emit_in_rounds).
 #include <algorithm>
 
 #include <cub/cub.cuh>
 
+#include "recall.cuh"
 #include "sparse.cuh"
 
 using namespace gb;
@@ -89,6 +94,8 @@ __device__ __forceinline__ int merge_warp(const float *ad, const int32_t *ai, in
 constexpr int TILE = 8192;              // rows per tile: a 32 KB accumulator, four CTAs per SM
 constexpr int NT = 256, NW = NT / 32;   // threads / warps of a work item's CTA; NT features per batch of posting ranges
 constexpr int MERGE_WARPS = 4;
+constexpr int LIST_K = 128;            // the largest k the warps' lists hold; larger k take the wide path
+constexpr int EMIT_THREADS = 256;
 
 struct Stored {   // the index's device layouts
     const int64_t *off; const uint32_t *ind; const float *val;    // CSR
@@ -125,11 +132,14 @@ __device__ __forceinline__ int64_t block_sum(int64_t v, int64_t *red)
     return s;
 }
 
-// one CTA per work item at a time, work items w = t * nqc + q (tile-major) taken from *next; the tile list of w goes to
-// tl_dot / tl_idx [w * k ...] (negated dots, best first) and tl_cnt[w]; paths[0] / [1] count the push / pull work items
+// one CTA per work item at a time, work items w = t * nqc + q (tile-major) taken from *next; paths[0] / [1] count the push /
+// pull work items.  The list instance (k <= 128) writes the tile list of w to tl_dot / tl_idx [w * k ...] (negated dots, best
+// first) and tl_cnt[w].  The wide instance writes the tile's segment of the query's score row sc[(q - qc0) * n ...]: the dot
+// of every candidate (positive, allowed, not the query itself), NaN for every other row; it adds the candidates to have[q - qc0].
+template <bool WIDE>
 __global__ void __launch_bounds__(NT, 4)
 sparse_tile_kernel(Stored S, Queries Q, int64_t qc0, int64_t nqc, int ntiles, int k, const uint8_t *allow, unsigned long long *next,
-                   float *tl_dot, int32_t *tl_idx, int32_t *tl_cnt, unsigned long long *paths)
+                   float *tl_dot, int32_t *tl_idx, int32_t *tl_cnt, unsigned long long *paths, float *sc, int32_t *have)
 {
     extern __shared__ __align__(16) unsigned char sm_raw[];
     float *acc = reinterpret_cast<float *>(sm_raw);                        // [TILE], zero between work items
@@ -137,7 +147,7 @@ sparse_tile_kernel(Stored S, Queries Q, int64_t qc0, int64_t nqc, int ntiles, in
     int64_t *r_lo = reinterpret_cast<int64_t *>(bits + TILE / 32);          // [NT] a batch of posting ranges and query values
     int64_t *r_hi = r_lo + NT;
     float *r_v = reinterpret_cast<float *>(r_hi + NT);
-    float *ld = r_v + NT;                                                    // [2][NW][k] the warps' lists, two buffers
+    float *ld = r_v + NT;                                                    // [2][NW][k] the warps' lists, two buffers (list instance)
     int32_t *li = reinterpret_cast<int32_t *>(ld + 2 * NW * k);
     __shared__ int64_t red[NW];
     __shared__ int lens[2][NW];
@@ -177,6 +187,8 @@ sparse_tile_kernel(Stored S, Queries Q, int64_t qc0, int64_t nqc, int ntiles, in
         float *wd = ld + wid * k;
         int32_t *wi = li + wid * k;
         int len = 0;   // this warp's list, warp-uniform
+        float *out = sc + (q - qc0) * S.n;   // the wide instance's score row
+        int64_t found = 0;                   // and this thread's candidates in it
         const bool pull = push_cost > pull_cost;
         if (push_cost == 0) {
             // the query shares no feature with the tile: nothing to add
@@ -202,15 +214,15 @@ sparse_tile_kernel(Stored S, Queries Q, int64_t qc0, int64_t nqc, int ntiles, in
                     for (int64_t p = plo + tid; p < phi; p += NT) {
                         const int c = S.frow[p] - (int)c0;
                         acc[c] = acc[c] + fv * S.fval[p];   // unfused multiply and add, like the oracle (-fmad=false)
-                        atomicOr(&bits[c >> 5], 1u << (c & 31));
+                        if (!WIDE) atomicOr(&bits[c >> 5], 1u << (c & 31));
                     }
                     __syncthreads();   // the next feature adds after this one: each sum in ascending feature order
                 }
                 __syncthreads();
             }
             // thread tid owns bitmap word tid (TILE / 32 == NT): its touched rows, read and cleared
-            uint32_t m = bits[tid];
-            bits[tid] = 0u;
+            uint32_t m = WIDE ? 0u : bits[tid];
+            if (!WIDE) bits[tid] = 0u;
             while (__any_sync(0xffffffffu, m != 0u)) {
                 float x = 0.f;
                 int32_t c = -1;
@@ -262,9 +274,31 @@ sparse_tile_kernel(Stored S, Queries Q, int64_t qc0, int64_t nqc, int ntiles, in
                     }
                     lo = __shfl_sync(0xffffffffu, pos, 31);
                 }
-                if (s > 0.f && r != row && (allow == nullptr || allow[r] != 0) && (len < k || before(-s, (int32_t)r, wd[k - 1], wi[k - 1])))
+                const bool cand = s > 0.f && r != row && (allow == nullptr || allow[r] != 0);
+                if (WIDE) {
+                    if (lane == 0) { out[r] = cand ? s : __int_as_float(0x7fffffff); found += cand; }
+                } else if (cand && (len < k || before(-s, (int32_t)r, wd[k - 1], wi[k - 1]))) {
                     list_insert_warp(wd, wi, len, k, -s, (int32_t)r, lane);
+                }
             }
+        }
+        if constexpr (WIDE) {
+            if (!pull)   // the push (or no feature in common) left the tile's dots in acc: every row of the tile, acc cleared
+                for (int i = tid; i < c1 - c0; i += NT) {
+                    const float x = acc[i];
+                    acc[i] = 0.f;
+                    const int64_t c = c0 + i;
+                    const bool cand = x > 0.f && c != row && (allow == nullptr || allow[c] != 0);
+                    out[c] = cand ? x : __int_as_float(0x7fffffff);
+                    found += cand;
+                }
+            found = block_sum(found, red);
+            if (tid == 0) {
+                atomicAdd(&have[q - qc0], (int32_t)found);
+                if (push_cost) atomicAdd(&paths[pull], 1ull);
+            }
+            __syncthreads();   // acc and `item` are reused by the next work item
+            continue;
         }
         // the warps' lists pairwise into one: NW -> NW / 2 -> ... -> 1, alternating buffers
         if (lane == 0) lens[0][wid] = len;
@@ -325,6 +359,35 @@ sparse_merge_kernel(int64_t qc0, int64_t nqc, int ntiles, int k, const float *tl
         out_dot[o + e] = has ? -bd[cur * k + e] : 0.f;
     }
     if (lane == 0) out_cnt[qc0 + q] = len;
+}
+
+// the wide path's answers: one CTA per query of the chunk emits the first min(k, have) entries of its score row in sorted
+// rounds (recall::emit_in_rounds, the exact kernel's emission) into out_*[(qc0 + q) * k ...], padded with -1 / 0; out_cnt holds
+// the chunk's candidate counts have[] on entry and the answers' lengths on exit
+__global__ void __launch_bounds__(EMIT_THREADS)
+sparse_emit_kernel(int64_t qc0, int64_t n, int k, float *sc, int32_t *out_idx, float *out_dot, int32_t *out_cnt)
+{
+    using namespace recall;
+    constexpr int T = EMIT_THREADS;
+    extern __shared__ __align__(16) unsigned char sm_raw[];
+    uint64_t *s_key = reinterpret_cast<uint64_t *>(sm_raw);         // [SORT_CAP]
+    float *s_val = reinterpret_cast<float *>(s_key + SORT_CAP);     // [SORT_CAP]
+    int *hist = reinterpret_cast<int *>(s_val + SORT_CAP);          // [256]
+    int *s_warp = hist + 256;                                       // [32]
+    int *s_bc = s_warp + 32;                                        // [4]
+    const int64_t q = qc0 + blockIdx.x, o = q * k;
+    const int K = min(k, out_cnt[q]);
+    __syncthreads();   // every thread has read out_cnt[q] before thread 0 overwrites it
+    int written = 0;
+    emit_in_rounds<T>(sc + (int64_t)blockIdx.x * n, n, K, s_key, s_val, hist, s_warp, s_bc, [&](int m) {
+        for (int i = threadIdx.x; i < m; i += T) {
+            out_idx[o + written + i] = (int32_t)(uint32_t)s_key[i];
+            out_dot[o + written + i] = s_val[i];
+        }
+        written += m;
+    });
+    for (int e = K + threadIdx.x; e < k; e += T) { out_idx[o + e] = -1; out_dot[o + e] = 0.f; }
+    if (threadIdx.x == 0) out_cnt[q] = K;
 }
 
 int32_t sync_device(gorse_b200_sparse_index *ix)
@@ -492,7 +555,7 @@ int32_t gorse_b200_sparse_index_search_range(gorse_b200_sparse_index *ix, int64_
                                              float *dot_out, int32_t *count_out)
 {
     GB_CHECK_ARG(ix != nullptr, "index is NULL");
-    GB_CHECK_ARG(k > 0 && k <= 128, "k must be in 1..128 (got %d)", k);
+    GB_CHECK_ARG(k > 0, "k must be positive (got %d)", k);
     std::lock_guard<std::mutex> lk(ix->mu);
     const int64_t n = (int64_t)ix->h_off.size() - 1;
     if (q0 < 0 || q1 < q0 || q1 > n) {
@@ -531,11 +594,14 @@ int32_t gorse_b200_sparse_index_stats(gorse_b200_sparse_index *ix, int64_t *push
 
 namespace gb {
 
-// the tile lists of a chunk take at most this many bytes; larger searches run in chunks of queries
+// the tile lists (k <= 128) or the score rows (k > 128) of a chunk take at most this many bytes; larger searches run in chunks
+// of queries, at least one query per chunk
 static constexpr int64_t TILE_LIST_BYTES = 512ll << 20;
 
 // the tiled search of nq queries (see the top of this file) into the device buffers d_idx / d_dot [nq x k] and d_cnt[nq],
-// enqueued on the context's stream; the index holds at least one vector and its device layouts are current
+// enqueued on the context's stream; the index holds at least one vector and its device layouts are current.  k <= 128: the
+// work items keep tile lists and a merge kernel folds them.  k > 128 (the wide path): the work items write each query's score
+// row [n], and one CTA per query emits its answer in sorted rounds.
 static int32_t tiled_search(gorse_b200_sparse_index *ix, const Queries &Q, int64_t nq, const uint8_t *d_allow, int k, int32_t *d_idx,
                             float *d_dot, int32_t *d_cnt)
 {
@@ -543,13 +609,17 @@ static int32_t tiled_search(gorse_b200_sparse_index *ix, const Queries &Q, int64
     cudaStream_t s = c->stream;
     const int64_t n = (int64_t)ix->h_off.size() - 1;
     const int ntiles = div_up(n, TILE);
-    const int64_t nqc_max = std::max<int64_t>(1, std::min<int64_t>(nq, TILE_LIST_BYTES / ((int64_t)ntiles * (8 * k + 4))));
+    const bool wide = k > LIST_K;
+    const int64_t per_query = wide ? (int64_t)sizeof(float) * n : (int64_t)ntiles * (8 * k + 4);
+    const int64_t nqc_max = std::max<int64_t>(1, std::min<int64_t>(nq, TILE_LIST_BYTES / per_query));
     const int64_t chunks = (nq + nqc_max - 1) / nqc_max;
     const size_t lists = (size_t)nqc_max * ntiles;
-    if (ix->tl_cnt.n < lists) GB_TRY(ix->tl_cnt.alloc(lists));
-    if (ix->tl_dot.n < lists * k) {
-        GB_TRY(ix->tl_dot.alloc(lists * k));
-        GB_TRY(ix->tl_idx.alloc(lists * k));
+    if (wide) {   // the score rows take the tile lists' dot buffer
+        if (ix->tl_dot.n < (size_t)nqc_max * n) GB_TRY(ix->tl_dot.alloc((size_t)nqc_max * n));
+    } else {
+        if (ix->tl_cnt.n < lists) GB_TRY(ix->tl_cnt.alloc(lists));
+        if (ix->tl_dot.n < lists * k) GB_TRY(ix->tl_dot.alloc(lists * k));
+        if (ix->tl_idx.n < lists * k) GB_TRY(ix->tl_idx.alloc(lists * k));
     }
     if (ix->next.n < (size_t)chunks) GB_TRY(ix->next.alloc((size_t)chunks));
     if (!ix->paths.p) {
@@ -559,23 +629,29 @@ static int32_t tiled_search(gorse_b200_sparse_index *ix, const Queries &Q, int64
     for (cudaEvent_t &e : ix->ev)
         if (!e) GB_CUDA(cudaEventCreate(&e));
     const size_t tile_smem = sizeof(float) * TILE + sizeof(uint32_t) * (TILE / 32) + (2 * sizeof(int64_t) + sizeof(float)) * NT +
-                             (size_t)2 * NW * k * (sizeof(float) + sizeof(int32_t));
+                             (wide ? 0 : (size_t)2 * NW * k * (sizeof(float) + sizeof(int32_t)));
     const size_t merge_smem = (size_t)MERGE_WARPS * 3 * k * (sizeof(float) + sizeof(int32_t));
-    GB_CUDA(cudaFuncSetAttribute(sparse_tile_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tile_smem));
+    const size_t emit_smem = (size_t)recall::SORT_CAP * (sizeof(uint64_t) + sizeof(float)) + (256 + 32 + 4) * sizeof(int);
+    auto *tile_kernel = wide ? sparse_tile_kernel<true> : sparse_tile_kernel<false>;
+    GB_CUDA(cudaFuncSetAttribute(tile_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tile_smem));
     int per_sm = 0;
-    GB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, sparse_tile_kernel, NT, tile_smem));
+    GB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, tile_kernel, NT, tile_smem));
     const int64_t grid = (int64_t)c->sm_count * std::max(1, per_sm);
     fold_time(ix);
     GB_CUDA(cudaMemsetAsync(ix->next.p, 0, sizeof(unsigned long long) * (size_t)chunks, s));
+    if (wide) GB_CUDA(cudaMemsetAsync(d_cnt, 0, sizeof(int32_t) * (size_t)nq, s));   // the candidate counts
     GB_CUDA(cudaEventRecord(ix->ev[0], s));
     const Stored S{ix->off.p, ix->ind.p, ix->val.p, ix->foff.p, ix->frow.p, ix->fval.p, n, ix->n_features};
     for (int64_t ch = 0; ch < chunks; ch++) {
         const int64_t qc0 = ch * nqc_max, nqc = std::min(nqc_max, nq - qc0);
-        sparse_tile_kernel<<<(unsigned)std::min<int64_t>(grid, nqc * ntiles), NT, tile_smem, s>>>(
-            S, Q, qc0, nqc, ntiles, k, d_allow, ix->next.p + ch, ix->tl_dot.p, ix->tl_idx.p, ix->tl_cnt.p, ix->paths.p);
+        tile_kernel<<<(unsigned)std::min<int64_t>(grid, nqc * ntiles), NT, tile_smem, s>>>(
+            S, Q, qc0, nqc, ntiles, k, d_allow, ix->next.p + ch, ix->tl_dot.p, ix->tl_idx.p, ix->tl_cnt.p, ix->paths.p, ix->tl_dot.p, d_cnt + qc0);
         GB_LAUNCHED(c);
-        sparse_merge_kernel<<<div_up(nqc, MERGE_WARPS), 32 * MERGE_WARPS, merge_smem, s>>>(qc0, nqc, ntiles, k, ix->tl_dot.p, ix->tl_idx.p,
-                                                                                         ix->tl_cnt.p, d_idx, d_dot, d_cnt);
+        if (wide)
+            sparse_emit_kernel<<<(unsigned)nqc, EMIT_THREADS, emit_smem, s>>>(qc0, n, k, ix->tl_dot.p, d_idx, d_dot, d_cnt);
+        else
+            sparse_merge_kernel<<<div_up(nqc, MERGE_WARPS), 32 * MERGE_WARPS, merge_smem, s>>>(qc0, nqc, ntiles, k, ix->tl_dot.p, ix->tl_idx.p,
+                                                                                             ix->tl_cnt.p, d_idx, d_dot, d_cnt);
         GB_LAUNCHED(c);
     }
     GB_CUDA(cudaEventRecord(ix->ev[1], s));
@@ -604,13 +680,14 @@ int32_t sparse_search_host(gorse_b200_sparse_index *ix, int64_t q0, int64_t nq, 
         for (int64_t q = 0; q < nq; q++) count_out[q] = 0;
         return GORSE_B200_OK;
     }
+    const int kc = (int)std::min<int64_t>(k, n);   // no answer is longer than n: the device holds kc columns, the host rows k
     DevBuf<int32_t> d_idx, d_cnt;
     DevBuf<float> d_dot, dq_val;
     DevBuf<int64_t> dq_off;
     DevBuf<uint32_t> dq_ind;
     int32_t st = GORSE_B200_OK;
     auto done = [&](int32_t s) { cudaStreamSynchronize(c->stream); d_idx.free(); d_cnt.free(); d_dot.free(); dq_val.free(); dq_off.free(); dq_ind.free(); return s; };
-    if ((st = d_idx.alloc((size_t)nq * k)) || (st = d_dot.alloc((size_t)nq * k)) || (st = d_cnt.alloc((size_t)nq))) return done(st);
+    if ((st = d_idx.alloc((size_t)nq * kc)) || (st = d_dot.alloc((size_t)nq * kc)) || (st = d_cnt.alloc((size_t)nq))) return done(st);
     cudaError_t e = cudaSuccess;
     if (q_off) {
         const int64_t qn = q_off[nq];
@@ -621,12 +698,23 @@ int32_t sparse_search_host(gorse_b200_sparse_index *ix, int64_t q0, int64_t nq, 
         if (e != cudaSuccess) { set_error("sparse search upload: %s", cudaGetErrorString(e)); return done(GORSE_B200_ERR_CUDA); }
     }
     const Queries Q = q_off ? Queries{dq_off.p, dq_ind.p, dq_val.p, nullptr, 0} : Queries{nullptr, nullptr, nullptr, nullptr, q0};
-    if ((st = tiled_search(ix, Q, nq, d_allow, k, d_idx.p, d_dot.p, d_cnt.p))) return done(st);
-    e = cudaMemcpyAsync(idx_out, d_idx.p, sizeof(int32_t) * (size_t)nq * k, cudaMemcpyDeviceToHost, c->stream);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(dot_out, d_dot.p, sizeof(float) * (size_t)nq * k, cudaMemcpyDeviceToHost, c->stream);
+    if ((st = tiled_search(ix, Q, nq, d_allow, kc, d_idx.p, d_dot.p, d_cnt.p))) return done(st);
+    if (kc == k) {
+        e = cudaMemcpyAsync(idx_out, d_idx.p, sizeof(int32_t) * (size_t)nq * k, cudaMemcpyDeviceToHost, c->stream);
+        if (e == cudaSuccess) e = cudaMemcpyAsync(dot_out, d_dot.p, sizeof(float) * (size_t)nq * k, cudaMemcpyDeviceToHost, c->stream);
+    } else {
+        e = cudaMemcpy2DAsync(idx_out, sizeof(int32_t) * k, d_idx.p, sizeof(int32_t) * kc, sizeof(int32_t) * kc, (size_t)nq, cudaMemcpyDeviceToHost,
+                              c->stream);
+        if (e == cudaSuccess)
+            e = cudaMemcpy2DAsync(dot_out, sizeof(float) * k, d_dot.p, sizeof(float) * kc, sizeof(float) * kc, (size_t)nq, cudaMemcpyDeviceToHost, c->stream);
+    }
     if (e == cudaSuccess) e = cudaMemcpyAsync(count_out, d_cnt.p, sizeof(int32_t) * (size_t)nq, cudaMemcpyDeviceToHost, c->stream);
     if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
     if (e != cudaSuccess) { set_error("sparse search: %s", cudaGetErrorString(e)); return done(GORSE_B200_ERR_CUDA); }
+    for (int64_t q = 0; q < nq && kc < k; q++) {
+        std::fill(idx_out + q * k + kc, idx_out + (q + 1) * k, -1);
+        std::fill(dot_out + q * k + kc, dot_out + (q + 1) * k, 0.f);
+    }
     return done(GORSE_B200_OK);
 }
 

@@ -18,8 +18,9 @@ struct gorse_b200_sparse_index {
     gb::DevBuf<uint32_t> ind;
     gb::DevBuf<float> val, fval;
     gb::DevBuf<int32_t> frow;
-    // grow-only work buffers of the tiled search: each (query, tile) work item's best k (tl_*), the chunks' work-item
-    // counters (next) and the push / pull work-item counts since the last gorse_b200_sparse_index_stats (paths)
+    // grow-only work buffers of the tiled search: each (query, tile) work item's best k (tl_*; for k > 128, tl_dot holds the
+    // chunk's score rows instead), the chunks' work-item counters (next) and the push / pull work-item counts since the last
+    // gorse_b200_sparse_index_stats (paths)
     gb::DevBuf<float> tl_dot;
     gb::DevBuf<int32_t> tl_idx, tl_cnt;
     gb::DevBuf<unsigned long long> next, paths;

@@ -31,13 +31,7 @@ namespace recall {
 
 constexpr int N_CLASSES = 3;
 constexpr int CLASS_K[N_CLASSES] = {128, 256, 512};
-constexpr int SORT_CAP = mma::CAP;   // entries one CTA sorts at a time (a window never holds more)
 constexpr int WIN_THREADS = 256, EXACT_THREADS = 256;
-
-// order key of a score: larger score = larger key; -0 and +0 are one score (the exact scan compares floats); NaN = 0 = no entry
-__device__ __forceinline__ uint32_t rank_key(float s) { return s != s ? 0u : float_key(s == 0.f ? 0.f : s); }
-// sort key: ascending order = score descending, then slot ascending
-__device__ __forceinline__ uint64_t sort_key(uint32_t key, int64_t slot) { return ((uint64_t)~key << 32) | (uint32_t)slot; }
 
 struct RowInfo {              // per row of a chunk (chunk-local row ids)
     const float *q;           // [rows][d] queries
@@ -231,35 +225,10 @@ recall_exact_kernel(const float *X, int64_t N, int d, int metric, const uint8_t 
         have = block_sum<NT>(have, s_warp);   // (synchronises: sc is complete)
         const int K = min(R.k[r], have);
         int written = 0;
-        // rounds of at most SORT_CAP: select the round's last key, gather, sort, emit, then retire the emitted entries
-        for (int emitted = 0; emitted < K;) {
-            const int m = min(SORT_CAP, K - emitted);
-            int ties;
-            const uint32_t t = block_select<NT>(N, m, [&](int64_t j) { return rank_key(sc[j]); }, hist, s_bc, &ties);
-            if (threadIdx.x == 0) s_bc[2] = 0;
-            int eq_taken = 0;   // entries equal to t go in slot order: the lowest slots win the tie
-            __syncthreads();
-            for (int64_t base = 0; base < N; base += NT) {
-                const int64_t j = base + threadIdx.x;
-                const uint32_t key = j < N ? rank_key(sc[j]) : 0u;
-                int n_eq;
-                const int er = block_rank<NT>(key == t, s_warp, n_eq);
-                int pos = -1;
-                if (key > t) pos = atomicAdd(&s_bc[2], 1);
-                else if (key == t && eq_taken + er < ties) pos = m - ties + eq_taken + er;
-                if (pos >= 0) { s_key[pos] = sort_key(key, j); s_val[pos] = sc[j]; }
-                eq_taken += n_eq;
-            }
-            const int p2 = pow2_at_least(m);
-            for (int j = m + threadIdx.x; j < p2; j += NT) s_key[j] = ~0ull;
-            __syncthreads();
-            block_sort<NT>(s_key, s_val, p2);
+        emit_in_rounds<NT>(sc, N, K, s_key, s_val, hist, s_warp, s_bc, [&](int m) {
             block_emit<NT>(s_key, s_val, m, R.ex + R.ex_off[r], R.ex_off[r + 1] - R.ex_off[r], R.slots + R.out_off[r], R.scores + R.out_off[r],
                            written, s_warp);
-            for (int j = threadIdx.x; j < m; j += NT) sc[(uint32_t)s_key[j]] = none;
-            __syncthreads();
-            emitted += m;
-        }
+        });
         if (threadIdx.x == 0) R.count[r] = written;
         __syncthreads();
     }

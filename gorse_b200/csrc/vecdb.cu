@@ -349,16 +349,23 @@ int32_t gorse_b200_vecdb_query(gorse_b200_vecdb *db, int64_t nq, const float *q_
         return recall::recall_rows(db->dense, db->d_allow.p, nq, q_values, nullptr, topk, nullptr, nullptr, nullptr, nullptr, slots_out, scores_out,
                                    count_out, nullptr);   // no exclusions: row q at q * topk
     }
-    GB_CHECK_ARG(topk <= 128, "sparse collections answer topK <= 128 (got %d)", topk);
     for (int64_t q = 0; q < nq; q++)
         for (int64_t t = q_sp_off[q]; t < q_sp_off[q + 1]; t++)
             GB_CHECK_ARG(t == q_sp_off[q] || q_sp_indices[t] > q_sp_indices[t - 1], "query %lld: indices not strictly ascending", (long long)q);
-    std::vector<int32_t> idx((size_t)nq * topk);
+    // no answer is longer than the collection: the search answers kc columns, the rest of each row is padding
+    const int32_t kc = (int32_t)std::min<int64_t>(topk, n);
+    std::vector<int32_t> idx((size_t)nq * kc);
+    std::vector<float> dot(kc < topk ? (size_t)nq * kc : 0);
     {
         std::lock_guard<std::mutex> lk2(db->sparse->mu);
-        GB_TRY(sparse_search_host(db->sparse, 0, nq, q_sp_off, q_sp_indices, q_values, db->d_allow.p, topk, idx.data(), scores_out, count_out));
+        GB_TRY(sparse_search_host(db->sparse, 0, nq, q_sp_off, q_sp_indices, q_values, db->d_allow.p, kc, idx.data(), kc < topk ? dot.data() : scores_out,
+                                  count_out));
     }
-    for (int64_t t = 0; t < nq * topk; t++) slots_out[t] = idx[(size_t)t];
+    for (int64_t q = 0; q < nq; q++)
+        for (int64_t t = 0; t < topk; t++) {
+            slots_out[q * topk + t] = t < kc ? idx[(size_t)(q * kc + t)] : -1;
+            if (kc < topk) scores_out[q * topk + t] = t < kc ? dot[(size_t)(q * kc + t)] : 0.f;
+        }
     return GORSE_B200_OK;
 }
 

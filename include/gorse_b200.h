@@ -344,9 +344,10 @@ int32_t gorse_b200_sparse_index_destroy(gorse_b200_sparse_index *ix);
 int32_t gorse_b200_sparse_index_add(gorse_b200_sparse_index *ix, const int64_t *off, const uint32_t *indices, const float *values,
                                     int64_t n, int64_t *count_out);
 int32_t gorse_b200_sparse_index_len(const gorse_b200_sparse_index *ix, int64_t *count_out);
-/* the k (<= 128) stored vectors with the largest POSITIVE dot with each stored vector in [q0, q1), the vector
- * itself excluded; best first (ties: lower index first); idx_out/dot_out are (q1-q0) x k padded with -1 / 0.
- * Feed a row to gorse_b200_similar_scores with GORSE_B200_METRIC_NEG_DOT after negating the dots. */
+/* the k (any k >= 1) stored vectors with the largest POSITIVE dot with each stored vector in [q0, q1), the vector
+ * itself excluded; best first (ties: lower index first); idx_out/dot_out are (q1-q0) x k padded with -1 / 0, and count_out
+ * may be less than k.  The device holds min(k, stored vectors) columns per row, so a k past the index's size costs no more
+ * device memory than its size.  Feed a row to gorse_b200_similar_scores with GORSE_B200_METRIC_NEG_DOT after negating the dots. */
 int32_t gorse_b200_sparse_index_search_range(gorse_b200_sparse_index *ix, int64_t q0, int64_t q1, int32_t k, int32_t *idx_out,
                                              float *dot_out, int32_t *count_out);
 /* measurement hook, like gorse_b200_index_stats: since the previous call, over every search of the index (search_range, the
@@ -404,7 +405,8 @@ int32_t gorse_b200_vecdb_compact(gorse_b200_vecdb *db, int64_t *new_slot_out, in
  * carry ALL of categories[n_categories] (CONTAIN_ALL, :381-389).  Results per query: slots_out / scores_out [nq x topk],
  * best first, count_out[nq]; entries past count_out[q] in a row are not part of the answer and are left unspecified; score = dot (Dot) or the NEGATED distance (Euclidean, Cosine) -- higher is more similar
  * (database.go:101, xvec.go:425-427).  Sparse: only positive dots are returned (the reference drops score 0, :421-423, and
- * its callers drop score <= 0, logics/item_to_item.go:73); topk <= 128.  topk <= 0 -> no results (:374-376). */
+ * its callers drop score <= 0, logics/item_to_item.go:73), at any topk, the rows padded with slot -1 / score 0.  topk <= 0 ->
+ * no results (:374-376). */
 /* Model hand-off (master/tasks.go:925-961): the item factors of every item with >= 1 training feedback (IsItemPredictable)
  * become vectors of a Dot collection, device to device -- no GetItemFactor round trip.  hidden[n_items], categories CSR over
  * items (may be NULL), one timestamp (the model id, :925).  slot_of_item_out[n_items]: slot per item, -1 = not predictable. */
