@@ -278,6 +278,101 @@ func (db *B200) AddVectors(ctx context.Context, name string, vectors []Vector) e
 	return nil
 }
 
+// AddIDFVectors is the master's rewrite of a sparse item-to-item or user-to-user collection (updateItemToItem /
+// updateUserToUser, master/tasks.go:783-877) with the vectors built on the device: row i's vector is appendSparseVector of
+// its sorted tag ids over tagsIDF, then of its sorted feedback ids over feedbackIDF at offset len(tagsIDF)
+// (logics/item_to_item.go:205-247, logics/user_to_user.go:194-237).  "users" and "items" pass feedback only (tags nil),
+// "tags" passes tags only, "auto" passes both.  An id repeated within one row's tags or feedback is kept once.  A row whose
+// vector is empty is not added, as VectorWriter.Add drops it (logics/vector_writer.go:84-92): its id keeps its previous
+// vector until DeleteVectors.  Otherwise an upsert by id, like AddVectors; an id may appear once per call.
+func (db *B200) AddIDFVectors(ctx context.Context, name string, ids []string, hidden []bool, categories [][]string, timestamp time.Time,
+	tags [][]int32, tagsIDF []float32, feedback [][]int32, feedbackIDF []float32) error {
+	n := len(ids)
+	if n == 0 {
+		return nil
+	}
+	if len(hidden) != n || len(categories) != n {
+		return errors.Errorf("%d ids with %d hidden flags and %d category lists", n, len(hidden), len(categories))
+	}
+	if (tags == nil && feedback == nil) || (tags != nil && len(tags) != n) || (feedback != nil && len(feedback) != n) {
+		return errors.Errorf("%d ids need %d rows of tags and/or feedback", n, n)
+	}
+	db.mu.Lock()
+	defer db.mu.Unlock()
+	c, err := db.collection(name)
+	if err != nil {
+		return err
+	}
+	aRows, aIDF, bRows, bIDF := tags, tagsIDF, feedback, feedbackIDF
+	if tags == nil {
+		aRows, aIDF, bRows, bIDF = feedback, feedbackIDF, nil, nil
+	}
+	aOff, aIDs := flattenCSR(aRows)
+	var bOff []int64
+	var bIDs []int32
+	if bRows != nil {
+		bOff, bIDs = flattenCSR(bRows)
+	}
+	hid, replace := make([]uint8, n), make([]int64, n)
+	catOff, cats := make([]int64, n+1), []int32{}
+	seen := make(map[string]struct{}, n)
+	for i, id := range ids {
+		if _, dup := seen[id]; dup {
+			return errors.Errorf("id %s twice in one call", id)
+		}
+		seen[id] = struct{}{}
+		if hidden[i] {
+			hid[i] = 1
+		}
+		for _, cat := range categories[i] {
+			cid, ok := c.catID[cat]
+			if !ok {
+				cid = int32(len(c.catName))
+				c.catID[cat], c.catName = cid, append(c.catName, cat)
+			}
+			cats = append(cats, cid)
+		}
+		catOff[i+1] = int64(len(cats))
+		replace[i] = -1
+		if old, ok := c.slotOf[id]; ok {
+			replace[i] = old
+		}
+	}
+	slotOut := make([]int64, n)
+	st := C.gorse_b200_vecdb_add_idf_vectors(c.handle, C.int64_t(n), i64p(aOff), i32p(aIDs), f32p(aIDF), C.int32_t(len(aIDF)), 0,
+		i64p(bOff), i32p(bIDs), f32p(bIDF), C.int32_t(len(bIDF)), C.uint32_t(len(tagsIDF)), u8p(hid), C.int64_t(timestamp.UnixMilli()),
+		i64p(catOff), i32p(cats), i64p(replace), i64p(slotOut))
+	runtime.KeepAlive(aIDs)
+	runtime.KeepAlive(bIDs)
+	runtime.KeepAlive(aIDF)
+	runtime.KeepAlive(bIDF)
+	if err := b200Err(st); err != nil {
+		return err
+	}
+	for i, id := range ids {
+		if slotOut[i] < 0 {
+			continue
+		}
+		c.slotOf[id] = slotOut[i]
+		c.idOf = append(c.idOf, id)
+		c.catsOf = append(c.catsOf, categories[i])
+	}
+	return nil
+}
+
+// flattenCSR packs rows of ids as offsets [len(rows)+1] from 0 and the ids, as go/model/cf/b200.go does
+func flattenCSR(rows [][]int32) ([]int64, []int32) {
+	off := make([]int64, len(rows)+1)
+	for r, row := range rows {
+		off[r+1] = off[r] + int64(len(row))
+	}
+	idx := make([]int32, off[len(rows)])
+	for r, row := range rows {
+		copy(idx[off[r]:], row)
+	}
+	return off, idx
+}
+
 func (db *B200) GetVectors(ctx context.Context, name string, ids []string) ([]Vector, error) {
 	if len(ids) == 0 {
 		return []Vector{}, nil

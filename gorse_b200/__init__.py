@@ -457,6 +457,34 @@ class VectorCollection:
         check(lib.gorse_b200_vecdb_add(self.h, n, ptr(values), ptr(sp_off), ptr(sp_ind), ptr(hid), ptr(ts), ptr(co), ptr(cv), ptr(rep), C.byref(first)))
         return first.value
 
+    def add_idf_vectors(self, a_rows, a_idf, a_offset=0, b_rows=None, b_idf=None, b_offset=0, hidden=None, timestamp_ms=0, categories=None,
+                        replace=None):
+        """Sparse vectors built on the device from id rows (gorse_b200_vecdb_add_idf_vectors; updateItemToItem / updateUserToUser,
+        master/tasks.go:783-877): row i's vector is appendSparseVector of its sorted, de-duplicated a_rows[i] over a_idf at
+        a_offset, then of b_rows[i] over b_idf at b_offset ("auto": tags as A, feedback as B at len(tags idf)).  Rows whose vector
+        is empty are not added.  -> slot_out int64 [n]: the slot of each row, -1 for an empty vector"""
+        n = len(a_rows)
+        aoff, aids = _flat(a_rows, np.int32)
+        aidf = np.ascontiguousarray(a_idf, np.float32).reshape(-1)
+        boff = bids = bidf = None
+        if b_rows is not None:
+            if len(b_rows) != n:
+                raise ValueError(f"{len(b_rows)} part-B rows for {n} rows")
+            boff, bids = _flat(b_rows, np.int32)
+            bidf = np.ascontiguousarray(b_idf, np.float32).reshape(-1)
+        hid = None if hidden is None else np.ascontiguousarray(hidden, np.uint8)
+        co = cv = None
+        if categories is not None:
+            co, cv = _flat(categories, np.int32)
+        rep = None if replace is None else np.ascontiguousarray(replace, np.int64)
+        slot_out = np.full(max(n, 1), -1, np.int64)
+        check(lib.gorse_b200_vecdb_add_idf_vectors(self.h, n, ptr(aoff), ptr(aids) if aids.size else None, ptr(aidf) if aidf.size else None,
+                                                   aidf.size, int(a_offset), ptr(boff), ptr(bids) if bids is not None and bids.size else None,
+                                                   ptr(bidf) if bidf is not None and bidf.size else None, 0 if bidf is None else bidf.size,
+                                                   int(b_offset), ptr(hid), int(timestamp_ms), ptr(co), ptr(cv) if cv is not None and cv.size else None,
+                                                   ptr(rep), ptr(slot_out)))
+        return slot_out[:n]
+
     def get(self, slots):
         slots = np.ascontiguousarray(slots, np.int64)
         n = slots.size

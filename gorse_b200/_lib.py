@@ -91,6 +91,8 @@ PROTOTYPES = {
     "gorse_b200_vecdb_destroy": (C.c_int32, [VP]),
     "gorse_b200_vecdb_count": (C.c_int32, [VP, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
     "gorse_b200_vecdb_add": (C.c_int32, [VP, C.c_int64, VP, VP, VP, VP, VP, VP, VP, VP, C.POINTER(C.c_int64)]),
+    "gorse_b200_vecdb_add_idf_vectors": (C.c_int32, [VP, C.c_int64, VP, VP, VP, C.c_int32, C.c_uint32, VP, VP, VP, C.c_int32, C.c_uint32, VP,
+                                                     C.c_int64, VP, VP, VP, VP]),
     "gorse_b200_vecdb_get": (C.c_int32, [VP, VP, C.c_int64, VP, VP, VP, VP]),
     "gorse_b200_vecdb_get_sparse": (C.c_int32, [VP, C.c_int64, VP, VP, C.c_int32, C.POINTER(C.c_int32)]),
     "gorse_b200_vecdb_delete_before": (C.c_int32, [VP, C.c_int64, VP, C.c_int64, C.POINTER(C.c_int64)]),

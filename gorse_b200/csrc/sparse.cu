@@ -390,42 +390,188 @@ sparse_emit_kernel(int64_t qc0, int64_t n, int k, float *sc, int32_t *out_idx, f
     if (threadIdx.x == 0) out_cnt[q] = K;
 }
 
+// ---- the CSC builder (csc_append): the postings of new rows, numbered above every stored row, go after the stored postings of
+// their feature.  A stable radix sort by feature keeps the new postings of one feature in row order.
+// pk[p] = (base + r) << 32 | bits(val[p]) for the entries p of row r: a posting's row and value in one sort value; one warp per row
+__global__ void csc_pack_kernel(const int64_t *off, int64_t m, const float *val, int64_t base, uint64_t *pk)
+{
+    const int lane = threadIdx.x & 31;
+    const int64_t nw = ((int64_t)gridDim.x * blockDim.x) >> 5;
+    for (int64_t r = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5; r < m; r += nw)
+        for (int64_t p = off[r] + lane; p < off[r + 1]; p += 32) pk[p] = (uint64_t)(base + r) << 32 | __float_as_uint(val[p]);
+}
+// for f in [0, F_new]: lb[f] = the new postings of features below f (keys: their features, sorted), foff_n[f] = foff[min(f, F_old)] + lb[f]
+__global__ void csc_bounds_kernel(const uint32_t *keys, int64_t nnz, const int64_t *foff, uint32_t F_old, uint32_t F_new, int64_t *lb, int64_t *foff_n)
+{
+    const int64_t st = (int64_t)gridDim.x * blockDim.x;
+    for (int64_t f = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; f <= F_new; f += st) {
+        int64_t a = 0, b = nnz;
+        while (a < b) {
+            const int64_t mid = (a + b) >> 1;
+            if (keys[mid] < f) a = mid + 1;
+            else b = mid;
+        }
+        lb[f] = a;
+        foff_n[f] = (foff ? foff[min(f, (int64_t)F_old)] : 0) + a;
+    }
+}
+// the stored postings of feature f move up by lb[f]; one warp per feature
+__global__ void csc_old_kernel(const int64_t *foff, uint32_t F_old, const int32_t *frow, const float *fval, const int64_t *lb, int32_t *frow_n, float *fval_n)
+{
+    const int lane = threadIdx.x & 31;
+    const int64_t nw = ((int64_t)gridDim.x * blockDim.x) >> 5;
+    for (int64_t f = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5; f < F_old; f += nw)
+        for (int64_t p = foff[f] + lane; p < foff[f + 1]; p += 32) { frow_n[p + lb[f]] = frow[p]; fval_n[p + lb[f]] = fval[p]; }
+}
+// the new posting s (sorted by feature) after every stored posting of its feature and the new ones before it:
+// foff_n[f] + (stored of f) + (s - lb[f]) = foff[f + 1] + s
+__global__ void csc_new_kernel(const uint32_t *keys, const uint64_t *pk, int64_t nnz, const int64_t *foff, uint32_t F_old, int32_t *frow_n, float *fval_n)
+{
+    const int64_t st = (int64_t)gridDim.x * blockDim.x;
+    for (int64_t s = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; s < nnz; s += st) {
+        const int64_t to = (foff ? foff[min((int64_t)keys[s] + 1, (int64_t)F_old)] : 0) + s;
+        frow_n[to] = (int32_t)(pk[s] >> 32);
+        fval_n[to] = __uint_as_float((uint32_t)pk[s]);
+    }
+}
+
+// the stored CSC (foff[F_old + 1] / frow / fval, nnz_old postings; foff == nullptr: none) with the postings of m new rows
+// appended: the device CSR off[m + 1] from 0 / ind / val (nnz entries, every index < F_new), rows base .. base + m - 1, above
+// every stored row.  Into foff_n[F_new + 1] / frow_n / fval_n (allocated here; F_new >= F_old), postings ascending by row within
+// each feature.  Enqueued on the context's stream; its scratch is released before it returns.
+int32_t csc_append(gorse_b200_ctx *c, const int64_t *off, const uint32_t *ind, const float *val, int64_t m, int64_t nnz, int64_t base,
+                   const int64_t *foff, const int32_t *frow, const float *fval, uint32_t F_old, int64_t nnz_old, uint32_t F_new,
+                   DevBuf<int64_t> &foff_n, DevBuf<int32_t> &frow_n, DevBuf<float> &fval_n)
+{
+    cudaStream_t s = c->stream;
+    DevBuf<uint32_t> keys;
+    DevBuf<uint64_t> pk, pk_s;
+    DevBuf<int64_t> lb;
+    DevBuf<uint8_t> tmp;
+    auto done = [&](int32_t st) { cudaStreamSynchronize(s); keys.free(); pk.free(); pk_s.free(); lb.free(); tmp.free(); return st; };
+    int32_t st;
+    if ((st = foff_n.alloc((size_t)F_new + 1)) || (st = frow_n.alloc((size_t)(nnz_old + nnz))) || (st = fval_n.alloc((size_t)(nnz_old + nnz))) ||
+        (st = keys.alloc((size_t)nnz)) || (st = pk.alloc((size_t)nnz)) || (st = pk_s.alloc((size_t)nnz)) || (st = lb.alloc((size_t)F_new + 1)))
+        return done(st);
+    int end_bit = 1;   // every feature index is below F_new
+    while (end_bit < 32 && ((uint64_t)F_new - 1) >> end_bit) end_bit++;
+    const unsigned grid = (unsigned)c->sm_count * 8;
+    cudaError_t e = cudaSuccess;
+    if (nnz) {
+        csc_pack_kernel<<<grid, 256, 0, s>>>(off, m, val, base, pk.p);
+        c->launches++;
+        size_t tmp_bytes = 0;
+        e = cudaGetLastError();
+        if (e == cudaSuccess) e = cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, ind, keys.p, pk.p, pk_s.p, nnz, 0, end_bit, s);
+        if (e == cudaSuccess && (st = tmp.alloc(tmp_bytes))) return done(st);
+        if (e == cudaSuccess) e = cub::DeviceRadixSort::SortPairs(tmp.p, tmp_bytes, ind, keys.p, pk.p, pk_s.p, nnz, 0, end_bit, s);
+    }
+    if (e == cudaSuccess) {
+        csc_bounds_kernel<<<div_up((int64_t)F_new + 1, 256), 256, 0, s>>>(keys.p, nnz, foff, F_old, F_new, lb.p, foff_n.p);
+        if (nnz_old) csc_old_kernel<<<grid, 256, 0, s>>>(foff, F_old, frow, fval, lb.p, frow_n.p, fval_n.p);
+        if (nnz) csc_new_kernel<<<grid, 256, 0, s>>>(keys.p, pk_s.p, nnz, foff, F_old, frow_n.p, fval_n.p);
+        c->launches += 3;
+        e = cudaGetLastError();
+    }
+    if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+    if (e != cudaSuccess) { set_error("sparse CSC: %s", cudaGetErrorString(e)); return done(e == cudaErrorMemoryAllocation ? GORSE_B200_ERR_OOM : GORSE_B200_ERR_CUDA); }
+    return done(GORSE_B200_OK);
+}
+
+// the device layouts from the host CSR: the CSR is uploaded and the CSC built from it on the device
 int32_t sync_device(gorse_b200_sparse_index *ix)
 {
     if (!ix->dirty) return GORSE_B200_OK;
     gorse_b200_ctx *c = ix->ctx;
     const int64_t n = (int64_t)ix->h_off.size() - 1, nnz = (int64_t)ix->h_ind.size();
-    // CSC by counting sort: postings of a feature in ascending row order
-    std::vector<int64_t> foff((size_t)ix->n_features + 1, 0);
-    for (int64_t t = 0; t < nnz; t++) foff[(size_t)ix->h_ind[(size_t)t] + 1]++;
-    for (size_t f = 0; f < ix->n_features; f++) foff[f + 1] += foff[f];
-    std::vector<int64_t> cur(foff.begin(), foff.end() - 1);
-    std::vector<int32_t> frow((size_t)nnz);
-    std::vector<float> fval((size_t)nnz);
-    for (int64_t r = 0; r < n; r++)
-        for (int64_t t = ix->h_off[(size_t)r]; t < ix->h_off[(size_t)r + 1]; t++) {
-            const int64_t p = cur[ix->h_ind[(size_t)t]]++;
-            frow[(size_t)p] = (int32_t)r;
-            fval[(size_t)p] = ix->h_val[(size_t)t];
-        }
     GB_TRY(ix->off.alloc((size_t)n + 1));
-    GB_TRY(ix->foff.alloc(foff.size()));
     GB_TRY(ix->ind.alloc((size_t)nnz));
     GB_TRY(ix->val.alloc((size_t)nnz));
-    GB_TRY(ix->frow.alloc((size_t)nnz));
-    GB_TRY(ix->fval.alloc((size_t)nnz));
     cudaStream_t s = c->stream;
     GB_CUDA(cudaMemcpyAsync(ix->off.p, ix->h_off.data(), sizeof(int64_t) * ((size_t)n + 1), cudaMemcpyHostToDevice, s));
-    GB_CUDA(cudaMemcpyAsync(ix->foff.p, foff.data(), sizeof(int64_t) * foff.size(), cudaMemcpyHostToDevice, s));
     if (nnz) {
         GB_CUDA(cudaMemcpyAsync(ix->ind.p, ix->h_ind.data(), sizeof(uint32_t) * (size_t)nnz, cudaMemcpyHostToDevice, s));
         GB_CUDA(cudaMemcpyAsync(ix->val.p, ix->h_val.data(), sizeof(float) * (size_t)nnz, cudaMemcpyHostToDevice, s));
-        GB_CUDA(cudaMemcpyAsync(ix->frow.p, frow.data(), sizeof(int32_t) * (size_t)nnz, cudaMemcpyHostToDevice, s));
-        GB_CUDA(cudaMemcpyAsync(ix->fval.p, fval.data(), sizeof(float) * (size_t)nnz, cudaMemcpyHostToDevice, s));
     }
-    GB_CUDA(cudaStreamSynchronize(s));   // the staging vectors die here
+    GB_TRY(csc_append(c, ix->off.p, ix->ind.p, ix->val.p, n, nnz, 0, nullptr, nullptr, nullptr, 0, 0, ix->n_features, ix->foff, ix->frow, ix->fval));
     ix->dirty = false;
     return GORSE_B200_OK;
+}
+
+// ---- vectors from id rows (sparse_idf_rows): appendSparseVector of every row on the device.  The rows are merged (row r: its
+// A ids, then its B ids), each merged row is sorted by key = part << 32 | (uint32)id, and the kept entries are scanned into place.
+struct IdfPart {
+    const int64_t *off; const int32_t *ids; const float *idf; int32_t n_idf; uint32_t offset;
+};
+// key[t] of merged entry t (m_off[n + 1]: the merged offsets), head[t] = 1 for the first entry of a row
+__global__ void idf_gather_kernel(IdfPart A, IdfPart B, const int64_t *m_off, int64_t n, int64_t total, uint64_t *key, uint8_t *head)
+{
+    const int64_t st = (int64_t)gridDim.x * blockDim.x;
+    for (int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; t < total; t += st) {
+        int64_t lo = 0, hi = n;   // m_off[lo] <= t < m_off[hi]: at the end, the (non-empty) row lo holds t
+        while (hi - lo > 1) {
+            const int64_t mid = (lo + hi) >> 1;
+            if (m_off[mid] <= t) lo = mid;
+            else hi = mid;
+        }
+        const int64_t j = t - m_off[lo], na = A.off[lo + 1] - A.off[lo];
+        key[t] = j < na ? (uint64_t)(uint32_t)A.ids[A.off[lo] + j] : 1ull << 32 | (uint32_t)B.ids[B.off[lo] + j - na];
+        head[t] = j == 0;
+    }
+}
+// keep[t] = 1 for a sorted entry that enters its vector: an id in [0, n_idf) whose idf is not <= 0 (a NaN idf enters, and is
+// refused by the scatter), not equal to the entry before it in its row; keep[total] = 0
+__global__ void idf_keep_kernel(IdfPart A, IdfPart B, const uint64_t *key, const uint8_t *head, int64_t total, int64_t *keep)
+{
+    const int64_t st = (int64_t)gridDim.x * blockDim.x;
+    for (int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; t <= total; t += st) {
+        if (t == total) { keep[t] = 0; continue; }
+        const uint64_t k = key[t];
+        const bool b = k >> 32;
+        const int32_t id = (int32_t)(uint32_t)k;
+        keep[t] = id >= 0 && id < (b ? B.n_idf : A.n_idf) && !((b ? B.idf : A.idf)[id] <= 0.f) && (head[t] || key[t - 1] != k);
+    }
+}
+// the kept entries to their scanned positions: index offset + id, value (float)sqrt((double)idf[id]).  err bit 1: a NaN value,
+// bit 2: an index >= 0x7fffffff (what gorse_b200_sparse_index_add refuses); stat[1] = the largest index
+__global__ void idf_scatter_kernel(IdfPart A, IdfPart B, const uint64_t *key, const int64_t *scan, int64_t total, uint32_t *ind, float *val,
+                                   unsigned *stat)
+{
+    const int64_t st = (int64_t)gridDim.x * blockDim.x;
+    unsigned err = 0, mx = 0;
+    for (int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; t < total; t += st) {
+        const int64_t p = scan[t];
+        if (scan[t + 1] == p) continue;
+        const uint64_t k = key[t];
+        const bool b = k >> 32;
+        const int32_t id = (int32_t)(uint32_t)k;
+        const uint32_t x = (b ? B.offset : A.offset) + (uint32_t)id;
+        const float v = (float)sqrt((double)(b ? B.idf : A.idf)[id]);
+        ind[p] = x;
+        val[p] = v;
+        err |= (v != v ? 1u : 0u) | (x >= 0x7fffffffu ? 2u : 0u);
+        mx = max(mx, x);
+    }
+    err = __reduce_or_sync(0xffffffffu, err);
+    mx = __reduce_max_sync(0xffffffffu, mx);
+    if ((threadIdx.x & 31) == 0) {
+        if (err) atomicOr(&stat[0], err);
+        atomicMax(&stat[1], mx);
+    }
+}
+// per row r: out_off[r] = its first entry in the built CSR, out_off[n] = the entries; err bit 4: the row's first B index does not
+// exceed its last A index (a_off == m_off without a part B).  Each part's kept indices ascend unless one is >= 0x7fffffff.
+__global__ void idf_rows_kernel(const int64_t *a_off, const int64_t *m_off, const int64_t *scan, int64_t n, const uint32_t *ind, int64_t *out_off,
+                                unsigned *stat)
+{
+    const int64_t st = (int64_t)gridDim.x * blockDim.x;
+    for (int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; r <= n; r += st) {
+        const int64_t a0 = scan[m_off[r]];
+        out_off[r] = a0;
+        if (r == n) continue;
+        const int64_t ab = scan[m_off[r] + a_off[r + 1] - a_off[r]], b1 = scan[m_off[r + 1]];
+        if (a0 < ab && ab < b1 && ind[ab] <= ind[ab - 1]) atomicOr(&stat[0], 4u);
+    }
 }
 
 // ---- compaction (sparse_compact): `scan` is the exclusive sum of the rows' live flags, row r is live iff scan[r + 1] != scan[r]
@@ -774,6 +920,154 @@ int32_t sparse_compact(gorse_b200_sparse_index *ix, const int64_t *scan, int64_t
     ix->off = off_n; ix->foff = foff_n; ix->ind = ind_n; ix->val = val_n; ix->frow = frow_n; ix->fval = fval_n;
     ix->h_off.swap(h_off); ix->h_ind.swap(h_ind); ix->h_val.swap(h_val);
     ix->tl_dot.free(); ix->tl_idx.free(); ix->tl_cnt.free(); ix->next.free();   // sized for the old N; the next search allocates them
+    return done(GORSE_B200_OK);
+}
+
+int32_t sparse_idf_rows(gorse_b200_ctx *c, int64_t n, const int64_t *a_off, const int32_t *a_ids, const float *a_idf, int32_t a_n_idf,
+                        uint32_t a_offset, const int64_t *b_off, const int32_t *b_ids, const float *b_idf, int32_t b_n_idf, uint32_t b_offset,
+                        SparseRows &out)
+{
+    cudaStream_t s = c->stream;
+    const int64_t total = a_off[n] + (b_off ? b_off[n] : 0);
+    out.free();
+    out.row_off.assign((size_t)n + 1, 0);
+    out.off.assign(1, 0);
+    if (total == 0) return GORSE_B200_OK;
+    if (total > INT32_MAX || n > INT32_MAX) {
+        set_error("%lld ids in %lld rows in one call (at most 2^31 - 1 of each)", (long long)total, (long long)n);
+        return GORSE_B200_ERR_UNSUPPORTED;
+    }
+    std::vector<int64_t> m_off;
+    if (b_off) {
+        m_off.resize((size_t)n + 1);
+        for (int64_t r = 0; r <= n; r++) m_off[(size_t)r] = a_off[r] + b_off[r];
+    }
+    DevBuf<int64_t> d_aoff, d_boff, d_moff, keep, d_out_off;
+    DevBuf<int32_t> d_aids, d_bids;
+    DevBuf<float> d_aidf, d_bidf;
+    DevBuf<uint64_t> key, key_s;
+    DevBuf<uint8_t> head, tmp;
+    DevBuf<unsigned> stat;
+    auto done = [&](int32_t st) {
+        cudaStreamSynchronize(s);
+        d_aoff.free(); d_boff.free(); d_moff.free(); keep.free(); d_out_off.free(); d_aids.free(); d_bids.free(); d_aidf.free(); d_bidf.free();
+        key.free(); key_s.free(); head.free(); tmp.free(); stat.free();
+        if (st) out.free();
+        return st;
+    };
+    int32_t st;
+    if ((st = d_aoff.alloc((size_t)n + 1)) || (st = d_aids.alloc((size_t)a_off[n])) || (st = d_aidf.alloc((size_t)a_n_idf)) ||
+        (b_off && ((st = d_boff.alloc((size_t)n + 1)) || (st = d_moff.alloc((size_t)n + 1)) || (st = d_bids.alloc((size_t)b_off[n])) ||
+                   (st = d_bidf.alloc((size_t)b_n_idf)))) ||
+        (st = key.alloc((size_t)total)) || (st = key_s.alloc((size_t)total)) || (st = head.alloc((size_t)total)) || (st = keep.alloc((size_t)total + 1)) ||
+        (st = d_out_off.alloc((size_t)n + 1)) || (st = stat.alloc(2)))
+        return done(st);
+    cudaError_t e = cudaMemcpyAsync(d_aoff.p, a_off, sizeof(int64_t) * ((size_t)n + 1), cudaMemcpyHostToDevice, s);
+    if (e == cudaSuccess && a_off[n]) e = cudaMemcpyAsync(d_aids.p, a_ids, sizeof(int32_t) * (size_t)a_off[n], cudaMemcpyHostToDevice, s);
+    if (e == cudaSuccess && a_n_idf) e = cudaMemcpyAsync(d_aidf.p, a_idf, sizeof(float) * (size_t)a_n_idf, cudaMemcpyHostToDevice, s);
+    if (b_off) {
+        if (e == cudaSuccess) e = cudaMemcpyAsync(d_boff.p, b_off, sizeof(int64_t) * ((size_t)n + 1), cudaMemcpyHostToDevice, s);
+        if (e == cudaSuccess) e = cudaMemcpyAsync(d_moff.p, m_off.data(), sizeof(int64_t) * ((size_t)n + 1), cudaMemcpyHostToDevice, s);
+        if (e == cudaSuccess && b_off[n]) e = cudaMemcpyAsync(d_bids.p, b_ids, sizeof(int32_t) * (size_t)b_off[n], cudaMemcpyHostToDevice, s);
+        if (e == cudaSuccess && b_n_idf) e = cudaMemcpyAsync(d_bidf.p, b_idf, sizeof(float) * (size_t)b_n_idf, cudaMemcpyHostToDevice, s);
+    }
+    if (e == cudaSuccess) e = cudaMemsetAsync(stat.p, 0, stat.bytes(), s);
+    const IdfPart A{d_aoff.p, d_aids.p, d_aidf.p, a_n_idf, a_offset};
+    const IdfPart B{d_boff.p, d_bids.p, d_bidf.p, b_off ? b_n_idf : 0, b_offset};
+    const int64_t *moff = b_off ? d_moff.p : d_aoff.p;
+    const unsigned grid = (unsigned)c->sm_count * 8;
+    size_t sort_bytes = 0, scan_bytes = 0;
+    if (e == cudaSuccess) {
+        idf_gather_kernel<<<grid, 256, 0, s>>>(A, B, moff, n, total, key.p, head.p);
+        c->launches++;
+        e = cudaGetLastError();
+    }
+    // each row sorted on its own: a few ids per row for most rows, hundreds of thousands for a head item
+    if (e == cudaSuccess) e = cub::DeviceSegmentedSort::SortKeys(nullptr, sort_bytes, key.p, key_s.p, (int)total, (int)n, moff, moff + 1, s);
+    if (e == cudaSuccess) e = cub::DeviceScan::ExclusiveSum(nullptr, scan_bytes, keep.p, total + 1, s);
+    if (e == cudaSuccess && (st = tmp.alloc(std::max(sort_bytes, scan_bytes)))) return done(st);
+    if (e == cudaSuccess) e = cub::DeviceSegmentedSort::SortKeys(tmp.p, sort_bytes, key.p, key_s.p, (int)total, (int)n, moff, moff + 1, s);
+    if (e == cudaSuccess) {
+        idf_keep_kernel<<<grid, 256, 0, s>>>(A, B, key_s.p, head.p, total, keep.p);
+        c->launches++;
+        e = cudaGetLastError();
+    }
+    if (e == cudaSuccess) e = cub::DeviceScan::ExclusiveSum(tmp.p, scan_bytes, keep.p, total + 1, s);
+    int64_t nnz = 0;
+    if (e == cudaSuccess) e = cudaMemcpyAsync(&nnz, keep.p + total, sizeof(int64_t), cudaMemcpyDeviceToHost, s);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+    if (e != cudaSuccess) { set_error("idf vectors: %s", cudaGetErrorString(e)); return done(GORSE_B200_ERR_CUDA); }
+    if ((st = out.ind.alloc((size_t)nnz)) || (st = out.val.alloc((size_t)nnz))) return done(st);
+    unsigned h_stat[2] = {0, 0};
+    idf_scatter_kernel<<<grid, 256, 0, s>>>(A, B, key_s.p, keep.p, total, out.ind.p, out.val.p, stat.p);
+    idf_rows_kernel<<<div_up(n + 1, 256), 256, 0, s>>>(d_aoff.p, moff, keep.p, n, out.ind.p, d_out_off.p, stat.p);
+    c->launches += 2;
+    e = cudaGetLastError();
+    if (e == cudaSuccess) e = cudaMemcpyAsync(out.row_off.data(), d_out_off.p, sizeof(int64_t) * ((size_t)n + 1), cudaMemcpyDeviceToHost, s);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(h_stat, stat.p, sizeof(h_stat), cudaMemcpyDeviceToHost, s);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+    if (e != cudaSuccess) { set_error("idf vectors: %s", cudaGetErrorString(e)); return done(GORSE_B200_ERR_CUDA); }
+    if (h_stat[0]) {
+        set_error(h_stat[0] & 1u ? "NaN value (an idf entry in use is NaN)"
+                  : h_stat[0] & 2u ? "feature index too large (offset + id >= 0x7fffffff)"
+                                   : "indices of a row are not strictly ascending (part B's offset does not place it after part A)");
+        return done(GORSE_B200_ERR_ARG);
+    }
+    // the CSR of the non-empty rows
+    for (int64_t r = 0; r < n; r++)
+        if (out.row_off[(size_t)r + 1] > out.row_off[(size_t)r]) out.off.push_back(out.row_off[(size_t)r + 1]);
+    out.n_features = nnz ? h_stat[1] + 1 : 0;
+    return done(GORSE_B200_OK);
+}
+
+int32_t sparse_append(gorse_b200_sparse_index *ix, const SparseRows &rows)
+{
+    GB_TRY(sync_device(ix));   // the device layouts hold every stored row
+    gorse_b200_ctx *c = ix->ctx;
+    cudaStream_t s = c->stream;
+    const int64_t n = (int64_t)ix->h_off.size() - 1, nnz_old = (int64_t)ix->h_ind.size();
+    const int64_t m = (int64_t)rows.off.size() - 1, nnz = rows.off.back();
+    if (m == 0) return GORSE_B200_OK;
+    if (n + m >= (1ll << 31)) { set_error("more than 2^31 vectors"); return GORSE_B200_ERR_UNSUPPORTED; }
+    const uint32_t F = std::max(ix->n_features, rows.n_features);
+    DevBuf<int64_t> off_n, foff_n, d_off;
+    DevBuf<uint32_t> ind_n;
+    DevBuf<float> val_n, fval_n;
+    DevBuf<int32_t> frow_n;
+    auto done = [&](int32_t st) {
+        cudaStreamSynchronize(s);
+        d_off.free();
+        if (st) { off_n.free(); foff_n.free(); ind_n.free(); val_n.free(); fval_n.free(); frow_n.free(); }
+        return st;
+    };
+    int32_t st;
+    if ((st = off_n.alloc((size_t)(n + m + 1))) || (st = ind_n.alloc((size_t)(nnz_old + nnz))) || (st = val_n.alloc((size_t)(nnz_old + nnz))) ||
+        (st = d_off.alloc((size_t)m + 1)))
+        return done(st);
+    // the new rows' offsets in the index and on the device; their entries from the staging buffers
+    std::vector<int64_t> h_off((size_t)m);
+    for (int64_t j = 0; j < m; j++) h_off[(size_t)j] = nnz_old + rows.off[(size_t)j + 1];
+    std::vector<uint32_t> h_ind((size_t)nnz);
+    std::vector<float> h_val((size_t)nnz);
+    cudaError_t e = cudaMemcpyAsync(d_off.p, rows.off.data(), sizeof(int64_t) * ((size_t)m + 1), cudaMemcpyHostToDevice, s);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(off_n.p, ix->off.p, sizeof(int64_t) * (size_t)(n + 1), cudaMemcpyDeviceToDevice, s);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(off_n.p + n + 1, h_off.data(), sizeof(int64_t) * (size_t)m, cudaMemcpyHostToDevice, s);
+    if (e == cudaSuccess && nnz_old) e = cudaMemcpyAsync(ind_n.p, ix->ind.p, sizeof(uint32_t) * (size_t)nnz_old, cudaMemcpyDeviceToDevice, s);
+    if (e == cudaSuccess && nnz_old) e = cudaMemcpyAsync(val_n.p, ix->val.p, sizeof(float) * (size_t)nnz_old, cudaMemcpyDeviceToDevice, s);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(ind_n.p + nnz_old, rows.ind.p, sizeof(uint32_t) * (size_t)nnz, cudaMemcpyDeviceToDevice, s);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(val_n.p + nnz_old, rows.val.p, sizeof(float) * (size_t)nnz, cudaMemcpyDeviceToDevice, s);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(h_ind.data(), rows.ind.p, sizeof(uint32_t) * (size_t)nnz, cudaMemcpyDeviceToHost, s);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(h_val.data(), rows.val.p, sizeof(float) * (size_t)nnz, cudaMemcpyDeviceToHost, s);
+    if (e != cudaSuccess) { set_error("sparse append: %s", cudaGetErrorString(e)); return done(GORSE_B200_ERR_CUDA); }
+    if ((st = csc_append(c, d_off.p, rows.ind.p, rows.val.p, m, nnz, n, ix->foff.p, ix->frow.p, ix->fval.p, ix->n_features, nnz_old, F, foff_n,
+                         frow_n, fval_n)))
+        return done(st);   // csc_append synchronised the stream: the host copies are complete
+    ix->off.free(); ix->foff.free(); ix->ind.free(); ix->val.free(); ix->frow.free(); ix->fval.free();
+    ix->off = off_n; ix->foff = foff_n; ix->ind = ind_n; ix->val = val_n; ix->frow = frow_n; ix->fval = fval_n;
+    ix->h_off.insert(ix->h_off.end(), h_off.begin(), h_off.end());
+    ix->h_ind.insert(ix->h_ind.end(), h_ind.begin(), h_ind.end());
+    ix->h_val.insert(ix->h_val.end(), h_val.begin(), h_val.end());
+    ix->n_features = F;
     return done(GORSE_B200_OK);
 }
 

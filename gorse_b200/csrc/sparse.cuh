@@ -47,4 +47,26 @@ int32_t sparse_search_rows(gorse_b200_sparse_index *ix, const int64_t *d_rows, i
 int32_t sparse_compact(gorse_b200_sparse_index *ix, const int64_t *scan, int64_t live);
 // device bytes held by the index
 size_t sparse_bytes(const gorse_b200_sparse_index *ix);
+
+// vectors built on the device by sparse_idf_rows and not yet part of any index: the CSR of the non-empty rows (off on the host,
+// m + 1 entries from 0; ind / val on the device), row_off[n + 1] = each input row's first entry (an empty row's equals the next
+// row's), n_features = the largest index + 1 (0 without entries)
+struct SparseRows {
+    std::vector<int64_t> off, row_off;
+    DevBuf<uint32_t> ind;
+    DevBuf<float> val;
+    uint32_t n_features = 0;
+    void free() { ind.free(); val.free(); }
+};
+// appendSparseVector of n rows on the device (gorse_b200_vecdb_add_idf_vectors): part A rows a_off[n + 1] / a_ids over
+// a_idf[a_n_idf] at a_offset, then optionally part B (b_off == nullptr: none).  The arguments are checked by the caller except
+// what needs the ids: a used NaN idf, an index >= 0x7fffffff or a row whose B indices do not follow its A indices is
+// GORSE_B200_ERR_ARG.  Nothing but `out` changes; on an error `out` holds no device memory.  The caller holds the device.
+int32_t sparse_idf_rows(gorse_b200_ctx *c, int64_t n, const int64_t *a_off, const int32_t *a_ids, const float *a_idf, int32_t a_n_idf,
+                        uint32_t a_offset, const int64_t *b_off, const int32_t *b_ids, const float *b_idf, int32_t b_n_idf, uint32_t b_offset,
+                        SparseRows &out);
+// appends the rows of `rows` to the index as rows n .. n + m - 1: the device CSR grows, the new postings are merged into the CSC
+// on the device, the host CSR is brought up to date from the device, and the index ends clean.  On an error the index's rows
+// are unchanged (its device layouts may have been brought up to date).  The caller holds ix->mu and the device.
+int32_t sparse_append(gorse_b200_sparse_index *ix, const SparseRows &rows);
 }

@@ -201,6 +201,72 @@ int32_t gorse_b200_vecdb_add(gorse_b200_vecdb *db, int64_t n, const float *value
     return GORSE_B200_OK;
 }
 
+// updateItemToItem / updateUserToUser (master/tasks.go:783-877) for the sparse types: the vectors of appendSparseVector
+// (logics/vector_writer.go:192-209) built from id rows on the device (sparse_idf_rows) and appended to the index without a host
+// rebuild (sparse_append).  Checks that need the ids run on the device into staging buffers; the collection changes after the
+// last check has passed.
+int32_t gorse_b200_vecdb_add_idf_vectors(gorse_b200_vecdb *db, int64_t n, const int64_t *a_off, const int32_t *a_ids, const float *a_idf,
+                                         int32_t a_n_idf, uint32_t a_offset, const int64_t *b_off, const int32_t *b_ids, const float *b_idf,
+                                         int32_t b_n_idf, uint32_t b_offset, const uint8_t *hidden, int64_t timestamp_ms, const int64_t *cat_off,
+                                         const int32_t *cats, const int64_t *replace, int64_t *slot_out)
+{
+    GB_CHECK_ARG(db != nullptr, "collection is NULL");
+    GB_CHECK_ARG(db->dim == 0, "not a sparse collection");
+    GB_CHECK_ARG(n >= 0, "negative n");
+    if (n == 0) return GORSE_B200_OK;
+    GB_CHECK_ARG(slot_out != nullptr, "slot_out is NULL");
+    GB_CHECK_ARG(a_off != nullptr && a_off[0] == 0, "a_off is NULL or a_off[0] != 0");
+    GB_CHECK_ARG(b_off == nullptr || b_off[0] == 0, "b_off[0] != 0");
+    GB_CHECK_ARG(cat_off == nullptr || cat_off[0] == 0, "cat_off[0] must be 0");
+    for (int64_t i = 0; i < n; i++) {
+        GB_CHECK_ARG(a_off[i + 1] >= a_off[i], "a_off decreases at row %lld", (long long)i);
+        GB_CHECK_ARG(b_off == nullptr || b_off[i + 1] >= b_off[i], "b_off decreases at row %lld", (long long)i);
+        GB_CHECK_ARG(cat_off == nullptr || cat_off[i + 1] >= cat_off[i], "cat_off not non-decreasing at %lld", (long long)i);
+    }
+    GB_CHECK_ARG(a_off[n] == 0 || a_ids != nullptr, "a_ids is NULL");
+    GB_CHECK_ARG(a_n_idf >= 0 && (a_n_idf == 0 || a_idf != nullptr), "bad a_idf");
+    GB_CHECK_ARG(b_off == nullptr || b_off[n] == 0 || b_ids != nullptr, "b_ids is NULL");
+    GB_CHECK_ARG(b_off == nullptr || (b_n_idf >= 0 && (b_n_idf == 0 || b_idf != nullptr)), "bad b_idf");
+    GB_CHECK_ARG(cat_off == nullptr || cat_off[n] == 0 || cats != nullptr, "cats is NULL");
+    std::lock_guard<std::mutex> lk(db->mu);
+    std::lock_guard<std::mutex> lk2(db->sparse->mu);
+    ScopedDevice sd(db->ctx->device);
+    SparseRows rows;
+    GB_TRY(sparse_idf_rows(db->ctx, n, a_off, a_ids, a_idf, a_n_idf, a_offset, b_off, b_ids, b_idf, b_n_idf, b_offset, rows));
+    // an empty vector is not added (VectorWriter.Add, logics/vector_writer.go:84-92)
+    const int64_t first = (int64_t)db->ts.size();
+    std::vector<int64_t> slot((size_t)n);
+    int64_t added = 0;
+    for (int64_t i = 0; i < n; i++) {
+        const bool add = rows.row_off[(size_t)i + 1] > rows.row_off[(size_t)i];
+        slot[(size_t)i] = add ? first + added++ : -1;
+        if (add && replace && replace[i] >= first) {
+            rows.free();
+            set_error("replace[%lld] = %lld is not an existing slot", (long long)i, (long long)replace[i]);
+            return GORSE_B200_ERR_ARG;
+        }
+    }
+    const int32_t st = sparse_append(db->sparse, rows);
+    rows.free();
+    if (st) return st;
+    for (int64_t i = 0; i < n; i++) {
+        slot_out[i] = slot[(size_t)i];
+        if (slot[(size_t)i] < 0) continue;
+        db->hidden.push_back(hidden ? (hidden[i] != 0) : 0);
+        db->dead.push_back(0);
+        db->ts.push_back(timestamp_ms);
+        if (cat_off) db->cats.insert(db->cats.end(), cats + cat_off[i], cats + cat_off[i + 1]);
+        db->cat_off.push_back((int64_t)db->cats.size());
+        db->live++;
+        if (replace && replace[i] >= 0 && !db->dead[(size_t)replace[i]]) {   // upsert: the old version disappears
+            db->dead[(size_t)replace[i]] = 1;
+            db->live--;
+        }
+    }
+    if (added) db->meta_dirty = true;
+    return GORSE_B200_OK;
+}
+
 int32_t gorse_b200_vecdb_get(gorse_b200_vecdb *db, const int64_t *slots, int64_t n, float *values_out, uint8_t *hidden_out,
                              int64_t *timestamp_out, uint8_t *live_out)
 {

@@ -381,6 +381,31 @@ int32_t gorse_b200_vecdb_count(gorse_b200_vecdb *db, int64_t *live_out, int64_t 
 int32_t gorse_b200_vecdb_add(gorse_b200_vecdb *db, int64_t n, const float *values, const int64_t *sp_off, const uint32_t *sp_indices,
                              const uint8_t *hidden, const int64_t *timestamp_ms, const int64_t *cat_off, const int32_t *cats,
                              const int64_t *replace, int64_t *first_slot_out);
+/* The master's rewrite of a sparse similarity collection (updateItemToItem / updateUserToUser, master/tasks.go:783-877) in one
+ * call: n vectors built from id rows as appendSparseVector builds them (logics/vector_writer.go:192-209), then added as
+ * gorse_b200_vecdb_add adds them.  Row i has part A (a_off[n+1] from 0 / a_ids, ids in any order) and optionally part B
+ * (b_off == NULL: none).  "users" / "items" / "tags" pass one part (logics/item_to_item.go:205-220, logics/user_to_user.go:194-210);
+ * "auto" passes the tag ids as A with offset 0 and the feedback ids as B with offset len(tagsIDF) (item_to_item.go:228-247,
+ * user_to_user.go:218-237).
+ *   Vector of row i: for part A, then part B: the row's ids sorted ascending (slices.Sort); ids < 0, ids >= n_idf and ids with
+ *   idf[id] <= 0 skipped; index offset + id, value (float)sqrt((double)idf[id]) -- gorse_b200_sparse_vector's values, bit for
+ *   bit.  An id repeated within one part's row is kept ONCE.  The reference's vector holds it once per repeat (dataset.AddFeedback,
+ *   dataset/dataset.go:231-240, appends every positive feedback record), and what its vector store does with repeated indices
+ *   is unpinned here (the xvec source is not available); gorse_b200_vecdb_add refuses such a vector.
+ *   An empty vector is not added (VectorWriter.Add, vector_writer.go:84-92): slot_out[i] = -1 and replace[i] is ignored, so the
+ *   previous version stays until gorse_b200_vecdb_delete_before.  The added rows take consecutive slots in row order
+ *   (slot_out[n]); hidden[n], categories (cat_off[n+1] / cats) and replace[n] (may be NULL) act on them as in gorse_b200_vecdb_add;
+ *   one timestamp_ms (the dataset's timestamp) for all of them.
+ *   GORSE_B200_ERR_ARG: a dense collection; NULL pointers; offsets that do not start at 0 or decrease; and what
+ *   gorse_b200_vecdb_add refuses -- a NaN value (an idf entry in use is NaN), an index >= 0x7fffffff, a row whose B indices do
+ *   not all exceed its A indices (a bad offset), a replace slot that does not exist yet.  GORSE_B200_ERR_UNSUPPORTED: more than
+ *   2^31 - 1 ids in one call.  The checks that need the ids run on the device into staging buffers; on any error the collection
+ *   is exactly as it was.  The new postings are merged into the index's device layouts, so the next query starts without a host
+ *   rebuild.  Takes the collection's lock, then its index's, as queries and compaction do. */
+int32_t gorse_b200_vecdb_add_idf_vectors(gorse_b200_vecdb *db, int64_t n, const int64_t *a_off, const int32_t *a_ids, const float *a_idf,
+                                         int32_t a_n_idf, uint32_t a_offset, const int64_t *b_off, const int32_t *b_ids, const float *b_idf,
+                                         int32_t b_n_idf, uint32_t b_offset, const uint8_t *hidden, int64_t timestamp_ms, const int64_t *cat_off,
+                                         const int32_t *cats, const int64_t *replace, int64_t *slot_out);
 /* GetVectors (xvec.go:320-363) by slot; live_out[i] = 0 for unknown or deleted slots.  Dense values_out[n*dim]. */
 int32_t gorse_b200_vecdb_get(gorse_b200_vecdb *db, const int64_t *slots, int64_t n, float *values_out, uint8_t *hidden_out,
                              int64_t *timestamp_out, uint8_t *live_out);
