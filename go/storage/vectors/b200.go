@@ -8,6 +8,11 @@
 // reach it with NO change to master / worker / logics -- set `database.vector_store = "b200://0"` (device ordinal) and the
 // init() below makes vectors.Open (database.go:168-175) return it.  The library works on slots and int32 category ids; this
 // file owns the id <-> slot and category string <-> id maps, which is all the reference's backends keep on the host too.
+//
+// "b200://<device>/<root>" also keeps every collection in <root>/<tablePrefix><name>.b200vec (root is an absolute path:
+// "b200://0/var/lib/gorse/vectors"), so that the master's collections reach a worker and a server that open the same URL on
+// a volume all of them mount, and survive a restart.  The process that writes a collection saves it; every process reloads a
+// collection whose file carries a newer generation before it reads it.  See INTEGRATION.md.
 
 //go:build b200 && cgo
 
@@ -17,13 +22,27 @@ package vectors
 #cgo LDFLAGS: -lgorse_b200
 #include <stdlib.h>
 #include "gorse_b200.h"
+
+// cgo cannot call Go closures from C directly: the snapshot stream goes through these exported trampolines.
+extern int32_t gorseB200SnapshotWrite(void *user, void *buf, int64_t n);
+extern int64_t gorseB200SnapshotRead(void *user, void *buf, int64_t n);
+static int32_t gorse_b200_snapshot_write_tramp(void *user, const void *buf, int64_t n) { return gorseB200SnapshotWrite(user, (void *)buf, n); }
+static int64_t gorse_b200_snapshot_read_tramp(void *user, void *buf, int64_t n) { return gorseB200SnapshotRead(user, buf, n); }
+static gorse_b200_write_fn gorse_b200_snapshot_write_ptr(void) { return gorse_b200_snapshot_write_tramp; }
+static gorse_b200_read_fn gorse_b200_snapshot_read_ptr(void) { return gorse_b200_snapshot_read_tramp; }
 */
 import "C"
 
 import (
+	"bufio"
 	"context"
+	"encoding/binary"
 	"fmt"
+	"io"
+	"os"
+	"path/filepath"
 	"runtime"
+	"runtime/cgo"
 	"sort"
 	"strconv"
 	"strings"
@@ -42,11 +61,15 @@ const b200Prefix = "b200://"
 
 func init() {
 	Register([]string{b200Prefix}, func(path, tablePrefix string, opts ...storage.Option) (Database, error) {
-		device, err := strconv.Atoi(strings.TrimPrefix(path, b200Prefix))
+		dev, root, _ := strings.Cut(strings.TrimPrefix(path, b200Prefix), "/")
+		device, err := strconv.Atoi(dev)
 		if err != nil {
 			device = 0
 		}
-		return &B200{device: device, tablePrefix: tablePrefix, collections: map[string]*b200Collection{}}, nil
+		if root != "" {
+			root = "/" + root
+		}
+		return &B200{device: device, tablePrefix: tablePrefix, root: root, collections: map[string]*b200Collection{}}, nil
 	})
 }
 
@@ -58,6 +81,12 @@ type b200Collection struct {
 	catsOf  [][]string       // slot -> categories (returned with query results, xvec.go:428-430)
 	catID   map[string]int32
 	catName []string
+	// with a root: the generation and the stat of the file last saved or loaded (generation 0: none yet), and writes not
+	// yet saved
+	generation int64
+	file       os.FileInfo
+	dirty      bool
+	lastWrite  time.Time
 }
 
 // B200 implements Database on one GPU.
@@ -65,8 +94,11 @@ type B200 struct {
 	mu          sync.RWMutex
 	device      int
 	tablePrefix string
+	root        string // "" = nothing is kept on disk
 	ctx         *C.gorse_b200_ctx
 	collections map[string]*b200Collection
+	stop        chan struct{}
+	flusher     sync.WaitGroup
 }
 
 var _ Database = (*B200)(nil)
@@ -78,13 +110,37 @@ func b200Err(st C.int32_t) error {
 	return errors.New(C.GoString(C.gorse_b200_last_error()))
 }
 
+// Init opens the device and, with a root, loads every <root>/<tablePrefix><name>.b200vec, as xvec's Init opens its
+// directories (xvec.go:60-123), and starts the flusher that saves collections 5 s after their last write.
 func (db *B200) Init() error {
 	db.mu.Lock()
 	defer db.mu.Unlock()
 	if db.ctx != nil {
 		return nil
 	}
-	return b200Err(C.gorse_b200_ctx_create(C.int32_t(db.device), &db.ctx))
+	if err := b200Err(C.gorse_b200_ctx_create(C.int32_t(db.device), &db.ctx)); err != nil {
+		return err
+	}
+	if db.root == "" {
+		return nil
+	}
+	if err := os.MkdirAll(db.root, 0o755); err != nil {
+		return errors.Trace(err)
+	}
+	files, err := filepath.Glob(filepath.Join(db.root, db.tablePrefix+"*"+b200FileSuffix))
+	if err != nil {
+		return errors.Trace(err)
+	}
+	for _, f := range files {
+		name := strings.TrimSuffix(strings.TrimPrefix(filepath.Base(f), db.tablePrefix), b200FileSuffix)
+		if err := db.reload(name); err != nil {
+			return err
+		}
+	}
+	db.stop = make(chan struct{})
+	db.flusher.Add(1)
+	go db.flush()
+	return nil
 }
 
 // Optimize reclaims the slots of deleted vectors (xvec.go:125-131 optimizes its index here): the live vectors keep their
@@ -96,7 +152,10 @@ func (db *B200) Optimize(ctx context.Context, name string) error {
 	if err != nil {
 		return err
 	}
-	return c.compact()
+	if err := c.compact(); err != nil {
+		return err
+	}
+	return db.save(name, c)
 }
 
 // compact runs gorse_b200_vecdb_compact and renames slotOf, idOf and catsOf through its map; the caller holds db.mu for
@@ -123,9 +182,18 @@ func (c *b200Collection) compact() error {
 }
 
 func (db *B200) Close() error {
+	if db.stop != nil {
+		close(db.stop)
+		db.flusher.Wait()
+		db.stop = nil
+	}
 	db.mu.Lock()
 	defer db.mu.Unlock()
+	var saveErr error
 	for name, c := range db.collections {
+		if err := db.save(name, c); err != nil && saveErr == nil {
+			saveErr = err
+		}
 		C.gorse_b200_vecdb_destroy(c.handle)
 		delete(db.collections, name)
 	}
@@ -133,10 +201,30 @@ func (db *B200) Close() error {
 		C.gorse_b200_ctx_destroy(db.ctx)
 		db.ctx = nil
 	}
-	return nil
+	return saveErr
 }
 
 func (db *B200) ListCollections(ctx context.Context) ([]string, error) {
+	if db.root != "" { // the collections another process saved
+		files, err := filepath.Glob(filepath.Join(db.root, db.tablePrefix+"*"+b200FileSuffix))
+		if err != nil {
+			return nil, errors.Trace(err)
+		}
+		names := map[string]struct{}{}
+		for _, f := range files {
+			names[strings.TrimSuffix(strings.TrimPrefix(filepath.Base(f), db.tablePrefix), b200FileSuffix)] = struct{}{}
+		}
+		db.mu.RLock()
+		for name := range db.collections { // and the ones whose file was removed: refresh forgets them
+			names[name] = struct{}{}
+		}
+		db.mu.RUnlock()
+		for name := range names {
+			if err := db.refresh(name); err != nil {
+				return nil, err
+			}
+		}
+	}
 	db.mu.RLock()
 	defer db.mu.RUnlock()
 	names := make([]string, 0, len(db.collections))
@@ -156,6 +244,9 @@ func (db *B200) collection(name string) (*b200Collection, error) {
 }
 
 func (db *B200) DescribeCollection(ctx context.Context, name string) (*CollectionInfo, error) {
+	if err := db.refresh(name); err != nil {
+		return nil, err
+	}
 	db.mu.RLock()
 	defer db.mu.RUnlock()
 	c, err := db.collection(name)
@@ -182,6 +273,7 @@ func (db *B200) AddCollection(ctx context.Context, name string, dimensions int, 
 		return err
 	}
 	db.collections[name] = c
+	c.touch()
 	return nil
 }
 
@@ -193,10 +285,18 @@ func (db *B200) DeleteCollection(ctx context.Context, name string) error {
 		return err
 	}
 	delete(db.collections, name)
+	if db.root != "" {
+		if err := os.Remove(db.path(name)); err != nil && !os.IsNotExist(err) {
+			return errors.Trace(err)
+		}
+	}
 	return b200Err(C.gorse_b200_vecdb_destroy(c.handle))
 }
 
 func (db *B200) CountVectors(ctx context.Context, name string) (int64, error) {
+	if err := db.refresh(name); err != nil {
+		return 0, err
+	}
 	db.mu.RLock()
 	defer db.mu.RUnlock()
 	c, err := db.collection(name)
@@ -275,6 +375,7 @@ func (db *B200) AddVectors(ctx context.Context, name string, vectors []Vector) e
 		c.idOf = append(c.idOf, v.Id)
 		c.catsOf = append(c.catsOf, v.Categories)
 	}
+	c.touch()
 	return nil
 }
 
@@ -357,6 +458,7 @@ func (db *B200) AddIDFVectors(ctx context.Context, name string, ids []string, hi
 		c.idOf = append(c.idOf, id)
 		c.catsOf = append(c.catsOf, categories[i])
 	}
+	c.touch()
 	return nil
 }
 
@@ -376,6 +478,9 @@ func flattenCSR(rows [][]int32) ([]int64, []int32) {
 func (db *B200) GetVectors(ctx context.Context, name string, ids []string) ([]Vector, error) {
 	if len(ids) == 0 {
 		return []Vector{}, nil
+	}
+	if err := db.refresh(name); err != nil {
+		return nil, err
 	}
 	db.mu.RLock()
 	defer db.mu.RUnlock()
@@ -442,6 +547,9 @@ func (db *B200) DeleteVectors(ctx context.Context, name string, timestamp time.T
 			delete(c.slotOf, c.idOf[slot])
 		}
 	}
+	if count > 0 {
+		c.touch()
+	}
 	// the master rewrites every vector once per cycle and then deletes the old versions here: compacting once the dead
 	// slots are as many as the live ones keeps a collection at most twice its live size
 	var live, total C.int64_t
@@ -449,15 +557,21 @@ func (db *B200) DeleteVectors(ctx context.Context, name string, timestamp time.T
 		return err
 	}
 	if total-live >= live {
-		return c.compact()
+		if err := c.compact(); err != nil {
+			return err
+		}
 	}
-	return nil
+	// VectorWriter.Clean ends every rewrite here: the rewritten collection goes to disk now
+	return db.save(name, c)
 }
 
 // QueryVectors: filter "hidden = false AND categories CONTAIN_ALL (...)" (xvec.go:381-389) evaluated on the device.
 func (db *B200) QueryVectors(ctx context.Context, name string, q Vector, categories []string, topK int) ([]ScoredVector, error) {
 	if topK <= 0 {
 		return []ScoredVector{}, nil
+	}
+	if err := db.refresh(name); err != nil {
+		return nil, err
 	}
 	db.mu.RLock()
 	defer db.mu.RUnlock()
@@ -518,6 +632,9 @@ func (db *B200) QueryVectorsExcluding(ctx context.Context, name string, queries 
 	results := make([][]ScoredVector, len(queries))
 	if len(queries) == 0 || n <= 0 {
 		return results, nil
+	}
+	if err := db.refresh(name); err != nil {
+		return nil, err
 	}
 	db.mu.RLock()
 	defer db.mu.RUnlock()
@@ -584,6 +701,9 @@ func (db *B200) ItemToItemRecommend(ctx context.Context, collection string, cont
 	results := make([][]cache.Score, len(contextIds))
 	if len(contextIds) == 0 || n <= 0 {
 		return results, nil
+	}
+	if err := db.refresh(collection); err != nil {
+		return nil, err
 	}
 	db.mu.RLock()
 	defer db.mu.RUnlock()
@@ -659,6 +779,9 @@ func (db *B200) UserToUserRecommend(ctx context.Context, collection string, user
 	results := make([][]cache.Score, len(userIds))
 	if len(userIds) == 0 || n <= 0 {
 		return results, nil
+	}
+	if err := db.refresh(collection); err != nil {
+		return nil, err
 	}
 	db.mu.RLock()
 	defer db.mu.RUnlock()
@@ -763,6 +886,9 @@ func (db *B200) SessionRecommend(ctx context.Context, collection string, context
 	if len(contextIds) == 0 || top <= 0 {
 		return results, nil
 	}
+	if err := db.refresh(collection); err != nil {
+		return nil, err
+	}
 	db.mu.RLock()
 	defer db.mu.RUnlock()
 	c, err := db.collection(collection)
@@ -865,4 +991,310 @@ func u8p(s []uint8) *C.uint8_t {
 		return nil
 	}
 	return (*C.uint8_t)(unsafe.Pointer(&s[0]))
+}
+
+// ---- collections on disk (a root in the URL) ----
+//
+// File <root>/<tablePrefix><name>.b200vec: the shim's header, little-endian --
+//   magic "GB200SHM", u32 version 1, i64 generation (the writer's clock in ns at the save), i32 dimension, i32 distance,
+//   u32 category names then each as u32 length + bytes, u64 vectors then per vector in saved-slot order its id (u32 length +
+//   bytes) and its categories (u32 count + u32 name indices)
+// -- then the library's stream (gorse_b200_vecdb_save; format in include/gorse_b200.h), whose vector i is the header's i-th.
+// A save writes <file>.tmp, fsyncs it and renames it into place, so a reader sees the previous file until the rename.
+
+const b200FileSuffix = ".b200vec"
+
+var b200FileMagic = [8]byte{'G', 'B', '2', '0', '0', 'S', 'H', 'M'}
+
+func (db *B200) path(name string) string {
+	return filepath.Join(db.root, db.tablePrefix+name+b200FileSuffix)
+}
+
+// touch marks a write of this process: the collection is saved by the next save point or 5 s after its last write
+func (c *b200Collection) touch() {
+	c.dirty, c.lastWrite = true, time.Now()
+}
+
+// flush saves every collection that has seen no write for 5 s: the CF hand-off (master/tasks.go:930-961) ends without a
+// closing call
+func (db *B200) flush() {
+	defer db.flusher.Done()
+	tick := time.NewTicker(time.Second)
+	defer tick.Stop()
+	for {
+		select {
+		case <-db.stop:
+			return
+		case <-tick.C:
+		}
+		db.mu.Lock()
+		for name, c := range db.collections {
+			if c.dirty && time.Since(c.lastWrite) >= 5*time.Second {
+				if err := db.save(name, c); err != nil {
+					log.Logger().Error("save vector collection", zap.String("collection", name), zap.Error(err))
+				}
+			}
+		}
+		db.mu.Unlock()
+	}
+}
+
+// save writes a collection with unsaved writes to its file; the caller holds db.mu for writing
+func (db *B200) save(name string, c *b200Collection) error {
+	if db.root == "" || !c.dirty {
+		return nil
+	}
+	path := db.path(name)
+	f, err := os.Create(path + ".tmp")
+	if err != nil {
+		return errors.Trace(err)
+	}
+	defer os.Remove(path + ".tmp") // after a successful rename there is nothing to remove
+	generation := time.Now().UnixNano()
+	if generation <= c.generation {
+		generation = c.generation + 1
+	}
+	// the library's live slots are the stream's vectors (an id added twice in one call holds two live slots)
+	slots, live := make([]int64, len(c.idOf)), make([]uint8, len(c.idOf))
+	for i := range slots {
+		slots[i] = int64(i)
+	}
+	if err := b200Err(C.gorse_b200_vecdb_get(c.handle, i64p(slots), C.int64_t(len(slots)), nil, nil, nil, u8p(live))); err != nil {
+		f.Close()
+		return err
+	}
+	w := bufio.NewWriterSize(f, 1<<20)
+	if err := c.writeHeader(w, generation, live); err != nil {
+		f.Close()
+		return err
+	}
+	h := cgo.NewHandle(io.Writer(w))
+	st := C.gorse_b200_vecdb_save(c.handle, C.gorse_b200_snapshot_write_ptr(), unsafe.Pointer(&h), nil, nil)
+	h.Delete()
+	if err := b200Err(st); err != nil {
+		f.Close()
+		return err
+	}
+	if err := w.Flush(); err != nil {
+		f.Close()
+		return errors.Trace(err)
+	}
+	if err := f.Sync(); err != nil {
+		f.Close()
+		return errors.Trace(err)
+	}
+	if err := f.Close(); err != nil {
+		return errors.Trace(err)
+	}
+	if err := os.Rename(path+".tmp", path); err != nil {
+		return errors.Trace(err)
+	}
+	st2, err := os.Stat(path)
+	if err != nil {
+		return errors.Trace(err)
+	}
+	c.generation, c.file, c.dirty = generation, st2, false
+	return nil
+}
+
+// writeHeader writes the shim's header: the ids of the live slots in slot order, which is the order of the library's stream
+func (c *b200Collection) writeHeader(w io.Writer, generation int64, live []uint8) error {
+	le := binary.LittleEndian
+	buf := append([]byte{}, b200FileMagic[:]...)
+	buf = le.AppendUint32(buf, 1)
+	buf = le.AppendUint64(buf, uint64(generation))
+	buf = le.AppendUint32(buf, uint32(int32(c.info.Dimension)))
+	buf = le.AppendUint32(buf, uint32(int32(c.info.Distance)))
+	buf = le.AppendUint32(buf, uint32(len(c.catName)))
+	for _, s := range c.catName {
+		buf = le.AppendUint32(buf, uint32(len(s)))
+		buf = append(buf, s...)
+	}
+	n := 0
+	for _, l := range live {
+		n += int(l)
+	}
+	buf = le.AppendUint64(buf, uint64(n))
+	for slot, id := range c.idOf {
+		if live[slot] == 0 {
+			continue // a deleted slot: not in the stream
+		}
+		buf = le.AppendUint32(buf, uint32(len(id)))
+		buf = append(buf, id...)
+		buf = le.AppendUint32(buf, uint32(len(c.catsOf[slot])))
+		for _, cat := range c.catsOf[slot] {
+			buf = le.AppendUint32(buf, uint32(c.catID[cat]))
+		}
+	}
+	_, err := w.Write(buf)
+	return errors.Trace(err)
+}
+
+// refresh reloads a collection whose file another process has replaced since this one last saved or loaded it, and forgets
+// one whose file another process has removed (DeleteCollection on the master: the CF collection of an older model); slot
+// maps taken earlier go stale, as after a compaction
+func (db *B200) refresh(name string) error {
+	if db.root == "" {
+		return nil
+	}
+	st, err := os.Stat(db.path(name))
+	if os.IsNotExist(err) {
+		db.mu.Lock()
+		defer db.mu.Unlock()
+		if c, ok := db.collections[name]; ok && !c.dirty && c.generation > 0 {
+			delete(db.collections, name)
+			return b200Err(C.gorse_b200_vecdb_destroy(c.handle))
+		}
+		return nil // never saved, or writes not saved yet: what this process holds stands
+	}
+	if err != nil {
+		return errors.Trace(err)
+	}
+	db.mu.RLock()
+	c, ok := db.collections[name]
+	current := ok && (c.dirty || sameFile(st, c.file))
+	db.mu.RUnlock()
+	if current {
+		return nil
+	}
+	db.mu.Lock()
+	defer db.mu.Unlock()
+	return db.reload(name)
+}
+
+// sameFile: the file last saved or loaded is still in place.  Every save renames a new file into place, so the inode
+// changes even when two saves land in one tick of a coarse modification time.
+func sameFile(st, last os.FileInfo) bool {
+	return last != nil && os.SameFile(st, last) && st.Size() == last.Size() && st.ModTime().Equal(last.ModTime())
+}
+
+// reload loads <root>/<name> when its generation is newer than the collection this process holds (or it holds none) and
+// swaps the handle and the id maps; the caller holds db.mu for writing
+func (db *B200) reload(name string) error {
+	old, ok := db.collections[name]
+	if ok && old.dirty {
+		return nil
+	}
+	f, err := os.Open(db.path(name))
+	if err != nil {
+		return errors.Trace(err)
+	}
+	defer f.Close()
+	st, err := f.Stat()
+	if err != nil {
+		return errors.Trace(err)
+	}
+	r := bufio.NewReaderSize(f, 1<<20)
+	c, err := readHeader(r, name)
+	if err != nil {
+		return errors.Annotatef(err, "vector collection file %s", db.path(name))
+	}
+	c.file = st
+	if ok && c.generation <= old.generation {
+		old.file = st
+		return nil
+	}
+	h := cgo.NewHandle(io.Reader(r))
+	var count C.int64_t
+	status := C.gorse_b200_vecdb_load(db.ctx, C.gorse_b200_snapshot_read_ptr(), unsafe.Pointer(&h), &c.handle, nil)
+	h.Delete()
+	if err := b200Err(status); err != nil {
+		return errors.Annotatef(err, "vector collection file %s", db.path(name))
+	}
+	if err := b200Err(C.gorse_b200_vecdb_count(c.handle, &count, nil)); err != nil || int(count) != len(c.idOf) {
+		C.gorse_b200_vecdb_destroy(c.handle)
+		return errors.Errorf("vector collection file %s: %d ids for %d vectors", db.path(name), len(c.idOf), int64(count))
+	}
+	if ok {
+		C.gorse_b200_vecdb_destroy(old.handle)
+	}
+	db.collections[name] = c
+	return nil
+}
+
+// readHeader reads the shim's header into a collection without a handle
+func readHeader(r io.Reader, name string) (*b200Collection, error) {
+	le := binary.LittleEndian
+	var fixed [32]byte
+	if _, err := io.ReadFull(r, fixed[:]); err != nil {
+		return nil, errors.Trace(err)
+	}
+	if [8]byte(fixed[:8]) != b200FileMagic || le.Uint32(fixed[8:]) != 1 {
+		return nil, errors.New("not a b200 collection file of version 1")
+	}
+	c := &b200Collection{info: CollectionInfo{Name: name, Dimension: int(int32(le.Uint32(fixed[20:]))), Distance: Distance(int32(le.Uint32(fixed[24:])))},
+		slotOf: map[string]int64{}, catID: map[string]int32{}, generation: int64(le.Uint64(fixed[12:]))}
+	u32 := func() (uint32, error) {
+		var b [4]byte
+		_, err := io.ReadFull(r, b[:])
+		return le.Uint32(b[:]), err
+	}
+	str := func() (string, error) {
+		n, err := u32()
+		if err != nil {
+			return "", err
+		}
+		b := make([]byte, n)
+		_, err = io.ReadFull(r, b)
+		return string(b), err
+	}
+	nCats := le.Uint32(fixed[28:])
+	for i := uint32(0); i < nCats; i++ {
+		s, err := str()
+		if err != nil {
+			return nil, errors.Trace(err)
+		}
+		c.catID[s], c.catName = int32(i), append(c.catName, s)
+	}
+	var nb [8]byte
+	if _, err := io.ReadFull(r, nb[:]); err != nil {
+		return nil, errors.Trace(err)
+	}
+	n := le.Uint64(nb[:])
+	for slot := uint64(0); slot < n; slot++ {
+		id, err := str()
+		if err != nil {
+			return nil, errors.Trace(err)
+		}
+		k, err := u32()
+		if err != nil {
+			return nil, errors.Trace(err)
+		}
+		cats := make([]string, 0, k)
+		for j := uint32(0); j < k; j++ {
+			x, err := u32()
+			if err != nil {
+				return nil, errors.Trace(err)
+			}
+			if x >= nCats {
+				return nil, errors.Errorf("category %d of %d names", x, nCats)
+			}
+			cats = append(cats, c.catName[x])
+		}
+		c.slotOf[id] = int64(slot) // an id held twice: the later slot, as after the add
+		c.idOf, c.catsOf = append(c.idOf, id), append(c.catsOf, cats)
+	}
+	return c, nil
+}
+
+//export gorseB200SnapshotWrite
+func gorseB200SnapshotWrite(user unsafe.Pointer, buf unsafe.Pointer, n C.int64_t) C.int32_t {
+	w := (*(*cgo.Handle)(user)).Value().(io.Writer) // user = &handle, the documented way to carry a Handle in a void*
+	if _, err := w.Write(unsafe.Slice((*byte)(buf), int(n))); err != nil {
+		return 1
+	}
+	return 0
+}
+
+//export gorseB200SnapshotRead
+func gorseB200SnapshotRead(user unsafe.Pointer, buf unsafe.Pointer, n C.int64_t) C.int64_t {
+	r := (*(*cgo.Handle)(user)).Value().(io.Reader)
+	k, err := io.ReadAtLeast(r, unsafe.Slice((*byte)(buf), int(n)), 1)
+	if k > 0 {
+		return C.int64_t(k)
+	}
+	if err == io.EOF {
+		return 0
+	}
+	return -1
 }

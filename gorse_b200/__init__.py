@@ -415,6 +415,13 @@ class SparseIndex:
         self.close()
 
 
+def _check_stream(status, err):
+    """check() for a call that ran a file object's callbacks: an exception raised there is the cause of the error"""
+    if status != _lib.OK and err:
+        raise GorseB200Error(status, lib.gorse_b200_last_error().decode("utf-8", "replace")) from err[0]
+    check(status)
+
+
 class VectorCollection:
     """One collection of a vectors.Database on the GPU (gorse_b200_vecdb_*; storage/vectors/database.go:107-120).  Works on
     slots and int category ids; the Go shim keeps the id / category string maps."""
@@ -511,6 +518,53 @@ class VectorCollection:
         new_slot, nbytes = np.zeros(max(slots, 1), np.int64), np.zeros(2, np.int64)
         check(lib.gorse_b200_vecdb_compact(self.h, ptr(new_slot), ptr(nbytes)))
         return new_slot[:slots], int(nbytes[0]), int(nbytes[1])
+
+    def save(self, fileobj):
+        """Write the collection to a binary file object as a snapshot stream (gorse_b200_vecdb_save; the format is in
+        include/gorse_b200.h).  The collection does not change.
+        -> new_slot int64 [slots]: the position of each slot's vector in the stream, -1 for a deleted slot (compact()'s map)"""
+        slots = self.count()[1]
+        new_slot, nbytes, err = np.zeros(max(slots, 1), np.int64), C.c_int64(0), []
+
+        def write(user, buf, n):
+            try:
+                mv = memoryview((C.c_char * n).from_address(buf)).cast("B")
+                while mv:   # a raw file may write part of the buffer
+                    k = fileobj.write(mv)
+                    mv = mv[len(mv) if k is None else k:]
+                return 0
+            except Exception as e:  # reported as GORSE_B200_ERR_IO, re-raised as the cause
+                err.append(e)
+                return 1
+
+        st = lib.gorse_b200_vecdb_save(self.h, _lib.WRITE_FN(write), None, ptr(new_slot), C.byref(nbytes))
+        _check_stream(st, err)
+        return new_slot[:slots]
+
+    @classmethod
+    def load(cls, ctx, fileobj):
+        """A collection on ctx rebuilt from a snapshot stream read from a binary file object (gorse_b200_vecdb_load): vector i
+        of the stream is in slot i, and every entry answers as the saved collection answers after compact().  Exactly the
+        stream's bytes are read."""
+        head, h, nbytes, err = bytearray(), C.c_void_p(), C.c_int64(0), []
+
+        def read(user, buf, n):
+            try:
+                mv = memoryview((C.c_char * n).from_address(buf)).cast("B")
+                got = fileobj.readinto(mv) or 0
+                if len(head) < 48:
+                    head.extend(mv[:min(got, 48 - len(head))])
+                return got
+            except Exception as e:
+                err.append(e)
+                return -1
+
+        st = lib.gorse_b200_vecdb_load(ctx.h, _lib.READ_FN(read), None, C.byref(h), C.byref(nbytes))
+        _check_stream(st, err)
+        self = cls.__new__(cls)
+        self.ctx, self.h = ctx, h
+        self.dim, self.distance = (int(x) for x in np.frombuffer(bytes(head[12:20]), "<i4"))
+        return self
 
     def query(self, q, categories=(), topk=10):
         """q: dense [nq, dim] array, or a list of (indices, values) for a sparse collection.

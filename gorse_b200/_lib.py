@@ -13,7 +13,7 @@ LIB_PATH = os.path.join(_HERE, "libgorse_b200.so")
 NCCL_ID_BYTES = 128
 
 OK = 0
-ERR_ARG, ERR_CUDA, ERR_NCCL, ERR_OOM, ERR_RANGE, ERR_STATE, ERR_UNSUPPORTED = -1, -2, -3, -4, -5, -6, -7
+ERR_ARG, ERR_CUDA, ERR_NCCL, ERR_OOM, ERR_RANGE, ERR_STATE, ERR_UNSUPPORTED, ERR_IO = -1, -2, -3, -4, -5, -6, -7, -8
 
 SCATTER_STORE, SCATTER_ATOMIC = 0, 1
 ORDER_HOGWILD, ORDER_SEQUENTIAL = 0, 1
@@ -97,6 +97,8 @@ PROTOTYPES = {
     "gorse_b200_vecdb_get_sparse": (C.c_int32, [VP, C.c_int64, VP, VP, C.c_int32, C.POINTER(C.c_int32)]),
     "gorse_b200_vecdb_delete_before": (C.c_int32, [VP, C.c_int64, VP, C.c_int64, C.POINTER(C.c_int64)]),
     "gorse_b200_vecdb_compact": (C.c_int32, [VP, VP, VP]),
+    "gorse_b200_vecdb_save": (C.c_int32, [VP, VP, VP, VP, C.POINTER(C.c_int64)]),
+    "gorse_b200_vecdb_load": (C.c_int32, [VP, VP, VP, PVP, C.POINTER(C.c_int64)]),
     "gorse_b200_vecdb_add_item_factors": (C.c_int32, [VP, VP, VP, C.c_int64, VP, VP, VP]),
     "gorse_b200_marshal_latent_factors": (C.c_int32, [VP, C.c_int32, C.c_int32, VP, VP, VP, C.c_size_t, C.POINTER(C.c_size_t)]),
     "gorse_b200_vecdb_query": (C.c_int32, [VP, C.c_int64, VP, VP, VP, VP, C.c_int32, C.c_int32, VP, VP, VP]),
@@ -188,6 +190,8 @@ class RecommendRanker(C.Structure):
 PROGRESS_FN = C.CFUNCTYPE(C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_float)
 TRIALS_PROGRESS_FN = C.CFUNCTYPE(C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.POINTER(TrialState))
 FM_TRIALS_PROGRESS_FN = C.CFUNCTYPE(C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.POINTER(FMTrialState))
+WRITE_FN = C.CFUNCTYPE(C.c_int32, C.c_void_p, C.c_void_p, C.c_int64)   # gorse_b200_write_fn
+READ_FN = C.CFUNCTYPE(C.c_int64, C.c_void_p, C.c_void_p, C.c_int64)    # gorse_b200_read_fn
 
 
 class GorseB200Error(RuntimeError):

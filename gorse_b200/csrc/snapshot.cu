@@ -1,0 +1,423 @@
+// snapshot.cu -- a vector collection written as a byte stream (gorse_b200_vecdb_save) and rebuilt from one on any context
+// (gorse_b200_vecdb_load): what lets a worker, a server or a restarted master hold the collections the master built, as the
+// reference's default backend reopens its collections from disk in Init (storage/vectors/xvec.go:60-123).  The stream format
+// is documented in include/gorse_b200.h.
+//
+// Dense rows never pass through a host copy of the collection: save gathers each chunk's live rows on the device (the live-slot
+// scan of compaction names them) and downloads it on the copy stream into one of two pinned staging buffers while the callback
+// writes the other; load fills one pinned buffer from the callback while the other is copied into the index's rows.  The
+// metadata and the sparse rows are host state of the collection already; they stream through the same staging buffer.
+#include <algorithm>
+#include <cmath>
+
+#include "sparse.cuh"
+#include "vecdb.cuh"
+
+namespace gb {
+namespace {
+
+constexpr char MAGIC[8] = {'G', 'B', '2', '0', '0', 'V', 'D', 'B'};
+constexpr uint32_t VERSION = 1;
+constexpr int64_t STAGE_BYTES = 64ll << 20;   // each of the two staging buffers, at most
+constexpr int64_t MIN_STAGE_BYTES = 64ll << 10;   // one row of the widest dense collection (16384 fp32)
+
+struct Header {
+    char magic[8];
+    uint32_t version;
+    int32_t dim, distance;
+    uint32_t reserved;
+    int64_t n, nnz, n_cats;
+};
+static_assert(sizeof(Header) == 48, "the stream header is 48 bytes without padding");
+
+// out[(j - j0) * d ..] = X[slot(j) * d ..] for the live rows j in [j0, j0 + m): slot(j) is the slot whose scan entry is j and
+// whose successor's is j + 1, found by a binary search of scan[0 .. n] (scan[n] = the live count).  One warp per row;
+// V = float4 when d % 4 == 0 (dv = d / 4), else float (dv = d).
+template <typename V>
+__global__ void snapshot_gather_kernel(const V *X, int dv, const int64_t *scan, int64_t n, int64_t j0, int64_t m, V *out)
+{
+    const int lane = threadIdx.x & 31;
+    const int64_t nw = ((int64_t)gridDim.x * blockDim.x) >> 5;
+    for (int64_t r = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5; r < m; r += nw) {
+        const int64_t j = j0 + r;
+        int64_t lo = 0, hi = n;   // scan[lo] <= j < scan[hi]
+        while (hi - lo > 1) {
+            const int64_t mid = (lo + hi) >> 1;
+            if (__ldg(scan + mid) <= j) lo = mid;
+            else hi = mid;
+        }
+        const V *src = X + lo * dv;
+        V *dst = out + r * dv;
+        for (int c = lane; c < dv; c += 32) dst[c] = src[c];
+    }
+}
+
+// the two pinned staging buffers, the device gather buffers and their events; released after both streams have drained
+struct Staging {
+    gorse_b200_ctx *c = nullptr;
+    void *h[2] = {nullptr, nullptr};
+    DevBuf<float> d[2];
+    cudaEvent_t gathered[2] = {nullptr, nullptr}, copied[2] = {nullptr, nullptr};
+    int32_t alloc(gorse_b200_ctx *ctx, int64_t bytes, int buffers, bool device)
+    {
+        c = ctx;
+        for (int b = 0; b < buffers; b++) {
+            GB_CUDA(cudaHostAlloc(&h[b], (size_t)bytes, cudaHostAllocDefault));
+            GB_CUDA(cudaEventCreateWithFlags(&copied[b], cudaEventDisableTiming));
+            if (!device) continue;
+            GB_TRY(d[b].alloc((size_t)bytes / sizeof(float)));
+            GB_CUDA(cudaEventCreateWithFlags(&gathered[b], cudaEventDisableTiming));
+        }
+        return GORSE_B200_OK;
+    }
+    ~Staging()
+    {
+        if (!c) return;
+        cudaStreamSynchronize(c->stream);
+        cudaStreamSynchronize(c->copy_stream);
+        for (int b = 0; b < 2; b++) {
+            if (h[b]) cudaFreeHost(h[b]);
+            d[b].free();
+            if (gathered[b]) cudaEventDestroy(gathered[b]);
+            if (copied[b]) cudaEventDestroy(copied[b]);
+        }
+    }
+};
+
+// the caller's write callback behind a staging buffer: put() appends and hands full buffers on, direct() hands a buffer of the
+// caller's on after the pending bytes
+struct Writer {
+    gorse_b200_write_fn fn;
+    void *user;
+    char *buf;
+    int64_t cap, used = 0, pos = 0;   // pos: bytes handed to the callback
+    int32_t direct(const void *p, int64_t bytes)
+    {
+        if (bytes == 0) return GORSE_B200_OK;
+        if (fn(user, p, bytes) != 0) {
+            set_error("snapshot save: the write callback failed at byte %lld", (long long)pos);
+            return GORSE_B200_ERR_IO;
+        }
+        pos += bytes;
+        return GORSE_B200_OK;
+    }
+    int32_t flush()
+    {
+        const int64_t m = used;
+        used = 0;
+        return direct(buf, m);
+    }
+    int32_t put(const void *src, int64_t bytes)
+    {
+        const char *s = static_cast<const char *>(src);
+        while (bytes > 0) {
+            const int64_t m = std::min(bytes, cap - used);
+            memcpy(buf + used, s, (size_t)m);
+            used += m; s += m; bytes -= m;
+            if (used == cap) GB_TRY(flush());
+        }
+        return GORSE_B200_OK;
+    }
+};
+
+// the caller's read callback: get() reads exactly `bytes` or fails, naming the field and its byte offset
+struct Reader {
+    gorse_b200_read_fn fn;
+    void *user;
+    int64_t pos = 0;   // bytes read
+    int32_t get(void *dst, int64_t bytes, const char *field)
+    {
+        char *d = static_cast<char *>(dst);
+        while (bytes > 0) {
+            const int64_t r = fn(user, d, bytes);
+            if (r < 0 || r > bytes) {
+                set_error("snapshot load: the read callback failed at byte %lld (%s)", (long long)pos, field);
+                return GORSE_B200_ERR_IO;
+            }
+            if (r == 0) {
+                set_error("snapshot load: the stream ends at byte %lld, inside %s", (long long)pos, field);
+                return GORSE_B200_ERR_ARG;
+            }
+            d += r; bytes -= r; pos += r;
+        }
+        return GORSE_B200_OK;
+    }
+    // count elements into v, grown piece by piece: a header that claims more than the stream holds allocates no more than arrived
+    template <typename T>
+    int32_t array(std::vector<T> &v, int64_t count, const char *field)
+    {
+        constexpr int64_t PIECE = (4ll << 20) / (int64_t)sizeof(T);
+        v.clear();
+        for (int64_t i = 0; i < count; i += PIECE) {
+            const int64_t m = std::min(PIECE, count - i);
+            v.resize((size_t)(i + m));
+            GB_TRY(get(v.data() + i, m * (int64_t)sizeof(T), field));
+        }
+        return GORSE_B200_OK;
+    }
+};
+
+#define SNAP_CHECK(cond, field, at, what)                                                                            \
+    do {                                                                                                             \
+        if (!(cond)) {                                                                                               \
+            gb::set_error("snapshot load: bad %s at byte %lld: %s", field, (long long)(at), what);                   \
+            return GORSE_B200_ERR_ARG;                                                                               \
+        }                                                                                                            \
+    } while (0)
+
+// offsets[n + 1] of a section starting at byte `at`: from 0, never decreasing, ending at `total`
+int32_t check_offsets(const std::vector<int64_t> &off, int64_t total, const char *field, int64_t at)
+{
+    SNAP_CHECK(off[0] == 0, field, at, "the first offset is not 0");
+    const int64_t n = (int64_t)off.size() - 1;
+    for (int64_t i = 0; i < n; i++) SNAP_CHECK(off[(size_t)i + 1] >= off[(size_t)i], field, at + 8 * (i + 1), "offsets decrease");
+    SNAP_CHECK(off[(size_t)n] == total, field, at + 8 * n, "the last offset disagrees with the header's count");
+    return GORSE_B200_OK;
+}
+
+int32_t save(gorse_b200_vecdb *db, gorse_b200_write_fn write, void *user, int64_t *new_slot_out, int64_t *bytes_out)
+{
+    std::lock_guard<std::mutex> lk(db->mu);
+    std::lock_guard<std::mutex> lk2(db->dense ? db->dense->mu : db->sparse->mu);
+    gorse_b200_ctx *c = db->ctx;
+    ScopedDevice sd(c->device);
+    const int64_t n = (int64_t)db->ts.size(), live = db->live, dim = db->dim;
+    const gorse_b200_sparse_index *sx = db->sparse;
+    Header h{};
+    memcpy(h.magic, MAGIC, sizeof(MAGIC));
+    h.version = VERSION;
+    h.dim = db->dim;
+    h.distance = db->distance;
+    h.n = live;
+    for (int64_t s = 0; s < n; s++) {
+        if (db->dead[(size_t)s]) continue;
+        h.n_cats += db->cat_off[(size_t)s + 1] - db->cat_off[(size_t)s];
+        if (sx) h.nnz += sx->h_off[(size_t)s + 1] - sx->h_off[(size_t)s];
+    }
+    const int64_t values = dim > 0 ? 4 * live * dim : 8 * (live + 1) + 8 * h.nnz;
+    const int64_t total = (int64_t)sizeof(Header) + 17 * live + 8 + 4 * h.n_cats + values;
+    Staging stg;
+    const int64_t cap = std::min(STAGE_BYTES, std::max(MIN_STAGE_BYTES, total));
+    GB_TRY(stg.alloc(c, cap, dim > 0 && live > 0 ? 2 : 1, dim > 0 && live > 0));
+    Writer w{write, user, static_cast<char *>(stg.h[0]), cap};
+    GB_TRY(w.put(&h, sizeof(h)));
+    for (int64_t s = 0; s < n; s++)
+        if (!db->dead[(size_t)s]) GB_TRY(w.put(&db->hidden[(size_t)s], 1));
+    for (int64_t s = 0; s < n; s++)
+        if (!db->dead[(size_t)s]) GB_TRY(w.put(&db->ts[(size_t)s], 8));
+    int64_t o = 0;
+    GB_TRY(w.put(&o, 8));
+    for (int64_t s = 0; s < n; s++)
+        if (!db->dead[(size_t)s]) {
+            o += db->cat_off[(size_t)s + 1] - db->cat_off[(size_t)s];
+            GB_TRY(w.put(&o, 8));
+        }
+    for (int64_t s = 0; s < n; s++)
+        if (!db->dead[(size_t)s])
+            GB_TRY(w.put(db->cats.data() + db->cat_off[(size_t)s], 4 * (db->cat_off[(size_t)s + 1] - db->cat_off[(size_t)s])));
+    if (sx) {
+        o = 0;
+        GB_TRY(w.put(&o, 8));
+        for (int64_t s = 0; s < n; s++)
+            if (!db->dead[(size_t)s]) {
+                o += sx->h_off[(size_t)s + 1] - sx->h_off[(size_t)s];
+                GB_TRY(w.put(&o, 8));
+            }
+        for (int64_t s = 0; s < n; s++)
+            if (!db->dead[(size_t)s]) GB_TRY(w.put(sx->h_ind.data() + sx->h_off[(size_t)s], 4 * (sx->h_off[(size_t)s + 1] - sx->h_off[(size_t)s])));
+        for (int64_t s = 0; s < n; s++)
+            if (!db->dead[(size_t)s]) GB_TRY(w.put(sx->h_val.data() + sx->h_off[(size_t)s], 4 * (sx->h_off[(size_t)s + 1] - sx->h_off[(size_t)s])));
+    }
+    GB_TRY(w.flush());
+    if (dim > 0 && live > 0) {
+        // chunk k = the live rows [k R, k R + R): gathered into d[k & 1] on the stream, downloaded into h[k & 1] on the copy
+        // stream, written while chunk k + 1 moves; chunk k + 2 reuses the buffers once chunk k is written
+        DevBuf<int64_t> scan;
+        int32_t st = vecdb_live_scan(db, scan, nullptr);
+        if (st) return st;
+        const gorse_b200_index *ix = db->dense;
+        const int64_t R = cap / (4 * dim), chunks = (live + R - 1) / R;
+        auto enqueue = [&](int64_t k) {
+            const int b = (int)(k & 1);
+            const int64_t j0 = k * R, m = std::min(R, live - j0);
+            const unsigned grid = (unsigned)std::min<int64_t>((m + 7) / 8, (int64_t)c->sm_count * 16);
+            if (dim % 4 == 0)
+                snapshot_gather_kernel<<<grid, 256, 0, c->stream>>>(reinterpret_cast<const float4 *>(ix->X.p), (int)(dim / 4), scan.p, n, j0, m,
+                                                                   reinterpret_cast<float4 *>(stg.d[b].p));
+            else
+                snapshot_gather_kernel<<<grid, 256, 0, c->stream>>>(ix->X.p, (int)dim, scan.p, n, j0, m, stg.d[b].p);
+            c->launches++;
+            cudaError_t e = cudaGetLastError();
+            if (e == cudaSuccess) e = cudaEventRecord(stg.gathered[b], c->stream);
+            if (e == cudaSuccess) e = cudaStreamWaitEvent(c->copy_stream, stg.gathered[b], 0);
+            if (e == cudaSuccess) e = cudaMemcpyAsync(stg.h[b], stg.d[b].p, (size_t)(4 * m * dim), cudaMemcpyDeviceToHost, c->copy_stream);
+            if (e == cudaSuccess) e = cudaEventRecord(stg.copied[b], c->copy_stream);
+            return e;
+        };
+        cudaError_t e = cudaSuccess;
+        for (int64_t k = 0; k < std::min<int64_t>(2, chunks) && e == cudaSuccess; k++) e = enqueue(k);
+        for (int64_t k = 0; k < chunks && e == cudaSuccess && st == GORSE_B200_OK; k++) {
+            const int b = (int)(k & 1);
+            e = cudaEventSynchronize(stg.copied[b]);
+            if (e == cudaSuccess) st = w.direct(stg.h[b], 4 * std::min(R, live - k * R) * dim);
+            if (e == cudaSuccess && st == GORSE_B200_OK && k + 2 < chunks) e = enqueue(k + 2);
+        }
+        cudaStreamSynchronize(c->copy_stream);
+        scan.free();
+        if (e != cudaSuccess) { set_error("snapshot save: %s", cudaGetErrorString(e)); return GORSE_B200_ERR_CUDA; }
+        if (st) return st;
+    }
+    if (new_slot_out)
+        for (int64_t s = 0, j = 0; s < n; s++) new_slot_out[s] = db->dead[(size_t)s] ? -1 : j++;
+    if (bytes_out) *bytes_out = w.pos;
+    return GORSE_B200_OK;
+}
+
+// the header's fields, each count against the others and against int64 overflow of its section
+int32_t check_header(const Header &h)
+{
+    SNAP_CHECK(memcmp(h.magic, MAGIC, sizeof(MAGIC)) == 0, "magic", 0, "not a gorse_b200 collection stream");
+    SNAP_CHECK(h.version == VERSION, "version", 8, "unknown version");
+    SNAP_CHECK(h.dim >= 0 && h.dim <= 16384, "dim", 12, "outside [0, 16384]");
+    SNAP_CHECK(h.distance == GORSE_B200_DISTANCE_EUCLIDEAN || h.distance == GORSE_B200_DISTANCE_DOT || h.distance == GORSE_B200_DISTANCE_COSINE,
+               "distance", 16, "unknown distance");
+    SNAP_CHECK(h.dim > 0 || h.distance == GORSE_B200_DISTANCE_DOT, "distance", 16, "a sparse collection is Dot");
+    SNAP_CHECK(h.reserved == 0, "reserved", 20, "not 0");
+    // every section's byte count, and their sum, fit in an int64 below 2^62
+    constexpr int64_t LIM = 1ll << 62;
+    SNAP_CHECK(h.n >= 0 && h.n < LIM / 32, "n", 24, "negative or too large");
+    SNAP_CHECK(h.dim > 0 || h.n < (1ll << 31) - 1, "n", 24, "more than 2^31 - 1 sparse vectors");
+    SNAP_CHECK(h.dim > 0 || h.n < LIM / 32, "n", 24, "too large");
+    SNAP_CHECK(h.dim == 0 || h.n <= LIM / 8 / h.dim, "n", 24, "n * dim overflows");
+    SNAP_CHECK(h.nnz >= 0 && h.nnz < LIM / 16, "nnz", 32, "negative or too large");
+    SNAP_CHECK(h.dim == 0 || h.nnz == 0, "nnz", 32, "not 0 in a dense collection");
+    SNAP_CHECK(h.n_cats >= 0 && h.n_cats < LIM / 16, "category count", 40, "negative or too large");
+    return GORSE_B200_OK;
+}
+
+int32_t load(gorse_b200_ctx *ctx, gorse_b200_read_fn read, void *user, gorse_b200_vecdb **out, int64_t *bytes_out)
+{
+    Reader r{read, user};
+    Header h;
+    GB_TRY(r.get(&h, sizeof(h), "header"));
+    GB_TRY(check_header(h));
+    const int64_t n = h.n, dim = h.dim;
+    std::vector<uint8_t> hidden;
+    std::vector<int64_t> ts, cat_off;
+    std::vector<int32_t> cats;
+    int64_t at = r.pos;
+    GB_TRY(r.array(hidden, n, "hidden"));
+    for (int64_t i = 0; i < n; i++) SNAP_CHECK(hidden[(size_t)i] <= 1, "hidden", at + i, "neither 0 nor 1");
+    GB_TRY(r.array(ts, n, "timestamp_ms"));
+    at = r.pos;
+    GB_TRY(r.array(cat_off, n + 1, "cat_off"));
+    GB_TRY(check_offsets(cat_off, h.n_cats, "cat_off", at));
+    GB_TRY(r.array(cats, h.n_cats, "cats"));
+    std::vector<int64_t> sp_off;
+    std::vector<uint32_t> sp_ind;
+    std::vector<float> sp_val;
+    uint32_t n_features = 0;
+    if (dim == 0) {
+        at = r.pos;
+        GB_TRY(r.array(sp_off, n + 1, "off"));
+        GB_TRY(check_offsets(sp_off, h.nnz, "off", at));
+        at = r.pos;
+        GB_TRY(r.array(sp_ind, h.nnz, "ind"));
+        for (int64_t i = 0; i < n; i++)
+            for (int64_t t = sp_off[(size_t)i]; t < sp_off[(size_t)i + 1]; t++) {
+                SNAP_CHECK(t == sp_off[(size_t)i] || sp_ind[(size_t)t] > sp_ind[(size_t)t - 1], "ind", at + 4 * t,
+                           "indices of a vector not strictly ascending");
+                SNAP_CHECK(sp_ind[(size_t)t] < 0x7fffffffu, "ind", at + 4 * t, "index >= 0x7fffffff");
+                n_features = std::max(n_features, sp_ind[(size_t)t] + 1);
+            }
+        at = r.pos;
+        GB_TRY(r.array(sp_val, h.nnz, "val"));
+        for (int64_t t = 0; t < h.nnz; t++) SNAP_CHECK(!std::isnan(sp_val[(size_t)t]), "val", at + 4 * t, "NaN value");
+    }
+    std::vector<uint8_t> dead((size_t)n, 0);
+    // the handle is this call's until it returns: nobody else can take its locks
+    gorse_b200_vecdb *db = nullptr;
+    GB_TRY(gorse_b200_vecdb_create(ctx, h.dim, h.distance, &db));
+    int32_t st = GORSE_B200_OK;
+    {
+        ScopedDevice sd(ctx->device);
+        if (dim == 0) {
+            gorse_b200_sparse_index *sx = db->sparse;
+            sx->h_off.swap(sp_off); sx->h_ind.swap(sp_ind); sx->h_val.swap(sp_val);
+            sx->n_features = n_features;
+            sx->dirty = true;
+            st = sparse_sync_device(sx);
+        } else if (n > 0) {
+            // chunk k = rows [k R, k R + R): read into h[k & 1] while chunk k - 1 is copied into X on the copy stream
+            gorse_b200_index *ix = db->dense;
+            Staging stg;
+            const int64_t cap = std::min(STAGE_BYTES, std::max(MIN_STAGE_BYTES, 4 * n * dim));
+            st = index_reserve(ix, n);
+            if (st == GORSE_B200_OK) st = stg.alloc(ctx, cap, 2, false);
+            const int64_t R = cap / (4 * dim), chunks = st ? 0 : (n + R - 1) / R;
+            cudaError_t e = cudaSuccess;
+            for (int64_t k = 0; k < chunks && e == cudaSuccess && st == GORSE_B200_OK; k++) {
+                const int b = (int)(k & 1);
+                const int64_t j0 = k * R, bytes = 4 * std::min(R, n - j0) * dim;
+                if (k >= 2) e = cudaEventSynchronize(stg.copied[b]);
+                if (e == cudaSuccess) st = r.get(stg.h[b], bytes, "values");
+                if (e == cudaSuccess && st == GORSE_B200_OK)
+                    e = cudaMemcpyAsync(ix->X.p + j0 * dim, stg.h[b], (size_t)bytes, cudaMemcpyHostToDevice, ctx->copy_stream);
+                if (e == cudaSuccess && st == GORSE_B200_OK) e = cudaEventRecord(stg.copied[b], ctx->copy_stream);
+            }
+            if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->copy_stream);
+            if (e != cudaSuccess && st == GORSE_B200_OK) {
+                set_error("snapshot load: %s", cudaGetErrorString(e));
+                st = e == cudaErrorMemoryAllocation ? GORSE_B200_ERR_OOM : GORSE_B200_ERR_CUDA;
+            }
+            ix->n = n;
+            ix->mma_ready = false;   // the bf16 mirror and the norms are built lazily, as after an add
+        }
+    }
+    if (st) {
+        gorse_b200_vecdb_destroy(db);
+        return st;
+    }
+    db->hidden.swap(hidden);
+    db->dead.swap(dead);
+    db->ts.swap(ts);
+    db->cat_off.swap(cat_off);
+    db->cats.swap(cats);
+    db->live = n;
+    db->meta_dirty = true;
+    *out = db;
+    if (bytes_out) *bytes_out = r.pos;
+    return GORSE_B200_OK;
+}
+
+}  // namespace
+}  // namespace gb
+
+using namespace gb;
+
+extern "C" {
+
+int32_t gorse_b200_vecdb_save(gorse_b200_vecdb *db, gorse_b200_write_fn write, void *user, int64_t *new_slot_out, int64_t *bytes_out)
+{
+    GB_CHECK_ARG(db != nullptr && write != nullptr, "NULL collection or write callback");
+    try {
+        return save(db, write, user, new_slot_out, bytes_out);
+    } catch (const std::bad_alloc &) {
+        set_error("snapshot save: host allocation failed");
+        return GORSE_B200_ERR_OOM;
+    }
+}
+
+int32_t gorse_b200_vecdb_load(gorse_b200_ctx *ctx, gorse_b200_read_fn read, void *user, gorse_b200_vecdb **out, int64_t *bytes_out)
+{
+    GB_CHECK_ARG(ctx != nullptr && read != nullptr && out != nullptr, "NULL context, read callback or out");
+    *out = nullptr;
+    try {
+        return load(ctx, read, user, out, bytes_out);
+    } catch (const std::bad_alloc &) {
+        set_error("snapshot load: host allocation failed");
+        return GORSE_B200_ERR_OOM;
+    }
+}
+
+}  // extern "C"

@@ -1071,6 +1071,8 @@ int32_t sparse_append(gorse_b200_sparse_index *ix, const SparseRows &rows)
     return done(GORSE_B200_OK);
 }
 
+int32_t sparse_sync_device(gorse_b200_sparse_index *ix) { return sync_device(ix); }
+
 size_t sparse_bytes(const gorse_b200_sparse_index *ix)
 {
     return ix->off.bytes() + ix->foff.bytes() + ix->ind.bytes() + ix->val.bytes() + ix->frow.bytes() + ix->fval.bytes() + ix->tl_dot.bytes() +

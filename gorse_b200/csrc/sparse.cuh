@@ -47,6 +47,9 @@ int32_t sparse_search_rows(gorse_b200_sparse_index *ix, const int64_t *d_rows, i
 int32_t sparse_compact(gorse_b200_sparse_index *ix, const int64_t *scan, int64_t live);
 // device bytes held by the index
 size_t sparse_bytes(const gorse_b200_sparse_index *ix);
+// the device layouts from the host CSR, as the next search would build them: the CSR is uploaded and the CSC built on the
+// device, and the index ends clean (gorse_b200_vecdb_load).  The caller holds ix->mu and the device.
+int32_t sparse_sync_device(gorse_b200_sparse_index *ix);
 
 // vectors built on the device by sparse_idf_rows and not yet part of any index: the CSR of the non-empty rows (off on the host,
 // m + 1 entries from 0; ind / val on the device), row_off[n + 1] = each input row's first entry (an empty row's equals the next

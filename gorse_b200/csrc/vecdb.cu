@@ -95,6 +95,31 @@ static int32_t sync_meta(gorse_b200_vecdb *db)
     return GORSE_B200_OK;
 }
 
+int32_t vecdb_live_scan(gorse_b200_vecdb *db, DevBuf<int64_t> &scan, int64_t *new_slot)
+{
+    gorse_b200_ctx *c = db->ctx;
+    const int64_t n = (int64_t)db->ts.size();
+    DevBuf<uint8_t> d_dead, tmp;
+    auto done = [&](int32_t st) { cudaStreamSynchronize(c->stream); d_dead.free(); tmp.free(); if (st) scan.free(); return st; };
+    int32_t st;
+    if ((st = d_dead.alloc((size_t)n)) || (st = scan.alloc((size_t)n + 1))) return done(st);
+    size_t tmp_bytes = 0;
+    cudaError_t e = n ? cudaMemcpyAsync(d_dead.p, db->dead.data(), (size_t)n, cudaMemcpyHostToDevice, c->stream) : cudaSuccess;
+    if (e == cudaSuccess) {
+        vecdb_live_kernel<<<div_up(n + 1, 256), 256, 0, c->stream>>>(d_dead.p, n, scan.p);
+        c->launches++;
+        e = cudaGetLastError();
+    }
+    if (e == cudaSuccess) e = cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, scan.p, n + 1, c->stream);
+    if (e != cudaSuccess) { set_error("live scan: %s", cudaGetErrorString(e)); return done(GORSE_B200_ERR_CUDA); }
+    if ((st = tmp.alloc(tmp_bytes))) return done(st);
+    e = cub::DeviceScan::ExclusiveSum(tmp.p, tmp_bytes, scan.p, n + 1, c->stream);
+    if (e == cudaSuccess && new_slot) e = cudaMemcpyAsync(new_slot, scan.p, sizeof(int64_t) * ((size_t)n + 1), cudaMemcpyDeviceToHost, c->stream);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
+    if (e != cudaSuccess) { set_error("live scan: %s", cudaGetErrorString(e)); return done(GORSE_B200_ERR_CUDA); }
+    return done(GORSE_B200_OK);
+}
+
 int32_t vecdb_allow(gorse_b200_vecdb *db, const int32_t *categories, int32_t n_categories)
 {
     gorse_b200_ctx *c = db->ctx;
@@ -339,26 +364,11 @@ int32_t gorse_b200_vecdb_compact(gorse_b200_vecdb *db, int64_t *new_slot_out, in
     }
     gorse_b200_ctx *c = db->ctx;
     ScopedDevice sd(c->device);
-    DevBuf<uint8_t> d_dead, tmp;
     DevBuf<int64_t> scan;
-    auto done = [&](int32_t st) { cudaStreamSynchronize(c->stream); d_dead.free(); tmp.free(); scan.free(); return st; };
+    auto done = [&](int32_t st) { cudaStreamSynchronize(c->stream); scan.free(); return st; };
     int32_t st;
-    if ((st = d_dead.alloc((size_t)n)) || (st = scan.alloc((size_t)n + 1))) return done(st);
-    size_t tmp_bytes = 0;
-    cudaError_t e = cudaMemcpyAsync(d_dead.p, db->dead.data(), (size_t)n, cudaMemcpyHostToDevice, c->stream);
-    if (e == cudaSuccess) {
-        vecdb_live_kernel<<<div_up(n + 1, 256), 256, 0, c->stream>>>(d_dead.p, n, scan.p);
-        c->launches++;
-        e = cudaGetLastError();
-    }
-    if (e == cudaSuccess) e = cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, scan.p, n + 1, c->stream);
-    if (e != cudaSuccess) { set_error("compact: %s", cudaGetErrorString(e)); return done(GORSE_B200_ERR_CUDA); }
-    if ((st = tmp.alloc(tmp_bytes))) return done(st);
     std::vector<int64_t> new_slot((size_t)n + 1);
-    e = cub::DeviceScan::ExclusiveSum(tmp.p, tmp_bytes, scan.p, n + 1, c->stream);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(new_slot.data(), scan.p, sizeof(int64_t) * ((size_t)n + 1), cudaMemcpyDeviceToHost, c->stream);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
-    if (e != cudaSuccess) { set_error("compact: %s", cudaGetErrorString(e)); return done(GORSE_B200_ERR_CUDA); }
+    if ((st = vecdb_live_scan(db, scan, new_slot.data()))) return done(st);
     // the compacted host metadata
     std::vector<uint8_t> hidden((size_t)live), dead((size_t)live, 0);
     std::vector<int64_t> ts((size_t)live), cat_off((size_t)live + 1, 0);

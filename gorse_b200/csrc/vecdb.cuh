@@ -73,4 +73,8 @@ struct gorse_b200_vecdb {
 namespace gb {
 // allow mask d_allow[slot] of one query filter (live, not hidden, every wanted category); the caller holds db->mu
 int32_t vecdb_allow(gorse_b200_vecdb *db, const int32_t *categories, int32_t n_categories);
+// the renumbering of compaction and snapshots: scan[slots + 1] (device, allocated here) = the exclusive sum of the live flags,
+// so slot s is live iff scan[s + 1] != scan[s] and then moves to scan[s]; new_slot[slots + 1] (host, may be nullptr) receives
+// a copy.  Ends with the stream synchronised; on an error scan holds no memory.  The caller holds db->mu and the device.
+int32_t vecdb_live_scan(gorse_b200_vecdb *db, DevBuf<int64_t> &scan, int64_t *new_slot);
 }  // namespace gb

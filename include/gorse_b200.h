@@ -40,7 +40,8 @@ typedef enum {
     GORSE_B200_ERR_OOM = -4,      /* device or host allocation failed */
     GORSE_B200_ERR_RANGE = -5,    /* index out of range (ann.Bruteforce.SearchIndex error, bruteforce.go:41-43) */
     GORSE_B200_ERR_STATE = -6,    /* call not valid in the object's current state */
-    GORSE_B200_ERR_UNSUPPORTED = -7
+    GORSE_B200_ERR_UNSUPPORTED = -7,
+    GORSE_B200_ERR_IO = -8        /* a caller's read or write callback reported a failure */
 } gorse_b200_status;
 
 typedef struct gorse_b200_ctx gorse_b200_ctx;     /* one GPU, one stream, optional NCCL rank */
@@ -426,6 +427,56 @@ int32_t gorse_b200_vecdb_delete_before(gorse_b200_vecdb *db, int64_t timestamp_m
  * any error the collection is unchanged.  Slots held by the caller (id maps, context and exclusion lists, per-slot
  * feedback rows and masks) must be renamed before they are passed again.  NULL db: GORSE_B200_ERR_ARG. */
 int32_t gorse_b200_vecdb_compact(gorse_b200_vecdb *db, int64_t *new_slot_out, int64_t *bytes_out);
+/* Snapshots: a collection written as a byte stream and rebuilt from one on any context (another device, another process), so
+ * that a restarted master, a worker and a server hold the collections the master built (the reference's default backend keeps
+ * each collection on disk and reopens it in Init, xvec.go:60-123).
+ *
+ * Stream format, version 1.  Every number is little-endian; there is no padding between fields or sections.
+ *   header, 48 bytes:
+ *     0  u8[8]  magic "GB200VDB"
+ *     8  u32    version (1)
+ *     12 i32    dim (0 = sparse, else 1 .. 16384)
+ *     16 i32    distance (gorse_b200_distance; a sparse collection is Dot)
+ *     20 u32    reserved, 0
+ *     24 i64    n: the live vectors
+ *     32 i64    nnz: the sparse entries (0 for a dense collection)
+ *     40 i64    c: the category entries
+ *   then the live vectors in slot order, deleted slots left out, as sections:
+ *     hidden        u8[n], 0 or 1
+ *     timestamp_ms  i64[n]
+ *     cat_off       i64[n + 1], from 0, never decreasing, cat_off[n] = c
+ *     cats          i32[c]: the caller's int32 category ids
+ *     dense:  values  f32[n * dim], the stored fp32 rows bit for bit
+ *     sparse: off     i64[n + 1], from 0, never decreasing, off[n] = nnz
+ *             ind     u32[nnz], strictly ascending within a vector, each below 0x7fffffff
+ *             val     f32[nnz], no NaN
+ *   Vector ids and category names belong to the caller (the Go shim writes them in its own header before the stream).  The
+ *   stream ends after its last section; a reader may keep reading the source for its own data.
+ *
+ * gorse_b200_vecdb_save: the stream of db through write(user, buf, n), which returns 0 once all n bytes are written.  The
+ *   collection does not change; the call holds its lock, as compaction does.  new_slot_out[slots] (may be NULL): the
+ *   position of each slot's vector in the stream, -1 for a deleted slot -- exactly the map gorse_b200_vecdb_compact would
+ *   return.  *bytes_out (may be NULL): the stream's length.  Dense rows are gathered on the device in chunks and downloaded
+ *   through two pinned staging buffers of at most 64 MB while the callback writes the previous chunk; no host copy of the
+ *   collection is made.  A write failure: GORSE_B200_ERR_IO, the collection untouched.
+ * gorse_b200_vecdb_load: a new collection on ctx from read(user, buf, n), which returns the bytes read (1 .. n), 0 at the
+ *   end of the source or < 0 on a failure; the call reads exactly the stream's bytes.  Vector i of the stream is in slot i,
+ *   and every entry (query, query_excluding, item_to_item, user_to_user, session_recommend, the gorse_b200_recommend stages,
+ *   get / get_sparse, count) answers exactly as the saved collection answers after gorse_b200_vecdb_compact: the same slots
+ *   through new_slot_out, the same score bits, the same tie order.  Later adds, deletes and compactions act on it as on the
+ *   original.  Dense rows go from the callback into the device rows through two pinned staging buffers of at most 64 MB
+ *   (the device rows are reserved once from the header); the bf16 mirror and the norms are built lazily, as after an add.
+ *   Sparse rows go into the index's CSR and the device CSC is built at once, so the first query starts without a rebuild.
+ *   *bytes_out (may be NULL): the bytes read.  Every field is checked as gorse_b200_vecdb_add checks its arguments (dense
+ *   values are taken as they are, as there): a wrong magic or version, an illegal dim / distance pair, a count that
+ *   overflows or disagrees with its section, a bad offset, hidden flag, sparse index or NaN sparse value, or a stream that
+ *   ends early is GORSE_B200_ERR_ARG, and gorse_b200_last_error names the field and its byte offset; a read failure is
+ *   GORSE_B200_ERR_IO.  On any error *out is NULL and nothing is left allocated.
+ * NULL db / ctx / callback / out: GORSE_B200_ERR_ARG before anything else. */
+typedef int32_t (*gorse_b200_write_fn)(void *user, const void *buf, int64_t n);
+typedef int64_t (*gorse_b200_read_fn)(void *user, void *buf, int64_t n);
+int32_t gorse_b200_vecdb_save(gorse_b200_vecdb *db, gorse_b200_write_fn write, void *user, int64_t *new_slot_out, int64_t *bytes_out);
+int32_t gorse_b200_vecdb_load(gorse_b200_ctx *ctx, gorse_b200_read_fn read, void *user, gorse_b200_vecdb **out, int64_t *bytes_out);
 /* QueryVectors (xvec.go:373-449) for nq query vectors sharing one category filter: candidates are live, not hidden and
  * carry ALL of categories[n_categories] (CONTAIN_ALL, :381-389).  Results per query: slots_out / scores_out [nq x topk],
  * best first, count_out[nq]; entries past count_out[q] in a row are not part of the answer and are left unspecified; score = dot (Dot) or the NEGATED distance (Euclidean, Cosine) -- higher is more similar
