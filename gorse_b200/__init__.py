@@ -14,12 +14,19 @@ from ._lib import (DISTANCE_COSINE, DISTANCE_DOT, DISTANCE_EUCLIDEAN, FM_ADAM, F
                    METRIC_NEG_DOT, ORDER_HOGWILD, ORDER_SEQUENTIAL,
                    SCATTER_ATOMIC, SCATTER_STORE, check, lib, ptr)
 
-__all__ = ["Context", "CFModel", "BruteforceIndex", "GorseB200Error", "csr_from_lists", "device_count"]
+__all__ = ["Context", "CFModel", "BruteforceIndex", "GorseB200Error", "csr_from_lists", "device_bytes", "device_count"]
 
 
 def device_count():
     n = C.c_int32(0)
     check(lib.gorse_b200_device_count(C.byref(n)))
+    return n.value
+
+
+def device_bytes():
+    """Device bytes held by the library's buffers in this process, over every context and handle."""
+    n = C.c_int64(0)
+    check(lib.gorse_b200_device_bytes(C.byref(n)))
     return n.value
 
 

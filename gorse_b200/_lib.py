@@ -43,6 +43,7 @@ PROTOTYPES = {
     "gorse_b200_ctx_timer_begin": (C.c_int32, [VP]),
     "gorse_b200_ctx_timer_end": (C.c_int32, [VP, C.POINTER(C.c_float)]),
     "gorse_b200_ctx_launch_count": (C.c_int32, [VP, C.POINTER(C.c_int64)]),
+    "gorse_b200_device_bytes": (C.c_int32, [C.POINTER(C.c_int64)]),
     "gorse_b200_ctx_flush_l2": (C.c_int32, [VP]),
     "gorse_b200_ctx_barrier": (C.c_int32, [VP]),
     "gorse_b200_host_alloc": (C.c_int32, [C.c_size_t, PVP]),

@@ -127,15 +127,5 @@ __device__ int select_first_n(int64_t range, int distinct, int n, int p2, IdAt i
 }
 #endif  // __CUDACC__
 
-// grow b to n entries; a new allocation is zeroed
-template <typename T>
-int32_t grow_zeroed(DevBuf<T> &b, size_t n, cudaStream_t s)
-{
-    if (b.n >= n) return GORSE_B200_OK;
-    GB_TRY(b.alloc(n));
-    GB_CUDA(cudaMemsetAsync(b.p, 0, sizeof(T) * n, s));
-    return GORSE_B200_OK;
-}
-
 }  // namespace agg
 }  // namespace gb

@@ -776,7 +776,7 @@ int32_t gb::als_epoch_tables(gorse_b200_cf *cf, float *P_own, float *Q, float re
     GB_TRY(prepare_als(cf));
     // scratch kept in the model: a cudaMalloc/cudaFree pair per epoch costs more than some of the kernels of a C3 epoch
     const size_t n_pred = (size_t)std::max<int64_t>(1, std::max(cf->n_feedback, cf->n_item_feedback));
-    if (cf->als_pred.n < n_pred) { cf->als_pred.free(); GB_TRY(cf->als_pred.alloc(n_pred)); }
+    GB_TRY(cf->als_pred.grow(n_pred));
     DevBuf<float> &pred = cf->als_pred;
     int32_t st;
     auto done = [&](int32_t s) {

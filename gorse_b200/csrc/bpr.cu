@@ -977,7 +977,6 @@ int32_t gorse_b200_bpr_apply_triples(gorse_b200_cf *cf, const int32_t *uij, int6
     GB_TRY(d_uij.alloc((size_t)3 * n));
     auto done = [&](int32_t s) {
         cudaStreamSynchronize(c->stream);
-        d_uij.free();
         return s;
     };
     auto check = [&]() -> int32_t {
@@ -1053,7 +1052,6 @@ int32_t gorse_b200_bpr_sample_triples(gorse_b200_cf *cf, uint64_t seed, int64_t 
     cudaError_t e = cudaGetLastError();
     if (e == cudaSuccess) e = cudaMemcpyAsync(uij_out, d.p, sizeof(int32_t) * 3 * n, cudaMemcpyDeviceToHost, c->stream);
     if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
-    d.free();
     if (e != cudaSuccess) { set_error("bpr_sample: %s", cudaGetErrorString(e)); return GORSE_B200_ERR_CUDA; }
     return GORSE_B200_OK;
 }

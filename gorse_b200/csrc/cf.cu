@@ -158,7 +158,6 @@ int32_t gorse_b200_cf_create(gorse_b200_ctx *ctx, int32_t n_users, int32_t n_ite
         ncclResult_t r = e == cudaSuccess ? nc->AllReduce(dcnt.p, dcnt.p, 3, ncclInt64, ncclSum, ctx->comm, ctx->stream) : ncclSuccess;
         if (e == cudaSuccess && r == ncclSuccess) e = cudaMemcpyAsync(h, dcnt.p, sizeof(h), cudaMemcpyDeviceToHost, ctx->stream);
         if (e == cudaSuccess && r == ncclSuccess) e = cudaStreamSynchronize(ctx->stream);
-        dcnt.free();
         if (r != ncclSuccess) { set_error("cf_create: ncclAllReduce -> %s", nc->GetErrorString(r)); return GORSE_B200_ERR_NCCL; }
         if (e != cudaSuccess) { set_error("cf_create: %s", cudaGetErrorString(e)); return GORSE_B200_ERR_CUDA; }
         if (vst != GORSE_B200_OK) { set_error("%s", keep.c_str()); return vst; }
@@ -286,17 +285,6 @@ int32_t gorse_b200_cf_destroy(gorse_b200_cf *cf)
     if (!cf) return GORSE_B200_OK;
     ScopedDevice sd(cf->ctx->device);
     cudaStreamSynchronize(cf->ctx->stream);
-    cf->P.free(); cf->Q.free(); cf->Q0.free(); cf->item_rate.free(); cf->xchg.free(); cf->P_all.free();
-    cf->user_off.free(); cf->item_off.free();
-    cf->user_items.free(); cf->item_users.free(); cf->active.free(); cf->user_meta.free(); cf->bpr_barrier.free();
-    cf->bpr_delta.free(); cf->bpr_rows.free();
-    cf->gram.free();
-    for (int a = 0; a < 2; a++) {
-        for (int b = 0; b < 7; b++) cf->als_rows[a][b].free();
-        cf->als_chunk_len[a].free(); cf->als_row_chunk0[a].free(); cf->als_chunk_begin[a].free();
-        cf->als_s_rows[a].free(); cf->als_s_len[a].free(); cf->als_s_begin[a].free();
-    }
-    cf->als_partial.free(); cf->als_pred.free();
     delete cf;
     return GORSE_B200_OK;
 }
@@ -354,20 +342,14 @@ int32_t gorse_b200_cf_predict(gorse_b200_cf *cf, const int32_t *users, const int
     gorse_b200_ctx *c = cf->ctx;
     DevBuf<int32_t> du, di;
     DevBuf<float> dout;
-    int32_t st;
-    if ((st = du.alloc(n)) || (st = di.alloc(n)) || (st = dout.alloc(n))) {
-        du.free(); di.free(); dout.free();
-        return st;
-    }
-    auto done = [&](int32_t s) {
-        du.free(); di.free(); dout.free();
-        return s;
-    };
+    GB_TRY(du.alloc(n));
+    GB_TRY(di.alloc(n));
+    GB_TRY(dout.alloc(n));
     cudaError_t e;
     if ((e = cudaMemcpyAsync(du.p, users, n * sizeof(int32_t), cudaMemcpyHostToDevice, c->stream)) != cudaSuccess ||
         (e = cudaMemcpyAsync(di.p, items, n * sizeof(int32_t), cudaMemcpyHostToDevice, c->stream)) != cudaSuccess) {
         set_error("predict upload: %s", cudaGetErrorString(e));
-        return done(GORSE_B200_ERR_CUDA);
+        return GORSE_B200_ERR_CUDA;
     }
     if (cf->d % 16 == 0) {
         int blocks = std::min<int64_t>(div_up(n * 4, 256), (int64_t)c->sm_count * 16);
@@ -381,9 +363,9 @@ int32_t gorse_b200_cf_predict(gorse_b200_cf *cf, const int32_t *users, const int
         (e = cudaMemcpyAsync(out, dout.p, n * sizeof(float), cudaMemcpyDeviceToHost, c->stream)) != cudaSuccess ||
         (e = cudaStreamSynchronize(c->stream)) != cudaSuccess) {
         set_error("predict: %s", cudaGetErrorString(e));
-        return done(GORSE_B200_ERR_CUDA);
+        return GORSE_B200_ERR_CUDA;
     }
-    return done(GORSE_B200_OK);
+    return GORSE_B200_OK;
 }
 
 }  // extern "C"

@@ -4,6 +4,8 @@
 #include <cuda_runtime.h>
 #include <nccl.h>
 
+#include <algorithm>
+#include <atomic>
 #include <cstdarg>
 #include <cstdint>
 #include <cstdio>
@@ -11,6 +13,8 @@
 #include <mutex>
 #include <new>
 #include <string>
+#include <type_traits>
+#include <utility>
 #include <vector>
 
 #include "../../include/gorse_b200.h"
@@ -80,48 +84,82 @@ const NcclApi *nccl();  // nullptr (and last_error set) when libnccl cannot be l
 
 }  // namespace gb
 
-struct gorse_b200_ctx {
-    int device = 0;
-    int sm_count = 132;
-    int rank = 0, world = 1;
-    cudaStream_t stream = nullptr;
-    cudaStream_t copy_stream = nullptr;   // result downloads that overlap the next chunk's kernels (topk)
-    cudaEvent_t copy_ev = nullptr;
-    cudaEvent_t ev0 = nullptr, ev1 = nullptr;
-    ncclComm_t comm = nullptr;
-    int64_t launches = 0;
-    void *flush_buf = nullptr;
-    size_t flush_bytes = 0;
-    int *nccl_token = nullptr;
-    void *rec_work = nullptr;   // gorse_b200_recommend's grow-only device buffers (recommend.cu)
-};
-
-namespace gb {
-void recommend_work_free(gorse_b200_ctx *ctx);   // frees ctx->rec_work (recommend.cu)
-}  // namespace gb
-
 namespace gb {
 
-// RAII-less device buffer (explicit free; objects live behind opaque handles)
+// device bytes held by every DevBuf of the process (gorse_b200_device_bytes)
+inline std::atomic<int64_t> g_device_bytes{0};
+
+// owning device buffer: the destructor frees; moves leave the source empty, copies do not compile
 template <typename T>
 struct DevBuf {
     T *p = nullptr;
     size_t n = 0;
+    DevBuf() = default;
+    DevBuf(const DevBuf &) = delete;
+    DevBuf &operator=(const DevBuf &) = delete;
+    DevBuf(DevBuf &&o) noexcept : p(o.p), n(o.n)
+    {
+        o.p = nullptr;
+        o.n = 0;
+    }
+    DevBuf &operator=(DevBuf &&o) noexcept
+    {
+        if (this != &o) {
+            free();
+            std::swap(p, o.p);
+            std::swap(n, o.n);
+        }
+        return *this;
+    }
+    ~DevBuf() { free(); }
     int32_t alloc(size_t count)
     {
         free();
         if (count == 0) return GORSE_B200_OK;
         GB_CUDA(cudaMalloc((void **)&p, count * sizeof(T)));
         n = count;   // only a successful allocation has a size
+        g_device_bytes += (int64_t)bytes();
         return GORSE_B200_OK;
     }
     void free()
     {
-        if (p) cudaFree(p);
+        if (p) {
+            cudaFree(p);
+            g_device_bytes -= (int64_t)bytes();
+        }
         p = nullptr;
         n = 0;
     }
+    // grow-only: reallocates (contents lost) when count exceeds the size
+    int32_t grow(size_t count) { return n >= count ? GORSE_B200_OK : alloc(count); }
+    // as grow; a new allocation is zeroed on stream s
+    int32_t grow_zeroed(size_t count, cudaStream_t s)
+    {
+        if (n >= count) return GORSE_B200_OK;
+        GB_TRY(alloc(count));
+        GB_CUDA(cudaMemsetAsync(p, 0, sizeof(T) * count, s));
+        return GORSE_B200_OK;
+    }
+    // grows to max(count, 1) and copies h[0, count) on stream s
+    int32_t upload(const T *h, size_t count, cudaStream_t s)
+    {
+        GB_TRY(grow(std::max<size_t>(count, 1)));
+        if (count) GB_CUDA(cudaMemcpyAsync(p, h, count * sizeof(T), cudaMemcpyHostToDevice, s));
+        return GORSE_B200_OK;
+    }
     size_t bytes() const { return n * sizeof(T); }
+};
+static_assert(!std::is_copy_constructible<DevBuf<int>>::value && !std::is_copy_assignable<DevBuf<int>>::value, "DevBuf owns its memory");
+static_assert(std::is_nothrow_move_constructible<DevBuf<int>>::value, "std::vector<DevBuf> moves on growth");
+
+// synchronises its streams when destroyed: declare it after the buffers the enqueued work reads, so it is destroyed first
+struct StreamSync {
+    cudaStream_t a, b = nullptr;
+    ~StreamSync()
+    {
+        cudaStreamSynchronize(a);
+        if (b) cudaStreamSynchronize(b);
+    }
 };
 
 struct ScopedDevice {
@@ -137,6 +175,30 @@ struct ScopedDevice {
         if (prev >= 0) cudaSetDevice(prev);
     }
 };
+
+namespace rec {
+struct Work;
+}  // namespace rec
+
+}  // namespace gb
+
+struct gorse_b200_ctx {
+    int device = 0;
+    int sm_count = 132;
+    int rank = 0, world = 1;
+    cudaStream_t stream = nullptr;
+    cudaStream_t copy_stream = nullptr;   // result downloads that overlap the next chunk's kernels (topk)
+    cudaEvent_t copy_ev = nullptr;
+    cudaEvent_t ev0 = nullptr, ev1 = nullptr;
+    ncclComm_t comm = nullptr;
+    int64_t launches = 0;
+    gb::DevBuf<float4> flush_buf;
+    gb::DevBuf<int> nccl_token;
+    gb::rec::Work *rec_work = nullptr;   // gorse_b200_recommend's grow-only device buffers (recommend.cu)
+};
+
+namespace gb {
+void recommend_work_free(gorse_b200_ctx *ctx);   // deletes ctx->rec_work (recommend.cu)
 
 inline int div_up(int64_t a, int64_t b) { return (int)((a + b - 1) / b); }
 

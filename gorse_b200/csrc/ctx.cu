@@ -135,8 +135,8 @@ int32_t gorse_b200_ctx_create_dist(int32_t device, int32_t rank, int32_t world, 
         ncclUniqueId id;
         memcpy(&id, nccl_id, sizeof(id));
         GB_NCCL(nc, CommInitRank(&c->comm, world, id, rank));
-        GB_CUDA(cudaMalloc((void **)&c->nccl_token, sizeof(int)));
-        GB_CUDA(cudaMemsetAsync(c->nccl_token, 0, sizeof(int), c->stream));
+        GB_TRY(c->nccl_token.alloc(1));
+        GB_CUDA(cudaMemsetAsync(c->nccl_token.p, 0, sizeof(int), c->stream));
     }
     return GORSE_B200_OK;
 }
@@ -147,8 +147,6 @@ int32_t gorse_b200_ctx_destroy(gorse_b200_ctx *ctx)
     gb::ScopedDevice sd(ctx->device);
     cudaStreamSynchronize(ctx->stream);
     if (ctx->comm && gb::nccl()) gb::nccl()->CommDestroy(ctx->comm);
-    if (ctx->nccl_token) cudaFree(ctx->nccl_token);
-    if (ctx->flush_buf) cudaFree(ctx->flush_buf);
     gb::recommend_work_free(ctx);
     cudaEventDestroy(ctx->ev0);
     cudaEventDestroy(ctx->ev1);
@@ -200,16 +198,19 @@ int32_t gorse_b200_ctx_launch_count(const gorse_b200_ctx *ctx, int64_t *count)
     return GORSE_B200_OK;
 }
 
+int32_t gorse_b200_device_bytes(int64_t *bytes)
+{
+    GB_CHECK_ARG(bytes != nullptr, "bytes is NULL");
+    *bytes = gb::g_device_bytes.load();
+    return GORSE_B200_OK;
+}
+
 int32_t gorse_b200_ctx_flush_l2(gorse_b200_ctx *ctx)
 {
     GB_CHECK_ARG(ctx != nullptr, "ctx is NULL");
     gb::ScopedDevice sd(ctx->device);
-    if (!ctx->flush_buf) {
-        ctx->flush_bytes = (size_t)256 << 20;  // 5x the 50 MB L2
-        GB_CUDA(cudaMalloc(&ctx->flush_buf, ctx->flush_bytes));
-    }
-    gb::flush_kernel<<<ctx->sm_count * 4, 256, 0, ctx->stream>>>((float4 *)ctx->flush_buf, ctx->flush_bytes / 16,
-                                                                (float)(ctx->launches & 7));
+    if (!ctx->flush_buf.p) GB_TRY(ctx->flush_buf.alloc(((size_t)256 << 20) / sizeof(float4)));  // 5x the 50 MB L2
+    gb::flush_kernel<<<ctx->sm_count * 4, 256, 0, ctx->stream>>>(ctx->flush_buf.p, ctx->flush_buf.n, (float)(ctx->launches & 7));
     GB_CUDA(cudaGetLastError());  // not counted: measurement hygiene, not the hot path
     return GORSE_B200_OK;
 }
@@ -235,7 +236,7 @@ int32_t gorse_b200_ctx_barrier(gorse_b200_ctx *ctx)
     gb::ScopedDevice sd(ctx->device);
     if (ctx->world > 1) {
         GB_NCCL_API(nc);
-        GB_NCCL(nc, AllReduce(ctx->nccl_token, ctx->nccl_token, 1, ncclInt32, ncclSum, ctx->comm, ctx->stream));
+        GB_NCCL(nc, AllReduce(ctx->nccl_token.p, ctx->nccl_token.p, 1, ncclInt32, ncclSum, ctx->comm, ctx->stream));
     }
     GB_CUDA(cudaStreamSynchronize(ctx->stream));
     return GORSE_B200_OK;

@@ -234,21 +234,7 @@ struct EmbWork {
     DevBuf<uint8_t> mask;
     DevBuf<int64_t> test_off, shot_off, excl_off, neg_off, cand_off, rt_off, tile_off, pair_base;
     DevBuf<int32_t> test_items, shot_items, excl_items, neg_items, cand_items, rt_items, count;
-    ~EmbWork()
-    {
-        emb.free(); dist.free(); score.free(); inv.free(); metrics.free(); mask.free();
-        test_off.free(); shot_off.free(); excl_off.free(); neg_off.free(); cand_off.free(); rt_off.free(); tile_off.free(); pair_base.free();
-        test_items.free(); shot_items.free(); excl_items.free(); neg_items.free(); cand_items.free(); rt_items.free(); count.free();
-    }
 };
-
-template <typename T>
-int32_t upload(DevBuf<T> &d, const T *h, size_t n, cudaStream_t s)
-{
-    GB_TRY(d.alloc(std::max<size_t>(n, 1)));
-    if (n) GB_CUDA(cudaMemcpyAsync(d.p, h, sizeof(T) * n, cudaMemcpyHostToDevice, s));
-    return GORSE_B200_OK;
-}
 
 // a CSR argument: offsets non-decreasing, ids in [0, n_items); rebased to start at 0
 int32_t check_csr(const char *what, int64_t n_users, const int64_t *off, const int32_t *items, int32_t n_items, std::vector<int64_t> &rebased)
@@ -331,12 +317,12 @@ extern "C" int32_t gorse_b200_embedding_eval(gorse_b200_ctx *ctx, int32_t n_item
         return err == cudaErrorMemoryAllocation ? GORSE_B200_ERR_OOM : GORSE_B200_ERR_CUDA;
     };
     const int ub = std::max(1, (U + 127) / 128);
-    GB_TRY(upload(W.emb, emb, (size_t)n_items * dim, s));
-    if (emb_mask) GB_TRY(upload(W.mask, emb_mask, (size_t)n_items, s));
-    GB_TRY(upload(W.test_off, toff.data(), (size_t)U + 1, s));
-    GB_TRY(upload(W.test_items, test_items, (size_t)toff[(size_t)U], s));
-    GB_TRY(upload(W.shot_off, vs_off.data(), (size_t)U + 1, s));
-    GB_TRY(upload(W.shot_items, vs_items.data(), vs_items.size(), s));
+    GB_TRY(W.emb.upload(emb, (size_t)n_items * dim, s));
+    if (emb_mask) GB_TRY(W.mask.upload(emb_mask, (size_t)n_items, s));
+    GB_TRY(W.test_off.upload(toff.data(), (size_t)U + 1, s));
+    GB_TRY(W.test_items.upload(test_items, (size_t)toff[(size_t)U], s));
+    GB_TRY(W.shot_off.upload(vs_off.data(), (size_t)U + 1, s));
+    GB_TRY(W.shot_items.upload(vs_items.data(), vs_items.size(), s));
     GB_TRY(W.count.alloc((size_t)U + 1));
     GB_CUDA(cudaMemsetAsync(W.count.p, 0, sizeof(int32_t) * ((size_t)U + 1), s));
     // one pass over the present rows before anything is scored: the reference would push NaN into its heap
@@ -347,8 +333,8 @@ extern "C" int32_t gorse_b200_embedding_eval(gorse_b200_ctx *ctx, int32_t n_item
     const uint64_t base = eval_negatives_base(seed);
     std::vector<int32_t> hc((size_t)U + 1);
     if (sample) {
-        GB_TRY(upload(W.excl_off, xoff.data(), (size_t)U + 1, s));
-        GB_TRY(upload(W.excl_items, xs.data(), xs.size(), s));
+        GB_TRY(W.excl_off.upload(xoff.data(), (size_t)U + 1, s));
+        GB_TRY(W.excl_items.upload(xs.data(), xs.size(), s));
         launch_eval_negatives(s, W.excl_off.p, W.excl_items.p, W.test_off.p, W.test_items.p, U, 0, n_items, n_candidates, base, true,
                               W.count.p, nullptr, nullptr);
         GB_LAUNCHED(ctx);
@@ -360,14 +346,14 @@ extern "C" int32_t gorse_b200_embedding_eval(gorse_b200_ctx *ctx, int32_t n_item
     if (sample) {
         noff.assign((size_t)U + 1, 0);
         for (int32_t u = 0; u < U; u++) noff[(size_t)u + 1] = noff[(size_t)u] + hc[(size_t)u];
-        GB_TRY(upload(W.neg_off, noff.data(), (size_t)U + 1, s));
+        GB_TRY(W.neg_off.upload(noff.data(), (size_t)U + 1, s));
         GB_TRY(W.neg_items.alloc(std::max<size_t>((size_t)noff[(size_t)U], 1)));
         launch_eval_negatives(s, W.excl_off.p, W.excl_items.p, W.test_off.p, W.test_items.p, U, 0, n_items, n_candidates, base, false,
                               nullptr, W.neg_off.p, W.neg_items.p);
         GB_LAUNCHED(ctx);
     } else {
-        GB_TRY(upload(W.neg_off, noff.data(), (size_t)U + 1, s));
-        GB_TRY(upload(W.neg_items, neg_items, (size_t)noff[(size_t)U], s));
+        GB_TRY(W.neg_off.upload(noff.data(), (size_t)U + 1, s));
+        GB_TRY(W.neg_items.upload(neg_items, (size_t)noff[(size_t)U], s));
     }
     if (U > 0) {
         emb_cand_kernel<<<ub, 128, 0, s>>>(W.test_off.p, W.test_items.p, W.neg_off.p, W.neg_items.p, emb_mask ? W.mask.p : nullptr, W.shot_off.p,
@@ -389,13 +375,13 @@ extern "C" int32_t gorse_b200_embedding_eval(gorse_b200_ctx *ctx, int32_t n_item
         tile_off[(size_t)u + 1] = tile_off[(size_t)u] + (m > 0 ? (((m + 3) / 4) * ((k + 3) / 4) + MT - 1) / MT : 0);
         pair_base[(size_t)u + 1] = pair_base[(size_t)u] + (m > 0 ? m * k : 0);
     }
-    GB_TRY(upload(W.cand_off, coff.data(), (size_t)U + 1, s));
+    GB_TRY(W.cand_off.upload(coff.data(), (size_t)U + 1, s));
     GB_TRY(W.cand_items.alloc(std::max<size_t>((size_t)coff[(size_t)U], 1)));
     GB_TRY(W.score.alloc(std::max<size_t>((size_t)coff[(size_t)U], 1)));
-    GB_TRY(upload(W.rt_off, rt_off.data(), (size_t)U + 1, s));
-    GB_TRY(upload(W.rt_items, rt_items.data(), rt_items.size(), s));
-    GB_TRY(upload(W.tile_off, tile_off.data(), (size_t)U + 1, s));
-    GB_TRY(upload(W.pair_base, pair_base.data(), (size_t)U + 1, s));
+    GB_TRY(W.rt_off.upload(rt_off.data(), (size_t)U + 1, s));
+    GB_TRY(W.rt_items.upload(rt_items.data(), rt_items.size(), s));
+    GB_TRY(W.tile_off.upload(tile_off.data(), (size_t)U + 1, s));
+    GB_TRY(W.pair_base.upload(pair_base.data(), (size_t)U + 1, s));
     if (U > 0) {
         emb_cand_kernel<<<ub, 128, 0, s>>>(W.test_off.p, W.test_items.p, W.neg_off.p, W.neg_items.p, emb_mask ? W.mask.p : nullptr, W.shot_off.p,
                                            U, false, nullptr, W.cand_off.p, W.cand_items.p);
@@ -431,7 +417,7 @@ extern "C" int32_t gorse_b200_embedding_eval(gorse_b200_ctx *ctx, int32_t n_item
 
     std::vector<float> inv((size_t)topk);
     eval_inv_log2(topk, inv.data());
-    GB_TRY(upload(W.inv, inv.data(), (size_t)topk, s));
+    GB_TRY(W.inv.upload(inv.data(), (size_t)topk, s));
     GB_TRY(W.metrics.alloc((size_t)4 * std::max(U, 1)));
     launch_eval_rank(s, W.cand_off.p, W.cand_items.p, W.score.p, W.rt_off.p, W.rt_items.p, U, topk, W.inv.p, W.metrics.p);
     GB_LAUNCHED(ctx);

@@ -278,7 +278,6 @@ int32_t gb::eval_run_tables(gorse_b200_eval *ev, const float *P, const float *Q,
         ncclResult_t r = e == cudaSuccess ? nc_api->AllReduce(dsum.p, dsum.p, 4, ncclFloat32, ncclSum, c->comm, s) : ncclSuccess;
         if (e == cudaSuccess && r == ncclSuccess) e = cudaMemcpyAsync(h, dsum.p, sizeof(h), cudaMemcpyDeviceToHost, s);
         if (e == cudaSuccess && r == ncclSuccess) e = cudaStreamSynchronize(s);
-        dsum.free();
         if (r != ncclSuccess) { set_error("evaluate: ncclAllReduce -> %s", nc_api->GetErrorString(r)); return GORSE_B200_ERR_NCCL; }
         if (e != cudaSuccess) { set_error("evaluate: %s", cudaGetErrorString(e)); return GORSE_B200_ERR_CUDA; }
         sum0 = h[0]; sum1 = h[1]; sum2 = h[2]; count = h[3];
@@ -295,9 +294,6 @@ int32_t gorse_b200_eval_destroy(gorse_b200_eval *ev)
     if (!ev) return GORSE_B200_OK;
     ScopedDevice sd(ev->cf->ctx->device);
     cudaStreamSynchronize(ev->cf->ctx->stream);
-    ev->test_off.free(); ev->neg_off.free(); ev->cand_off.free();
-    ev->test_items.free(); ev->neg_items.free(); ev->cand_user.free(); ev->cand_item.free();
-    ev->score.free(); ev->inv.free(); ev->metrics.free();
     delete ev;
     return GORSE_B200_OK;
 }
@@ -358,8 +354,8 @@ int32_t gorse_b200_eval_create(gorse_b200_cf *cf, const int64_t *test_off, const
         c->launches++;
         std::vector<int32_t> hc((size_t)U);
         if ((e = cudaMemcpyAsync(hc.data(), cnt.p, sizeof(int32_t) * (size_t)U, cudaMemcpyDeviceToHost, s)) != cudaSuccess ||
-            (e = cudaStreamSynchronize(s)) != cudaSuccess) { cnt.free(); return cuda_fail(e); }
-        cnt.free();
+            (e = cudaStreamSynchronize(s)) != cudaSuccess)
+            return cuda_fail(e);
         for (int32_t u = 0; u < U; u++) noff[(size_t)u + 1] = noff[(size_t)u] + hc[(size_t)u];
         n_neg = noff[(size_t)U];
         if ((st = ev->neg_items.alloc((size_t)n_neg))) return fail(st);

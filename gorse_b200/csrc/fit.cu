@@ -118,21 +118,16 @@ int32_t fit_trials(gorse_b200_cf *cf, int32_t n, const int32_t *als, const gorse
     gorse_b200_ctx *c = cf->ctx;
     Plan plan;
     GB_TRY(plan.create(cf, ev, &tp[0]));   // checks the test and negative rows before the device is touched
-    struct Tables {
-        std::vector<DevBuf<float>> P, Q;
-        ~Tables() { for (auto &b : P) b.free(); for (auto &b : Q) b.free(); }
-    } tab;
-    tab.P.resize((size_t)n);
-    tab.Q.resize((size_t)n);
+    std::vector<DevBuf<float>> tP((size_t)n), tQ((size_t)n);   // each trial's factor tables
     std::vector<FitState> st;
     std::vector<bool> done((size_t)n, false);
     float score[3];
     for (int32_t k = 0; k < n; k++) {
         st.emplace_back(&tp[k]);
-        GB_TRY(tab.P[k].alloc(cf->P.n));
-        GB_TRY(tab.Q[k].alloc(cf->Q.n));
-        GB_TRY(init_normal_tables(cf, tab.P[k].p, tab.Q[k].p, tp[k].init_mean, tp[k].init_stddev, tp[k].seed));
-        GB_TRY(eval_run_tables(plan.p, tab.P[k].p, tab.Q[k].p, score));
+        GB_TRY(tP[k].alloc(cf->P.n));
+        GB_TRY(tQ[k].alloc(cf->Q.n));
+        GB_TRY(init_normal_tables(cf, tP[k].p, tQ[k].p, tp[k].init_mean, tp[k].init_stddev, tp[k].seed));
+        GB_TRY(eval_run_tables(plan.p, tP[k].p, tQ[k].p, score));
         st[k].record(0, score);
         done[k] = tp[k].n_epochs == 0;
     }
@@ -142,17 +137,17 @@ int32_t fit_trials(gorse_b200_cf *cf, int32_t n, const int32_t *als, const gorse
     for (int32_t epoch = 1; std::find(done.begin(), done.end(), false) != done.end(); epoch++) {
         bP.clear(); bQ.clear(); blr.clear(); breg.clear();
         for (int32_t k = 0; k < n; k++)
-            if (!done[k] && !als[k]) { bP.push_back(tab.P[k].p); bQ.push_back(tab.Q[k].p); blr.push_back(tp[k].lr); breg.push_back(tp[k].reg); }
+            if (!done[k] && !als[k]) { bP.push_back(tP[k].p); bQ.push_back(tQ[k].p); blr.push_back(tp[k].lr); breg.push_back(tp[k].reg); }
         GB_TRY(bpr_trials_epoch(cf, (int)bP.size(), bP.data(), bQ.data(), blr.data(), breg.data(), tp[0].seed + (uint64_t)epoch));
         for (int32_t k = 0; k < n; k++)
-            if (!done[k] && als[k]) GB_TRY(als_epoch_tables(cf, tab.P[k].p, tab.Q[k].p, tp[k].reg, tp[k].alpha));
+            if (!done[k] && als[k]) GB_TRY(als_epoch_tables(cf, tP[k].p, tQ[k].p, tp[k].reg, tp[k].alpha));
         for (int32_t k = 0; k < n; k++) {
             gorse_b200_trial_state &s = states[k];
             s.ndcg = -1.0f;
             if (!done[k]) {
                 const bool evaluated = st[k].ran(epoch);
                 if (evaluated) {
-                    GB_TRY(eval_run_tables(plan.p, tab.P[k].p, tab.Q[k].p, score));
+                    GB_TRY(eval_run_tables(plan.p, tP[k].p, tQ[k].p, score));
                     st[k].record(epoch, score);
                     s.ndcg = score[0];
                 }
@@ -170,9 +165,9 @@ int32_t fit_trials(gorse_b200_cf *cf, int32_t n, const int32_t *als, const gorse
     for (int32_t k = 0; k < n; k++) {
         results[k] = st[k].result();
         if (P_out && P_out[k] && cf->P.n)
-            GB_CUDA(cudaMemcpyAsync(P_out[k], tab.P[k].p, cf->P.n * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
+            GB_CUDA(cudaMemcpyAsync(P_out[k], tP[k].p, cf->P.n * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
         if (Q_out && Q_out[k] && cf->Q.n)
-            GB_CUDA(cudaMemcpyAsync(Q_out[k], tab.Q[k].p, cf->Q.n * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
+            GB_CUDA(cudaMemcpyAsync(Q_out[k], tQ[k].p, cf->Q.n * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
     }
     GB_CUDA(cudaStreamSynchronize(c->stream));
     return GORSE_B200_OK;

@@ -222,8 +222,8 @@ int32_t item_tables(gorse_b200_fm *m, int64_t n_items, bool masked, Slot *S)
     const float *P = m->params.p;
     for (int s = 0; s < m->n_emb; s++) {
         const int d = m->dim[(size_t)s];
-        GB_TRY(recall::grow(m->z[s], (size_t)std::max<int64_t>(n_items, 1) * d));
-        GB_TRY(recall::grow(m->zmax[s], (size_t)std::max<int64_t>(n_items, 1)));
+        GB_TRY(m->z[s].grow((size_t)std::max<int64_t>(n_items, 1) * d));
+        GB_TRY(m->zmax[s].grow((size_t)std::max<int64_t>(n_items, 1)));
         const float *b = P + m->slot_off[(size_t)s];
         const size_t kd = (size_t)m->k * d;
         S[s] = Slot{b, b + kd, b + 2 * kd, b + 2 * kd + m->k, b + 3 * kd + m->k, m->emb[s].p, masked ? m->mask.p : nullptr,
@@ -261,8 +261,8 @@ int32_t rank_pass(gorse_b200_fm *m, const Feats &U, const Feats &I, const int64_
     if (*global_sort) {   // a global key / position buffer per CTA, at most 256 MB of them
         stride = max_p;
         sg = std::max<int64_t>(1, std::min<int64_t>(sg, (int64_t(256) << 20) / (max_p * 12)));
-        GB_TRY(recall::grow(m->sort_key, (size_t)(sg * stride)));
-        GB_TRY(recall::grow(m->sort_val, (size_t)(sg * stride)));
+        GB_TRY(m->sort_key.grow((size_t)(sg * stride)));
+        GB_TRY(m->sort_val.grow((size_t)(sg * stride)));
     }
     fm_sort_kernel<<<(unsigned)sg, SORT_THREADS, 0, st>>>(c_off, u0, u1, score, order, m->sort_key.p, m->sort_val.p, stride);
     GB_LAUNCHED(ctx);
@@ -314,7 +314,7 @@ extern "C" int32_t gorse_b200_fm_create(gorse_b200_ctx *ctx, int64_t n_features,
         set_error("fm: parameter upload failed");
         st = GORSE_B200_ERR_CUDA;
     }
-    if (st) { m->params.free(); delete m; return st; }
+    if (st) { delete m; return st; }
     *out = m;
     return GORSE_B200_OK;
 }
@@ -323,13 +323,6 @@ extern "C" int32_t gorse_b200_fm_destroy(gorse_b200_fm *m)
 {
     if (!m) return GORSE_B200_OK;
     ScopedDevice sd(m->ctx->device);
-    m->params.free();
-    for (auto *b : {&m->u_feat, &m->u_idx, &m->i_feat, &m->i_idx, &m->cand, &m->dims, &m->ch_rows, &m->order, &m->sort_val}) b->free();
-    for (auto *b : {&m->u_off, &m->i_off, &m->c_off, &m->ch_start}) b->free();
-    for (auto *b : {&m->u_val, &m->i_val, &m->score, &m->vx, &m->rowsum}) b->free();
-    for (int s = 0; s < fm::MAX_SLOTS; s++) { m->emb[s].free(); m->z[s].free(); m->zmax[s].free(); }
-    m->mask.free();
-    m->sort_key.free();
     delete m;
     return GORSE_B200_OK;
 }
@@ -413,28 +406,28 @@ extern "C" int32_t gorse_b200_fm_rank(gorse_b200_fm *m, int64_t n_users, const i
     gorse_b200_ctx *ctx = m->ctx;
     ScopedDevice sd(ctx->device);
     cudaStream_t st = ctx->stream;
-    GB_TRY(put(m->u_feat, user_feat, (size_t)n_users, st));
-    GB_TRY(put(m->u_off, user_lab_off, (size_t)n_users + 1, st));
-    GB_TRY(put(m->u_idx, user_lab_idx, (size_t)user_lab_off[n_users], st));
-    GB_TRY(put(m->u_val, user_lab_val, (size_t)user_lab_off[n_users], st));
-    GB_TRY(put(m->i_feat, item_feat, (size_t)n_items, st));
-    GB_TRY(put(m->i_off, item_lab_off, (size_t)n_items + 1, st));
-    GB_TRY(put(m->i_idx, item_lab_idx, (size_t)item_lab_off[n_items], st));
-    GB_TRY(put(m->i_val, item_lab_val, (size_t)item_lab_off[n_items], st));
-    GB_TRY(put(m->c_off, cand_off, (size_t)n_users + 1, st));
-    GB_TRY(put(m->cand, cand_items, (size_t)total, st));
-    GB_TRY(put(m->dims, dims.data(), dims.size(), st));
-    GB_TRY(recall::grow(m->score, (size_t)total));
-    GB_TRY(recall::grow(m->order, (size_t)total));
+    GB_TRY(m->u_feat.upload(user_feat, (size_t)n_users, st));
+    GB_TRY(m->u_off.upload(user_lab_off, (size_t)n_users + 1, st));
+    GB_TRY(m->u_idx.upload(user_lab_idx, (size_t)user_lab_off[n_users], st));
+    GB_TRY(m->u_val.upload(user_lab_val, (size_t)user_lab_off[n_users], st));
+    GB_TRY(m->i_feat.upload(item_feat, (size_t)n_items, st));
+    GB_TRY(m->i_off.upload(item_lab_off, (size_t)n_items + 1, st));
+    GB_TRY(m->i_idx.upload(item_lab_idx, (size_t)item_lab_off[n_items], st));
+    GB_TRY(m->i_val.upload(item_lab_val, (size_t)item_lab_off[n_items], st));
+    GB_TRY(m->c_off.upload(cand_off, (size_t)n_users + 1, st));
+    GB_TRY(m->cand.upload(cand_items, (size_t)total, st));
+    GB_TRY(m->dims.upload(dims.data(), dims.size(), st));
+    GB_TRY(m->score.grow((size_t)total));
+    GB_TRY(m->order.grow((size_t)total));
 
     Feats U{m->u_feat.p, m->u_off.p, m->u_idx.p, m->u_val.p};
     Feats I{m->i_feat.p, m->i_off.p, m->i_idx.p, m->i_val.p};
     Slot S[MAX_SLOTS];
     if (n_emb > 0) {
-        GB_TRY(put(m->ch_start, ch_start.data(), ch_start.size(), st));
-        GB_TRY(put(m->ch_rows, ch_rows.data(), ch_rows.size(), st));
-        if (item_emb_mask) GB_TRY(put(m->mask, item_emb_mask, (size_t)n_items * n_emb, st));
-        for (int s = 0; s < n_emb; s++) GB_TRY(put(m->emb[s], item_emb[s], (size_t)n_items * m->dim[(size_t)s], st));
+        GB_TRY(m->ch_start.upload(ch_start.data(), ch_start.size(), st));
+        GB_TRY(m->ch_rows.upload(ch_rows.data(), ch_rows.size(), st));
+        if (item_emb_mask) GB_TRY(m->mask.upload(item_emb_mask, (size_t)n_items * n_emb, st));
+        for (int s = 0; s < n_emb; s++) GB_TRY(m->emb[s].upload(item_emb[s], (size_t)n_items * m->dim[(size_t)s], st));
         GB_TRY(item_tables(m, n_items, item_emb_mask != nullptr, S));
     }
     // device passes over consecutive users holding at most GROUP_PAIRS pairs (or one user)
@@ -448,8 +441,8 @@ extern "C" int32_t gorse_b200_fm_rank(gorse_b200_fm *m, int64_t n_users, const i
         if (np > 0) {
             passes++;
             if (n_emb > 0) {
-                GB_TRY(recall::grow(m->vx, (size_t)np * m->k));
-                GB_TRY(recall::grow(m->rowsum, (size_t)np));
+                GB_TRY(m->vx.grow((size_t)np * m->k));
+                GB_TRY(m->rowsum.grow((size_t)np));
             }
             bool global_sort = false;
             GB_TRY(rank_pass(m, U, I, m->c_off.p, m->cand.p, m->dims.p, u0, u1, pb, S, m->ch_start.p, m->ch_rows.p, first_chunk[(size_t)u0],

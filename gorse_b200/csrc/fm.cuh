@@ -62,14 +62,6 @@ struct gorse_b200_fm {
 namespace gb {
 namespace fm {
 
-template <typename T>
-int32_t put(DevBuf<T> &b, const T *h, size_t n, cudaStream_t st)
-{
-    GB_TRY(recall::grow(b, std::max<size_t>(n, 1)));
-    if (n) GB_CUDA(cudaMemcpyAsync(b.p, h, n * sizeof(T), cudaMemcpyHostToDevice, st));
-    return GORSE_B200_OK;
-}
-
 // the row of V / W an index selects once it has travelled as float32; false when it leaves the table (Go panics there)
 inline bool feature_ok(int64_t idx, int64_t n_features)
 {

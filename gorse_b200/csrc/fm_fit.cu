@@ -506,20 +506,9 @@ inline bool feature_ok(int64_t idx, int64_t n_features)
     return (int64_t)(float)idx < n_features;
 }
 
-template <typename T>
-struct Buf : DevBuf<T> {
-    ~Buf() { this->free(); }
-    int32_t put(const std::vector<T> &h, cudaStream_t st)
-    {
-        GB_TRY(this->alloc(std::max<size_t>(h.size(), 1)));
-        if (!h.empty()) GB_CUDA(cudaMemcpyAsync(this->p, h.data(), h.size() * sizeof(T), cudaMemcpyHostToDevice, st));
-        return GORSE_B200_OK;
-    }
-};
-
 struct TestSet {                  // one list of EvaluateClassification: padded rows, their table rows and (per trial) their predictions
-    Buf<int32_t> idx, emb_row;
-    Buf<float> val;
+    DevBuf<int32_t> idx, emb_row;
+    DevBuf<float> val;
     float *pred = nullptr, *sorted = nullptr;
     int64_t n = 0;
     int32_t D = 0;
@@ -617,32 +606,32 @@ struct Fit {
     bool train = true;                     // false: predictions only (gorse_b200_fm_gauc), no optimiser tables
     int64_t n_params = 0, max_total = 0;   // max_total: the most optimiser steps of any trial
     // training set, shared by the trials (so is the stamp: they step in lockstep)
-    Buf<int32_t> tr_idx, tr_len, seg_start, seg_feat, seg_pos, stamp;
-    Buf<float> tr_val, tr_tgt;
-    Buf<int64_t> batch_seg, t_base;
+    DevBuf<int32_t> tr_idx, tr_len, seg_start, seg_feat, seg_pos, stamp;
+    DevBuf<float> tr_val, tr_tgt;
+    DevBuf<int64_t> batch_seg, t_base;
     int64_t n_train = 0, n_batches = 0;
     int32_t D = 0;
     unsigned grad_grid = 1;
     // evaluation lists, shared; the counts and sums: one set per trial of a group
     TestSet te[2];
-    Buf<unsigned long long> counts;
-    Buf<float> auc_sum;
-    Buf<unsigned char> cub_tmp;
+    DevBuf<unsigned long long> counts;
+    DevBuf<float> auc_sum;
+    DevBuf<unsigned char> cub_tmp;
     // item-embedding slots: the table and the row maps, shared
     int n_emb = 0, maxdim = 1;
     int64_t base = 0;             // parameters before the first slot
     const EmbArgs *E = nullptr;
-    Buf<uint16_t> table[MAX_SLOTS];
-    Buf<uint8_t> mask;
-    Buf<int32_t> tr_row;
+    DevBuf<uint16_t> table[MAX_SLOTS];
+    DevBuf<uint8_t> mask;
+    DevBuf<int32_t> tr_row;
     SlotTensors tens{};
     int64_t rows = 1, slot_rows = 1;   // a batch's rows; the slots' (the largest batch or evaluation chunk)
     unsigned row_grid = 1;
     // the group: G trials with an arena of `stride` bytes each; the pointers below are trial 0's
     int G = 0;
     int64_t stride = 0;
-    Buf<unsigned char> arena;
-    Buf<int32_t> on, ev_on;       // [MAX_TRIALS]: the trials stepping, the trials evaluated
+    DevBuf<unsigned char> arena;
+    DevBuf<int32_t> on, ev_on;       // [MAX_TRIALS]: the trials stepping, the trials evaluated
     float *P, *M, *Vm, *gV, *gW, *gB, *g, *dss, *dvx, *loss, *batch_loss, *lr_tab;
     int32_t *padnan, *below;
     float *gS, *zmax, *rowsum, *gx, *denc, *dh, *sumdx, *p, *vx;
@@ -679,12 +668,12 @@ int32_t Fit::upload_train(const int64_t *off, const int32_t *idx, const float *v
     std::vector<int32_t> pi;
     std::vector<float> pv;
     pad_rows(off, idx, val, rows_, D, pi, pv);
-    GB_TRY(tr_idx.put(pi, st));
-    GB_TRY(tr_val.put(pv, st));
-    GB_TRY(tr_tgt.put(std::vector<float>(tgt, tgt + n_train), st));
+    GB_TRY(tr_idx.upload(pi.data(), pi.size(), st));
+    GB_TRY(tr_val.upload(pv.data(), pv.size(), st));
+    GB_TRY(tr_tgt.upload(tgt, (size_t)n_train, st));
     std::vector<int32_t> len((size_t)n_train);
     for (int64_t r = 0; r < n_train; r++) len[(size_t)r] = (int32_t)(off[r + 1] - off[r]);
-    GB_TRY(tr_len.put(len, st));
+    GB_TRY(tr_len.upload(len.data(), len.size(), st));
     const int64_t n_real = n_train > 0 ? off[n_train] : 0;   // positions that are not padding
     GB_TRY(batch_seg.alloc((size_t)n_batches + 1));
     GB_CUDA(cudaMemsetAsync(batch_seg.p, 0, ((size_t)n_batches + 1) * sizeof(int64_t), st));
@@ -695,8 +684,8 @@ int32_t Fit::upload_train(const int64_t *off, const int32_t *idx, const float *v
     if (n_real > 0) {
         // the feature lists of every batch: a stable sort of (batch, feature) keys keeps each feature's positions in order;
         // the padding is left out (fm_fit_forward_kernel)
-        Buf<uint64_t> key, key2;
-        Buf<int32_t> pos, head, seg_id, seg_batch;
+        DevBuf<uint64_t> key, key2;
+        DevBuf<int32_t> pos, head, seg_id, seg_batch;
         GB_TRY(key.alloc((size_t)np));
         GB_TRY(key2.alloc((size_t)np));
         GB_TRY(pos.alloc((size_t)np));
@@ -746,12 +735,12 @@ int32_t Fit::upload_list(TestSet &T, const int64_t *off, const int32_t *idx, con
     std::vector<int32_t> pi;
     std::vector<float> pv;
     pad_rows(off, idx, val, rows_, T.D, pi, pv);
-    GB_TRY(T.idx.put(pi, st));
-    GB_TRY(T.val.put(pv, st));
+    GB_TRY(T.idx.upload(pi.data(), pi.size(), st));
+    GB_TRY(T.val.upload(pv.data(), pv.size(), st));
     if (emb_row) {
         std::vector<int32_t> er(rows_.size());
         for (size_t i = 0; i < er.size(); i++) er[i] = emb_row[rows_[i]];
-        GB_TRY(T.emb_row.put(er, st));
+        GB_TRY(T.emb_row.upload(er.data(), er.size(), st));
     }
     return GORSE_B200_OK;
 }
@@ -786,9 +775,9 @@ int32_t Fit::upload_slots()
         const int64_t kd = (int64_t)k * E->dim[s], len[5] = {kd, kd, k, kd, k};
         for (int q = 0; q < 5; q++) tens.end[tens.n++] = (int32_t)(total += len[q]);
     }
-    if (E->mask) GB_TRY(mask.put(std::vector<uint8_t>(E->mask, E->mask + E->n_rows * n_emb), st));
-    GB_TRY(tr_row.put(std::vector<int32_t>(E->train_row, E->train_row + n_train), st));
-    for (int s = 0; s < n_emb; s++) GB_TRY(table[s].put(std::vector<uint16_t>(E->table[s], E->table[s] + E->n_rows * E->dim[s]), st));
+    if (E->mask) GB_TRY(mask.upload(E->mask, (size_t)(E->n_rows * n_emb), st));
+    GB_TRY(tr_row.upload(E->train_row, (size_t)n_train, st));
+    for (int s = 0; s < n_emb; s++) GB_TRY(table[s].upload(E->table[s], (size_t)(E->n_rows * E->dim[s]), st));
     return GORSE_B200_OK;
 }
 
@@ -833,7 +822,6 @@ int32_t Fit::alloc_group(int g)
 {
     G = g;
     stride = (int64_t)carve(0);
-    arena.free();
     GB_TRY(arena.alloc((size_t)stride * g));
     carve((uintptr_t)arena.p);
     GB_CUDA(cudaMemsetAsync(arena.p, 0, arena.n, st));
@@ -1387,13 +1375,13 @@ int32_t gauc_run(gorse_b200_ctx *ctx, const Data &d, const gorse_b200_fm_fit_par
         GB_TRY(F.predict(Group{1, F.stride, F.ev_on.p}, T));
         if (o.pred) GB_CUDA(cudaMemcpyAsync(o.pred, T.pred, (size_t)n * sizeof(float), cudaMemcpyDeviceToHost, st));
         if (ns > 0) {
-            Buf<uint32_t> hi;
-            Buf<uint64_t> key, sorted;
-            Buf<GaucUser> us;
-            Buf<float> auc_d;
-            Buf<unsigned char> tmp;
-            GB_TRY(hi.put(row_hi, st));
-            GB_TRY(us.put(scored, st));
+            DevBuf<uint32_t> hi;
+            DevBuf<uint64_t> key, sorted;
+            DevBuf<GaucUser> us;
+            DevBuf<float> auc_d;
+            DevBuf<unsigned char> tmp;
+            GB_TRY(hi.upload(row_hi.data(), row_hi.size(), st));
+            GB_TRY(us.upload(scored.data(), scored.size(), st));
             GB_TRY(key.alloc((size_t)n));
             GB_TRY(sorted.alloc((size_t)n));
             GB_TRY(auc_d.alloc((size_t)ns));

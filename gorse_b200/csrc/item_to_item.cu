@@ -180,8 +180,6 @@ int32_t neighbour_sums(gorse_b200_vecdb *db, const char *name, int64_t n_users, 
                        const uint8_t *item_ok, int n, int need, int top, double score_scale, int64_t *slots_out, double *scores_out,
                        int32_t *count_out, int64_t *stats_out)
 {
-    using gb::agg::grow_zeroed;
-    using gb::recall::grow;
     const int64_t n_slots = (int64_t)db->ts.size();
     // the live context entries of every user as rows of the neighbour table.  -1 and deleted slots are skipped (GetVectors
     // returns nothing, logics/item_to_item.go:56-58) and never count for a session; hidden ones are queried.
@@ -210,8 +208,8 @@ int32_t neighbour_sums(gorse_b200_vecdb *db, const char *name, int64_t n_users, 
         cudaStreamSynchronize(c->copy_stream);
         return s;
     };
-    if ((st = grow(V.nb, (size_t)R)) || (st = grow(V.t_slot, (size_t)R * n)) || (st = grow(V.t_score, (size_t)R * n)) || (st = grow(V.t_cnt, (size_t)R)) ||
-        (item_ok && (st = grow(V.item_ok, (size_t)n_slots))))
+    if ((st = V.nb.grow((size_t)R)) || (st = V.t_slot.grow((size_t)R * n)) || (st = V.t_score.grow((size_t)R * n)) || (st = V.t_cnt.grow((size_t)R)) ||
+        (item_ok && (st = V.item_ok.grow((size_t)n_slots))))
         return done(st);
     cudaError_t e = cudaMemcpyAsync(V.nb.p, nb.data(), sizeof(int64_t) * R, cudaMemcpyHostToDevice, c->stream);
     if (e == cudaSuccess && item_ok) e = cudaMemcpyAsync(V.item_ok.p, item_ok, (size_t)n_slots, cudaMemcpyHostToDevice, c->stream);
@@ -227,9 +225,9 @@ int32_t neighbour_sums(gorse_b200_vecdb *db, const char *name, int64_t n_users, 
     const int64_t N = n_slots;
     const int hg = heavy_grid(c, N, ROW_BYTES);
     const int64_t total_ctx = c_off[(size_t)n_users];
-    if ((st = grow(V.c_off, (size_t)cu + 1)) || (st = grow(V.ex_off, (size_t)cu + 1)) || (st = grow(V.users, (size_t)cu)) ||
-        (st = grow(V.c_row, (size_t)std::max<int64_t>(total_ctx, 1))) || (st = grow(V.ex, std::max<size_t>(ex.size(), 1))) ||
-        (st = grow(V.slots, (size_t)n_users * top)) || (st = grow(V.scores, (size_t)n_users * top)) || (st = grow(V.count, (size_t)n_users)))
+    if ((st = V.c_off.grow((size_t)cu + 1)) || (st = V.ex_off.grow((size_t)cu + 1)) || (st = V.users.grow((size_t)cu)) ||
+        (st = V.c_row.grow((size_t)std::max<int64_t>(total_ctx, 1))) || (st = V.ex.grow(std::max<size_t>(ex.size(), 1))) ||
+        (st = V.slots.grow((size_t)n_users * top)) || (st = V.scores.grow((size_t)n_users * top)) || (st = V.count.grow((size_t)n_users)))
         return done(st);
     const NeighbourTable T{V.t_slot.p, V.t_score.p, V.t_cnt.p};
     const bool euclid = db->distance == GORSE_B200_DISTANCE_EUCLIDEAN;
@@ -247,8 +245,8 @@ int32_t neighbour_sums(gorse_b200_vecdb *db, const char *name, int64_t n_users, 
         const int64_t fill = route(h_coff.data(), rows, n, h_users);
         n_shared += fill;
         n_heavy += rows - fill;
-        if (rows - fill > 0 && ((st = grow(V.acc, (size_t)hg * N)) || (st = grow_zeroed(V.seen, (size_t)hg * N, c->stream)) ||
-                                (st = grow(V.touched, (size_t)hg * N))))
+        if (rows - fill > 0 && ((st = V.acc.grow((size_t)hg * N)) || (st = V.seen.grow_zeroed((size_t)hg * N, c->stream)) ||
+                                (st = V.touched.grow((size_t)hg * N))))
             return done(st);
         const int64_t n_c = h_coff[rows], n_e = h_exoff[rows];
         if ((e = cudaMemcpyAsync(V.c_off.p, h_coff.data(), sizeof(int64_t) * (rows + 1), cudaMemcpyHostToDevice, c->stream)) != cudaSuccess ||

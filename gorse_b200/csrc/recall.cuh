@@ -181,11 +181,5 @@ __device__ __forceinline__ void emit_in_rounds(float *sc, int64_t N, int K, uint
 
 #endif  // __CUDACC__
 
-template <typename T>
-int32_t grow(DevBuf<T> &b, size_t n)
-{
-    return b.n >= n ? GORSE_B200_OK : b.alloc(n);
-}
-
 }  // namespace recall
 }  // namespace gb

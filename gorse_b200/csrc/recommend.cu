@@ -341,14 +341,6 @@ __global__ void __launch_bounds__(NT) rec_emit_kernel(const int32_t *packed, con
 template <typename T>
 using Buf = DevBuf<T>;   // grow-only, kept with the context between calls
 
-template <typename T>
-int32_t upload(Buf<T> &b, const T *h, size_t n, cudaStream_t st)
-{
-    GB_TRY(recall::grow(b, std::max<size_t>(n, 1)));
-    if (n) GB_CUDA(cudaMemcpyAsync(b.p, h, n * sizeof(T), cudaMemcpyHostToDevice, st));
-    return GORSE_B200_OK;
-}
-
 // the host's preparation of one item-to-item / user-to-user stage, and its neighbour table
 struct StageData {
     std::vector<int64_t> nb;                 // distinct query slots
@@ -369,12 +361,6 @@ struct StageData {
         nb.clear(); c_off.clear(); c_row.clear(); q_row.clear(); es0.clear(); es0_off.clear();
         heavy = false;
     }
-    void free()
-    {
-        for (auto *b : {&d_nb, &d_map, &d_fb_off, &d_es0, &ES[0], &ES[1]}) b->free();
-        for (auto *b : {&t_slot, &t_cnt, &d_item_of_slot, &d_fb_items, &d_c_row, &d_q_row, &flag, &touched}) b->free();
-        t_score.free(); d_item_ok.free(); seen.free(); acc.free(); uacc.free();
-    }
 };
 
 // the device buffers of gorse_b200_recommend, grow-only and kept with the context (the global accumulator rows are zero
@@ -392,22 +378,6 @@ struct Work {
     Buf<int32_t> d_cand, d_cnt, d_start, d_users, d_list, d_work, d_route, d_rcount, d_out_items[2], d_out_cnt[2], d_dims;
     Buf<double> d_cscore, d_rscore, d_dscore, d_out_scores[2];
     Buf<u128> d_sort;
-    void free()
-    {
-        for (auto *b : {&d_live, &d_repl_pos}) b->free();
-        for (auto *b : {&d_repl_items, &d_cf_item_of_slot, &d_u_len, &d_i_len, &d_cand, &d_cnt, &d_start, &d_users, &d_list, &d_work, &d_route,
-                        &d_rcount, &d_out_items[0], &d_out_items[1], &d_out_cnt[0], &d_out_cnt[1], &d_dims})
-            b->free();
-        for (auto *b : {&d_repl_off, &d_cf_excl_off, &d_cand_off, &d_E_off, &d_e0_off, &d_e0, &d_E[0], &d_E[1], &d_i2i_off, &d_fm_off, &d_ch_off,
-                        &d_rids})
-            b->free();
-        for (auto *b : {&d_cscore, &d_rscore, &d_dscore, &d_out_scores[0], &d_out_scores[1]}) b->free();
-        d_sort.free();
-        for (auto &b : l_items) b.free();
-        for (auto &b : l_scores) b.free();
-        for (auto &b : l_off) b.free();
-        for (auto &s : sd) s.free();
-    }
 };
 
 std::mutex work_mu;   // guards the creation of a context's Work
@@ -416,17 +386,14 @@ Work *work(gorse_b200_ctx *ctx)
 {
     std::lock_guard<std::mutex> lk(work_mu);
     if (!ctx->rec_work) ctx->rec_work = new (std::nothrow) Work();
-    return static_cast<Work *>(ctx->rec_work);
+    return ctx->rec_work;
 }
 
 }  // namespace rec
 
 void recommend_work_free(gorse_b200_ctx *ctx)
 {
-    if (!ctx->rec_work) return;
-    auto *w = static_cast<rec::Work *>(ctx->rec_work);
-    w->free();
-    delete w;
+    delete ctx->rec_work;
     ctx->rec_work = nullptr;
 }
 
@@ -713,10 +680,10 @@ extern "C" int32_t gorse_b200_recommend(gorse_b200_ctx *ctx, int64_t n_users, co
     auto &d_cf_excl_off = W.d_cf_excl_off;
     auto &d_cf_item_of_slot = W.d_cf_item_of_slot;
     int32_t rs = GORSE_B200_OK;
-    if ((rs = upload(d_live, item_live, (size_t)n_items, st))) return done(rs);
-    if (with_repl && ((rs = upload(d_repl_off, repl_off, (size_t)n_users + 1, st)) ||
-                      (rs = upload(d_repl_items, repl_items, (size_t)repl_off[n_users], st)) ||
-                      (rs = upload(d_repl_pos, repl_positive, (size_t)repl_off[n_users], st))))
+    if ((rs = d_live.upload(item_live, (size_t)n_items, st))) return done(rs);
+    if (with_repl && ((rs = d_repl_off.upload(repl_off, (size_t)n_users + 1, st)) ||
+                      (rs = d_repl_items.upload(repl_items, (size_t)repl_off[n_users], st)) ||
+                      (rs = d_repl_pos.upload(repl_positive, (size_t)repl_off[n_users], st))))
         return done(rs);
     auto &l_items = W.l_items;
     auto &l_scores = W.l_scores;
@@ -731,8 +698,8 @@ extern "C" int32_t gorse_b200_recommend(gorse_b200_ctx *ctx, int64_t n_users, co
         StageData &D = sd[(size_t)s];
         if (g.kind == GORSE_B200_STAGE_LIST) {
             const int64_t total = g.list_off ? g.list_off[n_users] : g.list_len;
-            if ((rs = upload(l_items[(size_t)s], g.list_items, (size_t)total, st)) || (rs = upload(l_scores[(size_t)s], g.list_scores, (size_t)total, st)) ||
-                (g.list_off && (rs = upload(l_off[(size_t)s], g.list_off, (size_t)n_users + 1, st))))
+            if ((rs = l_items[(size_t)s].upload(g.list_items, (size_t)total, st)) || (rs = l_scores[(size_t)s].upload(g.list_scores, (size_t)total, st)) ||
+                (g.list_off && (rs = l_off[(size_t)s].upload(g.list_off, (size_t)n_users + 1, st))))
                 return done(rs);
             continue;
         }
@@ -741,18 +708,18 @@ extern "C" int32_t gorse_b200_recommend(gorse_b200_ctx *ctx, int64_t n_users, co
         const int64_t S = (int64_t)g.db->ts.size();
         const bool i2i = g.kind == GORSE_B200_STAGE_ITEM_TO_ITEM;
         if (i2i) {
-            if ((rs = upload(D.d_map, g.slot_of_item, (size_t)n_items, st)) || (rs = upload(D.d_item_of_slot, g.item_of_slot, (size_t)S, st)) ||
-                (rs = upload(D.d_c_row, D.c_row.data(), D.c_row.size(), st)))
+            if ((rs = D.d_map.upload(g.slot_of_item, (size_t)n_items, st)) || (rs = D.d_item_of_slot.upload(g.item_of_slot, (size_t)S, st)) ||
+                (rs = D.d_c_row.upload(D.c_row.data(), D.c_row.size(), st)))
                 return done(rs);
         } else {
             const int64_t nf = g.n_fb_rows ? g.fb_off[g.n_fb_rows] : 0;
-            if ((rs = upload(D.d_fb_off, g.fb_off, g.n_fb_rows ? (size_t)g.n_fb_rows + 1 : 0, st)) || (rs = upload(D.d_fb_items, g.fb_items, (size_t)nf, st)) ||
-                (g.item_ok && (rs = upload(D.d_item_ok, g.item_ok, (size_t)n_items, st))) || (rs = upload(D.d_q_row, D.q_row.data(), D.q_row.size(), st)))
+            if ((rs = D.d_fb_off.upload(g.fb_off, g.n_fb_rows ? (size_t)g.n_fb_rows + 1 : 0, st)) || (rs = D.d_fb_items.upload(g.fb_items, (size_t)nf, st)) ||
+                (g.item_ok && (rs = D.d_item_ok.upload(g.item_ok, (size_t)n_items, st))) || (rs = D.d_q_row.upload(D.q_row.data(), D.q_row.size(), st)))
                 return done(rs);
         }
         if (R == 0) continue;
-        if ((rs = upload(D.d_nb, D.nb.data(), (size_t)R, st)) || (rs = recall::grow(D.t_slot, (size_t)R * g.n)) ||
-            (rs = recall::grow(D.t_score, (size_t)R * g.n)) || (rs = recall::grow(D.t_cnt, (size_t)R)))
+        if ((rs = D.d_nb.upload(D.nb.data(), (size_t)R, st)) || (rs = D.t_slot.grow((size_t)R * g.n)) ||
+            (rs = D.t_score.grow((size_t)R * g.n)) || (rs = D.t_cnt.grow((size_t)R)))
             return done(rs);
         if ((rs = vecdb_allow(g.db, i2i ? g.categories : nullptr, i2i ? g.n_categories : 0))) return done(rs);
         int64_t exact = 0;
@@ -764,8 +731,8 @@ extern "C" int32_t gorse_b200_recommend(gorse_b200_ctx *ctx, int64_t n_users, co
     const float *cf_scores = nullptr;
     const int32_t *cf_count = nullptr;
     if (need_cf) {
-        if ((rs = upload(d_cf_excl_off, excl_off, (size_t)n_users + 1, st)) ||
-            (rs = upload(d_cf_item_of_slot, cf->item_of_slot, cf->db->ts.size(), st)))
+        if ((rs = d_cf_excl_off.upload(excl_off, (size_t)n_users + 1, st)) ||
+            (rs = d_cf_item_of_slot.upload(cf->item_of_slot, cf->db->ts.size(), st)))
             return done(rs);
         if (cf->n > 0 && !cf->db->ts.empty()) {
             if ((rs = vecdb_allow(cf->db, nullptr, 0))) return done(rs);
@@ -787,18 +754,18 @@ extern "C" int32_t gorse_b200_recommend(gorse_b200_ctx *ctx, int64_t n_users, co
     auto &d_i_len = W.d_i_len;
     if (m) {
         const auto &R = *ranker;
-        if ((rs = fm::put(m->u_feat, R.user_feat, (size_t)n_users, st)) || (rs = fm::put(m->u_off, R.user_lab_off, (size_t)n_users + 1, st)) ||
-            (rs = fm::put(m->u_idx, R.user_lab_idx, (size_t)R.user_lab_off[n_users], st)) ||
-            (rs = fm::put(m->u_val, R.user_lab_val, (size_t)R.user_lab_off[n_users], st)) || (rs = fm::put(m->i_feat, R.item_feat, (size_t)n_items, st)) ||
-            (rs = fm::put(m->i_off, R.item_lab_off, n_items ? (size_t)n_items + 1 : 0, st)) ||
-            (rs = fm::put(m->i_idx, R.item_lab_idx, n_items ? (size_t)R.item_lab_off[n_items] : 0, st)) ||
-            (rs = fm::put(m->i_val, R.item_lab_val, n_items ? (size_t)R.item_lab_off[n_items] : 0, st)) ||
-            (rs = upload(d_u_len, u_len.data(), u_len.size(), st)) || (rs = upload(d_i_len, i_len.data(), i_len.size(), st)))
+        if ((rs = m->u_feat.upload(R.user_feat, (size_t)n_users, st)) || (rs = m->u_off.upload(R.user_lab_off, (size_t)n_users + 1, st)) ||
+            (rs = m->u_idx.upload(R.user_lab_idx, (size_t)R.user_lab_off[n_users], st)) ||
+            (rs = m->u_val.upload(R.user_lab_val, (size_t)R.user_lab_off[n_users], st)) || (rs = m->i_feat.upload(R.item_feat, (size_t)n_items, st)) ||
+            (rs = m->i_off.upload(R.item_lab_off, n_items ? (size_t)n_items + 1 : 0, st)) ||
+            (rs = m->i_idx.upload(R.item_lab_idx, n_items ? (size_t)R.item_lab_off[n_items] : 0, st)) ||
+            (rs = m->i_val.upload(R.item_lab_val, n_items ? (size_t)R.item_lab_off[n_items] : 0, st)) ||
+            (rs = d_u_len.upload(u_len.data(), u_len.size(), st)) || (rs = d_i_len.upload(i_len.data(), i_len.size(), st)))
             return done(rs);
         if (m->n_emb > 0) {
-            if (R.item_emb_mask && (rs = fm::put(m->mask, R.item_emb_mask, (size_t)n_items * m->n_emb, st))) return done(rs);
+            if (R.item_emb_mask && (rs = m->mask.upload(R.item_emb_mask, (size_t)n_items * m->n_emb, st))) return done(rs);
             for (int s = 0; s < m->n_emb; s++)
-                if ((rs = fm::put(m->emb[s], n_items ? R.item_emb[s] : nullptr, (size_t)n_items * m->dim[(size_t)s], st))) return done(rs);
+                if ((rs = m->emb[s].upload(n_items ? R.item_emb[s] : nullptr, (size_t)n_items * m->dim[(size_t)s], st))) return done(rs);
             if ((rs = fm::item_tables(m, n_items, R.item_emb_mask != nullptr, FS))) return done(rs);
         }
         FI = fm::Feats{m->i_feat.p, m->i_off.p, m->i_idx.p, m->i_val.p};
@@ -872,50 +839,50 @@ extern "C" int32_t gorse_b200_recommend(gorse_b200_ctx *ctx, int64_t n_users, co
     const int64_t sort_stride = recall::pow2_at_least((int)std::max<int64_t>(max_bound, 1));
     // the re-sort's per-CTA key buffers, at most 256 MB of them (as fm_sort_kernel's)
     const int emit_grid = (int)std::max<int64_t>(1, std::min<int64_t>(grid, (int64_t(256) << 20) / (sort_stride * (int64_t)sizeof(u128))));
-    if ((rs = recall::grow(d_cand_off, (size_t)max_rows + 1)) || (rs = recall::grow(d_E_off, (size_t)max_rows + 1)) ||
-        (rs = recall::grow(d_e0_off, (size_t)max_rows + 1)) || (rs = recall::grow(d_e0, (size_t)std::max<int64_t>(max_e0, 1))) ||
-        (rs = recall::grow(d_E[0], (size_t)std::max<int64_t>(max_c, 1))) || (rs = recall::grow(d_E[1], (size_t)std::max<int64_t>(max_c, 1))) ||
-        (rs = recall::grow(d_cand, (size_t)std::max<int64_t>(max_b, 1))) || (rs = recall::grow(d_cscore, (size_t)std::max<int64_t>(max_b, 1))) ||
-        (rs = recall::grow(d_cnt, (size_t)max_rows)) || (rs = recall::grow(d_start, (size_t)max_rows)) || (rs = recall::grow(d_users, (size_t)max_rows)) ||
-        (rs = recall::grow(d_i2i_off, (size_t)max_rows + 1)) || (rs = recall::grow(d_rcount, (size_t)max_rows)) ||
-        (rs = recall::grow(d_rids, (size_t)std::max<int64_t>(max_rows * max_n, 1))) || (rs = recall::grow(d_rscore, (size_t)std::max<int64_t>(max_rows * max_n, 1))))
+    if ((rs = d_cand_off.grow((size_t)max_rows + 1)) || (rs = d_E_off.grow((size_t)max_rows + 1)) ||
+        (rs = d_e0_off.grow((size_t)max_rows + 1)) || (rs = d_e0.grow((size_t)std::max<int64_t>(max_e0, 1))) ||
+        (rs = d_E[0].grow((size_t)std::max<int64_t>(max_c, 1))) || (rs = d_E[1].grow((size_t)std::max<int64_t>(max_c, 1))) ||
+        (rs = d_cand.grow((size_t)std::max<int64_t>(max_b, 1))) || (rs = d_cscore.grow((size_t)std::max<int64_t>(max_b, 1))) ||
+        (rs = d_cnt.grow((size_t)max_rows)) || (rs = d_start.grow((size_t)max_rows)) || (rs = d_users.grow((size_t)max_rows)) ||
+        (rs = d_i2i_off.grow((size_t)max_rows + 1)) || (rs = d_rcount.grow((size_t)max_rows)) ||
+        (rs = d_rids.grow((size_t)std::max<int64_t>(max_rows * max_n, 1))) || (rs = d_rscore.grow((size_t)std::max<int64_t>(max_rows * max_n, 1))))
         return done(rs);
-    if (any_u2u && ((rs = recall::grow(d_list, (size_t)max_rows)) || (rs = recall::grow(d_work, (size_t)max_rows)) ||
-                    (rs = recall::grow(d_route, (size_t)n_chunks * 2 * n_stages))))
+    if (any_u2u && ((rs = d_list.grow((size_t)max_rows)) || (rs = d_work.grow((size_t)max_rows)) ||
+                    (rs = d_route.grow((size_t)n_chunks * 2 * n_stages))))
         return done(rs);
     if (any_u2u) GB_CUDA(cudaMemsetAsync(d_route.p, 0, sizeof(int32_t) * n_chunks * 2 * n_stages, st));
     for (int32_t s = 0; s < n_stages; s++) {
         StageData &D = sd[(size_t)s];
         const auto &g = stages[s];
         if (g.kind == GORSE_B200_STAGE_ITEM_TO_ITEM) {
-            if ((rs = upload(D.d_es0, D.es0.data(), D.es0.size(), st)) || (rs = recall::grow(D.ES[0], (size_t)std::max<int64_t>(max_c, 1))) ||
-                (rs = recall::grow(D.ES[1], (size_t)std::max<int64_t>(max_c, 1))))
+            if ((rs = D.d_es0.upload(D.es0.data(), D.es0.size(), st)) || (rs = D.ES[0].grow((size_t)std::max<int64_t>(max_c, 1))) ||
+                (rs = D.ES[1].grow((size_t)std::max<int64_t>(max_c, 1))))
                 return done(rs);
             const int64_t N = (int64_t)g.db->ts.size();
             std::vector<int32_t> routed;
             const bool heavy = i2i::route(D.c_off.data(), n_users, g.n, routed) < n_users;
             const int hg = heavy_grid(ctx, std::max<int64_t>(N, 1), i2i::ROW_BYTES);
-            if (heavy && N > 0 && ((rs = recall::grow(D.acc, (size_t)hg * N)) || (rs = agg::grow_zeroed(D.seen, (size_t)hg * N, st)) ||
-                                   (rs = recall::grow(D.touched, (size_t)hg * N))))
+            if (heavy && N > 0 && ((rs = D.acc.grow((size_t)hg * N)) || (rs = D.seen.grow_zeroed((size_t)hg * N, st)) ||
+                                   (rs = D.touched.grow((size_t)hg * N))))
                 return done(rs);
         } else if (g.kind == GORSE_B200_STAGE_USER_TO_USER && D.heavy) {
             const int64_t NI = std::max<int64_t>(n_items, 1);
             const int hg = heavy_grid(ctx, NI, u2u::ROW_BYTES);
-            if ((rs = agg::grow_zeroed(D.uacc, (size_t)hg * NI, st)) || (rs = agg::grow_zeroed(D.flag, (size_t)hg * NI, st)) ||
-                (rs = recall::grow(D.touched, (size_t)hg * NI)))
+            if ((rs = D.uacc.grow_zeroed((size_t)hg * NI, st)) || (rs = D.flag.grow_zeroed((size_t)hg * NI, st)) ||
+                (rs = D.touched.grow((size_t)hg * NI)))
                 return done(rs);
         }
     }
     for (int p = 0; p < 2; p++)
-        if ((rs = recall::grow(d_out_items[p], (size_t)std::max<int64_t>(max_b, 1))) || (rs = recall::grow(d_out_scores[p], (size_t)std::max<int64_t>(max_b, 1))) ||
-            (rs = recall::grow(d_out_cnt[p], (size_t)max_rows)))
+        if ((rs = d_out_items[p].grow((size_t)std::max<int64_t>(max_b, 1))) || (rs = d_out_scores[p].grow((size_t)std::max<int64_t>(max_b, 1))) ||
+            (rs = d_out_cnt[p].grow((size_t)max_rows)))
             return done(rs);
-    if (m && ((rs = recall::grow(d_fm_off, (size_t)max_rows + 1)) || (rs = recall::grow(d_dims, (size_t)max_rows)) ||
-              (rs = recall::grow(d_dscore, (size_t)std::max<int64_t>(max_b, 1))) || (rs = recall::grow(m->cand, (size_t)std::max<int64_t>(max_b, 1))) ||
-              (rs = recall::grow(m->score, (size_t)std::max<int64_t>(max_b, 1))) || (rs = recall::grow(m->order, (size_t)std::max<int64_t>(max_b, 1))) ||
-              (rs = recall::grow(d_sort, (size_t)emit_grid * sort_stride))))
+    if (m && ((rs = d_fm_off.grow((size_t)max_rows + 1)) || (rs = d_dims.grow((size_t)max_rows)) ||
+              (rs = d_dscore.grow((size_t)std::max<int64_t>(max_b, 1))) || (rs = m->cand.grow((size_t)std::max<int64_t>(max_b, 1))) ||
+              (rs = m->score.grow((size_t)std::max<int64_t>(max_b, 1))) || (rs = m->order.grow((size_t)std::max<int64_t>(max_b, 1))) ||
+              (rs = d_sort.grow((size_t)emit_grid * sort_stride))))
         return done(rs);
-    if (m && m->n_emb > 0 && ((rs = recall::grow(m->vx, (size_t)std::max<int64_t>(max_b, 1) * m->k)) || (rs = recall::grow(m->rowsum, (size_t)std::max<int64_t>(max_b, 1)))))
+    if (m && m->n_emb > 0 && ((rs = m->vx.grow((size_t)std::max<int64_t>(max_b, 1) * m->k)) || (rs = m->rowsum.grow((size_t)std::max<int64_t>(max_b, 1)))))
         return done(rs);
     cudaEvent_t reuse[2] = {nullptr, nullptr};
     GB_CUDA(cudaEventCreateWithFlags(&reuse[0], cudaEventDisableTiming));
@@ -1060,9 +1027,9 @@ extern "C" int32_t gorse_b200_recommend(gorse_b200_ctx *ctx, int64_t n_users, co
                 for (int64_t r = 0; r < rows; r++)
                     h_ch_off[(size_t)r + 1] = h_ch_off[(size_t)r] + (bound[(size_t)(u0 + r)] + m->batch_size - 1) / m->batch_size;
                 n_ch = h_ch_off[(size_t)rows];
-                REC_TRY(upload(d_ch_off, h_ch_off.data(), h_ch_off.size(), st));
-                REC_TRY(recall::grow(m->ch_start, (size_t)std::max<int64_t>(n_ch, 1)));
-                REC_TRY(recall::grow(m->ch_rows, (size_t)std::max<int64_t>(n_ch, 1)));
+                REC_TRY(d_ch_off.upload(h_ch_off.data(), h_ch_off.size(), st));
+                REC_TRY(m->ch_start.grow((size_t)std::max<int64_t>(n_ch, 1)));
+                REC_TRY(m->ch_rows.grow((size_t)std::max<int64_t>(n_ch, 1)));
                 ch_off = d_ch_off.p;
             }
             rec_pack_kernel<<<(unsigned)std::min<int64_t>((rows + 7) / 8, (int64_t)ctx->sm_count * 16), 256, 0, st>>>(

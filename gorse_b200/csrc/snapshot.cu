@@ -77,7 +77,6 @@ struct Staging {
         cudaStreamSynchronize(c->copy_stream);
         for (int b = 0; b < 2; b++) {
             if (h[b]) cudaFreeHost(h[b]);
-            d[b].free();
             if (gathered[b]) cudaEventDestroy(gathered[b]);
             if (copied[b]) cudaEventDestroy(copied[b]);
         }
@@ -263,7 +262,6 @@ int32_t save(gorse_b200_vecdb *db, gorse_b200_write_fn write, void *user, int64_
             if (e == cudaSuccess && st == GORSE_B200_OK && k + 2 < chunks) e = enqueue(k + 2);
         }
         cudaStreamSynchronize(c->copy_stream);
-        scan.free();
         if (e != cudaSuccess) { set_error("snapshot save: %s", cudaGetErrorString(e)); return GORSE_B200_ERR_CUDA; }
         if (st) return st;
     }

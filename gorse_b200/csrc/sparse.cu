@@ -448,11 +448,11 @@ int32_t csc_append(gorse_b200_ctx *c, const int64_t *off, const uint32_t *ind, c
     DevBuf<uint64_t> pk, pk_s;
     DevBuf<int64_t> lb;
     DevBuf<uint8_t> tmp;
-    auto done = [&](int32_t st) { cudaStreamSynchronize(s); keys.free(); pk.free(); pk_s.free(); lb.free(); tmp.free(); return st; };
+    StreamSync sync{s};
     int32_t st;
     if ((st = foff_n.alloc((size_t)F_new + 1)) || (st = frow_n.alloc((size_t)(nnz_old + nnz))) || (st = fval_n.alloc((size_t)(nnz_old + nnz))) ||
         (st = keys.alloc((size_t)nnz)) || (st = pk.alloc((size_t)nnz)) || (st = pk_s.alloc((size_t)nnz)) || (st = lb.alloc((size_t)F_new + 1)))
-        return done(st);
+        return st;
     int end_bit = 1;   // every feature index is below F_new
     while (end_bit < 32 && ((uint64_t)F_new - 1) >> end_bit) end_bit++;
     const unsigned grid = (unsigned)c->sm_count * 8;
@@ -463,7 +463,7 @@ int32_t csc_append(gorse_b200_ctx *c, const int64_t *off, const uint32_t *ind, c
         size_t tmp_bytes = 0;
         e = cudaGetLastError();
         if (e == cudaSuccess) e = cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, ind, keys.p, pk.p, pk_s.p, nnz, 0, end_bit, s);
-        if (e == cudaSuccess && (st = tmp.alloc(tmp_bytes))) return done(st);
+        if (e == cudaSuccess && (st = tmp.alloc(tmp_bytes))) return st;
         if (e == cudaSuccess) e = cub::DeviceRadixSort::SortPairs(tmp.p, tmp_bytes, ind, keys.p, pk.p, pk_s.p, nnz, 0, end_bit, s);
     }
     if (e == cudaSuccess) {
@@ -474,8 +474,8 @@ int32_t csc_append(gorse_b200_ctx *c, const int64_t *off, const uint32_t *ind, c
         e = cudaGetLastError();
     }
     if (e == cudaSuccess) e = cudaStreamSynchronize(s);
-    if (e != cudaSuccess) { set_error("sparse CSC: %s", cudaGetErrorString(e)); return done(e == cudaErrorMemoryAllocation ? GORSE_B200_ERR_OOM : GORSE_B200_ERR_CUDA); }
-    return done(GORSE_B200_OK);
+    if (e != cudaSuccess) { set_error("sparse CSC: %s", cudaGetErrorString(e)); return e == cudaErrorMemoryAllocation ? GORSE_B200_ERR_OOM : GORSE_B200_ERR_CUDA; }
+    return GORSE_B200_OK;
 }
 
 // the device layouts from the host CSR: the CSR is uploaded and the CSC built from it on the device
@@ -648,14 +648,10 @@ int32_t gorse_b200_sparse_index_create(gorse_b200_ctx *ctx, gorse_b200_sparse_in
 int32_t gorse_b200_sparse_index_destroy(gorse_b200_sparse_index *ix)
 {
     if (!ix) return GORSE_B200_OK;
-    {
-        ScopedDevice sd(ix->ctx->device);
-        cudaStreamSynchronize(ix->ctx->stream);
-        ix->off.free(); ix->foff.free(); ix->ind.free(); ix->val.free(); ix->frow.free(); ix->fval.free();
-        ix->tl_dot.free(); ix->tl_idx.free(); ix->tl_cnt.free(); ix->next.free(); ix->paths.free();
-        for (cudaEvent_t e : ix->ev)
-            if (e) cudaEventDestroy(e);
-    }
+    ScopedDevice sd(ix->ctx->device);
+    cudaStreamSynchronize(ix->ctx->stream);
+    for (cudaEvent_t e : ix->ev)
+        if (e) cudaEventDestroy(e);
     delete ix;
     return GORSE_B200_OK;
 }
@@ -831,20 +827,23 @@ int32_t sparse_search_host(gorse_b200_sparse_index *ix, int64_t q0, int64_t nq, 
     DevBuf<float> d_dot, dq_val;
     DevBuf<int64_t> dq_off;
     DevBuf<uint32_t> dq_ind;
-    int32_t st = GORSE_B200_OK;
-    auto done = [&](int32_t s) { cudaStreamSynchronize(c->stream); d_idx.free(); d_cnt.free(); d_dot.free(); dq_val.free(); dq_off.free(); dq_ind.free(); return s; };
-    if ((st = d_idx.alloc((size_t)nq * kc)) || (st = d_dot.alloc((size_t)nq * kc)) || (st = d_cnt.alloc((size_t)nq))) return done(st);
+    StreamSync sync{c->stream};
+    GB_TRY(d_idx.alloc((size_t)nq * kc));
+    GB_TRY(d_dot.alloc((size_t)nq * kc));
+    GB_TRY(d_cnt.alloc((size_t)nq));
     cudaError_t e = cudaSuccess;
     if (q_off) {
         const int64_t qn = q_off[nq];
-        if ((st = dq_off.alloc((size_t)nq + 1)) || (st = dq_ind.alloc((size_t)qn)) || (st = dq_val.alloc((size_t)qn))) return done(st);
+        GB_TRY(dq_off.alloc((size_t)nq + 1));
+        GB_TRY(dq_ind.alloc((size_t)qn));
+        GB_TRY(dq_val.alloc((size_t)qn));
         e = cudaMemcpyAsync(dq_off.p, q_off, sizeof(int64_t) * ((size_t)nq + 1), cudaMemcpyHostToDevice, c->stream);
         if (e == cudaSuccess && qn) e = cudaMemcpyAsync(dq_ind.p, q_ind, sizeof(uint32_t) * (size_t)qn, cudaMemcpyHostToDevice, c->stream);
         if (e == cudaSuccess && qn) e = cudaMemcpyAsync(dq_val.p, q_val, sizeof(float) * (size_t)qn, cudaMemcpyHostToDevice, c->stream);
-        if (e != cudaSuccess) { set_error("sparse search upload: %s", cudaGetErrorString(e)); return done(GORSE_B200_ERR_CUDA); }
+        if (e != cudaSuccess) { set_error("sparse search upload: %s", cudaGetErrorString(e)); return GORSE_B200_ERR_CUDA; }
     }
     const Queries Q = q_off ? Queries{dq_off.p, dq_ind.p, dq_val.p, nullptr, 0} : Queries{nullptr, nullptr, nullptr, nullptr, q0};
-    if ((st = tiled_search(ix, Q, nq, d_allow, kc, d_idx.p, d_dot.p, d_cnt.p))) return done(st);
+    GB_TRY(tiled_search(ix, Q, nq, d_allow, kc, d_idx.p, d_dot.p, d_cnt.p));
     if (kc == k) {
         e = cudaMemcpyAsync(idx_out, d_idx.p, sizeof(int32_t) * (size_t)nq * k, cudaMemcpyDeviceToHost, c->stream);
         if (e == cudaSuccess) e = cudaMemcpyAsync(dot_out, d_dot.p, sizeof(float) * (size_t)nq * k, cudaMemcpyDeviceToHost, c->stream);
@@ -856,12 +855,12 @@ int32_t sparse_search_host(gorse_b200_sparse_index *ix, int64_t q0, int64_t nq, 
     }
     if (e == cudaSuccess) e = cudaMemcpyAsync(count_out, d_cnt.p, sizeof(int32_t) * (size_t)nq, cudaMemcpyDeviceToHost, c->stream);
     if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
-    if (e != cudaSuccess) { set_error("sparse search: %s", cudaGetErrorString(e)); return done(GORSE_B200_ERR_CUDA); }
+    if (e != cudaSuccess) { set_error("sparse search: %s", cudaGetErrorString(e)); return GORSE_B200_ERR_CUDA; }
     for (int64_t q = 0; q < nq && kc < k; q++) {
         std::fill(idx_out + q * k + kc, idx_out + (q + 1) * k, -1);
         std::fill(dot_out + q * k + kc, dot_out + (q + 1) * k, 0.f);
     }
-    return done(GORSE_B200_OK);
+    return GORSE_B200_OK;
 }
 
 int32_t sparse_compact(gorse_b200_sparse_index *ix, const int64_t *scan, int64_t live)
@@ -870,19 +869,18 @@ int32_t sparse_compact(gorse_b200_sparse_index *ix, const int64_t *scan, int64_t
     gorse_b200_ctx *c = ix->ctx;
     cudaStream_t s = c->stream;
     const int64_t n = (int64_t)ix->h_off.size() - 1, nnz = (int64_t)ix->h_ind.size(), F = ix->n_features;
+    int64_t live_nnz = 0;
+    std::vector<int64_t> h_off((size_t)live + 1);   // the compacted host CSR
+    std::vector<uint32_t> h_ind;
+    std::vector<float> h_val;
     DevBuf<int64_t> rs, cs, off_n, foff_n;   // entry keep flags, scanned in place: CSR (rs) and CSC (cs)
     DevBuf<uint8_t> tmp;
     DevBuf<uint32_t> ind_n;
     DevBuf<float> val_n, fval_n;
     DevBuf<int32_t> frow_n;
-    auto done = [&](int32_t st) {
-        cudaStreamSynchronize(s);
-        rs.free(); cs.free(); tmp.free();
-        if (st) { off_n.free(); foff_n.free(); ind_n.free(); val_n.free(); fval_n.free(); frow_n.free(); }
-        return st;
-    };
-    int32_t st;
-    if ((st = rs.alloc((size_t)nnz + 1)) || (st = cs.alloc((size_t)nnz + 1))) return done(st);
+    StreamSync sync{s};
+    GB_TRY(rs.alloc((size_t)nnz + 1));
+    GB_TRY(cs.alloc((size_t)nnz + 1));
     const unsigned grid = (unsigned)c->sm_count * 8;
     sparse_row_keep_kernel<<<grid, 256, 0, s>>>(ix->off.p, n, scan, rs.p);
     sparse_col_keep_kernel<<<grid, 256, 0, s>>>(ix->frow.p, nnz, scan, cs.p);
@@ -890,21 +888,22 @@ int32_t sparse_compact(gorse_b200_sparse_index *ix, const int64_t *scan, int64_t
     size_t tmp_bytes = 0;
     cudaError_t e = cudaGetLastError();
     if (e == cudaSuccess) e = cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, rs.p, nnz + 1, s);
-    if (e != cudaSuccess) { set_error("sparse compact: %s", cudaGetErrorString(e)); return done(GORSE_B200_ERR_CUDA); }
-    if ((st = tmp.alloc(tmp_bytes))) return done(st);
-    int64_t live_nnz = 0;
+    if (e != cudaSuccess) { set_error("sparse compact: %s", cudaGetErrorString(e)); return GORSE_B200_ERR_CUDA; }
+    GB_TRY(tmp.alloc(tmp_bytes));
     e = cub::DeviceScan::ExclusiveSum(tmp.p, tmp_bytes, rs.p, nnz + 1, s);
     if (e == cudaSuccess) e = cub::DeviceScan::ExclusiveSum(tmp.p, tmp_bytes, cs.p, nnz + 1, s);
     if (e == cudaSuccess) e = cudaMemcpyAsync(&live_nnz, rs.p + nnz, sizeof(int64_t), cudaMemcpyDeviceToHost, s);
     if (e == cudaSuccess) e = cudaStreamSynchronize(s);
-    if (e != cudaSuccess) { set_error("sparse compact: %s", cudaGetErrorString(e)); return done(GORSE_B200_ERR_CUDA); }
+    if (e != cudaSuccess) { set_error("sparse compact: %s", cudaGetErrorString(e)); return GORSE_B200_ERR_CUDA; }
     // every buffer of the compacted index, then the host CSR, before any state changes
-    if ((st = off_n.alloc((size_t)live + 1)) || (st = foff_n.alloc((size_t)F + 1)) || (st = ind_n.alloc((size_t)live_nnz)) ||
-        (st = val_n.alloc((size_t)live_nnz)) || (st = frow_n.alloc((size_t)live_nnz)) || (st = fval_n.alloc((size_t)live_nnz)))
-        return done(st);
-    std::vector<int64_t> h_off((size_t)live + 1);
-    std::vector<uint32_t> h_ind((size_t)live_nnz);
-    std::vector<float> h_val((size_t)live_nnz);
+    GB_TRY(off_n.alloc((size_t)live + 1));
+    GB_TRY(foff_n.alloc((size_t)F + 1));
+    GB_TRY(ind_n.alloc((size_t)live_nnz));
+    GB_TRY(val_n.alloc((size_t)live_nnz));
+    GB_TRY(frow_n.alloc((size_t)live_nnz));
+    GB_TRY(fval_n.alloc((size_t)live_nnz));
+    h_ind.resize((size_t)live_nnz);
+    h_val.resize((size_t)live_nnz);
     sparse_compact_off_kernel<<<div_up(n + 1, 256), 256, 0, s>>>(ix->off.p, n, scan, rs.p, off_n.p);
     sparse_compact_off_kernel<<<div_up((int64_t)F + 1, 256), 256, 0, s>>>(ix->foff.p, F, nullptr, cs.p, foff_n.p);
     sparse_compact_csr_kernel<<<grid, 256, 0, s>>>(ix->ind.p, ix->val.p, nnz, rs.p, ind_n.p, val_n.p);
@@ -915,12 +914,12 @@ int32_t sparse_compact(gorse_b200_sparse_index *ix, const int64_t *scan, int64_t
     if (e == cudaSuccess && live_nnz) e = cudaMemcpyAsync(h_ind.data(), ind_n.p, sizeof(uint32_t) * h_ind.size(), cudaMemcpyDeviceToHost, s);
     if (e == cudaSuccess && live_nnz) e = cudaMemcpyAsync(h_val.data(), val_n.p, sizeof(float) * h_val.size(), cudaMemcpyDeviceToHost, s);
     if (e == cudaSuccess) e = cudaStreamSynchronize(s);
-    if (e != cudaSuccess) { set_error("sparse compact: %s", cudaGetErrorString(e)); return done(GORSE_B200_ERR_CUDA); }
-    ix->off.free(); ix->foff.free(); ix->ind.free(); ix->val.free(); ix->frow.free(); ix->fval.free();
-    ix->off = off_n; ix->foff = foff_n; ix->ind = ind_n; ix->val = val_n; ix->frow = frow_n; ix->fval = fval_n;
+    if (e != cudaSuccess) { set_error("sparse compact: %s", cudaGetErrorString(e)); return GORSE_B200_ERR_CUDA; }
+    ix->off = std::move(off_n); ix->foff = std::move(foff_n); ix->ind = std::move(ind_n);
+    ix->val = std::move(val_n); ix->frow = std::move(frow_n); ix->fval = std::move(fval_n);
     ix->h_off.swap(h_off); ix->h_ind.swap(h_ind); ix->h_val.swap(h_val);
     ix->tl_dot.free(); ix->tl_idx.free(); ix->tl_cnt.free(); ix->next.free();   // sized for the old N; the next search allocates them
-    return done(GORSE_B200_OK);
+    return GORSE_B200_OK;
 }
 
 int32_t sparse_idf_rows(gorse_b200_ctx *c, int64_t n, const int64_t *a_off, const int32_t *a_ids, const float *a_idf, int32_t a_n_idf,
@@ -929,7 +928,7 @@ int32_t sparse_idf_rows(gorse_b200_ctx *c, int64_t n, const int64_t *a_off, cons
 {
     cudaStream_t s = c->stream;
     const int64_t total = a_off[n] + (b_off ? b_off[n] : 0);
-    out.free();
+    out = SparseRows();
     out.row_off.assign((size_t)n + 1, 0);
     out.off.assign(1, 0);
     if (total == 0) return GORSE_B200_OK;
@@ -945,23 +944,18 @@ int32_t sparse_idf_rows(gorse_b200_ctx *c, int64_t n, const int64_t *a_off, cons
     DevBuf<int64_t> d_aoff, d_boff, d_moff, keep, d_out_off;
     DevBuf<int32_t> d_aids, d_bids;
     DevBuf<float> d_aidf, d_bidf;
+    unsigned h_stat[2] = {0, 0};
     DevBuf<uint64_t> key, key_s;
     DevBuf<uint8_t> head, tmp;
     DevBuf<unsigned> stat;
-    auto done = [&](int32_t st) {
-        cudaStreamSynchronize(s);
-        d_aoff.free(); d_boff.free(); d_moff.free(); keep.free(); d_out_off.free(); d_aids.free(); d_bids.free(); d_aidf.free(); d_bidf.free();
-        key.free(); key_s.free(); head.free(); tmp.free(); stat.free();
-        if (st) out.free();
-        return st;
-    };
+    StreamSync sync{s};
     int32_t st;
     if ((st = d_aoff.alloc((size_t)n + 1)) || (st = d_aids.alloc((size_t)a_off[n])) || (st = d_aidf.alloc((size_t)a_n_idf)) ||
         (b_off && ((st = d_boff.alloc((size_t)n + 1)) || (st = d_moff.alloc((size_t)n + 1)) || (st = d_bids.alloc((size_t)b_off[n])) ||
                    (st = d_bidf.alloc((size_t)b_n_idf)))) ||
         (st = key.alloc((size_t)total)) || (st = key_s.alloc((size_t)total)) || (st = head.alloc((size_t)total)) || (st = keep.alloc((size_t)total + 1)) ||
         (st = d_out_off.alloc((size_t)n + 1)) || (st = stat.alloc(2)))
-        return done(st);
+        return st;
     cudaError_t e = cudaMemcpyAsync(d_aoff.p, a_off, sizeof(int64_t) * ((size_t)n + 1), cudaMemcpyHostToDevice, s);
     if (e == cudaSuccess && a_off[n]) e = cudaMemcpyAsync(d_aids.p, a_ids, sizeof(int32_t) * (size_t)a_off[n], cudaMemcpyHostToDevice, s);
     if (e == cudaSuccess && a_n_idf) e = cudaMemcpyAsync(d_aidf.p, a_idf, sizeof(float) * (size_t)a_n_idf, cudaMemcpyHostToDevice, s);
@@ -985,7 +979,7 @@ int32_t sparse_idf_rows(gorse_b200_ctx *c, int64_t n, const int64_t *a_off, cons
     // each row sorted on its own: a few ids per row for most rows, hundreds of thousands for a head item
     if (e == cudaSuccess) e = cub::DeviceSegmentedSort::SortKeys(nullptr, sort_bytes, key.p, key_s.p, (int)total, (int)n, moff, moff + 1, s);
     if (e == cudaSuccess) e = cub::DeviceScan::ExclusiveSum(nullptr, scan_bytes, keep.p, total + 1, s);
-    if (e == cudaSuccess && (st = tmp.alloc(std::max(sort_bytes, scan_bytes)))) return done(st);
+    if (e == cudaSuccess && (st = tmp.alloc(std::max(sort_bytes, scan_bytes)))) return st;
     if (e == cudaSuccess) e = cub::DeviceSegmentedSort::SortKeys(tmp.p, sort_bytes, key.p, key_s.p, (int)total, (int)n, moff, moff + 1, s);
     if (e == cudaSuccess) {
         idf_keep_kernel<<<grid, 256, 0, s>>>(A, B, key_s.p, head.p, total, keep.p);
@@ -996,9 +990,9 @@ int32_t sparse_idf_rows(gorse_b200_ctx *c, int64_t n, const int64_t *a_off, cons
     int64_t nnz = 0;
     if (e == cudaSuccess) e = cudaMemcpyAsync(&nnz, keep.p + total, sizeof(int64_t), cudaMemcpyDeviceToHost, s);
     if (e == cudaSuccess) e = cudaStreamSynchronize(s);
-    if (e != cudaSuccess) { set_error("idf vectors: %s", cudaGetErrorString(e)); return done(GORSE_B200_ERR_CUDA); }
-    if ((st = out.ind.alloc((size_t)nnz)) || (st = out.val.alloc((size_t)nnz))) return done(st);
-    unsigned h_stat[2] = {0, 0};
+    if (e != cudaSuccess) { set_error("idf vectors: %s", cudaGetErrorString(e)); return GORSE_B200_ERR_CUDA; }
+    GB_TRY(out.ind.alloc((size_t)nnz));
+    GB_TRY(out.val.alloc((size_t)nnz));
     idf_scatter_kernel<<<grid, 256, 0, s>>>(A, B, key_s.p, keep.p, total, out.ind.p, out.val.p, stat.p);
     idf_rows_kernel<<<div_up(n + 1, 256), 256, 0, s>>>(d_aoff.p, moff, keep.p, n, out.ind.p, d_out_off.p, stat.p);
     c->launches += 2;
@@ -1006,18 +1000,18 @@ int32_t sparse_idf_rows(gorse_b200_ctx *c, int64_t n, const int64_t *a_off, cons
     if (e == cudaSuccess) e = cudaMemcpyAsync(out.row_off.data(), d_out_off.p, sizeof(int64_t) * ((size_t)n + 1), cudaMemcpyDeviceToHost, s);
     if (e == cudaSuccess) e = cudaMemcpyAsync(h_stat, stat.p, sizeof(h_stat), cudaMemcpyDeviceToHost, s);
     if (e == cudaSuccess) e = cudaStreamSynchronize(s);
-    if (e != cudaSuccess) { set_error("idf vectors: %s", cudaGetErrorString(e)); return done(GORSE_B200_ERR_CUDA); }
+    if (e != cudaSuccess) { set_error("idf vectors: %s", cudaGetErrorString(e)); return GORSE_B200_ERR_CUDA; }
     if (h_stat[0]) {
         set_error(h_stat[0] & 1u ? "NaN value (an idf entry in use is NaN)"
                   : h_stat[0] & 2u ? "feature index too large (offset + id >= 0x7fffffff)"
                                    : "indices of a row are not strictly ascending (part B's offset does not place it after part A)");
-        return done(GORSE_B200_ERR_ARG);
+        return GORSE_B200_ERR_ARG;
     }
     // the CSR of the non-empty rows
     for (int64_t r = 0; r < n; r++)
         if (out.row_off[(size_t)r + 1] > out.row_off[(size_t)r]) out.off.push_back(out.row_off[(size_t)r + 1]);
     out.n_features = nnz ? h_stat[1] + 1 : 0;
-    return done(GORSE_B200_OK);
+    return GORSE_B200_OK;
 }
 
 int32_t sparse_append(gorse_b200_sparse_index *ix, const SparseRows &rows)
@@ -1030,25 +1024,20 @@ int32_t sparse_append(gorse_b200_sparse_index *ix, const SparseRows &rows)
     if (m == 0) return GORSE_B200_OK;
     if (n + m >= (1ll << 31)) { set_error("more than 2^31 vectors"); return GORSE_B200_ERR_UNSUPPORTED; }
     const uint32_t F = std::max(ix->n_features, rows.n_features);
-    DevBuf<int64_t> off_n, foff_n, d_off;
-    DevBuf<uint32_t> ind_n;
-    DevBuf<float> val_n, fval_n;
-    DevBuf<int32_t> frow_n;
-    auto done = [&](int32_t st) {
-        cudaStreamSynchronize(s);
-        d_off.free();
-        if (st) { off_n.free(); foff_n.free(); ind_n.free(); val_n.free(); fval_n.free(); frow_n.free(); }
-        return st;
-    };
-    int32_t st;
-    if ((st = off_n.alloc((size_t)(n + m + 1))) || (st = ind_n.alloc((size_t)(nnz_old + nnz))) || (st = val_n.alloc((size_t)(nnz_old + nnz))) ||
-        (st = d_off.alloc((size_t)m + 1)))
-        return done(st);
     // the new rows' offsets in the index and on the device; their entries from the staging buffers
     std::vector<int64_t> h_off((size_t)m);
     for (int64_t j = 0; j < m; j++) h_off[(size_t)j] = nnz_old + rows.off[(size_t)j + 1];
     std::vector<uint32_t> h_ind((size_t)nnz);
     std::vector<float> h_val((size_t)nnz);
+    DevBuf<int64_t> off_n, foff_n, d_off;
+    DevBuf<uint32_t> ind_n;
+    DevBuf<float> val_n, fval_n;
+    DevBuf<int32_t> frow_n;
+    StreamSync sync{s};
+    GB_TRY(off_n.alloc((size_t)(n + m + 1)));
+    GB_TRY(ind_n.alloc((size_t)(nnz_old + nnz)));
+    GB_TRY(val_n.alloc((size_t)(nnz_old + nnz)));
+    GB_TRY(d_off.alloc((size_t)m + 1));
     cudaError_t e = cudaMemcpyAsync(d_off.p, rows.off.data(), sizeof(int64_t) * ((size_t)m + 1), cudaMemcpyHostToDevice, s);
     if (e == cudaSuccess) e = cudaMemcpyAsync(off_n.p, ix->off.p, sizeof(int64_t) * (size_t)(n + 1), cudaMemcpyDeviceToDevice, s);
     if (e == cudaSuccess) e = cudaMemcpyAsync(off_n.p + n + 1, h_off.data(), sizeof(int64_t) * (size_t)m, cudaMemcpyHostToDevice, s);
@@ -1058,17 +1047,16 @@ int32_t sparse_append(gorse_b200_sparse_index *ix, const SparseRows &rows)
     if (e == cudaSuccess) e = cudaMemcpyAsync(val_n.p + nnz_old, rows.val.p, sizeof(float) * (size_t)nnz, cudaMemcpyDeviceToDevice, s);
     if (e == cudaSuccess) e = cudaMemcpyAsync(h_ind.data(), rows.ind.p, sizeof(uint32_t) * (size_t)nnz, cudaMemcpyDeviceToHost, s);
     if (e == cudaSuccess) e = cudaMemcpyAsync(h_val.data(), rows.val.p, sizeof(float) * (size_t)nnz, cudaMemcpyDeviceToHost, s);
-    if (e != cudaSuccess) { set_error("sparse append: %s", cudaGetErrorString(e)); return done(GORSE_B200_ERR_CUDA); }
-    if ((st = csc_append(c, d_off.p, rows.ind.p, rows.val.p, m, nnz, n, ix->foff.p, ix->frow.p, ix->fval.p, ix->n_features, nnz_old, F, foff_n,
-                         frow_n, fval_n)))
-        return done(st);   // csc_append synchronised the stream: the host copies are complete
-    ix->off.free(); ix->foff.free(); ix->ind.free(); ix->val.free(); ix->frow.free(); ix->fval.free();
-    ix->off = off_n; ix->foff = foff_n; ix->ind = ind_n; ix->val = val_n; ix->frow = frow_n; ix->fval = fval_n;
+    if (e != cudaSuccess) { set_error("sparse append: %s", cudaGetErrorString(e)); return GORSE_B200_ERR_CUDA; }
+    GB_TRY(csc_append(c, d_off.p, rows.ind.p, rows.val.p, m, nnz, n, ix->foff.p, ix->frow.p, ix->fval.p, ix->n_features, nnz_old, F, foff_n,
+                      frow_n, fval_n));   // csc_append synchronised the stream: the host copies are complete
+    ix->off = std::move(off_n); ix->foff = std::move(foff_n); ix->ind = std::move(ind_n);
+    ix->val = std::move(val_n); ix->frow = std::move(frow_n); ix->fval = std::move(fval_n);
     ix->h_off.insert(ix->h_off.end(), h_off.begin(), h_off.end());
     ix->h_ind.insert(ix->h_ind.end(), h_ind.begin(), h_ind.end());
     ix->h_val.insert(ix->h_val.end(), h_val.begin(), h_val.end());
     ix->n_features = F;
-    return done(GORSE_B200_OK);
+    return GORSE_B200_OK;
 }
 
 int32_t sparse_sync_device(gorse_b200_sparse_index *ix) { return sync_device(ix); }

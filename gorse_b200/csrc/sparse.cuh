@@ -59,12 +59,11 @@ struct SparseRows {
     DevBuf<uint32_t> ind;
     DevBuf<float> val;
     uint32_t n_features = 0;
-    void free() { ind.free(); val.free(); }
 };
 // appendSparseVector of n rows on the device (gorse_b200_vecdb_add_idf_vectors): part A rows a_off[n + 1] / a_ids over
 // a_idf[a_n_idf] at a_offset, then optionally part B (b_off == nullptr: none).  The arguments are checked by the caller except
 // what needs the ids: a used NaN idf, an index >= 0x7fffffff or a row whose B indices do not follow its A indices is
-// GORSE_B200_ERR_ARG.  Nothing but `out` changes; on an error `out` holds no device memory.  The caller holds the device.
+// GORSE_B200_ERR_ARG.  Nothing but `out` changes; on an error the caller discards `out`.  The caller holds the device.
 int32_t sparse_idf_rows(gorse_b200_ctx *c, int64_t n, const int64_t *a_off, const int32_t *a_ids, const float *a_idf, int32_t a_n_idf,
                         uint32_t a_offset, const int64_t *b_off, const int32_t *b_ids, const float *b_idf, int32_t b_n_idf, uint32_t b_offset,
                         SparseRows &out);

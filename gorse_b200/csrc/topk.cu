@@ -304,10 +304,10 @@ int32_t recall_rows(gorse_b200_index *ix, const uint8_t *allow, int64_t nq, cons
         cudaStreamSynchronize(c->copy_stream);
         return s;
     };
-    if ((st = grow(W.q, (size_t)cq * d)) || (st = grow(W.k, (size_t)cq)) || (st = grow(W.ex_off, (size_t)cq + 1)) || (st = grow(W.out_off, (size_t)cq)) ||
-        (st = grow(W.rows, 2 * (size_t)cq)) || (st = grow(W.count, (size_t)nq)) || (st = grow(W.flags, 3)) ||
-        (st = grow(W.slots, (size_t)std::max<int64_t>(total_out, 1))) || (st = grow(W.scores, (size_t)std::max<int64_t>(total_out, 1))) ||
-        (st = grow(W.scratch, (size_t)exact_grid * N)) || (st = grow(W.ex, (size_t)std::max<int64_t>(excl_off ? ex_off[nq] : 0, 1))))
+    if ((st = W.q.grow((size_t)cq * d)) || (st = W.k.grow((size_t)cq)) || (st = W.ex_off.grow((size_t)cq + 1)) || (st = W.out_off.grow((size_t)cq)) ||
+        (st = W.rows.grow(2 * (size_t)cq)) || (st = W.count.grow((size_t)nq)) || (st = W.flags.grow(3)) ||
+        (st = W.slots.grow((size_t)std::max<int64_t>(total_out, 1))) || (st = W.scores.grow((size_t)std::max<int64_t>(total_out, 1))) ||
+        (st = W.scratch.grow((size_t)exact_grid * N)) || (st = W.ex.grow((size_t)std::max<int64_t>(excl_off ? ex_off[nq] : 0, 1))))
         return done(st);
     if (tensor && (st = mma_reserve(ix, cq))) return done(st);
     cudaError_t e = cudaFuncSetAttribute(recall_window_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)window_smem(d));
@@ -462,12 +462,12 @@ static int32_t search_common(gorse_b200_index *ix, const float *h_queries, const
     ScopedDevice sd(ix->ctx->device);
     gorse_b200_ctx *c = ix->ctx;
     DevBuf<int64_t> d_qidx;
-    int32_t st = GORSE_B200_OK;
-    auto done = [&](int32_t s) { cudaStreamSynchronize(c->stream); d_qidx.free(); return s; };
-    if ((st = recall::grow(ix->r_idx, (size_t)nq * k)) || (st = recall::grow(ix->r_dist, (size_t)nq * k)) || (st = recall::grow(ix->r_count, (size_t)nq)))
-        return done(st);
+    StreamSync sync{c->stream};
+    GB_TRY(ix->r_idx.grow((size_t)nq * k));
+    GB_TRY(ix->r_dist.grow((size_t)nq * k));
+    GB_TRY(ix->r_count.grow((size_t)nq));
     if (!h_queries) {   // stored rows: a device slot list
-        if ((st = d_qidx.alloc(nq))) return done(st);
+        GB_TRY(d_qidx.alloc(nq));
         cudaError_t e = cudaSuccess;
         if (h_qidx) e = cudaMemcpyAsync(d_qidx.p, h_qidx, sizeof(int64_t) * nq, cudaMemcpyHostToDevice, c->stream);
         else {
@@ -475,10 +475,10 @@ static int32_t search_common(gorse_b200_index *ix, const float *h_queries, const
             c->launches++;
         }
         if (e == cudaSuccess) e = cudaGetLastError();
-        if (e != cudaSuccess) { set_error("search upload: %s", cudaGetErrorString(e)); return done(GORSE_B200_ERR_CUDA); }
+        if (e != cudaSuccess) { set_error("search upload: %s", cudaGetErrorString(e)); return GORSE_B200_ERR_CUDA; }
     }
     const recall::Table table{ix->r_idx.p, ix->r_dist.p, ix->r_count.p, true, prune0 != 0, idx_out, dist_out, count_out};
-    return done(recall::recall_rows(ix, nullptr, nq, h_queries, d_qidx.p, k, nullptr, nullptr, nullptr, &table, nullptr, nullptr, nullptr, nullptr));
+    return recall::recall_rows(ix, nullptr, nq, h_queries, d_qidx.p, k, nullptr, nullptr, nullptr, &table, nullptr, nullptr, nullptr, nullptr);
 }
 
 // make room for `need` vectors (amortised doubling); the caller holds ix->mu
@@ -491,8 +491,7 @@ int32_t index_reserve(gorse_b200_index *ix, int64_t need)
     GB_TRY(nb.alloc((size_t)ncap * ix->d));
     if (ix->n) GB_CUDA(cudaMemcpyAsync(nb.p, ix->X.p, sizeof(float) * ix->n * ix->d, cudaMemcpyDeviceToDevice, s));
     GB_CUDA(cudaStreamSynchronize(s));
-    ix->X.free();
-    ix->X = nb;
+    ix->X = std::move(nb);
     ix->cap = ncap;
     return GORSE_B200_OK;
 }
@@ -529,11 +528,9 @@ int32_t index_compact(gorse_b200_index *ix, const int64_t *scan, int64_t live)
     if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
     if (e != cudaSuccess) {
         set_error("compact: %s", cudaGetErrorString(e));
-        nx.free();
         return GORSE_B200_ERR_CUDA;
     }
-    ix->X.free();
-    ix->X = nx;
+    ix->X = std::move(nx);
     ix->n = ix->cap = live;
     ix->mma_ready = false;   // the next sweep rebuilds the mirror, norms and permutation for the new n
     ix->Xb.free(); ix->norm.free(); ix->perm.free();
@@ -577,15 +574,8 @@ int32_t gorse_b200_index_destroy(gorse_b200_index *ix)
     if (!ix) return GORSE_B200_OK;
     ScopedDevice sd(ix->ctx->device);
     cudaStreamSynchronize(ix->ctx->stream);
-    ix->X.free();
-    ix->Xb.free();
-    ix->norm.free();
-    ix->perm.free();
     for (cudaEvent_t e : ix->ev)
         if (e) cudaEventDestroy(e);
-    ix->w_qb.free(); ix->w_eps.free(); ix->w_cval.free(); ix->w_theta.free(); ix->w_ccol.free(); ix->w_ccnt.free();
-    ix->recall.free();
-    ix->r_idx.free(); ix->r_count.free(); ix->r_dist.free();
     delete ix;
     return GORSE_B200_OK;
 }
@@ -679,7 +669,7 @@ int32_t gorse_b200_index_stage1_scores(gorse_b200_index *ix, int64_t q0, int64_t
     const int64_t nq = q1 - q0, n_cols = (ix->n + 127) / 128 * 128;
     DevBuf<float> dense;
     int32_t st;
-    auto done = [&](int32_t s) { cudaStreamSynchronize(c->stream); dense.free(); ix->dbg_scores = nullptr; return s; };
+    auto done = [&](int32_t s) { cudaStreamSynchronize(c->stream); ix->dbg_scores = nullptr; return s; };
     if ((st = dense.alloc((size_t)nq * n_cols)) || (st = mma_reserve(ix, nq))) return done(st);
     ix->dbg_scores = dense.p;
     if ((st = mma_sweep(ix, ix->X.p, nullptr, nullptr, q0, nq, mma_sample_tiles(ix, 4.0), nullptr, nullptr))) return done(st);

@@ -15,12 +15,6 @@ struct RecallWork {
     std::vector<int32_t> h_k;
     std::vector<int64_t> h_exoff, h_outoff, h_rows;
     std::vector<int8_t> h_cls;
-    void free()
-    {
-        q.free(); scores.free(); scratch.free();
-        ex_off.free(); ex.free(); out_off.free(); rows.free(); slots.free();
-        k.free(); count.free(); flags.free();
-    }
     size_t bytes() const
     {
         return q.bytes() + scores.bytes() + scratch.bytes() + ex_off.bytes() + ex.bytes() + out_off.bytes() + rows.bytes() + slots.bytes() +

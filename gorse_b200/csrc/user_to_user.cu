@@ -178,8 +178,6 @@ extern "C" int32_t gorse_b200_vecdb_user_to_user(gorse_b200_vecdb *db, int64_t n
                                                  int64_t *items_out, double *scores_out, int32_t *count_out, int64_t *stats_out)
 {
     using namespace gb::u2u;
-    using gb::agg::grow_zeroed;
-    using gb::recall::grow;
     GB_CHECK_ARG(db != nullptr, "collection is NULL");
     GB_CHECK_ARG(n_users >= 0 && n_fb_rows >= 0 && n_items >= 0, "negative count");
     if (stats_out) std::fill(stats_out, stats_out + 4, 0);
@@ -245,7 +243,7 @@ extern "C" int32_t gorse_b200_vecdb_user_to_user(gorse_b200_vecdb *db, int64_t n
         cudaStreamSynchronize(c->copy_stream);
         return s;
     };
-    if ((st = grow(V.nb, (size_t)R)) || (st = grow(V.t_slot, (size_t)R * n)) || (st = grow(V.t_score, (size_t)R * n)) || (st = grow(V.t_cnt, (size_t)R)))
+    if ((st = V.nb.grow((size_t)R)) || (st = V.t_slot.grow((size_t)R * n)) || (st = V.t_score.grow((size_t)R * n)) || (st = V.t_cnt.grow((size_t)R)))
         return done(st);
     cudaError_t e = cudaMemcpyAsync(V.nb.p, nb.data(), sizeof(int64_t) * R, cudaMemcpyHostToDevice, c->stream);
     if (e != cudaSuccess) { set_error("user_to_user upload: %s", cudaGetErrorString(e)); return done(GORSE_B200_ERR_CUDA); }
@@ -258,11 +256,11 @@ extern "C" int32_t gorse_b200_vecdb_user_to_user(gorse_b200_vecdb *db, int64_t n
     // ---- the feedback rows and the item filter, once per call
     const int64_t cu = std::min<int64_t>(n_users, (int64_t)c->sm_count * 1024);
     const int64_t n_chunks = (n_users + cu - 1) / cu;
-    if ((st = grow(V.fb_off, (size_t)n_fb_rows + 1)) || (st = grow(V.fb_items, (size_t)std::max<int64_t>(n_fb, 1))) ||
-        (st = grow(V.item_ok, (size_t)std::max<int32_t>(n_items, 1))) || (st = grow(V.q_row, (size_t)cu)) ||
-        (st = grow(V.ex_off, (size_t)cu + 1)) || (st = grow(V.ex, std::max<size_t>(ex.size(), 1))) || (st = grow(V.list, (size_t)cu)) ||
-        (st = grow(V.work, (size_t)cu)) || (st = grow(V.route_cnt, (size_t)n_chunks * 2)) || (st = grow(V.items, (size_t)n_users * n)) ||
-        (st = grow(V.scores, (size_t)n_users * n)) || (st = grow(V.count, (size_t)n_users)))
+    if ((st = V.fb_off.grow((size_t)n_fb_rows + 1)) || (st = V.fb_items.grow((size_t)std::max<int64_t>(n_fb, 1))) ||
+        (st = V.item_ok.grow((size_t)std::max<int32_t>(n_items, 1))) || (st = V.q_row.grow((size_t)cu)) ||
+        (st = V.ex_off.grow((size_t)cu + 1)) || (st = V.ex.grow(std::max<size_t>(ex.size(), 1))) || (st = V.list.grow((size_t)cu)) ||
+        (st = V.work.grow((size_t)cu)) || (st = V.route_cnt.grow((size_t)n_chunks * 2)) || (st = V.items.grow((size_t)n_users * n)) ||
+        (st = V.scores.grow((size_t)n_users * n)) || (st = V.count.grow((size_t)n_users)))
         return done(st);
     if ((n_fb_rows && (e = cudaMemcpyAsync(V.fb_off.p, fb_off, sizeof(int64_t) * (n_fb_rows + 1), cudaMemcpyHostToDevice, c->stream)) != cudaSuccess) ||
         (n_fb && (e = cudaMemcpyAsync(V.fb_items.p, fb_items, sizeof(int32_t) * n_fb, cudaMemcpyHostToDevice, c->stream)) != cudaSuccess) ||
@@ -276,8 +274,8 @@ extern "C" int32_t gorse_b200_vecdb_user_to_user(gorse_b200_vecdb *db, int64_t n
     // global accumulators: one [n_items] float64 row, flag row and item list per CTA, at most 512 MB
     const int64_t NI = std::max<int64_t>(n_items, 1);
     const int hg = heavy_grid(c, NI, ROW_BYTES);
-    if (heavy_possible && ((st = grow_zeroed(V.acc, (size_t)hg * NI, c->stream)) || (st = grow_zeroed(V.flag, (size_t)hg * NI, c->stream)) ||
-                           (st = grow(V.touched, (size_t)hg * NI))))
+    if (heavy_possible && ((st = V.acc.grow_zeroed((size_t)hg * NI, c->stream)) || (st = V.flag.grow_zeroed((size_t)hg * NI, c->stream)) ||
+                           (st = V.touched.grow((size_t)hg * NI))))
         return done(st);
     const NeighbourTable T{V.t_slot.p, V.t_score.p, V.t_cnt.p};
     Feedback F;

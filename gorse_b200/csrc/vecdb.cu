@@ -100,9 +100,9 @@ int32_t vecdb_live_scan(gorse_b200_vecdb *db, DevBuf<int64_t> &scan, int64_t *ne
     gorse_b200_ctx *c = db->ctx;
     const int64_t n = (int64_t)db->ts.size();
     DevBuf<uint8_t> d_dead, tmp;
-    auto done = [&](int32_t st) { cudaStreamSynchronize(c->stream); d_dead.free(); tmp.free(); if (st) scan.free(); return st; };
-    int32_t st;
-    if ((st = d_dead.alloc((size_t)n)) || (st = scan.alloc((size_t)n + 1))) return done(st);
+    StreamSync sync{c->stream};
+    GB_TRY(d_dead.alloc((size_t)n));
+    GB_TRY(scan.alloc((size_t)n + 1));
     size_t tmp_bytes = 0;
     cudaError_t e = n ? cudaMemcpyAsync(d_dead.p, db->dead.data(), (size_t)n, cudaMemcpyHostToDevice, c->stream) : cudaSuccess;
     if (e == cudaSuccess) {
@@ -111,13 +111,13 @@ int32_t vecdb_live_scan(gorse_b200_vecdb *db, DevBuf<int64_t> &scan, int64_t *ne
         e = cudaGetLastError();
     }
     if (e == cudaSuccess) e = cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, scan.p, n + 1, c->stream);
-    if (e != cudaSuccess) { set_error("live scan: %s", cudaGetErrorString(e)); return done(GORSE_B200_ERR_CUDA); }
-    if ((st = tmp.alloc(tmp_bytes))) return done(st);
+    if (e != cudaSuccess) { set_error("live scan: %s", cudaGetErrorString(e)); return GORSE_B200_ERR_CUDA; }
+    GB_TRY(tmp.alloc(tmp_bytes));
     e = cub::DeviceScan::ExclusiveSum(tmp.p, tmp_bytes, scan.p, n + 1, c->stream);
     if (e == cudaSuccess && new_slot) e = cudaMemcpyAsync(new_slot, scan.p, sizeof(int64_t) * ((size_t)n + 1), cudaMemcpyDeviceToHost, c->stream);
     if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
-    if (e != cudaSuccess) { set_error("live scan: %s", cudaGetErrorString(e)); return done(GORSE_B200_ERR_CUDA); }
-    return done(GORSE_B200_OK);
+    if (e != cudaSuccess) { set_error("live scan: %s", cudaGetErrorString(e)); return GORSE_B200_ERR_CUDA; }
+    return GORSE_B200_OK;
 }
 
 int32_t vecdb_allow(gorse_b200_vecdb *db, const int32_t *categories, int32_t n_categories)
@@ -166,13 +166,8 @@ int32_t gorse_b200_vecdb_create(gorse_b200_ctx *ctx, int32_t dim, int32_t distan
 int32_t gorse_b200_vecdb_destroy(gorse_b200_vecdb *db)
 {
     if (!db) return GORSE_B200_OK;
-    {
-        ScopedDevice sd(db->ctx->device);
-        cudaStreamSynchronize(db->ctx->stream);
-        db->d_blocked.free(); db->d_allow.free(); db->d_cat_off.free(); db->d_cats.free(); db->d_want.free();
-        db->i2i.free();
-        db->u2u.free();
-    }
+    ScopedDevice sd(db->ctx->device);
+    cudaStreamSynchronize(db->ctx->stream);
     gorse_b200_index_destroy(db->dense);
     gorse_b200_sparse_index_destroy(db->sparse);
     delete db;
@@ -266,14 +261,11 @@ int32_t gorse_b200_vecdb_add_idf_vectors(gorse_b200_vecdb *db, int64_t n, const 
         const bool add = rows.row_off[(size_t)i + 1] > rows.row_off[(size_t)i];
         slot[(size_t)i] = add ? first + added++ : -1;
         if (add && replace && replace[i] >= first) {
-            rows.free();
             set_error("replace[%lld] = %lld is not an existing slot", (long long)i, (long long)replace[i]);
             return GORSE_B200_ERR_ARG;
         }
     }
-    const int32_t st = sparse_append(db->sparse, rows);
-    rows.free();
-    if (st) return st;
+    GB_TRY(sparse_append(db->sparse, rows));
     for (int64_t i = 0; i < n; i++) {
         slot_out[i] = slot[(size_t)i];
         if (slot[(size_t)i] < 0) continue;
@@ -364,11 +356,10 @@ int32_t gorse_b200_vecdb_compact(gorse_b200_vecdb *db, int64_t *new_slot_out, in
     }
     gorse_b200_ctx *c = db->ctx;
     ScopedDevice sd(c->device);
-    DevBuf<int64_t> scan;
-    auto done = [&](int32_t st) { cudaStreamSynchronize(c->stream); scan.free(); return st; };
-    int32_t st;
     std::vector<int64_t> new_slot((size_t)n + 1);
-    if ((st = vecdb_live_scan(db, scan, new_slot.data()))) return done(st);
+    DevBuf<int64_t> scan;
+    StreamSync sync{c->stream};
+    GB_TRY(vecdb_live_scan(db, scan, new_slot.data()));
     // the compacted host metadata
     std::vector<uint8_t> hidden((size_t)live), dead((size_t)live, 0);
     std::vector<int64_t> ts((size_t)live), cat_off((size_t)live + 1, 0);
@@ -382,7 +373,7 @@ int32_t gorse_b200_vecdb_compact(gorse_b200_vecdb *db, int64_t *new_slot_out, in
         cats.insert(cats.end(), db->cats.begin() + db->cat_off[(size_t)s], db->cats.begin() + db->cat_off[(size_t)s + 1]);
         cat_off[to + 1] = (int64_t)cats.size();
     }
-    if ((st = db->dense ? index_compact(db->dense, scan.p, live) : sparse_compact(db->sparse, scan.p, live))) return done(st);
+    GB_TRY(db->dense ? index_compact(db->dense, scan.p, live) : sparse_compact(db->sparse, scan.p, live));
     db->hidden.swap(hidden); db->dead.swap(dead); db->ts.swap(ts); db->cat_off.swap(cat_off); db->cats.swap(cats);
     db->meta_dirty = true;
     // every device buffer whose size follows the slot count; the next call that needs one allocates (and zeroes) it again
@@ -392,7 +383,7 @@ int32_t gorse_b200_vecdb_compact(gorse_b200_vecdb *db, int64_t *new_slot_out, in
     if (new_slot_out)   // `dead` holds the old flags after the swap
         for (int64_t s = 0; s < n; s++) new_slot_out[s] = dead[(size_t)s] ? -1 : new_slot[(size_t)s];
     if (bytes_out) bytes_out[1] = vecdb_bytes(db);
-    return done(GORSE_B200_OK);
+    return GORSE_B200_OK;
 }
 
 int32_t gorse_b200_vecdb_query(gorse_b200_vecdb *db, int64_t nq, const float *q_values, const int64_t *q_sp_off, const uint32_t *q_sp_indices,
@@ -462,33 +453,31 @@ int32_t gorse_b200_vecdb_add_item_factors(gorse_b200_vecdb *db, gorse_b200_cf *c
     gorse_b200_ctx *c = db->ctx;
     ScopedDevice sd(c->device);
     const int32_t I = cf->n_items;
+    std::vector<int32_t> flag((size_t)I), items;
     DevBuf<int32_t> d_flag, d_items;
-    auto done = [&](int32_t s) { cudaStreamSynchronize(c->stream); d_flag.free(); d_items.free(); return s; };
-    int32_t st;
-    if ((st = d_flag.alloc((size_t)std::max(I, 1)))) return done(st);
+    StreamSync sync{c->stream};
+    GB_TRY(d_flag.alloc((size_t)std::max(I, 1)));
     cudaError_t e = cudaMemsetAsync(d_flag.p, 0, sizeof(int32_t) * (size_t)std::max(I, 1), c->stream);
     if (e == cudaSuccess && cf->n_feedback > 0) {
         vecdb_mark_items_kernel<<<c->sm_count * 4, 256, 0, c->stream>>>(cf->user_items.p, cf->n_feedback, d_flag.p);
         c->launches++;
         e = cudaGetLastError();
     }
-    std::vector<int32_t> flag((size_t)I);
     if (e == cudaSuccess && I) e = cudaMemcpyAsync(flag.data(), d_flag.p, sizeof(int32_t) * (size_t)I, cudaMemcpyDeviceToHost, c->stream);
     if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
-    if (e != cudaSuccess) { set_error("add_item_factors: %s", cudaGetErrorString(e)); return done(GORSE_B200_ERR_CUDA); }
-    std::vector<int32_t> items;
+    if (e != cudaSuccess) { set_error("add_item_factors: %s", cudaGetErrorString(e)); return GORSE_B200_ERR_CUDA; }
     const int64_t first = (int64_t)db->ts.size();
     for (int32_t i = 0; i < I; i++) {
         if (slot_of_item_out) slot_of_item_out[i] = flag[(size_t)i] ? first + (int64_t)items.size() : -1;
         if (flag[(size_t)i]) items.push_back(i);
     }
     const int64_t n = (int64_t)items.size();
-    if (n == 0) return done(GORSE_B200_OK);
+    if (n == 0) return GORSE_B200_OK;
     gorse_b200_index *ix = db->dense;
     {
         std::lock_guard<std::mutex> lk2(ix->mu);
-        if ((st = index_reserve(ix, ix->n + n))) return done(st);
-        if ((st = d_items.alloc((size_t)n))) return done(st);
+        GB_TRY(index_reserve(ix, ix->n + n));
+        GB_TRY(d_items.alloc((size_t)n));
         e = cudaMemcpyAsync(d_items.p, items.data(), sizeof(int32_t) * (size_t)n, cudaMemcpyHostToDevice, c->stream);
         if (e == cudaSuccess) {
             if (cf->d % 4 == 0) vecdb_copy_rows_kernel<<<c->sm_count * 8, 256, 0, c->stream>>>(cf->Q.p, cf->d / 4, d_items.p, n, ix->X.p + ix->n * ix->d);
@@ -498,7 +487,7 @@ int32_t gorse_b200_vecdb_add_item_factors(gorse_b200_vecdb *db, gorse_b200_cf *c
             if (e == cudaSuccess) e = cudaGetLastError();
         }
         if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
-        if (e != cudaSuccess) { set_error("add_item_factors: %s", cudaGetErrorString(e)); return done(GORSE_B200_ERR_CUDA); }
+        if (e != cudaSuccess) { set_error("add_item_factors: %s", cudaGetErrorString(e)); return GORSE_B200_ERR_CUDA; }
         ix->n += n;
         ix->mma_ready = false;
     }
@@ -512,7 +501,7 @@ int32_t gorse_b200_vecdb_add_item_factors(gorse_b200_vecdb *db, gorse_b200_cf *c
         db->live++;
     }
     db->meta_dirty = true;
-    return done(GORSE_B200_OK);
+    return GORSE_B200_OK;
 }
 
 }  // extern "C"

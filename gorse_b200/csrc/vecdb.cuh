@@ -14,12 +14,6 @@ struct ItemToItemWork {
     DevBuf<double> scores, acc;
     DevBuf<uint8_t> seen, item_ok;
     DevBuf<int32_t> touched;
-    void free()
-    {
-        nb.free(); c_off.free(); ex_off.free(); ex.free(); slots.free();
-        t_slot.free(); t_cnt.free(); c_row.free(); users.free(); count.free();
-        t_score.free(); scores.free(); acc.free(); seen.free(); item_ok.free(); touched.free();
-    }
     size_t bytes() const
     {
         return nb.bytes() + c_off.bytes() + ex_off.bytes() + ex.bytes() + slots.bytes() + t_slot.bytes() + t_cnt.bytes() + c_row.bytes() +
@@ -35,12 +29,6 @@ struct UserToUserWork {
     DevBuf<uint8_t> item_ok;
     DevBuf<float> t_score;
     DevBuf<double> scores, acc;
-    void free()
-    {
-        nb.free(); fb_off.free(); ex_off.free(); ex.free(); items.free();
-        t_slot.free(); t_cnt.free(); fb_items.free(); q_row.free(); list.free(); work.free(); route_cnt.free(); count.free(); flag.free(); touched.free();
-        item_ok.free(); t_score.free(); scores.free(); acc.free();
-    }
     size_t bytes() const
     {
         return nb.bytes() + fb_off.bytes() + ex_off.bytes() + ex.bytes() + items.bytes() + t_slot.bytes() + t_cnt.bytes() + fb_items.bytes() +
@@ -75,6 +63,6 @@ namespace gb {
 int32_t vecdb_allow(gorse_b200_vecdb *db, const int32_t *categories, int32_t n_categories);
 // the renumbering of compaction and snapshots: scan[slots + 1] (device, allocated here) = the exclusive sum of the live flags,
 // so slot s is live iff scan[s + 1] != scan[s] and then moves to scan[s]; new_slot[slots + 1] (host, may be nullptr) receives
-// a copy.  Ends with the stream synchronised; on an error scan holds no memory.  The caller holds db->mu and the device.
+// a copy.  Ends with the stream synchronised.  The caller holds db->mu and the device.
 int32_t vecdb_live_scan(gorse_b200_vecdb *db, DevBuf<int64_t> &scan, int64_t *new_slot);
 }  // namespace gb

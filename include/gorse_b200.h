@@ -72,6 +72,8 @@ int32_t gorse_b200_ctx_rank(const gorse_b200_ctx *ctx, int32_t *rank, int32_t *w
 int32_t gorse_b200_ctx_timer_begin(gorse_b200_ctx *ctx);
 int32_t gorse_b200_ctx_timer_end(gorse_b200_ctx *ctx, float *ms_out); /* records, syncs, returns elapsed */
 int32_t gorse_b200_ctx_launch_count(const gorse_b200_ctx *ctx, int64_t *count);
+/* device bytes held by all of this library's buffers in the process (every context and handle); needs no device */
+int32_t gorse_b200_device_bytes(int64_t *bytes);
 int32_t gorse_b200_ctx_flush_l2(gorse_b200_ctx *ctx); /* writes a buffer larger than L2 */
 int32_t gorse_b200_ctx_barrier(gorse_b200_ctx *ctx);  /* NCCL barrier across ranks (no-op for world 1) */
 /* page-locked host memory for the shim's flat factor mirror (SURVEY 8b "ownership"): factor uploads and
