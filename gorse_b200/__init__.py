@@ -526,6 +526,13 @@ class VectorCollection:
         check(lib.gorse_b200_vecdb_compact(self.h, ptr(new_slot), ptr(nbytes)))
         return new_slot[:slots], int(nbytes[0]), int(nbytes[1])
 
+    def storage(self):
+        """How the rows are stored (gorse_b200_vecdb_storage): bf16 while every value added is bf16-exact, fp32 after the first
+        that is not.  -> (value_bytes: 0 sparse, 2 bf16, 4 fp32; device bytes held, as compact() counts them)"""
+        vb, nbytes = C.c_int32(0), C.c_int64(0)
+        check(lib.gorse_b200_vecdb_storage(self.h, C.byref(vb), C.byref(nbytes)))
+        return vb.value, nbytes.value
+
     def save(self, fileobj):
         """Write the collection to a binary file object as a snapshot stream (gorse_b200_vecdb_save; the format is in
         include/gorse_b200.h).  The collection does not change.

@@ -194,21 +194,64 @@ __device__ __forceinline__ float quad_dot_global(const float *a, const float *b,
     return quad_tree(acc, mask);
 }
 
+// value i of a row: fp32, or bf16 kept as the high 16 bits of the fp32 pattern (a vector collection's rows, topk.cuh), widened
+// exactly by a shift
+template <typename I>
+__device__ __forceinline__ float row_val(const float *x, I i) { return x[i]; }
+template <typename I>
+__device__ __forceinline__ float row_val(const uint16_t *x, I i) { return __uint_as_float((uint32_t)__ldg(x + i) << 16); }
+
 // floats.Dot for any d, one thread, the reference's order: 16-lane body, 8-lane block, fused scalar tail
-// (common/floats/src/floats_avx512.c:306-367 and the committed assembly for which parts fuse)
-__device__ inline float dot_any(const float *a, const float *b, int n)
+// (common/floats/src/floats_avx512.c:306-367 and the committed assembly for which parts fuse).  TA, TB: float, or uint16_t for
+// bf16 rows (row_val).
+// values 0 .. 15 of a bf16 row chunk, widened: four 8-byte loads when the chunk is 8-byte aligned (d % 4 == 0), else 16
+// 2-byte loads.  The one-thread scans (dot_any, dist_any) read bf16 rows through it, so that a value costs fewer load
+// instructions than an fp32 value does.
+__device__ __forceinline__ void row_chunk16(const uint16_t *p, float (&v)[16])
+{
+    if ((reinterpret_cast<uintptr_t>(p) & 7u) == 0) {
+#pragma unroll
+        for (int i = 0; i < 4; i++) {
+            const uint2 u = __ldg(reinterpret_cast<const uint2 *>(p) + i);
+            v[4 * i] = __uint_as_float(u.x << 16);
+            v[4 * i + 1] = __uint_as_float(u.x & 0xffff0000u);
+            v[4 * i + 2] = __uint_as_float(u.y << 16);
+            v[4 * i + 3] = __uint_as_float(u.y & 0xffff0000u);
+        }
+    } else {
+#pragma unroll
+        for (int l = 0; l < 16; l++) v[l] = row_val(p, l);
+    }
+}
+
+template <typename TA, typename TB>
+__device__ inline float dot_any(const TA *a, const TB *b, int n)
 {
     int epoch = n / 16, remain = n % 16;
     float s[16];
 #pragma unroll
     for (int l = 0; l < 16; l++) s[l] = 0.f;
-    if (epoch > 0) {
+    if constexpr (std::is_same<TA, float>::value && std::is_same<TB, uint16_t>::value) {   // a bf16 row against an fp32 query
+        float bv[16];
+        if (epoch > 0) {
+            row_chunk16(b, bv);
 #pragma unroll
-        for (int l = 0; l < 16; l++) s[l] = __fmul_rn(a[l], b[l]);
-    }
-    for (int c = 1; c < epoch; c++) {
+            for (int l = 0; l < 16; l++) s[l] = __fmul_rn(a[l], bv[l]);
+        }
+        for (int c = 1; c < epoch; c++) {
+            row_chunk16(b + 16 * c, bv);
 #pragma unroll
-        for (int l = 0; l < 16; l++) s[l] = __fmaf_rn(a[16 * c + l], b[16 * c + l], s[l]);
+            for (int l = 0; l < 16; l++) s[l] = __fmaf_rn(a[16 * c + l], bv[l], s[l]);
+        }
+    } else {
+        if (epoch > 0) {
+#pragma unroll
+            for (int l = 0; l < 16; l++) s[l] = __fmul_rn(row_val(a, l), row_val(b, l));
+        }
+        for (int c = 1; c < epoch; c++) {
+#pragma unroll
+            for (int l = 0; l < 16; l++) s[l] = __fmaf_rn(row_val(a, 16 * c + l), row_val(b, 16 * c + l), s[l]);
+        }
     }
     float r4[4];
 #pragma unroll
@@ -219,13 +262,13 @@ __device__ inline float dot_any(const float *a, const float *b, int n)
     if (remain >= 8) {
         float q4[4];
 #pragma unroll
-        for (int l = 0; l < 4; l++) q4[l] = __fadd_rn(__fmul_rn(a[l + 4], b[l + 4]), __fmul_rn(a[l], b[l]));
+        for (int l = 0; l < 4; l++) q4[l] = __fadd_rn(__fmul_rn(row_val(a, l + 4), row_val(b, l + 4)), __fmul_rn(row_val(a, l), row_val(b, l)));
         sum = __fadd_rn(sum, __fadd_rn(__fadd_rn(q4[0], q4[2]), __fadd_rn(q4[1], q4[3])));
         a += 8;
         b += 8;
         remain -= 8;
     }
-    for (int i = 0; i < remain; i++) sum = __fmaf_rn(a[i], b[i], sum);
+    for (int i = 0; i < remain; i++) sum = __fmaf_rn(row_val(a, i), row_val(b, i), sum);
     return sum;
 }
 

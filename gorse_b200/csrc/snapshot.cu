@@ -32,9 +32,9 @@ static_assert(sizeof(Header) == 48, "the stream header is 48 bytes without paddi
 
 // out[(j - j0) * d ..] = X[slot(j) * d ..] for the live rows j in [j0, j0 + m): slot(j) is the slot whose scan entry is j and
 // whose successor's is j + 1, found by a binary search of scan[0 .. n] (scan[n] = the live count).  One warp per row;
-// V = float4 when d % 4 == 0 (dv = d / 4), else float (dv = d).
-template <typename V>
-__global__ void snapshot_gather_kernel(const V *X, int dv, const int64_t *scan, int64_t n, int64_t j0, int64_t m, V *out)
+// V = float4 when d % 4 == 0 (dv = d / 4), else float (dv = d); bf16 rows (V = uint2 / uint16_t) are widened to W on the way.
+template <typename V, typename W>
+__global__ void snapshot_gather_kernel(const V *X, int dv, const int64_t *scan, int64_t n, int64_t j0, int64_t m, W *out)
 {
     const int lane = threadIdx.x & 31;
     const int64_t nw = ((int64_t)gridDim.x * blockDim.x) >> 5;
@@ -47,8 +47,8 @@ __global__ void snapshot_gather_kernel(const V *X, int dv, const int64_t *scan, 
             else hi = mid;
         }
         const V *src = X + lo * dv;
-        V *dst = out + r * dv;
-        for (int c = lane; c < dv; c += 32) dst[c] = src[c];
+        W *dst = out + r * dv;
+        for (int c = lane; c < dv; c += 32) dst[c] = widen(src[c]);
     }
 }
 
@@ -58,6 +58,7 @@ struct Staging {
     void *h[2] = {nullptr, nullptr};
     DevBuf<float> d[2];
     cudaEvent_t gathered[2] = {nullptr, nullptr}, copied[2] = {nullptr, nullptr};
+    int32_t *flag = nullptr;   // [2] pinned: load's inexact flag of the chunk in each buffer
     int32_t alloc(gorse_b200_ctx *ctx, int64_t bytes, int buffers, bool device)
     {
         c = ctx;
@@ -67,6 +68,10 @@ struct Staging {
             if (!device) continue;
             GB_TRY(d[b].alloc((size_t)bytes / sizeof(float)));
             GB_CUDA(cudaEventCreateWithFlags(&gathered[b], cudaEventDisableTiming));
+        }
+        if (device) {
+            GB_CUDA(cudaHostAlloc((void **)&flag, 2 * sizeof(int32_t), cudaHostAllocDefault));
+            flag[0] = flag[1] = 0;   // pinned memory comes back uninitialised
         }
         return GORSE_B200_OK;
     }
@@ -80,6 +85,7 @@ struct Staging {
             if (gathered[b]) cudaEventDestroy(gathered[b]);
             if (copied[b]) cudaEventDestroy(copied[b]);
         }
+        if (flag) cudaFreeHost(flag);
     }
 };
 
@@ -240,11 +246,14 @@ int32_t save(gorse_b200_vecdb *db, gorse_b200_write_fn write, void *user, int64_
             const int b = (int)(k & 1);
             const int64_t j0 = k * R, m = std::min(R, live - j0);
             const unsigned grid = (unsigned)std::min<int64_t>((m + 7) / 8, (int64_t)c->sm_count * 16);
-            if (dim % 4 == 0)
-                snapshot_gather_kernel<<<grid, 256, 0, c->stream>>>(reinterpret_cast<const float4 *>(ix->X.p), (int)(dim / 4), scan.p, n, j0, m,
-                                                                   reinterpret_cast<float4 *>(stg.d[b].p));
-            else
-                snapshot_gather_kernel<<<grid, 256, 0, c->stream>>>(ix->X.p, (int)dim, scan.p, n, j0, m, stg.d[b].p);
+            with_rows(ix->rows(), [&](auto x) {   // the stream holds fp32 values: bf16 rows are widened by the gather
+                using Q = typename row_quad_type<row_elem_t<decltype(x)>>::type;
+                if (dim % 4 == 0)
+                    snapshot_gather_kernel<<<grid, 256, 0, c->stream>>>(reinterpret_cast<const Q *>(x), (int)(dim / 4), scan.p, n, j0, m,
+                                                                       reinterpret_cast<float4 *>(stg.d[b].p));
+                else
+                    snapshot_gather_kernel<<<grid, 256, 0, c->stream>>>(x, (int)dim, scan.p, n, j0, m, stg.d[b].p);
+            });
             c->launches++;
             cudaError_t e = cudaGetLastError();
             if (e == cudaSuccess) e = cudaEventRecord(stg.gathered[b], c->stream);
@@ -346,23 +355,45 @@ int32_t load(gorse_b200_ctx *ctx, gorse_b200_read_fn read, void *user, gorse_b20
             sx->dirty = true;
             st = sparse_sync_device(sx);
         } else if (n > 0) {
-            // chunk k = rows [k R, k R + R): read into h[k & 1] while chunk k - 1 is copied into X on the copy stream
+            // chunk k = rows [k R, k R + R): read into h[k & 1] while chunk k - 1 is copied on the copy stream.  While the
+            // collection is bf16 a chunk goes through the device buffer d[k & 1] and is narrowed into the rows there; its inexact
+            // flag comes back with it and is read when its buffers are reused (or at the end).  The first chunk k0 that was not
+            // bf16-exact promotes the collection: the rows before it are widened, and chunk k0 and the one after it, whose fp32
+            // values are still in the device buffers, are copied in; later chunks go straight into the fp32 rows.
             gorse_b200_index *ix = db->dense;
             Staging stg;
             const int64_t cap = std::min(STAGE_BYTES, std::max(MIN_STAGE_BYTES, 4 * n * dim));
             st = index_reserve(ix, n);
-            if (st == GORSE_B200_OK) st = stg.alloc(ctx, cap, 2, false);
+            if (st == GORSE_B200_OK) st = stg.alloc(ctx, cap, 2, ix->value_bytes == 2);
+            if (st == GORSE_B200_OK) st = ix->inexact.grow(2);
             const int64_t R = cap / (4 * dim), chunks = st ? 0 : (n + R - 1) / R;
+            auto rows_of = [&](int64_t k) { return std::min(R, n - k * R); };
             cudaError_t e = cudaSuccess;
+            auto promote_at = [&](int64_t k0, int64_t k1) {   // chunks [k0, k1) were narrowed; k0 was not exact
+                e = cudaStreamSynchronize(ctx->copy_stream);
+                if (e == cudaSuccess) st = index_promote(ix, k0 * R);
+                for (int64_t k = k0; k < k1 && e == cudaSuccess && st == GORSE_B200_OK; k++)
+                    e = cudaMemcpyAsync(ix->X.p + k * R * dim, stg.d[k & 1].p, sizeof(float) * rows_of(k) * dim, cudaMemcpyDeviceToDevice, ctx->copy_stream);
+            };
             for (int64_t k = 0; k < chunks && e == cudaSuccess && st == GORSE_B200_OK; k++) {
                 const int b = (int)(k & 1);
-                const int64_t j0 = k * R, bytes = 4 * std::min(R, n - j0) * dim;
+                const int64_t j0 = k * R, bytes = 4 * rows_of(k) * dim;
                 if (k >= 2) e = cudaEventSynchronize(stg.copied[b]);
-                if (e == cudaSuccess) st = r.get(stg.h[b], bytes, "values");
-                if (e == cudaSuccess && st == GORSE_B200_OK)
+                if (e == cudaSuccess && k >= 2 && ix->value_bytes == 2 && stg.flag[b]) promote_at(k - 2, k);   // chunk k - 2's flag
+                if (e == cudaSuccess && st == GORSE_B200_OK) st = r.get(stg.h[b], bytes, "values");
+                if (e != cudaSuccess || st != GORSE_B200_OK) break;
+                if (ix->value_bytes == 2) {
+                    e = cudaMemcpyAsync(stg.d[b].p, stg.h[b], (size_t)bytes, cudaMemcpyHostToDevice, ctx->copy_stream);
+                    if (e == cudaSuccess) e = cudaMemsetAsync(ix->inexact.p + b, 0, sizeof(int32_t), ctx->copy_stream);
+                    if (e == cudaSuccess) e = index_narrow((int)dim, ctx, ctx->copy_stream, stg.d[b].p, nullptr, rows_of(k), ix->Xh.p + j0 * dim, ix->inexact.p + b);
+                    if (e == cudaSuccess) e = cudaMemcpyAsync(stg.flag + b, ix->inexact.p + b, sizeof(int32_t), cudaMemcpyDeviceToHost, ctx->copy_stream);
+                } else
                     e = cudaMemcpyAsync(ix->X.p + j0 * dim, stg.h[b], (size_t)bytes, cudaMemcpyHostToDevice, ctx->copy_stream);
-                if (e == cudaSuccess && st == GORSE_B200_OK) e = cudaEventRecord(stg.copied[b], ctx->copy_stream);
+                if (e == cudaSuccess) e = cudaEventRecord(stg.copied[b], ctx->copy_stream);
             }
+            if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->copy_stream);
+            for (int64_t k = std::max<int64_t>(0, chunks - 2); k < chunks && e == cudaSuccess && st == GORSE_B200_OK; k++)
+                if (ix->value_bytes == 2 && stg.flag[k & 1]) promote_at(k, chunks);
             if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->copy_stream);
             if (e != cudaSuccess && st == GORSE_B200_OK) {
                 set_error("snapshot load: %s", cudaGetErrorString(e));

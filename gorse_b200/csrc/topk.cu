@@ -72,9 +72,9 @@ __device__ void block_emit(const uint64_t *key, const float *val, int m, const i
 }
 
 // score = -distance in the reference's arithmetic for count vectors: slot_at(j) < 0 skips entry j.
-// put(j, score, valid) is called once per entry.
-template <int NT, typename SlotAt, typename Put>
-__device__ __forceinline__ void block_score(const float *X, int d, int metric, const float *qs, float qq, int64_t count, SlotAt slot_at, Put put)
+// put(j, score, valid) is called once per entry.  T: the element type of the stored rows (float, or uint16_t for bf16).
+template <int NT, typename T, typename SlotAt, typename Put>
+__device__ __forceinline__ void block_score(const T *X, int d, int metric, const float *qs, float qq, int64_t count, SlotAt slot_at, Put put)
 {
     if (d % 16 == 0 && d <= 256) {
         const int lane4 = threadIdx.x & 3, chunks = d / 16;
@@ -106,9 +106,10 @@ __device__ __forceinline__ float load_query(const float *q, int d, int metric, f
 }
 
 // ---- stage 2: one CTA per row of a class (rows[i] = chunk-local row; candidate list i belongs to it) ------------------------
+template <typename T>
 __global__ void __launch_bounds__(WIN_THREADS)
 recall_window_kernel(const int32_t *cand_col, const float *cand_val, const int32_t *cand_cnt, const float *theta, const float *eps,
-                     const int32_t *perm, const uint8_t *allow, const float *X, int d, int metric, const int64_t *rows, int64_t n_rows,
+                     const int32_t *perm, const uint8_t *allow, const T *X, int d, int metric, const int64_t *rows, int64_t n_rows,
                      RowInfo R)
 {
     constexpr int NT = WIN_THREADS;
@@ -198,8 +199,9 @@ recall_window_kernel(const int32_t *cand_col, const float *cand_val, const int32
 }
 
 // ---- exact path: one CTA per row of R.exact; sc = this CTA's [N] score scratch ---------------------------------------------
+template <typename T>
 __global__ void __launch_bounds__(EXACT_THREADS)
-recall_exact_kernel(const float *X, int64_t N, int d, int metric, const uint8_t *allow, RowInfo R, float *scratch)
+recall_exact_kernel(const T *X, int64_t N, int d, int metric, const uint8_t *allow, RowInfo R, float *scratch)
 {
     constexpr int NT = EXACT_THREADS;
     extern __shared__ __align__(16) uint8_t sm[];
@@ -266,11 +268,12 @@ __global__ void range_slots_kernel(int64_t *slots, int64_t rows, int64_t q0)
     if (r < rows) slots[r] = q0 + r;
 }
 
-// q[r] = X[slots[r]]: the query rows of stored vectors, one CTA per row
-__global__ void recall_gather_kernel(const float *X, int d, const int64_t *slots, int64_t rows, float *q)
+// q[r] = X[slots[r]]: the query rows of stored vectors (fp32 values), one CTA per row
+template <typename T>
+__global__ void recall_gather_kernel(const T *X, int d, const int64_t *slots, int64_t rows, float *q)
 {
     for (int64_t r = blockIdx.x; r < rows; r += gridDim.x)
-        for (int e = threadIdx.x; e < d; e += blockDim.x) q[r * d + e] = X[slots[r] * d + e];
+        for (int e = threadIdx.x; e < d; e += blockDim.x) q[r * d + e] = row_val(X, slots[r] * d + e);
 }
 
 // the row tables of a chunk without exclusions: k = n, answers at q * n, one class in row order
@@ -310,8 +313,13 @@ int32_t recall_rows(gorse_b200_index *ix, const uint8_t *allow, int64_t nq, cons
         (st = W.scratch.grow((size_t)exact_grid * N)) || (st = W.ex.grow((size_t)std::max<int64_t>(excl_off ? ex_off[nq] : 0, 1))))
         return done(st);
     if (tensor && (st = mma_reserve(ix, cq))) return done(st);
-    cudaError_t e = cudaFuncSetAttribute(recall_window_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)window_smem(d));
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(recall_exact_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)exact_smem(d));
+    const RowView X = ix->rows();
+    cudaError_t e = with_rows(X, [&](auto x) {
+        using T = row_elem_t<decltype(x)>;
+        cudaError_t r = cudaFuncSetAttribute(recall_window_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)window_smem(d));
+        if (r == cudaSuccess) r = cudaFuncSetAttribute(recall_exact_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)exact_smem(d));
+        return r;
+    });
     if (e == cudaSuccess) e = cudaMemsetAsync(W.flags.p, 0, 2 * sizeof(int), c->stream);
     if (e != cudaSuccess) { set_error("top-k: %s", cudaGetErrorString(e)); return done(GORSE_B200_ERR_CUDA); }
     int64_t host_exact = 0;
@@ -329,7 +337,9 @@ int32_t recall_rows(gorse_b200_index *ix, const uint8_t *allow, int64_t nq, cons
     for (int64_t q0 = 0; q0 < nq; q0 += cq) {
         const int64_t rows = std::min(cq, nq - q0);
         if (!q_host) {   // stored vectors: gathered from the collection in place of the upload
-            recall_gather_kernel<<<(unsigned)std::min<int64_t>(rows, (int64_t)c->sm_count * 16), 128, 0, c->stream>>>(ix->X.p, d, d_qslots + q0, rows, W.q.p);
+            with_rows(X, [&](auto x) {
+                recall_gather_kernel<<<(unsigned)std::min<int64_t>(rows, (int64_t)c->sm_count * 16), 128, 0, c->stream>>>(x, d, d_qslots + q0, rows, W.q.p);
+            });
             c->launches++;
         }
         if ((q_host && (e = cudaMemcpyAsync(W.q.p, q_host + q0 * d, sizeof(float) * rows * d, cudaMemcpyHostToDevice, c->stream)) != cudaSuccess) ||
@@ -390,17 +400,21 @@ int32_t recall_rows(gorse_b200_index *ix, const uint8_t *allow, int64_t nq, cons
                     return done(GORSE_B200_ERR_CUDA);
                 }
             }
-            if ((st = mma_sweep(ix, W.q.p, nullptr, W.rows.p + cls_begin[t], 0, nr, m_tiles, ix->ev[2 * sweeps], ix->ev[2 * sweeps + 1])))
+            if ((st = mma_sweep(ix, RowView{W.q.p, false}, nullptr, W.rows.p + cls_begin[t], 0, nr, m_tiles, ix->ev[2 * sweeps], ix->ev[2 * sweeps + 1])))
                 return done(st);
             sweeps++;
             ix->stage1_flop += 2.0 * (double)nr * (double)N * (double)d;
-            recall_window_kernel<<<(unsigned)std::min<int64_t>(nr, (int64_t)c->sm_count * 16), WIN_THREADS, window_smem(d), c->stream>>>(
-                ix->w_ccol.p, ix->w_cval.p, ix->w_ccnt.p, ix->w_theta.p, ix->w_eps.p, ix->perm.p, allow, ix->X.p, d, ix->metric,
-                W.rows.p + cls_begin[t], nr, R);
+            with_rows(X, [&](auto x) {
+                recall_window_kernel<<<(unsigned)std::min<int64_t>(nr, (int64_t)c->sm_count * 16), WIN_THREADS, window_smem(d), c->stream>>>(
+                    ix->w_ccol.p, ix->w_cval.p, ix->w_ccnt.p, ix->w_theta.p, ix->w_eps.p, ix->perm.p, allow, x, d, ix->metric,
+                    W.rows.p + cls_begin[t], nr, R);
+            });
             c->launches++;
         }
-        recall_exact_kernel<<<(unsigned)std::min<int64_t>(rows, exact_grid), EXACT_THREADS, exact_smem(d), c->stream>>>(
-            ix->X.p, N, d, ix->metric, allow, R, W.scratch.p);
+        with_rows(X, [&](auto x) {
+            recall_exact_kernel<<<(unsigned)std::min<int64_t>(rows, exact_grid), EXACT_THREADS, exact_smem(d), c->stream>>>(
+                x, N, d, ix->metric, allow, R, W.scratch.p);
+        });
         c->launches++;
         const int64_t t0 = q0 * n;
         if (table) {
@@ -487,6 +501,15 @@ int32_t index_reserve(gorse_b200_index *ix, int64_t need)
     if (need <= ix->cap) return GORSE_B200_OK;
     cudaStream_t s = ix->ctx->stream;
     const int64_t ncap = std::max<int64_t>(need, ix->cap * 2);
+    if (ix->value_bytes == 2) {
+        DevBuf<uint16_t> nb;
+        GB_TRY(nb.alloc((size_t)ncap * ix->d));
+        if (ix->n) GB_CUDA(cudaMemcpyAsync(nb.p, ix->Xh.p, sizeof(uint16_t) * ix->n * ix->d, cudaMemcpyDeviceToDevice, s));
+        GB_CUDA(cudaStreamSynchronize(s));
+        ix->Xh = std::move(nb);
+        ix->cap = ncap;
+        return GORSE_B200_OK;
+    }
     DevBuf<float> nb;
     GB_TRY(nb.alloc((size_t)ncap * ix->d));
     if (ix->n) GB_CUDA(cudaMemcpyAsync(nb.p, ix->X.p, sizeof(float) * ix->n * ix->d, cudaMemcpyDeviceToDevice, s));
@@ -496,7 +519,214 @@ int32_t index_reserve(gorse_b200_index *ix, int64_t need)
     return GORSE_B200_OK;
 }
 
-// Xn[scan[s]] = X[s] for every live slot s (scan[s + 1] != scan[s]); V = float4 when d % 4 == 0, one V per thread
+// X[s] = src[map[s]] for m rows of d4 float4 (device to device)
+__global__ void index_gather_rows_kernel(const float *Q, int d4, const int32_t *items, int64_t n, float *X)
+{
+    int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    const int64_t total = n * d4, st = (int64_t)gridDim.x * blockDim.x;
+    for (; i < total; i += st) {
+        const int64_t s = i / d4, c = i - s * d4;
+        reinterpret_cast<float4 *>(X)[s * d4 + c] = reinterpret_cast<const float4 *>(Q)[(int64_t)items[s] * d4 + c];
+    }
+}
+
+// ---- bf16 rows: narrowing on upload, widening on promotion -------------------------------------------------------------------
+// narrowing keeps the high 16 bits; the value was bf16-exact iff the low 16 are zero
+__device__ __forceinline__ bool narrow(float v, uint16_t &h)
+{
+    const uint32_t u = __float_as_uint(v);
+    h = (uint16_t)(u >> 16);
+    return (u & 0xffffu) != 0u;
+}
+__device__ __forceinline__ bool narrow(float4 v, uint2 &h)
+{
+    const uint32_t a = __float_as_uint(v.x), b = __float_as_uint(v.y), c = __float_as_uint(v.z), e = __float_as_uint(v.w);
+    h.x = (a >> 16) | (b & 0xffff0000u);
+    h.y = (c >> 16) | (e & 0xffff0000u);
+    return ((a | b | c | e) & 0xffffu) != 0u;
+}
+
+// dst[s * dv + c] = narrow(src[(map ? map[s] : s) * dv + c]) for m rows; inexact[0] = 1 when a value is not bf16-exact.
+// V / H = float4 / uint2 when d % 4 == 0 (dv = d / 4), else float / uint16_t (dv = d).
+template <typename V, typename H>
+__global__ void narrow_rows_kernel(const V *src, const int32_t *map, int64_t m, int dv, H *dst, int32_t *inexact)
+{
+    int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    const int64_t total = m * dv, st = (int64_t)gridDim.x * blockDim.x;
+    bool bad = false;
+    for (; i < total; i += st) {
+        const int64_t s = i / dv, c = i - s * dv;
+        bad |= narrow(src[(map ? (int64_t)map[s] : s) * dv + c], dst[i]);
+    }
+    if (bad) *inexact = 1;
+}
+
+// dst[i] = widen(src[i]) for count elements: promotion's one pass over the bf16 rows
+template <typename H, typename V>
+__global__ void widen_rows_kernel(const H *src, int64_t count, V *dst)
+{
+    const int64_t st = (int64_t)gridDim.x * blockDim.x;
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < count; i += st) dst[i] = widen(src[i]);
+}
+
+cudaError_t index_narrow(int d, gorse_b200_ctx *c, cudaStream_t s, const float *src, const int32_t *map, int64_t m, uint16_t *dst,
+                         int32_t *inexact)
+{
+    if (m == 0) return cudaSuccess;
+    const unsigned grid = (unsigned)std::min<int64_t>(div_up(m * d, 256), (int64_t)c->sm_count * 8);
+    if (d % 4 == 0)
+        narrow_rows_kernel<<<grid, 256, 0, s>>>(reinterpret_cast<const float4 *>(src), map, m, d / 4, reinterpret_cast<uint2 *>(dst), inexact);
+    else
+        narrow_rows_kernel<<<grid, 256, 0, s>>>(src, map, m, d, dst, inexact);
+    c->launches++;
+    return cudaGetLastError();
+}
+
+// dst[0, rows * d) = the widened bf16 rows src, on the context's stream
+static cudaError_t widen_rows(gorse_b200_ctx *c, int d, const uint16_t *src, int64_t rows, float *dst)
+{
+    if (rows == 0) return cudaSuccess;
+    const unsigned grid = (unsigned)c->sm_count * 8;
+    if (d % 4 == 0)
+        widen_rows_kernel<<<grid, 256, 0, c->stream>>>(reinterpret_cast<const uint2 *>(src), rows * d / 4, reinterpret_cast<float4 *>(dst));
+    else
+        widen_rows_kernel<<<grid, 256, 0, c->stream>>>(src, rows * d, dst);
+    c->launches++;
+    return cudaGetLastError();
+}
+
+int32_t index_promote(gorse_b200_index *ix, int64_t rows)
+{
+    if (ix->value_bytes == 4) return GORSE_B200_OK;
+    gorse_b200_ctx *c = ix->ctx;
+    DevBuf<float> nx;
+    if (nx.alloc((size_t)ix->cap * ix->d)) {   // the documented code of a promotion that cannot allocate
+        set_error("promotion to fp32: cannot allocate %lld bytes", (long long)(4 * ix->cap * ix->d));
+        return GORSE_B200_ERR_CUDA;
+    }
+    cudaError_t e = widen_rows(c, ix->d, ix->Xh.p, rows, nx.p);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
+    if (e != cudaSuccess) { set_error("promote: %s", cudaGetErrorString(e)); return GORSE_B200_ERR_CUDA; }
+    ix->X = std::move(nx);
+    ix->Xh.free();
+    ix->stage.free();
+    ix->value_bytes = 4;
+    return GORSE_B200_OK;
+}
+
+// copies m fp32 rows (row s = src[(map ? map[s] : s) * d ..], host or device) into the fp32 rows dst on the context's stream
+static cudaError_t copy_rows_f32(gorse_b200_index *ix, const float *src, const int32_t *map, const int32_t *h_map, int64_t m, bool host, float *dst)
+{
+    gorse_b200_ctx *c = ix->ctx;
+    const int d = ix->d;
+    if (!map) return cudaMemcpyAsync(dst, src, sizeof(float) * m * d, host ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToDevice, c->stream);
+    cudaError_t e = cudaSuccess;
+    if (d % 4 == 0) {
+        index_gather_rows_kernel<<<c->sm_count * 8, 256, 0, c->stream>>>(src, d / 4, map, m, dst);
+        c->launches++;
+        e = cudaGetLastError();
+    } else
+        for (int64_t s = 0; s < m && e == cudaSuccess; s++)
+            e = cudaMemcpyAsync(dst + s * d, src + (int64_t)h_map[s] * d, sizeof(float) * d, cudaMemcpyDeviceToDevice, c->stream);
+    return e;
+}
+
+int32_t index_append(gorse_b200_index *ix, const float *src, const int32_t *map, int64_t m, bool host)
+{
+    if (m == 0) return GORSE_B200_OK;
+    gorse_b200_ctx *c = ix->ctx;
+    const int d = ix->d;
+    const int64_t n = ix->n, need = n + m;
+    std::vector<int32_t> h_map;
+    if (map && d % 4 != 0) {   // the row-by-row copy of an fp32 target reads the map on the host
+        h_map.resize((size_t)m);
+        GB_CUDA(cudaMemcpyAsync(h_map.data(), map, sizeof(int32_t) * m, cudaMemcpyDeviceToHost, c->stream));
+        GB_CUDA(cudaStreamSynchronize(c->stream));
+    }
+    if (ix->value_bytes == 4) {
+        GB_TRY(index_reserve(ix, need));
+        GB_CUDA(copy_rows_f32(ix, src, map, h_map.data(), m, host, ix->X.p + n * d));
+        GB_CUDA(cudaStreamSynchronize(c->stream));
+        ix->n = need;
+        ix->mma_ready = false;  // bf16 mirror and norms are rebuilt lazily
+        return GORSE_B200_OK;
+    }
+    // bf16: every chunk is narrowed into the free rows past n (or into a grown copy) on the stream, with no wait in between;
+    // one flag covers the call and is read at the end.  If a value was not exact, the narrowed rows are dropped: the stored
+    // rows are widened into new fp32 rows and the call's rows are copied in again from the caller's source.  The index takes
+    // the new buffers only at the end, so every error leaves it as it was.
+    const int64_t ncap = need > ix->cap ? std::max<int64_t>(need, ix->cap * 2) : ix->cap;
+    const int64_t R = host ? std::max<int64_t>(1, APPEND_STAGE_BYTES / 4 / d) : m;   // rows per chunk
+    DevBuf<uint16_t> nh;
+    StreamSync sync{c->stream};
+    GB_TRY(ix->inexact.grow(1));
+    if (host) GB_TRY(ix->stage.grow((size_t)std::min(R, m) * d));
+    uint16_t *th = ix->Xh.p;
+    if (ncap > ix->cap) {
+        GB_TRY(nh.alloc((size_t)ncap * d));
+        if (n) GB_CUDA(cudaMemcpyAsync(nh.p, ix->Xh.p, sizeof(uint16_t) * n * d, cudaMemcpyDeviceToDevice, c->stream));
+        th = nh.p;
+    }
+    GB_CUDA(cudaMemsetAsync(ix->inexact.p, 0, sizeof(int32_t), c->stream));
+    for (int64_t j0 = 0; j0 < m; j0 += R) {   // stream order keeps chunk k + 1's upload behind chunk k's narrowing
+        const int64_t rows = std::min(R, m - j0);
+        if (host) GB_CUDA(cudaMemcpyAsync(ix->stage.p, src + j0 * d, sizeof(float) * rows * d, cudaMemcpyHostToDevice, c->stream));
+        GB_CUDA(index_narrow(d, c, c->stream, host ? ix->stage.p : src, map ? map + j0 : nullptr, rows, th + (n + j0) * d, ix->inexact.p));
+    }
+    int32_t inexact = 0;
+    GB_CUDA(cudaMemcpyAsync(&inexact, ix->inexact.p, sizeof(int32_t), cudaMemcpyDeviceToHost, c->stream));
+    GB_CUDA(cudaStreamSynchronize(c->stream));
+    if (inexact) {   // promote: the stored rows [0, n) are exact (Xh holds them), the call's rows come from the source
+        nh.free();   // before the fp32 rows exist: an empty collection never holds both
+        DevBuf<float> nf;
+        if (nf.alloc((size_t)ncap * d)) {
+            set_error("promotion to fp32: cannot allocate %lld bytes", (long long)(4 * ncap * d));
+            return GORSE_B200_ERR_CUDA;
+        }
+        GB_CUDA(widen_rows(c, d, ix->Xh.p, n, nf.p));
+        GB_CUDA(copy_rows_f32(ix, src, map, h_map.data(), m, host, nf.p + n * d));
+        GB_CUDA(cudaStreamSynchronize(c->stream));
+        ix->X = std::move(nf);
+        ix->Xh.free();
+        ix->stage.free();   // an fp32 index adds without staging
+        ix->value_bytes = 4;
+    } else if (nh.p)
+        ix->Xh = std::move(nh);
+    ix->cap = ncap;
+    ix->n = need;
+    ix->mma_ready = false;
+    return GORSE_B200_OK;
+}
+
+int32_t index_download_rows(gorse_b200_index *ix, const int64_t *rows, int64_t n, float *out)
+{
+    gorse_b200_ctx *c = ix->ctx;
+    const int64_t d = ix->d;
+    if (ix->value_bytes == 4) {   // one copy per row, straight into the caller's buffer
+        for (int64_t i = 0; i < n; i++)
+            if (rows[i] >= 0)
+                GB_CUDA(cudaMemcpyAsync(out + i * d, ix->X.p + rows[i] * d, sizeof(float) * d, cudaMemcpyDeviceToHost, c->stream));
+        GB_CUDA(cudaStreamSynchronize(c->stream));
+        return GORSE_B200_OK;
+    }
+    // bf16: the rows' bits into a host buffer, one copy per row, then widened on the host (bits << 16, exact)
+    std::vector<uint16_t> h;
+    std::vector<int64_t> at;
+    for (int64_t i = 0; i < n; i++)
+        if (rows[i] >= 0) at.push_back(i);
+    h.resize(at.size() * (size_t)d);
+    for (size_t j = 0; j < at.size(); j++)
+        GB_CUDA(cudaMemcpyAsync(h.data() + j * d, ix->Xh.p + rows[at[j]] * d, sizeof(uint16_t) * d, cudaMemcpyDeviceToHost, c->stream));
+    GB_CUDA(cudaStreamSynchronize(c->stream));
+    for (size_t j = 0; j < at.size(); j++) {
+        uint32_t *o = reinterpret_cast<uint32_t *>(out + at[j] * d);
+        for (int64_t e = 0; e < d; e++) o[e] = (uint32_t)h[j * d + e] << 16;
+    }
+    return GORSE_B200_OK;
+}
+
+// Xn[scan[s]] = X[s] for every live slot s (scan[s + 1] != scan[s]); V = float4 when d % 4 == 0, one V per thread (bf16 rows:
+// uint2, 4 values, or uint16_t)
 template <typename V>
 __global__ void index_compact_rows_kernel(const V *X, int64_t n, int dv, const int64_t *scan, V *Xn)
 {
@@ -508,20 +738,20 @@ __global__ void index_compact_rows_kernel(const V *X, int64_t n, int dv, const i
     }
 }
 
-int32_t index_compact(gorse_b200_index *ix, const int64_t *scan, int64_t live)
+// the live rows of one element type into a new buffer nx: T = float (V4 = float4) or uint16_t (V4 = uint2)
+template <typename T, typename V4>
+static int32_t compact_rows(gorse_b200_index *ix, const T *X, const int64_t *scan, int64_t live, DevBuf<T> &nx)
 {
     gorse_b200_ctx *c = ix->ctx;
-    DevBuf<float> nx;
-    int32_t st = nx.alloc((size_t)live * ix->d);
-    if (st) return st;
+    GB_TRY(nx.alloc((size_t)live * ix->d));
     cudaError_t e = cudaSuccess;
     if (live > 0) {
         const unsigned grid = (unsigned)c->sm_count * 8;
         if (ix->d % 4 == 0)
-            index_compact_rows_kernel<<<grid, 256, 0, c->stream>>>(reinterpret_cast<const float4 *>(ix->X.p), ix->n, ix->d / 4, scan,
-                                                                   reinterpret_cast<float4 *>(nx.p));
+            index_compact_rows_kernel<<<grid, 256, 0, c->stream>>>(reinterpret_cast<const V4 *>(X), ix->n, ix->d / 4, scan,
+                                                                   reinterpret_cast<V4 *>(nx.p));
         else
-            index_compact_rows_kernel<<<grid, 256, 0, c->stream>>>(ix->X.p, ix->n, ix->d, scan, nx.p);
+            index_compact_rows_kernel<<<grid, 256, 0, c->stream>>>(X, ix->n, ix->d, scan, nx.p);
         c->launches++;
         e = cudaGetLastError();
     }
@@ -530,11 +760,25 @@ int32_t index_compact(gorse_b200_index *ix, const int64_t *scan, int64_t live)
         set_error("compact: %s", cudaGetErrorString(e));
         return GORSE_B200_ERR_CUDA;
     }
-    ix->X = std::move(nx);
+    return GORSE_B200_OK;
+}
+
+int32_t index_compact(gorse_b200_index *ix, const int64_t *scan, int64_t live)
+{
+    if (ix->value_bytes == 2) {   // bf16 rows stay bf16
+        DevBuf<uint16_t> nx;
+        GB_TRY((compact_rows<uint16_t, uint2>(ix, ix->Xh.p, scan, live, nx)));
+        ix->Xh = std::move(nx);
+    } else {
+        DevBuf<float> nx;
+        GB_TRY((compact_rows<float, float4>(ix, ix->X.p, scan, live, nx)));
+        ix->X = std::move(nx);
+    }
     ix->n = ix->cap = live;
     ix->mma_ready = false;   // the next sweep rebuilds the mirror, norms and permutation for the new n
     ix->Xb.free(); ix->norm.free(); ix->perm.free();
     ix->recall.scratch.free();   // [N] per exact CTA
+    ix->stage.free();            // the next bf16 add allocates its upload staging again
     ix->last_fallback_rows = 0;
     ix->stage1_ms = ix->stage1_flop = 0.0;
     return GORSE_B200_OK;
@@ -542,9 +786,9 @@ int32_t index_compact(gorse_b200_index *ix, const int64_t *scan, int64_t live)
 
 size_t index_bytes(const gorse_b200_index *ix)
 {
-    return ix->X.bytes() + ix->Xb.bytes() + ix->norm.bytes() + ix->perm.bytes() + ix->w_qb.bytes() + ix->w_eps.bytes() + ix->w_cval.bytes() +
-           ix->w_theta.bytes() + ix->w_ccol.bytes() + ix->w_ccnt.bytes() + ix->recall.bytes() + ix->r_idx.bytes() + ix->r_count.bytes() +
-           ix->r_dist.bytes();
+    return ix->X.bytes() + ix->Xh.bytes() + ix->stage.bytes() + ix->inexact.bytes() + ix->Xb.bytes() + ix->norm.bytes() + ix->perm.bytes() +
+           ix->w_qb.bytes() + ix->w_eps.bytes() + ix->w_cval.bytes() + ix->w_theta.bytes() + ix->w_ccol.bytes() + ix->w_ccnt.bytes() +
+           ix->recall.bytes() + ix->r_idx.bytes() + ix->r_count.bytes() + ix->r_dist.bytes();
 }
 
 }  // namespace gb
@@ -588,13 +832,7 @@ int32_t gorse_b200_index_add(gorse_b200_index *ix, const float *vectors, int64_t
     if (n > 0) {
         GB_CHECK_ARG(vectors != nullptr, "vectors is NULL");
         ScopedDevice sd(ix->ctx->device);
-        cudaStream_t s = ix->ctx->stream;
-        int64_t need = ix->n + n;
-        GB_TRY(index_reserve(ix, need));
-        GB_CUDA(cudaMemcpyAsync(ix->X.p + ix->n * ix->d, vectors, sizeof(float) * n * ix->d, cudaMemcpyHostToDevice, s));
-        GB_CUDA(cudaStreamSynchronize(s));
-        ix->n = need;
-        ix->mma_ready = false;  // bf16 mirror and norms are rebuilt lazily
+        GB_TRY(index_append(ix, vectors, nullptr, n, true));
     }
     if (count_out) *count_out = ix->n;
     return GORSE_B200_OK;
@@ -672,7 +910,7 @@ int32_t gorse_b200_index_stage1_scores(gorse_b200_index *ix, int64_t q0, int64_t
     auto done = [&](int32_t s) { cudaStreamSynchronize(c->stream); ix->dbg_scores = nullptr; return s; };
     if ((st = dense.alloc((size_t)nq * n_cols)) || (st = mma_reserve(ix, nq))) return done(st);
     ix->dbg_scores = dense.p;
-    if ((st = mma_sweep(ix, ix->X.p, nullptr, nullptr, q0, nq, mma_sample_tiles(ix, 4.0), nullptr, nullptr))) return done(st);
+    if ((st = mma_sweep(ix, ix->rows(), nullptr, nullptr, q0, nq, mma_sample_tiles(ix, 4.0), nullptr, nullptr))) return done(st);
     std::vector<float> h((size_t)nq * n_cols);
     std::vector<int32_t> perm((size_t)ix->n);
     cudaError_t e = cudaMemcpyAsync(h.data(), dense.p, sizeof(float) * h.size(), cudaMemcpyDeviceToHost, c->stream);

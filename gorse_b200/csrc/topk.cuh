@@ -21,13 +21,40 @@ struct RecallWork {
                k.bytes() + count.bytes() + flags.bytes();
     }
 };
+
+// the stored rows of an index as a kernel reads them: fp32 values, or bf16 values kept as the high 16 bits of their fp32 bit
+// patterns (uint16_t).  A launch picks its instantiation once, through with_rows; no kernel branches on the element type.
+struct RowView {
+    const void *p;
+    bool bf16;
+};
+template <typename F>
+inline auto with_rows(RowView v, F f)
+{
+    return v.bf16 ? f(static_cast<const uint16_t *>(v.p)) : f(static_cast<const float *>(v.p));
+}
+// the element type behind a row pointer of with_rows
+template <typename P>
+using row_elem_t = std::remove_const_t<std::remove_pointer_t<P>>;
+// the 4-value vector of an element type: one 16-byte (fp32) or 8-byte (bf16) load
+template <typename T>
+struct row_quad_type { using type = float4; };
+template <>
+struct row_quad_type<uint16_t> { using type = uint2; };
 }  // namespace gb
 
 struct gorse_b200_index {
     gorse_b200_ctx *ctx = nullptr;
     int32_t d = 0, metric = 0;
     int64_t n = 0, cap = 0;
-    gb::DevBuf<float> X;            // [cap x d] fp32, row-major: the vectors as added (exact re-rank reads these)
+    // the vectors as added, [cap x d] row-major, in exactly one of X (value_bytes 4) and Xh (value_bytes 2; the exact re-rank reads
+    // these).  The bare index is fp32.  A vector collection's index starts bf16 and stays so while every value it was given is
+    // bf16-exact (low 16 bits zero); the first value that is not promotes it to fp32 for good (index_append, index_promote).
+    gb::DevBuf<float> X;
+    gb::DevBuf<uint16_t> Xh;
+    int32_t value_bytes = 4;
+    gb::DevBuf<float> stage;        // grow-only fp32 staging of a bf16 index's host uploads (at most APPEND_STAGE_BYTES)
+    gb::DevBuf<int32_t> inexact;    // [1] the narrowing kernel's flag: a value was not bf16-exact
     gb::DevBuf<__nv_bfloat16> Xb;   // [n_pad x d] bf16 mirror feeding the tensor cores (built lazily)
     gb::DevBuf<float> norm;         // per-vector fp32 norms (+ max at [n], max |bf16(x) - x| at [n + 1]), built lazily
     gb::DevBuf<int32_t> perm;       // mirror row p holds vector perm[p] (random: the first columns are a uniform sample)
@@ -49,6 +76,7 @@ struct gorse_b200_index {
     gb::DevBuf<int32_t> r_idx, r_count;
     gb::DevBuf<float> r_dist;
     std::mutex mu;
+    gb::RowView rows() const { return value_bytes == 2 ? gb::RowView{Xh.p, true} : gb::RowView{X.p, false}; }
 };
 
 namespace gb {
@@ -69,17 +97,28 @@ constexpr uint32_t B_TILE_BYTES = BN * BK * 2; // one [128 x 64] bf16 k-block of
 }  // namespace mma
 
 #ifdef __CUDACC__
+// widening of stored bf16 values: bits << 16, exact (no flush of subnormals, NaN payloads kept); the fp32 forms are the identity
+__device__ __forceinline__ float widen(float v) { return v; }
+__device__ __forceinline__ float4 widen(float4 v) { return v; }
+__device__ __forceinline__ float widen(uint16_t h) { return __uint_as_float((uint32_t)h << 16); }
+__device__ __forceinline__ float4 widen(uint2 h)   // 4 bf16 values, little-endian: value 0 is the low half of h.x
+{
+    return make_float4(__uint_as_float(h.x << 16), __uint_as_float(h.x & 0xffff0000u), __uint_as_float(h.y << 16),
+                       __uint_as_float(h.y & 0xffff0000u));
+}
 // the exact scan's arithmetic, shared by the index search (topk.cu) and the batched recall (recall.cu)
 // exact distance by a quad, d % 16 == 0.  Euclidean: floats_avx512.c:374-441 (sub, mul, add: no fusing).
-__device__ __forceinline__ float quad_dist(const float4 *q /* C regs, query chunk c at q[c] */, const float *x, int chunks,
+// T = float or uint16_t (bf16 rows): the lane's 4 values of a 16-value chunk are one 16- or 8-byte load either way.
+template <typename T>
+__device__ __forceinline__ float quad_dist(const float4 *q /* C regs, query chunk c at q[c] */, const T *x, int chunks,
                                            int lane4, unsigned mask, int metric, float qq)
 {
-    const float4 *x4 = reinterpret_cast<const float4 *>(x) + lane4;
+    const auto *x4 = reinterpret_cast<const typename row_quad_type<T>::type *>(x) + lane4;
     float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
     if (metric == GORSE_B200_METRIC_COSINE) {   // 1 - q.x / (|q| |x|); the reference's arithmetic lives in its vector store (unpinned)
         float4 xx = make_float4(0.f, 0.f, 0.f, 0.f);
         for (int c = 0; c < chunks; c++) {
-            const float4 b = __ldg(x4 + 4 * c);
+            const float4 b = widen(__ldg(x4 + 4 * c));
             dot_chunk(acc, q[c], b, c == 0);
             dot_chunk(xx, b, b, c == 0);
         }
@@ -87,11 +126,11 @@ __device__ __forceinline__ float quad_dist(const float4 *q /* C regs, query chun
         return __fsub_rn(1.0f, __fdiv_rn(dot, __fmul_rn(__fsqrt_rn(qq), __fsqrt_rn(nx))));
     }
     if (metric == GORSE_B200_METRIC_NEG_DOT) {
-        for (int c = 0; c < chunks; c++) dot_chunk(acc, q[c], __ldg(x4 + 4 * c), c == 0);
+        for (int c = 0; c < chunks; c++) dot_chunk(acc, q[c], widen(__ldg(x4 + 4 * c)), c == 0);
         return -quad_tree(acc, mask);
     }
     for (int c = 0; c < chunks; c++) {
-        float4 b = __ldg(x4 + 4 * c), v;
+        float4 b = widen(__ldg(x4 + 4 * c)), v;
         v.x = __fsub_rn(q[c].x, b.x); v.y = __fsub_rn(q[c].y, b.y); v.z = __fsub_rn(q[c].z, b.z); v.w = __fsub_rn(q[c].w, b.w);
         v.x = __fmul_rn(v.x, v.x); v.y = __fmul_rn(v.y, v.y); v.z = __fmul_rn(v.z, v.z); v.w = __fmul_rn(v.w, v.w);
         if (c == 0) acc = v;
@@ -100,8 +139,9 @@ __device__ __forceinline__ float quad_dist(const float4 *q /* C regs, query chun
     return __fsqrt_rn(quad_tree(acc, mask));
 }
 
-// any d, one thread (8-lane block + fused tails as in the reference)
-__device__ inline float dist_any(const float *a, const float *b, int n, int metric, float qq)
+// any d, one thread (8-lane block + fused tails as in the reference); b = a stored row, T = float or uint16_t (bf16)
+template <typename T>
+__device__ inline float dist_any(const float *a, const T *b, int n, int metric, float qq)
 {
     if (metric == GORSE_B200_METRIC_NEG_DOT) return -dot_any(a, b, n);
     if (metric == GORSE_B200_METRIC_COSINE)
@@ -110,13 +150,27 @@ __device__ inline float dist_any(const float *a, const float *b, int n, int metr
     float s[16];
 #pragma unroll
     for (int l = 0; l < 16; l++) s[l] = 0.f;
-    if (epoch > 0) {
+    if constexpr (std::is_same<T, uint16_t>::value) {   // bf16 rows: 16 values by two loads (row_chunk16)
+        float bv[16];
+        if (epoch > 0) {
+            row_chunk16(b, bv);
 #pragma unroll
-        for (int l = 0; l < 16; l++) { float v = __fsub_rn(a[l], b[l]); s[l] = __fmul_rn(v, v); }
-    }
-    for (int c = 1; c < epoch; c++) {
+            for (int l = 0; l < 16; l++) { float v = __fsub_rn(a[l], bv[l]); s[l] = __fmul_rn(v, v); }
+        }
+        for (int c = 1; c < epoch; c++) {
+            row_chunk16(b + 16 * c, bv);
 #pragma unroll
-        for (int l = 0; l < 16; l++) { float v = __fsub_rn(a[16 * c + l], b[16 * c + l]); s[l] = __fadd_rn(__fmul_rn(v, v), s[l]); }
+            for (int l = 0; l < 16; l++) { float v = __fsub_rn(a[16 * c + l], bv[l]); s[l] = __fadd_rn(__fmul_rn(v, v), s[l]); }
+        }
+    } else {
+        if (epoch > 0) {
+#pragma unroll
+            for (int l = 0; l < 16; l++) { float v = __fsub_rn(a[l], row_val(b, l)); s[l] = __fmul_rn(v, v); }
+        }
+        for (int c = 1; c < epoch; c++) {
+#pragma unroll
+            for (int l = 0; l < 16; l++) { float v = __fsub_rn(a[16 * c + l], row_val(b, 16 * c + l)); s[l] = __fadd_rn(__fmul_rn(v, v), s[l]); }
+        }
     }
     float r4[4];
 #pragma unroll
@@ -126,14 +180,14 @@ __device__ inline float dist_any(const float *a, const float *b, int n, int metr
     if (remain >= 8) {
         float p[8];
 #pragma unroll
-        for (int l = 0; l < 8; l++) { float v = __fsub_rn(a[l], b[l]); p[l] = __fmul_rn(v, v); }
+        for (int l = 0; l < 8; l++) { float v = __fsub_rn(a[l], row_val(b, l)); p[l] = __fmul_rn(v, v); }
         float q4[4];
 #pragma unroll
         for (int l = 0; l < 4; l++) q4[l] = __fadd_rn(p[l + 4], p[l]);
         sum = __fadd_rn(sum, __fadd_rn(__fadd_rn(q4[0], q4[2]), __fadd_rn(q4[1], q4[3])));
         a += 8; b += 8; remain -= 8;
     }
-    for (int i = 0; i < remain; i++) { float v = __fsub_rn(a[i], b[i]); sum = __fmaf_rn(v, v, sum); }
+    for (int i = 0; i < remain; i++) { float v = __fsub_rn(a[i], row_val(b, i)); sum = __fmaf_rn(v, v, sum); }
     return __fsqrt_rn(sum);
 }
 
@@ -149,7 +203,23 @@ __device__ __forceinline__ float key_float(uint32_t k)
 }
 #endif  // __CUDACC__
 
+// make room for `need` vectors in the rows of the index's element type (amortised doubling); the caller holds ix->mu
 int32_t index_reserve(gorse_b200_index *ix, int64_t need);
+// the add path of every index: m rows, row s = src[(map ? map[s] : s) * d ..], src on the host (map == nullptr) or the device.
+// A bf16 index narrows them (host rows through ix->stage, at most APPEND_STAGE_BYTES at a time) and promotes itself to fp32 before
+// they land when one value is not bf16-exact.  On an error the index is exactly as it was.  The caller holds ix->mu.
+int32_t index_append(gorse_b200_index *ix, const float *src, const int32_t *map, int64_t m, bool host);
+constexpr int64_t APPEND_STAGE_BYTES = 64ll << 20;
+// launches the narrowing of m fp32 device rows (row s = src[(map ? map[s] : s) * d ..]) into the bf16 rows dst on stream s;
+// *inexact (device) becomes 1 when a value is not bf16-exact, and dst then holds its truncation
+cudaError_t index_narrow(int d, gorse_b200_ctx *c, cudaStream_t s, const float *src, const int32_t *map, int64_t m, uint16_t *dst,
+                         int32_t *inexact);
+// promotion of a bf16 index: fp32 rows of capacity ix->cap, rows [0, rows) widened from Xh in one pass, Xh released.  One-way.
+// On an error the index is unchanged.  The caller holds ix->mu.
+int32_t index_promote(gorse_b200_index *ix, int64_t rows);
+// out[i * d ..] (host) = the fp32 values of stored row rows[i] (host list), for every i with rows[i] >= 0; fp32 rows are copied
+// one by one into out, bf16 rows one by one into a host buffer and widened there.  Ends with the stream synchronised.
+int32_t index_download_rows(gorse_b200_index *ix, const int64_t *rows, int64_t n, float *out);
 // compaction (gorse_b200_vecdb_compact): scan[n + 1] (device) is the exclusive sum of the live flags, so slot s is live iff
 // scan[s + 1] != scan[s] and then moves to scan[s]; X becomes the live rows in order, live = scan[n] of them, with cap = live,
 // and everything built from the old rows (mirror, norms, permutation, exact scratch, stage-1 counters) is dropped.  On an
@@ -164,7 +234,7 @@ size_t index_bytes(const gorse_b200_index *ix);
 // nullptr) are recorded around the sweep kernel.
 int32_t mma_reserve(gorse_b200_index *ix, int64_t cq);
 int mma_sample_tiles(const gorse_b200_index *ix, double cands);
-int32_t mma_sweep(gorse_b200_index *ix, const float *q_base, const float *d_q, const int64_t *d_qidx, int64_t q0, int64_t nq, int m_tiles,
+int32_t mma_sweep(gorse_b200_index *ix, RowView q_base, const float *d_q, const int64_t *d_qidx, int64_t q0, int64_t nq, int m_tiles,
                   cudaEvent_t ev0, cudaEvent_t ev1);
 // the sweep serves Dot and Euclidean indexes of >= 32768 vectors for >= 64 rows; GORSE_B200_TOPK_EXACT=1 turns it off
 bool mma_path_eligible(const gorse_b200_index *ix, int64_t nq);

@@ -258,8 +258,10 @@ topk_mma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant
 
 // ---- mirror construction ----------------------------------------------------------------------------
 // row p of the mirror = bf16 of vector perm[p] (zero rows beyond n); Euclidean appends hi/lo of -|x|^2/2.
-// max_dx: running max over the vectors of |bf16(x) - x| (the ints of non-negative floats order as the floats; NaN -> Inf)
-__global__ void build_mirror_kernel(const float *X, int64_t n, int d, const int32_t *perm, int64_t n_pad, int kp, int metric,
+// max_dx: running max over the vectors of |bf16(x) - x| (the ints of non-negative floats order as the floats; NaN -> Inf).
+// T = uint16_t: bf16 rows, every value exact, so the mirror holds the rows' own bits and max_dx stays 0.
+template <typename T>
+__global__ void build_mirror_kernel(const T *X, int64_t n, int d, const int32_t *perm, int64_t n_pad, int kp, int metric,
                                     __nv_bfloat16 *Xb, float *norm /* [n] |x| by original index */, float *max_dx)
 {
     const int64_t p = blockIdx.x;
@@ -269,16 +271,20 @@ __global__ void build_mirror_kernel(const float *X, int64_t n, int d, const int3
         return;
     }
     const int64_t src = perm[p];
-    const float *x = X + src * d;
+    const T *x = X + src * d;
     __shared__ float s_sum[32], s_dd[32];
     float ss = 0.f, dd = 0.f;
     for (int k = threadIdx.x; k < d; k += blockDim.x) {
-        const float v = x[k];
-        const __nv_bfloat16 b = __float2bfloat16(v);
-        const float r = __fsub_rn(__bfloat162float(b), v);   // exact: the bits bf16 drops
+        const float v = row_val(x, k);
         ss = __fmaf_rn(v, v, ss);
-        dd = __fmaf_rn(r, r, dd);
-        dst[k] = b;
+        if constexpr (std::is_same<T, float>::value) {
+            const __nv_bfloat16 b = __float2bfloat16(v);
+            const float r = __fsub_rn(__bfloat162float(b), v);   // exact: the bits bf16 drops
+            dd = __fmaf_rn(r, r, dd);
+            dst[k] = b;
+        } else {
+            dst[k] = __nv_bfloat16_raw{x[k]};
+        }
     }
     for (int o = 16; o; o >>= 1) { ss += __shfl_xor_sync(0xffffffffu, ss, o); dd += __shfl_xor_sync(0xffffffffu, dd, o); }
     if ((threadIdx.x & 31) == 0) { s_sum[threadIdx.x >> 5] = ss; s_dd[threadIdx.x >> 5] = dd; }
@@ -287,8 +293,10 @@ __global__ void build_mirror_kernel(const float *X, int64_t n, int d, const int3
         float tot = 0.f, dtot = 0.f;
         for (int w = 0; w < (int)(blockDim.x >> 5); w++) { tot += s_sum[w]; dtot += s_dd[w]; }
         norm[src] = sqrtf(tot);
-        const float dx = sqrtf(dtot);
-        atomicMax(reinterpret_cast<int *>(max_dx), __float_as_int(dx == dx ? dx : INFINITY));
+        if constexpr (std::is_same<T, float>::value) {
+            const float dx = sqrtf(dtot);
+            atomicMax(reinterpret_cast<int *>(max_dx), __float_as_int(dx == dx ? dx : INFINITY));
+        }
         int k = d;
         if (metric == GORSE_B200_METRIC_EUCLIDEAN) {
             const float a = -0.5f * tot;
@@ -302,8 +310,9 @@ __global__ void build_mirror_kernel(const float *X, int64_t n, int d, const int3
     // (columns d.. are written by thread 0 only; columns < d by the loop above)
 }
 
-// query mirror rows + per-row eps; queries come from q_ptr, or from X rows (q_idx / q0 + i)
-__global__ void build_queries_kernel(const float *X, const float *q_ptr, const int64_t *q_idx, int64_t q0, int64_t nq, int64_t nq_pad,
+// query mirror rows + per-row eps; queries come from q_ptr, or from X rows (q_idx / q0 + i; T = uint16_t: bf16 rows, widened)
+template <typename T>
+__global__ void build_queries_kernel(const T *X, const float *q_ptr, const int64_t *q_idx, int64_t q0, int64_t nq, int64_t nq_pad,
                                      int d, int kp, int metric, float max_norm, float max_dx, __nv_bfloat16 *Qb, float *eps)
 {
     const int64_t r = blockIdx.x;
@@ -312,11 +321,16 @@ __global__ void build_queries_kernel(const float *X, const float *q_ptr, const i
         for (int k = threadIdx.x; k < kp; k += blockDim.x) dst[k] = __float2bfloat16(0.f);
         return;
     }
-    const float *q = q_ptr ? q_ptr + r * d : X + (q_idx ? q_idx[r] : q0 + r) * d;
+    constexpr bool f32 = std::is_same<T, float>::value;
+    const float *q = nullptr;   // fp32 rows are read in place; bf16 rows (x) are widened value by value
+    const T *x = nullptr;
+    if constexpr (f32) q = q_ptr ? q_ptr + r * d : X + (q_idx ? q_idx[r] : q0 + r) * d;
+    else if (q_ptr) q = q_ptr + r * d;
+    else x = X + (q_idx ? q_idx[r] : q0 + r) * d;
     __shared__ float s_sum[3][32];
     float ss = 0.f, sh = 0.f, sd = 0.f;   // |q|^2, |bf16(q)|^2, |bf16(q) - q|^2
     for (int k = threadIdx.x; k < d; k += blockDim.x) {
-        const float v = q[k];
+        const float v = f32 || q ? q[k] : row_val(x, k);
         const __nv_bfloat16 b = __float2bfloat16(v);
         const float h = __bfloat162float(b), rd = __fsub_rn(h, v);
         ss = __fmaf_rn(v, v, ss);
@@ -426,8 +440,10 @@ static int32_t ensure_mirror(gorse_b200_index *ix)
     std::shuffle(perm.begin(), perm.end(), rng);
     GB_CUDA(cudaMemcpyAsync(ix->perm.p, perm.data(), sizeof(int32_t) * perm.size(), cudaMemcpyHostToDevice, c->stream));
     GB_CUDA(cudaMemsetAsync(ix->norm.p + ix->n, 0, 2 * sizeof(float), c->stream));   // max |x|, max |bf16(x) - x|
-    mma::build_mirror_kernel<<<(unsigned)n_pad, 128, 0, c->stream>>>(ix->X.p, ix->n, ix->d, ix->perm.p, n_pad, kp, ix->metric, ix->Xb.p, ix->norm.p,
-                                                                     ix->norm.p + ix->n + 1);
+    with_rows(ix->rows(), [&](auto x) {
+        mma::build_mirror_kernel<<<(unsigned)n_pad, 128, 0, c->stream>>>(x, ix->n, ix->d, ix->perm.p, n_pad, kp, ix->metric, ix->Xb.p, ix->norm.p,
+                                                                         ix->norm.p + ix->n + 1);
+    });
     GB_LAUNCHED(c);
     mma::max_kernel<<<c->sm_count * 2, 256, 0, c->stream>>>(ix->norm.p, ix->n, ix->norm.p + ix->n);
     GB_LAUNCHED(c);
@@ -467,7 +483,7 @@ int mma_sample_tiles(const gorse_b200_index *ix, double cands)
     return std::max(1, std::min(m_tiles, n_tiles));
 }
 
-int32_t mma_sweep(gorse_b200_index *ix, const float *q_base, const float *d_q, const int64_t *d_qidx, int64_t q0, int64_t nq, int m_tiles,
+int32_t mma_sweep(gorse_b200_index *ix, RowView q_base, const float *d_q, const int64_t *d_qidx, int64_t q0, int64_t nq, int m_tiles,
                   cudaEvent_t ev0, cudaEvent_t ev1)
 {
     gorse_b200_ctx *c = ix->ctx;
@@ -487,8 +503,10 @@ int32_t mma_sweep(gorse_b200_index *ix, const float *q_base, const float *d_q, c
     CUtensorMap map_a, map_b;
     GB_TRY(make_map(&map_b, ix->Xb.p, n_pad, kp, mma::BN));
     const int64_t nq_pad = (nq + mma::GROUP_ROWS - 1) / mma::GROUP_ROWS * mma::GROUP_ROWS;
-    mma::build_queries_kernel<<<(unsigned)nq_pad, 128, 0, c->stream>>>(q_base, d_q, d_qidx, q0, nq, nq_pad, ix->d, kp, ix->metric, ix->max_norm,
-                                                                      ix->max_dx, ix->w_qb.p, ix->w_eps.p);
+    with_rows(q_base, [&](auto x) {
+        mma::build_queries_kernel<<<(unsigned)nq_pad, 128, 0, c->stream>>>(x, d_q, d_qidx, q0, nq, nq_pad, ix->d, kp, ix->metric, ix->max_norm,
+                                                                          ix->max_dx, ix->w_qb.p, ix->w_eps.p);
+    });
     c->launches++;
     GB_TRY(make_map(&map_a, ix->w_qb.p, nq_pad, kp, mma::BM));
     mma::Params P;

@@ -51,17 +51,6 @@ __global__ void vecdb_mark_items_kernel(const int32_t *user_items, int64_t n, in
     const int64_t st = (int64_t)gridDim.x * blockDim.x;
     for (; i < n; i += st) flag[user_items[i]] = 1;
 }
-// X[first + s] = Q[items[s]]  (device to device, float4 per thread)
-__global__ void vecdb_copy_rows_kernel(const float *Q, int d4, const int32_t *items, int64_t n, float *X)
-{
-    int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    const int64_t total = n * d4, st = (int64_t)gridDim.x * blockDim.x;
-    for (; i < total; i += st) {
-        const int64_t s = i / d4, c = i - s * d4;
-        reinterpret_cast<float4 *>(X)[s * d4 + c] = reinterpret_cast<const float4 *>(Q)[(int64_t)items[s] * d4 + c];
-    }
-}
-
 // flag[s] = 1 for a live slot, flag[n] = 0: the input of the exclusive scan that renumbers the slots
 __global__ void vecdb_live_kernel(const uint8_t *dead, int64_t n, int64_t *flag)
 {
@@ -159,6 +148,7 @@ int32_t gorse_b200_vecdb_create(gorse_b200_ctx *ctx, int32_t dim, int32_t distan
     int32_t st = dim > 0 ? gorse_b200_index_create(ctx, dim, metric, &db->dense)
                          : gorse_b200_sparse_index_create(ctx, &db->sparse);
     if (st) { delete db; return st; }
+    if (db->dense) db->dense->value_bytes = 2;   // bf16 rows until a value that is not bf16-exact arrives (topk.cuh)
     *out = db;
     return GORSE_B200_OK;
 }
@@ -292,19 +282,20 @@ int32_t gorse_b200_vecdb_get(gorse_b200_vecdb *db, const int64_t *slots, int64_t
     std::lock_guard<std::mutex> lk(db->mu);
     const int64_t total = (int64_t)db->ts.size();
     ScopedDevice sd(db->ctx->device);
+    std::vector<int64_t> rows(values_out && db->dim > 0 ? (size_t)n : 0);   // the stored row of each entry, -1 for none
     for (int64_t i = 0; i < n; i++) {
         const int64_t s = slots[i];
         const bool ok = s >= 0 && s < total && !db->dead[(size_t)s];
         if (live_out) live_out[i] = ok;
         if (hidden_out) hidden_out[i] = ok ? db->hidden[(size_t)s] : 0;
         if (timestamp_out) timestamp_out[i] = ok ? db->ts[(size_t)s] : 0;
-        if (values_out && db->dim > 0) {
-            if (ok) GB_CUDA(cudaMemcpyAsync(values_out + i * db->dim, db->dense->X.p + s * db->dim, sizeof(float) * db->dim, cudaMemcpyDeviceToHost, db->ctx->stream));
-            else memset(values_out + i * db->dim, 0, sizeof(float) * db->dim);
+        if (!rows.empty()) {
+            rows[(size_t)i] = ok ? s : -1;
+            if (!ok) memset(values_out + i * db->dim, 0, sizeof(float) * db->dim);
         }
     }
-    GB_CUDA(cudaStreamSynchronize(db->ctx->stream));
-    return GORSE_B200_OK;
+    if (rows.empty()) return GORSE_B200_OK;
+    return index_download_rows(db->dense, rows.data(), n, values_out);
 }
 
 int32_t gorse_b200_vecdb_get_sparse(gorse_b200_vecdb *db, int64_t slot, uint32_t *indices_out, float *values_out, int32_t cap, int32_t *nnz_out)
@@ -383,6 +374,16 @@ int32_t gorse_b200_vecdb_compact(gorse_b200_vecdb *db, int64_t *new_slot_out, in
     if (new_slot_out)   // `dead` holds the old flags after the swap
         for (int64_t s = 0; s < n; s++) new_slot_out[s] = dead[(size_t)s] ? -1 : new_slot[(size_t)s];
     if (bytes_out) bytes_out[1] = vecdb_bytes(db);
+    return GORSE_B200_OK;
+}
+
+int32_t gorse_b200_vecdb_storage(gorse_b200_vecdb *db, int32_t *value_bytes_out, int64_t *device_bytes_out)
+{
+    GB_CHECK_ARG(db != nullptr, "collection is NULL");
+    std::lock_guard<std::mutex> lk(db->mu);
+    std::lock_guard<std::mutex> lk2(db->dense ? db->dense->mu : db->sparse->mu);
+    if (value_bytes_out) *value_bytes_out = db->dense ? db->dense->value_bytes : 0;
+    if (device_bytes_out) *device_bytes_out = vecdb_bytes(db);
     return GORSE_B200_OK;
 }
 
@@ -474,22 +475,10 @@ int32_t gorse_b200_vecdb_add_item_factors(gorse_b200_vecdb *db, gorse_b200_cf *c
     const int64_t n = (int64_t)items.size();
     if (n == 0) return GORSE_B200_OK;
     gorse_b200_index *ix = db->dense;
-    {
+    {   // the factor rows go device to device; a bf16 collection checks them there and promotes when one is not bf16-exact
         std::lock_guard<std::mutex> lk2(ix->mu);
-        GB_TRY(index_reserve(ix, ix->n + n));
-        GB_TRY(d_items.alloc((size_t)n));
-        e = cudaMemcpyAsync(d_items.p, items.data(), sizeof(int32_t) * (size_t)n, cudaMemcpyHostToDevice, c->stream);
-        if (e == cudaSuccess) {
-            if (cf->d % 4 == 0) vecdb_copy_rows_kernel<<<c->sm_count * 8, 256, 0, c->stream>>>(cf->Q.p, cf->d / 4, d_items.p, n, ix->X.p + ix->n * ix->d);
-            else for (int64_t s2 = 0; s2 < n && e == cudaSuccess; s2++)
-                e = cudaMemcpyAsync(ix->X.p + (ix->n + s2) * ix->d, cf->Q.p + (int64_t)items[(size_t)s2] * cf->d, sizeof(float) * cf->d, cudaMemcpyDeviceToDevice, c->stream);
-            c->launches++;
-            if (e == cudaSuccess) e = cudaGetLastError();
-        }
-        if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
-        if (e != cudaSuccess) { set_error("add_item_factors: %s", cudaGetErrorString(e)); return GORSE_B200_ERR_CUDA; }
-        ix->n += n;
-        ix->mma_ready = false;
+        GB_TRY(d_items.upload(items.data(), (size_t)n, c->stream));
+        GB_TRY(index_append(ix, cf->Q.p, d_items.p, n, false));
     }
     for (int64_t s2 = 0; s2 < n; s2++) {
         const int32_t it = items[(size_t)s2];

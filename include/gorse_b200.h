@@ -373,6 +373,14 @@ typedef enum {   /* vectors.Distance, storage/vectors/database.go:27-33 */
     GORSE_B200_DISTANCE_DOT = 2
 } gorse_b200_distance;
 typedef struct gorse_b200_vecdb gorse_b200_vecdb;
+/* Storage of a dense collection's rows: bf16 while every value it has been given is bf16-exact (a float32 whose low 16 bits are
+ * zero: +-0, +-Inf, subnormals and NaN payloads with zero low bits included), so 2 bytes a value; the first call that brings a
+ * value that is not (gorse_b200_vecdb_add, gorse_b200_vecdb_add_item_factors, gorse_b200_vecdb_load) promotes the collection
+ * to fp32, 4 bytes a value, before its rows land, widening the stored rows on the device in one pass.  Promotion is one-way:
+ * deleting or compacting away the inexact vectors does not demote.  An empty collection promotes for free.  If promotion
+ * cannot allocate, the call fails with GORSE_B200_ERR_CUDA and the collection is as it was.  Narrowing keeps the top 16 bits
+ * and widening is bits << 16, so every kernel sees exactly the fp32 values it was given: every answer, score bit, tie order
+ * and snapshot stream is the same in either storage.  There is no option; the bare index (gorse_b200_index_*) is fp32. */
 int32_t gorse_b200_vecdb_create(gorse_b200_ctx *ctx, int32_t dim, int32_t distance, gorse_b200_vecdb **out); /* AddCollection */
 int32_t gorse_b200_vecdb_destroy(gorse_b200_vecdb *db);                                                     /* DeleteCollection */
 /* CountVectors (xvec.go:274-286): live vectors; *slots_out = slots ever assigned */
@@ -429,6 +437,10 @@ int32_t gorse_b200_vecdb_delete_before(gorse_b200_vecdb *db, int64_t timestamp_m
  * any error the collection is unchanged.  Slots held by the caller (id maps, context and exclusion lists, per-slot
  * feedback rows and masks) must be renamed before they are passed again.  NULL db: GORSE_B200_ERR_ARG. */
 int32_t gorse_b200_vecdb_compact(gorse_b200_vecdb *db, int64_t *new_slot_out, int64_t *bytes_out);
+/* The storage of a collection (see gorse_b200_vecdb_create): *value_bytes_out (may be NULL) = 0 for a sparse collection, 2 for
+ * bf16 rows, 4 for fp32 rows; *device_bytes_out (may be NULL) = the device bytes the collection holds, counted as
+ * gorse_b200_vecdb_compact's bytes_out counts them.  NULL db: GORSE_B200_ERR_ARG. */
+int32_t gorse_b200_vecdb_storage(gorse_b200_vecdb *db, int32_t *value_bytes_out, int64_t *device_bytes_out);
 /* Snapshots: a collection written as a byte stream and rebuilt from one on any context (another device, another process), so
  * that a restarted master, a worker and a server hold the collections the master built (the reference's default backend keeps
  * each collection on disk and reopens it in Init, xvec.go:60-123).
@@ -468,6 +480,8 @@ int32_t gorse_b200_vecdb_compact(gorse_b200_vecdb *db, int64_t *new_slot_out, in
  *   through new_slot_out, the same score bits, the same tie order.  Later adds, deletes and compactions act on it as on the
  *   original.  Dense rows go from the callback into the device rows through two pinned staging buffers of at most 64 MB
  *   (the device rows are reserved once from the header); the bf16 mirror and the norms are built lazily, as after an add.
+ *   The stream's values are fp32 whatever the storage (gorse_b200_vecdb_create): save widens bf16 rows as it gathers them,
+ *   and load narrows each chunk on the device while it is bf16-exact and promotes the collection at the first chunk that is not.
  *   Sparse rows go into the index's CSR and the device CSC is built at once, so the first query starts without a rebuild.
  *   *bytes_out (may be NULL): the bytes read.  Every field is checked as gorse_b200_vecdb_add checks its arguments (dense
  *   values are taken as they are, as there): a wrong magic or version, an illegal dim / distance pair, a count that
