@@ -9,8 +9,8 @@
 //
 //   routing   rows with k_q <= 128 / 256 / 512 form classes; each class is swept by the tensor-core stage 1 (topk_mma.cu) with
 //             a sample aimed at min(4 x the class's largest k_q, CAP / 2) columns per row.  Rows above 512, calls the sweep does
-//             not serve (mma_path_eligible: small indexes, few rows, Cosine) and rows whose window cannot be certified go to
-//             the exact kernel.
+//             not serve (mma_path_eligible: small indexes, few rows, Cosine, d > 4096), calls whose mirror or work buffers
+//             cannot be allocated and rows whose window cannot be certified go to the exact kernel.
 //   stage 2   recall_window_kernel, one CTA per row: drops the candidates the filter rejects and the row's own vector,
 //             certifies the row against its own k_q (k_q-th best approximate score >= theta + 2 eps), re-scores the window
 //             exactly, sorts it in shared memory and writes the first k_q minus the row's exclusions.
@@ -297,7 +297,7 @@ int32_t recall_rows(gorse_b200_index *ix, const uint8_t *allow, int64_t nq, cons
     const int d = ix->d;
     auto out_at = [&](int64_t q) { return q * (int64_t)n + (excl_off ? excl_off[q] : 0); };
     const int64_t N = ix->n, total_out = out_at(nq);
-    const bool tensor = mma_path_eligible(ix, nq);
+    bool tensor = mma_path_eligible(ix, nq);
     const int64_t cq = std::min<int64_t>(nq, (int64_t)c->sm_count * mma::GROUP_ROWS * 8);
     // exact scratch: one [N] score row per CTA, at most 512 MB
     const int exact_grid = (int)std::max<int64_t>(1, std::min<int64_t>({(int64_t)c->sm_count * 2, cq, (512ll << 20) / (4 * N)}));
@@ -312,7 +312,10 @@ int32_t recall_rows(gorse_b200_index *ix, const uint8_t *allow, int64_t nq, cons
         (st = W.slots.grow((size_t)std::max<int64_t>(total_out, 1))) || (st = W.scores.grow((size_t)std::max<int64_t>(total_out, 1))) ||
         (st = W.scratch.grow((size_t)exact_grid * N)) || (st = W.ex.grow((size_t)std::max<int64_t>(excl_off ? ex_off[nq] : 0, 1))))
         return done(st);
-    if (tensor && (st = mma_reserve(ix, cq))) return done(st);
+    if (tensor && (st = mma_reserve(ix, cq))) {
+        if (st != GORSE_B200_ERR_OOM) return done(st);
+        tensor = false;   // no room for the mirror or the sweep's buffers: every row takes the exact kernel, with the same answers
+    }
     const RowView X = ix->rows();
     cudaError_t e = with_rows(X, [&](auto x) {
         using T = row_elem_t<decltype(x)>;

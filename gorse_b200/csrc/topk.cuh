@@ -86,7 +86,10 @@ namespace mma {
 constexpr int BM = 64, BN = 128, BK = 64;      // rows per consumer warpgroup (queries), tile columns (vectors), k-block (bf16)
 constexpr int CONSUMERS = 2;                   // consumer warpgroups per CTA; both multiply every B tile
 constexpr int GROUP_ROWS = CONSUMERS * BM;     // query rows of one CTA pass over all vectors
-constexpr int MAX_KB = 3;                      // k-blocks per tile: Kp <= 192
+constexpr int MAX_KB = 3;                      // k-blocks per tile with the queries resident: Kp <= 192
+constexpr int MAX_D = 4096;                    // the widest rows the sweep takes
+constexpr int WIDE_MAX_KB = (MAX_D + 2 + BK - 1) / BK;   // k-blocks per tile of the wide sweep (both operands streamed): Kp <= 4160
+                                               // with the two norm columns of Euclidean at d = 4096
 constexpr int CAP = 2048;                      // candidate slots per query row
 constexpr int PARTS = 4;                       // a row's columns are split over the 4 threads of an accumulator quad
 constexpr int PART_CAP = CAP / PARTS;          // candidate slots per (row, part)
@@ -94,6 +97,11 @@ constexpr int R_TOP = 16;                      // sample order statistic that fi
 constexpr int THREADS = 128 * (1 + CONSUMERS); // warpgroup 0: warp 0 = TMA producer, warps 1-3 idle; then the consumers
 constexpr uint32_t A_TILE_BYTES = BM * BK * 2; // one [64 x 64] bf16 k-block of queries = 8 KB
 constexpr uint32_t B_TILE_BYTES = BN * BK * 2; // one [128 x 64] bf16 k-block of vectors = 16 KB
+// a ring slot of the wide sweep: one k-block of both consumers' queries and of the vector tile = 32 KB.  6 slots (193 KB with
+// the alignment and barriers) leave about as much L1 beside the 227 KB shared-memory budget as the narrow sweep's ring does.
+constexpr uint32_t WIDE_STAGE_BYTES = CONSUMERS * A_TILE_BYTES + B_TILE_BYTES;
+constexpr int WIDE_STAGES = 6;
+static_assert(WIDE_STAGES * WIDE_STAGE_BYTES + 1024 + 256 <= 227 * 1024, "the wide ring fits the shared-memory budget");
 }  // namespace mma
 
 #ifdef __CUDACC__
@@ -228,7 +236,8 @@ int32_t index_compact(gorse_b200_index *ix, const int64_t *scan, int64_t live);
 // device bytes held by the index and its work buffers
 size_t index_bytes(const gorse_b200_index *ix);
 // the tensor-core candidate sweep (topk_mma.cu) of the top-k pipeline (recall_rows) and of the stage-1 test hook.
-// mma_reserve: the bf16 mirror and the work buffers for up to cq query rows per sweep.  mma_sample_tiles: the sample size
+// mma_reserve: the bf16 mirror and the work buffers for up to cq query rows per sweep; GORSE_B200_ERR_OOM when they do not fit,
+// with none of them held (the caller answers through the exact kernel).  mma_sample_tiles: the sample size
 // that leaves about `cands` columns per row above its threshold.  mma_sweep: query rows (q_base, d_q, d_qidx, q0 as in
 // build_queries_kernel) -> candidate lists in ix->w_ccol / w_cval / w_ccnt / w_theta, eps in ix->w_eps; ev0 / ev1 (may be
 // nullptr) are recorded around the sweep kernel.
@@ -236,7 +245,7 @@ int32_t mma_reserve(gorse_b200_index *ix, int64_t cq);
 int mma_sample_tiles(const gorse_b200_index *ix, double cands);
 int32_t mma_sweep(gorse_b200_index *ix, RowView q_base, const float *d_q, const int64_t *d_qidx, int64_t q0, int64_t nq, int m_tiles,
                   cudaEvent_t ev0, cudaEvent_t ev1);
-// the sweep serves Dot and Euclidean indexes of >= 32768 vectors for >= 64 rows; GORSE_B200_TOPK_EXACT=1 turns it off
+// the sweep serves Dot and Euclidean indexes of >= 32768 vectors, d <= 4096, for >= 64 rows; GORSE_B200_TOPK_EXACT=1 turns it off
 bool mma_path_eligible(const gorse_b200_index *ix, int64_t nq);
 
 namespace recall {

@@ -50,18 +50,23 @@ struct Params {
 // each consumer warpgroup multiplies its 64 query rows with every tile (8 or fewer wgmma, K = 16 each, into one 64 x 128
 // accumulator), waits, hands the ring slot back and examines the scores in registers.  The two consumers meet on the same
 // slots, so the tensor core runs one warpgroup's MMAs while the other examines its scores.
+// WIDE (Kp > BK * MAX_KB): the group's query rows no longer fit in shared memory beside the ring, so a ring slot holds ONE
+// k-block of both operands (the two consumers' query k-blocks and the tile's vector k-block, WIDE_STAGE_BYTES) and a tile
+// takes kb slots.  A consumer accumulates the tile's kb k-blocks, one wgmma group each, keeping one group in flight: the
+// slot of k-block j - 1 goes back to the producer once group j is issued.  The epilogue is the same code for both.
 // Accumulator fragment (wgmma.cuh): a thread holds 2 rows x 32 columns of a tile, and the 4 threads of a quad share their
 // rows; a (row, quad lane) pair is a PART with its own sample, candidate list and push count.  The 4 parts of a row merge
 // their 16 best into ONE threshold by shuffles.
-template <int STAGES, bool DBG>
+template <int STAGES, bool DBG, bool WIDE = false>
 __global__ void __launch_bounds__(THREADS, 1)
 topk_mma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b, Params P)
 {
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-    uint8_t *smem_a = smem;                                                  // [CONSUMERS][kb] query tiles
-    uint8_t *smem_b = smem_a + (size_t)CONSUMERS * P.kb * A_TILE_BYTES;      // [STAGES][kb] vector tiles
-    uint64_t *bars = reinterpret_cast<uint64_t *>(smem_b + (size_t)STAGES * P.kb * B_TILE_BYTES);
+    uint8_t *smem_a = smem;                                                  // [CONSUMERS][kb] query tiles (WIDE: the ring)
+    uint8_t *smem_b = smem_a + (size_t)CONSUMERS * P.kb * A_TILE_BYTES;      // [STAGES][kb] vector tiles (WIDE: unused)
+    uint64_t *bars = reinterpret_cast<uint64_t *>(WIDE ? smem + (size_t)STAGES * WIDE_STAGE_BYTES
+                                                       : smem_b + (size_t)STAGES * P.kb * B_TILE_BYTES);
     uint64_t *full = bars, *empty = bars + STAGES, *a_full = bars + 2 * STAGES, *a_empty = a_full + 1;
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -75,7 +80,26 @@ topk_mma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant
     __syncthreads();
     const int total_tiles = P.n_tiles + P.m_tiles;
 
-    if (warp == 0) {
+    if (WIDE && warp == 0) {
+        // ===== TMA producer of the k-block ring: slot `slot` of pass `phase`
+        uint32_t slot = 0, phase = 0;
+        for (int g = blockIdx.x; g < P.n_groups; g += gridDim.x)
+            for (int t = 0; t < total_tiles; t++) {
+                const int bt = t < P.n_tiles ? t : t - P.n_tiles;
+                for (int kb = 0; kb < P.kb; kb++) {
+                    mbar_wait_backoff(&empty[slot], phase ^ 1);
+                    if (elect_one()) {
+                        uint8_t *st = smem + (size_t)slot * WIDE_STAGE_BYTES;
+                        mbar_expect_tx(&full[slot], WIDE_STAGE_BYTES);
+                        for (int m = 0; m < CONSUMERS; m++)
+                            tma_load_2d(st + m * A_TILE_BYTES, &map_a, kb * BK, (g * CONSUMERS + m) * BM, &full[slot]);
+                        tma_load_2d(st + CONSUMERS * A_TILE_BYTES, &map_b, kb * BK, bt * BN, &full[slot]);
+                    }
+                    __syncwarp();
+                    if (++slot == STAGES) { slot = 0; phase ^= 1; }
+                }
+            }
+    } else if (warp == 0) {
         // ===== TMA producer: the warp waits together, one elected lane issues
         uint32_t it = 0, ag = 0;
         for (int g = blockIdx.x; g < P.n_groups; g += gridDim.x, ag++) {
@@ -104,8 +128,35 @@ topk_mma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant
         const int wg = (warp >> 2) - 1, quad = lane & 3;
         const uint32_t a_base = s32(smem_a) + (uint32_t)wg * (uint32_t)P.kb * A_TILE_BYTES, b_base = s32(smem_b);
         float acc[64];
-        // the MMAs of one ring slot into acc, then the slot goes back to the producer
-        auto mma_tile = [&](uint32_t s) {
+        uint32_t slot = 0, phase = 0;   // WIDE: the k-block ring's position, as the producer's
+        // the MMAs of tile `it` into acc; every ring slot it read goes back to the producer
+        auto mma_tile = [&](uint32_t it) {
+            if constexpr (WIDE) {
+                uint32_t prev = 0;
+                for (int kb = 0; kb < P.kb; kb++) {
+                    mbar_wait(&full[slot], phase);
+                    const uint32_t a_k = s32(smem) + slot * WIDE_STAGE_BYTES + (uint32_t)wg * A_TILE_BYTES;
+                    const uint32_t b_k = s32(smem) + slot * WIDE_STAGE_BYTES + CONSUMERS * A_TILE_BYTES;
+                    wgmma_fence();
+#pragma unroll
+                    for (int k = 0; k < BK / 16; k++)
+                        wgmma_m64n128k16_bf16(acc, wgmma_desc(a_k + (uint32_t)k * 32u), wgmma_desc(b_k + (uint32_t)k * 32u), (kb | k) != 0);
+                    wgmma_commit();
+                    if (kb > 0) {   // k-block kb - 1's group is done: its slot is free
+                        wgmma_wait<1>();
+                        __syncwarp();
+                        if (lane == 0) mbar_arrive(&empty[prev]);
+                    }
+                    prev = slot;
+                    if (++slot == STAGES) { slot = 0; phase ^= 1; }
+                }
+                wgmma_wait<0>();
+                __syncwarp();
+                if (lane == 0) mbar_arrive(&empty[prev]);
+                return;
+            }
+            const uint32_t s = it % STAGES;
+            mbar_wait(&full[s], (it / STAGES) & 1);
             const uint32_t b_slot = b_base + s * (uint32_t)P.kb * B_TILE_BYTES;
             wgmma_fence();
             for (int kb = 0; kb < P.kb; kb++) {
@@ -143,7 +194,7 @@ topk_mma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant
                         }
                 }
             };
-            mbar_wait(a_full, ag & 1);
+            if constexpr (!WIDE) mbar_wait(a_full, ag & 1);
             float theta[2];
             {
                 // ---- the sample: each part's R_TOP best scores of the first m_tiles tiles
@@ -161,9 +212,7 @@ topk_mma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant
                     }
                 };
                 for (int t = 0; t < P.m_tiles; t++, it++) {
-                    const uint32_t s = it % STAGES;
-                    mbar_wait(&full[s], (it / STAGES) & 1);
-                    mma_tile(s);
+                    mma_tile(it);
                     const int64_t col0 = (int64_t)t * BN + 2 * quad;
                     if constexpr (DBG) dump(col0);
 #pragma unroll
@@ -212,10 +261,8 @@ topk_mma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant
                 cval[h] = P.cand_val + base;
             }
             for (int t = P.m_tiles; t < total_tiles; t++, it++) {
-                const uint32_t s = it % STAGES;
                 const int bt = t < P.n_tiles ? t : t - P.n_tiles;
-                mbar_wait(&full[s], (it / STAGES) & 1);
-                mma_tile(s);
+                mma_tile(it);
                 const int64_t col0 = (int64_t)bt * BN + 2 * quad;
                 if constexpr (DBG) {
                     if (t < P.n_tiles) dump(col0);
@@ -250,8 +297,10 @@ topk_mma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant
 #pragma unroll
             for (int h = 0; h < 2; h++)
                 if (row_ok[h]) { P.cand_cnt[PARTS * row[h] + quad] = cnt[h]; P.theta[PARTS * row[h] + quad] = theta[h]; }
-            __syncwarp();
-            if (lane == 0) mbar_arrive(a_empty);   // this warp's MMAs of the group have all been waited for
+            if constexpr (!WIDE) {
+                __syncwarp();
+                if (lane == 0) mbar_arrive(a_empty);   // this warp's MMAs of the group have all been waited for
+            }
         }
     }
 }
@@ -419,10 +468,10 @@ static int kp_of(const gorse_b200_index *ix)
 bool mma_path_eligible(const gorse_b200_index *ix, int64_t nq)
 {
     if (const char *e = getenv("GORSE_B200_TOPK_EXACT")) if (*e == '1') return false;
-    const int kp = kp_of(ix);
-    // the sample needs >= 32 tiles to make theta tight; small problems are faster on the exact scan anyway
+    // the sample needs >= 32 tiles to make theta tight; small problems are faster on the exact scan anyway.  Kp <= 192: the
+    // kernel with the queries resident; up to d = 4096 the wide kernel; wider rows take the exact scan.
     if (ix->metric != GORSE_B200_METRIC_EUCLIDEAN && ix->metric != GORSE_B200_METRIC_NEG_DOT) return false;   // cosine (vecdb.cu): exact scan
-    return kp <= mma::BK * mma::MAX_KB && ix->n >= 32768 && nq >= 64 && ix->n < (1ll << 31);
+    return ix->d <= mma::MAX_D && ix->n >= 32768 && nq >= 64 && ix->n < (1ll << 31);
 }
 
 static int32_t ensure_mirror(gorse_b200_index *ix)
@@ -431,6 +480,8 @@ static int32_t ensure_mirror(gorse_b200_index *ix)
     gorse_b200_ctx *c = ix->ctx;
     const int kp = kp_of(ix);
     const int64_t n_pad = (ix->n + mma::BN - 1) / mma::BN * mma::BN;
+    if (const char *e = getenv("GORSE_B200_TOPK_MAX_MIRROR_BYTES"))   // tests of the exact fallback: a mirror that does not fit
+        if (2.0 * (double)n_pad * kp > atof(e)) { set_error("top-k mirror: %lld bytes over the limit", (long long)(2 * n_pad * kp)); return GORSE_B200_ERR_OOM; }
     GB_TRY(ix->Xb.alloc((size_t)n_pad * kp));
     GB_TRY(ix->norm.alloc((size_t)ix->n + 2));
     GB_TRY(ix->perm.alloc((size_t)ix->n));
@@ -456,7 +507,7 @@ static int32_t ensure_mirror(gorse_b200_index *ix)
     return GORSE_B200_OK;
 }
 
-int32_t mma_reserve(gorse_b200_index *ix, int64_t cq)
+static int32_t reserve(gorse_b200_index *ix, int64_t cq)
 {
     GB_TRY(ensure_mirror(ix));
     const int kp = kp_of(ix);
@@ -475,6 +526,19 @@ int32_t mma_reserve(gorse_b200_index *ix, int64_t cq)
     return GORSE_B200_OK;
 }
 
+int32_t mma_reserve(gorse_b200_index *ix, int64_t cq)
+{
+    const int32_t st = reserve(ix, cq);
+    if (st == GORSE_B200_ERR_OOM) {   // hold none of it: the exact kernel answers without it
+        ix->Xb.free(); ix->norm.free(); ix->perm.free();
+        ix->w_qb.free(); ix->w_eps.free(); ix->w_cval.free(); ix->w_theta.free(); ix->w_ccol.free(); ix->w_ccnt.free();
+        ix->mma_ready = false;
+        ix->w_cq = 0;
+        cudaGetLastError();   // the failed cudaMalloc's error is not the caller's
+    }
+    return st;
+}
+
 // sample size: the R_TOP-th best of m random columns leaves on average R_TOP * N / m columns above it (Gamma(R_TOP) spread)
 int mma_sample_tiles(const gorse_b200_index *ix, double cands)
 {
@@ -489,15 +553,19 @@ int32_t mma_sweep(gorse_b200_index *ix, RowView q_base, const float *d_q, const 
     gorse_b200_ctx *c = ix->ctx;
     const int kp = kp_of(ix), kb = kp / mma::BK;
     const int64_t n_pad = (ix->n + mma::BN - 1) / mma::BN * mma::BN;
-    // stages from the shared-memory budget (227 KB per block), at most 4: the epilogue's global traffic keeps some L1
+    // stages from the shared-memory budget (227 KB per block), at most 4: the epilogue's global traffic keeps some L1.
+    // Kp > 192: the wide kernel's k-block ring (WIDE_STAGES slots of WIDE_STAGE_BYTES).
+    const bool wide = kb > mma::MAX_KB;
     const size_t a_bytes = (size_t)mma::CONSUMERS * kb * mma::A_TILE_BYTES, b_stage = (size_t)kb * mma::B_TILE_BYTES;
-    const int stages = (int)std::min<size_t>(4, (227 * 1024 - 1280 - a_bytes) / b_stage);
-    if (stages < 2) { set_error("mma_sweep: Kp = %d does not fit", kp); return GORSE_B200_ERR_UNSUPPORTED; }
-    const size_t smem = a_bytes + (size_t)stages * b_stage + 1024 /*align*/ + 256 /*barriers*/;
+    const int stages = wide ? mma::WIDE_STAGES : (int)std::min<size_t>(4, (227 * 1024 - 1280 - a_bytes) / b_stage);
+    if (kb > mma::WIDE_MAX_KB || stages < 2) { set_error("mma_sweep: Kp = %d does not fit", kp); return GORSE_B200_ERR_UNSUPPORTED; }
+    const size_t smem = (wide ? (size_t)mma::WIDE_STAGES * mma::WIDE_STAGE_BYTES : a_bytes + (size_t)stages * b_stage) + 1024 /*align*/ +
+                        256 /*barriers*/;
     const bool dbg = ix->dbg_scores != nullptr;   // the dense score dump of the test hook is compiled out of the production kernel
     auto pick = [&](auto s4, auto s3, auto s2) { return stages >= 4 ? s4 : stages == 3 ? s3 : s2; };
-    auto kern = dbg ? pick(mma::topk_mma_kernel<4, true>, mma::topk_mma_kernel<3, true>, mma::topk_mma_kernel<2, true>)
-                    : pick(mma::topk_mma_kernel<4, false>, mma::topk_mma_kernel<3, false>, mma::topk_mma_kernel<2, false>);
+    auto kern = wide ? (dbg ? mma::topk_mma_kernel<mma::WIDE_STAGES, true, true> : mma::topk_mma_kernel<mma::WIDE_STAGES, false, true>)
+                : dbg ? pick(mma::topk_mma_kernel<4, true>, mma::topk_mma_kernel<3, true>, mma::topk_mma_kernel<2, true>)
+                      : pick(mma::topk_mma_kernel<4, false>, mma::topk_mma_kernel<3, false>, mma::topk_mma_kernel<2, false>);
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) { set_error("mma_sweep smem attr: %s", cudaGetErrorString(e)); return GORSE_B200_ERR_CUDA; }
     CUtensorMap map_a, map_b;

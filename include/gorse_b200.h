@@ -294,6 +294,10 @@ int32_t gorse_b200_index_search_indices(gorse_b200_index *ix, const int64_t *q_i
  * (what logics.item_to_item asks its vector store for, logics/item_to_item.go:50-62) */
 int32_t gorse_b200_index_search_range(gorse_b200_index *ix, int64_t q0, int64_t q1, int32_t k, int32_t prune0,
                                       int32_t *idx_out, float *dist_out, int32_t *count_out);
+/* The searches of an index of >= 32768 vectors, Dot or Euclidean, d <= 4096, for >= 64 rows take a tensor-core candidate
+ * sweep (bf16 mirror of 2 Kp bytes per vector, Kp = d [+ 2 for Euclidean] rounded up to 64, built on the first such call)
+ * and an exact re-rank; other calls, rows whose candidates cannot be certified and calls for which the mirror or its work
+ * buffers cannot be allocated take the exact scan.  The answers do not depend on the path. */
 /* measurement hook (bench.py), like gorse_b200_ctx_timer_*: since the previous call, the device time (ms) and algorithmic
  * flop (2 nq N d) of the tensor-core candidate sweep, and the number of query rows that were redone by the exact scan because
  * their candidate set could not be certified.  Any pointer may be NULL. */
