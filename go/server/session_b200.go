@@ -20,12 +20,14 @@ import (
 
 	mapset "github.com/deckarep/golang-set/v2"
 	"github.com/gorse-io/gorse/common/expression"
+	"github.com/gorse-io/gorse/common/log"
 	"github.com/gorse-io/gorse/config"
 	"github.com/gorse-io/gorse/storage"
 	"github.com/gorse-io/gorse/storage/cache"
 	"github.com/gorse-io/gorse/storage/data"
 	"github.com/gorse-io/gorse/storage/vectors"
 	"github.com/samber/lo"
+	"go.uber.org/zap"
 )
 
 // sessionRequest is one posted session after the handler's pre-processing: its feedback sorted by data.SortFeedbacks, the
@@ -84,6 +86,12 @@ func (s *RestServer) sessionRecommendB200(ctx context.Context, cfg config.ItemTo
 				}
 			}
 			return lo.Map(ids, func(id string, _ int) bool { return visible.Contains(id) }), nil
+		}
+		// the neighbour rows of earlier requests serve this one; answers do not depend on the cache, so the request goes on
+		// without it whatever NeighbourCache returns
+		if err := store.NeighbourCache(vectors.ItemToItemCollection(cfg.Name), s.Config.Recommend.CacheSize); err != nil &&
+			!errors.Is(err, storage.ErrNotSupported) {
+			log.Logger().Warn("session recommendation without the neighbour cache", zap.Error(err))
 		}
 		rows, err := store.SessionRecommend(ctx, vectors.ItemToItemCollection(cfg.Name), contextIds, excludeIds, itemOK,
 			s.Config.Recommend.CacheSize, s.Config.Recommend.ContextSize, top, scoreScale)

@@ -39,6 +39,7 @@ import (
 	"encoding/binary"
 	"fmt"
 	"io"
+	"net/url"
 	"os"
 	"path/filepath"
 	"runtime"
@@ -59,8 +60,13 @@ import (
 
 const b200Prefix = "b200://"
 
+// the device memory one collection's neighbour cache may take unless the URL sets neighbour_cache_mb
+const b200NeighbourCacheMB = 1024
+
 func init() {
 	Register([]string{b200Prefix}, func(path, tablePrefix string, opts ...storage.Option) (Database, error) {
+		// b200://<device>[/<root>][?neighbour_cache_mb=<MB>]
+		path, query, _ := strings.Cut(path, "?")
 		dev, root, _ := strings.Cut(strings.TrimPrefix(path, b200Prefix), "/")
 		device, err := strconv.Atoi(dev)
 		if err != nil {
@@ -69,7 +75,21 @@ func init() {
 		if root != "" {
 			root = "/" + root
 		}
-		return &B200{device: device, tablePrefix: tablePrefix, root: root, collections: map[string]*b200Collection{}}, nil
+		cacheMB := int64(b200NeighbourCacheMB)
+		q, err := url.ParseQuery(query)
+		if err != nil {
+			return nil, errors.Annotatef(err, "b200 store URL %q", path)
+		}
+		if q.Has("neighbour_cache_mb") {
+			// a typo must not leave the default budget in place: anything but a whole number of MB in [0, 2^30] is refused
+			mb, err := strconv.ParseInt(q.Get("neighbour_cache_mb"), 10, 64)
+			if err != nil || mb < 0 || mb > 1<<30 {
+				return nil, errors.Errorf("b200 store URL: neighbour_cache_mb = %q is not a number of MB in [0, 2^30] (0 turns the cache off)",
+					q.Get("neighbour_cache_mb"))
+			}
+			cacheMB = mb
+		}
+		return &B200{device: device, tablePrefix: tablePrefix, root: root, cacheMB: cacheMB, collections: map[string]*b200Collection{}}, nil
 	})
 }
 
@@ -95,6 +115,7 @@ type B200 struct {
 	device      int
 	tablePrefix string
 	root        string // "" = nothing is kept on disk
+	cacheMB     int64  // neighbour cache budget per collection, MB (0 = off)
 	ctx         *C.gorse_b200_ctx
 	collections map[string]*b200Collection
 	stop        chan struct{}
@@ -859,6 +880,37 @@ func (db *B200) UserToUserRecommend(ctx context.Context, collection string, user
 		results[i] = row
 	}
 	return results, nil
+}
+
+// NeighbourCache keeps the first n neighbours of the collection's vectors on the device between the item-to-item, session
+// and user-to-user calls that ask for n neighbours without a category filter (gorse_b200_vecdb_neighbour_cache); every
+// answer stays the same.  The pool holds min(live vectors, neighbour_cache_mb MB / (8 n + 4)) rows; the per-call work
+// buffers of a cached call (the rows it computes and each table row's source, about 8 n + 12 bytes per row of the call)
+// come on top of that budget.  The cache empties itself when the collection changes.  A reload replaces the collection's
+// handle, which starts without a cache, so callers call this before each batch or request: with the same n and size it
+// keeps what it holds and does nothing else.  With neighbour_cache_mb = 0, or an n outside [1, 1024] (which the
+// neighbour entries themselves refuse or skip), it does nothing and returns nil.  An error wrapping
+// storage.ErrNotSupported is a collection the cache does not serve (Cosine, or a sparse one with n above 128).  Answers do
+// not depend on the cache, so a caller may go on without it after any error.
+func (db *B200) NeighbourCache(name string, n int) error {
+	if db.cacheMB == 0 || n < 1 || n > 1024 {
+		return nil
+	}
+	if err := db.refresh(name); err != nil {
+		return err
+	}
+	db.mu.RLock()
+	defer db.mu.RUnlock()
+	c, err := db.collection(name)
+	if err != nil {
+		return err
+	}
+	rows := min(int64(len(c.slotOf)), (db.cacheMB<<20)/(8*int64(n)+4))
+	st := C.gorse_b200_vecdb_neighbour_cache(c.handle, C.int32_t(n), C.int64_t(rows))
+	if st == C.GORSE_B200_ERR_UNSUPPORTED { // a Cosine collection, or n above 128 for a sparse one
+		return fmt.Errorf("%s: %w", C.GoString(C.gorse_b200_last_error()), storage.ErrNotSupported)
+	}
+	return b200Err(st)
 }
 
 // SessionRecommend answers the REST server's session recommendation (RestServer.sessionRecommend, server/rest.go:1069-1173)

@@ -25,12 +25,17 @@ package worker
 import "C"
 
 import (
+	"errors"
 	"fmt"
 	"strings"
 	"unsafe"
 
+	"github.com/gorse-io/gorse/common/log"
 	"github.com/gorse-io/gorse/config"
 	"github.com/gorse-io/gorse/logics"
+	"github.com/gorse-io/gorse/storage"
+	"github.com/gorse-io/gorse/storage/vectors"
+	"go.uber.org/zap"
 )
 
 // B200Stage is one recommender of the sequence.  Kind is a gorse_b200_stage_kind; Name is the configured full name.  The
@@ -86,6 +91,28 @@ func B200Stages(cfg *config.RecommendConfig) ([]B200Stage, error) {
 		stages = append(stages, s)
 	}
 	return stages, nil
+}
+
+// B200NeighbourCaches turns on the neighbour cache of every item-to-item and user-to-user stage's collection for the
+// stage's N (CacheSize) before B200Recommend, so that the batches of a worker pass reuse the neighbour rows earlier batches
+// computed ((*vectors.B200).NeighbourCache).  Call it before every batch: a reload replaces a collection's handle, and with
+// an unchanged size the call keeps what the cache holds.  Answers do not depend on the cache, so a stage whose collection
+// it cannot serve, or whose sizing fails, runs without it; a failure other than storage.ErrNotSupported is logged.
+func B200NeighbourCaches(store *vectors.B200, stages []B200Stage) {
+	for _, s := range stages {
+		var collection string
+		switch s.Kind {
+		case C.GORSE_B200_STAGE_ITEM_TO_ITEM:
+			collection = vectors.ItemToItemCollection(strings.TrimPrefix(s.Name, logics.ItemToItemRecommender))
+		case C.GORSE_B200_STAGE_USER_TO_USER:
+			collection = vectors.UserToUserCollection(strings.TrimPrefix(s.Name, logics.UserToUserRecommender))
+		default:
+			continue
+		}
+		if err := store.NeighbourCache(collection, int(s.N)); err != nil && !errors.Is(err, storage.ErrNotSupported) {
+			log.Logger().Warn("recommender without the neighbour cache", zap.String("recommender", s.Name), zap.Error(err))
+		}
+	}
 }
 
 // B200CF is the CF recall input (updateCollaborativeRecommend, pipeline.go:403-449).

@@ -533,6 +533,20 @@ class VectorCollection:
         check(lib.gorse_b200_vecdb_storage(self.h, C.byref(vb), C.byref(nbytes)))
         return vb.value, nbytes.value
 
+    def neighbour_cache(self, n, rows):
+        """Keep the first n neighbours of up to `rows` stored vectors on the device between calls
+        (gorse_b200_vecdb_neighbour_cache): item_to_item, session_recommend, user_to_user and the gorse_b200 recommend stages
+        with this n and no category filter reuse them until the collection changes, with every answer unchanged.  rows = 0
+        turns the cache off; the same (n, rows) again keeps what it holds."""
+        check(lib.gorse_b200_vecdb_neighbour_cache(self.h, int(n), int(rows)))
+
+    def neighbour_cache_stats(self):
+        """gorse_b200_vecdb_neighbour_cache_stats -> {n, capacity, rows, device_bytes, served, computed, emptied}: the last
+        three since the cache was sized (rows served from it, rows computed for it, times a change of the collection emptied it)"""
+        s = np.zeros(7, np.int64)
+        check(lib.gorse_b200_vecdb_neighbour_cache_stats(self.h, ptr(s)))
+        return dict(zip(("n", "capacity", "rows", "device_bytes", "served", "computed", "emptied"), (int(x) for x in s)))
+
     def save(self, fileobj):
         """Write the collection to a binary file object as a snapshot stream (gorse_b200_vecdb_save; the format is in
         include/gorse_b200.h).  The collection does not change.

@@ -13,7 +13,8 @@
 //             row never returns its own vector), and its table keeps Dot scores > 0 only.  Sparse collections run
 //             the tiled sparse search (sparse.cu) on the list of stored rows (a row never finds itself; it keeps positive dots only).
 //             The table holds n (int32 slot, float32 score) entries per item, scores bit-identical to gorse_b200_vecdb_query.
-//             A session's walk cannot stop at its cut here: whether an entry counts depends on its filtered list.
+//             A session's walk cannot stop at its cut here: whether an entry counts depends on its filtered list.  With the
+//             collection's neighbour cache on, only the rows it does not hold are computed (neighbour_table, below).
 //   stage B   i2i_aggregate_kernel, one CTA per user: for a session, first the cut (context_cut); then walks C_u (the
 //             session's prefix) in order and adds s = (double)score * scale (Euclidean: 1 / (1 - s)) per neighbour slot that
 //             item_ok passes and that is not in E_u, with a barrier between context entries so that every sum is formed in
@@ -200,7 +201,6 @@ int32_t neighbour_sums(gorse_b200_vecdb *db, const char *name, int64_t n_users, 
     }
     gorse_b200_ctx *c = db->ctx;
     ScopedDevice sd(c->device);
-    GB_TRY(vecdb_allow(db, categories, n_categories));
     ItemToItemWork &V = db->i2i;
     int32_t st = GORSE_B200_OK;
     auto done = [&](int32_t s) {
@@ -211,13 +211,12 @@ int32_t neighbour_sums(gorse_b200_vecdb *db, const char *name, int64_t n_users, 
     if ((st = V.nb.grow((size_t)R)) || (st = V.t_slot.grow((size_t)R * n)) || (st = V.t_score.grow((size_t)R * n)) || (st = V.t_cnt.grow((size_t)R)) ||
         (item_ok && (st = V.item_ok.grow((size_t)n_slots))))
         return done(st);
-    cudaError_t e = cudaMemcpyAsync(V.nb.p, nb.data(), sizeof(int64_t) * R, cudaMemcpyHostToDevice, c->stream);
-    if (e == cudaSuccess && item_ok) e = cudaMemcpyAsync(V.item_ok.p, item_ok, (size_t)n_slots, cudaMemcpyHostToDevice, c->stream);
+    cudaError_t e = item_ok ? cudaMemcpyAsync(V.item_ok.p, item_ok, (size_t)n_slots, cudaMemcpyHostToDevice, c->stream) : cudaSuccess;
     if (e != cudaSuccess) { set_error("%s upload: %s", name, cudaGetErrorString(e)); return done(GORSE_B200_ERR_CUDA); }
 
     // ---- stage A: the neighbour table
     int64_t exact_rows = 0;
-    if ((st = neighbour_table(db, R, V.nb.p, n, V.t_slot.p, V.t_score.p, V.t_cnt.p, &exact_rows))) return done(st);
+    if ((st = neighbour_table(db, nb, V.nb.p, n, categories, n_categories, V.t_slot.p, V.t_score.p, V.t_cnt.p, &exact_rows))) return done(st);
     if ((e = cudaGetLastError()) != cudaSuccess) { set_error("%s: %s", name, cudaGetErrorString(e)); return done(GORSE_B200_ERR_CUDA); }
 
     // ---- stage B: users in chunks; a finished chunk is downloaded on the copy stream while the next one computes
@@ -285,8 +284,9 @@ int32_t neighbour_sums(gorse_b200_vecdb *db, const char *name, int64_t n_users, 
 
 }  // namespace i2i
 
-int32_t neighbour_table(gorse_b200_vecdb *db, int64_t R, const int64_t *d_nb, int n, int32_t *t_slot, float *t_score, int32_t *t_cnt,
-                        int64_t *exact_rows)
+// stage A proper: the table rows of the R stored vectors d_nb (device) under db->d_allow
+static int32_t compute_rows(gorse_b200_vecdb *db, int64_t R, const int64_t *d_nb, int n, int32_t *t_slot, float *t_score, int32_t *t_cnt,
+                            int64_t *exact_rows)
 {
     if (db->dim > 0) {
         std::lock_guard<std::mutex> lk2(db->dense->mu);
@@ -298,9 +298,160 @@ int32_t neighbour_table(gorse_b200_vecdb *db, int64_t R, const int64_t *d_nb, in
     return sparse_search_rows(db->sparse, d_nb, R, db->d_allow.p, n, t_slot, t_score, t_cnt);
 }
 
+constexpr int ASSEMBLE_THREADS = 256;
+
+// The call's table from the neighbour cache and the rows stage A computed, one warp per table row r: src[r] >= 0 is the
+// pool row that holds r, else r is computed row m = -1 - src[r], and ins[m] >= 0 is the pool row it is also stored in.
+// Only the first cnt entries of a row are read by stage B, so only they are copied.
+__global__ void __launch_bounds__(ASSEMBLE_THREADS)
+ncache_assemble_kernel(const int32_t *src, const int32_t *ins, int64_t R, int n, const int32_t *m_slot, const float *m_score, const int32_t *m_cnt,
+                       uint2 *pool, int32_t *pool_cnt, int32_t *t_slot, float *t_score, int32_t *t_cnt)
+{
+    const int64_t r = ((int64_t)blockIdx.x * ASSEMBLE_THREADS + threadIdx.x) >> 5;
+    const int lane = threadIdx.x & 31;
+    if (r >= R) return;
+    const int32_t s = src[r];
+    int32_t *ts = t_slot + r * n;
+    float *tv = t_score + r * n;
+    if (s >= 0) {
+        const uint2 *e = pool + (int64_t)s * n;
+        const int c = pool_cnt[s];
+        for (int j = lane; j < c; j += 32) {
+            const uint2 x = e[j];
+            ts[j] = (int32_t)x.x;
+            tv[j] = __uint_as_float(x.y);
+        }
+        if (lane == 0) t_cnt[r] = c;
+        return;
+    }
+    const int64_t m = -1 - (int64_t)s;
+    const int32_t p = ins[m];
+    const int c = m_cnt[m];
+    const int32_t *ms = m_slot + m * n;
+    const float *mv = m_score + m * n;
+    uint2 *e = pool + (int64_t)max(p, 0) * n;
+    for (int j = lane; j < c; j += 32) {
+        const int32_t slot = ms[j];
+        const float score = mv[j];
+        ts[j] = slot;
+        tv[j] = score;
+        if (p >= 0) e[j] = make_uint2((uint32_t)slot, __float_as_uint(score));
+    }
+    if (lane == 0) {
+        t_cnt[r] = c;
+        if (p >= 0) pool_cnt[p] = c;
+    }
+}
+
+// the cache as it was turned on: nothing held, every slot of the collection's current generation unknown
+static void ncache_reset(gorse_b200_vecdb *db)
+{
+    NeighbourCache &K = db->ncache;
+    K.used = 0;
+    K.row_of_slot.assign(db->ts.size(), -1);
+    K.gen = db->gen;
+}
+
+int32_t neighbour_table(gorse_b200_vecdb *db, const std::vector<int64_t> &nb, int64_t *d_nb, int n, const int32_t *categories,
+                        int32_t n_categories, int32_t *t_slot, float *t_score, int32_t *t_cnt, int64_t *exact_rows)
+{
+    gorse_b200_ctx *c = db->ctx;
+    const int64_t R = (int64_t)nb.size();
+    GB_TRY(vecdb_allow(db, categories, n_categories));
+    NeighbourCache &K = db->ncache;
+    if (K.cap == 0 || n != K.n || n_categories > 0) {
+        GB_CUDA(cudaMemcpyAsync(d_nb, nb.data(), sizeof(int64_t) * R, cudaMemcpyHostToDevice, c->stream));
+        return compute_rows(db, R, d_nb, n, t_slot, t_score, t_cnt, exact_rows);
+    }
+    if (K.gen != db->gen) {
+        if (K.used > 0) K.emptied++;
+        ncache_reset(db);
+    }
+    // hits and misses; a miss takes the next free pool row while there is one
+    std::vector<int32_t> src((size_t)R);
+    std::vector<int64_t> miss;
+    std::vector<int32_t> ins;
+    for (int64_t r = 0; r < R; r++) {
+        int32_t &p = K.row_of_slot[(size_t)nb[(size_t)r]];
+        if (p >= 0) {
+            src[(size_t)r] = p;
+            continue;
+        }
+        src[(size_t)r] = -1 - (int32_t)miss.size();
+        miss.push_back(nb[(size_t)r]);
+        ins.push_back(K.used < K.cap ? (int32_t)K.used++ : -1);
+        p = ins.back();
+    }
+    const int64_t M = (int64_t)miss.size();
+    src.insert(src.end(), ins.begin(), ins.end());
+    auto fail = [&](int32_t st) {   // the rows claimed above may not have been written
+        ncache_reset(db);
+        return st;
+    };
+    int32_t st = GORSE_B200_OK;
+    if (exact_rows) *exact_rows = 0;
+    if (M > 0) {
+        if ((st = K.m_slot.grow((size_t)M * n)) || (st = K.m_score.grow((size_t)M * n)) || (st = K.m_cnt.grow((size_t)M))) return fail(st);
+        cudaError_t e = cudaMemcpyAsync(d_nb, miss.data(), sizeof(int64_t) * M, cudaMemcpyHostToDevice, c->stream);
+        if (e != cudaSuccess) { set_error("neighbour cache upload: %s", cudaGetErrorString(e)); return fail(GORSE_B200_ERR_CUDA); }
+        if ((st = compute_rows(db, M, d_nb, n, K.m_slot.p, K.m_score.p, K.m_cnt.p, exact_rows))) return fail(st);
+    }
+    if ((st = K.src.upload(src.data(), src.size(), c->stream))) return fail(st);
+    ncache_assemble_kernel<<<div_up(R * 32, ASSEMBLE_THREADS), ASSEMBLE_THREADS, 0, c->stream>>>(
+        K.src.p, K.src.p + R, R, n, K.m_slot.p, K.m_score.p, K.m_cnt.p, K.entry.p, K.cnt.p, t_slot, t_score, t_cnt);
+    c->launches++;
+    const cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) { set_error("neighbour cache: %s", cudaGetErrorString(e)); return fail(GORSE_B200_ERR_CUDA); }
+    K.served += R - M;
+    K.computed += M;
+    return GORSE_B200_OK;
+}
+
 }  // namespace gb
 
 using namespace gb;
+
+extern "C" int32_t gorse_b200_vecdb_neighbour_cache(gorse_b200_vecdb *db, int32_t n, int64_t rows)
+{
+    GB_CHECK_ARG(rows >= 0, "negative rows");
+    GB_CHECK_ARG(n >= 1 && n <= MAX_N_DENSE, "n = %d outside [1, %d]", n, MAX_N_DENSE);
+    GB_CHECK_ARG(db != nullptr, "collection is NULL");
+    if (db->distance == GORSE_B200_DISTANCE_COSINE) {
+        set_error("neighbour cache: no neighbour entry serves a Cosine collection");
+        return GORSE_B200_ERR_UNSUPPORTED;
+    }
+    if (db->dim == 0 && n > MAX_N_SPARSE) {
+        set_error("neighbour cache: n = %d above %d for a sparse collection", n, MAX_N_SPARSE);
+        return GORSE_B200_ERR_UNSUPPORTED;
+    }
+    std::lock_guard<std::mutex> lk(db->mu);
+    NeighbourCache &K = db->ncache;
+    if (rows == K.cap && (rows == 0 || n == K.n)) return GORSE_B200_OK;
+    GB_CHECK_ARG(rows <= INT32_MAX, "rows = %lld above 2^31 - 1", (long long)rows);
+    ScopedDevice sd(db->ctx->device);   // the old pool is freed on the collection's device too
+    if (rows == 0) {
+        K = NeighbourCache();
+        return GORSE_B200_OK;
+    }
+    NeighbourCache fresh;   // allocated before the old pool goes, so a failure leaves the cache as it was
+    GB_TRY(fresh.entry.alloc((size_t)rows * n));
+    GB_TRY(fresh.cnt.alloc((size_t)rows));
+    fresh.n = n;
+    fresh.cap = rows;
+    K = std::move(fresh);
+    ncache_reset(db);
+    return GORSE_B200_OK;
+}
+
+extern "C" int32_t gorse_b200_vecdb_neighbour_cache_stats(gorse_b200_vecdb *db, int64_t *stats_out)
+{
+    GB_CHECK_ARG(db != nullptr && stats_out != nullptr, "NULL collection or stats_out");
+    std::lock_guard<std::mutex> lk(db->mu);
+    const NeighbourCache &K = db->ncache;
+    const int64_t s[7] = {K.cap ? K.n : 0, K.cap, K.used, (int64_t)K.bytes(), K.served, K.computed, K.emptied};
+    std::copy(s, s + 7, stats_out);
+    return GORSE_B200_OK;
+}
 
 extern "C" int32_t gorse_b200_vecdb_item_to_item(gorse_b200_vecdb *db, int64_t n_users, const int64_t *ctx_off, const int64_t *ctx_slots,
                                                  const int64_t *excl_off, const int64_t *excl_slots, const int32_t *categories,

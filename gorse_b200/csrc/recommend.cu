@@ -718,12 +718,13 @@ extern "C" int32_t gorse_b200_recommend(gorse_b200_ctx *ctx, int64_t n_users, co
                 return done(rs);
         }
         if (R == 0) continue;
-        if ((rs = D.d_nb.upload(D.nb.data(), (size_t)R, st)) || (rs = D.t_slot.grow((size_t)R * g.n)) ||
-            (rs = D.t_score.grow((size_t)R * g.n)) || (rs = D.t_cnt.grow((size_t)R)))
+        if ((rs = D.d_nb.grow((size_t)R)) || (rs = D.t_slot.grow((size_t)R * g.n)) || (rs = D.t_score.grow((size_t)R * g.n)) ||
+            (rs = D.t_cnt.grow((size_t)R)))
             return done(rs);
-        if ((rs = vecdb_allow(g.db, i2i ? g.categories : nullptr, i2i ? g.n_categories : 0))) return done(rs);
         int64_t exact = 0;
-        if ((rs = neighbour_table(g.db, R, D.d_nb.p, g.n, D.t_slot.p, D.t_score.p, D.t_cnt.p, &exact))) return done(rs);
+        if ((rs = neighbour_table(g.db, D.nb, D.d_nb.p, g.n, i2i ? g.categories : nullptr, i2i ? g.n_categories : 0, D.t_slot.p, D.t_score.p,
+                                  D.t_cnt.p, &exact)))
+            return done(rs);
         exact_total += exact;
     }
     // the CF recall rows stay in the CF index's recall buffers; computed after every neighbour table, which may use the same index

@@ -414,6 +414,7 @@ int32_t load(gorse_b200_ctx *ctx, gorse_b200_read_fn read, void *user, gorse_b20
     db->cats.swap(cats);
     db->live = n;
     db->meta_dirty = true;
+    db->gen++;
     *out = db;
     if (bytes_out) *bytes_out = r.pos;
     return GORSE_B200_OK;

@@ -13,12 +13,14 @@ namespace gb {
 constexpr int MAX_N_DENSE = 1024;                // the sort buffer of agg::select_first_n holds n (session: top) entries
 constexpr int MAX_N_SPARSE = 128;                // the sparse search's k
 
-// stage A of every neighbour recommender: the first n neighbours of each of the R stored vectors d_nb[R] (device) of db, as
-// a table of n (int32 slot, float32 score) entries per row, Dot collections keeping scores > 0 only (dense: the index's top-k
-// pipeline; sparse: sparse_search_rows).  The caller holds db->mu and has filled db->d_allow.  *exact_rows: rows of the exact
-// scan.
-int32_t neighbour_table(gorse_b200_vecdb *db, int64_t R, const int64_t *d_nb, int n, int32_t *t_slot, float *t_score, int32_t *t_cnt,
-                        int64_t *exact_rows);
+// stage A of every neighbour recommender: the first n neighbours of each of the distinct stored vectors nb (host slots) of db
+// among the vectors that pass categories[n_categories] (vecdb_allow runs here), as a table of n (int32 slot, float32 score)
+// entries per row, Dot collections keeping scores > 0 only (dense: the index's top-k pipeline; sparse: sparse_search_rows).
+// A call with the neighbour cache's n and no category filter takes the rows the cache holds and computes only the others
+// (gorse_b200_vecdb_neighbour_cache); every row is the same either way.  d_nb: device scratch of nb.size() entries.  The
+// caller holds db->mu.  *exact_rows: computed rows the exact scan answered.
+int32_t neighbour_table(gorse_b200_vecdb *db, const std::vector<int64_t> &nb, int64_t *d_nb, int n, const int32_t *categories,
+                        int32_t n_categories, int32_t *t_slot, float *t_score, int32_t *t_cnt, int64_t *exact_rows);
 
 struct NeighbourTable {       // stage A: the first n neighbours of each distinct query
     const int32_t *slot;      // [rows x n]

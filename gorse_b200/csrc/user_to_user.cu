@@ -235,7 +235,6 @@ extern "C" int32_t gorse_b200_vecdb_user_to_user(gorse_b200_vecdb *db, int64_t n
 
     gorse_b200_ctx *c = db->ctx;
     ScopedDevice sd(c->device);
-    GB_TRY(vecdb_allow(db, nullptr, 0));
     UserToUserWork &V = db->u2u;
     int32_t st = GORSE_B200_OK;
     auto done = [&](int32_t s) {
@@ -245,12 +244,11 @@ extern "C" int32_t gorse_b200_vecdb_user_to_user(gorse_b200_vecdb *db, int64_t n
     };
     if ((st = V.nb.grow((size_t)R)) || (st = V.t_slot.grow((size_t)R * n)) || (st = V.t_score.grow((size_t)R * n)) || (st = V.t_cnt.grow((size_t)R)))
         return done(st);
-    cudaError_t e = cudaMemcpyAsync(V.nb.p, nb.data(), sizeof(int64_t) * R, cudaMemcpyHostToDevice, c->stream);
-    if (e != cudaSuccess) { set_error("user_to_user upload: %s", cudaGetErrorString(e)); return done(GORSE_B200_ERR_CUDA); }
 
     // ---- stage A: the neighbour table
     int64_t exact_rows = 0;
-    if ((st = neighbour_table(db, R, V.nb.p, n, V.t_slot.p, V.t_score.p, V.t_cnt.p, &exact_rows))) return done(st);
+    if ((st = neighbour_table(db, nb, V.nb.p, n, nullptr, 0, V.t_slot.p, V.t_score.p, V.t_cnt.p, &exact_rows))) return done(st);
+    cudaError_t e;
     if ((e = cudaGetLastError()) != cudaSuccess) { set_error("user_to_user: %s", cudaGetErrorString(e)); return done(GORSE_B200_ERR_CUDA); }
 
     // ---- the feedback rows and the item filter, once per call

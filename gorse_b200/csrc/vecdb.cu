@@ -58,11 +58,11 @@ __global__ void vecdb_live_kernel(const uint8_t *dead, int64_t n, int64_t *flag)
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i <= n; i += st) flag[i] = i < n && dead[i] == 0;
 }
 
-// device bytes held by the collection, its index and its work buffers
+// device bytes held by the collection, its index, its work buffers and its neighbour cache
 static int64_t vecdb_bytes(const gorse_b200_vecdb *db)
 {
     return (int64_t)(db->d_blocked.bytes() + db->d_allow.bytes() + db->d_cat_off.bytes() + db->d_cats.bytes() + db->d_want.bytes() +
-                     db->i2i.bytes() + db->u2u.bytes() + (db->dense ? index_bytes(db->dense) : sparse_bytes(db->sparse)));
+                     db->i2i.bytes() + db->u2u.bytes() + db->ncache.bytes() + (db->dense ? index_bytes(db->dense) : sparse_bytes(db->sparse)));
 }
 
 static int32_t sync_meta(gorse_b200_vecdb *db)
@@ -208,6 +208,7 @@ int32_t gorse_b200_vecdb_add(gorse_b200_vecdb *db, int64_t n, const float *value
         }
     }
     db->meta_dirty = true;
+    db->gen++;
     return GORSE_B200_OK;
 }
 
@@ -270,7 +271,10 @@ int32_t gorse_b200_vecdb_add_idf_vectors(gorse_b200_vecdb *db, int64_t n, const 
             db->live--;
         }
     }
-    if (added) db->meta_dirty = true;
+    if (added) {
+        db->meta_dirty = true;
+        db->gen++;
+    }
     return GORSE_B200_OK;
 }
 
@@ -325,7 +329,10 @@ int32_t gorse_b200_vecdb_delete_before(gorse_b200_vecdb *db, int64_t timestamp_m
             if (slots_out && cnt < cap) slots_out[cnt] = (int64_t)i;
             cnt++;
         }
-    if (cnt) db->meta_dirty = true;
+    if (cnt) {
+        db->meta_dirty = true;
+        db->gen++;
+    }
     if (count_out) *count_out = cnt;
     return GORSE_B200_OK;
 }
@@ -367,6 +374,7 @@ int32_t gorse_b200_vecdb_compact(gorse_b200_vecdb *db, int64_t *new_slot_out, in
     GB_TRY(db->dense ? index_compact(db->dense, scan.p, live) : sparse_compact(db->sparse, scan.p, live));
     db->hidden.swap(hidden); db->dead.swap(dead); db->ts.swap(ts); db->cat_off.swap(cat_off); db->cats.swap(cats);
     db->meta_dirty = true;
+    db->gen++;
     // every device buffer whose size follows the slot count; the next call that needs one allocates (and zeroes) it again
     db->d_blocked.free(); db->d_allow.free(); db->d_cat_off.free(); db->d_cats.free();
     db->i2i.acc.free(); db->i2i.seen.free(); db->i2i.touched.free(); db->i2i.item_ok.free();
@@ -490,6 +498,7 @@ int32_t gorse_b200_vecdb_add_item_factors(gorse_b200_vecdb *db, gorse_b200_cf *c
         db->live++;
     }
     db->meta_dirty = true;
+    db->gen++;
     return GORSE_B200_OK;
 }
 

@@ -36,6 +36,24 @@ struct UserToUserWork {
                item_ok.bytes() + t_score.bytes() + scores.bytes() + acc.bytes();
     }
 };
+
+// gorse_b200_vecdb_neighbour_cache: the first n neighbours of up to `cap` stored vectors, as stage A (neighbour_table,
+// item_to_item.cu) computes them without a category filter.  Pool row p holds cnt[p] entries (int32 slot, float32 score
+// bits) of 8 bytes each at entry[p * n].  Rows are taken in the order they are computed and never evicted; the cache empties
+// when the collection's generation moves past `gen`.
+struct NeighbourCache {
+    int32_t n = 0;
+    int64_t cap = 0, used = 0;             // cap = 0: off
+    DevBuf<uint2> entry;                   // [cap x n]
+    DevBuf<int32_t> cnt;                   // [cap]
+    std::vector<int32_t> row_of_slot;      // [slots]: the pool row of a slot, -1 = not held
+    uint64_t gen = 0;                      // the collection's generation the held rows belong to
+    int64_t served = 0, computed = 0, emptied = 0;
+    // one call's work: the rows stage A computes, their table and each table row's source (see ncache_assemble_kernel)
+    DevBuf<int32_t> m_slot, m_cnt, src;
+    DevBuf<float> m_score;
+    size_t bytes() const { return entry.bytes() + cnt.bytes() + m_slot.bytes() + m_cnt.bytes() + src.bytes() + m_score.bytes(); }
+};
 }  // namespace gb
 
 struct gorse_b200_vecdb {
@@ -51,11 +69,13 @@ struct gorse_b200_vecdb {
     std::vector<int32_t> cats;
     int64_t live = 0;
     bool meta_dirty = true;
+    uint64_t gen = 0;   // moves with every change of the collection (wherever meta_dirty is set): empties the neighbour cache
     gb::DevBuf<uint8_t> d_blocked, d_allow;   // blocked = hidden | dead
     gb::DevBuf<int64_t> d_cat_off;
     gb::DevBuf<int32_t> d_cats, d_want;
     gb::ItemToItemWork i2i;  // batched item-to-item and session recommendation (item_to_item.cu)
     gb::UserToUserWork u2u;  // batched user-to-user recommendation (user_to_user.cu)
+    gb::NeighbourCache ncache;   // stage A's rows kept between calls (gorse_b200_vecdb_neighbour_cache, item_to_item.cu)
 };
 
 namespace gb {

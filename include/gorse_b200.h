@@ -445,6 +445,32 @@ int32_t gorse_b200_vecdb_compact(gorse_b200_vecdb *db, int64_t *new_slot_out, in
  * bf16 rows, 4 for fp32 rows; *device_bytes_out (may be NULL) = the device bytes the collection holds, counted as
  * gorse_b200_vecdb_compact's bytes_out counts them.  NULL db: GORSE_B200_ERR_ARG. */
 int32_t gorse_b200_vecdb_storage(gorse_b200_vecdb *db, int32_t *value_bytes_out, int64_t *device_bytes_out);
+/* Neighbour cache of a collection: the first n neighbours of each stored vector, as stage A of the batched neighbour entries
+ * (gorse_b200_vecdb_item_to_item, gorse_b200_vecdb_session_recommend, gorse_b200_vecdb_user_to_user and the item-to-item and
+ * user-to-user stages of gorse_b200_recommend) computes them for a call without a category filter, kept on the device and
+ * reused until the collection changes.  Off by default.
+ *   n in [1, 1024] dense / [1, 128] sparse; rows >= 0: how many stored vectors' lists it may hold.  rows = 0 turns the cache
+ *   off and frees it (n is still checked).  Calling again with the same n and rows keeps the cached lists; any other n or
+ *   rows drops them and restarts the counters.  The pool of rows * (8 n + 4) bytes is allocated here: GORSE_B200_ERR_CUDA /
+ *   GORSE_B200_ERR_OOM if it cannot be, and the collection is then as it was.  Negative rows, n outside [1, 1024] or a NULL
+ *   db: GORSE_B200_ERR_ARG (checked in that order, before the collection is read).  Cosine collections:
+ *   GORSE_B200_ERR_UNSUPPORTED (no neighbour entry serves them); so is n above 128 for a sparse collection.
+ *   Which calls use it: a stage A with the cache's n and no category filter takes the rows the cache holds and computes only
+ *   the others, inserting each computed row while the pool has room; once it is full, computed rows serve their call and are
+ *   not kept (no eviction: the cache holds the rows computed first).  A call with a category filter or another n neither
+ *   reads nor fills it.  Any change of the collection empties it before its next read: gorse_b200_vecdb_add (upserts and
+ *   hidden flags included), gorse_b200_vecdb_add_idf_vectors and gorse_b200_vecdb_add_item_factors when they add a vector,
+ *   gorse_b200_vecdb_delete_before when it deletes one, gorse_b200_vecdb_compact when it reclaims a slot (and with them a
+ *   promotion from bf16 to fp32).  gorse_b200_vecdb_load makes a collection without a cache.
+ *   Answers: every entry's slots, score bits and counts are the same with the cache on or off, in any order of calls: each
+ *   row is ordered by (score desc, slot asc) and certified by the exact rules of the top-k pipeline, so it does not depend
+ *   on the batch it was computed in.  Per-call stats keep their meaning, except that "neighbour rows answered by the exact
+ *   scan" counts computed rows only (a cached row is not scanned).  gorse_b200_vecdb_storage's device bytes include the
+ *   cache; snapshots (gorse_b200_vecdb_save) do not contain it, and their stream is the same with or without it.
+ * stats_out[7]: n (0 when off), capacity rows, rows held, device bytes (the pool and the last call's work buffers), and since
+ * the cache was sized: rows served from it, rows computed for it, times it was emptied because the collection changed. */
+int32_t gorse_b200_vecdb_neighbour_cache(gorse_b200_vecdb *db, int32_t n, int64_t rows);
+int32_t gorse_b200_vecdb_neighbour_cache_stats(gorse_b200_vecdb *db, int64_t *stats_out);
 /* Snapshots: a collection written as a byte stream and rebuilt from one on any context (another device, another process), so
  * that a restarted master, a worker and a server hold the collections the master built (the reference's default backend keeps
  * each collection on disk and reopens it in Init, xvec.go:60-123).
