@@ -162,6 +162,23 @@ struct StreamSync {
     }
 };
 
+// an owning CUDA event without timing; declare it before the StreamSync that waits for the work it records
+struct Event {
+    cudaEvent_t e = nullptr;
+    Event() = default;
+    Event(const Event &) = delete;
+    Event &operator=(const Event &) = delete;
+    ~Event()
+    {
+        if (e) cudaEventDestroy(e);
+    }
+    int32_t create()
+    {
+        GB_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+        return GORSE_B200_OK;
+    }
+};
+
 struct ScopedDevice {
     int prev = -1;
     bool ok = true;

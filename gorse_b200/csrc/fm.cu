@@ -327,25 +327,28 @@ extern "C" int32_t gorse_b200_fm_destroy(gorse_b200_fm *m)
     return GORSE_B200_OK;
 }
 
-namespace {
-// a features CSR (id feature + labels) of `rows` rows, checked on the host
-int32_t check_feats(const char *what, int64_t rows, const int32_t *feat, const int64_t *off, const int32_t *idx, int64_t n_features)
+namespace gb {
+namespace fm {
+int32_t upload_feats(gorse_b200_fm *m, int64_t n_users, const int32_t *user_feat, const int64_t *user_lab_off, const int32_t *user_lab_idx,
+                     const float *user_lab_val, int64_t n_items, const int32_t *item_feat, const int64_t *item_lab_off, const int32_t *item_lab_idx,
+                     const float *item_lab_val, const uint16_t *const *item_emb, const uint8_t *item_emb_mask, Slot *S)
 {
-    GB_CHECK_ARG(rows == 0 || (feat != nullptr && off != nullptr), "%s: NULL id features or label offsets", what);
-    if (rows == 0) return GORSE_B200_OK;
-    GB_CHECK_ARG(off[0] == 0, "%s: label offsets must start at 0", what);
-    for (int64_t r = 0; r < rows; r++) {
-        GB_CHECK_ARG(off[r + 1] >= off[r], "%s %lld: label offsets decrease", what, (long long)r);
-        GB_CHECK_ARG(feat[r] == -1 || gb::fm::feature_ok(feat[r], n_features), "%s %lld: id feature %d is not -1 or a feature of [0, %lld)",
-                     what, (long long)r, feat[r], (long long)n_features);
-    }
-    GB_CHECK_ARG(off[rows] == 0 || idx != nullptr, "%s: NULL label indices", what);
-    for (int64_t j = 0; j < off[rows]; j++)
-        GB_CHECK_ARG(gb::fm::feature_ok(idx[j], n_features), "%s label entry %lld: feature %d is not in [0, %lld) once rounded to float32",
-                     what, (long long)j, idx[j], (long long)n_features);
-    return GORSE_B200_OK;
+    const cudaStream_t st = m->ctx->stream;
+    GB_TRY(m->u_feat.upload(user_feat, (size_t)n_users, st));
+    GB_TRY(m->u_off.upload(user_lab_off, (size_t)n_users + 1, st));
+    GB_TRY(m->u_idx.upload(user_lab_idx, (size_t)user_lab_off[n_users], st));
+    GB_TRY(m->u_val.upload(user_lab_val, (size_t)user_lab_off[n_users], st));
+    GB_TRY(m->i_feat.upload(item_feat, (size_t)n_items, st));
+    GB_TRY(m->i_off.upload(item_lab_off, n_items ? (size_t)n_items + 1 : 0, st));
+    GB_TRY(m->i_idx.upload(item_lab_idx, n_items ? (size_t)item_lab_off[n_items] : 0, st));
+    GB_TRY(m->i_val.upload(item_lab_val, n_items ? (size_t)item_lab_off[n_items] : 0, st));
+    if (m->n_emb == 0) return GORSE_B200_OK;
+    if (item_emb_mask) GB_TRY(m->mask.upload(item_emb_mask, (size_t)n_items * m->n_emb, st));
+    for (int s = 0; s < m->n_emb; s++) GB_TRY(m->emb[s].upload(n_items ? item_emb[s] : nullptr, (size_t)n_items * m->dim[(size_t)s], st));
+    return item_tables(m, n_items, item_emb_mask != nullptr, S);
 }
-}  // namespace
+}  // namespace fm
+}  // namespace gb
 
 extern "C" int32_t gorse_b200_fm_rank(gorse_b200_fm *m, int64_t n_users, const int32_t *user_feat, const int64_t *user_lab_off,
                                       const int32_t *user_lab_idx, const float *user_lab_val, int64_t n_items, const int32_t *item_feat,
@@ -367,10 +370,8 @@ extern "C" int32_t gorse_b200_fm_rank(gorse_b200_fm *m, int64_t n_users, const i
     for (int64_t t = 0; t < total; t++)
         GB_CHECK_ARG(cand_items[t] >= 0 && cand_items[t] < n_items, "candidate %lld: item row %d is not in [0, %lld)", (long long)t,
                      cand_items[t], (long long)n_items);
-    GB_TRY(check_feats("user", n_users, user_feat, user_lab_off, user_lab_idx, m->n_features));
-    GB_TRY(check_feats("item", n_items, item_feat, item_lab_off, item_lab_idx, m->n_features));
-    GB_CHECK_ARG(user_lab_off[n_users] == 0 || user_lab_val != nullptr, "user: NULL label values");
-    GB_CHECK_ARG(n_items == 0 || item_lab_off[n_items] == 0 || item_lab_val != nullptr, "item: NULL label values");
+    GB_TRY(check_feats("user", n_users, user_feat, user_lab_off, user_lab_idx, user_lab_val, m->n_features));
+    GB_TRY(check_feats("item", n_items, item_feat, item_lab_off, item_lab_idx, item_lab_val, m->n_features));
     const int n_emb = m->n_emb;
     if (n_emb > 0 && n_items > 0) {
         GB_CHECK_ARG(item_emb != nullptr, "item_emb is NULL");
@@ -406,14 +407,9 @@ extern "C" int32_t gorse_b200_fm_rank(gorse_b200_fm *m, int64_t n_users, const i
     gorse_b200_ctx *ctx = m->ctx;
     ScopedDevice sd(ctx->device);
     cudaStream_t st = ctx->stream;
-    GB_TRY(m->u_feat.upload(user_feat, (size_t)n_users, st));
-    GB_TRY(m->u_off.upload(user_lab_off, (size_t)n_users + 1, st));
-    GB_TRY(m->u_idx.upload(user_lab_idx, (size_t)user_lab_off[n_users], st));
-    GB_TRY(m->u_val.upload(user_lab_val, (size_t)user_lab_off[n_users], st));
-    GB_TRY(m->i_feat.upload(item_feat, (size_t)n_items, st));
-    GB_TRY(m->i_off.upload(item_lab_off, (size_t)n_items + 1, st));
-    GB_TRY(m->i_idx.upload(item_lab_idx, (size_t)item_lab_off[n_items], st));
-    GB_TRY(m->i_val.upload(item_lab_val, (size_t)item_lab_off[n_items], st));
+    Slot S[MAX_SLOTS];
+    GB_TRY(upload_feats(m, n_users, user_feat, user_lab_off, user_lab_idx, user_lab_val, n_items, item_feat, item_lab_off, item_lab_idx,
+                        item_lab_val, item_emb, item_emb_mask, S));
     GB_TRY(m->c_off.upload(cand_off, (size_t)n_users + 1, st));
     GB_TRY(m->cand.upload(cand_items, (size_t)total, st));
     GB_TRY(m->dims.upload(dims.data(), dims.size(), st));
@@ -422,13 +418,9 @@ extern "C" int32_t gorse_b200_fm_rank(gorse_b200_fm *m, int64_t n_users, const i
 
     Feats U{m->u_feat.p, m->u_off.p, m->u_idx.p, m->u_val.p};
     Feats I{m->i_feat.p, m->i_off.p, m->i_idx.p, m->i_val.p};
-    Slot S[MAX_SLOTS];
     if (n_emb > 0) {
         GB_TRY(m->ch_start.upload(ch_start.data(), ch_start.size(), st));
         GB_TRY(m->ch_rows.upload(ch_rows.data(), ch_rows.size(), st));
-        if (item_emb_mask) GB_TRY(m->mask.upload(item_emb_mask, (size_t)n_items * n_emb, st));
-        for (int s = 0; s < n_emb; s++) GB_TRY(m->emb[s].upload(item_emb[s], (size_t)n_items * m->dim[(size_t)s], st));
-        GB_TRY(item_tables(m, n_items, item_emb_mask != nullptr, S));
     }
     // device passes over consecutive users holding at most GROUP_PAIRS pairs (or one user)
     int64_t passes = 0, global_sorts = 0;

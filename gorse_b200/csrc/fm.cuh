@@ -69,12 +69,37 @@ inline bool feature_ok(int64_t idx, int64_t n_features)
     return (int64_t)(float)idx < n_features;
 }
 
+// a features CSR (id feature + labels) of `rows` rows, checked on the host; `what` ("user", "item") names it
+inline int32_t check_feats(const char *what, int64_t rows, const int32_t *feat, const int64_t *off, const int32_t *idx, const float *val,
+                           int64_t n_features)
+{
+    GB_CHECK_ARG(rows == 0 || (feat != nullptr && off != nullptr), "%s: NULL id features or label offsets", what);
+    if (rows == 0) return GORSE_B200_OK;
+    GB_CHECK_ARG(off[0] == 0, "%s: label offsets must start at 0", what);
+    for (int64_t r = 0; r < rows; r++) {
+        GB_CHECK_ARG(off[r + 1] >= off[r], "%s %lld: label offsets decrease", what, (long long)r);
+        GB_CHECK_ARG(feat[r] == -1 || feature_ok(feat[r], n_features), "%s %lld: id feature %d is not -1 or a feature of [0, %lld)", what,
+                     (long long)r, feat[r], (long long)n_features);
+    }
+    GB_CHECK_ARG(off[rows] == 0 || (idx != nullptr && val != nullptr), "%s: NULL label indices / values", what);
+    for (int64_t j = 0; j < off[rows]; j++)
+        GB_CHECK_ARG(feature_ok(idx[j], n_features), "%s label entry %lld: feature %d is not in [0, %lld) once rounded to float32", what,
+                     (long long)j, idx[j], (long long)n_features);
+    return GORSE_B200_OK;
+}
+
 // the model's parameters as the kernels read them
 Model model(const gorse_b200_fm *m);
 
 // per slot: the slot's parameters and the item table m->emb[s] / m->mask (uploaded by the caller; mask used when `masked`)
 // in S[s], and fm_item_kernel over the n_items rows into m->z[s] / m->zmax[s] (grown here).  The caller holds m->mu.
 int32_t item_tables(gorse_b200_fm *m, int64_t n_items, bool masked, Slot *S);
+
+// the users' and the item table's feature CSRs into m->u_* / m->i_*, and with slots the item embeddings (and the mask, when
+// given) and their tables in S (item_tables).  The caller holds m->mu.
+int32_t upload_feats(gorse_b200_fm *m, int64_t n_users, const int32_t *user_feat, const int64_t *user_lab_off, const int32_t *user_lab_idx,
+                     const float *user_lab_val, int64_t n_items, const int32_t *item_feat, const int64_t *item_lab_off, const int32_t *item_lab_idx,
+                     const float *item_lab_val, const uint16_t *const *item_emb, const uint8_t *item_emb_mask, Slot *S);
 
 // one device pass over users [u0, u1) of the device candidate CSR c_off / cand (dims[u] = D_u): fm_pair_kernel, fm_attn_kernel
 // per slot over the attention chunks [ch0, ch1) of ch_start / ch_rows, and fm_sort_kernel.  Pair p's vx / row sum sit at

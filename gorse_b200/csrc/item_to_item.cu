@@ -174,115 +174,115 @@ int32_t aggregate(gorse_b200_ctx *c, const int32_t *d_users, int64_t fill, int64
     return GORSE_B200_OK;
 }
 
-// Both vecdb entries after their own checks: the caller holds db->mu, every context slot is in [-1, slots) and ex / ex_off
-// are the checked exclusion rows.  categories: the neighbour query's filter; item_ok, need, top: aggregate's.
-int32_t neighbour_sums(gorse_b200_vecdb *db, const char *name, int64_t n_users, const int64_t *ctx_off, const int64_t *ctx_slots,
-                       const std::vector<int64_t> &ex, const std::vector<int64_t> &ex_off, const int32_t *categories, int32_t n_categories,
-                       const uint8_t *item_ok, int n, int need, int top, double score_scale, int64_t *slots_out, double *scores_out,
-                       int32_t *count_out, int64_t *stats_out)
+}  // namespace i2i
+
+int32_t NeighbourStage::table(const int32_t *categories, int32_t n_categories, int64_t *exact_rows)
 {
-    const int64_t n_slots = (int64_t)db->ts.size();
-    // the live context entries of every user as rows of the neighbour table.  -1 and deleted slots are skipped (GetVectors
-    // returns nothing, logics/item_to_item.go:56-58) and never count for a session; hidden ones are queried.
-    std::vector<int32_t> row_of((size_t)n_slots, -1), c_row;
-    std::vector<int64_t> nb, c_off((size_t)n_users + 1, 0);
-    c_row.reserve((size_t)ctx_off[n_users]);
-    for (int64_t u = 0; u < n_users; u++) {
-        for (int64_t t = ctx_off[u]; t < ctx_off[u + 1]; t++) {
-            const int32_t r = table_row(db, ctx_slots[t], row_of, nb);
-            if (r >= 0) c_row.push_back(r);
-        }
-        c_off[(size_t)u + 1] = (int64_t)c_row.size();
+    cudaStream_t s = db->ctx->stream;
+    if (users) {
+        GB_TRY(row.upload(q_row.data(), q_row.size(), s));
+        GB_TRY(fb_off.upload(h_fb_off, fb_rows ? (size_t)fb_rows + 1 : 0, s));
+        GB_TRY(fb_items.upload(h_fb_items, fb_rows ? (size_t)h_fb_off[fb_rows] : 0, s));
+    } else {
+        GB_TRY(row.upload(c_row.data(), c_row.size(), s));
+        GB_TRY(d_c_off.upload(c_off.data(), c_off.size(), s));
     }
+    if (h_item_ok) GB_TRY(item_ok.upload(h_item_ok, (size_t)item_ok_len, s));
     const int64_t R = (int64_t)nb.size();
+    if (R == 0) return GORSE_B200_OK;
+    GB_TRY(d_nb.grow((size_t)R));
+    GB_TRY(t_slot.grow((size_t)R * n));
+    GB_TRY(t_score.grow((size_t)R * n));
+    GB_TRY(t_cnt.grow((size_t)R));
+    return neighbour_table(db, nb, d_nb.p, n, categories, n_categories, t_slot.p, t_score.p, t_cnt.p, exact_rows);
+}
+
+int32_t NeighbourStage::reserve(int64_t max_rows, int64_t n_chunks)
+{
+    gorse_b200_ctx *c = db->ctx;
+    GB_TRY(list.grow((size_t)max_rows));
+    if (users) {
+        GB_TRY(work.grow((size_t)max_rows));
+        GB_TRY(route.grow((size_t)n_chunks * 2));
+        GB_CUDA(cudaMemsetAsync(route.p, 0, sizeof(int32_t) * n_chunks * 2, c->stream));
+    }
+    if (!heavy) return GORSE_B200_OK;
+    const size_t rows = (size_t)heavy_grid(c, N, users ? u2u::ROW_BYTES : i2i::ROW_BYTES) * N;
+    if (users) {
+        GB_TRY(uacc.grow_zeroed(rows, c->stream));
+        GB_TRY(flag.grow_zeroed(rows, c->stream));
+    } else {
+        GB_TRY(acc.grow(rows));
+        GB_TRY(seen.grow_zeroed(rows, c->stream));
+    }
+    return touched.grow(rows);
+}
+
+int32_t NeighbourStage::run_chunk(int64_t k, int64_t u0, int64_t rows, const int64_t *ex_off_, const int64_t *ex_, int64_t *ids_, double *scores_,
+                                  int32_t *count_)
+{
+    gorse_b200_ctx *c = db->ctx;
+    const NeighbourTable T{t_slot.p, t_score.p, t_cnt.p};
+    const bool euclid = db->distance == GORSE_B200_DISTANCE_EUCLIDEAN;
+    const uint8_t *ok = h_item_ok ? item_ok.p : nullptr;
+    if (users) {
+        const u2u::Users U{row.p + u0, ex_off_, ex_, ok, ids_, scores_, count_};
+        const u2u::Route Rt{list.p, route.p + 2 * k, work.p, rows};
+        return u2u::aggregate(c, Rt, U, T, u2u::Feedback{fb_off.p, fb_items.p, fb_rows}, n, scale, euclid, N, heavy, uacc.p, flag.p, touched.p);
+    }
+    // the chunk's users routed by |C_u| n
+    const int64_t fill = i2i::route(c_off.data() + u0, rows, n, h_users);
+    n_shared += fill;
+    GB_CUDA(cudaMemcpyAsync(list.p, h_users.data(), sizeof(int32_t) * rows, cudaMemcpyHostToDevice, c->stream));
+    const i2i::Users U{d_c_off.p + u0, row.p, ex_off_, ex_, ids_, scores_, count_};
+    return i2i::aggregate(c, list.p, fill, rows - fill, U, T, ok, n, need, top, scale, euclid, N, acc.p, seen.p, touched.p);
+}
+
+int32_t neighbour_call(NeighbourStage &S, int64_t n_users, const int32_t *categories, int32_t n_categories, const std::vector<int64_t> &ex,
+                       const std::vector<int64_t> &ex_off, int64_t *ids_out, double *scores_out, int32_t *count_out, int64_t *stats_out)
+{
+    const int64_t R = (int64_t)S.nb.size();
     if (R == 0) {
         std::fill(count_out, count_out + n_users, 0);
         return GORSE_B200_OK;
     }
-    gorse_b200_ctx *c = db->ctx;
+    gorse_b200_ctx *c = S.db->ctx;
     ScopedDevice sd(c->device);
-    ItemToItemWork &V = db->i2i;
-    int32_t st = GORSE_B200_OK;
-    auto done = [&](int32_t s) {
-        cudaStreamSynchronize(c->stream);
-        cudaStreamSynchronize(c->copy_stream);
-        return s;
-    };
-    if ((st = V.nb.grow((size_t)R)) || (st = V.t_slot.grow((size_t)R * n)) || (st = V.t_score.grow((size_t)R * n)) || (st = V.t_cnt.grow((size_t)R)) ||
-        (item_ok && (st = V.item_ok.grow((size_t)n_slots))))
-        return done(st);
-    cudaError_t e = item_ok ? cudaMemcpyAsync(V.item_ok.p, item_ok, (size_t)n_slots, cudaMemcpyHostToDevice, c->stream) : cudaSuccess;
-    if (e != cudaSuccess) { set_error("%s upload: %s", name, cudaGetErrorString(e)); return done(GORSE_B200_ERR_CUDA); }
-
-    // ---- stage A: the neighbour table
+    StreamSync sync{c->stream, c->copy_stream};
     int64_t exact_rows = 0;
-    if ((st = neighbour_table(db, nb, V.nb.p, n, categories, n_categories, V.t_slot.p, V.t_score.p, V.t_cnt.p, &exact_rows))) return done(st);
-    if ((e = cudaGetLastError()) != cudaSuccess) { set_error("%s: %s", name, cudaGetErrorString(e)); return done(GORSE_B200_ERR_CUDA); }
-
-    // ---- stage B: users in chunks; a finished chunk is downloaded on the copy stream while the next one computes
-    const int64_t cu = std::min<int64_t>(n_users, (int64_t)c->sm_count * 1024);
-    const int64_t N = n_slots;
-    const int hg = heavy_grid(c, N, ROW_BYTES);
-    const int64_t total_ctx = c_off[(size_t)n_users];
-    if ((st = V.c_off.grow((size_t)cu + 1)) || (st = V.ex_off.grow((size_t)cu + 1)) || (st = V.users.grow((size_t)cu)) ||
-        (st = V.c_row.grow((size_t)std::max<int64_t>(total_ctx, 1))) || (st = V.ex.grow(std::max<size_t>(ex.size(), 1))) ||
-        (st = V.slots.grow((size_t)n_users * top)) || (st = V.scores.grow((size_t)n_users * top)) || (st = V.count.grow((size_t)n_users)))
-        return done(st);
-    const NeighbourTable T{V.t_slot.p, V.t_score.p, V.t_cnt.p};
-    const bool euclid = db->distance == GORSE_B200_DISTANCE_EUCLIDEAN;
-    const uint8_t *d_ok = item_ok ? V.item_ok.p : nullptr;
-    int64_t n_shared = 0, n_heavy = 0;
-    std::vector<int64_t> h_coff, h_exoff;
-    std::vector<int32_t> h_users;
-    for (int64_t u0 = 0; u0 < n_users; u0 += cu) {
+    GB_TRY(S.table(categories, n_categories, &exact_rows));
+    GB_CUDA(cudaGetLastError());
+    const int64_t cu = std::min<int64_t>(n_users, (int64_t)c->sm_count * 1024), n_chunks = div_up(n_users, cu), top = S.top;
+    GB_TRY(S.reserve(cu, n_chunks));
+    GB_TRY(S.ex_off.upload(ex_off.data(), ex_off.size(), c->stream));
+    GB_TRY(S.ex.upload(ex.data(), ex.size(), c->stream));
+    GB_TRY(S.ids.grow((size_t)n_users * top));
+    GB_TRY(S.scores.grow((size_t)n_users * top));
+    GB_TRY(S.count.grow((size_t)n_users));
+    for (int64_t k = 0, u0 = 0; u0 < n_users; k++, u0 += cu) {
         const int64_t rows = std::min(cu, n_users - u0);
-        h_coff.resize(rows + 1); h_exoff.resize(rows + 1);
-        for (int64_t r = 0; r <= rows; r++) {
-            h_coff[r] = c_off[u0 + r] - c_off[u0];
-            h_exoff[r] = ex_off[u0 + r] - ex_off[u0];
-        }
-        const int64_t fill = route(h_coff.data(), rows, n, h_users);
-        n_shared += fill;
-        n_heavy += rows - fill;
-        if (rows - fill > 0 && ((st = V.acc.grow((size_t)hg * N)) || (st = V.seen.grow_zeroed((size_t)hg * N, c->stream)) ||
-                                (st = V.touched.grow((size_t)hg * N))))
-            return done(st);
-        const int64_t n_c = h_coff[rows], n_e = h_exoff[rows];
-        if ((e = cudaMemcpyAsync(V.c_off.p, h_coff.data(), sizeof(int64_t) * (rows + 1), cudaMemcpyHostToDevice, c->stream)) != cudaSuccess ||
-            (e = cudaMemcpyAsync(V.ex_off.p, h_exoff.data(), sizeof(int64_t) * (rows + 1), cudaMemcpyHostToDevice, c->stream)) != cudaSuccess ||
-            (e = cudaMemcpyAsync(V.users.p, h_users.data(), sizeof(int32_t) * rows, cudaMemcpyHostToDevice, c->stream)) != cudaSuccess ||
-            (n_c && (e = cudaMemcpyAsync(V.c_row.p + c_off[u0], c_row.data() + c_off[u0], sizeof(int32_t) * n_c, cudaMemcpyHostToDevice, c->stream)) != cudaSuccess) ||
-            (n_e && (e = cudaMemcpyAsync(V.ex.p + ex_off[u0], ex.data() + ex_off[u0], sizeof(int64_t) * n_e, cudaMemcpyHostToDevice, c->stream)) != cudaSuccess)) {
-            set_error("%s upload: %s", name, cudaGetErrorString(e));
-            return done(GORSE_B200_ERR_CUDA);
-        }
-        Users U;
-        U.c_off = V.c_off.p; U.c_row = V.c_row.p + c_off[u0]; U.ex_off = V.ex_off.p; U.ex = V.ex.p + ex_off[u0];
-        U.slots = V.slots.p + u0 * top; U.scores = V.scores.p + u0 * top; U.count = V.count.p + u0;
-        if ((st = aggregate(c, V.users.p, fill, rows - fill, U, T, d_ok, n, need, top, score_scale, euclid, N, V.acc.p, V.seen.p, V.touched.p)))
-            return done(st);
-        if ((e = cudaEventRecord(c->copy_ev, c->stream)) != cudaSuccess || (e = cudaStreamWaitEvent(c->copy_stream, c->copy_ev, 0)) != cudaSuccess ||
-            (e = cudaMemcpyAsync(count_out + u0, V.count.p + u0, sizeof(int32_t) * rows, cudaMemcpyDeviceToHost, c->copy_stream)) != cudaSuccess ||
-            (e = cudaMemcpyAsync(slots_out + u0 * top, V.slots.p + u0 * top, sizeof(int64_t) * rows * top, cudaMemcpyDeviceToHost, c->copy_stream)) != cudaSuccess ||
-            (e = cudaMemcpyAsync(scores_out + u0 * top, V.scores.p + u0 * top, sizeof(double) * rows * top, cudaMemcpyDeviceToHost, c->copy_stream)) != cudaSuccess) {
-            set_error("%s download: %s", name, cudaGetErrorString(e));
-            return done(GORSE_B200_ERR_CUDA);
-        }
+        GB_TRY(S.run_chunk(k, u0, rows, S.ex_off.p + u0, S.ex.p, S.ids.p + u0 * top, S.scores.p + u0 * top, S.count.p + u0));
+        // a finished chunk is downloaded on the copy stream while the next one computes
+        GB_CUDA(cudaEventRecord(c->copy_ev, c->stream));
+        GB_CUDA(cudaStreamWaitEvent(c->copy_stream, c->copy_ev, 0));
+        GB_CUDA(cudaMemcpyAsync(count_out + u0, S.count.p + u0, sizeof(int32_t) * rows, cudaMemcpyDeviceToHost, c->copy_stream));
+        GB_CUDA(cudaMemcpyAsync(ids_out + u0 * top, S.ids.p + u0 * top, sizeof(int64_t) * rows * top, cudaMemcpyDeviceToHost, c->copy_stream));
+        GB_CUDA(cudaMemcpyAsync(scores_out + u0 * top, S.scores.p + u0 * top, sizeof(double) * rows * top, cudaMemcpyDeviceToHost, c->copy_stream));
     }
-    if ((e = cudaStreamSynchronize(c->stream)) != cudaSuccess || (e = cudaStreamSynchronize(c->copy_stream)) != cudaSuccess) {
-        set_error("%s: %s", name, cudaGetErrorString(e));
-        return done(GORSE_B200_ERR_CUDA);
+    // the users per accumulator: item-to-item routes on the host (run_chunk counts), user-to-user on the device
+    std::vector<int32_t> routed(S.users ? (size_t)n_chunks * 2 : 0);
+    if (S.users)
+        GB_CUDA(cudaMemcpyAsync(routed.data(), S.route.p, sizeof(int32_t) * n_chunks * 2, cudaMemcpyDeviceToHost, c->stream));
+    GB_CUDA(cudaStreamSynchronize(c->stream));
+    GB_CUDA(cudaStreamSynchronize(c->copy_stream));
+    int64_t st[4] = {R, exact_rows, S.n_shared, S.users ? 0 : n_users - S.n_shared};
+    for (size_t k = 0; k < routed.size(); k += 2) {
+        st[2] += routed[k];
+        st[3] += routed[k + 1];
     }
-    if (stats_out) {
-        stats_out[0] = R;
-        stats_out[1] = exact_rows;
-        stats_out[2] = n_shared;
-        stats_out[3] = n_heavy;
-    }
-    return done(GORSE_B200_OK);
+    if (stats_out) std::copy(st, st + 4, stats_out);
+    return GORSE_B200_OK;
 }
-
-}  // namespace i2i
 
 // stage A proper: the table rows of the R stored vectors d_nb (device) under db->d_allow
 static int32_t compute_rows(gorse_b200_vecdb *db, int64_t R, const int64_t *d_nb, int n, int32_t *t_slot, float *t_score, int32_t *t_cnt,
@@ -416,15 +416,8 @@ extern "C" int32_t gorse_b200_vecdb_neighbour_cache(gorse_b200_vecdb *db, int32_
     GB_CHECK_ARG(rows >= 0, "negative rows");
     GB_CHECK_ARG(n >= 1 && n <= MAX_N_DENSE, "n = %d outside [1, %d]", n, MAX_N_DENSE);
     GB_CHECK_ARG(db != nullptr, "collection is NULL");
-    if (db->distance == GORSE_B200_DISTANCE_COSINE) {
-        set_error("neighbour cache: no neighbour entry serves a Cosine collection");
-        return GORSE_B200_ERR_UNSUPPORTED;
-    }
-    if (db->dim == 0 && n > MAX_N_SPARSE) {
-        set_error("neighbour cache: n = %d above %d for a sparse collection", n, MAX_N_SPARSE);
-        return GORSE_B200_ERR_UNSUPPORTED;
-    }
     std::lock_guard<std::mutex> lk(db->mu);
+    GB_TRY(check_stage_db(db, n, "neighbour cache"));
     NeighbourCache &K = db->ncache;
     if (rows == K.cap && (rows == 0 || n == K.n)) return GORSE_B200_OK;
     GB_CHECK_ARG(rows <= INT32_MAX, "rows = %lld above 2^31 - 1", (long long)rows);
@@ -453,6 +446,18 @@ extern "C" int32_t gorse_b200_vecdb_neighbour_cache_stats(gorse_b200_vecdb *db, 
     return GORSE_B200_OK;
 }
 
+// the context and exclusion rows of both entries
+static int32_t check_rows(const char *who, int64_t rows, const int32_t *count_out, const int64_t *ctx_off, const int64_t *ctx_slots,
+                          const int64_t *excl_off, const int64_t *excl_slots)
+{
+    GB_CHECK_ARG(count_out != nullptr && ctx_off != nullptr && excl_off != nullptr, "count_out / ctx_off / excl_off is NULL");
+    GB_TRY(check_offsets(ctx_off, rows, who, "ctx_off"));
+    GB_TRY(check_offsets(excl_off, rows, who, "excl_off"));
+    GB_CHECK_ARG(ctx_off[rows] == 0 || ctx_slots != nullptr, "ctx_slots is NULL");
+    GB_CHECK_ARG(excl_off[rows] == 0 || excl_slots != nullptr, "excl_slots is NULL");
+    return GORSE_B200_OK;
+}
+
 extern "C" int32_t gorse_b200_vecdb_item_to_item(gorse_b200_vecdb *db, int64_t n_users, const int64_t *ctx_off, const int64_t *ctx_slots,
                                                  const int64_t *excl_off, const int64_t *excl_slots, const int32_t *categories,
                                                  int32_t n_categories, int32_t n, double score_scale, int64_t *slots_out, double *scores_out,
@@ -462,41 +467,25 @@ extern "C" int32_t gorse_b200_vecdb_item_to_item(gorse_b200_vecdb *db, int64_t n
     GB_CHECK_ARG(n_users >= 0 && n_categories >= 0, "negative count");
     if (stats_out) std::fill(stats_out, stats_out + 4, 0);
     if (n_users == 0) return GORSE_B200_OK;
-    GB_CHECK_ARG(count_out != nullptr && ctx_off != nullptr && excl_off != nullptr, "count_out / ctx_off / excl_off is NULL");
-    GB_CHECK_ARG(ctx_off[0] == 0 && excl_off[0] == 0, "ctx_off[0] and excl_off[0] must be 0");
-    for (int64_t u = 0; u < n_users; u++) {
-        GB_CHECK_ARG(ctx_off[u + 1] >= ctx_off[u], "ctx_off not non-decreasing at %lld", (long long)u);
-        GB_CHECK_ARG(excl_off[u + 1] >= excl_off[u], "excl_off not non-decreasing at %lld", (long long)u);
-    }
-    GB_CHECK_ARG(ctx_off[n_users] == 0 || ctx_slots != nullptr, "ctx_slots is NULL");
-    GB_CHECK_ARG(excl_off[n_users] == 0 || excl_slots != nullptr, "excl_slots is NULL");
+    GB_TRY(check_rows("item_to_item", n_users, count_out, ctx_off, ctx_slots, excl_off, excl_slots));
     GB_CHECK_ARG(score_scale == score_scale, "score_scale is NaN");
-    if (db->distance == GORSE_B200_DISTANCE_COSINE) {
-        set_error("item-to-item collections are Dot or Euclidean");
-        return GORSE_B200_ERR_UNSUPPORTED;
-    }
+    std::lock_guard<std::mutex> lk(db->mu);
+    GB_TRY(check_stage_db(db, n, "item_to_item"));
     if (n <= 0) {
-        for (int64_t u = 0; u < n_users; u++) count_out[u] = 0;
+        std::fill(count_out, count_out + n_users, 0);
         return GORSE_B200_OK;
-    }
-    const bool sparse = db->dim == 0;
-    if (n > (sparse ? MAX_N_SPARSE : MAX_N_DENSE)) {
-        set_error("item_to_item: n = %d above %d for a %s collection", n, sparse ? MAX_N_SPARSE : MAX_N_DENSE, sparse ? "sparse" : "dense");
-        return GORSE_B200_ERR_UNSUPPORTED;
     }
     GB_CHECK_ARG(slots_out != nullptr && scores_out != nullptr, "NULL output");
     GB_CHECK_ARG(n_categories == 0 || categories != nullptr, "categories is NULL");
-    std::lock_guard<std::mutex> lk(db->mu);
     const int64_t n_slots = (int64_t)db->ts.size();
-    if (n_slots > INT32_MAX) { set_error("item_to_item: more than 2^31 slots"); return GORSE_B200_ERR_UNSUPPORTED; }
     for (int64_t u = 0; u < n_users; u++)
         for (int64_t t = ctx_off[u]; t < ctx_off[u + 1]; t++)
             GB_CHECK_ARG(ctx_slots[t] >= -1 && ctx_slots[t] < n_slots, "user %lld: context slot %lld is not a slot of the collection",
                          (long long)u, (long long)ctx_slots[t]);
     std::vector<int64_t> ex, ex_off;
     GB_TRY(exclusion_rows(n_users, excl_off, excl_slots, n_slots, "user", "slot", ex, ex_off));
-    return i2i::neighbour_sums(db, "item_to_item", n_users, ctx_off, ctx_slots, ex, ex_off, categories, n_categories, nullptr, n, 0, n,
-                               score_scale, slots_out, scores_out, count_out, stats_out);
+    db->stage.prepare_items(db, n_users, ctx_off, ctx_slots, nullptr, n, 0, n, score_scale, nullptr);
+    return neighbour_call(db->stage, n_users, categories, n_categories, ex, ex_off, slots_out, scores_out, count_out, stats_out);
 }
 
 extern "C" int32_t gorse_b200_vecdb_session_recommend(gorse_b200_vecdb *db, int64_t n_sessions, const int64_t *ctx_off, const int64_t *ctx_slots,
@@ -509,14 +498,7 @@ extern "C" int32_t gorse_b200_vecdb_session_recommend(gorse_b200_vecdb *db, int6
     if (stats_out) std::fill(stats_out, stats_out + 4, 0);
     std::vector<int64_t> ex, ex_off;
     if (n_sessions > 0) {
-        GB_CHECK_ARG(count_out != nullptr && ctx_off != nullptr && excl_off != nullptr, "count_out / ctx_off / excl_off is NULL");
-        GB_CHECK_ARG(ctx_off[0] == 0 && excl_off[0] == 0, "ctx_off[0] and excl_off[0] must be 0");
-        for (int64_t u = 0; u < n_sessions; u++) {
-            GB_CHECK_ARG(ctx_off[u + 1] >= ctx_off[u], "ctx_off decreases at %lld", (long long)u);
-            GB_CHECK_ARG(excl_off[u + 1] >= excl_off[u], "excl_off decreases at %lld", (long long)u);
-        }
-        GB_CHECK_ARG(ctx_off[n_sessions] == 0 || ctx_slots != nullptr, "ctx_slots is NULL");
-        GB_CHECK_ARG(excl_off[n_sessions] == 0 || excl_slots != nullptr, "excl_slots is NULL");
+        GB_TRY(check_rows("session_recommend", n_sessions, count_out, ctx_off, ctx_slots, excl_off, excl_slots));
         GB_CHECK_ARG(top <= 0 || (slots_out != nullptr && scores_out != nullptr), "slots_out / scores_out is NULL");
         for (int64_t t = 0; t < ctx_off[n_sessions]; t++)
             GB_CHECK_ARG(ctx_slots[t] >= -1, "context slot %lld is not a slot of the collection", (long long)ctx_slots[t]);
@@ -529,20 +511,14 @@ extern "C" int32_t gorse_b200_vecdb_session_recommend(gorse_b200_vecdb *db, int6
         return GORSE_B200_ERR_UNSUPPORTED;
     }
     GB_CHECK_ARG(db != nullptr, "collection is NULL");
-    if (db->distance == GORSE_B200_DISTANCE_COSINE) {
-        set_error("session collections are Dot or Euclidean");
-        return GORSE_B200_ERR_UNSUPPORTED;
-    }
-    const bool sparse = db->dim == 0;
-    const int max_n = sparse ? MAX_N_SPARSE : MAX_N_DENSE;
-    if (n <= 0 || n > max_n) {   // n = 0 asks the store for one neighbour (n + 1) and keeps it: not served here
-        set_error("session_recommend: n = %d outside [1, %d] for a %s collection", n, max_n, sparse ? "sparse" : "dense");
+    std::lock_guard<std::mutex> lk(db->mu);
+    GB_TRY(check_stage_db(db, n, "session_recommend"));
+    if (n <= 0) {   // n = 0 asks the store for one neighbour (n + 1) and keeps it: not served here
+        set_error("session_recommend: n = %d is not at least 1", n);
         return GORSE_B200_ERR_UNSUPPORTED;
     }
     if (n_sessions == 0) return GORSE_B200_OK;
-    std::lock_guard<std::mutex> lk(db->mu);
     const int64_t n_slots = (int64_t)db->ts.size();
-    if (n_slots > INT32_MAX) { set_error("session_recommend: more than 2^31 slots"); return GORSE_B200_ERR_UNSUPPORTED; }
     for (int64_t t = 0; t < ctx_off[n_sessions]; t++)
         GB_CHECK_ARG(ctx_slots[t] < n_slots, "context slot %lld is not a slot of the collection", (long long)ctx_slots[t]);
     for (int64_t t = 0; t < (int64_t)ex.size(); t++)
@@ -552,6 +528,6 @@ extern "C" int32_t gorse_b200_vecdb_session_recommend(gorse_b200_vecdb *db, int6
         return GORSE_B200_OK;
     }
     const int need = std::max(context_size, 1);   // the handler stops once used >= ContextSize, after at least one list
-    return i2i::neighbour_sums(db, "session_recommend", n_sessions, ctx_off, ctx_slots, ex, ex_off, nullptr, 0, item_ok, n, need, top,
-                               score_scale, slots_out, scores_out, count_out, stats_out);
+    db->stage.prepare_items(db, n_sessions, ctx_off, ctx_slots, nullptr, n, need, top, score_scale, item_ok);
+    return neighbour_call(db->stage, n_sessions, nullptr, 0, ex, ex_off, slots_out, scores_out, count_out, stats_out);
 }

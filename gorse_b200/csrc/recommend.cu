@@ -24,7 +24,6 @@
 //                         position asc) with 128-bit keys; else the FM order.
 //   A finished chunk is downloaded on the copy stream while the next one computes (two output buffers, alternating).
 #include <algorithm>
-#include <numeric>
 
 #include "fm.cuh"
 #include "stages.cuh"
@@ -341,28 +340,6 @@ __global__ void __launch_bounds__(NT) rec_emit_kernel(const int32_t *packed, con
 template <typename T>
 using Buf = DevBuf<T>;   // grow-only, kept with the context between calls
 
-// the host's preparation of one item-to-item / user-to-user stage, and its neighbour table
-struct StageData {
-    std::vector<int64_t> nb;                 // distinct query slots
-    std::vector<int64_t> c_off;              // i2i: [n_users + 1] live context entries
-    std::vector<int32_t> c_row;              // i2i: their table rows
-    std::vector<int32_t> q_row;              // u2u: [n_users] table row, -1
-    std::vector<int64_t> es0, es0_off;       // i2i: E0 in slots, sorted, per user
-    bool heavy = false;                      // u2u: a user may need a global row
-    Buf<int64_t> d_nb, d_map, d_fb_off, d_es0;   // d_map: i2i slot_of_item
-    Buf<int32_t> t_slot, t_cnt, d_item_of_slot, d_fb_items, d_c_row, d_q_row;
-    Buf<float> t_score;
-    Buf<uint8_t> d_item_ok, seen;
-    Buf<double> acc, uacc;                   // i2i / u2u global rows (u2u's must be zero between users, i2i's need not)
-    Buf<int32_t> flag, touched;
-    Buf<int64_t> ES[2];                      // i2i: the exclude set in slots, ping-pong
-    void clear_host()
-    {
-        nb.clear(); c_off.clear(); c_row.clear(); q_row.clear(); es0.clear(); es0_off.clear();
-        heavy = false;
-    }
-};
-
 // the device buffers of gorse_b200_recommend, grow-only and kept with the context (the global accumulator rows are zero
 // between calls: the aggregation kernels clear what they touch), so a worker's batches do not allocate
 struct Work {
@@ -370,12 +347,11 @@ struct Work {
     Buf<uint8_t> d_live, d_repl_pos;
     Buf<int32_t> d_repl_items, d_cf_item_of_slot, d_u_len, d_i_len;
     Buf<int64_t> d_repl_off, d_cf_excl_off;
-    std::vector<Buf<int32_t>> l_items;
-    std::vector<Buf<double>> l_scores;
-    std::vector<Buf<int64_t>> l_off;
-    std::vector<StageData> sd;
-    Buf<int64_t> d_cand_off, d_E_off, d_e0_off, d_e0, d_E[2], d_i2i_off, d_fm_off, d_ch_off, d_rids;
-    Buf<int32_t> d_cand, d_cnt, d_start, d_users, d_list, d_work, d_route, d_rcount, d_out_items[2], d_out_cnt[2], d_dims;
+    struct List { Buf<int32_t> items; Buf<double> scores; Buf<int64_t> off; };
+    std::vector<List> lists;                 // per list stage
+    std::vector<NeighbourStage> sd;          // per item-to-item / user-to-user stage
+    Buf<int64_t> d_cand_off, d_E_off, d_e0_off, d_e0, d_E[2], d_fm_off, d_ch_off, d_rids;
+    Buf<int32_t> d_cand, d_cnt, d_start, d_rcount, d_out_items[2], d_out_cnt[2], d_dims;
     Buf<double> d_cscore, d_rscore, d_dscore, d_out_scores[2];
     Buf<u128> d_sort;
 };
@@ -399,27 +375,52 @@ void recommend_work_free(gorse_b200_ctx *ctx)
 
 }  // namespace gb
 
-using namespace gb;
+namespace gb {
+namespace rec {
 
-extern "C" int32_t gorse_b200_recommend(gorse_b200_ctx *ctx, int64_t n_users, const int64_t *excl_off, const int32_t *excl_items, int32_t n_items,
-                                        const uint8_t *item_live, int32_t n_stages, const gorse_b200_recommend_stage *stages,
-                                        const gorse_b200_recommend_cf *cf, const gorse_b200_recommend_ranker *ranker, const int64_t *repl_off,
-                                        const int32_t *repl_items, const uint8_t *repl_positive, double positive_decay, double read_decay,
-                                        int32_t *items_out, double *scores_out, int32_t *count_out, int64_t *stats_out)
-{
-    using namespace gb::rec;
-    GB_CHECK_ARG(n_users >= 0 && n_items >= 0 && n_stages >= 0, "negative count");
-    if (stats_out) std::fill(stats_out, stats_out + 4, 0);
-    if (n_users == 0) return GORSE_B200_OK;
-    GB_CHECK_ARG(count_out != nullptr && excl_off != nullptr && excl_off[0] == 0, "count_out / excl_off is NULL or excl_off[0] != 0");
-    GB_CHECK_ARG(n_stages == 0 || stages != nullptr, "stages is NULL");
-    GB_CHECK_ARG(n_items == 0 || item_live != nullptr, "item_live is NULL");
-    for (int64_t u = 0; u < n_users; u++) GB_CHECK_ARG(excl_off[u + 1] >= excl_off[u], "excl_off not non-decreasing at %lld", (long long)u);
-    GB_CHECK_ARG(excl_off[n_users] == 0 || excl_items != nullptr, "excl_items is NULL");
-    // E0: each user's items once, sorted, -1 dropped
-    std::vector<int64_t> e0, e0_off;
-    GB_TRY(exclusion_rows(n_users, excl_off, excl_items, n_items, "user", "item", e0, e0_off));
-    auto check_map = [&](const char *what, gorse_b200_vecdb *db, const int64_t *slot_of_item, const int32_t *item_of_slot) -> int32_t {
+// one call: its arguments, what its phases hand on to each other, and the phases
+struct Call {
+    gorse_b200_ctx *ctx;
+    int64_t n_users;
+    const int64_t *excl_off;
+    const int32_t *excl_items;
+    int32_t n_items;
+    const uint8_t *item_live;
+    int32_t n_stages;
+    const gorse_b200_recommend_stage *stages;
+    const gorse_b200_recommend_cf *cf;
+    const gorse_b200_recommend_ranker *ranker;
+    const int64_t *repl_off;
+    const int32_t *repl_items;
+    const uint8_t *repl_positive;
+    double positive_decay, read_decay;
+    int32_t *items_out;
+    double *scores_out;
+    int32_t *count_out;
+    // checks
+    bool with_repl = false;
+    gorse_b200_fm *m = nullptr;
+    std::vector<int64_t> e0, e0_off;         // E0: each user's items once, sorted, -1 dropped
+    std::vector<int64_t> bound, cap;         // per user: the most candidates, and the most exclude-set entries a stage reads
+    std::vector<int32_t> u_len, i_len;       // the ranker's row lengths, for D_u
+    std::vector<std::unique_lock<std::mutex>> locks;   // the collections, each locked once, in address order
+    std::unique_lock<std::mutex> fm_lock;
+    // tables, CF recall and FM tables
+    int64_t total_rows = 0, exact_total = 0;
+    const int64_t *cf_slots = nullptr;       // the CF recall rows, in the CF index's recall buffers
+    const float *cf_scores = nullptr;
+    const int32_t *cf_count = nullptr;
+    fm::Feats FI{};
+    fm::Slot FS[fm::MAX_SLOTS];
+    // the chunk plan
+    std::vector<int64_t> chunk_at{0}, out_at;
+    int64_t n_chunks = 0, sort_stride = 0;
+    int grid = 0, emit_grid = 0;
+    std::vector<int64_t> h_cand_off, h_E_off, h_e0_off, h_ch_off;
+
+    // slot_of_item / item_of_slot of a stage's collection: one slot per item and back
+    int32_t check_map(const char *what, gorse_b200_vecdb *db, const int64_t *slot_of_item, const int32_t *item_of_slot) const
+    {
         GB_CHECK_ARG(slot_of_item != nullptr && (item_of_slot != nullptr || db->ts.empty()), "%s: slot_of_item / item_of_slot is NULL", what);
         const int64_t S = (int64_t)db->ts.size();
         for (int32_t i = 0; i < n_items; i++)
@@ -436,46 +437,18 @@ extern "C" int32_t gorse_b200_recommend(gorse_b200_ctx *ctx, int64_t n_users, co
             GB_CHECK_ARG(slot_of_item[it] == s, "%s: live slot %lld holds item %d whose slot is %lld", what, (long long)s, it, (long long)slot_of_item[it]);
         }
         return GORSE_B200_OK;
-    };
-    // the collections, each locked once, in address order
-    std::vector<gorse_b200_vecdb *> dbs;
-    for (int32_t s = 0; s < n_stages; s++) {
-        const auto &g = stages[s];
-        GB_CHECK_ARG(g.kind >= GORSE_B200_STAGE_LIST && g.kind <= GORSE_B200_STAGE_USER_TO_USER, "stage %d: unknown kind %d", s, g.kind);
-        if (g.kind == GORSE_B200_STAGE_ITEM_TO_ITEM || g.kind == GORSE_B200_STAGE_USER_TO_USER) {
-            GB_CHECK_ARG(g.db != nullptr && g.db->ctx == ctx, "stage %d: collection is NULL or of another context", s);
-            dbs.push_back(g.db);
-        }
-        if (g.kind == GORSE_B200_STAGE_COLLABORATIVE) GB_CHECK_ARG(cf != nullptr, "stage %d: a collaborative stage needs the CF inputs", s);
-    }
-    if (cf) {
-        GB_CHECK_ARG(cf->db != nullptr && cf->db->ctx == ctx, "CF collection is NULL or of another context");
-        dbs.push_back(cf->db);
-    }
-    std::sort(dbs.begin(), dbs.end());
-    dbs.erase(std::unique(dbs.begin(), dbs.end()), dbs.end());
-    std::vector<std::unique_lock<std::mutex>> locks;
-    for (auto *db : dbs) locks.emplace_back(db->mu);
-    std::unique_lock<std::mutex> fm_lock;
-    if (ranker) {
-        GB_CHECK_ARG(ranker->fm != nullptr && ranker->fm->ctx == ctx, "ranker: fm handle is NULL or of another context");
-        fm_lock = std::unique_lock<std::mutex>(ranker->fm->mu);
     }
 
-    // per stage: checks and the per-user bound
-    std::vector<int64_t> bound((size_t)n_users, 0), cap((size_t)n_users, 0);
-    for (int64_t u = 0; u < n_users; u++) cap[(size_t)u] = e0_off[(size_t)u + 1] - e0_off[(size_t)u];
-    int32_t err = GORSE_B200_OK;
-    for (int32_t s = 0; s < n_stages; s++) {
+    // stage s's arguments, and the most candidates it gives each user, in b
+    int32_t check_stage(int32_t s, std::vector<int64_t> &b) const
+    {
         const auto &g = stages[s];
-        std::vector<int64_t> b((size_t)n_users, 0);
+        char who[32];
+        snprintf(who, sizeof who, "stage %d", s);
         if (g.kind == GORSE_B200_STAGE_LIST) {
             if (g.list_off) {
-                GB_CHECK_ARG(g.list_off[0] == 0, "stage %d: list_off[0] != 0", s);
-                for (int64_t u = 0; u < n_users; u++) {
-                    GB_CHECK_ARG(g.list_off[u + 1] >= g.list_off[u], "stage %d: list_off decreases at %lld", s, (long long)u);
-                    b[(size_t)u] = g.list_off[u + 1] - g.list_off[u];
-                }
+                GB_TRY(check_offsets(g.list_off, n_users, who, "list_off"));
+                for (int64_t u = 0; u < n_users; u++) b[(size_t)u] = g.list_off[u + 1] - g.list_off[u];
             } else {
                 GB_CHECK_ARG(g.list_len >= 0, "stage %d: negative list_len", s);
                 std::fill(b.begin(), b.end(), g.list_len);
@@ -492,97 +465,40 @@ extern "C" int32_t gorse_b200_recommend(gorse_b200_ctx *ctx, int64_t n_users, co
                     set_error("stage %d: a list of %lld entries, at most %d", s, (long long)b[(size_t)u], MAX_LIST);
                     return GORSE_B200_ERR_UNSUPPORTED;
                 }
-        } else if (g.kind == GORSE_B200_STAGE_COLLABORATIVE) {
-            std::fill(b.begin(), b.end(), std::max(cf->n, 0));
-        } else {
-            gorse_b200_vecdb *db = g.db;
-            const bool i2i = g.kind == GORSE_B200_STAGE_ITEM_TO_ITEM;
-            GB_CHECK_ARG(g.score_scale == g.score_scale, "stage %d: score_scale is NaN", s);
-            if (db->distance == GORSE_B200_DISTANCE_COSINE) {
-                set_error("stage %d: item-to-item / user-to-user collections are Dot or Euclidean", s);
-                return GORSE_B200_ERR_UNSUPPORTED;
-            }
-            const int lim = db->dim == 0 ? MAX_N_SPARSE : MAX_N_DENSE;
-            if (g.n > lim) {
-                set_error("stage %d: n = %d above %d", s, g.n, lim);
-                return GORSE_B200_ERR_UNSUPPORTED;
-            }
-            if ((int64_t)db->ts.size() > INT32_MAX) { set_error("stage %d: more than 2^31 slots", s); return GORSE_B200_ERR_UNSUPPORTED; }
-            std::fill(b.begin(), b.end(), std::max(g.n, 0));
-            const int64_t S = (int64_t)db->ts.size();
-            if (i2i) {
-                if ((err = check_map("item-to-item stage", db, g.slot_of_item, g.item_of_slot))) return err;
-                GB_CHECK_ARG(g.ctx_off != nullptr && g.ctx_off[0] == 0, "stage %d: ctx_off is NULL or ctx_off[0] != 0", s);
-                GB_CHECK_ARG(g.n_categories >= 0 && (g.n_categories == 0 || g.categories != nullptr), "stage %d: categories", s);
-                for (int64_t u = 0; u < n_users; u++) GB_CHECK_ARG(g.ctx_off[u + 1] >= g.ctx_off[u], "stage %d: ctx_off decreases at %lld", s, (long long)u);
-                GB_CHECK_ARG(g.ctx_off[n_users] == 0 || g.ctx_items != nullptr, "stage %d: ctx_items is NULL", s);
-                for (int64_t t = 0; t < g.ctx_off[n_users]; t++)
-                    GB_CHECK_ARG(g.ctx_items[t] >= -1 && g.ctx_items[t] < n_items, "stage %d: context entry %lld: item %d is not in [-1, %d)", s,
-                                 (long long)t, g.ctx_items[t], n_items);
-            } else {
-                GB_CHECK_ARG(g.user_slots != nullptr && g.n_fb_rows >= 0, "stage %d: user_slots is NULL or n_fb_rows < 0", s);
-                for (int64_t u = 0; u < n_users; u++)
-                    GB_CHECK_ARG(g.user_slots[u] >= -1 && g.user_slots[u] < S, "stage %d: user %lld: slot %lld is not a slot", s, (long long)u,
-                                 (long long)g.user_slots[u]);
-                GB_CHECK_ARG(g.n_fb_rows == 0 || (g.fb_off != nullptr && g.fb_off[0] == 0), "stage %d: fb_off is NULL or fb_off[0] != 0", s);
-                for (int64_t v = 0; v < g.n_fb_rows; v++) GB_CHECK_ARG(g.fb_off[v + 1] >= g.fb_off[v], "stage %d: fb_off decreases at %lld", s, (long long)v);
-                const int64_t nf = g.n_fb_rows ? g.fb_off[g.n_fb_rows] : 0;
-                GB_CHECK_ARG(nf == 0 || g.fb_items != nullptr, "stage %d: fb_items is NULL", s);
-                for (int64_t t = 0; t < nf; t++)
-                    GB_CHECK_ARG(g.fb_items[t] >= 0 && g.fb_items[t] < n_items, "stage %d: feedback entry %lld: item %d is not in [0, %d)", s,
-                                 (long long)t, g.fb_items[t], n_items);
-            }
-        }
-        for (int64_t u = 0; u < n_users; u++) {
-            bound[(size_t)u] += b[(size_t)u];
-            if (s + 1 < n_stages) cap[(size_t)u] += b[(size_t)u];
-        }
-    }
-    if (cf) {
-        gorse_b200_vecdb *db = cf->db;
-        if (db->dim == 0) { set_error("the CF collection must be dense"); return GORSE_B200_ERR_UNSUPPORTED; }
-        GB_CHECK_ARG(cf->n >= 0 && cf->n <= MAX_N_DENSE, "CF n = %d is not in [0, %d]", cf->n, MAX_N_DENSE);
-        GB_CHECK_ARG(cf->user_vectors != nullptr, "CF user_vectors is NULL");
-        if ((err = check_map("CF", db, cf->slot_of_item, cf->item_of_slot))) return err;
-        for (int64_t u = 0; u < n_users; u++)
-            GB_CHECK_ARG((int64_t)cf->n + (excl_off[u + 1] - excl_off[u]) <= INT32_MAX, "user %lld: n + |E0| overflows", (long long)u);
-    }
-    const bool with_repl = ranker && repl_off;
-    if (with_repl) {
-        GB_CHECK_ARG(repl_off[0] == 0, "repl_off[0] != 0");
-        GB_CHECK_ARG(positive_decay == positive_decay && read_decay == read_decay, "a decay is NaN");
-        for (int64_t u = 0; u < n_users; u++) GB_CHECK_ARG(repl_off[u + 1] >= repl_off[u], "repl_off decreases at %lld", (long long)u);
-        GB_CHECK_ARG(repl_off[n_users] == 0 || (repl_items != nullptr && repl_positive != nullptr), "repl_items / repl_positive is NULL");
-        std::vector<int32_t> row;
-        for (int64_t u = 0; u < n_users; u++) {
-            row.assign(repl_items + repl_off[u], repl_items + repl_off[u + 1]);
-            for (int32_t it : row) GB_CHECK_ARG(it >= 0 && it < n_items, "user %lld: replacement item %d is not in [0, %d)", (long long)u, it, n_items);
-            std::sort(row.begin(), row.end());
-            GB_CHECK_ARG(std::adjacent_find(row.begin(), row.end()) == row.end(), "user %lld: a replacement item twice", (long long)u);
-            bound[(size_t)u] += repl_off[u + 1] - repl_off[u];
-        }
-    }
-    // the ranker: features checked as gorse_b200_fm_rank checks them; row lengths for D_u
-    gorse_b200_fm *m = ranker ? ranker->fm : nullptr;
-    std::vector<int32_t> u_len, i_len;
-    if (m) {
-        const auto &R = *ranker;
-        auto check_feats = [&](const char *what, int64_t rows, const int32_t *feat, const int64_t *off, const int32_t *idx, const float *val) -> int32_t {
-            GB_CHECK_ARG(rows == 0 || (feat != nullptr && off != nullptr), "%s: NULL id features or label offsets", what);
-            if (rows == 0) return GORSE_B200_OK;
-            GB_CHECK_ARG(off[0] == 0, "%s: label offsets must start at 0", what);
-            for (int64_t r = 0; r < rows; r++) {
-                GB_CHECK_ARG(off[r + 1] >= off[r], "%s %lld: label offsets decrease", what, (long long)r);
-                GB_CHECK_ARG(feat[r] == -1 || fm::feature_ok(feat[r], m->n_features), "%s %lld: id feature %d is not -1 or a feature", what, (long long)r, feat[r]);
-            }
-            GB_CHECK_ARG(off[rows] == 0 || (idx != nullptr && val != nullptr), "%s: NULL label indices / values", what);
-            for (int64_t j = 0; j < off[rows]; j++)
-                GB_CHECK_ARG(fm::feature_ok(idx[j], m->n_features), "%s label entry %lld: feature %d is not in [0, %lld) once rounded to float32", what,
-                             (long long)j, idx[j], (long long)m->n_features);
             return GORSE_B200_OK;
-        };
-        if ((err = check_feats("user", n_users, R.user_feat, R.user_lab_off, R.user_lab_idx, R.user_lab_val))) return err;
-        if ((err = check_feats("item", n_items, R.item_feat, R.item_lab_off, R.item_lab_idx, R.item_lab_val))) return err;
+        }
+        if (g.kind == GORSE_B200_STAGE_COLLABORATIVE) {
+            std::fill(b.begin(), b.end(), std::max(cf->n, 0));
+            return GORSE_B200_OK;
+        }
+        gorse_b200_vecdb *db = g.db;
+        GB_CHECK_ARG(g.score_scale == g.score_scale, "stage %d: score_scale is NaN", s);
+        GB_TRY(check_stage_db(db, g.n, who));
+        std::fill(b.begin(), b.end(), std::max(g.n, 0));
+        if (g.kind == GORSE_B200_STAGE_ITEM_TO_ITEM) {
+            GB_TRY(check_map("item-to-item stage", db, g.slot_of_item, g.item_of_slot));
+            GB_CHECK_ARG(g.ctx_off != nullptr, "stage %d: ctx_off is NULL", s);
+            GB_TRY(check_offsets(g.ctx_off, n_users, who, "ctx_off"));
+            GB_CHECK_ARG(g.n_categories >= 0 && (g.n_categories == 0 || g.categories != nullptr), "stage %d: categories", s);
+            GB_CHECK_ARG(g.ctx_off[n_users] == 0 || g.ctx_items != nullptr, "stage %d: ctx_items is NULL", s);
+            for (int64_t t = 0; t < g.ctx_off[n_users]; t++)
+                GB_CHECK_ARG(g.ctx_items[t] >= -1 && g.ctx_items[t] < n_items, "stage %d: context entry %lld: item %d is not in [-1, %d)", s,
+                             (long long)t, g.ctx_items[t], n_items);
+            return GORSE_B200_OK;
+        }
+        GB_CHECK_ARG(g.user_slots != nullptr, "stage %d: user_slots is NULL", s);
+        for (int64_t u = 0; u < n_users; u++)
+            GB_CHECK_ARG(g.user_slots[u] >= -1 && g.user_slots[u] < (int64_t)db->ts.size(), "stage %d: user %lld: slot %lld is not a slot", s,
+                         (long long)u, (long long)g.user_slots[u]);
+        return check_feedback(who, g.n_fb_rows, g.fb_off, g.fb_items, n_items);
+    }
+
+    // the ranker: features checked as gorse_b200_fm_rank checks them; the row lengths for D_u
+    int32_t check_ranker()
+    {
+        const auto &R = *ranker;
+        GB_TRY(fm::check_feats("user", n_users, R.user_feat, R.user_lab_off, R.user_lab_idx, R.user_lab_val, m->n_features));
+        GB_TRY(fm::check_feats("item", n_items, R.item_feat, R.item_lab_off, R.item_lab_idx, R.item_lab_val, m->n_features));
         if (m->n_emb > 0 && n_items > 0) {
             GB_CHECK_ARG(R.item_emb != nullptr, "item_emb is NULL");
             for (int s = 0; s < m->n_emb; s++) GB_CHECK_ARG(R.item_emb[s] != nullptr, "item_emb[%d] is NULL", s);
@@ -601,425 +517,325 @@ extern "C" int32_t gorse_b200_recommend(gorse_b200_ctx *ctx, int64_t n_users, co
             GB_CHECK_ARG(l + longest_item <= INT32_MAX, "user %lld: rows of 2^31 or more features", (long long)u);
             u_len[(size_t)u] = (int32_t)l;
         }
-    }
-    for (int64_t u = 0; u < n_users; u++)
-        GB_CHECK_ARG(bound[(size_t)u] <= INT32_MAX / 2, "user %lld: %lld candidates at most, above 2^30", (long long)u, (long long)bound[(size_t)u]);
-    GB_CHECK_ARG(items_out != nullptr && scores_out != nullptr, "NULL output");
-
-    // the context last: every other argument is checked without it
-    GB_CHECK_ARG(ctx != nullptr, "ctx is NULL");
-    Work *Wp = work(ctx);
-    if (!Wp) { set_error("host allocation failed"); return GORSE_B200_ERR_OOM; }
-    Work &W = *Wp;
-    std::lock_guard<std::mutex> wlk(W.mu);
-
-    // ---- host preparation of the item-to-item / user-to-user stages (the neighbour-table rows of the batch)
-    auto &sd = W.sd;
-    if (sd.size() < (size_t)n_stages) sd.resize((size_t)n_stages);
-    for (auto &x : sd) x.clear_host();
-    int64_t total_rows = 0, exact_total = 0;
-    for (int32_t s = 0; s < n_stages; s++) {
-        const auto &g = stages[s];
-        StageData &D = sd[(size_t)s];
-        if (g.kind == GORSE_B200_STAGE_ITEM_TO_ITEM) {
-            std::vector<int32_t> row_of(g.db->ts.size(), -1);
-            D.c_off.assign((size_t)n_users + 1, 0);
-            for (int64_t u = 0; u < n_users; u++) {
-                for (int64_t t = g.ctx_off[u]; t < g.ctx_off[u + 1]; t++) {
-                    const int64_t it = g.ctx_items[t];
-                    const int32_t r = table_row(g.db, it < 0 ? -1 : g.slot_of_item[it], row_of, D.nb);
-                    if (r >= 0) D.c_row.push_back(r);
-                }
-                D.c_off[(size_t)u + 1] = (int64_t)D.c_row.size();
-            }
-            D.es0_off.assign((size_t)n_users + 1, 0);
-            D.es0.reserve(e0.size());
-            for (int64_t u = 0; u < n_users; u++) {
-                const size_t b = D.es0.size();
-                for (int64_t t = e0_off[(size_t)u]; t < e0_off[(size_t)u + 1]; t++)
-                    if (g.slot_of_item[e0[(size_t)t]] >= 0) D.es0.push_back(g.slot_of_item[e0[(size_t)t]]);
-                std::sort(D.es0.begin() + b, D.es0.end());
-                D.es0_off[(size_t)u + 1] = (int64_t)D.es0.size();
-            }
-        } else if (g.kind == GORSE_B200_STAGE_USER_TO_USER) {
-            std::vector<int32_t> row_of(g.db->ts.size(), -1);
-            D.q_row.resize((size_t)n_users);
-            for (int64_t u = 0; u < n_users; u++) D.q_row[(size_t)u] = table_row(g.db, g.user_slots[u], row_of, D.nb);
-            int64_t longest = 0;
-            for (int64_t v = 0; v < g.n_fb_rows; v++) longest = std::max(longest, g.fb_off[v + 1] - g.fb_off[v]);
-            D.heavy = longest * std::max(g.n, 0) > agg::TABLE_KEYS;
-        }
-        total_rows += (int64_t)D.nb.size();
-    }
-    bool need_cf = false;
-    for (int32_t s = 0; s < n_stages; s++) need_cf |= stages[s].kind == GORSE_B200_STAGE_COLLABORATIVE;
-    std::vector<int64_t> cf_ex, cf_ex_off;
-    if (need_cf) {
-        cf_ex_off.assign((size_t)n_users + 1, 0);
-        for (int64_t u = 0; u < n_users; u++) {
-            const size_t b = cf_ex.size();
-            for (int64_t t = e0_off[(size_t)u]; t < e0_off[(size_t)u + 1]; t++)
-                if (cf->slot_of_item[e0[(size_t)t]] >= 0) cf_ex.push_back(cf->slot_of_item[e0[(size_t)t]]);
-            std::sort(cf_ex.begin() + b, cf_ex.end());
-            cf_ex_off[(size_t)u + 1] = (int64_t)cf_ex.size();
-        }
+        return GORSE_B200_OK;
     }
 
-    // ---- device: once per call
-    ScopedDevice sdev(ctx->device);
-    cudaStream_t st = ctx->stream;
-    auto done = [&](int32_t s) {
-        cudaStreamSynchronize(ctx->stream);
-        cudaStreamSynchronize(ctx->copy_stream);
-        return s;
-    };
-    auto &d_live = W.d_live;
-    auto &d_repl_pos = W.d_repl_pos;
-    auto &d_repl_items = W.d_repl_items;
-    auto &d_repl_off = W.d_repl_off;
-    auto &d_cf_excl_off = W.d_cf_excl_off;
-    auto &d_cf_item_of_slot = W.d_cf_item_of_slot;
-    int32_t rs = GORSE_B200_OK;
-    if ((rs = d_live.upload(item_live, (size_t)n_items, st))) return done(rs);
-    if (with_repl && ((rs = d_repl_off.upload(repl_off, (size_t)n_users + 1, st)) ||
-                      (rs = d_repl_items.upload(repl_items, (size_t)repl_off[n_users], st)) ||
-                      (rs = d_repl_pos.upload(repl_positive, (size_t)repl_off[n_users], st))))
-        return done(rs);
-    auto &l_items = W.l_items;
-    auto &l_scores = W.l_scores;
-    auto &l_off = W.l_off;
-    if (l_items.size() < (size_t)n_stages) {
-        l_items.resize((size_t)n_stages);
-        l_scores.resize((size_t)n_stages);
-        l_off.resize((size_t)n_stages);
-    }
-    for (int32_t s = 0; s < n_stages; s++) {
-        const auto &g = stages[s];
-        StageData &D = sd[(size_t)s];
-        if (g.kind == GORSE_B200_STAGE_LIST) {
-            const int64_t total = g.list_off ? g.list_off[n_users] : g.list_len;
-            if ((rs = l_items[(size_t)s].upload(g.list_items, (size_t)total, st)) || (rs = l_scores[(size_t)s].upload(g.list_scores, (size_t)total, st)) ||
-                (g.list_off && (rs = l_off[(size_t)s].upload(g.list_off, (size_t)n_users + 1, st))))
-                return done(rs);
-            continue;
-        }
-        if (g.kind == GORSE_B200_STAGE_COLLABORATIVE || g.n <= 0) continue;
-        const int64_t R = (int64_t)D.nb.size();
-        const int64_t S = (int64_t)g.db->ts.size();
-        const bool i2i = g.kind == GORSE_B200_STAGE_ITEM_TO_ITEM;
-        if (i2i) {
-            if ((rs = D.d_map.upload(g.slot_of_item, (size_t)n_items, st)) || (rs = D.d_item_of_slot.upload(g.item_of_slot, (size_t)S, st)) ||
-                (rs = D.d_c_row.upload(D.c_row.data(), D.c_row.size(), st)))
-                return done(rs);
-        } else {
-            const int64_t nf = g.n_fb_rows ? g.fb_off[g.n_fb_rows] : 0;
-            if ((rs = D.d_fb_off.upload(g.fb_off, g.n_fb_rows ? (size_t)g.n_fb_rows + 1 : 0, st)) || (rs = D.d_fb_items.upload(g.fb_items, (size_t)nf, st)) ||
-                (g.item_ok && (rs = D.d_item_ok.upload(g.item_ok, (size_t)n_items, st))) || (rs = D.d_q_row.upload(D.q_row.data(), D.q_row.size(), st)))
-                return done(rs);
-        }
-        if (R == 0) continue;
-        if ((rs = D.d_nb.grow((size_t)R)) || (rs = D.t_slot.grow((size_t)R * g.n)) || (rs = D.t_score.grow((size_t)R * g.n)) ||
-            (rs = D.t_cnt.grow((size_t)R)))
-            return done(rs);
-        int64_t exact = 0;
-        if ((rs = neighbour_table(g.db, D.nb, D.d_nb.p, g.n, i2i ? g.categories : nullptr, i2i ? g.n_categories : 0, D.t_slot.p, D.t_score.p,
-                                  D.t_cnt.p, &exact)))
-            return done(rs);
-        exact_total += exact;
-    }
-    // the CF recall rows stay in the CF index's recall buffers; computed after every neighbour table, which may use the same index
-    const int64_t *cf_slots = nullptr;
-    const float *cf_scores = nullptr;
-    const int32_t *cf_count = nullptr;
-    if (need_cf) {
-        if ((rs = d_cf_excl_off.upload(excl_off, (size_t)n_users + 1, st)) ||
-            (rs = d_cf_item_of_slot.upload(cf->item_of_slot, cf->db->ts.size(), st)))
-            return done(rs);
-        if (cf->n > 0 && !cf->db->ts.empty()) {
-            if ((rs = vecdb_allow(cf->db, nullptr, 0))) return done(rs);
-            std::lock_guard<std::mutex> lk2(cf->db->dense->mu);
-            int64_t exact = 0;
-            if ((rs = recall::recall_rows(cf->db->dense, cf->db->d_allow.p, n_users, cf->user_vectors, nullptr, cf->n, excl_off, cf_ex.data(),
-                                          cf_ex_off.data(), nullptr, nullptr, nullptr, nullptr, &exact)))
-                return done(rs);
-            exact_total += exact;
-            cf_slots = cf->db->dense->recall.slots.p;
-            cf_scores = cf->db->dense->recall.scores.p;
-            cf_count = cf->db->dense->recall.count.p;
-        }
-    }
-    // the ranker's user rows and the dictionary's item table, once
-    fm::Feats FU{}, FI{};
-    fm::Slot FS[fm::MAX_SLOTS];
-    auto &d_u_len = W.d_u_len;
-    auto &d_i_len = W.d_i_len;
-    if (m) {
-        const auto &R = *ranker;
-        if ((rs = m->u_feat.upload(R.user_feat, (size_t)n_users, st)) || (rs = m->u_off.upload(R.user_lab_off, (size_t)n_users + 1, st)) ||
-            (rs = m->u_idx.upload(R.user_lab_idx, (size_t)R.user_lab_off[n_users], st)) ||
-            (rs = m->u_val.upload(R.user_lab_val, (size_t)R.user_lab_off[n_users], st)) || (rs = m->i_feat.upload(R.item_feat, (size_t)n_items, st)) ||
-            (rs = m->i_off.upload(R.item_lab_off, n_items ? (size_t)n_items + 1 : 0, st)) ||
-            (rs = m->i_idx.upload(R.item_lab_idx, n_items ? (size_t)R.item_lab_off[n_items] : 0, st)) ||
-            (rs = m->i_val.upload(R.item_lab_val, n_items ? (size_t)R.item_lab_off[n_items] : 0, st)) ||
-            (rs = d_u_len.upload(u_len.data(), u_len.size(), st)) || (rs = d_i_len.upload(i_len.data(), i_len.size(), st)))
-            return done(rs);
-        if (m->n_emb > 0) {
-            if (R.item_emb_mask && (rs = m->mask.upload(R.item_emb_mask, (size_t)n_items * m->n_emb, st))) return done(rs);
-            for (int s = 0; s < m->n_emb; s++)
-                if ((rs = m->emb[s].upload(n_items ? R.item_emb[s] : nullptr, (size_t)n_items * m->dim[(size_t)s], st))) return done(rs);
-            if ((rs = fm::item_tables(m, n_items, R.item_emb_mask != nullptr, FS))) return done(rs);
-        }
-        FI = fm::Feats{m->i_feat.p, m->i_off.p, m->i_idx.p, m->i_val.p};
-    }
-
-    // ---- chunks: at most sm_count * 1024 users and CHUNK_ENTRIES candidate / exclude-set entries (or one user)
-    // (with embedding slots a sixteenth: the attention's vx rows take n_factors floats per candidate)
-    std::vector<int64_t> chunk_at{0};
+    // every argument but the context, on the host; locks the collections and the ranker
+    int32_t check()
     {
-        const int64_t lim = m && m->n_emb > 0 ? CHUNK_ENTRIES / 16 : CHUNK_ENTRIES;
-        int64_t b = 0, c = 0, users = 0;
-        for (int64_t u = 0; u < n_users; u++) {
-            if (users > 0 && (users == (int64_t)ctx->sm_count * 1024 || b + bound[(size_t)u] > lim || c + cap[(size_t)u] > lim)) {
-                chunk_at.push_back(u);
-                b = c = users = 0;
-            }
-            b += bound[(size_t)u];
-            c += cap[(size_t)u];
-            users++;
-        }
-        chunk_at.push_back(n_users);
-    }
-    const int64_t n_chunks = (int64_t)chunk_at.size() - 1;
-    int64_t max_rows = 0, max_b = 0, max_c = 0, max_e0 = 0, max_bound = 0;
-    for (int64_t k = 0; k < n_chunks; k++) {
-        const int64_t a = chunk_at[(size_t)k], z = chunk_at[(size_t)k + 1];
-        int64_t b = 0, c = 0;
-        for (int64_t u = a; u < z; u++) { b += bound[(size_t)u]; c += cap[(size_t)u]; max_bound = std::max(max_bound, bound[(size_t)u]); }
-        max_rows = std::max(max_rows, z - a);
-        max_b = std::max(max_b, b);
-        max_c = std::max(max_c, c);
-        max_e0 = std::max(max_e0, e0_off[(size_t)z] - e0_off[(size_t)a]);
-    }
-    // the output rows of the whole call at the bound prefix
-    std::vector<int64_t> out_at((size_t)n_users + 1, 0);
-    for (int64_t u = 0; u < n_users; u++) out_at[(size_t)u + 1] = out_at[(size_t)u] + bound[(size_t)u];
-
-    auto &d_cand_off = W.d_cand_off;
-    auto &d_E_off = W.d_E_off;
-    auto &d_e0_off = W.d_e0_off;
-    auto &d_e0 = W.d_e0;
-    auto &d_E = W.d_E;
-    auto &d_i2i_off = W.d_i2i_off;
-    auto &d_fm_off = W.d_fm_off;
-    auto &d_ch_off = W.d_ch_off;
-    auto &d_rids = W.d_rids;
-    auto &d_cand = W.d_cand;
-    auto &d_cnt = W.d_cnt;
-    auto &d_start = W.d_start;
-    auto &d_users = W.d_users;
-    auto &d_list = W.d_list;
-    auto &d_work = W.d_work;
-    auto &d_route = W.d_route;
-    auto &d_rcount = W.d_rcount;
-    auto &d_out_items = W.d_out_items;
-    auto &d_out_cnt = W.d_out_cnt;
-    auto &d_dims = W.d_dims;
-    auto &d_cscore = W.d_cscore;
-    auto &d_rscore = W.d_rscore;
-    auto &d_dscore = W.d_dscore;
-    auto &d_out_scores = W.d_out_scores;
-    auto &d_sort = W.d_sort;
-    int max_n = 0;
-    bool any_u2u = false;
-    for (int32_t s = 0; s < n_stages; s++)
-        if (stages[s].kind >= GORSE_B200_STAGE_ITEM_TO_ITEM) {
-            max_n = std::max(max_n, stages[s].n);
-            any_u2u |= stages[s].kind == GORSE_B200_STAGE_USER_TO_USER;
-        }
-    const int grid = (int)std::min<int64_t>(max_rows, (int64_t)ctx->sm_count * 8);
-    const int64_t sort_stride = recall::pow2_at_least((int)std::max<int64_t>(max_bound, 1));
-    // the re-sort's per-CTA key buffers, at most 256 MB of them (as fm_sort_kernel's)
-    const int emit_grid = (int)std::max<int64_t>(1, std::min<int64_t>(grid, (int64_t(256) << 20) / (sort_stride * (int64_t)sizeof(u128))));
-    if ((rs = d_cand_off.grow((size_t)max_rows + 1)) || (rs = d_E_off.grow((size_t)max_rows + 1)) ||
-        (rs = d_e0_off.grow((size_t)max_rows + 1)) || (rs = d_e0.grow((size_t)std::max<int64_t>(max_e0, 1))) ||
-        (rs = d_E[0].grow((size_t)std::max<int64_t>(max_c, 1))) || (rs = d_E[1].grow((size_t)std::max<int64_t>(max_c, 1))) ||
-        (rs = d_cand.grow((size_t)std::max<int64_t>(max_b, 1))) || (rs = d_cscore.grow((size_t)std::max<int64_t>(max_b, 1))) ||
-        (rs = d_cnt.grow((size_t)max_rows)) || (rs = d_start.grow((size_t)max_rows)) || (rs = d_users.grow((size_t)max_rows)) ||
-        (rs = d_i2i_off.grow((size_t)max_rows + 1)) || (rs = d_rcount.grow((size_t)max_rows)) ||
-        (rs = d_rids.grow((size_t)std::max<int64_t>(max_rows * max_n, 1))) || (rs = d_rscore.grow((size_t)std::max<int64_t>(max_rows * max_n, 1))))
-        return done(rs);
-    if (any_u2u && ((rs = d_list.grow((size_t)max_rows)) || (rs = d_work.grow((size_t)max_rows)) ||
-                    (rs = d_route.grow((size_t)n_chunks * 2 * n_stages))))
-        return done(rs);
-    if (any_u2u) GB_CUDA(cudaMemsetAsync(d_route.p, 0, sizeof(int32_t) * n_chunks * 2 * n_stages, st));
-    for (int32_t s = 0; s < n_stages; s++) {
-        StageData &D = sd[(size_t)s];
-        const auto &g = stages[s];
-        if (g.kind == GORSE_B200_STAGE_ITEM_TO_ITEM) {
-            if ((rs = D.d_es0.upload(D.es0.data(), D.es0.size(), st)) || (rs = D.ES[0].grow((size_t)std::max<int64_t>(max_c, 1))) ||
-                (rs = D.ES[1].grow((size_t)std::max<int64_t>(max_c, 1))))
-                return done(rs);
-            const int64_t N = (int64_t)g.db->ts.size();
-            std::vector<int32_t> routed;
-            const bool heavy = i2i::route(D.c_off.data(), n_users, g.n, routed) < n_users;
-            const int hg = heavy_grid(ctx, std::max<int64_t>(N, 1), i2i::ROW_BYTES);
-            if (heavy && N > 0 && ((rs = D.acc.grow((size_t)hg * N)) || (rs = D.seen.grow_zeroed((size_t)hg * N, st)) ||
-                                   (rs = D.touched.grow((size_t)hg * N))))
-                return done(rs);
-        } else if (g.kind == GORSE_B200_STAGE_USER_TO_USER && D.heavy) {
-            const int64_t NI = std::max<int64_t>(n_items, 1);
-            const int hg = heavy_grid(ctx, NI, u2u::ROW_BYTES);
-            if ((rs = D.uacc.grow_zeroed((size_t)hg * NI, st)) || (rs = D.flag.grow_zeroed((size_t)hg * NI, st)) ||
-                (rs = D.touched.grow((size_t)hg * NI)))
-                return done(rs);
-        }
-    }
-    for (int p = 0; p < 2; p++)
-        if ((rs = d_out_items[p].grow((size_t)std::max<int64_t>(max_b, 1))) || (rs = d_out_scores[p].grow((size_t)std::max<int64_t>(max_b, 1))) ||
-            (rs = d_out_cnt[p].grow((size_t)max_rows)))
-            return done(rs);
-    if (m && ((rs = d_fm_off.grow((size_t)max_rows + 1)) || (rs = d_dims.grow((size_t)max_rows)) ||
-              (rs = d_dscore.grow((size_t)std::max<int64_t>(max_b, 1))) || (rs = m->cand.grow((size_t)std::max<int64_t>(max_b, 1))) ||
-              (rs = m->score.grow((size_t)std::max<int64_t>(max_b, 1))) || (rs = m->order.grow((size_t)std::max<int64_t>(max_b, 1))) ||
-              (rs = d_sort.grow((size_t)emit_grid * sort_stride))))
-        return done(rs);
-    if (m && m->n_emb > 0 && ((rs = m->vx.grow((size_t)std::max<int64_t>(max_b, 1) * m->k)) || (rs = m->rowsum.grow((size_t)std::max<int64_t>(max_b, 1)))))
-        return done(rs);
-    cudaEvent_t reuse[2] = {nullptr, nullptr};
-    GB_CUDA(cudaEventCreateWithFlags(&reuse[0], cudaEventDisableTiming));
-    if (cudaEventCreateWithFlags(&reuse[1], cudaEventDisableTiming) != cudaSuccess) {
-        cudaEventDestroy(reuse[0]);
-        set_error("recommend: event creation failed");
-        return GORSE_B200_ERR_CUDA;
-    }
-    auto finish = [&](int32_t s) {
-        done(s);
-        cudaEventDestroy(reuse[0]);
-        cudaEventDestroy(reuse[1]);
-        return s;
-    };
-#define REC_TRY(call)                          \
-    do {                                       \
-        int32_t s_ = (call);                   \
-        if (s_ != GORSE_B200_OK) return finish(s_); \
-    } while (0)
-#define REC_CUDA(call)                                                                        \
-    do {                                                                                      \
-        cudaError_t e_ = (call);                                                              \
-        if (e_ != cudaSuccess) {                                                              \
-            set_error("recommend: %s -> %s", #call, cudaGetErrorString(e_));                  \
-            return finish(e_ == cudaErrorMemoryAllocation ? GORSE_B200_ERR_OOM : GORSE_B200_ERR_CUDA); \
-        }                                                                                     \
-    } while (0)
-
-    int64_t ranked = 0;
-    std::vector<int64_t> h_cand_off, h_E_off, h_e0_off, h_i2i_off, h_ch_off;
-    std::vector<int32_t> h_users;
-    for (int64_t k = 0; k < n_chunks; k++) {
-        const int64_t u0 = chunk_at[(size_t)k], rows = chunk_at[(size_t)k + 1] - u0;
-        const int p = (int)(k & 1);
-        h_cand_off.assign((size_t)rows + 1, 0);
-        h_E_off.assign((size_t)rows + 1, 0);
-        h_e0_off.assign((size_t)rows + 1, 0);
-        for (int64_t r = 0; r < rows; r++) {
-            h_cand_off[(size_t)r + 1] = h_cand_off[(size_t)r] + bound[(size_t)(u0 + r)];
-            h_E_off[(size_t)r + 1] = h_E_off[(size_t)r] + cap[(size_t)(u0 + r)];
-            h_e0_off[(size_t)r + 1] = e0_off[(size_t)(u0 + r + 1)] - e0_off[(size_t)u0];
-        }
-        REC_CUDA(cudaMemcpyAsync(d_cand_off.p, h_cand_off.data(), sizeof(int64_t) * (rows + 1), cudaMemcpyHostToDevice, st));
-        REC_CUDA(cudaMemcpyAsync(d_E_off.p, h_E_off.data(), sizeof(int64_t) * (rows + 1), cudaMemcpyHostToDevice, st));
-        REC_CUDA(cudaMemcpyAsync(d_e0_off.p, h_e0_off.data(), sizeof(int64_t) * (rows + 1), cudaMemcpyHostToDevice, st));
-        if (h_e0_off[(size_t)rows])
-            REC_CUDA(cudaMemcpyAsync(d_e0.p, e0.data() + e0_off[(size_t)u0], sizeof(int64_t) * h_e0_off[(size_t)rows], cudaMemcpyHostToDevice, st));
-        REC_CUDA(cudaMemsetAsync(d_cnt.p, 0, sizeof(int32_t) * rows, st));
-        // E_u from E0, and the item-to-item stages' sets in slots
-        int e_cur = 0;
-        rec_grow_kernel<<<grid, NT, 0, st>>>(d_e0.p, d_e0_off.p, d_E[0].p, d_E_off.p, nullptr, nullptr, nullptr, nullptr, nullptr, rows);
-        ctx->launches++;
-        for (int32_t s = 0; s < n_stages; s++) {
-            StageData &D = sd[(size_t)s];
-            if (stages[s].kind != GORSE_B200_STAGE_ITEM_TO_ITEM) continue;
-            for (int64_t r = 0; r <= rows; r++) h_e0_off[(size_t)r] = D.es0_off[(size_t)(u0 + r)] - D.es0_off[(size_t)u0];
-            REC_CUDA(cudaMemcpyAsync(d_i2i_off.p, h_e0_off.data(), sizeof(int64_t) * (rows + 1), cudaMemcpyHostToDevice, st));
-            rec_grow_kernel<<<grid, NT, 0, st>>>(D.d_es0.p + D.es0_off[(size_t)u0], d_i2i_off.p, D.ES[0].p, d_E_off.p, nullptr, nullptr, nullptr, nullptr,
-                                                 nullptr, rows);
-            ctx->launches++;
-        }
-        REC_CUDA(cudaGetLastError());
+        GB_CHECK_ARG(count_out != nullptr && excl_off != nullptr, "count_out / excl_off is NULL");
+        GB_CHECK_ARG(n_stages == 0 || stages != nullptr, "stages is NULL");
+        GB_CHECK_ARG(n_items == 0 || item_live != nullptr, "item_live is NULL");
+        GB_TRY(check_offsets(excl_off, n_users, "recommend", "excl_off"));
+        GB_CHECK_ARG(excl_off[n_users] == 0 || excl_items != nullptr, "excl_items is NULL");
+        GB_TRY(exclusion_rows(n_users, excl_off, excl_items, n_items, "user", "item", e0, e0_off));
+        std::vector<gorse_b200_vecdb *> dbs;
         for (int32_t s = 0; s < n_stages; s++) {
             const auto &g = stages[s];
-            StageData &D = sd[(size_t)s];
-            REC_CUDA(cudaMemcpyAsync(d_start.p, d_cnt.p, sizeof(int32_t) * rows, cudaMemcpyDeviceToDevice, st));
-            const int64_t *E = d_E[e_cur].p;
+            GB_CHECK_ARG(g.kind >= GORSE_B200_STAGE_LIST && g.kind <= GORSE_B200_STAGE_USER_TO_USER, "stage %d: unknown kind %d", s, g.kind);
+            if (g.kind == GORSE_B200_STAGE_ITEM_TO_ITEM || g.kind == GORSE_B200_STAGE_USER_TO_USER) {
+                GB_CHECK_ARG(g.db != nullptr && g.db->ctx == ctx, "stage %d: collection is NULL or of another context", s);
+                dbs.push_back(g.db);
+            }
+            if (g.kind == GORSE_B200_STAGE_COLLABORATIVE) GB_CHECK_ARG(cf != nullptr, "stage %d: a collaborative stage needs the CF inputs", s);
+        }
+        if (cf) {
+            GB_CHECK_ARG(cf->db != nullptr && cf->db->ctx == ctx, "CF collection is NULL or of another context");
+            dbs.push_back(cf->db);
+        }
+        std::sort(dbs.begin(), dbs.end());
+        dbs.erase(std::unique(dbs.begin(), dbs.end()), dbs.end());
+        for (auto *db : dbs) locks.emplace_back(db->mu);
+        if (ranker) {
+            GB_CHECK_ARG(ranker->fm != nullptr && ranker->fm->ctx == ctx, "ranker: fm handle is NULL or of another context");
+            fm_lock = std::unique_lock<std::mutex>(ranker->fm->mu);
+        }
+
+        // per stage: checks and the per-user bound
+        bound.assign((size_t)n_users, 0);
+        cap.resize((size_t)n_users);
+        for (int64_t u = 0; u < n_users; u++) cap[(size_t)u] = e0_off[(size_t)u + 1] - e0_off[(size_t)u];
+        std::vector<int64_t> b((size_t)n_users);
+        for (int32_t s = 0; s < n_stages; s++) {
+            std::fill(b.begin(), b.end(), 0);
+            GB_TRY(check_stage(s, b));
+            for (int64_t u = 0; u < n_users; u++) {
+                bound[(size_t)u] += b[(size_t)u];
+                if (s + 1 < n_stages) cap[(size_t)u] += b[(size_t)u];
+            }
+        }
+        if (cf) {
+            if (cf->db->dim == 0) { set_error("the CF collection must be dense"); return GORSE_B200_ERR_UNSUPPORTED; }
+            GB_CHECK_ARG(cf->n >= 0 && cf->n <= MAX_N_DENSE, "CF n = %d is not in [0, %d]", cf->n, MAX_N_DENSE);
+            GB_CHECK_ARG(cf->user_vectors != nullptr, "CF user_vectors is NULL");
+            GB_TRY(check_map("CF", cf->db, cf->slot_of_item, cf->item_of_slot));
+            for (int64_t u = 0; u < n_users; u++)
+                GB_CHECK_ARG((int64_t)cf->n + (excl_off[u + 1] - excl_off[u]) <= INT32_MAX, "user %lld: n + |E0| overflows", (long long)u);
+        }
+        with_repl = ranker && repl_off;
+        if (with_repl) {
+            GB_TRY(check_offsets(repl_off, n_users, "recommend", "repl_off"));
+            GB_CHECK_ARG(positive_decay == positive_decay && read_decay == read_decay, "a decay is NaN");
+            GB_CHECK_ARG(repl_off[n_users] == 0 || (repl_items != nullptr && repl_positive != nullptr), "repl_items / repl_positive is NULL");
+            std::vector<int32_t> row;
+            for (int64_t u = 0; u < n_users; u++) {
+                row.assign(repl_items + repl_off[u], repl_items + repl_off[u + 1]);
+                for (int32_t it : row) GB_CHECK_ARG(it >= 0 && it < n_items, "user %lld: replacement item %d is not in [0, %d)", (long long)u, it, n_items);
+                std::sort(row.begin(), row.end());
+                GB_CHECK_ARG(std::adjacent_find(row.begin(), row.end()) == row.end(), "user %lld: a replacement item twice", (long long)u);
+                bound[(size_t)u] += repl_off[u + 1] - repl_off[u];
+            }
+        }
+        m = ranker ? ranker->fm : nullptr;
+        if (m) GB_TRY(check_ranker());
+        for (int64_t u = 0; u < n_users; u++)
+            GB_CHECK_ARG(bound[(size_t)u] <= INT32_MAX / 2, "user %lld: %lld candidates at most, above 2^30", (long long)u, (long long)bound[(size_t)u]);
+        GB_CHECK_ARG(items_out != nullptr && scores_out != nullptr, "NULL output");
+        return GORSE_B200_OK;
+    }
+
+    // E0 of every user through slot_of_item, -1 dropped, sorted: the exclude sets in a collection's slots
+    void slot_rows(const int64_t *slot_of_item, std::vector<int64_t> &ex, std::vector<int64_t> &ex_off) const
+    {
+        ex.reserve(e0.size());
+        ex_off.assign((size_t)n_users + 1, 0);
+        for (int64_t u = 0; u < n_users; u++) {
+            const size_t b = ex.size();
+            for (int64_t t = e0_off[(size_t)u]; t < e0_off[(size_t)u + 1]; t++)
+                if (slot_of_item[e0[(size_t)t]] >= 0) ex.push_back(slot_of_item[e0[(size_t)t]]);
+            std::sort(ex.begin() + b, ex.end());
+            ex_off[(size_t)u + 1] = (int64_t)ex.size();
+        }
+    }
+
+    // once per call: the live and replacement items, the list stages' rows, and every item-to-item / user-to-user stage's table
+    // rows and neighbour table
+    int32_t tables(Work &W)
+    {
+        const cudaStream_t st = ctx->stream;
+        GB_TRY(W.d_live.upload(item_live, (size_t)n_items, st));
+        if (with_repl) {
+            GB_TRY(W.d_repl_off.upload(repl_off, (size_t)n_users + 1, st));
+            GB_TRY(W.d_repl_items.upload(repl_items, (size_t)repl_off[n_users], st));
+            GB_TRY(W.d_repl_pos.upload(repl_positive, (size_t)repl_off[n_users], st));
+        }
+        if (W.lists.size() < (size_t)n_stages) W.lists.resize((size_t)n_stages);
+        if (W.sd.size() < (size_t)n_stages) W.sd.resize((size_t)n_stages);
+        for (int32_t s = 0; s < n_stages; s++) {
+            const auto &g = stages[s];
             if (g.kind == GORSE_B200_STAGE_LIST) {
-                rec_list_kernel<<<grid, NT, 0, st>>>(l_items[(size_t)s].p, l_scores[(size_t)s].p, g.list_off ? l_off[(size_t)s].p : nullptr, g.list_len, u0,
-                                                     E, d_E_off.p, d_cand.p, d_cscore.p, d_cand_off.p, d_cnt.p, rows);
+                const int64_t total = g.list_off ? g.list_off[n_users] : g.list_len;
+                Work::List &L = W.lists[(size_t)s];
+                GB_TRY(L.items.upload(g.list_items, (size_t)total, st));
+                GB_TRY(L.scores.upload(g.list_scores, (size_t)total, st));
+                if (g.list_off) GB_TRY(L.off.upload(g.list_off, (size_t)n_users + 1, st));
+                continue;
+            }
+            if (g.kind == GORSE_B200_STAGE_COLLABORATIVE) continue;
+            NeighbourStage &D = W.sd[(size_t)s];
+            const bool i2i = g.kind == GORSE_B200_STAGE_ITEM_TO_ITEM;
+            if (i2i) {
+                D.prepare_items(g.db, n_users, g.ctx_off, g.ctx_items, g.slot_of_item, g.n, 0, g.n, g.score_scale, nullptr);
+                slot_rows(g.slot_of_item, D.es0, D.es0_off);
+            } else {
+                D.prepare_users(g.db, n_users, g.user_slots, g.n_fb_rows, g.fb_off, g.fb_items, n_items, g.n, g.score_scale, g.item_ok);
+            }
+            total_rows += (int64_t)D.nb.size();
+            if (g.n <= 0) continue;
+            if (i2i) {
+                GB_TRY(D.map.upload(g.slot_of_item, (size_t)n_items, st));
+                GB_TRY(D.item_of_slot.upload(g.item_of_slot, g.db->ts.size(), st));
+            }
+            int64_t exact = 0;
+            GB_TRY(D.table(i2i ? g.categories : nullptr, i2i ? g.n_categories : 0, &exact));
+            exact_total += exact;
+        }
+        return GORSE_B200_OK;
+    }
+
+    // once per call, after every neighbour table (which may use the CF index): the CF recall rows, left in the CF index's recall
+    // buffers; the ranker's user rows and the dictionary's item table
+    int32_t recall_and_ranker(Work &W)
+    {
+        const cudaStream_t st = ctx->stream;
+        bool need_cf = false;
+        for (int32_t s = 0; s < n_stages; s++) need_cf |= stages[s].kind == GORSE_B200_STAGE_COLLABORATIVE;
+        if (need_cf) {
+            std::vector<int64_t> cf_ex, cf_ex_off;
+            slot_rows(cf->slot_of_item, cf_ex, cf_ex_off);
+            GB_TRY(W.d_cf_excl_off.upload(excl_off, (size_t)n_users + 1, st));
+            GB_TRY(W.d_cf_item_of_slot.upload(cf->item_of_slot, cf->db->ts.size(), st));
+            if (cf->n > 0 && !cf->db->ts.empty()) {
+                GB_TRY(vecdb_allow(cf->db, nullptr, 0));
+                std::lock_guard<std::mutex> lk2(cf->db->dense->mu);
+                int64_t exact = 0;
+                GB_TRY(recall::recall_rows(cf->db->dense, cf->db->d_allow.p, n_users, cf->user_vectors, nullptr, cf->n, excl_off, cf_ex.data(),
+                                           cf_ex_off.data(), nullptr, nullptr, nullptr, nullptr, &exact));
+                exact_total += exact;
+                cf_slots = cf->db->dense->recall.slots.p;
+                cf_scores = cf->db->dense->recall.scores.p;
+                cf_count = cf->db->dense->recall.count.p;
+            }
+        }
+        if (!m) return GORSE_B200_OK;
+        const auto &R = *ranker;
+        GB_TRY(fm::upload_feats(m, n_users, R.user_feat, R.user_lab_off, R.user_lab_idx, R.user_lab_val, n_items, R.item_feat, R.item_lab_off,
+                                R.item_lab_idx, R.item_lab_val, R.item_emb, R.item_emb_mask, FS));
+        GB_TRY(W.d_u_len.upload(u_len.data(), u_len.size(), st));
+        GB_TRY(W.d_i_len.upload(i_len.data(), i_len.size(), st));
+        FI = fm::Feats{m->i_feat.p, m->i_off.p, m->i_idx.p, m->i_val.p};
+        return GORSE_B200_OK;
+    }
+
+    // the chunks: at most sm_count * 1024 users and CHUNK_ENTRIES candidate / exclude-set entries (or one user; with embedding
+    // slots a sixteenth: the attention's vx rows take n_factors floats per candidate), and every buffer sized for the largest
+    int32_t plan(Work &W)
+    {
+        const cudaStream_t st = ctx->stream;
+        const int64_t lim = m && m->n_emb > 0 ? CHUNK_ENTRIES / 16 : CHUNK_ENTRIES;
+        // one pass: the cuts, each chunk's rows and entries, and the output rows of the whole call at the bound prefix
+        int64_t max_rows = 0, max_b = 0, max_c = 0, max_e0 = 0, max_bound = 0, b = 0, c = 0;
+        out_at.assign((size_t)n_users + 1, 0);
+        for (int64_t u = 0; u <= n_users; u++) {
+            const int64_t a = chunk_at.back();
+            if (u == n_users ||
+                (u > a && (u - a == (int64_t)ctx->sm_count * 1024 || b + bound[(size_t)u] > lim || c + cap[(size_t)u] > lim))) {
+                max_rows = std::max(max_rows, u - a);
+                max_b = std::max(max_b, b);
+                max_c = std::max(max_c, c);
+                max_e0 = std::max(max_e0, e0_off[(size_t)u] - e0_off[(size_t)a]);
+                chunk_at.push_back(u);
+                b = c = 0;
+            }
+            if (u == n_users) break;
+            b += bound[(size_t)u];
+            c += cap[(size_t)u];
+            max_bound = std::max(max_bound, bound[(size_t)u]);
+            out_at[(size_t)u + 1] = out_at[(size_t)u] + bound[(size_t)u];
+        }
+        n_chunks = (int64_t)chunk_at.size() - 1;
+        int max_n = 0;
+        for (int32_t s = 0; s < n_stages; s++)
+            if (stages[s].kind >= GORSE_B200_STAGE_ITEM_TO_ITEM) max_n = std::max(max_n, stages[s].n);
+        grid = (int)std::min<int64_t>(max_rows, (int64_t)ctx->sm_count * 8);
+        sort_stride = recall::pow2_at_least((int)std::max<int64_t>(max_bound, 1));
+        // the re-sort's per-CTA key buffers, at most 256 MB of them (as fm_sort_kernel's)
+        emit_grid = (int)std::max<int64_t>(1, std::min<int64_t>(grid, (int64_t(256) << 20) / (sort_stride * (int64_t)sizeof(u128))));
+        const size_t rows = (size_t)max_rows, B = (size_t)std::max<int64_t>(max_b, 1), Cn = (size_t)std::max<int64_t>(max_c, 1);
+        for (auto *b : {&W.d_cand_off, &W.d_E_off, &W.d_e0_off}) GB_TRY(b->grow(rows + 1));
+        for (auto *b : {&W.d_cnt, &W.d_start, &W.d_rcount, &W.d_out_cnt[0], &W.d_out_cnt[1]}) GB_TRY(b->grow(rows));
+        for (auto *b : {&W.d_cand, &W.d_out_items[0], &W.d_out_items[1]}) GB_TRY(b->grow(B));
+        for (auto *b : {&W.d_cscore, &W.d_out_scores[0], &W.d_out_scores[1]}) GB_TRY(b->grow(B));
+        GB_TRY(W.d_e0.grow((size_t)std::max<int64_t>(max_e0, 1)));
+        GB_TRY(W.d_E[0].grow(Cn));
+        GB_TRY(W.d_E[1].grow(Cn));
+        GB_TRY(W.d_rids.grow((size_t)std::max<int64_t>(max_rows * max_n, 1)));
+        GB_TRY(W.d_rscore.grow((size_t)std::max<int64_t>(max_rows * max_n, 1)));
+        for (int32_t s = 0; s < n_stages; s++) {
+            const auto &g = stages[s];
+            NeighbourStage &D = W.sd[(size_t)s];
+            if (g.kind == GORSE_B200_STAGE_ITEM_TO_ITEM) {
+                GB_TRY(D.d_es0.upload(D.es0.data(), D.es0.size(), st));
+                GB_TRY(D.d_es0_off.upload(D.es0_off.data(), D.es0_off.size(), st));
+                GB_TRY(D.es[0].grow(Cn));
+                GB_TRY(D.es[1].grow(Cn));
+            }
+            if (g.kind >= GORSE_B200_STAGE_ITEM_TO_ITEM && g.n > 0) GB_TRY(D.reserve(max_rows, n_chunks));
+        }
+        if (!m) return GORSE_B200_OK;
+        GB_TRY(W.d_fm_off.grow(rows + 1));
+        GB_TRY(W.d_dims.grow(rows));
+        GB_TRY(W.d_dscore.grow(B));
+        for (auto *b : {&m->cand, &m->order}) GB_TRY(b->grow(B));
+        GB_TRY(m->score.grow(B));
+        GB_TRY(W.d_sort.grow((size_t)emit_grid * sort_stride));
+        if (m->n_emb > 0) {
+            GB_TRY(m->vx.grow(B * m->k));
+            GB_TRY(m->rowsum.grow(B));
+        }
+        return GORSE_B200_OK;
+    }
+
+    // chunk k: E_u, every stage in order, the assembly, the ranking, and the download of its answer on the copy stream into the
+    // output buffers of parity k & 1, free once the download of chunk k - 2 has finished (reuse[k & 1])
+    int32_t run_chunk(Work &W, int64_t k, Event *reuse)
+    {
+        const cudaStream_t st = ctx->stream;
+        const int64_t u0 = chunk_at[(size_t)k], rows = chunk_at[(size_t)k + 1] - u0;
+        const int p = (int)(k & 1);
+        h_cand_off.resize((size_t)rows + 1);
+        h_E_off.assign((size_t)rows + 1, 0);
+        h_e0_off.resize((size_t)rows + 1);
+        for (int64_t r = 0; r <= rows; r++) {
+            h_cand_off[(size_t)r] = out_at[(size_t)(u0 + r)] - out_at[(size_t)u0];
+            h_e0_off[(size_t)r] = e0_off[(size_t)(u0 + r)] - e0_off[(size_t)u0];
+            if (r < rows) h_E_off[(size_t)r + 1] = h_E_off[(size_t)r] + cap[(size_t)(u0 + r)];
+        }
+        GB_CUDA(cudaMemcpyAsync(W.d_cand_off.p, h_cand_off.data(), sizeof(int64_t) * (rows + 1), cudaMemcpyHostToDevice, st));
+        GB_CUDA(cudaMemcpyAsync(W.d_E_off.p, h_E_off.data(), sizeof(int64_t) * (rows + 1), cudaMemcpyHostToDevice, st));
+        GB_CUDA(cudaMemcpyAsync(W.d_e0_off.p, h_e0_off.data(), sizeof(int64_t) * (rows + 1), cudaMemcpyHostToDevice, st));
+        if (h_e0_off[(size_t)rows])
+            GB_CUDA(cudaMemcpyAsync(W.d_e0.p, e0.data() + e0_off[(size_t)u0], sizeof(int64_t) * h_e0_off[(size_t)rows], cudaMemcpyHostToDevice, st));
+        GB_CUDA(cudaMemsetAsync(W.d_cnt.p, 0, sizeof(int32_t) * rows, st));
+        // E_u from E0, and the item-to-item stages' sets in slots
+        int e_cur = 0;
+        rec_grow_kernel<<<grid, NT, 0, st>>>(W.d_e0.p, W.d_e0_off.p, W.d_E[0].p, W.d_E_off.p, nullptr, nullptr, nullptr, nullptr, nullptr, rows);
+        ctx->launches++;
+        for (int32_t s = 0; s < n_stages; s++) {
+            NeighbourStage &D = W.sd[(size_t)s];
+            if (stages[s].kind != GORSE_B200_STAGE_ITEM_TO_ITEM) continue;
+            rec_grow_kernel<<<grid, NT, 0, st>>>(D.d_es0.p, D.d_es0_off.p + u0, D.es[0].p, W.d_E_off.p, nullptr, nullptr, nullptr, nullptr, nullptr,
+                                                 rows);
+            ctx->launches++;
+        }
+        GB_CUDA(cudaGetLastError());
+        for (int32_t s = 0; s < n_stages; s++) {
+            const auto &g = stages[s];
+            NeighbourStage &D = W.sd[(size_t)s];
+            GB_CUDA(cudaMemcpyAsync(W.d_start.p, W.d_cnt.p, sizeof(int32_t) * rows, cudaMemcpyDeviceToDevice, st));
+            const int64_t *E = W.d_E[e_cur].p;
+            if (g.kind == GORSE_B200_STAGE_LIST) {
+                const Work::List &L = W.lists[(size_t)s];
+                rec_list_kernel<<<grid, NT, 0, st>>>(L.items.p, L.scores.p, g.list_off ? L.off.p : nullptr, g.list_len, u0, E, W.d_E_off.p, W.d_cand.p,
+                                                     W.d_cscore.p, W.d_cand_off.p, W.d_cnt.p, rows);
                 ctx->launches++;
             } else if (g.kind == GORSE_B200_STAGE_COLLABORATIVE) {
                 if (cf_slots) {
-                    rec_cf_kernel<<<grid, NT, 0, st>>>(cf_slots, cf_scores, cf_count, d_cf_excl_off.p, cf->n, u0, d_cf_item_of_slot.p, d_live.p, E,
-                                                       d_E_off.p, d_cand.p, d_cscore.p, d_cand_off.p, d_cnt.p, rows);
+                    rec_cf_kernel<<<grid, NT, 0, st>>>(cf_slots, cf_scores, cf_count, W.d_cf_excl_off.p, cf->n, u0, W.d_cf_item_of_slot.p,
+                                                       W.d_live.p, E, W.d_E_off.p, W.d_cand.p, W.d_cscore.p, W.d_cand_off.p, W.d_cnt.p, rows);
                     ctx->launches++;
                 }
             } else if (g.n > 0 && !D.nb.empty()) {
-                const bool euclid = g.db->distance == GORSE_B200_DISTANCE_EUCLIDEAN;
-                if (g.kind == GORSE_B200_STAGE_ITEM_TO_ITEM) {
-                    // the context rows of the chunk, users routed by |C_u| n as gorse_b200_vecdb_item_to_item routes them
-                    h_i2i_off.resize((size_t)rows + 1);
-                    for (int64_t r = 0; r <= rows; r++) h_i2i_off[(size_t)r] = D.c_off[(size_t)(u0 + r)] - D.c_off[(size_t)u0];
-                    const int64_t fill = i2i::route(h_i2i_off.data(), rows, g.n, h_users);
-                    REC_CUDA(cudaMemcpyAsync(d_i2i_off.p, h_i2i_off.data(), sizeof(int64_t) * (rows + 1), cudaMemcpyHostToDevice, st));
-                    REC_CUDA(cudaMemcpyAsync(d_users.p, h_users.data(), sizeof(int32_t) * rows, cudaMemcpyHostToDevice, st));
-                    i2i::Users U;
-                    U.c_off = d_i2i_off.p; U.c_row = D.d_c_row.p + D.c_off[(size_t)u0]; U.ex_off = d_E_off.p; U.ex = D.ES[e_cur].p;
-                    U.slots = d_rids.p; U.scores = d_rscore.p; U.count = d_rcount.p;
-                    const NeighbourTable T{D.t_slot.p, D.t_score.p, D.t_cnt.p};
-                    REC_TRY(i2i::aggregate(ctx, d_users.p, fill, rows - fill, U, T, nullptr, g.n, 0, g.n, g.score_scale, euclid,
-                                           (int64_t)g.db->ts.size(), D.acc.p, D.seen.p, D.touched.p));
-                    rec_append_kernel<<<grid, NT, 0, st>>>(d_rids.p, d_rscore.p, d_rcount.p, g.n, D.d_item_of_slot.p, d_cand.p, d_cscore.p,
-                                                           d_cand_off.p, d_cnt.p, rows);
-                } else {
-                    u2u::Users U;
-                    U.q_row = D.d_q_row.p + u0; U.ex_off = d_E_off.p; U.ex = E; U.item_ok = g.item_ok ? D.d_item_ok.p : nullptr;
-                    U.items = d_rids.p; U.scores = d_rscore.p; U.count = d_rcount.p;
-                    const NeighbourTable T{D.t_slot.p, D.t_score.p, D.t_cnt.p};
-                    const u2u::Feedback F{D.d_fb_off.p, D.d_fb_items.p, g.n_fb_rows};
-                    u2u::Route Rt;
-                    Rt.list = d_list.p; Rt.cnt = d_route.p + 2 * (k * n_stages + s); Rt.work = d_work.p; Rt.users = rows;
-                    REC_TRY(u2u::aggregate(ctx, Rt, U, T, F, g.n, g.score_scale, euclid, std::max<int64_t>(n_items, 1), D.heavy, D.uacc.p, D.flag.p,
-                                           D.touched.p));
-                    rec_append_kernel<<<grid, NT, 0, st>>>(d_rids.p, d_rscore.p, d_rcount.p, g.n, nullptr, d_cand.p, d_cscore.p, d_cand_off.p,
-                                                           d_cnt.p, rows);
-                }
+                // the item-to-item stage excludes in its collection's slots and maps its row back to items
+                const bool i2i = g.kind == GORSE_B200_STAGE_ITEM_TO_ITEM;
+                GB_TRY(D.run_chunk(k, u0, rows, W.d_E_off.p, i2i ? D.es[e_cur].p : E, W.d_rids.p, W.d_rscore.p, W.d_rcount.p));
+                rec_append_kernel<<<grid, NT, 0, st>>>(W.d_rids.p, W.d_rscore.p, W.d_rcount.p, g.n, i2i ? D.item_of_slot.p : nullptr, W.d_cand.p,
+                                                       W.d_cscore.p, W.d_cand_off.p, W.d_cnt.p, rows);
                 ctx->launches++;
             }
-            REC_CUDA(cudaGetLastError());
+            GB_CUDA(cudaGetLastError());
             if (s + 1 == n_stages) break;
             // E_u grows by what the stage appended, after the whole stage
-            rec_grow_kernel<<<grid, NT, 0, st>>>(d_E[e_cur].p, d_E_off.p, d_E[e_cur ^ 1].p, d_E_off.p, d_cand.p, d_cand_off.p, d_start.p, d_cnt.p,
-                                                 nullptr, rows);
+            rec_grow_kernel<<<grid, NT, 0, st>>>(W.d_E[e_cur].p, W.d_E_off.p, W.d_E[e_cur ^ 1].p, W.d_E_off.p, W.d_cand.p, W.d_cand_off.p, W.d_start.p,
+                                                 W.d_cnt.p, nullptr, rows);
             ctx->launches++;
-            for (int32_t t = 0; t < n_stages; t++) {
-                StageData &Dt = sd[(size_t)t];
-                if (stages[t].kind != GORSE_B200_STAGE_ITEM_TO_ITEM || t <= s) continue;
-                rec_grow_kernel<<<grid, NT, 0, st>>>(Dt.ES[e_cur].p, d_E_off.p, Dt.ES[e_cur ^ 1].p, d_E_off.p, d_cand.p, d_cand_off.p, d_start.p,
-                                                     d_cnt.p, Dt.d_map.p, rows);
+            for (int32_t t = s + 1; t < n_stages; t++) {
+                NeighbourStage &Dt = W.sd[(size_t)t];
+                if (stages[t].kind != GORSE_B200_STAGE_ITEM_TO_ITEM) continue;
+                rec_grow_kernel<<<grid, NT, 0, st>>>(Dt.es[e_cur].p, W.d_E_off.p, Dt.es[e_cur ^ 1].p, W.d_E_off.p, W.d_cand.p, W.d_cand_off.p,
+                                                     W.d_start.p, W.d_cnt.p, Dt.map.p, rows);
                 ctx->launches++;
             }
-            REC_CUDA(cudaGetLastError());
+            GB_CUDA(cudaGetLastError());
             e_cur ^= 1;
         }
-        rec_assemble_kernel<<<grid, NT, 0, st>>>(d_live.p, with_repl ? d_repl_off.p : nullptr, d_repl_items.p, u0, d_cand.p, d_cscore.p, d_cand_off.p,
-                                                 d_cnt.p, rows);
+        const int64_t *repl_off = with_repl ? W.d_repl_off.p : nullptr;
+        rec_assemble_kernel<<<grid, NT, 0, st>>>(W.d_live.p, repl_off, W.d_repl_items.p, u0, W.d_cand.p, W.d_cscore.p, W.d_cand_off.p, W.d_cnt.p, rows);
         ctx->launches++;
-        REC_CUDA(cudaGetLastError());
-        // the output buffers of this parity are free once the download of two chunks ago has finished
-        if (k >= 2) REC_CUDA(cudaStreamWaitEvent(st, reuse[p], 0));
-        const int32_t *res_items = d_cand.p;
-        const double *res_scores = d_cscore.p;
-        const int32_t *res_cnt = d_cnt.p;
+        GB_CUDA(cudaGetLastError());
+        if (k >= 2) GB_CUDA(cudaStreamWaitEvent(st, reuse[p].e, 0));
         if (m) {
-            rec_scan_kernel<<<1, 1024, 0, st>>>(d_cnt.p, rows, d_fm_off.p);
+            rec_scan_kernel<<<1, 1024, 0, st>>>(W.d_cnt.p, rows, W.d_fm_off.p);
             ctx->launches++;
             const int64_t *ch_off = nullptr;
             int64_t n_ch = 0;
@@ -1028,58 +844,87 @@ extern "C" int32_t gorse_b200_recommend(gorse_b200_ctx *ctx, int64_t n_users, co
                 for (int64_t r = 0; r < rows; r++)
                     h_ch_off[(size_t)r + 1] = h_ch_off[(size_t)r] + (bound[(size_t)(u0 + r)] + m->batch_size - 1) / m->batch_size;
                 n_ch = h_ch_off[(size_t)rows];
-                REC_TRY(d_ch_off.upload(h_ch_off.data(), h_ch_off.size(), st));
-                REC_TRY(m->ch_start.grow((size_t)std::max<int64_t>(n_ch, 1)));
-                REC_TRY(m->ch_rows.grow((size_t)std::max<int64_t>(n_ch, 1)));
-                ch_off = d_ch_off.p;
+                GB_TRY(W.d_ch_off.upload(h_ch_off.data(), h_ch_off.size(), st));
+                GB_TRY(m->ch_start.grow((size_t)std::max<int64_t>(n_ch, 1)));
+                GB_TRY(m->ch_rows.grow((size_t)std::max<int64_t>(n_ch, 1)));
+                ch_off = W.d_ch_off.p;
             }
             rec_pack_kernel<<<(unsigned)std::min<int64_t>((rows + 7) / 8, (int64_t)ctx->sm_count * 16), 256, 0, st>>>(
-                d_cand.p, d_cand_off.p, d_cnt.p, d_fm_off.p, d_u_len.p + u0, d_i_len.p, m->num_dimension, m->cand.p, d_dims.p, ch_off, m->batch_size,
-                m->ch_start.p, m->ch_rows.p, rows);
+                W.d_cand.p, W.d_cand_off.p, W.d_cnt.p, W.d_fm_off.p, W.d_u_len.p + u0, W.d_i_len.p, m->num_dimension, m->cand.p, W.d_dims.p, ch_off,
+                m->batch_size, m->ch_start.p, m->ch_rows.p, rows);
             ctx->launches++;
-            REC_CUDA(cudaGetLastError());
+            GB_CUDA(cudaGetLastError());
             const fm::Feats U{m->u_feat.p + u0, m->u_off.p + u0, m->u_idx.p, m->u_val.p};
             int64_t mb = 0;
             for (int64_t r = 0; r < rows; r++) mb = std::max(mb, bound[(size_t)(u0 + r)]);
             bool gs = false;
-            REC_TRY(fm::rank_pass(m, U, FI, d_fm_off.p, m->cand.p, d_dims.p, 0, rows, 0, FS, m->ch_start.p, m->ch_rows.p, 0, n_ch, mb, m->score.p,
-                                  m->order.p, &gs));
-            rec_emit_kernel<<<emit_grid, NT, 0, st>>>(m->cand.p, d_fm_off.p, m->score.p, m->order.p, with_repl ? d_repl_off.p : nullptr, d_repl_items.p,
-                                                 d_repl_pos.p, u0, positive_decay, read_decay, d_dscore.p, d_sort.p, sort_stride, d_cand_off.p,
-                                                 d_out_items[p].p, d_out_scores[p].p, d_out_cnt[p].p, rows);
+            GB_TRY(fm::rank_pass(m, U, FI, W.d_fm_off.p, m->cand.p, W.d_dims.p, 0, rows, 0, FS, m->ch_start.p, m->ch_rows.p, 0, n_ch, mb, m->score.p,
+                                 m->order.p, &gs));
+            rec_emit_kernel<<<emit_grid, NT, 0, st>>>(m->cand.p, W.d_fm_off.p, m->score.p, m->order.p, repl_off, W.d_repl_items.p, W.d_repl_pos.p, u0,
+                                                        positive_decay, read_decay, W.d_dscore.p, W.d_sort.p, sort_stride, W.d_cand_off.p,
+                                                        W.d_out_items[p].p, W.d_out_scores[p].p, W.d_out_cnt[p].p, rows);
             ctx->launches++;
-            REC_CUDA(cudaGetLastError());
-            res_items = d_out_items[p].p;
-            res_scores = d_out_scores[p].p;
-            res_cnt = d_out_cnt[p].p;
+            GB_CUDA(cudaGetLastError());
         } else {   // the merged candidates are the answer; copied so that the next chunk may reuse the work buffers
-            REC_CUDA(cudaMemcpyAsync(d_out_items[p].p, d_cand.p, sizeof(int32_t) * h_cand_off[(size_t)rows], cudaMemcpyDeviceToDevice, st));
-            REC_CUDA(cudaMemcpyAsync(d_out_scores[p].p, d_cscore.p, sizeof(double) * h_cand_off[(size_t)rows], cudaMemcpyDeviceToDevice, st));
-            REC_CUDA(cudaMemcpyAsync(d_out_cnt[p].p, d_cnt.p, sizeof(int32_t) * rows, cudaMemcpyDeviceToDevice, st));
-            res_items = d_out_items[p].p;
-            res_scores = d_out_scores[p].p;
-            res_cnt = d_out_cnt[p].p;
+            GB_CUDA(cudaMemcpyAsync(W.d_out_items[p].p, W.d_cand.p, sizeof(int32_t) * h_cand_off[(size_t)rows], cudaMemcpyDeviceToDevice, st));
+            GB_CUDA(cudaMemcpyAsync(W.d_out_scores[p].p, W.d_cscore.p, sizeof(double) * h_cand_off[(size_t)rows], cudaMemcpyDeviceToDevice, st));
+            GB_CUDA(cudaMemcpyAsync(W.d_out_cnt[p].p, W.d_cnt.p, sizeof(int32_t) * rows, cudaMemcpyDeviceToDevice, st));
         }
         const int64_t ob = out_at[(size_t)u0], on = h_cand_off[(size_t)rows];
-        REC_CUDA(cudaEventRecord(ctx->copy_ev, st));
-        REC_CUDA(cudaStreamWaitEvent(ctx->copy_stream, ctx->copy_ev, 0));
-        REC_CUDA(cudaMemcpyAsync(count_out + u0, res_cnt, sizeof(int32_t) * rows, cudaMemcpyDeviceToHost, ctx->copy_stream));
+        GB_CUDA(cudaEventRecord(ctx->copy_ev, st));
+        GB_CUDA(cudaStreamWaitEvent(ctx->copy_stream, ctx->copy_ev, 0));
+        GB_CUDA(cudaMemcpyAsync(count_out + u0, W.d_out_cnt[p].p, sizeof(int32_t) * rows, cudaMemcpyDeviceToHost, ctx->copy_stream));
         if (on) {
-            REC_CUDA(cudaMemcpyAsync(items_out + ob, res_items, sizeof(int32_t) * on, cudaMemcpyDeviceToHost, ctx->copy_stream));
-            REC_CUDA(cudaMemcpyAsync(scores_out + ob, res_scores, sizeof(double) * on, cudaMemcpyDeviceToHost, ctx->copy_stream));
+            GB_CUDA(cudaMemcpyAsync(items_out + ob, W.d_out_items[p].p, sizeof(int32_t) * on, cudaMemcpyDeviceToHost, ctx->copy_stream));
+            GB_CUDA(cudaMemcpyAsync(scores_out + ob, W.d_out_scores[p].p, sizeof(double) * on, cudaMemcpyDeviceToHost, ctx->copy_stream));
         }
-        REC_CUDA(cudaEventRecord(reuse[p], ctx->copy_stream));
+        GB_CUDA(cudaEventRecord(reuse[p].e, ctx->copy_stream));
+        return GORSE_B200_OK;
     }
-    REC_CUDA(cudaStreamSynchronize(st));
-    REC_CUDA(cudaStreamSynchronize(ctx->copy_stream));
+};
+
+}  // namespace rec
+}  // namespace gb
+
+using namespace gb;
+
+extern "C" int32_t gorse_b200_recommend(gorse_b200_ctx *ctx, int64_t n_users, const int64_t *excl_off, const int32_t *excl_items, int32_t n_items,
+                                        const uint8_t *item_live, int32_t n_stages, const gorse_b200_recommend_stage *stages,
+                                        const gorse_b200_recommend_cf *cf, const gorse_b200_recommend_ranker *ranker, const int64_t *repl_off,
+                                        const int32_t *repl_items, const uint8_t *repl_positive, double positive_decay, double read_decay,
+                                        int32_t *items_out, double *scores_out, int32_t *count_out, int64_t *stats_out)
+{
+    using namespace gb::rec;
+    GB_CHECK_ARG(n_users >= 0 && n_items >= 0 && n_stages >= 0, "negative count");
+    if (stats_out) std::fill(stats_out, stats_out + 4, 0);
+    if (n_users == 0) return GORSE_B200_OK;
+    Call C{ctx, n_users, excl_off, excl_items, n_items, item_live, n_stages, stages, cf, ranker, repl_off, repl_items, repl_positive,
+           positive_decay, read_decay, items_out, scores_out, count_out};
+    GB_TRY(C.check());
+    // the context last: every other argument is checked without it
+    GB_CHECK_ARG(ctx != nullptr, "ctx is NULL");
+    Work *Wp = work(ctx);
+    if (!Wp) { set_error("host allocation failed"); return GORSE_B200_ERR_OOM; }
+    Work &W = *Wp;
+    std::lock_guard<std::mutex> wlk(W.mu);
+    ScopedDevice sdev(ctx->device);
+    Event reuse[2];
+    StreamSync sync{ctx->stream, ctx->copy_stream};
+    GB_TRY(C.tables(W));
+    GB_TRY(C.recall_and_ranker(W));
+    GB_TRY(C.plan(W));
+    GB_TRY(reuse[0].create());
+    GB_TRY(reuse[1].create());
+    for (int64_t k = 0; k < C.n_chunks; k++) GB_TRY(C.run_chunk(W, k, reuse));
+    GB_CUDA(cudaStreamSynchronize(ctx->stream));
+    GB_CUDA(cudaStreamSynchronize(ctx->copy_stream));
+    int64_t ranked = 0;
     for (int64_t u = 0; u < n_users; u++) ranked += count_out[u];
     if (stats_out) {
-        stats_out[0] = n_chunks;
+        stats_out[0] = C.n_chunks;
         stats_out[1] = ranked;
-        stats_out[2] = total_rows;
-        stats_out[3] = exact_total;
+        stats_out[2] = C.total_rows;
+        stats_out[3] = C.exact_total;
     }
-#undef REC_TRY
-#undef REC_CUDA
-    return finish(GORSE_B200_OK);
+    return GORSE_B200_OK;
 }

@@ -138,4 +138,95 @@ int32_t aggregate(gorse_b200_ctx *c, const Route &R, const Users &U, const Neigh
                   bool euclid, int64_t NI, bool heavy, double *acc, int32_t *flag, int32_t *touched);
 }  // namespace u2u
 
+// -1 and deleted slots are skipped (GetVectors returns nothing, logics/item_to_item.go:56-58) and never count for a session;
+// hidden ones are queried
+template <typename Id>
+void NeighbourStage::prepare_items(gorse_b200_vecdb *d, int64_t n_users, const int64_t *ctx_off, const Id *ctx, const int64_t *slot_of_item,
+                                   int n_, int need_, int top_, double scale_, const uint8_t *item_ok_)
+{
+    start(d, false, n_, scale_, item_ok_, (int64_t)d->ts.size());
+    need = need_;
+    top = top_;
+    N = std::max<int64_t>((int64_t)d->ts.size(), 1);
+    std::vector<int32_t> row_of(d->ts.size(), -1);
+    c_off.assign((size_t)n_users + 1, 0);
+    c_row.reserve((size_t)ctx_off[n_users]);
+    for (int64_t u = 0; u < n_users; u++) {
+        for (int64_t t = ctx_off[u]; t < ctx_off[u + 1]; t++) {
+            const int64_t id = ctx[t];
+            const int32_t r = table_row(d, id < 0 || !slot_of_item ? id : slot_of_item[id], row_of, nb);
+            if (r >= 0) c_row.push_back(r);
+        }
+        c_off[(size_t)u + 1] = (int64_t)c_row.size();
+    }
+    heavy = i2i::route(c_off.data(), n_users, n, h_users) < n_users;
+}
+
+// -1 and deleted slots have no row (GetVectors returns nothing, logics/user_to_user.go:55-58); hidden ones are searched
+inline void NeighbourStage::prepare_users(gorse_b200_vecdb *d, int64_t n_users, const int64_t *user_slots, int64_t fb_rows_, const int64_t *fb_off_,
+                                          const int32_t *fb_items_, int32_t n_items, int n_, double scale_, const uint8_t *item_ok_)
+{
+    start(d, true, n_, scale_, item_ok_, n_items);
+    top = n_;
+    N = std::max<int64_t>(n_items, 1);
+    h_fb_off = fb_off_;
+    h_fb_items = fb_items_;
+    fb_rows = fb_rows_;
+    std::vector<int32_t> row_of(d->ts.size(), -1);
+    q_row.resize((size_t)n_users);
+    for (int64_t u = 0; u < n_users; u++) q_row[(size_t)u] = table_row(d, user_slots[u], row_of, nb);
+    // the most any user can add: n neighbours with the longest feedback row.  Below the table's limit no user needs a
+    // global row, so none is allocated.
+    int64_t longest = 0;
+    for (int64_t v = 0; v < fb_rows; v++) longest = std::max(longest, fb_off_[v + 1] - fb_off_[v]);
+    heavy = longest * std::max(n, 0) > agg::TABLE_KEYS;
+}
+
+// The collection entries after their checks and prepare: stage A, then the users in chunks of sm_count * 1024 against the
+// checked exclusion rows ex / ex_off, each finished chunk downloaded on the copy stream while the next one computes.
+// stats_out: the table's rows, those the exact scan answered, the users per accumulator.  The caller holds db->mu.
+int32_t neighbour_call(NeighbourStage &S, int64_t n_users, const int32_t *categories, int32_t n_categories, const std::vector<int64_t> &ex,
+                       const std::vector<int64_t> &ex_off, int64_t *ids_out, double *scores_out, int32_t *count_out, int64_t *stats_out);
+
+// The checks every neighbour stage makes of its collection at n: Cosine, n above the dense or sparse limit and 2^31 slots
+// or more are GORSE_B200_ERR_UNSUPPORTED.  In this and the checks below, `who` names the caller or stage in the message.
+inline int32_t check_stage_db(const gorse_b200_vecdb *db, int n, const char *who)
+{
+    if (db->distance == GORSE_B200_DISTANCE_COSINE) {
+        set_error("%s: item-to-item, session and user-to-user collections are Dot or Euclidean", who);
+        return GORSE_B200_ERR_UNSUPPORTED;
+    }
+    const bool sparse = db->dim == 0;
+    if (n > (sparse ? MAX_N_SPARSE : MAX_N_DENSE)) {
+        set_error("%s: n = %d above %d for a %s collection", who, n, sparse ? MAX_N_SPARSE : MAX_N_DENSE, sparse ? "sparse" : "dense");
+        return GORSE_B200_ERR_UNSUPPORTED;
+    }
+    if ((int64_t)db->ts.size() > INT32_MAX) {
+        set_error("%s: more than 2^31 slots", who);
+        return GORSE_B200_ERR_UNSUPPORTED;
+    }
+    return GORSE_B200_OK;
+}
+
+// off[0, rows] of a CSR named `what`: off[0] == 0 and non-decreasing
+inline int32_t check_offsets(const int64_t *off, int64_t rows, const char *who, const char *what)
+{
+    GB_CHECK_ARG(off[0] == 0, "%s: %s[0] must be 0", who, what);
+    for (int64_t r = 0; r < rows; r++) GB_CHECK_ARG(off[r + 1] >= off[r], "%s: %s decreases at %lld", who, what, (long long)r);
+    return GORSE_B200_OK;
+}
+
+// a feedback CSR of rows rows whose entries are items of [0, n_items)
+inline int32_t check_feedback(const char *who, int64_t rows, const int64_t *fb_off, const int32_t *fb_items, int32_t n_items)
+{
+    GB_CHECK_ARG(rows >= 0 && (rows == 0 || fb_off != nullptr), "%s: fb_off is NULL or n_fb_rows < 0", who);
+    if (rows == 0) return GORSE_B200_OK;
+    GB_TRY(check_offsets(fb_off, rows, who, "fb_off"));
+    GB_CHECK_ARG(fb_off[rows] == 0 || fb_items != nullptr, "%s: fb_items is NULL", who);
+    for (int64_t t = 0; t < fb_off[rows]; t++)
+        GB_CHECK_ARG(fb_items[t] >= 0 && fb_items[t] < n_items, "%s: feedback entry %lld: item %d is not in [0, %d)", who, (long long)t, fb_items[t],
+                     n_items);
+    return GORSE_B200_OK;
+}
+
 }  // namespace gb

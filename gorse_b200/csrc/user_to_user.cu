@@ -177,147 +177,28 @@ extern "C" int32_t gorse_b200_vecdb_user_to_user(gorse_b200_vecdb *db, int64_t n
                                                  const int64_t *excl_off, const int64_t *excl_items, int32_t n, double score_scale,
                                                  int64_t *items_out, double *scores_out, int32_t *count_out, int64_t *stats_out)
 {
-    using namespace gb::u2u;
     GB_CHECK_ARG(db != nullptr, "collection is NULL");
     GB_CHECK_ARG(n_users >= 0 && n_fb_rows >= 0 && n_items >= 0, "negative count");
     if (stats_out) std::fill(stats_out, stats_out + 4, 0);
     if (n_users == 0) return GORSE_B200_OK;
     GB_CHECK_ARG(count_out != nullptr && user_slots != nullptr && excl_off != nullptr, "count_out / user_slots / excl_off is NULL");
-    GB_CHECK_ARG(n_fb_rows == 0 || fb_off != nullptr, "fb_off is NULL");
-    GB_CHECK_ARG(excl_off[0] == 0 && (n_fb_rows == 0 || fb_off[0] == 0), "fb_off[0] and excl_off[0] must be 0");
-    for (int64_t u = 0; u < n_users; u++)
-        GB_CHECK_ARG(excl_off[u + 1] >= excl_off[u], "excl_off not non-decreasing at %lld", (long long)u);
-    for (int64_t v = 0; v < n_fb_rows; v++)
-        GB_CHECK_ARG(fb_off[v + 1] >= fb_off[v], "fb_off not non-decreasing at %lld", (long long)v);
-    const int64_t n_fb = n_fb_rows ? fb_off[n_fb_rows] : 0;
-    GB_CHECK_ARG(n_fb == 0 || fb_items != nullptr, "fb_items is NULL");
+    GB_TRY(check_offsets(excl_off, n_users, "user_to_user", "excl_off"));
     GB_CHECK_ARG(excl_off[n_users] == 0 || excl_items != nullptr, "excl_items is NULL");
-    for (int64_t t = 0; t < n_fb; t++)
-        GB_CHECK_ARG(fb_items[t] >= 0 && fb_items[t] < n_items, "feedback entry %lld: item %d is not in [0, %d)", (long long)t, fb_items[t], n_items);
+    GB_TRY(check_feedback("user_to_user", n_fb_rows, fb_off, fb_items, n_items));
     GB_CHECK_ARG(score_scale == score_scale, "score_scale is NaN");
-    if (db->distance == GORSE_B200_DISTANCE_COSINE) {
-        set_error("user-to-user collections are Dot or Euclidean");
-        return GORSE_B200_ERR_UNSUPPORTED;
-    }
+    std::lock_guard<std::mutex> lk(db->mu);
+    GB_TRY(check_stage_db(db, n, "user_to_user"));
     if (n <= 0) {
-        for (int64_t u = 0; u < n_users; u++) count_out[u] = 0;
+        std::fill(count_out, count_out + n_users, 0);
         return GORSE_B200_OK;
     }
-    const bool sparse = db->dim == 0;
-    if (n > (sparse ? MAX_N_SPARSE : MAX_N_DENSE)) {
-        set_error("user_to_user: n = %d above %d for a %s collection", n, sparse ? MAX_N_SPARSE : MAX_N_DENSE, sparse ? "sparse" : "dense");
-        return GORSE_B200_ERR_UNSUPPORTED;
-    }
     GB_CHECK_ARG(items_out != nullptr && scores_out != nullptr, "NULL output");
-    std::lock_guard<std::mutex> lk(db->mu);
     const int64_t n_slots = (int64_t)db->ts.size();
-    if (n_slots > INT32_MAX) { set_error("user_to_user: more than 2^31 slots"); return GORSE_B200_ERR_UNSUPPORTED; }
     for (int64_t u = 0; u < n_users; u++)
         GB_CHECK_ARG(user_slots[u] >= -1 && user_slots[u] < n_slots, "user %lld: slot %lld is not a slot of the collection", (long long)u,
                      (long long)user_slots[u]);
     std::vector<int64_t> ex, ex_off;
     GB_TRY(exclusion_rows(n_users, excl_off, excl_items, n_items, "user", "item", ex, ex_off));
-    // the live query slots as rows of the neighbour table.  -1 and deleted slots have no row (GetVectors returns nothing,
-    // logics/user_to_user.go:55-58); hidden ones are searched.
-    std::vector<int32_t> row_of((size_t)n_slots, -1), q_row((size_t)n_users);
-    std::vector<int64_t> nb;
-    for (int64_t u = 0; u < n_users; u++) q_row[(size_t)u] = table_row(db, user_slots[u], row_of, nb);
-    const int64_t R = (int64_t)nb.size();
-    if (R == 0) {
-        for (int64_t u = 0; u < n_users; u++) count_out[u] = 0;
-        return GORSE_B200_OK;
-    }
-    // the most any user can add: n neighbours with the longest feedback row.  Below the table's limit no user needs a
-    // global row, so none is allocated.
-    int64_t longest = 0;
-    for (int64_t v = 0; v < n_fb_rows; v++) longest = std::max(longest, fb_off[v + 1] - fb_off[v]);
-    const bool heavy_possible = longest * n > TABLE_KEYS;
-
-    gorse_b200_ctx *c = db->ctx;
-    ScopedDevice sd(c->device);
-    UserToUserWork &V = db->u2u;
-    int32_t st = GORSE_B200_OK;
-    auto done = [&](int32_t s) {
-        cudaStreamSynchronize(c->stream);
-        cudaStreamSynchronize(c->copy_stream);
-        return s;
-    };
-    if ((st = V.nb.grow((size_t)R)) || (st = V.t_slot.grow((size_t)R * n)) || (st = V.t_score.grow((size_t)R * n)) || (st = V.t_cnt.grow((size_t)R)))
-        return done(st);
-
-    // ---- stage A: the neighbour table
-    int64_t exact_rows = 0;
-    if ((st = neighbour_table(db, nb, V.nb.p, n, nullptr, 0, V.t_slot.p, V.t_score.p, V.t_cnt.p, &exact_rows))) return done(st);
-    cudaError_t e;
-    if ((e = cudaGetLastError()) != cudaSuccess) { set_error("user_to_user: %s", cudaGetErrorString(e)); return done(GORSE_B200_ERR_CUDA); }
-
-    // ---- the feedback rows and the item filter, once per call
-    const int64_t cu = std::min<int64_t>(n_users, (int64_t)c->sm_count * 1024);
-    const int64_t n_chunks = (n_users + cu - 1) / cu;
-    if ((st = V.fb_off.grow((size_t)n_fb_rows + 1)) || (st = V.fb_items.grow((size_t)std::max<int64_t>(n_fb, 1))) ||
-        (st = V.item_ok.grow((size_t)std::max<int32_t>(n_items, 1))) || (st = V.q_row.grow((size_t)cu)) ||
-        (st = V.ex_off.grow((size_t)cu + 1)) || (st = V.ex.grow(std::max<size_t>(ex.size(), 1))) || (st = V.list.grow((size_t)cu)) ||
-        (st = V.work.grow((size_t)cu)) || (st = V.route_cnt.grow((size_t)n_chunks * 2)) || (st = V.items.grow((size_t)n_users * n)) ||
-        (st = V.scores.grow((size_t)n_users * n)) || (st = V.count.grow((size_t)n_users)))
-        return done(st);
-    if ((n_fb_rows && (e = cudaMemcpyAsync(V.fb_off.p, fb_off, sizeof(int64_t) * (n_fb_rows + 1), cudaMemcpyHostToDevice, c->stream)) != cudaSuccess) ||
-        (n_fb && (e = cudaMemcpyAsync(V.fb_items.p, fb_items, sizeof(int32_t) * n_fb, cudaMemcpyHostToDevice, c->stream)) != cudaSuccess) ||
-        (item_ok && n_items && (e = cudaMemcpyAsync(V.item_ok.p, item_ok, n_items, cudaMemcpyHostToDevice, c->stream)) != cudaSuccess) ||
-        (e = cudaMemsetAsync(V.route_cnt.p, 0, sizeof(int32_t) * n_chunks * 2, c->stream)) != cudaSuccess) {
-        set_error("user_to_user upload: %s", cudaGetErrorString(e));
-        return done(GORSE_B200_ERR_CUDA);
-    }
-
-    // ---- routing and stage B: users in chunks; a finished chunk is downloaded on the copy stream while the next one computes
-    // global accumulators: one [n_items] float64 row, flag row and item list per CTA, at most 512 MB
-    const int64_t NI = std::max<int64_t>(n_items, 1);
-    const int hg = heavy_grid(c, NI, ROW_BYTES);
-    if (heavy_possible && ((st = V.acc.grow_zeroed((size_t)hg * NI, c->stream)) || (st = V.flag.grow_zeroed((size_t)hg * NI, c->stream)) ||
-                           (st = V.touched.grow((size_t)hg * NI))))
-        return done(st);
-    const NeighbourTable T{V.t_slot.p, V.t_score.p, V.t_cnt.p};
-    Feedback F;
-    F.off = V.fb_off.p; F.items = V.fb_items.p; F.rows = n_fb_rows;
-    const bool euclid = db->distance == GORSE_B200_DISTANCE_EUCLIDEAN;
-    std::vector<int64_t> h_exoff;
-    for (int64_t ci = 0, u0 = 0; u0 < n_users; ci++, u0 += cu) {
-        const int64_t rows = std::min(cu, n_users - u0);
-        h_exoff.resize(rows + 1);
-        for (int64_t r = 0; r <= rows; r++) h_exoff[r] = ex_off[u0 + r] - ex_off[u0];
-        const int64_t n_e = h_exoff[rows];
-        if ((e = cudaMemcpyAsync(V.q_row.p, q_row.data() + u0, sizeof(int32_t) * rows, cudaMemcpyHostToDevice, c->stream)) != cudaSuccess ||
-            (e = cudaMemcpyAsync(V.ex_off.p, h_exoff.data(), sizeof(int64_t) * (rows + 1), cudaMemcpyHostToDevice, c->stream)) != cudaSuccess ||
-            (n_e && (e = cudaMemcpyAsync(V.ex.p + ex_off[u0], ex.data() + ex_off[u0], sizeof(int64_t) * n_e, cudaMemcpyHostToDevice, c->stream)) != cudaSuccess)) {
-            set_error("user_to_user upload: %s", cudaGetErrorString(e));
-            return done(GORSE_B200_ERR_CUDA);
-        }
-        Users U;
-        U.q_row = V.q_row.p; U.ex_off = V.ex_off.p; U.ex = V.ex.p + ex_off[u0]; U.item_ok = item_ok ? V.item_ok.p : nullptr;
-        U.items = V.items.p + u0 * n; U.scores = V.scores.p + u0 * n; U.count = V.count.p + u0;
-        Route Rt;
-        Rt.list = V.list.p; Rt.cnt = V.route_cnt.p + 2 * ci; Rt.work = V.work.p; Rt.users = rows;
-        if ((st = aggregate(c, Rt, U, T, F, n, score_scale, euclid, NI, heavy_possible, V.acc.p, V.flag.p, V.touched.p))) return done(st);
-        if ((e = cudaEventRecord(c->copy_ev, c->stream)) != cudaSuccess || (e = cudaStreamWaitEvent(c->copy_stream, c->copy_ev, 0)) != cudaSuccess ||
-            (e = cudaMemcpyAsync(count_out + u0, V.count.p + u0, sizeof(int32_t) * rows, cudaMemcpyDeviceToHost, c->copy_stream)) != cudaSuccess ||
-            (e = cudaMemcpyAsync(items_out + u0 * n, V.items.p + u0 * n, sizeof(int64_t) * rows * n, cudaMemcpyDeviceToHost, c->copy_stream)) != cudaSuccess ||
-            (e = cudaMemcpyAsync(scores_out + u0 * n, V.scores.p + u0 * n, sizeof(double) * rows * n, cudaMemcpyDeviceToHost, c->copy_stream)) != cudaSuccess) {
-            set_error("user_to_user download: %s", cudaGetErrorString(e));
-            return done(GORSE_B200_ERR_CUDA);
-        }
-    }
-    std::vector<int32_t> routed((size_t)n_chunks * 2);
-    if ((e = cudaMemcpyAsync(routed.data(), V.route_cnt.p, sizeof(int32_t) * n_chunks * 2, cudaMemcpyDeviceToHost, c->stream)) != cudaSuccess ||
-        (e = cudaStreamSynchronize(c->stream)) != cudaSuccess || (e = cudaStreamSynchronize(c->copy_stream)) != cudaSuccess) {
-        set_error("user_to_user: %s", cudaGetErrorString(e));
-        return done(GORSE_B200_ERR_CUDA);
-    }
-    if (stats_out) {
-        stats_out[0] = R;
-        stats_out[1] = exact_rows;
-        for (int64_t ci = 0; ci < n_chunks; ci++) {
-            stats_out[2] += routed[(size_t)ci * 2];
-            stats_out[3] += routed[(size_t)ci * 2 + 1];
-        }
-    }
-    return done(GORSE_B200_OK);
+    db->stage.prepare_users(db, n_users, user_slots, n_fb_rows, fb_off, fb_items, n_items, n, score_scale, item_ok);
+    return neighbour_call(db->stage, n_users, nullptr, 0, ex, ex_off, items_out, scores_out, count_out, stats_out);
 }

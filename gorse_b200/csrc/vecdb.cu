@@ -62,7 +62,7 @@ __global__ void vecdb_live_kernel(const uint8_t *dead, int64_t n, int64_t *flag)
 static int64_t vecdb_bytes(const gorse_b200_vecdb *db)
 {
     return (int64_t)(db->d_blocked.bytes() + db->d_allow.bytes() + db->d_cat_off.bytes() + db->d_cats.bytes() + db->d_want.bytes() +
-                     db->i2i.bytes() + db->u2u.bytes() + db->ncache.bytes() + (db->dense ? index_bytes(db->dense) : sparse_bytes(db->sparse)));
+                     db->stage.bytes() + db->ncache.bytes() + (db->dense ? index_bytes(db->dense) : sparse_bytes(db->sparse)));
 }
 
 static int32_t sync_meta(gorse_b200_vecdb *db)
@@ -377,8 +377,7 @@ int32_t gorse_b200_vecdb_compact(gorse_b200_vecdb *db, int64_t *new_slot_out, in
     db->gen++;
     // every device buffer whose size follows the slot count; the next call that needs one allocates (and zeroes) it again
     db->d_blocked.free(); db->d_allow.free(); db->d_cat_off.free(); db->d_cats.free();
-    db->i2i.acc.free(); db->i2i.seen.free(); db->i2i.touched.free(); db->i2i.item_ok.free();
-    db->u2u.acc.free(); db->u2u.flag.free(); db->u2u.touched.free();
+    db->stage.acc.free(); db->stage.seen.free(); db->stage.uacc.free(); db->stage.flag.free(); db->stage.touched.free(); db->stage.item_ok.free();
     if (new_slot_out)   // `dead` holds the old flags after the swap
         for (int64_t s = 0; s < n; s++) new_slot_out[s] = dead[(size_t)s] ? -1 : new_slot[(size_t)s];
     if (bytes_out) bytes_out[1] = vecdb_bytes(db);

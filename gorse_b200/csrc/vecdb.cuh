@@ -4,37 +4,88 @@
 #include "topk.cuh"
 
 namespace gb {
-// grow-only work buffers of gorse_b200_vecdb_item_to_item and gorse_b200_vecdb_session_recommend (item_to_item.cu),
-// which both hold the collection's lock: the neighbour table of stage A, the user or session batches, answers
-// and accumulator scratch of stage B, and the session call's item mask
-struct ItemToItemWork {
-    DevBuf<int64_t> nb, c_off, ex_off, ex, slots;
-    DevBuf<int32_t> t_slot, t_cnt, c_row, users, count;
-    DevBuf<float> t_score;
-    DevBuf<double> scores, acc;
-    DevBuf<uint8_t> seen, item_ok;
-    DevBuf<int32_t> touched;
-    size_t bytes() const
-    {
-        return nb.bytes() + c_off.bytes() + ex_off.bytes() + ex.bytes() + slots.bytes() + t_slot.bytes() + t_cnt.bytes() + c_row.bytes() +
-               users.bytes() + count.bytes() + t_score.bytes() + scores.bytes() + acc.bytes() + seen.bytes() + item_ok.bytes() + touched.bytes();
-    }
-};
+// One item-to-item or user-to-user stage over a collection: a batch's table rows on the host, and the grow-only device
+// buffers of stage A and stage B.  The collection keeps one for its entries (db->stage, under db->mu), gorse_b200_recommend
+// one per stage (rec::Work).  A call runs prepare_items or prepare_users, table, reserve, then run_chunk per chunk of users.
+struct NeighbourStage {
+    gorse_b200_vecdb *db = nullptr;
+    bool users = false;                      // user-to-user; else item-to-item (session: need > 0)
+    int n = 0, need = 0, top = 0;            // top: the answer row length (user-to-user: n)
+    double scale = 1.0;
+    int64_t N = 0;                           // the length of a global accumulator row: slots, or items (at least 1)
+    bool heavy = false;                      // some user may need a global accumulator row
+    int64_t n_shared = 0;                    // item-to-item: the users run_chunk routed to the shared-memory table
+    std::vector<int64_t> nb;                 // the distinct query slots, as the table's rows
+    std::vector<int64_t> c_off;              // item-to-item: [users + 1] into c_row
+    std::vector<int32_t> c_row;              // item-to-item: the table row of each live context entry, in order
+    std::vector<int32_t> q_row;              // user-to-user: [users] the table row of each user, -1 = no vector
+    const uint8_t *h_item_ok = nullptr;      // the caller's item mask (session: slots; user-to-user: items) or NULL
+    int64_t item_ok_len = 0;
+    const int64_t *h_fb_off = nullptr;       // user-to-user: the caller's feedback CSR
+    const int32_t *h_fb_items = nullptr;
+    int64_t fb_rows = 0;
+    std::vector<int32_t> h_users;            // item-to-item: one chunk's routing
 
-// grow-only work buffers of gorse_b200_vecdb_user_to_user (user_to_user.cu): the neighbour table of stage A, the caller's
-// feedback rows and item filter, the user chunks, their routing and answers, and the global-row accumulators of stage B
-struct UserToUserWork {
-    DevBuf<int64_t> nb, fb_off, ex_off, ex, items;
-    DevBuf<int32_t> t_slot, t_cnt, fb_items, q_row, list, work, route_cnt, count, flag, touched;
-    DevBuf<uint8_t> item_ok;
+    DevBuf<int64_t> d_nb, fb_off, d_c_off, ex_off, ex, ids;
+    DevBuf<int32_t> t_slot, t_cnt, row, fb_items, list, work, route, count, flag, touched;
     DevBuf<float> t_score;
-    DevBuf<double> scores, acc;
+    DevBuf<uint8_t> item_ok, seen;
+    // the global rows: item-to-item leaves acc dirty (seen is zero between users), user-to-user's uacc must be zero
+    // between users (its kernel adds into it), so the two are kept apart
+    DevBuf<double> scores, acc, uacc;
+    // gorse_b200_recommend's item-to-item stage, whose exclude sets hold items: slot_of_item and item_of_slot on the
+    // device, and the exclude set in slots (E0 on the host and the device, and two copies that take turns)
+    std::vector<int64_t> es0, es0_off;
+    DevBuf<int64_t> map, d_es0, d_es0_off, es[2];
+    DevBuf<int32_t> item_of_slot;
+
     size_t bytes() const
     {
-        return nb.bytes() + fb_off.bytes() + ex_off.bytes() + ex.bytes() + items.bytes() + t_slot.bytes() + t_cnt.bytes() + fb_items.bytes() +
-               q_row.bytes() + list.bytes() + work.bytes() + route_cnt.bytes() + count.bytes() + flag.bytes() + touched.bytes() +
-               item_ok.bytes() + t_score.bytes() + scores.bytes() + acc.bytes();
+        size_t b = 0;
+        for (const auto *x : {&d_nb, &fb_off, &d_c_off, &ex_off, &ex, &ids, &map, &d_es0, &d_es0_off, &es[0], &es[1]}) b += x->bytes();
+        for (const auto *x : {&t_slot, &t_cnt, &row, &fb_items, &list, &work, &route, &count, &flag, &touched, &item_of_slot}) b += x->bytes();
+        for (const auto *x : {&scores, &acc, &uacc}) b += x->bytes();
+        return b + t_score.bytes() + item_ok.bytes() + seen.bytes();
     }
+
+    // item-to-item: the live context entries ctx[ctx_off[u], ctx_off[u + 1]) of each user as table rows, the entries being
+    // slots, or items through slot_of_item when it is given.  item_ok: a slot mask or NULL; need > 0: session
+    // (i2i::aggregate).  stages.cuh.
+    template <typename Id>
+    void prepare_items(gorse_b200_vecdb *d, int64_t n_users, const int64_t *ctx_off, const Id *ctx, const int64_t *slot_of_item, int n_,
+                       int need_, int top_, double scale_, const uint8_t *item_ok_);
+    // user-to-user: the live query slot of each user as a table row, and the caller's feedback rows (slots at or beyond
+    // fb_rows have none).  item_ok: an item mask or NULL.  stages.cuh.
+    void prepare_users(gorse_b200_vecdb *d, int64_t n_users, const int64_t *user_slots, int64_t fb_rows_, const int64_t *fb_off_,
+                       const int32_t *fb_items_, int32_t n_items, int n_, double scale_, const uint8_t *item_ok_);
+    // the inputs of stage B (table rows, feedback, item mask), then stage A (neighbour_table) when the batch has rows.
+    // categories: the neighbour query's filter (item-to-item only).  The caller holds db->mu.
+    int32_t table(const int32_t *categories, int32_t n_categories, int64_t *exact_rows);
+    // the chunk buffers for chunks of at most max_rows users, n_chunks of them, and the global rows when heavy
+    int32_t reserve(int64_t max_rows, int64_t n_chunks);
+    // stage B of chunk k, the users [u0, u0 + rows), against their exclusion rows ex_off [rows + 1] / ex on the device
+    // (ascending per user; slots for item-to-item, items for user-to-user); answer row u of the chunk at ids / scores +
+    // u * top, its length in count[u]
+    int32_t run_chunk(int64_t k, int64_t u0, int64_t rows, const int64_t *ex_off, const int64_t *ex, int64_t *ids, double *scores,
+                      int32_t *count);
+
+private:
+    void start(gorse_b200_vecdb *d, bool users_, int n_, double scale_, const uint8_t *item_ok_, int64_t item_ok_len_)
+    {
+        db = d;
+        users = users_;
+        n = n_;
+        scale = scale_;
+        h_item_ok = item_ok_;
+        item_ok_len = item_ok_len_;
+        heavy = false;
+        n_shared = 0;
+        h_fb_off = nullptr;
+        h_fb_items = nullptr;
+        fb_rows = 0;
+        nb.clear(); c_off.clear(); c_row.clear(); q_row.clear(); es0.clear(); es0_off.clear();
+    }
+
 };
 
 // gorse_b200_vecdb_neighbour_cache: the first n neighbours of up to `cap` stored vectors, as stage A (neighbour_table,
@@ -73,8 +124,7 @@ struct gorse_b200_vecdb {
     gb::DevBuf<uint8_t> d_blocked, d_allow;   // blocked = hidden | dead
     gb::DevBuf<int64_t> d_cat_off;
     gb::DevBuf<int32_t> d_cats, d_want;
-    gb::ItemToItemWork i2i;  // batched item-to-item and session recommendation (item_to_item.cu)
-    gb::UserToUserWork u2u;  // batched user-to-user recommendation (user_to_user.cu)
+    gb::NeighbourStage stage;   // item-to-item, session and user-to-user recommendation (item_to_item.cu, user_to_user.cu)
     gb::NeighbourCache ncache;   // stage A's rows kept between calls (gorse_b200_vecdb_neighbour_cache, item_to_item.cu)
 };
 

@@ -27,8 +27,8 @@ def dense_chunk(sm_count):
 
 
 def user_chunk(sm_count):
-    """users of one stage-B chunk: item-to-item and session (item_to_item.cu: cu = sm_count * 1024), user-to-user
-    (user_to_user.cu: cu = sm_count * 1024) and gorse_b200_recommend (recommend.cu: at most sm_count * 1024 users)"""
+    """users of one stage-B chunk: item-to-item, session and user-to-user (neighbour_call in item_to_item.cu:
+    cu = sm_count * 1024) and gorse_b200_recommend (plan in recommend.cu: at most sm_count * 1024 users)"""
     return sm_count * 1024
 
 
