@@ -65,7 +65,7 @@ const b200NeighbourCacheMB = 1024
 
 func init() {
 	Register([]string{b200Prefix}, func(path, tablePrefix string, opts ...storage.Option) (Database, error) {
-		// b200://<device>[/<root>][?neighbour_cache_mb=<MB>]
+		// b200://<device>[/<root>][?neighbour_cache_mb=<MB>&neighbour_fill_n=<n>]
 		path, query, _ := strings.Cut(path, "?")
 		dev, root, _ := strings.Cut(strings.TrimPrefix(path, b200Prefix), "/")
 		device, err := strconv.Atoi(dev)
@@ -89,7 +89,17 @@ func init() {
 			}
 			cacheMB = mb
 		}
-		return &B200{device: device, tablePrefix: tablePrefix, root: root, cacheMB: cacheMB, collections: map[string]*b200Collection{}}, nil
+		fillN := 0
+		if q.Has("neighbour_fill_n") {
+			n, err := strconv.Atoi(q.Get("neighbour_fill_n"))
+			if err != nil || n < 0 || n > 1024 {
+				return nil, errors.Errorf("b200 store URL: neighbour_fill_n = %q is not an n in [0, 1024] (0 turns the fill off)",
+					q.Get("neighbour_fill_n"))
+			}
+			fillN = n
+		}
+		return &B200{device: device, tablePrefix: tablePrefix, root: root, cacheMB: cacheMB, fillN: fillN,
+			collections: map[string]*b200Collection{}}, nil
 	})
 }
 
@@ -107,6 +117,8 @@ type b200Collection struct {
 	file       os.FileInfo
 	dirty      bool
 	lastWrite  time.Time
+	// the neighbour lists saved with this generation (<file>.nbr) are loaded at most once into this handle
+	nbrOnce sync.Once
 }
 
 // B200 implements Database on one GPU.
@@ -116,6 +128,7 @@ type B200 struct {
 	tablePrefix string
 	root        string // "" = nothing is kept on disk
 	cacheMB     int64  // neighbour cache budget per collection, MB (0 = off)
+	fillN       int    // with a root: the n at which the writing process fills and saves neighbour lists (0 = off)
 	ctx         *C.gorse_b200_ctx
 	collections map[string]*b200Collection
 	stop        chan struct{}
@@ -308,6 +321,9 @@ func (db *B200) DeleteCollection(ctx context.Context, name string) error {
 	delete(db.collections, name)
 	if db.root != "" {
 		if err := os.Remove(db.path(name)); err != nil && !os.IsNotExist(err) {
+			return errors.Trace(err)
+		}
+		if err := os.Remove(db.path(name) + b200NbrSuffix); err != nil && !os.IsNotExist(err) {
 			return errors.Trace(err)
 		}
 	}
@@ -905,6 +921,16 @@ func (db *B200) NeighbourCache(name string, n int) error {
 	if err != nil {
 		return err
 	}
+	if err := db.sizeNeighbourCache(c, n); err != nil {
+		return err
+	}
+	c.nbrOnce.Do(func() { db.loadNeighbours(name, c, n) })
+	return nil
+}
+
+// sizeNeighbourCache turns on c's neighbour cache at n with min(live vectors, neighbour_cache_mb MB / (8 n + 4)) rows; the
+// same n and size again keep what it holds
+func (db *B200) sizeNeighbourCache(c *b200Collection, n int) error {
 	rows := min(int64(len(c.slotOf)), (db.cacheMB<<20)/(8*int64(n)+4))
 	st := C.gorse_b200_vecdb_neighbour_cache(c.handle, C.int32_t(n), C.int64_t(rows))
 	if st == C.GORSE_B200_ERR_UNSUPPORTED { // a Cosine collection, or n above 128 for a sparse one
@@ -1138,6 +1164,9 @@ func (db *B200) save(name string, c *b200Collection) error {
 	if err := f.Close(); err != nil {
 		return errors.Trace(err)
 	}
+	// the lists of this generation are in place before the collection file is: a reader that reloads the new file finds
+	// them at once
+	db.saveNeighbours(name, c, generation)
 	if err := os.Rename(path+".tmp", path); err != nil {
 		return errors.Trace(err)
 	}
@@ -1147,6 +1176,130 @@ func (db *B200) save(name string, c *b200Collection) error {
 	}
 	c.generation, c.file, c.dirty = generation, st2, false
 	return nil
+}
+
+// ---- neighbour lists on disk (neighbour_fill_n in the URL) ----
+//
+// File <root>/<tablePrefix><name>.b200vec.nbr: magic "GB200NBS", u32 version 1, i64 generation (the collection file's),
+// i32 n, then the library's neighbour stream (gorse_b200_vecdb_neighbour_cache_save; format in include/gorse_b200.h).  The
+// process that writes an item-to-item or user-to-user collection fills its neighbour cache at neighbour_fill_n and renames
+// this file into place before the collection file of the same generation, so a reader that loads the new collection file
+// finds the lists already there; every process that loads the collection loads the lists when the generation matches, so
+// its first batches and sessions start warm.  The library refuses lists of another collection itself (their
+// fingerprint).  Lists only save work: every failure is logged and the process goes on cold.
+
+const b200NbrSuffix = ".nbr"
+
+var b200NbrMagic = [8]byte{'G', 'B', '2', '0', '0', 'N', 'B', 'S'}
+
+func b200FillsNeighbours(name string) bool {
+	return strings.HasPrefix(name, ItemToItemPrefix+"_") || strings.HasPrefix(name, UserToUserPrefix+"_")
+}
+
+// saveNeighbours fills c's neighbour cache at neighbour_fill_n and writes <file>.nbr (tmp, fsync, rename) with the
+// generation of the collection file being saved; the caller holds db.mu for writing and renames the collection file into
+// place afterwards.  A process whose cache was off (the master, which never reads the lists) turns it off again, so the
+// pool does not stay on its device.
+func (db *B200) saveNeighbours(name string, c *b200Collection, generation int64) {
+	if db.fillN == 0 || db.cacheMB == 0 || !b200FillsNeighbours(name) {
+		return
+	}
+	stats := make([]int64, 7)
+	if err := b200Err(C.gorse_b200_vecdb_neighbour_cache_stats(c.handle, i64p(stats))); err != nil {
+		log.Logger().Warn("save neighbour lists; readers start cold", zap.String("collection", name), zap.Error(err))
+		return
+	}
+	if err := db.writeNeighbours(name, c, generation); err != nil {
+		log.Logger().Warn("save neighbour lists; readers start cold", zap.String("collection", name), zap.Error(err))
+	}
+	if stats[1] == 0 { // the capacity before the fill: off
+		if err := b200Err(C.gorse_b200_vecdb_neighbour_cache(c.handle, C.int32_t(db.fillN), 0)); err != nil {
+			log.Logger().Warn("turn the neighbour cache off after saving it", zap.String("collection", name), zap.Error(err))
+		}
+	}
+}
+
+func (db *B200) writeNeighbours(name string, c *b200Collection, generation int64) error {
+	if err := db.sizeNeighbourCache(c, db.fillN); err != nil {
+		return err
+	}
+	if err := b200Err(C.gorse_b200_vecdb_neighbour_cache_fill(c.handle, nil)); err != nil {
+		return err
+	}
+	path := db.path(name) + b200NbrSuffix
+	f, err := os.Create(path + ".tmp")
+	if err != nil {
+		return errors.Trace(err)
+	}
+	defer os.Remove(path + ".tmp")
+	le := binary.LittleEndian
+	head := le.AppendUint32(append([]byte{}, b200NbrMagic[:]...), 1)
+	head = le.AppendUint64(head, uint64(generation))
+	head = le.AppendUint32(head, uint32(int32(db.fillN)))
+	w := bufio.NewWriterSize(f, 1<<20)
+	if _, err := w.Write(head); err != nil {
+		f.Close()
+		return errors.Trace(err)
+	}
+	h := cgo.NewHandle(io.Writer(w))
+	st := C.gorse_b200_vecdb_neighbour_cache_save(c.handle, C.gorse_b200_snapshot_write_ptr(), unsafe.Pointer(&h), nil)
+	h.Delete()
+	if err := b200Err(st); err != nil {
+		f.Close()
+		return err
+	}
+	if err := w.Flush(); err != nil {
+		f.Close()
+		return errors.Trace(err)
+	}
+	if err := f.Sync(); err != nil {
+		f.Close()
+		return errors.Trace(err)
+	}
+	if err := f.Close(); err != nil {
+		return errors.Trace(err)
+	}
+	return errors.Trace(os.Rename(path+".tmp", path))
+}
+
+// loadNeighbours loads <file>.nbr into c's neighbour cache when it carries c's generation and, with n > 0, lists of n
+// neighbours (n = 0: the file's n).  A missing file, another generation or n, and every failure leave c cold.
+func (db *B200) loadNeighbours(name string, c *b200Collection, n int) {
+	if db.root == "" || db.cacheMB == 0 || !b200FillsNeighbours(name) {
+		return
+	}
+	warn := func(err error) {
+		log.Logger().Warn("load neighbour lists; going on cold", zap.String("collection", name), zap.Error(err))
+	}
+	f, err := os.Open(db.path(name) + b200NbrSuffix)
+	if err != nil {
+		if !os.IsNotExist(err) {
+			warn(errors.Trace(err))
+		}
+		return
+	}
+	defer f.Close()
+	le := binary.LittleEndian
+	r := bufio.NewReaderSize(f, 1<<20)
+	var head [24]byte
+	if _, err := io.ReadFull(r, head[:]); err != nil || [8]byte(head[:8]) != b200NbrMagic || le.Uint32(head[8:]) != 1 {
+		warn(errors.New("not a b200 neighbour file of version 1"))
+		return
+	}
+	fileN := int(int32(le.Uint32(head[20:])))
+	if int64(le.Uint64(head[12:])) != c.generation || (n > 0 && fileN != n) {
+		return // lists of another save, or of another n: this process computes its own
+	}
+	if err := db.sizeNeighbourCache(c, fileN); err != nil {
+		warn(err)
+		return
+	}
+	h := cgo.NewHandle(io.Reader(r))
+	st := C.gorse_b200_vecdb_neighbour_cache_load(c.handle, C.gorse_b200_snapshot_read_ptr(), unsafe.Pointer(&h), nil)
+	h.Delete()
+	if err := b200Err(st); err != nil {
+		warn(err)
+	}
 }
 
 // writeHeader writes the shim's header: the ids of the live slots in slot order, which is the order of the library's stream
@@ -1261,6 +1414,7 @@ func (db *B200) reload(name string) error {
 		C.gorse_b200_vecdb_destroy(old.handle)
 	}
 	db.collections[name] = c
+	c.nbrOnce.Do(func() { db.loadNeighbours(name, c, 0) })
 	return nil
 }
 

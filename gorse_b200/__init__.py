@@ -547,6 +547,50 @@ class VectorCollection:
         check(lib.gorse_b200_vecdb_neighbour_cache_stats(self.h, ptr(s)))
         return dict(zip(("n", "capacity", "rows", "device_bytes", "served", "computed", "emptied"), (int(x) for x in s)))
 
+    def neighbour_cache_fill(self):
+        """Compute and keep the list of every live vector the neighbour cache does not hold yet, in slot order, until the pool
+        is full (gorse_b200_vecdb_neighbour_cache_fill).  -> {computed, rows, left_out, device_us}"""
+        s = np.zeros(4, np.int64)
+        check(lib.gorse_b200_vecdb_neighbour_cache_fill(self.h, ptr(s)))
+        return dict(zip(("computed", "rows", "left_out", "device_us"), (int(x) for x in s)))
+
+    def save_neighbour_cache(self, fileobj):
+        """Write the neighbour cache's held rows to a binary file object (gorse_b200_vecdb_neighbour_cache_save; the format is
+        in include/gorse_b200.h).  -> the stream's length in bytes"""
+        nbytes, err = C.c_int64(0), []
+
+        def write(user, buf, n):
+            try:
+                mv = memoryview((C.c_char * n).from_address(buf)).cast("B")
+                while mv:
+                    k = fileobj.write(mv)
+                    mv = mv[len(mv) if k is None else k:]
+                return 0
+            except Exception as e:
+                err.append(e)
+                return 1
+
+        st = lib.gorse_b200_vecdb_neighbour_cache_save(self.h, _lib.WRITE_FN(write), None, C.byref(nbytes))
+        _check_stream(st, err)
+        return nbytes.value
+
+    def load_neighbour_cache(self, fileobj):
+        """Replace the neighbour cache's rows by a stream read from a binary file object (gorse_b200_vecdb_neighbour_cache_load):
+        the cache must be on with the stream's n, and the stream must come from this collection's live vectors.  Exactly the
+        stream's bytes are read.  -> {loaded, dropped, bytes}"""
+        s, err = np.zeros(3, np.int64), []
+
+        def read(user, buf, n):
+            try:
+                return fileobj.readinto(memoryview((C.c_char * n).from_address(buf)).cast("B")) or 0
+            except Exception as e:
+                err.append(e)
+                return -1
+
+        st = lib.gorse_b200_vecdb_neighbour_cache_load(self.h, _lib.READ_FN(read), None, ptr(s))
+        _check_stream(st, err)
+        return dict(zip(("loaded", "dropped", "bytes"), (int(x) for x in s)))
+
     def save(self, fileobj):
         """Write the collection to a binary file object as a snapshot stream (gorse_b200_vecdb_save; the format is in
         include/gorse_b200.h).  The collection does not change.

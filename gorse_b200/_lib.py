@@ -101,6 +101,9 @@ PROTOTYPES = {
     "gorse_b200_vecdb_storage": (C.c_int32, [VP, C.POINTER(C.c_int32), C.POINTER(C.c_int64)]),
     "gorse_b200_vecdb_neighbour_cache": (C.c_int32, [VP, C.c_int32, C.c_int64]),
     "gorse_b200_vecdb_neighbour_cache_stats": (C.c_int32, [VP, VP]),
+    "gorse_b200_vecdb_neighbour_cache_fill": (C.c_int32, [VP, VP]),
+    "gorse_b200_vecdb_neighbour_cache_save": (C.c_int32, [VP, VP, VP, C.POINTER(C.c_int64)]),
+    "gorse_b200_vecdb_neighbour_cache_load": (C.c_int32, [VP, VP, VP, VP]),
     "gorse_b200_vecdb_save": (C.c_int32, [VP, VP, VP, VP, C.POINTER(C.c_int64)]),
     "gorse_b200_vecdb_load": (C.c_int32, [VP, VP, VP, PVP, C.POINTER(C.c_int64)]),
     "gorse_b200_vecdb_add_item_factors": (C.c_int32, [VP, VP, VP, C.c_int64, VP, VP, VP]),

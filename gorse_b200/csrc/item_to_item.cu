@@ -343,8 +343,7 @@ ncache_assemble_kernel(const int32_t *src, const int32_t *ins, int64_t R, int n,
     }
 }
 
-// the cache as it was turned on: nothing held, every slot of the collection's current generation unknown
-static void ncache_reset(gorse_b200_vecdb *db)
+void ncache_reset(gorse_b200_vecdb *db)
 {
     NeighbourCache &K = db->ncache;
     K.used = 0;
@@ -407,6 +406,71 @@ int32_t neighbour_table(gorse_b200_vecdb *db, const std::vector<int64_t> &nb, in
     return GORSE_B200_OK;
 }
 
+// the bytes per row of one fill chunk: the stage's table and slot list (8 n + 12), the cache's computed rows and sources
+// (8 n + 12); their sum over a chunk stays within FILL_CHUNK_BYTES.  Stage A's own work buffers (recall_rows,
+// sparse_search_rows) are sized by the chunk's rows as for any call of that many rows, and are not part of the bound.
+constexpr int64_t FILL_CHUNK_BYTES = 64ll << 20;
+
+// gorse_b200_vecdb_neighbour_cache_fill: the rows of every live slot the cache does not hold, in slot order, while the pool
+// has room, through neighbour_table in chunks (every row a miss), so that each row is exactly what stage A stores for it.
+// The chunk's table lands in the collection stage's grow-only buffers, which stage A of the entries uses as well.
+static int32_t ncache_fill(gorse_b200_vecdb *db, int64_t *stats_out)
+{
+    gorse_b200_ctx *c = db->ctx;
+    NeighbourCache &K = db->ncache;
+    if (K.gen != db->gen) {
+        if (K.used > 0) K.emptied++;
+        ncache_reset(db);
+    }
+    const int n = K.n;
+    std::vector<int64_t> todo;
+    int64_t left = 0;
+    for (size_t s = 0; s < db->dead.size(); s++) {
+        if (db->dead[s] || K.row_of_slot[s] >= 0) continue;
+        if (K.used + (int64_t)todo.size() < K.cap) todo.push_back((int64_t)s);
+        else left++;
+    }
+    const int64_t chunk = std::max<int64_t>(1, FILL_CHUNK_BYTES / (16ll * n + 24));
+    NeighbourStage &S = db->stage;
+    cudaEvent_t ev[2] = {nullptr, nullptr};
+    auto done = [&](int32_t st) {
+        for (cudaEvent_t e : ev)
+            if (e) cudaEventDestroy(e);
+        return st;
+    };
+    GB_CUDA(cudaEventCreate(&ev[0]));
+    if (cudaEventCreate(&ev[1]) != cudaSuccess || cudaEventRecord(ev[0], c->stream) != cudaSuccess) {
+        set_error("neighbour cache fill: events");
+        return done(GORSE_B200_ERR_CUDA);
+    }
+    const int64_t computed = K.computed;
+    std::vector<int64_t> nb;
+    for (size_t i = 0; i < todo.size(); i += (size_t)chunk) {
+        nb.assign(todo.begin() + (ptrdiff_t)i, todo.begin() + (ptrdiff_t)std::min(todo.size(), i + (size_t)chunk));
+        const size_t R = nb.size();
+        int32_t st = S.d_nb.grow(R);
+        if (!st) st = S.t_slot.grow(R * n);
+        if (!st) st = S.t_score.grow(R * n);
+        if (!st) st = S.t_cnt.grow(R);
+        if (!st) st = neighbour_table(db, nb, S.d_nb.p, n, nullptr, 0, S.t_slot.p, S.t_score.p, S.t_cnt.p, nullptr);
+        if (st) {
+            cudaStreamSynchronize(c->stream);
+            return done(st);
+        }
+    }
+    float ms = 0.f;
+    cudaError_t e = cudaEventRecord(ev[1], c->stream);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
+    if (e == cudaSuccess) e = cudaEventElapsedTime(&ms, ev[0], ev[1]);
+    if (e != cudaSuccess) {
+        set_error("neighbour cache fill: %s", cudaGetErrorString(e));
+        return done(GORSE_B200_ERR_CUDA);
+    }
+    const int64_t st[4] = {K.computed - computed, K.used, left, (int64_t)(ms * 1000.0 + 0.5)};
+    if (stats_out) std::copy(st, st + 4, stats_out);
+    return done(GORSE_B200_OK);
+}
+
 }  // namespace gb
 
 using namespace gb;
@@ -444,6 +508,25 @@ extern "C" int32_t gorse_b200_vecdb_neighbour_cache_stats(gorse_b200_vecdb *db, 
     const int64_t s[7] = {K.cap ? K.n : 0, K.cap, K.used, (int64_t)K.bytes(), K.served, K.computed, K.emptied};
     std::copy(s, s + 7, stats_out);
     return GORSE_B200_OK;
+}
+
+extern "C" int32_t gorse_b200_vecdb_neighbour_cache_fill(gorse_b200_vecdb *db, int64_t *stats_out)
+{
+    GB_CHECK_ARG(db != nullptr, "collection is NULL");
+    std::lock_guard<std::mutex> lk(db->mu);
+    NeighbourCache &K = db->ncache;
+    GB_TRY(check_stage_db(db, K.n, "neighbour cache fill"));
+    if (K.cap == 0) {
+        set_error("neighbour cache fill: the collection's neighbour cache is off");
+        return GORSE_B200_ERR_STATE;
+    }
+    ScopedDevice sd(db->ctx->device);
+    try {
+        return ncache_fill(db, stats_out);
+    } catch (const std::bad_alloc &) {
+        set_error("neighbour cache fill: host allocation failed");
+        return GORSE_B200_ERR_OOM;
+    }
 }
 
 // the context and exclusion rows of both entries

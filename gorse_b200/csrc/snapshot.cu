@@ -96,11 +96,12 @@ struct Writer {
     void *user;
     char *buf;
     int64_t cap, used = 0, pos = 0;   // pos: bytes handed to the callback
+    const char *who = "snapshot save";
     int32_t direct(const void *p, int64_t bytes)
     {
         if (bytes == 0) return GORSE_B200_OK;
         if (fn(user, p, bytes) != 0) {
-            set_error("snapshot save: the write callback failed at byte %lld", (long long)pos);
+            set_error("%s: the write callback failed at byte %lld", who, (long long)pos);
             return GORSE_B200_ERR_IO;
         }
         pos += bytes;
@@ -130,17 +131,18 @@ struct Reader {
     gorse_b200_read_fn fn;
     void *user;
     int64_t pos = 0;   // bytes read
+    const char *who = "snapshot load";
     int32_t get(void *dst, int64_t bytes, const char *field)
     {
         char *d = static_cast<char *>(dst);
         while (bytes > 0) {
             const int64_t r = fn(user, d, bytes);
             if (r < 0 || r > bytes) {
-                set_error("snapshot load: the read callback failed at byte %lld (%s)", (long long)pos, field);
+                set_error("%s: the read callback failed at byte %lld (%s)", who, (long long)pos, field);
                 return GORSE_B200_ERR_IO;
             }
             if (r == 0) {
-                set_error("snapshot load: the stream ends at byte %lld, inside %s", (long long)pos, field);
+                set_error("%s: the stream ends at byte %lld, inside %s", who, (long long)pos, field);
                 return GORSE_B200_ERR_ARG;
             }
             d += r; bytes -= r; pos += r;
@@ -420,6 +422,374 @@ int32_t load(gorse_b200_ctx *ctx, gorse_b200_read_fn read, void *user, gorse_b20
     return GORSE_B200_OK;
 }
 
+// ---- the neighbour cache's stream (gorse_b200_vecdb_neighbour_cache_save / _load) ----------------------------------------
+//
+// Slots are written as live ranks (a slot's position among the live slots, gorse_b200_vecdb_save's new_slot_out), so a stream
+// saved from a collection with deleted slots loads into the collection its snapshot restores.  The header carries a
+// fingerprint of everything the lists depend on, so a stream never loads into another collection.
+
+constexpr char NBR_MAGIC[8] = {'G', 'B', '2', '0', '0', 'N', 'B', 'R'};
+constexpr uint32_t NBR_VERSION = 1;
+constexpr int NBR_THREADS = 256;
+constexpr int64_t NBR_AHEAD_BYTES = 4ll << 20;   // load reads at most this far past the field it parses
+
+struct NbrHeader {
+    char magic[8];
+    uint32_t version;
+    int32_t n, dim, distance;
+    int64_t live;
+    uint64_t fingerprint;
+    int64_t rows;
+};
+static_assert(sizeof(NbrHeader) == 48, "the neighbour stream header is 48 bytes without padding");
+
+// splitmix64's finaliser: integer arithmetic only, so every device and host computes the same value
+__host__ __device__ inline uint64_t mix64(uint64_t x)
+{
+    x ^= x >> 30;
+    x *= 0xbf58476d1ce4e5b9ull;
+    x ^= x >> 27;
+    x *= 0x94d049bb133111ebull;
+    return x ^ (x >> 31);
+}
+
+// The fingerprint's terms, one warp per live rank r (slot live_slot[r], hidden flag hidden[r]): the row's hash is the sum of
+// mix64(index << 32 | fp32 bits) over its values (dense: every column, a bf16 value widened first; sparse: each (index,
+// value) entry), and mix64(row hash + mix64(seed ^ (r << 1 | hidden))) is added into *out.  Every sum is modulo 2^64, so the
+// result depends on neither the lanes' nor the warps' order.
+template <typename T>
+__global__ void __launch_bounds__(NBR_THREADS)
+ncache_fingerprint_kernel(const T *X, int dim, const int64_t *sp_off, const uint32_t *sp_ind, const float *sp_val, const int64_t *live_slot,
+                          const uint8_t *hidden, int64_t live, uint64_t seed, unsigned long long *out)
+{
+    const int lane = threadIdx.x & 31;
+    const int64_t nw = ((int64_t)gridDim.x * NBR_THREADS) >> 5;
+    for (int64_t r = ((int64_t)blockIdx.x * NBR_THREADS + threadIdx.x) >> 5; r < live; r += nw) {
+        const int64_t s = live_slot[r];
+        uint64_t h = 0;
+        if (dim > 0) {
+            const T *x = X + s * dim;
+            for (int j = lane; j < dim; j += 32) h += mix64((uint64_t)j << 32 | __float_as_uint(widen(x[j])));
+        } else {
+            for (int64_t t = sp_off[s] + lane; t < sp_off[s + 1]; t += 32) h += mix64((uint64_t)sp_ind[t] << 32 | __float_as_uint(sp_val[t]));
+        }
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) h += __shfl_xor_sync(0xffffffffu, h, o);
+        if (lane == 0) atomicAdd(out, (unsigned long long)mix64(h + mix64(seed ^ ((uint64_t)r << 1 | hidden[r]))));
+    }
+}
+
+// One save chunk of m rows, one warp per row i: pool row prow[i] of the neighbour cache as the stream's 32-bit words at
+// out + woff[i] - woff[0]: the row's live rank rank[i], its entry count, then each entry as (the live rank of its slot, score
+// bits).  Every neighbour of a held row is a live slot of the generation the row belongs to.
+__global__ void __launch_bounds__(NBR_THREADS)
+ncache_gather_kernel(const uint2 *pool, const int32_t *pool_cnt, int n, const int32_t *prow, const int32_t *rank, const int64_t *woff, int64_t m,
+                     const int32_t *rank_of_slot, uint32_t *out)
+{
+    const int lane = threadIdx.x & 31;
+    const int64_t nw = ((int64_t)gridDim.x * NBR_THREADS) >> 5;
+    for (int64_t i = ((int64_t)blockIdx.x * NBR_THREADS + threadIdx.x) >> 5; i < m; i += nw) {
+        const int32_t p = prow[i];
+        const int c = pool_cnt[p];
+        uint32_t *o = out + (woff[i] - woff[0]);
+        if (lane == 0) {
+            o[0] = (uint32_t)rank[i];
+            o[1] = (uint32_t)c;
+        }
+        const uint2 *e = pool + (int64_t)p * n;
+        for (int j = lane; j < c; j += 32) {
+            const uint2 x = e[j];
+            o[2 + 2 * j] = (uint32_t)rank_of_slot[x.x];
+            o[3 + 2 * j] = x.y;
+        }
+    }
+}
+
+// the live slots of db in slot order (live_slot[rank]); rank_of_slot (may be nullptr): [slots], -1 for a deleted slot
+void live_ranks(const gorse_b200_vecdb *db, std::vector<int64_t> &live_slot, std::vector<int32_t> *rank_of_slot)
+{
+    live_slot.clear();
+    live_slot.reserve((size_t)db->live);
+    if (rank_of_slot) rank_of_slot->assign(db->dead.size(), -1);
+    for (size_t s = 0; s < db->dead.size(); s++) {
+        if (db->dead[s]) continue;
+        if (rank_of_slot) (*rank_of_slot)[s] = (int32_t)live_slot.size();
+        live_slot.push_back((int64_t)s);
+    }
+}
+
+// The fingerprint of what db's neighbour lists at n depend on: the kind, distance, dim, live count and n, then each live
+// vector in rank order (its hidden flag and its values) through ncache_fingerprint_kernel.  The caller holds db->mu, the
+// index's lock and the device.
+int32_t ncache_fingerprint(gorse_b200_vecdb *db, int n, const std::vector<int64_t> &live_slot, uint64_t *fp)
+{
+    gorse_b200_ctx *c = db->ctx;
+    const int64_t live = (int64_t)live_slot.size();
+    uint64_t seed = mix64(NBR_VERSION);
+    for (int64_t v : {(int64_t)(db->dim == 0), (int64_t)db->distance, (int64_t)db->dim, live, (int64_t)n}) seed = mix64(seed ^ (uint64_t)v);
+    std::vector<uint8_t> hid((size_t)live);
+    for (int64_t r = 0; r < live; r++) hid[(size_t)r] = db->hidden[(size_t)live_slot[(size_t)r]];
+    DevBuf<int64_t> d_slot;
+    DevBuf<uint8_t> d_hid;
+    DevBuf<unsigned long long> d_sum;
+    GB_TRY(d_slot.upload(live_slot.data(), (size_t)live, c->stream));
+    GB_TRY(d_hid.upload(hid.data(), (size_t)live, c->stream));
+    GB_TRY(d_sum.alloc(1));
+    GB_CUDA(cudaMemsetAsync(d_sum.p, 0, sizeof(unsigned long long), c->stream));
+    if (live > 0) {
+        const unsigned grid = (unsigned)std::min<int64_t>(div_up(live * 32, NBR_THREADS), (int64_t)c->sm_count * 16);
+        if (db->dim > 0) {
+            with_rows(db->dense->rows(), [&](auto x) {
+                ncache_fingerprint_kernel<<<grid, NBR_THREADS, 0, c->stream>>>(x, db->dim, nullptr, nullptr, nullptr, d_slot.p, d_hid.p, live, seed,
+                                                                              d_sum.p);
+            });
+        } else {
+            gorse_b200_sparse_index *sx = db->sparse;
+            GB_TRY(sparse_sync_device(sx));
+            ncache_fingerprint_kernel<float><<<grid, NBR_THREADS, 0, c->stream>>>(nullptr, 0, sx->off.p, sx->ind.p, sx->val.p, d_slot.p, d_hid.p,
+                                                                                  live, seed, d_sum.p);
+        }
+        c->launches++;
+        GB_CUDA(cudaGetLastError());
+    }
+    unsigned long long sum = 0;
+    GB_CUDA(cudaMemcpyAsync(&sum, d_sum.p, sizeof(sum), cudaMemcpyDeviceToHost, c->stream));
+    GB_CUDA(cudaStreamSynchronize(c->stream));
+    *fp = mix64(seed ^ (uint64_t)sum);
+    return GORSE_B200_OK;
+}
+
+int32_t ncache_off(const char *who)
+{
+    set_error("neighbour cache %s: the collection's neighbour cache is off", who);
+    return GORSE_B200_ERR_STATE;
+}
+
+int32_t ncache_save(gorse_b200_vecdb *db, gorse_b200_write_fn write, void *user, int64_t *bytes_out)
+{
+    std::lock_guard<std::mutex> lk(db->mu);
+    const NeighbourCache &K = db->ncache;
+    if (K.cap == 0) return ncache_off("save");
+    std::lock_guard<std::mutex> lk2(db->dense ? db->dense->mu : db->sparse->mu);
+    gorse_b200_ctx *c = db->ctx;
+    ScopedDevice sd(c->device);
+    StreamSync sync{c->stream, c->copy_stream};
+    const int n = K.n;
+    std::vector<int64_t> live_slot;
+    std::vector<int32_t> rank_of_slot;
+    live_ranks(db, live_slot, &rank_of_slot);
+    NbrHeader h{};
+    memcpy(h.magic, NBR_MAGIC, sizeof(NBR_MAGIC));
+    h.version = NBR_VERSION;
+    h.n = n;
+    h.dim = db->dim;
+    h.distance = db->distance;
+    h.live = (int64_t)live_slot.size();
+    GB_TRY(ncache_fingerprint(db, n, live_slot, &h.fingerprint));
+    // the held rows in ascending rank; a cache of an older generation holds nothing (it empties at its next read)
+    std::vector<int32_t> prow, rank;
+    if (K.gen == db->gen)
+        for (int64_t r = 0; r < h.live; r++) {
+            const int32_t p = K.row_of_slot[(size_t)live_slot[(size_t)r]];
+            if (p < 0) continue;
+            prow.push_back(p);
+            rank.push_back((int32_t)r);
+        }
+    const int64_t rows = (int64_t)prow.size();
+    h.rows = rows;
+    std::vector<int32_t> cnt((size_t)K.used);
+    if (rows > 0) {
+        GB_CUDA(cudaMemcpyAsync(cnt.data(), K.cnt.p, sizeof(int32_t) * (size_t)K.used, cudaMemcpyDeviceToHost, c->stream));
+        GB_CUDA(cudaStreamSynchronize(c->stream));
+    }
+    std::vector<int64_t> woff((size_t)rows + 1, 0);   // each row's first 32-bit word after the header
+    for (int64_t i = 0; i < rows; i++) woff[(size_t)i + 1] = woff[(size_t)i] + 2 + 2 * (int64_t)cnt[(size_t)prow[(size_t)i]];
+    Staging stg;
+    const int64_t cap = std::min(STAGE_BYTES, std::max(MIN_STAGE_BYTES, 4 * woff[(size_t)rows]));   // a row is at most 8 + 8 * 1024 bytes
+    GB_TRY(stg.alloc(c, cap, rows > 0 ? 2 : 1, rows > 0));
+    Writer w{write, user, static_cast<char *>(stg.h[0]), cap, 0, 0, "neighbour cache save"};
+    GB_TRY(w.put(&h, sizeof(h)));
+    GB_TRY(w.flush());
+    if (rows > 0) {
+        // chunk k = rows [r0[k], r0[k + 1]) of at most cap bytes: gathered into d[k & 1], downloaded into h[k & 1] on the copy
+        // stream and written while chunk k + 1 moves, as the snapshot's dense rows are
+        std::vector<int64_t> r0{0};
+        while (r0.back() < rows) {
+            int64_t e = r0.back();
+            while (e < rows && 4 * (woff[(size_t)e + 1] - woff[(size_t)r0.back()]) <= cap) e++;
+            r0.push_back(e);
+        }
+        const int64_t chunks = (int64_t)r0.size() - 1;
+        DevBuf<int32_t> d_prow, d_rank, d_ros;
+        DevBuf<int64_t> d_woff;
+        GB_TRY(d_prow.upload(prow.data(), prow.size(), c->stream));
+        GB_TRY(d_rank.upload(rank.data(), rank.size(), c->stream));
+        GB_TRY(d_ros.upload(rank_of_slot.data(), rank_of_slot.size(), c->stream));
+        GB_TRY(d_woff.upload(woff.data(), woff.size(), c->stream));
+        auto bytes_of = [&](int64_t k) { return 4 * (woff[(size_t)r0[(size_t)k + 1]] - woff[(size_t)r0[(size_t)k]]); };
+        auto enqueue = [&](int64_t k) {
+            const int b = (int)(k & 1);
+            const int64_t i0 = r0[(size_t)k], m = r0[(size_t)k + 1] - i0;
+            const unsigned grid = (unsigned)std::min<int64_t>(div_up(m * 32, NBR_THREADS), (int64_t)c->sm_count * 16);
+            ncache_gather_kernel<<<grid, NBR_THREADS, 0, c->stream>>>(K.entry.p, K.cnt.p, n, d_prow.p + i0, d_rank.p + i0, d_woff.p + i0, m, d_ros.p,
+                                                                      reinterpret_cast<uint32_t *>(stg.d[b].p));
+            c->launches++;
+            cudaError_t e = cudaGetLastError();
+            if (e == cudaSuccess) e = cudaEventRecord(stg.gathered[b], c->stream);
+            if (e == cudaSuccess) e = cudaStreamWaitEvent(c->copy_stream, stg.gathered[b], 0);
+            if (e == cudaSuccess) e = cudaMemcpyAsync(stg.h[b], stg.d[b].p, (size_t)bytes_of(k), cudaMemcpyDeviceToHost, c->copy_stream);
+            if (e == cudaSuccess) e = cudaEventRecord(stg.copied[b], c->copy_stream);
+            return e;
+        };
+        cudaError_t e = cudaSuccess;
+        int32_t st = GORSE_B200_OK;
+        for (int64_t k = 0; k < std::min<int64_t>(2, chunks) && e == cudaSuccess; k++) e = enqueue(k);
+        for (int64_t k = 0; k < chunks && e == cudaSuccess && st == GORSE_B200_OK; k++) {
+            const int b = (int)(k & 1);
+            e = cudaEventSynchronize(stg.copied[b]);
+            if (e == cudaSuccess) st = w.direct(stg.h[b], bytes_of(k));
+            if (e == cudaSuccess && st == GORSE_B200_OK && k + 2 < chunks) e = enqueue(k + 2);
+        }
+        cudaStreamSynchronize(c->copy_stream);
+        if (e != cudaSuccess) { set_error("neighbour cache save: %s", cudaGetErrorString(e)); return GORSE_B200_ERR_CUDA; }
+        if (st) return st;
+    }
+    if (bytes_out) *bytes_out = w.pos;
+    return GORSE_B200_OK;
+}
+
+#define NBR_CHECK(cond, field, at, what)                                                                             \
+    do {                                                                                                             \
+        if (!(cond)) {                                                                                               \
+            gb::set_error("neighbour cache load: bad %s at byte %lld: %s", field, (long long)(at), what);            \
+            return GORSE_B200_ERR_ARG;                                                                               \
+        }                                                                                                            \
+    } while (0)
+
+// the reader behind load's parser: take() hands out the next k bytes, reading ahead at most `more` bytes (capped at
+// NBR_AHEAD_BYTES) that a well-formed stream holds after them, so the call never reads past the stream's end
+struct Ahead {
+    Reader &r;
+    std::vector<char> buf;
+    size_t at = 0, end = 0;
+    int64_t pos() const { return r.pos - (int64_t)(end - at); }
+    int32_t take(void *dst, int64_t k, int64_t more)
+    {
+        if ((int64_t)(end - at) < k) {
+            memmove(buf.data(), buf.data() + at, end - at);
+            end -= at;
+            at = 0;
+            const int64_t want = k - (int64_t)end + std::min(more, NBR_AHEAD_BYTES);
+            buf.resize(end + (size_t)want);
+            GB_TRY(r.get(buf.data() + end, want, "rows"));
+            end += (size_t)want;
+        }
+        memcpy(dst, buf.data() + at, (size_t)k);
+        at += (size_t)k;
+        return GORSE_B200_OK;
+    }
+};
+
+int32_t ncache_load(gorse_b200_vecdb *db, gorse_b200_read_fn read, void *user, int64_t *stats_out)
+{
+    std::lock_guard<std::mutex> lk(db->mu);
+    NeighbourCache &K = db->ncache;
+    if (K.cap == 0) return ncache_off("load");
+    std::lock_guard<std::mutex> lk2(db->dense ? db->dense->mu : db->sparse->mu);
+    gorse_b200_ctx *c = db->ctx;
+    ScopedDevice sd(c->device);
+    StreamSync sync{c->stream, c->copy_stream};
+    Reader r{read, user, 0, "neighbour cache load"};
+    NbrHeader h;
+    GB_TRY(r.get(&h, sizeof(h), "header"));
+    NBR_CHECK(memcmp(h.magic, NBR_MAGIC, sizeof(NBR_MAGIC)) == 0, "magic", 0, "not a gorse_b200 neighbour cache stream");
+    NBR_CHECK(h.version == NBR_VERSION, "version", 8, "unknown version");
+    if (h.n != K.n) {
+        set_error("neighbour cache load: the stream holds lists of n = %d, the cache keeps n = %d", h.n, K.n);
+        return GORSE_B200_ERR_STATE;
+    }
+    const int n = K.n;
+    NBR_CHECK(h.dim == db->dim, "dim", 16, "not the collection's");
+    NBR_CHECK(h.distance == db->distance, "distance", 20, "not the collection's");
+    std::vector<int64_t> live_slot;
+    live_ranks(db, live_slot, nullptr);
+    const int64_t live = (int64_t)live_slot.size();
+    NBR_CHECK(h.live == live, "live count", 24, "not the collection's");
+    uint64_t fp = 0;
+    GB_TRY(ncache_fingerprint(db, n, live_slot, &fp));
+    NBR_CHECK(h.fingerprint == fp, "fingerprint", 32, "not the collection's: saved from another collection, or before a change of this one");
+    NBR_CHECK(h.rows >= 0 && h.rows <= live, "row count", 40, "negative or above the live count");
+    // the rows the pool keeps (the lowest ranks) go into device staging in chunks of R rows through two pinned buffers (R n
+    // entries, then R counts); the pool is touched only once the whole stream has been read and checked
+    const int64_t rows = h.rows, kept = std::min(rows, K.cap);
+    const int64_t R = std::max<int64_t>(1, std::min<int64_t>(kept, STAGE_BYTES / (8ll * n + 4)));
+    DevBuf<uint2> s_entry;
+    DevBuf<int32_t> s_cnt;
+    Staging stg;
+    if (kept > 0) {
+        GB_TRY(s_entry.alloc((size_t)(kept * n)));
+        GB_TRY(s_cnt.alloc((size_t)kept));
+        GB_TRY(stg.alloc(c, R * (8ll * n + 4), 2, false));
+    }
+    std::vector<int64_t> kept_slot((size_t)kept);
+    std::vector<uint2> spill((size_t)n);
+    Ahead a{r};
+    cudaError_t e = cudaSuccess;
+    int64_t prev = -1;
+    for (int64_t i = 0; i < rows; i++) {
+        const int64_t at = a.pos(), k = i / R, j = i % R;
+        const int b = (int)(k & 1);
+        int32_t rc[2];
+        GB_TRY(a.take(rc, 8, 8 * (rows - i - 1)));
+        NBR_CHECK(rc[0] >= 0 && rc[0] < live, "row rank", at, "outside [0, live count)");
+        NBR_CHECK(rc[0] > prev, "row rank", at, "not above the previous row's");
+        NBR_CHECK(rc[1] >= 0 && rc[1] <= n, "entry count", at + 4, "outside [0, n]");
+        prev = rc[0];
+        if (i < kept && j == 0 && k >= 2) {
+            e = cudaEventSynchronize(stg.copied[b]);
+            if (e != cudaSuccess) break;
+        }
+        uint2 *row = i < kept ? static_cast<uint2 *>(stg.h[b]) + j * n : spill.data();
+        GB_TRY(a.take(row, 8ll * rc[1], 8 * (rows - i - 1)));
+        for (int t = 0; t < rc[1]; t++) {
+            NBR_CHECK((int32_t)row[t].x >= 0 && (int32_t)row[t].x < live, "entry rank", at + 8 + 8ll * t, "outside [0, live count)");
+            row[t].x = (uint32_t)live_slot[row[t].x];
+        }
+        if (i >= kept) continue;
+        kept_slot[(size_t)i] = live_slot[(size_t)rc[0]];
+        int32_t *cnt = reinterpret_cast<int32_t *>(static_cast<uint2 *>(stg.h[b]) + R * n);
+        cnt[j] = rc[1];
+        if (j == R - 1 || i == kept - 1) {
+            const int64_t m = j + 1;
+            e = cudaMemcpyAsync(s_entry.p + k * R * n, stg.h[b], sizeof(uint2) * (size_t)(m * n), cudaMemcpyHostToDevice, c->copy_stream);
+            if (e == cudaSuccess) e = cudaMemcpyAsync(s_cnt.p + k * R, cnt, sizeof(int32_t) * (size_t)m, cudaMemcpyHostToDevice, c->copy_stream);
+            if (e == cudaSuccess) e = cudaEventRecord(stg.copied[b], c->copy_stream);
+            if (e != cudaSuccess) break;
+        }
+    }
+    if (e == cudaSuccess) e = cudaStreamSynchronize(c->copy_stream);
+    if (e != cudaSuccess) {
+        set_error("neighbour cache load: %s", cudaGetErrorString(e));
+        return GORSE_B200_ERR_CUDA;
+    }
+    // every check has passed: the stream's rows replace the held ones, in pool rows 0 .. kept - 1
+    ncache_reset(db);
+    if (kept > 0) {
+        e = cudaMemcpyAsync(K.entry.p, s_entry.p, sizeof(uint2) * (size_t)(kept * n), cudaMemcpyDeviceToDevice, c->stream);
+        if (e == cudaSuccess) e = cudaMemcpyAsync(K.cnt.p, s_cnt.p, sizeof(int32_t) * (size_t)kept, cudaMemcpyDeviceToDevice, c->stream);
+        if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
+        if (e != cudaSuccess) {
+            set_error("neighbour cache load: %s", cudaGetErrorString(e));
+            return GORSE_B200_ERR_CUDA;
+        }
+    }
+    for (int64_t i = 0; i < kept; i++) K.row_of_slot[(size_t)kept_slot[(size_t)i]] = (int32_t)i;
+    K.used = kept;
+    const int64_t st[3] = {kept, rows - kept, r.pos};
+    if (stats_out) std::copy(st, st + 3, stats_out);
+    return GORSE_B200_OK;
+}
+
 }  // namespace
 }  // namespace gb
 
@@ -446,6 +816,28 @@ int32_t gorse_b200_vecdb_load(gorse_b200_ctx *ctx, gorse_b200_read_fn read, void
         return load(ctx, read, user, out, bytes_out);
     } catch (const std::bad_alloc &) {
         set_error("snapshot load: host allocation failed");
+        return GORSE_B200_ERR_OOM;
+    }
+}
+
+int32_t gorse_b200_vecdb_neighbour_cache_save(gorse_b200_vecdb *db, gorse_b200_write_fn write, void *user, int64_t *bytes_out)
+{
+    GB_CHECK_ARG(db != nullptr && write != nullptr, "NULL collection or write callback");
+    try {
+        return ncache_save(db, write, user, bytes_out);
+    } catch (const std::bad_alloc &) {
+        set_error("neighbour cache save: host allocation failed");
+        return GORSE_B200_ERR_OOM;
+    }
+}
+
+int32_t gorse_b200_vecdb_neighbour_cache_load(gorse_b200_vecdb *db, gorse_b200_read_fn read, void *user, int64_t *stats_out)
+{
+    GB_CHECK_ARG(db != nullptr && read != nullptr, "NULL collection or read callback");
+    try {
+        return ncache_load(db, read, user, stats_out);
+    } catch (const std::bad_alloc &) {
+        set_error("neighbour cache load: host allocation failed");
         return GORSE_B200_ERR_OOM;
     }
 }

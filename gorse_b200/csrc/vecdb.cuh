@@ -135,4 +135,7 @@ int32_t vecdb_allow(gorse_b200_vecdb *db, const int32_t *categories, int32_t n_c
 // so slot s is live iff scan[s + 1] != scan[s] and then moves to scan[s]; new_slot[slots + 1] (host, may be nullptr) receives
 // a copy.  Ends with the stream synchronised.  The caller holds db->mu and the device.
 int32_t vecdb_live_scan(gorse_b200_vecdb *db, DevBuf<int64_t> &scan, int64_t *new_slot);
+// the neighbour cache as it was turned on: nothing held, every slot of the collection's current generation unknown
+// (item_to_item.cu).  The caller holds db->mu.
+void ncache_reset(gorse_b200_vecdb *db);
 }  // namespace gb

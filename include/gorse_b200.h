@@ -461,7 +461,8 @@ int32_t gorse_b200_vecdb_storage(gorse_b200_vecdb *db, int32_t *value_bytes_out,
  *   reads nor fills it.  Any change of the collection empties it before its next read: gorse_b200_vecdb_add (upserts and
  *   hidden flags included), gorse_b200_vecdb_add_idf_vectors and gorse_b200_vecdb_add_item_factors when they add a vector,
  *   gorse_b200_vecdb_delete_before when it deletes one, gorse_b200_vecdb_compact when it reclaims a slot (and with them a
- *   promotion from bf16 to fp32).  gorse_b200_vecdb_load makes a collection without a cache.
+ *   promotion from bf16 to fp32).  gorse_b200_vecdb_load makes a collection without a cache; the lists saved with
+ *   gorse_b200_vecdb_neighbour_cache_save load into it with gorse_b200_vecdb_neighbour_cache_load.
  *   Answers: every entry's slots, score bits and counts are the same with the cache on or off, in any order of calls: each
  *   row is ordered by (score desc, slot asc) and certified by the exact rules of the top-k pipeline, so it does not depend
  *   on the batch it was computed in.  Per-call stats keep their meaning, except that "neighbour rows answered by the exact
@@ -523,6 +524,62 @@ typedef int32_t (*gorse_b200_write_fn)(void *user, const void *buf, int64_t n);
 typedef int64_t (*gorse_b200_read_fn)(void *user, void *buf, int64_t n);
 int32_t gorse_b200_vecdb_save(gorse_b200_vecdb *db, gorse_b200_write_fn write, void *user, int64_t *new_slot_out, int64_t *bytes_out);
 int32_t gorse_b200_vecdb_load(gorse_b200_ctx *ctx, gorse_b200_read_fn read, void *user, gorse_b200_vecdb **out, int64_t *bytes_out);
+/* Neighbour caches shared between processes: the process that writes a collection fills its neighbour cache
+ * (gorse_b200_vecdb_neighbour_cache) and saves the lists beside the collection's snapshot; every process that loads the
+ * snapshot loads the lists too and answers its first calls warm.  Every row is certified exact and depends only on the live
+ * vectors, their hidden flags and n, so a loaded row is the row the loading process would compute.
+ *
+ * gorse_b200_vecdb_neighbour_cache_fill: computes the list of every live stored vector (hidden ones included: stage A queries
+ *   them as context items) that the cache does not hold yet, in slot order, and keeps it; it stops when the pool is full.
+ *   Each row is computed by stage A itself (dense: the tensor-core sweep where it is eligible, else the exact scan; sparse: the
+ *   tiled sparse search) in chunks, so a row is exactly what an entry would store for it.  A chunk's table and the cache's
+ *   per-row work buffers stay within 64 MB; stage A's own work buffers (the top-k pipeline's, the sparse search's) are sized
+ *   by the chunk's rows as for any call of that many rows.  The rows count as "rows computed for it" in gorse_b200_vecdb_neighbour_cache_stats.  A second fill computes
+ *   nothing.  stats_out[4] (may be NULL): rows computed by this call, rows held afterwards, live rows left out because the
+ *   pool is full, device time of the call in microseconds.  The cache off: GORSE_B200_ERR_STATE; a Cosine collection:
+ *   GORSE_B200_ERR_UNSUPPORTED; NULL db: GORSE_B200_ERR_ARG.
+ *
+ * Neighbour stream format, version 1.  Every number is little-endian; there is no padding.  Slots are written as live ranks:
+ * a slot's position among the live slots, which is gorse_b200_vecdb_save's new_slot_out, for a row's own slot and for every
+ * neighbour.  So a stream saved from a collection with deleted slots loads into the collection its snapshot restores.
+ *   header, 48 bytes:
+ *     0  u8[8]  magic "GB200NBR"
+ *     8  u32    version (1)
+ *     12 i32    n: entries per list at most
+ *     16 i32    dim (0 = sparse)
+ *     20 i32    distance (gorse_b200_distance)
+ *     24 i64    live: the live vectors
+ *     32 u64    fingerprint of the live vectors (below)
+ *     40 i64    rows: the held rows that follow, at most live
+ *   then each held row in ascending live rank: i32 rank, i32 count (0 .. n), then count entries of (i32 neighbour rank, u32
+ *   score bits), in the list's order (score desc, slot asc).  The stream ends after its last row.  For the same held rows
+ *   the stream is the same bytes whatever order the rows were computed in.
+ *   The fingerprint hashes, on the device and in integer arithmetic only, each live vector in rank order: its hidden flag and
+ *   its values (dense: the fp32 bits of each value, a bf16 row widened first, so a bf16 collection and its fp32 twin agree;
+ *   sparse: each index and value), combined with the kind, distance, dim, live count and n.  Categories and timestamps are
+ *   not part of it: lists without a category filter do not depend on them.  It guards against an accidental mismatch (a
+ *   stream of another collection, or of this one before a change); it is not a cryptographic hash.
+ *
+ * gorse_b200_vecdb_neighbour_cache_save: the held rows of db's cache through write (as gorse_b200_vecdb_save), gathered and
+ *   renumbered on the device and downloaded through two pinned staging buffers of at most 64 MB.  A cache whose collection
+ *   changed since its rows were computed holds none.  *bytes_out (may be NULL): the stream's length.  The cache off:
+ *   GORSE_B200_ERR_STATE.  A write failure: GORSE_B200_ERR_IO, the cache untouched.
+ * gorse_b200_vecdb_neighbour_cache_load: replaces the rows db's cache holds by the stream's, read through read (as
+ *   gorse_b200_vecdb_load; the call reads exactly the stream's bytes).  The cache must be on with the stream's n, else
+ *   GORSE_B200_ERR_STATE.  Everything is checked before a held row is touched: magic, version, dim, distance, live count and
+ *   fingerprint against db; row ranks in [0, live), strictly ascending; counts <= n; entry ranks in [0, live); a stream that
+ *   ends early.  A bad stream is GORSE_B200_ERR_ARG and gorse_b200_last_error names the field and its byte offset; a read
+ *   failure is GORSE_B200_ERR_IO; in both cases the cache is exactly as it was.  When the pool has fewer rows than the
+ *   stream, the lowest ranks are kept and the others are reported as dropped.  The loaded rows belong to db's current
+ *   generation: the next change of db empties them as it empties computed rows.  Memory: so that a bad stream leaves the
+ *   cache as it was, the kept rows are staged on the device before they replace the held ones: min(rows, pool rows) *
+ *   (8 n + 4) bytes of device memory on top of the pool while the call runs (as much again as a full pool), and two pinned
+ *   host buffers of at most 64 MB; a staging allocation that fails is GORSE_B200_ERR_OOM / GORSE_B200_ERR_CUDA with the
+ *   cache as it was.  stats_out[3] (may be NULL): rows loaded, rows dropped, bytes read.
+ * NULL db / callback: GORSE_B200_ERR_ARG before anything else. */
+int32_t gorse_b200_vecdb_neighbour_cache_fill(gorse_b200_vecdb *db, int64_t *stats_out);
+int32_t gorse_b200_vecdb_neighbour_cache_save(gorse_b200_vecdb *db, gorse_b200_write_fn write, void *user, int64_t *bytes_out);
+int32_t gorse_b200_vecdb_neighbour_cache_load(gorse_b200_vecdb *db, gorse_b200_read_fn read, void *user, int64_t *stats_out);
 /* QueryVectors (xvec.go:373-449) for nq query vectors sharing one category filter: candidates are live, not hidden and
  * carry ALL of categories[n_categories] (CONTAIN_ALL, :381-389).  Results per query: slots_out / scores_out [nq x topk],
  * best first, count_out[nq]; entries past count_out[q] in a row are not part of the answer and are left unspecified; score = dot (Dot) or the NEGATED distance (Euclidean, Cosine) -- higher is more similar
