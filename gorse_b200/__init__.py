@@ -422,6 +422,41 @@ class SparseIndex:
         self.close()
 
 
+def _writer(fileobj, err):
+    """a gorse_b200_write_fn that writes to a binary file object; an exception raised there is appended to err"""
+
+    def write(user, buf, n):
+        try:
+            mv = memoryview((C.c_char * n).from_address(buf)).cast("B")
+            while mv:   # a raw file may write part of the buffer
+                k = fileobj.write(mv)
+                mv = mv[len(mv) if k is None else k:]
+            return 0
+        except Exception as e:  # reported as GORSE_B200_ERR_IO, re-raised as the cause
+            err.append(e)
+            return 1
+
+    return _lib.WRITE_FN(write)
+
+
+def _reader(fileobj, err, head=None):
+    """a gorse_b200_read_fn that reads from a binary file object; an exception raised there is appended to err.  head (a
+    bytearray), when given, collects the stream's first 48 bytes"""
+
+    def read(user, buf, n):
+        try:
+            mv = memoryview((C.c_char * n).from_address(buf)).cast("B")
+            got = fileobj.readinto(mv) or 0
+            if head is not None and len(head) < 48:
+                head.extend(mv[:min(got, 48 - len(head))])
+            return got
+        except Exception as e:
+            err.append(e)
+            return -1
+
+    return _lib.READ_FN(read)
+
+
 def _check_stream(status, err):
     """check() for a call that ran a file object's callbacks: an exception raised there is the cause of the error"""
     if status != _lib.OK and err:
@@ -558,19 +593,7 @@ class VectorCollection:
         """Write the neighbour cache's held rows to a binary file object (gorse_b200_vecdb_neighbour_cache_save; the format is
         in include/gorse_b200.h).  -> the stream's length in bytes"""
         nbytes, err = C.c_int64(0), []
-
-        def write(user, buf, n):
-            try:
-                mv = memoryview((C.c_char * n).from_address(buf)).cast("B")
-                while mv:
-                    k = fileobj.write(mv)
-                    mv = mv[len(mv) if k is None else k:]
-                return 0
-            except Exception as e:
-                err.append(e)
-                return 1
-
-        st = lib.gorse_b200_vecdb_neighbour_cache_save(self.h, _lib.WRITE_FN(write), None, C.byref(nbytes))
+        st = lib.gorse_b200_vecdb_neighbour_cache_save(self.h, _writer(fileobj, err), None, C.byref(nbytes))
         _check_stream(st, err)
         return nbytes.value
 
@@ -579,15 +602,7 @@ class VectorCollection:
         the cache must be on with the stream's n, and the stream must come from this collection's live vectors.  Exactly the
         stream's bytes are read.  -> {loaded, dropped, bytes}"""
         s, err = np.zeros(3, np.int64), []
-
-        def read(user, buf, n):
-            try:
-                return fileobj.readinto(memoryview((C.c_char * n).from_address(buf)).cast("B")) or 0
-            except Exception as e:
-                err.append(e)
-                return -1
-
-        st = lib.gorse_b200_vecdb_neighbour_cache_load(self.h, _lib.READ_FN(read), None, ptr(s))
+        st = lib.gorse_b200_vecdb_neighbour_cache_load(self.h, _reader(fileobj, err), None, ptr(s))
         _check_stream(st, err)
         return dict(zip(("loaded", "dropped", "bytes"), (int(x) for x in s)))
 
@@ -597,19 +612,7 @@ class VectorCollection:
         -> new_slot int64 [slots]: the position of each slot's vector in the stream, -1 for a deleted slot (compact()'s map)"""
         slots = self.count()[1]
         new_slot, nbytes, err = np.zeros(max(slots, 1), np.int64), C.c_int64(0), []
-
-        def write(user, buf, n):
-            try:
-                mv = memoryview((C.c_char * n).from_address(buf)).cast("B")
-                while mv:   # a raw file may write part of the buffer
-                    k = fileobj.write(mv)
-                    mv = mv[len(mv) if k is None else k:]
-                return 0
-            except Exception as e:  # reported as GORSE_B200_ERR_IO, re-raised as the cause
-                err.append(e)
-                return 1
-
-        st = lib.gorse_b200_vecdb_save(self.h, _lib.WRITE_FN(write), None, ptr(new_slot), C.byref(nbytes))
+        st = lib.gorse_b200_vecdb_save(self.h, _writer(fileobj, err), None, ptr(new_slot), C.byref(nbytes))
         _check_stream(st, err)
         return new_slot[:slots]
 
@@ -619,19 +622,7 @@ class VectorCollection:
         of the stream is in slot i, and every entry answers as the saved collection answers after compact().  Exactly the
         stream's bytes are read."""
         head, h, nbytes, err = bytearray(), C.c_void_p(), C.c_int64(0), []
-
-        def read(user, buf, n):
-            try:
-                mv = memoryview((C.c_char * n).from_address(buf)).cast("B")
-                got = fileobj.readinto(mv) or 0
-                if len(head) < 48:
-                    head.extend(mv[:min(got, 48 - len(head))])
-                return got
-            except Exception as e:
-                err.append(e)
-                return -1
-
-        st = lib.gorse_b200_vecdb_load(ctx.h, _lib.READ_FN(read), None, C.byref(h), C.byref(nbytes))
+        st = lib.gorse_b200_vecdb_load(ctx.h, _reader(fileobj, err, head), None, C.byref(h), C.byref(nbytes))
         _check_stream(st, err)
         self = cls.__new__(cls)
         self.ctx, self.h = ctx, h

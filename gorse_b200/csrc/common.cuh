@@ -152,6 +152,25 @@ struct DevBuf {
 static_assert(!std::is_copy_constructible<DevBuf<int>>::value && !std::is_copy_assignable<DevBuf<int>>::value, "DevBuf owns its memory");
 static_assert(std::is_nothrow_move_constructible<DevBuf<int>>::value, "std::vector<DevBuf> moves on growth");
 
+// owning pinned host buffer (cudaHostAlloc), allocated once: the destructor frees; host memory, so not counted in
+// g_device_bytes
+template <typename T>
+struct PinnedBuf {
+    T *p = nullptr;
+    PinnedBuf() = default;
+    PinnedBuf(const PinnedBuf &) = delete;
+    PinnedBuf &operator=(const PinnedBuf &) = delete;
+    ~PinnedBuf()
+    {
+        if (p) cudaFreeHost(p);
+    }
+    int32_t alloc(size_t count)
+    {
+        GB_CUDA(cudaHostAlloc((void **)&p, count * sizeof(T), cudaHostAllocDefault));
+        return GORSE_B200_OK;
+    }
+};
+
 // synchronises its streams when destroyed: declare it after the buffers the enqueued work reads, so it is destroyed first
 struct StreamSync {
     cudaStream_t a, b = nullptr;
@@ -162,7 +181,8 @@ struct StreamSync {
     }
 };
 
-// an owning CUDA event without timing; declare it before the StreamSync that waits for the work it records
+// an owning CUDA event, without timing unless create() is asked for it; declare it before the StreamSync that waits for the
+// work it records
 struct Event {
     cudaEvent_t e = nullptr;
     Event() = default;
@@ -172,9 +192,9 @@ struct Event {
     {
         if (e) cudaEventDestroy(e);
     }
-    int32_t create()
+    int32_t create(unsigned flags = cudaEventDisableTiming)
     {
-        GB_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+        GB_CUDA(cudaEventCreateWithFlags(&e, flags));
         return GORSE_B200_OK;
     }
 };

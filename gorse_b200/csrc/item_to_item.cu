@@ -432,16 +432,11 @@ static int32_t ncache_fill(gorse_b200_vecdb *db, int64_t *stats_out)
     }
     const int64_t chunk = std::max<int64_t>(1, FILL_CHUNK_BYTES / (16ll * n + 24));
     NeighbourStage &S = db->stage;
-    cudaEvent_t ev[2] = {nullptr, nullptr};
-    auto done = [&](int32_t st) {
-        for (cudaEvent_t e : ev)
-            if (e) cudaEventDestroy(e);
-        return st;
-    };
-    GB_CUDA(cudaEventCreate(&ev[0]));
-    if (cudaEventCreate(&ev[1]) != cudaSuccess || cudaEventRecord(ev[0], c->stream) != cudaSuccess) {
+    Event ev[2];   // timed: the device time of the fill
+    GB_TRY(ev[0].create(cudaEventDefault));
+    if (ev[1].create(cudaEventDefault) != GORSE_B200_OK || cudaEventRecord(ev[0].e, c->stream) != cudaSuccess) {
         set_error("neighbour cache fill: events");
-        return done(GORSE_B200_ERR_CUDA);
+        return GORSE_B200_ERR_CUDA;
     }
     const int64_t computed = K.computed;
     std::vector<int64_t> nb;
@@ -455,20 +450,20 @@ static int32_t ncache_fill(gorse_b200_vecdb *db, int64_t *stats_out)
         if (!st) st = neighbour_table(db, nb, S.d_nb.p, n, nullptr, 0, S.t_slot.p, S.t_score.p, S.t_cnt.p, nullptr);
         if (st) {
             cudaStreamSynchronize(c->stream);
-            return done(st);
+            return st;
         }
     }
     float ms = 0.f;
-    cudaError_t e = cudaEventRecord(ev[1], c->stream);
+    cudaError_t e = cudaEventRecord(ev[1].e, c->stream);
     if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
-    if (e == cudaSuccess) e = cudaEventElapsedTime(&ms, ev[0], ev[1]);
+    if (e == cudaSuccess) e = cudaEventElapsedTime(&ms, ev[0].e, ev[1].e);
     if (e != cudaSuccess) {
         set_error("neighbour cache fill: %s", cudaGetErrorString(e));
-        return done(GORSE_B200_ERR_CUDA);
+        return GORSE_B200_ERR_CUDA;
     }
     const int64_t st[4] = {K.computed - computed, K.used, left, (int64_t)(ms * 1000.0 + 0.5)};
     if (stats_out) std::copy(st, st + 4, stats_out);
-    return done(GORSE_B200_OK);
+    return GORSE_B200_OK;
 }
 
 }  // namespace gb

@@ -52,41 +52,35 @@ __global__ void snapshot_gather_kernel(const V *X, int dv, const int64_t *scan, 
     }
 }
 
-// the two pinned staging buffers, the device gather buffers and their events; released after both streams have drained
+// the two pinned staging buffers, the device gather buffers and their events; `sync`, declared last and so destroyed first,
+// drains both streams before any of them is freed
 struct Staging {
-    gorse_b200_ctx *c = nullptr;
-    void *h[2] = {nullptr, nullptr};
+    gorse_b200_ctx *c;
+    PinnedBuf<char> h[2];
     DevBuf<float> d[2];
-    cudaEvent_t gathered[2] = {nullptr, nullptr}, copied[2] = {nullptr, nullptr};
-    int32_t *flag = nullptr;   // [2] pinned: load's inexact flag of the chunk in each buffer
-    int32_t alloc(gorse_b200_ctx *ctx, int64_t bytes, int buffers, bool device)
+    Event gathered[2], copied[2];
+    PinnedBuf<int32_t> flag;   // [2]: load's inexact flag of the chunk in each buffer
+    StreamSync sync;
+    explicit Staging(gorse_b200_ctx *ctx) : c(ctx), sync{ctx->stream, ctx->copy_stream} {}
+    int32_t alloc(int64_t bytes, int buffers, bool device)
     {
-        c = ctx;
         for (int b = 0; b < buffers; b++) {
-            GB_CUDA(cudaHostAlloc(&h[b], (size_t)bytes, cudaHostAllocDefault));
-            GB_CUDA(cudaEventCreateWithFlags(&copied[b], cudaEventDisableTiming));
+            GB_TRY(h[b].alloc((size_t)bytes));
+            GB_TRY(copied[b].create());
             if (!device) continue;
             GB_TRY(d[b].alloc((size_t)bytes / sizeof(float)));
-            GB_CUDA(cudaEventCreateWithFlags(&gathered[b], cudaEventDisableTiming));
+            GB_TRY(gathered[b].create());
         }
         if (device) {
-            GB_CUDA(cudaHostAlloc((void **)&flag, 2 * sizeof(int32_t), cudaHostAllocDefault));
-            flag[0] = flag[1] = 0;   // pinned memory comes back uninitialised
+            GB_TRY(flag.alloc(2));
+            flag.p[0] = flag.p[1] = 0;   // pinned memory comes back uninitialised
         }
         return GORSE_B200_OK;
     }
-    ~Staging()
-    {
-        if (!c) return;
-        cudaStreamSynchronize(c->stream);
-        cudaStreamSynchronize(c->copy_stream);
-        for (int b = 0; b < 2; b++) {
-            if (h[b]) cudaFreeHost(h[b]);
-            if (gathered[b]) cudaEventDestroy(gathered[b]);
-            if (copied[b]) cudaEventDestroy(copied[b]);
-        }
-        if (flag) cudaFreeHost(flag);
-    }
+    // a load's chunk k fills h[k & 1]: wait_free waits until chunk k - 2's upload from it has finished, and in_flight marks
+    // it busy again once chunk k's upload is queued on the copy stream
+    cudaError_t wait_free(int64_t k) { return k >= 2 ? cudaEventSynchronize(copied[k & 1].e) : cudaSuccess; }
+    cudaError_t in_flight(int64_t k) { return cudaEventRecord(copied[k & 1].e, c->copy_stream); }
 };
 
 // the caller's write callback behind a staging buffer: put() appends and hands full buffers on, direct() hands a buffer of the
@@ -126,6 +120,38 @@ struct Writer {
     }
 };
 
+// A save's chunks 0 .. chunks - 1 through the staging buffers: gather(k, d) launches chunk k's gather into the device buffer d
+// on the context's stream, and bytes(k) is the chunk's length.  Chunk k is downloaded into h[k & 1] on the copy stream and
+// written while chunk k + 1 is gathered and downloaded; chunk k + 2 reuses the buffers once chunk k is written.
+template <typename Bytes, typename Gather>
+int32_t write_chunks(Staging &stg, Writer &w, int64_t chunks, Bytes bytes, Gather gather)
+{
+    gorse_b200_ctx *c = stg.c;
+    auto enqueue = [&](int64_t k) {
+        const int b = (int)(k & 1);
+        gather(k, stg.d[b].p);
+        c->launches++;
+        cudaError_t e = cudaGetLastError();
+        if (e == cudaSuccess) e = cudaEventRecord(stg.gathered[b].e, c->stream);
+        if (e == cudaSuccess) e = cudaStreamWaitEvent(c->copy_stream, stg.gathered[b].e, 0);
+        if (e == cudaSuccess) e = cudaMemcpyAsync(stg.h[b].p, stg.d[b].p, (size_t)bytes(k), cudaMemcpyDeviceToHost, c->copy_stream);
+        if (e == cudaSuccess) e = cudaEventRecord(stg.copied[b].e, c->copy_stream);
+        return e;
+    };
+    cudaError_t e = cudaSuccess;
+    int32_t st = GORSE_B200_OK;
+    for (int64_t k = 0; k < std::min<int64_t>(2, chunks) && e == cudaSuccess; k++) e = enqueue(k);
+    for (int64_t k = 0; k < chunks && e == cudaSuccess && st == GORSE_B200_OK; k++) {
+        const int b = (int)(k & 1);
+        e = cudaEventSynchronize(stg.copied[b].e);
+        if (e == cudaSuccess) st = w.direct(stg.h[b].p, bytes(k));
+        if (e == cudaSuccess && st == GORSE_B200_OK && k + 2 < chunks) e = enqueue(k + 2);
+    }
+    cudaStreamSynchronize(c->copy_stream);
+    if (e != cudaSuccess) { set_error("%s: %s", w.who, cudaGetErrorString(e)); return GORSE_B200_ERR_CUDA; }
+    return st;
+}
+
 // the caller's read callback: get() reads exactly `bytes` or fails, naming the field and its byte offset
 struct Reader {
     gorse_b200_read_fn fn;
@@ -149,6 +175,12 @@ struct Reader {
         }
         return GORSE_B200_OK;
     }
+    // ERR_ARG for a field that fails its check, naming the field and its byte offset
+    int32_t bad(const char *field, int64_t at, const char *what) const
+    {
+        set_error("%s: bad %s at byte %lld: %s", who, field, (long long)at, what);
+        return GORSE_B200_ERR_ARG;
+    }
     // count elements into v, grown piece by piece: a header that claims more than the stream holds allocates no more than arrived
     template <typename T>
     int32_t array(std::vector<T> &v, int64_t count, const char *field)
@@ -164,21 +196,19 @@ struct Reader {
     }
 };
 
-#define SNAP_CHECK(cond, field, at, what)                                                                            \
-    do {                                                                                                             \
-        if (!(cond)) {                                                                                               \
-            gb::set_error("snapshot load: bad %s at byte %lld: %s", field, (long long)(at), what);                   \
-            return GORSE_B200_ERR_ARG;                                                                               \
-        }                                                                                                            \
+// a field read through Reader r that fails cond ends the call with r.bad(field, at, what)
+#define STREAM_CHECK(r, cond, field, at, what)          \
+    do {                                                \
+        if (!(cond)) return (r).bad(field, at, what);   \
     } while (0)
 
 // offsets[n + 1] of a section starting at byte `at`: from 0, never decreasing, ending at `total`
-int32_t check_offsets(const std::vector<int64_t> &off, int64_t total, const char *field, int64_t at)
+int32_t check_offsets(const Reader &r, const std::vector<int64_t> &off, int64_t total, const char *field, int64_t at)
 {
-    SNAP_CHECK(off[0] == 0, field, at, "the first offset is not 0");
+    STREAM_CHECK(r, off[0] == 0, field, at, "the first offset is not 0");
     const int64_t n = (int64_t)off.size() - 1;
-    for (int64_t i = 0; i < n; i++) SNAP_CHECK(off[(size_t)i + 1] >= off[(size_t)i], field, at + 8 * (i + 1), "offsets decrease");
-    SNAP_CHECK(off[(size_t)n] == total, field, at + 8 * n, "the last offset disagrees with the header's count");
+    for (int64_t i = 0; i < n; i++) STREAM_CHECK(r, off[(size_t)i + 1] >= off[(size_t)i], field, at + 8 * (i + 1), "offsets decrease");
+    STREAM_CHECK(r, off[(size_t)n] == total, field, at + 8 * n, "the last offset disagrees with the header's count");
     return GORSE_B200_OK;
 }
 
@@ -203,10 +233,10 @@ int32_t save(gorse_b200_vecdb *db, gorse_b200_write_fn write, void *user, int64_
     }
     const int64_t values = dim > 0 ? 4 * live * dim : 8 * (live + 1) + 8 * h.nnz;
     const int64_t total = (int64_t)sizeof(Header) + 17 * live + 8 + 4 * h.n_cats + values;
-    Staging stg;
+    Staging stg(c);
     const int64_t cap = std::min(STAGE_BYTES, std::max(MIN_STAGE_BYTES, total));
-    GB_TRY(stg.alloc(c, cap, dim > 0 && live > 0 ? 2 : 1, dim > 0 && live > 0));
-    Writer w{write, user, static_cast<char *>(stg.h[0]), cap};
+    GB_TRY(stg.alloc(cap, dim > 0 && live > 0 ? 2 : 1, dim > 0 && live > 0));
+    Writer w{write, user, stg.h[0].p, cap};
     GB_TRY(w.put(&h, sizeof(h)));
     for (int64_t s = 0; s < n; s++)
         if (!db->dead[(size_t)s]) GB_TRY(w.put(&db->hidden[(size_t)s], 1));
@@ -237,44 +267,24 @@ int32_t save(gorse_b200_vecdb *db, gorse_b200_write_fn write, void *user, int64_
     }
     GB_TRY(w.flush());
     if (dim > 0 && live > 0) {
-        // chunk k = the live rows [k R, k R + R): gathered into d[k & 1] on the stream, downloaded into h[k & 1] on the copy
-        // stream, written while chunk k + 1 moves; chunk k + 2 reuses the buffers once chunk k is written
+        // chunk k = the live rows [k R, k R + R)
         DevBuf<int64_t> scan;
-        int32_t st = vecdb_live_scan(db, scan, nullptr);
-        if (st) return st;
+        GB_TRY(vecdb_live_scan(db, scan, nullptr));
         const gorse_b200_index *ix = db->dense;
         const int64_t R = cap / (4 * dim), chunks = (live + R - 1) / R;
-        auto enqueue = [&](int64_t k) {
-            const int b = (int)(k & 1);
-            const int64_t j0 = k * R, m = std::min(R, live - j0);
+        auto rows_of = [&](int64_t k) { return std::min(R, live - k * R); };
+        GB_TRY(write_chunks(stg, w, chunks, [&](int64_t k) { return 4 * rows_of(k) * dim; }, [&](int64_t k, float *d) {
+            const int64_t m = rows_of(k);
             const unsigned grid = (unsigned)std::min<int64_t>((m + 7) / 8, (int64_t)c->sm_count * 16);
             with_rows(ix->rows(), [&](auto x) {   // the stream holds fp32 values: bf16 rows are widened by the gather
                 using Q = typename row_quad_type<row_elem_t<decltype(x)>>::type;
                 if (dim % 4 == 0)
-                    snapshot_gather_kernel<<<grid, 256, 0, c->stream>>>(reinterpret_cast<const Q *>(x), (int)(dim / 4), scan.p, n, j0, m,
-                                                                       reinterpret_cast<float4 *>(stg.d[b].p));
+                    snapshot_gather_kernel<<<grid, 256, 0, c->stream>>>(reinterpret_cast<const Q *>(x), (int)(dim / 4), scan.p, n, k * R, m,
+                                                                       reinterpret_cast<float4 *>(d));
                 else
-                    snapshot_gather_kernel<<<grid, 256, 0, c->stream>>>(x, (int)dim, scan.p, n, j0, m, stg.d[b].p);
+                    snapshot_gather_kernel<<<grid, 256, 0, c->stream>>>(x, (int)dim, scan.p, n, k * R, m, d);
             });
-            c->launches++;
-            cudaError_t e = cudaGetLastError();
-            if (e == cudaSuccess) e = cudaEventRecord(stg.gathered[b], c->stream);
-            if (e == cudaSuccess) e = cudaStreamWaitEvent(c->copy_stream, stg.gathered[b], 0);
-            if (e == cudaSuccess) e = cudaMemcpyAsync(stg.h[b], stg.d[b].p, (size_t)(4 * m * dim), cudaMemcpyDeviceToHost, c->copy_stream);
-            if (e == cudaSuccess) e = cudaEventRecord(stg.copied[b], c->copy_stream);
-            return e;
-        };
-        cudaError_t e = cudaSuccess;
-        for (int64_t k = 0; k < std::min<int64_t>(2, chunks) && e == cudaSuccess; k++) e = enqueue(k);
-        for (int64_t k = 0; k < chunks && e == cudaSuccess && st == GORSE_B200_OK; k++) {
-            const int b = (int)(k & 1);
-            e = cudaEventSynchronize(stg.copied[b]);
-            if (e == cudaSuccess) st = w.direct(stg.h[b], 4 * std::min(R, live - k * R) * dim);
-            if (e == cudaSuccess && st == GORSE_B200_OK && k + 2 < chunks) e = enqueue(k + 2);
-        }
-        cudaStreamSynchronize(c->copy_stream);
-        if (e != cudaSuccess) { set_error("snapshot save: %s", cudaGetErrorString(e)); return GORSE_B200_ERR_CUDA; }
-        if (st) return st;
+        }));
     }
     if (new_slot_out)
         for (int64_t s = 0, j = 0; s < n; s++) new_slot_out[s] = db->dead[(size_t)s] ? -1 : j++;
@@ -283,24 +293,24 @@ int32_t save(gorse_b200_vecdb *db, gorse_b200_write_fn write, void *user, int64_
 }
 
 // the header's fields, each count against the others and against int64 overflow of its section
-int32_t check_header(const Header &h)
+int32_t check_header(const Reader &r, const Header &h)
 {
-    SNAP_CHECK(memcmp(h.magic, MAGIC, sizeof(MAGIC)) == 0, "magic", 0, "not a gorse_b200 collection stream");
-    SNAP_CHECK(h.version == VERSION, "version", 8, "unknown version");
-    SNAP_CHECK(h.dim >= 0 && h.dim <= 16384, "dim", 12, "outside [0, 16384]");
-    SNAP_CHECK(h.distance == GORSE_B200_DISTANCE_EUCLIDEAN || h.distance == GORSE_B200_DISTANCE_DOT || h.distance == GORSE_B200_DISTANCE_COSINE,
+    STREAM_CHECK(r, memcmp(h.magic, MAGIC, sizeof(MAGIC)) == 0, "magic", 0, "not a gorse_b200 collection stream");
+    STREAM_CHECK(r, h.version == VERSION, "version", 8, "unknown version");
+    STREAM_CHECK(r, h.dim >= 0 && h.dim <= 16384, "dim", 12, "outside [0, 16384]");
+    STREAM_CHECK(r, h.distance == GORSE_B200_DISTANCE_EUCLIDEAN || h.distance == GORSE_B200_DISTANCE_DOT || h.distance == GORSE_B200_DISTANCE_COSINE,
                "distance", 16, "unknown distance");
-    SNAP_CHECK(h.dim > 0 || h.distance == GORSE_B200_DISTANCE_DOT, "distance", 16, "a sparse collection is Dot");
-    SNAP_CHECK(h.reserved == 0, "reserved", 20, "not 0");
+    STREAM_CHECK(r, h.dim > 0 || h.distance == GORSE_B200_DISTANCE_DOT, "distance", 16, "a sparse collection is Dot");
+    STREAM_CHECK(r, h.reserved == 0, "reserved", 20, "not 0");
     // every section's byte count, and their sum, fit in an int64 below 2^62
     constexpr int64_t LIM = 1ll << 62;
-    SNAP_CHECK(h.n >= 0 && h.n < LIM / 32, "n", 24, "negative or too large");
-    SNAP_CHECK(h.dim > 0 || h.n < (1ll << 31) - 1, "n", 24, "more than 2^31 - 1 sparse vectors");
-    SNAP_CHECK(h.dim > 0 || h.n < LIM / 32, "n", 24, "too large");
-    SNAP_CHECK(h.dim == 0 || h.n <= LIM / 8 / h.dim, "n", 24, "n * dim overflows");
-    SNAP_CHECK(h.nnz >= 0 && h.nnz < LIM / 16, "nnz", 32, "negative or too large");
-    SNAP_CHECK(h.dim == 0 || h.nnz == 0, "nnz", 32, "not 0 in a dense collection");
-    SNAP_CHECK(h.n_cats >= 0 && h.n_cats < LIM / 16, "category count", 40, "negative or too large");
+    STREAM_CHECK(r, h.n >= 0 && h.n < LIM / 32, "n", 24, "negative or too large");
+    STREAM_CHECK(r, h.dim > 0 || h.n < (1ll << 31) - 1, "n", 24, "more than 2^31 - 1 sparse vectors");
+    STREAM_CHECK(r, h.dim > 0 || h.n < LIM / 32, "n", 24, "too large");
+    STREAM_CHECK(r, h.dim == 0 || h.n <= LIM / 8 / h.dim, "n", 24, "n * dim overflows");
+    STREAM_CHECK(r, h.nnz >= 0 && h.nnz < LIM / 16, "nnz", 32, "negative or too large");
+    STREAM_CHECK(r, h.dim == 0 || h.nnz == 0, "nnz", 32, "not 0 in a dense collection");
+    STREAM_CHECK(r, h.n_cats >= 0 && h.n_cats < LIM / 16, "category count", 40, "negative or too large");
     return GORSE_B200_OK;
 }
 
@@ -309,18 +319,18 @@ int32_t load(gorse_b200_ctx *ctx, gorse_b200_read_fn read, void *user, gorse_b20
     Reader r{read, user};
     Header h;
     GB_TRY(r.get(&h, sizeof(h), "header"));
-    GB_TRY(check_header(h));
+    GB_TRY(check_header(r, h));
     const int64_t n = h.n, dim = h.dim;
     std::vector<uint8_t> hidden;
     std::vector<int64_t> ts, cat_off;
     std::vector<int32_t> cats;
     int64_t at = r.pos;
     GB_TRY(r.array(hidden, n, "hidden"));
-    for (int64_t i = 0; i < n; i++) SNAP_CHECK(hidden[(size_t)i] <= 1, "hidden", at + i, "neither 0 nor 1");
+    for (int64_t i = 0; i < n; i++) STREAM_CHECK(r, hidden[(size_t)i] <= 1, "hidden", at + i, "neither 0 nor 1");
     GB_TRY(r.array(ts, n, "timestamp_ms"));
     at = r.pos;
     GB_TRY(r.array(cat_off, n + 1, "cat_off"));
-    GB_TRY(check_offsets(cat_off, h.n_cats, "cat_off", at));
+    GB_TRY(check_offsets(r, cat_off, h.n_cats, "cat_off", at));
     GB_TRY(r.array(cats, h.n_cats, "cats"));
     std::vector<int64_t> sp_off;
     std::vector<uint32_t> sp_ind;
@@ -329,19 +339,19 @@ int32_t load(gorse_b200_ctx *ctx, gorse_b200_read_fn read, void *user, gorse_b20
     if (dim == 0) {
         at = r.pos;
         GB_TRY(r.array(sp_off, n + 1, "off"));
-        GB_TRY(check_offsets(sp_off, h.nnz, "off", at));
+        GB_TRY(check_offsets(r, sp_off, h.nnz, "off", at));
         at = r.pos;
         GB_TRY(r.array(sp_ind, h.nnz, "ind"));
         for (int64_t i = 0; i < n; i++)
             for (int64_t t = sp_off[(size_t)i]; t < sp_off[(size_t)i + 1]; t++) {
-                SNAP_CHECK(t == sp_off[(size_t)i] || sp_ind[(size_t)t] > sp_ind[(size_t)t - 1], "ind", at + 4 * t,
+                STREAM_CHECK(r, t == sp_off[(size_t)i] || sp_ind[(size_t)t] > sp_ind[(size_t)t - 1], "ind", at + 4 * t,
                            "indices of a vector not strictly ascending");
-                SNAP_CHECK(sp_ind[(size_t)t] < 0x7fffffffu, "ind", at + 4 * t, "index >= 0x7fffffff");
+                STREAM_CHECK(r, sp_ind[(size_t)t] < 0x7fffffffu, "ind", at + 4 * t, "index >= 0x7fffffff");
                 n_features = std::max(n_features, sp_ind[(size_t)t] + 1);
             }
         at = r.pos;
         GB_TRY(r.array(sp_val, h.nnz, "val"));
-        for (int64_t t = 0; t < h.nnz; t++) SNAP_CHECK(!std::isnan(sp_val[(size_t)t]), "val", at + 4 * t, "NaN value");
+        for (int64_t t = 0; t < h.nnz; t++) STREAM_CHECK(r, !std::isnan(sp_val[(size_t)t]), "val", at + 4 * t, "NaN value");
     }
     std::vector<uint8_t> dead((size_t)n, 0);
     // the handle is this call's until it returns: nobody else can take its locks
@@ -363,10 +373,10 @@ int32_t load(gorse_b200_ctx *ctx, gorse_b200_read_fn read, void *user, gorse_b20
             // bf16-exact promotes the collection: the rows before it are widened, and chunk k0 and the one after it, whose fp32
             // values are still in the device buffers, are copied in; later chunks go straight into the fp32 rows.
             gorse_b200_index *ix = db->dense;
-            Staging stg;
+            Staging stg(ctx);
             const int64_t cap = std::min(STAGE_BYTES, std::max(MIN_STAGE_BYTES, 4 * n * dim));
             st = index_reserve(ix, n);
-            if (st == GORSE_B200_OK) st = stg.alloc(ctx, cap, 2, ix->value_bytes == 2);
+            if (st == GORSE_B200_OK) st = stg.alloc(cap, 2, ix->value_bytes == 2);
             if (st == GORSE_B200_OK) st = ix->inexact.grow(2);
             const int64_t R = cap / (4 * dim), chunks = st ? 0 : (n + R - 1) / R;
             auto rows_of = [&](int64_t k) { return std::min(R, n - k * R); };
@@ -380,22 +390,22 @@ int32_t load(gorse_b200_ctx *ctx, gorse_b200_read_fn read, void *user, gorse_b20
             for (int64_t k = 0; k < chunks && e == cudaSuccess && st == GORSE_B200_OK; k++) {
                 const int b = (int)(k & 1);
                 const int64_t j0 = k * R, bytes = 4 * rows_of(k) * dim;
-                if (k >= 2) e = cudaEventSynchronize(stg.copied[b]);
-                if (e == cudaSuccess && k >= 2 && ix->value_bytes == 2 && stg.flag[b]) promote_at(k - 2, k);   // chunk k - 2's flag
-                if (e == cudaSuccess && st == GORSE_B200_OK) st = r.get(stg.h[b], bytes, "values");
+                e = stg.wait_free(k);
+                if (e == cudaSuccess && k >= 2 && ix->value_bytes == 2 && stg.flag.p[b]) promote_at(k - 2, k);   // chunk k - 2's flag
+                if (e == cudaSuccess && st == GORSE_B200_OK) st = r.get(stg.h[b].p, bytes, "values");
                 if (e != cudaSuccess || st != GORSE_B200_OK) break;
                 if (ix->value_bytes == 2) {
-                    e = cudaMemcpyAsync(stg.d[b].p, stg.h[b], (size_t)bytes, cudaMemcpyHostToDevice, ctx->copy_stream);
+                    e = cudaMemcpyAsync(stg.d[b].p, stg.h[b].p, (size_t)bytes, cudaMemcpyHostToDevice, ctx->copy_stream);
                     if (e == cudaSuccess) e = cudaMemsetAsync(ix->inexact.p + b, 0, sizeof(int32_t), ctx->copy_stream);
                     if (e == cudaSuccess) e = index_narrow((int)dim, ctx, ctx->copy_stream, stg.d[b].p, nullptr, rows_of(k), ix->Xh.p + j0 * dim, ix->inexact.p + b);
-                    if (e == cudaSuccess) e = cudaMemcpyAsync(stg.flag + b, ix->inexact.p + b, sizeof(int32_t), cudaMemcpyDeviceToHost, ctx->copy_stream);
+                    if (e == cudaSuccess) e = cudaMemcpyAsync(stg.flag.p + b, ix->inexact.p + b, sizeof(int32_t), cudaMemcpyDeviceToHost, ctx->copy_stream);
                 } else
-                    e = cudaMemcpyAsync(ix->X.p + j0 * dim, stg.h[b], (size_t)bytes, cudaMemcpyHostToDevice, ctx->copy_stream);
-                if (e == cudaSuccess) e = cudaEventRecord(stg.copied[b], ctx->copy_stream);
+                    e = cudaMemcpyAsync(ix->X.p + j0 * dim, stg.h[b].p, (size_t)bytes, cudaMemcpyHostToDevice, ctx->copy_stream);
+                if (e == cudaSuccess) e = stg.in_flight(k);
             }
             if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->copy_stream);
             for (int64_t k = std::max<int64_t>(0, chunks - 2); k < chunks && e == cudaSuccess && st == GORSE_B200_OK; k++)
-                if (ix->value_bytes == 2 && stg.flag[k & 1]) promote_at(k, chunks);
+                if (ix->value_bytes == 2 && stg.flag.p[k & 1]) promote_at(k, chunks);
             if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->copy_stream);
             if (e != cudaSuccess && st == GORSE_B200_OK) {
                 set_error("snapshot load: %s", cudaGetErrorString(e));
@@ -442,16 +452,6 @@ struct NbrHeader {
     int64_t rows;
 };
 static_assert(sizeof(NbrHeader) == 48, "the neighbour stream header is 48 bytes without padding");
-
-// splitmix64's finaliser: integer arithmetic only, so every device and host computes the same value
-__host__ __device__ inline uint64_t mix64(uint64_t x)
-{
-    x ^= x >> 30;
-    x *= 0xbf58476d1ce4e5b9ull;
-    x ^= x >> 27;
-    x *= 0x94d049bb133111ebull;
-    return x ^ (x >> 31);
-}
 
 // The fingerprint's terms, one warp per live rank r (slot live_slot[r], hidden flag hidden[r]): the row's hash is the sum of
 // mix64(index << 32 | fp32 bits) over its values (dense: every column, a bf16 value widened first; sparse: each (index,
@@ -604,15 +604,14 @@ int32_t ncache_save(gorse_b200_vecdb *db, gorse_b200_write_fn write, void *user,
     }
     std::vector<int64_t> woff((size_t)rows + 1, 0);   // each row's first 32-bit word after the header
     for (int64_t i = 0; i < rows; i++) woff[(size_t)i + 1] = woff[(size_t)i] + 2 + 2 * (int64_t)cnt[(size_t)prow[(size_t)i]];
-    Staging stg;
+    Staging stg(c);
     const int64_t cap = std::min(STAGE_BYTES, std::max(MIN_STAGE_BYTES, 4 * woff[(size_t)rows]));   // a row is at most 8 + 8 * 1024 bytes
-    GB_TRY(stg.alloc(c, cap, rows > 0 ? 2 : 1, rows > 0));
-    Writer w{write, user, static_cast<char *>(stg.h[0]), cap, 0, 0, "neighbour cache save"};
+    GB_TRY(stg.alloc(cap, rows > 0 ? 2 : 1, rows > 0));
+    Writer w{write, user, stg.h[0].p, cap, 0, 0, "neighbour cache save"};
     GB_TRY(w.put(&h, sizeof(h)));
     GB_TRY(w.flush());
     if (rows > 0) {
-        // chunk k = rows [r0[k], r0[k + 1]) of at most cap bytes: gathered into d[k & 1], downloaded into h[k & 1] on the copy
-        // stream and written while chunk k + 1 moves, as the snapshot's dense rows are
+        // chunk k = rows [r0[k], r0[k + 1]) of at most cap bytes
         std::vector<int64_t> r0{0};
         while (r0.back() < rows) {
             int64_t e = r0.back();
@@ -627,44 +626,16 @@ int32_t ncache_save(gorse_b200_vecdb *db, gorse_b200_write_fn write, void *user,
         GB_TRY(d_ros.upload(rank_of_slot.data(), rank_of_slot.size(), c->stream));
         GB_TRY(d_woff.upload(woff.data(), woff.size(), c->stream));
         auto bytes_of = [&](int64_t k) { return 4 * (woff[(size_t)r0[(size_t)k + 1]] - woff[(size_t)r0[(size_t)k]]); };
-        auto enqueue = [&](int64_t k) {
-            const int b = (int)(k & 1);
+        GB_TRY(write_chunks(stg, w, chunks, bytes_of, [&](int64_t k, float *d) {
             const int64_t i0 = r0[(size_t)k], m = r0[(size_t)k + 1] - i0;
             const unsigned grid = (unsigned)std::min<int64_t>(div_up(m * 32, NBR_THREADS), (int64_t)c->sm_count * 16);
             ncache_gather_kernel<<<grid, NBR_THREADS, 0, c->stream>>>(K.entry.p, K.cnt.p, n, d_prow.p + i0, d_rank.p + i0, d_woff.p + i0, m, d_ros.p,
-                                                                      reinterpret_cast<uint32_t *>(stg.d[b].p));
-            c->launches++;
-            cudaError_t e = cudaGetLastError();
-            if (e == cudaSuccess) e = cudaEventRecord(stg.gathered[b], c->stream);
-            if (e == cudaSuccess) e = cudaStreamWaitEvent(c->copy_stream, stg.gathered[b], 0);
-            if (e == cudaSuccess) e = cudaMemcpyAsync(stg.h[b], stg.d[b].p, (size_t)bytes_of(k), cudaMemcpyDeviceToHost, c->copy_stream);
-            if (e == cudaSuccess) e = cudaEventRecord(stg.copied[b], c->copy_stream);
-            return e;
-        };
-        cudaError_t e = cudaSuccess;
-        int32_t st = GORSE_B200_OK;
-        for (int64_t k = 0; k < std::min<int64_t>(2, chunks) && e == cudaSuccess; k++) e = enqueue(k);
-        for (int64_t k = 0; k < chunks && e == cudaSuccess && st == GORSE_B200_OK; k++) {
-            const int b = (int)(k & 1);
-            e = cudaEventSynchronize(stg.copied[b]);
-            if (e == cudaSuccess) st = w.direct(stg.h[b], bytes_of(k));
-            if (e == cudaSuccess && st == GORSE_B200_OK && k + 2 < chunks) e = enqueue(k + 2);
-        }
-        cudaStreamSynchronize(c->copy_stream);
-        if (e != cudaSuccess) { set_error("neighbour cache save: %s", cudaGetErrorString(e)); return GORSE_B200_ERR_CUDA; }
-        if (st) return st;
+                                                                      reinterpret_cast<uint32_t *>(d));
+        }));
     }
     if (bytes_out) *bytes_out = w.pos;
     return GORSE_B200_OK;
 }
-
-#define NBR_CHECK(cond, field, at, what)                                                                             \
-    do {                                                                                                             \
-        if (!(cond)) {                                                                                               \
-            gb::set_error("neighbour cache load: bad %s at byte %lld: %s", field, (long long)(at), what);            \
-            return GORSE_B200_ERR_ARG;                                                                               \
-        }                                                                                                            \
-    } while (0)
 
 // the reader behind load's parser: take() hands out the next k bytes, reading ahead at most `more` bytes (capped at
 // NBR_AHEAD_BYTES) that a well-formed stream holds after them, so the call never reads past the stream's end
@@ -702,34 +673,34 @@ int32_t ncache_load(gorse_b200_vecdb *db, gorse_b200_read_fn read, void *user, i
     Reader r{read, user, 0, "neighbour cache load"};
     NbrHeader h;
     GB_TRY(r.get(&h, sizeof(h), "header"));
-    NBR_CHECK(memcmp(h.magic, NBR_MAGIC, sizeof(NBR_MAGIC)) == 0, "magic", 0, "not a gorse_b200 neighbour cache stream");
-    NBR_CHECK(h.version == NBR_VERSION, "version", 8, "unknown version");
+    STREAM_CHECK(r, memcmp(h.magic, NBR_MAGIC, sizeof(NBR_MAGIC)) == 0, "magic", 0, "not a gorse_b200 neighbour cache stream");
+    STREAM_CHECK(r, h.version == NBR_VERSION, "version", 8, "unknown version");
     if (h.n != K.n) {
         set_error("neighbour cache load: the stream holds lists of n = %d, the cache keeps n = %d", h.n, K.n);
         return GORSE_B200_ERR_STATE;
     }
     const int n = K.n;
-    NBR_CHECK(h.dim == db->dim, "dim", 16, "not the collection's");
-    NBR_CHECK(h.distance == db->distance, "distance", 20, "not the collection's");
+    STREAM_CHECK(r, h.dim == db->dim, "dim", 16, "not the collection's");
+    STREAM_CHECK(r, h.distance == db->distance, "distance", 20, "not the collection's");
     std::vector<int64_t> live_slot;
     live_ranks(db, live_slot, nullptr);
     const int64_t live = (int64_t)live_slot.size();
-    NBR_CHECK(h.live == live, "live count", 24, "not the collection's");
+    STREAM_CHECK(r, h.live == live, "live count", 24, "not the collection's");
     uint64_t fp = 0;
     GB_TRY(ncache_fingerprint(db, n, live_slot, &fp));
-    NBR_CHECK(h.fingerprint == fp, "fingerprint", 32, "not the collection's: saved from another collection, or before a change of this one");
-    NBR_CHECK(h.rows >= 0 && h.rows <= live, "row count", 40, "negative or above the live count");
+    STREAM_CHECK(r, h.fingerprint == fp, "fingerprint", 32, "not the collection's: saved from another collection, or before a change of this one");
+    STREAM_CHECK(r, h.rows >= 0 && h.rows <= live, "row count", 40, "negative or above the live count");
     // the rows the pool keeps (the lowest ranks) go into device staging in chunks of R rows through two pinned buffers (R n
     // entries, then R counts); the pool is touched only once the whole stream has been read and checked
     const int64_t rows = h.rows, kept = std::min(rows, K.cap);
     const int64_t R = std::max<int64_t>(1, std::min<int64_t>(kept, STAGE_BYTES / (8ll * n + 4)));
     DevBuf<uint2> s_entry;
     DevBuf<int32_t> s_cnt;
-    Staging stg;
+    Staging stg(c);
     if (kept > 0) {
         GB_TRY(s_entry.alloc((size_t)(kept * n)));
         GB_TRY(s_cnt.alloc((size_t)kept));
-        GB_TRY(stg.alloc(c, R * (8ll * n + 4), 2, false));
+        GB_TRY(stg.alloc(R * (8ll * n + 4), 2, false));
     }
     std::vector<int64_t> kept_slot((size_t)kept);
     std::vector<uint2> spill((size_t)n);
@@ -741,29 +712,29 @@ int32_t ncache_load(gorse_b200_vecdb *db, gorse_b200_read_fn read, void *user, i
         const int b = (int)(k & 1);
         int32_t rc[2];
         GB_TRY(a.take(rc, 8, 8 * (rows - i - 1)));
-        NBR_CHECK(rc[0] >= 0 && rc[0] < live, "row rank", at, "outside [0, live count)");
-        NBR_CHECK(rc[0] > prev, "row rank", at, "not above the previous row's");
-        NBR_CHECK(rc[1] >= 0 && rc[1] <= n, "entry count", at + 4, "outside [0, n]");
+        STREAM_CHECK(r, rc[0] >= 0 && rc[0] < live, "row rank", at, "outside [0, live count)");
+        STREAM_CHECK(r, rc[0] > prev, "row rank", at, "not above the previous row's");
+        STREAM_CHECK(r, rc[1] >= 0 && rc[1] <= n, "entry count", at + 4, "outside [0, n]");
         prev = rc[0];
-        if (i < kept && j == 0 && k >= 2) {
-            e = cudaEventSynchronize(stg.copied[b]);
+        if (i < kept && j == 0) {
+            e = stg.wait_free(k);
             if (e != cudaSuccess) break;
         }
-        uint2 *row = i < kept ? static_cast<uint2 *>(stg.h[b]) + j * n : spill.data();
+        uint2 *row = i < kept ? reinterpret_cast<uint2 *>(stg.h[b].p) + j * n : spill.data();
         GB_TRY(a.take(row, 8ll * rc[1], 8 * (rows - i - 1)));
         for (int t = 0; t < rc[1]; t++) {
-            NBR_CHECK((int32_t)row[t].x >= 0 && (int32_t)row[t].x < live, "entry rank", at + 8 + 8ll * t, "outside [0, live count)");
+            STREAM_CHECK(r, (int32_t)row[t].x >= 0 && (int32_t)row[t].x < live, "entry rank", at + 8 + 8ll * t, "outside [0, live count)");
             row[t].x = (uint32_t)live_slot[row[t].x];
         }
         if (i >= kept) continue;
         kept_slot[(size_t)i] = live_slot[(size_t)rc[0]];
-        int32_t *cnt = reinterpret_cast<int32_t *>(static_cast<uint2 *>(stg.h[b]) + R * n);
+        int32_t *cnt = reinterpret_cast<int32_t *>(reinterpret_cast<uint2 *>(stg.h[b].p) + R * n);
         cnt[j] = rc[1];
         if (j == R - 1 || i == kept - 1) {
             const int64_t m = j + 1;
-            e = cudaMemcpyAsync(s_entry.p + k * R * n, stg.h[b], sizeof(uint2) * (size_t)(m * n), cudaMemcpyHostToDevice, c->copy_stream);
+            e = cudaMemcpyAsync(s_entry.p + k * R * n, stg.h[b].p, sizeof(uint2) * (size_t)(m * n), cudaMemcpyHostToDevice, c->copy_stream);
             if (e == cudaSuccess) e = cudaMemcpyAsync(s_cnt.p + k * R, cnt, sizeof(int32_t) * (size_t)m, cudaMemcpyHostToDevice, c->copy_stream);
-            if (e == cudaSuccess) e = cudaEventRecord(stg.copied[b], c->copy_stream);
+            if (e == cudaSuccess) e = stg.in_flight(k);
             if (e != cudaSuccess) break;
         }
     }
@@ -790,6 +761,18 @@ int32_t ncache_load(gorse_b200_vecdb *db, gorse_b200_read_fn read, void *user, i
     return GORSE_B200_OK;
 }
 
+// one of the entries below: a host allocation that throws is GORSE_B200_ERR_OOM, naming the call
+template <typename F>
+int32_t guard(const char *who, F f)
+{
+    try {
+        return f();
+    } catch (const std::bad_alloc &) {
+        set_error("%s: host allocation failed", who);
+        return GORSE_B200_ERR_OOM;
+    }
+}
+
 }  // namespace
 }  // namespace gb
 
@@ -800,46 +783,26 @@ extern "C" {
 int32_t gorse_b200_vecdb_save(gorse_b200_vecdb *db, gorse_b200_write_fn write, void *user, int64_t *new_slot_out, int64_t *bytes_out)
 {
     GB_CHECK_ARG(db != nullptr && write != nullptr, "NULL collection or write callback");
-    try {
-        return save(db, write, user, new_slot_out, bytes_out);
-    } catch (const std::bad_alloc &) {
-        set_error("snapshot save: host allocation failed");
-        return GORSE_B200_ERR_OOM;
-    }
+    return guard("snapshot save", [&] { return save(db, write, user, new_slot_out, bytes_out); });
 }
 
 int32_t gorse_b200_vecdb_load(gorse_b200_ctx *ctx, gorse_b200_read_fn read, void *user, gorse_b200_vecdb **out, int64_t *bytes_out)
 {
     GB_CHECK_ARG(ctx != nullptr && read != nullptr && out != nullptr, "NULL context, read callback or out");
     *out = nullptr;
-    try {
-        return load(ctx, read, user, out, bytes_out);
-    } catch (const std::bad_alloc &) {
-        set_error("snapshot load: host allocation failed");
-        return GORSE_B200_ERR_OOM;
-    }
+    return guard("snapshot load", [&] { return load(ctx, read, user, out, bytes_out); });
 }
 
 int32_t gorse_b200_vecdb_neighbour_cache_save(gorse_b200_vecdb *db, gorse_b200_write_fn write, void *user, int64_t *bytes_out)
 {
     GB_CHECK_ARG(db != nullptr && write != nullptr, "NULL collection or write callback");
-    try {
-        return ncache_save(db, write, user, bytes_out);
-    } catch (const std::bad_alloc &) {
-        set_error("neighbour cache save: host allocation failed");
-        return GORSE_B200_ERR_OOM;
-    }
+    return guard("neighbour cache save", [&] { return ncache_save(db, write, user, bytes_out); });
 }
 
 int32_t gorse_b200_vecdb_neighbour_cache_load(gorse_b200_vecdb *db, gorse_b200_read_fn read, void *user, int64_t *stats_out)
 {
     GB_CHECK_ARG(db != nullptr && read != nullptr, "NULL collection or read callback");
-    try {
-        return ncache_load(db, read, user, stats_out);
-    } catch (const std::bad_alloc &) {
-        set_error("neighbour cache load: host allocation failed");
-        return GORSE_B200_ERR_OOM;
-    }
+    return guard("neighbour cache load", [&] { return ncache_load(db, read, user, stats_out); });
 }
 
 }  // extern "C"
